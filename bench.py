@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — PromQL range-query throughput on B200 (BASELINE.json metric), all four GPU configs in one JSON line.
+"""bench.py — PromQL range-query throughput on H100 (BASELINE.json metric), all four GPU configs in one JSON line.
 
   python bench.py --gpus N --steps K --warmup W            # our CUDA path  (one JSON line on rank 0)
   python bench.py --impl reference --gpus N --steps K --warmup W   # reference CPU path (oracle port)
+  python bench.py ... --dump-outputs DIR   # also write what the timed steps computed as DIR/<name>.npy
 
 Headline (`value`, `roofline`, `e2e`, `cpu_baseline`): BASELINE config 2 — a "step" is one pass of the hot path (K0
 series offsets + the fused normalize/range/rate stage: K2L first tier, K2 / its long-window instantiation / the slow
@@ -23,7 +24,8 @@ kernel, roofline and — on rank 0 at N=1 — cpu_baseline:
        (1 M histograms over 8 GPUs): K0 + rate + HistogramFold (K5); shards hold whole histograms, no collective;
   "5"  avg_over_time wide-events scan: 12.5 M rows x 32 f64 columns per GPU (100 M rows over 8 GPUs): K6 per-column
        (sum, count) + for N>1 the all-reduce of the 32 x 2 scalars.
-Inputs are far larger than L2 (126 MB) in every config, so no explicit L2 flush is needed between steps.
+Inputs are far larger than the H100's L2 (50 MB) in every config, so no explicit L2 flush is needed between steps.
+Every config's K timed steps are exactly --steps.
 """
 from __future__ import annotations
 
@@ -50,22 +52,51 @@ UNIT = "samples/s"
 
 
 def load_peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
-def load_traffic(key="range_lean_kernel"):
-    """dram__bytes_read.sum + dram__bytes_write.sum per input sample of the dominant kernel, from the committed ncu
-    --set full capture of the shipped kernel (profiles/r2_traffic.json, written by profiles/summarize_ncu.py)."""
+def gpu_identity(index: int):
+    """Name and power limit of the card the numbers are measured on (a power-capped card runs lower clocks)."""
+    info = {"name": None, "power_limit_w": None}
     try:
-        with open(os.path.join(ROOT, "profiles", "r2_traffic.json")) as f:
-            d = json.load(f)
-        return float(d[key]["dram_bytes_per_sample"]), f"profiles/r2_traffic.json[{key}] ({d[key].get('kernel', '')})"
+        import torch
+        info["name"] = torch.cuda.get_device_name(index)
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                           capture_output=True, text=True, timeout=30)
+        info["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
     except Exception:
-        return None, None
+        pass
+    return info
+
+
+class Dump:
+    """--dump-outputs DIR: what the timed path computed in its last step, as DIR/<name>.npy (float64 values, float32 0/1
+    validity).  Large outputs are represented by a fixed, seeded sample of their rows (under 64 MB in all); a cell whose
+    validity bit is 0 carries no result (the reference emits no row there) and is written as 0.0, like an Arrow null slot,
+    so that every value written is finite and comparable; <name>_valid.npy tells the two apart."""
+    def __init__(self, path):
+        self.path = path
+        if path:
+            os.makedirs(path, exist_ok=True)
+
+    @staticmethod
+    def rows(n: int, k: int, seed: int):
+        import numpy as np
+        return np.sort(np.random.default_rng(seed).choice(n, size=min(n, k), replace=False))
+
+    def save(self, name, arr):
+        import numpy as np
+        if self.path:
+            np.save(os.path.join(self.path, f"{name}.npy"), np.ascontiguousarray(arr))
+
+    def grid(self, name, values, valid_words, T, rows):
+        """values [R, T] f64 and valid_words [R, ceil(T/32)] bit words (host arrays) -> <name>.npy, <name>_valid.npy"""
+        import numpy as np
+        v = np.asarray(values, dtype=np.float64)[rows]
+        w = np.ascontiguousarray(np.asarray(valid_words)[rows]).view(np.uint8)
+        bits = np.unpackbits(w, axis=1, bitorder="little")[:, :T].astype(bool)
+        self.save(name, np.where(bits, v, 0.0))
+        self.save(f"{name}_valid", bits.astype(np.float32))
 
 
 class ClockSampler:
@@ -306,6 +337,7 @@ class Harness:
             dist.init_process_group("nccl", device_id=self.dev)
         self.ctx = Context(self.local)
         self.ctx.use_torch_stream()
+        self.dump = Dump(args.dump_outputs if self.rank == 0 else None)
         if self.world > 1:
             # the library's own communicator (the collective on the data path lives behind the C ABI); torch.distributed
             # only ships the 128-byte id and provides the barrier / max-over-ranks of the timing contract
@@ -395,6 +427,11 @@ def bench_config2(h: Harness, sampler):
     ctx.sync()
 
     ms, launches, window = h.timed(step, args.steps, args.warmup)
+    if h.dump.path:
+        rows = h.dump.rows(S, 2048, SEED)
+        ix = torch.from_numpy(rows).to(dev)
+        h.dump.grid("rate_out", out.view(S, T).index_select(0, ix).cpu().numpy(),
+                    valid.view(S, Tw).index_select(0, ix).cpu().numpy(), T, slice(None))
     slow_series, warp_tier_series = ctx.last_slow_series(), ctx.last_warp_tier_series()
     clocks = sampler.stop(*window) if sampler else None
     st = h.stage_ms(step, (0, 1), reps=min(args.steps, 5))
@@ -449,6 +486,9 @@ def bench_config2(h: Harness, sampler):
         torch.cuda.synchronize()
         dt_off = h.max_over_ranks(time.perf_counter() - t0)
         h2d_off = ctx.last_h2d_bytes()
+        if h.dump.path:
+            h.dump.grid("rate_e2e_out", h_out.numpy().reshape(Se, T), h_valid.numpy().reshape(Se, Tw), T,
+                        h.dump.rows(Se, 512, SEED + 1))
         res["e2e"] = {"value": Se * N_SAMPLES * h.world * n_e2e / dt, "unit": UNIT,
                       "h2d_bytes_per_step": h2d_ids, "d2h_bytes_per_step": Se * T * 8 + Se * Tw * 4,
                       "host_columns_bytes_per_step": Se * N_SAMPLES * 20,
@@ -494,8 +534,12 @@ def bench_config3(h: Harness):
         ctx.series_offsets_dev(sid, n_rows, S, offsets)
         ctx.range_group_sum_allreduce_dev(p, ts, val, offsets, n_rows, S, ix, tiles, gsum, gcnt)
 
-    steps = max(3, args.steps // 2) if args.steps > 4 else args.steps
+    steps = args.steps
     ms, launches, _ = h.timed(step, steps, max(3, args.warmup))
+    if h.dump.path:
+        ix_g = torch.from_numpy(h.dump.rows(G, 1024, SEED + 3)).to(dev)
+        h.dump.save("sumby_sum", gsum.view(G, T).index_select(0, ix_g).cpu().numpy())
+        h.dump.save("sumby_count", gcnt.view(G, T).index_select(0, ix_g).cpu().numpy().astype(np.float32))
     st = h.stage_ms(step, (0, 1, 4))
     # compute-only variant of the same step (no collective) on N>1, to name the collective's share
     ms_nocoll = None
@@ -564,8 +608,11 @@ def bench_config4(h: Harness):
         ctx.range_eval_dev(p, ts, val, offsets, n_rows, S, rates, rvalid)
         ctx.histogram_quantile_dev(0.99, le, B, rates, rvalid, H, T, out, ovalid)
 
-    steps = max(3, h.args.steps // 2) if h.args.steps > 4 else h.args.steps
+    steps = args.steps
     ms, launches, _ = h.timed(step, steps, max(3, args.warmup))
+    if h.dump.path:
+        h.dump.grid("hist_quantile", out.view(H, T).cpu().numpy(), ovalid.view(H, Tw).cpu().numpy(), T,
+                    h.dump.rows(H, 4096, SEED + 4))
     st = h.stage_ms(step, (0, 1, 3))
     peak, _ = load_peaks()
     alg_range = 16.0 * n_rows + 8.0 * S * T + 4.0 * S * Tw + 8.0 * (S + 1)
@@ -593,9 +640,12 @@ def bench_config4(h: Harness):
 
 def bench_config5(h: Harness):
     """avg_over_time wide-events scan: per-column (sum, count) of 32 f64 columns + (N>1) the all-reduce of the scalars."""
+    import numpy as np
     torch, args, ctx, dev = h.torch, h.args, h.ctx, h.dev
     rows, cols = args.wide_rows_per_gpu, 32
-    data = torch.rand((cols, rows), dtype=torch.float64, device=dev)
+    gen = torch.Generator(device=dev)
+    gen.manual_seed(SEED + h.rank)   # the same table in every run with the same arguments
+    data = torch.rand((cols, rows), dtype=torch.float64, device=dev, generator=gen)
     data[:, ::1009] = float("nan")     # stale markers are skipped like SeriesNormalize's filter
     ptrs = torch.tensor([data[c].data_ptr() for c in range(cols)], dtype=torch.int64, device=dev)
     col_sum = torch.zeros(cols, dtype=torch.float64, device=dev)
@@ -607,8 +657,10 @@ def bench_config5(h: Harness):
         ctx.column_reduce_dev(ptrs, cols, rows, col_sum, col_cnt)
         ctx.allreduce_columns_dev(col_sum, col_cnt, cols)
 
-    steps = max(3, h.args.steps // 2) if h.args.steps > 4 else h.args.steps
+    steps = args.steps
     ms, launches, _ = h.timed(step, steps, max(3, args.warmup))
+    h.dump.save("wide_sum", col_sum.cpu().numpy())
+    h.dump.save("wide_count", col_cnt.cpu().numpy().astype(np.float64))
     st = h.stage_ms(step, (3, 4))
     avg = (col_sum / col_cnt.to(torch.float64)).cpu()
     peak, _ = load_peaks()
@@ -668,13 +720,11 @@ def run_ours(args):
     else:
         kernel_name = ("range_lean_kernel<rate> (+ range_fast_kernel<rate> over the series it hands off)" if lean_on
                        else "range_fast_kernel<rate>")
-    uniform = lean_on and not args.resets and args.jitter_ms == 0 and os.environ.get("B2P_UNIFORM", "") != "0"
-    per_sample, traffic_src = load_traffic("range_lean_kernel_uniform" if uniform else "range_lean_kernel")
     value = S * N_SAMPLES * h.world / (step_ms * 1e-3)
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": h.world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": step_ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64",
-        "data": "synthetic",
+        "data": "synthetic", "gpu": gpu_identity(h.local),
         "config": {"workload": f"rate(x[5m]) step 15s over {S} series x {N_SAMPLES} samples per GPU per step "
                                f"(BASELINE config 2 = 10M series processed as chunks of {S}); resets={args.resets}; "
                                + ("scrapes on the 15 s schedule (BASELINE.md section 4 main shape)" if args.jitter_ms == 0
@@ -686,13 +736,9 @@ def run_ours(args):
                    "series_per_gpu_per_step": S, "samples_per_series": N_SAMPLES, "eval_steps": T,
                    "parallelism": f"series-sharded x{h.world}, no data-path collective in config 2 "
                                   "(configs.3 / configs.5 carry the collectives)",
-                   "l2": "inputs (16-25 GB per step) >> 126 MB L2; no flush needed"},
+                   "l2": "inputs (16-25 GB per step) >> 50 MB L2; no flush needed"},
         "roofline": {"bound": "hbm", "kernel": kernel_name, "achieved": achieved, "peak": peak,
-                     "unit": "GB/s", "frac": achieved / peak,
-                     # dram__bytes_read.sum + dram__bytes_write.sum per launch: bytes per sample of the committed ncu
-                     # --set full capture of the shipped kernel (profiles/r2_traffic.json) x the samples of this launch
-                     "traffic": per_sample * n_rows if (per_sample and lean_on) else None, "traffic_source": traffic_src,
-                     "peak_source": peak_src,
+                     "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": alg_k2, "kernel_ms": k2, "k0_series_offsets_ms": k0,
                      "hbm_read_frac_whole_step": 20.0 * n_rows / (step_ms * 1e-3) / 1e9 / peak},
         "gpu_launches": c2["launches"], "slow_path_series": c2["slow_series"], "warp_tier_series": c2["warp_tier_series"],
@@ -749,6 +795,8 @@ def main():
                     help="config 3, N>1: group ranges the partials are computed and all-reduced in (overlap)")
     ap.add_argument("--hist-per-gpu", type=int, default=125_000)
     ap.add_argument("--wide-rows-per-gpu", type=int, default=12_500_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what they computed (a seeded sample of large outputs) as DIR/<name>.npy")
     args = ap.parse_args()
     global JITTER_MS
     JITTER_MS = args.jitter_ms

@@ -1,6 +1,6 @@
-"""greptimedb_b200 — B200-native evaluator for GreptimeDB's PromQL range-query hot path.
+"""greptimedb_b200 — H100-native evaluator for GreptimeDB's PromQL range-query hot path.
 
-The product is libb200promql.so (hand-written CUDA for sm_100a behind the C ABI of
+The product is libb200promql.so (hand-written CUDA for sm_90a behind the C ABI of
 include/b200promql.h); this package is the thin Python handle used by tests and bench.py.
 Importing the package does not load the library; `engine.Context()` does, and fails loudly if the
 library or a CUDA device is missing (there is no CPU fallback).

@@ -126,9 +126,9 @@ struct DevBuf {
 constexpr int kRing = 256;
 constexpr int kBigRing = 1024;        // long-window instantiation of the warp-per-series kernel (one CTA per SM)
 constexpr int kStatusSlots = 32;      // range calls that may be outstanding between two b2p_sync
-constexpr int kSlowCtas = 148;        // slow-path grid (4 warps per CTA)
+constexpr int kSlowCtas = 132;        // slow-path grid (4 warps per CTA): one CTA per SM of an H100
 constexpr int kSlowWarps = kSlowCtas * 4;
-constexpr size_t kArenaDefaultRows = 1u << 21;  // 32 MB: regions of 3 542 rows for the 592 slow-path warps
+constexpr size_t kArenaDefaultRows = 1u << 21;  // 32 MB: regions of 3 971 rows for the 528 slow-path warps
 
 }  // namespace
 
@@ -143,7 +143,7 @@ struct b2p_group_index {
 
 struct b2p_ctx {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   cudaStream_t own_stream = nullptr, stream = nullptr;
   // Device-side status.  Every range call owns one slot of d_ring until b2p_sync has read it back, so any number
   // (<= kStatusSlots, then the library synchronises by itself) of *_dev range calls may be outstanding; the verdict
@@ -163,10 +163,9 @@ struct b2p_ctx {
   // multi-GPU (one process per GPU): communicator of the by-label all-reduce, its stream and join event
   Nccl::comm_t comm = nullptr;
   int comm_ranks = 1, comm_rank = 0;
-  long long comm_headstart_cycles = 60000;  // ~30 us at 1.965 GHz (B2P_COMM_HEADSTART_US overrides)
-  // SMs the fused tier leaves to the tile all-reduce (B2P_COMM_RESERVE_SMS).  Off: measured at 2 GPUs, 0 / 8 / 16 SMs
-  // left free give 12.0 / 12.3 / 14.2 ms per step — the all-reduce of a tile still does not run beside the next tile's
-  // kernel, the step only loses the SMs (DESIGN.md section 7)
+  long long comm_headstart_cycles = 60000;  // ~30 us at 1.98 GHz, the H100's top SM clock (B2P_COMM_HEADSTART_US overrides)
+  // SMs the fused tier leaves to the tile all-reduce (B2P_COMM_RESERVE_SMS).  Off: SMs left free do not make the
+  // all-reduce of a tile run beside the next tile's kernel, the step only loses them (DESIGN.md section 7)
   int comm_reserve_sms = 0;
   int comm_reserve_now = 0;                 // ... in effect for the launch being issued
   cudaStream_t s_comm = nullptr;
@@ -174,8 +173,8 @@ struct b2p_ctx {
   DevBuf m_tmp0, m_tmp1;             // scratch of the variance merge
   DevBuf w_skip, b_skip, slow_skip;  // fused by-label partials: steps already added, parallel to the work lists
   bool fused_pending = false;        // a fused call is outstanding: its work lists must survive until b2p_sync
-  // K2T (thread per series) in front of K2 for rate/increase/delta.  Measured slower than K2 on B200
-  // (28 vs 64 G samples/s, profiles/r1_thread_tier.md), so it is opt-in: B2P_ENABLE_THREAD_TIER=1.
+  // K2T (thread per series) in front of K2 for rate/increase/delta.  Slower than K2 on the benchmark shape, so it
+  // is opt-in: B2P_ENABLE_THREAD_TIER=1.
   bool thread_tier = false;
   // K2L, the lean warp-per-series tier in front of K2 (default on; B2P_DISABLE_LEAN_TIER=1 turns it off)
   bool lean_tier = true;
@@ -563,7 +562,7 @@ int ensure_slow_scratch(b2p_ctx* c, uint32_t n_series, int64_t T) {
 extern "C" {
 
 const char* b2p_last_error(void) { return g_err.c_str(); }
-const char* b2p_version(void) { return "b200promql 0.1 (sm_100a)"; }
+const char* b2p_version(void) { return "b200promql 0.1 (sm_90a)"; }
 
 int64_t b2p_num_steps(int64_t start, int64_t end, int64_t interval) {
   if (interval <= 0 || end < start) return 0;
@@ -623,7 +622,7 @@ b2p_ctx* b2p_create(int device) {
   if (const char* e = getenv("B2P_HOST_TS_SCAN")) c->host_ts_scan = (e[0] != '0');
   if (const char* e = getenv("B2P_UNIFORM")) c->uniform_mode = (e[0] == '0') ? 0 : (e[0] == '1' ? 1 : -1);
   if (const char* e = getenv("B2P_COMM_RESERVE_SMS")) c->comm_reserve_sms = atoi(e);
-  if (const char* e = getenv("B2P_COMM_HEADSTART_US")) c->comm_headstart_cycles = (long long)(atof(e) * 1965.0);
+  if (const char* e = getenv("B2P_COMM_HEADSTART_US")) c->comm_headstart_cycles = (long long)(atof(e) * 1980.0);
   if (const char* e = getenv("B2P_ARENA_ROWS")) c->arena_rows_wanted = (size_t)strtoull(e, nullptr, 10);
   return c;
 }
@@ -1490,7 +1489,7 @@ int b2p_synth_fill_dev(b2p_ctx* c, uint64_t series_begin, uint64_t n_series, uin
 
 // One chunk, no overlap: H2D -> K0/K2 -> D2H on the context stream.  sid values are global ids
 // (sid_base is subtracted on the device); offsets_host, when given, is already rebased to the chunk.
-// Host-side SeriesDivide + cadence scan (see the header).  Plain sequential passes: memory bound, ~8-10 GB/s per thread;
+// Host-side SeriesDivide + cadence scan (see the header).  Plain sequential passes, memory bound;
 // b2p_range_eval runs one of these per chunk on a few worker threads while earlier chunks are on the bus.
 static int host_scan_series(const int64_t* ts, const uint32_t* sid, const uint64_t* offsets_in, uint64_t n_rows,
                             uint32_t n_series, uint32_t sid_base, uint64_t* offsets_out, int64_t* t0, int64_t* cadence,
@@ -1656,7 +1655,7 @@ int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, con
   // descriptor arrays), 2 = take the ordinary route (ids out of order included: K0 reports those as before)
   // (only when the batch comes with its id column: then the descriptors replace 12 of the 20 B/row and K0; with offsets
   // handed over the call is already at 16 B/row, and the scan's per-call cost — pinned descriptor arrays, worker
-  // threads — measured more than the 8 B/row it saves: 2.36 vs 3.0 G samples/s)
+  // threads — costs more than the 8 B/row it saves)
   const bool scan = c->host_ts_scan && !offsets_host;
   uint64_t* h_doff = nullptr;
   int64_t *h_t0 = nullptr, *h_cad = nullptr;

@@ -39,10 +39,10 @@
 namespace b2p {
 
 // Warps per CTA of the first tier and resident CTAs per SM, tuned together with the register budget: ONE CTA of 24
-// warps per SM (80 registers).  Measured on the BASELINE shape (profiles/r2_range_lean_kernel.md): 3 x 8 warps 8.51 ms,
-// 2 x 12 warps 8.28 ms, 1 x 24 warps 7.88 ms, 1 x 28 warps (72 registers) 7.91 ms, 1 x 32 warps (64 registers) 8.04 ms —
-// the warps of a CTA work on ADJACENT series, so with one CTA the SM's concurrent streams (ts, val, out) each stay
-// inside one contiguous 192 KB region instead of three regions megabytes apart.  (B2P_LEAN_CONTIG = 1 additionally
+// warps per SM (80 registers; 172 KB of shared memory in the uniform-cadence variant, 196 KB with the fused by-label
+// counters, within the H100's 227 KB per block).  The warps of a CTA work on ADJACENT series, so with one CTA the SM's
+// concurrent streams (ts, val, out) each stay inside one contiguous 192 KB region instead of several regions megabytes
+// apart (H100 timings of the alternatives: DESIGN.md section 5).  (B2P_LEAN_CONTIG = 1 additionally
 // gives every CTA one contiguous range of series over time: no measurable difference, off.)
 #ifndef B2P_LEAN_MIN_BLOCKS
 #define B2P_LEAN_MIN_BLOCKS 1
@@ -61,7 +61,6 @@ constexpr int kLeanWarps = B2P_LEAN_WARPS;
 #endif
 constexpr int kLeanDepth = B2P_LEAN_DEPTH;
 // ... of the uniform-cadence kernel: with its steady form it is no longer issue bound and a third block in flight pays
-// (1.25 M series: 6.03 -> 5.80 ms; the general kernel: 7.62 -> 7.69)
 #ifndef B2P_LEAN_DEPTH_UNI
 #define B2P_LEAN_DEPTH_UNI 3
 #endif
@@ -334,9 +333,9 @@ __device__ __forceinline__ int lean_group(const RangeArgs& a, LeanState& st, Lea
 
 // The uniform-cadence path is compiled into the plain variants of the extrapolated functions (rate / increase / delta):
 // there the per-step arithmetic it removes dominates.  (With the reset bit words the correction scan dominates, and the
-// *_over_time functions walk their windows anyway: measured, no gain.)
+// *_over_time functions walk their windows anyway: no gain.)
 // It is a kernel variant of its own (template parameter UNI) — compiled into the general kernel it costs the jittered
-// case 6 % through register pressure — and cadence_probe_kernel picks one of the two per call on the device.
+// case time through register pressure — and cadence_probe_kernel picks one of the two per call on the device.
 template <int FN, bool FLAGS>
 constexpr bool kLeanUniform = B2P_LEAN_UNIFORM && !FLAGS && FnTraits<FN>::kExtrapolated;
 
@@ -1004,7 +1003,7 @@ __global__ void __launch_bounds__(kProbeThreads) cadence_probe_kernel(const Rang
 #pragma unroll
       for (int i = 0; i < 9; ++i) t[i] = (uint64_t)i < m ? a.ts[r0 + i] : 0;  // (independent loads, one round trip)
       // (short series spend their steps in the head / tail groups, which the uniform-cadence path does not cover, and
-      // never reach its steady form: config 4's 128-sample series measured 6 % slower on it)
+      // never reach its steady form: config 4's 128-sample series are slower on it)
       bool regular = r1 - r0 >= 256ull;
 #pragma unroll
       for (int i = 1; i < 9; ++i) regular = regular && ((uint64_t)i >= m || t[i] - t[i - 1] == a.interval);

@@ -1,5 +1,5 @@
 /*
- * b200promql.h — C ABI of libb200promql.so: a B200 (sm_100a) evaluator for GreptimeDB's
+ * b200promql.h — C ABI of libb200promql.so: an H100 (sm_90a) evaluator for GreptimeDB's
  * PromQL range-query hot path.  Plain pointers and sizes only (no torch / Arrow C++ types), so
  * the reference's Rust host can bind it with `extern "C"` / cxx (see INTEGRATION.md).
  *

@@ -2,7 +2,7 @@
  * promql_oracle.c — CPU ORACLE (test infrastructure only; see promql_oracle.h).
  *
  * Plain-C restatement of GreptimeDB's PromQL range-query hot path.  Each function names the
- * reference file:line it follows (relative to /root/reference).  Nothing here is derived from
+ * reference file:line it follows (relative to the GreptimeDB source tree).  Nothing here is derived from
  * the CUDA code; the CUDA code is checked AGAINST this.
  */
 #include "promql_oracle.h"

@@ -8,12 +8,12 @@
  * It is a plain-C restatement of the reference's (GreptimeTeam/greptimedb, Rust)
  * algorithm for the path  SeriesDivide -> SeriesNormalize -> RangeManipulate ->
  * prom_* range UDF -> Filter(IS NOT NULL) -> Aggregate / HistogramFold / InstantManipulate.
- * Every function cites the reference file:line it follows (paths relative to
- * /root/reference).  The reference itself (Rust nightly + ~1000 crates) cannot be
- * compiled in this image, so parity is pinned on the reference's OWN unit-test
+ * Every function cites the reference file:line it follows (paths relative to the
+ * GreptimeDB source tree).  The reference itself (Rust nightly + ~1000 crates) is not
+ * built by this project, so parity is pinned on the reference's OWN unit-test
  * golden vectors (tests/golden/ *.json, ported from the #[test] bodies cited there).
  *
- * Third-party arithmetic that is NOT under /root/reference and is restated from its
+ * Third-party arithmetic that is NOT in the GreptimeDB tree and is restated from its
  * published algorithm (unit-level parity UNPINNED beyond the reference's 1e-4 tests):
  *   - arrow-rs 57.3.0 compute::sum / min / max   (Cargo.lock:318-321) -> orc_arrow_sum/min/max
  *   - datafusion 52.1 (GreptimeTeam fork rev 02b82535) sum/avg/count/min/max accumulators

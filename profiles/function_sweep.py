@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Throughput of every range function on the BASELINE config-2 shape (device-resident inputs, K0 + K2 per pass).
-usage (on a B200): python profiles/function_sweep.py [series]  -> markdown table on stdout"""
+usage (on an H100): python profiles/function_sweep.py [series]  -> markdown table on stdout"""
 import os
 import sys
 

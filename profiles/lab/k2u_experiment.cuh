@@ -1,7 +1,7 @@
 // k2u_experiment.cuh — K2U, an EXPERIMENT that is not part of the library: a ring-free first tier for series sampled
 // exactly at the eval interval (rate / increase / delta).  Bit-identical to the shipped kernels and parity-green when it
-// was wired in, but no faster than the uniform-cadence variant of range_lean_kernel (6.3 - 6.5 ms vs 6.31 ms per 1.25 M
-// series; stream_test.cu puts the bound of its access pattern at 5.15 ms), so the library keeps one kernel.  Build:
+// was wired in, but no faster than the uniform-cadence variant of range_lean_kernel when it was measured (stream_test.cu
+// gives the bound of its access pattern), so the library keeps one kernel.  Build:
 // k2l_lab.cu with -DLAB_K2U -I profiles/lab.
 //
 // Same contract as range_lean_kernel (SeriesNormalize -> RangeManipulate -> prom_* UDF -> IS NOT NULL, one warp per
@@ -45,9 +45,8 @@ namespace b2p {
 #endif
 constexpr int kUniWarps = B2P_UNI_WARPS;
 // 32-step chunks a warp fetches in one go: kUniUnroll * 256 contiguous bytes of each column requested back to back keep
-// DRAM rows open, and they are the bytes in flight per warp (profiles/lab/stream_test.cu: this access pattern reaches
-// 6.2 TB/s at 4 chunks x 32 warps per SM; 1 chunk 5.2, 8 chunks 6.0; cp.async staging queues of 4 - 16 chunks in
-// shared memory were all slower, 7.0 - 8.5 ms vs 6.3 ms per 1.25 M series)
+// DRAM rows open, and they are the bytes in flight per warp (profiles/lab/stream_test.cu measures this access pattern
+// for 1 - 8 chunks; cp.async staging queues of 4 - 16 chunks in shared memory were slower)
 constexpr int kUniUnroll = B2P_UNI_UNROLL;
 #ifndef B2P_UNI_SHUF
 #define B2P_UNI_SHUF 1

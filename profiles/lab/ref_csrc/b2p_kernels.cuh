@@ -1,4 +1,4 @@
-// b2p_kernels.cuh — CUDA kernels (sm_100a) of the PromQL range-query path.
+// b2p_kernels.cuh — CUDA kernels of the PromQL range-query path.
 //
 //  K0 series_offsets_kernel   SeriesDivide: series boundaries from the sorted u32 id column
 //  K2L range_lean_kernel<FN>  (b2p_kernel_lean.cuh) first tier of the same fused stage: regular series only,

@@ -111,6 +111,8 @@ __global__ void rows_neighbours(const long long* __restrict__ ts, const double* 
   }
 }
 int main(int argc, char** argv) {
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   const unsigned S = 1250000; const int N = 1000; const size_t n = (size_t)S * N;
   long long* ts; double *val, *out;
   CK(cudaMalloc(&ts, n * 8)); CK(cudaMalloc(&val, n * 8)); CK(cudaMalloc(&out, n * 8));
@@ -122,8 +124,8 @@ int main(int argc, char** argv) {
     float ms; CK(cudaEventElapsedTime(&ms, e0, e1)); ms /= 5; CK(cudaGetLastError());
     printf("%-32s %.3f ms  %.2f TB/s\n", tag, ms, 24.0 * n / (ms * 1e-3) / 1e12);
   };
-  timeit("contiguous 148x8x256", [&] { contiguous<<<148 * 8, 256>>>(ts, val, out, n); });
-  timeit("contiguous 148x4x512", [&] { contiguous<<<148 * 4, 512>>>(ts, val, out, n); });
+  timeit("contiguous SMx8x256", [&] { contiguous<<<sms * 8, 256>>>(ts, val, out, n); });
+  timeit("contiguous SMx4x512", [&] { contiguous<<<sms * 4, 512>>>(ts, val, out, n); });
   unsigned long long* offsets; unsigned* vw;
   CK(cudaMalloc(&offsets, ((size_t)S + 1) * 8)); CK(cudaMalloc(&vw, (size_t)S * 32 * 4));
   {
@@ -131,24 +133,24 @@ int main(int argc, char** argv) {
     for (size_t i = 0; i <= S; ++i) h[i] = i * N;
     CK(cudaMemcpy(offsets, h, ((size_t)S + 1) * 8, cudaMemcpyHostToDevice)); free(h);
   }
-  timeit("extras 0", [&] { rows_extras<4, 0><<<148 * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("extras 1 (first)", [&] { rows_extras<4, 1><<<148 * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("extras 3 (first+prev)", [&] { rows_extras<4, 3><<<148 * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("extras 4 (vw)", [&] { rows_extras<4, 4><<<148 * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("extras 8 (setup)", [&] { rows_extras<4, 8><<<148 * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("extras 7 (first+prev+vw)", [&] { rows_extras<4, 7><<<148 * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("extras 15 (all)", [&] { rows_extras<4, 15><<<148 * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("extras 15 (all) U=2 x6", [&] { rows_extras<2, 15><<<148 * 6, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("neighbours shuffle U=4 x4", [&] { rows_neighbours<4, 1><<<148 * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("neighbours smem    U=4 x4", [&] { rows_neighbours<4, 2><<<148 * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("neighbours shuffle U=2 x6", [&] { rows_neighbours<2, 1><<<148 * 6, 256>>>(ts, val, out, offsets, vw, S, N); });
-  timeit("neighbours smem    U=2 x6", [&] { rows_neighbours<2, 2><<<148 * 6, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("extras 0", [&] { rows_extras<4, 0><<<sms * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("extras 1 (first)", [&] { rows_extras<4, 1><<<sms * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("extras 3 (first+prev)", [&] { rows_extras<4, 3><<<sms * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("extras 4 (vw)", [&] { rows_extras<4, 4><<<sms * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("extras 8 (setup)", [&] { rows_extras<4, 8><<<sms * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("extras 7 (first+prev+vw)", [&] { rows_extras<4, 7><<<sms * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("extras 15 (all)", [&] { rows_extras<4, 15><<<sms * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("extras 15 (all) U=2 x6", [&] { rows_extras<2, 15><<<sms * 6, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("neighbours shuffle U=4 x4", [&] { rows_neighbours<4, 1><<<sms * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("neighbours smem    U=4 x4", [&] { rows_neighbours<4, 2><<<sms * 4, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("neighbours shuffle U=2 x6", [&] { rows_neighbours<2, 1><<<sms * 6, 256>>>(ts, val, out, offsets, vw, S, N); });
+  timeit("neighbours smem    U=2 x6", [&] { rows_neighbours<2, 2><<<sms * 6, 256>>>(ts, val, out, offsets, vw, S, N); });
   for (int ctas : {4}) {
     char tag[64];
-    snprintf(tag, 64, "rows U=1 %dx256", ctas); timeit(tag, [&] { per_warp_rows<1><<<148 * ctas, 256>>>(ts, val, out, S, N); });
-    snprintf(tag, 64, "rows U=2 %dx256", ctas); timeit(tag, [&] { per_warp_rows<2><<<148 * ctas, 256>>>(ts, val, out, S, N); });
-    snprintf(tag, 64, "rows U=4 %dx256", ctas); timeit(tag, [&] { per_warp_rows<4><<<148 * ctas, 256>>>(ts, val, out, S, N); });
-    snprintf(tag, 64, "rows U=8 %dx256", ctas); timeit(tag, [&] { per_warp_rows<8><<<148 * ctas, 256>>>(ts, val, out, S, N); });
+    snprintf(tag, 64, "rows U=1 %dx256", ctas); timeit(tag, [&] { per_warp_rows<1><<<sms * ctas, 256>>>(ts, val, out, S, N); });
+    snprintf(tag, 64, "rows U=2 %dx256", ctas); timeit(tag, [&] { per_warp_rows<2><<<sms * ctas, 256>>>(ts, val, out, S, N); });
+    snprintf(tag, 64, "rows U=4 %dx256", ctas); timeit(tag, [&] { per_warp_rows<4><<<sms * ctas, 256>>>(ts, val, out, S, N); });
+    snprintf(tag, 64, "rows U=8 %dx256", ctas); timeit(tag, [&] { per_warp_rows<8><<<sms * ctas, 256>>>(ts, val, out, S, N); });
   }
   return 0;
 }

@@ -3,8 +3,7 @@
 
     summarize_ncu.py rep.ncu-rep [...]                       markdown on stdout
     summarize_ncu.py --traffic-json OUT SAMPLES rep.ncu-rep  also write {kernel: dram bytes per input sample} (first
-                                                             launch of each kernel; SAMPLES = input samples per launch)
-bench.py reads profiles/r2_traffic.json written this way for roofline.traffic."""
+                                                             launch of each kernel; SAMPLES = input samples per launch)"""
 import csv
 import subprocess
 import sys

@@ -1,4 +1,4 @@
-//! GPU execution of GreptimeDB's PromQL range-query sub-plan on B200 (`libb200promql.so`).
+//! GPU execution of GreptimeDB's PromQL range-query sub-plan on an H100 (`libb200promql.so`).
 //!
 //! * [`ffi`]   — `#[repr(C)]` / `extern "C"` mirror of every declaration in `include/b200promql.h`
 //!               (layouts are checked from the C side by `tests/layout.c`).

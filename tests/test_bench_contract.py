@@ -1,22 +1,35 @@
-"""CPU checks of bench.py's contract pieces that do not need a GPU: the committed ncu traffic file carries the kernel
-variants the JSON line's roofline.traffic is read from, and the reference arm (--impl reference: the oracle port timed on
-the host cores) prints one JSON line with the keys the driver reads."""
+"""CPU checks of bench.py's contract pieces that do not need a GPU: --dump-outputs writes the validity bit words as a
+0/1 grid and invalid cells as 0.0 from a fixed row sample, and the reference arm (--impl reference: the oracle port
+timed on the host cores) prints one JSON line with the keys a reader of the result expects."""
 import json
 import os
 import subprocess
 import sys
 
+import numpy as np
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_committed_traffic_file_has_the_kernel_variants_the_bench_reads():
+def test_dump_outputs_grid_unpacks_validity_words_and_samples_rows_reproducibly(tmp_path):
     sys.path.insert(0, ROOT)
     import bench
-    for key in ("range_lean_kernel", "range_lean_kernel_uniform"):
-        per_sample, src = bench.load_traffic(key)
-        assert per_sample is not None and src, key
-        # ts 8 + val 8 read, 8 B + 1 bit written per step (steps ~ samples in config 2): ~24 B per input sample
-        assert 20.0 < per_sample < 30.0, (key, per_sample)
+    R, T = 5, 40
+    Tw = (T + 31) // 32
+    vals = np.arange(R * T, dtype=np.float64).reshape(R, T)
+    vals[:, 5] = np.nan   # what an invalid cell may hold in the library's output
+    words = np.zeros((R, Tw), np.uint32)
+    words[:, 0] = 0x80000001   # steps 0 and 31
+    words[:, 1] = 0x00000080   # step 39
+    rows = bench.Dump.rows(R, 3, 7)
+    assert rows.tolist() == bench.Dump.rows(R, 3, 7).tolist() and len(set(rows.tolist())) == 3
+    d = bench.Dump(str(tmp_path / "out"))
+    d.grid("g", vals, words.view(np.int32), T, rows)
+    v, ok = np.load(tmp_path / "out" / "g.npy"), np.load(tmp_path / "out" / "g_valid.npy")
+    assert v.dtype == np.float64 and ok.dtype == np.float32 and v.shape == ok.shape == (3, T)
+    assert (np.flatnonzero(ok[0]) == [0, 31, 39]).all() and (ok == ok[0]).all()
+    assert (v[:, [0, 31, 39]] == vals[rows][:, [0, 31, 39]]).all() and (v[:, 1:31] == 0.0).all() and np.isfinite(v).all()
+    bench.Dump(None).save("x", vals)   # without --dump-outputs nothing is written
 
 
 def test_reference_arm_prints_one_contract_line():

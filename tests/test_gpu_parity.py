@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box with -m gpu): the CUDA path, called through the C ABI,
+"""GPU parity tests (run on an H100 with -m gpu): the CUDA path, called through the C ABI,
 against (1) the reference's own golden vectors and (2) the CPU oracle on seeded inputs.
 
 Tolerances: resets / changes / count_over_time / validity bitmaps are compared BIT-EXACT.  Every
@@ -1104,20 +1104,25 @@ def test_full_size_chunk_properties_and_tier_equivalence(ctx, ctx_no_lean):
         if name == "lean":
             assert c.last_warp_tier_series() <= S // 64
     r_lean, v_lean = outs[("lean", "rate")]
-    r_k2, v_k2 = outs[("k2", "rate")]
+    r_k2, v_k2 = outs.pop(("k2", "rate"))
     assert torch.equal(v_lean, v_k2)
     assert torch.equal(r_lean.view(torch.int64), r_k2.view(torch.int64))
+    del r_k2, v_k2  # 80 GB hold the inputs and three [S x T] outputs, not the temporaries below on top of them
     # validity: steps 1 .. 999 have >= 2 samples in (t - 5m, t] unless a zero-jitter sample sits on an edge; step 0 never
     bits = v_lean.view(S, Tw)
     popc = sum(((bits >> b) & 1).sum(dtype=torch.int64) for b in range(32))
     n_valid = int(popc.item())
     assert S * 997 <= n_valid <= S * 999, n_valid
-    # linearity of increase against rate
+    # linearity of increase against rate (every valid step, taken in slices of series)
     inc, v_inc = outs[("lean", "increase")]
     assert torch.equal(v_inc, v_lean)
-    vb = ((bits.unsqueeze(-1) >> torch.arange(32, device=dev, dtype=torch.int32)) & 1).bool().reshape(S, Tw * 32)[:, :T]
-    mask = vb.reshape(-1)
-    rel = ((inc[mask] - r_lean[mask] * 300.0).abs() / inc[mask].abs().clamp_min(1e-300)).max().item()
+    lanes = torch.arange(32, device=dev, dtype=torch.int32)
+    rel = 0.0
+    for a in range(0, S, 125_000):
+        b = min(S, a + 125_000)
+        mask = ((bits[a:b].unsqueeze(-1) >> lanes) & 1).bool().reshape(b - a, Tw * 32)[:, :T].reshape(-1)
+        i_, r_ = inc[a * T:b * T][mask], r_lean[a * T:b * T][mask]
+        rel = max(rel, ((i_ - r_ * 300.0).abs() / i_.abs().clamp_min(1e-300)).max().item())
     assert rel <= 1e-15, rel
     # a slice evaluated alone gives the same bits
     s0, ns = 777_216, 4096
