@@ -143,13 +143,19 @@ __global__ void __launch_bounds__(256) group_finalize_kernel(int32_t agg, double
   }
 }
 
-// Cross-rank merge helpers of the by-label partials (b2p_allreduce_partials_dev).
-// phase 0: groups this rank has no row for become the neutral element of min / max; phase 1 (after the all-reduce,
-// cnt = global count): groups absent everywhere read 0.0 again, like a freshly built partial.
+// Cross-rank merge helpers of the by-label partials (b2p_allreduce_partials_dev).  The extremes travel as f64::total_cmp
+// keys (int64, all-reduced with MIN / MAX), so the merge follows the same total order as the single-pass fold: +NaN is
+// the greatest value, -NaN the least, -0.0 < +0.0.  An IEEE f64 min / max would not (it ignores or propagates NaN
+// depending on the operand order and treats the zeros as equal).
+// phase 0: every value becomes its key in place; groups this rank has no row for become the neutral key of min / max
+// (INT64_MAX / INT64_MIN).  phase 1 (after the all-reduce, cnt = global count): keys map back to values (total_key is an
+// involution, NaN payloads survive), groups absent everywhere read 0.0 again, like a freshly built partial.
 __global__ void __launch_bounds__(256) minmax_neutral_kernel(bool is_min, double* val, const uint32_t* cnt, uint64_t n, int phase) {
-  const double inf = __longlong_as_double(0x7ff0000000000000ll);
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
-    if (cnt[i] == 0) val[i] = phase == 0 ? (is_min ? inf : -inf) : 0.0;
+  long long* key = reinterpret_cast<long long*>(val);
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    if (phase == 0) key[i] = cnt[i] ? total_key(val[i]) : (is_min ? 0x7fffffffffffffffll : (-0x7fffffffffffffffll - 1));
+    else val[i] = cnt[i] ? __longlong_as_double(total_key(__longlong_as_double(key[i]))) : 0.0;
+  }
 }
 // (cnt, mean, M2) states of population variance.  phase 0: wsum = cnt * mean, cnt_r = cnt (kept: cnt becomes global);
 // phase 1 (wsum, cnt all-reduced): mean_g = wsum / cnt; M2 += cnt_r * (mean_r - mean_g)^2 — the all-reduce of M2 that

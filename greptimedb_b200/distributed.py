@@ -67,22 +67,32 @@ def finalize_host(agg: str, sum_a: np.ndarray, cnt_a: np.ndarray) -> np.ndarray:
     return out
 
 
+def total_key(x):
+    """f64::total_cmp key of a float64 tensor as int64: the bit pattern with the 63 low bits flipped where the sign bit
+    is set.  Applied to the int64 keys (or their bit patterns) it gives the bit patterns back: an involution."""
+    import torch
+    b = x.view(torch.int64)
+    return b ^ ((b >> 63) & torch.iinfo(torch.int64).max)
+
+
 def merge_partials(agg: str, val_t, cnt_t, mean_t=None, group=None):
     """Host mirror of b2p_allreduce_partials_dev (same formulas, torch.distributed instead of the library's NCCL
     communicator; used by the gloo tests): in-place merge of every rank's by-label partials.
       sum / avg / count : val and cnt are added                       (commutativity.rs:85-113)
-      min / max         : groups absent on a rank (cnt == 0) are neutral (+inf / -inf), val is reduced with
-                          min / max, cnt is added, groups absent everywhere read 0.0 again
+      min / max         : val is reduced as f64::total_cmp keys (int64 min / max), the order of the single-pass
+                          aggregate (+NaN greatest, -NaN least, -0.0 < +0.0); groups absent on a rank (cnt == 0) get
+                          the neutral key, cnt is added, groups absent everywhere read 0.0 again
       stddev / stdvar   : per-rank (cnt, mean, M2 = val) states; global mean from an all-reduce of cnt * mean,
                           M2 = sum_r [M2_r + cnt_r (mean_r - mean)^2]  (commutativity.rs:158-191)"""
     import torch
     import torch.distributed as dist
     cnt64 = cnt_t.to(torch.int64)
     if agg in ("min", "max"):
-        neutral = float("inf") if agg == "min" else float("-inf")
-        val_t[cnt64 == 0] = neutral
-        dist.all_reduce(val_t, op=dist.ReduceOp.MIN if agg == "min" else dist.ReduceOp.MAX, group=group)
+        key = total_key(val_t.contiguous())
+        key[cnt64 == 0] = torch.iinfo(torch.int64).max if agg == "min" else torch.iinfo(torch.int64).min
+        dist.all_reduce(key, op=dist.ReduceOp.MIN if agg == "min" else dist.ReduceOp.MAX, group=group)
         dist.all_reduce(cnt64, op=dist.ReduceOp.SUM, group=group)
+        val_t.copy_(total_key(key).view(torch.float64))
         val_t[cnt64 == 0] = 0.0
     elif agg in ("stddev", "stdvar"):
         cnt_r = cnt64.clone()

@@ -68,6 +68,31 @@ def pack_series(series_dict):
             np.array(offsets, np.uint64))
 
 
+# Members whose order under f64::total_cmp differs from IEEE min / max: NaN of both signs (one with a payload), the two
+# zeros, and ordinary values around them.
+SPECIALS = np.array([0x7FF8000000000000, 0xFFF8000000000000, 0x7FF8000000000123, 0x8000000000000000, 0x0000000000000000,
+                     0x4008000000000000, 0xC008000000000000, 0x7FF0000000000000, 0xFFF0000000000000],
+                    dtype=np.uint64).view(np.float64)   # +NaN, -NaN, +NaN payload, -0.0, +0.0, 3.0, -3.0, +inf, -inf
+
+
+def total_order_case():
+    """One group per ordered pair of SPECIALS, its first member in the first half of the series and its second in the
+    second half (one half per rank or shard, so every placement order occurs), at T = 3 steps: both members valid at
+    step 0, only the first-half member at step 1, none at step 2.
+    -> (vals [2G x T], valid words [2G x 1], gid [2G], G); rows 0..G-1 are the first half, rows G..2G-1 the second."""
+    pairs = [(a, b) for a in range(SPECIALS.size) for b in range(SPECIALS.size)]
+    G, T = len(pairs), 3
+    vals = np.zeros((2 * G, T))
+    valid = np.zeros((2 * G, 1), np.uint32)
+    for g, (a, b) in enumerate(pairs):
+        vals[g, :] = SPECIALS[a]
+        vals[G + g, :] = SPECIALS[b]
+        valid[g, 0] = 0b011
+        valid[G + g, 0] = 0b001
+    gid = np.concatenate([np.arange(G), np.arange(G)]).astype(np.uint32)
+    return vals, valid, gid, G
+
+
 def promql_series(spec):
     """Prometheus test-series notation 'a+bxN a-bxN ...' (double_exponential_smoothing.rs:466-494)."""
     out = []

@@ -52,6 +52,7 @@ def main():
     for tiles in (1, 3):
         gsum = torch.zeros(G * T, dtype=torch.float64, device=dev)
         gcnt = torch.zeros(G * T, dtype=torch.int32, device=dev)
+        torch.cuda.synchronize()   # the library runs on its own stream: the zero fills must land first
         ctx.range_group_sum_allreduce_dev(p, d_ts, d_val, d_off, rows.size, ns, ix, tiles, gsum, gcnt)
         ctx.sync()
         got, cnt = gsum.cpu().numpy().reshape(G, T), gcnt.cpu().numpy().view(np.uint32).reshape(G, T)
@@ -72,6 +73,7 @@ def main():
         pc = torch.zeros(G * T, dtype=torch.int32, device=dev)
         pm = torch.zeros(G * T, dtype=torch.float64, device=dev)
         var = agg in ("stddev", "stdvar")
+        torch.cuda.synchronize()   # the library runs on its own stream: the zero fills must land first
         ctx.group_aggregate_partial_dev(agg, out, valid, d_gid, ns, G, T, pv, pc, pm if var else None)
         ctx.allreduce_partials_dev(agg, pv, pc, pm if var else None, G * T)
         if agg in ("stddev", "stdvar", "avg"):
@@ -86,6 +88,29 @@ def main():
             err = np.abs(got[m] - e_val[m])
             bad = (err > 1e-9 * np.maximum(np.abs(e_val[m]), 1e-300)) & (err > 1e-9 * scale)
             ok = ok and not bool(bad.any())
+
+    # min / max in the total order: NaN (both signs, with a payload) and +-0.0 members of one group on ranks 0 and 1 in
+    # every placement order, groups absent on one rank or everywhere; other ranks hold no member.  Bit for bit.
+    from tests.helpers import total_order_case
+    tv, tvalid, tgid, TG = total_order_case()
+    mine = slice(rank * TG, (rank + 1) * TG) if rank < 2 else slice(0, 0)
+    n_mine = mine.stop - mine.start
+    TT = tv.shape[1]
+    d_tv = torch.from_numpy(np.ascontiguousarray(tv[mine]) if n_mine else np.zeros((1, TT))).to(dev)
+    d_tvalid = torch.from_numpy((tvalid[mine] if n_mine else np.zeros((1, 1), np.uint32)).astype(np.int32)).to(dev)
+    d_tgid = torch.from_numpy((tgid[mine] if n_mine else np.zeros(1, np.uint32)).astype(np.int32)).to(dev)
+    torch.cuda.synchronize()
+    for agg in ("min", "max"):
+        e_val, e_c = orc.group_aggregate(agg, tv, tvalid, tgid, TG)
+        pv = torch.zeros(TG * TT, dtype=torch.float64, device=dev)
+        pc = torch.zeros(TG * TT, dtype=torch.int32, device=dev)
+        torch.cuda.synchronize()   # the library runs on its own stream: the zero fills must land first
+        if n_mine:
+            ctx.group_aggregate_partial_dev(agg, d_tv, d_tvalid, d_tgid, n_mine, TG, TT, pv, pc, None)
+        ctx.allreduce_partials_dev(agg, pv, pc, None, TG * TT)
+        ctx.sync()
+        got, cnt = pv.cpu().numpy().reshape(TG, TT), pc.cpu().numpy().view(np.uint32).reshape(TG, TT)
+        ok = ok and bool((cnt == e_c).all()) and bool((got.view(np.uint64) == e_val.view(np.uint64)).all())
     ctx.comm_destroy()
     ctx.close()
     verdict = torch.tensor([1.0 if (ok and worst <= 1e-9) else 0.0], device=dev)

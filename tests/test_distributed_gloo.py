@@ -78,18 +78,59 @@ def _worker(rank, world, port, q):
     dist.destroy_process_group()
 
 
-def test_sharded_partials_allreduce_equals_unsharded():
-    world = 2
+def _run(target, world=2):
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
+    procs = [ctx.Process(target=target, args=(r, world, port, q)) for r in range(world)]
     for p in procs:
         p.start()
     results = [q.get(timeout=240) for _ in range(world)]
     for p in procs:
         p.join(timeout=60)
         assert p.exitcode == 0
+    return results
+
+
+def _worker_total_order(rank, world, port, q):
+    sys.path.insert(0, ROOT)
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    from greptimedb_b200 import distributed as D
+    from oracle import oracle as orc
+    from tests.helpers import total_order_case
+    vals, valid, gid, G = total_order_case()
+    mine = slice(rank * G, (rank + 1) * G)
+    bad = []
+    for agg in ("min", "max"):
+        e_val, e_cnt = orc.group_aggregate(agg, vals, valid, gid, G)
+        pv, pc = orc.group_aggregate(agg, vals[mine], valid[mine], gid[mine], G)
+        vt, ct = torch.from_numpy(pv.copy()), torch.from_numpy(pc.astype(np.int64))
+        D.merge_partials(agg, vt, ct)
+        got = vt.numpy()
+        if not (ct.numpy() == e_cnt).all():
+            bad.append(f"{agg}: counts differ")
+        diff = np.argwhere(got.view(np.uint64) != e_val.view(np.uint64))
+        for g, k in diff[:4]:
+            bad.append(f"{agg} group {g} step {k}: merged {got[g, k]!r} ({got[g, k:k + 1].view(np.uint64)[0]:#x}), "
+                       f"single pass {e_val[g, k]!r} ({e_val[g, k:k + 1].view(np.uint64)[0]:#x})")
+    q.put((not bad, "; ".join(bad), 0))
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+def test_min_max_merge_follows_the_total_order_across_ranks():
+    """NaN (both signs, with and without payload), -0.0 and +0.0 members of one group on different ranks, in every
+    placement order: the merged min / max equals the single-pass total-order aggregate bit for bit, and a group absent on
+    one rank or on both merges like the single pass too (the neutral element, then 0.0)."""
+    for ok, msg, _ in _run(_worker_total_order):
+        assert ok, msg
+
+
+def test_sharded_partials_allreduce_equals_unsharded():
+    world = 2
+    results = _run(_worker, world)
     assert all(r[0] for r in results)
     assert max(r[1] for r in results) <= 1e-9          # summation order differs across shards: 1e-9 rel, like the reference
     assert sum(r[2] for r in results) == 96              # every series owned exactly once
