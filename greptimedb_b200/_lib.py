@@ -23,8 +23,9 @@ EXPORTED_SYMBOLS = [
     "b2p_range_group_sum_allreduce_dev", "b2p_allreduce_columns_dev", "b2p_histogram_fold_dev", "b2p_range_histogram_fold",
     "b2p_column_reduce_dev", "b2p_host_scan_series", "b2p_range_eval", "b2p_range_udf", "b2p_instant_select", "b2p_group_aggregate",
     "b2p_histogram_quantile", "b2p_synth_fill_dev",
+    "b2p_binary_op_dev", "b2p_scalar_op_dev", "b2p_count_valid_words_dev", "b2p_binary_op", "b2p_scalar_op",
     "b2p_plan_range_create", "b2p_plan_set_instant", "b2p_plan_set_histogram_quantile", "b2p_plan_push_batch", "b2p_plan_execute", "b2p_plan_num_series", "b2p_plan_destroy",
-    "b2p_plan_last_error",
+    "b2p_plan_last_error", "b2p_plan_set_scalar_op", "b2p_plan_binary_create",
 ]
 
 
@@ -98,6 +99,11 @@ def load() -> C.CDLL:
         "b2p_group_aggregate": (C.c_int, [vp, i32, vp, vp, vp, u32, u32, u64, vp, vp]),
         "b2p_histogram_quantile": (C.c_int, [vp, dbl, vp, u32, vp, vp, u32, u64, vp, vp]),
         "b2p_synth_fill_dev": (C.c_int, [vp, u64, u64, u32, i64, i64, u32, i32, u64, vp, vp, vp]),
+        "b2p_binary_op_dev": (C.c_int, [vp, i32, i32, vp, vp, vp, u32, vp, vp, vp, u32, u64, u64, vp, vp]),
+        "b2p_scalar_op_dev": (C.c_int, [vp, i32, i32, i32, dbl, vp, vp, u64, u64, vp, vp]),
+        "b2p_count_valid_words_dev": (C.c_int, [vp, vp, u64, u64, vp]),
+        "b2p_binary_op": (C.c_int, [vp, i32, i32, vp, vp, vp, u32, vp, vp, vp, u32, u64, u64, vp, vp]),
+        "b2p_scalar_op": (C.c_int, [vp, i32, i32, i32, dbl, vp, vp, u64, u64, vp, vp]),
         "b2p_plan_range_create": (vp, [vp, C.c_char_p, P, C.c_char_p, C.c_char_p, C.POINTER(C.c_char_p), i32, C.c_char_p,
                                        C.POINTER(C.c_char_p), i32]),
         "b2p_plan_set_instant": (C.c_int, [vp, i64]),
@@ -107,6 +113,8 @@ def load() -> C.CDLL:
         "b2p_plan_num_series": (i64, [vp]),
         "b2p_plan_destroy": (None, [vp]),
         "b2p_plan_last_error": (C.c_char_p, []),
+        "b2p_plan_set_scalar_op": (C.c_int, [vp, i32, dbl, i32, i32]),
+        "b2p_plan_binary_create": (vp, [vp, i32, i32, vp, vp, C.c_char_p, C.POINTER(C.c_char_p), i32, C.c_char_p]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)  # AttributeError here means the .so does not match the header

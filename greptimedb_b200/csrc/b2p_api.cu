@@ -20,6 +20,7 @@
 
 #include "../../include/b200promql.h"
 #include "b2p_aggregate.cuh"
+#include "b2p_binary.cuh"
 #include "b2p_kernel_t.cuh"
 #include "b2p_kernel_lean.cuh"
 #include "b2p_kernels.cuh"
@@ -130,6 +131,13 @@ constexpr int kSlowCtas = 132;        // slow-path grid (4 warps per CTA): one C
 constexpr int kSlowWarps = kSlowCtas * 4;
 constexpr size_t kArenaDefaultRows = 1u << 21;  // 32 MB: regions of 3 971 rows for the 528 slow-path warps
 
+// error of a non-zero Status::k0_errors word
+int k0_fail(uint32_t k0) {
+  if (k0 & kBinRowError) return fail(B2P_E_INVALID, "binary operator: a pair's row index is out of range");
+  if (k0 & 1u) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");
+  return fail(B2P_E_UNSORTED, "series id >= n_series");
+}
+
 }  // namespace
 
 // group -> member-series CSR of one gid[] assignment (b2p_group_index_create_dev), reusable across calls
@@ -219,6 +227,8 @@ struct b2p_ctx {
   DevBuf g_keys_in, g_keys_out, g_vals_in, g_vals_out, g_goff, g_tmp;
   // column reduce scratch
   DevBuf c_psum, c_pcnt;
+  // host-API staging of the binary operators: lhs, lhs validity, lhs rows, rhs, rhs validity, rhs rows, out, out validity
+  DevBuf bin[8];
   int fast_blocks_per_sm[B2P_FN__COUNT][2] = {};
   int big_blocks_per_sm[B2P_FN__COUNT] = {};
 };
@@ -557,6 +567,63 @@ int ensure_slow_scratch(b2p_ctx* c, uint32_t n_series, int64_t T) {
   return B2P_OK;
 }
 
+// ---- binary operators: OP / MODE / FORM are template arguments, chosen here once per call ----------------------------
+template <int OP, int MODE, int FORM>
+int launch_binary(b2p_ctx* c, const BinaryArgs& a, bool vec) {
+  const uint64_t steps = vec ? 64 : 32;
+  const uint64_t units = a.n_pairs * ((a.T + steps - 1) / steps);
+  uint64_t blocks = (units + 7) / 8;  // 8 warps per CTA, one unit each, grid-stride beyond the cap
+  const uint64_t cap = (uint64_t)c->num_sms * 16;
+  if (blocks > cap) blocks = cap;
+  if (blocks == 0) return B2P_OK;
+  if (vec) binary_op_kernel<OP, MODE, FORM, true><<<(unsigned)blocks, 256, 0, c->stream>>>(a);
+  else binary_op_kernel<OP, MODE, FORM, false><<<(unsigned)blocks, 256, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+template <int FORM>
+int dispatch_binary(b2p_ctx* c, int op, bool return_bool, const BinaryArgs& a, bool vec) {
+#define B2P_CMP_CASE(OPV)                                                                                \
+  case OPV:                                                                                              \
+    return return_bool ? launch_binary<OPV, kBool, FORM>(c, a, vec) : launch_binary<OPV, kFilter, FORM>(c, a, vec);
+  switch (op) {
+    case kOpAdd: return launch_binary<kOpAdd, kArith, FORM>(c, a, vec);
+    case kOpSub: return launch_binary<kOpSub, kArith, FORM>(c, a, vec);
+    case kOpMul: return launch_binary<kOpMul, kArith, FORM>(c, a, vec);
+    case kOpDiv: return launch_binary<kOpDiv, kArith, FORM>(c, a, vec);
+    case kOpMod: return launch_binary<kOpMod, kArith, FORM>(c, a, vec);
+    case kOpPow: return launch_binary<kOpPow, kArith, FORM>(c, a, vec);
+    case kOpAtan2: return launch_binary<kOpAtan2, kArith, FORM>(c, a, vec);
+    B2P_CMP_CASE(kOpEq)
+    B2P_CMP_CASE(kOpNe)
+    B2P_CMP_CASE(kOpGt)
+    B2P_CMP_CASE(kOpLt)
+    B2P_CMP_CASE(kOpGe)
+    B2P_CMP_CASE(kOpLe)
+    default: return fail(B2P_E_INVALID, "unknown binary operator %d", op);
+  }
+#undef B2P_CMP_CASE
+}
+
+int check_binop(int32_t op, int32_t return_bool) {
+  if (op < 0 || op >= kOpCount) return fail(B2P_E_INVALID, "unknown binary operator %d", op);
+  if (return_bool && op < kOpEq) return fail(B2P_E_INVALID, "the bool modifier needs a comparison operator, got %d", op);
+  return B2P_OK;
+}
+
+// clears bit kBinRowError of the status word after a synchronous call has read it; B2P_E_INVALID when it was set
+int take_bin_row_error(b2p_ctx* c) {
+  CU(cudaMemcpyAsync(c->h_k0, c->d_k0, sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  const uint32_t k0 = c->h_k0->k0_errors;
+  if (!(k0 & kBinRowError)) return B2P_OK;
+  const uint32_t rest = k0 & ~kBinRowError;
+  CU(cudaMemcpy(&c->d_k0->k0_errors, &rest, sizeof rest, cudaMemcpyHostToDevice));
+  return k0_fail(kBinRowError);
+}
+
 }  // namespace
 
 extern "C" {
@@ -652,6 +719,7 @@ void b2p_destroy(b2p_ctx* c) {
     if (c->ev_d2h[i]) cudaEventDestroy(c->ev_d2h[i]);
   }
   c->p_status.release();
+  for (DevBuf& b : c->bin) b.release();
   if (c->s_h2d) cudaStreamDestroy(c->s_h2d);
   if (c->s_d2h) cudaStreamDestroy(c->s_d2h);
   if (c->d_ring) cudaFree(c->d_ring);
@@ -741,8 +809,7 @@ int b2p_sync(b2p_ctx* c) {
     if (k0) {
       CU(cudaMemsetAsync(c->d_k0, 0, sizeof(Status), c->stream));
       c->pending.clear();
-      if (k0 & 1u) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");
-      return fail(B2P_E_UNSORTED, "series id >= n_series");
+      return k0_fail(k0);
     }
     // verdicts of the outstanding range calls, oldest first; a call whose slow path ran out of arena is redone
     // as a whole (all tiers, same modes) after the arena has grown to what the largest of them needs
@@ -1470,6 +1537,65 @@ int b2p_column_reduce_dev(b2p_ctx* c, const double* const* cols, uint32_t n_cols
   return B2P_OK;
 }
 
+/* ---- binary operators ---------------------------------------------------------------------------------------- */
+int b2p_binary_op_dev(b2p_ctx* c, int32_t op, int32_t return_bool, const double* lhs, const uint32_t* lhs_valid,
+                      const uint32_t* lhs_row, uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid,
+                      const uint32_t* rhs_row, uint32_t n_rhs_rows, uint64_t n_pairs, uint64_t T, double* out,
+                      uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int rc;
+  if ((rc = check_binop(op, return_bool))) return rc;
+  if (n_pairs == 0 || T == 0) return B2P_OK;
+  if (!lhs_row || !rhs_row || !out || !out_valid || (n_lhs_rows && (!lhs || !lhs_valid)) ||
+      (n_rhs_rows && (!rhs || !rhs_valid)))
+    return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  BinaryArgs a{};
+  a.lhs = lhs; a.lvalid = lhs_valid; a.lrow = lhs_row; a.n_lhs = n_lhs_rows;
+  a.rhs = rhs; a.rvalid = rhs_valid; a.rrow = rhs_row; a.n_rhs = n_rhs_rows;
+  a.n_pairs = n_pairs; a.T = T; a.Tw = (uint32_t)((T + 31) / 32); a.out = out; a.out_valid = out_valid; a.status = c->d_k0;
+  const bool vec = (T % 2) == 0 && aligned16(lhs) && aligned16(rhs) && aligned16(out);
+  stage_begin(c, 3);
+  rc = dispatch_binary<kVecVec>(c, op, return_bool != 0, a, vec);
+  stage_end(c, 3);
+  return rc;
+}
+
+int b2p_scalar_op_dev(b2p_ctx* c, int32_t op, int32_t return_bool, int32_t scalar_on_left, double scalar,
+                      const double* vals, const uint32_t* valid, uint64_t n_rows, uint64_t T, double* out,
+                      uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int rc;
+  if ((rc = check_binop(op, return_bool))) return rc;
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !out || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  BinaryArgs a{};
+  a.lhs = vals; a.lvalid = valid; a.scalar = scalar;
+  a.n_pairs = n_rows; a.T = T; a.Tw = (uint32_t)((T + 31) / 32); a.out = out; a.out_valid = out_valid; a.status = c->d_k0;
+  const bool vec = (T % 2) == 0 && aligned16(vals) && aligned16(out);
+  stage_begin(c, 3);
+  rc = scalar_on_left ? dispatch_binary<kScalarLeft>(c, op, return_bool != 0, a, vec)
+                      : dispatch_binary<kScalarRight>(c, op, return_bool != 0, a, vec);
+  stage_end(c, 3);
+  return rc;
+}
+
+int b2p_count_valid_words_dev(b2p_ctx* c, const uint32_t* cnt, uint64_t n_rows, uint64_t T, uint32_t* valid_words) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!cnt || !valid_words) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  uint64_t blocks = (n_rows * Tw + 7) / 8;
+  const uint64_t cap = (uint64_t)c->num_sms * 16;
+  if (blocks > cap) blocks = cap;
+  count_valid_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(cnt, n_rows, T, Tw, valid_words);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
 int b2p_synth_fill_dev(b2p_ctx* c, uint64_t series_begin, uint64_t n_series, uint32_t n_samples, int64_t t0,
                        int64_t scrape_ms, uint32_t jitter_ms, int32_t with_resets, uint64_t seed, int64_t* ts,
                        double* val, uint32_t* sid) {
@@ -1789,8 +1915,7 @@ int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, con
   CU(cudaStreamSynchronize(c->s_d2h));
   if (const uint32_t k0 = c->h_k0->k0_errors) {
     CU(cudaMemsetAsync(c->d_k0, 0, sizeof(Status), c->stream));
-    if (k0 & 1u) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");
-    return fail(B2P_E_UNSORTED, "series id >= n_series");
+    return k0_fail(k0);
   }
   // per-chunk verdicts; a chunk whose slow path ran out of arena is redone alone (b2p_sync grows the arena)
   long long slow_total = 0, w_total = 0;
@@ -1995,6 +2120,57 @@ int b2p_range_histogram_fold(b2p_ctx* c, const b2p_range_params* p, const int64_
     return rc;
   CU(cudaMemcpyAsync(out, c->h_aux2.p, (size_t)n_hist * (size_t)T * 8, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaMemcpyAsync(out_valid_words, c->h_aux3.p, (size_t)n_hist * Tw * 4, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return B2P_OK;
+}
+
+int b2p_binary_op(b2p_ctx* c, int32_t op, int32_t return_bool, const double* lhs, const uint32_t* lhs_valid,
+                  const uint32_t* lhs_row, uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid,
+                  const uint32_t* rhs_row, uint32_t n_rhs_rows, uint64_t n_pairs, uint64_t T, double* out,
+                  uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int rc;
+  if ((rc = check_binop(op, return_bool))) return rc;
+  if (n_pairs == 0 || T == 0) return B2P_OK;
+  if (!lhs_row || !rhs_row || !out || !out_valid || (n_lhs_rows && (!lhs || !lhs_valid)) ||
+      (n_rhs_rows && (!rhs || !rhs_valid)))
+    return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  const size_t nl = n_lhs_rows, nr = n_rhs_rows, np = (size_t)n_pairs;
+  const size_t bytes[8] = {nl * T * 8, nl * Tw * 4, np * 4, nr * T * 8, nr * Tw * 4, np * 4, np * T * 8, np * Tw * 4};
+  for (int i = 0; i < 8; ++i)
+    if ((rc = c->bin[i].ensure(bytes[i] ? bytes[i] : 16))) return rc;
+  const void* src[6] = {lhs, lhs_valid, lhs_row, rhs, rhs_valid, rhs_row};
+  for (int i = 0; i < 6; ++i)
+    if (bytes[i]) CU(cudaMemcpyAsync(c->bin[i].p, src[i], bytes[i], cudaMemcpyHostToDevice, c->stream));
+  if ((rc = b2p_binary_op_dev(c, op, return_bool, c->bin[0].as<double>(), c->bin[1].as<uint32_t>(), c->bin[2].as<uint32_t>(),
+                              n_lhs_rows, c->bin[3].as<double>(), c->bin[4].as<uint32_t>(), c->bin[5].as<uint32_t>(),
+                              n_rhs_rows, n_pairs, T, c->bin[6].as<double>(), c->bin[7].as<uint32_t>())))
+    return rc;
+  CU(cudaMemcpyAsync(out, c->bin[6].p, bytes[6], cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaMemcpyAsync(out_valid, c->bin[7].p, bytes[7], cudaMemcpyDeviceToHost, c->stream));
+  return take_bin_row_error(c);  // (synchronises)
+}
+
+int b2p_scalar_op(b2p_ctx* c, int32_t op, int32_t return_bool, int32_t scalar_on_left, double scalar, const double* vals,
+                  const uint32_t* valid, uint64_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int rc;
+  if ((rc = check_binop(op, return_bool))) return rc;
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !out || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  const size_t vb = (size_t)n_rows * T * 8, wb = (size_t)n_rows * Tw * 4;
+  if ((rc = c->bin[6].ensure(vb)) || (rc = c->bin[7].ensure(wb))) return rc;
+  CU(cudaMemcpyAsync(c->bin[6].p, vals, vb, cudaMemcpyHostToDevice, c->stream));
+  CU(cudaMemcpyAsync(c->bin[7].p, valid, wb, cudaMemcpyHostToDevice, c->stream));
+  if ((rc = b2p_scalar_op_dev(c, op, return_bool, scalar_on_left, scalar, c->bin[6].as<double>(), c->bin[7].as<uint32_t>(),
+                              n_rows, T, c->bin[6].as<double>(), c->bin[7].as<uint32_t>())))  // in place
+    return rc;
+  CU(cudaMemcpyAsync(out, c->bin[6].p, vb, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaMemcpyAsync(out_valid, c->bin[7].p, wb, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   return B2P_OK;
 }

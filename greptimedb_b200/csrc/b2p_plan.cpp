@@ -163,7 +163,7 @@ int RecordBatch::find(const std::string& name) const {
 }
 
 // ---- PromRangePlan -------------------------------------------------------------------------------------
-PromRangePlan::PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args) : ctx_(ctx), args_(std::move(args)) {
+PromRangePlan::PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args) : PlanNode(ctx), args_(std::move(args)) {
   if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromRangeExec: NULL context");
   fn_id_ = args_.function.empty() ? -1 : function_id_from_name(args_.function);
   if (fn_id_ < 0 && !args_.function.empty())
@@ -315,8 +315,7 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
   have_last_ = true;
 }
 
-void PromRangePlan::execute(ArrowArray* out, ArrowSchema* out_schema) {
-  if (!out || !out_schema) throw PlanError(ErrorKind::Internal, "execute: NULL output structs");
+void PromRangePlan::compute(NodeResult& r) {
   b2p_range_params p{};
   p.fn_id = fn_id_;
   p.filter_nan = args_.need_filter_out_nan ? 1 : 0;
@@ -350,18 +349,12 @@ void PromRangePlan::execute(ArrowArray* out, ArrowSchema* out_schema) {
     if (rc == B2P_E_UNSORTED) throw PlanError(ErrorKind::Internal, b2p_last_error());
     if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
   }
-  const std::string value_name =
+  r = NodeResult();
+  r.T = T;
+  r.Tw = Tw;
+  r.time_index = args_.time_index;
+  r.value_name =
       fn_id_ >= 0 ? args_.function + "(" + args_.time_index + "_range," + args_.field_column + ")" : args_.field_column;
-
-  auto ob = std::make_unique<OwnedBatch>();
-  auto os = std::make_unique<OwnedSchema>();
-  auto add_col = [&](const std::string& name, const std::string& fmt) -> OwnedColumn* {
-    ob->cols.push_back(std::make_unique<OwnedColumn>());
-    os->names.push_back(name);
-    os->formats.push_back(fmt);
-    return ob->cols.back().get();
-  };
-  int64_t n_out = 0;
 
   if (args_.histogram) {
     // HistogramFold (histogram_fold.rs:754-820): group the series by their tags without `le`, order each group's
@@ -399,7 +392,7 @@ void PromRangePlan::execute(ArrowArray* out, ArrowSchema* out_schema) {
     for (uint32_t h = 0; h < H; ++h) hist_order[h] = h;
     std::sort(hist_order.begin(), hist_order.end(), [&](uint32_t x, uint32_t y) { return hist_keys[x] < hist_keys[y]; });
     std::vector<uint32_t> rank(H);
-    for (uint32_t r = 0; r < H; ++r) rank[hist_order[r]] = r;
+    for (uint32_t q = 0; q < H; ++q) rank[hist_order[q]] = q;
     // buckets of every histogram in ascending le order, NaN bounds last, ties in scan order (a strict weak ordering)
     std::vector<uint32_t> bucket_series(S);
     for (uint32_t s = 0; s < S; ++s) bucket_series[s] = s;
@@ -416,63 +409,36 @@ void PromRangePlan::execute(ArrowArray* out, ArrowSchema* out_schema) {
       hist_off[rank[hid[bucket_series[i]]] + 1]++;
     }
     for (uint32_t h = 0; h < H; ++h) hist_off[h + 1] += hist_off[h];
-    std::vector<double> hq((size_t)H * (size_t)T);
-    std::vector<uint32_t> hqv((size_t)H * Tw);
+    r.val.assign((size_t)H * (size_t)T, 0.0);
+    r.valid.assign((size_t)H * Tw, 0u);
     if (H > 0 && T > 0) {
       if (fn_id_ < 0) throw PlanError(ErrorKind::Plan, "HistogramFold over an instant selector is not supported by this node");
       const int rc = b2p_range_histogram_fold(ctx_, &p, ts_.data(), val_.data(), nullptr, offsets_.data(), ts_.size(), S,
                                               args_.quantile, hist_off.data(), bucket_series.data(), bucket_le.data(), H,
-                                              hq.data(), hqv.data());
+                                              r.val.data(), r.valid.data());
       if (rc == B2P_E_INVALID || rc == B2P_E_TOO_LARGE) throw PlanError(ErrorKind::Plan, b2p_last_error());
       if (rc == B2P_E_UNSORTED) throw PlanError(ErrorKind::Internal, b2p_last_error());
       if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
       for (int64_t k = 0; k < T; ++k) eval_ts[(size_t)k] = p.start + k * p.interval;
     }
-    OwnedColumn* c_ts = add_col(args_.time_index, "tsm:");
-    OwnedColumn* c_val = add_col(value_name, "g");
-    std::vector<OwnedColumn*> c_tags;
+    // rows of histogram hist_order[h] (tag-sorted)
     for (size_t t = 0; t < args_.tag_columns.size(); ++t)
-      if (t != le_idx) {
-        c_tags.push_back(add_col(args_.tag_columns[t], "u"));
-        c_tags.back()->offsets.push_back(0);
-      }
-    for (uint32_t h = 0; h < H; ++h) {  // rows of histogram hist_order[h] (tag-sorted), one per eval step with a row
+      if (t != le_idx) r.tag_names.push_back(args_.tag_columns[t]);
+    r.tags.resize(r.tag_names.size());
+    for (uint32_t h = 0; h < H; ++h) {
       const std::vector<std::string>& key = hist_keys[hist_order[h]];
-      for (int64_t k = 0; k < T; ++k) {
-        if (!((hqv[(size_t)h * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u)) continue;
-        c_ts->i64.push_back(eval_ts[(size_t)k]);
-        c_val->f64.push_back(hq[(size_t)h * (size_t)T + (size_t)k]);
-        for (size_t t = 0; t < c_tags.size(); ++t) {
-          c_tags[t]->chars += key[t];
-          c_tags[t]->offsets.push_back((int32_t)c_tags[t]->chars.size());
-        }
-        ++n_out;
-      }
+      for (size_t t = 0; t < key.size(); ++t) r.tags[t].push_back(key[t]);
     }
+    r.rows = H;
   } else if (agg_id_ < 0) {
     // rows of Filter(prom_fn IS NOT NULL): {time_index (eval ts), prom_fn(...), tags...}, series-major order
-    OwnedColumn* c_ts = add_col(args_.time_index, "tsm:");
-    OwnedColumn* c_val = add_col(value_name, "g");
-    std::vector<OwnedColumn*> c_tags;
-    for (size_t t = 0; t < args_.tag_columns.size(); ++t) {
-      c_tags.push_back(add_col(args_.tag_columns[t], key_is_id_ ? "L" : "u"));
-      if (!key_is_id_) c_tags.back()->offsets.push_back(0);
-    }
-    for (uint32_t s = 0; s < S; ++s)
-      for (int64_t k = 0; k < T; ++k) {
-        if (!((valid[(size_t)s * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u)) continue;
-        c_ts->i64.push_back(eval_ts[(size_t)k]);
-        c_val->f64.push_back(dense[(size_t)s * (size_t)T + (size_t)k]);
-        for (size_t t = 0; t < c_tags.size(); ++t) {
-          if (key_is_id_) {
-            c_tags[t]->i64.push_back((int64_t)tags_.tsid[s]);
-          } else {
-            c_tags[t]->chars += tags_.utf8[t][s];
-            c_tags[t]->offsets.push_back((int32_t)c_tags[t]->chars.size());
-          }
-        }
-        ++n_out;
-      }
+    r.tag_names = args_.tag_columns;
+    r.id_keyed = key_is_id_;
+    if (key_is_id_) r.ids = tags_.tsid;
+    else r.tags = tags_.utf8;
+    r.val = std::move(dense);
+    r.valid = std::move(valid);
+    r.rows = S;
   } else {
     // prom_aggr_expr_to_plan: group keys = by-labels + eval ts; output sorted by (labels asc, ts asc)
     std::vector<size_t> by_idx;
@@ -496,27 +462,95 @@ void PromRangePlan::execute(ArrowArray* out, ArrowSchema* out_schema) {
                                          gval.data(), gcnt.data());
       if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
     }
-    std::vector<OwnedColumn*> c_by;
-    for (const auto& bname : args_.by_columns) {
-      c_by.push_back(add_col(bname, "u"));
-      c_by.back()->offsets.push_back(0);
-    }
-    OwnedColumn* c_ts = add_col(args_.time_index, "tsm:");
-    OwnedColumn* c_val = add_col(args_.aggregate + "(" + (fn_id_ >= 0 ? args_.function : args_.field_column) + ")", "g");
-    for (const auto& kv : groups) {  // std::map iterates in key order
+    // rows in key order (std::map iterates sorted); a group has a row at step k iff its count is non-zero
+    r.tag_names = args_.by_columns;
+    r.tags.resize(r.tag_names.size());
+    r.tags_first = true;
+    r.value_name = args_.aggregate + "(" + (fn_id_ >= 0 ? args_.function : args_.field_column) + ")";
+    r.val.assign((size_t)G * (size_t)T, 0.0);
+    r.valid.assign((size_t)G * Tw, 0u);
+    uint32_t row = 0;
+    for (const auto& kv : groups) {
       const uint32_t g = kv.second;
+      for (size_t b = 0; b < r.tags.size(); ++b) r.tags[b].push_back(kv.first[b]);
       for (int64_t k = 0; k < T; ++k) {
         if (gcnt[(size_t)g * (size_t)T + (size_t)k] == 0) continue;
-        for (size_t b = 0; b < c_by.size(); ++b) {
-          c_by[b]->chars += kv.first[b];
-          c_by[b]->offsets.push_back((int32_t)c_by[b]->chars.size());
-        }
-        c_ts->i64.push_back(eval_ts[(size_t)k]);
-        c_val->f64.push_back(gval[(size_t)g * (size_t)T + (size_t)k]);
-        ++n_out;
+        r.val[(size_t)row * (size_t)T + (size_t)k] = gval[(size_t)g * (size_t)T + (size_t)k];
+        r.valid[(size_t)row * Tw + (size_t)(k >> 5)] |= 1u << (k & 31);
       }
+      ++row;
     }
+    r.rows = G;
   }
+  r.eval_ts = std::move(eval_ts);
+}
+
+namespace {
+
+const char* const kOpSymbols[] = {"+", "-", "*", "/", "%", "^", "atan2", "==", "!=", ">", "<", ">=", "<="};
+
+bool is_comparison(int op) { return op >= B2P_OP_EQ && op <= B2P_OP_LE; }
+
+void check_op(int op, bool return_bool) {
+  if (op < B2P_OP_ADD || op > B2P_OP_LE) throw PlanError(ErrorKind::Plan, "unknown binary operator " + std::to_string(op));
+  if (return_bool && !is_comparison(op))
+    throw PlanError(ErrorKind::Plan, "bool modifier can only be used on comparison operators");
+}
+
+// a number literal as DataFusion displays it in a column name: Float64(100), Float64(0.5)
+std::string float_literal(double x) {
+  char buf[64];
+  const auto res = std::to_chars(buf, buf + sizeof buf, x);
+  return "Float64(" + std::string(buf, res.ptr) + ")";
+}
+
+// the key tuple of row r over the given tag columns, length-prefixed so that no two tuples share an encoding
+void append_key(const NodeResult& n, const std::vector<int>& cols, uint32_t r, std::string& key) {
+  key.clear();
+  for (int c : cols) {
+    const std::string v = n.id_keyed ? std::to_string(n.ids[r]) : n.tags[(size_t)c][r];
+    key += std::to_string(v.size());
+    key.push_back(':');
+    key += v;
+  }
+}
+
+void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema) {
+  auto ob = std::make_unique<OwnedBatch>();
+  auto os = std::make_unique<OwnedSchema>();
+  auto add_col = [&](const std::string& name, const std::string& fmt) -> OwnedColumn* {
+    ob->cols.push_back(std::make_unique<OwnedColumn>());
+    os->names.push_back(name);
+    os->formats.push_back(fmt);
+    return ob->cols.back().get();
+  };
+  std::vector<OwnedColumn*> c_tags;
+  auto add_tags = [&]() {
+    for (const auto& tn : r.tag_names) {
+      c_tags.push_back(add_col(tn, r.id_keyed ? "L" : "u"));
+      if (!r.id_keyed) c_tags.back()->offsets.push_back(0);
+    }
+  };
+  if (r.tags_first) add_tags();
+  OwnedColumn* c_ts = add_col(r.time_index, "tsm:");
+  OwnedColumn* c_val = add_col(r.value_name, "g");
+  if (!r.tags_first) add_tags();
+  int64_t n_out = 0;
+  for (uint32_t row = 0; row < r.rows; ++row)
+    for (int64_t k = 0; k < r.T; ++k) {
+      if (!r.valid_at(row, k)) continue;
+      c_ts->i64.push_back(r.eval_ts[(size_t)k]);
+      c_val->f64.push_back(r.val[(size_t)row * (size_t)r.T + (size_t)k]);
+      for (size_t t = 0; t < c_tags.size(); ++t) {
+        if (r.id_keyed) {
+          c_tags[t]->i64.push_back((int64_t)r.ids[row]);
+        } else {
+          c_tags[t]->chars += r.tags[t][row];
+          c_tags[t]->offsets.push_back((int32_t)c_tags[t]->chars.size());
+        }
+      }
+      ++n_out;
+    }
 
   // ---- wire up the Arrow C structs ------------------------------------------------------------------
   const size_t nc = ob->cols.size();
@@ -571,11 +605,138 @@ void PromRangePlan::execute(ArrowArray* out, ArrowSchema* out_schema) {
   out_schema->private_data = os.release();
 }
 
+}  // namespace
+
+// ---- PlanNode ------------------------------------------------------------------------------------------
+void PlanNode::add_scalar_op(int op, double scalar, bool scalar_on_left, bool return_bool) {
+  check_op(op, return_bool);
+  scalar_ops_.push_back(ScalarOp{op, scalar, scalar_on_left, return_bool});
+}
+
+void PlanNode::run(NodeResult& r) {
+  compute(r);
+  for (const ScalarOp& s : scalar_ops_) {
+    if (r.rows > 0 && r.T > 0) {
+      const int rc = b2p_scalar_op(ctx_, s.op, s.return_bool ? 1 : 0, s.scalar_on_left ? 1 : 0, s.scalar, r.val.data(),
+                                   r.valid.data(), r.rows, (uint64_t)r.T, r.val.data(), r.valid.data());
+      if (rc == B2P_E_INVALID) throw PlanError(ErrorKind::Plan, b2p_last_error());
+      if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
+    }
+    if (!is_comparison(s.op) || s.return_bool) {  // a projection names its expression; a filter keeps the column
+      const std::string lit = float_literal(s.scalar), sym = kOpSymbols[s.op];
+      r.value_name = s.scalar_on_left ? lit + " " + sym + " " + r.value_name : r.value_name + " " + sym + " " + lit;
+    }
+  }
+}
+
+void PlanNode::execute(ArrowArray* out, ArrowSchema* out_schema) {
+  if (!out || !out_schema) throw PlanError(ErrorKind::Internal, "execute: NULL output structs");
+  NodeResult r;
+  run(r);
+  export_result(r, out, out_schema);
+}
+
+// ---- BinaryPlan ----------------------------------------------------------------------------------------
+BinaryPlan::BinaryPlan(b2p_ctx* ctx, int op, bool return_bool, std::shared_ptr<PlanNode> lhs,
+                       std::shared_ptr<PlanNode> rhs, Matching matching, std::vector<std::string> labels,
+                       bool labels_from_lhs)
+    : PlanNode(ctx), op_(op), return_bool_(return_bool), lhs_(std::move(lhs)), rhs_(std::move(rhs)),
+      matching_(matching), labels_(std::move(labels)), labels_from_lhs_(labels_from_lhs) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromBinaryExec: NULL context");
+  if (!lhs_ || !rhs_) throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: NULL child");
+  check_op(op_, return_bool_);
+}
+
+void BinaryPlan::compute(NodeResult& r) {
+  NodeResult L, R;
+  lhs_->run(L);
+  rhs_->run(R);
+  if (L.T != R.T) throw PlanError(ErrorKind::Plan, "both sides of a binary operator must be evaluated on the same steps");
+  // join keys (planner.rs:696-729, 3436-3468): the rhs context's tag columns, narrowed by on / ignoring; none when a
+  // side has no tags (every row pairs with every row); two id-keyed sides without a modifier join on the id
+  std::vector<int> lcols, rcols;
+  const bool by_id = L.id_keyed && R.id_keyed && matching_ == Matching::None;
+  if (by_id) {
+    lcols.push_back(0);
+    rcols.push_back(0);
+  } else if (!L.tag_names.empty() && !R.tag_names.empty()) {
+    for (size_t t = 0; t < R.tag_names.size(); ++t) {
+      const std::string& name = R.tag_names[t];
+      const bool listed = std::find(labels_.begin(), labels_.end(), name) != labels_.end();
+      if (matching_ == Matching::On ? !listed : (matching_ == Matching::Ignoring && listed)) continue;
+      const auto li = std::find(L.tag_names.begin(), L.tag_names.end(), name);
+      if (li == L.tag_names.end()) throw PlanError(ErrorKind::Plan, "No field named " + name);
+      lcols.push_back((int)(li - L.tag_names.begin()));
+      rcols.push_back((int)t);
+    }
+  }
+  // hash join of the series: rhs rows by key (in row order), then every lhs row in order against its key's rhs rows
+  std::unordered_map<std::string, std::vector<uint32_t>> rhs_by_key;
+  std::string key;
+  rhs_by_key.reserve(R.rows);
+  for (uint32_t q = 0; q < R.rows; ++q) {
+    append_key(R, rcols, q, key);
+    rhs_by_key[key].push_back(q);
+  }
+  std::vector<uint32_t> lrow, rrow;
+  for (uint32_t q = 0; q < L.rows; ++q) {
+    append_key(L, lcols, q, key);
+    const auto it = rhs_by_key.find(key);
+    if (it == rhs_by_key.end()) continue;
+    for (uint32_t m : it->second) {
+      lrow.push_back(q);
+      rrow.push_back(m);
+    }
+  }
+  const uint64_t n_pairs = lrow.size();
+  if (n_pairs > UINT32_MAX) throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: more than 2^32 - 1 matched series pairs");
+  r = NodeResult();
+  r.T = L.T;
+  r.Tw = L.Tw;
+  r.rows = (uint32_t)n_pairs;
+  r.eval_ts = L.eval_ts;
+  r.val.assign((size_t)n_pairs * (size_t)r.T, 0.0);
+  r.valid.assign((size_t)n_pairs * r.Tw, 0u);
+  if (n_pairs > 0 && r.T > 0) {
+    const int rc = b2p_binary_op(ctx_, op_, return_bool_ ? 1 : 0, L.val.data(), L.valid.data(), lrow.data(), L.rows,
+                                 R.val.data(), R.valid.data(), rrow.data(), R.rows, n_pairs, (uint64_t)r.T,
+                                 r.val.data(), r.valid.data());
+    if (rc == B2P_E_INVALID) throw PlanError(ErrorKind::Plan, b2p_last_error());
+    if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
+  }
+  // output labels: a filter passes the lhs rows through; a projection emits the tag columns of `label_side`
+  const bool filter = is_comparison(op_) && !return_bool_;
+  const bool from_lhs = filter || labels_from_lhs_;
+  const NodeResult& side = from_lhs ? L : R;
+  const std::vector<uint32_t>& srow = from_lhs ? lrow : rrow;
+  r.time_index = side.time_index;
+  r.tag_names = side.tag_names;
+  r.id_keyed = side.id_keyed;
+  if (side.id_keyed) {
+    r.ids.resize(n_pairs);
+    for (uint64_t p = 0; p < n_pairs; ++p) r.ids[p] = side.ids[srow[p]];
+  } else {
+    r.tags.resize(side.tags.size());
+    for (size_t t = 0; t < side.tags.size(); ++t) {
+      r.tags[t].resize(n_pairs);
+      for (uint64_t p = 0; p < n_pairs; ++p) r.tags[t][p] = side.tags[t][srow[p]];
+    }
+  }
+  if (filter) {
+    r.tags_first = L.tags_first;
+    r.value_name = L.value_name;
+  } else {
+    r.tags_first = true;
+    r.value_name = L.value_name + " " + kOpSymbols[op_] + " " + R.value_name;
+  }
+}
+
 }  // namespace b2p
 
 // ---- C entry points -----------------------------------------------------------------------------------
 struct b2p_plan {
-  std::unique_ptr<b2p::PromRangePlan> plan;
+  std::shared_ptr<b2p::PlanNode> node;  // shared with the binary nodes built on top of it
+  b2p::PromRangePlan* range() const { return dynamic_cast<b2p::PromRangePlan*>(node.get()); }
 };
 
 namespace {
@@ -587,6 +748,10 @@ int plan_fail(const b2p::PlanError& e) {
     case b2p::ErrorKind::Internal: return B2P_E_UNSORTED;
     default: return B2P_E_CUDA;
   }
+}
+int not_a_range_node() {
+  g_err = "this call needs a range / instant node (b2p_plan_range_create)";
+  return B2P_E_INVALID;
 }
 }  // namespace
 
@@ -615,7 +780,38 @@ b2p_plan* b2p_plan_range_create(b2p_ctx* ctx, const char* function, const b2p_ra
     if (aggregate && aggregate[0]) a.aggregate = aggregate;
     for (int32_t i = 0; i < n_by; ++i) a.by_columns.emplace_back(by_columns[i]);
     auto* h = new b2p_plan();
-    h->plan = std::make_unique<b2p::PromRangePlan>(ctx, std::move(a));
+    h->node = std::make_shared<b2p::PromRangePlan>(ctx, std::move(a));
+    return h;
+  } catch (const b2p::PlanError& e) {
+    plan_fail(e);
+  } catch (const std::exception& e) {
+    g_err = e.what();
+  }
+  return nullptr;
+}
+
+b2p_plan* b2p_plan_binary_create(b2p_ctx* ctx, int32_t op, int32_t return_bool, b2p_plan* lhs, b2p_plan* rhs,
+                                 const char* matching, const char* const* labels, int32_t n_labels,
+                                 const char* label_side) {
+  try {
+    if (!lhs || !rhs || !label_side || (n_labels > 0 && !labels))
+      throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    b2p::BinaryPlan::Matching m = b2p::BinaryPlan::Matching::None;
+    if (matching && std::strcmp(matching, "on") == 0) m = b2p::BinaryPlan::Matching::On;
+    else if (matching && std::strcmp(matching, "ignoring") == 0) m = b2p::BinaryPlan::Matching::Ignoring;
+    else if (matching && matching[0]) throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("unknown matching ") + matching);
+    const bool from_lhs = std::strcmp(label_side, "lhs") == 0;
+    if (!from_lhs && std::strcmp(label_side, "rhs") != 0)
+      throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("label_side must be \"lhs\" or \"rhs\", got ") + label_side);
+    std::vector<std::string> ls;
+    for (int32_t i = 0; i < n_labels; ++i) ls.emplace_back(labels[i]);
+    auto* h = new b2p_plan();
+    try {
+      h->node = std::make_shared<b2p::BinaryPlan>(ctx, op, return_bool != 0, lhs->node, rhs->node, m, std::move(ls), from_lhs);
+    } catch (...) {
+      delete h;
+      throw;
+    }
     return h;
   } catch (const b2p::PlanError& e) {
     plan_fail(e);
@@ -627,13 +823,25 @@ b2p_plan* b2p_plan_range_create(b2p_ctx* ctx, const char* function, const b2p_ra
 
 int b2p_plan_set_instant(b2p_plan* plan, int64_t lookback_delta) {
   if (!plan) return B2P_E_INVALID;
-  return plan->plan->set_instant(lookback_delta);
+  if (!plan->range()) return not_a_range_node();
+  return plan->range()->set_instant(lookback_delta);
 }
 
 int b2p_plan_set_histogram_quantile(b2p_plan* plan, const char* le_column, double quantile) {
   if (!plan || !le_column) return B2P_E_INVALID;
+  if (!plan->range()) return not_a_range_node();
   try {
-    plan->plan->set_histogram(le_column, quantile);
+    plan->range()->set_histogram(le_column, quantile);
+    return B2P_OK;
+  } catch (const b2p::PlanError& e) {
+    return plan_fail(e);
+  }
+}
+
+int b2p_plan_set_scalar_op(b2p_plan* plan, int32_t op, double scalar, int32_t scalar_on_left, int32_t return_bool) {
+  if (!plan) return B2P_E_INVALID;
+  try {
+    plan->node->add_scalar_op(op, scalar, scalar_on_left != 0, return_bool != 0);
     return B2P_OK;
   } catch (const b2p::PlanError& e) {
     return plan_fail(e);
@@ -642,8 +850,9 @@ int b2p_plan_set_histogram_quantile(b2p_plan* plan, const char* le_column, doubl
 
 int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema) {
   if (!plan) return B2P_E_INVALID;
+  if (!plan->range()) return not_a_range_node();
   try {
-    plan->plan->push(std::make_unique<b2p::RecordBatch>(batch, schema));
+    plan->range()->push(std::make_unique<b2p::RecordBatch>(batch, schema));
     return B2P_OK;
   } catch (const b2p::PlanError& e) {
     return plan_fail(e);
@@ -656,7 +865,7 @@ int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSc
 int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema) {
   if (!plan) return B2P_E_INVALID;
   try {
-    plan->plan->execute(out, out_schema);
+    plan->node->execute(out, out_schema);
     return B2P_OK;
   } catch (const b2p::PlanError& e) {
     return plan_fail(e);
@@ -666,7 +875,7 @@ int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema*
   }
 }
 
-int64_t b2p_plan_num_series(b2p_plan* plan) { return plan ? plan->plan->num_series() : -1; }
+int64_t b2p_plan_num_series(b2p_plan* plan) { return plan && plan->range() ? plan->range()->num_series() : -1; }
 
 void b2p_plan_destroy(b2p_plan* plan) { delete plan; }
 

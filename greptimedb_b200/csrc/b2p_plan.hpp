@@ -77,14 +77,56 @@ struct PromRangePlanArgs {
   double quantile = 0.0;
 };
 
-class PromRangePlan {
+// What a node computed, before it becomes Arrow: a dense [rows x T] grid with validity, the eval timestamps and one label
+// tuple per row.  Exported, row r emits one Arrow row per valid step k (rows in order, steps ascending).
+struct NodeResult {
+  int64_t T = 0;
+  uint32_t Tw = 0;
+  uint32_t rows = 0;
+  std::vector<int64_t> eval_ts;  // [T]
+  std::vector<double> val;       // [rows x T]; empty when rows == 0 or T == 0
+  std::vector<uint32_t> valid;   // [rows x Tw]
+  std::string time_index, value_name;
+  std::vector<std::string> tag_names;
+  std::vector<std::vector<std::string>> tags;  // [tag][row] label values (NULL labels as "\0null")
+  bool id_keyed = false;                       // the one tag column is a UInt64 id (values in `ids`, not `tags`)
+  std::vector<uint64_t> ids;                   // [row] when id_keyed
+  bool tags_first = false;                     // columns {tags.., time index, value} instead of {time index, value, tags..}
+  bool valid_at(uint32_t r, int64_t k) const { return (valid[(size_t)r * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u; }
+};
+
+// `node op scalar` / `scalar op node` applied to a node's result (b2p_plan_set_scalar_op)
+struct ScalarOp {
+  int op;
+  double scalar;
+  bool scalar_on_left, return_bool;
+};
+
+// A plan node: computes its result (step 1), then exports it as one Arrow batch (step 2).
+class PlanNode {
+ public:
+  explicit PlanNode(b2p_ctx* ctx) : ctx_(ctx) {}
+  virtual ~PlanNode() = default;
+  // the node's result with its scalar operators applied
+  void run(NodeResult& r);
+  // runs the node and exports the result batch (caller releases it)
+  void execute(ArrowArray* out, ArrowSchema* out_schema);
+  void add_scalar_op(int op, double scalar, bool scalar_on_left, bool return_bool);
+
+ protected:
+  virtual void compute(NodeResult& r) = 0;
+  b2p_ctx* ctx_;
+
+ private:
+  std::vector<ScalarOp> scalar_ops_;
+};
+
+class PromRangePlan : public PlanNode {
  public:
   PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args);
   const char* name() const { return "GpuPromRangeExec"; }
   // input stream, in order; batches of one partition (sorted by tags, ts)
   void push(std::unique_ptr<RecordBatch> batch);
-  // runs the sub-plan on the device and exports the result batch (caller releases it)
-  void execute(ArrowArray* out, ArrowSchema* out_schema);
   int64_t num_series() const { return num_series_; }  // the reference's `num_series` metric (range_manipulate.rs:610-619)
   // switch the node to the instant-vector form (InstantManipulate) / add a HistogramFold on top; before execute()
   int set_instant(Millisecond lookback_delta) {
@@ -95,12 +137,15 @@ class PromRangePlan {
   }
   void set_histogram(const std::string& le_column, double quantile);
 
+ protected:
+  // runs the sub-plan on the device
+  void compute(NodeResult& r) override;
+
  private:
   struct TagStore {
     std::vector<std::vector<std::string>> utf8;  // [tag][series] label values of each series' first row
     std::vector<uint64_t> tsid;                 // when the key is a UInt64 id
   };
-  b2p_ctx* ctx_;
   PromRangePlanArgs args_;
   int fn_id_;
   int agg_id_;
@@ -114,6 +159,28 @@ class PromRangePlan {
   std::vector<std::string> last_key_;
   uint64_t last_id_ = 0;
   bool have_last_ = false;
+};
+
+// Vector-vector binary operator over two nodes (b2p_plan_binary_create): the reference's ProjectionExec / FilterExec
+// over an inner HashJoinExec on (key columns, time index), planner.rs:556-777, 3436-3546.  The join is a match between
+// series on the host (hash of the key tuples, O(rows + pairs)); the per-step work is b2p_binary_op.
+class BinaryPlan : public PlanNode {
+ public:
+  enum class Matching { None, On, Ignoring };
+  BinaryPlan(b2p_ctx* ctx, int op, bool return_bool, std::shared_ptr<PlanNode> lhs, std::shared_ptr<PlanNode> rhs,
+             Matching matching, std::vector<std::string> labels, bool labels_from_lhs);
+  const char* name() const { return "GpuPromBinaryExec"; }
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  int op_;
+  bool return_bool_;
+  std::shared_ptr<PlanNode> lhs_, rhs_;
+  Matching matching_;
+  std::vector<std::string> labels_;
+  bool labels_from_lhs_;
 };
 
 int function_id_from_name(const std::string& prom_name);  // -1 when unknown

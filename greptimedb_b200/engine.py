@@ -24,6 +24,13 @@ FN_IDS = {
     "quantile_over_time": 19, "holt_winters": 20,
 }
 AGG_IDS = {"sum": 0, "avg": 1, "count": 2, "min": 3, "max": 4, "stddev": 5, "stdvar": 6}
+# enum b2p_binop: PromQL binary operators, arithmetic first, then the comparisons
+OP_IDS = {"+": 0, "-": 1, "*": 2, "/": 3, "%": 4, "^": 5, "atan2": 6,
+          "==": 7, "!=": 8, ">": 9, "<": 10, ">=": 11, "<=": 12}
+
+
+def op_id(op) -> int:
+    return OP_IDS[op] if isinstance(op, str) else int(op)
 
 E_UNSORTED = -3
 
@@ -205,6 +212,34 @@ class Context:
                                                    _ptr(out), _ptr(ov)))
         return out, ov
 
+    def binary_op(self, op, lhs, lhs_valid, lhs_row, rhs, rhs_valid, rhs_row, return_bool=False):
+        """lhs[lhs_row[p]] op rhs[rhs_row[p]] for every pair p -> (out [P,T] f64, valid_words [P,Tw] u32)."""
+        lhs = np.ascontiguousarray(lhs, np.float64)
+        rhs = np.ascontiguousarray(rhs, np.float64)
+        lhs_valid = np.ascontiguousarray(lhs_valid, np.uint32)
+        rhs_valid = np.ascontiguousarray(rhs_valid, np.uint32)
+        lhs_row = np.ascontiguousarray(lhs_row, np.uint32)
+        rhs_row = np.ascontiguousarray(rhs_row, np.uint32)
+        T = lhs.shape[1] if lhs.ndim == 2 else rhs.shape[1]
+        P = lhs_row.size
+        out = np.zeros((P, T), np.float64)
+        ov = np.zeros((P, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_binary_op(self._h, op_id(op), int(bool(return_bool)), _ptr(lhs), _ptr(lhs_valid),
+                                          _ptr(lhs_row), lhs.shape[0], _ptr(rhs), _ptr(rhs_valid), _ptr(rhs_row),
+                                          rhs.shape[0], P, T, _ptr(out), _ptr(ov)))
+        return out, ov
+
+    def scalar_op(self, op, scalar, vals, valid, scalar_on_left=False, return_bool=False):
+        """`vals op scalar` (or `scalar op vals`) -> (out [S,T] f64, valid_words [S,Tw] u32)."""
+        vals = np.ascontiguousarray(vals, np.float64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        S, T = vals.shape
+        out = np.zeros((S, T), np.float64)
+        ov = np.zeros((S, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_scalar_op(self._h, op_id(op), int(bool(return_bool)), int(bool(scalar_on_left)),
+                                          float(scalar), _ptr(vals), _ptr(valid), S, T, _ptr(out), _ptr(ov)))
+        return out, ov
+
     # -- device API (torch tensors or raw pointers; asynchronous) ----------------------------------
     def series_offsets_dev(self, sid, n_rows, n_series, offsets):
         self._check(self._L.b2p_series_offsets_dev(self._h, _ptr(sid), n_rows, n_series, _ptr(offsets)))
@@ -293,6 +328,20 @@ class Context:
 
     def column_reduce_dev(self, col_ptrs, n_cols, n_rows, out_sum, out_cnt):
         self._check(self._L.b2p_column_reduce_dev(self._h, _ptr(col_ptrs), n_cols, n_rows, _ptr(out_sum), _ptr(out_cnt)))
+
+    def binary_op_dev(self, op, lhs, lhs_valid, lhs_row, n_lhs_rows, rhs, rhs_valid, rhs_row, n_rhs_rows, n_pairs, T,
+                      out, out_valid, return_bool=False):
+        self._check(self._L.b2p_binary_op_dev(self._h, op_id(op), int(bool(return_bool)), _ptr(lhs), _ptr(lhs_valid),
+                                              _ptr(lhs_row), n_lhs_rows, _ptr(rhs), _ptr(rhs_valid), _ptr(rhs_row),
+                                              n_rhs_rows, n_pairs, T, _ptr(out), _ptr(out_valid)))
+
+    def scalar_op_dev(self, op, scalar, vals, valid, n_rows, T, out, out_valid, scalar_on_left=False, return_bool=False):
+        self._check(self._L.b2p_scalar_op_dev(self._h, op_id(op), int(bool(return_bool)), int(bool(scalar_on_left)),
+                                              float(scalar), _ptr(vals), _ptr(valid), n_rows, T, _ptr(out),
+                                              _ptr(out_valid)))
+
+    def count_valid_words_dev(self, cnt, n_rows, T, valid_words):
+        self._check(self._L.b2p_count_valid_words_dev(self._h, _ptr(cnt), n_rows, T, _ptr(valid_words)))
 
     def synth_fill_dev(self, series_begin, n_series, n_samples, t0, scrape_ms, jitter_ms, with_resets, seed, ts, val, sid):
         self._check(self._L.b2p_synth_fill_dev(self._h, series_begin, n_series, n_samples, t0, scrape_ms, jitter_ms,

@@ -3,7 +3,8 @@
 `PromRangeExec` takes the constructor arguments of the reference's plan nodes with their own names
 (SeriesDivide tag_columns/time_index, SeriesNormalize offset/need_filter_out_nan, RangeManipulate
 start/end/interval/range/field column, the prom_* UDF name, optional by-label aggregate) and is fed
-pyarrow RecordBatches exactly like the reference's tests feed a MemoryExec.
+pyarrow RecordBatches exactly like the reference's tests feed a MemoryExec.  `scalar_op` puts `node op number` on
+top of any node, and `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels).
 """
 from __future__ import annotations
 
@@ -11,7 +12,7 @@ import ctypes as C
 from typing import Optional, Sequence
 
 from . import _lib
-from .engine import B2PError, Context, make_params
+from .engine import B2PError, Context, make_params, op_id
 
 
 class _ArrowArray(C.Structure):
@@ -33,7 +34,40 @@ def _cstr_array(items: Sequence[str]):
     return arr
 
 
-class PromRangeExec:
+class _PlanNode:
+    """What every node handle has: scalar operators on top, execute, close."""
+    _h = None
+
+    def scalar_op(self, op, scalar: float, scalar_on_left: bool = False, return_bool: bool = False) -> "_PlanNode":
+        """`node op scalar` (or `scalar op node`) on top of this node; calls chain in order.  Returns self."""
+        rc = self._L.b2p_plan_set_scalar_op(self._h, op_id(op), float(scalar), int(bool(scalar_on_left)),
+                                            int(bool(return_bool)))
+        if rc != 0:
+            raise B2PError(rc, self._L.b2p_plan_last_error().decode())
+        return self
+
+    def execute(self):
+        """-> pyarrow.RecordBatch with the rows the reference's plan would emit."""
+        import pyarrow as pa
+        arr, sch = _ArrowArray(), _ArrowSchema()
+        rc = self._L.b2p_plan_execute(self._h, C.addressof(arr), C.addressof(sch))
+        if rc != 0:
+            raise B2PError(rc, self._L.b2p_plan_last_error().decode())
+        return pa.RecordBatch._import_from_c(C.addressof(arr), C.addressof(sch))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.b2p_plan_destroy(self._h)
+            self._h = None
+
+    def __del__(self):  # pragma: no cover
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class PromRangeExec(_PlanNode):
     def __init__(self, ctx: Context, function: str, start: int, end: int, interval: int, range: int, time_index: str,
                  field_column: str, tag_columns: Sequence[str], offset: int = 0, need_filter_out_nan: bool = True,
                  param0: float = 0.0, param1: float = 0.0, aggregate: Optional[str] = None,
@@ -64,25 +98,28 @@ class PromRangeExec:
         if rc != 0:
             raise B2PError(rc, self._L.b2p_plan_last_error().decode())
 
-    def execute(self):
-        """-> pyarrow.RecordBatch with the rows the reference's Filter / Aggregate+Sort would emit."""
-        import pyarrow as pa
-        arr, sch = _ArrowArray(), _ArrowSchema()
-        rc = self._L.b2p_plan_execute(self._h, C.addressof(arr), C.addressof(sch))
-        if rc != 0:
-            raise B2PError(rc, self._L.b2p_plan_last_error().decode())
-        return pa.RecordBatch._import_from_c(C.addressof(arr), C.addressof(sch))
-
     def num_series(self) -> int:
         return int(self._L.b2p_plan_num_series(self._h))
 
-    def close(self):
-        if getattr(self, "_h", None):
-            self._L.b2p_plan_destroy(self._h)
-            self._h = None
 
-    def __del__(self):  # pragma: no cover
-        try:
-            self.close()
-        except Exception:
-            pass
+class BinaryPlan(_PlanNode):
+    """`lhs op rhs` over two nodes (PromRangeExec or BinaryPlan), matched like the reference's inner join on the tag
+    columns of the rhs (narrowed by `on` / `ignoring`) and the time index.  `label_side` names the node whose tag
+    columns an arithmetic / `bool` result carries ("rhs" unless the rhs has no tags, for two sides over one table).
+    The children stay usable (push batches into them before execute()) and are kept alive by this node."""
+
+    def __init__(self, ctx: Context, op, lhs: _PlanNode, rhs: _PlanNode, return_bool: bool = False,
+                 on: Optional[Sequence[str]] = None, ignoring: Optional[Sequence[str]] = None,
+                 label_side: str = "rhs"):
+        if on is not None and ignoring is not None:
+            raise ValueError("on and ignoring are exclusive")
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (lhs, rhs)
+        matching, labels = (b"on", list(on)) if on is not None else (b"ignoring", list(ignoring)) if ignoring is not None \
+            else (None, [])
+        arr = _cstr_array(labels)
+        self._h = self._L.b2p_plan_binary_create(ctx._h, op_id(op), int(bool(return_bool)), lhs._h, rhs._h, matching,
+                                                 arr, len(labels), label_side.encode())
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())

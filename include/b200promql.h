@@ -28,6 +28,10 @@
  *   b2p_histogram_quantile[_dev] HistogramFoldStream::fold_buf + evaluate_row
  *                              histogram_fold.rs:754-820, 1046-1118
  *   b2p_column_reduce_dev      avg_over_time over a wide table (config 5): per-column sum,count
+ *   b2p_binary_op[_dev]        vector-vector arithmetic / comparison: ProjectionExec / FilterExec over the inner
+ *                              HashJoinExec on (tag columns, time index), planner.rs:556-777, 3436-3546; the join is a
+ *                              host-side series match that yields (lhs row, rhs row) pairs
+ *   b2p_scalar_op[_dev]        vector-scalar arithmetic / comparison (ProjectionExec / FilterExec, planner.rs:556-777)
  *
  * Data layout (HBM, struct-of-arrays, all row-sorted by (series id, timestamp) exactly like
  * the reference's required_input_ordering, series_divide.rs:410-440):
@@ -102,6 +106,12 @@ enum b2p_fn {
 enum b2p_agg { B2P_AGG_SUM = 0, B2P_AGG_AVG = 1, B2P_AGG_COUNT = 2, B2P_AGG_MIN = 3, B2P_AGG_MAX = 4,
                B2P_AGG_STDDEV = 5, B2P_AGG_STDVAR = 6 };
 
+/* PromQL binary operators (planner.rs:3915-3990): arithmetic on Float64 operands, then the comparisons, which order
+ * floats by IEEE 754 totalOrder like arrow-rs' cmp kernels (NaN == NaN, -0.0 < +0.0, +NaN above +inf). */
+enum b2p_binop { B2P_OP_ADD = 0, B2P_OP_SUB = 1, B2P_OP_MUL = 2, B2P_OP_DIV = 3, B2P_OP_MOD = 4, B2P_OP_POW = 5,
+                 B2P_OP_ATAN2 = 6, B2P_OP_EQ = 7, B2P_OP_NE = 8, B2P_OP_GT = 9, B2P_OP_LT = 10, B2P_OP_GE = 11,
+                 B2P_OP_LE = 12 };
+
 /* Parameters of the fused sub-plan.  Field-for-field the arguments of
  * RangeManipulate::new(start,end,interval,range,..) (range_manipulate.rs:86-110),
  * SeriesNormalize::new(offset,..,need_filter_out_nan,..) (normalize.rs:66-83) and the UDF scalars. */
@@ -140,7 +150,7 @@ B2P_API int64_t b2p_last_h2d_bytes(b2p_ctx* ctx);
 B2P_API int64_t b2p_last_warp_tier_series(b2p_ctx* ctx);
 /* CUDA-event time (ms) of the kernels of the last *_dev / host call, by stage index:
  * 0 = series_offsets, 1 = range/instant fast kernel, 2 = slow-path kernel, 3 = aggregate /
- * histogram / reduce kernel.  Valid after b2p_sync(). */
+ * histogram / reduce / binary-operator kernel.  Valid after b2p_sync(). */
 B2P_API double b2p_last_kernel_ms(b2p_ctx* ctx, int stage);
 /* Kernels launched by this context since creation (the bench's gpu_launches claim). */
 B2P_API int64_t b2p_launch_count(b2p_ctx* ctx);
@@ -243,6 +253,26 @@ B2P_API int b2p_histogram_fold_dev(b2p_ctx* ctx, double phi, const uint32_t* his
 B2P_API int b2p_column_reduce_dev(b2p_ctx* ctx, const double* const* cols, uint32_t n_cols, uint64_t n_rows,
                           double* out_sum, uint64_t* out_cnt);
 
+/* Binary operator over two dense grids matched into pairs: for pair p and step k, lhs[lhs_row[p]*T + k] op
+ * rhs[rhs_row[p]*T + k] -> out[p*T + k], out_valid [n_pairs*Tw].  A cell is valid iff both operands are; a comparison
+ * without `bool` (return_bool == 0) also drops the cells where it is false and keeps the lhs value; with `bool` the
+ * value is 1.0 / 0.0.  Invalid cells hold 0.0.  Pairs may come in any order and repeat rows (group_left / right).
+ * B2P_E_INVALID: unknown op, return_bool on an arithmetic op; a row index >= n_lhs_rows / n_rhs_rows is found on the
+ * device (that pair's cells are written invalid) and reported by b2p_sync. */
+B2P_API int b2p_binary_op_dev(b2p_ctx* ctx, int32_t op /* enum b2p_binop */, int32_t return_bool, const double* lhs,
+                              const uint32_t* lhs_valid, const uint32_t* lhs_row /* [n_pairs] */, uint32_t n_lhs_rows,
+                              const double* rhs, const uint32_t* rhs_valid, const uint32_t* rhs_row /* [n_pairs] */,
+                              uint32_t n_rhs_rows, uint64_t n_pairs, uint64_t T, double* out, uint32_t* out_valid);
+/* One grid against a number: `scalar op vals` (scalar_on_left) or `vals op scalar`; a filtering comparison keeps the
+ * vector's value.  out / out_valid may be vals / valid (in place). */
+B2P_API int b2p_scalar_op_dev(b2p_ctx* ctx, int32_t op, int32_t return_bool, int32_t scalar_on_left, double scalar,
+                              const double* vals, const uint32_t* valid, uint64_t n_rows, uint64_t T, double* out,
+                              uint32_t* out_valid);
+/* cnt [n_rows*T] of a by-label aggregate (0 <=> no row) -> valid_words [n_rows*Tw], so that a finalized aggregate
+ * feeds b2p_binary_op_dev without a host round trip. */
+B2P_API int b2p_count_valid_words_dev(b2p_ctx* ctx, const uint32_t* cnt, uint64_t n_rows, uint64_t T,
+                                      uint32_t* valid_words);
+
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
  * the id column `sid` (ids sid_base .. sid_base + n_series - 1, non-decreasing), or copied from `offsets_in`
@@ -280,6 +310,14 @@ B2P_API int b2p_range_histogram_fold(b2p_ctx* ctx, const b2p_range_params* p, co
                              const uint32_t* sid, const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series,
                              double phi, const uint32_t* hist_off, const uint32_t* bucket_series, const double* bucket_le,
                              uint32_t n_hist, double* out, uint32_t* out_valid_words);
+/* Host-pointer forms of b2p_binary_op_dev / b2p_scalar_op_dev (synchronous; row-index errors are returned directly). */
+B2P_API int b2p_binary_op(b2p_ctx* ctx, int32_t op, int32_t return_bool, const double* lhs, const uint32_t* lhs_valid,
+                          const uint32_t* lhs_row, uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid,
+                          const uint32_t* rhs_row, uint32_t n_rhs_rows, uint64_t n_pairs, uint64_t T, double* out,
+                          uint32_t* out_valid);
+B2P_API int b2p_scalar_op(b2p_ctx* ctx, int32_t op, int32_t return_bool, int32_t scalar_on_left, double scalar,
+                          const double* vals, const uint32_t* valid, uint64_t n_rows, uint64_t T, double* out,
+                          uint32_t* out_valid);
 
 /* ---- plan-level API over the Arrow C Data Interface ------------------------------------------------
  * GpuPromRangeExec: the whole sub-tree SeriesDivide -> SeriesNormalize -> RangeManipulate ->
@@ -330,6 +368,22 @@ B2P_API int b2p_plan_set_instant(b2p_plan* plan, int64_t lookback_delta);
 /* Add HistogramFold(le_column, field, time_index, quantile) (histogram_fold.rs:104-130) on top of the per-series
  * result: series that agree on every tag except `le` form one histogram. */
 B2P_API int b2p_plan_set_histogram_quantile(b2p_plan* plan, const char* le_column, double quantile);
+/* `node op scalar` (or `scalar op node` with scalar_on_left) on top of any node, binary nodes included; calls chain in
+ * order (rate(x[1m]) * 60 > 1 is two calls).  Arithmetic and `bool` keep every row (the value column is renamed like
+ * the reference's projection); a comparison without `bool` is a filter and keeps the node's value. */
+B2P_API int b2p_plan_set_scalar_op(b2p_plan* plan, int32_t op, double scalar, int32_t scalar_on_left, int32_t return_bool);
+/* Vector-vector binary node over two nodes (range, instant, aggregate, histogram or binary).  Series are matched on the
+ * host like the reference's inner join on (key columns, time index): key = the rhs node's tag columns, intersected with
+ * `labels` for matching "on", without them for "ignoring" (matching NULL: all of them); no key when either side has no
+ * tags (every row pairs with every row); two id-keyed (__tsid) nodes without a modifier match on the id.  Every lhs
+ * series pairs with every rhs series of the same key.  Output rows: {tag columns of label_side ("lhs" | "rhs"), time
+ * index, value} for arithmetic / `bool`, the lhs node's rows for a filtering comparison; pairs in lhs then rhs row
+ * order, steps ascending.  The node shares ownership of both children: their handles stay usable for push_batch and
+ * must still be destroyed.  NULL on error (b2p_plan_last_error); the children are untouched then. */
+B2P_API b2p_plan* b2p_plan_binary_create(b2p_ctx* ctx, int32_t op, int32_t return_bool, b2p_plan* lhs, b2p_plan* rhs,
+                                         const char* matching /* NULL | "on" | "ignoring" */,
+                                         const char* const* labels, int32_t n_labels,
+                                         const char* label_side /* "lhs" | "rhs" */);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

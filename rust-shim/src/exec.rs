@@ -61,6 +61,8 @@ pub struct GpuPromRangeParams {
     pub by_columns: Vec<String>,
     /// HistogramFold::new(le_column, .., quantile) on top (histogram_fold.rs:104-130).
     pub histogram: Option<(String, f64)>,
+    /// `node op scalar` projections / filters on top, in order: (op, scalar, scalar_on_left, return_bool).
+    pub scalar_ops: Vec<(ffi::B2pBinOp, f64, bool, bool)>,
 }
 
 #[derive(Debug)]
@@ -97,6 +99,11 @@ impl GpuPromRangeExec {
 
     pub fn params(&self) -> &GpuPromRangeParams {
         &self.params
+    }
+
+    /// the scan the node reads (what a rule stacking more onto the node rebuilds it over)
+    pub fn input(&self) -> &Arc<dyn ExecutionPlan> {
+        &self.input
     }
 }
 
@@ -267,6 +274,11 @@ impl PlanHandle {
             if let Some((le, q)) = &p.histogram {
                 let le = c(le);
                 if ffi::b2p_plan_set_histogram_quantile(plan, le.as_ptr(), *q) != ffi::B2P_OK {
+                    return Err(DataFusionError::Plan(ffi::plan_last_error()));
+                }
+            }
+            for (op, scalar, on_left, return_bool) in &p.scalar_ops {
+                if ffi::b2p_plan_set_scalar_op(plan, *op as i32, *scalar, *on_left as i32, *return_bool as i32) != ffi::B2P_OK {
                     return Err(DataFusionError::Plan(ffi::plan_last_error()));
                 }
             }

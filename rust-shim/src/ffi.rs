@@ -89,6 +89,32 @@ pub enum B2pAgg {
     Stdvar = 6,
 }
 
+/// `enum b2p_binop` — PromQL binary operators (planner.rs:3915-3990); the comparisons order f64 by IEEE totalOrder.
+#[repr(i32)]
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub enum B2pBinOp {
+    Add = 0,
+    Sub = 1,
+    Mul = 2,
+    Div = 3,
+    Mod = 4,
+    Pow = 5,
+    Atan2 = 6,
+    Eq = 7,
+    Ne = 8,
+    Gt = 9,
+    Lt = 10,
+    Ge = 11,
+    Le = 12,
+}
+
+impl B2pBinOp {
+    /// true for `== != > < >= <=` (a filter without `bool`)
+    pub fn is_comparison(self) -> bool {
+        self as i32 >= B2pBinOp::Eq as i32
+    }
+}
+
 /// `struct b2p_range_params`: RangeManipulate::new(start, end, interval, range, ..) (range_manipulate.rs:86-110),
 /// SeriesNormalize::new(offset, .., need_filter_out_nan, ..) (normalize.rs:66-83) and the UDF scalars.
 #[repr(C)]
@@ -202,6 +228,18 @@ extern "C" {
         ctx: *mut b2p_ctx, cols: *const *const f64, n_cols: u32, n_rows: u64, out_sum: *mut f64, out_cnt: *mut u64,
     ) -> c_int;
 
+    // ---- binary operators ---------------------------------------------------------------------------------------------
+    pub fn b2p_binary_op_dev(
+        ctx: *mut b2p_ctx, op: i32, return_bool: i32, lhs: *const f64, lhs_valid: *const u32, lhs_row: *const u32,
+        n_lhs_rows: u32, rhs: *const f64, rhs_valid: *const u32, rhs_row: *const u32, n_rhs_rows: u32, n_pairs: u64,
+        t: u64, out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
+    pub fn b2p_scalar_op_dev(
+        ctx: *mut b2p_ctx, op: i32, return_bool: i32, scalar_on_left: i32, scalar: f64, vals: *const f64,
+        valid: *const u32, n_rows: u64, t: u64, out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
+    pub fn b2p_count_valid_words_dev(ctx: *mut b2p_ctx, cnt: *const u32, n_rows: u64, t: u64, valid_words: *mut u32) -> c_int;
+
     // ---- host-side helper (no device work): SeriesDivide + cadence scan of one sorted batch ---------------------------
     pub fn b2p_host_scan_series(
         ts: *const i64, sid: *const u32, offsets_in: *const u64, n_rows: u64, n_series: u32, sid_base: u32,
@@ -235,6 +273,15 @@ extern "C" {
         offsets_host: *const u64, n_rows: u64, n_series: u32, phi: f64, hist_off: *const u32,
         bucket_series: *const u32, bucket_le: *const f64, n_hist: u32, out: *mut f64, out_valid_words: *mut u32,
     ) -> c_int;
+    pub fn b2p_binary_op(
+        ctx: *mut b2p_ctx, op: i32, return_bool: i32, lhs: *const f64, lhs_valid: *const u32, lhs_row: *const u32,
+        n_lhs_rows: u32, rhs: *const f64, rhs_valid: *const u32, rhs_row: *const u32, n_rhs_rows: u32, n_pairs: u64,
+        t: u64, out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
+    pub fn b2p_scalar_op(
+        ctx: *mut b2p_ctx, op: i32, return_bool: i32, scalar_on_left: i32, scalar: f64, vals: *const f64,
+        valid: *const u32, n_rows: u64, t: u64, out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- plan-level API over the Arrow C Data Interface -----------------------------------------------------------------
     pub fn b2p_plan_range_create(
@@ -244,6 +291,12 @@ extern "C" {
     ) -> *mut b2p_plan;
     pub fn b2p_plan_set_instant(plan: *mut b2p_plan, lookback_delta: i64) -> c_int;
     pub fn b2p_plan_set_histogram_quantile(plan: *mut b2p_plan, le_column: *const c_char, quantile: f64) -> c_int;
+    pub fn b2p_plan_set_scalar_op(plan: *mut b2p_plan, op: i32, scalar: f64, scalar_on_left: i32, return_bool: i32) -> c_int;
+    /// The node shares ownership of both children; their handles stay valid and must still be destroyed.
+    pub fn b2p_plan_binary_create(
+        ctx: *mut b2p_ctx, op: i32, return_bool: i32, lhs: *mut b2p_plan, rhs: *mut b2p_plan, matching: *const c_char,
+        labels: *const *const c_char, n_labels: i32, label_side: *const c_char,
+    ) -> *mut b2p_plan;
     /// MOVES the batch: on success the release callbacks now belong to the plan.
     pub fn b2p_plan_push_batch(plan: *mut b2p_plan, batch: *mut FFI_ArrowArray, schema: *mut FFI_ArrowSchema) -> c_int;
     pub fn b2p_plan_execute(plan: *mut b2p_plan, out: *mut FFI_ArrowArray, out_schema: *mut FFI_ArrowSchema) -> c_int;

@@ -15,6 +15,17 @@
 //!   <input: CooperativeExec <- SeriesScan / MergeScanExec>
 //! ```
 //!
+//! Binary operators on top of an already rewritten `GpuPromRangeExec` (planner.rs:556-777, 3436-3546):
+//!
+//! ```text
+//!   ProjectionExec: expr=[.., col op Float64(c) | Float64(c) op col, ..]   (arithmetic, or a comparison with `bool`)
+//!   FilterExec: col cmp Float64(c)                                        (comparison without `bool`)
+//!     <- GpuPromRangeExec                     => the same node with b2p_plan_set_scalar_op appended
+//!
+//!   ProjectionExec | FilterExec <- HashJoinExec(Inner, on = [(tag, tag).., (ts, ts)])
+//!     <- GpuPromRangeExec, GpuPromRangeExec   => `match_binary_join`: the b2p_plan_binary_create arguments
+//! ```
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
@@ -23,17 +34,20 @@ use std::sync::Arc;
 use datafusion::common::tree_node::{Transformed, TreeNode};
 use datafusion::common::{Result as DataFusionResult, ScalarValue};
 use datafusion::config::ConfigOptions;
-use datafusion::physical_expr::expressions::{Column, IsNotNullExpr, Literal};
+use datafusion::common::JoinType;
+use datafusion::logical_expr::Operator;
+use datafusion::physical_expr::expressions::{BinaryExpr, CastExpr, Column, IsNotNullExpr, Literal};
 use datafusion::physical_expr::{PhysicalExpr, ScalarFunctionExpr};
 use datafusion::physical_optimizer::PhysicalOptimizerRule;
 use datafusion::physical_plan::aggregates::{AggregateExec, AggregateMode};
 use datafusion::physical_plan::filter::FilterExec;
+use datafusion::physical_plan::joins::HashJoinExec;
 use datafusion::physical_plan::projection::ProjectionExec;
 use datafusion::physical_plan::repartition::RepartitionExec;
 use datafusion::physical_plan::ExecutionPlan;
 
 use crate::exec::{GpuPromRangeExec, GpuPromRangeParams};
-use crate::ffi::B2pFn;
+use crate::ffi::{B2pBinOp, B2pFn};
 // In-tree these are `crate::extension_plan::{..}`; named here the way the reference names them.
 use promql::extension_plan::{RangeManipulateExec, SeriesDivideExec, SeriesNormalizeExec};
 
@@ -92,6 +106,7 @@ impl GpuPromRewrite {
             aggregate: None,
             by_columns: vec![],
             histogram: None,
+            scalar_ops: vec![],
         };
         Some((params, divide.input().clone()))
     }
@@ -136,6 +151,143 @@ impl GpuPromRewrite {
     }
 }
 
+/// What `b2p_plan_binary_create` takes for `lhs op rhs` over two rewritten nodes.
+#[derive(Debug)]
+pub struct GpuPromBinarySpec {
+    pub op: B2pBinOp,
+    pub return_bool: bool,
+    pub lhs: GpuPromRangeParams,
+    pub rhs: GpuPromRangeParams,
+    /// the join's tag keys, passed as `on(..)`
+    pub on: Vec<String>,
+    /// "lhs" | "rhs": the side whose tag columns the projection emits (planner.rs:696-711)
+    pub label_side: &'static str,
+}
+
+/// DataFusion operator -> b2p_binop; `pow` / `atan2` arrive as scalar functions (planner.rs:3915-3990).
+fn binop_of(expr: &Arc<dyn PhysicalExpr>) -> Option<(B2pBinOp, Arc<dyn PhysicalExpr>, Arc<dyn PhysicalExpr>, bool)> {
+    // `bool`: CAST(cmp AS Float64)
+    let (expr, cast) = match expr.as_any().downcast_ref::<CastExpr>() {
+        Some(c) => (c.expr().clone(), true),
+        None => (expr.clone(), false),
+    };
+    if let Some(b) = expr.as_any().downcast_ref::<BinaryExpr>() {
+        let op = match b.op() {
+            Operator::Plus => B2pBinOp::Add,
+            Operator::Minus => B2pBinOp::Sub,
+            Operator::Multiply => B2pBinOp::Mul,
+            Operator::Divide => B2pBinOp::Div,
+            Operator::Modulo => B2pBinOp::Mod,
+            Operator::Eq => B2pBinOp::Eq,
+            Operator::NotEq => B2pBinOp::Ne,
+            Operator::Gt => B2pBinOp::Gt,
+            Operator::Lt => B2pBinOp::Lt,
+            Operator::GtEq => B2pBinOp::Ge,
+            Operator::LtEq => B2pBinOp::Le,
+            _ => return None,
+        };
+        if cast != op.is_comparison() {
+            return None;
+        }
+        return Some((op, b.left().clone(), b.right().clone(), cast));
+    }
+    let f = expr.as_any().downcast_ref::<ScalarFunctionExpr>()?;
+    let op = match f.name() {
+        "power" => B2pBinOp::Pow,
+        "atan2" => B2pBinOp::Atan2,
+        _ => return None,
+    };
+    Some((op, f.args().first()?.clone(), f.args().get(1)?.clone(), false))
+}
+
+fn float_literal(e: &Arc<dyn PhysicalExpr>) -> Option<f64> {
+    match e.as_any().downcast_ref::<Literal>()?.value() {
+        ScalarValue::Float64(Some(v)) => Some(*v),
+        _ => None,
+    }
+}
+
+impl GpuPromRewrite {
+    /// `ProjectionExec(col op lit)` / `FilterExec(col cmp lit)` over a `GpuPromRangeExec` -> the node's parameters with
+    /// the scalar operator appended; every other projected expression must be a plain column.
+    fn match_scalar_op(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<(GpuPromRangeParams, Arc<dyn ExecutionPlan>)> {
+        let (expr, input, filter) = if let Some(f) = plan.as_any().downcast_ref::<FilterExec>() {
+            (f.predicate().clone(), f.input().clone(), true)
+        } else {
+            let p = plan.as_any().downcast_ref::<ProjectionExec>()?;
+            let mut value = None;
+            for e in p.expr() {
+                if e.expr.as_any().downcast_ref::<Column>().is_none() {
+                    if value.is_some() {
+                        return None;
+                    }
+                    value = Some(e.expr.clone());
+                }
+            }
+            (value?, p.input().clone(), false)
+        };
+        let node = input.as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let (op, l, r, return_bool) = binop_of(&expr)?;
+        if filter != (op.is_comparison() && !return_bool) {
+            return None;
+        }
+        let (scalar, on_left) = match (float_literal(&l), float_literal(&r)) {
+            (None, Some(v)) if l.as_any().downcast_ref::<Column>().is_some() => (v, false),
+            (Some(v), None) if r.as_any().downcast_ref::<Column>().is_some() => (v, true),
+            _ => return None,
+        };
+        let mut params = node.params().clone();
+        params.scalar_ops.push((op, scalar, on_left, return_bool));
+        Some((params, node.input().clone()))
+    }
+
+    /// `ProjectionExec | FilterExec <- HashJoinExec(Inner, tags.. + ts)` over two `GpuPromRangeExec` -> the arguments of
+    /// `b2p_plan_binary_create`.  The join keys become `on(..)`; the projection's tag columns tell the label side.
+    pub fn match_binary_join(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromBinarySpec> {
+        let (expr, join_plan) = if let Some(f) = plan.as_any().downcast_ref::<FilterExec>() {
+            (f.predicate().clone(), f.input().clone())
+        } else {
+            let p = plan.as_any().downcast_ref::<ProjectionExec>()?;
+            let value = p.expr().iter().find(|e| e.expr.as_any().downcast_ref::<Column>().is_none())?;
+            (value.expr.clone(), p.input().clone())
+        };
+        let join = join_plan.as_any().downcast_ref::<HashJoinExec>()?;
+        if *join.join_type() != JoinType::Inner || join.filter().is_some() {
+            return None;
+        }
+        let lhs = join.left().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let rhs = join.right().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let (op, _, _, return_bool) = binop_of(&expr)?;
+        let mut on = Vec::new();
+        let mut has_ts = false;
+        for (l, r) in join.on() {
+            let (l, r) = (l.as_any().downcast_ref::<Column>()?, r.as_any().downcast_ref::<Column>()?);
+            if l.name() != r.name() {
+                return None;
+            }
+            if l.name() == rhs.params().time_index_column {
+                has_ts = true;
+            } else {
+                on.push(l.name().to_string());
+            }
+        }
+        if !has_ts {
+            return None;
+        }
+        // a projection emits the tag columns of one side: the lhs's when every projected tag column is on the lhs of the
+        // join's output schema (planner.rs:696-711)
+        let label_side = match plan.as_any().downcast_ref::<ProjectionExec>() {
+            Some(p) => {
+                let n_left = join.left().schema().fields().len();
+                let from_left = p.expr().iter().filter_map(|e| e.expr.as_any().downcast_ref::<Column>()).all(|c| c.index() < n_left);
+                if from_left { "lhs" } else { "rhs" }
+            }
+            None => "lhs",
+        };
+        Some(GpuPromBinarySpec { op, return_bool, lhs: lhs.params().clone(), rhs: rhs.params().clone(), on, label_side })
+    }
+}
+
 /// The scalar UDF arguments the kernels take as (param0, param1); `None` when an argument is not a literal.
 fn scalar_params(function: &str, args: &[Arc<dyn PhysicalExpr>]) -> Option<(f64, f64)> {
     let lit = |e: &Arc<dyn PhysicalExpr>| -> Option<f64> {
@@ -158,7 +310,10 @@ impl PhysicalOptimizerRule for GpuPromRewrite {
     fn optimize(&self, plan: Arc<dyn ExecutionPlan>, _config: &ConfigOptions) -> DataFusionResult<Arc<dyn ExecutionPlan>> {
         plan.transform_down(|node| {
             // the widest match first: aggregate over the range sub-tree, then the range sub-tree alone
-            let matched = self.match_aggregate(&node).or_else(|| self.match_range_subtree(&node));
+            let matched = self
+                .match_aggregate(&node)
+                .or_else(|| self.match_range_subtree(&node))
+                .or_else(|| self.match_scalar_op(&node));
             match matched {
                 Some((params, input)) => {
                     // the replaced node's schema is kept verbatim, so parents (Sort, CoalesceBatches, MergeScan ..) see no change

@@ -1,7 +1,7 @@
 /* Compile-time check of every layout assumption rust-shim/src/ffi.rs makes about include/b200promql.h.
  *   gcc -std=c11 -fsyntax-only -I../../include layout.c        (tests/test_abi.py runs exactly this)
  * If a field of struct b2p_range_params moves, or an enum value changes, this file stops compiling — and
- * B2pRangeParams / B2pFn / B2pAgg in ffi.rs have to follow. */
+ * B2pRangeParams / B2pFn / B2pAgg / B2pBinOp in ffi.rs have to follow. */
 #include <stddef.h>
 #include <stdint.h>
 
@@ -32,6 +32,11 @@ SA(B2P_FN_QUANTILE_OVER_TIME == 19 && B2P_FN_HOLT_WINTERS == 20 && B2P_FN__COUNT
 /* #[repr(i32)] enum B2pAgg */
 SA(B2P_AGG_SUM == 0 && B2P_AGG_AVG == 1 && B2P_AGG_COUNT == 2 && B2P_AGG_MIN == 3 && B2P_AGG_MAX == 4, "B2pAgg 0-4");
 SA(B2P_AGG_STDDEV == 5 && B2P_AGG_STDVAR == 6, "B2pAgg 5-6");
+/* #[repr(i32)] enum B2pBinOp: arithmetic 0-6, comparisons 7-12 (B2pBinOp::is_comparison tests >= Eq) */
+SA(B2P_OP_ADD == 0 && B2P_OP_SUB == 1 && B2P_OP_MUL == 2 && B2P_OP_DIV == 3 && B2P_OP_MOD == 4, "B2pBinOp 0-4");
+SA(B2P_OP_POW == 5 && B2P_OP_ATAN2 == 6 && B2P_OP_EQ == 7 && B2P_OP_NE == 8 && B2P_OP_GT == 9, "B2pBinOp 5-9");
+SA(B2P_OP_LT == 10 && B2P_OP_GE == 11 && B2P_OP_LE == 12, "B2pBinOp 10-12");
+SA(sizeof(enum b2p_binop) == 4, "b2p_binop is passed as i32");
 /* status codes and sizes the shim hard-codes */
 SA(B2P_OK == 0 && B2P_E_INVALID == -1 && B2P_E_CUDA == -2 && B2P_E_UNSORTED == -3 && B2P_E_NOMEM == -4 && B2P_E_TOO_LARGE == -5, "codes");
 SA(B2P_COMM_ID_BYTES == 128, "communicator id");
