@@ -26,6 +26,7 @@ EXPORTED_SYMBOLS = [
     "b2p_binary_op_dev", "b2p_scalar_op_dev", "b2p_count_valid_words_dev", "b2p_binary_op", "b2p_scalar_op",
     "b2p_plan_range_create", "b2p_plan_set_instant", "b2p_plan_set_histogram_quantile", "b2p_plan_push_batch", "b2p_plan_execute", "b2p_plan_num_series", "b2p_plan_destroy",
     "b2p_plan_last_error", "b2p_plan_set_scalar_op", "b2p_plan_binary_create",
+    "b2p_setop_dev", "b2p_setop", "b2p_plan_setop_create",
 ]
 
 
@@ -115,6 +116,9 @@ def load() -> C.CDLL:
         "b2p_plan_last_error": (C.c_char_p, []),
         "b2p_plan_set_scalar_op": (C.c_int, [vp, i32, dbl, i32, i32]),
         "b2p_plan_binary_create": (vp, [vp, i32, i32, vp, vp, C.c_char_p, C.POINTER(C.c_char_p), i32, C.c_char_p]),
+        "b2p_setop_dev": (C.c_int, [vp, i32, vp, vp, vp, u32, vp, vp, vp, u32, u32, u64, vp, vp]),
+        "b2p_setop": (C.c_int, [vp, i32, vp, vp, vp, u32, vp, vp, vp, u32, u32, u64, vp, vp]),
+        "b2p_plan_setop_create": (vp, [vp, i32, vp, vp, C.c_char_p, C.POINTER(C.c_char_p), i32]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)  # AttributeError here means the .so does not match the header

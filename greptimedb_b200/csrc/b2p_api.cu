@@ -21,6 +21,7 @@
 #include "../../include/b200promql.h"
 #include "b2p_aggregate.cuh"
 #include "b2p_binary.cuh"
+#include "b2p_setop.cuh"
 #include "b2p_kernel_t.cuh"
 #include "b2p_kernel_lean.cuh"
 #include "b2p_kernels.cuh"
@@ -134,6 +135,7 @@ constexpr size_t kArenaDefaultRows = 1u << 21;  // 32 MB: regions of 3 971 rows 
 // error of a non-zero Status::k0_errors word
 int k0_fail(uint32_t k0) {
   if (k0 & kBinRowError) return fail(B2P_E_INVALID, "binary operator: a pair's row index is out of range");
+  if (k0 & kSetKeyError) return fail(B2P_E_INVALID, "set operator: a row's key is >= n_keys");
   if (k0 & 1u) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");
   return fail(B2P_E_UNSORTED, "series id >= n_series");
 }
@@ -229,6 +231,8 @@ struct b2p_ctx {
   DevBuf c_psum, c_pcnt;
   // host-API staging of the binary operators: lhs, lhs validity, lhs rows, rhs, rhs validity, rhs rows, out, out validity
   DevBuf bin[8];
+  // set operators: the key -> member-row CSR of each side and the per-key validity mask
+  DevBuf s_goff[2], s_members[2], s_mask;
   int fast_blocks_per_sm[B2P_FN__COUNT][2] = {};
   int big_blocks_per_sm[B2P_FN__COUNT] = {};
 };
@@ -613,15 +617,16 @@ int check_binop(int32_t op, int32_t return_bool) {
   return B2P_OK;
 }
 
-// clears bit kBinRowError of the status word after a synchronous call has read it; B2P_E_INVALID when it was set
-int take_bin_row_error(b2p_ctx* c) {
+// clears `bit` (kBinRowError / kSetKeyError) of the status word after a synchronous call has read it; B2P_E_INVALID
+// when it was set
+int take_row_error(b2p_ctx* c, uint32_t bit) {
   CU(cudaMemcpyAsync(c->h_k0, c->d_k0, sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   const uint32_t k0 = c->h_k0->k0_errors;
-  if (!(k0 & kBinRowError)) return B2P_OK;
-  const uint32_t rest = k0 & ~kBinRowError;
+  if (!(k0 & bit)) return B2P_OK;
+  const uint32_t rest = k0 & ~bit;
   CU(cudaMemcpy(&c->d_k0->k0_errors, &rest, sizeof rest, cudaMemcpyHostToDevice));
-  return k0_fail(kBinRowError);
+  return k0_fail(bit);
 }
 
 }  // namespace
@@ -720,6 +725,7 @@ void b2p_destroy(b2p_ctx* c) {
   }
   c->p_status.release();
   for (DevBuf& b : c->bin) b.release();
+  for (DevBuf* b : {&c->s_goff[0], &c->s_goff[1], &c->s_members[0], &c->s_members[1], &c->s_mask}) b->release();
   if (c->s_h2d) cudaStreamDestroy(c->s_h2d);
   if (c->s_d2h) cudaStreamDestroy(c->s_d2h);
   if (c->d_ring) cudaFree(c->d_ring);
@@ -1596,6 +1602,125 @@ int b2p_count_valid_words_dev(b2p_ctx* c, const uint32_t* cnt, uint64_t n_rows, 
   return B2P_OK;
 }
 
+/* ---- set operators ------------------------------------------------------------------------------------------- */
+}  // extern "C"
+
+namespace {
+// CTAs of 8 warps for `units` warp units, at most 16 per SM (grid-stride beyond)
+unsigned warp_grid(const b2p_ctx* c, uint64_t units) {
+  const uint64_t blocks = (units + 7) / 8, cap = (uint64_t)c->num_sms * 16;
+  return (unsigned)(blocks < cap ? blocks : cap);
+}
+
+int setop_key_check(b2p_ctx* c, const uint32_t* key, uint32_t n, uint32_t n_keys) {
+  if (n == 0) return B2P_OK;
+  const uint64_t blocks = ((uint64_t)n + 255) / 256, cap = (uint64_t)c->num_sms * 8;
+  setop_key_check_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, c->stream>>>(key, n, n_keys, c->d_k0);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// the rows of one side grouped by key (CSR s_goff[side] / s_members[side], members in row order: the sort is stable)
+int setop_group(b2p_ctx* c, int side, const uint32_t* key, uint32_t n_rows, uint32_t n_keys) {
+  int rc;
+  if ((rc = c->s_goff[side].ensure(((size_t)n_keys + 1) * 4))) return rc;
+  if ((rc = c->s_members[side].ensure((size_t)(n_rows ? n_rows : 1) * 4))) return rc;
+  return build_group_csr(c, key, n_rows, n_keys, c->s_goff[side].as<uint32_t>(), c->s_members[side].as<uint32_t>());
+}
+
+// s_mask[g] = OR of the validity words of side `side`'s rows with key g
+int setop_mask(b2p_ctx* c, int side, const uint32_t* valid, uint32_t n_keys, uint32_t Tw) {
+  const unsigned grid = warp_grid(c, (uint64_t)n_keys * ((Tw + 31) / 32));
+  if (grid == 0) return B2P_OK;
+  setop_mask_kernel<<<grid, 256, 0, c->stream>>>(valid, c->s_goff[side].as<uint32_t>(), c->s_members[side].as<uint32_t>(),
+                                                 n_keys, Tw, c->s_mask.as<uint32_t>());
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+template <int MODE>
+int setop_copy(b2p_ctx* c, const SetCopyArgs& a, bool vec) {
+  const uint64_t steps = vec ? 64 : 32;
+  const unsigned grid = warp_grid(c, a.n_rows * ((a.T + steps - 1) / steps));
+  if (grid == 0) return B2P_OK;
+  if (vec) setop_copy_kernel<MODE, true><<<grid, 256, 0, c->stream>>>(a);
+  else setop_copy_kernel<MODE, false><<<grid, 256, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+int setop_run(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key,
+              uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid, const uint32_t* rhs_key,
+              uint32_t n_rhs_rows, uint32_t n_keys, uint64_t T, double* out, uint32_t* out_valid) {
+  int rc;
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  if ((rc = setop_key_check(c, lhs_key, n_lhs_rows, n_keys)) || (rc = setop_key_check(c, rhs_key, n_rhs_rows, n_keys)))
+    return rc;
+  if (n_keys > 0 && (rc = c->s_mask.ensure((size_t)n_keys * Tw * 4))) return rc;
+  const bool vec = (T % 2) == 0 && aligned16(lhs) && aligned16(out) && (op != kSetOr || aligned16(rhs));
+  SetCopyArgs a{};
+  a.src = lhs; a.svalid = lhs_valid; a.key = lhs_key; a.n_rows = n_lhs_rows; a.n_keys = n_keys;
+  a.mask = c->s_mask.as<uint32_t>(); a.T = T; a.Tw = Tw; a.out = out; a.out_valid = out_valid;
+  if (op != kSetOr) {
+    if (n_keys > 0) {
+      if ((rc = setop_group(c, 1, rhs_key, n_rhs_rows, n_keys)) || (rc = setop_mask(c, 1, rhs_valid, n_keys, Tw))) return rc;
+    }
+    return op == kSetAnd ? setop_copy<kCopyAnd>(c, a, vec) : setop_copy<kCopyUnless>(c, a, vec);
+  }
+  // or: the steps each key's lhs rows claim, then the rhs words deduplicated into the rhs part of out_valid
+  uint32_t* rwords = out_valid + (size_t)n_lhs_rows * Tw;
+  if (n_keys > 0) {
+    if ((rc = setop_group(c, 0, lhs_key, n_lhs_rows, n_keys)) || (rc = setop_mask(c, 0, lhs_valid, n_keys, Tw)) ||
+        (rc = setop_group(c, 1, rhs_key, n_rhs_rows, n_keys)))
+      return rc;
+    const unsigned grid = warp_grid(c, (uint64_t)n_keys * ((Tw + 31) / 32));
+    setop_dedupe_kernel<<<grid, 256, 0, c->stream>>>(rhs_valid, c->s_goff[1].as<uint32_t>(), c->s_members[1].as<uint32_t>(),
+                                                     c->s_mask.as<uint32_t>(), n_keys, Tw, rwords);
+    c->launches++;
+    CU(cudaGetLastError());
+  }
+  if ((rc = setop_copy<kCopyKeep>(c, a, vec))) return rc;
+  SetCopyArgs b = a;
+  b.src = rhs; b.svalid = rhs_valid; b.key = rhs_key; b.n_rows = n_rhs_rows; b.mask = nullptr; b.words = rwords;
+  b.out = out + (size_t)n_lhs_rows * T; b.out_valid = rwords;
+  return setop_copy<kCopyWords>(c, b, vec);
+}
+
+int check_setop_args(int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key, uint32_t n_lhs_rows,
+                     const double* rhs, const uint32_t* rhs_valid, const uint32_t* rhs_key, uint32_t n_rhs_rows,
+                     double* out, uint32_t* out_valid) {
+  if (op < kSetAnd || op > kSetUnless) return fail(B2P_E_INVALID, "unknown set operator %d", op);
+  const uint64_t n_out = op == kSetOr ? (uint64_t)n_lhs_rows + n_rhs_rows : n_lhs_rows;
+  if (n_out > UINT32_MAX) return fail(B2P_E_INVALID, "set operator: more than 2^32 - 1 output rows");
+  if ((n_lhs_rows && (!lhs || !lhs_valid || !lhs_key)) || (n_rhs_rows && (!rhs_valid || !rhs_key)) ||
+      (n_rhs_rows && op == kSetOr && !rhs) || (n_out && (!out || !out_valid)))
+    return fail(B2P_E_INVALID, "NULL argument");
+  return B2P_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_setop_dev(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key,
+                  uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid, const uint32_t* rhs_key,
+                  uint32_t n_rhs_rows, uint32_t n_keys, uint64_t T, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int rc;
+  if ((rc = check_setop_args(op, lhs, lhs_valid, lhs_key, n_lhs_rows, rhs, rhs_valid, rhs_key, n_rhs_rows, out,
+                             out_valid)))
+    return rc;
+  if (T == 0) return B2P_OK;
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  rc = setop_run(c, op, lhs, lhs_valid, lhs_key, n_lhs_rows, rhs, rhs_valid, rhs_key, n_rhs_rows, n_keys, T, out,
+                 out_valid);
+  stage_end(c, 3);
+  return rc;
+}
+
 int b2p_synth_fill_dev(b2p_ctx* c, uint64_t series_begin, uint64_t n_series, uint32_t n_samples, int64_t t0,
                        int64_t scrape_ms, uint32_t jitter_ms, int32_t with_resets, uint64_t seed, int64_t* ts,
                        double* val, uint32_t* sid) {
@@ -2150,7 +2275,7 @@ int b2p_binary_op(b2p_ctx* c, int32_t op, int32_t return_bool, const double* lhs
     return rc;
   CU(cudaMemcpyAsync(out, c->bin[6].p, bytes[6], cudaMemcpyDeviceToHost, c->stream));
   CU(cudaMemcpyAsync(out_valid, c->bin[7].p, bytes[7], cudaMemcpyDeviceToHost, c->stream));
-  return take_bin_row_error(c);  // (synchronises)
+  return take_row_error(c, kBinRowError);  // (synchronises)
 }
 
 int b2p_scalar_op(b2p_ctx* c, int32_t op, int32_t return_bool, int32_t scalar_on_left, double scalar, const double* vals,
@@ -2173,6 +2298,34 @@ int b2p_scalar_op(b2p_ctx* c, int32_t op, int32_t return_bool, int32_t scalar_on
   CU(cudaMemcpyAsync(out_valid, c->bin[7].p, wb, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   return B2P_OK;
+}
+
+int b2p_setop(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key,
+              uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid, const uint32_t* rhs_key,
+              uint32_t n_rhs_rows, uint32_t n_keys, uint64_t T, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int rc;
+  if ((rc = check_setop_args(op, lhs, lhs_valid, lhs_key, n_lhs_rows, rhs, rhs_valid, rhs_key, n_rhs_rows, out,
+                             out_valid)))
+    return rc;
+  if (T == 0) return B2P_OK;
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  const size_t nl = n_lhs_rows, nr = n_rhs_rows, no = op == kSetOr ? nl + nr : nl;
+  const bool rvals = op == kSetOr && rhs;  // and / unless never read the rhs values
+  const size_t bytes[8] = {nl * T * 8, nl * Tw * 4, nl * 4, rvals ? nr * T * 8 : 0, nr * Tw * 4, nr * 4, no * T * 8, no * Tw * 4};
+  for (int i = 0; i < 8; ++i)
+    if ((rc = c->bin[i].ensure(bytes[i] ? bytes[i] : 16))) return rc;
+  const void* src[6] = {lhs, lhs_valid, lhs_key, rhs, rhs_valid, rhs_key};
+  for (int i = 0; i < 6; ++i)
+    if (bytes[i]) CU(cudaMemcpyAsync(c->bin[i].p, src[i], bytes[i], cudaMemcpyHostToDevice, c->stream));
+  if ((rc = b2p_setop_dev(c, op, c->bin[0].as<double>(), c->bin[1].as<uint32_t>(), c->bin[2].as<uint32_t>(), n_lhs_rows,
+                          c->bin[3].as<double>(), c->bin[4].as<uint32_t>(), c->bin[5].as<uint32_t>(), n_rhs_rows, n_keys,
+                          T, c->bin[6].as<double>(), c->bin[7].as<uint32_t>())))
+    return rc;
+  if (bytes[6]) CU(cudaMemcpyAsync(out, c->bin[6].p, bytes[6], cudaMemcpyDeviceToHost, c->stream));
+  if (bytes[7]) CU(cudaMemcpyAsync(out_valid, c->bin[7].p, bytes[7], cudaMemcpyDeviceToHost, c->stream));
+  return take_row_error(c, kSetKeyError);  // (synchronises)
 }
 
 }  // extern "C"

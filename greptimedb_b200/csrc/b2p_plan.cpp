@@ -41,12 +41,18 @@ bool starts_with(const char* s, const char* p) { return std::strncmp(s, p, std::
 
 bool bit_set(const uint8_t* bits, int64_t i) { return bits == nullptr || ((bits[i >> 3] >> (i & 7)) & 1); }
 
+// a NULL label: distinct from every string, equal to every other NULL label (NullEquality::NullEqualsNull)
+const std::string kNullLabel("\0null", 5);
+constexpr int64_t kArrowFlagNullable = 2;  // ARROW_FLAG_NULLABLE of the C Data Interface
+
 // ---- export helpers: an ArrowArray whose buffers live in a heap object ---------------------------------
 struct OwnedColumn {
   std::vector<int64_t> i64;
   std::vector<double> f64;
   std::vector<int32_t> offsets;
   std::string chars;
+  std::vector<uint8_t> validity;  // Utf8 tags: bit i clear = row i is NULL (allocated at the first NULL)
+  int64_t nulls = 0;
   const void* buffers[3] = {nullptr, nullptr, nullptr};
 };
 struct OwnedBatch {
@@ -248,7 +254,7 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
   auto tag_at = [&](size_t t, int64_t row) -> std::string {
     const TagCol& tc = tcols[t];
     const int64_t r = tc.base + row;
-    if (!bit_set(tc.valid, r)) return std::string("\0null", 5);  // NULL label: distinct from every string
+    if (!bit_set(tc.valid, r)) return kNullLabel;
     return std::string(tc.data + tc.off[r], (size_t)(tc.off[r + 1] - tc.off[r]));
   };
 
@@ -504,15 +510,36 @@ std::string float_literal(double x) {
   return "Float64(" + std::string(buf, res.ptr) + ")";
 }
 
-// the key tuple of row r over the given tag columns, length-prefixed so that no two tuples share an encoding
+// the key tuple of row r over the given tag columns (-1: a tag the node lacks, read as NULL), length-prefixed so that
+// no two tuples share an encoding
 void append_key(const NodeResult& n, const std::vector<int>& cols, uint32_t r, std::string& key) {
   key.clear();
   for (int c : cols) {
-    const std::string v = n.id_keyed ? std::to_string(n.ids[r]) : n.tags[(size_t)c][r];
+    const std::string v = c < 0 ? kNullLabel : n.id_keyed ? std::to_string(n.ids[r]) : n.tags[(size_t)c][r];
     key += std::to_string(v.size());
     key.push_back(':');
     key += v;
   }
+}
+
+// the tags a matching modifier keeps: those listed in `labels` for On, those not listed for Ignoring, all for None
+std::vector<std::string> narrow_tags(const std::vector<std::string>& tags, Matching m, const std::vector<std::string>& labels) {
+  std::vector<std::string> out;
+  for (const std::string& t : tags) {
+    const bool listed = std::find(labels.begin(), labels.end(), t) != labels.end();
+    if (m == Matching::On ? listed : !(m == Matching::Ignoring && listed)) out.push_back(t);
+  }
+  return out;
+}
+
+// the column of each name among n's tags; -1 where n has no such tag
+std::vector<int> tag_columns(const NodeResult& n, const std::vector<std::string>& names) {
+  std::vector<int> cols;
+  for (const std::string& name : names) {
+    const auto it = std::find(n.tag_names.begin(), n.tag_names.end(), name);
+    cols.push_back(it == n.tag_names.end() ? -1 : (int)(it - n.tag_names.begin()));
+  }
+  return cols;
 }
 
 void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema) {
@@ -531,10 +558,30 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       if (!r.id_keyed) c_tags.back()->offsets.push_back(0);
     }
   };
-  if (r.tags_first) add_tags();
-  OwnedColumn* c_ts = add_col(r.time_index, "tsm:");
-  OwnedColumn* c_val = add_col(r.value_name, "g");
-  if (!r.tags_first) add_tags();
+  OwnedColumn* c_ts = nullptr;
+  OwnedColumn* c_val = nullptr;
+  if (r.sorted_columns) {  // {time index, then the tags and the value column in name order}
+    c_ts = add_col(r.time_index, "tsm:");
+    std::vector<std::string> names = r.tag_names;
+    names.push_back(r.value_name);
+    std::sort(names.begin(), names.end());
+    std::vector<OwnedColumn*> by_tag(r.tag_names.size());
+    for (const std::string& name : names) {
+      if (name == r.value_name && !c_val) {
+        c_val = add_col(name, "g");
+        continue;
+      }
+      const size_t t = (size_t)(std::find(r.tag_names.begin(), r.tag_names.end(), name) - r.tag_names.begin());
+      by_tag[t] = add_col(name, r.id_keyed ? "L" : "u");
+      if (!r.id_keyed) by_tag[t]->offsets.push_back(0);
+    }
+    c_tags = by_tag;
+  } else {
+    if (r.tags_first) add_tags();
+    c_ts = add_col(r.time_index, "tsm:");
+    c_val = add_col(r.value_name, "g");
+    if (!r.tags_first) add_tags();
+  }
   int64_t n_out = 0;
   for (uint32_t row = 0; row < r.rows; ++row)
     for (int64_t k = 0; k < r.T; ++k) {
@@ -545,8 +592,16 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
         if (r.id_keyed) {
           c_tags[t]->i64.push_back((int64_t)r.ids[row]);
         } else {
-          c_tags[t]->chars += r.tags[t][row];
-          c_tags[t]->offsets.push_back((int32_t)c_tags[t]->chars.size());
+          OwnedColumn* c = c_tags[t];
+          const std::string& v = r.tags[t][row];
+          if (v == kNullLabel) {  // a real Arrow null
+            if (c->validity.size() <= (size_t)(n_out >> 3)) c->validity.resize((size_t)(n_out >> 3) + 1, 0xFF);
+            c->validity[(size_t)n_out >> 3] &= (uint8_t)~(1u << (n_out & 7));
+            ++c->nulls;
+          } else {
+            c->chars += v;
+          }
+          c->offsets.push_back((int32_t)c->chars.size());
         }
       }
       ++n_out;
@@ -569,6 +624,11 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     if (fmt == "u") {
       if (c->offsets.empty()) c->offsets.push_back(0);
       c->buffers[0] = nullptr;
+      if (c->nulls > 0) {
+        c->validity.resize((size_t)(n_out + 7) / 8, 0xFF);
+        c->buffers[0] = c->validity.data();
+        a.null_count = c->nulls;
+      }
       c->buffers[1] = c->offsets.data();
       c->buffers[2] = c->chars.data();
       a.n_buffers = 3;
@@ -584,7 +644,7 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     std::memset(&sc, 0, sizeof sc);
     sc.format = os->formats[i].c_str();
     sc.name = os->names[i].c_str();
-    sc.flags = 0;
+    sc.flags = c->nulls > 0 ? kArrowFlagNullable : 0;
     sc.release = release_child_schema;
     os->child_ptrs[i] = &sc;
   }
@@ -660,15 +720,11 @@ void BinaryPlan::compute(NodeResult& r) {
     lcols.push_back(0);
     rcols.push_back(0);
   } else if (!L.tag_names.empty() && !R.tag_names.empty()) {
-    for (size_t t = 0; t < R.tag_names.size(); ++t) {
-      const std::string& name = R.tag_names[t];
-      const bool listed = std::find(labels_.begin(), labels_.end(), name) != labels_.end();
-      if (matching_ == Matching::On ? !listed : (matching_ == Matching::Ignoring && listed)) continue;
-      const auto li = std::find(L.tag_names.begin(), L.tag_names.end(), name);
-      if (li == L.tag_names.end()) throw PlanError(ErrorKind::Plan, "No field named " + name);
-      lcols.push_back((int)(li - L.tag_names.begin()));
-      rcols.push_back((int)t);
-    }
+    const std::vector<std::string> names = narrow_tags(R.tag_names, matching_, labels_);
+    lcols = tag_columns(L, names);
+    rcols = tag_columns(R, names);
+    for (size_t i = 0; i < names.size(); ++i)
+      if (lcols[i] < 0) throw PlanError(ErrorKind::Plan, "No field named " + names[i]);
   }
   // hash join of the series: rhs rows by key (in row order), then every lhs row in order against its key's rhs rows
   std::unordered_map<std::string, std::vector<uint32_t>> rhs_by_key;
@@ -724,10 +780,163 @@ void BinaryPlan::compute(NodeResult& r) {
   }
   if (filter) {
     r.tags_first = L.tags_first;
+    r.sorted_columns = L.sorted_columns;
     r.value_name = L.value_name;
   } else {
     r.tags_first = true;
     r.value_name = L.value_name + " " + kOpSymbols[op_] + " " + R.value_name;
+  }
+}
+
+// ---- SetOpPlan -----------------------------------------------------------------------------------------
+namespace {
+
+const char* const kSetNames[] = {"and", "or", "unless"};
+
+// dense ids of key tuples, in first-insertion order
+struct KeyIds {
+  std::unordered_map<std::string, uint32_t> ids;
+  uint32_t add(const std::string& k) { return ids.emplace(k, (uint32_t)ids.size()).first->second; }
+  uint32_t find(const std::string& k) const {
+    const auto it = ids.find(k);
+    return it == ids.end() ? B2P_NO_KEY : it->second;
+  }
+};
+
+// left.distinct() of `and` / `unless` (planner.rs:3549-3703): a cell whose labels, step and value bits (DataFusion's
+// group equality on f64) equal those of a cell of an earlier row is dropped.  Only rows that share a label tuple can
+// hold such cells, so only they are compared.
+void drop_duplicate_cells(NodeResult& n) {
+  if (n.rows < 2 || n.T == 0) return;
+  std::vector<int> all(n.tag_names.size());
+  std::iota(all.begin(), all.end(), 0);
+  std::unordered_map<std::string, std::vector<uint32_t>> by_labels;
+  std::string key;
+  for (uint32_t q = 0; q < n.rows; ++q) {
+    append_key(n, all, q, key);
+    by_labels[key].push_back(q);
+  }
+  for (const auto& kv : by_labels) {
+    const std::vector<uint32_t>& g = kv.second;
+    for (size_t i = 1; i < g.size(); ++i)
+      for (int64_t k = 0; k < n.T; ++k) {
+        if (!n.valid_at(g[i], k)) continue;
+        const double x = n.val[(size_t)g[i] * (size_t)n.T + (size_t)k];
+        for (size_t j = 0; j < i; ++j) {
+          const double y = n.val[(size_t)g[j] * (size_t)n.T + (size_t)k];
+          if (n.valid_at(g[j], k) && std::memcmp(&x, &y, sizeof x) == 0) {
+            n.valid[(size_t)g[i] * n.Tw + (size_t)(k >> 5)] &= ~(1u << (k & 31));
+            n.val[(size_t)g[i] * (size_t)n.T + (size_t)k] = 0.0;
+            break;
+          }
+        }
+      }
+  }
+}
+
+void check_setop(int rc) {
+  if (rc == B2P_E_INVALID) throw PlanError(ErrorKind::Plan, b2p_last_error());
+  if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
+}
+
+}  // namespace
+
+SetOpPlan::SetOpPlan(b2p_ctx* ctx, int op, std::shared_ptr<PlanNode> lhs, std::shared_ptr<PlanNode> rhs,
+                     Matching matching, std::vector<std::string> labels)
+    : PlanNode(ctx), op_(op), lhs_(std::move(lhs)), rhs_(std::move(rhs)), matching_(matching), labels_(std::move(labels)) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromSetOpExec: NULL context");
+  if (!lhs_ || !rhs_) throw PlanError(ErrorKind::Plan, "GpuPromSetOpExec: NULL child");
+  if (op_ < B2P_SET_AND || op_ > B2P_SET_UNLESS) throw PlanError(ErrorKind::Plan, "unknown set operator " + std::to_string(op_));
+}
+
+void SetOpPlan::compute(NodeResult& r) {
+  NodeResult L, R;
+  lhs_->run(L);
+  rhs_->run(R);
+  const std::string what = std::string("set operator `") + kSetNames[op_] + "`: ";
+  if (L.T != R.T || (L.rows > 0 && R.rows > 0 && L.eval_ts != R.eval_ts))
+    throw PlanError(ErrorKind::Plan, what + "both sides must be evaluated on the same steps");
+  // the reference matches set operators on label values (planner.rs:3626-3630), which an id-keyed node does not carry
+  if (L.id_keyed || R.id_keyed) throw PlanError(ErrorKind::Plan, what + "an id-keyed (__tsid) side has no label values to match");
+  const int64_t T = L.T;
+  std::vector<std::string> names;  // match columns
+  std::vector<std::string> all;    // `or`: the union of both sides' tags, sorted
+  if (op_ != B2P_SET_OR) {
+    // each side's tags narrowed by on / ignoring; the two key sets must be equal (CombineTableColumnMismatch)
+    names = narrow_tags(L.tag_names, matching_, labels_);
+    std::vector<std::string> rn = narrow_tags(R.tag_names, matching_, labels_);
+    std::sort(names.begin(), names.end());
+    std::sort(rn.begin(), rn.end());
+    if (names != rn) {
+      auto list = [](const std::vector<std::string>& v) {
+        std::string s;
+        for (const std::string& x : v) s += (s.empty() ? "" : ", ") + x;
+        return "[" + s + "]";
+      };
+      throw PlanError(ErrorKind::Plan, what + "the key columns of the two sides differ: " + list(names) + " vs " + list(rn));
+    }
+  } else {
+    all = L.tag_names;
+    all.insert(all.end(), R.tag_names.begin(), R.tag_names.end());
+    std::sort(all.begin(), all.end());
+    all.erase(std::unique(all.begin(), all.end()), all.end());
+    if (matching_ == Matching::On) {
+      names = labels_;
+      for (const std::string& l : names)
+        if (!std::binary_search(all.begin(), all.end(), l)) throw PlanError(ErrorKind::Plan, what + "Column " + l + " not found");
+    } else {
+      names = narrow_tags(all, matching_, labels_);
+    }
+  }
+  const std::vector<int> lcols = tag_columns(L, names), rcols = tag_columns(R, names);
+  KeyIds keys;
+  std::vector<uint32_t> lkey(L.rows), rkey(R.rows);
+  std::string key;
+  if (op_ == B2P_SET_OR) {
+    for (uint32_t q = 0; q < L.rows; ++q) {
+      append_key(L, lcols, q, key);
+      lkey[q] = keys.add(key);
+    }
+  }
+  for (uint32_t q = 0; q < R.rows; ++q) {
+    append_key(R, rcols, q, key);
+    rkey[q] = keys.add(key);
+  }
+  if (op_ != B2P_SET_OR) {
+    for (uint32_t q = 0; q < L.rows; ++q) {
+      append_key(L, lcols, q, key);
+      lkey[q] = keys.find(key);
+    }
+    drop_duplicate_cells(L);
+    if (L.rows > 0 && T > 0)
+      check_setop(b2p_setop(ctx_, op_, L.val.data(), L.valid.data(), lkey.data(), L.rows, nullptr, R.valid.data(),
+                            rkey.data(), R.rows, (uint32_t)keys.ids.size(), (uint64_t)T, L.val.data(), L.valid.data()));
+    r = std::move(L);  // the lhs rows, columns and values
+    return;
+  }
+  // or: the lhs rows, then the rhs rows, over the union of the tags (NULL where a side lacks one)
+  const uint64_t n = (uint64_t)L.rows + R.rows;
+  if (n > UINT32_MAX) throw PlanError(ErrorKind::Plan, what + "more than 2^32 - 1 rows");
+  r = NodeResult();
+  r.T = T;
+  r.Tw = L.Tw;
+  r.rows = (uint32_t)n;
+  r.eval_ts = L.rows > 0 ? L.eval_ts : R.eval_ts;
+  r.val.assign((size_t)n * (size_t)T, 0.0);
+  r.valid.assign((size_t)n * r.Tw, 0u);
+  if (n > 0 && T > 0)
+    check_setop(b2p_setop(ctx_, op_, L.val.data(), L.valid.data(), lkey.data(), L.rows, R.val.data(), R.valid.data(),
+                          rkey.data(), R.rows, (uint32_t)keys.ids.size(), (uint64_t)T, r.val.data(), r.valid.data()));
+  r.time_index = L.time_index;
+  r.value_name = L.value_name;
+  r.tag_names = all;
+  r.sorted_columns = true;
+  const std::vector<int> lall = tag_columns(L, all), rall = tag_columns(R, all);
+  r.tags.resize(all.size());
+  for (size_t t = 0; t < all.size(); ++t) {
+    r.tags[t].reserve((size_t)n);
+    for (uint32_t q = 0; q < L.rows; ++q) r.tags[t].push_back(lall[t] < 0 ? kNullLabel : L.tags[(size_t)lall[t]][q]);
+    for (uint32_t q = 0; q < R.rows; ++q) r.tags[t].push_back(rall[t] < 0 ? kNullLabel : R.tags[(size_t)rall[t]][q]);
   }
 }
 
@@ -808,6 +1017,32 @@ b2p_plan* b2p_plan_binary_create(b2p_ctx* ctx, int32_t op, int32_t return_bool, 
     auto* h = new b2p_plan();
     try {
       h->node = std::make_shared<b2p::BinaryPlan>(ctx, op, return_bool != 0, lhs->node, rhs->node, m, std::move(ls), from_lhs);
+    } catch (...) {
+      delete h;
+      throw;
+    }
+    return h;
+  } catch (const b2p::PlanError& e) {
+    plan_fail(e);
+  } catch (const std::exception& e) {
+    g_err = e.what();
+  }
+  return nullptr;
+}
+
+b2p_plan* b2p_plan_setop_create(b2p_ctx* ctx, int32_t op, b2p_plan* lhs, b2p_plan* rhs, const char* matching,
+                                const char* const* labels, int32_t n_labels) {
+  try {
+    if (!lhs || !rhs || (n_labels > 0 && !labels)) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    b2p::Matching m = b2p::Matching::None;
+    if (matching && std::strcmp(matching, "on") == 0) m = b2p::Matching::On;
+    else if (matching && std::strcmp(matching, "ignoring") == 0) m = b2p::Matching::Ignoring;
+    else if (matching && matching[0]) throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("unknown matching ") + matching);
+    std::vector<std::string> ls;
+    for (int32_t i = 0; i < n_labels; ++i) ls.emplace_back(labels[i]);
+    auto* h = new b2p_plan();
+    try {
+      h->node = std::make_shared<b2p::SetOpPlan>(ctx, op, lhs->node, rhs->node, m, std::move(ls));
     } catch (...) {
       delete h;
       throw;

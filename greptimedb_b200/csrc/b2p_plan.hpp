@@ -92,6 +92,7 @@ struct NodeResult {
   bool id_keyed = false;                       // the one tag column is a UInt64 id (values in `ids`, not `tags`)
   std::vector<uint64_t> ids;                   // [row] when id_keyed
   bool tags_first = false;                     // columns {tags.., time index, value} instead of {time index, value, tags..}
+  bool sorted_columns = false;                 // columns {time index, then tags and value sorted by name} (`or`)
   bool valid_at(uint32_t r, int64_t k) const { return (valid[(size_t)r * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u; }
 };
 
@@ -161,12 +162,15 @@ class PromRangePlan : public PlanNode {
   bool have_last_ = false;
 };
 
+// Label matching modifier of a binary or set operator
+enum class Matching { None, On, Ignoring };
+
 // Vector-vector binary operator over two nodes (b2p_plan_binary_create): the reference's ProjectionExec / FilterExec
 // over an inner HashJoinExec on (key columns, time index), planner.rs:556-777, 3436-3546.  The join is a match between
 // series on the host (hash of the key tuples, O(rows + pairs)); the per-step work is b2p_binary_op.
 class BinaryPlan : public PlanNode {
  public:
-  enum class Matching { None, On, Ignoring };
+  using Matching = b2p::Matching;
   BinaryPlan(b2p_ctx* ctx, int op, bool return_bool, std::shared_ptr<PlanNode> lhs, std::shared_ptr<PlanNode> rhs,
              Matching matching, std::vector<std::string> labels, bool labels_from_lhs);
   const char* name() const { return "GpuPromBinaryExec"; }
@@ -181,6 +185,25 @@ class BinaryPlan : public PlanNode {
   Matching matching_;
   std::vector<std::string> labels_;
   bool labels_from_lhs_;
+};
+
+// Set operator `and` / `or` / `unless` over two nodes (b2p_plan_setop_create): the reference's left.distinct()
+// LeftSemi / LeftAnti HashJoinExec on (key columns, time index), planner.rs:3549-3703, and UnionDistinctOnExec,
+// planner.rs:3707-3906.  Labels are matched on the host into one dense key id per row; the per-cell work is b2p_setop.
+class SetOpPlan : public PlanNode {
+ public:
+  SetOpPlan(b2p_ctx* ctx, int op, std::shared_ptr<PlanNode> lhs, std::shared_ptr<PlanNode> rhs, Matching matching,
+            std::vector<std::string> labels);
+  const char* name() const { return "GpuPromSetOpExec"; }
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  int op_;
+  std::shared_ptr<PlanNode> lhs_, rhs_;
+  Matching matching_;
+  std::vector<std::string> labels_;
 };
 
 int function_id_from_name(const std::string& prom_name);  // -1 when unknown

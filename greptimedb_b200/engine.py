@@ -29,8 +29,17 @@ OP_IDS = {"+": 0, "-": 1, "*": 2, "/": 3, "%": 4, "^": 5, "atan2": 6,
           "==": 7, "!=": 8, ">": 9, "<": 10, ">=": 11, "<=": 12}
 
 
+# enum b2p_setop, and the key of a row that matches nothing on the other side
+SETOP_IDS = {"and": 0, "or": 1, "unless": 2}
+NO_KEY = 0xFFFFFFFF
+
+
 def op_id(op) -> int:
     return OP_IDS[op] if isinstance(op, str) else int(op)
+
+
+def setop_id(op) -> int:
+    return SETOP_IDS[op] if isinstance(op, str) else int(op)
 
 E_UNSORTED = -3
 
@@ -240,6 +249,24 @@ class Context:
                                           float(scalar), _ptr(vals), _ptr(valid), S, T, _ptr(out), _ptr(ov)))
         return out, ov
 
+    def setop(self, op, lhs, lhs_valid, lhs_key, rhs, rhs_valid, rhs_key, n_keys):
+        """`lhs op rhs` for op in and / or / unless, rows keyed by dense match-key ids (NO_KEY: no match)
+        -> (out f64, valid_words u32): [L,T] / [L,Tw] for and / unless, [L+R,T] / [L+R,Tw] (lhs rows first) for or."""
+        lhs = np.ascontiguousarray(lhs, np.float64)
+        rhs = np.ascontiguousarray(rhs, np.float64)
+        lhs_valid = np.ascontiguousarray(lhs_valid, np.uint32)
+        rhs_valid = np.ascontiguousarray(rhs_valid, np.uint32)
+        lhs_key = np.ascontiguousarray(lhs_key, np.uint32)
+        rhs_key = np.ascontiguousarray(rhs_key, np.uint32)
+        T = lhs.shape[1] if lhs.ndim == 2 else rhs.shape[1]
+        L, R = lhs_key.size, rhs_key.size
+        n = L + R if setop_id(op) == SETOP_IDS["or"] else L
+        out = np.zeros((n, T), np.float64)
+        ov = np.zeros((n, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_setop(self._h, setop_id(op), _ptr(lhs), _ptr(lhs_valid), _ptr(lhs_key), L, _ptr(rhs),
+                                      _ptr(rhs_valid), _ptr(rhs_key), R, int(n_keys), T, _ptr(out), _ptr(ov)))
+        return out, ov
+
     # -- device API (torch tensors or raw pointers; asynchronous) ----------------------------------
     def series_offsets_dev(self, sid, n_rows, n_series, offsets):
         self._check(self._L.b2p_series_offsets_dev(self._h, _ptr(sid), n_rows, n_series, _ptr(offsets)))
@@ -339,6 +366,12 @@ class Context:
         self._check(self._L.b2p_scalar_op_dev(self._h, op_id(op), int(bool(return_bool)), int(bool(scalar_on_left)),
                                               float(scalar), _ptr(vals), _ptr(valid), n_rows, T, _ptr(out),
                                               _ptr(out_valid)))
+
+    def setop_dev(self, op, lhs, lhs_valid, lhs_key, n_lhs_rows, rhs, rhs_valid, rhs_key, n_rhs_rows, n_keys, T, out,
+                  out_valid):
+        self._check(self._L.b2p_setop_dev(self._h, setop_id(op), _ptr(lhs), _ptr(lhs_valid), _ptr(lhs_key), n_lhs_rows,
+                                          _ptr(rhs), _ptr(rhs_valid), _ptr(rhs_key), n_rhs_rows, int(n_keys), T,
+                                          _ptr(out), _ptr(out_valid)))
 
     def count_valid_words_dev(self, cnt, n_rows, T, valid_words):
         self._check(self._L.b2p_count_valid_words_dev(self._h, _ptr(cnt), n_rows, T, _ptr(valid_words)))

@@ -4,7 +4,8 @@
 (SeriesDivide tag_columns/time_index, SeriesNormalize offset/need_filter_out_nan, RangeManipulate
 start/end/interval/range/field column, the prom_* UDF name, optional by-label aggregate) and is fed
 pyarrow RecordBatches exactly like the reference's tests feed a MemoryExec.  `scalar_op` puts `node op number` on
-top of any node, and `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels).
+top of any node, `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels) and `SetOpPlan` applies
+`and` / `or` / `unless` to two nodes.
 """
 from __future__ import annotations
 
@@ -12,7 +13,7 @@ import ctypes as C
 from typing import Optional, Sequence
 
 from . import _lib
-from .engine import B2PError, Context, make_params, op_id
+from .engine import B2PError, Context, make_params, op_id, setop_id
 
 
 class _ArrowArray(C.Structure):
@@ -121,5 +122,26 @@ class BinaryPlan(_PlanNode):
         arr = _cstr_array(labels)
         self._h = self._L.b2p_plan_binary_create(ctx._h, op_id(op), int(bool(return_bool)), lhs._h, rhs._h, matching,
                                                  arr, len(labels), label_side.encode())
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class SetOpPlan(_PlanNode):
+    """`lhs and / or / unless rhs` over two nodes (any node handle).  `and` / `unless` keep the lhs rows and columns and
+    match on each side's tags narrowed by `on` / `ignoring` (the two must agree); `or` emits the lhs rows, then the rhs
+    rows no lhs row (or earlier rhs row) of the same key covers, with the time index first and then the union of the tags
+    and the value column in name order.  The children stay usable and are kept alive by this node."""
+
+    def __init__(self, ctx: Context, op, lhs: _PlanNode, rhs: _PlanNode, on: Optional[Sequence[str]] = None,
+                 ignoring: Optional[Sequence[str]] = None):
+        if on is not None and ignoring is not None:
+            raise ValueError("on and ignoring are exclusive")
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (lhs, rhs)
+        matching, labels = (b"on", list(on)) if on is not None else (b"ignoring", list(ignoring)) if ignoring is not None \
+            else (None, [])
+        arr = _cstr_array(labels)
+        self._h = self._L.b2p_plan_setop_create(ctx._h, setop_id(op), lhs._h, rhs._h, matching, arr, len(labels))
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())

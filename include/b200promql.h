@@ -32,6 +32,9 @@
  *                              HashJoinExec on (tag columns, time index), planner.rs:556-777, 3436-3546; the join is a
  *                              host-side series match that yields (lhs row, rhs row) pairs
  *   b2p_scalar_op[_dev]        vector-scalar arithmetic / comparison (ProjectionExec / FilterExec, planner.rs:556-777)
+ *   b2p_setop[_dev]            set operators: `and` / `unless` = left.distinct() LeftSemi / LeftAnti HashJoinExec on
+ *                              (key columns, time index), planner.rs:3549-3703; `or` = UnionDistinctOnExec,
+ *                              planner.rs:3707-3906, union_distinct_on.rs:338-577; the key match is done by the caller
  *
  * Data layout (HBM, struct-of-arrays, all row-sorted by (series id, timestamp) exactly like
  * the reference's required_input_ordering, series_divide.rs:410-440):
@@ -111,6 +114,10 @@ enum b2p_agg { B2P_AGG_SUM = 0, B2P_AGG_AVG = 1, B2P_AGG_COUNT = 2, B2P_AGG_MIN 
 enum b2p_binop { B2P_OP_ADD = 0, B2P_OP_SUB = 1, B2P_OP_MUL = 2, B2P_OP_DIV = 3, B2P_OP_MOD = 4, B2P_OP_POW = 5,
                  B2P_OP_ATAN2 = 6, B2P_OP_EQ = 7, B2P_OP_NE = 8, B2P_OP_GT = 9, B2P_OP_LT = 10, B2P_OP_GE = 11,
                  B2P_OP_LE = 12 };
+
+/* PromQL set operators; they work per (match key, step) cell and copy cells, never compute values. */
+enum b2p_setop { B2P_SET_AND = 0, B2P_SET_OR = 1, B2P_SET_UNLESS = 2 };
+#define B2P_NO_KEY 0xFFFFFFFFu /* a row whose labels no row of the other side has */
 
 /* Parameters of the fused sub-plan.  Field-for-field the arguments of
  * RangeManipulate::new(start,end,interval,range,..) (range_manipulate.rs:86-110),
@@ -273,6 +280,22 @@ B2P_API int b2p_scalar_op_dev(b2p_ctx* ctx, int32_t op, int32_t return_bool, int
 B2P_API int b2p_count_valid_words_dev(b2p_ctx* ctx, const uint32_t* cnt, uint64_t n_rows, uint64_t T,
                                       uint32_t* valid_words);
 
+/* Set operator over two dense grids whose rows carry dense match-key ids (the caller matches the labels, as for
+ * b2p_binary_op; lhs_key / rhs_key [rows] in [0, n_keys) or B2P_NO_KEY).  Per step k:
+ *   and:    lhs row r keeps its cell iff some rhs row with the same key has a cell at k; B2P_NO_KEY rows keep nothing
+ *   unless: lhs row r keeps its cell iff no rhs row with the same key has one; B2P_NO_KEY rows keep every cell
+ *   or:     every lhs cell; an rhs cell iff no lhs row and no EARLIER rhs row (row order) with the same key has one;
+ *           B2P_NO_KEY rhs rows keep every cell
+ * and / unless: out [n_lhs_rows x T], out_valid [n_lhs_rows x Tw]; out / out_valid may be lhs / lhs_valid (in place);
+ * rhs (the values) is not read and may be NULL.  or: out [(n_lhs_rows + n_rhs_rows) x T] = the lhs rows, then the rhs
+ * rows; out_valid likewise; out must not overlap the inputs.  A kept cell is a bit copy of the input (NaN payloads,
+ * -0.0); every other cell is 0.0.  The library groups the rows by key itself.  B2P_E_INVALID: unknown op; a key
+ * >= n_keys other than B2P_NO_KEY is found on the device (that row is written invalid) and reported by b2p_sync. */
+B2P_API int b2p_setop_dev(b2p_ctx* ctx, int32_t op /* enum b2p_setop */, const double* lhs, const uint32_t* lhs_valid,
+                          const uint32_t* lhs_key, uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid,
+                          const uint32_t* rhs_key, uint32_t n_rhs_rows, uint32_t n_keys, uint64_t T, double* out,
+                          uint32_t* out_valid);
+
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
  * the id column `sid` (ids sid_base .. sid_base + n_series - 1, non-decreasing), or copied from `offsets_in`
@@ -318,6 +341,10 @@ B2P_API int b2p_binary_op(b2p_ctx* ctx, int32_t op, int32_t return_bool, const d
 B2P_API int b2p_scalar_op(b2p_ctx* ctx, int32_t op, int32_t return_bool, int32_t scalar_on_left, double scalar,
                           const double* vals, const uint32_t* valid, uint64_t n_rows, uint64_t T, double* out,
                           uint32_t* out_valid);
+/* Host-pointer form of b2p_setop_dev (synchronous; key errors are returned directly). */
+B2P_API int b2p_setop(b2p_ctx* ctx, int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key,
+                      uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid, const uint32_t* rhs_key,
+                      uint32_t n_rhs_rows, uint32_t n_keys, uint64_t T, double* out, uint32_t* out_valid);
 
 /* ---- plan-level API over the Arrow C Data Interface ------------------------------------------------
  * GpuPromRangeExec: the whole sub-tree SeriesDivide -> SeriesNormalize -> RangeManipulate ->
@@ -384,6 +411,19 @@ B2P_API b2p_plan* b2p_plan_binary_create(b2p_ctx* ctx, int32_t op, int32_t retur
                                          const char* matching /* NULL | "on" | "ignoring" */,
                                          const char* const* labels, int32_t n_labels,
                                          const char* label_side /* "lhs" | "rhs" */);
+/* Set operator node over two nodes (range, instant, aggregate, histogram, binary or set).  Labels are matched on the
+ * host; both sides must be evaluated on the same steps and carry Utf8 tags (an id-keyed __tsid side is refused: the
+ * reference matches set operators on label values).
+ *   and / unless: key = each side's tags, kept by "on" (listed) or "ignoring" (not listed); the two key sets must be
+ *     equal.  Output: the lhs node's rows and columns, cells filtered; an lhs cell equal in labels, step and value bits
+ *     to one of an earlier lhs row is dropped first (the reference's left.distinct()).
+ *   or: key = the "on" labels (one that neither side has is an error), or the union of both sides' tags without the
+ *     "ignoring" ones, or that union.  Output: the lhs rows, then the rhs rows; columns {lhs time index, then the sorted
+ *     union of both sides' tags and the lhs value name}; a tag a side lacks is NULL on its rows.
+ * Ownership as for b2p_plan_binary_create.  NULL on error (b2p_plan_last_error). */
+B2P_API b2p_plan* b2p_plan_setop_create(b2p_ctx* ctx, int32_t op /* enum b2p_setop */, b2p_plan* lhs, b2p_plan* rhs,
+                                        const char* matching /* NULL | "on" | "ignoring" */,
+                                        const char* const* labels, int32_t n_labels);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

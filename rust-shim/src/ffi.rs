@@ -108,6 +108,18 @@ pub enum B2pBinOp {
     Le = 12,
 }
 
+/// `enum b2p_setop` — PromQL set operators (planner.rs:3549-3906).
+#[repr(i32)]
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub enum B2pSetOp {
+    And = 0,
+    Or = 1,
+    Unless = 2,
+}
+
+/// `B2P_NO_KEY`: the key of a row that no row of the other side matches.
+pub const B2P_NO_KEY: u32 = 0xFFFF_FFFF;
+
 impl B2pBinOp {
     /// true for `== != > < >= <=` (a filter without `bool`)
     pub fn is_comparison(self) -> bool {
@@ -239,6 +251,11 @@ extern "C" {
         valid: *const u32, n_rows: u64, t: u64, out: *mut f64, out_valid: *mut u32,
     ) -> c_int;
     pub fn b2p_count_valid_words_dev(ctx: *mut b2p_ctx, cnt: *const u32, n_rows: u64, t: u64, valid_words: *mut u32) -> c_int;
+    pub fn b2p_setop_dev(
+        ctx: *mut b2p_ctx, op: i32, lhs: *const f64, lhs_valid: *const u32, lhs_key: *const u32, n_lhs_rows: u32,
+        rhs: *const f64, rhs_valid: *const u32, rhs_key: *const u32, n_rhs_rows: u32, n_keys: u32, t: u64,
+        out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- host-side helper (no device work): SeriesDivide + cadence scan of one sorted batch ---------------------------
     pub fn b2p_host_scan_series(
@@ -282,6 +299,11 @@ extern "C" {
         ctx: *mut b2p_ctx, op: i32, return_bool: i32, scalar_on_left: i32, scalar: f64, vals: *const f64,
         valid: *const u32, n_rows: u64, t: u64, out: *mut f64, out_valid: *mut u32,
     ) -> c_int;
+    pub fn b2p_setop(
+        ctx: *mut b2p_ctx, op: i32, lhs: *const f64, lhs_valid: *const u32, lhs_key: *const u32, n_lhs_rows: u32,
+        rhs: *const f64, rhs_valid: *const u32, rhs_key: *const u32, n_rhs_rows: u32, n_keys: u32, t: u64,
+        out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- plan-level API over the Arrow C Data Interface -----------------------------------------------------------------
     pub fn b2p_plan_range_create(
@@ -296,6 +318,11 @@ extern "C" {
     pub fn b2p_plan_binary_create(
         ctx: *mut b2p_ctx, op: i32, return_bool: i32, lhs: *mut b2p_plan, rhs: *mut b2p_plan, matching: *const c_char,
         labels: *const *const c_char, n_labels: i32, label_side: *const c_char,
+    ) -> *mut b2p_plan;
+    /// Ownership as for b2p_plan_binary_create.
+    pub fn b2p_plan_setop_create(
+        ctx: *mut b2p_ctx, op: i32, lhs: *mut b2p_plan, rhs: *mut b2p_plan, matching: *const c_char,
+        labels: *const *const c_char, n_labels: i32,
     ) -> *mut b2p_plan;
     /// MOVES the batch: on success the release callbacks now belong to the plan.
     pub fn b2p_plan_push_batch(plan: *mut b2p_plan, batch: *mut FFI_ArrowArray, schema: *mut FFI_ArrowSchema) -> c_int;

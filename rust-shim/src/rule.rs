@@ -26,6 +26,16 @@
 //!     <- GpuPromRangeExec, GpuPromRangeExec   => `match_binary_join`: the b2p_plan_binary_create arguments
 //! ```
 //!
+//! Set operators (planner.rs:3549-3906):
+//!
+//! ```text
+//!   HashJoinExec(LeftSemi | LeftAnti, on = [(tag, tag).., (ts, ts)])      (`and` / `unless`)
+//!     <- AggregateExec(group by every column, no aggregates) <- GpuPromRangeExec   (left.distinct())
+//!     <- GpuPromRangeExec
+//!   UnionDistinctOnExec(compare_keys) <- GpuPromRangeExec, GpuPromRangeExec         (`or`)
+//!                                           => `match_set_op`: the b2p_plan_setop_create arguments
+//! ```
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
@@ -47,9 +57,9 @@ use datafusion::physical_plan::repartition::RepartitionExec;
 use datafusion::physical_plan::ExecutionPlan;
 
 use crate::exec::{GpuPromRangeExec, GpuPromRangeParams};
-use crate::ffi::{B2pBinOp, B2pFn};
+use crate::ffi::{B2pBinOp, B2pFn, B2pSetOp};
 // In-tree these are `crate::extension_plan::{..}`; named here the way the reference names them.
-use promql::extension_plan::{RangeManipulateExec, SeriesDivideExec, SeriesNormalizeExec};
+use promql::extension_plan::{RangeManipulateExec, SeriesDivideExec, SeriesNormalizeExec, UnionDistinctOnExec};
 
 #[derive(Debug)]
 pub struct GpuPromRewrite {
@@ -162,6 +172,16 @@ pub struct GpuPromBinarySpec {
     pub on: Vec<String>,
     /// "lhs" | "rhs": the side whose tag columns the projection emits (planner.rs:696-711)
     pub label_side: &'static str,
+}
+
+/// What `b2p_plan_setop_create` takes for `lhs and | or | unless rhs` over two rewritten nodes.
+#[derive(Debug)]
+pub struct GpuPromSetOpSpec {
+    pub op: B2pSetOp,
+    pub lhs: GpuPromRangeParams,
+    pub rhs: GpuPromRangeParams,
+    /// passed as `on(..)`: the join's tag keys (`and` / `unless`), or UnionDistinctOn's compare keys (`or`)
+    pub on: Vec<String>,
 }
 
 /// DataFusion operator -> b2p_binop; `pow` / `atan2` arrive as scalar functions (planner.rs:3915-3990).
@@ -285,6 +305,51 @@ impl GpuPromRewrite {
             None => "lhs",
         };
         Some(GpuPromBinarySpec { op, return_bool, lhs: lhs.params().clone(), rhs: rhs.params().clone(), on, label_side })
+    }
+
+    /// `HashJoinExec(LeftSemi | LeftAnti, tags.. + ts) <- AggregateExec(distinct) <- GpuPromRangeExec` (and / unless,
+    /// planner.rs:3549-3703) or `UnionDistinctOnExec` (or, planner.rs:3707-3906) over two `GpuPromRangeExec` -> the
+    /// arguments of `b2p_plan_setop_create`.  The join keys / compare keys become `on(..)`.
+    pub fn match_set_op(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromSetOpSpec> {
+        if let Some(u) = plan.as_any().downcast_ref::<UnionDistinctOnExec>() {
+            let lhs = u.left().as_any().downcast_ref::<GpuPromRangeExec>()?;
+            let rhs = u.right().as_any().downcast_ref::<GpuPromRangeExec>()?;
+            let on = u.compare_keys().clone();
+            return Some(GpuPromSetOpSpec { op: B2pSetOp::Or, lhs: lhs.params().clone(), rhs: rhs.params().clone(), on });
+        }
+        let join = plan.as_any().downcast_ref::<HashJoinExec>()?;
+        let op = match join.join_type() {
+            JoinType::LeftSemi => B2pSetOp::And,
+            JoinType::LeftAnti => B2pSetOp::Unless,
+            _ => return None,
+        };
+        if join.filter().is_some() {
+            return None;
+        }
+        // left.distinct(): an AggregateExec that groups by every column and computes nothing
+        let distinct = join.left().as_any().downcast_ref::<AggregateExec>()?;
+        if !distinct.aggr_expr().is_empty() {
+            return None;
+        }
+        let lhs = distinct.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let rhs = join.right().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let mut on = Vec::new();
+        let mut has_ts = false;
+        for (l, r) in join.on() {
+            let (l, r) = (l.as_any().downcast_ref::<Column>()?, r.as_any().downcast_ref::<Column>()?);
+            if l.name() != r.name() {
+                return None;
+            }
+            if l.name() == rhs.params().time_index_column {
+                has_ts = true;
+            } else {
+                on.push(l.name().to_string());
+            }
+        }
+        if !has_ts {
+            return None;
+        }
+        Some(GpuPromSetOpSpec { op, lhs: lhs.params().clone(), rhs: rhs.params().clone(), on })
     }
 }
 

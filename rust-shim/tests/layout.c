@@ -37,6 +37,9 @@ SA(B2P_OP_ADD == 0 && B2P_OP_SUB == 1 && B2P_OP_MUL == 2 && B2P_OP_DIV == 3 && B
 SA(B2P_OP_POW == 5 && B2P_OP_ATAN2 == 6 && B2P_OP_EQ == 7 && B2P_OP_NE == 8 && B2P_OP_GT == 9, "B2pBinOp 5-9");
 SA(B2P_OP_LT == 10 && B2P_OP_GE == 11 && B2P_OP_LE == 12, "B2pBinOp 10-12");
 SA(sizeof(enum b2p_binop) == 4, "b2p_binop is passed as i32");
+SA(B2P_SET_AND == 0 && B2P_SET_OR == 1 && B2P_SET_UNLESS == 2, "B2pSetOp");
+SA(sizeof(enum b2p_setop) == 4, "b2p_setop is passed as i32");
+SA(B2P_NO_KEY == 0xFFFFFFFFu, "B2P_NO_KEY");
 /* status codes and sizes the shim hard-codes */
 SA(B2P_OK == 0 && B2P_E_INVALID == -1 && B2P_E_CUDA == -2 && B2P_E_UNSORTED == -3 && B2P_E_NOMEM == -4 && B2P_E_TOO_LARGE == -5, "codes");
 SA(B2P_COMM_ID_BYTES == 128, "communicator id");
