@@ -14,6 +14,8 @@
 #include <new>
 #include <string>
 #include <thread>
+#include <type_traits>
+#include <unordered_map>
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -131,6 +133,7 @@ constexpr int kStatusSlots = 32;      // range calls that may be outstanding bet
 constexpr int kSlowCtas = 132;        // slow-path grid (4 warps per CTA): one CTA per SM of an H100
 constexpr int kSlowWarps = kSlowCtas * 4;
 constexpr size_t kArenaDefaultRows = 1u << 21;  // 32 MB: regions of 3 971 rows for the 528 slow-path warps
+constexpr int kStageSlots = 11;       // device buffers of one host call, at most: b2p_range_histogram_fold's
 
 // error of a non-zero Status::k0_errors word
 int k0_fail(uint32_t k0) {
@@ -200,7 +203,6 @@ struct b2p_ctx {
   int last_range_fn = 0;
   bool last_used_lean = false;  // the pending / last range call started with K2L
   uint32_t last_range_series = 0;
-  int lean_blocks_per_sm[B2P_FN__COUNT][2][2] = {};  // [fn][FLAGS][UNI]
   // first-tier variant for equally spaced samples (rate / increase / delta): -1 = cadence_probe_kernel decides per call
   // on the device, 0 / 1 = forced (B2P_UNIFORM)
   int uniform_mode = -1;
@@ -211,8 +213,8 @@ struct b2p_ctx {
   long long launches = 0;
   long long last_slow = 0;
   long long last_w = 0;
-  // host-API staging
-  DevBuf h_ts, h_val, h_sid, h_off, h_out, h_valid, h_aux0, h_aux1, h_aux2, h_aux3;
+  // host-API staging: buffer i holds the i-th device copy a synchronous host call hands out (struct Staging)
+  DevBuf stage[kStageSlots];
   // host-API pipeline (double-buffered staging, separate copy streams)
   bool pipe_ready = false;
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
@@ -225,16 +227,16 @@ struct b2p_ctx {
   long long last_h2d_bytes = 0;
   // uniform histogram layout -> fold index (b2p_histogram_quantile_dev)
   DevBuf hq_off, hq_series, hq_les;
+  // [n_series x T] range results of a by-label sum that cannot run fused (b2p_range_group_sum_indexed_dev)
+  DevBuf rg_out, rg_valid;
   // group aggregate scratch
   DevBuf g_keys_in, g_keys_out, g_vals_in, g_vals_out, g_goff, g_tmp;
   // column reduce scratch
   DevBuf c_psum, c_pcnt;
-  // host-API staging of the binary operators: lhs, lhs validity, lhs rows, rhs, rhs validity, rhs rows, out, out validity
-  DevBuf bin[8];
   // set operators: the key -> member-row CSR of each side and the per-key validity mask
   DevBuf s_goff[2], s_members[2], s_mask;
-  int fast_blocks_per_sm[B2P_FN__COUNT][2] = {};
-  int big_blocks_per_sm[B2P_FN__COUNT] = {};
+  // resident CTAs per SM of each persistent kernel instantiation (persistent_grid)
+  std::unordered_map<const void*, int> blocks_per_sm;
 };
 
 namespace {
@@ -265,20 +267,52 @@ void stage_end_on(b2p_ctx* c, int stage, cudaStream_t s) {
   c->ev_used[stage] = true;
 }
 
+// CTAs for `units` work units, `per_block` per CTA, at most `per_sm` CTAs per SM (grid-stride beyond)
+unsigned capped_grid(const b2p_ctx* c, uint64_t units, uint64_t per_block, uint64_t per_sm) {
+  const uint64_t blocks = (units + per_block - 1) / per_block, cap = (uint64_t)c->num_sms * per_sm;
+  return (unsigned)(blocks < cap ? blocks : cap);
+}
+
+constexpr uint64_t kAllResident = ~0ull;  // persistent_grid units: every CTA that stays resident
+
+// Grid of a persistent kernel over `units` warp units, `warps` per CTA: at most the CTAs that stay resident.  The
+// dynamic shared-memory attribute is set, and the occupancy queried, once per context and kernel instantiation.
+template <class Kern>
+int persistent_grid(b2p_ctx* c, Kern* kern, size_t smem, int warps, uint64_t units, unsigned* grid) {
+  int& per_sm = c->blocks_per_sm[reinterpret_cast<const void*>(kern)];
+  if (per_sm == 0) {
+    int nb = 0;
+    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, warps * 32, smem));
+    per_sm = nb > 0 ? nb : 1;
+  }
+  const uint64_t need = units / warps + (units % warps != 0), cap = (uint64_t)c->num_sms * per_sm;
+  *grid = (unsigned)(need < cap ? need : cap);
+  return B2P_OK;
+}
+
+// f(std::integral_constant<int, ID>{}) for the run-time id `id` in [0, COUNT): one instantiation of f per id
+template <int COUNT, int ID = 0, class F>
+int with_id(int id, const char* what, F&& f) {
+  if constexpr (ID == COUNT) {
+    return fail(B2P_E_INVALID, "unknown %s %d", what, id);
+  } else {
+    return id == ID ? f(std::integral_constant<int, ID>{}) : with_id<COUNT, ID + 1>(id, what, f);
+  }
+}
+// range function id -> compile-time FN
+template <class F>
+int with_fn(int fn, F&& f) { return with_id<B2P_FN__COUNT>(fn, "fn_id", f); }
+
+// rate / increase / delta: the functions of the thread tier and of the fused by-label first tier
+constexpr bool rate_like(int fn) { return fn == B2P_FN_RATE || fn == B2P_FN_INCREASE || fn == B2P_FN_DELTA; }
+
 template <int FN, bool TS32>
 int launch_fast_t(b2p_ctx* c, const RangeArgs& a) {
   constexpr size_t smem = (size_t)kWarpsPerCta * (2 * kRing * (8 + (TS32 ? 4 : 8)) + kRing / 8) + kRcpTable * 8;
   auto kern = range_fast_kernel<FN, kRing, TS32>;
-  int& cached = c->fast_blocks_per_sm[FN][TS32 ? 1 : 0];
-  if (cached == 0) {
-    int nb = 0;
-    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kWarpsPerCta * 32, smem));
-    cached = nb > 0 ? nb : 1;
-  }
-  const unsigned need = (a.n_series + kWarpsPerCta - 1) / kWarpsPerCta;
-  const unsigned cap = (unsigned)(c->num_sms * cached);
-  const unsigned grid = need < cap ? need : cap;
+  unsigned grid = 0;
+  if (int rc = persistent_grid(c, kern, smem, kWarpsPerCta, a.n_series, &grid)) return rc;
   if (grid == 0) return B2P_OK;
   kern<<<grid, kWarpsPerCta * 32, smem, c->stream>>>(a);
   c->launches++;
@@ -293,14 +327,9 @@ int launch_big(b2p_ctx* c, const RangeArgs& a0) {
   a.use_w_list = 2;
   constexpr size_t smem = (size_t)kWarpsPerCta * (2 * kBigRing * (8 + 4) + kBigRing / 8) + kRcpTable * 8;
   auto kern = range_fast_kernel<FN, kBigRing, true>;
-  int& cached = c->big_blocks_per_sm[FN];
-  if (cached == 0) {
-    int nb = 0;
-    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kWarpsPerCta * 32, smem));
-    cached = nb > 0 ? nb : 1;
-  }
-  kern<<<(unsigned)(c->num_sms * cached), kWarpsPerCta * 32, smem, c->stream>>>(a);
+  unsigned grid = 0;  // the length of b_list is known on the device only
+  if (int rc = persistent_grid(c, kern, smem, kWarpsPerCta, kAllResident, &grid)) return rc;
+  kern<<<grid, kWarpsPerCta * 32, smem, c->stream>>>(a);
   c->launches++;
   CU(cudaGetLastError());
   return B2P_OK;
@@ -312,9 +341,6 @@ bool fits_ts32(const RangeArgs& a) {
   return span >= 0 && span < 2147483000.0 && a.interval < 2147483000ll && a.range < 2147483000ll;
 }
 
-template <int FN>
-constexpr bool lean_supports() { return LeanTraits<FN>::kSupported; }
-
 // Adaptive tiering verdict of a finished range call that started with K2L: more than half of the series handed on ->
 // the next 32 calls of this function use the next mode (plain -> bit words for rate / increase -> skip).
 void lean_verdict(b2p_ctx* c, int fn, uint64_t handed, uint64_t n_series) {
@@ -324,17 +350,19 @@ void lean_verdict(b2p_ctx* c, int fn, uint64_t handed, uint64_t n_series) {
   c->lean_backoff[fn] = 32;
 }
 
-bool lean_fn_supported(int fn) {
-  switch (fn) {
-#define X(N) case N: return lean_supports<N>();
-    X(0) X(1) X(2) X(3) X(4) X(5) X(6) X(7) X(8) X(9) X(10) X(11) X(12) X(13) X(14) X(15) X(16) X(17) X(18) X(19) X(20)
-#undef X
-  }
-  return false;
+bool lean_supported(int fn) {
+  bool supported = false;
+  if (fn >= 0 && fn < B2P_FN__COUNT)
+    with_fn(fn, [&](auto k) { supported = LeanTraits<decltype(k)::value>::kSupported; return B2P_OK; });
+  return supported;
 }
 
+// Lean first tier (K2L): rate / increase / delta in the 32-bit time domain.  The gates are what the kernel
+// relies on: exact reciprocal division by range/1000, range >= interval (steps evaluated before the end of a
+// series are below the trimmed end), start >= 0 (truncating division == floor in the end trim), and window
+// ends of the 31 steps past the grid still below the 0xFFFFFFFF end sentinel.
 bool lean_ok(const b2p_ctx* c, int fn, const RangeArgs& a) {
-  if (!c->lean_tier || !lean_fn_supported(fn)) return false;
+  if (!c->lean_tier || !lean_supported(fn)) return false;
   if (!fits_ts32(a) || a.range < a.interval || a.start < 0) return false;
   if (fn == B2P_FN_RATE && a.rcp_rs == 0.0) return false;
   return (double)a.rel_max + 64.0 * (double)a.interval < 4294967295.0;
@@ -344,12 +372,6 @@ template <int FN>
 int launch_fast(b2p_ctx* c, const RangeArgs& a) {
   return fits_ts32(a) ? launch_fast_t<FN, true>(c, a) : launch_fast_t<FN, false>(c, a);
 }
-
-// Lean first tier (K2L): rate / increase / delta in the 32-bit time domain.  The gates are what the kernel
-// relies on: exact reciprocal division by range/1000, range >= interval (steps evaluated before the end of a
-// series are below the trimmed end), start >= 0 (truncating division == floor in the end trim), and window
-// ends of the 31 steps past the grid still below the 0xFFFFFFFF end sentinel.
-bool lean_ok(const b2p_ctx* c, int fn, const RangeArgs& a);
 
 // Functions whose first tier has a uniform-cadence variant: the probe (or B2P_UNIFORM) writes Status::uniform, then
 // both variants are launched and the one the verdict does not name returns at once — no host round trip.
@@ -368,16 +390,8 @@ template <int FN, bool FLAGS, bool UNI>
 int launch_lean_variant(b2p_ctx* c, const RangeArgs& a) {
   constexpr size_t smem = lean_smem_bytes(UNI);
   auto kern = range_lean_kernel<FN, FLAGS, false, UNI>;
-  int& cached = c->lean_blocks_per_sm[FN][FLAGS ? 1 : 0][UNI ? 1 : 0];
-  if (cached == 0) {
-    int nb = 0;
-    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kLeanWarps * 32, smem));
-    cached = nb > 0 ? nb : 1;
-  }
-  const unsigned need = (a.n_series + kLeanWarps - 1) / kLeanWarps;
-  const unsigned cap = (unsigned)(c->num_sms * cached);
-  const unsigned grid = need < cap ? need : cap;
+  unsigned grid = 0;
+  if (int rc = persistent_grid(c, kern, smem, kLeanWarps, a.n_series, &grid)) return rc;
   if (grid == 0) return B2P_OK;
   kern<<<grid, kLeanWarps * 32, smem, c->stream>>>(a);
   c->launches++;
@@ -418,19 +432,12 @@ template <int FN, bool FLAGS, bool UNI>
 int launch_lean_grouped_variant(b2p_ctx* c, const RangeArgs& a) {
   constexpr size_t smem = lean_grouped_smem_bytes(UNI);
   auto kern = range_lean_kernel<FN, FLAGS, true, UNI>;
-  static int cached_nb[16] = {};  // per device
-  int& cached = cached_nb[c->device & 15];
-  if (cached == 0) {
-    int nb = 0;
-    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kLeanWarps * 32, smem));
-    cached = nb > 0 ? nb : 1;
-  }
+  unsigned cap = 0;
+  if (int rc = persistent_grid(c, kern, smem, kLeanWarps, kAllResident, &cap)) return rc;
   const unsigned n_g = a.g_hi - a.g_lo;
   const unsigned need = (n_g + kLeanWarps - 1) / kLeanWarps;
   // The grid is one CTA per SM and takes its groups from a counter, so it can be any size: while tiles are being
   // all-reduced a few SMs are left to the collective's CTAs (they cannot be placed beside a resident 24-warp CTA).
-  unsigned cap = (unsigned)(c->num_sms * cached);
   if (c->comm_reserve_now > 0 && cap > (unsigned)c->comm_reserve_now + 8u) cap -= (unsigned)c->comm_reserve_now;
   const unsigned grid = need < cap ? need : cap;
   if (grid == 0) return B2P_OK;
@@ -450,35 +457,30 @@ int launch_lean_grouped(b2p_ctx* c, const RangeArgs& a) {
     return launch_lean_grouped_variant<FN, FLAGS, false>(c, a);
   }
 }
-bool lean_grouped_fn(int fn) { return fn == B2P_FN_RATE || fn == B2P_FN_INCREASE || fn == B2P_FN_DELTA; }
-int dispatch_lean_grouped(b2p_ctx* c, int fn, const RangeArgs& a, bool with_flags) {
-  switch (fn) {
-    case B2P_FN_RATE: return with_flags ? launch_lean_grouped<B2P_FN_RATE, true>(c, a) : launch_lean_grouped<B2P_FN_RATE, false>(c, a);
-    case B2P_FN_INCREASE: return with_flags ? launch_lean_grouped<B2P_FN_INCREASE, true>(c, a) : launch_lean_grouped<B2P_FN_INCREASE, false>(c, a);
-    case B2P_FN_DELTA: return launch_lean_grouped<B2P_FN_DELTA, false>(c, a);
+template <int FN>
+int launch_lean_grouped_if_supported(b2p_ctx* c, const RangeArgs& a, bool with_flags) {
+  if constexpr (!rate_like(FN)) {
+    return fail(B2P_E_INVALID, "fn_id %d has no fused by-label tier", FN);
+  } else if constexpr (LeanTraits<FN>::kHasFlagsVariant) {
+    return with_flags ? launch_lean_grouped<FN, true>(c, a) : launch_lean_grouped<FN, false>(c, a);
+  } else {
+    return launch_lean_grouped<FN, false>(c, a);
   }
-  return fail(B2P_E_INVALID, "fn_id %d has no fused by-label tier", fn);
-}
-
-int dispatch_lean(b2p_ctx* c, int fn, const RangeArgs& a, bool with_flags) {
-  switch (fn) {
-#define X(N) case N: return launch_lean_if_supported<N>(c, a, with_flags);
-    X(0) X(1) X(2) X(3) X(4) X(5) X(6) X(7) X(8) X(9) X(10) X(11) X(12) X(13) X(14) X(15) X(16) X(17) X(18) X(19) X(20)
-#undef X
-  }
-  return fail(B2P_E_INVALID, "unknown fn_id %d", fn);
 }
 
 template <int FN>
 int launch_thread_tier(b2p_ctx* c, const RangeArgs& a) {
-  const unsigned batches = (a.n_series + 31) / 32;
-  const unsigned cap = (unsigned)c->num_sms * (unsigned)(220 * 1024 / (kTRing * 32 * 12 + 512));  // shared memory per 1-warp CTA
-  const unsigned grid = batches < cap ? batches : cap;
-  if (grid == 0) return B2P_OK;
-  range_thread_kernel<FN><<<grid, 32, 0, c->stream>>>(a);
-  c->launches++;
-  CU(cudaGetLastError());
-  return B2P_OK;
+  if constexpr (!rate_like(FN)) {
+    return fail(B2P_E_INVALID, "fn_id %d has no thread tier", FN);
+  } else {
+    // at most the 1-warp CTAs whose rings fit in shared memory
+    const unsigned grid = capped_grid(c, a.n_series, 32, 220 * 1024 / (kTRing * 32 * 12 + 512));
+    if (grid == 0) return B2P_OK;
+    range_thread_kernel<FN><<<grid, 32, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    return B2P_OK;
+  }
 }
 
 template <int FN>
@@ -489,55 +491,8 @@ int launch_slow(b2p_ctx* c, const RangeArgs& a) {
   return B2P_OK;
 }
 
-template <int FN>
-int launch_udf(b2p_ctx* c, const int64_t* ts, const double* val, const int64_t* packed, const int64_t* eval_ts,
-               uint64_t n_win, int64_t range_length, double p0, double p1, double* out, uint8_t* valid) {
-  if (n_win == 0) return B2P_OK;
-  uint64_t blocks = (n_win + 127) / 128;
-  if (blocks > (uint64_t)c->num_sms * 32) blocks = (uint64_t)c->num_sms * 32;
-  range_udf_kernel<FN><<<(unsigned)blocks, 128, 0, c->stream>>>(ts, val, packed, eval_ts, n_win, range_length, p0, p1,
-                                                                 out, valid);
-  c->launches++;
-  CU(cudaGetLastError());
-  return B2P_OK;
-}
-
-#define B2P_FOR_EACH_FN(X) \
-  X(0) X(1) X(2) X(3) X(4) X(5) X(6) X(7) X(8) X(9) X(10) X(11) X(12) X(13) X(14) X(15) X(16) X(17) X(18) X(19) X(20)
-
-int dispatch_fast(b2p_ctx* c, int fn, const RangeArgs& a) {
-  switch (fn) {
-#define X(N) case N: return launch_fast<N>(c, a);
-    B2P_FOR_EACH_FN(X)
-#undef X
-  }
-  return fail(B2P_E_INVALID, "unknown fn_id %d", fn);
-}
-int dispatch_big(b2p_ctx* c, int fn, const RangeArgs& a) {
-  switch (fn) {
-#define X(N) case N: return launch_big<N>(c, a);
-    B2P_FOR_EACH_FN(X)
-#undef X
-  }
-  return fail(B2P_E_INVALID, "unknown fn_id %d", fn);
-}
 int dispatch_slow(b2p_ctx* c, int fn, const RangeArgs& a) {
-  switch (fn) {
-#define X(N) case N: return launch_slow<N>(c, a);
-    B2P_FOR_EACH_FN(X)
-#undef X
-  }
-  return fail(B2P_E_INVALID, "unknown fn_id %d", fn);
-}
-int dispatch_udf(b2p_ctx* c, int fn, const int64_t* ts, const double* val, const int64_t* packed,
-                 const int64_t* eval_ts, uint64_t n_win, int64_t range_length, double p0, double p1, double* out,
-                 uint8_t* valid) {
-  switch (fn) {
-#define X(N) case N: return launch_udf<N>(c, ts, val, packed, eval_ts, n_win, range_length, p0, p1, out, valid);
-    B2P_FOR_EACH_FN(X)
-#undef X
-  }
-  return fail(B2P_E_INVALID, "unknown fn_id %d", fn);
+  return with_fn(fn, [&](auto k) { return launch_slow<decltype(k)::value>(c, a); });
 }
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
@@ -554,7 +509,25 @@ int check_grid(const b2p_range_params* p, uint32_t n_series, int64_t* T_out) {
   return B2P_OK;
 }
 
-int reset_status(b2p_ctx*) { return B2P_OK; }  // (every range call resets its own status slot; K0's verdict is sticky)
+// The window and time-domain fields of a range call over T steps (check_grid has accepted p); the first tier's gates
+// (lean_ok) read them.
+RangeArgs range_geometry(const b2p_range_params* p, int64_t T) {
+  RangeArgs a{};
+  a.start = p->start; a.end = p->end; a.interval = p->interval; a.range = p->range;
+  a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
+  a.tb = p->start - p->range;
+  if (fits_ts32(a)) a.rel_max = (uint32_t)(p->range + (T - 1) * p->interval + 1);
+  // exact two-FMA division by range/1000 needs RN(1/b) and a significand that is not all ones
+  const double rs = (double)p->range / 1000.0;
+  uint64_t bits;
+  memcpy(&bits, &rs, 8);
+  const bool all_ones = (bits & 0x000fffffffffffffull) == 0x000fffffffffffffull;
+  a.rcp_rs = (p->range > 0 && !all_ones) ? 1.0 / rs : 0.0;
+  a.range_secs = rs;
+  a.rcp_interval = 1.0 / (double)p->interval;
+  a.start_mod = p->start >= 0 ? (uint32_t)(p->start % p->interval) : 0u;
+  return a;
+}
 
 int ensure_slow_scratch(b2p_ctx* c, uint32_t n_series, int64_t T) {
   int rc;
@@ -575,13 +548,11 @@ int ensure_slow_scratch(b2p_ctx* c, uint32_t n_series, int64_t T) {
 template <int OP, int MODE, int FORM>
 int launch_binary(b2p_ctx* c, const BinaryArgs& a, bool vec) {
   const uint64_t steps = vec ? 64 : 32;
-  const uint64_t units = a.n_pairs * ((a.T + steps - 1) / steps);
-  uint64_t blocks = (units + 7) / 8;  // 8 warps per CTA, one unit each, grid-stride beyond the cap
-  const uint64_t cap = (uint64_t)c->num_sms * 16;
-  if (blocks > cap) blocks = cap;
+  // 8 warps per CTA, one unit each, grid-stride beyond the cap
+  const unsigned blocks = capped_grid(c, a.n_pairs * ((a.T + steps - 1) / steps), 8, 16);
   if (blocks == 0) return B2P_OK;
-  if (vec) binary_op_kernel<OP, MODE, FORM, true><<<(unsigned)blocks, 256, 0, c->stream>>>(a);
-  else binary_op_kernel<OP, MODE, FORM, false><<<(unsigned)blocks, 256, 0, c->stream>>>(a);
+  if (vec) binary_op_kernel<OP, MODE, FORM, true><<<blocks, 256, 0, c->stream>>>(a);
+  else binary_op_kernel<OP, MODE, FORM, false><<<blocks, 256, 0, c->stream>>>(a);
   c->launches++;
   CU(cudaGetLastError());
   return B2P_OK;
@@ -709,11 +680,11 @@ void b2p_destroy(b2p_ctx* c) {
   if (c->ev_comm_done) cudaEventDestroy(c->ev_comm_done);
   if (c->ev_comm_go) cudaEventDestroy(c->ev_comm_go);
   for (DevBuf* b : {&c->w_skip, &c->b_skip, &c->slow_skip, &c->m_tmp0, &c->m_tmp1, &c->hq_off, &c->hq_series, &c->hq_les}) b->release();
-  for (DevBuf* b : {&c->slow_list, &c->w_list, &c->b_list, &c->arena_ts, &c->arena_val, &c->win_scratch, &c->h_ts, &c->h_val, &c->h_sid,
-                    &c->h_off, &c->h_out, &c->h_valid, &c->h_aux0, &c->h_aux1, &c->h_aux2, &c->h_aux3,
-                    &c->g_keys_in, &c->g_keys_out, &c->g_vals_in, &c->g_vals_out, &c->g_goff, &c->g_tmp, &c->c_psum,
-                    &c->c_pcnt})
+  for (DevBuf* b : {&c->slow_list, &c->w_list, &c->b_list, &c->arena_ts, &c->arena_val, &c->win_scratch, &c->rg_out,
+                    &c->rg_valid, &c->g_keys_in, &c->g_keys_out, &c->g_vals_in, &c->g_vals_out, &c->g_goff, &c->g_tmp,
+                    &c->c_psum, &c->c_pcnt})
     b->release();
+  for (DevBuf& b : c->stage) b.release();
   for (int i = 0; i < 5; ++i)
     for (int j = 0; j < 2; ++j)
       if (c->ev[i][j]) cudaEventDestroy(c->ev[i][j]);
@@ -724,7 +695,6 @@ void b2p_destroy(b2p_ctx* c) {
     if (c->ev_d2h[i]) cudaEventDestroy(c->ev_d2h[i]);
   }
   c->p_status.release();
-  for (DevBuf& b : c->bin) b.release();
   for (DevBuf* b : {&c->s_goff[0], &c->s_goff[1], &c->s_members[0], &c->s_members[1], &c->s_mask}) b->release();
   if (c->s_h2d) cudaStreamDestroy(c->s_h2d);
   if (c->s_d2h) cudaStreamDestroy(c->s_d2h);
@@ -784,18 +754,21 @@ static int launch_range_tiers(b2p_ctx* c, int fn, RangeArgs a, bool thread_tier,
     CU(cudaMemsetAsync(&a.status->w_count, 0, 3 * sizeof(uint32_t), c->stream));  // w_count, b_count, g_next
   }
   stage_begin(c, 1);
-  if (thread_tier) {
-    if (fn == B2P_FN_RATE) rc = launch_thread_tier<B2P_FN_RATE>(c, a);
-    else if (fn == B2P_FN_INCREASE) rc = launch_thread_tier<B2P_FN_INCREASE>(c, a);
-    else rc = launch_thread_tier<B2P_FN_DELTA>(c, a);
+  if (thread_tier || used_lean) {
+    rc = with_fn(fn, [&](auto k) {
+      constexpr int FN = decltype(k)::value;
+      if (thread_tier) return launch_thread_tier<FN>(c, a);
+      return a.gsum ? launch_lean_grouped_if_supported<FN>(c, a, lean_mode == 1)
+                    : launch_lean_if_supported<FN>(c, a, lean_mode == 1);
+    });
     if (rc) return rc;
     a.use_w_list = 1;
-  } else if (used_lean) {
-    if ((rc = a.gsum ? dispatch_lean_grouped(c, fn, a, lean_mode == 1) : dispatch_lean(c, fn, a, lean_mode == 1))) return rc;
-    a.use_w_list = 1;
   }
-  rc = dispatch_fast(c, fn, a);
-  if (!rc && a.b_list) rc = dispatch_big(c, fn, a);
+  rc = with_fn(fn, [&](auto k) {
+    constexpr int FN = decltype(k)::value;
+    const int r = launch_fast<FN>(c, a);
+    return (r || !a.b_list) ? r : launch_big<FN>(c, a);
+  });
   stage_end(c, 1);
   if (rc) return rc;
   stage_begin(c, 2);
@@ -884,12 +857,10 @@ static int series_offsets_impl(b2p_ctx* c, const uint32_t* sid, uint64_t n_rows,
   if (!c || !offsets || (!sid && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
   if (!aligned16(sid)) return fail(B2P_E_INVALID, "sid must be 16-byte aligned");
   DeviceGuard g(c->device);
-  uint64_t blocks = (n_rows / 16 + 255) / 256;
-  const uint64_t cap = (uint64_t)c->num_sms * 16;
-  if (blocks > cap) blocks = cap;
+  unsigned blocks = capped_grid(c, n_rows / 16, 256, 16);
   if (blocks == 0) blocks = 1;
   stage_begin(c, 0);
-  series_offsets_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(sid, n_rows, n_series, sid_base, offsets, c->d_k0);
+  series_offsets_kernel<<<blocks, 256, 0, c->stream>>>(sid, n_rows, n_series, sid_base, offsets, c->d_k0);
   c->launches++;
   stage_end(c, 0);
   CU(cudaGetLastError());
@@ -911,20 +882,9 @@ struct GroupTarget {
 // Can this range call add its results straight into by-label partials?  (first tier available for the function and
 // the query shape, and not switched off by the adaptive policy; groups balanced enough for group-exclusive warps)
 static bool fused_group_ok(b2p_ctx* c, const b2p_range_params* p, int64_t T, const b2p_group_index* idx) {
-  if (!lean_grouped_fn(p->fn_id) || c->thread_tier) return false;
+  if (!rate_like(p->fn_id) || c->thread_tier) return false;
   if (T > 32 * (int64_t)kLeanFullWords) return false;  // per-warp word counters of the first tier
-  RangeArgs a{};
-  a.start = p->start; a.end = p->end; a.interval = p->interval; a.range = p->range;
-  a.T = T;
-  a.rcp_rs = 1.0;
-  if (fits_ts32(a)) a.rel_max = (uint32_t)(p->range + (T - 1) * p->interval + 1);
-  {
-    const double rs = (double)p->range / 1000.0;
-    uint64_t bits;
-    memcpy(&bits, &rs, 8);
-    if (p->range <= 0 || (bits & 0x000fffffffffffffull) == 0x000fffffffffffffull) a.rcp_rs = 0.0;
-  }
-  if (!lean_ok(c, p->fn_id, a)) return false;
+  if (!lean_ok(c, p->fn_id, range_geometry(p, T))) return false;
   if (c->lean_backoff[p->fn_id] > 0 && c->lean_mode[p->fn_id] == 2) return false;
   // a group is walked by ONE warp: the largest group may not exceed a few times a warp's fair share
   const uint64_t warps = (uint64_t)c->num_sms * B2P_LEAN_MIN_BLOCKS * kLeanWarps;
@@ -954,24 +914,8 @@ static int range_call(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, 
   if (!aligned16(ts) || !aligned16(val)) return fail(B2P_E_INVALID, "ts/val must be 16-byte aligned");
   DeviceGuard g(c->device);
   if ((rc = ensure_slow_scratch(c, n_series, T))) return rc;
-  RangeArgs a{};
-  a.start = p->start; a.end = p->end; a.interval = p->interval; a.range = p->range; a.offset = p->offset;
-  a.p0 = p->param0; a.p1 = p->param1; a.filter_nan = p->filter_nan;
-  a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
-  a.tb = p->start - p->range;
-  a.rel_max = 0;
-  if (fits_ts32(a)) a.rel_max = (uint32_t)(p->range + (T - 1) * p->interval + 1);
-  {
-    // exact two-FMA division by range/1000 needs RN(1/b) and a significand that is not all ones
-    const double rs = (double)p->range / 1000.0;
-    uint64_t bits;
-    memcpy(&bits, &rs, 8);
-    const bool all_ones = (bits & 0x000fffffffffffffull) == 0x000fffffffffffffull;
-    a.rcp_rs = (p->range > 0 && !all_ones) ? 1.0 / rs : 0.0;
-    a.range_secs = rs;
-    a.rcp_interval = 1.0 / (double)p->interval;
-    a.start_mod = p->start >= 0 ? (uint32_t)(p->start % p->interval) : 0u;
-  }
+  RangeArgs a = range_geometry(p, T);
+  a.offset = p->offset; a.p0 = p->param0; a.p1 = p->param1; a.filter_nan = p->filter_nan;
   a.ts = ts; a.val = val; a.offsets = offsets; a.n_rows = n_rows; a.n_series = n_series;
   a.out = out; a.valid = valid_words;
   // a fused call keeps the work lists until its verdict is in: nothing else is admitted before that
@@ -997,8 +941,7 @@ static int range_call(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, 
   // tier 1 (rate / increase / delta, 32-bit time domain): thread per series (opt-in) or the lean warp-per-series
   // kernel; what it declines goes to tier 2 (warp per series) through w_list, long windows from there to the
   // 1024-sample instantiation through b_list, and what that declines to the exact slow kernel
-  const bool tier1 = c->thread_tier && fits_ts32(a) &&
-                     (p->fn_id == B2P_FN_RATE || p->fn_id == B2P_FN_INCREASE || p->fn_id == B2P_FN_DELTA);
+  const bool tier1 = c->thread_tier && fits_ts32(a) && rate_like(p->fn_id);
   bool used_lean = false;
   int mode = 0;
   if (!tier1 && lean_ok(c, p->fn_id, a)) {
@@ -1071,7 +1014,13 @@ int b2p_range_udf_dev(b2p_ctx* c, int32_t fn_id, const int64_t* ts, const double
   if (!packed_ranges || !out || !valid) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
   stage_begin(c, 1);
-  int rc = dispatch_udf(c, fn_id, ts, val, packed_ranges, eval_ts, n_win, range_length, param0, param1, out, valid);
+  const int rc = with_fn(fn_id, [&](auto k) {
+    range_udf_kernel<decltype(k)::value><<<capped_grid(c, n_win, 128, 32), 128, 0, c->stream>>>(
+        ts, val, packed_ranges, eval_ts, n_win, range_length, param0, param1, out, valid);
+    c->launches++;
+    CU(cudaGetLastError());
+    return B2P_OK;
+  });
   stage_end(c, 1);
   return rc;
 }
@@ -1093,10 +1042,8 @@ int b2p_instant_select_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t inter
   a.start = start; a.end = end; a.interval = interval; a.lookback = lookback; a.offset = offset;
   a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
   a.ts = ts; a.val = val; a.offsets = offsets; a.n_series = n_series; a.out = out; a.valid = valid_words;
-  unsigned need = (n_series + kWarpsPerCta - 1) / kWarpsPerCta;
-  unsigned cap = (unsigned)c->num_sms * 8;
   stage_begin(c, 1);
-  instant_kernel<<<need < cap ? need : cap, kWarpsPerCta * 32, 0, c->stream>>>(a);
+  instant_kernel<<<capped_grid(c, n_series, kWarpsPerCta, 8), kWarpsPerCta * 32, 0, c->stream>>>(a);
   c->launches++;
   stage_end(c, 1);
   CU(cudaGetLastError());
@@ -1137,22 +1084,13 @@ int group_aggregate_csr(b2p_ctx* c, int32_t agg, const double* vals, const uint3
   a.agg = agg; a.vals = vals; a.valid = valid_words; a.goff = goff;
   a.members = members; a.n_groups = n_groups; a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
   a.out_val = out_val; a.out_cnt = out_cnt; a.accumulate = accumulate;
-  const uint64_t warps = (uint64_t)n_groups * ((T + 31) / 32);
-  uint64_t blocks = (warps + 7) / 8;
-  const uint64_t cap = (uint64_t)c->num_sms * 32;
-  if (blocks > cap) blocks = cap;
-  switch (agg) {
-    case B2P_AGG_SUM: group_aggregate_kernel<B2P_AGG_SUM><<<(unsigned)blocks, 256, 0, c->stream>>>(a); break;
-    case B2P_AGG_AVG: group_aggregate_kernel<B2P_AGG_AVG><<<(unsigned)blocks, 256, 0, c->stream>>>(a); break;
-    case B2P_AGG_COUNT: group_aggregate_kernel<B2P_AGG_COUNT><<<(unsigned)blocks, 256, 0, c->stream>>>(a); break;
-    case B2P_AGG_MIN: group_aggregate_kernel<B2P_AGG_MIN><<<(unsigned)blocks, 256, 0, c->stream>>>(a); break;
-    case B2P_AGG_MAX: group_aggregate_kernel<B2P_AGG_MAX><<<(unsigned)blocks, 256, 0, c->stream>>>(a); break;
-    case B2P_AGG_STDVAR: group_aggregate_kernel<B2P_AGG_STDVAR><<<(unsigned)blocks, 256, 0, c->stream>>>(a); break;
-    default: group_aggregate_kernel<B2P_AGG_STDDEV><<<(unsigned)blocks, 256, 0, c->stream>>>(a); break;
-  }
-  c->launches++;
-  CU(cudaGetLastError());
-  return B2P_OK;
+  const unsigned blocks = capped_grid(c, (uint64_t)n_groups * ((T + 31) / 32), 8, 32);
+  return with_id<B2P_AGG_STDVAR + 1>(agg, "aggregator", [&](auto k) {
+    group_aggregate_kernel<decltype(k)::value><<<blocks, 256, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    return B2P_OK;
+  });
 }
 
 int group_aggregate_impl(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* gid,
@@ -1272,14 +1210,14 @@ int b2p_range_group_sum_indexed_dev(b2p_ctx* c, const b2p_range_params* p, const
   if (g_lo != 0 || g_hi != ix->n_groups)
     return fail(B2P_E_INVALID, "group ranges need the fused tier (rate / increase / delta in the 32-bit time domain)");
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
-  if ((rc = c->h_aux0.ensure((size_t)n_series * (size_t)T * 8))) return rc;
-  if ((rc = c->h_aux1.ensure((size_t)n_series * Tw * 4))) return rc;
-  if ((rc = b2p_range_eval_dev(c, p, ts, val, offsets, n_rows, n_series, c->h_aux0.as<double>(),
-                               c->h_aux1.as<uint32_t>())))
+  if ((rc = c->rg_out.ensure((size_t)n_series * (size_t)T * 8))) return rc;
+  if ((rc = c->rg_valid.ensure((size_t)n_series * Tw * 4))) return rc;
+  if ((rc = b2p_range_eval_dev(c, p, ts, val, offsets, n_rows, n_series, c->rg_out.as<double>(),
+                               c->rg_valid.as<uint32_t>())))
     return rc;
   if ((rc = b2p_sync(c))) return rc;  // slow-path fix-ups must land before the aggregate reads
   stage_begin(c, 3);
-  rc = group_aggregate_csr(c, B2P_AGG_SUM, c->h_aux0.as<double>(), c->h_aux1.as<uint32_t>(), ix->goff, ix->members,
+  rc = group_aggregate_csr(c, B2P_AGG_SUM, c->rg_out.as<double>(), c->rg_valid.as<uint32_t>(), ix->goff, ix->members,
                            ix->n_groups, (uint64_t)T, out_sum, out_cnt, 1);
   stage_end(c, 3);
   return rc;
@@ -1310,7 +1248,7 @@ int b2p_range_group_sum_allreduce_dev(b2p_ctx* c, const b2p_range_params* p, con
 }
 
 int b2p_range_group_sum_fused(b2p_ctx* c, const b2p_range_params* p, const b2p_group_index* ix) {
-  if (!c || !ix || !p) return 0;
+  if (!c || !ix || !p || p->interval <= 0) return 0;  // (a grid the range call itself would reject)
   int64_t T = b2p_num_steps(p->start, p->end, p->interval);
   return fused_group_ok(c, p, T, ix) ? 1 : 0;
 }
@@ -1397,8 +1335,7 @@ int b2p_allreduce_partials_dev(b2p_ctx* c, int32_t agg, double* val, uint32_t* c
     return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
   }
   DeviceGuard g(c->device);
-  uint64_t blocks = (n + 255) / 256;
-  if (blocks > (uint64_t)c->num_sms * 16) blocks = (uint64_t)c->num_sms * 16;
+  const unsigned blocks = capped_grid(c, n, 256, 16);
   if (agg == B2P_AGG_MIN || agg == B2P_AGG_MAX) {
     minmax_neutral_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(agg == B2P_AGG_MIN, val, cnt, n, 0);
     NCCL_TRY(g_nccl.GroupStart());
@@ -1455,9 +1392,7 @@ int b2p_group_finalize_dev(b2p_ctx* c, int32_t agg, double* val, const uint32_t*
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   if (n == 0) return B2P_OK;
   DeviceGuard g(c->device);
-  uint64_t blocks = (n + 255) / 256;
-  if (blocks > (uint64_t)c->num_sms * 16) blocks = (uint64_t)c->num_sms * 16;
-  group_finalize_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(agg, val, cnt, n);
+  group_finalize_kernel<<<capped_grid(c, n, 256, 16), 256, 0, c->stream>>>(agg, val, cnt, n);
   c->launches++;
   CU(cudaGetLastError());
   return B2P_OK;
@@ -1475,18 +1410,12 @@ int b2p_histogram_fold_dev(b2p_ctx* c, double phi, const uint32_t* hist_off, con
   HistFoldArgs a{};
   a.phi = phi; a.hist_off = hist_off; a.bucket_series = bucket_series; a.bucket_le = bucket_le; a.n_hist = n_hist;
   a.rates = rates; a.valid = valid_words; a.T = T; a.Tw = (uint32_t)((T + 31) / 32); a.out = out; a.out_valid = out_valid_words;
-  const uint64_t warps = (uint64_t)n_hist * ((T + 31) / 32);
-  uint64_t blocks = (warps + kHistWarps - 1) / kHistWarps;
-  const uint64_t cap = (uint64_t)c->num_sms * 3;  // 72 KB of counters + slots per CTA: three CTAs per SM
-  if (blocks > cap) blocks = cap;
-  constexpr size_t smem = (size_t)kHistWarps * kHistSmemBuckets * 32 * (8 + 1);
-  static bool attr_set[16] = {};
-  if (!attr_set[c->device & 15]) {
-    CU(cudaFuncSetAttribute(histogram_fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set[c->device & 15] = true;
-  }
+  constexpr size_t smem = (size_t)kHistWarps * kHistSmemBuckets * 32 * (8 + 1);  // 72 KB: three CTAs per SM
+  unsigned blocks = 0;
+  int rc = persistent_grid(c, histogram_fold_kernel, smem, kHistWarps, (uint64_t)n_hist * ((T + 31) / 32), &blocks);
+  if (rc) return rc;
   stage_begin(c, 3);
-  histogram_fold_kernel<<<(unsigned)blocks, kHistWarps * 32, smem, c->stream>>>(a);
+  histogram_fold_kernel<<<blocks, kHistWarps * 32, smem, c->stream>>>(a);
   c->launches++;
   stage_end(c, 3);
   CU(cudaGetLastError());
@@ -1508,9 +1437,8 @@ int b2p_histogram_quantile_dev(b2p_ctx* c, double phi, const double* le, uint32_
   {  // the fold index of the uniform layout (12 B per bucket series, rebuilt per call: microseconds)
     if ((rc = c->hq_off.ensure(((size_t)n_hist + 1) * 4)) || (rc = c->hq_series.ensure(nb * 4)) || (rc = c->hq_les.ensure(nb * 8)))
       return rc;
-    uint64_t blocks = (nb + 255) / 256;
-    if (blocks > (uint64_t)c->num_sms * 16) blocks = (uint64_t)c->num_sms * 16;
-    histogram_uniform_index_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(le, n_buckets, n_hist, c->hq_off.as<uint32_t>(),
+    const unsigned blocks = capped_grid(c, nb, 256, 16);
+    histogram_uniform_index_kernel<<<blocks, 256, 0, c->stream>>>(le, n_buckets, n_hist, c->hq_off.as<uint32_t>(),
                                                                             c->hq_series.as<uint32_t>(), c->hq_les.as<double>());
     c->launches++;
     CU(cudaGetLastError());
@@ -1593,10 +1521,7 @@ int b2p_count_valid_words_dev(b2p_ctx* c, const uint32_t* cnt, uint64_t n_rows, 
   if (!cnt || !valid_words) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
-  uint64_t blocks = (n_rows * Tw + 7) / 8;
-  const uint64_t cap = (uint64_t)c->num_sms * 16;
-  if (blocks > cap) blocks = cap;
-  count_valid_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(cnt, n_rows, T, Tw, valid_words);
+  count_valid_kernel<<<capped_grid(c, n_rows * Tw, 8, 16), 256, 0, c->stream>>>(cnt, n_rows, T, Tw, valid_words);
   c->launches++;
   CU(cudaGetLastError());
   return B2P_OK;
@@ -1606,16 +1531,9 @@ int b2p_count_valid_words_dev(b2p_ctx* c, const uint32_t* cnt, uint64_t n_rows, 
 }  // extern "C"
 
 namespace {
-// CTAs of 8 warps for `units` warp units, at most 16 per SM (grid-stride beyond)
-unsigned warp_grid(const b2p_ctx* c, uint64_t units) {
-  const uint64_t blocks = (units + 7) / 8, cap = (uint64_t)c->num_sms * 16;
-  return (unsigned)(blocks < cap ? blocks : cap);
-}
-
 int setop_key_check(b2p_ctx* c, const uint32_t* key, uint32_t n, uint32_t n_keys) {
   if (n == 0) return B2P_OK;
-  const uint64_t blocks = ((uint64_t)n + 255) / 256, cap = (uint64_t)c->num_sms * 8;
-  setop_key_check_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, c->stream>>>(key, n, n_keys, c->d_k0);
+  setop_key_check_kernel<<<capped_grid(c, n, 256, 8), 256, 0, c->stream>>>(key, n, n_keys, c->d_k0);
   c->launches++;
   CU(cudaGetLastError());
   return B2P_OK;
@@ -1631,7 +1549,7 @@ int setop_group(b2p_ctx* c, int side, const uint32_t* key, uint32_t n_rows, uint
 
 // s_mask[g] = OR of the validity words of side `side`'s rows with key g
 int setop_mask(b2p_ctx* c, int side, const uint32_t* valid, uint32_t n_keys, uint32_t Tw) {
-  const unsigned grid = warp_grid(c, (uint64_t)n_keys * ((Tw + 31) / 32));
+  const unsigned grid = capped_grid(c, (uint64_t)n_keys * ((Tw + 31) / 32), 8, 16);
   if (grid == 0) return B2P_OK;
   setop_mask_kernel<<<grid, 256, 0, c->stream>>>(valid, c->s_goff[side].as<uint32_t>(), c->s_members[side].as<uint32_t>(),
                                                  n_keys, Tw, c->s_mask.as<uint32_t>());
@@ -1643,7 +1561,7 @@ int setop_mask(b2p_ctx* c, int side, const uint32_t* valid, uint32_t n_keys, uin
 template <int MODE>
 int setop_copy(b2p_ctx* c, const SetCopyArgs& a, bool vec) {
   const uint64_t steps = vec ? 64 : 32;
-  const unsigned grid = warp_grid(c, a.n_rows * ((a.T + steps - 1) / steps));
+  const unsigned grid = capped_grid(c, a.n_rows * ((a.T + steps - 1) / steps), 8, 16);
   if (grid == 0) return B2P_OK;
   if (vec) setop_copy_kernel<MODE, true><<<grid, 256, 0, c->stream>>>(a);
   else setop_copy_kernel<MODE, false><<<grid, 256, 0, c->stream>>>(a);
@@ -1676,7 +1594,7 @@ int setop_run(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_val
     if ((rc = setop_group(c, 0, lhs_key, n_lhs_rows, n_keys)) || (rc = setop_mask(c, 0, lhs_valid, n_keys, Tw)) ||
         (rc = setop_group(c, 1, rhs_key, n_rhs_rows, n_keys)))
       return rc;
-    const unsigned grid = warp_grid(c, (uint64_t)n_keys * ((Tw + 31) / 32));
+    const unsigned grid = capped_grid(c, (uint64_t)n_keys * ((Tw + 31) / 32), 8, 16);
     setop_dedupe_kernel<<<grid, 256, 0, c->stream>>>(rhs_valid, c->s_goff[1].as<uint32_t>(), c->s_members[1].as<uint32_t>(),
                                                      c->s_mask.as<uint32_t>(), n_keys, Tw, rwords);
     c->launches++;
@@ -1728,19 +1646,91 @@ int b2p_synth_fill_dev(b2p_ctx* c, uint64_t series_begin, uint64_t n_series, uin
   DeviceGuard g(c->device);
   const uint64_t total = n_series * (uint64_t)n_samples;
   if (total == 0) return B2P_OK;
-  uint64_t blocks = (total + 255) / 256;
-  if (blocks > (uint64_t)c->num_sms * 32) blocks = (uint64_t)c->num_sms * 32;
-  synth_fill_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(series_begin, n_series, n_samples, t0, scrape_ms,
-                                                             jitter_ms, with_resets, seed, ts, val, sid);
+  synth_fill_kernel<<<capped_grid(c, total, 256, 32), 256, 0, c->stream>>>(series_begin, n_series, n_samples, t0,
+                                                                           scrape_ms, jitter_ms, with_resets, seed, ts,
+                                                                           val, sid);
   c->launches++;
   CU(cudaGetLastError());
   return B2P_OK;
 }
 
 /* ---- host-pointer API ------------------------------------------------------------------------ */
+}  // extern "C"
 
-// One chunk, no overlap: H2D -> K0/K2 -> D2H on the context stream.  sid values are global ids
-// (sid_base is subtracted on the device); offsets_host, when given, is already rebased to the chunk.
+namespace {
+// Device copies of one synchronous host call's columns, in the context's staging buffers: the i-th buffer handed out
+// is c->stage[i].  Inputs are copied to the device as they are handed out; the results noted by out() / copy_back()
+// go back to the host, in that order, in download().  The first failure sticks in `rc` (later calls hand out NULL).
+struct Staging {
+  static constexpr int kOutputs = 2;  // a host call returns two columns
+  b2p_ctx* c;
+  int next = 0, rc = B2P_OK;
+  struct Back { void* host; const void* dev; size_t bytes; };
+  Back back[kOutputs];
+  int n_back = 0;
+
+  void cuda(cudaError_t e, const char* what) {  // a failed CUDA call becomes the sticky error
+    if (e != cudaSuccess && !rc) rc = fail(B2P_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
+  }
+  void* buf(size_t bytes) {  // (16 bytes more: never NULL, even for an empty column)
+    if (!rc && next == kStageSlots) rc = fail(B2P_E_INVALID, "host call stages more than %d buffers", kStageSlots);
+    if (!rc) rc = c->stage[next].ensure(bytes + 16);
+    return rc ? nullptr : c->stage[next++].p;
+  }
+  // device copy of a host column; NULL for an absent one
+  template <class T>
+  T* in(const T* host, size_t bytes) {
+    if (!host) return nullptr;
+    void* d = buf(bytes);
+    if (d && bytes) cuda(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, c->stream), "host-to-device copy");
+    return static_cast<T*>(d);
+  }
+  void copy_back(void* host, const void* dev, size_t bytes) {
+    if (!rc && n_back == kOutputs) rc = fail(B2P_E_INVALID, "host call returns more than %d columns", kOutputs);
+    if (!rc) back[n_back++] = Back{host, dev, bytes};
+  }
+  // a result buffer, copied to `host` by download()
+  template <class T>
+  T* out(T* host, size_t bytes) {
+    T* d = static_cast<T*>(buf(bytes));
+    copy_back(host, d, bytes);
+    return d;
+  }
+  int download() {
+    for (int i = 0; !rc && i < n_back; ++i)
+      if (back[i].bytes)
+        cuda(cudaMemcpyAsync(back[i].host, back[i].dev, back[i].bytes, cudaMemcpyDeviceToHost, c->stream),
+             "device-to-host copy");
+    return rc;
+  }
+  int finish() {  // download() and wait for it
+    if (!download()) cuda(cudaStreamSynchronize(c->stream), "cudaStreamSynchronize");
+    return rc;
+  }
+};
+
+// The series columns of a host call: ts and val, then the offsets, or the id column and K0 (ids rebased by sid_base)
+struct SeriesIn {
+  const int64_t* ts;
+  const double* val;
+  uint64_t* offsets;
+};
+SeriesIn stage_series(Staging& s, const int64_t* ts, const double* val, const uint32_t* sid, uint32_t sid_base,
+                      const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series) {
+  SeriesIn in{s.in(ts, n_rows * 8), s.in(val, n_rows * 8), nullptr};
+  if (offsets_host) {
+    in.offsets = s.in(offsets_host, ((size_t)n_series + 1) * 8);
+  } else {
+    const uint32_t* d_sid = s.in(sid, n_rows * 4);
+    in.offsets = static_cast<uint64_t*>(s.buf(((size_t)n_series + 1) * 8));
+    if (!s.rc) s.rc = series_offsets_impl(s.c, d_sid, n_rows, n_series, sid_base, in.offsets);
+  }
+  return in;
+}
+}  // namespace
+
+extern "C" {
+
 // Host-side SeriesDivide + cadence scan (see the header).  Plain sequential passes, memory bound;
 // b2p_range_eval runs one of these per chunk on a few worker threads while earlier chunks are on the bus.
 static int host_scan_series(const int64_t* ts, const uint32_t* sid, const uint64_t* offsets_in, uint64_t n_rows,
@@ -1795,37 +1785,22 @@ int b2p_host_scan_series(const int64_t* ts, const uint32_t* sid, const uint64_t*
   return rc;
 }
 
+// One chunk, no overlap: H2D -> K0/K2 -> D2H on the context stream.  sid values are global ids
+// (sid_base is subtracted on the device); offsets_host, when given, is already rebased to the chunk.
 static int range_eval_host_simple(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
                                   const uint32_t* sid, uint32_t sid_base, const uint64_t* offsets_host, uint64_t n_rows,
                                   uint32_t n_series, int64_t T, double* out, uint32_t* valid_words) {
   int rc;
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
-  const size_t rows = n_rows ? n_rows : 1;
-  if ((rc = c->h_ts.ensure(rows * 8 + 16))) return rc;
-  if ((rc = c->h_val.ensure(rows * 8 + 16))) return rc;
-  if ((rc = c->h_off.ensure(((size_t)n_series + 1) * 8))) return rc;
-  if ((rc = c->h_out.ensure((size_t)n_series * (size_t)T * 8))) return rc;
-  if ((rc = c->h_valid.ensure((size_t)n_series * Tw * 4))) return rc;
-  if ((rc = reset_status(c))) return rc;
   c->last_h2d_bytes = (long long)(n_rows * 16 + (offsets_host ? ((size_t)n_series + 1) * 8 : n_rows * 4));
-  CU(cudaMemcpyAsync(c->h_ts.p, ts, n_rows * 8, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->h_val.p, val, n_rows * 8, cudaMemcpyHostToDevice, c->stream));
-  if (offsets_host) {
-    CU(cudaMemcpyAsync(c->h_off.p, offsets_host, ((size_t)n_series + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-  } else {
-    if ((rc = c->h_sid.ensure(rows * 4 + 16))) return rc;
-    CU(cudaMemcpyAsync(c->h_sid.p, sid, n_rows * 4, cudaMemcpyHostToDevice, c->stream));
-    if ((rc = series_offsets_impl(c, c->h_sid.as<uint32_t>(), n_rows, n_series, sid_base, c->h_off.as<uint64_t>())))
-      return rc;
-  }
-  if ((rc = b2p_range_eval_dev(c, p, c->h_ts.as<int64_t>(), c->h_val.as<double>(), c->h_off.as<uint64_t>(), n_rows,
-                               n_series, c->h_out.as<double>(), c->h_valid.as<uint32_t>())))
+  Staging s{c};
+  const SeriesIn in = stage_series(s, ts, val, sid, sid_base, offsets_host, n_rows, n_series);
+  double* d_out = s.out(out, (size_t)n_series * (size_t)T * 8);
+  uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
+  if ((rc = s.rc) || (rc = b2p_range_eval_dev(c, p, in.ts, in.val, in.offsets, n_rows, n_series, d_out, d_valid)) ||
+      (rc = b2p_sync(c)))
     return rc;
-  if ((rc = b2p_sync(c))) return rc;
-  CU(cudaMemcpyAsync(out, c->h_out.p, (size_t)n_series * (size_t)T * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(valid_words, c->h_valid.p, (size_t)n_series * Tw * 4, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return B2P_OK;
+  return s.finish();
 }
 
 // first row whose id is >= key in a non-decreasing id column
@@ -2005,12 +1980,9 @@ int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, con
     // compute: after its inputs landed and after chunk i-2's results left the output buffers
     CU(cudaStreamWaitEvent(c->stream, c->ev_h2d[b], 0));
     if (i >= 2) CU(cudaStreamWaitEvent(c->stream, c->ev_d2h[b], 0));
-    if ((rc = reset_status(c))) return rc;
     if (described == 1) {
-      unsigned blocks = (ns + 7) / 8;
-      if (blocks > (unsigned)c->num_sms * 8u) blocks = (unsigned)c->num_sms * 8u;
-      ts_expand_kernel<<<blocks, 256, 0, c->stream>>>(c->p_off[b].as<uint64_t>(), c->p_t0[b].as<int64_t>(),
-                                                      c->p_cad[b].as<int64_t>(), ns, c->p_ts[b].as<int64_t>());
+      ts_expand_kernel<<<capped_grid(c, ns, 8, 8), 256, 0, c->stream>>>(
+          c->p_off[b].as<uint64_t>(), c->p_t0[b].as<int64_t>(), c->p_cad[b].as<int64_t>(), ns, c->p_ts[b].as<int64_t>());
       c->launches++;
       CU(cudaGetLastError());
     } else if (!offsets_host &&
@@ -2079,30 +2051,20 @@ int b2p_range_udf(b2p_ctx* c, int32_t fn_id, const int64_t* ts, const double* va
                   double param0, double param1, double* out, uint8_t* valid) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   if (n_win == 0) return B2P_OK;
-  if (!packed_ranges || !out || !valid) return fail(B2P_E_INVALID, "NULL argument");
+  if (!packed_ranges || !out || !valid || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
   int rc;
-  const size_t rows = n_rows ? n_rows : 1;
-  if ((rc = c->h_ts.ensure(rows * 8 + 16))) return rc;
-  if ((rc = c->h_val.ensure(rows * 8 + 16))) return rc;
-  if ((rc = c->h_aux0.ensure(n_win * 8))) return rc;
-  if ((rc = c->h_aux1.ensure(n_win * 8))) return rc;
-  if ((rc = c->h_out.ensure(n_win * 8))) return rc;
-  if ((rc = c->h_valid.ensure(n_win))) return rc;
-  if (n_rows) {
-    CU(cudaMemcpyAsync(c->h_ts.p, ts, n_rows * 8, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->h_val.p, val, n_rows * 8, cudaMemcpyHostToDevice, c->stream));
-  }
-  CU(cudaMemcpyAsync(c->h_aux0.p, packed_ranges, n_win * 8, cudaMemcpyHostToDevice, c->stream));
-  if (eval_ts) CU(cudaMemcpyAsync(c->h_aux1.p, eval_ts, n_win * 8, cudaMemcpyHostToDevice, c->stream));
-  if ((rc = b2p_range_udf_dev(c, fn_id, c->h_ts.as<int64_t>(), c->h_val.as<double>(), n_rows, c->h_aux0.as<int64_t>(),
-                              eval_ts ? c->h_aux1.as<int64_t>() : nullptr, n_win, range_length, param0, param1,
-                              c->h_out.as<double>(), c->h_valid.as<uint8_t>())))
+  Staging s{c};
+  const int64_t* d_ts = s.in(ts, n_rows * 8);
+  const double* d_val = s.in(val, n_rows * 8);
+  const int64_t* d_packed = s.in(packed_ranges, n_win * 8);
+  const int64_t* d_eval_ts = s.in(eval_ts, n_win * 8);
+  double* d_out = s.out(out, n_win * 8);
+  uint8_t* d_valid = s.out(valid, n_win);
+  if ((rc = s.rc) || (rc = b2p_range_udf_dev(c, fn_id, d_ts, d_val, n_rows, d_packed, d_eval_ts, n_win, range_length,
+                                             param0, param1, d_out, d_valid)))
     return rc;
-  CU(cudaMemcpyAsync(out, c->h_out.p, n_win * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(valid, c->h_valid.p, n_win, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return B2P_OK;
+  return s.finish();
 }
 
 int b2p_instant_select(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
@@ -2116,58 +2078,40 @@ int b2p_instant_select(b2p_ctx* c, int64_t start, int64_t end, int64_t interval,
   if (rc) return rc;
   if (n_series == 0 || T == 0) return B2P_OK;
   if (!sid && !offsets_host) return fail(B2P_E_INVALID, "need sid or offsets_host");
+  if (!out || !valid_words || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
-  const size_t rows = n_rows ? n_rows : 1;
-  if ((rc = c->h_ts.ensure(rows * 8 + 16))) return rc;
-  if ((rc = c->h_val.ensure(rows * 8 + 16))) return rc;
-  if ((rc = c->h_off.ensure(((size_t)n_series + 1) * 8))) return rc;
-  if ((rc = c->h_out.ensure((size_t)n_series * (size_t)T * 8))) return rc;
-  if ((rc = c->h_valid.ensure((size_t)n_series * Tw * 4))) return rc;
-  if ((rc = reset_status(c))) return rc;
-  CU(cudaMemcpyAsync(c->h_ts.p, ts, n_rows * 8, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->h_val.p, val, n_rows * 8, cudaMemcpyHostToDevice, c->stream));
-  if (offsets_host) {
-    CU(cudaMemcpyAsync(c->h_off.p, offsets_host, ((size_t)n_series + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-  } else {
-    if ((rc = c->h_sid.ensure(rows * 4 + 16))) return rc;
-    CU(cudaMemcpyAsync(c->h_sid.p, sid, n_rows * 4, cudaMemcpyHostToDevice, c->stream));
-    if ((rc = b2p_series_offsets_dev(c, c->h_sid.as<uint32_t>(), n_rows, n_series, c->h_off.as<uint64_t>()))) return rc;
-  }
-  if ((rc = b2p_instant_select_dev(c, start, end, interval, lookback, offset, c->h_ts.as<int64_t>(),
-                                   c->h_val.as<double>(), c->h_off.as<uint64_t>(), n_rows, n_series,
-                                   c->h_out.as<double>(), c->h_valid.as<uint32_t>())))
+  Staging s{c};
+  const SeriesIn in = stage_series(s, ts, val, sid, 0u, offsets_host, n_rows, n_series);
+  double* d_out = s.out(out, (size_t)n_series * (size_t)T * 8);
+  uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
+  if ((rc = s.rc) ||
+      (rc = b2p_instant_select_dev(c, start, end, interval, lookback, offset, in.ts, in.val, in.offsets, n_rows,
+                                   n_series, d_out, d_valid)) ||
+      (rc = b2p_sync(c)))
     return rc;
-  if ((rc = b2p_sync(c))) return rc;
-  CU(cudaMemcpyAsync(out, c->h_out.p, (size_t)n_series * (size_t)T * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(valid_words, c->h_valid.p, (size_t)n_series * Tw * 4, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return B2P_OK;
+  return s.finish();
 }
 
 int b2p_group_aggregate(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* gid,
                         uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (agg < 0 || agg > B2P_AGG_STDVAR) return fail(B2P_E_INVALID, "unknown aggregator %d", agg);
   if (n_groups == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid_words || !gid || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
   int rc;
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
-  const size_t ns = n_series ? n_series : 1;
-  if ((rc = c->h_aux0.ensure(ns * T * 8))) return rc;
-  if ((rc = c->h_aux1.ensure(ns * Tw * 4))) return rc;
-  if ((rc = c->h_aux2.ensure(ns * 4))) return rc;
-  if ((rc = c->h_out.ensure((size_t)n_groups * T * 8))) return rc;
-  if ((rc = c->h_valid.ensure((size_t)n_groups * T * 4))) return rc;
-  CU(cudaMemcpyAsync(c->h_aux0.p, vals, (size_t)n_series * T * 8, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->h_aux1.p, valid_words, (size_t)n_series * Tw * 4, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->h_aux2.p, gid, (size_t)n_series * 4, cudaMemcpyHostToDevice, c->stream));
-  if ((rc = b2p_group_aggregate_dev(c, agg, c->h_aux0.as<double>(), c->h_aux1.as<uint32_t>(), c->h_aux2.as<uint32_t>(),
-                                    n_series, n_groups, T, c->h_out.as<double>(), c->h_valid.as<uint32_t>())))
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_series * T * 8);
+  const uint32_t* d_valid = s.in(valid_words, (size_t)n_series * Tw * 4);
+  const uint32_t* d_gid = s.in(gid, (size_t)n_series * 4);
+  double* d_out = s.out(out_val, (size_t)n_groups * T * 8);
+  uint32_t* d_cnt = s.out(out_cnt, (size_t)n_groups * T * 4);
+  if ((rc = s.rc) ||
+      (rc = b2p_group_aggregate_dev(c, agg, d_vals, d_valid, d_gid, n_series, n_groups, T, d_out, d_cnt)))
     return rc;
-  CU(cudaMemcpyAsync(out_val, c->h_out.p, (size_t)n_groups * T * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(out_cnt, c->h_valid.p, (size_t)n_groups * T * 4, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return B2P_OK;
+  return s.finish();
 }
 
 int b2p_histogram_quantile(b2p_ctx* c, double phi, const double* le, uint32_t n_buckets, const double* rates,
@@ -2175,26 +2119,23 @@ int b2p_histogram_quantile(b2p_ctx* c, double phi, const double* le, uint32_t n_
                            uint32_t* out_valid_words) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   if (n_hist == 0 || T == 0) return B2P_OK;
+  if (!le || !rates || !valid_words || !out || !out_valid_words || n_buckets == 0)
+    return fail(B2P_E_INVALID, "NULL argument");
+  if ((uint64_t)n_hist * n_buckets > 0xffffffffull) return fail(B2P_E_TOO_LARGE, "more than 2^32 bucket series");
   DeviceGuard g(c->device);
   int rc;
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
   const size_t ns = (size_t)n_hist * n_buckets;
-  if ((rc = c->h_aux0.ensure(ns * T * 8))) return rc;
-  if ((rc = c->h_aux1.ensure(ns * Tw * 4))) return rc;
-  if ((rc = c->h_aux2.ensure((size_t)n_buckets * 8))) return rc;
-  if ((rc = c->h_out.ensure((size_t)n_hist * T * 8))) return rc;
-  if ((rc = c->h_valid.ensure((size_t)n_hist * Tw * 4))) return rc;
-  CU(cudaMemcpyAsync(c->h_aux0.p, rates, ns * T * 8, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->h_aux1.p, valid_words, ns * Tw * 4, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->h_aux2.p, le, (size_t)n_buckets * 8, cudaMemcpyHostToDevice, c->stream));
-  if ((rc = b2p_histogram_quantile_dev(c, phi, c->h_aux2.as<double>(), n_buckets, c->h_aux0.as<double>(),
-                                       c->h_aux1.as<uint32_t>(), n_hist, T, c->h_out.as<double>(),
-                                       c->h_valid.as<uint32_t>())))
+  Staging s{c};
+  const double* d_rates = s.in(rates, ns * T * 8);
+  const uint32_t* d_valid = s.in(valid_words, ns * Tw * 4);
+  const double* d_le = s.in(le, (size_t)n_buckets * 8);
+  double* d_out = s.out(out, (size_t)n_hist * T * 8);
+  uint32_t* d_out_valid = s.out(out_valid_words, (size_t)n_hist * Tw * 4);
+  if ((rc = s.rc) ||
+      (rc = b2p_histogram_quantile_dev(c, phi, d_le, n_buckets, d_rates, d_valid, n_hist, T, d_out, d_out_valid)))
     return rc;
-  CU(cudaMemcpyAsync(out, c->h_out.p, (size_t)n_hist * T * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(out_valid_words, c->h_valid.p, (size_t)n_hist * Tw * 4, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return B2P_OK;
+  return s.finish();
 }
 
 // histogram_quantile(phi, fn(bucket_series[range])) from host buffers to host rows without the dense [n_series x T]
@@ -2215,38 +2156,24 @@ int b2p_range_histogram_fold(b2p_ctx* c, const b2p_range_params* p, const int64_
   DeviceGuard g(c->device);
   if (!c->pending.empty() && (rc = b2p_sync(c))) return rc;
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
-  const size_t rows = n_rows ? n_rows : 1;
   const size_t nb = hist_off[n_hist];
-  if ((rc = c->h_ts.ensure(rows * 8 + 16)) || (rc = c->h_val.ensure(rows * 8 + 16)) ||
-      (rc = c->h_off.ensure(((size_t)n_series + 1) * 8)) || (rc = c->h_out.ensure((size_t)n_series * (size_t)T * 8)) ||
-      (rc = c->h_valid.ensure((size_t)n_series * Tw * 4)) || (rc = c->hq_off.ensure(((size_t)n_hist + 1) * 4)) ||
-      (rc = c->hq_series.ensure((nb ? nb : 1) * 4)) || (rc = c->hq_les.ensure((nb ? nb : 1) * 8)) ||
-      (rc = c->h_aux2.ensure((size_t)n_hist * (size_t)T * 8)) || (rc = c->h_aux3.ensure((size_t)n_hist * Tw * 4)))
+  Staging s{c};
+  const SeriesIn in = stage_series(s, ts, val, sid, 0u, offsets_host, n_rows, n_series);
+  const uint32_t* d_hist_off = s.in(hist_off, ((size_t)n_hist + 1) * 4);
+  const uint32_t* d_bucket_series = s.in(bucket_series, nb * 4);
+  const double* d_bucket_le = s.in(bucket_le, nb * 8);
+  double* d_rates = static_cast<double*>(s.buf((size_t)n_series * (size_t)T * 8));
+  uint32_t* d_rates_valid = static_cast<uint32_t*>(s.buf((size_t)n_series * Tw * 4));
+  double* d_out = s.out(out, (size_t)n_hist * (size_t)T * 8);
+  uint32_t* d_out_valid = s.out(out_valid_words, (size_t)n_hist * Tw * 4);
+  if ((rc = s.rc) ||
+      (rc = b2p_range_eval_dev(c, p, in.ts, in.val, in.offsets, n_rows, n_series, d_rates, d_rates_valid)) ||
+      (rc = b2p_sync(c)))  // slow-path fix-ups land before the fold reads
     return rc;
-  CU(cudaMemcpyAsync(c->h_ts.p, ts, n_rows * 8, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->h_val.p, val, n_rows * 8, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->hq_off.p, hist_off, ((size_t)n_hist + 1) * 4, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->hq_series.p, bucket_series, nb * 4, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->hq_les.p, bucket_le, nb * 8, cudaMemcpyHostToDevice, c->stream));
-  if (offsets_host) {
-    CU(cudaMemcpyAsync(c->h_off.p, offsets_host, ((size_t)n_series + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-  } else {
-    if ((rc = c->h_sid.ensure(rows * 4 + 16))) return rc;
-    CU(cudaMemcpyAsync(c->h_sid.p, sid, n_rows * 4, cudaMemcpyHostToDevice, c->stream));
-    if ((rc = series_offsets_impl(c, c->h_sid.as<uint32_t>(), n_rows, n_series, 0u, c->h_off.as<uint64_t>()))) return rc;
-  }
-  if ((rc = b2p_range_eval_dev(c, p, c->h_ts.as<int64_t>(), c->h_val.as<double>(), c->h_off.as<uint64_t>(), n_rows, n_series,
-                               c->h_out.as<double>(), c->h_valid.as<uint32_t>())))
+  if ((rc = b2p_histogram_fold_dev(c, phi, d_hist_off, d_bucket_series, d_bucket_le, n_hist, d_rates, d_rates_valid,
+                                   (uint64_t)T, d_out, d_out_valid)))
     return rc;
-  if ((rc = b2p_sync(c))) return rc;  // slow-path fix-ups land before the fold reads
-  if ((rc = b2p_histogram_fold_dev(c, phi, c->hq_off.as<uint32_t>(), c->hq_series.as<uint32_t>(), c->hq_les.as<double>(), n_hist,
-                                   c->h_out.as<double>(), c->h_valid.as<uint32_t>(), (uint64_t)T, c->h_aux2.as<double>(),
-                                   c->h_aux3.as<uint32_t>())))
-    return rc;
-  CU(cudaMemcpyAsync(out, c->h_aux2.p, (size_t)n_hist * (size_t)T * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(out_valid_words, c->h_aux3.p, (size_t)n_hist * Tw * 4, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return B2P_OK;
+  return s.finish();
 }
 
 int b2p_binary_op(b2p_ctx* c, int32_t op, int32_t return_bool, const double* lhs, const uint32_t* lhs_valid,
@@ -2263,18 +2190,20 @@ int b2p_binary_op(b2p_ctx* c, int32_t op, int32_t return_bool, const double* lhs
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
   const size_t nl = n_lhs_rows, nr = n_rhs_rows, np = (size_t)n_pairs;
-  const size_t bytes[8] = {nl * T * 8, nl * Tw * 4, np * 4, nr * T * 8, nr * Tw * 4, np * 4, np * T * 8, np * Tw * 4};
-  for (int i = 0; i < 8; ++i)
-    if ((rc = c->bin[i].ensure(bytes[i] ? bytes[i] : 16))) return rc;
-  const void* src[6] = {lhs, lhs_valid, lhs_row, rhs, rhs_valid, rhs_row};
-  for (int i = 0; i < 6; ++i)
-    if (bytes[i]) CU(cudaMemcpyAsync(c->bin[i].p, src[i], bytes[i], cudaMemcpyHostToDevice, c->stream));
-  if ((rc = b2p_binary_op_dev(c, op, return_bool, c->bin[0].as<double>(), c->bin[1].as<uint32_t>(), c->bin[2].as<uint32_t>(),
-                              n_lhs_rows, c->bin[3].as<double>(), c->bin[4].as<uint32_t>(), c->bin[5].as<uint32_t>(),
-                              n_rhs_rows, n_pairs, T, c->bin[6].as<double>(), c->bin[7].as<uint32_t>())))
+  Staging s{c};
+  const double* d_lhs = s.in(lhs, nl * T * 8);
+  const uint32_t* d_lhs_valid = s.in(lhs_valid, nl * Tw * 4);
+  const uint32_t* d_lhs_row = s.in(lhs_row, np * 4);
+  const double* d_rhs = s.in(rhs, nr * T * 8);
+  const uint32_t* d_rhs_valid = s.in(rhs_valid, nr * Tw * 4);
+  const uint32_t* d_rhs_row = s.in(rhs_row, np * 4);
+  double* d_out = s.out(out, np * T * 8);
+  uint32_t* d_out_valid = s.out(out_valid, np * Tw * 4);
+  if ((rc = s.rc) ||
+      (rc = b2p_binary_op_dev(c, op, return_bool, d_lhs, d_lhs_valid, d_lhs_row, n_lhs_rows, d_rhs, d_rhs_valid,
+                              d_rhs_row, n_rhs_rows, n_pairs, T, d_out, d_out_valid)) ||
+      (rc = s.download()))
     return rc;
-  CU(cudaMemcpyAsync(out, c->bin[6].p, bytes[6], cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(out_valid, c->bin[7].p, bytes[7], cudaMemcpyDeviceToHost, c->stream));
   return take_row_error(c, kBinRowError);  // (synchronises)
 }
 
@@ -2288,16 +2217,15 @@ int b2p_scalar_op(b2p_ctx* c, int32_t op, int32_t return_bool, int32_t scalar_on
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
   const size_t vb = (size_t)n_rows * T * 8, wb = (size_t)n_rows * Tw * 4;
-  if ((rc = c->bin[6].ensure(vb)) || (rc = c->bin[7].ensure(wb))) return rc;
-  CU(cudaMemcpyAsync(c->bin[6].p, vals, vb, cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->bin[7].p, valid, wb, cudaMemcpyHostToDevice, c->stream));
-  if ((rc = b2p_scalar_op_dev(c, op, return_bool, scalar_on_left, scalar, c->bin[6].as<double>(), c->bin[7].as<uint32_t>(),
-                              n_rows, T, c->bin[6].as<double>(), c->bin[7].as<uint32_t>())))  // in place
+  Staging s{c};
+  double* d_vals = s.in(vals, vb);  // the operator runs in place
+  uint32_t* d_valid = s.in(valid, wb);
+  s.copy_back(out, d_vals, vb);
+  s.copy_back(out_valid, d_valid, wb);
+  if ((rc = s.rc) ||
+      (rc = b2p_scalar_op_dev(c, op, return_bool, scalar_on_left, scalar, d_vals, d_valid, n_rows, T, d_vals, d_valid)))
     return rc;
-  CU(cudaMemcpyAsync(out, c->bin[6].p, vb, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(out_valid, c->bin[7].p, wb, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return B2P_OK;
+  return s.finish();
 }
 
 int b2p_setop(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key,
@@ -2312,19 +2240,20 @@ int b2p_setop(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_val
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
   const size_t nl = n_lhs_rows, nr = n_rhs_rows, no = op == kSetOr ? nl + nr : nl;
-  const bool rvals = op == kSetOr && rhs;  // and / unless never read the rhs values
-  const size_t bytes[8] = {nl * T * 8, nl * Tw * 4, nl * 4, rvals ? nr * T * 8 : 0, nr * Tw * 4, nr * 4, no * T * 8, no * Tw * 4};
-  for (int i = 0; i < 8; ++i)
-    if ((rc = c->bin[i].ensure(bytes[i] ? bytes[i] : 16))) return rc;
-  const void* src[6] = {lhs, lhs_valid, lhs_key, rhs, rhs_valid, rhs_key};
-  for (int i = 0; i < 6; ++i)
-    if (bytes[i]) CU(cudaMemcpyAsync(c->bin[i].p, src[i], bytes[i], cudaMemcpyHostToDevice, c->stream));
-  if ((rc = b2p_setop_dev(c, op, c->bin[0].as<double>(), c->bin[1].as<uint32_t>(), c->bin[2].as<uint32_t>(), n_lhs_rows,
-                          c->bin[3].as<double>(), c->bin[4].as<uint32_t>(), c->bin[5].as<uint32_t>(), n_rhs_rows, n_keys,
-                          T, c->bin[6].as<double>(), c->bin[7].as<uint32_t>())))
+  Staging s{c};
+  const double* d_lhs = s.in(lhs, nl * T * 8);
+  const uint32_t* d_lhs_valid = s.in(lhs_valid, nl * Tw * 4);
+  const uint32_t* d_lhs_key = s.in(lhs_key, nl * 4);
+  const double* d_rhs = s.in(op == kSetOr ? rhs : nullptr, nr * T * 8);  // and / unless never read the rhs values
+  const uint32_t* d_rhs_valid = s.in(rhs_valid, nr * Tw * 4);
+  const uint32_t* d_rhs_key = s.in(rhs_key, nr * 4);
+  double* d_out = s.out(out, no * T * 8);
+  uint32_t* d_out_valid = s.out(out_valid, no * Tw * 4);
+  if ((rc = s.rc) ||
+      (rc = b2p_setop_dev(c, op, d_lhs, d_lhs_valid, d_lhs_key, n_lhs_rows, d_rhs, d_rhs_valid, d_rhs_key, n_rhs_rows,
+                          n_keys, T, d_out, d_out_valid)) ||
+      (rc = s.download()))
     return rc;
-  if (bytes[6]) CU(cudaMemcpyAsync(out, c->bin[6].p, bytes[6], cudaMemcpyDeviceToHost, c->stream));
-  if (bytes[7]) CU(cudaMemcpyAsync(out_valid, c->bin[7].p, bytes[7], cudaMemcpyDeviceToHost, c->stream));
   return take_row_error(c, kSetKeyError);  // (synchronises)
 }
 
