@@ -27,6 +27,8 @@ EXPORTED_SYMBOLS = [
     "b2p_plan_range_create", "b2p_plan_set_instant", "b2p_plan_set_histogram_quantile", "b2p_plan_push_batch", "b2p_plan_execute", "b2p_plan_num_series", "b2p_plan_destroy",
     "b2p_plan_last_error", "b2p_plan_set_scalar_op", "b2p_plan_binary_create",
     "b2p_setop_dev", "b2p_setop", "b2p_plan_setop_create",
+    "b2p_instant_fn_dev", "b2p_instant_fn", "b2p_scalar_calculate_dev", "b2p_scalar_calculate",
+    "b2p_plan_set_function", "b2p_plan_scalar_create",
 ]
 
 
@@ -119,6 +121,12 @@ def load() -> C.CDLL:
         "b2p_setop_dev": (C.c_int, [vp, i32, vp, vp, vp, u32, vp, vp, vp, u32, u32, u64, vp, vp]),
         "b2p_setop": (C.c_int, [vp, i32, vp, vp, vp, u32, vp, vp, vp, u32, u32, u64, vp, vp]),
         "b2p_plan_setop_create": (vp, [vp, i32, vp, vp, C.c_char_p, C.POINTER(C.c_char_p), i32]),
+        "b2p_instant_fn_dev": (C.c_int, [vp, i32, dbl, dbl, vp, vp, u64, u64, vp, vp]),
+        "b2p_instant_fn": (C.c_int, [vp, i32, dbl, dbl, vp, vp, u64, u64, vp, vp]),
+        "b2p_scalar_calculate_dev": (C.c_int, [vp, vp, vp, vp, u32, u64, vp, vp]),
+        "b2p_scalar_calculate": (C.c_int, [vp, vp, vp, vp, u32, u64, vp, vp]),
+        "b2p_plan_set_function": (C.c_int, [vp, C.c_char_p, C.POINTER(dbl), i32]),
+        "b2p_plan_scalar_create": (vp, [vp, vp]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)  # AttributeError here means the .so does not match the header

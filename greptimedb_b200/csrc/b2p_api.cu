@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 
+#include <cfloat>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -23,6 +24,7 @@
 #include "../../include/b200promql.h"
 #include "b2p_aggregate.cuh"
 #include "b2p_binary.cuh"
+#include "b2p_instant.cuh"
 #include "b2p_setop.cuh"
 #include "b2p_kernel_t.cuh"
 #include "b2p_kernel_lean.cuh"
@@ -139,6 +141,9 @@ constexpr int kStageSlots = 11;       // device buffers of one host call, at mos
 int k0_fail(uint32_t k0) {
   if (k0 & kBinRowError) return fail(B2P_E_INVALID, "binary operator: a pair's row index is out of range");
   if (k0 & kSetKeyError) return fail(B2P_E_INVALID, "set operator: a row's key is >= n_keys");
+  if (k0 & kScalarKeyError) return fail(B2P_E_INVALID, "scalar(): a row's series key is >= n_rows");
+  if (k0 & kScalarOverlapError)
+    return fail(B2P_E_INVALID, "scalar(): two rows of one series have a cell at the same step");
   if (k0 & 1u) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");
   return fail(B2P_E_UNSORTED, "series id >= n_series");
 }
@@ -235,6 +240,8 @@ struct b2p_ctx {
   DevBuf c_psum, c_pcnt;
   // set operators: the key -> member-row CSR of each side and the per-key validity mask
   DevBuf s_goff[2], s_members[2], s_mask;
+  // scalar(): the reduction's verdict (struct ScalarState), read by the write pass on the device
+  DevBuf sc_state;
   // resident CTAs per SM of each persistent kernel instantiation (persistent_grid)
   std::unordered_map<const void*, int> blocks_per_sm;
 };
@@ -588,7 +595,7 @@ int check_binop(int32_t op, int32_t return_bool) {
   return B2P_OK;
 }
 
-// clears `bit` (kBinRowError / kSetKeyError) of the status word after a synchronous call has read it; B2P_E_INVALID
+// clears `bit` (kBinRowError / kSetKeyError / the scalar() bits) of the status word after a synchronous call has read it; B2P_E_INVALID
 // when it was set
 int take_row_error(b2p_ctx* c, uint32_t bit) {
   CU(cudaMemcpyAsync(c->h_k0, c->d_k0, sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
@@ -597,7 +604,7 @@ int take_row_error(b2p_ctx* c, uint32_t bit) {
   if (!(k0 & bit)) return B2P_OK;
   const uint32_t rest = k0 & ~bit;
   CU(cudaMemcpy(&c->d_k0->k0_errors, &rest, sizeof rest, cudaMemcpyHostToDevice));
-  return k0_fail(bit);
+  return k0_fail(k0 & bit);
 }
 
 }  // namespace
@@ -1527,6 +1534,92 @@ int b2p_count_valid_words_dev(b2p_ctx* c, const uint32_t* cnt, uint64_t n_rows, 
   return B2P_OK;
 }
 
+/* ---- instant-vector functions and scalar() --------------------------------------------------------------------- */
+}  // extern "C"
+
+namespace {
+// clamp_min / clamp_max -> clamp with the other bound at ∓f64::MAX (ScalarValue::max / min of Float64, clamp.rs:258-271,
+// 312-325); every bound check (`lo > hi`, IEEE: a NaN bound passes) happens here, once per call
+int instant_fn_bounds(int32_t fn, double arg0, double arg1, int* kfn, double* lo, double* hi) {
+  *kfn = fn;
+  *lo = arg0;
+  *hi = arg1;
+  if (fn == B2P_IFN_CLAMP_MIN) *hi = DBL_MAX;
+  if (fn == B2P_IFN_CLAMP_MAX) *lo = -DBL_MAX, *hi = arg0;
+  if (fn == B2P_IFN_CLAMP_MIN || fn == B2P_IFN_CLAMP_MAX) *kfn = B2P_IFN_CLAMP;
+  if (fn < 0 || fn >= B2P_IFN__COUNT) return fail(B2P_E_INVALID, "unknown instant function %d", fn);
+  if (*kfn == B2P_IFN_CLAMP && *lo > *hi) return fail(B2P_E_INVALID, "clamp: min %.17g > max %.17g", *lo, *hi);
+  return B2P_OK;
+}
+static_assert((int)B2P_IFN_CLAMP == (int)kFnClamp && (int)B2P_IFN_CLAMP + 1 == (int)kFnKernelCount, "enum b2p_ifn and InstantFn disagree");
+
+// the scalar() reduction and write pass; the verdict stays on the device
+int scalar_calculate_run(b2p_ctx* c, const ScalarArgs& a0) {
+  int rc;
+  if ((rc = c->sc_state.ensure(sizeof(ScalarState)))) return rc;
+  ScalarArgs a = a0;
+  a.state = c->sc_state.as<ScalarState>();
+  a.status = c->d_k0;
+  // min_key, first_live = 0xFFFFFFFF; the rest 0
+  CU(cudaMemsetAsync(a.state, 0xFF, 2 * sizeof(uint32_t), c->stream));
+  CU(cudaMemsetAsync(&a.state->max_key, 0, sizeof(ScalarState) - 2 * sizeof(uint32_t), c->stream));
+  if (a.n_rows > 0) {
+    scalar_reduce_kernel<<<capped_grid(c, a.n_rows, 8, 16), 256, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+  }
+  scalar_write_kernel<<<capped_grid(c, a.Tw, 8, 16), 256, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_instant_fn_dev(b2p_ctx* c, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
+                       uint64_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int rc, kfn;
+  InstantFnArgs a{};
+  if ((rc = instant_fn_bounds(fn, arg0, arg1, &kfn, &a.arg0, &a.arg1))) return rc;
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !out || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  a.vals = vals; a.valid = valid; a.n_rows = n_rows; a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
+  a.out = out; a.out_valid = out_valid;
+  const bool vec = (T % 2) == 0 && aligned16(vals) && aligned16(out);
+  const uint64_t steps = vec ? 64 : 32;
+  // 8 warps per CTA, one unit each, grid-stride beyond the cap
+  const unsigned blocks = capped_grid(c, n_rows * ((T + steps - 1) / steps), 8, 16);
+  stage_begin(c, 3);
+  rc = with_id<kFnKernelCount>(kfn, "instant function", [&](auto k) {
+    constexpr int FN = decltype(k)::value;
+    if (vec) instant_fn_kernel<FN, true><<<blocks, 256, 0, c->stream>>>(a);
+    else instant_fn_kernel<FN, false><<<blocks, 256, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    return B2P_OK;
+  });
+  stage_end(c, 3);
+  return rc;
+}
+
+int b2p_scalar_calculate_dev(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* row_key,
+                             uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (T == 0) return B2P_OK;
+  if ((n_rows && (!vals || !valid || !row_key)) || !out || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  ScalarArgs a{};
+  a.vals = vals; a.valid = valid; a.key = row_key; a.n_rows = n_rows; a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
+  a.out = out; a.out_valid = out_valid;
+  stage_begin(c, 3);
+  const int rc = scalar_calculate_run(c, a);
+  stage_end(c, 3);
+  return rc;
+}
+
 /* ---- set operators ------------------------------------------------------------------------------------------- */
 }  // extern "C"
 
@@ -2255,6 +2348,47 @@ int b2p_setop(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_val
       (rc = s.download()))
     return rc;
   return take_row_error(c, kSetKeyError);  // (synchronises)
+}
+
+int b2p_instant_fn(b2p_ctx* c, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
+                   uint64_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int rc, kfn;
+  double lo, hi;
+  if ((rc = instant_fn_bounds(fn, arg0, arg1, &kfn, &lo, &hi))) return rc;
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !out || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  const size_t vb = (size_t)n_rows * T * 8, wb = (size_t)n_rows * Tw * 4;
+  Staging s{c};
+  double* d_vals = s.in(vals, vb);  // the function runs in place; validity is unchanged
+  uint32_t* d_valid = s.in(valid, wb);
+  s.copy_back(out, d_vals, vb);
+  if (out_valid != valid) s.copy_back(out_valid, d_valid, wb);
+  if ((rc = s.rc) || (rc = b2p_instant_fn_dev(c, fn, arg0, arg1, d_vals, d_valid, n_rows, T, d_vals, d_valid)))
+    return rc;
+  return s.finish();
+}
+
+int b2p_scalar_calculate(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* row_key,
+                         uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (T == 0) return B2P_OK;
+  if ((n_rows && (!vals || !valid || !row_key)) || !out || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  int rc;
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
+  const uint32_t* d_key = s.in(row_key, (size_t)n_rows * 4);
+  double* d_out = s.out(out, (size_t)T * 8);
+  uint32_t* d_out_valid = s.out(out_valid, Tw * 4);
+  if ((rc = s.rc) || (rc = b2p_scalar_calculate_dev(c, d_vals, d_valid, d_key, n_rows, T, d_out, d_out_valid)) ||
+      (rc = s.download()))
+    return rc;
+  return take_row_error(c, kScalarKeyError | kScalarOverlapError);  // (synchronises)
 }
 
 }  // extern "C"

@@ -4,6 +4,7 @@
 
 #include <algorithm>
 #include <cctype>
+#include <cfloat>
 #include <charconv>
 #include <cmath>
 #include <cstdlib>
@@ -341,6 +342,7 @@ void PromRangePlan::compute(NodeResult& r) {
   std::vector<double> dense(fold_on_device ? 0 : (size_t)S * (size_t)T);
   std::vector<uint32_t> valid(fold_on_device ? 0 : (size_t)S * Tw);
   std::vector<int64_t> eval_ts((size_t)T);
+  for (int64_t k = 0; k < T; ++k) eval_ts[(size_t)k] = p.start + k * p.interval;  // (scalar() of a node without rows)
   if (S > 0 && T > 0 && !(args_.histogram && fn_id_ >= 0)) {
     int rc;
     if (fn_id_ >= 0) {
@@ -668,15 +670,92 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
 }  // namespace
 
 // ---- PlanNode ------------------------------------------------------------------------------------------
+namespace {
+
+struct FnName {
+  const char* name;  // as the reference's projection shows it (ScalarFunctionExpr::name)
+  int id;            // enum b2p_ifn
+  int min_args, max_args;
+};
+// planner.rs:2368-2413: DataFusion math builtins under their own names, rad / deg / sgn as radians / degrees / signum,
+// round as the prom_round UDF (a missing argument becomes 0.0), clamp* from GreptimeDB's scalar functions
+const FnName kInstantFns[] = {
+    {"abs", B2P_IFN_ABS, 0, 0},       {"ceil", B2P_IFN_CEIL, 0, 0},     {"floor", B2P_IFN_FLOOR, 0, 0},
+    {"sqrt", B2P_IFN_SQRT, 0, 0},     {"exp", B2P_IFN_EXP, 0, 0},       {"ln", B2P_IFN_LN, 0, 0},
+    {"log2", B2P_IFN_LOG2, 0, 0},     {"log10", B2P_IFN_LOG10, 0, 0},   {"sin", B2P_IFN_SIN, 0, 0},
+    {"cos", B2P_IFN_COS, 0, 0},       {"tan", B2P_IFN_TAN, 0, 0},       {"asin", B2P_IFN_ASIN, 0, 0},
+    {"acos", B2P_IFN_ACOS, 0, 0},     {"atan", B2P_IFN_ATAN, 0, 0},     {"sinh", B2P_IFN_SINH, 0, 0},
+    {"cosh", B2P_IFN_COSH, 0, 0},     {"tanh", B2P_IFN_TANH, 0, 0},     {"asinh", B2P_IFN_ASINH, 0, 0},
+    {"acosh", B2P_IFN_ACOSH, 0, 0},   {"atanh", B2P_IFN_ATANH, 0, 0},   {"prom_round", B2P_IFN_ROUND, 0, 1},
+    {"degrees", B2P_IFN_DEG, 0, 0},   {"radians", B2P_IFN_RAD, 0, 0},   {"signum", B2P_IFN_SGN, 0, 0},
+    {"clamp", B2P_IFN_CLAMP, 2, 2},   {"clamp_min", B2P_IFN_CLAMP_MIN, 1, 1}, {"clamp_max", B2P_IFN_CLAMP_MAX, 1, 1},
+};
+
+// an f64 as Rust's Display writes it: the shortest digits that round-trip, never an exponent ("12", "0.5", "inf")
+std::string rust_display(double x) {
+  if (std::isnan(x)) return "NaN";
+  char buf[400];
+  const auto res = std::to_chars(buf, buf + sizeof buf, x, std::chars_format::fixed);
+  return std::string(buf, res.ptr);
+}
+
+}  // namespace
+
 void PlanNode::add_scalar_op(int op, double scalar, bool scalar_on_left, bool return_bool) {
   check_op(op, return_bool);
-  scalar_ops_.push_back(ScalarOp{op, scalar, scalar_on_left, return_bool});
+  Stage s;
+  s.op = op;
+  s.scalar = scalar;
+  s.scalar_on_left = scalar_on_left;
+  s.return_bool = return_bool;
+  stages_.push_back(s);
+}
+
+void PlanNode::add_function(const std::string& name, const std::vector<double>& args) {
+  for (const FnName& f : kInstantFns) {
+    if (name != f.name) continue;
+    const int n = (int)args.size();
+    if (n < f.min_args || n > f.max_args)
+      throw PlanError(ErrorKind::Plan, name + " takes " + std::to_string(f.min_args) +
+                                           (f.max_args != f.min_args ? " or " + std::to_string(f.max_args) : "") +
+                                           " argument(s) after the vector, got " + std::to_string(n));
+    Stage s;
+    s.is_fn = true;
+    s.op = f.id;
+    s.fn_name = name;
+    s.args = args;
+    if (f.id == B2P_IFN_ROUND && args.empty()) s.args.push_back(0.0);
+    stages_.push_back(s);
+    return;
+  }
+  throw PlanError(ErrorKind::Plan, "unsupported instant-vector function " + name);
 }
 
 void PlanNode::run(NodeResult& r) {
   compute(r);
-  for (const ScalarOp& s : scalar_ops_) {
-    if (r.rows > 0 && r.T > 0) {
+  for (const Stage& s : stages_) {
+    const bool work = r.rows > 0 && r.T > 0;
+    if (s.is_fn) {
+      const double a0 = s.args.size() > 0 ? s.args[0] : 0.0, a1 = s.args.size() > 1 ? s.args[1] : 0.0;
+      // clamp's bound check (clamp.rs:212-217); clamp_min / clamp_max meet the other bound at ±f64::MAX.  The reference
+      // checks inside the function's invoke, once per input batch, so a node without rows gives no error
+      const double lo = s.op == B2P_IFN_CLAMP_MAX ? -DBL_MAX : a0;
+      const double hi = s.op == B2P_IFN_CLAMP ? a1 : s.op == B2P_IFN_CLAMP_MIN ? DBL_MAX : a0;
+      const bool has_rows = std::any_of(r.valid.begin(), r.valid.end(), [](uint32_t w) { return w != 0; });
+      if (s.op >= B2P_IFN_CLAMP && lo > hi && has_rows)
+        throw PlanError(ErrorKind::Execution, "min '" + rust_display(lo) + "' > max '" + rust_display(hi) + "'");
+      if (work) {
+        const int rc = b2p_instant_fn(ctx_, s.op, a0, a1, r.val.data(), r.valid.data(), r.rows, (uint64_t)r.T,
+                                      r.val.data(), r.valid.data());
+        if (rc == B2P_E_INVALID) throw PlanError(ErrorKind::Plan, b2p_last_error());
+        if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
+      }
+      std::string name = s.fn_name + "(" + r.value_name;
+      for (double a : s.args) name += "," + float_literal(a);
+      r.value_name = name + ")";
+      continue;
+    }
+    if (work) {
       const int rc = b2p_scalar_op(ctx_, s.op, s.return_bool ? 1 : 0, s.scalar_on_left ? 1 : 0, s.scalar, r.val.data(),
                                    r.valid.data(), r.rows, (uint64_t)r.T, r.val.data(), r.valid.data());
       if (rc == B2P_E_INVALID) throw PlanError(ErrorKind::Plan, b2p_last_error());
@@ -940,6 +1019,48 @@ void SetOpPlan::compute(NodeResult& r) {
   }
 }
 
+// ---- ScalarPlan ----------------------------------------------------------------------------------------
+ScalarPlan::ScalarPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child) : PlanNode(ctx), child_(std::move(child)) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromScalarExec: NULL context");
+  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromScalarExec: NULL child");
+}
+
+void ScalarPlan::compute(NodeResult& r) {
+  NodeResult C;
+  child_->run(C);
+  // one dense key per label tuple over the child's tag columns (a tagless child is one series, an id-keyed one is keyed
+  // by the id); a tuple with a NULL label gets B2P_NO_KEY (scalar_calculate.rs:543-569 compares NULL as None against
+  // the "" it recorded)
+  std::vector<uint32_t> key(C.rows, 0u);
+  if (!C.tag_names.empty()) {
+    KeyIds ids;
+    std::vector<int> all(C.tag_names.size());
+    std::iota(all.begin(), all.end(), 0);
+    std::string k;
+    for (uint32_t q = 0; q < C.rows; ++q) {
+      bool null_label = false;
+      if (!C.id_keyed)
+        for (const auto& col : C.tags) null_label |= col[q] == kNullLabel;
+      append_key(C, all, q, k);
+      key[q] = null_label ? B2P_NO_KEY : ids.add(k);
+    }
+  }
+  r = NodeResult();
+  r.T = C.T;
+  r.Tw = C.Tw;
+  r.rows = 1;
+  r.eval_ts = C.eval_ts;
+  r.time_index = C.time_index;
+  r.value_name = "scalar(" + C.value_name + ")";
+  r.val.assign((size_t)r.T, 0.0);
+  r.valid.assign((size_t)r.Tw, 0u);
+  if (r.T > 0) {
+    const int rc = b2p_scalar_calculate(ctx_, C.val.data(), C.valid.data(), key.data(), C.rows, (uint64_t)r.T,
+                                        r.val.data(), r.valid.data());
+    if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
+  }
+}
+
 }  // namespace b2p
 
 // ---- C entry points -----------------------------------------------------------------------------------
@@ -1081,6 +1202,35 @@ int b2p_plan_set_scalar_op(b2p_plan* plan, int32_t op, double scalar, int32_t sc
   } catch (const b2p::PlanError& e) {
     return plan_fail(e);
   }
+}
+
+int b2p_plan_set_function(b2p_plan* plan, const char* name, const double* args, int32_t n_args) {
+  if (!plan || !name || n_args < 0 || (n_args > 0 && !args)) return B2P_E_INVALID;
+  try {
+    plan->node->add_function(name, std::vector<double>(args, args + n_args));
+    return B2P_OK;
+  } catch (const b2p::PlanError& e) {
+    return plan_fail(e);
+  }
+}
+
+b2p_plan* b2p_plan_scalar_create(b2p_ctx* ctx, b2p_plan* child) {
+  try {
+    if (!child) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    auto* h = new b2p_plan();
+    try {
+      h->node = std::make_shared<b2p::ScalarPlan>(ctx, child->node);
+    } catch (...) {
+      delete h;
+      throw;
+    }
+    return h;
+  } catch (const b2p::PlanError& e) {
+    plan_fail(e);
+  } catch (const std::exception& e) {
+    g_err = e.what();
+  }
+  return nullptr;
 }
 
 int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema) {

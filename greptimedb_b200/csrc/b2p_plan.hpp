@@ -96,11 +96,15 @@ struct NodeResult {
   bool valid_at(uint32_t r, int64_t k) const { return (valid[(size_t)r * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u; }
 };
 
-// `node op scalar` / `scalar op node` applied to a node's result (b2p_plan_set_scalar_op)
-struct ScalarOp {
-  int op;
-  double scalar;
-  bool scalar_on_left, return_bool;
+// One element-wise stage on top of a node's result: `node op scalar` / `scalar op node` (b2p_plan_set_scalar_op), or an
+// instant-vector function (b2p_plan_set_function).  A node applies its stages in the order they were added.
+struct Stage {
+  bool is_fn = false;
+  int op = 0;                 // enum b2p_binop; enum b2p_ifn when is_fn
+  double scalar = 0.0;
+  bool scalar_on_left = false, return_bool = false;
+  std::string fn_name;        // the function as the reference's projection names it ("abs", "prom_round", ...)
+  std::vector<double> args;   // its literal arguments after the value column
 };
 
 // A plan node: computes its result (step 1), then exports it as one Arrow batch (step 2).
@@ -108,18 +112,19 @@ class PlanNode {
  public:
   explicit PlanNode(b2p_ctx* ctx) : ctx_(ctx) {}
   virtual ~PlanNode() = default;
-  // the node's result with its scalar operators applied
+  // the node's result with its element-wise stages applied
   void run(NodeResult& r);
   // runs the node and exports the result batch (caller releases it)
   void execute(ArrowArray* out, ArrowSchema* out_schema);
   void add_scalar_op(int op, double scalar, bool scalar_on_left, bool return_bool);
+  void add_function(const std::string& name, const std::vector<double>& args);
 
  protected:
   virtual void compute(NodeResult& r) = 0;
   b2p_ctx* ctx_;
 
  private:
-  std::vector<ScalarOp> scalar_ops_;
+  std::vector<Stage> stages_;
 };
 
 class PromRangePlan : public PlanNode {
@@ -204,6 +209,21 @@ class SetOpPlan : public PlanNode {
   std::shared_ptr<PlanNode> lhs_, rhs_;
   Matching matching_;
   std::vector<std::string> labels_;
+};
+
+// scalar(child), the reference's ScalarCalculateExec (planner.rs:3141-3183, scalar_calculate.rs:532-637): a tagless node
+// with one row over the child's steps.  The child's label tuples become dense series keys on the host (a tuple with a
+// NULL label: B2P_NO_KEY); the decision and the copy are b2p_scalar_calculate.
+class ScalarPlan : public PlanNode {
+ public:
+  ScalarPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child);
+  const char* name() const { return "GpuPromScalarExec"; }
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  std::shared_ptr<PlanNode> child_;
 };
 
 int function_id_from_name(const std::string& prom_name);  // -1 when unknown

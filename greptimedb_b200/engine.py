@@ -34,6 +34,17 @@ SETOP_IDS = {"and": 0, "or": 1, "unless": 2}
 NO_KEY = 0xFFFFFFFF
 
 
+# enum b2p_ifn: instant-vector math functions under their PromQL names
+IFN_IDS = {"abs": 0, "ceil": 1, "floor": 2, "sqrt": 3, "exp": 4, "ln": 5, "log2": 6, "log10": 7, "sin": 8, "cos": 9,
+           "tan": 10, "asin": 11, "acos": 12, "atan": 13, "sinh": 14, "cosh": 15, "tanh": 16, "asinh": 17,
+           "acosh": 18, "atanh": 19, "round": 20, "deg": 21, "rad": 22, "sgn": 23, "clamp": 24, "clamp_min": 25,
+           "clamp_max": 26}
+
+
+def ifn_id(fn) -> int:
+    return IFN_IDS[fn] if isinstance(fn, str) else int(fn)
+
+
 def op_id(op) -> int:
     return OP_IDS[op] if isinstance(op, str) else int(op)
 
@@ -267,6 +278,31 @@ class Context:
                                       _ptr(rhs_valid), _ptr(rhs_key), R, int(n_keys), T, _ptr(out), _ptr(ov)))
         return out, ov
 
+    def instant_fn(self, fn, vals, valid, arg0=0.0, arg1=0.0):
+        """fn(vals) where valid (round: arg0 = to_nearest; clamp: arg0, arg1 = lo, hi; clamp_min / clamp_max: arg0)
+        -> (out [S,T] f64, valid_words [S,Tw] u32, unchanged)."""
+        vals = np.ascontiguousarray(vals, np.float64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        S, T = vals.shape
+        out = np.zeros((S, T), np.float64)
+        ov = np.zeros((S, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_instant_fn(self._h, ifn_id(fn), float(arg0), float(arg1), _ptr(vals), _ptr(valid), S, T,
+                                           _ptr(out), _ptr(ov)))
+        return out, ov
+
+    def scalar_calculate(self, vals, valid, row_key):
+        """scalar() over a grid whose rows carry dense series keys (NO_KEY: a label tuple with a NULL)
+        -> (out [T] f64, valid_words [Tw] u32)."""
+        vals = np.ascontiguousarray(vals, np.float64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        row_key = np.ascontiguousarray(row_key, np.uint32)
+        S, T = vals.shape
+        out = np.zeros(T, np.float64)
+        ov = np.zeros((T + 31) // 32, np.uint32)
+        self._check(self._L.b2p_scalar_calculate(self._h, _ptr(vals), _ptr(valid), _ptr(row_key), S, T, _ptr(out),
+                                                 _ptr(ov)))
+        return out, ov
+
     # -- device API (torch tensors or raw pointers; asynchronous) ----------------------------------
     def series_offsets_dev(self, sid, n_rows, n_series, offsets):
         self._check(self._L.b2p_series_offsets_dev(self._h, _ptr(sid), n_rows, n_series, _ptr(offsets)))
@@ -372,6 +408,14 @@ class Context:
         self._check(self._L.b2p_setop_dev(self._h, setop_id(op), _ptr(lhs), _ptr(lhs_valid), _ptr(lhs_key), n_lhs_rows,
                                           _ptr(rhs), _ptr(rhs_valid), _ptr(rhs_key), n_rhs_rows, int(n_keys), T,
                                           _ptr(out), _ptr(out_valid)))
+
+    def instant_fn_dev(self, fn, vals, valid, n_rows, T, out, out_valid, arg0=0.0, arg1=0.0):
+        self._check(self._L.b2p_instant_fn_dev(self._h, ifn_id(fn), float(arg0), float(arg1), _ptr(vals), _ptr(valid),
+                                               n_rows, T, _ptr(out), _ptr(out_valid)))
+
+    def scalar_calculate_dev(self, vals, valid, row_key, n_rows, T, out, out_valid):
+        self._check(self._L.b2p_scalar_calculate_dev(self._h, _ptr(vals), _ptr(valid), _ptr(row_key), n_rows, T,
+                                                     _ptr(out), _ptr(out_valid)))
 
     def count_valid_words_dev(self, cnt, n_rows, T, valid_words):
         self._check(self._L.b2p_count_valid_words_dev(self._h, _ptr(cnt), n_rows, T, _ptr(valid_words)))

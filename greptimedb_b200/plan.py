@@ -4,8 +4,9 @@
 (SeriesDivide tag_columns/time_index, SeriesNormalize offset/need_filter_out_nan, RangeManipulate
 start/end/interval/range/field column, the prom_* UDF name, optional by-label aggregate) and is fed
 pyarrow RecordBatches exactly like the reference's tests feed a MemoryExec.  `scalar_op` puts `node op number` on
-top of any node, `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels) and `SetOpPlan` applies
-`and` / `or` / `unless` to two nodes.
+top of any node, `function` an instant-vector function (abs, clamp_min, prom_round, ...; the two chain in call order),
+`BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels), `SetOpPlan` applies `and` / `or` / `unless`
+to two nodes and `ScalarPlan` is scalar(node).
 """
 from __future__ import annotations
 
@@ -43,6 +44,16 @@ class _PlanNode:
         """`node op scalar` (or `scalar op node`) on top of this node; calls chain in order.  Returns self."""
         rc = self._L.b2p_plan_set_scalar_op(self._h, op_id(op), float(scalar), int(bool(scalar_on_left)),
                                             int(bool(return_bool)))
+        if rc != 0:
+            raise B2PError(rc, self._L.b2p_plan_last_error().decode())
+        return self
+
+    def function(self, name: str, *args: float) -> "_PlanNode":
+        """`name(node, args...)` on top of this node, `name` as the reference's projection shows it ("abs", "radians",
+        "degrees", "signum", "prom_round", "clamp", "clamp_min", ...); chains with scalar_op in call order.  Returns
+        self."""
+        arr = (C.c_double * max(len(args), 1))(*[float(a) for a in args])
+        rc = self._L.b2p_plan_set_function(self._h, name.encode(), arr, len(args))
         if rc != 0:
             raise B2PError(rc, self._L.b2p_plan_last_error().decode())
         return self
@@ -143,5 +154,19 @@ class SetOpPlan(_PlanNode):
             else (None, [])
         arr = _cstr_array(labels)
         self._h = self._L.b2p_plan_setop_create(ctx._h, setop_id(op), lhs._h, rhs._h, matching, arr, len(labels))
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class ScalarPlan(_PlanNode):
+    """scalar(child): a tagless one-row node over the child's steps.  The child's one series (every row one label
+    tuple) as it is, or NaN at every step when the child has no rows or two or more series.  The child stays usable
+    and is kept alive by this node."""
+
+    def __init__(self, ctx: Context, child: _PlanNode):
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (child,)
+        self._h = self._L.b2p_plan_scalar_create(ctx._h, child._h)
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())

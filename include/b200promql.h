@@ -32,6 +32,9 @@
  *                              HashJoinExec on (tag columns, time index), planner.rs:556-777, 3436-3546; the join is a
  *                              host-side series match that yields (lhs row, rhs row) pairs
  *   b2p_scalar_op[_dev]        vector-scalar arithmetic / comparison (ProjectionExec / FilterExec, planner.rs:556-777)
+ *   b2p_instant_fn[_dev]       instant-vector math functions: the Projection of planner.rs:2368-2413 (DataFusion math
+ *                              builtins, prom_round round.rs:52-105, clamp / clamp_min / clamp_max clamp.rs:75-325)
+ *   b2p_scalar_calculate[_dev] scalar(): ScalarCalculateStream, scalar_calculate.rs:532-637
  *   b2p_setop[_dev]            set operators: `and` / `unless` = left.distinct() LeftSemi / LeftAnti HashJoinExec on
  *                              (key columns, time index), planner.rs:3549-3703; `or` = UnionDistinctOnExec,
  *                              planner.rs:3707-3906, union_distinct_on.rs:338-577; the key match is done by the caller
@@ -114,6 +117,16 @@ enum b2p_agg { B2P_AGG_SUM = 0, B2P_AGG_AVG = 1, B2P_AGG_COUNT = 2, B2P_AGG_MIN 
 enum b2p_binop { B2P_OP_ADD = 0, B2P_OP_SUB = 1, B2P_OP_MUL = 2, B2P_OP_DIV = 3, B2P_OP_MOD = 4, B2P_OP_POW = 5,
                  B2P_OP_ATAN2 = 6, B2P_OP_EQ = 7, B2P_OP_NE = 8, B2P_OP_GT = 9, B2P_OP_LT = 10, B2P_OP_GE = 11,
                  B2P_OP_LE = 12 };
+
+/* PromQL instant-vector math functions (planner.rs:2368-2413): element-wise over a node's value column, validity
+ * unchanged.  ROUND takes arg0 = to_nearest (0: to an integer); CLAMP takes arg0 = lo, arg1 = hi; CLAMP_MIN takes arg0 = lo
+ * (hi = f64::MAX); CLAMP_MAX takes arg0 = hi (lo = -f64::MAX).  The other functions take no argument. */
+enum b2p_ifn { B2P_IFN_ABS = 0, B2P_IFN_CEIL = 1, B2P_IFN_FLOOR = 2, B2P_IFN_SQRT = 3, B2P_IFN_EXP = 4, B2P_IFN_LN = 5,
+               B2P_IFN_LOG2 = 6, B2P_IFN_LOG10 = 7, B2P_IFN_SIN = 8, B2P_IFN_COS = 9, B2P_IFN_TAN = 10, B2P_IFN_ASIN = 11,
+               B2P_IFN_ACOS = 12, B2P_IFN_ATAN = 13, B2P_IFN_SINH = 14, B2P_IFN_COSH = 15, B2P_IFN_TANH = 16,
+               B2P_IFN_ASINH = 17, B2P_IFN_ACOSH = 18, B2P_IFN_ATANH = 19, B2P_IFN_ROUND = 20, B2P_IFN_DEG = 21,
+               B2P_IFN_RAD = 22, B2P_IFN_SGN = 23, B2P_IFN_CLAMP = 24, B2P_IFN_CLAMP_MIN = 25, B2P_IFN_CLAMP_MAX = 26,
+               B2P_IFN__COUNT = 27 };
 
 /* PromQL set operators; they work per (match key, step) cell and copy cells, never compute values. */
 enum b2p_setop { B2P_SET_AND = 0, B2P_SET_OR = 1, B2P_SET_UNLESS = 2 };
@@ -296,6 +309,22 @@ B2P_API int b2p_setop_dev(b2p_ctx* ctx, int32_t op /* enum b2p_setop */, const d
                           const uint32_t* rhs_key, uint32_t n_rhs_rows, uint32_t n_keys, uint64_t T, double* out,
                           uint32_t* out_valid);
 
+/* Instant-vector function `fn` (enum b2p_ifn) over a dense grid: out[r*T + k] = fn(vals[r*T + k]) where the validity
+ * bit is set, 0.0 elsewhere; out_valid = valid (copied when out_valid != valid).  out / out_valid may be vals / valid
+ * (in place).  abs ceil floor sqrt round deg rad sgn clamp* are bit-identical to the reference's Rust; the
+ * transcendental functions are CUDA's, within the ulp bound DESIGN.md section 2 states.  B2P_E_INVALID: unknown fn;
+ * a clamp bound pair with lo > hi (clamp_min(v, +inf) and clamp_max(v, -inf) included). */
+B2P_API int b2p_instant_fn_dev(b2p_ctx* ctx, int32_t fn /* enum b2p_ifn */, double arg0, double arg1, const double* vals,
+                               const uint32_t* valid, uint64_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
+/* scalar(v), the reference's ScalarCalculate (scalar_calculate.rs:532-637), over the whole grid: row_key[r] is a dense
+ * series id (< n_rows) or B2P_NO_KEY for a row whose labels include a NULL.  When every row with a cell carries one key
+ * (a B2P_NO_KEY row: only while it has exactly one cell), out [T] / out_valid [Tw] are that series' cells, bit copies;
+ * otherwise (no cells, or two or more series) out is NaN at every step with every bit valid.  Two rows of one key with
+ * a cell at the same step, or a key >= n_rows other than B2P_NO_KEY, are found on the device (B2P_E_INVALID from
+ * b2p_sync).  No host round trip between the two passes. */
+B2P_API int b2p_scalar_calculate_dev(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const uint32_t* row_key,
+                                     uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
+
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
  * the id column `sid` (ids sid_base .. sid_base + n_series - 1, non-decreasing), or copied from `offsets_in`
@@ -345,6 +374,12 @@ B2P_API int b2p_scalar_op(b2p_ctx* ctx, int32_t op, int32_t return_bool, int32_t
 B2P_API int b2p_setop(b2p_ctx* ctx, int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key,
                       uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid, const uint32_t* rhs_key,
                       uint32_t n_rhs_rows, uint32_t n_keys, uint64_t T, double* out, uint32_t* out_valid);
+
+/* Host-pointer forms of b2p_instant_fn_dev / b2p_scalar_calculate_dev (synchronous; device-found errors returned). */
+B2P_API int b2p_instant_fn(b2p_ctx* ctx, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
+                           uint64_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
+B2P_API int b2p_scalar_calculate(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const uint32_t* row_key,
+                                 uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
 
 /* ---- plan-level API over the Arrow C Data Interface ------------------------------------------------
  * GpuPromRangeExec: the whole sub-tree SeriesDivide -> SeriesNormalize -> RangeManipulate ->
@@ -424,6 +459,17 @@ B2P_API b2p_plan* b2p_plan_binary_create(b2p_ctx* ctx, int32_t op, int32_t retur
 B2P_API b2p_plan* b2p_plan_setop_create(b2p_ctx* ctx, int32_t op /* enum b2p_setop */, b2p_plan* lhs, b2p_plan* rhs,
                                         const char* matching /* NULL | "on" | "ignoring" */,
                                         const char* const* labels, int32_t n_labels);
+/* Instant-vector function on top of any node, named as the reference's projection shows it: abs ceil floor sqrt exp ln
+ * log2 log10 sin cos tan asin acos atan sinh cosh tanh asinh acosh atanh, degrees, radians, signum (no argument),
+ * prom_round (0 or 1: to_nearest, default 0), clamp (lo, hi), clamp_min (lo), clamp_max (hi).  Functions and
+ * b2p_plan_set_scalar_op calls form one chain, applied in call order; the value column is renamed like the projection
+ * (abs(val), clamp(val,Float64(0),Float64(12))).  B2P_E_INVALID: unknown name or wrong argument count.  A clamp with
+ * lo > hi fails at execute, when the node has rows, with the reference's Execution error "min '12' > max '0'". */
+B2P_API int b2p_plan_set_function(b2p_plan* plan, const char* name, const double* args, int32_t n_args);
+/* scalar(child), GpuPromScalarExec: a tagless node with one row over the child's steps, columns {time index,
+ * scalar(<value name>)}; usable under scalar operators and functions and as a child of the binary and set nodes (a
+ * tagless side pairs with every row).  Ownership as for b2p_plan_binary_create.  NULL on error. */
+B2P_API b2p_plan* b2p_plan_scalar_create(b2p_ctx* ctx, b2p_plan* child);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

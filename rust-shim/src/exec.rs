@@ -61,8 +61,17 @@ pub struct GpuPromRangeParams {
     pub by_columns: Vec<String>,
     /// HistogramFold::new(le_column, .., quantile) on top (histogram_fold.rs:104-130).
     pub histogram: Option<(String, f64)>,
-    /// `node op scalar` projections / filters on top, in order: (op, scalar, scalar_on_left, return_bool).
-    pub scalar_ops: Vec<(ffi::B2pBinOp, f64, bool, bool)>,
+    /// Element-wise stages on top, in order: `node op scalar` projections / filters and instant-vector functions.
+    pub stages: Vec<GpuPromStage>,
+}
+
+/// One element-wise stage of a `GpuPromRangeExec` (b2p_plan_set_scalar_op / b2p_plan_set_function).
+#[derive(Clone, Debug)]
+pub enum GpuPromStage {
+    /// `node op scalar` (or `scalar op node`): (op, scalar, scalar_on_left, return_bool)
+    ScalarOp(ffi::B2pBinOp, f64, bool, bool),
+    /// `name(node, args..)`, `name` as the projection's ScalarFunctionExpr::name() ("abs", "prom_round", "clamp", ..)
+    Function(String, Vec<f64>),
 }
 
 #[derive(Debug)]
@@ -277,8 +286,17 @@ impl PlanHandle {
                     return Err(DataFusionError::Plan(ffi::plan_last_error()));
                 }
             }
-            for (op, scalar, on_left, return_bool) in &p.scalar_ops {
-                if ffi::b2p_plan_set_scalar_op(plan, *op as i32, *scalar, *on_left as i32, *return_bool as i32) != ffi::B2P_OK {
+            for stage in &p.stages {
+                let rc = match stage {
+                    GpuPromStage::ScalarOp(op, scalar, on_left, return_bool) => {
+                        ffi::b2p_plan_set_scalar_op(plan, *op as i32, *scalar, *on_left as i32, *return_bool as i32)
+                    }
+                    GpuPromStage::Function(name, args) => {
+                        let name = c(name);
+                        ffi::b2p_plan_set_function(plan, name.as_ptr(), args.as_ptr(), args.len() as i32)
+                    }
+                };
+                if rc != ffi::B2P_OK {
                     return Err(DataFusionError::Plan(ffi::plan_last_error()));
                 }
             }

@@ -117,7 +117,40 @@ pub enum B2pSetOp {
     Unless = 2,
 }
 
-/// `B2P_NO_KEY`: the key of a row that no row of the other side matches.
+/// `enum b2p_ifn` — PromQL instant-vector math functions (planner.rs:2368-2413).
+#[repr(i32)]
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub enum B2pIfn {
+    Abs = 0,
+    Ceil = 1,
+    Floor = 2,
+    Sqrt = 3,
+    Exp = 4,
+    Ln = 5,
+    Log2 = 6,
+    Log10 = 7,
+    Sin = 8,
+    Cos = 9,
+    Tan = 10,
+    Asin = 11,
+    Acos = 12,
+    Atan = 13,
+    Sinh = 14,
+    Cosh = 15,
+    Tanh = 16,
+    Asinh = 17,
+    Acosh = 18,
+    Atanh = 19,
+    Round = 20,
+    Deg = 21,
+    Rad = 22,
+    Sgn = 23,
+    Clamp = 24,
+    ClampMin = 25,
+    ClampMax = 26,
+}
+
+/// `B2P_NO_KEY`: the key of a row that no row of the other side matches (scalar(): a row with a NULL label).
 pub const B2P_NO_KEY: u32 = 0xFFFF_FFFF;
 
 impl B2pBinOp {
@@ -256,6 +289,14 @@ extern "C" {
         rhs: *const f64, rhs_valid: *const u32, rhs_key: *const u32, n_rhs_rows: u32, n_keys: u32, t: u64,
         out: *mut f64, out_valid: *mut u32,
     ) -> c_int;
+    pub fn b2p_instant_fn_dev(
+        ctx: *mut b2p_ctx, fn_: i32, arg0: f64, arg1: f64, vals: *const f64, valid: *const u32, n_rows: u64, t: u64,
+        out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
+    pub fn b2p_scalar_calculate_dev(
+        ctx: *mut b2p_ctx, vals: *const f64, valid: *const u32, row_key: *const u32, n_rows: u32, t: u64,
+        out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- host-side helper (no device work): SeriesDivide + cadence scan of one sorted batch ---------------------------
     pub fn b2p_host_scan_series(
@@ -304,6 +345,14 @@ extern "C" {
         rhs: *const f64, rhs_valid: *const u32, rhs_key: *const u32, n_rhs_rows: u32, n_keys: u32, t: u64,
         out: *mut f64, out_valid: *mut u32,
     ) -> c_int;
+    pub fn b2p_instant_fn(
+        ctx: *mut b2p_ctx, fn_: i32, arg0: f64, arg1: f64, vals: *const f64, valid: *const u32, n_rows: u64, t: u64,
+        out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
+    pub fn b2p_scalar_calculate(
+        ctx: *mut b2p_ctx, vals: *const f64, valid: *const u32, row_key: *const u32, n_rows: u32, t: u64,
+        out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- plan-level API over the Arrow C Data Interface -----------------------------------------------------------------
     pub fn b2p_plan_range_create(
@@ -324,6 +373,10 @@ extern "C" {
         ctx: *mut b2p_ctx, op: i32, lhs: *mut b2p_plan, rhs: *mut b2p_plan, matching: *const c_char,
         labels: *const *const c_char, n_labels: i32,
     ) -> *mut b2p_plan;
+    /// `name` as the reference's projection shows it (ScalarFunctionExpr::name): "abs", "radians", "prom_round", ...
+    pub fn b2p_plan_set_function(plan: *mut b2p_plan, name: *const c_char, args: *const f64, n_args: i32) -> c_int;
+    /// Ownership as for b2p_plan_binary_create.
+    pub fn b2p_plan_scalar_create(ctx: *mut b2p_ctx, child: *mut b2p_plan) -> *mut b2p_plan;
     /// MOVES the batch: on success the release callbacks now belong to the plan.
     pub fn b2p_plan_push_batch(plan: *mut b2p_plan, batch: *mut FFI_ArrowArray, schema: *mut FFI_ArrowSchema) -> c_int;
     pub fn b2p_plan_execute(plan: *mut b2p_plan, out: *mut FFI_ArrowArray, out_schema: *mut FFI_ArrowSchema) -> c_int;

@@ -26,6 +26,16 @@
 //!     <- GpuPromRangeExec, GpuPromRangeExec   => `match_binary_join`: the b2p_plan_binary_create arguments
 //! ```
 //!
+//! Instant-vector functions (planner.rs:2368-2413) and scalar() (planner.rs:3141-3183):
+//!
+//! ```text
+//!   ProjectionExec: expr=[.., fn(col [, Float64(c)..]), ..]   (abs .. atanh, radians, degrees, signum, prom_round, clamp*)
+//!     <- GpuPromRangeExec                     => the same node with b2p_plan_set_function appended
+//!
+//!   ScalarCalculateExec(start, end, interval, time index, tag columns, field)
+//!     <- GpuPromRangeExec                     => `match_scalar`: the b2p_plan_scalar_create child
+//! ```
+//!
 //! Set operators (planner.rs:3549-3906):
 //!
 //! ```text
@@ -56,10 +66,12 @@ use datafusion::physical_plan::projection::ProjectionExec;
 use datafusion::physical_plan::repartition::RepartitionExec;
 use datafusion::physical_plan::ExecutionPlan;
 
-use crate::exec::{GpuPromRangeExec, GpuPromRangeParams};
+use crate::exec::{GpuPromRangeExec, GpuPromRangeParams, GpuPromStage};
 use crate::ffi::{B2pBinOp, B2pFn, B2pSetOp};
 // In-tree these are `crate::extension_plan::{..}`; named here the way the reference names them.
-use promql::extension_plan::{RangeManipulateExec, SeriesDivideExec, SeriesNormalizeExec, UnionDistinctOnExec};
+use promql::extension_plan::{
+    RangeManipulateExec, ScalarCalculateExec, SeriesDivideExec, SeriesNormalizeExec, UnionDistinctOnExec,
+};
 
 #[derive(Debug)]
 pub struct GpuPromRewrite {
@@ -116,7 +128,7 @@ impl GpuPromRewrite {
             aggregate: None,
             by_columns: vec![],
             histogram: None,
-            scalar_ops: vec![],
+            stages: vec![],
         };
         Some((params, divide.input().clone()))
     }
@@ -183,6 +195,21 @@ pub struct GpuPromSetOpSpec {
     /// passed as `on(..)`: the join's tag keys (`and` / `unless`), or UnionDistinctOn's compare keys (`or`)
     pub on: Vec<String>,
 }
+
+/// What `b2p_plan_scalar_create` takes for `scalar(child)` over a rewritten node.
+#[derive(Debug)]
+pub struct GpuPromScalarSpec {
+    pub child: GpuPromRangeParams,
+}
+
+/// The instant-vector functions the library evaluates, by ScalarFunctionExpr::name(), with the number of literal
+/// arguments after the value column (planner.rs:2368-2413; prom_round always gets its to_nearest, 0.0 when omitted).
+const INSTANT_FNS: &[(&str, usize)] = &[
+    ("abs", 0), ("ceil", 0), ("floor", 0), ("sqrt", 0), ("exp", 0), ("ln", 0), ("log2", 0), ("log10", 0),
+    ("sin", 0), ("cos", 0), ("tan", 0), ("asin", 0), ("acos", 0), ("atan", 0), ("sinh", 0), ("cosh", 0),
+    ("tanh", 0), ("asinh", 0), ("acosh", 0), ("atanh", 0), ("prom_round", 1), ("degrees", 0), ("radians", 0),
+    ("signum", 0), ("clamp", 2), ("clamp_min", 1), ("clamp_max", 1),
+];
 
 /// DataFusion operator -> b2p_binop; `pow` / `atan2` arrive as scalar functions (planner.rs:3915-3990).
 fn binop_of(expr: &Arc<dyn PhysicalExpr>) -> Option<(B2pBinOp, Arc<dyn PhysicalExpr>, Arc<dyn PhysicalExpr>, bool)> {
@@ -257,8 +284,45 @@ impl GpuPromRewrite {
             _ => return None,
         };
         let mut params = node.params().clone();
-        params.scalar_ops.push((op, scalar, on_left, return_bool));
+        params.stages.push(GpuPromStage::ScalarOp(op, scalar, on_left, return_bool));
         Some((params, node.input().clone()))
+    }
+
+    /// `ProjectionExec(fn(col, lit..))` over a `GpuPromRangeExec` -> the node's parameters with the function appended
+    /// as one more stage; every other projected expression must be a plain column.
+    fn match_function(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<(GpuPromRangeParams, Arc<dyn ExecutionPlan>)> {
+        let p = plan.as_any().downcast_ref::<ProjectionExec>()?;
+        let mut value = None;
+        for e in p.expr() {
+            if e.expr.as_any().downcast_ref::<Column>().is_none() {
+                if value.is_some() {
+                    return None;
+                }
+                value = Some(e.expr.clone());
+            }
+        }
+        let value = value?;
+        let node = p.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let f = value.as_any().downcast_ref::<ScalarFunctionExpr>()?;
+        let name = f.name();
+        let &(_, n_args) = INSTANT_FNS.iter().find(|(n, _)| *n == name)?;
+        let (col, lits) = f.args().split_first()?;
+        col.as_any().downcast_ref::<Column>()?;
+        if lits.len() != n_args {
+            return None;
+        }
+        let args = lits.iter().map(float_literal).collect::<Option<Vec<f64>>>()?;
+        let mut params = node.params().clone();
+        params.stages.push(GpuPromStage::Function(name.to_string(), args));
+        Some((params, node.input().clone()))
+    }
+
+    /// `ScalarCalculateExec <- GpuPromRangeExec` -> the child of `b2p_plan_scalar_create` (no Rust execution node for the
+    /// scalar node yet, as for the binary join).
+    pub fn match_scalar(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromScalarSpec> {
+        let s = plan.as_any().downcast_ref::<ScalarCalculateExec>()?;
+        let child = s.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        Some(GpuPromScalarSpec { child: child.params().clone() })
     }
 
     /// `ProjectionExec | FilterExec <- HashJoinExec(Inner, tags.. + ts)` over two `GpuPromRangeExec` -> the arguments of
@@ -378,7 +442,8 @@ impl PhysicalOptimizerRule for GpuPromRewrite {
             let matched = self
                 .match_aggregate(&node)
                 .or_else(|| self.match_range_subtree(&node))
-                .or_else(|| self.match_scalar_op(&node));
+                .or_else(|| self.match_scalar_op(&node))
+                .or_else(|| self.match_function(&node));
             match matched {
                 Some((params, input)) => {
                     // the replaced node's schema is kept verbatim, so parents (Sort, CoalesceBatches, MergeScan ..) see no change

@@ -1,7 +1,7 @@
 /* Compile-time check of every layout assumption rust-shim/src/ffi.rs makes about include/b200promql.h.
  *   gcc -std=c11 -fsyntax-only -I../../include layout.c        (tests/test_abi.py runs exactly this)
  * If a field of struct b2p_range_params moves, or an enum value changes, this file stops compiling — and
- * B2pRangeParams / B2pFn / B2pAgg / B2pBinOp in ffi.rs have to follow. */
+ * B2pRangeParams / B2pFn / B2pAgg / B2pBinOp / B2pIfn in ffi.rs have to follow. */
 #include <stddef.h>
 #include <stdint.h>
 
@@ -40,6 +40,14 @@ SA(sizeof(enum b2p_binop) == 4, "b2p_binop is passed as i32");
 SA(B2P_SET_AND == 0 && B2P_SET_OR == 1 && B2P_SET_UNLESS == 2, "B2pSetOp");
 SA(sizeof(enum b2p_setop) == 4, "b2p_setop is passed as i32");
 SA(B2P_NO_KEY == 0xFFFFFFFFu, "B2P_NO_KEY");
+/* #[repr(i32)] enum B2pIfn */
+SA(B2P_IFN_ABS == 0 && B2P_IFN_CEIL == 1 && B2P_IFN_FLOOR == 2 && B2P_IFN_SQRT == 3 && B2P_IFN_EXP == 4, "B2pIfn 0-4");
+SA(B2P_IFN_LN == 5 && B2P_IFN_LOG2 == 6 && B2P_IFN_LOG10 == 7 && B2P_IFN_SIN == 8 && B2P_IFN_COS == 9, "B2pIfn 5-9");
+SA(B2P_IFN_TAN == 10 && B2P_IFN_ASIN == 11 && B2P_IFN_ACOS == 12 && B2P_IFN_ATAN == 13 && B2P_IFN_SINH == 14, "B2pIfn 10-14");
+SA(B2P_IFN_COSH == 15 && B2P_IFN_TANH == 16 && B2P_IFN_ASINH == 17 && B2P_IFN_ACOSH == 18 && B2P_IFN_ATANH == 19, "B2pIfn 15-19");
+SA(B2P_IFN_ROUND == 20 && B2P_IFN_DEG == 21 && B2P_IFN_RAD == 22 && B2P_IFN_SGN == 23 && B2P_IFN_CLAMP == 24, "B2pIfn 20-24");
+SA(B2P_IFN_CLAMP_MIN == 25 && B2P_IFN_CLAMP_MAX == 26 && B2P_IFN__COUNT == 27, "B2pIfn 25-27");
+SA(sizeof(enum b2p_ifn) == 4, "b2p_ifn is passed as i32");
 /* status codes and sizes the shim hard-codes */
 SA(B2P_OK == 0 && B2P_E_INVALID == -1 && B2P_E_CUDA == -2 && B2P_E_UNSORTED == -3 && B2P_E_NOMEM == -4 && B2P_E_TOO_LARGE == -5, "codes");
 SA(B2P_COMM_ID_BYTES == 128, "communicator id");
