@@ -9,7 +9,6 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
-#include <map>
 #include <numeric>
 #include <unordered_map>
 
@@ -42,9 +41,25 @@ bool starts_with(const char* s, const char* p) { return std::strncmp(s, p, std::
 
 bool bit_set(const uint8_t* bits, int64_t i) { return bits == nullptr || ((bits[i >> 3] >> (i & 7)) & 1); }
 
-// a NULL label: distinct from every string, equal to every other NULL label (NullEquality::NullEqualsNull)
-const std::string kNullLabel("\0null", 5);
 constexpr int64_t kArrowFlagNullable = 2;  // ARROW_FLAG_NULLABLE of the C Data Interface
+
+// Throws the PlanError of a failed b2p_* call, with the call's message: arguments the call rejects (B2P_E_INVALID,
+// B2P_E_TOO_LARGE) as `invalid`, input out of series order (B2P_E_UNSORTED) as Internal, anything else as Execution.
+void check(int rc, ErrorKind invalid = ErrorKind::Plan) {
+  if (rc == B2P_OK) return;
+  if (rc == B2P_E_INVALID || rc == B2P_E_TOO_LARGE) throw PlanError(invalid, b2p_last_error());
+  throw PlanError(rc == B2P_E_UNSORTED ? ErrorKind::Internal : ErrorKind::Execution, b2p_last_error());
+}
+
+// dense ids of keys, in first-insertion order
+struct KeyIds {
+  std::unordered_map<std::string, uint32_t> ids;
+  uint32_t add(const std::string& k) { return ids.emplace(k, (uint32_t)ids.size()).first->second; }
+  uint32_t find(const std::string& k) const {
+    const auto it = ids.find(k);
+    return it == ids.end() ? B2P_NO_KEY : it->second;
+  }
+};
 
 // ---- export helpers: an ArrowArray whose buffers live in a heap object ---------------------------------
 struct OwnedColumn {
@@ -169,18 +184,115 @@ int RecordBatch::find(const std::string& name) const {
   return -1;
 }
 
+// ---- Labels --------------------------------------------------------------------------------------------
+int Labels::column(const std::string& name) const {
+  const auto it = std::find(names.begin(), names.end(), name);
+  return it == names.end() ? -1 : (int)(it - names.begin());
+}
+
+std::vector<int> Labels::columns(const std::vector<std::string>& ns) const {
+  std::vector<int> cols;
+  for (const std::string& n : ns) cols.push_back(column(n));
+  return cols;
+}
+
+Label Labels::value(int c, uint32_t r) const {
+  if (c < 0) return std::nullopt;
+  return id_keyed ? Label(std::to_string(ids[r])) : values[(size_t)c][r];
+}
+
+// NULL is "-"; a string is its length, ':' and its bytes.  No encoding is a prefix of another, so no two tuples share one.
+void Labels::key(uint32_t r, const std::vector<int>& cols, std::string& key) const {
+  key.clear();
+  auto put = [&](const std::string& v) {
+    key += std::to_string(v.size());
+    key.push_back(':');
+    key += v;
+  };
+  for (int c : cols) {
+    if (c >= 0 && id_keyed) {
+      put(std::to_string(ids[r]));
+    } else if (c >= 0 && values[(size_t)c][r]) {
+      put(*values[(size_t)c][r]);
+    } else {
+      key.push_back('-');
+    }
+  }
+}
+
+Labels Labels::gather(const std::vector<uint32_t>& rows) const {
+  Labels out;
+  out.names = names;
+  out.id_keyed = id_keyed;
+  if (id_keyed)
+    for (uint32_t r : rows) out.ids.push_back(ids[r]);
+  out.values.resize(values.size());
+  for (size_t t = 0; t < values.size(); ++t) {
+    out.values[t].reserve(rows.size());
+    for (uint32_t r : rows) out.values[t].push_back(values[t][r]);
+  }
+  return out;
+}
+
+// "" first, then NULL, then every other string in byte order, the order this plan layer's sorted output has always had.
+// The reference's aggregate sorts NULLs last instead (planner.rs:443, `sort(true, false)`); DESIGN.md §2 lists this as
+// a known divergence.
+bool Labels::less(const Label& a, const Label& b) {
+  auto rank = [](const Label& v) { return !v ? 1 : v->empty() ? 0 : 2; };
+  if (rank(a) != rank(b)) return rank(a) < rank(b);
+  return rank(a) == 2 && *a < *b;
+}
+
+namespace {
+
+// The rows of `in` grouped by their tuple over `cols`, for output in label order (the by-label aggregate, HistogramFold)
+struct Groups {
+  std::vector<uint32_t> id;    // [row] its group, numbered in order of first appearance
+  std::vector<uint32_t> rank;  // [group] its place in label order
+  Labels labels;               // [place] the group's tuple over `cols` (ids as decimal strings)
+};
+
+Groups group_rows(const Labels& in, const std::vector<int>& cols, uint32_t rows) {
+  Groups g;
+  g.id.resize(rows);
+  KeyIds ids;
+  std::vector<uint32_t> first;  // [group] its first row
+  std::string key;
+  for (uint32_t r = 0; r < rows; ++r) {
+    in.key(r, cols, key);
+    g.id[r] = ids.add(key);
+    if (g.id[r] == first.size()) first.push_back(r);
+  }
+  const uint32_t G = (uint32_t)first.size();
+  Labels tuples;  // [group]
+  tuples.values.resize(cols.size());
+  for (size_t t = 0; t < cols.size(); ++t) {
+    tuples.names.push_back(in.names[(size_t)cols[t]]);
+    for (uint32_t f : first) tuples.values[t].push_back(in.value(cols[t], f));
+  }
+  std::vector<uint32_t> order(G);
+  std::iota(order.begin(), order.end(), 0u);
+  std::sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) {
+    for (const std::vector<Label>& col : tuples.values) {
+      if (Labels::less(col[x], col[y])) return true;
+      if (Labels::less(col[y], col[x])) return false;
+    }
+    return false;
+  });
+  g.rank.resize(G);
+  for (uint32_t q = 0; q < G; ++q) g.rank[order[q]] = q;
+  g.labels = tuples.gather(order);
+  return g;
+}
+
+}  // namespace
+
 // ---- PromRangePlan -------------------------------------------------------------------------------------
 PromRangePlan::PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args) : PlanNode(ctx), args_(std::move(args)) {
   if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromRangeExec: NULL context");
   fn_id_ = args_.function.empty() ? -1 : function_id_from_name(args_.function);
   if (fn_id_ < 0 && !args_.function.empty())
     throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: unknown range function " + args_.function);
-  if (args_.histogram) {
-    if (std::find(args_.tag_columns.begin(), args_.tag_columns.end(), args_.le_column) == args_.tag_columns.end())
-      throw PlanError(ErrorKind::Plan, "HistogramFold: le column " + args_.le_column + " is not a tag column");
-    if (!args_.aggregate.empty())
-      throw PlanError(ErrorKind::Plan, "HistogramFold over an aggregate is not supported by this node");
-  }
   agg_id_ = -1;
   if (!args_.aggregate.empty()) {
     agg_id_ = aggregate_id_from_name(args_.aggregate);
@@ -192,7 +304,8 @@ PromRangePlan::PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args) : PlanNode(ct
   if (args_.interval <= 0) throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: interval must be positive");
   if (args_.time_index.empty() || args_.field_column.empty())
     throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: time index and field column are required");
-  tags_.utf8.resize(args_.tag_columns.size());
+  series_.names = args_.tag_columns;
+  series_.values.resize(args_.tag_columns.size());
 }
 
 void PromRangePlan::set_histogram(const std::string& le_column, double quantile) {
@@ -246,16 +359,17 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
       tc.data = static_cast<const char*>(ca.buffers[2]);
     } else if (std::strcmp(fmt, "L") == 0 && args_.tag_columns.size() == 1) {
       tc.ids = static_cast<const uint64_t*>(ca.buffers[1]);
-      key_is_id_ = true;
+      series_.id_keyed = true;
+      series_.values.clear();
     } else {
       throw PlanError(ErrorKind::Execution, "tag column " + args_.tag_columns[t] + " must be Utf8 (or one UInt64 id)");
     }
     tcols.push_back(tc);
   }
-  auto tag_at = [&](size_t t, int64_t row) -> std::string {
+  auto tag_at = [&](size_t t, int64_t row) -> Label {
     const TagCol& tc = tcols[t];
     const int64_t r = tc.base + row;
-    if (!bit_set(tc.valid, r)) return kNullLabel;
+    if (!bit_set(tc.valid, r)) return std::nullopt;
     return std::string(tc.data + tc.off[r], (size_t)(tc.off[r + 1] - tc.off[r]));
   };
 
@@ -275,16 +389,16 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
     offsets_.push_back((uint64_t)(row_base + (size_t)row));
     ++num_series_;
   };
-  if (key_is_id_) {
+  if (series_.id_keyed) {
     const uint64_t* ids = tcols[0].ids + tcols[0].base;
     int64_t row = 0;
     if (!have_last_ || ids[0] != last_id_) {
-      tags_.tsid.push_back(ids[0]);
+      series_.ids.push_back(ids[0]);
       start_series(0);
     }
     for (row = 1; row < n; ++row)
       if (ids[row] != ids[row - 1]) {  // (a tight compare loop the compiler vectorises)
-        tags_.tsid.push_back(ids[row]);
+        series_.ids.push_back(ids[row]);
         start_series(row);
       }
     last_id_ = ids[n - 1];
@@ -308,7 +422,7 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
       return true;
     };
     auto open_series = [&](int64_t row) {
-      for (size_t t = 0; t < tcols.size(); ++t) tags_.utf8[t].push_back(tag_at(t, row));
+      for (size_t t = 0; t < tcols.size(); ++t) series_.values[t].push_back(tag_at(t, row));
       start_series(row);
     };
     if (!have_last_ || !same_as_last_key()) open_series(0);
@@ -341,25 +455,17 @@ void PromRangePlan::compute(NodeResult& r) {
   const bool fold_on_device = args_.histogram && fn_id_ >= 0;  // the dense matrix then never reaches the host
   std::vector<double> dense(fold_on_device ? 0 : (size_t)S * (size_t)T);
   std::vector<uint32_t> valid(fold_on_device ? 0 : (size_t)S * Tw);
-  std::vector<int64_t> eval_ts((size_t)T);
-  for (int64_t k = 0; k < T; ++k) eval_ts[(size_t)k] = p.start + k * p.interval;  // (scalar() of a node without rows)
-  if (S > 0 && T > 0 && !(args_.histogram && fn_id_ >= 0)) {
-    int rc;
-    if (fn_id_ >= 0) {
-      rc = b2p_range_eval(ctx_, &p, ts_.data(), val_.data(), nullptr, offsets_.data(), ts_.size(), S, dense.data(),
-                          valid.data(), eval_ts.data());
-    } else {  // InstantManipulate
-      rc = b2p_instant_select(ctx_, p.start, p.end, p.interval, args_.lookback_delta, p.offset, ts_.data(),
-                              val_.data(), nullptr, offsets_.data(), ts_.size(), S, dense.data(), valid.data());
-      for (int64_t k = 0; k < T; ++k) eval_ts[(size_t)k] = p.start + k * p.interval;
-    }
-    if (rc == B2P_E_INVALID || rc == B2P_E_TOO_LARGE) throw PlanError(ErrorKind::Plan, b2p_last_error());
-    if (rc == B2P_E_UNSORTED) throw PlanError(ErrorKind::Internal, b2p_last_error());
-    if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
-  }
+  if (S > 0 && T > 0 && !fold_on_device)
+    check(fn_id_ >= 0 ? b2p_range_eval(ctx_, &p, ts_.data(), val_.data(), nullptr, offsets_.data(), ts_.size(), S,
+                                       dense.data(), valid.data(), nullptr)
+                      : b2p_instant_select(ctx_, p.start, p.end, p.interval, args_.lookback_delta, p.offset, ts_.data(),
+                                           val_.data(), nullptr, offsets_.data(), ts_.size(), S, dense.data(),
+                                           valid.data()));  // InstantManipulate
   r = NodeResult();
   r.T = T;
   r.Tw = Tw;
+  r.eval_ts.resize((size_t)T);  // also when there are no series: scalar() of such a node has a NaN row at every step
+  for (int64_t k = 0; k < T; ++k) r.eval_ts[(size_t)k] = p.start + k * p.interval;
   r.time_index = args_.time_index;
   r.value_name =
       fn_id_ >= 0 ? args_.function + "(" + args_.time_index + "_range," + args_.field_column + ")" : args_.field_column;
@@ -367,45 +473,24 @@ void PromRangePlan::compute(NodeResult& r) {
   if (args_.histogram) {
     // HistogramFold (histogram_fold.rs:754-820): group the series by their tags without `le`, order each group's
     // buckets by le ascending (parsed as f64, "+Inf" last), one output row per (group, eval ts)
-    if (key_is_id_) throw PlanError(ErrorKind::Plan, "HistogramFold needs the le tag column, not a tsid key");
-    const size_t le_idx = (size_t)(std::find(args_.tag_columns.begin(), args_.tag_columns.end(), args_.le_column) -
-                                   args_.tag_columns.begin());
-    // histogram id of every series (hash of the tag tuple without le; ids in first-appearance order), its bound
-    std::unordered_map<std::string, uint32_t> hist_ids;
-    std::vector<std::vector<std::string>> hist_keys;
-    std::vector<uint32_t> hid(S);
-    std::vector<double> sle(S);
-    std::string flat;
+    if (series_.id_keyed) throw PlanError(ErrorKind::Plan, "HistogramFold needs the le tag column, not a tsid key");
+    const int le = series_.column(args_.le_column);
+    std::vector<int> cols;  // the tags without le
+    for (int t = 0; t < (int)series_.names.size(); ++t)
+      if (t != le) cols.push_back(t);
+    Groups hist = group_rows(series_, cols, S);
+    const uint32_t H = (uint32_t)hist.rank.size();
+    std::vector<double> sle(S);  // le.parse::<f64>().unwrap_or(NaN), histogram_fold.rs:791-796
     for (uint32_t s = 0; s < S; ++s) {
-      flat.clear();
-      for (size_t t = 0; t < args_.tag_columns.size(); ++t)
-        if (t != le_idx) {
-          flat += tags_.utf8[t][s];
-          flat.push_back('\x1f');
-        }
-      auto it = hist_ids.find(flat);
-      if (it == hist_ids.end()) {
-        it = hist_ids.emplace(flat, (uint32_t)hist_keys.size()).first;
-        std::vector<std::string> key;
-        for (size_t t = 0; t < args_.tag_columns.size(); ++t)
-          if (t != le_idx) key.push_back(tags_.utf8[t][s]);
-        hist_keys.push_back(std::move(key));
-      }
-      hid[s] = it->second;
-      sle[s] = parse_f64_like_rust(tags_.utf8[le_idx][s]);  // le.parse::<f64>().unwrap_or(NaN), histogram_fold.rs:791-796
+      const Label& v = series_.values[(size_t)le][s];
+      sle[s] = v ? parse_f64_like_rust(*v) : std::nan("");
     }
-    const uint32_t H = (uint32_t)hist_keys.size();
-    // output order = the reference's: rows sorted by the remaining tags (std::map order of the old implementation)
-    std::vector<uint32_t> hist_order(H);
-    for (uint32_t h = 0; h < H; ++h) hist_order[h] = h;
-    std::sort(hist_order.begin(), hist_order.end(), [&](uint32_t x, uint32_t y) { return hist_keys[x] < hist_keys[y]; });
-    std::vector<uint32_t> rank(H);
-    for (uint32_t q = 0; q < H; ++q) rank[hist_order[q]] = q;
     // buckets of every histogram in ascending le order, NaN bounds last, ties in scan order (a strict weak ordering)
+    auto place = [&](uint32_t s) { return hist.rank[hist.id[s]]; };
     std::vector<uint32_t> bucket_series(S);
-    for (uint32_t s = 0; s < S; ++s) bucket_series[s] = s;
+    std::iota(bucket_series.begin(), bucket_series.end(), 0u);
     std::stable_sort(bucket_series.begin(), bucket_series.end(), [&](uint32_t x, uint32_t y) {
-      if (rank[hid[x]] != rank[hid[y]]) return rank[hid[x]] < rank[hid[y]];
+      if (place(x) != place(y)) return place(x) < place(y);
       const bool nx = std::isnan(sle[x]), ny = std::isnan(sle[y]);
       if (nx != ny) return ny;
       return !nx && sle[x] < sle[y];
@@ -414,83 +499,52 @@ void PromRangePlan::compute(NodeResult& r) {
     std::vector<double> bucket_le(S);
     for (uint32_t i = 0; i < S; ++i) {
       bucket_le[i] = sle[bucket_series[i]];
-      hist_off[rank[hid[bucket_series[i]]] + 1]++;
+      hist_off[place(bucket_series[i]) + 1]++;
     }
     for (uint32_t h = 0; h < H; ++h) hist_off[h + 1] += hist_off[h];
     r.val.assign((size_t)H * (size_t)T, 0.0);
     r.valid.assign((size_t)H * Tw, 0u);
     if (H > 0 && T > 0) {
       if (fn_id_ < 0) throw PlanError(ErrorKind::Plan, "HistogramFold over an instant selector is not supported by this node");
-      const int rc = b2p_range_histogram_fold(ctx_, &p, ts_.data(), val_.data(), nullptr, offsets_.data(), ts_.size(), S,
-                                              args_.quantile, hist_off.data(), bucket_series.data(), bucket_le.data(), H,
-                                              r.val.data(), r.valid.data());
-      if (rc == B2P_E_INVALID || rc == B2P_E_TOO_LARGE) throw PlanError(ErrorKind::Plan, b2p_last_error());
-      if (rc == B2P_E_UNSORTED) throw PlanError(ErrorKind::Internal, b2p_last_error());
-      if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
-      for (int64_t k = 0; k < T; ++k) eval_ts[(size_t)k] = p.start + k * p.interval;
+      check(b2p_range_histogram_fold(ctx_, &p, ts_.data(), val_.data(), nullptr, offsets_.data(), ts_.size(), S,
+                                     args_.quantile, hist_off.data(), bucket_series.data(), bucket_le.data(), H,
+                                     r.val.data(), r.valid.data()));
     }
-    // rows of histogram hist_order[h] (tag-sorted)
-    for (size_t t = 0; t < args_.tag_columns.size(); ++t)
-      if (t != le_idx) r.tag_names.push_back(args_.tag_columns[t]);
-    r.tags.resize(r.tag_names.size());
-    for (uint32_t h = 0; h < H; ++h) {
-      const std::vector<std::string>& key = hist_keys[hist_order[h]];
-      for (size_t t = 0; t < key.size(); ++t) r.tags[t].push_back(key[t]);
-    }
+    r.labels = std::move(hist.labels);
     r.rows = H;
   } else if (agg_id_ < 0) {
     // rows of Filter(prom_fn IS NOT NULL): {time_index (eval ts), prom_fn(...), tags...}, series-major order
-    r.tag_names = args_.tag_columns;
-    r.id_keyed = key_is_id_;
-    if (key_is_id_) r.ids = tags_.tsid;
-    else r.tags = tags_.utf8;
+    r.labels = series_;
     r.val = std::move(dense);
     r.valid = std::move(valid);
     r.rows = S;
   } else {
-    // prom_aggr_expr_to_plan: group keys = by-labels + eval ts; output sorted by (labels asc, ts asc)
-    std::vector<size_t> by_idx;
-    for (const auto& bname : args_.by_columns)
-      by_idx.push_back((size_t)(std::find(args_.tag_columns.begin(), args_.tag_columns.end(), bname) -
-                                args_.tag_columns.begin()));
-    std::map<std::vector<std::string>, uint32_t> groups;  // ordered => label-sorted output
-    std::vector<uint32_t> gid(S);
-    for (uint32_t s = 0; s < S; ++s) {
-      std::vector<std::string> key;
-      for (size_t bi : by_idx) key.push_back(key_is_id_ ? std::to_string(tags_.tsid[s]) : tags_.utf8[bi][s]);
-      auto it = groups.find(key);
-      if (it == groups.end()) it = groups.emplace(std::move(key), (uint32_t)groups.size()).first;
-      gid[s] = it->second;
-    }
-    const uint32_t G = (uint32_t)groups.size();
+    // prom_aggr_expr_to_plan: group keys = by-labels + eval ts; output sorted by (labels asc, ts asc).  Over an id key
+    // the by-label is the id's decimal string, so those rows sort as strings ("10" before "9").
+    Groups groups = group_rows(series_, series_.columns(args_.by_columns), S);
+    const uint32_t G = (uint32_t)groups.rank.size();
     std::vector<double> gval((size_t)G * (size_t)T);
     std::vector<uint32_t> gcnt((size_t)G * (size_t)T);
-    if (G > 0 && T > 0) {
-      const int rc = b2p_group_aggregate(ctx_, agg_id_, dense.data(), valid.data(), gid.data(), S, G, (uint64_t)T,
-                                         gval.data(), gcnt.data());
-      if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
-    }
-    // rows in key order (std::map iterates sorted); a group has a row at step k iff its count is non-zero
-    r.tag_names = args_.by_columns;
-    r.tags.resize(r.tag_names.size());
-    r.tags_first = true;
+    if (G > 0 && T > 0)
+      check(b2p_group_aggregate(ctx_, agg_id_, dense.data(), valid.data(), groups.id.data(), S, G, (uint64_t)T,
+                                gval.data(), gcnt.data()),
+            ErrorKind::Execution);
+    // a group has a row at step k iff its count is non-zero
+    r.labels = std::move(groups.labels);
+    r.columns = Columns::TagsTimeValue;
     r.value_name = args_.aggregate + "(" + (fn_id_ >= 0 ? args_.function : args_.field_column) + ")";
     r.val.assign((size_t)G * (size_t)T, 0.0);
     r.valid.assign((size_t)G * Tw, 0u);
-    uint32_t row = 0;
-    for (const auto& kv : groups) {
-      const uint32_t g = kv.second;
-      for (size_t b = 0; b < r.tags.size(); ++b) r.tags[b].push_back(kv.first[b]);
+    for (uint32_t g = 0; g < G; ++g) {
+      const uint32_t row = groups.rank[g];
       for (int64_t k = 0; k < T; ++k) {
         if (gcnt[(size_t)g * (size_t)T + (size_t)k] == 0) continue;
         r.val[(size_t)row * (size_t)T + (size_t)k] = gval[(size_t)g * (size_t)T + (size_t)k];
         r.valid[(size_t)row * Tw + (size_t)(k >> 5)] |= 1u << (k & 31);
       }
-      ++row;
     }
     r.rows = G;
   }
-  r.eval_ts = std::move(eval_ts);
 }
 
 namespace {
@@ -512,18 +566,6 @@ std::string float_literal(double x) {
   return "Float64(" + std::string(buf, res.ptr) + ")";
 }
 
-// the key tuple of row r over the given tag columns (-1: a tag the node lacks, read as NULL), length-prefixed so that
-// no two tuples share an encoding
-void append_key(const NodeResult& n, const std::vector<int>& cols, uint32_t r, std::string& key) {
-  key.clear();
-  for (int c : cols) {
-    const std::string v = c < 0 ? kNullLabel : n.id_keyed ? std::to_string(n.ids[r]) : n.tags[(size_t)c][r];
-    key += std::to_string(v.size());
-    key.push_back(':');
-    key += v;
-  }
-}
-
 // the tags a matching modifier keeps: those listed in `labels` for On, those not listed for Ignoring, all for None
 std::vector<std::string> narrow_tags(const std::vector<std::string>& tags, Matching m, const std::vector<std::string>& labels) {
   std::vector<std::string> out;
@@ -532,16 +574,6 @@ std::vector<std::string> narrow_tags(const std::vector<std::string>& tags, Match
     if (m == Matching::On ? listed : !(m == Matching::Ignoring && listed)) out.push_back(t);
   }
   return out;
-}
-
-// the column of each name among n's tags; -1 where n has no such tag
-std::vector<int> tag_columns(const NodeResult& n, const std::vector<std::string>& names) {
-  std::vector<int> cols;
-  for (const std::string& name : names) {
-    const auto it = std::find(n.tag_names.begin(), n.tag_names.end(), name);
-    cols.push_back(it == n.tag_names.end() ? -1 : (int)(it - n.tag_names.begin()));
-  }
-  return cols;
 }
 
 void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema) {
@@ -553,36 +585,36 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     os->formats.push_back(fmt);
     return ob->cols.back().get();
   };
-  std::vector<OwnedColumn*> c_tags;
-  auto add_tags = [&]() {
-    for (const auto& tn : r.tag_names) {
-      c_tags.push_back(add_col(tn, r.id_keyed ? "L" : "u"));
-      if (!r.id_keyed) c_tags.back()->offsets.push_back(0);
-    }
+  const Labels& L = r.labels;
+  std::vector<OwnedColumn*> c_tags(L.names.size());
+  auto add_tag = [&](size_t t) {
+    c_tags[t] = add_col(L.names[t], L.id_keyed ? "L" : "u");
+    if (!L.id_keyed) c_tags[t]->offsets.push_back(0);
   };
   OwnedColumn* c_ts = nullptr;
   OwnedColumn* c_val = nullptr;
-  if (r.sorted_columns) {  // {time index, then the tags and the value column in name order}
-    c_ts = add_col(r.time_index, "tsm:");
-    std::vector<std::string> names = r.tag_names;
-    names.push_back(r.value_name);
-    std::sort(names.begin(), names.end());
-    std::vector<OwnedColumn*> by_tag(r.tag_names.size());
-    for (const std::string& name : names) {
-      if (name == r.value_name && !c_val) {
-        c_val = add_col(name, "g");
-        continue;
+  switch (r.columns) {
+    case Columns::TimeValueTags:
+      c_ts = add_col(r.time_index, "tsm:");
+      c_val = add_col(r.value_name, "g");
+      for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
+      break;
+    case Columns::TagsTimeValue:
+      for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
+      c_ts = add_col(r.time_index, "tsm:");
+      c_val = add_col(r.value_name, "g");
+      break;
+    case Columns::TimeSorted: {
+      c_ts = add_col(r.time_index, "tsm:");
+      std::vector<std::string> names = L.names;
+      names.push_back(r.value_name);
+      std::sort(names.begin(), names.end());
+      for (const std::string& name : names) {
+        if (name == r.value_name && !c_val) c_val = add_col(name, "g");
+        else add_tag((size_t)L.column(name));
       }
-      const size_t t = (size_t)(std::find(r.tag_names.begin(), r.tag_names.end(), name) - r.tag_names.begin());
-      by_tag[t] = add_col(name, r.id_keyed ? "L" : "u");
-      if (!r.id_keyed) by_tag[t]->offsets.push_back(0);
+      break;
     }
-    c_tags = by_tag;
-  } else {
-    if (r.tags_first) add_tags();
-    c_ts = add_col(r.time_index, "tsm:");
-    c_val = add_col(r.value_name, "g");
-    if (!r.tags_first) add_tags();
   }
   int64_t n_out = 0;
   for (uint32_t row = 0; row < r.rows; ++row)
@@ -591,17 +623,17 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       c_ts->i64.push_back(r.eval_ts[(size_t)k]);
       c_val->f64.push_back(r.val[(size_t)row * (size_t)r.T + (size_t)k]);
       for (size_t t = 0; t < c_tags.size(); ++t) {
-        if (r.id_keyed) {
-          c_tags[t]->i64.push_back((int64_t)r.ids[row]);
+        if (L.id_keyed) {
+          c_tags[t]->i64.push_back((int64_t)L.ids[row]);
         } else {
           OwnedColumn* c = c_tags[t];
-          const std::string& v = r.tags[t][row];
-          if (v == kNullLabel) {  // a real Arrow null
+          const Label& v = L.values[t][row];
+          if (!v) {  // a real Arrow null
             if (c->validity.size() <= (size_t)(n_out >> 3)) c->validity.resize((size_t)(n_out >> 3) + 1, 0xFF);
             c->validity[(size_t)n_out >> 3] &= (uint8_t)~(1u << (n_out & 7));
             ++c->nulls;
           } else {
-            c->chars += v;
+            c->chars += *v;
           }
           c->offsets.push_back((int32_t)c->chars.size());
         }
@@ -744,23 +776,17 @@ void PlanNode::run(NodeResult& r) {
       const bool has_rows = std::any_of(r.valid.begin(), r.valid.end(), [](uint32_t w) { return w != 0; });
       if (s.op >= B2P_IFN_CLAMP && lo > hi && has_rows)
         throw PlanError(ErrorKind::Execution, "min '" + rust_display(lo) + "' > max '" + rust_display(hi) + "'");
-      if (work) {
-        const int rc = b2p_instant_fn(ctx_, s.op, a0, a1, r.val.data(), r.valid.data(), r.rows, (uint64_t)r.T,
-                                      r.val.data(), r.valid.data());
-        if (rc == B2P_E_INVALID) throw PlanError(ErrorKind::Plan, b2p_last_error());
-        if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
-      }
+      if (work)
+        check(b2p_instant_fn(ctx_, s.op, a0, a1, r.val.data(), r.valid.data(), r.rows, (uint64_t)r.T, r.val.data(),
+                             r.valid.data()));
       std::string name = s.fn_name + "(" + r.value_name;
       for (double a : s.args) name += "," + float_literal(a);
       r.value_name = name + ")";
       continue;
     }
-    if (work) {
-      const int rc = b2p_scalar_op(ctx_, s.op, s.return_bool ? 1 : 0, s.scalar_on_left ? 1 : 0, s.scalar, r.val.data(),
-                                   r.valid.data(), r.rows, (uint64_t)r.T, r.val.data(), r.valid.data());
-      if (rc == B2P_E_INVALID) throw PlanError(ErrorKind::Plan, b2p_last_error());
-      if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
-    }
+    if (work)
+      check(b2p_scalar_op(ctx_, s.op, s.return_bool ? 1 : 0, s.scalar_on_left ? 1 : 0, s.scalar, r.val.data(),
+                          r.valid.data(), r.rows, (uint64_t)r.T, r.val.data(), r.valid.data()));
     if (!is_comparison(s.op) || s.return_bool) {  // a projection names its expression; a filter keeps the column
       const std::string lit = float_literal(s.scalar), sym = kOpSymbols[s.op];
       r.value_name = s.scalar_on_left ? lit + " " + sym + " " + r.value_name : r.value_name + " " + sym + " " + lit;
@@ -794,14 +820,14 @@ void BinaryPlan::compute(NodeResult& r) {
   // join keys (planner.rs:696-729, 3436-3468): the rhs context's tag columns, narrowed by on / ignoring; none when a
   // side has no tags (every row pairs with every row); two id-keyed sides without a modifier join on the id
   std::vector<int> lcols, rcols;
-  const bool by_id = L.id_keyed && R.id_keyed && matching_ == Matching::None;
+  const bool by_id = L.labels.id_keyed && R.labels.id_keyed && matching_ == Matching::None;
   if (by_id) {
     lcols.push_back(0);
     rcols.push_back(0);
-  } else if (!L.tag_names.empty() && !R.tag_names.empty()) {
-    const std::vector<std::string> names = narrow_tags(R.tag_names, matching_, labels_);
-    lcols = tag_columns(L, names);
-    rcols = tag_columns(R, names);
+  } else if (!L.labels.names.empty() && !R.labels.names.empty()) {
+    const std::vector<std::string> names = narrow_tags(R.labels.names, matching_, labels_);
+    lcols = L.labels.columns(names);
+    rcols = R.labels.columns(names);
     for (size_t i = 0; i < names.size(); ++i)
       if (lcols[i] < 0) throw PlanError(ErrorKind::Plan, "No field named " + names[i]);
   }
@@ -810,12 +836,12 @@ void BinaryPlan::compute(NodeResult& r) {
   std::string key;
   rhs_by_key.reserve(R.rows);
   for (uint32_t q = 0; q < R.rows; ++q) {
-    append_key(R, rcols, q, key);
+    R.labels.key(q, rcols, key);
     rhs_by_key[key].push_back(q);
   }
   std::vector<uint32_t> lrow, rrow;
   for (uint32_t q = 0; q < L.rows; ++q) {
-    append_key(L, lcols, q, key);
+    L.labels.key(q, lcols, key);
     const auto it = rhs_by_key.find(key);
     if (it == rhs_by_key.end()) continue;
     for (uint32_t m : it->second) {
@@ -832,37 +858,21 @@ void BinaryPlan::compute(NodeResult& r) {
   r.eval_ts = L.eval_ts;
   r.val.assign((size_t)n_pairs * (size_t)r.T, 0.0);
   r.valid.assign((size_t)n_pairs * r.Tw, 0u);
-  if (n_pairs > 0 && r.T > 0) {
-    const int rc = b2p_binary_op(ctx_, op_, return_bool_ ? 1 : 0, L.val.data(), L.valid.data(), lrow.data(), L.rows,
-                                 R.val.data(), R.valid.data(), rrow.data(), R.rows, n_pairs, (uint64_t)r.T,
-                                 r.val.data(), r.valid.data());
-    if (rc == B2P_E_INVALID) throw PlanError(ErrorKind::Plan, b2p_last_error());
-    if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
-  }
+  if (n_pairs > 0 && r.T > 0)
+    check(b2p_binary_op(ctx_, op_, return_bool_ ? 1 : 0, L.val.data(), L.valid.data(), lrow.data(), L.rows, R.val.data(),
+                        R.valid.data(), rrow.data(), R.rows, n_pairs, (uint64_t)r.T, r.val.data(), r.valid.data()));
   // output labels: a filter passes the lhs rows through; a projection emits the tag columns of `label_side`
   const bool filter = is_comparison(op_) && !return_bool_;
   const bool from_lhs = filter || labels_from_lhs_;
   const NodeResult& side = from_lhs ? L : R;
   const std::vector<uint32_t>& srow = from_lhs ? lrow : rrow;
   r.time_index = side.time_index;
-  r.tag_names = side.tag_names;
-  r.id_keyed = side.id_keyed;
-  if (side.id_keyed) {
-    r.ids.resize(n_pairs);
-    for (uint64_t p = 0; p < n_pairs; ++p) r.ids[p] = side.ids[srow[p]];
-  } else {
-    r.tags.resize(side.tags.size());
-    for (size_t t = 0; t < side.tags.size(); ++t) {
-      r.tags[t].resize(n_pairs);
-      for (uint64_t p = 0; p < n_pairs; ++p) r.tags[t][p] = side.tags[t][srow[p]];
-    }
-  }
+  r.labels = side.labels.gather(srow);
   if (filter) {
-    r.tags_first = L.tags_first;
-    r.sorted_columns = L.sorted_columns;
+    r.columns = L.columns;
     r.value_name = L.value_name;
   } else {
-    r.tags_first = true;
+    r.columns = Columns::TagsTimeValue;
     r.value_name = L.value_name + " " + kOpSymbols[op_] + " " + R.value_name;
   }
 }
@@ -872,27 +882,17 @@ namespace {
 
 const char* const kSetNames[] = {"and", "or", "unless"};
 
-// dense ids of key tuples, in first-insertion order
-struct KeyIds {
-  std::unordered_map<std::string, uint32_t> ids;
-  uint32_t add(const std::string& k) { return ids.emplace(k, (uint32_t)ids.size()).first->second; }
-  uint32_t find(const std::string& k) const {
-    const auto it = ids.find(k);
-    return it == ids.end() ? B2P_NO_KEY : it->second;
-  }
-};
-
 // left.distinct() of `and` / `unless` (planner.rs:3549-3703): a cell whose labels, step and value bits (DataFusion's
 // group equality on f64) equal those of a cell of an earlier row is dropped.  Only rows that share a label tuple can
 // hold such cells, so only they are compared.
 void drop_duplicate_cells(NodeResult& n) {
   if (n.rows < 2 || n.T == 0) return;
-  std::vector<int> all(n.tag_names.size());
+  std::vector<int> all(n.labels.names.size());
   std::iota(all.begin(), all.end(), 0);
   std::unordered_map<std::string, std::vector<uint32_t>> by_labels;
   std::string key;
   for (uint32_t q = 0; q < n.rows; ++q) {
-    append_key(n, all, q, key);
+    n.labels.key(q, all, key);
     by_labels[key].push_back(q);
   }
   for (const auto& kv : by_labels) {
@@ -913,11 +913,6 @@ void drop_duplicate_cells(NodeResult& n) {
   }
 }
 
-void check_setop(int rc) {
-  if (rc == B2P_E_INVALID) throw PlanError(ErrorKind::Plan, b2p_last_error());
-  if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
-}
-
 }  // namespace
 
 SetOpPlan::SetOpPlan(b2p_ctx* ctx, int op, std::shared_ptr<PlanNode> lhs, std::shared_ptr<PlanNode> rhs,
@@ -936,14 +931,14 @@ void SetOpPlan::compute(NodeResult& r) {
   if (L.T != R.T || (L.rows > 0 && R.rows > 0 && L.eval_ts != R.eval_ts))
     throw PlanError(ErrorKind::Plan, what + "both sides must be evaluated on the same steps");
   // the reference matches set operators on label values (planner.rs:3626-3630), which an id-keyed node does not carry
-  if (L.id_keyed || R.id_keyed) throw PlanError(ErrorKind::Plan, what + "an id-keyed (__tsid) side has no label values to match");
+  if (L.labels.id_keyed || R.labels.id_keyed) throw PlanError(ErrorKind::Plan, what + "an id-keyed (__tsid) side has no label values to match");
   const int64_t T = L.T;
   std::vector<std::string> names;  // match columns
   std::vector<std::string> all;    // `or`: the union of both sides' tags, sorted
   if (op_ != B2P_SET_OR) {
     // each side's tags narrowed by on / ignoring; the two key sets must be equal (CombineTableColumnMismatch)
-    names = narrow_tags(L.tag_names, matching_, labels_);
-    std::vector<std::string> rn = narrow_tags(R.tag_names, matching_, labels_);
+    names = narrow_tags(L.labels.names, matching_, labels_);
+    std::vector<std::string> rn = narrow_tags(R.labels.names, matching_, labels_);
     std::sort(names.begin(), names.end());
     std::sort(rn.begin(), rn.end());
     if (names != rn) {
@@ -955,8 +950,8 @@ void SetOpPlan::compute(NodeResult& r) {
       throw PlanError(ErrorKind::Plan, what + "the key columns of the two sides differ: " + list(names) + " vs " + list(rn));
     }
   } else {
-    all = L.tag_names;
-    all.insert(all.end(), R.tag_names.begin(), R.tag_names.end());
+    all = L.labels.names;
+    all.insert(all.end(), R.labels.names.begin(), R.labels.names.end());
     std::sort(all.begin(), all.end());
     all.erase(std::unique(all.begin(), all.end()), all.end());
     if (matching_ == Matching::On) {
@@ -967,28 +962,28 @@ void SetOpPlan::compute(NodeResult& r) {
       names = narrow_tags(all, matching_, labels_);
     }
   }
-  const std::vector<int> lcols = tag_columns(L, names), rcols = tag_columns(R, names);
+  const std::vector<int> lcols = L.labels.columns(names), rcols = R.labels.columns(names);
   KeyIds keys;
   std::vector<uint32_t> lkey(L.rows), rkey(R.rows);
   std::string key;
   if (op_ == B2P_SET_OR) {
     for (uint32_t q = 0; q < L.rows; ++q) {
-      append_key(L, lcols, q, key);
+      L.labels.key(q, lcols, key);
       lkey[q] = keys.add(key);
     }
   }
   for (uint32_t q = 0; q < R.rows; ++q) {
-    append_key(R, rcols, q, key);
+    R.labels.key(q, rcols, key);
     rkey[q] = keys.add(key);
   }
   if (op_ != B2P_SET_OR) {
     for (uint32_t q = 0; q < L.rows; ++q) {
-      append_key(L, lcols, q, key);
+      L.labels.key(q, lcols, key);
       lkey[q] = keys.find(key);
     }
     drop_duplicate_cells(L);
     if (L.rows > 0 && T > 0)
-      check_setop(b2p_setop(ctx_, op_, L.val.data(), L.valid.data(), lkey.data(), L.rows, nullptr, R.valid.data(),
+      check(b2p_setop(ctx_, op_, L.val.data(), L.valid.data(), lkey.data(), L.rows, nullptr, R.valid.data(),
                             rkey.data(), R.rows, (uint32_t)keys.ids.size(), (uint64_t)T, L.val.data(), L.valid.data()));
     r = std::move(L);  // the lhs rows, columns and values
     return;
@@ -1004,18 +999,18 @@ void SetOpPlan::compute(NodeResult& r) {
   r.val.assign((size_t)n * (size_t)T, 0.0);
   r.valid.assign((size_t)n * r.Tw, 0u);
   if (n > 0 && T > 0)
-    check_setop(b2p_setop(ctx_, op_, L.val.data(), L.valid.data(), lkey.data(), L.rows, R.val.data(), R.valid.data(),
+    check(b2p_setop(ctx_, op_, L.val.data(), L.valid.data(), lkey.data(), L.rows, R.val.data(), R.valid.data(),
                           rkey.data(), R.rows, (uint32_t)keys.ids.size(), (uint64_t)T, r.val.data(), r.valid.data()));
   r.time_index = L.time_index;
   r.value_name = L.value_name;
-  r.tag_names = all;
-  r.sorted_columns = true;
-  const std::vector<int> lall = tag_columns(L, all), rall = tag_columns(R, all);
-  r.tags.resize(all.size());
+  r.columns = Columns::TimeSorted;
+  r.labels.names = all;
+  r.labels.values.resize(all.size());
+  const std::vector<int> lall = L.labels.columns(all), rall = R.labels.columns(all);
   for (size_t t = 0; t < all.size(); ++t) {
-    r.tags[t].reserve((size_t)n);
-    for (uint32_t q = 0; q < L.rows; ++q) r.tags[t].push_back(lall[t] < 0 ? kNullLabel : L.tags[(size_t)lall[t]][q]);
-    for (uint32_t q = 0; q < R.rows; ++q) r.tags[t].push_back(rall[t] < 0 ? kNullLabel : R.tags[(size_t)rall[t]][q]);
+    r.labels.values[t].reserve((size_t)n);
+    for (uint32_t q = 0; q < L.rows; ++q) r.labels.values[t].push_back(L.labels.value(lall[t], q));
+    for (uint32_t q = 0; q < R.rows; ++q) r.labels.values[t].push_back(R.labels.value(rall[t], q));
   }
 }
 
@@ -1032,16 +1027,15 @@ void ScalarPlan::compute(NodeResult& r) {
   // by the id); a tuple with a NULL label gets B2P_NO_KEY (scalar_calculate.rs:543-569 compares NULL as None against
   // the "" it recorded)
   std::vector<uint32_t> key(C.rows, 0u);
-  if (!C.tag_names.empty()) {
+  if (!C.labels.names.empty()) {
     KeyIds ids;
-    std::vector<int> all(C.tag_names.size());
+    std::vector<int> all(C.labels.names.size());
     std::iota(all.begin(), all.end(), 0);
     std::string k;
     for (uint32_t q = 0; q < C.rows; ++q) {
-      bool null_label = false;
-      if (!C.id_keyed)
-        for (const auto& col : C.tags) null_label |= col[q] == kNullLabel;
-      append_key(C, all, q, k);
+      const bool null_label = std::any_of(C.labels.values.begin(), C.labels.values.end(),
+                                          [&](const std::vector<Label>& col) { return !col[q]; });
+      C.labels.key(q, all, k);
       key[q] = null_label ? B2P_NO_KEY : ids.add(k);
     }
   }
@@ -1054,11 +1048,10 @@ void ScalarPlan::compute(NodeResult& r) {
   r.value_name = "scalar(" + C.value_name + ")";
   r.val.assign((size_t)r.T, 0.0);
   r.valid.assign((size_t)r.Tw, 0u);
-  if (r.T > 0) {
-    const int rc = b2p_scalar_calculate(ctx_, C.val.data(), C.valid.data(), key.data(), C.rows, (uint64_t)r.T,
-                                        r.val.data(), r.valid.data());
-    if (rc != B2P_OK) throw PlanError(ErrorKind::Execution, b2p_last_error());
-  }
+  if (r.T > 0)  // two rows of one series with a cell at the same step are bad data here, not a bad plan
+    check(b2p_scalar_calculate(ctx_, C.val.data(), C.valid.data(), key.data(), C.rows, (uint64_t)r.T, r.val.data(),
+                               r.valid.data()),
+          ErrorKind::Execution);
 }
 
 }  // namespace b2p
@@ -1083,6 +1076,47 @@ int not_a_range_node() {
   g_err = "this call needs a range / instant node (b2p_plan_range_create)";
   return B2P_E_INVALID;
 }
+
+// The body of a b2p_plan_*_create: a handle on the node make() returns, or NULL with the error for b2p_plan_last_error()
+template <class Make>
+b2p_plan* create(Make make) {
+  try {
+    return new b2p_plan{make()};
+  } catch (const b2p::PlanError& e) {
+    plan_fail(e);
+  } catch (const std::exception& e) {
+    g_err = e.what();
+  }
+  return nullptr;
+}
+
+// The body of an entry point that works on a node: B2P_OK, or the code of the error fn() throws
+template <class Fn>
+int guarded(Fn fn) {
+  try {
+    fn();
+    return B2P_OK;
+  } catch (const b2p::PlanError& e) {
+    return plan_fail(e);
+  } catch (const std::exception& e) {
+    g_err = e.what();
+    return B2P_E_NOMEM;
+  }
+}
+
+// "on" / "ignoring"; NULL or "" is no modifier
+b2p::Matching parse_matching(const char* m) {
+  if (!m || !m[0]) return b2p::Matching::None;
+  if (std::strcmp(m, "on") == 0) return b2p::Matching::On;
+  if (std::strcmp(m, "ignoring") == 0) return b2p::Matching::Ignoring;
+  throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("unknown matching ") + m);
+}
+
+std::vector<std::string> strings(const char* const* v, int32_t n) {
+  std::vector<std::string> out;
+  for (int32_t i = 0; i < n; ++i) out.emplace_back(v[i]);
+  return out;
+}
 }  // namespace
 
 extern "C" {
@@ -1092,7 +1126,7 @@ const char* b2p_plan_last_error(void) { return g_err.c_str(); }
 b2p_plan* b2p_plan_range_create(b2p_ctx* ctx, const char* function, const b2p_range_params* p, const char* time_index,
                                 const char* field_column, const char* const* tag_columns, int32_t n_tags,
                                 const char* aggregate, const char* const* by_columns, int32_t n_by) {
-  try {
+  return create([&] {
     if (!function || !p || !time_index || !field_column) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
     b2p::PromRangePlanArgs a;
     a.function = function;
@@ -1106,75 +1140,42 @@ b2p_plan* b2p_plan_range_create(b2p_ctx* ctx, const char* function, const b2p_ra
     a.param1 = p->param1;
     a.time_index = time_index;
     a.field_column = field_column;
-    for (int32_t i = 0; i < n_tags; ++i) a.tag_columns.emplace_back(tag_columns[i]);
+    a.tag_columns = strings(tag_columns, n_tags);
     if (aggregate && aggregate[0]) a.aggregate = aggregate;
-    for (int32_t i = 0; i < n_by; ++i) a.by_columns.emplace_back(by_columns[i]);
-    auto* h = new b2p_plan();
-    h->node = std::make_shared<b2p::PromRangePlan>(ctx, std::move(a));
-    return h;
-  } catch (const b2p::PlanError& e) {
-    plan_fail(e);
-  } catch (const std::exception& e) {
-    g_err = e.what();
-  }
-  return nullptr;
+    a.by_columns = strings(by_columns, n_by);
+    return std::make_shared<b2p::PromRangePlan>(ctx, std::move(a));
+  });
 }
 
 b2p_plan* b2p_plan_binary_create(b2p_ctx* ctx, int32_t op, int32_t return_bool, b2p_plan* lhs, b2p_plan* rhs,
                                  const char* matching, const char* const* labels, int32_t n_labels,
                                  const char* label_side) {
-  try {
+  return create([&] {
     if (!lhs || !rhs || !label_side || (n_labels > 0 && !labels))
       throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
-    b2p::BinaryPlan::Matching m = b2p::BinaryPlan::Matching::None;
-    if (matching && std::strcmp(matching, "on") == 0) m = b2p::BinaryPlan::Matching::On;
-    else if (matching && std::strcmp(matching, "ignoring") == 0) m = b2p::BinaryPlan::Matching::Ignoring;
-    else if (matching && matching[0]) throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("unknown matching ") + matching);
+    const b2p::Matching m = parse_matching(matching);
     const bool from_lhs = std::strcmp(label_side, "lhs") == 0;
     if (!from_lhs && std::strcmp(label_side, "rhs") != 0)
       throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("label_side must be \"lhs\" or \"rhs\", got ") + label_side);
-    std::vector<std::string> ls;
-    for (int32_t i = 0; i < n_labels; ++i) ls.emplace_back(labels[i]);
-    auto* h = new b2p_plan();
-    try {
-      h->node = std::make_shared<b2p::BinaryPlan>(ctx, op, return_bool != 0, lhs->node, rhs->node, m, std::move(ls), from_lhs);
-    } catch (...) {
-      delete h;
-      throw;
-    }
-    return h;
-  } catch (const b2p::PlanError& e) {
-    plan_fail(e);
-  } catch (const std::exception& e) {
-    g_err = e.what();
-  }
-  return nullptr;
+    return std::make_shared<b2p::BinaryPlan>(ctx, op, return_bool != 0, lhs->node, rhs->node, m,
+                                             strings(labels, n_labels), from_lhs);
+  });
 }
 
 b2p_plan* b2p_plan_setop_create(b2p_ctx* ctx, int32_t op, b2p_plan* lhs, b2p_plan* rhs, const char* matching,
                                 const char* const* labels, int32_t n_labels) {
-  try {
+  return create([&] {
     if (!lhs || !rhs || (n_labels > 0 && !labels)) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
-    b2p::Matching m = b2p::Matching::None;
-    if (matching && std::strcmp(matching, "on") == 0) m = b2p::Matching::On;
-    else if (matching && std::strcmp(matching, "ignoring") == 0) m = b2p::Matching::Ignoring;
-    else if (matching && matching[0]) throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("unknown matching ") + matching);
-    std::vector<std::string> ls;
-    for (int32_t i = 0; i < n_labels; ++i) ls.emplace_back(labels[i]);
-    auto* h = new b2p_plan();
-    try {
-      h->node = std::make_shared<b2p::SetOpPlan>(ctx, op, lhs->node, rhs->node, m, std::move(ls));
-    } catch (...) {
-      delete h;
-      throw;
-    }
-    return h;
-  } catch (const b2p::PlanError& e) {
-    plan_fail(e);
-  } catch (const std::exception& e) {
-    g_err = e.what();
-  }
-  return nullptr;
+    const b2p::Matching m = parse_matching(matching);
+    return std::make_shared<b2p::SetOpPlan>(ctx, op, lhs->node, rhs->node, m, strings(labels, n_labels));
+  });
+}
+
+b2p_plan* b2p_plan_scalar_create(b2p_ctx* ctx, b2p_plan* child) {
+  return create([&] {
+    if (!child) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    return std::make_shared<b2p::ScalarPlan>(ctx, child->node);
+  });
 }
 
 int b2p_plan_set_instant(b2p_plan* plan, int64_t lookback_delta) {
@@ -1186,78 +1187,28 @@ int b2p_plan_set_instant(b2p_plan* plan, int64_t lookback_delta) {
 int b2p_plan_set_histogram_quantile(b2p_plan* plan, const char* le_column, double quantile) {
   if (!plan || !le_column) return B2P_E_INVALID;
   if (!plan->range()) return not_a_range_node();
-  try {
-    plan->range()->set_histogram(le_column, quantile);
-    return B2P_OK;
-  } catch (const b2p::PlanError& e) {
-    return plan_fail(e);
-  }
+  return guarded([&] { plan->range()->set_histogram(le_column, quantile); });
 }
 
 int b2p_plan_set_scalar_op(b2p_plan* plan, int32_t op, double scalar, int32_t scalar_on_left, int32_t return_bool) {
   if (!plan) return B2P_E_INVALID;
-  try {
-    plan->node->add_scalar_op(op, scalar, scalar_on_left != 0, return_bool != 0);
-    return B2P_OK;
-  } catch (const b2p::PlanError& e) {
-    return plan_fail(e);
-  }
+  return guarded([&] { plan->node->add_scalar_op(op, scalar, scalar_on_left != 0, return_bool != 0); });
 }
 
 int b2p_plan_set_function(b2p_plan* plan, const char* name, const double* args, int32_t n_args) {
   if (!plan || !name || n_args < 0 || (n_args > 0 && !args)) return B2P_E_INVALID;
-  try {
-    plan->node->add_function(name, std::vector<double>(args, args + n_args));
-    return B2P_OK;
-  } catch (const b2p::PlanError& e) {
-    return plan_fail(e);
-  }
-}
-
-b2p_plan* b2p_plan_scalar_create(b2p_ctx* ctx, b2p_plan* child) {
-  try {
-    if (!child) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
-    auto* h = new b2p_plan();
-    try {
-      h->node = std::make_shared<b2p::ScalarPlan>(ctx, child->node);
-    } catch (...) {
-      delete h;
-      throw;
-    }
-    return h;
-  } catch (const b2p::PlanError& e) {
-    plan_fail(e);
-  } catch (const std::exception& e) {
-    g_err = e.what();
-  }
-  return nullptr;
+  return guarded([&] { plan->node->add_function(name, std::vector<double>(args, args + n_args)); });
 }
 
 int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema) {
   if (!plan) return B2P_E_INVALID;
   if (!plan->range()) return not_a_range_node();
-  try {
-    plan->range()->push(std::make_unique<b2p::RecordBatch>(batch, schema));
-    return B2P_OK;
-  } catch (const b2p::PlanError& e) {
-    return plan_fail(e);
-  } catch (const std::exception& e) {
-    g_err = e.what();
-    return B2P_E_NOMEM;
-  }
+  return guarded([&] { plan->range()->push(std::make_unique<b2p::RecordBatch>(batch, schema)); });
 }
 
 int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema) {
   if (!plan) return B2P_E_INVALID;
-  try {
-    plan->node->execute(out, out_schema);
-    return B2P_OK;
-  } catch (const b2p::PlanError& e) {
-    return plan_fail(e);
-  } catch (const std::exception& e) {
-    g_err = e.what();
-    return B2P_E_NOMEM;
-  }
+  return guarded([&] { plan->node->execute(out, out_schema); });
 }
 
 int64_t b2p_plan_num_series(b2p_plan* plan) { return plan && plan->range() ? plan->range()->num_series() : -1; }

@@ -16,6 +16,7 @@
 #include <cstdint>
 #include <cstring>
 #include <memory>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -77,6 +78,35 @@ struct PromRangePlanArgs {
   double quantile = 0.0;
 };
 
+// A label value: a Utf8 string, or NULL (std::nullopt).  NULL equals NULL and differs from every string, as the
+// reference's joins compare keys (NullEquality::NullEqualsNull).
+using Label = std::optional<std::string>;
+
+// The label tuples of a node's rows: the tag names and, per row, either one UInt64 id (the single tag column is an id
+// such as __tsid) or one Label per tag.
+struct Labels {
+  std::vector<std::string> names;
+  bool id_keyed = false;
+  std::vector<uint64_t> ids;               // [row] when id_keyed
+  std::vector<std::vector<Label>> values;  // [tag][row] when not id_keyed (empty when it is)
+
+  int column(const std::string& name) const;  // -1 when absent
+  std::vector<int> columns(const std::vector<std::string>& names) const;
+  // row r's value in column c: NULL when c < 0 (a tag the node lacks); an id reads as its decimal string
+  Label value(int c, uint32_t r) const;
+  // sets `key` to the key of row r over `cols`, read as value() reads them: two keys are equal iff the tuples are
+  void key(uint32_t r, const std::vector<int>& cols, std::string& key) const;
+  Labels gather(const std::vector<uint32_t>& rows) const;  // the given rows, in that order
+  static bool less(const Label& a, const Label& b);         // the order of label values in sorted output
+};
+
+// The column order of an exported batch
+enum class Columns {
+  TimeValueTags,  // {time index, value, tags..}: range and instant nodes, and the filters over them
+  TagsTimeValue,  // {tags.., time index, value}: the by-label aggregate, and arithmetic between two vectors
+  TimeSorted,     // {time index, then the tags and the value column in name order}: `or`
+};
+
 // What a node computed, before it becomes Arrow: a dense [rows x T] grid with validity, the eval timestamps and one label
 // tuple per row.  Exported, row r emits one Arrow row per valid step k (rows in order, steps ascending).
 struct NodeResult {
@@ -87,12 +117,8 @@ struct NodeResult {
   std::vector<double> val;       // [rows x T]; empty when rows == 0 or T == 0
   std::vector<uint32_t> valid;   // [rows x Tw]
   std::string time_index, value_name;
-  std::vector<std::string> tag_names;
-  std::vector<std::vector<std::string>> tags;  // [tag][row] label values (NULL labels as "\0null")
-  bool id_keyed = false;                       // the one tag column is a UInt64 id (values in `ids`, not `tags`)
-  std::vector<uint64_t> ids;                   // [row] when id_keyed
-  bool tags_first = false;                     // columns {tags.., time index, value} instead of {time index, value, tags..}
-  bool sorted_columns = false;                 // columns {time index, then tags and value sorted by name} (`or`)
+  Labels labels;
+  Columns columns = Columns::TimeValueTags;
   bool valid_at(uint32_t r, int64_t k) const { return (valid[(size_t)r * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u; }
 };
 
@@ -130,7 +156,6 @@ class PlanNode {
 class PromRangePlan : public PlanNode {
  public:
   PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args);
-  const char* name() const { return "GpuPromRangeExec"; }
   // input stream, in order; batches of one partition (sorted by tags, ts)
   void push(std::unique_ptr<RecordBatch> batch);
   int64_t num_series() const { return num_series_; }  // the reference's `num_series` metric (range_manipulate.rs:610-619)
@@ -148,21 +173,16 @@ class PromRangePlan : public PlanNode {
   void compute(NodeResult& r) override;
 
  private:
-  struct TagStore {
-    std::vector<std::vector<std::string>> utf8;  // [tag][series] label values of each series' first row
-    std::vector<uint64_t> tsid;                 // when the key is a UInt64 id
-  };
   PromRangePlanArgs args_;
   int fn_id_;
   int agg_id_;
   std::vector<int64_t> ts_;
   std::vector<double> val_;
   std::vector<uint64_t> offsets_;  // first row of every series (SeriesDivide's output), end marker added by execute()
-  TagStore tags_;
-  bool key_is_id_ = false;
+  Labels series_;                  // [series] the labels of each series' first row
   int64_t num_series_ = 0;
   // last row's key, to continue a series across batch boundaries (series_divide.rs:636-645)
-  std::vector<std::string> last_key_;
+  std::vector<Label> last_key_;
   uint64_t last_id_ = 0;
   bool have_last_ = false;
 };
@@ -175,10 +195,8 @@ enum class Matching { None, On, Ignoring };
 // series on the host (hash of the key tuples, O(rows + pairs)); the per-step work is b2p_binary_op.
 class BinaryPlan : public PlanNode {
  public:
-  using Matching = b2p::Matching;
   BinaryPlan(b2p_ctx* ctx, int op, bool return_bool, std::shared_ptr<PlanNode> lhs, std::shared_ptr<PlanNode> rhs,
              Matching matching, std::vector<std::string> labels, bool labels_from_lhs);
-  const char* name() const { return "GpuPromBinaryExec"; }
 
  protected:
   void compute(NodeResult& r) override;
@@ -199,7 +217,6 @@ class SetOpPlan : public PlanNode {
  public:
   SetOpPlan(b2p_ctx* ctx, int op, std::shared_ptr<PlanNode> lhs, std::shared_ptr<PlanNode> rhs, Matching matching,
             std::vector<std::string> labels);
-  const char* name() const { return "GpuPromSetOpExec"; }
 
  protected:
   void compute(NodeResult& r) override;
@@ -217,7 +234,6 @@ class SetOpPlan : public PlanNode {
 class ScalarPlan : public PlanNode {
  public:
   ScalarPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child);
-  const char* name() const { return "GpuPromScalarExec"; }
 
  protected:
   void compute(NodeResult& r) override;
