@@ -5,7 +5,9 @@
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 
+#include <algorithm>
 #include <cfloat>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -26,6 +28,7 @@
 #include "b2p_binary.cuh"
 #include "b2p_instant.cuh"
 #include "b2p_setop.cuh"
+#include "b2p_topk.cuh"
 #include "b2p_kernel_t.cuh"
 #include "b2p_kernel_lean.cuh"
 #include "b2p_kernels.cuh"
@@ -157,6 +160,7 @@ struct b2p_group_index {
   uint32_t* gid = nullptr;       // [n_series] device copy
   uint32_t* goff = nullptr;      // [n_groups + 1]
   uint32_t* members = nullptr;   // [n_series] series ids ordered by (group, series id)
+  std::vector<uint32_t> goff_host;  // host copy of goff (topk's chunk table)
 };
 
 struct b2p_ctx {
@@ -242,6 +246,8 @@ struct b2p_ctx {
   DevBuf s_goff[2], s_members[2], s_mask;
   // scalar(): the reduction's verdict (struct ScalarState), read by the write pass on the device
   DevBuf sc_state;
+  // topk / bottomk: chunk and merge tables, candidate lists, selection state (b2p_topk.cuh; bound in topk_run)
+  DevBuf t_table, t_cand, t_state;
   // resident CTAs per SM of each persistent kernel instantiation (persistent_grid)
   std::unordered_map<const void*, int> blocks_per_sm;
 };
@@ -703,6 +709,7 @@ void b2p_destroy(b2p_ctx* c) {
   }
   c->p_status.release();
   for (DevBuf* b : {&c->s_goff[0], &c->s_goff[1], &c->s_members[0], &c->s_members[1], &c->s_mask}) b->release();
+  for (DevBuf* b : {&c->t_table, &c->t_cand, &c->t_state}) b->release();
   if (c->s_h2d) cudaStreamDestroy(c->s_h2d);
   if (c->s_d2h) cudaStreamDestroy(c->s_d2h);
   if (c->d_ring) cudaFree(c->d_ring);
@@ -1160,6 +1167,7 @@ int b2p_group_index_create_dev(b2p_ctx* c, const uint32_t* gid, uint32_t n_serie
     if (e != cudaSuccess) rc = fail(B2P_E_CUDA, "group index read-back: %s", cudaGetErrorString(e));
     for (uint32_t i = 0; !rc && i < n_groups; ++i)
       if (h[i + 1] - h[i] > ix->max_members) ix->max_members = h[i + 1] - h[i];
+    if (!rc) ix->goff_host = std::move(h);
   }
   if (rc) {
     b2p_group_index_destroy(c, ix);
@@ -1728,6 +1736,156 @@ int b2p_setop_dev(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs
   stage_begin(c, 3);
   rc = setop_run(c, op, lhs, lhs_valid, lhs_key, n_lhs_rows, rhs, rhs_valid, rhs_key, n_rhs_rows, n_keys, T, out,
                  out_valid);
+  stage_end(c, 3);
+  return rc;
+}
+
+/* ---- topk / bottomk ------------------------------------------------------------------------------------------ */
+}  // extern "C"
+
+namespace {
+// k -> the number of ranks kept: row_number <= k in the f64 total order (the reference's Filter compares the UInt64
+// row number coerced to Float64 with the Float64 literal k): floor(k) for finite k >= 1; none for k < 1, -inf and
+// -NaN; every rank for +inf and +NaN
+uint32_t topk_ranks(double k) {
+  if (std::isnan(k)) return std::signbit(k) ? 0u : UINT32_MAX;
+  if (!(k >= 1.0)) return 0u;
+  if (k >= 4294967295.0) return UINT32_MAX;
+  return (uint32_t)std::floor(k);
+}
+
+// grid of a topk kernel with `smem` bytes of dynamic shared memory over `units` warp units, kTopkWarps per CTA
+template <class Kern>
+int topk_grid(b2p_ctx* c, Kern* kern, size_t smem, uint64_t units, unsigned* grid) {
+  int per_sm = 0;
+  CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kTopkWarps * 32, smem));
+  const uint64_t need = (units + kTopkWarps - 1) / kTopkWarps, cap = (uint64_t)c->num_sms * (per_sm > 0 ? per_sm : 1);
+  *grid = (unsigned)(need < cap ? need : cap);
+  return B2P_OK;
+}
+
+// Scratch (context buffers t_table / t_cand / t_state), with C the chunk size below and U 7/8 of the warps of
+// topk_chunk_kernel that stay resident (1 386 at K = 32, 3 234 at K = 10 on a 132-SM H100):
+//   tables:     16 B per chunk and per multi-chunk group;
+//   candidates: (K * 32 * 16 + 128) B per (chunk of a multi-chunk group, tile).  Such chunks hold more than C / 2
+//               members and C >= members * tiles / U, so there are at most 2 * U of these units: 46 MB at K = 32,
+//               34 MB at K = 10 on a 132-SM H100, whatever the input;
+//   state:      640 B per (group with a state, tile), i.e. 20 B per (group, step): multi-chunk groups, and on the
+//               general path every group of more than kk >= 33 members, so at most 0.61 B per input cell.
+int topk_run(b2p_ctx* c, int bottom, uint32_t kk, const double* vals, const uint32_t* valid, const b2p_group_index* ix,
+             const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
+  int rc;
+  const uint32_t R = ix->n_series, G = ix->n_groups;
+  const uint32_t Tw = (uint32_t)((T + 31) / 32), tiles = Tw;
+  const size_t words = (size_t)R * Tw;
+  auto copy = [&](int mode) {
+    topk_copy_kernel<<<capped_grid(c, words, 256, 16), 256, 0, c->stream>>>(valid, ix->gid, G, R, T, Tw, mode, out_valid);
+    c->launches++;
+    CU(cudaGetLastError());
+    return B2P_OK;
+  };
+  if (kk == 0) {
+    CU(cudaMemsetAsync(out_valid, 0, words * 4, c->stream));
+    return B2P_OK;
+  }
+  if (kk >= ix->max_members) return copy(0);  // every valid cell of every group is kept
+  const uint32_t in_groups = G ? ix->goff_host[G] : 0;
+  if (in_groups < R && (rc = copy(1))) return rc;  // rows whose group id is out of range keep nothing
+  const bool general = kk > kTopkMax;
+  const uint32_t K = general ? kTopkMax : kk;
+  // chunk size: at most about one warp unit per resident warp (a second, partial wave would double the time; the 1/8
+  // slack absorbs the rounding of the chunk counts), and at least 256 members
+  const size_t smem = kTopkWarps * topk_warp_bytes(K);
+  int per_sm = 0;
+  CU(cudaFuncSetAttribute(topk_chunk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, topk_chunk_kernel, kTopkWarps * 32, smem));
+  const uint64_t resident = (uint64_t)c->num_sms * (uint64_t)(per_sm > 0 ? per_sm : 1) * kTopkWarps;
+  const uint64_t U = resident - resident / 8;
+  const uint64_t C = std::max<uint64_t>(256, ((uint64_t)in_groups * tiles + U - 1) / U);
+  std::vector<TopkChunk> chunks;
+  std::vector<TopkMerge> merges;
+  uint32_t n_cand = 0, n_state = 0;
+  for (uint32_t g = 0; g < G; ++g) {
+    const uint32_t b = ix->goff_host[g], e = ix->goff_host[g + 1], s = e - b;
+    if (s == 0) continue;
+    if (general && s <= kk) {  // keeps every valid cell
+      chunks.push_back(TopkChunk{b, e, kTopkNone, kTopkNone});
+    } else if (s <= C) {
+      chunks.push_back(TopkChunk{b, e, kTopkNone, general ? n_state++ : kTopkNone});
+    } else {
+      const uint32_t nc = (uint32_t)((s + C - 1) / C);
+      merges.push_back(TopkMerge{n_cand, n_cand + nc, n_state, 0});
+      for (uint32_t i = 0; i < nc; ++i)
+        chunks.push_back(TopkChunk{b + (uint32_t)((uint64_t)s * i / nc), b + (uint32_t)((uint64_t)s * (i + 1) / nc),
+                                   n_cand++, n_state});
+      ++n_state;
+    }
+  }
+  if (chunks.empty()) return B2P_OK;
+  const size_t tb_chunks = chunks.size() * sizeof(TopkChunk), tb_merges = merges.size() * sizeof(TopkMerge);
+  if ((rc = c->t_table.ensure(tb_chunks + tb_merges + 16))) return rc;
+  CU(cudaMemcpyAsync(c->t_table.p, chunks.data(), tb_chunks, cudaMemcpyHostToDevice, c->stream));
+  if (tb_merges)
+    CU(cudaMemcpyAsync(c->t_table.as<char>() + tb_chunks, merges.data(), tb_merges, cudaMemcpyHostToDevice, c->stream));
+  const size_t cand_units = (size_t)n_cand * tiles, state_cells = (size_t)n_state * tiles * 32;
+  const size_t cand_slots = cand_units * K * 32;
+  if ((rc = c->t_cand.ensure(cand_slots * 16 + cand_units * 32 * 4 + 64))) return rc;
+  if ((rc = c->t_state.ensure(state_cells * 20 + 64))) return rc;
+  TopkArgs a{};
+  a.vals = vals; a.valid = valid; a.members = ix->members; a.tie = tie;
+  a.chunks = c->t_table.as<TopkChunk>(); a.n_chunks = (uint32_t)chunks.size();
+  a.merges = reinterpret_cast<const TopkMerge*>(c->t_table.as<char>() + tb_chunks); a.n_merges = (uint32_t)merges.size();
+  a.T = T; a.Tw = Tw; a.tiles = tiles; a.K = K; a.kk = kk; a.bottom = bottom ? 1 : 0; a.general = general ? 1 : 0;
+  a.c_hi = c->t_cand.as<unsigned long long>();
+  a.c_lo = reinterpret_cast<uint32_t*>(a.c_hi + cand_slots);
+  a.c_pos = a.c_lo + cand_slots;
+  a.c_n = a.c_pos + cand_slots;
+  a.s_hi = c->t_state.as<unsigned long long>();
+  a.s_lo = reinterpret_cast<uint32_t*>(a.s_hi + state_cells);
+  a.s_rem = a.s_lo + state_cells;
+  a.s_flags = a.s_rem + state_cells;
+  a.out_valid = out_valid;
+  const uint64_t chunk_units = (uint64_t)chunks.size() * tiles, merge_units = (uint64_t)merges.size() * tiles;
+  unsigned g_chunk = 0, g_merge = 0, g_mark = 0;
+  if ((rc = topk_grid(c, topk_chunk_kernel, smem, chunk_units, &g_chunk))) return rc;
+  if (merge_units && (rc = topk_grid(c, topk_merge_kernel, smem, merge_units, &g_merge))) return rc;
+  const uint32_t rounds = general ? (kk + kTopkMax - 1) / kTopkMax : 1;
+  for (uint32_t r = 0; r < rounds; ++r) {
+    a.round = (int)r;
+    topk_chunk_kernel<<<g_chunk, kTopkWarps * 32, smem, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    if (merge_units) {
+      topk_merge_kernel<<<g_merge, kTopkWarps * 32, smem, c->stream>>>(a);
+      c->launches++;
+      CU(cudaGetLastError());
+    }
+  }
+  if (general) {
+    topk_select_kernel<<<capped_grid(c, chunk_units, 8, 16), 256, 0, c->stream>>>(a);
+  } else if (merge_units) {
+    if ((rc = topk_grid(c, topk_mark_kernel, 0, chunk_units, &g_mark))) return rc;
+    topk_mark_kernel<<<g_mark, kTopkWarps * 32, 0, c->stream>>>(a);
+  } else {
+    return B2P_OK;
+  }
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_topk_dev(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uint32_t* valid,
+                 const b2p_group_index* ix, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_series == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !tie || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  const int rc = topk_run(c, bottom, topk_ranks(k), vals, valid, ix, tie, T, out_valid);
   stage_end(c, 3);
   return rc;
 }
@@ -2389,6 +2547,29 @@ int b2p_scalar_calculate(b2p_ctx* c, const double* vals, const uint32_t* valid, 
       (rc = s.download()))
     return rc;
   return take_row_error(c, kScalarKeyError | kScalarOverlapError);  // (synchronises)
+}
+
+int b2p_topk(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uint32_t* valid, const uint32_t* gid,
+             uint32_t n_rows, uint32_t n_groups, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !gid || !tie || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  int rc;
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
+  uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);  // topk runs in place
+  const uint32_t* d_gid = s.in(gid, (size_t)n_rows * 4);
+  const uint32_t* d_tie = s.in(tie, (size_t)n_rows * 4);
+  s.copy_back(out_valid, d_valid, (size_t)n_rows * Tw * 4);
+  if ((rc = s.rc)) return rc;
+  b2p_group_index* ix = nullptr;
+  if ((rc = b2p_group_index_create_dev(c, d_gid, n_rows, n_groups, &ix))) return rc;
+  rc = b2p_topk_dev(c, bottom, k, d_vals, d_valid, ix, d_tie, T, d_valid);
+  if (!rc) rc = s.finish();
+  b2p_group_index_destroy(c, ix);
+  return rc;
 }
 
 }  // extern "C"

@@ -604,6 +604,11 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       c_ts = add_col(r.time_index, "tsm:");
       c_val = add_col(r.value_name, "g");
       break;
+    case Columns::ValueTagsTime:
+      c_val = add_col(r.value_name, "g");
+      for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
+      c_ts = add_col(r.time_index, "tsm:");
+      break;
     case Columns::TimeSorted: {
       c_ts = add_col(r.time_index, "tsm:");
       std::vector<std::string> names = L.names;
@@ -617,29 +622,33 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     }
   }
   int64_t n_out = 0;
-  for (uint32_t row = 0; row < r.rows; ++row)
-    for (int64_t k = 0; k < r.T; ++k) {
-      if (!r.valid_at(row, k)) continue;
-      c_ts->i64.push_back(r.eval_ts[(size_t)k]);
-      c_val->f64.push_back(r.val[(size_t)row * (size_t)r.T + (size_t)k]);
-      for (size_t t = 0; t < c_tags.size(); ++t) {
-        if (L.id_keyed) {
-          c_tags[t]->i64.push_back((int64_t)L.ids[row]);
+  const bool ordered = !r.cell_order.empty();
+  const uint64_t n_cells = ordered ? r.cell_order.size() : (uint64_t)r.rows * (uint64_t)r.T;
+  for (uint64_t i = 0; i < n_cells; ++i) {
+    const uint64_t cell = ordered ? r.cell_order[i] : i;
+    const uint32_t row = (uint32_t)(cell / (uint64_t)r.T);
+    const int64_t k = (int64_t)(cell % (uint64_t)r.T);
+    if (!r.valid_at(row, k)) continue;
+    c_ts->i64.push_back(r.eval_ts[(size_t)k]);
+    c_val->f64.push_back(r.val[(size_t)row * (size_t)r.T + (size_t)k]);
+    for (size_t t = 0; t < c_tags.size(); ++t) {
+      if (L.id_keyed) {
+        c_tags[t]->i64.push_back((int64_t)L.ids[row]);
+      } else {
+        OwnedColumn* c = c_tags[t];
+        const Label& v = L.values[t][row];
+        if (!v) {  // a real Arrow null
+          if (c->validity.size() <= (size_t)(n_out >> 3)) c->validity.resize((size_t)(n_out >> 3) + 1, 0xFF);
+          c->validity[(size_t)n_out >> 3] &= (uint8_t)~(1u << (n_out & 7));
+          ++c->nulls;
         } else {
-          OwnedColumn* c = c_tags[t];
-          const Label& v = L.values[t][row];
-          if (!v) {  // a real Arrow null
-            if (c->validity.size() <= (size_t)(n_out >> 3)) c->validity.resize((size_t)(n_out >> 3) + 1, 0xFF);
-            c->validity[(size_t)n_out >> 3] &= (uint8_t)~(1u << (n_out & 7));
-            ++c->nulls;
-          } else {
-            c->chars += *v;
-          }
-          c->offsets.push_back((int32_t)c->chars.size());
+          c->chars += *v;
         }
+        c->offsets.push_back((int32_t)c->chars.size());
       }
-      ++n_out;
     }
+    ++n_out;
+  }
 
   // ---- wire up the Arrow C structs ------------------------------------------------------------------
   const size_t nc = ob->cols.size();
@@ -1054,6 +1063,87 @@ void ScalarPlan::compute(NodeResult& r) {
           ErrorKind::Execution);
 }
 
+// ---- TopkPlan ------------------------------------------------------------------------------------------
+namespace {
+int64_t total_key_host(double x) {  // f64::total_cmp's key
+  int64_t b;
+  std::memcpy(&b, &x, sizeof b);
+  return b ^ (int64_t)((uint64_t)(b >> 63) >> 1);
+}
+}  // namespace
+
+TopkPlan::TopkPlan(b2p_ctx* ctx, bool bottom, double k, std::shared_ptr<PlanNode> child, Modifier modifier,
+                   std::vector<std::string> labels)
+    : PlanNode(ctx), bottom_(bottom), k_(k), child_(std::move(child)), modifier_(modifier), labels_(std::move(labels)) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromTopkExec: NULL context");
+  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromTopkExec: NULL child");
+}
+
+void TopkPlan::compute(NodeResult& r) {
+  child_->run(r);
+  const char* what = bottom_ ? "bottomk: " : "topk: ";
+  // the window orders ties by the label values (planner.rs:2980-2996), which an id-keyed node does not carry
+  if (r.labels.id_keyed) throw PlanError(ErrorKind::Plan, std::string(what) + "an id-keyed (__tsid) child has no label values to order by");
+  const Labels& L = r.labels;
+  // group labels (agg_modifier_to_col, planner.rs:1400-1480): `by` the listed labels the child has, in the listed order;
+  // `without` the child's tags that are not listed, in name order; none: the time index alone
+  std::vector<std::string> gnames;
+  if (modifier_ == Modifier::By) {
+    for (const std::string& l : labels_)
+      if (L.column(l) >= 0) gnames.push_back(l);
+  } else if (modifier_ == Modifier::Without) {
+    gnames = narrow_tags(L.names, Matching::Ignoring, labels_);
+    std::sort(gnames.begin(), gnames.end());
+  }
+  const std::vector<int> gcols = L.columns(gnames);
+  KeyIds groups;
+  std::vector<uint32_t> gid(r.rows);
+  std::string key;
+  for (uint32_t q = 0; q < r.rows; ++q) {
+    L.key(q, gcols, key);
+    gid[q] = groups.add(key);
+  }
+  // the tie ordinal: rows ranked by their tuple as the window orders them after the value (every tag in column order,
+  // descending for topk and ascending for bottomk, NULL first); identical tuples in row order.  Larger is better for
+  // topk, smaller for bottomk, as b2p_topk compares (value, tie).
+  auto tuple_before = [&](uint32_t a, uint32_t b) {  // a ranks before b
+    for (const std::vector<Label>& col : L.values) {
+      const Label &x = col[a], &y = col[b];
+      if (x == y) continue;
+      if (!x || !y) return !x;  // NULL first
+      return bottom_ ? *x < *y : *x > *y;
+    }
+    return a < b;
+  };
+  std::vector<uint32_t> order(r.rows);
+  std::iota(order.begin(), order.end(), 0u);
+  std::sort(order.begin(), order.end(), tuple_before);
+  std::vector<uint32_t> tie(r.rows);
+  for (uint32_t p = 0; p < r.rows; ++p) tie[order[p]] = bottom_ ? p : r.rows - 1 - p;
+  if (r.rows > 0 && r.T > 0)
+    check(b2p_topk(ctx_, bottom_ ? 1 : 0, k_, r.val.data(), r.valid.data(), gid.data(), r.rows,
+                   (uint32_t)groups.ids.size(), tie.data(), (uint64_t)r.T, r.valid.data()));
+  // export order (Sort(group labels, ts, rank)): group labels by Labels::less, then the step, then the rank
+  r.cell_order.clear();
+  for (uint32_t q = 0; q < r.rows; ++q)
+    for (int64_t k = 0; k < r.T; ++k)
+      if (r.valid_at(q, k)) r.cell_order.push_back((uint64_t)q * (uint64_t)r.T + (uint64_t)k);
+  const uint64_t T = (uint64_t)r.T;
+  std::sort(r.cell_order.begin(), r.cell_order.end(), [&](uint64_t a, uint64_t b) {
+    const uint32_t ra = (uint32_t)(a / T), rb = (uint32_t)(b / T);
+    for (int c : gcols) {
+      const Label &x = L.values[(size_t)c][ra], &y = L.values[(size_t)c][rb];
+      if (x != y) return Labels::less(x, y);
+    }
+    const uint64_t ka = a % T, kb = b % T;
+    if (ka != kb) return ka < kb;
+    const int64_t va = total_key_host(r.val[a]), vb = total_key_host(r.val[b]);
+    if (va != vb) return bottom_ ? va < vb : va > vb;
+    return bottom_ ? tie[ra] < tie[rb] : tie[ra] > tie[rb];
+  });
+  r.columns = Columns::ValueTagsTime;
+}
+
 }  // namespace b2p
 
 // ---- C entry points -----------------------------------------------------------------------------------
@@ -1175,6 +1265,18 @@ b2p_plan* b2p_plan_scalar_create(b2p_ctx* ctx, b2p_plan* child) {
   return create([&] {
     if (!child) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
     return std::make_shared<b2p::ScalarPlan>(ctx, child->node);
+  });
+}
+
+b2p_plan* b2p_plan_topk_create(b2p_ctx* ctx, int32_t bottom, double k, b2p_plan* child, const char* modifier,
+                               const char* const* labels, int32_t n_labels) {
+  return create([&] {
+    if (!child || (n_labels > 0 && !labels)) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    b2p::TopkPlan::Modifier m = b2p::TopkPlan::Modifier::None;
+    if (modifier && std::strcmp(modifier, "by") == 0) m = b2p::TopkPlan::Modifier::By;
+    else if (modifier && std::strcmp(modifier, "without") == 0) m = b2p::TopkPlan::Modifier::Without;
+    else if (modifier && modifier[0]) throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("unknown modifier ") + modifier);
+    return std::make_shared<b2p::TopkPlan>(ctx, bottom != 0, k, child->node, m, strings(labels, n_labels));
   });
 }
 

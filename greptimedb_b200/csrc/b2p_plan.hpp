@@ -105,6 +105,7 @@ enum class Columns {
   TimeValueTags,  // {time index, value, tags..}: range and instant nodes, and the filters over them
   TagsTimeValue,  // {tags.., time index, value}: the by-label aggregate, and arithmetic between two vectors
   TimeSorted,     // {time index, then the tags and the value column in name order}: `or`
+  ValueTagsTime,  // {value, tags.., time index}: topk / bottomk
 };
 
 // What a node computed, before it becomes Arrow: a dense [rows x T] grid with validity, the eval timestamps and one label
@@ -119,6 +120,9 @@ struct NodeResult {
   std::string time_index, value_name;
   Labels labels;
   Columns columns = Columns::TimeValueTags;
+  // when not empty, the export emits these cells (row * T + step), in this order, instead of rows then steps; a cell
+  // whose bit a later stage cleared is skipped
+  std::vector<uint64_t> cell_order;
   bool valid_at(uint32_t r, int64_t k) const { return (valid[(size_t)r * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u; }
 };
 
@@ -240,6 +244,29 @@ class ScalarPlan : public PlanNode {
 
  private:
   std::shared_ptr<PlanNode> child_;
+};
+
+// topk(k, child) / bottomk(k, child) [by | without (labels)], the reference's Window(row_number()) -> Filter(rank <= k)
+// -> Sort(group labels, ts, rank), planner.rs:454-541, 2963-3016.  The host computes each row's group (over the group
+// labels) and a tie ordinal from the label tuples in the window's order (tags descending for topk, ascending for
+// bottomk, NULL first; identical tuples in row order); the per-step selection is b2p_topk.  The result is the child's
+// rows, labels and values with the kept cells' bits, so nodes above see the child's row order; the export emits
+// {value, tags.., time index} by group labels (Labels::less), ts, rank.
+class TopkPlan : public PlanNode {
+ public:
+  enum class Modifier { None, By, Without };
+  TopkPlan(b2p_ctx* ctx, bool bottom, double k, std::shared_ptr<PlanNode> child, Modifier modifier,
+           std::vector<std::string> labels);
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  bool bottom_;
+  double k_;
+  std::shared_ptr<PlanNode> child_;
+  Modifier modifier_;
+  std::vector<std::string> labels_;
 };
 
 int function_id_from_name(const std::string& prom_name);  // -1 when unknown

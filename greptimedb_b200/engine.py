@@ -52,6 +52,13 @@ def op_id(op) -> int:
 def setop_id(op) -> int:
     return SETOP_IDS[op] if isinstance(op, str) else int(op)
 
+
+def topk_bottom(op) -> int:
+    """"topk" -> 0, "bottomk" -> 1 (the `bottom` argument of b2p_topk)"""
+    if isinstance(op, str):
+        return {"topk": 0, "bottomk": 1}[op]
+    return int(op)
+
 E_UNSORTED = -3
 
 
@@ -303,6 +310,19 @@ class Context:
                                                  _ptr(ov)))
         return out, ov
 
+    def topk(self, op, k, vals, valid, gid, n_groups, tie):
+        """topk / bottomk (op) of k per (group, step): rows grouped by gid (>= n_groups: no group), ranked by (value in the
+        f64 total order, tie) -> the kept cells' validity words [S,Tw] u32 (the values are not touched)."""
+        vals = np.ascontiguousarray(vals, np.float64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        gid = np.ascontiguousarray(gid, np.uint32)
+        tie = np.ascontiguousarray(tie, np.uint32)
+        S, T = vals.shape
+        ov = np.zeros((S, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_topk(self._h, topk_bottom(op), float(k), _ptr(vals), _ptr(valid), _ptr(gid), S,
+                                     int(n_groups), _ptr(tie), T, _ptr(ov)))
+        return ov
+
     # -- device API (torch tensors or raw pointers; asynchronous) ----------------------------------
     def series_offsets_dev(self, sid, n_rows, n_series, offsets):
         self._check(self._L.b2p_series_offsets_dev(self._h, _ptr(sid), n_rows, n_series, _ptr(offsets)))
@@ -416,6 +436,11 @@ class Context:
     def scalar_calculate_dev(self, vals, valid, row_key, n_rows, T, out, out_valid):
         self._check(self._L.b2p_scalar_calculate_dev(self._h, _ptr(vals), _ptr(valid), _ptr(row_key), n_rows, T,
                                                      _ptr(out), _ptr(out_valid)))
+
+    def topk_dev(self, op, k, vals, valid, index, tie, T, out_valid):
+        """topk / bottomk over the rows of a group index (group_index_create_dev); out_valid may be valid."""
+        self._check(self._L.b2p_topk_dev(self._h, topk_bottom(op), float(k), _ptr(vals), _ptr(valid), index, _ptr(tie),
+                                         T, _ptr(out_valid)))
 
     def count_valid_words_dev(self, cnt, n_rows, T, valid_words):
         self._check(self._L.b2p_count_valid_words_dev(self._h, _ptr(cnt), n_rows, T, _ptr(valid_words)))

@@ -6,7 +6,7 @@ start/end/interval/range/field column, the prom_* UDF name, optional by-label ag
 pyarrow RecordBatches exactly like the reference's tests feed a MemoryExec.  `scalar_op` puts `node op number` on
 top of any node, `function` an instant-vector function (abs, clamp_min, prom_round, ...; the two chain in call order),
 `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels), `SetOpPlan` applies `and` / `or` / `unless`
-to two nodes and `ScalarPlan` is scalar(node).
+to two nodes, `ScalarPlan` is scalar(node) and `TopkPlan` is topk / bottomk(k, node) [by | without (labels)].
 """
 from __future__ import annotations
 
@@ -14,7 +14,7 @@ import ctypes as C
 from typing import Optional, Sequence
 
 from . import _lib
-from .engine import B2PError, Context, make_params, op_id, setop_id
+from .engine import B2PError, Context, make_params, op_id, setop_id, topk_bottom
 
 
 class _ArrowArray(C.Structure):
@@ -168,5 +168,26 @@ class ScalarPlan(_PlanNode):
         self._ctx = ctx
         self._children = (child,)
         self._h = self._L.b2p_plan_scalar_create(ctx._h, child._h)
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class TopkPlan(_PlanNode):
+    """topk(k, child) / bottomk(k, child) (op "topk" | "bottomk") per (group labels, step), with `by` or `without`
+    labels (neither: one group per step).  Cells rank by value in the f64 total order, then by the child's tags (NULL
+    first).  Nodes above see the child's rows with the kept cells; execute() emits {value, tags.., time index} by group
+    labels, ts, rank.  The child stays usable and is kept alive by this node."""
+
+    def __init__(self, ctx: Context, op, k: float, child: _PlanNode, by: Optional[Sequence[str]] = None,
+                 without: Optional[Sequence[str]] = None):
+        if by is not None and without is not None:
+            raise ValueError("by and without are exclusive")
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (child,)
+        modifier, labels = (b"by", list(by)) if by is not None else (b"without", list(without)) if without is not None \
+            else (None, [])
+        arr = _cstr_array(labels)
+        self._h = self._L.b2p_plan_topk_create(ctx._h, topk_bottom(op), float(k), child._h, modifier, arr, len(labels))
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())

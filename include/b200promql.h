@@ -38,6 +38,9 @@
  *   b2p_setop[_dev]            set operators: `and` / `unless` = left.distinct() LeftSemi / LeftAnti HashJoinExec on
  *                              (key columns, time index), planner.rs:3549-3703; `or` = UnionDistinctOnExec,
  *                              planner.rs:3707-3906, union_distinct_on.rs:338-577; the key match is done by the caller
+ *   b2p_topk[_dev]             topk / bottomk: Window(row_number() OVER (PARTITION BY group labels, ts ORDER BY value,
+ *                              tags)) -> Filter(row_number <= k), planner.rs:454-541, 2963-3016; the caller groups the
+ *                              rows and ranks the label tuples
  *
  * Data layout (HBM, struct-of-arrays, all row-sorted by (series id, timestamp) exactly like
  * the reference's required_input_ordering, series_divide.rs:410-440):
@@ -325,6 +328,18 @@ B2P_API int b2p_instant_fn_dev(b2p_ctx* ctx, int32_t fn /* enum b2p_ifn */, doub
 B2P_API int b2p_scalar_calculate_dev(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const uint32_t* row_key,
                                      uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
 
+/* topk(k, v) / bottomk(k, v) per (group, step) over a dense grid whose rows are grouped by `index` (a row whose group id
+ * is >= n_groups belongs to no group and keeps nothing).  A cell's rank key is (value in the f64 total order, tie[row]),
+ * compared descending for topk (bottom == 0) and ascending for bottomk; tie [rows] must be distinct per row (the caller
+ * derives it from the label tuples in the direction of the op, b2p_plan.cpp), so the order is strict and the result
+ * deterministic.  The ranks kept follow the reference's Filter(row_number <= k) on Float64: floor(k) for finite k >= 1,
+ * none for k < 1, -inf and -NaN, all for +inf and +NaN.  Per (group, step) exactly the min(kept ranks, valid cells) best
+ * cells keep their bit.  Only out_valid [rows x Tw] is written (bits at or past T are 0); it may be valid (in place).
+ * vals is never written: topk is a filter, and every consumer reads a cell only where its bit is set.  Scratch comes
+ * from the context and is bounded (b2p_api.cu, topk_run).  B2P_E_INVALID: a NULL argument. */
+B2P_API int b2p_topk_dev(b2p_ctx* ctx, int32_t bottom, double k, const double* vals, const uint32_t* valid,
+                         const b2p_group_index* index, const uint32_t* tie, uint64_t T, uint32_t* out_valid);
+
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
  * the id column `sid` (ids sid_base .. sid_base + n_series - 1, non-decreasing), or copied from `offsets_in`
@@ -374,6 +389,12 @@ B2P_API int b2p_scalar_op(b2p_ctx* ctx, int32_t op, int32_t return_bool, int32_t
 B2P_API int b2p_setop(b2p_ctx* ctx, int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key,
                       uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid, const uint32_t* rhs_key,
                       uint32_t n_rhs_rows, uint32_t n_keys, uint64_t T, double* out, uint32_t* out_valid);
+
+/* Host-pointer form of b2p_topk_dev (synchronous): the rows' group ids gid [n_rows] (>= n_groups: no group) instead of
+ * an index, which the call builds itself; errors are returned directly. */
+B2P_API int b2p_topk(b2p_ctx* ctx, int32_t bottom, double k, const double* vals, const uint32_t* valid,
+                     const uint32_t* gid, uint32_t n_rows, uint32_t n_groups, const uint32_t* tie, uint64_t T,
+                     uint32_t* out_valid);
 
 /* Host-pointer forms of b2p_instant_fn_dev / b2p_scalar_calculate_dev (synchronous; device-found errors returned). */
 B2P_API int b2p_instant_fn(b2p_ctx* ctx, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
@@ -470,6 +491,16 @@ B2P_API int b2p_plan_set_function(b2p_plan* plan, const char* name, const double
  * scalar(<value name>)}; usable under scalar operators and functions and as a child of the binary and set nodes (a
  * tagless side pairs with every row).  Ownership as for b2p_plan_binary_create.  NULL on error. */
 B2P_API b2p_plan* b2p_plan_scalar_create(b2p_ctx* ctx, b2p_plan* child);
+/* topk(k, child) / bottomk(k, child) (bottom != 0) with an optional `by` / `without` modifier, GpuPromTopkExec: groups are
+ * (group labels, step), the group labels being the listed ones the child has in the listed order (by), the child's
+ * tags that are not listed in name order (without), or none.  Within a group the cells rank by value in the f64 total
+ * order, then by every tag in column order (descending for topk, ascending for bottomk, NULL first); identical label
+ * tuples rank in row order.  k follows b2p_topk_dev.  Nodes above see the child's rows, labels and values with the
+ * kept cells; the export has columns {value, tags.., time index} and rows by group labels, ts, rank.  The child may be
+ * any node; an id-keyed (__tsid) child is refused.  Ownership as for b2p_plan_binary_create.  NULL on error. */
+B2P_API b2p_plan* b2p_plan_topk_create(b2p_ctx* ctx, int32_t bottom, double k, b2p_plan* child,
+                                       const char* modifier /* NULL | "by" | "without" */, const char* const* labels,
+                                       int32_t n_labels);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

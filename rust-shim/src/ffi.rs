@@ -297,6 +297,11 @@ extern "C" {
         ctx: *mut b2p_ctx, vals: *const f64, valid: *const u32, row_key: *const u32, n_rows: u32, t: u64,
         out: *mut f64, out_valid: *mut u32,
     ) -> c_int;
+    /// topk (bottom = 0) / bottomk per (group, step); writes validity words only (`out_valid` may be `valid`).
+    pub fn b2p_topk_dev(
+        ctx: *mut b2p_ctx, bottom: i32, k: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index,
+        tie: *const u32, t: u64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- host-side helper (no device work): SeriesDivide + cadence scan of one sorted batch ---------------------------
     pub fn b2p_host_scan_series(
@@ -353,6 +358,10 @@ extern "C" {
         ctx: *mut b2p_ctx, vals: *const f64, valid: *const u32, row_key: *const u32, n_rows: u32, t: u64,
         out: *mut f64, out_valid: *mut u32,
     ) -> c_int;
+    pub fn b2p_topk(
+        ctx: *mut b2p_ctx, bottom: i32, k: f64, vals: *const f64, valid: *const u32, gid: *const u32, n_rows: u32,
+        n_groups: u32, tie: *const u32, t: u64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- plan-level API over the Arrow C Data Interface -----------------------------------------------------------------
     pub fn b2p_plan_range_create(
@@ -377,6 +386,11 @@ extern "C" {
     pub fn b2p_plan_set_function(plan: *mut b2p_plan, name: *const c_char, args: *const f64, n_args: i32) -> c_int;
     /// Ownership as for b2p_plan_binary_create.
     pub fn b2p_plan_scalar_create(ctx: *mut b2p_ctx, child: *mut b2p_plan) -> *mut b2p_plan;
+    /// `modifier`: NULL, "by" or "without"; ownership of `child` as for b2p_plan_binary_create.
+    pub fn b2p_plan_topk_create(
+        ctx: *mut b2p_ctx, bottom: i32, k: f64, child: *mut b2p_plan, modifier: *const c_char,
+        labels: *const *const c_char, n_labels: i32,
+    ) -> *mut b2p_plan;
     /// MOVES the batch: on success the release callbacks now belong to the plan.
     pub fn b2p_plan_push_batch(plan: *mut b2p_plan, batch: *mut FFI_ArrowArray, schema: *mut FFI_ArrowSchema) -> c_int;
     pub fn b2p_plan_execute(plan: *mut b2p_plan, out: *mut FFI_ArrowArray, out_schema: *mut FFI_ArrowSchema) -> c_int;

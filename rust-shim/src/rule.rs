@@ -46,6 +46,15 @@
 //!                                           => `match_set_op`: the b2p_plan_setop_create arguments
 //! ```
 //!
+//! topk / bottomk (planner.rs:454-541, 2963-3016):
+//!
+//! ```text
+//!   ProjectionExec(value, tags.., ts) <- SortExec(group labels, ts, rank)
+//!     <- FilterExec(rank <= Float64(k))
+//!     <- BoundedWindowAggExec(row_number() PARTITION BY group labels, ts ORDER BY value, tags)
+//!     <- GpuPromRangeExec                     => `match_topk`: the b2p_plan_topk_create arguments
+//! ```
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
@@ -64,6 +73,8 @@ use datafusion::physical_plan::filter::FilterExec;
 use datafusion::physical_plan::joins::HashJoinExec;
 use datafusion::physical_plan::projection::ProjectionExec;
 use datafusion::physical_plan::repartition::RepartitionExec;
+use datafusion::physical_plan::sorts::sort::SortExec;
+use datafusion::physical_plan::windows::BoundedWindowAggExec;
 use datafusion::physical_plan::ExecutionPlan;
 
 use crate::exec::{GpuPromRangeExec, GpuPromRangeParams, GpuPromStage};
@@ -155,7 +166,7 @@ impl GpuPromRewrite {
             "max" => "max",
             "stddev_pop" => "stddev",
             "var_pop" => "stdvar",
-            _ => return None, // quantile / topk / count_values are not all-reduce-able: stay on the CPU
+            _ => return None, // quantile / count_values are not all-reduce-able: stay on the CPU (topk: match_topk)
         };
         let mut by = Vec::new();
         for (expr, _name) in partial.group_expr().expr() {
@@ -199,6 +210,16 @@ pub struct GpuPromSetOpSpec {
 /// What `b2p_plan_scalar_create` takes for `scalar(child)` over a rewritten node.
 #[derive(Debug)]
 pub struct GpuPromScalarSpec {
+    pub child: GpuPromRangeParams,
+}
+
+/// What `b2p_plan_topk_create` takes for a matched topk / bottomk: the op, the literal k, the group labels (passed as
+/// `by`, in the window's partition order, the time index left out) and the child node.
+#[derive(Debug, Clone)]
+pub struct GpuPromTopkSpec {
+    pub bottom: bool,
+    pub k: f64,
+    pub by: Vec<String>,
     pub child: GpuPromRangeParams,
 }
 
@@ -323,6 +344,38 @@ impl GpuPromRewrite {
         let s = plan.as_any().downcast_ref::<ScalarCalculateExec>()?;
         let child = s.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
         Some(GpuPromScalarSpec { child: child.params().clone() })
+    }
+
+    /// `ProjectionExec <- SortExec <- FilterExec(rank <= k) <- BoundedWindowAggExec(row_number()) <- GpuPromRangeExec`
+    /// (prom_topk_bottomk_to_plan, planner.rs:454-541) -> the arguments of `b2p_plan_topk_create`.  The window's partition
+    /// keys other than the time index become `by(..)`; the first sort key's direction tells topk (descending) from bottomk.
+    pub fn match_topk(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromTopkSpec> {
+        let p = plan.as_any().downcast_ref::<ProjectionExec>()?;
+        let sort = p.input().as_any().downcast_ref::<SortExec>()?;
+        let filter = sort.input().as_any().downcast_ref::<FilterExec>()?;
+        let window = filter.input().as_any().downcast_ref::<BoundedWindowAggExec>()?;
+        let [w] = window.window_expr() else { return None };
+        if w.name() != "row_number()" && !w.name().starts_with("row_number") {
+            return None;
+        }
+        let child = window.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        // rank <= Float64(k) (the UInt64 rank is cast to Float64, planner.rs:475)
+        let pred = filter.predicate().as_any().downcast_ref::<BinaryExpr>()?;
+        if *pred.op() != Operator::LtEq {
+            return None;
+        }
+        let k = float_literal(pred.right())?;
+        let order = w.order_by();
+        let bottom = !order.first()?.options.descending;
+        let ts = &child.params().time_index_column;
+        let mut by = Vec::new();
+        for e in w.partition_by() {
+            let c = e.as_any().downcast_ref::<Column>()?;
+            if c.name() != ts.as_str() {
+                by.push(c.name().to_string());
+            }
+        }
+        Some(GpuPromTopkSpec { bottom, k, by, child: child.params().clone() })
     }
 
     /// `ProjectionExec | FilterExec <- HashJoinExec(Inner, tags.. + ts)` over two `GpuPromRangeExec` -> the arguments of
