@@ -28,6 +28,7 @@
 #include "b2p_binary.cuh"
 #include "b2p_instant.cuh"
 #include "b2p_setop.cuh"
+#include "b2p_quantile.cuh"
 #include "b2p_topk.cuh"
 #include "b2p_kernel_t.cuh"
 #include "b2p_kernel_lean.cuh"
@@ -248,6 +249,8 @@ struct b2p_ctx {
   DevBuf sc_state;
   // topk / bottomk: chunk and merge tables, candidate lists, selection state (b2p_topk.cuh; bound in topk_run)
   DevBuf t_table, t_cand, t_state;
+  // quantile: chunk table, state and histograms of the groups of several chunks (b2p_quantile.cuh; bound in quantile_run)
+  DevBuf q_table, q_state, q_hist;
   // resident CTAs per SM of each persistent kernel instantiation (persistent_grid)
   std::unordered_map<const void*, int> blocks_per_sm;
 };
@@ -709,7 +712,7 @@ void b2p_destroy(b2p_ctx* c) {
   }
   c->p_status.release();
   for (DevBuf* b : {&c->s_goff[0], &c->s_goff[1], &c->s_members[0], &c->s_members[1], &c->s_mask}) b->release();
-  for (DevBuf* b : {&c->t_table, &c->t_cand, &c->t_state}) b->release();
+  for (DevBuf* b : {&c->t_table, &c->t_cand, &c->t_state, &c->q_table, &c->q_state, &c->q_hist}) b->release();
   if (c->s_h2d) cudaStreamDestroy(c->s_h2d);
   if (c->s_d2h) cudaStreamDestroy(c->s_d2h);
   if (c->d_ring) cudaFree(c->d_ring);
@@ -1890,6 +1893,112 @@ int b2p_topk_dev(b2p_ctx* c, int32_t bottom, double k, const double* vals, const
   return rc;
 }
 
+/* ---- quantile ------------------------------------------------------------------------------------------------ */
+}  // extern "C"
+
+namespace {
+template <class Kern>
+int quantile_launch(b2p_ctx* c, Kern* kern, uint64_t units, const QuantArgs& a) {
+  const size_t smem = kQuantWarps * kQuantWarpBytes;
+  unsigned grid = 0;
+  if (int rc = persistent_grid(c, kern, smem, kQuantWarps, units, &grid)) return rc;
+  if (grid == 0) return B2P_OK;
+  kern<<<grid, kQuantWarps * 32, smem, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// Resident limit: groups of at most kQuantResident (64) members are read once and finished in shared memory.  A larger
+// group takes at most kQuantPasses (9) reads of its cells: one per 8-bit digit of the key, one for the extremes; a
+// (group, step) stops as soon as both order statistics are known, a warp as soon as its 32 steps are.  Such a group is
+// cut into chunks of C members, C about its share of one wave of the pass kernel's resident warps (U below) and at
+// most kQuantChunkMax; a group of one chunk is finished by one warp in one launch.
+// Scratch (context buffers q_table / q_state / q_hist) for the groups of several chunks: 16 B per chunk and 4 B per
+// such group; 56 B of state per (group, step); 32 KB of histogram per (group, tile).  Each such group has more than
+// C >= min(members * tiles / U, kQuantChunkMax) members, so there are at most max(U, members * tiles / kQuantChunkMax)
+// of these (group, tile) units: 44 MB of histograms with the 1 386 warps U is on a 132-SM H100 (three 64 KB CTAs of
+// four warps per SM), until the large groups' members times tiles pass 45 M.
+int quantile_run(b2p_ctx* c, double phi, const double* vals, const uint32_t* valid, const b2p_group_index* ix,
+                 uint64_t T, double* out_val, uint32_t* out_cnt) {
+  int rc;
+  const uint32_t G = ix->n_groups, Tw = (uint32_t)((T + 31) / 32);
+  QuantArgs a{};
+  a.vals = vals; a.valid = valid; a.goff = ix->goff; a.members = ix->members; a.n_groups = G;
+  a.T = T; a.Tw = Tw; a.tiles = Tw; a.phi = phi;
+  a.count_only = !(phi >= 0.0 && phi <= 1.0) ? 1 : 0;
+  a.out_val = out_val; a.out_cnt = out_cnt;
+  if ((rc = quantile_launch(c, quantile_resident_kernel, (uint64_t)G * Tw, a))) return rc;
+  if (a.count_only || ix->max_members <= kQuantResident) return B2P_OK;
+  unsigned cap = 0;
+  if ((rc = persistent_grid(c, quantile_pass_kernel, kQuantWarps * kQuantWarpBytes, kQuantWarps, kAllResident, &cap)))
+    return rc;
+  const uint64_t resident = (uint64_t)cap * kQuantWarps, U = resident - resident / 8;
+  uint64_t large = 0;
+  for (uint32_t g = 0; g < G; ++g) {
+    const uint32_t s = ix->goff_host[g + 1] - ix->goff_host[g];
+    if (s > kQuantResident) large += s;
+  }
+  const uint64_t C = std::min<uint64_t>(kQuantChunkMax, std::max<uint64_t>(256, (large * Tw + U - 1) / U));
+  std::vector<QuantChunk> chunks;
+  std::vector<uint32_t> slot_group;
+  for (uint32_t g = 0; g < G; ++g) {
+    const uint32_t b = ix->goff_host[g], e = ix->goff_host[g + 1], s = e - b;
+    if (s <= kQuantResident) continue;
+    if (s <= C) {
+      chunks.push_back(QuantChunk{b, e, g, kQuantNone});
+      continue;
+    }
+    const uint32_t nc = (uint32_t)((s + C - 1) / C), slot = (uint32_t)slot_group.size();
+    slot_group.push_back(g);
+    for (uint32_t i = 0; i < nc; ++i)
+      chunks.push_back(QuantChunk{b + (uint32_t)((uint64_t)s * i / nc), b + (uint32_t)((uint64_t)s * (i + 1) / nc), g, slot});
+  }
+  const size_t tb_chunks = chunks.size() * sizeof(QuantChunk), tb_slots = slot_group.size() * 4;
+  if ((rc = c->q_table.ensure(tb_chunks + tb_slots + 16))) return rc;
+  CU(cudaMemcpyAsync(c->q_table.p, chunks.data(), tb_chunks, cudaMemcpyHostToDevice, c->stream));
+  if (tb_slots)
+    CU(cudaMemcpyAsync(c->q_table.as<char>() + tb_chunks, slot_group.data(), tb_slots, cudaMemcpyHostToDevice, c->stream));
+  a.chunks = c->q_table.as<QuantChunk>(); a.n_chunks = (uint32_t)chunks.size();
+  a.slot_group = reinterpret_cast<const uint32_t*>(c->q_table.as<char>() + tb_chunks);
+  a.n_slots = (uint32_t)slot_group.size();
+  if (a.n_slots) {
+    const size_t state_bytes = (size_t)a.n_slots * T * sizeof(QuantState);
+    const size_t hist_bytes = (size_t)a.n_slots * Tw * 256 * 32 * 4;
+    if ((rc = c->q_state.ensure(state_bytes))) return rc;
+    if ((rc = c->q_hist.ensure(hist_bytes))) return rc;
+    CU(cudaMemsetAsync(c->q_state.p, 0, state_bytes, c->stream));
+    CU(cudaMemsetAsync(c->q_hist.p, 0, hist_bytes, c->stream));
+    a.state = c->q_state.as<QuantState>();
+    a.hist = c->q_hist.as<uint32_t>();
+  }
+  const uint64_t units = (uint64_t)chunks.size() * Tw;
+  for (uint32_t p = 0; p < (a.n_slots ? kQuantPasses : 1u); ++p) {
+    a.pass = (int)p;
+    if ((rc = quantile_launch(c, quantile_pass_kernel, units, a))) return rc;
+    if (!a.n_slots) break;
+    quantile_advance_kernel<<<capped_grid(c, (uint64_t)a.n_slots * T, 256, 8), 256, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+  }
+  return B2P_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_group_quantile_dev(b2p_ctx* c, double phi, const double* vals, const uint32_t* valid, const b2p_group_index* ix,
+                           uint64_t T, double* out_val, uint32_t* out_cnt) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_groups == 0 || T == 0) return B2P_OK;
+  if ((ix->n_series && (!vals || !valid)) || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  const int rc = quantile_run(c, phi, vals, valid, ix, T, out_val, out_cnt);
+  stage_end(c, 3);
+  return rc;
+}
+
 int b2p_synth_fill_dev(b2p_ctx* c, uint64_t series_begin, uint64_t n_series, uint32_t n_samples, int64_t t0,
                        int64_t scrape_ms, uint32_t jitter_ms, int32_t with_resets, uint64_t seed, int64_t* ts,
                        double* val, uint32_t* sid) {
@@ -2567,6 +2676,29 @@ int b2p_topk(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uin
   b2p_group_index* ix = nullptr;
   if ((rc = b2p_group_index_create_dev(c, d_gid, n_rows, n_groups, &ix))) return rc;
   rc = b2p_topk_dev(c, bottom, k, d_vals, d_valid, ix, d_tie, T, d_valid);
+  if (!rc) rc = s.finish();
+  b2p_group_index_destroy(c, ix);
+  return rc;
+}
+
+int b2p_group_quantile(b2p_ctx* c, double phi, const double* vals, const uint32_t* valid, const uint32_t* gid,
+                       uint32_t n_rows, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_groups == 0 || T == 0) return B2P_OK;
+  if ((n_rows && (!vals || !valid || !gid)) || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  int rc;
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
+  const uint32_t* d_gid = s.in(gid, (size_t)n_rows * 4);
+  double* d_out = s.out(out_val, (size_t)n_groups * T * 8);
+  uint32_t* d_cnt = s.out(out_cnt, (size_t)n_groups * T * 4);
+  if ((rc = s.rc)) return rc;
+  b2p_group_index* ix = nullptr;
+  if ((rc = b2p_group_index_create_dev(c, d_gid, n_rows, n_groups, &ix))) return rc;
+  rc = b2p_group_quantile_dev(c, phi, d_vals, d_valid, ix, T, d_out, d_cnt);
   if (!rc) rc = s.finish();
   b2p_group_index_destroy(c, ix);
   return rc;

@@ -285,6 +285,42 @@ Groups group_rows(const Labels& in, const std::vector<int>& cols, uint32_t rows)
   return g;
 }
 
+// Aggregators beyond enum b2p_agg that the aggregate node offers
+constexpr int kAggGroup = B2P_AGG_STDVAR + 1, kAggQuantile = B2P_AGG_STDVAR + 2;
+
+// The by-label aggregate of r's [rows x T] grid (the leaf's aggregate stage and AggregatePlan): r's rows grouped by
+// their tuple over `cols` (of r.labels), folded on the device in row order, become one row per group in label order,
+// a group having a cell at step k iff one of its rows has.  op: enum b2p_agg, kAggGroup (1.0 wherever count is
+// non-zero) or kAggQuantile (param = φ).  Sets the rows, labels, grid and column layout; keeps T and the time index.
+void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& cols, NodeResult& r) {
+  Groups groups = group_rows(r.labels, cols, r.rows);
+  const uint32_t G = (uint32_t)groups.rank.size(), Tw = r.Tw;
+  const size_t T = (size_t)r.T;
+  std::vector<double> gval((size_t)G * T);
+  std::vector<uint32_t> gcnt((size_t)G * T);
+  if (G > 0 && T > 0)
+    check(op == kAggQuantile ? b2p_group_quantile(ctx, param, r.val.data(), r.valid.data(), groups.id.data(), r.rows, G,
+                                                  (uint64_t)T, gval.data(), gcnt.data())
+                             : b2p_group_aggregate(ctx, op == kAggGroup ? B2P_AGG_COUNT : op, r.val.data(),
+                                                   r.valid.data(), groups.id.data(), r.rows, G, (uint64_t)T,
+                                                   gval.data(), gcnt.data()),
+          ErrorKind::Execution);
+  r.labels = std::move(groups.labels);
+  r.columns = Columns::TagsTimeValue;
+  r.cell_order.clear();
+  r.val.assign((size_t)G * T, 0.0);
+  r.valid.assign((size_t)G * Tw, 0u);
+  for (uint32_t g = 0; g < G; ++g) {
+    const uint32_t row = groups.rank[g];
+    for (size_t k = 0; k < T; ++k) {
+      if (gcnt[g * T + k] == 0) continue;
+      r.val[row * T + k] = op == kAggGroup ? 1.0 : gval[g * T + k];
+      r.valid[(size_t)row * Tw + (k >> 5)] |= 1u << (k & 31);
+    }
+  }
+  r.rows = G;
+}
+
 }  // namespace
 
 // ---- PromRangePlan -------------------------------------------------------------------------------------
@@ -512,38 +548,18 @@ void PromRangePlan::compute(NodeResult& r) {
     }
     r.labels = std::move(hist.labels);
     r.rows = H;
-  } else if (agg_id_ < 0) {
+  } else {
     // rows of Filter(prom_fn IS NOT NULL): {time_index (eval ts), prom_fn(...), tags...}, series-major order
     r.labels = series_;
     r.val = std::move(dense);
     r.valid = std::move(valid);
     r.rows = S;
-  } else {
-    // prom_aggr_expr_to_plan: group keys = by-labels + eval ts; output sorted by (labels asc, ts asc).  Over an id key
-    // the by-label is the id's decimal string, so those rows sort as strings ("10" before "9").
-    Groups groups = group_rows(series_, series_.columns(args_.by_columns), S);
-    const uint32_t G = (uint32_t)groups.rank.size();
-    std::vector<double> gval((size_t)G * (size_t)T);
-    std::vector<uint32_t> gcnt((size_t)G * (size_t)T);
-    if (G > 0 && T > 0)
-      check(b2p_group_aggregate(ctx_, agg_id_, dense.data(), valid.data(), groups.id.data(), S, G, (uint64_t)T,
-                                gval.data(), gcnt.data()),
-            ErrorKind::Execution);
-    // a group has a row at step k iff its count is non-zero
-    r.labels = std::move(groups.labels);
-    r.columns = Columns::TagsTimeValue;
-    r.value_name = args_.aggregate + "(" + (fn_id_ >= 0 ? args_.function : args_.field_column) + ")";
-    r.val.assign((size_t)G * (size_t)T, 0.0);
-    r.valid.assign((size_t)G * Tw, 0u);
-    for (uint32_t g = 0; g < G; ++g) {
-      const uint32_t row = groups.rank[g];
-      for (int64_t k = 0; k < T; ++k) {
-        if (gcnt[(size_t)g * (size_t)T + (size_t)k] == 0) continue;
-        r.val[(size_t)row * (size_t)T + (size_t)k] = gval[(size_t)g * (size_t)T + (size_t)k];
-        r.valid[(size_t)row * Tw + (size_t)(k >> 5)] |= 1u << (k & 31);
-      }
+    if (agg_id_ >= 0) {
+      // prom_aggr_expr_to_plan: group keys = by-labels + eval ts; output sorted by (labels asc, ts asc).  Over an id key
+      // the by-label is the id's decimal string, so those rows sort as strings ("10" before "9").
+      aggregate_rows(ctx_, agg_id_, 0.0, series_.columns(args_.by_columns), r);
+      r.value_name = args_.aggregate + "(" + (fn_id_ >= 0 ? args_.function : args_.field_column) + ")";
     }
-    r.rows = G;
   }
 }
 
@@ -1070,6 +1086,20 @@ int64_t total_key_host(double x) {  // f64::total_cmp's key
   std::memcpy(&b, &x, sizeof b);
   return b ^ (int64_t)((uint64_t)(b >> 63) >> 1);
 }
+
+// The columns of L an aggregation groups by (agg_modifier_to_col, planner.rs:1400-1480): `by` the listed labels L has,
+// in the listed order; `without` L's tags that are not listed, in name order; none: no column (the time index alone)
+std::vector<int> group_columns(const Labels& L, Modifier modifier, const std::vector<std::string>& labels) {
+  std::vector<std::string> names;
+  if (modifier == Modifier::By) {
+    for (const std::string& l : labels)
+      if (L.column(l) >= 0) names.push_back(l);
+  } else if (modifier == Modifier::Without) {
+    names = narrow_tags(L.names, Matching::Ignoring, labels);
+    std::sort(names.begin(), names.end());
+  }
+  return L.columns(names);
+}
 }  // namespace
 
 TopkPlan::TopkPlan(b2p_ctx* ctx, bool bottom, double k, std::shared_ptr<PlanNode> child, Modifier modifier,
@@ -1085,17 +1115,7 @@ void TopkPlan::compute(NodeResult& r) {
   // the window orders ties by the label values (planner.rs:2980-2996), which an id-keyed node does not carry
   if (r.labels.id_keyed) throw PlanError(ErrorKind::Plan, std::string(what) + "an id-keyed (__tsid) child has no label values to order by");
   const Labels& L = r.labels;
-  // group labels (agg_modifier_to_col, planner.rs:1400-1480): `by` the listed labels the child has, in the listed order;
-  // `without` the child's tags that are not listed, in name order; none: the time index alone
-  std::vector<std::string> gnames;
-  if (modifier_ == Modifier::By) {
-    for (const std::string& l : labels_)
-      if (L.column(l) >= 0) gnames.push_back(l);
-  } else if (modifier_ == Modifier::Without) {
-    gnames = narrow_tags(L.names, Matching::Ignoring, labels_);
-    std::sort(gnames.begin(), gnames.end());
-  }
-  const std::vector<int> gcols = L.columns(gnames);
+  const std::vector<int> gcols = group_columns(L, modifier_, labels_);
   KeyIds groups;
   std::vector<uint32_t> gid(r.rows);
   std::string key;
@@ -1142,6 +1162,34 @@ void TopkPlan::compute(NodeResult& r) {
     return bottom_ ? tie[ra] < tie[rb] : tie[ra] > tie[rb];
   });
   r.columns = Columns::ValueTagsTime;
+}
+
+// ---- AggregatePlan -------------------------------------------------------------------------------------
+AggregatePlan::AggregatePlan(b2p_ctx* ctx, const std::string& op, double param, std::shared_ptr<PlanNode> child,
+                             Modifier modifier, std::vector<std::string> labels)
+    : PlanNode(ctx), param_(param), child_(std::move(child)), modifier_(modifier), labels_(std::move(labels)) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromAggregateExec: NULL context");
+  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromAggregateExec: NULL child");
+  // create_aggregate_exprs, planner.rs:2808-2897: the DataFusion function each aggregator becomes
+  if (op == "count_values") throw PlanError(ErrorKind::Plan, "GpuPromAggregateExec: count_values is not supported by this node");
+  if (op == "topk" || op == "bottomk")
+    throw PlanError(ErrorKind::Plan, "GpuPromAggregateExec: " + op + " is a filter, not an aggregate: use b2p_plan_topk_create");
+  op_ = op == "group" ? kAggGroup : op == "quantile" ? kAggQuantile : aggregate_id_from_name(op);
+  if (op_ < 0) throw PlanError(ErrorKind::Plan, "GpuPromAggregateExec: unknown aggregator " + op);
+  df_name_ = op == "stddev" ? "stddev_pop" : op == "stdvar" ? "var_pop" : op;
+}
+
+void AggregatePlan::compute(NodeResult& r) {
+  child_->run(r);
+  // the reference would re-attach the tag columns of an id-keyed input (ensure_tag_columns_available); this layer has
+  // only the id, so it can group such a node as a whole and nothing else
+  if (r.labels.id_keyed && modifier_ != Modifier::None)
+    throw PlanError(ErrorKind::Plan, "GpuPromAggregateExec: an id-keyed (__tsid) child can only be aggregated without by / without");
+  const std::string child_value = r.value_name;
+  aggregate_rows(ctx_, op_, param_, group_columns(r.labels, modifier_, labels_), r);
+  r.value_name = op_ == kAggGroup      ? "max(" + float_literal(1.0) + ")"
+                 : op_ == kAggQuantile ? "quantile(" + float_literal(param_) + "," + child_value + ")"
+                                       : df_name_ + "(" + child_value + ")";
 }
 
 }  // namespace b2p
@@ -1200,6 +1248,14 @@ b2p::Matching parse_matching(const char* m) {
   if (std::strcmp(m, "on") == 0) return b2p::Matching::On;
   if (std::strcmp(m, "ignoring") == 0) return b2p::Matching::Ignoring;
   throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("unknown matching ") + m);
+}
+
+// "by" / "without"; NULL or "" is no modifier
+b2p::Modifier parse_modifier(const char* m) {
+  if (!m || !m[0]) return b2p::Modifier::None;
+  if (std::strcmp(m, "by") == 0) return b2p::Modifier::By;
+  if (std::strcmp(m, "without") == 0) return b2p::Modifier::Without;
+  throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("unknown modifier ") + m);
 }
 
 std::vector<std::string> strings(const char* const* v, int32_t n) {
@@ -1272,11 +1328,17 @@ b2p_plan* b2p_plan_topk_create(b2p_ctx* ctx, int32_t bottom, double k, b2p_plan*
                                const char* const* labels, int32_t n_labels) {
   return create([&] {
     if (!child || (n_labels > 0 && !labels)) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
-    b2p::TopkPlan::Modifier m = b2p::TopkPlan::Modifier::None;
-    if (modifier && std::strcmp(modifier, "by") == 0) m = b2p::TopkPlan::Modifier::By;
-    else if (modifier && std::strcmp(modifier, "without") == 0) m = b2p::TopkPlan::Modifier::Without;
-    else if (modifier && modifier[0]) throw b2p::PlanError(b2p::ErrorKind::Plan, std::string("unknown modifier ") + modifier);
-    return std::make_shared<b2p::TopkPlan>(ctx, bottom != 0, k, child->node, m, strings(labels, n_labels));
+    return std::make_shared<b2p::TopkPlan>(ctx, bottom != 0, k, child->node, parse_modifier(modifier),
+                                           strings(labels, n_labels));
+  });
+}
+
+b2p_plan* b2p_plan_aggregate_create(b2p_ctx* ctx, const char* op, double param, b2p_plan* child, const char* modifier,
+                                    const char* const* labels, int32_t n_labels) {
+  return create([&] {
+    if (!op || !child || (n_labels > 0 && !labels)) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    return std::make_shared<b2p::AggregatePlan>(ctx, op, param, child->node, parse_modifier(modifier),
+                                                strings(labels, n_labels));
   });
 }
 

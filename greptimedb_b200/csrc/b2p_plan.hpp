@@ -194,6 +194,9 @@ class PromRangePlan : public PlanNode {
 // Label matching modifier of a binary or set operator
 enum class Matching { None, On, Ignoring };
 
+// Label modifier of an aggregation (topk / bottomk, the aggregate node)
+enum class Modifier { None, By, Without };
+
 // Vector-vector binary operator over two nodes (b2p_plan_binary_create): the reference's ProjectionExec / FilterExec
 // over an inner HashJoinExec on (key columns, time index), planner.rs:556-777, 3436-3546.  The join is a match between
 // series on the host (hash of the key tuples, O(rows + pairs)); the per-step work is b2p_binary_op.
@@ -254,7 +257,6 @@ class ScalarPlan : public PlanNode {
 // {value, tags.., time index} by group labels (Labels::less), ts, rank.
 class TopkPlan : public PlanNode {
  public:
-  enum class Modifier { None, By, Without };
   TopkPlan(b2p_ctx* ctx, bool bottom, double k, std::shared_ptr<PlanNode> child, Modifier modifier,
            std::vector<std::string> labels);
 
@@ -264,6 +266,28 @@ class TopkPlan : public PlanNode {
  private:
   bool bottom_;
   double k_;
+  std::shared_ptr<PlanNode> child_;
+  Modifier modifier_;
+  std::vector<std::string> labels_;
+};
+
+// <op>(child) [by | without (labels)] over any node, GpuPromAggregateExec: the reference's Aggregate(group labels + ts,
+// op(value)).sort(group labels, ts) (prom_aggr_expr_to_plan, planner.rs:334-452; create_aggregate_exprs 2808-2897).
+// Group labels as for TopkPlan; the fold is b2p_group_aggregate (sum avg count min max stddev stdvar, and group as count
+// with the value 1.0) or b2p_group_quantile, members in the child's row order.  Rows: the groups in Labels::less order;
+// columns {group labels.., time index, <df name>(<child value name>)}.
+class AggregatePlan : public PlanNode {
+ public:
+  AggregatePlan(b2p_ctx* ctx, const std::string& op, double param, std::shared_ptr<PlanNode> child, Modifier modifier,
+                std::vector<std::string> labels);
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  int op_;
+  std::string df_name_;  // DataFusion's name of the aggregate function ("var_pop", "quantile", ...)
+  double param_;
   std::shared_ptr<PlanNode> child_;
   Modifier modifier_;
   std::vector<std::string> labels_;

@@ -323,6 +323,19 @@ class Context:
                                      int(n_groups), _ptr(tie), T, _ptr(ov)))
         return ov
 
+    def group_quantile(self, phi, vals, valid, gid, n_groups):
+        """quantile(phi) per (group, step): rows grouped by gid (>= n_groups: no group) -> (out [G,T] f64, cnt [G,T]
+        u32); cnt 0 is "no row" (value 0.0)."""
+        vals = np.ascontiguousarray(vals, np.float64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        gid = np.ascontiguousarray(gid, np.uint32)
+        S, T = vals.shape
+        out = np.zeros((n_groups, T), np.float64)
+        cnt = np.zeros((n_groups, T), np.uint32)
+        self._check(self._L.b2p_group_quantile(self._h, float(phi), _ptr(vals), _ptr(valid), _ptr(gid), S,
+                                               int(n_groups), T, _ptr(out), _ptr(cnt)))
+        return out, cnt
+
     # -- device API (torch tensors or raw pointers; asynchronous) ----------------------------------
     def series_offsets_dev(self, sid, n_rows, n_series, offsets):
         self._check(self._L.b2p_series_offsets_dev(self._h, _ptr(sid), n_rows, n_series, _ptr(offsets)))
@@ -441,6 +454,11 @@ class Context:
         """topk / bottomk over the rows of a group index (group_index_create_dev); out_valid may be valid."""
         self._check(self._L.b2p_topk_dev(self._h, topk_bottom(op), float(k), _ptr(vals), _ptr(valid), index, _ptr(tie),
                                          T, _ptr(out_valid)))
+
+    def group_quantile_dev(self, phi, vals, valid, index, T, out_val, out_cnt):
+        """quantile(phi) over the rows of a group index (group_index_create_dev) into out_val / out_cnt [G,T]."""
+        self._check(self._L.b2p_group_quantile_dev(self._h, float(phi), _ptr(vals), _ptr(valid), index, T,
+                                                   _ptr(out_val), _ptr(out_cnt)))
 
     def count_valid_words_dev(self, cnt, n_rows, T, valid_words):
         self._check(self._L.b2p_count_valid_words_dev(self._h, _ptr(cnt), n_rows, T, _ptr(valid_words)))

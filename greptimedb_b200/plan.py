@@ -191,3 +191,25 @@ class TopkPlan(_PlanNode):
         self._h = self._L.b2p_plan_topk_create(ctx._h, topk_bottom(op), float(k), child._h, modifier, arr, len(labels))
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class AggregatePlan(_PlanNode):
+    """op(child) per (group labels, step), with `by` or `without` labels (neither: one group per step): op is one of sum
+    avg count min max stddev stdvar group quantile (param = phi).  Members fold in the child's row order; execute()
+    emits {group labels.., time index, value} with rows in group label order.  The child may be any node; it stays
+    usable and is kept alive by this node."""
+
+    def __init__(self, ctx: Context, op: str, child: _PlanNode, param: Optional[float] = None,
+                 by: Optional[Sequence[str]] = None, without: Optional[Sequence[str]] = None):
+        if by is not None and without is not None:
+            raise ValueError("by and without are exclusive")
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (child,)
+        modifier, labels = (b"by", list(by)) if by is not None else (b"without", list(without)) if without is not None \
+            else (None, [])
+        arr = _cstr_array(labels)
+        phi = 0.0 if param is None else float(param)  # (-0.0 stays -0.0: it names the column Float64(-0))
+        self._h = self._L.b2p_plan_aggregate_create(ctx._h, op.encode(), phi, child._h, modifier, arr, len(labels))
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())

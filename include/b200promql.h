@@ -41,6 +41,8 @@
  *   b2p_topk[_dev]             topk / bottomk: Window(row_number() OVER (PARTITION BY group labels, ts ORDER BY value,
  *                              tags)) -> Filter(row_number <= k), planner.rs:454-541, 2963-3016; the caller groups the
  *                              rows and ranks the label tuples
+ *   b2p_group_quantile[_dev]   quantile by label: Aggregate(quantile(φ, value)), QuantileAccumulator::evaluate,
+ *                              quantile_aggr.rs:110-116, quantile.rs:201-225
  *
  * Data layout (HBM, struct-of-arrays, all row-sorted by (series id, timestamp) exactly like
  * the reference's required_input_ordering, series_divide.rs:410-440):
@@ -340,6 +342,16 @@ B2P_API int b2p_scalar_calculate_dev(b2p_ctx* ctx, const double* vals, const uin
 B2P_API int b2p_topk_dev(b2p_ctx* ctx, int32_t bottom, double k, const double* vals, const uint32_t* valid,
                          const b2p_group_index* index, const uint32_t* tie, uint64_t T, uint32_t* out_valid);
 
+/* quantile(phi, v) by label (K11, QuantileAccumulator::evaluate, src/promql/src/functions/quantile_aggr.rs:110-116 over
+ * quantile_with_scratch, quantile.rs:201-225): per (group, step) the n valid cells of the index's member rows; phi NaN
+ * gives NaN, phi < 0 -inf, phi > 1 +inf; otherwise, sorted by f64::total_cmp, rank = phi (n - 1), lo = floor(rank),
+ * hi = min(n - 1, lo + 1), w = rank - floor(rank) and the result s[lo] (1 - w) + s[hi] w, evaluated as written (so
+ * quantile(0, {1, +inf}) is NaN).  Output out_val / out_cnt [n_groups x T] as b2p_group_aggregate_dev: out_cnt = n, and
+ * n = 0 (value 0.0) is "no row".  Rows of the index's gid >= n_groups take part in nothing.  Deterministic; scratch
+ * comes from the context and is bounded (b2p_api.cu, quantile_run).  B2P_E_INVALID: a NULL argument. */
+B2P_API int b2p_group_quantile_dev(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid,
+                                   const b2p_group_index* index, uint64_t T, double* out_val, uint32_t* out_cnt);
+
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
  * the id column `sid` (ids sid_base .. sid_base + n_series - 1, non-decreasing), or copied from `offsets_in`
@@ -395,6 +407,11 @@ B2P_API int b2p_setop(b2p_ctx* ctx, int32_t op, const double* lhs, const uint32_
 B2P_API int b2p_topk(b2p_ctx* ctx, int32_t bottom, double k, const double* vals, const uint32_t* valid,
                      const uint32_t* gid, uint32_t n_rows, uint32_t n_groups, const uint32_t* tie, uint64_t T,
                      uint32_t* out_valid);
+
+/* Host-pointer form of b2p_group_quantile_dev (synchronous): the rows' group ids gid [n_rows] (>= n_groups: no group)
+ * instead of an index, which the call builds itself. */
+B2P_API int b2p_group_quantile(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid, const uint32_t* gid,
+                               uint32_t n_rows, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt);
 
 /* Host-pointer forms of b2p_instant_fn_dev / b2p_scalar_calculate_dev (synchronous; device-found errors returned). */
 B2P_API int b2p_instant_fn(b2p_ctx* ctx, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
@@ -501,6 +518,18 @@ B2P_API b2p_plan* b2p_plan_scalar_create(b2p_ctx* ctx, b2p_plan* child);
 B2P_API b2p_plan* b2p_plan_topk_create(b2p_ctx* ctx, int32_t bottom, double k, b2p_plan* child,
                                        const char* modifier /* NULL | "by" | "without" */, const char* const* labels,
                                        int32_t n_labels);
+/* <op>(child) with an optional `by` / `without` modifier, GpuPromAggregateExec (prom_aggr_expr_to_plan,
+ * planner.rs:334-452): groups are (group labels, step), the group labels as for b2p_plan_topk_create; a group has a row
+ * at a step iff one of its members has a cell there, members folding in the child's row order.  op: sum avg count min
+ * max stddev stdvar (as b2p_group_aggregate), group (1.0 wherever count does), quantile (param = phi, as
+ * b2p_group_quantile_dev).  count_values, topk, bottomk and any other name are refused.  An id-keyed (__tsid) child is
+ * only accepted without a modifier (one group per step).  The result has columns {group labels.., time index, value}
+ * with rows in group label order; the value is named <df name>(<child's value name>), e.g. var_pop(val),
+ * quantile(Float64(0.5),val), max(Float64(1)) for group.  The child may be any node.  Ownership as for
+ * b2p_plan_binary_create.  NULL on error (b2p_plan_last_error). */
+B2P_API b2p_plan* b2p_plan_aggregate_create(b2p_ctx* ctx, const char* op, double param, b2p_plan* child,
+                                            const char* modifier /* NULL | "by" | "without" */,
+                                            const char* const* labels, int32_t n_labels);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

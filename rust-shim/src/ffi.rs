@@ -302,6 +302,11 @@ extern "C" {
         ctx: *mut b2p_ctx, bottom: i32, k: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index,
         tie: *const u32, t: u64, out_valid: *mut u32,
     ) -> c_int;
+    /// quantile(phi) per (group, step) into out_val / out_cnt [n_groups x T]; cnt 0 = no row.
+    pub fn b2p_group_quantile_dev(
+        ctx: *mut b2p_ctx, phi: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index, t: u64,
+        out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
 
     // ---- host-side helper (no device work): SeriesDivide + cadence scan of one sorted batch ---------------------------
     pub fn b2p_host_scan_series(
@@ -362,6 +367,10 @@ extern "C" {
         ctx: *mut b2p_ctx, bottom: i32, k: f64, vals: *const f64, valid: *const u32, gid: *const u32, n_rows: u32,
         n_groups: u32, tie: *const u32, t: u64, out_valid: *mut u32,
     ) -> c_int;
+    pub fn b2p_group_quantile(
+        ctx: *mut b2p_ctx, phi: f64, vals: *const f64, valid: *const u32, gid: *const u32, n_rows: u32, n_groups: u32,
+        t: u64, out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
 
     // ---- plan-level API over the Arrow C Data Interface -----------------------------------------------------------------
     pub fn b2p_plan_range_create(
@@ -389,6 +398,12 @@ extern "C" {
     /// `modifier`: NULL, "by" or "without"; ownership of `child` as for b2p_plan_binary_create.
     pub fn b2p_plan_topk_create(
         ctx: *mut b2p_ctx, bottom: i32, k: f64, child: *mut b2p_plan, modifier: *const c_char,
+        labels: *const *const c_char, n_labels: i32,
+    ) -> *mut b2p_plan;
+    /// `op`: sum avg count min max stddev stdvar group quantile (`param` = phi); `modifier`: NULL, "by" or "without";
+    /// ownership of `child` as for b2p_plan_binary_create.
+    pub fn b2p_plan_aggregate_create(
+        ctx: *mut b2p_ctx, op: *const c_char, param: f64, child: *mut b2p_plan, modifier: *const c_char,
         labels: *const *const c_char, n_labels: i32,
     ) -> *mut b2p_plan;
     /// MOVES the batch: on success the release callbacks now belong to the plan.

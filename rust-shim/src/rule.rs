@@ -55,6 +55,15 @@
 //!     <- GpuPromRangeExec                     => `match_topk`: the b2p_plan_topk_create arguments
 //! ```
 //!
+//! The aggregate node over any rewritten node (prom_aggr_expr_to_plan, planner.rs:334-452, create_aggregate_exprs
+//! 2808-2897):
+//!
+//! ```text
+//!   AggregateExec(Final | FinalPartitioned) <- RepartitionExec <- AggregateExec(Partial, group labels + ts)
+//!     <- GpuPromRangeExec                     => `match_aggregate_node`: the b2p_plan_aggregate_create arguments
+//!         (sum avg count min max stddev_pop var_pop, quantile(Float64(φ), col), max(Float64(1)) = group)
+//! ```
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
@@ -223,6 +232,16 @@ pub struct GpuPromTopkSpec {
     pub child: GpuPromRangeParams,
 }
 
+/// What `b2p_plan_aggregate_create` takes for an aggregate over a rewritten node: the op name, its literal parameter
+/// (quantile's φ, else 0), the group labels (passed as `by`, in the group-by order, the time index left out) and the child.
+#[derive(Debug, Clone)]
+pub struct GpuPromAggregateSpec {
+    pub op: &'static str,
+    pub param: f64,
+    pub by: Vec<String>,
+    pub child: GpuPromRangeParams,
+}
+
 /// The instant-vector functions the library evaluates, by ScalarFunctionExpr::name(), with the number of literal
 /// arguments after the value column (planner.rs:2368-2413; prom_round always gets its to_nearest, 0.0 when omitted).
 const INSTANT_FNS: &[(&str, usize)] = &[
@@ -376,6 +395,53 @@ impl GpuPromRewrite {
             }
         }
         Some(GpuPromTopkSpec { bottom, k, by, child: child.params().clone() })
+    }
+
+    /// `AggregateExec(Final) <- RepartitionExec <- AggregateExec(Partial)` over a `GpuPromRangeExec` -> the arguments of
+    /// `b2p_plan_aggregate_create`.  `quantile(Float64(φ), col)` needs a literal φ; `max(Float64(1))` is `group`
+    /// (planner.rs:2836-2838).  count_values, a non-literal φ and group columns that are not tags of the child stay on the
+    /// CPU.
+    pub fn match_aggregate_node(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromAggregateSpec> {
+        let fin = plan.as_any().downcast_ref::<AggregateExec>()?;
+        if !matches!(fin.mode(), AggregateMode::FinalPartitioned | AggregateMode::Final) {
+            return None;
+        }
+        let repart = fin.input().as_any().downcast_ref::<RepartitionExec>()?;
+        let partial = repart.input().as_any().downcast_ref::<AggregateExec>()?;
+        let [a] = partial.aggr_expr() else { return None };
+        if !matches!(partial.mode(), AggregateMode::Partial) {
+            return None;
+        }
+        let child = partial.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let args = a.expressions();
+        let first_literal = args.first().and_then(float_literal);
+        let (op, param) = match a.fun().name() {
+            "sum" => ("sum", 0.0),
+            "avg" => ("avg", 0.0),
+            "count" => ("count", 0.0),
+            "min" => ("min", 0.0),
+            "max" if first_literal == Some(1.0) => ("group", 0.0),
+            "max" => ("max", 0.0),
+            "stddev_pop" => ("stddev", 0.0),
+            "var_pop" => ("stdvar", 0.0),
+            "quantile" => ("quantile", first_literal?),
+            _ => return None,
+        };
+        // every group column other than the time index must be one of the child's tags: count_values (planned as
+        // count with the value column among the group columns, planner.rs:420-424, 2833) and any other grouping the
+        // node cannot express stay on the CPU
+        let params = child.params();
+        let mut by = Vec::new();
+        for (expr, _name) in partial.group_expr().expr() {
+            let c = expr.as_any().downcast_ref::<Column>()?;
+            if c.name() != params.time_index_column {
+                if !params.tag_columns.iter().any(|t| t == c.name()) {
+                    return None;
+                }
+                by.push(c.name().to_string());
+            }
+        }
+        Some(GpuPromAggregateSpec { op, param, by, child: params.clone() })
     }
 
     /// `ProjectionExec | FilterExec <- HashJoinExec(Inner, tags.. + ts)` over two `GpuPromRangeExec` -> the arguments of
