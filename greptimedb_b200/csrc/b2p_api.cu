@@ -22,10 +22,13 @@
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+#include <cub/device/device_segmented_sort.cuh>
 
 #include "../../include/b200promql.h"
 #include "b2p_aggregate.cuh"
 #include "b2p_binary.cuh"
+#include "b2p_count_values.cuh"
 #include "b2p_instant.cuh"
 #include "b2p_setop.cuh"
 #include "b2p_quantile.cuh"
@@ -251,6 +254,9 @@ struct b2p_ctx {
   DevBuf t_table, t_cand, t_state;
   // quantile: chunk table, state and histograms of the groups of several chunks (b2p_quantile.cuh; bound in quantile_run)
   DevBuf q_table, q_state, q_hist;
+  // count_values: key and sorted-key buffers, ranks and starts, segment tables, member groups, CUB's temp (bound in
+  // count_values_run)
+  DevBuf v_keys, v_alt, v_rank, v_seg, v_group, v_tmp;
   // resident CTAs per SM of each persistent kernel instantiation (persistent_grid)
   std::unordered_map<const void*, int> blocks_per_sm;
 };
@@ -713,6 +719,7 @@ void b2p_destroy(b2p_ctx* c) {
   c->p_status.release();
   for (DevBuf* b : {&c->s_goff[0], &c->s_goff[1], &c->s_members[0], &c->s_members[1], &c->s_mask}) b->release();
   for (DevBuf* b : {&c->t_table, &c->t_cand, &c->t_state, &c->q_table, &c->q_state, &c->q_hist}) b->release();
+  for (DevBuf* b : {&c->v_keys, &c->v_alt, &c->v_rank, &c->v_seg, &c->v_group, &c->v_tmp}) b->release();
   if (c->s_h2d) cudaStreamDestroy(c->s_h2d);
   if (c->s_d2h) cudaStreamDestroy(c->s_d2h);
   if (c->d_ring) cudaFree(c->d_ring);
@@ -1999,6 +2006,122 @@ int b2p_group_quantile_dev(b2p_ctx* c, double phi, const double* vals, const uin
   return rc;
 }
 
+/* ---- count_values -------------------------------------------------------------------------------------------- */
+}  // extern "C"
+
+namespace {
+// A run of groups [g0, g1) over steps [k0, k0 + W) (b2p_count_values.cuh)
+struct CvBatch {
+  uint32_t g0, g1, k0, W;
+  uint64_t cells, segments;
+};
+
+// Batches: windows of W steps (every step when the largest group's cells fit kCvBatchCells, else a multiple of 32),
+// each cut into runs of whole groups whose cells (members x W) and segments (groups x W) fit kCvBatchCells; a group
+// too large for that alone is a batch of its own.  Per batch: the segment table, the scatter, CUB's segmented sort, the
+// head flags, CUB's scan over them, the rank and count passes; no host round trip.
+// Scratch (context buffers v_*): 20 B per cell of a batch (8 B key, 8 B sorted key, 4 B rank; the start table reuses
+// the key buffer once the sort has left it), so at most 20 B x kCvBatchCells = 2.7 GB unless one group alone has more
+// than kCvBatchCells / 32 = 4.2 M members (then 20 B x its members x 32); 8 B per (group, step) of a batch; 4 B per
+// in-range row; CUB's temp storage for the sort and the scan.
+int count_values_run(b2p_ctx* c, const double* vals, const uint32_t* valid, const b2p_group_index* ix, uint64_t T,
+                     double* out_val, uint32_t* out_cnt) {
+  int rc;
+  const uint32_t R = ix->n_series, G = ix->n_groups, Tw = (uint32_t)((T + 31) / 32);
+  const uint32_t in_rows = G ? ix->goff_host[G] : 0u;
+  if (in_rows < R) {  // rows whose group id is out of range take part in nothing: count 0
+    CU(cudaMemsetAsync(out_val + (uint64_t)in_rows * T, 0, (uint64_t)(R - in_rows) * T * 8, c->stream));
+    CU(cudaMemsetAsync(out_cnt + (uint64_t)in_rows * T, 0, (uint64_t)(R - in_rows) * T * 4, c->stream));
+  }
+  if (in_rows == 0) return B2P_OK;
+  const uint64_t W = std::min<uint64_t>((T + 31) / 32 * 32, std::max<uint64_t>(32, kCvBatchCells / ix->max_members / 32 * 32));
+  if ((uint64_t)ix->max_members * std::min<uint64_t>(W, T) > (uint64_t)INT32_MAX)
+    return fail(B2P_E_TOO_LARGE, "count_values: a group of %u members is too large", ix->max_members);
+  std::vector<CvBatch> batches;
+  uint64_t max_cells = 0, max_segs = 0;
+  for (uint64_t k0 = 0; k0 < T; k0 += W) {
+    const uint64_t Wb = std::min<uint64_t>(W, T - k0);
+    for (uint32_t g = 0; g < G;) {
+      const uint32_t g0 = g;
+      uint64_t members = 0;
+      for (; g < G; ++g) {
+        const uint64_t s = ix->goff_host[g + 1] - ix->goff_host[g];
+        if (g > g0 && std::max<uint64_t>(members + s, g + 1 - g0) * Wb > kCvBatchCells) break;
+        members += s;
+      }
+      if (members == 0) continue;  // empty groups only: no output row
+      batches.push_back(CvBatch{g0, g, (uint32_t)k0, (uint32_t)Wb, members * Wb, (uint64_t)(g - g0) * Wb});
+      max_cells = std::max(max_cells, members * Wb);
+      max_segs = std::max(max_segs, (uint64_t)(g - g0) * Wb);
+    }
+  }
+  size_t tmp = 16;
+  for (const CvBatch& b : batches) {
+    size_t sort_bytes = 0, scan_bytes = 0;
+    cub::DoubleBuffer<unsigned long long> db(nullptr, nullptr);
+    CU(cub::DeviceSegmentedSort::SortKeys(nullptr, sort_bytes, db, (int)b.cells, (int)b.segments, (const uint32_t*)nullptr,
+                                          (const uint32_t*)nullptr, c->stream));
+    CU(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)b.cells, c->stream));
+    tmp = std::max({tmp, sort_bytes, scan_bytes});
+  }
+  if ((rc = c->v_keys.ensure(max_cells * 8)) || (rc = c->v_alt.ensure(max_cells * 8)) ||
+      (rc = c->v_rank.ensure(max_cells * 4)) || (rc = c->v_seg.ensure((2 * max_segs + 1) * 4)) ||
+      (rc = c->v_group.ensure((size_t)in_rows * 4)) || (rc = c->v_tmp.ensure(tmp)))
+    return rc;
+  count_values_member_group_kernel<<<capped_grid(c, in_rows, 256, 16), 256, 0, c->stream>>>(
+      ix->gid, ix->members, in_rows, c->v_group.as<uint32_t>());
+  c->launches++;
+  CU(cudaGetLastError());
+  CvArgs a{};
+  a.vals = vals; a.valid = valid; a.members = ix->members; a.goff = ix->goff; a.mgroup = c->v_group.as<uint32_t>();
+  a.T = T; a.Tw = Tw;
+  a.seg_off = c->v_seg.as<uint32_t>(); a.seg_n = a.seg_off + max_segs + 1;
+  a.rank = c->v_rank.as<uint32_t>();
+  a.out_val = out_val; a.out_cnt = out_cnt;
+  for (const CvBatch& b : batches) {
+    a.g0 = b.g0; a.g1 = b.g1; a.m0 = ix->goff_host[b.g0]; a.m1 = ix->goff_host[b.g1]; a.k0 = b.k0; a.W = b.W;
+    a.cells = (uint32_t)b.cells;
+    a.keys = c->v_keys.as<unsigned long long>();
+    const unsigned cell_grid = capped_grid(c, b.cells, 256, 8);
+    count_values_segments_kernel<<<capped_grid(c, b.segments, 256, 8), 256, 0, c->stream>>>(a);
+    const uint64_t tiles = (uint64_t)((a.m1 - a.m0 + 31) / 32) * ((b.W + 31) / 32);
+    count_values_scatter_kernel<<<capped_grid(c, tiles, 1, 8), 256, 0, c->stream>>>(a);
+    c->launches += 2;
+    CU(cudaGetLastError());
+    cub::DoubleBuffer<unsigned long long> db(c->v_keys.as<unsigned long long>(), c->v_alt.as<unsigned long long>());
+    size_t bytes = c->v_tmp.cap;
+    CU(cub::DeviceSegmentedSort::SortKeys(c->v_tmp.p, bytes, db, (int)b.cells, (int)b.segments, a.seg_off, a.seg_off + 1,
+                                          c->stream));
+    a.sorted = db.Current();
+    a.start = reinterpret_cast<uint32_t*>(db.Alternate());
+    count_values_head_kernel<<<cell_grid, 256, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    bytes = c->v_tmp.cap;
+    CU(cub::DeviceScan::InclusiveSum(c->v_tmp.p, bytes, a.rank, a.rank, (int)b.cells, c->stream));
+    count_values_rank_kernel<<<cell_grid, 256, 0, c->stream>>>(a);
+    count_values_count_kernel<<<cell_grid, 256, 0, c->stream>>>(a);
+    c->launches += 2;
+    CU(cudaGetLastError());
+  }
+  return B2P_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_count_values_dev(b2p_ctx* c, const double* vals, const uint32_t* valid, const b2p_group_index* ix, uint64_t T,
+                         double* out_val, uint32_t* out_cnt) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_series == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  const int rc = count_values_run(c, vals, valid, ix, T, out_val, out_cnt);
+  stage_end(c, 3);
+  return rc;
+}
+
 int b2p_synth_fill_dev(b2p_ctx* c, uint64_t series_begin, uint64_t n_series, uint32_t n_samples, int64_t t0,
                        int64_t scrape_ms, uint32_t jitter_ms, int32_t with_resets, uint64_t seed, int64_t* ts,
                        double* val, uint32_t* sid) {
@@ -2699,6 +2822,29 @@ int b2p_group_quantile(b2p_ctx* c, double phi, const double* vals, const uint32_
   b2p_group_index* ix = nullptr;
   if ((rc = b2p_group_index_create_dev(c, d_gid, n_rows, n_groups, &ix))) return rc;
   rc = b2p_group_quantile_dev(c, phi, d_vals, d_valid, ix, T, d_out, d_cnt);
+  if (!rc) rc = s.finish();
+  b2p_group_index_destroy(c, ix);
+  return rc;
+}
+
+int b2p_count_values(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* gid, uint32_t n_rows,
+                     uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !gid || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  int rc;
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
+  const uint32_t* d_gid = s.in(gid, (size_t)n_rows * 4);
+  double* d_out = s.out(out_val, (size_t)n_rows * T * 8);
+  uint32_t* d_cnt = s.out(out_cnt, (size_t)n_rows * T * 4);
+  if ((rc = s.rc)) return rc;
+  b2p_group_index* ix = nullptr;
+  if ((rc = b2p_group_index_create_dev(c, d_gid, n_rows, n_groups, &ix))) return rc;
+  rc = b2p_count_values_dev(c, d_vals, d_valid, ix, T, d_out, d_cnt);
   if (!rc) rc = s.finish();
   b2p_group_index_destroy(c, ix);
   return rc;

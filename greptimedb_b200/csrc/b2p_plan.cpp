@@ -609,6 +609,8 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
   };
   OwnedColumn* c_ts = nullptr;
   OwnedColumn* c_val = nullptr;
+  OwnedColumn* c_label = nullptr;  // count_values' counted value
+  const bool int_val = r.columns == Columns::CountTagsTimeLabel && r.value_is_count;
   switch (r.columns) {
     case Columns::TimeValueTags:
       c_ts = add_col(r.time_index, "tsm:");
@@ -624,6 +626,12 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       c_val = add_col(r.value_name, "g");
       for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
       c_ts = add_col(r.time_index, "tsm:");
+      break;
+    case Columns::CountTagsTimeLabel:
+      c_val = add_col(r.value_name, int_val ? "l" : "g");
+      for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
+      c_ts = add_col(r.time_index, "tsm:");
+      c_label = add_col(r.label_name, "g");
       break;
     case Columns::TimeSorted: {
       c_ts = add_col(r.time_index, "tsm:");
@@ -646,7 +654,10 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     const int64_t k = (int64_t)(cell % (uint64_t)r.T);
     if (!r.valid_at(row, k)) continue;
     c_ts->i64.push_back(r.eval_ts[(size_t)k]);
-    c_val->f64.push_back(r.val[(size_t)row * (size_t)r.T + (size_t)k]);
+    const double v = r.val[(size_t)row * (size_t)r.T + (size_t)k];
+    if (int_val) c_val->i64.push_back((int64_t)v);
+    else c_val->f64.push_back(v);
+    if (c_label) c_label->f64.push_back(r.label_val[(size_t)row * (size_t)r.T + (size_t)k]);
     for (size_t t = 0; t < c_tags.size(); ++t) {
       if (L.id_keyed) {
         c_tags[t]->i64.push_back((int64_t)L.ids[row]);
@@ -790,6 +801,7 @@ void PlanNode::add_function(const std::string& name, const std::vector<double>& 
 
 void PlanNode::run(NodeResult& r) {
   compute(r);
+  if (!stages_.empty()) r.value_is_count = false;  // a stage's result is a Float64 projection
   for (const Stage& s : stages_) {
     const bool work = r.rows > 0 && r.T > 0;
     if (s.is_fn) {
@@ -896,6 +908,13 @@ void BinaryPlan::compute(NodeResult& r) {
   if (filter) {
     r.columns = L.columns;
     r.value_name = L.value_name;
+    r.label_name = L.label_name;
+    r.value_is_count = L.value_is_count;
+    if (!L.label_val.empty()) {
+      r.label_val.resize((size_t)n_pairs * (size_t)r.T);
+      for (uint64_t p = 0; p < n_pairs; ++p)
+        std::copy_n(L.label_val.begin() + (size_t)lrow[p] * (size_t)r.T, (size_t)r.T, r.label_val.begin() + (size_t)p * (size_t)r.T);
+    }
   } else {
     r.columns = Columns::TagsTimeValue;
     r.value_name = L.value_name + " " + kOpSymbols[op_] + " " + R.value_name;
@@ -909,7 +928,7 @@ const char* const kSetNames[] = {"and", "or", "unless"};
 
 // left.distinct() of `and` / `unless` (planner.rs:3549-3703): a cell whose labels, step and value bits (DataFusion's
 // group equality on f64) equal those of a cell of an earlier row is dropped.  Only rows that share a label tuple can
-// hold such cells, so only they are compared.
+// hold such cells, so only they are compared.  count_values' counted value is a column of the row too.
 void drop_duplicate_cells(NodeResult& n) {
   if (n.rows < 2 || n.T == 0) return;
   std::vector<int> all(n.labels.names.size());
@@ -928,7 +947,9 @@ void drop_duplicate_cells(NodeResult& n) {
         const double x = n.val[(size_t)g[i] * (size_t)n.T + (size_t)k];
         for (size_t j = 0; j < i; ++j) {
           const double y = n.val[(size_t)g[j] * (size_t)n.T + (size_t)k];
-          if (n.valid_at(g[j], k) && std::memcmp(&x, &y, sizeof x) == 0) {
+          const size_t a = (size_t)g[i] * (size_t)n.T + (size_t)k, b = (size_t)g[j] * (size_t)n.T + (size_t)k;
+          if (n.valid_at(g[j], k) && std::memcmp(&x, &y, sizeof x) == 0 &&
+              (n.label_val.empty() || std::memcmp(&n.label_val[a], &n.label_val[b], sizeof(double)) == 0)) {
             n.valid[(size_t)g[i] * n.Tw + (size_t)(k >> 5)] &= ~(1u << (k & 31));
             n.val[(size_t)g[i] * (size_t)n.T + (size_t)k] = 0.0;
             break;
@@ -1192,6 +1213,76 @@ void AggregatePlan::compute(NodeResult& r) {
                                        : df_name_ + "(" + child_value + ")";
 }
 
+// ---- CountValuesPlan -----------------------------------------------------------------------------------
+CountValuesPlan::CountValuesPlan(b2p_ctx* ctx, std::string label, std::shared_ptr<PlanNode> child, Modifier modifier,
+                                 std::vector<std::string> labels)
+    : PlanNode(ctx), label_(std::move(label)), child_(std::move(child)), modifier_(modifier), labels_(std::move(labels)) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromCountValuesExec: NULL context");
+  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromCountValuesExec: NULL child");
+}
+
+void CountValuesPlan::compute(NodeResult& r) {
+  child_->run(r);
+  // keep_tsid is false for count_values (planner.rs:402): as for AggregatePlan, an id-keyed child groups as a whole only
+  if (r.labels.id_keyed && modifier_ != Modifier::None)
+    throw PlanError(ErrorKind::Plan, "GpuPromCountValuesExec: an id-keyed (__tsid) child can only be counted without by / without");
+  const std::vector<int> cols = group_columns(r.labels, modifier_, labels_);
+  const std::string count_name = "count(" + r.value_name + ")";
+  // the projection would have two columns of one name (planner.rs:425-430)
+  bool clash = label_ == r.time_index || label_ == count_name;
+  for (int c : cols) clash = clash || r.labels.names[(size_t)c] == label_;
+  if (clash) throw PlanError(ErrorKind::Plan, "GpuPromCountValuesExec: the label \"" + label_ + "\" names another column of the result");
+  Groups groups = group_rows(r.labels, cols, r.rows);
+  const uint32_t G = (uint32_t)groups.rank.size(), R = r.rows, Tw = r.Tw;
+  const size_t T = (size_t)r.T;
+  std::vector<double> cval((size_t)R * T);
+  std::vector<uint32_t> ccnt((size_t)R * T);
+  if (R > 0 && T > 0)
+    check(b2p_count_values(ctx_, r.val.data(), r.valid.data(), groups.id.data(), R, G, (uint64_t)T, cval.data(),
+                           ccnt.data()),
+          ErrorKind::Execution);
+  // b2p_count_values' rows: group g's members (rank rows) from goff[g]
+  std::vector<uint32_t> goff((size_t)G + 1, 0u), place(G);
+  for (uint32_t q = 0; q < R; ++q) ++goff[groups.id[q] + 1];
+  std::partial_sum(goff.begin(), goff.end(), goff.begin());
+  for (uint32_t g = 0; g < G; ++g) place[groups.rank[g]] = g;
+  // output rows: the groups in label order, each with its rank rows that hold a value at some step
+  std::vector<uint32_t> src, lab, first(1, 0u);
+  for (uint32_t p = 0; p < G; ++p) {
+    for (uint32_t q = goff[place[p]]; q < goff[place[p] + 1]; ++q) {
+      if (!std::any_of(ccnt.begin() + (size_t)q * T, ccnt.begin() + (size_t)(q + 1) * T, [](uint32_t n) { return n != 0; }))
+        break;  // ranks are dense: no later rank has a value either
+      src.push_back(q);
+      lab.push_back(p);
+    }
+    first.push_back((uint32_t)src.size());
+  }
+  const uint32_t n = (uint32_t)src.size();
+  r.labels = groups.labels.gather(lab);
+  r.val.assign((size_t)n * T, 0.0);
+  r.valid.assign((size_t)n * Tw, 0u);
+  r.label_val.assign((size_t)n * T, 0.0);
+  r.cell_order.clear();
+  for (uint32_t o = 0; o < n; ++o)
+    for (size_t k = 0; k < T; ++k) {
+      const size_t c = (size_t)src[o] * T + k;
+      if (ccnt[c] == 0) continue;
+      r.val[(size_t)o * T + k] = (double)ccnt[c];
+      r.label_val[(size_t)o * T + k] = cval[c];
+      r.valid[(size_t)o * Tw + (k >> 5)] |= 1u << (k & 31);
+    }
+  // export order Sort(group labels, ts, value): a group's rows by step, then rank (rank order is value order)
+  for (uint32_t p = 0; p < G; ++p)
+    for (size_t k = 0; k < T; ++k)
+      for (uint32_t o = first[p]; o < first[p + 1]; ++o)
+        if (r.valid_at(o, (int64_t)k)) r.cell_order.push_back((uint64_t)o * T + k);
+  r.rows = n;
+  r.columns = Columns::CountTagsTimeLabel;
+  r.value_name = count_name;
+  r.label_name = label_;
+  r.value_is_count = true;
+}
+
 }  // namespace b2p
 
 // ---- C entry points -----------------------------------------------------------------------------------
@@ -1339,6 +1430,15 @@ b2p_plan* b2p_plan_aggregate_create(b2p_ctx* ctx, const char* op, double param, 
     if (!op || !child || (n_labels > 0 && !labels)) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
     return std::make_shared<b2p::AggregatePlan>(ctx, op, param, child->node, parse_modifier(modifier),
                                                 strings(labels, n_labels));
+  });
+}
+
+b2p_plan* b2p_plan_count_values_create(b2p_ctx* ctx, const char* label, b2p_plan* child, const char* modifier,
+                                       const char* const* labels, int32_t n_labels) {
+  return create([&] {
+    if (!label || !child || (n_labels > 0 && !labels)) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    return std::make_shared<b2p::CountValuesPlan>(ctx, label, child->node, parse_modifier(modifier),
+                                                  strings(labels, n_labels));
   });
 }
 

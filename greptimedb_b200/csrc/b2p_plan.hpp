@@ -106,6 +106,7 @@ enum class Columns {
   TagsTimeValue,  // {tags.., time index, value}: the by-label aggregate, and arithmetic between two vectors
   TimeSorted,     // {time index, then the tags and the value column in name order}: `or`
   ValueTagsTime,  // {value, tags.., time index}: topk / bottomk
+  CountTagsTimeLabel,  // {count Int64 (Float64 under an element-wise stage), tags.., time index, label}: count_values
 };
 
 // What a node computed, before it becomes Arrow: a dense [rows x T] grid with validity, the eval timestamps and one label
@@ -123,6 +124,11 @@ struct NodeResult {
   // when not empty, the export emits these cells (row * T + step), in this order, instead of rows then steps; a cell
   // whose bit a later stage cleared is skipped
   std::vector<uint64_t> cell_order;
+  // count_values (Columns::CountTagsTimeLabel): each cell's counted value [rows x T], exported as the column label_name;
+  // value_is_count exports the value column as Int64 (an element-wise stage on top clears it)
+  std::vector<double> label_val;
+  std::string label_name;
+  bool value_is_count = false;
   bool valid_at(uint32_t r, int64_t k) const { return (valid[(size_t)r * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u; }
 };
 
@@ -288,6 +294,27 @@ class AggregatePlan : public PlanNode {
   int op_;
   std::string df_name_;  // DataFusion's name of the aggregate function ("var_pop", "quantile", ...)
   double param_;
+  std::shared_ptr<PlanNode> child_;
+  Modifier modifier_;
+  std::vector<std::string> labels_;
+};
+
+// count_values(label, child) [by | without (labels)], GpuPromCountValuesExec: the reference's Aggregate(groupBy = [group
+// labels.., ts, value], count(value)) -> Projection(count, group labels.., ts, value AS label) -> Sort(group labels, ts,
+// value), planner.rs:402-445.  Group labels as for AggregatePlan (group_rows / group_columns); the per-step distinct
+// values and counts are b2p_count_values.  Rows: per group in Labels::less order, one for each rank of a distinct value
+// that occurs at some step, labelled with the group labels and holding the count (named count(<child value name>)), so
+// the nodes above count, sum or compare them; the counted values ride along in label_val for the export.
+class CountValuesPlan : public PlanNode {
+ public:
+  CountValuesPlan(b2p_ctx* ctx, std::string label, std::shared_ptr<PlanNode> child, Modifier modifier,
+                  std::vector<std::string> labels);
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  std::string label_;
   std::shared_ptr<PlanNode> child_;
   Modifier modifier_;
   std::vector<std::string> labels_;

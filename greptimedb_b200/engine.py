@@ -336,6 +336,20 @@ class Context:
                                                int(n_groups), T, _ptr(out), _ptr(cnt)))
         return out, cnt
 
+    def count_values(self, vals, valid, gid, n_groups):
+        """count_values per (group, step): rows grouped by gid (>= n_groups: no group) -> (out [R,T] f64, cnt [R,T] u32)
+        with rows in the order of a stable sort of the rows by gid: at each step a group's j-th row holds its j-th
+        smallest distinct value (by bits, in the f64 total order) and its multiplicity; cnt 0 past the last."""
+        vals = np.ascontiguousarray(vals, np.float64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        gid = np.ascontiguousarray(gid, np.uint32)
+        S, T = vals.shape
+        out = np.zeros((S, T), np.float64)
+        cnt = np.zeros((S, T), np.uint32)
+        self._check(self._L.b2p_count_values(self._h, _ptr(vals), _ptr(valid), _ptr(gid), S, int(n_groups), T,
+                                             _ptr(out), _ptr(cnt)))
+        return out, cnt
+
     # -- device API (torch tensors or raw pointers; asynchronous) ----------------------------------
     def series_offsets_dev(self, sid, n_rows, n_series, offsets):
         self._check(self._L.b2p_series_offsets_dev(self._h, _ptr(sid), n_rows, n_series, _ptr(offsets)))
@@ -459,6 +473,12 @@ class Context:
         """quantile(phi) over the rows of a group index (group_index_create_dev) into out_val / out_cnt [G,T]."""
         self._check(self._L.b2p_group_quantile_dev(self._h, float(phi), _ptr(vals), _ptr(valid), index, T,
                                                    _ptr(out_val), _ptr(out_cnt)))
+
+    def count_values_dev(self, vals, valid, index, T, out_val, out_cnt):
+        """count_values over the rows of a group index (group_index_create_dev) into out_val / out_cnt [rows,T], rows in
+        the index's member order."""
+        self._check(self._L.b2p_count_values_dev(self._h, _ptr(vals), _ptr(valid), index, T, _ptr(out_val),
+                                                 _ptr(out_cnt)))
 
     def count_valid_words_dev(self, cnt, n_rows, T, valid_words):
         self._check(self._L.b2p_count_valid_words_dev(self._h, _ptr(cnt), n_rows, T, _ptr(valid_words)))

@@ -213,3 +213,25 @@ class AggregatePlan(_PlanNode):
         self._h = self._L.b2p_plan_aggregate_create(ctx._h, op.encode(), phi, child._h, modifier, arr, len(labels))
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class CountValuesPlan(_PlanNode):
+    """count_values(label, child) per (group labels, step), with `by` or `without` labels (neither: one group per step):
+    one row per distinct value (by bits) of the group's cells at the step.  Nodes above see rows labelled with the group
+    labels whose value is the count; execute() emits {count(<child value>) Int64, group labels.., time index,
+    <label> Float64} by group labels, ts, value (Float64 counts under an element-wise stage).  The child may be any
+    node; it stays usable and is kept alive by this node."""
+
+    def __init__(self, ctx: Context, label: str, child: _PlanNode, by: Optional[Sequence[str]] = None,
+                 without: Optional[Sequence[str]] = None):
+        if by is not None and without is not None:
+            raise ValueError("by and without are exclusive")
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (child,)
+        modifier, labels = (b"by", list(by)) if by is not None else (b"without", list(without)) if without is not None \
+            else (None, [])
+        arr = _cstr_array(labels)
+        self._h = self._L.b2p_plan_count_values_create(ctx._h, label.encode(), child._h, modifier, arr, len(labels))
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())

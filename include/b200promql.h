@@ -43,6 +43,8 @@
  *                              rows and ranks the label tuples
  *   b2p_group_quantile[_dev]   quantile by label: Aggregate(quantile(φ, value)), QuantileAccumulator::evaluate,
  *                              quantile_aggr.rs:110-116, quantile.rs:201-225
+ *   b2p_count_values[_dev]     count_values by label: Aggregate(groupBy = [labels.., ts, value], count(value)) ->
+ *                              Sort(labels, ts, value), planner.rs:402-445
  *
  * Data layout (HBM, struct-of-arrays, all row-sorted by (series id, timestamp) exactly like
  * the reference's required_input_ordering, series_divide.rs:410-440):
@@ -352,6 +354,17 @@ B2P_API int b2p_topk_dev(b2p_ctx* ctx, int32_t bottom, double k, const double* v
 B2P_API int b2p_group_quantile_dev(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid,
                                    const b2p_group_index* index, uint64_t T, double* out_val, uint32_t* out_cnt);
 
+/* count_values(label, v) by label (K12; the reference's Aggregate(groupBy = [group labels.., ts, value], count(value)),
+ * planner.rs:402-445): per (group, step) the distinct values of the valid cells of the index's member rows, a value
+ * being its bits (-0.0 and +0.0 are two values, and so are NaNs with different bits), in the f64 total order.  Output
+ * out_val (f64) / out_cnt (u32) [n_series x T] with rows in the index's member order (a group's rows ordered by row
+ * index, the groups by id; rows of gid >= n_groups last): at step k, the group's j-th row holds its j-th smallest
+ * distinct value and how many of its cells have it; out_cnt 0 (value 0.0) past the last, and on every row of
+ * gid >= n_groups.  Exact and deterministic; scratch comes from the context and is bounded (b2p_api.cu,
+ * count_values_run).  B2P_E_INVALID: a NULL argument; B2P_E_TOO_LARGE: a group of more than 67 M members. */
+B2P_API int b2p_count_values_dev(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const b2p_group_index* index,
+                                 uint64_t T, double* out_val, uint32_t* out_cnt);
+
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
  * the id column `sid` (ids sid_base .. sid_base + n_series - 1, non-decreasing), or copied from `offsets_in`
@@ -412,6 +425,12 @@ B2P_API int b2p_topk(b2p_ctx* ctx, int32_t bottom, double k, const double* vals,
  * instead of an index, which the call builds itself. */
 B2P_API int b2p_group_quantile(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid, const uint32_t* gid,
                                uint32_t n_rows, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt);
+
+/* Host-pointer form of b2p_count_values_dev (synchronous): the rows' group ids gid [n_rows] (>= n_groups: no group)
+ * instead of an index, which the call builds itself.  out_val / out_cnt [n_rows x T] in the order of a stable sort of the
+ * rows by gid. */
+B2P_API int b2p_count_values(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const uint32_t* gid,
+                             uint32_t n_rows, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt);
 
 /* Host-pointer forms of b2p_instant_fn_dev / b2p_scalar_calculate_dev (synchronous; device-found errors returned). */
 B2P_API int b2p_instant_fn(b2p_ctx* ctx, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
@@ -530,6 +549,18 @@ B2P_API b2p_plan* b2p_plan_topk_create(b2p_ctx* ctx, int32_t bottom, double k, b
 B2P_API b2p_plan* b2p_plan_aggregate_create(b2p_ctx* ctx, const char* op, double param, b2p_plan* child,
                                             const char* modifier /* NULL | "by" | "without" */,
                                             const char* const* labels, int32_t n_labels);
+/* count_values(label, child) with an optional `by` / `without` modifier, GpuPromCountValuesExec (planner.rs:402-445):
+ * groups as for b2p_plan_aggregate_create; per (group, step) one row for each distinct value of the child's cells (as
+ * b2p_count_values_dev).  Nodes above see one row per (group, rank of the value), with the group labels as its labels
+ * and the count as its value, named count(<child's value name>): count(count_values(..)), sum by (..)(count_values(..))
+ * and count_values(..) > 1 compose.  The export has columns {count(<child value>) Int64, group labels.., time index,
+ * <label> Float64 (the value)} with rows by group labels, ts, value in the f64 total order; with an element-wise stage
+ * on top the first column is Float64.  A label equal to a group label, the time index or the count column, and an
+ * id-keyed (__tsid) child with a modifier, are Plan errors at execute.  Ownership as for b2p_plan_binary_create.  NULL
+ * on error (b2p_plan_last_error). */
+B2P_API b2p_plan* b2p_plan_count_values_create(b2p_ctx* ctx, const char* label, b2p_plan* child,
+                                               const char* modifier /* NULL | "by" | "without" */,
+                                               const char* const* labels, int32_t n_labels);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

@@ -307,6 +307,12 @@ extern "C" {
         ctx: *mut b2p_ctx, phi: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index, t: u64,
         out_val: *mut f64, out_cnt: *mut u32,
     ) -> c_int;
+    /// count_values per (group, step) into out_val / out_cnt [n_series x T], rows in the index's member order: a group's
+    /// j-th row holds its j-th smallest distinct value (by bits, f64 total order) and its multiplicity; cnt 0 = none.
+    pub fn b2p_count_values_dev(
+        ctx: *mut b2p_ctx, vals: *const f64, valid: *const u32, index: *const b2p_group_index, t: u64,
+        out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
 
     // ---- host-side helper (no device work): SeriesDivide + cadence scan of one sorted batch ---------------------------
     pub fn b2p_host_scan_series(
@@ -371,6 +377,10 @@ extern "C" {
         ctx: *mut b2p_ctx, phi: f64, vals: *const f64, valid: *const u32, gid: *const u32, n_rows: u32, n_groups: u32,
         t: u64, out_val: *mut f64, out_cnt: *mut u32,
     ) -> c_int;
+    pub fn b2p_count_values(
+        ctx: *mut b2p_ctx, vals: *const f64, valid: *const u32, gid: *const u32, n_rows: u32, n_groups: u32, t: u64,
+        out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
 
     // ---- plan-level API over the Arrow C Data Interface -----------------------------------------------------------------
     pub fn b2p_plan_range_create(
@@ -404,6 +414,12 @@ extern "C" {
     /// ownership of `child` as for b2p_plan_binary_create.
     pub fn b2p_plan_aggregate_create(
         ctx: *mut b2p_ctx, op: *const c_char, param: f64, child: *mut b2p_plan, modifier: *const c_char,
+        labels: *const *const c_char, n_labels: i32,
+    ) -> *mut b2p_plan;
+    /// count_values(`label`, child); `modifier`: NULL, "by" or "without"; ownership of `child` as for
+    /// b2p_plan_binary_create.
+    pub fn b2p_plan_count_values_create(
+        ctx: *mut b2p_ctx, label: *const c_char, child: *mut b2p_plan, modifier: *const c_char,
         labels: *const *const c_char, n_labels: i32,
     ) -> *mut b2p_plan;
     /// MOVES the batch: on success the release callbacks now belong to the plan.

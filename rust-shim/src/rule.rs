@@ -64,6 +64,16 @@
 //!         (sum avg count min max stddev_pop var_pop, quantile(Float64(φ), col), max(Float64(1)) = group)
 //! ```
 //!
+//! count_values (planner.rs:402-445):
+//!
+//! ```text
+//!   ProjectionExec(count, group labels.., ts, label) <- SortExec(group labels, ts, value)
+//!     <- ProjectionExec(count, group labels.., ts, value AS label, value)
+//!     <- AggregateExec(Final | FinalPartitioned) <- RepartitionExec
+//!     <- AggregateExec(Partial, group labels + ts + value, count(value))
+//!     <- GpuPromRangeExec                     => `match_count_values`: the b2p_plan_count_values_create arguments
+//! ```
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
@@ -175,7 +185,9 @@ impl GpuPromRewrite {
             "max" => "max",
             "stddev_pop" => "stddev",
             "var_pop" => "stdvar",
-            _ => return None, // quantile / count_values are not all-reduce-able: stay on the CPU (topk: match_topk)
+            // quantile / count_values are not all-reduce-able here (match_aggregate_node, match_count_values; topk:
+            // match_topk)
+            _ => return None,
         };
         let mut by = Vec::new();
         for (expr, _name) in partial.group_expr().expr() {
@@ -238,6 +250,15 @@ pub struct GpuPromTopkSpec {
 pub struct GpuPromAggregateSpec {
     pub op: &'static str,
     pub param: f64,
+    pub by: Vec<String>,
+    pub child: GpuPromRangeParams,
+}
+
+/// What `b2p_plan_count_values_create` takes for a matched count_values: the label (the value column's alias), the
+/// group labels (passed as `by`, in the group-by order, the time index and the value left out) and the child node.
+#[derive(Debug, Clone)]
+pub struct GpuPromCountValuesSpec {
+    pub label: String,
     pub by: Vec<String>,
     pub child: GpuPromRangeParams,
 }
@@ -399,8 +420,8 @@ impl GpuPromRewrite {
 
     /// `AggregateExec(Final) <- RepartitionExec <- AggregateExec(Partial)` over a `GpuPromRangeExec` -> the arguments of
     /// `b2p_plan_aggregate_create`.  `quantile(Float64(φ), col)` needs a literal φ; `max(Float64(1))` is `group`
-    /// (planner.rs:2836-2838).  count_values, a non-literal φ and group columns that are not tags of the child stay on the
-    /// CPU.
+    /// (planner.rs:2836-2838).  A non-literal φ and group columns that are not tags of the child stay on the CPU;
+    /// count_values (which groups by the value column too) is `match_count_values`.
     pub fn match_aggregate_node(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromAggregateSpec> {
         let fin = plan.as_any().downcast_ref::<AggregateExec>()?;
         if !matches!(fin.mode(), AggregateMode::FinalPartitioned | AggregateMode::Final) {
@@ -428,8 +449,8 @@ impl GpuPromRewrite {
             _ => return None,
         };
         // every group column other than the time index must be one of the child's tags: count_values (planned as
-        // count with the value column among the group columns, planner.rs:420-424, 2833) and any other grouping the
-        // node cannot express stay on the CPU
+        // count with the value column among the group columns, planner.rs:420-424, 2833) goes to match_count_values,
+        // and any other grouping the node cannot express stays on the CPU
         let params = child.params();
         let mut by = Vec::new();
         for (expr, _name) in partial.group_expr().expr() {
@@ -442,6 +463,51 @@ impl GpuPromRewrite {
             }
         }
         Some(GpuPromAggregateSpec { op, param, by, child: params.clone() })
+    }
+
+    /// `ProjectionExec <- SortExec <- ProjectionExec(value AS label) <- AggregateExec(Final) <- RepartitionExec <-
+    /// AggregateExec(Partial, groupBy [tags.., ts, value], count(value))` over a `GpuPromRangeExec` (planner.rs:402-445)
+    /// -> the arguments of `b2p_plan_count_values_create`.  Exactly one group column is neither the time index nor a
+    /// tag of the child: the counted value, which must be count's argument; the inner projection names its alias.
+    pub fn match_count_values(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromCountValuesSpec> {
+        let top = plan.as_any().downcast_ref::<ProjectionExec>()?;
+        let sort = top.input().as_any().downcast_ref::<SortExec>()?;
+        let inner = sort.input().as_any().downcast_ref::<ProjectionExec>()?;
+        let fin = inner.input().as_any().downcast_ref::<AggregateExec>()?;
+        if !matches!(fin.mode(), AggregateMode::FinalPartitioned | AggregateMode::Final) {
+            return None;
+        }
+        let repart = fin.input().as_any().downcast_ref::<RepartitionExec>()?;
+        let partial = repart.input().as_any().downcast_ref::<AggregateExec>()?;
+        let [a] = partial.aggr_expr() else { return None };
+        if !matches!(partial.mode(), AggregateMode::Partial) || a.fun().name() != "count" {
+            return None;
+        }
+        let child = partial.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let params = child.params();
+        let mut by = Vec::new();
+        let mut value = None;
+        for (expr, _name) in partial.group_expr().expr() {
+            let c = expr.as_any().downcast_ref::<Column>()?;
+            if c.name() == params.time_index_column {
+                continue;
+            }
+            if params.tag_columns.iter().any(|t| t == c.name()) {
+                by.push(c.name().to_string());
+            } else if value.replace(c.name().to_string()).is_some() {
+                return None;
+            }
+        }
+        let value = value?;
+        let [arg] = a.expressions().as_slice() else { return None };
+        if arg.as_any().downcast_ref::<Column>()?.name() != value {
+            return None;
+        }
+        let label = inner.expr().iter().find_map(|e| {
+            let c = e.expr.as_any().downcast_ref::<Column>()?;
+            (c.name() == value && e.alias != value).then(|| e.alias.clone())
+        })?;
+        Some(GpuPromCountValuesSpec { label, by, child: params.clone() })
     }
 
     /// `ProjectionExec | FilterExec <- HashJoinExec(Inner, tags.. + ts)` over two `GpuPromRangeExec` -> the arguments of
