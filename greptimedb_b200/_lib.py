@@ -32,6 +32,7 @@ EXPORTED_SYMBOLS = [
     "b2p_topk_dev", "b2p_topk", "b2p_plan_topk_create",
     "b2p_group_quantile_dev", "b2p_group_quantile", "b2p_plan_aggregate_create",
     "b2p_count_values_dev", "b2p_count_values", "b2p_plan_count_values_create",
+    "b2p_subquery_dev", "b2p_subquery", "b2p_plan_subquery_create",
 ]
 
 
@@ -137,6 +138,9 @@ def load() -> C.CDLL:
         "b2p_count_values_dev": (C.c_int, [vp, vp, vp, vp, u64, vp, vp]),
         "b2p_count_values": (C.c_int, [vp, vp, vp, vp, u32, u32, u64, vp, vp]),
         "b2p_plan_count_values_create": (vp, [vp, C.c_char_p, vp, C.c_char_p, C.POINTER(C.c_char_p), i32]),
+        "b2p_subquery_dev": (C.c_int, [vp, P, i64, i64, vp, vp, u32, u64, vp, vp]),
+        "b2p_subquery": (C.c_int, [vp, P, i64, i64, vp, vp, u32, u64, vp, vp]),
+        "b2p_plan_subquery_create": (vp, [vp, C.c_char_p, P, vp]),
         "b2p_plan_set_function": (C.c_int, [vp, C.c_char_p, C.POINTER(dbl), i32]),
         "b2p_plan_scalar_create": (vp, [vp, vp]),
     }

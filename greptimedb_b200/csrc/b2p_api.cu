@@ -31,6 +31,7 @@
 #include "b2p_count_values.cuh"
 #include "b2p_instant.cuh"
 #include "b2p_setop.cuh"
+#include "b2p_subquery.cuh"
 #include "b2p_quantile.cuh"
 #include "b2p_topk.cuh"
 #include "b2p_kernel_t.cuh"
@@ -257,6 +258,8 @@ struct b2p_ctx {
   // count_values: key and sorted-key buffers, ranks and starts, segment tables, member groups, CUB's temp (bound in
   // count_values_run)
   DevBuf v_keys, v_alt, v_rank, v_seg, v_group, v_tmp;
+  // subquery: the sample rows of one batch of child rows (ts, val, offsets) and CUB's temp (bound in subquery_run)
+  DevBuf sq_ts, sq_val, sq_off, sq_tmp;
   // resident CTAs per SM of each persistent kernel instantiation (persistent_grid)
   std::unordered_map<const void*, int> blocks_per_sm;
 };
@@ -720,6 +723,7 @@ void b2p_destroy(b2p_ctx* c) {
   for (DevBuf* b : {&c->s_goff[0], &c->s_goff[1], &c->s_members[0], &c->s_members[1], &c->s_mask}) b->release();
   for (DevBuf* b : {&c->t_table, &c->t_cand, &c->t_state, &c->q_table, &c->q_state, &c->q_hist}) b->release();
   for (DevBuf* b : {&c->v_keys, &c->v_alt, &c->v_rank, &c->v_seg, &c->v_group, &c->v_tmp}) b->release();
+  for (DevBuf* b : {&c->sq_ts, &c->sq_val, &c->sq_off, &c->sq_tmp}) b->release();
   if (c->s_h2d) cudaStreamDestroy(c->s_h2d);
   if (c->s_d2h) cudaStreamDestroy(c->s_d2h);
   if (c->d_ring) cudaFree(c->d_ring);
@@ -2122,6 +2126,90 @@ int b2p_count_values_dev(b2p_ctx* c, const double* vals, const uint32_t* valid, 
   return rc;
 }
 
+/* ---- subqueries ---------------------------------------------------------------------------------------------- */
+}  // extern "C"
+
+namespace {
+// A range call of this context that reads the subquery scratch and whose verdict b2p_sync has not taken yet: b2p_sync
+// may run it again from the scratch (slow-path arena overflow), so the scratch must not change before that.
+bool subquery_scratch_pending(const b2p_ctx* c) {
+  for (const b2p_ctx::Pending& pc : c->pending)
+    if (pc.args.ts == c->sq_ts.as<int64_t>()) return true;
+  return false;
+}
+
+// Rows are processed in batches of at most kSqBatchCells / T_inner rows (one row when a row alone is larger).  Per
+// batch: K13's count kernel, CUB's exclusive scan of the counts, K13's scatter, then the range call over the batch's
+// sample rows into its rows of out / out_valid.  The range call is given the batch's cell count as its row count: the
+// extent of the scratch, which the tiers only use to bound their paired loads, so the sample total is never read back.
+// A batch waits (b2p_sync) for the verdict of the range call before it, since the scratch is rewritten; so does the
+// first batch for that of an earlier call.  A grid of one batch makes no host round trip.
+// Scratch (context buffers sq_*): 16 B per grid cell of a batch (8 B timestamp, 8 B value: at most 2.1 GB unless one
+// row alone has more than kSqBatchCells steps), 8 B per row of a batch plus one for the offsets, and CUB's scan temp.
+int subquery_run(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval, const double* vals,
+                 const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, int64_t T, double* out, uint32_t* out_valid) {
+  int rc;
+  const uint32_t Tw_in = (uint32_t)((T_inner + 31) / 32), Tw = (uint32_t)((T + 31) / 32);
+  const uint32_t batch_rows = (uint32_t)std::min<uint64_t>(n_rows, std::max<uint64_t>(1, kSqBatchCells / T_inner));
+  const uint64_t cells = (uint64_t)batch_rows * T_inner;
+  size_t scan_bytes = 0;
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                   (int)batch_rows + 1, c->stream));
+  if (subquery_scratch_pending(c) && (rc = b2p_sync(c))) return rc;
+  if ((rc = c->sq_ts.ensure(cells * 8)) || (rc = c->sq_val.ensure(cells * 8)) ||
+      (rc = c->sq_off.ensure(((size_t)batch_rows + 1) * 8)) || (rc = c->sq_tmp.ensure(std::max<size_t>(scan_bytes, 16))))
+    return rc;
+  b2p_range_params q = *p;
+  for (uint32_t r0 = 0; r0 < n_rows; r0 += batch_rows) {
+    const uint32_t nb = std::min(batch_rows, n_rows - r0);
+    if (r0 > 0 && (rc = b2p_sync(c))) return rc;
+    SubqueryArgs a{};
+    a.vals = vals + (uint64_t)r0 * T_inner; a.valid = valid + (uint64_t)r0 * Tw_in;
+    a.T = T_inner; a.Tw = Tw_in; a.rows = nb;
+    a.start = inner_start; a.interval = inner_interval;
+    a.offsets = c->sq_off.as<unsigned long long>(); a.ts = c->sq_ts.as<int64_t>(); a.val = c->sq_val.as<double>();
+    const unsigned grid = std::max(1u, capped_grid(c, (uint64_t)nb * 32, 256, 8));
+    stage_begin(c, 3);
+    subquery_count_kernel<<<grid, 256, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    size_t bytes = c->sq_tmp.cap;
+    CU(cub::DeviceScan::ExclusiveSum(c->sq_tmp.p, bytes, a.offsets, a.offsets, (int)nb + 1, c->stream));
+    subquery_scatter_kernel<<<grid, 256, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    stage_end(c, 3);
+    if ((rc = range_call(c, &q, a.ts, a.val, c->sq_off.as<uint64_t>(), (uint64_t)nb * T_inner, nb,
+                         out + (uint64_t)r0 * T, out_valid + (uint64_t)r0 * Tw, nullptr)))
+      return rc;
+  }
+  return B2P_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_subquery_dev(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval,
+                     const double* vals, const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, double* out,
+                     uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int64_t T = 0;
+  int rc = check_grid(p, n_rows, &T);
+  if (rc) return rc;
+  if (p->range == 0) return fail(B2P_E_INVALID, "subquery: zero range");
+  if (p->offset != 0 || p->filter_nan != 0) return fail(B2P_E_INVALID, "subquery: offset and filter_nan must be 0");
+  if (inner_interval <= 0) return fail(B2P_E_INVALID, "subquery: inner interval must be > 0 (got %lld)", (long long)inner_interval);
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!out || !out_valid || (T_inner && (!vals || !valid))) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  if (T_inner == 0) {  // no inner steps: no samples, no cell
+    CU(cudaMemsetAsync(out, 0, (size_t)n_rows * (size_t)T * 8, c->stream));
+    CU(cudaMemsetAsync(out_valid, 0, (size_t)n_rows * (size_t)((T + 31) / 32) * 4, c->stream));
+    return B2P_OK;
+  }
+  return subquery_run(c, p, inner_start, inner_interval, vals, valid, n_rows, T_inner, T, out, out_valid);
+}
+
 int b2p_synth_fill_dev(b2p_ctx* c, uint64_t series_begin, uint64_t n_series, uint32_t n_samples, int64_t t0,
                        int64_t scrape_ms, uint32_t jitter_ms, int32_t with_resets, uint64_t seed, int64_t* ts,
                        double* val, uint32_t* sid) {
@@ -2848,6 +2936,29 @@ int b2p_count_values(b2p_ctx* c, const double* vals, const uint32_t* valid, cons
   if (!rc) rc = s.finish();
   b2p_group_index_destroy(c, ix);
   return rc;
+}
+
+int b2p_subquery(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval, const double* vals,
+                 const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int64_t T = 0;
+  int rc = check_grid(p, n_rows, &T);
+  if (rc) return rc;
+  if (n_rows == 0 || T == 0) return b2p_subquery_dev(c, p, inner_start, inner_interval, nullptr, nullptr, 0, 0, nullptr,
+                                                     nullptr);  // (the argument checks only)
+  if (!out || !out_valid || (T_inner && (!vals || !valid))) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const size_t Tw_in = (size_t)((T_inner + 31) / 32), Tw = (size_t)((T + 31) / 32);
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_rows * T_inner * 8);
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw_in * 4);
+  double* d_out = s.out(out, (size_t)n_rows * (size_t)T * 8);
+  uint32_t* d_valid_out = s.out(out_valid, (size_t)n_rows * Tw * 4);
+  if ((rc = s.rc) ||
+      (rc = b2p_subquery_dev(c, p, inner_start, inner_interval, d_vals, d_valid, n_rows, T_inner, d_out, d_valid_out)) ||
+      (rc = b2p_sync(c)))
+    return rc;
+  return s.finish();
 }
 
 }  // extern "C"

@@ -1283,6 +1283,51 @@ void CountValuesPlan::compute(NodeResult& r) {
   r.value_is_count = true;
 }
 
+// ---- SubqueryPlan --------------------------------------------------------------------------------------
+SubqueryPlan::SubqueryPlan(b2p_ctx* ctx, std::string function, const b2p_range_params& p, std::shared_ptr<PlanNode> child)
+    : PlanNode(ctx), function_(std::move(function)), p_(p), child_(std::move(child)) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromSubqueryExec: NULL context");
+  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: NULL child");
+  p_.fn_id = function_id_from_name(function_);
+  if (p_.fn_id < 0) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: unknown range function " + function_);
+  if (p_.interval <= 0) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: interval must be positive");
+  if (p_.range <= 0) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: range must be positive (zero range selector)");
+  if (p_.offset != 0 || p_.filter_nan != 0)
+    throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: offset and filter_nan must be 0 (RangeManipulate has neither)");
+}
+
+void SubqueryPlan::compute(NodeResult& r) {
+  NodeResult C;
+  child_->run(C);
+  const int64_t T_in = C.T;
+  const int64_t step = T_in > 1 ? C.eval_ts[1] - C.eval_ts[0] : p_.interval;  // (one inner step: any positive step)
+  bool regular = step > 0;
+  for (int64_t k = 1; regular && k < T_in; ++k) regular = C.eval_ts[(size_t)k] == C.eval_ts[0] + k * step;
+  if (!regular) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: the child's eval timestamps are not a regular grid");
+  r = NodeResult();
+  r.T = b2p_num_steps(p_.start, p_.end, p_.interval);
+  r.Tw = (uint32_t)((r.T + 31) / 32);
+  r.rows = C.rows;
+  r.eval_ts.resize((size_t)r.T);
+  for (int64_t k = 0; k < r.T; ++k) r.eval_ts[(size_t)k] = p_.start + k * p_.interval;
+  r.val.assign((size_t)r.rows * (size_t)r.T, 0.0);
+  r.valid.assign((size_t)r.rows * r.Tw, 0u);
+  if (r.rows > 0 && r.T > 0)
+    check(b2p_subquery(ctx_, &p_, T_in > 0 ? C.eval_ts[0] : p_.start, step, C.val.data(), C.valid.data(), C.rows,
+                       (uint64_t)T_in, r.val.data(), r.valid.data()));
+  r.time_index = C.time_index;
+  r.labels = std::move(C.labels);
+  std::string name = function_ + "(" + C.time_index + "_range," + C.value_name;
+  if (p_.fn_id == B2P_FN_RATE || p_.fn_id == B2P_FN_INCREASE || p_.fn_id == B2P_FN_DELTA) {
+    name += "," + C.time_index + ",Int64(" + std::to_string(p_.range) + ")";
+  } else if (p_.fn_id == B2P_FN_PREDICT_LINEAR || p_.fn_id == B2P_FN_QUANTILE_OVER_TIME) {
+    name += "," + float_literal(p_.param0);
+  } else if (p_.fn_id == B2P_FN_HOLT_WINTERS) {
+    name += "," + float_literal(p_.param0) + "," + float_literal(p_.param1);
+  }
+  r.value_name = name + ")";
+}
+
 }  // namespace b2p
 
 // ---- C entry points -----------------------------------------------------------------------------------
@@ -1439,6 +1484,13 @@ b2p_plan* b2p_plan_count_values_create(b2p_ctx* ctx, const char* label, b2p_plan
     if (!label || !child || (n_labels > 0 && !labels)) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
     return std::make_shared<b2p::CountValuesPlan>(ctx, label, child->node, parse_modifier(modifier),
                                                   strings(labels, n_labels));
+  });
+}
+
+b2p_plan* b2p_plan_subquery_create(b2p_ctx* ctx, const char* function, const b2p_range_params* p, b2p_plan* child) {
+  return create([&] {
+    if (!function || !p || !child) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    return std::make_shared<b2p::SubqueryPlan>(ctx, function, *p, child->node);
   });
 }
 

@@ -320,6 +320,28 @@ class CountValuesPlan : public PlanNode {
   std::vector<std::string> labels_;
 };
 
+// fn(child[range:step]), GpuPromSubqueryExec: the reference's RangeManipulate(start, end, interval, range) directly over
+// the inner plan, then Projection(prom_fn) and Filter(IS NOT NULL) (prom_subquery_expr_to_plan, planner.rs:292-332).
+// The child is any node, evaluated on its own grid (the reference's start' = start - range + step, step' = step or the
+// outer interval, the outer end), which must be regular; its step is read from its eval timestamps.  Every row is one
+// series whose samples are its valid cells (NaN included); the windows are b2p_subquery.  Rows and labels: the child's;
+// columns {time index, value, tags..}.  The value is named as the reference's projection names it over the child's value
+// column: fn(<ti>_range,<child value>) with ,<ti>,Int64(range) for rate / increase / delta and ,Float64(p) per literal
+// argument of predict_linear, quantile_over_time and holt_winters, e.g.
+// prom_max_over_time(ts_range,prom_rate(ts_range,val)) over a range leaf.
+class SubqueryPlan : public PlanNode {
+ public:
+  SubqueryPlan(b2p_ctx* ctx, std::string function, const b2p_range_params& p, std::shared_ptr<PlanNode> child);
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  std::string function_;
+  b2p_range_params p_;
+  std::shared_ptr<PlanNode> child_;
+};
+
 int function_id_from_name(const std::string& prom_name);  // -1 when unknown
 int aggregate_id_from_name(const std::string& name);      // -1 when unknown
 

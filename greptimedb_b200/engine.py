@@ -350,6 +350,20 @@ class Context:
                                              _ptr(out), _ptr(cnt)))
         return out, cnt
 
+    def subquery(self, p: RangeParams, inner_start, inner_interval, vals, valid):
+        """fn(<child>[range:step]): vals [R,T'] / valid [R,Tw'] u32 are the child's grid on the inner steps
+        inner_start + k * inner_interval; every valid cell of a row is a sample of its series (NaN included).  p is the
+        outer grid, range and function (offset 0, filter_nan False).  -> (out [R,T] f64, valid_words [R,Tw] u32)."""
+        vals = np.ascontiguousarray(vals, np.float64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        R, T_in = vals.shape
+        T = num_steps(p.start, p.end, p.interval)
+        out = np.zeros((R, T), np.float64)
+        ov = np.zeros((R, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_subquery(self._h, C.byref(p), int(inner_start), int(inner_interval), _ptr(vals),
+                                         _ptr(valid), R, T_in, _ptr(out), _ptr(ov)))
+        return out, ov
+
     # -- device API (torch tensors or raw pointers; asynchronous) ----------------------------------
     def series_offsets_dev(self, sid, n_rows, n_series, offsets):
         self._check(self._L.b2p_series_offsets_dev(self._h, _ptr(sid), n_rows, n_series, _ptr(offsets)))
@@ -479,6 +493,11 @@ class Context:
         the index's member order."""
         self._check(self._L.b2p_count_values_dev(self._h, _ptr(vals), _ptr(valid), index, T, _ptr(out_val),
                                                  _ptr(out_cnt)))
+
+    def subquery_dev(self, p, inner_start, inner_interval, vals, valid, n_rows, T_inner, out, out_valid):
+        """Device form of subquery(): vals [n_rows,T_inner] / valid [n_rows,Tw'] into out [n_rows,T] / out_valid."""
+        self._check(self._L.b2p_subquery_dev(self._h, C.byref(p), int(inner_start), int(inner_interval), _ptr(vals),
+                                             _ptr(valid), n_rows, T_inner, _ptr(out), _ptr(out_valid)))
 
     def count_valid_words_dev(self, cnt, n_rows, T, valid_words):
         self._check(self._L.b2p_count_valid_words_dev(self._h, _ptr(cnt), n_rows, T, _ptr(valid_words)))

@@ -6,7 +6,8 @@ start/end/interval/range/field column, the prom_* UDF name, optional by-label ag
 pyarrow RecordBatches exactly like the reference's tests feed a MemoryExec.  `scalar_op` puts `node op number` on
 top of any node, `function` an instant-vector function (abs, clamp_min, prom_round, ...; the two chain in call order),
 `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels), `SetOpPlan` applies `and` / `or` / `unless`
-to two nodes, `ScalarPlan` is scalar(node) and `TopkPlan` is topk / bottomk(k, node) [by | without (labels)].
+to two nodes, `ScalarPlan` is scalar(node), `TopkPlan` is topk / bottomk(k, node) [by | without (labels)] and
+`SubqueryPlan` is fn(node[range:step]).
 """
 from __future__ import annotations
 
@@ -233,5 +234,23 @@ class CountValuesPlan(_PlanNode):
             else (None, [])
         arr = _cstr_array(labels)
         self._h = self._L.b2p_plan_count_values_create(ctx._h, label.encode(), child._h, modifier, arr, len(labels))
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class SubqueryPlan(_PlanNode):
+    """function(child[range:step]): RangeManipulate(start, end, interval, range) directly over any node, then the range
+    function `function` ("prom_max_over_time", ...; param0 / param1 as for PromRangeExec).  Build the child on the inner
+    grid: start - range + step .. end every step (step = the subquery's step, or interval when it has none).  Each
+    child row is one series whose samples are its valid cells, NaN included.  Rows and labels are the child's; execute()
+    emits {time index, value, tags..}.  The child stays usable and is kept alive by this node."""
+
+    def __init__(self, ctx: Context, function: str, child: _PlanNode, start: int, end: int, interval: int, range: int,
+                 param0: float = 0.0, param1: float = 0.0, offset: int = 0):
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (child,)
+        p = make_params(0, start, end, interval, range, offset=offset, filter_nan=False, param0=param0, param1=param1)
+        self._h = self._L.b2p_plan_subquery_create(ctx._h, function.encode(), C.byref(p), child._h)
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())

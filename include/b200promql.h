@@ -45,6 +45,8 @@
  *                              quantile_aggr.rs:110-116, quantile.rs:201-225
  *   b2p_count_values[_dev]     count_values by label: Aggregate(groupBy = [labels.., ts, value], count(value)) ->
  *                              Sort(labels, ts, value), planner.rs:402-445
+ *   b2p_subquery[_dev]         fn(<expr>[range:step]): RangeManipulate directly over the inner plan + Projection(prom_fn)
+ *                              + Filter, planner.rs:292-332
  *
  * Data layout (HBM, struct-of-arrays, all row-sorted by (series id, timestamp) exactly like
  * the reference's required_input_ordering, series_divide.rs:410-440):
@@ -365,6 +367,22 @@ B2P_API int b2p_group_quantile_dev(b2p_ctx* ctx, double phi, const double* vals,
 B2P_API int b2p_count_values_dev(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const b2p_group_index* index,
                                  uint64_t T, double* out_val, uint32_t* out_cnt);
 
+/* Subquery fn(<expr>[range:step]) (K13; RangeManipulate(start, end, interval, range) directly over the inner plan,
+ * prom_subquery_expr_to_plan, planner.rs:292-332): vals / valid [n_rows x T_inner] are a child's grid on the inner steps
+ * inner_start + k * inner_interval (the reference plans them from start - range + inner_interval to end).  Every valid
+ * cell of a row is one sample of that row's series, its value a bit copy (no SeriesNormalize: NaN is a sample); p gives
+ * the outer grid (start, end, interval), the range, fn_id and param0 / param1 as for b2p_range_eval_dev, whose tiers
+ * evaluate the windows over those samples.  Output out [n_rows x T] / out_valid [n_rows x Tw] on the outer grid, row for
+ * row, exactly as b2p_range_eval_dev over the same samples.  Each row is one series: the reference's RangeManipulate
+ * windows each input batch as one series (range_manipulate.rs:603-630), which is the row's series whenever the child
+ * hands it one series per batch.  Scratch comes from the context (16 B per grid cell of a batch of rows, b2p_api.cu,
+ * subquery_run); a grid of more than one batch waits for each batch's range call before the next.
+ * B2P_E_INVALID: an unknown fn_id, a non-positive interval or inner_interval, a zero range, a non-zero offset or
+ * filter_nan, a NULL argument. */
+B2P_API int b2p_subquery_dev(b2p_ctx* ctx, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval,
+                             const double* vals, const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, double* out,
+                             uint32_t* out_valid);
+
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
  * the id column `sid` (ids sid_base .. sid_base + n_series - 1, non-decreasing), or copied from `offsets_in`
@@ -431,6 +449,12 @@ B2P_API int b2p_group_quantile(b2p_ctx* ctx, double phi, const double* vals, con
  * rows by gid. */
 B2P_API int b2p_count_values(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const uint32_t* gid,
                              uint32_t n_rows, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt);
+
+/* Host-pointer form of b2p_subquery_dev (synchronous): the grid and its bitmap go to the device, the sample rows are
+ * made there. */
+B2P_API int b2p_subquery(b2p_ctx* ctx, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval,
+                         const double* vals, const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, double* out,
+                         uint32_t* out_valid);
 
 /* Host-pointer forms of b2p_instant_fn_dev / b2p_scalar_calculate_dev (synchronous; device-found errors returned). */
 B2P_API int b2p_instant_fn(b2p_ctx* ctx, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
@@ -561,6 +585,18 @@ B2P_API b2p_plan* b2p_plan_aggregate_create(b2p_ctx* ctx, const char* op, double
 B2P_API b2p_plan* b2p_plan_count_values_create(b2p_ctx* ctx, const char* label, b2p_plan* child,
                                                const char* modifier /* NULL | "by" | "without" */,
                                                const char* const* labels, int32_t n_labels);
+/* function(child[range:step]), GpuPromSubqueryExec (planner.rs:292-332): RangeManipulate(p->start, p->end, p->interval,
+ * p->range) directly over the child, then the range function `function` ("prom_max_over_time", ...; p->fn_id is
+ * ignored; param0 / param1 as for b2p_plan_range_create) and Filter(IS NOT NULL).  The child is any node; the caller
+ * builds it on the inner grid (start - range + step .. end, step = the subquery's step or the outer interval), and
+ * its eval timestamps must be a regular grid.  Each child row is one series whose samples are its valid cells, NaN
+ * included (b2p_subquery).  Output: the child's rows and labels with columns {time index, value, tags..}, the value
+ * named fn(<ti>_range,<child value>) (rate / increase / delta append ,<ti>,Int64(range); predict_linear,
+ * quantile_over_time and holt_winters append their literals as Float64(..)), e.g. prom_rate(ts_range,val,ts,Int64(20000)).
+ * Plan errors: an unknown function, a non-positive interval, a zero range, a non-zero offset or filter_nan (at create;
+ * NULL is returned), a child whose grid is not regular (at execute).  Ownership as for b2p_plan_binary_create. */
+B2P_API b2p_plan* b2p_plan_subquery_create(b2p_ctx* ctx, const char* function, const b2p_range_params* p,
+                                           b2p_plan* child);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

@@ -313,6 +313,13 @@ extern "C" {
         ctx: *mut b2p_ctx, vals: *const f64, valid: *const u32, index: *const b2p_group_index, t: u64,
         out_val: *mut f64, out_cnt: *mut u32,
     ) -> c_int;
+    /// fn(<child>[range:step]) over a child's grid [n_rows x T_inner] on the inner steps inner_start + k * inner_interval:
+    /// every valid cell of a row is one sample of its series (NaN included); p is the outer grid, range and function
+    /// (offset and filter_nan 0).  out [n_rows x T] / out_valid [n_rows x Tw] as b2p_range_eval_dev.
+    pub fn b2p_subquery_dev(
+        ctx: *mut b2p_ctx, p: *const B2pRangeParams, inner_start: i64, inner_interval: i64, vals: *const f64,
+        valid: *const u32, n_rows: u32, t_inner: u64, out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- host-side helper (no device work): SeriesDivide + cadence scan of one sorted batch ---------------------------
     pub fn b2p_host_scan_series(
@@ -381,6 +388,10 @@ extern "C" {
         ctx: *mut b2p_ctx, vals: *const f64, valid: *const u32, gid: *const u32, n_rows: u32, n_groups: u32, t: u64,
         out_val: *mut f64, out_cnt: *mut u32,
     ) -> c_int;
+    pub fn b2p_subquery(
+        ctx: *mut b2p_ctx, p: *const B2pRangeParams, inner_start: i64, inner_interval: i64, vals: *const f64,
+        valid: *const u32, n_rows: u32, t_inner: u64, out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- plan-level API over the Arrow C Data Interface -----------------------------------------------------------------
     pub fn b2p_plan_range_create(
@@ -421,6 +432,11 @@ extern "C" {
     pub fn b2p_plan_count_values_create(
         ctx: *mut b2p_ctx, label: *const c_char, child: *mut b2p_plan, modifier: *const c_char,
         labels: *const *const c_char, n_labels: i32,
+    ) -> *mut b2p_plan;
+    /// `function`(child[range:step]): RangeManipulate(p.start, p.end, p.interval, p.range) directly over the child (built
+    /// on the inner grid); offset and filter_nan must be 0.  Ownership of `child` as for b2p_plan_binary_create.
+    pub fn b2p_plan_subquery_create(
+        ctx: *mut b2p_ctx, function: *const c_char, p: *const B2pRangeParams, child: *mut b2p_plan,
     ) -> *mut b2p_plan;
     /// MOVES the batch: on success the release callbacks now belong to the plan.
     pub fn b2p_plan_push_batch(plan: *mut b2p_plan, batch: *mut FFI_ArrowArray, schema: *mut FFI_ArrowSchema) -> c_int;

@@ -74,6 +74,14 @@
 //!     <- GpuPromRangeExec                     => `match_count_values`: the b2p_plan_count_values_create arguments
 //! ```
 //!
+//! Subqueries fn(<expr>[range:step]) (planner.rs:292-332):
+//!
+//! ```text
+//!   FilterExec(prom_fn IS NOT NULL) <- ProjectionExec(prom_fn(..)) <- PromRangeManipulateExec (no SeriesNormalize)
+//!     <- GpuPromRangeExec (one series per batch: no by-label aggregate, no HistogramFold)
+//!                                           => `match_subquery`: the b2p_plan_subquery_create arguments
+//! ```
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
@@ -260,6 +268,20 @@ pub struct GpuPromAggregateSpec {
 pub struct GpuPromCountValuesSpec {
     pub label: String,
     pub by: Vec<String>,
+    pub child: GpuPromRangeParams,
+}
+
+/// What `b2p_plan_subquery_create` takes for a matched subquery: the range function, RangeManipulate's outer grid and
+/// range, the function's literal arguments and the child node (evaluated on the inner grid).
+#[derive(Debug, Clone)]
+pub struct GpuPromSubquerySpec {
+    pub function: String,
+    pub start: i64,
+    pub end: i64,
+    pub interval: i64,
+    pub range: i64,
+    pub param0: f64,
+    pub param1: f64,
     pub child: GpuPromRangeParams,
 }
 
@@ -508,6 +530,49 @@ impl GpuPromRewrite {
             (c.name() == value && e.alias != value).then(|| e.alias.clone())
         })?;
         Some(GpuPromCountValuesSpec { label, by, child: params.clone() })
+    }
+
+    /// `FilterExec(prom_fn IS NOT NULL) <- ProjectionExec(prom_fn(..)) <- RangeManipulate <- GpuPromRangeExec`, the
+    /// subquery fn(<expr>[range:step]) (prom_subquery_expr_to_plan, planner.rs:292-332: no SeriesNormalize between the
+    /// RangeManipulate and the inner plan) -> the arguments of `b2p_plan_subquery_create`.  The reference's
+    /// RangeManipulate windows every input batch as one series (range_manipulate.rs:603-630) and the node windows every
+    /// child row, so only a child that hands one series per batch is taken: a range or instant node (SeriesDivide's
+    /// batches), with or without element-wise stages, or its aggregate without `by` (one series).  An aggregate by labels
+    /// or a HistogramFold child stays on the CPU.
+    pub fn match_subquery(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromSubquerySpec> {
+        let filter = plan.as_any().downcast_ref::<FilterExec>()?;
+        let not_null = filter.predicate().as_any().downcast_ref::<IsNotNullExpr>()?;
+        let filtered_col = not_null.arg().as_any().downcast_ref::<Column>()?.index();
+        let projection = filter.input().as_any().downcast_ref::<ProjectionExec>()?;
+        let udf_expr = projection.expr().get(filtered_col)?.expr.clone();
+        let udf = udf_expr.as_any().downcast_ref::<ScalarFunctionExpr>()?;
+        let function = udf.name().to_string();
+        B2pFn::from_udf_name(&function)?;
+        for (i, e) in projection.expr().iter().enumerate() {
+            if i != filtered_col && e.expr.as_any().downcast_ref::<Column>().is_none() {
+                return None;
+            }
+        }
+        let range_exec = projection.input().as_any().downcast_ref::<RangeManipulateExec>()?;
+        if range_exec.field_columns().len() != 1 || range_exec.range() <= 0 {
+            return None;
+        }
+        let child = range_exec.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let params = child.params();
+        if params.histogram.is_some() || (params.aggregate.is_some() && !params.by_columns.is_empty()) {
+            return None;
+        }
+        let (param0, param1) = scalar_params(&function, udf.args())?;
+        Some(GpuPromSubquerySpec {
+            function,
+            start: range_exec.start(),
+            end: range_exec.end(),
+            interval: range_exec.interval(),
+            range: range_exec.range(),
+            param0,
+            param1,
+            child: params.clone(),
+        })
     }
 
     /// `ProjectionExec | FilterExec <- HashJoinExec(Inner, tags.. + ts)` over two `GpuPromRangeExec` -> the arguments of
