@@ -6,7 +6,8 @@
 #pragma once
 #include <cstdint>
 
-#include "b2p_kernels.cuh"
+#include "b2p_status.cuh"
+#include "b2p_window.cuh"
 
 namespace b2p {
 

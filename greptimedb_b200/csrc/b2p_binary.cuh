@@ -24,14 +24,14 @@
 #pragma once
 #include <cstdint>
 
-#include "b2p_kernels.cuh"
+#include "b2p_status.cuh"
+#include "b2p_window.cuh"
 
 namespace b2p {
 
 enum BinOp { kOpAdd = 0, kOpSub, kOpMul, kOpDiv, kOpMod, kOpPow, kOpAtan2, kOpEq, kOpNe, kOpGt, kOpLt, kOpGe, kOpLe, kOpCount };
 enum BinMode { kArith = 0, kFilter = 1, kBool = 2 };
 enum BinForm { kVecVec = 0, kScalarLeft = 1, kScalarRight = 2 };
-constexpr uint32_t kBinRowError = 4u;  // Status::k0_errors bit: a pair's row index >= the operand's row count
 
 struct BinaryArgs {
   const double* lhs;        // vector-vector: lhs grid; scalar forms: the vector operand

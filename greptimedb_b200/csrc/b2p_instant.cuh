@@ -31,7 +31,8 @@
 #pragma once
 #include <cstdint>
 
-#include "b2p_kernels.cuh"
+#include "b2p_status.cuh"
+#include "b2p_window.cuh"
 
 namespace b2p {
 
@@ -40,8 +41,6 @@ enum InstantFn {
   kFnAtan, kFnSinh, kFnCosh, kFnTanh, kFnAsinh, kFnAcosh, kFnAtanh, kFnRound, kFnDeg, kFnRad, kFnSgn, kFnClamp,
   kFnKernelCount  // clamp_min / clamp_max (ids kFnClamp + 1, + 2) run as kFnClamp
 };
-constexpr uint32_t kScalarKeyError = 16u;      // Status::k0_errors bit: a row key >= n_rows and not B2P_NO_KEY
-constexpr uint32_t kScalarOverlapError = 32u;  // Status::k0_errors bit: two rows of one key have a cell at one step
 constexpr uint32_t kScalarNoKey = 0xFFFFFFFFu;
 
 struct InstantFnArgs {

@@ -1,0 +1,1188 @@
+// b2p_range.cu — range-query entry points of the C ABI: the range tiers (first tier, warp per series, long windows,
+// exact slow path) and their completion in b2p_sync, series offsets, range_eval (device columns, and host columns
+// through the chunked copy pipeline and the host timestamp scan), prom_* UDF calls, the instant selector, the fused and
+// all-reduced sum by, subqueries and the synthetic data generator.
+#include <algorithm>
+#include <atomic>
+#include <cstring>
+#include <memory>
+#include <string>
+#include <thread>
+#include <vector>
+
+#include <cub/device/device_scan.cuh>
+
+#include "b2p_runtime.cuh"
+#include "b2p_subquery.cuh"
+#include "b2p_kernel_t.cuh"
+#include "b2p_kernel_lean.cuh"
+#include "b2p_kernels.cuh"
+
+using namespace b2p;
+
+namespace {
+
+constexpr int kRing = 256;
+constexpr int kBigRing = 1024;        // long-window instantiation of the warp-per-series kernel (one CTA per SM)
+constexpr int kSlowCtas = 132;        // slow-path grid (4 warps per CTA): one CTA per SM of an H100
+constexpr int kSlowWarps = kSlowCtas * 4;
+constexpr size_t kArenaDefaultRows = 1u << 21;  // 32 MB: regions of 3 971 rows for the 528 slow-path warps
+
+void stage_begin_on(b2p_ctx* c, int stage, cudaStream_t s) { cudaEventRecord(c->ev[stage][0], s); }
+void stage_end_on(b2p_ctx* c, int stage, cudaStream_t s) {
+  cudaEventRecord(c->ev[stage][1], s);
+  c->ev_used[stage] = true;
+}
+
+// rate / increase / delta: the functions of the thread tier and of the fused by-label first tier
+constexpr bool rate_like(int fn) { return fn == B2P_FN_RATE || fn == B2P_FN_INCREASE || fn == B2P_FN_DELTA; }
+
+template <int FN, bool TS32>
+int launch_fast_t(b2p_ctx* c, const RangeArgs& a) {
+  constexpr size_t smem = (size_t)kWarpsPerCta * (2 * kRing * (8 + (TS32 ? 4 : 8)) + kRing / 8) + kRcpTable * 8;
+  auto kern = range_fast_kernel<FN, kRing, TS32>;
+  unsigned grid = 0;
+  if (int rc = persistent_grid(c, kern, smem, kWarpsPerCta, a.n_series, &grid)) return rc;
+  if (grid == 0) return B2P_OK;
+  kern<<<grid, kWarpsPerCta * 32, smem, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// Long-window instantiation (32-bit time domain only): RING = kBigRing, one CTA per SM, over RangeArgs::b_list.
+template <int FN>
+int launch_big(b2p_ctx* c, const RangeArgs& a0) {
+  RangeArgs a = a0;
+  a.use_w_list = 2;
+  constexpr size_t smem = (size_t)kWarpsPerCta * (2 * kBigRing * (8 + 4) + kBigRing / 8) + kRcpTable * 8;
+  auto kern = range_fast_kernel<FN, kBigRing, true>;
+  unsigned grid = 0;  // the length of b_list is known on the device only
+  if (int rc = persistent_grid(c, kern, smem, kWarpsPerCta, kAllResident, &grid)) return rc;
+  kern<<<grid, kWarpsPerCta * 32, smem, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// 32-bit relative timestamps when the whole query span (plus one lookback) fits 31 bits of ms.
+bool fits_ts32(const RangeArgs& a) {
+  const double span = (double)a.end - (double)a.start + (double)a.range;
+  return span >= 0 && span < 2147483000.0 && a.interval < 2147483000ll && a.range < 2147483000ll;
+}
+
+// Adaptive tiering verdict of a finished range call that started with K2L: more than half of the series handed on ->
+// the next 32 calls of this function use the next mode (plain -> bit words for rate / increase -> skip).
+void lean_verdict(b2p_ctx* c, int fn, uint64_t handed, uint64_t n_series) {
+  if (!c->lean_adaptive || handed * 2 <= n_series) return;
+  const bool counter = (fn == B2P_FN_RATE || fn == B2P_FN_INCREASE);
+  c->lean_mode[fn] = (c->last_lean_mode == 0 && counter) ? 1 : 2;
+  c->lean_backoff[fn] = 32;
+}
+
+bool lean_supported(int fn) {
+  bool supported = false;
+  if (fn >= 0 && fn < B2P_FN__COUNT)
+    with_fn(fn, [&](auto k) { supported = LeanTraits<decltype(k)::value>::kSupported; return B2P_OK; });
+  return supported;
+}
+
+// Lean first tier (K2L): rate / increase / delta in the 32-bit time domain.  The gates are what the kernel
+// relies on: exact reciprocal division by range/1000, range >= interval (steps evaluated before the end of a
+// series are below the trimmed end), start >= 0 (truncating division == floor in the end trim), and window
+// ends of the 31 steps past the grid still below the 0xFFFFFFFF end sentinel.
+bool lean_ok(const b2p_ctx* c, int fn, const RangeArgs& a) {
+  if (!c->lean_tier || !lean_supported(fn)) return false;
+  if (!fits_ts32(a) || a.range < a.interval || a.start < 0) return false;
+  if (fn == B2P_FN_RATE && a.rcp_rs == 0.0) return false;
+  return (double)a.rel_max + 64.0 * (double)a.interval < 4294967295.0;
+}
+
+template <int FN>
+int launch_fast(b2p_ctx* c, const RangeArgs& a) {
+  return fits_ts32(a) ? launch_fast_t<FN, true>(c, a) : launch_fast_t<FN, false>(c, a);
+}
+
+// Functions whose first tier has a uniform-cadence variant: the probe (or B2P_UNIFORM) writes Status::uniform, then
+// both variants are launched and the one the verdict does not name returns at once — no host round trip.
+static int cadence_verdict(b2p_ctx* c, const RangeArgs& a) {
+  if (c->uniform_mode < 0) {
+    cadence_probe_kernel<<<1, kProbeThreads, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+  } else {
+    CU(cudaMemsetAsync(&a.status->uniform, c->uniform_mode ? 1 : 0, sizeof(uint32_t), c->stream));
+  }
+  return B2P_OK;
+}
+
+template <int FN, bool FLAGS, bool UNI>
+int launch_lean_variant(b2p_ctx* c, const RangeArgs& a) {
+  constexpr size_t smem = lean_smem_bytes(UNI);
+  auto kern = range_lean_kernel<FN, FLAGS, false, UNI>;
+  unsigned grid = 0;
+  if (int rc = persistent_grid(c, kern, smem, kLeanWarps, a.n_series, &grid)) return rc;
+  if (grid == 0) return B2P_OK;
+  kern<<<grid, kLeanWarps * 32, smem, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+template <int FN, bool FLAGS>
+int launch_lean(b2p_ctx* c, const RangeArgs& a) {
+  if constexpr (kLeanUniform<FN, FLAGS>) {
+    int rc = cadence_verdict(c, a);
+    if (!rc && c->uniform_mode != 0) rc = launch_lean_variant<FN, FLAGS, true>(c, a);
+    if (!rc && c->uniform_mode != 1) rc = launch_lean_variant<FN, FLAGS, false>(c, a);
+    return rc;
+  } else {
+    return launch_lean_variant<FN, FLAGS, false>(c, a);
+  }
+}
+
+// `with_flags`: the variant whose ring carries the reset / change bit words (always for resets() / changes(); for
+// rate / increase when the adaptive policy picked it; never for the other functions).
+template <int FN>
+int launch_lean_if_supported(b2p_ctx* c, const RangeArgs& a, bool with_flags) {
+  if constexpr (!LeanTraits<FN>::kSupported) {
+    return fail(B2P_E_INVALID, "fn_id %d has no lean tier", FN);
+  } else if constexpr (LeanTraits<FN>::kNeedsFlags) {
+    return launch_lean<FN, true>(c, a);
+  } else if constexpr (LeanTraits<FN>::kHasFlagsVariant) {
+    return with_flags ? launch_lean<FN, true>(c, a) : launch_lean<FN, false>(c, a);
+  } else {
+    return launch_lean<FN, false>(c, a);
+  }
+}
+
+// First tier of the fused by-label SUM: rate / increase / delta walk the series group by group and add into
+// gsum / gcnt (range_lean_kernel<FN, FLAGS, GROUPED = true>).
+template <int FN, bool FLAGS, bool UNI>
+int launch_lean_grouped_variant(b2p_ctx* c, const RangeArgs& a) {
+  constexpr size_t smem = lean_grouped_smem_bytes(UNI);
+  auto kern = range_lean_kernel<FN, FLAGS, true, UNI>;
+  unsigned cap = 0;
+  if (int rc = persistent_grid(c, kern, smem, kLeanWarps, kAllResident, &cap)) return rc;
+  const unsigned n_g = a.g_hi - a.g_lo;
+  const unsigned need = (n_g + kLeanWarps - 1) / kLeanWarps;
+  // The grid is one CTA per SM and takes its groups from a counter, so it can be any size: while tiles are being
+  // all-reduced a few SMs are left to the collective's CTAs (they cannot be placed beside a resident 24-warp CTA).
+  if (c->comm_reserve_now > 0 && cap > (unsigned)c->comm_reserve_now + 8u) cap -= (unsigned)c->comm_reserve_now;
+  const unsigned grid = need < cap ? need : cap;
+  if (grid == 0) return B2P_OK;
+  kern<<<grid, kLeanWarps * 32, smem, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+template <int FN, bool FLAGS>
+int launch_lean_grouped(b2p_ctx* c, const RangeArgs& a) {
+  if constexpr (kLeanUniform<FN, FLAGS>) {
+    int rc = cadence_verdict(c, a);
+    if (!rc && c->uniform_mode != 0) rc = launch_lean_grouped_variant<FN, FLAGS, true>(c, a);
+    if (!rc && c->uniform_mode != 1) rc = launch_lean_grouped_variant<FN, FLAGS, false>(c, a);
+    return rc;
+  } else {
+    return launch_lean_grouped_variant<FN, FLAGS, false>(c, a);
+  }
+}
+template <int FN>
+int launch_lean_grouped_if_supported(b2p_ctx* c, const RangeArgs& a, bool with_flags) {
+  if constexpr (!rate_like(FN)) {
+    return fail(B2P_E_INVALID, "fn_id %d has no fused by-label tier", FN);
+  } else if constexpr (LeanTraits<FN>::kHasFlagsVariant) {
+    return with_flags ? launch_lean_grouped<FN, true>(c, a) : launch_lean_grouped<FN, false>(c, a);
+  } else {
+    return launch_lean_grouped<FN, false>(c, a);
+  }
+}
+
+template <int FN>
+int launch_thread_tier(b2p_ctx* c, const RangeArgs& a) {
+  if constexpr (!rate_like(FN)) {
+    return fail(B2P_E_INVALID, "fn_id %d has no thread tier", FN);
+  } else {
+    // at most the 1-warp CTAs whose rings fit in shared memory
+    const unsigned grid = capped_grid(c, a.n_series, 32, 220 * 1024 / (kTRing * 32 * 12 + 512));
+    if (grid == 0) return B2P_OK;
+    range_thread_kernel<FN><<<grid, 32, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    return B2P_OK;
+  }
+}
+
+template <int FN>
+int launch_slow(b2p_ctx* c, const RangeArgs& a) {
+  range_slow_kernel<FN><<<kSlowCtas, 128, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+int dispatch_slow(b2p_ctx* c, int fn, const RangeArgs& a) {
+  return with_fn(fn, [&](auto k) { return launch_slow<decltype(k)::value>(c, a); });
+}
+
+// The window and time-domain fields of a range call over T steps (check_grid has accepted p); the first tier's gates
+// (lean_ok) read them.
+RangeArgs range_geometry(const b2p_range_params* p, int64_t T) {
+  RangeArgs a{};
+  a.start = p->start; a.end = p->end; a.interval = p->interval; a.range = p->range;
+  a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
+  a.tb = p->start - p->range;
+  if (fits_ts32(a)) a.rel_max = (uint32_t)(p->range + (T - 1) * p->interval + 1);
+  // exact two-FMA division by range/1000 needs RN(1/b) and a significand that is not all ones
+  const double rs = (double)p->range / 1000.0;
+  uint64_t bits;
+  memcpy(&bits, &rs, 8);
+  const bool all_ones = (bits & 0x000fffffffffffffull) == 0x000fffffffffffffull;
+  a.rcp_rs = (p->range > 0 && !all_ones) ? 1.0 / rs : 0.0;
+  a.range_secs = rs;
+  a.rcp_interval = 1.0 / (double)p->interval;
+  a.start_mod = p->start >= 0 ? (uint32_t)(p->start % p->interval) : 0u;
+  return a;
+}
+
+int ensure_slow_scratch(b2p_ctx* c, uint32_t n_series, int64_t T) {
+  int rc;
+  if ((rc = c->slow_list.ensure((size_t)(n_series ? n_series : 1) * 4))) return rc;
+  if ((rc = c->w_list.ensure((size_t)(n_series ? n_series : 1) * 4))) return rc;
+  if ((rc = c->b_list.ensure((size_t)(n_series ? n_series : 1) * 4))) return rc;
+  if ((rc = c->win_scratch.ensure((size_t)kSlowWarps * (size_t)(T > 0 ? T : 1) * 8))) return rc;
+  if (c->arena_rows == 0) {
+    const size_t rows = c->arena_rows_wanted > kArenaDefaultRows ? c->arena_rows_wanted : kArenaDefaultRows;
+    if ((rc = c->arena_ts.ensure(rows * 8))) return rc;
+    if ((rc = c->arena_val.ensure(rows * 8))) return rc;
+    c->arena_rows = rows;
+  }
+  return B2P_OK;
+}
+
+}  // namespace
+
+int check_grid(const b2p_range_params* p, uint32_t n_series, int64_t* T_out) {
+  if (!p) return fail(B2P_E_INVALID, "params is NULL");
+  if (p->interval <= 0) return fail(B2P_E_INVALID, "interval must be > 0 (got %lld)", (long long)p->interval);
+  if (p->range < 0) return fail(B2P_E_INVALID, "range must be >= 0");
+  if (p->fn_id < 0 || p->fn_id >= B2P_FN__COUNT) return fail(B2P_E_INVALID, "unknown fn_id %d", p->fn_id);
+  const int64_t T = b2p_num_steps(p->start, p->end, p->interval);
+  if (T > (int64_t)0x7fffff00) return fail(B2P_E_TOO_LARGE, "%lld eval steps: trim [start,end] to the data extent first", (long long)T);
+  if ((double)T * (double)n_series > 1.0e12) return fail(B2P_E_TOO_LARGE, "dense grid %lld x %u too large", (long long)T, n_series);
+  *T_out = T;
+  return B2P_OK;
+}
+
+// The thread tier's reciprocal table is a __constant__ of b2p_kernel_t.cuh, so it exists in this module only, where
+// range_thread_kernel is launched; b2p_create fills it through this function.
+int upload_rcp_table() {
+  double tab[kRcpTable];
+  tab[0] = 0.0;
+  for (int i = 1; i < kRcpTable; ++i) tab[i] = 1.0 / (double)i;
+  if (cudaMemcpyToSymbol(c_rcp_table, tab, sizeof tab) != cudaSuccess)
+    return fail(B2P_E_CUDA, "constant table upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+  return B2P_OK;
+}
+
+extern "C" {
+
+__global__ void comm_marker_kernel() {}
+// holds the compute stream back for a few microseconds so that the all-reduce released at the same instant on the
+// communication stream has its CTAs placed before the persistent range kernel asks for every SM
+__global__ void comm_headstart_kernel(long long cycles) {
+  const long long t0 = clock64();
+  while (clock64() - t0 < cycles) {}
+}
+
+// Launches every tier of one range call (first tier when `used_lean`/`thread_tier`, warp-per-series kernel, its
+// long-window instantiation, exact slow kernel) on the context's stream.
+static int launch_range_tiers(b2p_ctx* c, int fn, RangeArgs a, bool thread_tier, bool used_lean, int lean_mode,
+                              bool later_tile = false) {
+  int rc;
+  if (!later_tile) {
+    CU(cudaMemsetAsync(a.status, 0, sizeof(Status), c->stream));
+  } else {  // a further tile of the same fused call: new work lists, same verdict (overflow / arena fields stay)
+    CU(cudaMemsetAsync(&a.status->slow_count, 0, sizeof(uint32_t), c->stream));
+    CU(cudaMemsetAsync(&a.status->w_count, 0, 3 * sizeof(uint32_t), c->stream));  // w_count, b_count, g_next
+  }
+  stage_begin(c, 1);
+  if (thread_tier || used_lean) {
+    rc = with_fn(fn, [&](auto k) {
+      constexpr int FN = decltype(k)::value;
+      if (thread_tier) return launch_thread_tier<FN>(c, a);
+      return a.gsum ? launch_lean_grouped_if_supported<FN>(c, a, lean_mode == 1)
+                    : launch_lean_if_supported<FN>(c, a, lean_mode == 1);
+    });
+    if (rc) return rc;
+    a.use_w_list = 1;
+  }
+  rc = with_fn(fn, [&](auto k) {
+    constexpr int FN = decltype(k)::value;
+    const int r = launch_fast<FN>(c, a);
+    return (r || !a.b_list) ? r : launch_big<FN>(c, a);
+  });
+  stage_end(c, 1);
+  if (rc) return rc;
+  stage_begin(c, 2);
+  rc = dispatch_slow(c, fn, a);
+  stage_end(c, 2);
+  return rc;
+}
+
+int b2p_sync(b2p_ctx* c) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  DeviceGuard g(c->device);
+  for (int attempt = 0; attempt < 4; ++attempt) {
+    CU(cudaMemcpyAsync(c->h_ring, c->d_ring, kStatusSlots * sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(c->h_k0, c->d_k0, sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    const uint32_t k0 = c->h_k0->k0_errors;
+    if (k0) {
+      CU(cudaMemsetAsync(c->d_k0, 0, sizeof(Status), c->stream));
+      c->pending.clear();
+      return k0_fail(k0);
+    }
+    // verdicts of the outstanding range calls, oldest first; a call whose slow path ran out of arena is redone
+    // as a whole (all tiers, same modes) after the arena has grown to what the largest of them needs
+    size_t need = 0;
+    std::vector<b2p_ctx::Pending> redo;
+    for (auto& pc : c->pending) {
+      const Status st = c->h_ring[pc.slot];
+      c->last_slow = st.slow_count;
+      c->last_w = st.w_count;
+      if (pc.used_lean && !pc.verdict_taken) {
+        c->last_lean_mode = pc.lean_mode;
+        lean_verdict(c, pc.fn, st.w_count, pc.n_series);
+        pc.verdict_taken = true;
+      }
+      if (st.arena_overflow) {
+        if ((size_t)st.arena_needed + 1024 > need) need = (size_t)st.arena_needed + 1024;
+        redo.push_back(pc);
+      }
+    }
+    c->pending.clear();
+    c->fused_pending = false;
+    if (redo.empty()) return B2P_OK;
+    int rc;
+    if ((rc = c->arena_ts.ensure(need * 8))) return rc;
+    if ((rc = c->arena_val.ensure(need * 8))) return rc;
+    c->arena_rows = need;
+    for (auto& pc : redo) {
+      pc.args.arena_ts = c->arena_ts.as<int64_t>();
+      pc.args.arena_val = c->arena_val.as<double>();
+      pc.args.arena_cap = need;
+      if (pc.merged)
+        return fail(B2P_E_TOO_LARGE, "a series of %llu+ rows needs the exact slow path but does not fit its arena region; "
+                    "the merged partials are incomplete — set B2P_ARENA_ROWS >= %zu and repeat the query",
+                    (unsigned long long)(need / (size_t)kSlowWarps), need);
+      if (pc.fused) {
+        // partials were added in place: only the slow kernel runs again, over its intact work list (a series that
+        // did not fit the arena added nothing); no other range call was admitted while this one was outstanding
+        Status patch = c->h_ring[pc.slot];
+        patch.arena_overflow = 0; patch.arena_used = 0; patch.arena_needed = 0;
+        c->h_ring[pc.slot] = patch;
+        CU(cudaMemcpyAsync(c->d_ring + pc.slot, c->h_ring + pc.slot, sizeof(Status), cudaMemcpyHostToDevice, c->stream));
+        if ((rc = dispatch_slow(c, pc.fn, pc.args))) return rc;
+        c->pending.push_back(pc);
+        CU(cudaStreamSynchronize(c->stream));
+        continue;
+      }
+      if ((rc = launch_range_tiers(c, pc.fn, pc.args, pc.thread_tier, pc.used_lean, pc.lean_mode))) return rc;
+      c->pending.push_back(pc);
+      CU(cudaStreamSynchronize(c->stream));  // one redone call at a time: they share the arena from offset 0
+    }
+  }
+  return fail(B2P_E_NOMEM, "slow-path arena could not be sized");
+}
+
+/* ---- device-pointer API ---------------------------------------------------------------------- */
+
+static int series_offsets_impl(b2p_ctx* c, const uint32_t* sid, uint64_t n_rows, uint32_t n_series, uint32_t sid_base,
+                               uint64_t* offsets);
+
+int b2p_series_offsets_dev(b2p_ctx* c, const uint32_t* sid, uint64_t n_rows, uint32_t n_series, uint64_t* offsets) {
+  return series_offsets_impl(c, sid, n_rows, n_series, 0u, offsets);
+}
+
+static int series_offsets_impl(b2p_ctx* c, const uint32_t* sid, uint64_t n_rows, uint32_t n_series, uint32_t sid_base,
+                               uint64_t* offsets) {
+  if (!c || !offsets || (!sid && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
+  if (!aligned16(sid)) return fail(B2P_E_INVALID, "sid must be 16-byte aligned");
+  DeviceGuard g(c->device);
+  unsigned blocks = capped_grid(c, n_rows / 16, 256, 16);
+  if (blocks == 0) blocks = 1;
+  stage_begin(c, 0);
+  series_offsets_kernel<<<blocks, 256, 0, c->stream>>>(sid, n_rows, n_series, sid_base, offsets, c->d_k0);
+  c->launches++;
+  stage_end(c, 0);
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// Target of a fused by-label SUM / COUNT (b2p_range_group_sum*_dev): groups [g_lo, g_hi) of an index.
+struct GroupTarget {
+  const b2p_group_index* idx;
+  uint32_t g_lo, g_hi;
+  double* gsum;
+  uint32_t* gcnt;
+  // > 0: the group range is processed in this many tiles and every tile's rows of gsum / gcnt are all-reduced over
+  // the context's communicator as soon as the tile is complete, on the (high-priority) communication stream, while
+  // the next tile computes
+  int allreduce_tiles;
+};
+
+// Can this range call add its results straight into by-label partials?  (first tier available for the function and
+// the query shape, and not switched off by the adaptive policy; groups balanced enough for group-exclusive warps)
+static bool fused_group_ok(b2p_ctx* c, const b2p_range_params* p, int64_t T, const b2p_group_index* idx) {
+  if (!rate_like(p->fn_id) || c->thread_tier) return false;
+  if (T > 32 * (int64_t)kLeanFullWords) return false;  // per-warp word counters of the first tier
+  if (!lean_ok(c, p->fn_id, range_geometry(p, T))) return false;
+  if (c->lean_backoff[p->fn_id] > 0 && c->lean_mode[p->fn_id] == 2) return false;
+  // a group is walked by ONE warp: the largest group may not exceed a few times a warp's fair share
+  const uint64_t warps = (uint64_t)c->num_sms * B2P_LEAN_MIN_BLOCKS * kLeanWarps;
+  const uint64_t share = idx->n_series / warps + 1;
+  return (uint64_t)idx->max_members <= 8 * share + 64;
+}
+
+static int range_call(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
+                      const uint64_t* offsets, uint64_t n_rows, uint32_t n_series, double* out, uint32_t* valid_words,
+                      const GroupTarget* gt);
+
+int b2p_range_eval_dev(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
+                       const uint64_t* offsets, uint64_t n_rows, uint32_t n_series, double* out,
+                       uint32_t* valid_words) {
+  return range_call(c, p, ts, val, offsets, n_rows, n_series, out, valid_words, nullptr);
+}
+
+static int range_call(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
+                      const uint64_t* offsets, uint64_t n_rows, uint32_t n_series, double* out, uint32_t* valid_words,
+                      const GroupTarget* gt) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int64_t T = 0;
+  int rc = check_grid(p, n_series, &T);
+  if (rc) return rc;
+  if (n_series == 0 || T == 0) return B2P_OK;
+  if (!offsets || (!gt && (!out || !valid_words)) || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
+  if (!aligned16(ts) || !aligned16(val)) return fail(B2P_E_INVALID, "ts/val must be 16-byte aligned");
+  DeviceGuard g(c->device);
+  if ((rc = ensure_slow_scratch(c, n_series, T))) return rc;
+  RangeArgs a = range_geometry(p, T);
+  a.offset = p->offset; a.p0 = p->param0; a.p1 = p->param1; a.filter_nan = p->filter_nan;
+  a.ts = ts; a.val = val; a.offsets = offsets; a.n_rows = n_rows; a.n_series = n_series;
+  a.out = out; a.valid = valid_words;
+  // a fused call keeps the work lists until its verdict is in: nothing else is admitted before that
+  if (c->fused_pending && (rc = b2p_sync(c))) return rc;
+  if (gt) {
+    if (!c->pending.empty() && (rc = b2p_sync(c))) return rc;
+    const size_t ns = n_series;
+    if ((rc = c->w_skip.ensure(ns * 4)) || (rc = c->b_skip.ensure(ns * 4)) || (rc = c->slow_skip.ensure(ns * 4))) return rc;
+    a.gsum = gt->gsum; a.gcnt = gt->gcnt; a.gid = gt->idx->gid; a.g_off = gt->idx->goff; a.g_members = gt->idx->members;
+    a.n_groups = gt->idx->n_groups; a.g_lo = gt->g_lo; a.g_hi = gt->g_hi;
+    a.w_skip = c->w_skip.as<uint32_t>(); a.b_skip = c->b_skip.as<uint32_t>(); a.slow_skip = c->slow_skip.as<uint32_t>();
+  }
+  // every call owns a status slot until b2p_sync has read it; with all slots taken the library synchronises itself
+  if ((int)c->pending.size() >= kStatusSlots && (rc = b2p_sync(c))) return rc;
+  const int slot = c->next_slot;
+  c->next_slot = (c->next_slot + 1) % kStatusSlots;
+  a.status = c->d_ring + slot; a.slow_list = c->slow_list.as<uint32_t>();
+  a.w_list = c->w_list.as<uint32_t>();
+  a.b_list = fits_ts32(a) ? c->b_list.as<uint32_t>() : nullptr;  // long windows: the 1024-sample ring (32-bit domain)
+  a.use_w_list = 0;
+  a.arena_ts = c->arena_ts.as<int64_t>(); a.arena_val = c->arena_val.as<double>(); a.arena_cap = c->arena_rows;
+  a.win_scratch = c->win_scratch.as<unsigned long long>();
+  // tier 1 (rate / increase / delta, 32-bit time domain): thread per series (opt-in) or the lean warp-per-series
+  // kernel; what it declines goes to tier 2 (warp per series) through w_list, long windows from there to the
+  // 1024-sample instantiation through b_list, and what that declines to the exact slow kernel
+  const bool tier1 = c->thread_tier && fits_ts32(a) && rate_like(p->fn_id);
+  bool used_lean = false;
+  int mode = 0;
+  if (!tier1 && lean_ok(c, p->fn_id, a)) {
+    if (c->lean_backoff[p->fn_id] > 0) {
+      c->lean_backoff[p->fn_id]--;
+      mode = c->lean_mode[p->fn_id];
+    }
+    if (mode != 2) used_lean = true;
+    if (mode == 0 && c->lean_force_flags) mode = 1;
+  }
+  if (gt && !used_lean) return fail(B2P_E_INVALID, "fused by-label call without its first tier (internal)");
+  c->last_lean_mode = mode;
+  c->last_used_lean = used_lean;
+  c->last_range_series = n_series;
+  c->last_range_fn = p->fn_id;
+  if (gt && gt->allreduce_tiles > 0) {
+    if (!c->comm && c->comm_ranks > 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
+    const uint32_t n_t = (uint32_t)gt->allreduce_tiles;
+    const uint64_t span = (uint64_t)gt->g_hi - gt->g_lo;
+    c->comm_reserve_now = (c->comm && n_t > 1) ? c->comm_reserve_sms : 0;
+    for (uint32_t t = 0; t < n_t; ++t) {
+      a.g_lo = gt->g_lo + (uint32_t)(span * t / n_t);
+      a.g_hi = gt->g_lo + (uint32_t)(span * (t + 1) / n_t);
+      if (a.g_hi == a.g_lo) continue;
+      if ((rc = launch_range_tiers(c, p->fn_id, a, tier1, used_lean, mode, t > 0))) return rc;
+      if (c->comm) {
+        const size_t off = (size_t)a.g_lo * (size_t)T, cnt_n = (size_t)(a.g_hi - a.g_lo) * (size_t)T;
+        CU(cudaEventRecord(c->ev_comm_in, c->stream));
+        CU(cudaStreamWaitEvent(c->s_comm, c->ev_comm_in, 0));
+        // The next tile's kernels are released by a marker that sits directly IN FRONT of the all-reduce on the
+        // communication stream: when they become runnable the (few) NCCL CTAs are already next in line on the
+        // high-priority stream and get their SMs first; the persistent first-tier kernel fills what is left and its
+        // dynamic group counter keeps late CTAs from becoming a tail.
+        comm_marker_kernel<<<1, 32, 0, c->s_comm>>>();
+        CU(cudaEventRecord(c->ev_comm_go, c->s_comm));
+        CU(cudaStreamWaitEvent(c->stream, c->ev_comm_go, 0));
+        if (c->comm_headstart_cycles > 0) comm_headstart_kernel<<<1, 32, 0, c->stream>>>(c->comm_headstart_cycles);
+        stage_begin_on(c, 4, c->s_comm);
+        NCCL_TRY(g_nccl.GroupStart());
+        NCCL_TRY(g_nccl.AllReduce(a.gsum + off, a.gsum + off, cnt_n, Nccl::kFloat64, Nccl::kSum, c->comm, c->s_comm));
+        NCCL_TRY(g_nccl.AllReduce(a.gcnt + off, a.gcnt + off, cnt_n, Nccl::kUint32, Nccl::kSum, c->comm, c->s_comm));
+        NCCL_TRY(g_nccl.GroupEnd());
+        stage_end_on(c, 4, c->s_comm);
+      }
+    }
+    c->comm_reserve_now = 0;
+    if (c->comm) {  // everything after this call on the context's stream sees the merged partials
+      CU(cudaEventRecord(c->ev_comm_done, c->s_comm));
+      CU(cudaStreamWaitEvent(c->stream, c->ev_comm_done, 0));
+    }
+    a.g_lo = gt->g_lo; a.g_hi = gt->g_hi;
+  } else if ((rc = launch_range_tiers(c, p->fn_id, a, tier1, used_lean, mode))) {
+    return rc;
+  }
+  b2p_ctx::Pending pc{};
+  pc.slot = slot; pc.fn = p->fn_id; pc.args = a; pc.lean_mode = mode; pc.thread_tier = tier1; pc.used_lean = used_lean;
+  pc.n_series = n_series; pc.verdict_taken = false; pc.fused = gt != nullptr;
+  pc.merged = gt && gt->allreduce_tiles > 0;
+  c->pending.push_back(pc);
+  if (gt) c->fused_pending = true;
+  return B2P_OK;
+}
+
+int b2p_range_udf_dev(b2p_ctx* c, int32_t fn_id, const int64_t* ts, const double* val, uint64_t n_rows,
+                      const int64_t* packed_ranges, const int64_t* eval_ts, uint64_t n_win, int64_t range_length,
+                      double param0, double param1, double* out, uint8_t* valid) {
+  (void)n_rows;
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_win == 0) return B2P_OK;
+  if (!packed_ranges || !out || !valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  stage_begin(c, 1);
+  const int rc = with_fn(fn_id, [&](auto k) {
+    range_udf_kernel<decltype(k)::value><<<capped_grid(c, n_win, 128, 32), 128, 0, c->stream>>>(
+        ts, val, packed_ranges, eval_ts, n_win, range_length, param0, param1, out, valid);
+    c->launches++;
+    CU(cudaGetLastError());
+    return B2P_OK;
+  });
+  stage_end(c, 1);
+  return rc;
+}
+
+int b2p_instant_select_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
+                           const int64_t* ts, const double* val, const uint64_t* offsets, uint64_t n_rows,
+                           uint32_t n_series, double* out, uint32_t* valid_words) {
+  (void)n_rows;
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  b2p_range_params p{};
+  p.start = start; p.end = end; p.interval = interval; p.range = lookback;
+  int64_t T = 0;
+  int rc = check_grid(&p, n_series, &T);
+  if (rc) return rc;
+  if (n_series == 0 || T == 0) return B2P_OK;
+  if (!offsets || !out || !valid_words) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  InstantArgs a{};
+  a.start = start; a.end = end; a.interval = interval; a.lookback = lookback; a.offset = offset;
+  a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
+  a.ts = ts; a.val = val; a.offsets = offsets; a.n_series = n_series; a.out = out; a.valid = valid_words;
+  stage_begin(c, 1);
+  instant_kernel<<<capped_grid(c, n_series, kWarpsPerCta, 8), kWarpsPerCta * 32, 0, c->stream>>>(a);
+  c->launches++;
+  stage_end(c, 1);
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// sum by (..)(fn(..)) partials of groups [g_lo, g_hi) added into out_sum / out_cnt [n_groups x T].
+// Fused (no [n_series x T] intermediate) for rate / increase / delta whenever the first tier applies; otherwise the
+// range function is evaluated into context scratch and folded by the by-label kernel (two passes, synchronous).
+int b2p_range_group_sum_indexed_dev(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
+                                    const uint64_t* offsets, uint64_t n_rows, uint32_t n_series,
+                                    const b2p_group_index* ix, uint32_t g_lo, uint32_t g_hi, double* out_sum,
+                                    uint32_t* out_cnt) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_series != n_series) return fail(B2P_E_INVALID, "group index was built for %u series, call has %u", ix->n_series, n_series);
+  if (g_hi > ix->n_groups) g_hi = ix->n_groups;
+  int64_t T = 0;
+  int rc = check_grid(p, n_series, &T);
+  if (rc) return rc;
+  if (n_series == 0 || T == 0 || g_lo >= g_hi) return B2P_OK;
+  if (!out_sum || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  if (fused_group_ok(c, p, T, ix)) {
+    GroupTarget gt{ix, g_lo, g_hi, out_sum, out_cnt, 0};
+    return range_call(c, p, ts, val, offsets, n_rows, n_series, nullptr, nullptr, &gt);
+  }
+  if (g_lo != 0 || g_hi != ix->n_groups)
+    return fail(B2P_E_INVALID, "group ranges need the fused tier (rate / increase / delta in the 32-bit time domain)");
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  if ((rc = c->rg_out.ensure((size_t)n_series * (size_t)T * 8))) return rc;
+  if ((rc = c->rg_valid.ensure((size_t)n_series * Tw * 4))) return rc;
+  if ((rc = b2p_range_eval_dev(c, p, ts, val, offsets, n_rows, n_series, c->rg_out.as<double>(),
+                               c->rg_valid.as<uint32_t>())))
+    return rc;
+  if ((rc = b2p_sync(c))) return rc;  // slow-path fix-ups must land before the aggregate reads
+  stage_begin(c, 3);
+  rc = group_aggregate_csr(c, B2P_AGG_SUM, c->rg_out.as<double>(), c->rg_valid.as<uint32_t>(), ix->goff, ix->members,
+                           ix->n_groups, (uint64_t)T, out_sum, out_cnt, 1);
+  stage_end(c, 3);
+  return rc;
+}
+
+// sum by over all ranks: the fused partials of this rank's series, tile by tile, each tile all-reduced over the
+// communicator while the next one computes.  Falls back to partials + one all-reduce when the call cannot run fused.
+int b2p_range_group_sum_allreduce_dev(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
+                                      const uint64_t* offsets, uint64_t n_rows, uint32_t n_series,
+                                      const b2p_group_index* ix, int32_t n_tiles, double* out_sum, uint32_t* out_cnt) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_series != n_series) return fail(B2P_E_INVALID, "group index was built for %u series, call has %u", ix->n_series, n_series);
+  int64_t T = 0;
+  int rc = check_grid(p, n_series, &T);
+  if (rc) return rc;
+  if (T == 0 || ix->n_groups == 0) return B2P_OK;
+  if (!out_sum || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  if (n_tiles < 1) n_tiles = 1;
+  DeviceGuard g(c->device);
+  if (n_series > 0 && fused_group_ok(c, p, T, ix)) {
+    GroupTarget gt{ix, 0, ix->n_groups, out_sum, out_cnt, n_tiles};
+    return range_call(c, p, ts, val, offsets, n_rows, n_series, nullptr, nullptr, &gt);
+  }
+  if (n_series > 0 &&
+      (rc = b2p_range_group_sum_indexed_dev(c, p, ts, val, offsets, n_rows, n_series, ix, 0, ix->n_groups, out_sum, out_cnt)))
+    return rc;
+  return b2p_allreduce_partials_dev(c, B2P_AGG_SUM, out_sum, out_cnt, nullptr, (uint64_t)ix->n_groups * (uint64_t)T);
+}
+
+int b2p_range_group_sum_fused(b2p_ctx* c, const b2p_range_params* p, const b2p_group_index* ix) {
+  if (!c || !ix || !p || p->interval <= 0) return 0;  // (a grid the range call itself would reject)
+  int64_t T = b2p_num_steps(p->start, p->end, p->interval);
+  return fused_group_ok(c, p, T, ix) ? 1 : 0;
+}
+
+int b2p_range_group_sum_dev(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
+                            const uint64_t* offsets, uint64_t n_rows, uint32_t n_series, const uint32_t* gid,
+                            uint32_t n_groups, double* out_sum, uint32_t* out_cnt) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_series == 0 || n_groups == 0) return B2P_OK;
+  b2p_group_index* ix = nullptr;
+  int rc = b2p_group_index_create_dev(c, gid, n_series, n_groups, &ix);
+  if (rc) return rc;
+  rc = b2p_range_group_sum_indexed_dev(c, p, ts, val, offsets, n_rows, n_series, ix, 0, n_groups, out_sum, out_cnt);
+  if (!rc) rc = b2p_sync(c);  // the temporary index must outlive the kernels that read it
+  b2p_group_index_destroy(c, ix);
+  return rc;
+}
+
+/* ---- subqueries ---------------------------------------------------------------------------------------------- */
+}  // extern "C"
+
+namespace {
+// A range call of this context that reads the subquery scratch and whose verdict b2p_sync has not taken yet: b2p_sync
+// may run it again from the scratch (slow-path arena overflow), so the scratch must not change before that.
+bool subquery_scratch_pending(const b2p_ctx* c) {
+  for (const b2p_ctx::Pending& pc : c->pending)
+    if (pc.args.ts == c->sq_ts.as<int64_t>()) return true;
+  return false;
+}
+
+// Rows are processed in batches of at most kSqBatchCells / T_inner rows (one row when a row alone is larger).  Per
+// batch: K13's count kernel, CUB's exclusive scan of the counts, K13's scatter, then the range call over the batch's
+// sample rows into its rows of out / out_valid.  The range call is given the batch's cell count as its row count: the
+// extent of the scratch, which the tiers only use to bound their paired loads, so the sample total is never read back.
+// A batch waits (b2p_sync) for the verdict of the range call before it, since the scratch is rewritten; so does the
+// first batch for that of an earlier call.  A grid of one batch makes no host round trip.
+// Scratch (context buffers sq_*): 16 B per grid cell of a batch (8 B timestamp, 8 B value: at most 2.1 GB unless one
+// row alone has more than kSqBatchCells steps), 8 B per row of a batch plus one for the offsets, and CUB's scan temp.
+int subquery_run(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval, const double* vals,
+                 const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, int64_t T, double* out, uint32_t* out_valid) {
+  int rc;
+  const uint32_t Tw_in = (uint32_t)((T_inner + 31) / 32), Tw = (uint32_t)((T + 31) / 32);
+  const uint32_t batch_rows = (uint32_t)std::min<uint64_t>(n_rows, std::max<uint64_t>(1, kSqBatchCells / T_inner));
+  const uint64_t cells = (uint64_t)batch_rows * T_inner;
+  size_t scan_bytes = 0;
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                   (int)batch_rows + 1, c->stream));
+  if (subquery_scratch_pending(c) && (rc = b2p_sync(c))) return rc;
+  if ((rc = c->sq_ts.ensure(cells * 8)) || (rc = c->sq_val.ensure(cells * 8)) ||
+      (rc = c->sq_off.ensure(((size_t)batch_rows + 1) * 8)) || (rc = c->sq_tmp.ensure(std::max<size_t>(scan_bytes, 16))))
+    return rc;
+  b2p_range_params q = *p;
+  for (uint32_t r0 = 0; r0 < n_rows; r0 += batch_rows) {
+    const uint32_t nb = std::min(batch_rows, n_rows - r0);
+    if (r0 > 0 && (rc = b2p_sync(c))) return rc;
+    SubqueryArgs a{};
+    a.vals = vals + (uint64_t)r0 * T_inner; a.valid = valid + (uint64_t)r0 * Tw_in;
+    a.T = T_inner; a.Tw = Tw_in; a.rows = nb;
+    a.start = inner_start; a.interval = inner_interval;
+    a.offsets = c->sq_off.as<unsigned long long>(); a.ts = c->sq_ts.as<int64_t>(); a.val = c->sq_val.as<double>();
+    const unsigned grid = std::max(1u, capped_grid(c, (uint64_t)nb * 32, 256, 8));
+    stage_begin(c, 3);
+    subquery_count_kernel<<<grid, 256, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    size_t bytes = c->sq_tmp.cap;
+    CU(cub::DeviceScan::ExclusiveSum(c->sq_tmp.p, bytes, a.offsets, a.offsets, (int)nb + 1, c->stream));
+    subquery_scatter_kernel<<<grid, 256, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    stage_end(c, 3);
+    if ((rc = range_call(c, &q, a.ts, a.val, c->sq_off.as<uint64_t>(), (uint64_t)nb * T_inner, nb,
+                         out + (uint64_t)r0 * T, out_valid + (uint64_t)r0 * Tw, nullptr)))
+      return rc;
+  }
+  return B2P_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_subquery_dev(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval,
+                     const double* vals, const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, double* out,
+                     uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int64_t T = 0;
+  int rc = check_grid(p, n_rows, &T);
+  if (rc) return rc;
+  if (p->range == 0) return fail(B2P_E_INVALID, "subquery: zero range");
+  if (p->offset != 0 || p->filter_nan != 0) return fail(B2P_E_INVALID, "subquery: offset and filter_nan must be 0");
+  if (inner_interval <= 0) return fail(B2P_E_INVALID, "subquery: inner interval must be > 0 (got %lld)", (long long)inner_interval);
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!out || !out_valid || (T_inner && (!vals || !valid))) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  if (T_inner == 0) {  // no inner steps: no samples, no cell
+    CU(cudaMemsetAsync(out, 0, (size_t)n_rows * (size_t)T * 8, c->stream));
+    CU(cudaMemsetAsync(out_valid, 0, (size_t)n_rows * (size_t)((T + 31) / 32) * 4, c->stream));
+    return B2P_OK;
+  }
+  return subquery_run(c, p, inner_start, inner_interval, vals, valid, n_rows, T_inner, T, out, out_valid);
+}
+
+int b2p_synth_fill_dev(b2p_ctx* c, uint64_t series_begin, uint64_t n_series, uint32_t n_samples, int64_t t0,
+                       int64_t scrape_ms, uint32_t jitter_ms, int32_t with_resets, uint64_t seed, int64_t* ts,
+                       double* val, uint32_t* sid) {
+  if (!c || !ts || !val) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const uint64_t total = n_series * (uint64_t)n_samples;
+  if (total == 0) return B2P_OK;
+  synth_fill_kernel<<<capped_grid(c, total, 256, 32), 256, 0, c->stream>>>(series_begin, n_series, n_samples, t0,
+                                                                           scrape_ms, jitter_ms, with_resets, seed, ts,
+                                                                           val, sid);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+/* ---- host-pointer API ------------------------------------------------------------------------ */
+}  // extern "C"
+
+SeriesIn stage_series(Staging& s, const int64_t* ts, const double* val, const uint32_t* sid, uint32_t sid_base,
+                      const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series) {
+  SeriesIn in{s.in(ts, n_rows * 8), s.in(val, n_rows * 8), nullptr};
+  if (offsets_host) {
+    in.offsets = s.in(offsets_host, ((size_t)n_series + 1) * 8);
+  } else {
+    const uint32_t* d_sid = s.in(sid, n_rows * 4);
+    in.offsets = static_cast<uint64_t*>(s.buf(((size_t)n_series + 1) * 8));
+    if (!s.rc) s.rc = series_offsets_impl(s.c, d_sid, n_rows, n_series, sid_base, in.offsets);
+  }
+  return in;
+}
+
+extern "C" {
+
+// Host-side SeriesDivide + cadence scan (see the header).  Plain sequential passes, memory bound;
+// b2p_range_eval runs one of these per chunk on a few worker threads while earlier chunks are on the bus.
+static int host_scan_series(const int64_t* ts, const uint32_t* sid, const uint64_t* offsets_in, uint64_t n_rows,
+                            uint32_t n_series, uint32_t sid_base, uint64_t* offsets_out, int64_t* t0, int64_t* cadence,
+                            int32_t* all_regular) {
+  if (sid) {
+    uint64_t r = 0;
+    uint32_t prev = sid_base;
+    offsets_out[0] = 0;
+    uint32_t next = 0;  // next local series whose start is still to be written (offsets_out[next + 1 ..] pending)
+    for (; r < n_rows; ++r) {
+      const uint32_t id = sid[r];
+      if (id < prev || id - sid_base >= n_series) return B2P_E_UNSORTED;
+      const uint32_t local = id - sid_base;
+      while (next < local) offsets_out[++next] = r;  // series without rows in between start (and end) here
+      prev = id;
+    }
+    while (next < n_series) offsets_out[++next] = n_rows;
+  } else {
+    for (uint32_t s = 0; s <= n_series; ++s) offsets_out[s] = offsets_in[s] - offsets_in[0];
+    for (uint32_t s = 0; s < n_series; ++s)
+      if (offsets_out[s + 1] < offsets_out[s] || offsets_out[s + 1] > n_rows) return B2P_E_INVALID;
+  }
+  bool regular = true;
+  for (uint32_t s = 0; s < n_series; ++s) {
+    const uint64_t r0 = offsets_out[s], r1 = offsets_out[s + 1];
+    const int64_t first = r1 > r0 ? ts[r0] : 0;
+    // (wrapping arithmetic: the device rebuilds the column with the same operations)
+    const int64_t step = r1 - r0 >= 2 ? (int64_t)((uint64_t)ts[r0 + 1] - (uint64_t)first) : 0;
+    if (t0) t0[s] = first;
+    if (cadence) cadence[s] = step;
+    if (regular) {
+      uint64_t expect = (uint64_t)first;
+      for (uint64_t r = r0; r < r1; ++r) {
+        if ((uint64_t)ts[r] != expect) { regular = false; break; }
+        expect += (uint64_t)step;
+      }
+    }
+    if (!regular && !t0 && !cadence) break;
+  }
+  if (all_regular) *all_regular = regular ? 1 : 0;
+  return B2P_OK;
+}
+
+int b2p_host_scan_series(const int64_t* ts, const uint32_t* sid, const uint64_t* offsets_in, uint64_t n_rows,
+                         uint32_t n_series, uint32_t sid_base, uint64_t* offsets_out, int64_t* t0, int64_t* cadence,
+                         int32_t* all_regular) {
+  if (!offsets_out || (!sid && !offsets_in) || (!ts && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
+  const int rc = host_scan_series(ts, sid, offsets_in, n_rows, n_series, sid_base, offsets_out, t0, cadence, all_regular);
+  if (rc == B2P_E_UNSORTED) return fail(rc, "series-id column is not non-decreasing or out of range");
+  if (rc) return fail(rc, "offsets are not non-decreasing or exceed n_rows");
+  return rc;
+}
+
+// One chunk, no overlap: H2D -> K0/K2 -> D2H on the context stream.  sid values are global ids
+// (sid_base is subtracted on the device); offsets_host, when given, is already rebased to the chunk.
+static int range_eval_host_simple(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
+                                  const uint32_t* sid, uint32_t sid_base, const uint64_t* offsets_host, uint64_t n_rows,
+                                  uint32_t n_series, int64_t T, double* out, uint32_t* valid_words) {
+  int rc;
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  c->last_h2d_bytes = (long long)(n_rows * 16 + (offsets_host ? ((size_t)n_series + 1) * 8 : n_rows * 4));
+  Staging s{c};
+  const SeriesIn in = stage_series(s, ts, val, sid, sid_base, offsets_host, n_rows, n_series);
+  double* d_out = s.out(out, (size_t)n_series * (size_t)T * 8);
+  uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
+  if ((rc = s.rc) || (rc = b2p_range_eval_dev(c, p, in.ts, in.val, in.offsets, n_rows, n_series, d_out, d_valid)) ||
+      (rc = b2p_sync(c)))
+    return rc;
+  return s.finish();
+}
+
+// first row whose id is >= key in a non-decreasing id column
+static uint64_t lower_bound_sid(const uint32_t* sid, uint64_t n, uint64_t key) {
+  uint64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const uint64_t mid = (lo + hi) >> 1;
+    if ((uint64_t)sid[mid] < key) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val, const uint32_t* sid,
+                   const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* out,
+                   uint32_t* valid_words, int64_t* out_ts) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int64_t T = 0;
+  int rc = check_grid(p, n_series, &T);
+  if (rc) return rc;
+  if (out_ts)
+    for (int64_t k = 0; k < T; ++k) out_ts[k] = p->start + k * p->interval;
+  if (n_series == 0 || T == 0) return B2P_OK;
+  if (!sid && !offsets_host) return fail(B2P_E_INVALID, "need sid or offsets_host");
+  if (!out || !valid_words || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  if (!c->pending.empty() && (rc = b2p_sync(c))) return rc;  // earlier asynchronous calls finish first
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+
+  // ---- small inputs: one shot -------------------------------------------------------------------
+  constexpr uint64_t kChunkRows = 4u << 20;  // ~84 MB of H2D per chunk
+  if (n_rows <= kChunkRows + kChunkRows / 2 || n_series < 64)
+    return range_eval_host_simple(c, p, ts, val, sid, 0u, offsets_host, n_rows, n_series, T, out, valid_words);
+
+  // ---- large inputs: series chunks, double-buffered; H2D(i+1) | K0+K2(i) | D2H(i-1) overlap -----------
+  const uint64_t avg_rows = n_rows / n_series + 1;
+  uint32_t C = (uint32_t)(kChunkRows / avg_rows);
+  if (C < 64) C = 64;
+  const uint32_t n_chunks = (n_series + C - 1) / C;
+  if (!c->pipe_ready) {
+    bool ok = cudaStreamCreateWithFlags(&c->s_h2d, cudaStreamNonBlocking) == cudaSuccess;
+    ok = ok && cudaStreamCreateWithFlags(&c->s_d2h, cudaStreamNonBlocking) == cudaSuccess;
+    for (int i = 0; ok && i < 2; ++i) {
+      ok = ok && cudaEventCreateWithFlags(&c->ev_h2d[i], cudaEventDisableTiming) == cudaSuccess;
+      ok = ok && cudaEventCreateWithFlags(&c->ev_comp[i], cudaEventDisableTiming) == cudaSuccess;
+      ok = ok && cudaEventCreateWithFlags(&c->ev_d2h[i], cudaEventDisableTiming) == cudaSuccess;
+    }
+    if (!ok) return fail(B2P_E_CUDA, "pipeline stream/event creation failed");
+    c->pipe_ready = true;
+  }
+  if ((rc = c->p_status.ensure((size_t)n_chunks * sizeof(Status)))) return rc;  // device copies of each chunk's status
+  Status* h_stat = nullptr;
+  CU(cudaMallocHost(&h_stat, (size_t)n_chunks * sizeof(Status)));
+  uint64_t* h_offs[2] = {nullptr, nullptr};
+  if (offsets_host) {
+    for (int i = 0; i < 2; ++i) CU(cudaMallocHost(&h_offs[i], ((size_t)C + 1) * 8));
+  }
+  struct Cleanup {
+    Status* s; uint64_t* o0; uint64_t* o1;
+    ~Cleanup() { if (s) cudaFreeHost(s); if (o0) cudaFreeHost(o0); if (o1) cudaFreeHost(o1); }
+  } cleanup{h_stat, h_offs[0], h_offs[1]};
+
+  // worst-case chunk row count (chunks are whole series)
+  uint64_t max_rows = 0;
+  std::vector<uint64_t> chunk_row(n_chunks + 1, 0);
+  {
+    uint64_t prev = 0;
+    for (uint32_t i = 0; i < n_chunks; ++i) {
+      const uint64_t s1 = (uint64_t)(i + 1) * C < n_series ? (uint64_t)(i + 1) * C : n_series;
+      const uint64_t r1 = offsets_host ? offsets_host[s1] : lower_bound_sid(sid, n_rows, s1);
+      if (r1 < prev) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");
+      if (r1 - prev > max_rows) max_rows = r1 - prev;
+      prev = r1;
+      chunk_row[i + 1] = r1;
+    }
+    if (!offsets_host && prev != n_rows) return fail(B2P_E_UNSORTED, "series id >= n_series");
+  }
+  // Host scan of every chunk, ahead of the copies (worker k takes chunks k, k + W, ..): 0 = not scanned yet, 1 = every
+  // series of the chunk is equally spaced (its rebased offsets, first timestamps and cadences are in the pinned
+  // descriptor arrays), 2 = take the ordinary route (ids out of order included: K0 reports those as before)
+  // (only when the batch comes with its id column: then the descriptors replace 12 of the 20 B/row and K0; with offsets
+  // handed over the call is already at 16 B/row, and the scan's per-call cost — pinned descriptor arrays, worker
+  // threads — costs more than the 8 B/row it saves)
+  const bool scan = c->host_ts_scan && !offsets_host;
+  uint64_t* h_doff = nullptr;
+  int64_t *h_t0 = nullptr, *h_cad = nullptr;
+  std::unique_ptr<std::atomic<int>[]> scan_state;
+  std::atomic<bool> scan_stop{false};
+  std::vector<std::thread> scan_workers;
+  struct ScanJoin {
+    std::atomic<bool>& stop; std::vector<std::thread>& w; uint64_t*& a; int64_t*& b; int64_t*& d;
+    ~ScanJoin() {
+      stop.store(true);
+      for (auto& t : w) if (t.joinable()) t.join();
+      if (a) cudaFreeHost(a);
+      if (b) cudaFreeHost(b);
+      if (d) cudaFreeHost(d);
+    }
+  } scan_join{scan_stop, scan_workers, h_doff, h_t0, h_cad};
+  if (scan) {
+    CU(cudaMallocHost(&h_doff, ((size_t)n_series + n_chunks) * 8));
+    CU(cudaMallocHost(&h_t0, (size_t)n_series * 8));
+    CU(cudaMallocHost(&h_cad, (size_t)n_series * 8));
+    scan_state.reset(new std::atomic<int>[n_chunks]);
+    for (uint32_t i = 0; i < n_chunks; ++i) scan_state[i].store(0);
+    unsigned hw = std::thread::hardware_concurrency();
+    unsigned W = hw >= 64 ? 16u : (hw >= 8 ? hw / 4 : 1u);
+    if (W > n_chunks) W = n_chunks;
+    std::atomic<int>* state = scan_state.get();
+    const uint64_t* rows = chunk_row.data();
+    try {
+    for (unsigned k = 0; k < W; ++k) {
+      scan_workers.emplace_back([=, &scan_stop]() {
+        for (uint32_t i = k; i < n_chunks && !scan_stop.load(std::memory_order_relaxed); i += W) {
+          const uint32_t s0 = i * C;
+          const uint32_t s1 = (uint64_t)s0 + C < n_series ? s0 + C : n_series;
+          const uint64_t r0 = rows[i], nr = rows[i + 1] - rows[i];
+          int32_t regular = 0;
+          const int rc_scan = host_scan_series(ts + r0, sid ? sid + r0 : nullptr, offsets_host ? offsets_host + s0 : nullptr, nr,
+                                               s1 - s0, s0, h_doff + s0 + i, h_t0 + s0, h_cad + s0, &regular);
+          state[i].store((rc_scan == B2P_OK && regular) ? 1 : 2, std::memory_order_release);
+        }
+      });
+    }
+    } catch (...) {  // no threads to be had: every chunk the started workers do not reach takes the ordinary route
+      scan_stop.store(true);
+      for (auto& t : scan_workers) if (t.joinable()) t.join();
+      for (uint32_t i = 0; i < n_chunks; ++i) {
+        int zero = 0;
+        state[i].compare_exchange_strong(zero, 2);
+      }
+    }
+  }
+  for (int i = 0; i < 2; ++i) {
+    if (scan && (rc = c->p_t0[i].ensure((size_t)C * 8))) return rc;
+    if (scan && (rc = c->p_cad[i].ensure((size_t)C * 8))) return rc;
+    if ((rc = c->p_ts[i].ensure(max_rows * 8 + 16))) return rc;
+    if ((rc = c->p_val[i].ensure(max_rows * 8 + 16))) return rc;
+    if (!offsets_host && (rc = c->p_sid[i].ensure(max_rows * 4 + 16))) return rc;
+    if ((rc = c->p_off[i].ensure(((size_t)C + 1) * 8))) return rc;
+    if ((rc = c->p_out[i].ensure((size_t)C * (size_t)T * 8))) return rc;
+    if ((rc = c->p_valid[i].ensure((size_t)C * Tw * 4))) return rc;
+  }
+  CU(cudaStreamSynchronize(c->stream));
+  c->last_h2d_bytes = 0;
+  uint64_t row_lo = 0;
+  for (uint32_t i = 0; i < n_chunks; ++i) {
+    const int b = (int)(i & 1);
+    const uint32_t s0 = i * C;
+    const uint32_t s1 = (uint64_t)s0 + C < n_series ? s0 + C : n_series;
+    const uint32_t ns = s1 - s0;
+    const uint64_t row_hi = offsets_host ? offsets_host[s1] : lower_bound_sid(sid, n_rows, s1);
+    const uint64_t nr = row_hi - row_lo;
+    int described = 2;  // 1: the chunk's timestamp (and id) column is described by (offsets, t0, cadence)
+    if (scan)
+      while ((described = scan_state[i].load(std::memory_order_acquire)) == 0) std::this_thread::yield();
+    // H2D of chunk i may start once chunk i-2's kernels no longer read this buffer pair
+    if (i >= 2) CU(cudaStreamWaitEvent(c->s_h2d, c->ev_comp[b], 0));
+    CU(cudaMemcpyAsync(c->p_val[b].p, val + row_lo, nr * 8, cudaMemcpyHostToDevice, c->s_h2d));
+    c->last_h2d_bytes += (long long)(nr * 8);
+    if (described == 1) {
+      c->last_h2d_bytes += (long long)(((size_t)ns + 1) * 8 + (size_t)ns * 16);
+      CU(cudaMemcpyAsync(c->p_off[b].p, h_doff + s0 + i, ((size_t)ns + 1) * 8, cudaMemcpyHostToDevice, c->s_h2d));
+      CU(cudaMemcpyAsync(c->p_t0[b].p, h_t0 + s0, (size_t)ns * 8, cudaMemcpyHostToDevice, c->s_h2d));
+      CU(cudaMemcpyAsync(c->p_cad[b].p, h_cad + s0, (size_t)ns * 8, cudaMemcpyHostToDevice, c->s_h2d));
+    } else {
+    c->last_h2d_bytes += (long long)(nr * 8 + (offsets_host ? ((size_t)ns + 1) * 8 : nr * 4));
+    CU(cudaMemcpyAsync(c->p_ts[b].p, ts + row_lo, nr * 8, cudaMemcpyHostToDevice, c->s_h2d));
+    if (offsets_host) {
+      if (i >= 2) CU(cudaEventSynchronize(c->ev_h2d[b]));  // the pinned rebase buffer is free again
+      for (uint32_t q = 0; q <= ns; ++q) h_offs[b][q] = offsets_host[s0 + q] - row_lo;
+      CU(cudaMemcpyAsync(c->p_off[b].p, h_offs[b], ((size_t)ns + 1) * 8, cudaMemcpyHostToDevice, c->s_h2d));
+    } else {
+      CU(cudaMemcpyAsync(c->p_sid[b].p, sid + row_lo, nr * 4, cudaMemcpyHostToDevice, c->s_h2d));
+    }
+    }
+    CU(cudaEventRecord(c->ev_h2d[b], c->s_h2d));
+    // compute: after its inputs landed and after chunk i-2's results left the output buffers
+    CU(cudaStreamWaitEvent(c->stream, c->ev_h2d[b], 0));
+    if (i >= 2) CU(cudaStreamWaitEvent(c->stream, c->ev_d2h[b], 0));
+    if (described == 1) {
+      ts_expand_kernel<<<capped_grid(c, ns, 8, 8), 256, 0, c->stream>>>(
+          c->p_off[b].as<uint64_t>(), c->p_t0[b].as<int64_t>(), c->p_cad[b].as<int64_t>(), ns, c->p_ts[b].as<int64_t>());
+      c->launches++;
+      CU(cudaGetLastError());
+    } else if (!offsets_host &&
+        (rc = series_offsets_impl(c, c->p_sid[b].as<uint32_t>(), nr, ns, s0, c->p_off[b].as<uint64_t>())))
+      return rc;
+    if ((rc = b2p_range_eval_dev(c, p, c->p_ts[b].as<int64_t>(), c->p_val[b].as<double>(), c->p_off[b].as<uint64_t>(),
+                                 nr, ns, c->p_out[b].as<double>(), c->p_valid[b].as<uint32_t>())))
+      return rc;
+    {  // this chunk's verdict is read with all the others below: take the call out of the pending queue
+      const int slot = c->pending.back().slot;
+      c->pending.pop_back();
+      CU(cudaMemcpyAsync(c->p_status.as<Status>() + i, c->d_ring + slot, sizeof(Status), cudaMemcpyDeviceToDevice, c->stream));
+    }
+    CU(cudaEventRecord(c->ev_comp[b], c->stream));
+    // D2H
+    CU(cudaStreamWaitEvent(c->s_d2h, c->ev_comp[b], 0));
+    CU(cudaMemcpyAsync(out + (size_t)s0 * (size_t)T, c->p_out[b].p, (size_t)ns * (size_t)T * 8, cudaMemcpyDeviceToHost,
+                       c->s_d2h));
+    CU(cudaMemcpyAsync(valid_words + (size_t)s0 * Tw, c->p_valid[b].p, (size_t)ns * Tw * 4, cudaMemcpyDeviceToHost,
+                       c->s_d2h));
+    CU(cudaEventRecord(c->ev_d2h[b], c->s_d2h));
+    row_lo = row_hi;
+  }
+  CU(cudaMemcpyAsync(h_stat, c->p_status.p, (size_t)n_chunks * sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaMemcpyAsync(c->h_k0, c->d_k0, sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  CU(cudaStreamSynchronize(c->s_d2h));
+  if (const uint32_t k0 = c->h_k0->k0_errors) {
+    CU(cudaMemsetAsync(c->d_k0, 0, sizeof(Status), c->stream));
+    return k0_fail(k0);
+  }
+  // per-chunk verdicts; a chunk whose slow path ran out of arena is redone alone (b2p_sync grows the arena)
+  long long slow_total = 0, w_total = 0;
+  row_lo = 0;
+  for (uint32_t i = 0; i < n_chunks; ++i) {
+    const uint32_t s0 = i * C;
+    const uint32_t s1 = (uint64_t)s0 + C < n_series ? s0 + C : n_series;
+    const uint64_t row_hi = offsets_host ? offsets_host[s1] : lower_bound_sid(sid, n_rows, s1);
+    const Status st = h_stat[i];
+    slow_total += st.slow_count;
+    w_total += st.w_count;
+    if (st.arena_overflow) {
+      std::string tmp_offs;
+      const uint64_t* offs_chunk = nullptr;
+      if (offsets_host) {
+        tmp_offs.resize(((size_t)(s1 - s0) + 1) * 8);
+        uint64_t* o = reinterpret_cast<uint64_t*>(&tmp_offs[0]);
+        for (uint32_t q = 0; q <= s1 - s0; ++q) o[q] = offsets_host[s0 + q] - row_lo;
+        offs_chunk = o;
+      }
+      if ((rc = range_eval_host_simple(c, p, ts + row_lo, val + row_lo, sid ? sid + row_lo : nullptr, s0, offs_chunk,
+                                       row_hi - row_lo, s1 - s0, T, out + (size_t)s0 * (size_t)T,
+                                       valid_words + (size_t)s0 * Tw)))
+        return rc;
+    }
+    row_lo = row_hi;
+  }
+  c->last_slow = slow_total;
+  c->last_w = w_total;
+  if (c->last_used_lean) lean_verdict(c, p->fn_id, (uint64_t)w_total, n_series);
+  return B2P_OK;
+}
+
+int b2p_range_udf(b2p_ctx* c, int32_t fn_id, const int64_t* ts, const double* val, uint64_t n_rows,
+                  const int64_t* packed_ranges, const int64_t* eval_ts, uint64_t n_win, int64_t range_length,
+                  double param0, double param1, double* out, uint8_t* valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_win == 0) return B2P_OK;
+  if (!packed_ranges || !out || !valid || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  int rc;
+  Staging s{c};
+  const int64_t* d_ts = s.in(ts, n_rows * 8);
+  const double* d_val = s.in(val, n_rows * 8);
+  const int64_t* d_packed = s.in(packed_ranges, n_win * 8);
+  const int64_t* d_eval_ts = s.in(eval_ts, n_win * 8);
+  double* d_out = s.out(out, n_win * 8);
+  uint8_t* d_valid = s.out(valid, n_win);
+  if ((rc = s.rc) || (rc = b2p_range_udf_dev(c, fn_id, d_ts, d_val, n_rows, d_packed, d_eval_ts, n_win, range_length,
+                                             param0, param1, d_out, d_valid)))
+    return rc;
+  return s.finish();
+}
+
+int b2p_instant_select(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
+                       const int64_t* ts, const double* val, const uint32_t* sid, const uint64_t* offsets_host,
+                       uint64_t n_rows, uint32_t n_series, double* out, uint32_t* valid_words) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  b2p_range_params p{};
+  p.start = start; p.end = end; p.interval = interval; p.range = lookback;
+  int64_t T = 0;
+  int rc = check_grid(&p, n_series, &T);
+  if (rc) return rc;
+  if (n_series == 0 || T == 0) return B2P_OK;
+  if (!sid && !offsets_host) return fail(B2P_E_INVALID, "need sid or offsets_host");
+  if (!out || !valid_words || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  Staging s{c};
+  const SeriesIn in = stage_series(s, ts, val, sid, 0u, offsets_host, n_rows, n_series);
+  double* d_out = s.out(out, (size_t)n_series * (size_t)T * 8);
+  uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
+  if ((rc = s.rc) ||
+      (rc = b2p_instant_select_dev(c, start, end, interval, lookback, offset, in.ts, in.val, in.offsets, n_rows,
+                                   n_series, d_out, d_valid)) ||
+      (rc = b2p_sync(c)))
+    return rc;
+  return s.finish();
+}
+
+int b2p_subquery(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval, const double* vals,
+                 const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int64_t T = 0;
+  int rc = check_grid(p, n_rows, &T);
+  if (rc) return rc;
+  if (n_rows == 0 || T == 0) return b2p_subquery_dev(c, p, inner_start, inner_interval, nullptr, nullptr, 0, 0, nullptr,
+                                                     nullptr);  // (the argument checks only)
+  if (!out || !out_valid || (T_inner && (!vals || !valid))) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const size_t Tw_in = (size_t)((T_inner + 31) / 32), Tw = (size_t)((T + 31) / 32);
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_rows * T_inner * 8);
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw_in * 4);
+  double* d_out = s.out(out, (size_t)n_rows * (size_t)T * 8);
+  uint32_t* d_valid_out = s.out(out_valid, (size_t)n_rows * Tw * 4);
+  if ((rc = s.rc) ||
+      (rc = b2p_subquery_dev(c, p, inner_start, inner_interval, d_vals, d_valid, n_rows, T_inner, d_out, d_valid_out)) ||
+      (rc = b2p_sync(c)))
+    return rc;
+  return s.finish();
+}
+
+}  // extern "C"

@@ -24,7 +24,8 @@
 #pragma once
 #include <cstdint>
 
-#include "b2p_kernels.cuh"
+#include "b2p_status.cuh"
+#include "b2p_window.cuh"
 
 namespace b2p {
 
@@ -37,7 +38,6 @@ enum SetCopyMode {
   kCopyWords = 3,   // the row's word of `words` (the dedupe's result); no key -> lv
 };
 constexpr uint32_t kSetNoKey = 0xFFFFFFFFu;
-constexpr uint32_t kSetKeyError = 8u;  // Status::k0_errors bit: a row's key is >= n_keys and not B2P_NO_KEY
 
 __global__ void __launch_bounds__(256) setop_key_check_kernel(const uint32_t* key, uint64_t n, uint32_t n_keys,
                                                               Status* status) {

@@ -342,7 +342,7 @@ B2P_API int b2p_scalar_calculate_dev(b2p_ctx* ctx, const double* vals, const uin
  * none for k < 1, -inf and -NaN, all for +inf and +NaN.  Per (group, step) exactly the min(kept ranks, valid cells) best
  * cells keep their bit.  Only out_valid [rows x Tw] is written (bits at or past T are 0); it may be valid (in place).
  * vals is never written: topk is a filter, and every consumer reads a cell only where its bit is set.  Scratch comes
- * from the context and is bounded (b2p_api.cu, topk_run).  B2P_E_INVALID: a NULL argument. */
+ * from the context and is bounded (b2p_aggregation.cu, topk_run).  B2P_E_INVALID: a NULL argument. */
 B2P_API int b2p_topk_dev(b2p_ctx* ctx, int32_t bottom, double k, const double* vals, const uint32_t* valid,
                          const b2p_group_index* index, const uint32_t* tie, uint64_t T, uint32_t* out_valid);
 
@@ -352,7 +352,7 @@ B2P_API int b2p_topk_dev(b2p_ctx* ctx, int32_t bottom, double k, const double* v
  * hi = min(n - 1, lo + 1), w = rank - floor(rank) and the result s[lo] (1 - w) + s[hi] w, evaluated as written (so
  * quantile(0, {1, +inf}) is NaN).  Output out_val / out_cnt [n_groups x T] as b2p_group_aggregate_dev: out_cnt = n, and
  * n = 0 (value 0.0) is "no row".  Rows of the index's gid >= n_groups take part in nothing.  Deterministic; scratch
- * comes from the context and is bounded (b2p_api.cu, quantile_run).  B2P_E_INVALID: a NULL argument. */
+ * comes from the context and is bounded (b2p_aggregation.cu, quantile_run).  B2P_E_INVALID: a NULL argument. */
 B2P_API int b2p_group_quantile_dev(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid,
                                    const b2p_group_index* index, uint64_t T, double* out_val, uint32_t* out_cnt);
 
@@ -362,7 +362,7 @@ B2P_API int b2p_group_quantile_dev(b2p_ctx* ctx, double phi, const double* vals,
  * out_val (f64) / out_cnt (u32) [n_series x T] with rows in the index's member order (a group's rows ordered by row
  * index, the groups by id; rows of gid >= n_groups last): at step k, the group's j-th row holds its j-th smallest
  * distinct value and how many of its cells have it; out_cnt 0 (value 0.0) past the last, and on every row of
- * gid >= n_groups.  Exact and deterministic; scratch comes from the context and is bounded (b2p_api.cu,
+ * gid >= n_groups.  Exact and deterministic; scratch comes from the context and is bounded (b2p_aggregation.cu,
  * count_values_run).  B2P_E_INVALID: a NULL argument; B2P_E_TOO_LARGE: a group of more than 67 M members. */
 B2P_API int b2p_count_values_dev(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const b2p_group_index* index,
                                  uint64_t T, double* out_val, uint32_t* out_cnt);
@@ -375,7 +375,7 @@ B2P_API int b2p_count_values_dev(b2p_ctx* ctx, const double* vals, const uint32_
  * evaluate the windows over those samples.  Output out [n_rows x T] / out_valid [n_rows x Tw] on the outer grid, row for
  * row, exactly as b2p_range_eval_dev over the same samples.  Each row is one series: the reference's RangeManipulate
  * windows each input batch as one series (range_manipulate.rs:603-630), which is the row's series whenever the child
- * hands it one series per batch.  Scratch comes from the context (16 B per grid cell of a batch of rows, b2p_api.cu,
+ * hands it one series per batch.  Scratch comes from the context (16 B per grid cell of a batch of rows, b2p_range.cu,
  * subquery_run); a grid of more than one batch waits for each batch's range call before the next.
  * B2P_E_INVALID: an unknown fn_id, a non-positive interval or inner_interval, a zero range, a non-zero offset or
  * filter_nan, a NULL argument. */

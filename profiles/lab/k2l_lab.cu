@@ -1,6 +1,6 @@
 // k2l_lab.cu — standalone timing / bit-compare harness for the dominant kernel (K2L, rate) and the series-offset stage.
 // Not product code: it includes the product's kernel headers from the tree given with -I and launches them the way
-// b2p_api.cu does, on the BASELINE config-2 chunk shape, so that kernel variants can be compared in one run
+// b2p_range.cu does, on the BASELINE config-2 chunk shape, so that kernel variants can be compared in one run
 // without the Python stack.  Prints one line per run:
 //   tag S ms_k0 ms_k2l ms_step checksum_out checksum_valid handed_off
 // Two binaries built from two source trees agree bit for bit iff their checksums agree.
