@@ -33,6 +33,7 @@ EXPORTED_SYMBOLS = [
     "b2p_group_quantile_dev", "b2p_group_quantile", "b2p_plan_aggregate_create",
     "b2p_count_values_dev", "b2p_count_values", "b2p_plan_count_values_create",
     "b2p_subquery_dev", "b2p_subquery", "b2p_plan_subquery_create",
+    "b2p_histogram_fold", "b2p_plan_histogram_quantile_create",
 ]
 
 
@@ -141,6 +142,8 @@ def load() -> C.CDLL:
         "b2p_subquery_dev": (C.c_int, [vp, P, i64, i64, vp, vp, u32, u64, vp, vp]),
         "b2p_subquery": (C.c_int, [vp, P, i64, i64, vp, vp, u32, u64, vp, vp]),
         "b2p_plan_subquery_create": (vp, [vp, C.c_char_p, P, vp]),
+        "b2p_histogram_fold": (C.c_int, [vp, dbl, vp, vp, vp, u32, vp, vp, u32, u64, vp, vp]),
+        "b2p_plan_histogram_quantile_create": (vp, [vp, C.c_char_p, dbl, vp]),
         "b2p_plan_set_function": (C.c_int, [vp, C.c_char_p, C.POINTER(dbl), i32]),
         "b2p_plan_scalar_create": (vp, [vp, vp]),
     }

@@ -353,6 +353,39 @@ int b2p_histogram_quantile(b2p_ctx* c, double phi, const double* le, uint32_t n_
   return s.finish();
 }
 
+// HistogramFold over any [n_rows x T] grid: the index is checked on the host, so a bad one never reaches K5; then the
+// grid, its bitmap and the index go to the device, and [n_hist x T] comes back.
+int b2p_histogram_fold(b2p_ctx* c, double phi, const uint32_t* hist_off, const uint32_t* bucket_series,
+                       const double* bucket_le, uint32_t n_hist, const double* rates, const uint32_t* valid_words,
+                       uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid_words) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_hist == 0 || T == 0) return B2P_OK;
+  if (!hist_off || !bucket_series || !bucket_le || !rates || !valid_words || !out || !out_valid_words)
+    return fail(B2P_E_INVALID, "NULL argument");
+  if (hist_off[0] != 0) return fail(B2P_E_INVALID, "hist_off[0] is %u, not 0", hist_off[0]);
+  for (uint32_t h = 0; h < n_hist; ++h)
+    if (hist_off[h + 1] < hist_off[h]) return fail(B2P_E_INVALID, "hist_off decreases at histogram %u", h);
+  const size_t nb = hist_off[n_hist];
+  for (size_t i = 0; i < nb; ++i)
+    if (bucket_series[i] >= n_rows)
+      return fail(B2P_E_INVALID, "bucket_series[%zu] = %u is not a row (n_rows = %u)", i, bucket_series[i], n_rows);
+  DeviceGuard g(c->device);
+  int rc;
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  Staging s{c};
+  const double* d_rates = s.in(rates, (size_t)n_rows * T * 8);
+  const uint32_t* d_valid = s.in(valid_words, (size_t)n_rows * Tw * 4);
+  const uint32_t* d_hist_off = s.in(hist_off, ((size_t)n_hist + 1) * 4);
+  const uint32_t* d_bucket_series = s.in(bucket_series, nb * 4);
+  const double* d_bucket_le = s.in(bucket_le, nb * 8);
+  double* d_out = s.out(out, (size_t)n_hist * T * 8);
+  uint32_t* d_out_valid = s.out(out_valid_words, (size_t)n_hist * Tw * 4);
+  if ((rc = s.rc) || (rc = b2p_histogram_fold_dev(c, phi, d_hist_off, d_bucket_series, d_bucket_le, n_hist, d_rates,
+                                                  d_valid, T, d_out, d_out_valid)))
+    return rc;
+  return s.finish();
+}
+
 // histogram_quantile(phi, fn(bucket_series[range])) from host buffers to host rows without the dense [n_series x T]
 // matrix ever leaving the device: H2D of the samples, series offsets, the range function into context scratch, the
 // HistogramFold over the caller's (histogram -> buckets in le order) index, D2H of [n_hist x T] only.

@@ -321,6 +321,48 @@ void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& 
   r.rows = G;
 }
 
+// The HistogramFold index over `rows` rows labelled `in` (histogram_fold.rs:754-820): rows that agree on every tag but
+// column `le` form one histogram, histograms in label order; each histogram's buckets in ascending le order (parsed as
+// le.parse::<f64>().unwrap_or(NaN), :791-796, NULL as NaN), NaN bounds last, ties in row order.  The CSR
+// hist_off / bucket_series / bucket_le is what b2p_histogram_fold[_dev] and b2p_range_histogram_fold take.
+struct HistogramIndex {
+  Groups hist;  // the histograms; hist.labels are their tags without le
+  std::vector<uint32_t> hist_off, bucket_series;
+  std::vector<double> bucket_le;
+};
+
+HistogramIndex histogram_index(const Labels& in, int le, uint32_t rows) {
+  HistogramIndex ix;
+  std::vector<int> cols;  // the tags without le
+  for (int t = 0; t < (int)in.names.size(); ++t)
+    if (t != le) cols.push_back(t);
+  ix.hist = group_rows(in, cols, rows);
+  const uint32_t H = (uint32_t)ix.hist.rank.size();
+  std::vector<double> sle(rows);
+  for (uint32_t s = 0; s < rows; ++s) {
+    const Label& v = in.values[(size_t)le][s];
+    sle[s] = v ? parse_f64_like_rust(*v) : std::nan("");
+  }
+  // a strict weak ordering: histogram, then le ascending with NaN last; stable_sort keeps ties in row order
+  auto place = [&](uint32_t s) { return ix.hist.rank[ix.hist.id[s]]; };
+  ix.bucket_series.resize(rows);
+  std::iota(ix.bucket_series.begin(), ix.bucket_series.end(), 0u);
+  std::stable_sort(ix.bucket_series.begin(), ix.bucket_series.end(), [&](uint32_t x, uint32_t y) {
+    if (place(x) != place(y)) return place(x) < place(y);
+    const bool nx = std::isnan(sle[x]), ny = std::isnan(sle[y]);
+    if (nx != ny) return ny;
+    return !nx && sle[x] < sle[y];
+  });
+  ix.hist_off.assign((size_t)H + 1, 0u);
+  ix.bucket_le.resize(rows);
+  for (uint32_t i = 0; i < rows; ++i) {
+    ix.bucket_le[i] = sle[ix.bucket_series[i]];
+    ix.hist_off[place(ix.bucket_series[i]) + 1]++;
+  }
+  for (uint32_t h = 0; h < H; ++h) ix.hist_off[h + 1] += ix.hist_off[h];
+  return ix;
+}
+
 }  // namespace
 
 // ---- PromRangePlan -------------------------------------------------------------------------------------
@@ -510,43 +552,17 @@ void PromRangePlan::compute(NodeResult& r) {
     // HistogramFold (histogram_fold.rs:754-820): group the series by their tags without `le`, order each group's
     // buckets by le ascending (parsed as f64, "+Inf" last), one output row per (group, eval ts)
     if (series_.id_keyed) throw PlanError(ErrorKind::Plan, "HistogramFold needs the le tag column, not a tsid key");
-    const int le = series_.column(args_.le_column);
-    std::vector<int> cols;  // the tags without le
-    for (int t = 0; t < (int)series_.names.size(); ++t)
-      if (t != le) cols.push_back(t);
-    Groups hist = group_rows(series_, cols, S);
-    const uint32_t H = (uint32_t)hist.rank.size();
-    std::vector<double> sle(S);  // le.parse::<f64>().unwrap_or(NaN), histogram_fold.rs:791-796
-    for (uint32_t s = 0; s < S; ++s) {
-      const Label& v = series_.values[(size_t)le][s];
-      sle[s] = v ? parse_f64_like_rust(*v) : std::nan("");
-    }
-    // buckets of every histogram in ascending le order, NaN bounds last, ties in scan order (a strict weak ordering)
-    auto place = [&](uint32_t s) { return hist.rank[hist.id[s]]; };
-    std::vector<uint32_t> bucket_series(S);
-    std::iota(bucket_series.begin(), bucket_series.end(), 0u);
-    std::stable_sort(bucket_series.begin(), bucket_series.end(), [&](uint32_t x, uint32_t y) {
-      if (place(x) != place(y)) return place(x) < place(y);
-      const bool nx = std::isnan(sle[x]), ny = std::isnan(sle[y]);
-      if (nx != ny) return ny;
-      return !nx && sle[x] < sle[y];
-    });
-    std::vector<uint32_t> hist_off(H + 1, 0);
-    std::vector<double> bucket_le(S);
-    for (uint32_t i = 0; i < S; ++i) {
-      bucket_le[i] = sle[bucket_series[i]];
-      hist_off[place(bucket_series[i]) + 1]++;
-    }
-    for (uint32_t h = 0; h < H; ++h) hist_off[h + 1] += hist_off[h];
+    HistogramIndex ix = histogram_index(series_, series_.column(args_.le_column), S);
+    const uint32_t H = (uint32_t)ix.hist.rank.size();
     r.val.assign((size_t)H * (size_t)T, 0.0);
     r.valid.assign((size_t)H * Tw, 0u);
     if (H > 0 && T > 0) {
       if (fn_id_ < 0) throw PlanError(ErrorKind::Plan, "HistogramFold over an instant selector is not supported by this node");
       check(b2p_range_histogram_fold(ctx_, &p, ts_.data(), val_.data(), nullptr, offsets_.data(), ts_.size(), S,
-                                     args_.quantile, hist_off.data(), bucket_series.data(), bucket_le.data(), H,
-                                     r.val.data(), r.valid.data()));
+                                     args_.quantile, ix.hist_off.data(), ix.bucket_series.data(), ix.bucket_le.data(),
+                                     H, r.val.data(), r.valid.data()));
     }
-    r.labels = std::move(hist.labels);
+    r.labels = std::move(ix.hist.labels);
     r.rows = H;
   } else {
     // rows of Filter(prom_fn IS NOT NULL): {time_index (eval ts), prom_fn(...), tags...}, series-major order
@@ -644,6 +660,8 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       }
       break;
     }
+    case Columns::None:  // (no rows either)
+      break;
   }
   int64_t n_out = 0;
   const bool ordered = !r.cell_order.empty();
@@ -1328,6 +1346,44 @@ void SubqueryPlan::compute(NodeResult& r) {
   r.value_name = name + ")";
 }
 
+// ---- HistogramQuantilePlan -----------------------------------------------------------------------------
+HistogramQuantilePlan::HistogramQuantilePlan(b2p_ctx* ctx, std::string le_column, double phi,
+                                             std::shared_ptr<PlanNode> child)
+    : PlanNode(ctx), le_column_(std::move(le_column)), phi_(phi), child_(std::move(child)) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromHistogramFoldExec: NULL context");
+  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: NULL child");
+}
+
+void HistogramQuantilePlan::compute(NodeResult& r) {
+  child_->run(r);
+  if (r.labels.id_keyed)
+    throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: an id-keyed (__tsid) child carries no " + le_column_ + " label");
+  if (r.columns == Columns::CountTagsTimeLabel)
+    throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: a count_values child is not supported by this node");
+  r.cell_order.clear();
+  const int le = r.labels.column(le_column_);
+  if (le < 0) {  // create_histogram_plan: no le tag -> EmptyRelation, no rows and no columns
+    r.rows = 0;
+    r.val.clear();
+    r.valid.clear();
+    r.labels = Labels();
+    r.columns = Columns::None;
+    return;
+  }
+  HistogramIndex ix = histogram_index(r.labels, le, r.rows);
+  const uint32_t H = (uint32_t)ix.hist.rank.size();
+  std::vector<double> out((size_t)H * (size_t)r.T, 0.0);
+  std::vector<uint32_t> out_valid((size_t)H * r.Tw, 0u);
+  if (H > 0 && r.T > 0)
+    check(b2p_histogram_fold(ctx_, phi_, ix.hist_off.data(), ix.bucket_series.data(), ix.bucket_le.data(), H,
+                             r.val.data(), r.valid.data(), r.rows, (uint64_t)r.T, out.data(), out_valid.data()),
+          ErrorKind::Execution);
+  r.val = std::move(out);
+  r.valid = std::move(out_valid);
+  r.labels = std::move(ix.hist.labels);
+  r.rows = H;
+}
+
 }  // namespace b2p
 
 // ---- C entry points -----------------------------------------------------------------------------------
@@ -1491,6 +1547,13 @@ b2p_plan* b2p_plan_subquery_create(b2p_ctx* ctx, const char* function, const b2p
   return create([&] {
     if (!function || !p || !child) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
     return std::make_shared<b2p::SubqueryPlan>(ctx, function, *p, child->node);
+  });
+}
+
+b2p_plan* b2p_plan_histogram_quantile_create(b2p_ctx* ctx, const char* le_column, double phi, b2p_plan* child) {
+  return create([&] {
+    if (!child) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    return std::make_shared<b2p::HistogramQuantilePlan>(ctx, le_column ? le_column : "le", phi, child->node);
   });
 }
 

@@ -107,6 +107,7 @@ enum class Columns {
   TimeSorted,     // {time index, then the tags and the value column in name order}: `or`
   ValueTagsTime,  // {value, tags.., time index}: topk / bottomk
   CountTagsTimeLabel,  // {count Int64 (Float64 under an element-wise stage), tags.., time index, label}: count_values
+  None,                // no column at all: histogram_quantile over a child without the le tag (an EmptyRelation)
 };
 
 // What a node computed, before it becomes Arrow: a dense [rows x T] grid with validity, the eval timestamps and one label
@@ -339,6 +340,27 @@ class SubqueryPlan : public PlanNode {
  private:
   std::string function_;
   b2p_range_params p_;
+  std::shared_ptr<PlanNode> child_;
+};
+
+// histogram_quantile(φ, child), GpuPromHistogramFoldExec: the reference's HistogramFold(le, field, time index, φ) over
+// any input (create_histogram_plan, planner.rs:3041-3108; histogram_fold.rs).  The child's rows that agree on every tag
+// but le form one histogram (histogram_index, as the range leaf builds it); the fold over the child's grid is
+// b2p_histogram_fold.  Rows: the histograms in Labels::less order; labels: the child's tags without le; the value keeps
+// the child's value name, and the export the child's column layout (a topk child's cell_order is dropped).  A child
+// without the le tag gives no rows and an export without columns (the reference's EmptyRelation).  Plan errors at
+// execute: an id-keyed child (this layer's __tsid form has no le label) and a count_values child (its counted value
+// would be a Float64 tag of the fold in the reference, which is not modelled here).
+class HistogramQuantilePlan : public PlanNode {
+ public:
+  HistogramQuantilePlan(b2p_ctx* ctx, std::string le_column, double phi, std::shared_ptr<PlanNode> child);
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  std::string le_column_;
+  double phi_;
   std::shared_ptr<PlanNode> child_;
 };
 

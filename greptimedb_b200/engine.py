@@ -239,6 +239,29 @@ class Context:
                                                    _ptr(out), _ptr(ov)))
         return out, ov
 
+    def histogram_fold(self, phi, hist_off, bucket_series, bucket_le, rates, valid):
+        """HistogramFold over any grid rates [R,T] / valid [R,Tw] u32 through the index hist_off [H+1], bucket_series /
+        bucket_le [hist_off[H]] (each histogram's buckets in ascending le order, NaN bounds last) -> (out [H,T] f64,
+        valid_words [H,Tw] u32).  A malformed index is rejected on the host (B2P_E_INVALID)."""
+        hist_off = np.ascontiguousarray(hist_off, np.uint32)
+        bucket_series = np.ascontiguousarray(bucket_series, np.uint32)
+        bucket_le = np.ascontiguousarray(bucket_le, np.float64)
+        rates = np.ascontiguousarray(rates, np.float64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        R, T = rates.shape
+        if valid.shape != (R, (T + 31) // 32):
+            raise ValueError(f"valid must be [{R}, {(T + 31) // 32}] u32 words, got {valid.shape}")
+        if hist_off.ndim != 1 or hist_off.size == 0:
+            raise ValueError("hist_off must hold n_hist + 1 >= 1 offsets")
+        H = hist_off.size - 1
+        if bucket_series.size < hist_off[-1] or bucket_le.size < hist_off[-1]:
+            raise ValueError(f"bucket_series / bucket_le must hold hist_off[-1] = {int(hist_off[-1])} entries")
+        out = np.zeros((H, T), np.float64)
+        ov = np.zeros((H, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_histogram_fold(self._h, float(phi), _ptr(hist_off), _ptr(bucket_series),
+                                               _ptr(bucket_le), H, _ptr(rates), _ptr(valid), R, T, _ptr(out), _ptr(ov)))
+        return out, ov
+
     def binary_op(self, op, lhs, lhs_valid, lhs_row, rhs, rhs_valid, rhs_row, return_bool=False):
         """lhs[lhs_row[p]] op rhs[rhs_row[p]] for every pair p -> (out [P,T] f64, valid_words [P,Tw] u32)."""
         lhs = np.ascontiguousarray(lhs, np.float64)

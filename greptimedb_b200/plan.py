@@ -6,8 +6,8 @@ start/end/interval/range/field column, the prom_* UDF name, optional by-label ag
 pyarrow RecordBatches exactly like the reference's tests feed a MemoryExec.  `scalar_op` puts `node op number` on
 top of any node, `function` an instant-vector function (abs, clamp_min, prom_round, ...; the two chain in call order),
 `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels), `SetOpPlan` applies `and` / `or` / `unless`
-to two nodes, `ScalarPlan` is scalar(node), `TopkPlan` is topk / bottomk(k, node) [by | without (labels)] and
-`SubqueryPlan` is fn(node[range:step]).
+to two nodes, `ScalarPlan` is scalar(node), `TopkPlan` is topk / bottomk(k, node) [by | without (labels)],
+`SubqueryPlan` is fn(node[range:step]) and `HistogramQuantilePlan` is histogram_quantile(phi, node).
 """
 from __future__ import annotations
 
@@ -252,5 +252,20 @@ class SubqueryPlan(_PlanNode):
         self._children = (child,)
         p = make_params(0, start, end, interval, range, offset=offset, filter_nan=False, param0=param0, param1=param1)
         self._h = self._L.b2p_plan_subquery_create(ctx._h, function.encode(), C.byref(p), child._h)
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class HistogramQuantilePlan(_PlanNode):
+    """histogram_quantile(phi, child) over any node: the child's rows that agree on every tag but `le` form one
+    histogram, its buckets in numeric `le` order (+Inf last).  One row per histogram in label order, labelled with the
+    child's tags without `le`; execute() keeps the child's column layout without `le` and its value name.  A child
+    without the `le` tag gives an empty batch with no columns.  The child stays usable and is kept alive by this node."""
+
+    def __init__(self, ctx: Context, phi: float, child: _PlanNode, le: str = "le"):
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (child,)
+        self._h = self._L.b2p_plan_histogram_quantile_create(ctx._h, le.encode(), float(phi), child._h)
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())

@@ -27,6 +27,8 @@
  *                              (sum/avg/count/min/max/stddev/stdvar by labels + eval ts)
  *   b2p_histogram_quantile[_dev] HistogramFoldStream::fold_buf + evaluate_row
  *                              histogram_fold.rs:754-820, 1046-1118
+ *   b2p_histogram_fold[_dev]   the same fold over an explicit (histogram -> buckets in le order) index and any grid:
+ *                              safe mode histogram_fold.rs:834-981 + evaluate_row :1046-1118
  *   b2p_column_reduce_dev      avg_over_time over a wide table (config 5): per-column sum,count
  *   b2p_binary_op[_dev]        vector-vector arithmetic / comparison: ProjectionExec / FilterExec over the inner
  *                              HashJoinExec on (tag columns, time index), planner.rs:556-777, 3436-3546; the join is a
@@ -420,6 +422,13 @@ B2P_API int b2p_range_histogram_fold(b2p_ctx* ctx, const b2p_range_params* p, co
                              const uint32_t* sid, const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series,
                              double phi, const uint32_t* hist_off, const uint32_t* bucket_series, const double* bucket_le,
                              uint32_t n_hist, double* out, uint32_t* out_valid_words);
+/* Host-pointer form of b2p_histogram_fold_dev (synchronous): rates / valid_words are any [n_rows x T] grid and its
+ * bitmap; the index (hist_off [n_hist + 1], bucket_series / bucket_le [hist_off[n_hist]]) as for the device form.  The
+ * index is checked on the host before anything is launched: hist_off[0] != 0, a decreasing hist_off or a bucket_series
+ * entry >= n_rows is B2P_E_INVALID.  out [n_hist x T], out_valid_words [n_hist x Tw]. */
+B2P_API int b2p_histogram_fold(b2p_ctx* ctx, double phi, const uint32_t* hist_off, const uint32_t* bucket_series,
+                               const double* bucket_le, uint32_t n_hist, const double* rates, const uint32_t* valid_words,
+                               uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid_words);
 /* Host-pointer forms of b2p_binary_op_dev / b2p_scalar_op_dev (synchronous; row-index errors are returned directly). */
 B2P_API int b2p_binary_op(b2p_ctx* ctx, int32_t op, int32_t return_bool, const double* lhs, const uint32_t* lhs_valid,
                           const uint32_t* lhs_row, uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid,
@@ -597,6 +606,17 @@ B2P_API b2p_plan* b2p_plan_count_values_create(b2p_ctx* ctx, const char* label, 
  * NULL is returned), a child whose grid is not regular (at execute).  Ownership as for b2p_plan_binary_create. */
 B2P_API b2p_plan* b2p_plan_subquery_create(b2p_ctx* ctx, const char* function, const b2p_range_params* p,
                                            b2p_plan* child);
+/* histogram_quantile(phi, child), GpuPromHistogramFoldExec (create_histogram_plan, planner.rs:3041-3108; HistogramFold,
+ * histogram_fold.rs): the child is any node.  Its rows that agree on every tag except le_column (NULL: "le") form one
+ * histogram; its buckets are ordered by le parsed as Rust's str::parse::<f64> (NULL or unparsable: NaN, last), ties in
+ * row order, and folded per step as b2p_histogram_fold_dev (the buckets with a cell at that step).  Rows: one per
+ * histogram in label order; labels: the child's tags without le; the value keeps the child's value name.  The export
+ * keeps the child's column layout without le (a topk child's rank order is dropped).  A child without the le tag gives
+ * an empty result (no rows, and an export without columns, as the reference's EmptyRelation); nodes above see no rows
+ * over the child's steps.  Plan errors at execute: an id-keyed (__tsid) child, which carries no le; a count_values
+ * child, whose counted value would be one more Float64 tag of the fold in the reference, which this layer does not
+ * model.  Ownership as for b2p_plan_binary_create.  NULL on error (b2p_plan_last_error). */
+B2P_API b2p_plan* b2p_plan_histogram_quantile_create(b2p_ctx* ctx, const char* le_column, double phi, b2p_plan* child);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

@@ -354,6 +354,12 @@ extern "C" {
         offsets_host: *const u64, n_rows: u64, n_series: u32, phi: f64, hist_off: *const u32,
         bucket_series: *const u32, bucket_le: *const f64, n_hist: u32, out: *mut f64, out_valid_words: *mut u32,
     ) -> c_int;
+    /// HistogramFold over any host grid [n_rows x T]; a malformed index is B2P_E_INVALID before anything is launched.
+    pub fn b2p_histogram_fold(
+        ctx: *mut b2p_ctx, phi: f64, hist_off: *const u32, bucket_series: *const u32, bucket_le: *const f64,
+        n_hist: u32, rates: *const f64, valid_words: *const u32, n_rows: u32, t: u64, out: *mut f64,
+        out_valid_words: *mut u32,
+    ) -> c_int;
     pub fn b2p_binary_op(
         ctx: *mut b2p_ctx, op: i32, return_bool: i32, lhs: *const f64, lhs_valid: *const u32, lhs_row: *const u32,
         n_lhs_rows: u32, rhs: *const f64, rhs_valid: *const u32, rhs_row: *const u32, n_rhs_rows: u32, n_pairs: u64,
@@ -437,6 +443,11 @@ extern "C" {
     /// on the inner grid); offset and filter_nan must be 0.  Ownership of `child` as for b2p_plan_binary_create.
     pub fn b2p_plan_subquery_create(
         ctx: *mut b2p_ctx, function: *const c_char, p: *const B2pRangeParams, child: *mut b2p_plan,
+    ) -> *mut b2p_plan;
+    /// histogram_quantile(`phi`, child) over any node; `le_column` NULL means "le".  Ownership of `child` as for
+    /// b2p_plan_binary_create.
+    pub fn b2p_plan_histogram_quantile_create(
+        ctx: *mut b2p_ctx, le_column: *const c_char, phi: f64, child: *mut b2p_plan,
     ) -> *mut b2p_plan;
     /// MOVES the batch: on success the release callbacks now belong to the plan.
     pub fn b2p_plan_push_batch(plan: *mut b2p_plan, batch: *mut FFI_ArrowArray, schema: *mut FFI_ArrowSchema) -> c_int;

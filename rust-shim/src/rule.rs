@@ -82,6 +82,14 @@
 //!                                           => `match_subquery`: the b2p_plan_subquery_create arguments
 //! ```
 //!
+//! histogram_quantile over a rewritten node (create_histogram_plan, planner.rs:3041-3108):
+//!
+//! ```text
+//!   HistogramFoldExec(le, field, ts, φ) <- SortExec(tags.., ts, CAST(le AS Float64)) [<- RepartitionExec]
+//!     <- GpuPromRangeExec (Utf8 tags including le, without its own HistogramFold)
+//!                                           => `match_histogram_quantile`: the b2p_plan_histogram_quantile_create arguments
+//! ```
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
@@ -108,7 +116,8 @@ use crate::exec::{GpuPromRangeExec, GpuPromRangeParams, GpuPromStage};
 use crate::ffi::{B2pBinOp, B2pFn, B2pSetOp};
 // In-tree these are `crate::extension_plan::{..}`; named here the way the reference names them.
 use promql::extension_plan::{
-    RangeManipulateExec, ScalarCalculateExec, SeriesDivideExec, SeriesNormalizeExec, UnionDistinctOnExec,
+    HistogramFoldExec, RangeManipulateExec, ScalarCalculateExec, SeriesDivideExec, SeriesNormalizeExec,
+    UnionDistinctOnExec,
 };
 
 #[derive(Debug)]
@@ -282,6 +291,15 @@ pub struct GpuPromSubquerySpec {
     pub range: i64,
     pub param0: f64,
     pub param1: f64,
+    pub child: GpuPromRangeParams,
+}
+
+/// What `b2p_plan_histogram_quantile_create` takes for a matched HistogramFold: the le column, the literal φ and the
+/// child node.
+#[derive(Debug, Clone)]
+pub struct GpuPromHistogramQuantileSpec {
+    pub le_column: String,
+    pub phi: f64,
     pub child: GpuPromRangeParams,
 }
 
@@ -573,6 +591,31 @@ impl GpuPromRewrite {
             param1,
             child: params.clone(),
         })
+    }
+
+    /// `HistogramFoldExec <- SortExec(tags.., ts, CAST(le AS Float64)) [<- RepartitionExec] <- GpuPromRangeExec`
+    /// (create_histogram_plan, planner.rs:3041-3108) -> the arguments of `b2p_plan_histogram_quantile_create`.  The
+    /// child must be a `GpuPromRangeExec` (a range or instant leaf, or the leaf with its aggregate stage, with or without
+    /// element-wise stages) whose Utf8 tag columns include the le column; the library's node accepts any node, but
+    /// this matcher only builds the ones the rule rewrites into a `GpuPromRangeExec`.  Left on the CPU: a leaf that
+    /// already carries its own HistogramFold, and a `__tsid`-keyed input.  The reference strips `__tsid` with a
+    /// `ProjectionExec` before the fold (strip_tsid_column, planner.rs:3064), so such an input does not match here.
+    /// The library could not fold it anyway: an id-keyed node carries no le label.
+    pub fn match_histogram_quantile(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromHistogramQuantileSpec> {
+        let fold = plan.as_any().downcast_ref::<HistogramFoldExec>()?;
+        let mut input = fold.input().clone();
+        if let Some(s) = input.as_any().downcast_ref::<SortExec>() {
+            input = s.input().clone();
+        }
+        if let Some(r) = input.as_any().downcast_ref::<RepartitionExec>() {
+            input = r.input().clone();
+        }
+        let child = input.as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let le_column = fold.input().schema().field(fold.le_column_index()).name().to_string();
+        if child.params().histogram.is_some() || !child.params().tag_columns.iter().any(|t| *t == le_column) {
+            return None;
+        }
+        Some(GpuPromHistogramQuantileSpec { le_column, phi: fold.quantile(), child: child.params().clone() })
     }
 
     /// `ProjectionExec | FilterExec <- HashJoinExec(Inner, tags.. + ts)` over two `GpuPromRangeExec` -> the arguments of
