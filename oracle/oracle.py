@@ -107,9 +107,10 @@ def lib():
         L.orc_holt_winters.restype = C.c_double
         L.orc_holt_winters.argtypes = [f64p, C.c_size_t, C.c_double, C.c_double]
         L.orc_range_query_faithful.restype = None
-        L.orc_range_query_faithful.argtypes = [C.POINTER(Params), i64p, f64p, u32p, u64p, C.c_size_t, C.c_size_t, f64p, u32p]
+        L.orc_range_query_faithful.argtypes = [C.POINTER(Params), i64p, f64p, u32p, u64p, C.c_size_t, C.c_size_t, f64p, u32p,
+                                                C.c_int]
         L.orc_range_query_flat.restype = None
-        L.orc_range_query_flat.argtypes = [C.POINTER(Params), i64p, f64p, u64p, C.c_size_t, C.c_size_t, f64p, u32p]
+        L.orc_range_query_flat.argtypes = [C.POINTER(Params), i64p, f64p, u64p, C.c_size_t, C.c_size_t, f64p, u32p, C.c_int]
         L.orc_range_query_mt.restype = C.c_int
         L.orc_range_query_mt.argtypes = [C.POINTER(Params), i64p, f64p, u32p, u64p, C.c_size_t, f64p, u32p, C.c_int, C.c_int]
         L.orc_instant_query.restype = None
@@ -219,8 +220,10 @@ def make_params(fn, start, end, interval, rng, offset=0, filter_nan=True, param0
     return Params(fid, int(bool(filter_nan)), start, end, interval, rng, offset, float(param0), float(param1))
 
 
-def range_query(p: Params, ts, val, sid, offsets, mode="flat", threads=1):
-    """Whole sub-plan, dense [S x T] + validity words.  mode in {"flat","faithful"}."""
+def range_query(p: Params, ts, val, sid, offsets, mode="flat", threads=1, rescan=False):
+    """Whole sub-plan, dense [S x T] + validity words.  mode in {"flat","faithful"}.  rescan=True evaluates every
+    window with the rescan restatement (range_udf(..., rescan=True)): rate / increase recompute the counter correction
+    per window instead of sliding it (extrapolate_rate.rs:216-238); every other function is unaffected."""
     ts, val = _i64(ts), _f64(val)
     offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
     S = offsets.size - 1
@@ -231,7 +234,7 @@ def range_query(p: Params, ts, val, sid, offsets, mode="flat", threads=1):
     valid = np.zeros((S, Tw), np.uint32)
     rc = lib().orc_range_query_mt(C.byref(p), _p(ts, C.c_int64), _p(val, C.c_double), _p(sid, C.c_uint32),
                                   _p(offsets, C.c_uint64), S, _p(out, C.c_double), _p(valid, C.c_uint32),
-                                  int(threads), 1 if mode == "faithful" else 0)
+                                  int(threads), (1 if mode == "faithful" else 0) | (2 if rescan else 0))
     if rc != 0:
         raise RuntimeError("orc_range_query_mt failed")
     return out, valid

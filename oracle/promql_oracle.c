@@ -668,9 +668,13 @@ static void scatter_series_result(const orc_params* p, size_t s, int64_t T, int6
   }
 }
 
+typedef void (*range_udf_fn)(int, const int64_t*, const double*, const uint32_t*, const uint32_t*, const int64_t*,
+                             size_t, int64_t, double, double, double*, uint8_t*);
+
 void orc_range_query_flat(const orc_params* p, const int64_t* ts, const double* val,
                           const uint64_t* offsets, size_t s_begin, size_t s_end, double* out,
-                          uint32_t* valid_words) {
+                          uint32_t* valid_words, int rescan) {
+  const range_udf_fn udf = rescan ? orc_range_udf_rescan : orc_range_udf;
   int64_t T = orc_num_steps(p->start, p->end, p->interval);
   int64_t Tw = (T + 31) / 32;
   size_t cap = 0;
@@ -697,7 +701,7 @@ void orc_range_query_flat(const orc_params* p, const int64_t* ts, const double* 
       if (len[j] != 0) all_empty = 0;
     if (nwin == 0 || all_empty) continue; /* range_manipulate.rs:641-643 */
     for (int64_t j = 0; j < nwin; j++) ets[j] = s2 + j * p->interval;
-    orc_range_udf(p->fn_id, nts, nval, off, len, ets, (size_t)nwin, p->range, p->param0, p->param1, r, v);
+    udf(p->fn_id, nts, nval, off, len, ets, (size_t)nwin, p->range, p->param0, p->param1, r, v);
     scatter_series_result(p, s, T, Tw, s2, nwin, r, v, out, valid_words);
   }
   free(nts); free(nval); free(off); free(len); free(ets); free(r); free(v);
@@ -705,7 +709,8 @@ void orc_range_query_flat(const orc_params* p, const int64_t* ts, const double* 
 
 void orc_range_query_faithful(const orc_params* p, const int64_t* ts, const double* val,
                               const uint32_t* sid, const uint64_t* offsets, size_t s_begin, size_t s_end,
-                              double* out, uint32_t* valid_words) {
+                              double* out, uint32_t* valid_words, int rescan) {
+  const range_udf_fn udf = rescan ? orc_range_udf_rescan : orc_range_udf;
   int64_t T = orc_num_steps(p->start, p->end, p->interval);
   int64_t Tw = (T + 31) / 32;
   for (size_t s = s_begin; s < s_end; s++) {
@@ -772,7 +777,7 @@ void orc_range_query_faithful(const orc_params* p, const int64_t* ts, const doub
       double* r = (double*)malloc((size_t)nwin * 8);
       uint8_t* v = (uint8_t*)malloc((size_t)nwin);
       if (same)
-        orc_range_udf(p->fn_id, n_ts, n_val, u_off, u_len, ets, (size_t)nwin, p->range, p->param0, p->param1, r, v);
+        udf(p->fn_id, n_ts, n_val, u_off, u_len, ets, (size_t)nwin, p->range, p->param0, p->param1, r, v);
       /* Filter value IS NOT NULL (planner.rs:1063): copies the surviving rows of every column */
       double* f_val = (double*)malloc((size_t)nwin * 8);
       int64_t* f_ts = (int64_t*)malloc((size_t)nwin * 8);
@@ -813,10 +818,12 @@ typedef struct {
 
 static void* mt_worker(void* arg) {
   mt_job* j = (mt_job*)arg;
-  if (j->faithful)
-    orc_range_query_faithful(j->p, j->ts, j->val, j->sid, j->offsets, j->s_begin, j->s_end, j->out, j->valid_words);
+  const int rescan = (j->faithful & ORC_RESCAN) != 0;
+  if (j->faithful & 1)
+    orc_range_query_faithful(j->p, j->ts, j->val, j->sid, j->offsets, j->s_begin, j->s_end, j->out, j->valid_words,
+                             rescan);
   else
-    orc_range_query_flat(j->p, j->ts, j->val, j->offsets, j->s_begin, j->s_end, j->out, j->valid_words);
+    orc_range_query_flat(j->p, j->ts, j->val, j->offsets, j->s_begin, j->s_end, j->out, j->valid_words, rescan);
   return NULL;
 }
 

@@ -140,15 +140,19 @@ double orc_holt_winters(const double* v, size_t n, double sf, double tf);
  * the ranges Vec + two packed-key arrays + T-long tag take (range_manipulate.rs:636-681), the UDF
  * loop, and the IS NOT NULL filter copy (planner.rs:1063).
  * orc_range_query_flat: algorithm only, flat arrays, no per-series allocation.
- * Both are sequential over [s_begin, s_end). rows of series s = [offsets[s], offsets[s+1]). */
+ * Both are sequential over [s_begin, s_end). rows of series s = [offsets[s], offsets[s+1]).
+ * rescan != 0 evaluates the windows with orc_range_udf_rescan (rate / increase recompute the counter
+ * correction of every window) instead of the reference's sliding orc_range_udf. */
 void orc_range_query_faithful(const orc_params* p, const int64_t* ts, const double* val,
                               const uint32_t* sid, const uint64_t* offsets, size_t s_begin, size_t s_end,
-                              double* out, uint32_t* valid_words);
+                              double* out, uint32_t* valid_words, int rescan);
 void orc_range_query_flat(const orc_params* p, const int64_t* ts, const double* val,
                           const uint64_t* offsets, size_t s_begin, size_t s_end, double* out,
-                          uint32_t* valid_words);
+                          uint32_t* valid_words, int rescan);
 /* pthread fan-out over series (hash-partition analogue of target_partitions, state.rs:125-128).
- * faithful != 0 selects orc_range_query_faithful. Returns 0 on success. */
+ * Bit 0 of `faithful` selects orc_range_query_faithful, bit ORC_RESCAN the rescan UDF.  Returns 0 on
+ * success. */
+#define ORC_RESCAN 2
 int orc_range_query_mt(const orc_params* p, const int64_t* ts, const double* val, const uint32_t* sid,
                        const uint64_t* offsets, size_t n_series, double* out, uint32_t* valid_words,
                        int n_threads, int faithful);
