@@ -34,6 +34,7 @@ EXPORTED_SYMBOLS = [
     "b2p_count_values_dev", "b2p_count_values", "b2p_plan_count_values_create",
     "b2p_subquery_dev", "b2p_subquery", "b2p_plan_subquery_create",
     "b2p_histogram_fold", "b2p_plan_histogram_quantile_create",
+    "b2p_sort_cells_dev", "b2p_sort_cells", "b2p_plan_sort_create",
 ]
 
 
@@ -144,6 +145,9 @@ def load() -> C.CDLL:
         "b2p_plan_subquery_create": (vp, [vp, C.c_char_p, P, vp]),
         "b2p_histogram_fold": (C.c_int, [vp, dbl, vp, vp, vp, u32, vp, vp, u32, u64, vp, vp]),
         "b2p_plan_histogram_quantile_create": (vp, [vp, C.c_char_p, dbl, vp]),
+        "b2p_sort_cells_dev": (C.c_int, [vp, i32, vp, vp, u32, u64, vp, vp]),
+        "b2p_sort_cells": (C.c_int, [vp, i32, vp, vp, u32, u64, vp, vp]),
+        "b2p_plan_sort_create": (vp, [vp, C.c_char_p, vp, C.POINTER(C.c_char_p), i32]),
         "b2p_plan_set_function": (C.c_int, [vp, C.c_char_p, C.POINTER(dbl), i32]),
         "b2p_plan_scalar_create": (vp, [vp, vp]),
     }

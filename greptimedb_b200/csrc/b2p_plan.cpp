@@ -1384,6 +1384,64 @@ void HistogramQuantilePlan::compute(NodeResult& r) {
   r.rows = H;
 }
 
+// ---- SortPlan ------------------------------------------------------------------------------------------
+SortPlan::SortPlan(b2p_ctx* ctx, const std::string& function, std::shared_ptr<PlanNode> child,
+                   std::vector<std::string> labels)
+    : PlanNode(ctx), child_(std::move(child)), labels_(std::move(labels)) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromSortExec: NULL context");
+  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromSortExec: NULL child");
+  if (function != "sort" && function != "sort_desc" && function != "sort_by_label" && function != "sort_by_label_desc")
+    throw PlanError(ErrorKind::Plan, "GpuPromSortExec: unknown function " + function);
+  by_label_ = function.compare(0, 13, "sort_by_label") == 0;
+  desc_ = function == "sort_desc" || function == "sort_by_label_desc";
+  // planner.rs:2743-2772: sort_by_label* needs at least one label (FunctionInvalidArgument)
+  if (by_label_ && labels_.empty()) throw PlanError(ErrorKind::Plan, "GpuPromSortExec: " + function + " needs at least one label");
+  if (!by_label_ && !labels_.empty()) throw PlanError(ErrorKind::Plan, "GpuPromSortExec: " + function + " takes no label");
+}
+
+void SortPlan::compute(NodeResult& r) {
+  child_->run(r);
+  // the reference carries count_values' counted value as a tag, which this layer does not model
+  if (r.columns == Columns::CountTagsTimeLabel)
+    throw PlanError(ErrorKind::Plan, "GpuPromSortExec: a count_values child is not supported by this node");
+  r.cell_order.clear();
+  if (r.columns == Columns::None) return;  // no columns, no rows: the same empty batch
+  r.columns = Columns::TimeValueTags;
+  const uint64_t T = (uint64_t)r.T;
+  if (!by_label_) {
+    if (r.rows == 0 || T == 0) return;
+    r.cell_order.resize((size_t)r.rows * (size_t)T);
+    uint64_t n = 0;
+    check(b2p_sort_cells(ctx_, desc_ ? 1 : 0, r.val.data(), r.valid.data(), r.rows, T, r.cell_order.data(), &n),
+          ErrorKind::Execution);
+    r.cell_order.resize((size_t)n);
+    return;
+  }
+  if (r.labels.id_keyed) throw PlanError(ErrorKind::Plan, "GpuPromSortExec: an id-keyed (__tsid) child has no label values to sort by");
+  std::vector<const std::vector<Label>*> cols;
+  for (const std::string& l : labels_) {
+    const int c = r.labels.column(l);
+    if (c < 0) throw PlanError(ErrorKind::Plan, "GpuPromSortExec: No field named " + l);
+    cols.push_back(&r.labels.values[(size_t)c]);
+  }
+  // arrow's Utf8 order: bytes (std::string compares chars as unsigned), "" first; NULL last in both directions
+  auto before = [&](uint32_t a, uint32_t b) {
+    for (const std::vector<Label>* col : cols) {
+      const Label &x = (*col)[a], &y = (*col)[b];
+      if (x == y) continue;
+      if (!x || !y) return !y;
+      return desc_ ? *y < *x : *x < *y;
+    }
+    return false;
+  };
+  std::vector<uint32_t> order(r.rows);
+  std::iota(order.begin(), order.end(), 0u);
+  std::stable_sort(order.begin(), order.end(), before);
+  for (uint32_t q : order)
+    for (uint64_t k = 0; k < T; ++k)
+      if (r.valid_at(q, (int64_t)k)) r.cell_order.push_back((uint64_t)q * T + k);
+}
+
 }  // namespace b2p
 
 // ---- C entry points -----------------------------------------------------------------------------------
@@ -1554,6 +1612,15 @@ b2p_plan* b2p_plan_histogram_quantile_create(b2p_ctx* ctx, const char* le_column
   return create([&] {
     if (!child) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
     return std::make_shared<b2p::HistogramQuantilePlan>(ctx, le_column ? le_column : "le", phi, child->node);
+  });
+}
+
+b2p_plan* b2p_plan_sort_create(b2p_ctx* ctx, const char* function, b2p_plan* child, const char* const* labels,
+                               int32_t n_labels) {
+  return create([&] {
+    if (!function || !child || n_labels < 0 || (n_labels > 0 && !labels))
+      throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    return std::make_shared<b2p::SortPlan>(ctx, function, child->node, strings(labels, n_labels));
   });
 }
 

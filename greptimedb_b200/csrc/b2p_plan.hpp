@@ -364,6 +364,26 @@ class HistogramQuantilePlan : public PlanNode {
   std::shared_ptr<PlanNode> child_;
 };
 
+// sort / sort_desc / sort_by_label / sort_by_label_desc (child [, labels]), GpuPromSortExec: the reference's
+// Projection(time index, value, tags..) -> Filter(value IS NOT NULL) -> Sort(keys) over the child (planner.rs:1060-1089,
+// 2743-2772).  The result is the child's (rows, row order, values and bits, so nodes above see the child) with its export
+// order in cell_order: the valid cells by value in the f64 total order (b2p_sort_cells, K14), or the rows ranked by the
+// listed labels on the host (byte order, NULL last in both directions) with each row's cells in step order; ties keep
+// row-major order.  Columns {time index, value, tags..}; a child without columns stays so.  Plan errors at execute:
+// sort_by_label* over a label the child lacks or an id-keyed child, and any sort over a count_values child.
+class SortPlan : public PlanNode {
+ public:
+  SortPlan(b2p_ctx* ctx, const std::string& function, std::shared_ptr<PlanNode> child, std::vector<std::string> labels);
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  bool desc_ = false, by_label_ = false;
+  std::shared_ptr<PlanNode> child_;
+  std::vector<std::string> labels_;
+};
+
 int function_id_from_name(const std::string& prom_name);  // -1 when unknown
 int aggregate_id_from_name(const std::string& name);      // -1 when unknown
 

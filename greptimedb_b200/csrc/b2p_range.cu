@@ -686,6 +686,22 @@ int b2p_range_group_sum_dev(b2p_ctx* c, const b2p_range_params* p, const int64_t
 /* ---- subqueries ---------------------------------------------------------------------------------------------- */
 }  // extern "C"
 
+// K13's count kernel, then CUB's exclusive scan of the counts in place (declared in b2p_runtime.cuh; K14 uses it too)
+int scan_valid_cells(b2p_ctx* c, const uint32_t* valid, uint64_t T, uint32_t rows, unsigned long long* offsets,
+                     DevBuf& tmp) {
+  size_t bytes = 0;
+  CU(cub::DeviceScan::ExclusiveSum(nullptr, bytes, offsets, offsets, (int)rows + 1, c->stream));
+  if (int rc = tmp.ensure(std::max<size_t>(bytes, 16))) return rc;
+  SubqueryArgs a{};
+  a.valid = valid; a.T = T; a.Tw = (uint32_t)((T + 31) / 32); a.rows = rows; a.offsets = offsets;
+  subquery_count_kernel<<<cell_rows_grid(c, rows), 256, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  bytes = tmp.cap;
+  CU(cub::DeviceScan::ExclusiveSum(tmp.p, bytes, offsets, offsets, (int)rows + 1, c->stream));
+  return B2P_OK;
+}
+
 namespace {
 // A range call of this context that reads the subquery scratch and whose verdict b2p_sync has not taken yet: b2p_sync
 // may run it again from the scratch (slow-path arena overflow), so the scratch must not change before that.
@@ -709,12 +725,9 @@ int subquery_run(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int
   const uint32_t Tw_in = (uint32_t)((T_inner + 31) / 32), Tw = (uint32_t)((T + 31) / 32);
   const uint32_t batch_rows = (uint32_t)std::min<uint64_t>(n_rows, std::max<uint64_t>(1, kSqBatchCells / T_inner));
   const uint64_t cells = (uint64_t)batch_rows * T_inner;
-  size_t scan_bytes = 0;
-  CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                   (int)batch_rows + 1, c->stream));
   if (subquery_scratch_pending(c) && (rc = b2p_sync(c))) return rc;
   if ((rc = c->sq_ts.ensure(cells * 8)) || (rc = c->sq_val.ensure(cells * 8)) ||
-      (rc = c->sq_off.ensure(((size_t)batch_rows + 1) * 8)) || (rc = c->sq_tmp.ensure(std::max<size_t>(scan_bytes, 16))))
+      (rc = c->sq_off.ensure(((size_t)batch_rows + 1) * 8)))
     return rc;
   b2p_range_params q = *p;
   for (uint32_t r0 = 0; r0 < n_rows; r0 += batch_rows) {
@@ -725,14 +738,9 @@ int subquery_run(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int
     a.T = T_inner; a.Tw = Tw_in; a.rows = nb;
     a.start = inner_start; a.interval = inner_interval;
     a.offsets = c->sq_off.as<unsigned long long>(); a.ts = c->sq_ts.as<int64_t>(); a.val = c->sq_val.as<double>();
-    const unsigned grid = std::max(1u, capped_grid(c, (uint64_t)nb * 32, 256, 8));
     stage_begin(c, 3);
-    subquery_count_kernel<<<grid, 256, 0, c->stream>>>(a);
-    c->launches++;
-    CU(cudaGetLastError());
-    size_t bytes = c->sq_tmp.cap;
-    CU(cub::DeviceScan::ExclusiveSum(c->sq_tmp.p, bytes, a.offsets, a.offsets, (int)nb + 1, c->stream));
-    subquery_scatter_kernel<<<grid, 256, 0, c->stream>>>(a);
+    if ((rc = scan_valid_cells(c, a.valid, T_inner, nb, a.offsets, c->sq_tmp))) return rc;
+    subquery_scatter_kernel<<<cell_rows_grid(c, nb), 256, 0, c->stream>>>(a);
     c->launches++;
     CU(cudaGetLastError());
     stage_end(c, 3);

@@ -6,6 +6,7 @@
 //   b2p_group.cu        group index, by-label aggregates, all-reduce of partials, HistogramFold, column reduce
 //   b2p_elementwise.cu  binary operators, instant-vector functions, scalar(), set operators
 //   b2p_aggregation.cu  topk / bottomk, quantile, count_values
+//   b2p_sort.cu         sort / sort_desc
 // There is NO CPU fallback anywhere: every entry point either launches the CUDA kernels or returns an error.
 #pragma once
 #include <cuda_runtime.h>
@@ -219,6 +220,8 @@ struct b2p_ctx {
   DevBuf v_keys, v_alt, v_rank, v_seg, v_group, v_tmp;
   // subquery: the sample rows of one batch of child rows (ts, val, offsets) and CUB's temp (bound in subquery_run)
   DevBuf sq_ts, sq_val, sq_off, sq_tmp;
+  // sort / sort_desc: row offsets, keys (double-buffered), the alternate cell buffer and CUB's temp (bound in sort_run)
+  DevBuf so_off, so_keys, so_cells, so_tmp;
   // resident CTAs per SM of each persistent kernel instantiation and dynamic shared-memory size (persistent_grid)
   std::map<std::pair<const void*, size_t>, int> blocks_per_sm;
 };
@@ -353,6 +356,15 @@ SeriesIn stage_series(Staging& s, const int64_t* ts, const double* val, const ui
 // ---- internals of one file that another one calls -----------------------------------------------------------------
 // b2p_range.cu: uploads the reciprocal table of the thread tier (b2p_kernel_t.cuh) to this module's constant memory
 int upload_rcp_table();
+// b2p_range.cu: K13's per-row count of the valid cells of a [rows x T] grid (bits past T ignored), then CUB's exclusive
+// scan in place: offsets[r] = the valid cells of the rows before r, offsets[rows] = the total.  `tmp` grows to CUB's temp.
+int scan_valid_cells(b2p_ctx* c, const uint32_t* valid, uint64_t T, uint32_t rows, unsigned long long* offsets,
+                     DevBuf& tmp);
+// the grid of a warp-per-row kernel over the rows of such a grid (256 threads per CTA)
+inline unsigned cell_rows_grid(const b2p_ctx* c, uint32_t rows) {
+  const unsigned g = capped_grid(c, (uint64_t)rows * 32, 256, 8);
+  return g ? g : 1u;
+}
 // b2p_group.cu: group -> member series CSR: stable radix sort of (gid, series index), then lower bounds per group
 int build_group_csr(b2p_ctx* c, const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint32_t* goff,
                     uint32_t* members);

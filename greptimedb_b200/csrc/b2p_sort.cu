@@ -1,0 +1,105 @@
+// b2p_sort.cu — sort / sort_desc of the C ABI (K14, b2p_sort.cuh): the valid cells of a [rows x T] grid as cell
+// indices in value order.
+#include <algorithm>
+
+#include <cub/device/device_radix_sort.cuh>
+
+#include "b2p_runtime.cuh"
+#include "b2p_sort.cuh"
+
+using namespace b2p;
+
+namespace {
+// K13's count and scan (scan_valid_cells), a read-back of the total (the radix sort takes its item count on the host:
+// the one synchronisation of the call), K14's scatter into (keys, out_cells), then CUB's stable radix sort of the pairs
+// over all 64 key bits.  The cell indices ping-pong between out_cells and the context's so_cells; if the sort ends in
+// the latter they are copied back.  Scratch (context buffers so_*): 8 B per row plus one (offsets), 24 B per valid cell
+// (two key buffers, one cell buffer) and CUB's temp storage.  *n_host is the number of valid cells.
+int sort_run(b2p_ctx* c, int desc, const double* vals, const uint32_t* valid, uint32_t rows, uint64_t T,
+             uint64_t* out_cells, uint64_t* out_n, uint64_t* n_host) {
+  int rc;
+  if ((rc = c->so_off.ensure(((size_t)rows + 1) * 8))) return rc;
+  unsigned long long* off = c->so_off.as<unsigned long long>();
+  if ((rc = scan_valid_cells(c, valid, T, rows, off, c->so_tmp))) return rc;
+  CU(cudaMemcpyAsync(out_n, off + rows, 8, cudaMemcpyDeviceToDevice, c->stream));
+  uint64_t n = 0;
+  CU(cudaMemcpyAsync(&n, off + rows, 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  *n_host = n;
+  if (n == 0) return B2P_OK;
+  if ((rc = c->so_keys.ensure(n * 16)) || (rc = c->so_cells.ensure(n * 8))) return rc;
+  SortArgs a{};
+  a.vals = vals; a.valid = valid; a.T = T; a.Tw = (uint32_t)((T + 31) / 32); a.rows = rows; a.desc = desc ? 1 : 0;
+  a.offsets = off;
+  a.keys = c->so_keys.as<unsigned long long>();
+  a.cells = reinterpret_cast<unsigned long long*>(out_cells);
+  sort_scatter_kernel<<<cell_rows_grid(c, rows), 256, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  cub::DoubleBuffer<unsigned long long> keys(a.keys, a.keys + n);
+  cub::DoubleBuffer<unsigned long long> cells(a.cells, c->so_cells.as<unsigned long long>());
+  size_t bytes = 0;
+  CU(cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys, cells, n, 0, 64, c->stream));
+  if ((rc = c->so_tmp.ensure(std::max<size_t>(bytes, 16)))) return rc;
+  bytes = c->so_tmp.cap;
+  CU(cub::DeviceRadixSort::SortPairs(c->so_tmp.p, bytes, keys, cells, n, 0, 64, c->stream));
+  if (cells.Current() != a.cells)
+    CU(cudaMemcpyAsync(a.cells, cells.Current(), n * 8, cudaMemcpyDeviceToDevice, c->stream));
+  return B2P_OK;
+}
+
+int check_sort_shape(uint32_t n_rows, uint64_t T) {
+  if (n_rows >= (uint32_t)INT32_MAX) return fail(B2P_E_TOO_LARGE, "sort: %u rows, at most %d", n_rows, INT32_MAX - 1);
+  if (T > 0 && n_rows > UINT64_MAX / 8 / T) return fail(B2P_E_TOO_LARGE, "sort: %u rows x %llu steps", n_rows,
+                                                        (unsigned long long)T);
+  return B2P_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_sort_cells_dev(b2p_ctx* c, int32_t desc, const double* vals, const uint32_t* valid, uint32_t n_rows,
+                       uint64_t T, uint64_t* out_cells, uint64_t* out_n) {
+  if (!c || !out_n) return fail(B2P_E_INVALID, "NULL argument");
+  if (int rc = check_sort_shape(n_rows, T)) return rc;
+  DeviceGuard g(c->device);
+  if (n_rows == 0 || T == 0) {
+    CU(cudaMemsetAsync(out_n, 0, 8, c->stream));
+    return B2P_OK;
+  }
+  if (!vals || !valid || !out_cells) return fail(B2P_E_INVALID, "NULL argument");
+  uint64_t n = 0;
+  stage_begin(c, 3);
+  const int rc = sort_run(c, desc, vals, valid, n_rows, T, out_cells, out_n, &n);
+  stage_end(c, 3);
+  return rc;
+}
+
+/* ---- host-pointer API ------------------------------------------------------------------------ */
+
+int b2p_sort_cells(b2p_ctx* c, int32_t desc, const double* vals, const uint32_t* valid, uint32_t n_rows, uint64_t T,
+                   uint64_t* out_cells, uint64_t* out_n) {
+  if (!c || !out_n) return fail(B2P_E_INVALID, "NULL argument");
+  if (int rc = check_sort_shape(n_rows, T)) return rc;
+  *out_n = 0;
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !out_cells) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const uint64_t cells = (uint64_t)n_rows * T, Tw = (T + 31) / 32;
+  int rc;
+  Staging s{c};
+  const double* d_vals = s.in(vals, cells * 8);
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
+  uint64_t* d_cells = static_cast<uint64_t*>(s.buf(cells * 8));
+  uint64_t* d_n = s.out(out_n, 8);
+  if ((rc = s.rc)) return rc;
+  uint64_t n = 0;
+  stage_begin(c, 3);
+  rc = sort_run(c, desc, d_vals, d_valid, n_rows, T, d_cells, d_n, &n);
+  stage_end(c, 3);
+  if (rc) return rc;
+  s.copy_back(out_cells, d_cells, n * 8);  // only the valid cells' entries
+  return s.finish();
+}
+
+}  // extern "C"

@@ -16,6 +16,8 @@
 #pragma once
 #include <cstdint>
 
+#include "b2p_cells.cuh"
+
 namespace b2p {
 
 constexpr uint64_t kSqBatchCells = 1ull << 27;  // grid cells of one batch of rows: 16 B each of scratch, 2.1 GB
@@ -33,9 +35,7 @@ struct SubqueryArgs {
 
 // bits of validity word w that are steps of the grid (a word past T's last step may carry stray bits)
 __device__ __forceinline__ uint32_t sq_word(const SubqueryArgs& a, uint64_t row, uint32_t w) {
-  const uint32_t word = __ldg(a.valid + row * a.Tw + w);
-  const uint32_t tail = (uint32_t)(a.T & 31);
-  return (w == a.Tw - 1 && tail) ? word & ((1u << tail) - 1u) : word;
+  return grid_word(a.valid, row, a.Tw, w, a.T);
 }
 
 __global__ void __launch_bounds__(256) subquery_count_kernel(const SubqueryArgs a) {

@@ -387,6 +387,20 @@ class Context:
                                          _ptr(valid), R, T_in, _ptr(out), _ptr(ov)))
         return out, ov
 
+    def sort_cells(self, desc, vals, valid):
+        """sort / sort_desc (desc) over any grid vals [R,T] / valid [R,Tw] u32: the valid cells' indices r * T + k in
+        value order (the f64 total order; equal values in row-major order) -> u64 [n valid cells]."""
+        vals = np.ascontiguousarray(vals, np.float64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        R, T = vals.shape
+        if valid.shape != (R, (T + 31) // 32):
+            raise ValueError(f"valid must be [{R}, {(T + 31) // 32}] u32 words, got {valid.shape}")
+        out = np.zeros(max(R * T, 1), np.uint64)
+        n = C.c_uint64(0)
+        self._check(self._L.b2p_sort_cells(self._h, int(bool(desc)), _ptr(vals), _ptr(valid), R, T, _ptr(out),
+                                           C.byref(n)))
+        return out[:n.value].copy()
+
     # -- device API (torch tensors or raw pointers; asynchronous) ----------------------------------
     def series_offsets_dev(self, sid, n_rows, n_series, offsets):
         self._check(self._L.b2p_series_offsets_dev(self._h, _ptr(sid), n_rows, n_series, _ptr(offsets)))
@@ -521,6 +535,12 @@ class Context:
         """Device form of subquery(): vals [n_rows,T_inner] / valid [n_rows,Tw'] into out [n_rows,T] / out_valid."""
         self._check(self._L.b2p_subquery_dev(self._h, C.byref(p), int(inner_start), int(inner_interval), _ptr(vals),
                                              _ptr(valid), n_rows, T_inner, _ptr(out), _ptr(out_valid)))
+
+    def sort_cells_dev(self, desc, vals, valid, n_rows, T, out_cells, out_n):
+        """Device form of sort_cells(): vals [n_rows,T] / valid [n_rows,Tw] into out_cells (room for n_rows * T u64, the
+        first out_n written) and out_n (one device u64).  Synchronises the context's stream once (the cell count)."""
+        self._check(self._L.b2p_sort_cells_dev(self._h, int(bool(desc)), _ptr(vals), _ptr(valid), n_rows, T,
+                                               _ptr(out_cells), _ptr(out_n)))
 
     def count_valid_words_dev(self, cnt, n_rows, T, valid_words):
         self._check(self._L.b2p_count_valid_words_dev(self._h, _ptr(cnt), n_rows, T, _ptr(valid_words)))

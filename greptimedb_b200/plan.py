@@ -7,7 +7,8 @@ pyarrow RecordBatches exactly like the reference's tests feed a MemoryExec.  `sc
 top of any node, `function` an instant-vector function (abs, clamp_min, prom_round, ...; the two chain in call order),
 `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels), `SetOpPlan` applies `and` / `or` / `unless`
 to two nodes, `ScalarPlan` is scalar(node), `TopkPlan` is topk / bottomk(k, node) [by | without (labels)],
-`SubqueryPlan` is fn(node[range:step]) and `HistogramQuantilePlan` is histogram_quantile(phi, node).
+`SubqueryPlan` is fn(node[range:step]), `HistogramQuantilePlan` is histogram_quantile(phi, node) and `SortPlan` is
+sort / sort_desc / sort_by_label / sort_by_label_desc(node).
 """
 from __future__ import annotations
 
@@ -267,5 +268,22 @@ class HistogramQuantilePlan(_PlanNode):
         self._ctx = ctx
         self._children = (child,)
         self._h = self._L.b2p_plan_histogram_quantile_create(ctx._h, le.encode(), float(phi), child._h)
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class SortPlan(_PlanNode):
+    """sort(child) / sort_desc(child) (function "sort" | "sort_desc": the cells by value in the f64 total order) or
+    sort_by_label(child, labels..) / sort_by_label_desc (the rows by the listed labels, byte order, NULL last); equal keys
+    keep the child's row-major order.  execute() emits {time index, value, tags..} in that order; nodes above see the
+    child's result unchanged.  The child stays usable and is kept alive by this node."""
+
+    def __init__(self, ctx: Context, function: str, child: _PlanNode, labels: Sequence[str] = ()):
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (child,)
+        labels = list(labels)
+        arr = _cstr_array(labels)
+        self._h = self._L.b2p_plan_sort_create(ctx._h, function.encode(), child._h, arr, len(labels))
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())

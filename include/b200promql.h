@@ -49,6 +49,8 @@
  *                              Sort(labels, ts, value), planner.rs:402-445
  *   b2p_subquery[_dev]         fn(<expr>[range:step]): RangeManipulate directly over the inner plan + Projection(prom_fn)
  *                              + Filter, planner.rs:292-332
+ *   b2p_sort_cells[_dev]       sort / sort_desc: Filter(value IS NOT NULL) -> Sort(value ASC | DESC, NULLS FIRST),
+ *                              planner.rs:1060-1089, 2743-2772
  *
  * Data layout (HBM, struct-of-arrays, all row-sorted by (series id, timestamp) exactly like
  * the reference's required_input_ordering, series_divide.rs:410-440):
@@ -385,6 +387,18 @@ B2P_API int b2p_subquery_dev(b2p_ctx* ctx, const b2p_range_params* p, int64_t in
                              const double* vals, const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, double* out,
                              uint32_t* out_valid);
 
+/* sort / sort_desc (K14; the reference's Sort(value ASC | DESC, NULLS FIRST) over the child's rows, planner.rs:1060-1089):
+ * the valid cells of vals / valid [n_rows x T] (bits past T in a row's last word are ignored) as cell indices
+ * row * T + k into out_cells, ordered by value in the f64 total order (-NaN < -inf < .. < -0.0 < +0.0 < .. < +inf <
+ * +NaN), ascending, or descending when desc != 0.  Equal values keep row-major order (row, then step) in both
+ * directions: a stable radix sort over the key total_key(v) ^ 2^63, bitwise inverted for desc.  out_cells has room for
+ * n_rows * T entries; the first *out_n (a device u64) are written.  The call reads the number of valid cells back
+ * once, so it synchronises the context's stream.  Scratch comes from the context (24 B per valid cell and 8 B per row,
+ * b2p_sort.cu, sort_run).  B2P_E_INVALID: a NULL argument; B2P_E_NOMEM: the scratch could not be allocated;
+ * B2P_E_TOO_LARGE: n_rows >= 2^31 - 1. */
+B2P_API int b2p_sort_cells_dev(b2p_ctx* ctx, int32_t desc, const double* vals, const uint32_t* valid, uint32_t n_rows,
+                               uint64_t T, uint64_t* out_cells, uint64_t* out_n);
+
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
  * the id column `sid` (ids sid_base .. sid_base + n_series - 1, non-decreasing), or copied from `offsets_in`
@@ -464,6 +478,11 @@ B2P_API int b2p_count_values(b2p_ctx* ctx, const double* vals, const uint32_t* v
 B2P_API int b2p_subquery(b2p_ctx* ctx, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval,
                          const double* vals, const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, double* out,
                          uint32_t* out_valid);
+
+/* Host-pointer form of b2p_sort_cells_dev (synchronous): the grid and its bitmap go to the device; out_cells (room for
+ * n_rows * T entries, the first *out_n written) and out_n are host pointers. */
+B2P_API int b2p_sort_cells(b2p_ctx* ctx, int32_t desc, const double* vals, const uint32_t* valid, uint32_t n_rows,
+                           uint64_t T, uint64_t* out_cells, uint64_t* out_n);
 
 /* Host-pointer forms of b2p_instant_fn_dev / b2p_scalar_calculate_dev (synchronous; device-found errors returned). */
 B2P_API int b2p_instant_fn(b2p_ctx* ctx, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
@@ -617,6 +636,20 @@ B2P_API b2p_plan* b2p_plan_subquery_create(b2p_ctx* ctx, const char* function, c
  * child, whose counted value would be one more Float64 tag of the fold in the reference, which this layer does not
  * model.  Ownership as for b2p_plan_binary_create.  NULL on error (b2p_plan_last_error). */
 B2P_API b2p_plan* b2p_plan_histogram_quantile_create(b2p_ctx* ctx, const char* le_column, double phi, b2p_plan* child);
+/* sort(child) / sort_desc(child) / sort_by_label(child, labels..) / sort_by_label_desc(child, labels..),
+ * GpuPromSortExec: the reference's Projection(time index, value, tags..) -> Filter(value IS NOT NULL) -> Sort(keys) over
+ * the child (planner.rs:1060-1089, 2743-2772).  `function` is "sort" (value ASC), "sort_desc" (value DESC), both NULLS
+ * FIRST in the f64 total order (b2p_sort_cells), "sort_by_label" or "sort_by_label_desc" (the listed labels in order,
+ * byte-wise, "" before every other string and NULL after every string in both directions, ranked on the host).
+ * Equal keys keep the child's row-major order (row, then step).  The export has columns {time index, value, tags..}
+ * (tags in the child's order, the value keeps the child's value name) in that order; a child that exports no columns
+ * gives the same empty result.  Nodes above see the child's result unchanged (rows, row order, values, bits);
+ * element-wise stages on this node apply after the order is fixed, and a cell whose bit a stage clears is not
+ * exported.  Plan errors at create (NULL is returned): an unknown function, sort_by_label* without a label, sort /
+ * sort_desc with labels.  Plan errors at execute: sort_by_label* naming a label the child lacks or over an id-keyed
+ * (__tsid) child, and any sort over a count_values child.  Ownership as for b2p_plan_binary_create. */
+B2P_API b2p_plan* b2p_plan_sort_create(b2p_ctx* ctx, const char* function, b2p_plan* child, const char* const* labels,
+                                       int32_t n_labels);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

@@ -320,6 +320,12 @@ extern "C" {
         ctx: *mut b2p_ctx, p: *const B2pRangeParams, inner_start: i64, inner_interval: i64, vals: *const f64,
         valid: *const u32, n_rows: u32, t_inner: u64, out: *mut f64, out_valid: *mut u32,
     ) -> c_int;
+    /// sort / sort_desc (K14): the valid cells of a device grid [n_rows x T] as cell indices row * T + k in value order
+    /// (f64 total order, ties in row-major order); `out_n` is a device u64.  Synchronises the context's stream once.
+    pub fn b2p_sort_cells_dev(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const f64, valid: *const u32, n_rows: u32, t: u64, out_cells: *mut u64,
+        out_n: *mut u64,
+    ) -> c_int;
 
     // ---- host-side helper (no device work): SeriesDivide + cadence scan of one sorted batch ---------------------------
     pub fn b2p_host_scan_series(
@@ -398,6 +404,11 @@ extern "C" {
         ctx: *mut b2p_ctx, p: *const B2pRangeParams, inner_start: i64, inner_interval: i64, vals: *const f64,
         valid: *const u32, n_rows: u32, t_inner: u64, out: *mut f64, out_valid: *mut u32,
     ) -> c_int;
+    /// Host-pointer form of b2p_sort_cells_dev (synchronous); `out_cells` has room for n_rows * T entries.
+    pub fn b2p_sort_cells(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const f64, valid: *const u32, n_rows: u32, t: u64, out_cells: *mut u64,
+        out_n: *mut u64,
+    ) -> c_int;
 
     // ---- plan-level API over the Arrow C Data Interface -----------------------------------------------------------------
     pub fn b2p_plan_range_create(
@@ -448,6 +459,11 @@ extern "C" {
     /// b2p_plan_binary_create.
     pub fn b2p_plan_histogram_quantile_create(
         ctx: *mut b2p_ctx, le_column: *const c_char, phi: f64, child: *mut b2p_plan,
+    ) -> *mut b2p_plan;
+    /// `function` ("sort" | "sort_desc" | "sort_by_label" | "sort_by_label_desc") over any node; `labels` for the
+    /// sort_by_label forms only.  Ownership of `child` as for b2p_plan_binary_create.
+    pub fn b2p_plan_sort_create(
+        ctx: *mut b2p_ctx, function: *const c_char, child: *mut b2p_plan, labels: *const *const c_char, n_labels: i32,
     ) -> *mut b2p_plan;
     /// MOVES the batch: on success the release callbacks now belong to the plan.
     pub fn b2p_plan_push_batch(plan: *mut b2p_plan, batch: *mut FFI_ArrowArray, schema: *mut FFI_ArrowSchema) -> c_int;

@@ -90,6 +90,14 @@
 //!                                           => `match_histogram_quantile`: the b2p_plan_histogram_quantile_create arguments
 //! ```
 //!
+//! sort / sort_desc / sort_by_label / sort_by_label_desc over a rewritten node (planner.rs:1060-1089, 2743-2772):
+//!
+//! ```text
+//!   [SortPreservingMergeExec <-] SortExec(value ASC | DESC NULLS FIRST  |  tags.. ASC | DESC NULLS LAST)
+//!     <- FilterExec(value IS NOT NULL) <- ProjectionExec(ts, value, tags..)
+//!     <- GpuPromRangeExec                     => `match_sort`: the b2p_plan_sort_create arguments
+//! ```
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
@@ -109,6 +117,7 @@ use datafusion::physical_plan::joins::HashJoinExec;
 use datafusion::physical_plan::projection::ProjectionExec;
 use datafusion::physical_plan::repartition::RepartitionExec;
 use datafusion::physical_plan::sorts::sort::SortExec;
+use datafusion::physical_plan::sorts::sort_preserving_merge::SortPreservingMergeExec;
 use datafusion::physical_plan::windows::BoundedWindowAggExec;
 use datafusion::physical_plan::ExecutionPlan;
 
@@ -300,6 +309,15 @@ pub struct GpuPromSubquerySpec {
 pub struct GpuPromHistogramQuantileSpec {
     pub le_column: String,
     pub phi: f64,
+    pub child: GpuPromRangeParams,
+}
+
+/// What `b2p_plan_sort_create` takes for a matched sort: the function ("sort" | "sort_desc" | "sort_by_label" |
+/// "sort_by_label_desc"), the labels of the sort_by_label forms in key order and the child node.
+#[derive(Debug, Clone)]
+pub struct GpuPromSortSpec {
+    pub function: String,
+    pub labels: Vec<String>,
     pub child: GpuPromRangeParams,
 }
 
@@ -616,6 +634,63 @@ impl GpuPromRewrite {
             return None;
         }
         Some(GpuPromHistogramQuantileSpec { le_column, phi: fold.quantile(), child: child.params().clone() })
+    }
+
+    /// `[SortPreservingMergeExec <-] SortExec(keys) <- FilterExec(value IS NOT NULL) <- ProjectionExec(ts, value, tags..)
+    /// <- GpuPromRangeExec` (planner.rs:1060-1089, 2743-2772) -> the arguments of `b2p_plan_sort_create`.  The keys must
+    /// be the value column alone, NULLS FIRST (ascending: sort, descending: sort_desc), or one or more tag columns of the
+    /// child, all in one direction, NULLS LAST (sort_by_label / sort_by_label_desc).  Any other key stays on the CPU: the
+    /// time index, a column that is not a tag, mixed directions or null orderings.  The projection must pass the time
+    /// index, the value and the tags through as plain columns.
+    pub fn match_sort(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromSortSpec> {
+        let plan = match plan.as_any().downcast_ref::<SortPreservingMergeExec>() {
+            Some(m) => m.input(),
+            None => plan,
+        };
+        let sort = plan.as_any().downcast_ref::<SortExec>()?;
+        let filter = sort.input().as_any().downcast_ref::<FilterExec>()?;
+        let not_null = filter.predicate().as_any().downcast_ref::<IsNotNullExpr>()?;
+        let value_index = not_null.arg().as_any().downcast_ref::<Column>()?.index();
+        let projection = filter.input().as_any().downcast_ref::<ProjectionExec>()?;
+        let child = projection.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let params = child.params();
+        let mut names = Vec::new();
+        for e in projection.expr() {
+            e.expr.as_any().downcast_ref::<Column>()?;
+            names.push(e.alias.clone());
+        }
+        let value = names.get(value_index)?.clone();
+        let keys: Vec<(String, bool, bool)> = sort
+            .expr()
+            .iter()
+            .map(|k| {
+                let c = k.expr.as_any().downcast_ref::<Column>()?;
+                Some((c.name().to_string(), k.options.descending, k.options.nulls_first))
+            })
+            .collect::<Option<_>>()?;
+        let (_, descending, nulls_first) = keys.first()?.clone();
+        if keys.iter().any(|(_, d, n)| *d != descending || *n != nulls_first) {
+            return None;
+        }
+        if keys.len() == 1 && keys[0].0 == value {
+            if !nulls_first {
+                return None;
+            }
+            let function = if descending { "sort_desc" } else { "sort" };
+            return Some(GpuPromSortSpec { function: function.to_string(), labels: vec![], child: params.clone() });
+        }
+        if nulls_first || params.tag_columns == [String::from("__tsid")] {
+            return None;
+        }
+        let mut labels = Vec::new();
+        for (name, _, _) in &keys {
+            if !params.tag_columns.iter().any(|t| t == name) || !names.iter().any(|n| n == name) {
+                return None;
+            }
+            labels.push(name.clone());
+        }
+        let function = if descending { "sort_by_label_desc" } else { "sort_by_label" };
+        Some(GpuPromSortSpec { function: function.to_string(), labels, child: params.clone() })
     }
 
     /// `ProjectionExec | FilterExec <- HashJoinExec(Inner, tags.. + ts)` over two `GpuPromRangeExec` -> the arguments of
