@@ -316,6 +316,20 @@ int count_values_run(b2p_ctx* c, const double* vals, const uint32_t* valid, cons
   }
   return B2P_OK;
 }
+
+// The end of a host call over a group index: stages gid, builds a temporary index of it, runs `dev(ix)`, finishes `s`
+// and destroys the index once the copies have completed.
+template <class Dev>
+int end_indexed(Staging& s, const uint32_t* gid, uint32_t n_rows, uint32_t n_groups, Dev&& dev) {
+  const uint32_t* d_gid = s.in(gid, (size_t)n_rows * 4);
+  b2p_group_index* ix = nullptr;
+  const int rc = s.end([&] {
+    const int r = b2p_group_index_create_dev(s.c, d_gid, n_rows, n_groups, &ix);
+    return r ? r : dev(ix);
+  });
+  b2p_group_index_destroy(s.c, ix);
+  return rc;
+}
 }  // namespace
 
 extern "C" {
@@ -367,70 +381,49 @@ int b2p_count_values_dev(b2p_ctx* c, const double* vals, const uint32_t* valid, 
 int b2p_topk(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uint32_t* valid, const uint32_t* gid,
              uint32_t n_rows, uint32_t n_groups, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  if (n_rows == 0 || T == 0) return B2P_OK;
-  if (!vals || !valid || !gid || !tie || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  if (n_rows == 0 || T == 0) return B2P_OK;  // (no group index to build)
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
-  int rc;
   Staging s{c};
   const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
-  uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);  // topk runs in place
-  const uint32_t* d_gid = s.in(gid, (size_t)n_rows * 4);
+  uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
   const uint32_t* d_tie = s.in(tie, (size_t)n_rows * 4);
-  s.copy_back(out_valid, d_valid, (size_t)n_rows * Tw * 4);
-  if ((rc = s.rc)) return rc;
-  b2p_group_index* ix = nullptr;
-  if ((rc = b2p_group_index_create_dev(c, d_gid, n_rows, n_groups, &ix))) return rc;
-  rc = b2p_topk_dev(c, bottom, k, d_vals, d_valid, ix, d_tie, T, d_valid);
-  if (!rc) rc = s.finish();
-  b2p_group_index_destroy(c, ix);
-  return rc;
+  uint32_t* d_out = s.copy_back(out_valid, d_valid, (size_t)n_rows * Tw * 4);  // topk runs in place
+  return end_indexed(s, gid, n_rows, n_groups, [&](const b2p_group_index* ix) {
+    return b2p_topk_dev(c, bottom, k, d_vals, d_valid, ix, d_tie, T, d_out);
+  });
 }
 
 int b2p_group_quantile(b2p_ctx* c, double phi, const double* vals, const uint32_t* valid, const uint32_t* gid,
                        uint32_t n_rows, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  if (n_groups == 0 || T == 0) return B2P_OK;
-  if ((n_rows && (!vals || !valid || !gid)) || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  if (n_groups == 0 || T == 0) return B2P_OK;  // (no group index to build)
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
-  int rc;
   Staging s{c};
   const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
   const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
-  const uint32_t* d_gid = s.in(gid, (size_t)n_rows * 4);
   double* d_out = s.out(out_val, (size_t)n_groups * T * 8);
   uint32_t* d_cnt = s.out(out_cnt, (size_t)n_groups * T * 4);
-  if ((rc = s.rc)) return rc;
-  b2p_group_index* ix = nullptr;
-  if ((rc = b2p_group_index_create_dev(c, d_gid, n_rows, n_groups, &ix))) return rc;
-  rc = b2p_group_quantile_dev(c, phi, d_vals, d_valid, ix, T, d_out, d_cnt);
-  if (!rc) rc = s.finish();
-  b2p_group_index_destroy(c, ix);
-  return rc;
+  return end_indexed(s, gid, n_rows, n_groups, [&](const b2p_group_index* ix) {
+    return b2p_group_quantile_dev(c, phi, d_vals, d_valid, ix, T, d_out, d_cnt);
+  });
 }
 
 int b2p_count_values(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* gid, uint32_t n_rows,
                      uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  if (n_rows == 0 || T == 0) return B2P_OK;
-  if (!vals || !valid || !gid || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  if (n_rows == 0 || T == 0) return B2P_OK;  // (no group index to build)
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
-  int rc;
   Staging s{c};
   const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
   const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
-  const uint32_t* d_gid = s.in(gid, (size_t)n_rows * 4);
   double* d_out = s.out(out_val, (size_t)n_rows * T * 8);
   uint32_t* d_cnt = s.out(out_cnt, (size_t)n_rows * T * 4);
-  if ((rc = s.rc)) return rc;
-  b2p_group_index* ix = nullptr;
-  if ((rc = b2p_group_index_create_dev(c, d_gid, n_rows, n_groups, &ix))) return rc;
-  rc = b2p_count_values_dev(c, d_vals, d_valid, ix, T, d_out, d_cnt);
-  if (!rc) rc = s.finish();
-  b2p_group_index_destroy(c, ix);
-  return rc;
+  return end_indexed(s, gid, n_rows, n_groups, [&](const b2p_group_index* ix) {
+    return b2p_count_values_dev(c, d_vals, d_valid, ix, T, d_out, d_cnt);
+  });
 }
 
 }  // extern "C"

@@ -321,12 +321,7 @@ int b2p_binary_op(b2p_ctx* c, int32_t op, int32_t return_bool, const double* lhs
                   const uint32_t* rhs_row, uint32_t n_rhs_rows, uint64_t n_pairs, uint64_t T, double* out,
                   uint32_t* out_valid) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  int rc;
-  if ((rc = check_binop(op, return_bool))) return rc;
-  if (n_pairs == 0 || T == 0) return B2P_OK;
-  if (!lhs_row || !rhs_row || !out || !out_valid || (n_lhs_rows && (!lhs || !lhs_valid)) ||
-      (n_rhs_rows && (!rhs || !rhs_valid)))
-    return fail(B2P_E_INVALID, "NULL argument");
+  if (int rc = check_binop(op, return_bool)) return rc;
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
   const size_t nl = n_lhs_rows, nr = n_rhs_rows, np = (size_t)n_pairs;
@@ -339,44 +334,37 @@ int b2p_binary_op(b2p_ctx* c, int32_t op, int32_t return_bool, const double* lhs
   const uint32_t* d_rhs_row = s.in(rhs_row, np * 4);
   double* d_out = s.out(out, np * T * 8);
   uint32_t* d_out_valid = s.out(out_valid, np * Tw * 4);
-  if ((rc = s.rc) ||
-      (rc = b2p_binary_op_dev(c, op, return_bool, d_lhs, d_lhs_valid, d_lhs_row, n_lhs_rows, d_rhs, d_rhs_valid,
-                              d_rhs_row, n_rhs_rows, n_pairs, T, d_out, d_out_valid)) ||
-      (rc = s.download()))
-    return rc;
-  return take_row_error(c, kBinRowError);  // (synchronises)
+  const int rc = s.end([&] {
+    return b2p_binary_op_dev(c, op, return_bool, d_lhs, d_lhs_valid, d_lhs_row, n_lhs_rows, d_rhs, d_rhs_valid,
+                             d_rhs_row, n_rhs_rows, n_pairs, T, d_out, d_out_valid);
+  }, false);
+  return rc ? rc : take_row_error(c, kBinRowError);  // (synchronises)
 }
 
 int b2p_scalar_op(b2p_ctx* c, int32_t op, int32_t return_bool, int32_t scalar_on_left, double scalar, const double* vals,
                   const uint32_t* valid, uint64_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  int rc;
-  if ((rc = check_binop(op, return_bool))) return rc;
-  if (n_rows == 0 || T == 0) return B2P_OK;
-  if (!vals || !valid || !out || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  if (int rc = check_binop(op, return_bool)) return rc;
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
   const size_t vb = (size_t)n_rows * T * 8, wb = (size_t)n_rows * Tw * 4;
   Staging s{c};
   double* d_vals = s.in(vals, vb);  // the operator runs in place
   uint32_t* d_valid = s.in(valid, wb);
-  s.copy_back(out, d_vals, vb);
-  s.copy_back(out_valid, d_valid, wb);
-  if ((rc = s.rc) ||
-      (rc = b2p_scalar_op_dev(c, op, return_bool, scalar_on_left, scalar, d_vals, d_valid, n_rows, T, d_vals, d_valid)))
-    return rc;
-  return s.finish();
+  double* d_out = s.copy_back(out, d_vals, vb);
+  uint32_t* d_out_valid = s.copy_back(out_valid, d_valid, wb);
+  return s.end([&] {
+    return b2p_scalar_op_dev(c, op, return_bool, scalar_on_left, scalar, d_vals, d_valid, n_rows, T, d_out, d_out_valid);
+  });
 }
 
 int b2p_setop(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key,
               uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid, const uint32_t* rhs_key,
               uint32_t n_rhs_rows, uint32_t n_keys, uint64_t T, double* out, uint32_t* out_valid) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  int rc;
-  if ((rc = check_setop_args(op, lhs, lhs_valid, lhs_key, n_lhs_rows, rhs, rhs_valid, rhs_key, n_rhs_rows, out,
-                             out_valid)))
+  if (int rc = check_setop_args(op, lhs, lhs_valid, lhs_key, n_lhs_rows, rhs, rhs_valid, rhs_key, n_rhs_rows, out,
+                                out_valid))
     return rc;
-  if (T == 0) return B2P_OK;
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
   const size_t nl = n_lhs_rows, nr = n_rhs_rows, no = op == kSetOr ? nl + nr : nl;
@@ -389,53 +377,44 @@ int b2p_setop(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_val
   const uint32_t* d_rhs_key = s.in(rhs_key, nr * 4);
   double* d_out = s.out(out, no * T * 8);
   uint32_t* d_out_valid = s.out(out_valid, no * Tw * 4);
-  if ((rc = s.rc) ||
-      (rc = b2p_setop_dev(c, op, d_lhs, d_lhs_valid, d_lhs_key, n_lhs_rows, d_rhs, d_rhs_valid, d_rhs_key, n_rhs_rows,
-                          n_keys, T, d_out, d_out_valid)) ||
-      (rc = s.download()))
-    return rc;
-  return take_row_error(c, kSetKeyError);  // (synchronises)
+  const int rc = s.end([&] {
+    return b2p_setop_dev(c, op, d_lhs, d_lhs_valid, d_lhs_key, n_lhs_rows, d_rhs, d_rhs_valid, d_rhs_key, n_rhs_rows,
+                         n_keys, T, d_out, d_out_valid);
+  }, false);
+  return rc ? rc : take_row_error(c, kSetKeyError);  // (synchronises)
 }
 
 int b2p_instant_fn(b2p_ctx* c, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
                    uint64_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  int rc, kfn;
+  int kfn;
   double lo, hi;
-  if ((rc = instant_fn_bounds(fn, arg0, arg1, &kfn, &lo, &hi))) return rc;
-  if (n_rows == 0 || T == 0) return B2P_OK;
-  if (!vals || !valid || !out || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  if (int rc = instant_fn_bounds(fn, arg0, arg1, &kfn, &lo, &hi)) return rc;
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
   const size_t vb = (size_t)n_rows * T * 8, wb = (size_t)n_rows * Tw * 4;
   Staging s{c};
   double* d_vals = s.in(vals, vb);  // the function runs in place; validity is unchanged
   uint32_t* d_valid = s.in(valid, wb);
-  s.copy_back(out, d_vals, vb);
-  if (out_valid != valid) s.copy_back(out_valid, d_valid, wb);
-  if ((rc = s.rc) || (rc = b2p_instant_fn_dev(c, fn, arg0, arg1, d_vals, d_valid, n_rows, T, d_vals, d_valid)))
-    return rc;
-  return s.finish();
+  double* d_out = s.copy_back(out, d_vals, vb);
+  uint32_t* d_out_valid = out_valid == valid ? d_valid : s.copy_back(out_valid, d_valid, wb);
+  return s.end([&] { return b2p_instant_fn_dev(c, fn, arg0, arg1, d_vals, d_valid, n_rows, T, d_out, d_out_valid); });
 }
 
 int b2p_scalar_calculate(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* row_key,
                          uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  if (T == 0) return B2P_OK;
-  if ((n_rows && (!vals || !valid || !row_key)) || !out || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
   const size_t Tw = (size_t)((T + 31) / 32);
-  int rc;
   Staging s{c};
   const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
   const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
   const uint32_t* d_key = s.in(row_key, (size_t)n_rows * 4);
   double* d_out = s.out(out, (size_t)T * 8);
   uint32_t* d_out_valid = s.out(out_valid, Tw * 4);
-  if ((rc = s.rc) || (rc = b2p_scalar_calculate_dev(c, d_vals, d_valid, d_key, n_rows, T, d_out, d_out_valid)) ||
-      (rc = s.download()))
-    return rc;
-  return take_row_error(c, kScalarKeyError | kScalarOverlapError);  // (synchronises)
+  const int rc =
+      s.end([&] { return b2p_scalar_calculate_dev(c, d_vals, d_valid, d_key, n_rows, T, d_out, d_out_valid); }, false);
+  return rc ? rc : take_row_error(c, kScalarKeyError | kScalarOverlapError);  // (synchronises)
 }
 
 }  // extern "C"

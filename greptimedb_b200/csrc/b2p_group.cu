@@ -311,11 +311,7 @@ int b2p_column_reduce_dev(b2p_ctx* c, const double* const* cols, uint32_t n_cols
 int b2p_group_aggregate(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* gid,
                         uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  if (agg < 0 || agg > B2P_AGG_STDVAR) return fail(B2P_E_INVALID, "unknown aggregator %d", agg);
-  if (n_groups == 0 || T == 0) return B2P_OK;
-  if (!vals || !valid_words || !gid || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
-  int rc;
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
   Staging s{c};
   const double* d_vals = s.in(vals, (size_t)n_series * T * 8);
@@ -323,22 +319,16 @@ int b2p_group_aggregate(b2p_ctx* c, int32_t agg, const double* vals, const uint3
   const uint32_t* d_gid = s.in(gid, (size_t)n_series * 4);
   double* d_out = s.out(out_val, (size_t)n_groups * T * 8);
   uint32_t* d_cnt = s.out(out_cnt, (size_t)n_groups * T * 4);
-  if ((rc = s.rc) ||
-      (rc = b2p_group_aggregate_dev(c, agg, d_vals, d_valid, d_gid, n_series, n_groups, T, d_out, d_cnt)))
-    return rc;
-  return s.finish();
+  return s.end([&] {
+    return b2p_group_aggregate_dev(c, agg, d_vals, d_valid, d_gid, n_series, n_groups, T, d_out, d_cnt);
+  });
 }
 
 int b2p_histogram_quantile(b2p_ctx* c, double phi, const double* le, uint32_t n_buckets, const double* rates,
                            const uint32_t* valid_words, uint32_t n_hist, uint64_t T, double* out,
                            uint32_t* out_valid_words) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  if (n_hist == 0 || T == 0) return B2P_OK;
-  if (!le || !rates || !valid_words || !out || !out_valid_words || n_buckets == 0)
-    return fail(B2P_E_INVALID, "NULL argument");
-  if ((uint64_t)n_hist * n_buckets > 0xffffffffull) return fail(B2P_E_TOO_LARGE, "more than 2^32 bucket series");
   DeviceGuard g(c->device);
-  int rc;
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
   const size_t ns = (size_t)n_hist * n_buckets;
   Staging s{c};
@@ -347,10 +337,9 @@ int b2p_histogram_quantile(b2p_ctx* c, double phi, const double* le, uint32_t n_
   const double* d_le = s.in(le, (size_t)n_buckets * 8);
   double* d_out = s.out(out, (size_t)n_hist * T * 8);
   uint32_t* d_out_valid = s.out(out_valid_words, (size_t)n_hist * Tw * 4);
-  if ((rc = s.rc) ||
-      (rc = b2p_histogram_quantile_dev(c, phi, d_le, n_buckets, d_rates, d_valid, n_hist, T, d_out, d_out_valid)))
-    return rc;
-  return s.finish();
+  return s.end([&] {
+    return b2p_histogram_quantile_dev(c, phi, d_le, n_buckets, d_rates, d_valid, n_hist, T, d_out, d_out_valid);
+  });
 }
 
 // HistogramFold over any [n_rows x T] grid: the index is checked on the host, so a bad one never reaches K5; then the
@@ -359,9 +348,8 @@ int b2p_histogram_fold(b2p_ctx* c, double phi, const uint32_t* hist_off, const u
                        const double* bucket_le, uint32_t n_hist, const double* rates, const uint32_t* valid_words,
                        uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid_words) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  if (n_hist == 0 || T == 0) return B2P_OK;
-  if (!hist_off || !bucket_series || !bucket_le || !rates || !valid_words || !out || !out_valid_words)
-    return fail(B2P_E_INVALID, "NULL argument");
+  if (n_hist == 0 || T == 0) return B2P_OK;  // (no fold: the index is not read)
+  if (!hist_off || !bucket_series) return fail(B2P_E_INVALID, "NULL argument");
   if (hist_off[0] != 0) return fail(B2P_E_INVALID, "hist_off[0] is %u, not 0", hist_off[0]);
   for (uint32_t h = 0; h < n_hist; ++h)
     if (hist_off[h + 1] < hist_off[h]) return fail(B2P_E_INVALID, "hist_off decreases at histogram %u", h);
@@ -370,7 +358,6 @@ int b2p_histogram_fold(b2p_ctx* c, double phi, const uint32_t* hist_off, const u
     if (bucket_series[i] >= n_rows)
       return fail(B2P_E_INVALID, "bucket_series[%zu] = %u is not a row (n_rows = %u)", i, bucket_series[i], n_rows);
   DeviceGuard g(c->device);
-  int rc;
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
   Staging s{c};
   const double* d_rates = s.in(rates, (size_t)n_rows * T * 8);
@@ -380,10 +367,10 @@ int b2p_histogram_fold(b2p_ctx* c, double phi, const uint32_t* hist_off, const u
   const double* d_bucket_le = s.in(bucket_le, nb * 8);
   double* d_out = s.out(out, (size_t)n_hist * T * 8);
   uint32_t* d_out_valid = s.out(out_valid_words, (size_t)n_hist * Tw * 4);
-  if ((rc = s.rc) || (rc = b2p_histogram_fold_dev(c, phi, d_hist_off, d_bucket_series, d_bucket_le, n_hist, d_rates,
-                                                  d_valid, T, d_out, d_out_valid)))
-    return rc;
-  return s.finish();
+  return s.end([&] {
+    return b2p_histogram_fold_dev(c, phi, d_hist_off, d_bucket_series, d_bucket_le, n_hist, d_rates, d_valid, T, d_out,
+                                  d_out_valid);
+  });
 }
 
 // histogram_quantile(phi, fn(bucket_series[range])) from host buffers to host rows without the dense [n_series x T]
@@ -397,10 +384,8 @@ int b2p_range_histogram_fold(b2p_ctx* c, const b2p_range_params* p, const int64_
   int64_t T = 0;
   int rc = check_grid(p, n_series, &T);
   if (rc) return rc;
-  if (n_hist == 0 || T == 0) return B2P_OK;
-  if (!sid && !offsets_host) return fail(B2P_E_INVALID, "need sid or offsets_host");
-  if (!hist_off || !bucket_series || !bucket_le || !out || !out_valid_words || ((!ts || !val) && n_rows))
-    return fail(B2P_E_INVALID, "NULL argument");
+  if (n_hist == 0 || T == 0) return B2P_OK;  // (no range evaluation whose rates nothing folds)
+  if (!hist_off) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
   if (!c->pending.empty() && (rc = b2p_sync(c))) return rc;
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
@@ -414,14 +399,12 @@ int b2p_range_histogram_fold(b2p_ctx* c, const b2p_range_params* p, const int64_
   uint32_t* d_rates_valid = static_cast<uint32_t*>(s.buf((size_t)n_series * Tw * 4));
   double* d_out = s.out(out, (size_t)n_hist * (size_t)T * 8);
   uint32_t* d_out_valid = s.out(out_valid_words, (size_t)n_hist * Tw * 4);
-  if ((rc = s.rc) ||
-      (rc = b2p_range_eval_dev(c, p, in.ts, in.val, in.offsets, n_rows, n_series, d_rates, d_rates_valid)) ||
-      (rc = b2p_sync(c)))  // slow-path fix-ups land before the fold reads
-    return rc;
-  if ((rc = b2p_histogram_fold_dev(c, phi, d_hist_off, d_bucket_series, d_bucket_le, n_hist, d_rates, d_rates_valid,
-                                   (uint64_t)T, d_out, d_out_valid)))
-    return rc;
-  return s.finish();
+  return s.end([&] {
+    int r = b2p_range_eval_dev(c, p, in.ts, in.val, in.offsets, n_rows, n_series, d_rates, d_rates_valid);
+    if (!r) r = b2p_sync(c);  // slow-path fix-ups land before the fold reads
+    return r ? r : b2p_histogram_fold_dev(c, phi, d_hist_off, d_bucket_series, d_bucket_le, n_hist, d_rates,
+                                          d_rates_valid, (uint64_t)T, d_out, d_out_valid);
+  });
 }
 
 }  // extern "C"

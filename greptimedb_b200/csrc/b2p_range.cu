@@ -561,10 +561,9 @@ static int range_call(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, 
 int b2p_range_udf_dev(b2p_ctx* c, int32_t fn_id, const int64_t* ts, const double* val, uint64_t n_rows,
                       const int64_t* packed_ranges, const int64_t* eval_ts, uint64_t n_win, int64_t range_length,
                       double param0, double param1, double* out, uint8_t* valid) {
-  (void)n_rows;
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   if (n_win == 0) return B2P_OK;
-  if (!packed_ranges || !out || !valid) return fail(B2P_E_INVALID, "NULL argument");
+  if (!packed_ranges || !out || !valid || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
   stage_begin(c, 1);
   const int rc = with_fn(fn_id, [&](auto k) {
@@ -581,7 +580,6 @@ int b2p_range_udf_dev(b2p_ctx* c, int32_t fn_id, const int64_t* ts, const double
 int b2p_instant_select_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
                            const int64_t* ts, const double* val, const uint64_t* offsets, uint64_t n_rows,
                            uint32_t n_series, double* out, uint32_t* valid_words) {
-  (void)n_rows;
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   b2p_range_params p{};
   p.start = start; p.end = end; p.interval = interval; p.range = lookback;
@@ -589,7 +587,7 @@ int b2p_instant_select_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t inter
   int rc = check_grid(&p, n_series, &T);
   if (rc) return rc;
   if (n_series == 0 || T == 0) return B2P_OK;
-  if (!offsets || !out || !valid_words) return fail(B2P_E_INVALID, "NULL argument");
+  if (!offsets || !out || !valid_words || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
   InstantArgs a{};
   a.start = start; a.end = end; a.interval = interval; a.lookback = lookback; a.offset = offset;
@@ -795,6 +793,7 @@ int b2p_synth_fill_dev(b2p_ctx* c, uint64_t series_begin, uint64_t n_series, uin
 
 SeriesIn stage_series(Staging& s, const int64_t* ts, const double* val, const uint32_t* sid, uint32_t sid_base,
                       const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series) {
+  if (!sid && !offsets_host && !s.rc) s.rc = fail(B2P_E_INVALID, "need sid or offsets_host");
   SeriesIn in{s.in(ts, n_rows * 8), s.in(val, n_rows * 8), nullptr};
   if (offsets_host) {
     in.offsets = s.in(offsets_host, ((size_t)n_series + 1) * 8);
@@ -1127,10 +1126,7 @@ int b2p_range_udf(b2p_ctx* c, int32_t fn_id, const int64_t* ts, const double* va
                   const int64_t* packed_ranges, const int64_t* eval_ts, uint64_t n_win, int64_t range_length,
                   double param0, double param1, double* out, uint8_t* valid) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  if (n_win == 0) return B2P_OK;
-  if (!packed_ranges || !out || !valid || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
-  int rc;
   Staging s{c};
   const int64_t* d_ts = s.in(ts, n_rows * 8);
   const double* d_val = s.in(val, n_rows * 8);
@@ -1138,10 +1134,10 @@ int b2p_range_udf(b2p_ctx* c, int32_t fn_id, const int64_t* ts, const double* va
   const int64_t* d_eval_ts = s.in(eval_ts, n_win * 8);
   double* d_out = s.out(out, n_win * 8);
   uint8_t* d_valid = s.out(valid, n_win);
-  if ((rc = s.rc) || (rc = b2p_range_udf_dev(c, fn_id, d_ts, d_val, n_rows, d_packed, d_eval_ts, n_win, range_length,
-                                             param0, param1, d_out, d_valid)))
-    return rc;
-  return s.finish();
+  return s.end([&] {
+    return b2p_range_udf_dev(c, fn_id, d_ts, d_val, n_rows, d_packed, d_eval_ts, n_win, range_length, param0, param1,
+                             d_out, d_valid);
+  });
 }
 
 int b2p_instant_select(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
@@ -1151,34 +1147,26 @@ int b2p_instant_select(b2p_ctx* c, int64_t start, int64_t end, int64_t interval,
   b2p_range_params p{};
   p.start = start; p.end = end; p.interval = interval; p.range = lookback;
   int64_t T = 0;
-  int rc = check_grid(&p, n_series, &T);
-  if (rc) return rc;
-  if (n_series == 0 || T == 0) return B2P_OK;
-  if (!sid && !offsets_host) return fail(B2P_E_INVALID, "need sid or offsets_host");
-  if (!out || !valid_words || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
+  if (int rc = check_grid(&p, n_series, &T)) return rc;
+  if (n_series == 0 || T == 0) return B2P_OK;  // (no sample copies, no series offsets)
   DeviceGuard g(c->device);
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
   Staging s{c};
   const SeriesIn in = stage_series(s, ts, val, sid, 0u, offsets_host, n_rows, n_series);
   double* d_out = s.out(out, (size_t)n_series * (size_t)T * 8);
   uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
-  if ((rc = s.rc) ||
-      (rc = b2p_instant_select_dev(c, start, end, interval, lookback, offset, in.ts, in.val, in.offsets, n_rows,
-                                   n_series, d_out, d_valid)) ||
-      (rc = b2p_sync(c)))
-    return rc;
-  return s.finish();
+  return s.end([&] {
+    const int rc = b2p_instant_select_dev(c, start, end, interval, lookback, offset, in.ts, in.val, in.offsets, n_rows,
+                                          n_series, d_out, d_valid);
+    return rc ? rc : b2p_sync(c);
+  });
 }
 
 int b2p_subquery(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval, const double* vals,
                  const uint32_t* valid, uint32_t n_rows, uint64_t T_inner, double* out, uint32_t* out_valid) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   int64_t T = 0;
-  int rc = check_grid(p, n_rows, &T);
-  if (rc) return rc;
-  if (n_rows == 0 || T == 0) return b2p_subquery_dev(c, p, inner_start, inner_interval, nullptr, nullptr, 0, 0, nullptr,
-                                                     nullptr);  // (the argument checks only)
-  if (!out || !out_valid || (T_inner && (!vals || !valid))) return fail(B2P_E_INVALID, "NULL argument");
+  if (int rc = check_grid(p, n_rows, &T)) return rc;
   DeviceGuard g(c->device);
   const size_t Tw_in = (size_t)((T_inner + 31) / 32), Tw = (size_t)((T + 31) / 32);
   Staging s{c};
@@ -1186,11 +1174,11 @@ int b2p_subquery(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int
   const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw_in * 4);
   double* d_out = s.out(out, (size_t)n_rows * (size_t)T * 8);
   uint32_t* d_valid_out = s.out(out_valid, (size_t)n_rows * Tw * 4);
-  if ((rc = s.rc) ||
-      (rc = b2p_subquery_dev(c, p, inner_start, inner_interval, d_vals, d_valid, n_rows, T_inner, d_out, d_valid_out)) ||
-      (rc = b2p_sync(c)))
-    return rc;
-  return s.finish();
+  return s.end([&] {
+    const int rc = b2p_subquery_dev(c, p, inner_start, inner_interval, d_vals, d_valid, n_rows, T_inner, d_out,
+                                    d_valid_out);
+    return rc ? rc : b2p_sync(c);
+  });
 }
 
 }  // extern "C"

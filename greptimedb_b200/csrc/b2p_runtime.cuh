@@ -296,6 +296,8 @@ int check_grid(const b2p_range_params* p, uint32_t n_series, int64_t* T_out);
 // Device copies of one synchronous host call's columns, in the context's staging buffers: the i-th buffer handed out
 // is c->stage[i].  Inputs are copied to the device as they are handed out; the results noted by out() / copy_back()
 // go back to the host, in that order, in download().  The first failure sticks in `rc` (later calls hand out NULL).
+// An absent (NULL) host column is handed out as NULL and queues nothing, so the device form's argument check rejects
+// it.  A host call reads: stage the inputs, stage the outputs, end() with the device form.
 struct Staging {
   static constexpr int kOutputs = 2;  // a host call returns two columns
   b2p_ctx* c;
@@ -320,27 +322,38 @@ struct Staging {
     if (d && bytes) cuda(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, c->stream), "host-to-device copy");
     return static_cast<T*>(d);
   }
-  void copy_back(void* host, const void* dev, size_t bytes) {
+  // `dev` as the result buffer of `host` (copied there by download()); NULL for an absent one
+  template <class T>
+  T* copy_back(T* host, T* dev, size_t bytes) {
+    if (!host) return nullptr;
     if (!rc && n_back == kOutputs) rc = fail(B2P_E_INVALID, "host call returns more than %d columns", kOutputs);
     if (!rc) back[n_back++] = Back{host, dev, bytes};
+    return dev;
   }
-  // a result buffer, copied to `host` by download()
+  // a result buffer, copied to `host` by download(); NULL for an absent one
   template <class T>
   T* out(T* host, size_t bytes) {
-    T* d = static_cast<T*>(buf(bytes));
-    copy_back(host, d, bytes);
-    return d;
+    return host ? copy_back(host, static_cast<T*>(buf(bytes)), bytes) : nullptr;
   }
-  int download() {
+  int download() {  // the results noted since the last download()
     for (int i = 0; !rc && i < n_back; ++i)
       if (back[i].bytes)
         cuda(cudaMemcpyAsync(back[i].host, back[i].dev, back[i].bytes, cudaMemcpyDeviceToHost, c->stream),
              "device-to-host copy");
+    n_back = 0;
     return rc;
   }
   int finish() {  // download() and wait for it
     if (!download()) cuda(cudaStreamSynchronize(c->stream), "cudaStreamSynchronize");
     return rc;
+  }
+  // The end of a host call: `dev()` (the device form, and whatever has to follow it before the results are read),
+  // skipped once staging has failed so that its error stands; then finish(), or only download() when `wait` is false
+  // and the caller synchronises by itself.  Returns the first error.
+  template <class Dev>
+  int end(Dev&& dev, bool wait = true) {
+    if (!rc) rc = dev();
+    return wait ? finish() : download();
   }
 };
 

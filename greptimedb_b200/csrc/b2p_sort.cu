@@ -79,26 +79,17 @@ int b2p_sort_cells_dev(b2p_ctx* c, int32_t desc, const double* vals, const uint3
 
 int b2p_sort_cells(b2p_ctx* c, int32_t desc, const double* vals, const uint32_t* valid, uint32_t n_rows, uint64_t T,
                    uint64_t* out_cells, uint64_t* out_n) {
-  if (!c || !out_n) return fail(B2P_E_INVALID, "NULL argument");
-  if (int rc = check_sort_shape(n_rows, T)) return rc;
-  *out_n = 0;
-  if (n_rows == 0 || T == 0) return B2P_OK;
-  if (!vals || !valid || !out_cells) return fail(B2P_E_INVALID, "NULL argument");
+  if (!c) return fail(B2P_E_INVALID, "NULL argument");
+  if (int rc = check_sort_shape(n_rows, T)) return rc;  // (before the cell column is sized)
   DeviceGuard g(c->device);
   const uint64_t cells = (uint64_t)n_rows * T, Tw = (T + 31) / 32;
-  int rc;
   Staging s{c};
   const double* d_vals = s.in(vals, cells * 8);
   const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
-  uint64_t* d_cells = static_cast<uint64_t*>(s.buf(cells * 8));
+  uint64_t* d_cells = out_cells ? static_cast<uint64_t*>(s.buf(cells * 8)) : nullptr;
   uint64_t* d_n = s.out(out_n, 8);
-  if ((rc = s.rc)) return rc;
-  uint64_t n = 0;
-  stage_begin(c, 3);
-  rc = sort_run(c, desc, d_vals, d_valid, n_rows, T, d_cells, d_n, &n);
-  stage_end(c, 3);
-  if (rc) return rc;
-  s.copy_back(out_cells, d_cells, n * 8);  // only the valid cells' entries
+  if (int rc = s.end([&] { return b2p_sort_cells_dev(c, desc, d_vals, d_valid, n_rows, T, d_cells, d_n); })) return rc;
+  s.copy_back(out_cells, d_cells, *out_n * 8);  // only the valid cells' entries, now that their count is here
   return s.finish();
 }
 

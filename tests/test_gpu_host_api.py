@@ -333,69 +333,124 @@ def test_setop(pair, op, L, R, K, T):
 # ---- a NULL host column where there is work -------------------------------------------------------------------------
 
 def host_calls(ctx):
-    """name -> (C entry point, arguments, index of the host column to pass as NULL, the two output columns)"""
+    """name -> (C entry point, arguments before the outputs, index of the input column to pass as NULL, the output
+    columns as (shape, dtype, initial value), index of the output column to pass as NULL)"""
     from greptimedb_b200 import make_params, pack_ranges
     from greptimedb_b200.engine import _ptr as P
     ts, val, sid, offsets = samples(99, 20)
     S, T, Tw = 20, 32, 1
     p = make_params("rate", T0, grid_end(T), 30_000, 120_000)
+    p_sub = make_params("sum_over_time", T0, grid_end(T), 30_000, 120_000, filter_nan=False)
     vals, words = dense(5, S, T)
     rates = np.abs(vals)
     gid = (np.arange(S) % 4).astype(np.uint32)
     rows = np.arange(S, dtype=np.uint32)
     keys = (np.arange(S) % 6).astype(np.uint32)
+    tie = rows[::-1].copy()
     hist_off, bucket_series, bucket_le = fold_index(4, 5)
     packed = pack_ranges(np.stack([np.arange(10) * 3, np.full(10, 5)], axis=1))
     H = ctx._h
+    f8, u4 = np.float64, np.uint32
+    grid = lambda n, m=Tw: [((n, T), f8, -1.0), ((n, m), u4, 7)]
     calls = {
-        "range_eval": ("b2p_range_eval", [H, C.byref(p), P(ts), P(val), P(sid), None, ts.size, S], 2, (S, T), (S, Tw)),
+        "range_eval": ("b2p_range_eval", [H, C.byref(p), P(ts), P(val), P(sid), None, ts.size, S], 2, grid(S), 0),
         "range_udf": ("b2p_range_udf", [H, 0, P(ts), P(val), ts.size, P(packed), None, 10, 60_000, 0.0, 0.0], 2,
-                      (10,), None),
+                      [((10,), f8, -1.0), ((10,), np.uint8, 7)], 1),
         "instant_select": ("b2p_instant_select", [H, T0, grid_end(T), 30_000, 300_000, 0, P(ts), P(val), None,
-                                                  P(offsets), ts.size, S], 6, (S, T), (S, Tw)),
-        "group_aggregate": ("b2p_group_aggregate", [H, 0, P(vals), P(words), P(gid), S, 4, T], 2, (4, T), (4, T)),
+                                                  P(offsets), ts.size, S], 6, grid(S), 0),
+        "group_aggregate": ("b2p_group_aggregate", [H, 0, P(vals), P(words), P(gid), S, 4, T], 2, grid(4, T), 1),
         "histogram_quantile": ("b2p_histogram_quantile", [H, 0.5, P(bucket_le), 5, P(rates), P(words), 4,
-                                                          T], 4, (4, T), (4, Tw)),
+                                                          T], 4, grid(4), 0),
+        "histogram_fold": ("b2p_histogram_fold", [H, 0.5, P(hist_off), P(bucket_series), P(bucket_le), 4, P(rates),
+                                                  P(words), S, T], 6, grid(4), 1),
         "range_histogram_fold": ("b2p_range_histogram_fold", [H, C.byref(p), P(ts), P(val), P(sid), None, ts.size, S,
                                                               0.5, P(hist_off), P(bucket_series), P(bucket_le), 4],
-                                 11, (4, T), (4, Tw)),
+                                 11, grid(4), 0),
         "binary_op": ("b2p_binary_op", [H, 0, 0, P(vals), P(words), P(rows), S, P(vals), P(words), P(rows), S, S, T],
-                      8, (S, T), (S, Tw)),
-        "scalar_op": ("b2p_scalar_op", [H, 0, 0, 0, 1.5, P(vals), P(words), S, T], 6, (S, T), (S, Tw)),
-        "setop": ("b2p_setop", [H, 0, P(vals), P(words), P(keys), S, P(vals), P(words), P(keys), S, 6, T], 4, (S, T),
-                  (S, Tw)),
+                      8, grid(S), 1),
+        "scalar_op": ("b2p_scalar_op", [H, 0, 0, 0, 1.5, P(vals), P(words), S, T], 6, grid(S), 0),
+        "setop": ("b2p_setop", [H, 0, P(vals), P(words), P(keys), S, P(vals), P(words), P(keys), S, 6, T], 4, grid(S),
+                  1),
+        "instant_fn": ("b2p_instant_fn", [H, 3, 0.0, 0.0, P(rates), P(words), S, T], 4, grid(S), 1),
+        "scalar_calculate": ("b2p_scalar_calculate", [H, P(vals), P(words), P(rows), S, T], 3,
+                             [((T,), f8, -1.0), ((Tw,), u4, 7)], 0),
+        "topk": ("b2p_topk", [H, 0, 3.0, P(vals), P(words), P(gid), S, 4, P(tie), T], 5, [((S, Tw), u4, 7)], 0),
+        "group_quantile": ("b2p_group_quantile", [H, 0.25, P(vals), P(words), P(gid), S, 4, T], 2, grid(4, T), 1),
+        "count_values": ("b2p_count_values", [H, P(vals), P(words), P(gid), S, 4, T], 3, grid(S, T), 0),
+        "subquery": ("b2p_subquery", [H, C.byref(p_sub), T0 - 60_000, 15_000, P(vals), P(words), S, T], 4, grid(S),
+                     1),
+        # (the cell count starts at 0: a rejected call may leave an empty result's count)
+        "sort_cells": ("b2p_sort_cells", [H, 0, P(vals), P(words), S, T], 3,
+                       [((S * T,), np.uint64, 7), ((1,), np.uint64, 0)], 1),
     }
-    keep = (ts, val, sid, offsets, vals, rates, words, gid, rows, keys, hist_off, bucket_series, bucket_le, packed, p)
+    keep = (ts, val, sid, offsets, vals, rates, words, gid, rows, keys, tie, hist_off, bucket_series, bucket_le, packed,
+            p, p_sub)
     return calls, keep
 
 
-def run(ctx, fn, args, out_shape, words_shape):
-    """one call with fresh output columns (range_udf's validity is one byte per window) -> (rc, out, valid)"""
+def run(ctx, fn, args, outs, null_out=None):
+    """one call with fresh output columns, output `null_out` passed as NULL -> (rc, the output columns)"""
     from greptimedb_b200.engine import _ptr
-    out = np.full(out_shape, -1.0)
-    valid = np.full(words_shape, 7, np.uint32) if words_shape else np.full(out_shape, 7, np.uint8)
+    cols = [np.full(shape, init, dtype) for shape, dtype, init in outs]
+    ptrs = [None if i == null_out else _ptr(col) for i, col in enumerate(cols)]
     tail = [None] if fn == "b2p_range_eval" else []  # (out_ts)
-    return getattr(ctx._L, fn)(*args, _ptr(out), _ptr(valid), *tail), out, valid
+    return getattr(ctx._L, fn)(*args, *ptrs, *tail), cols
 
 
-@pytest.mark.parametrize("name", ["range_eval", "range_udf", "instant_select", "group_aggregate", "histogram_quantile",
-                                  "range_histogram_fold", "binary_op", "scalar_op", "setop"])
+HOST_FORMS = ["range_eval", "range_udf", "instant_select", "group_aggregate", "histogram_quantile",
+              "range_histogram_fold", "binary_op", "scalar_op", "setop", "instant_fn", "scalar_calculate", "topk",
+              "group_quantile", "count_values", "subquery", "histogram_fold", "sort_cells"]
+
+
+@pytest.mark.parametrize("name", HOST_FORMS + [f"{n}:out" for n in HOST_FORMS])
 def test_null_host_column_is_rejected_and_the_context_stays_usable(name):
+    """a call with one NULL input column (`<form>:out`: output column) where there is work fails with B2P_E_INVALID
+    and writes nothing; the same call with every column then gives the same bits as before it"""
+    form, _, output = name.partition(":")
     ctx = _ctx()
     try:
         calls, _keep = host_calls(ctx)
-        fn, args, null_at, out_shape, words_shape = calls[name]
-        rc, out0, valid0 = run(ctx, fn, args, out_shape, words_shape)
+        fn, args, null_in, outs, null_out = calls[form]
+        rc, good = run(ctx, fn, args, outs)
         assert rc == 0, ctx._L.b2p_last_error().decode()
         bad = list(args)
-        bad[null_at] = None
-        rc, out1, valid1 = run(ctx, fn, bad, out_shape, words_shape)
+        if not output:
+            bad[null_in] = None
+        rc, cols = run(ctx, fn, bad, outs, null_out if output else None)
         assert rc == E_INVALID and "NULL" in ctx._L.b2p_last_error().decode()
-        assert (out1 == -1.0).all() and (valid1 == 7).all()  # nothing was written
-        rc, out2, valid2 = run(ctx, fn, args, out_shape, words_shape)
+        for col, (_, _, init) in zip(cols, outs):
+            assert (col == init).all()  # nothing was written
+        rc, again = run(ctx, fn, args, outs)
         assert rc == 0, ctx._L.b2p_last_error().decode()
-        np.testing.assert_array_equal(out2.view(np.uint64), out0.view(np.uint64))
-        np.testing.assert_array_equal(valid2, valid0)
+        for a, b in zip(again, good):
+            np.testing.assert_array_equal(a.view(f"u{a.itemsize}"), b.view(f"u{b.itemsize}"))
+    finally:
+        ctx.close()
+
+
+# ---- the device forms check the sample columns themselves ------------------------------------------------------------
+
+@pytest.mark.parametrize("column", ["ts", "val"])
+def test_null_sample_column_of_a_device_form_is_rejected(column):
+    """range_udf / instant_select on the device with a NULL sample column and rows to read: B2P_E_INVALID, no launch"""
+    import torch
+    from greptimedb_b200 import pack_ranges
+    from greptimedb_b200.engine import _ptr
+    ctx = _ctx(torch_stream=True)
+    try:
+        ts, val, _sid, offsets = samples(3, 8)
+        cols = {"ts": dev(ts), "val": dev(val)}
+        cols[column] = None
+        packed = dev(pack_ranges(np.stack([np.arange(4) * 2, np.full(4, 3)], axis=1)))
+        out, valid = zeros(4, torch.float64), zeros(4, torch.uint8)
+        rc = ctx._L.b2p_range_udf_dev(ctx._h, 0, _ptr(cols["ts"]), _ptr(cols["val"]), ts.size, _ptr(packed), None, 4,
+                                      60_000, 0.0, 0.0, _ptr(out), _ptr(valid))
+        assert rc == E_INVALID and "NULL" in ctx._L.b2p_last_error().decode()
+        out, valid = zeros(8 * 32, torch.float64), zeros(8, torch.int32)
+        rc = ctx._L.b2p_instant_select_dev(ctx._h, T0, grid_end(32), 30_000, 300_000, 0, _ptr(cols["ts"]),
+                                           _ptr(cols["val"]), _ptr(dev(offsets)), ts.size, 8, _ptr(out), _ptr(valid))
+        assert rc == E_INVALID and "NULL" in ctx._L.b2p_last_error().decode()
+        assert ctx._L.b2p_sync(ctx._h) == 0, ctx._L.b2p_last_error().decode()
     finally:
         ctx.close()
 
