@@ -35,6 +35,7 @@ EXPORTED_SYMBOLS = [
     "b2p_subquery_dev", "b2p_subquery", "b2p_plan_subquery_create",
     "b2p_histogram_fold", "b2p_plan_histogram_quantile_create",
     "b2p_sort_cells_dev", "b2p_sort_cells", "b2p_plan_sort_create",
+    "b2p_absent_dev", "b2p_absent", "b2p_plan_absent_create",
 ]
 
 
@@ -148,6 +149,10 @@ def load() -> C.CDLL:
         "b2p_sort_cells_dev": (C.c_int, [vp, i32, vp, vp, u32, u64, vp, vp]),
         "b2p_sort_cells": (C.c_int, [vp, i32, vp, vp, u32, u64, vp, vp]),
         "b2p_plan_sort_create": (vp, [vp, C.c_char_p, vp, C.POINTER(C.c_char_p), i32]),
+        "b2p_absent_dev": (C.c_int, [vp, vp, u32, u64, vp, vp]),
+        "b2p_absent": (C.c_int, [vp, vp, u32, u64, vp, vp]),
+        "b2p_plan_absent_create": (vp, [vp, i64, i64, i64, C.c_char_p, C.c_char_p, C.POINTER(C.c_char_p),
+                                        C.POINTER(C.c_char_p), i32, vp]),
         "b2p_plan_set_function": (C.c_int, [vp, C.c_char_p, C.POINTER(dbl), i32]),
         "b2p_plan_scalar_create": (vp, [vp, vp]),
     }

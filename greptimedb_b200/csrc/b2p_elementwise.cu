@@ -1,8 +1,10 @@
-// b2p_elementwise.cu — per-cell entry points of the C ABI: binary operators, instant-vector functions, scalar() and the
-// set operators `and` / `or` / `unless`.
+// b2p_elementwise.cu — per-cell entry points of the C ABI: binary operators, instant-vector functions, scalar(),
+// absent() and the set operators `and` / `or` / `unless`.
+#include <algorithm>
 #include <cfloat>
 
 #include "b2p_runtime.cuh"
+#include "b2p_absent.cuh"
 #include "b2p_binary.cuh"
 #include "b2p_instant.cuh"
 #include "b2p_setop.cuh"
@@ -98,6 +100,33 @@ int scalar_calculate_run(b2p_ctx* c, const ScalarArgs& a0) {
     CU(cudaGetLastError());
   }
   scalar_write_kernel<<<capped_grid(c, a.Tw, 8, 16), 256, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// absent(): steps up to 32 * (2^32 - 1), so that a row's validity words are counted in 32 bits
+int check_absent_shape(uint64_t T) {
+  if (T > 32ull * UINT32_MAX) return fail(B2P_E_TOO_LARGE, "absent: %llu steps, at most 32 x (2^32 - 1)", (unsigned long long)T);
+  return B2P_OK;
+}
+
+// K15: acc = 0, the OR pass over the rows' validity words (none without rows: every step is absent), the write pass.
+// Scratch: 4 B per output word (ab_acc).
+int absent_run(b2p_ctx* c, const uint32_t* valid, uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
+  AbsentArgs a{};
+  a.valid = valid; a.rows = n_rows; a.T = T; a.Tw = (uint32_t)((T + 31) / 32); a.out = out; a.out_valid = out_valid;
+  if (int rc = c->ab_acc.ensure((size_t)a.Tw * 4)) return rc;
+  a.acc = c->ab_acc.as<uint32_t>();
+  CU(cudaMemsetAsync(a.acc, 0, (size_t)a.Tw * 4, c->stream));
+  if (n_rows > 0) {
+    // at least 4 words per thread, at most 8 CTAs per SM; the kernel sweeps whole rows beyond that
+    const unsigned grid = std::max(1u, capped_grid(c, (uint64_t)n_rows * a.Tw, kAbsentThreads * 4, 8));
+    absent_or_kernel<<<grid, kAbsentThreads, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+  }
+  absent_write_kernel<<<capped_grid(c, a.Tw, 8, 16), 256, 0, c->stream>>>(a);
   c->launches++;
   CU(cudaGetLastError());
   return B2P_OK;
@@ -295,6 +324,18 @@ int b2p_scalar_calculate_dev(b2p_ctx* c, const double* vals, const uint32_t* val
   return rc;
 }
 
+int b2p_absent_dev(b2p_ctx* c, const uint32_t* valid, uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (int rc = check_absent_shape(T)) return rc;
+  if ((n_rows && !valid) || (T && (!out || !out_valid))) return fail(B2P_E_INVALID, "NULL argument");
+  if (T == 0) return B2P_OK;
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  const int rc = absent_run(c, valid, n_rows, T, out, out_valid);
+  stage_end(c, 3);
+  return rc;
+}
+
 /* ---- set operators ------------------------------------------------------------------------------------------- */
 
 int b2p_setop_dev(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key,
@@ -415,6 +456,18 @@ int b2p_scalar_calculate(b2p_ctx* c, const double* vals, const uint32_t* valid, 
   const int rc =
       s.end([&] { return b2p_scalar_calculate_dev(c, d_vals, d_valid, d_key, n_rows, T, d_out, d_out_valid); }, false);
   return rc ? rc : take_row_error(c, kScalarKeyError | kScalarOverlapError);  // (synchronises)
+}
+
+int b2p_absent(b2p_ctx* c, const uint32_t* valid, uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (int rc = check_absent_shape(T)) return rc;
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  Staging s{c};
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
+  double* d_out = s.out(out, (size_t)T * 8);
+  uint32_t* d_out_valid = s.out(out_valid, Tw * 4);
+  return s.end([&] { return b2p_absent_dev(c, d_valid, n_rows, T, d_out, d_out_valid); });
 }
 
 }  // extern "C"

@@ -9,6 +9,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <numeric>
 #include <unordered_map>
 
@@ -1442,6 +1443,50 @@ void SortPlan::compute(NodeResult& r) {
       if (r.valid_at(q, (int64_t)k)) r.cell_order.push_back((uint64_t)q * T + k);
 }
 
+// ---- AbsentPlan ----------------------------------------------------------------------------------------
+AbsentPlan::AbsentPlan(b2p_ctx* ctx, Millisecond start, Millisecond end, Millisecond interval, std::string time_index,
+                       std::string value_column, const std::vector<std::pair<std::string, std::string>>& labels,
+                       std::shared_ptr<PlanNode> child)
+    : PlanNode(ctx), start_(start), end_(end), interval_(interval), time_index_(std::move(time_index)),
+      value_column_(std::move(value_column)), child_(std::move(child)) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromAbsentExec: NULL context");
+  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromAbsentExec: NULL child");
+  if (interval_ <= 0) throw PlanError(ErrorKind::Plan, "GpuPromAbsentExec: interval must be positive");
+  // Absent::try_new: the fake labels collected into a HashMap (the last value of a name wins), sorted by name
+  std::map<std::string, std::string> by_name;
+  for (const auto& [name, value] : labels) {
+    if (name == time_index_ || name == value_column_)
+      throw PlanError(ErrorKind::Plan, "GpuPromAbsentExec: the label " + name + " is named like the time index or the value column");
+    by_name[name] = value;
+  }
+  labels_.assign(by_name.begin(), by_name.end());
+}
+
+void AbsentPlan::compute(NodeResult& r) {
+  NodeResult C;
+  child_->run(C);
+  r = NodeResult();
+  r.T = b2p_num_steps(start_, end_, interval_);
+  r.Tw = (uint32_t)((r.T + 31) / 32);
+  r.rows = 1;
+  r.eval_ts.resize((size_t)r.T);
+  for (int64_t k = 0; k < r.T; ++k) r.eval_ts[(size_t)k] = start_ + k * interval_;
+  // the reference's cursor walks this grid and skips a step only when a child timestamp equals it
+  if (C.rows > 0 && C.eval_ts != r.eval_ts)
+    throw PlanError(ErrorKind::Plan, "GpuPromAbsentExec: the child's eval timestamps are not the grid (start, end, interval)");
+  r.val.assign((size_t)r.T, 0.0);
+  r.valid.assign((size_t)r.Tw, 0u);
+  if (r.T > 0)
+    check(b2p_absent(ctx_, C.rows > 0 ? C.valid.data() : nullptr, C.rows, (uint64_t)r.T, r.val.data(), r.valid.data()),
+          ErrorKind::Execution);
+  r.time_index = time_index_;
+  r.value_name = value_column_;
+  for (const auto& [name, value] : labels_) {
+    r.labels.names.push_back(name);
+    r.labels.values.push_back({Label(value)});
+  }
+}
+
 }  // namespace b2p
 
 // ---- C entry points -----------------------------------------------------------------------------------
@@ -1621,6 +1666,22 @@ b2p_plan* b2p_plan_sort_create(b2p_ctx* ctx, const char* function, b2p_plan* chi
     if (!function || !child || n_labels < 0 || (n_labels > 0 && !labels))
       throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
     return std::make_shared<b2p::SortPlan>(ctx, function, child->node, strings(labels, n_labels));
+  });
+}
+
+b2p_plan* b2p_plan_absent_create(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval, const char* time_index,
+                                 const char* value_column, const char* const* label_names,
+                                 const char* const* label_values, int32_t n_labels, b2p_plan* child) {
+  return create([&] {
+    if (!time_index || !value_column || !child || (n_labels > 0 && (!label_names || !label_values)))
+      throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    if (n_labels < 0) throw b2p::PlanError(b2p::ErrorKind::Plan, "n_labels < 0");
+    std::vector<std::pair<std::string, std::string>> labels;
+    for (int32_t i = 0; i < n_labels; ++i) {
+      if (!label_names[i] || !label_values[i]) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL label name or value");
+      labels.emplace_back(label_names[i], label_values[i]);
+    }
+    return std::make_shared<b2p::AbsentPlan>(ctx, start, end, interval, time_index, value_column, labels, child->node);
   });
 }
 

@@ -384,6 +384,29 @@ class SortPlan : public PlanNode {
   std::vector<std::string> labels_;
 };
 
+// absent(child), GpuPromAbsentExec: the reference's PromAbsentExec(start, end, interval, time index, value column, fake
+// labels) over Aggregate(ts, first_value) -> Sort(ts) of the child (create_absent_plan, planner.rs:3186-3245; absent.rs).
+// One row over the grid start + k * interval <= end, valid with the value 1.0 at every step at which no child row has a
+// valid cell (b2p_absent, K15; NaN cells count as present).  Its labels are the fake labels: a name given twice keeps
+// its last value (the reference's HashMap collect), ordered by name byte-wise.  Columns {time index, value, labels..}.
+// The child is any node; only its validity is read, so an id-keyed or count_values child is fine.  Plan error at
+// execute: a child with rows whose eval timestamps are not this node's grid.
+class AbsentPlan : public PlanNode {
+ public:
+  AbsentPlan(b2p_ctx* ctx, Millisecond start, Millisecond end, Millisecond interval, std::string time_index,
+             std::string value_column, const std::vector<std::pair<std::string, std::string>>& labels,
+             std::shared_ptr<PlanNode> child);
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  Millisecond start_, end_, interval_;
+  std::string time_index_, value_column_;
+  std::vector<std::pair<std::string, std::string>> labels_;  // by name, one per name
+  std::shared_ptr<PlanNode> child_;
+};
+
 int function_id_from_name(const std::string& prom_name);  // -1 when unknown
 int aggregate_id_from_name(const std::string& name);      // -1 when unknown
 

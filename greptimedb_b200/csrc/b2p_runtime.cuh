@@ -4,7 +4,7 @@
 //   b2p_context.cu      create / destroy, streams, counters, errors, NCCL communicator
 //   b2p_range.cu        range tiers, series offsets, range / instant selectors, fused sum by, subqueries
 //   b2p_group.cu        group index, by-label aggregates, all-reduce of partials, HistogramFold, column reduce
-//   b2p_elementwise.cu  binary operators, instant-vector functions, scalar(), set operators
+//   b2p_elementwise.cu  binary operators, instant-vector functions, scalar(), absent(), set operators
 //   b2p_aggregation.cu  topk / bottomk, quantile, count_values
 //   b2p_sort.cu         sort / sort_desc
 // There is NO CPU fallback anywhere: every entry point either launches the CUDA kernels or returns an error.
@@ -211,6 +211,8 @@ struct b2p_ctx {
   DevBuf s_goff[2], s_members[2], s_mask;
   // scalar(): the reduction's verdict (struct ScalarState), read by the write pass on the device
   DevBuf sc_state;
+  // absent(): the OR over rows of each validity word of the child's grid (b2p_absent.cuh; bound in absent_run)
+  DevBuf ab_acc;
   // topk / bottomk: chunk and merge tables, candidate lists, selection state (b2p_topk.cuh; bound in topk_run)
   DevBuf t_table, t_cand, t_state;
   // quantile: chunk table, state and histograms of the groups of several chunks (b2p_quantile.cuh; bound in quantile_run)

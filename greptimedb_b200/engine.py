@@ -401,6 +401,18 @@ class Context:
                                            C.byref(n)))
         return out[:n.value].copy()
 
+    def absent(self, valid, T):
+        """absent() over any grid's validity valid [R,Tw] u32 with T steps -> (out [T] f64, out_valid [Tw] u32): the steps
+        at which no row has a valid cell (bits past T ignored), with the value 1.0; 0.0 and a clear bit elsewhere."""
+        valid = np.ascontiguousarray(valid, np.uint32)
+        Tw = (T + 31) // 32
+        if valid.ndim != 2 or valid.shape[1] != Tw:
+            raise ValueError(f"valid must be [rows, {Tw}] u32 words, got {valid.shape}")
+        out = np.zeros(T, np.float64)
+        ov = np.zeros(Tw, np.uint32)
+        self._check(self._L.b2p_absent(self._h, _ptr(valid), valid.shape[0], T, _ptr(out), _ptr(ov)))
+        return out, ov
+
     # -- device API (torch tensors or raw pointers; asynchronous) ----------------------------------
     def series_offsets_dev(self, sid, n_rows, n_series, offsets):
         self._check(self._L.b2p_series_offsets_dev(self._h, _ptr(sid), n_rows, n_series, _ptr(offsets)))
@@ -541,6 +553,10 @@ class Context:
         first out_n written) and out_n (one device u64).  Synchronises the context's stream once (the cell count)."""
         self._check(self._L.b2p_sort_cells_dev(self._h, int(bool(desc)), _ptr(vals), _ptr(valid), n_rows, T,
                                                _ptr(out_cells), _ptr(out_n)))
+
+    def absent_dev(self, valid, n_rows, T, out, out_valid):
+        """Device form of absent(): valid [n_rows,Tw] into out [T] / out_valid [Tw].  No host round trip."""
+        self._check(self._L.b2p_absent_dev(self._h, _ptr(valid), n_rows, T, _ptr(out), _ptr(out_valid)))
 
     def count_valid_words_dev(self, cnt, n_rows, T, valid_words):
         self._check(self._L.b2p_count_valid_words_dev(self._h, _ptr(cnt), n_rows, T, _ptr(valid_words)))

@@ -7,8 +7,8 @@ pyarrow RecordBatches exactly like the reference's tests feed a MemoryExec.  `sc
 top of any node, `function` an instant-vector function (abs, clamp_min, prom_round, ...; the two chain in call order),
 `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels), `SetOpPlan` applies `and` / `or` / `unless`
 to two nodes, `ScalarPlan` is scalar(node), `TopkPlan` is topk / bottomk(k, node) [by | without (labels)],
-`SubqueryPlan` is fn(node[range:step]), `HistogramQuantilePlan` is histogram_quantile(phi, node) and `SortPlan` is
-sort / sort_desc / sort_by_label / sort_by_label_desc(node).
+`SubqueryPlan` is fn(node[range:step]), `HistogramQuantilePlan` is histogram_quantile(phi, node), `SortPlan` is
+sort / sort_desc / sort_by_label / sort_by_label_desc(node) and `AbsentPlan` is absent(node).
 """
 from __future__ import annotations
 
@@ -285,5 +285,25 @@ class SortPlan(_PlanNode):
         labels = list(labels)
         arr = _cstr_array(labels)
         self._h = self._L.b2p_plan_sort_create(ctx._h, function.encode(), child._h, arr, len(labels))
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class AbsentPlan(_PlanNode):
+    """absent(child): one row over the grid start, start + interval, .. <= end with the value 1.0 at every step at which
+    no child row has a valid cell (NaN counts as present).  `labels` are the (name, value) equality matchers of the
+    argument's selector in matcher order: a name given twice keeps its last value, names are ordered byte-wise.
+    execute() emits {time_index, value_column, labels..}.  The child is any node, built on the same grid when it has
+    rows; it stays usable and is kept alive by this node."""
+
+    def __init__(self, ctx: Context, child: _PlanNode, start: int, end: int, interval: int, time_index: str,
+                 value_column: str, labels: Sequence[tuple] = ()):
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (child,)
+        labels = list(labels)
+        names, values = _cstr_array([n for n, _ in labels]), _cstr_array([v for _, v in labels])
+        self._h = self._L.b2p_plan_absent_create(ctx._h, int(start), int(end), int(interval), time_index.encode(),
+                                                 value_column.encode(), names, values, len(labels), child._h)
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())

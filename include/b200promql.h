@@ -37,6 +37,8 @@
  *   b2p_instant_fn[_dev]       instant-vector math functions: the Projection of planner.rs:2368-2413 (DataFusion math
  *                              builtins, prom_round round.rs:52-105, clamp / clamp_min / clamp_max clamp.rs:75-325)
  *   b2p_scalar_calculate[_dev] scalar(): ScalarCalculateStream, scalar_calculate.rs:532-637
+ *   b2p_absent[_dev]           absent(): AbsentStream over Aggregate(ts, first_value) -> Sort(ts), absent.rs,
+ *                              planner.rs:3186-3245
  *   b2p_setop[_dev]            set operators: `and` / `unless` = left.distinct() LeftSemi / LeftAnti HashJoinExec on
  *                              (key columns, time index), planner.rs:3549-3703; `or` = UnionDistinctOnExec,
  *                              planner.rs:3707-3906, union_distinct_on.rs:338-577; the key match is done by the caller
@@ -337,6 +339,14 @@ B2P_API int b2p_instant_fn_dev(b2p_ctx* ctx, int32_t fn /* enum b2p_ifn */, doub
  * b2p_sync).  No host round trip between the two passes. */
 B2P_API int b2p_scalar_calculate_dev(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const uint32_t* row_key,
                                      uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
+/* absent(v) (K15), the reference's AbsentStream (absent.rs) over the grid of its child: the steps at which no row has a
+ * valid cell.  out_valid [Tw] word w = ~(OR over rows of valid[r * Tw + w]) with the bits past T cleared, and out [T]
+ * = 1.0 where that bit is set, 0.0 elsewhere.  A valid cell counts whatever its value (NaN included); the values are
+ * never read, only the validity words (bits past T in a row's last word are ignored).  No rows: every step is set.
+ * Asynchronous: no host round trip; scratch is 4 B per output word from the context.  valid may be NULL only when
+ * n_rows == 0, out / out_valid only when T == 0.  B2P_E_INVALID: a NULL argument; B2P_E_TOO_LARGE: T > 32 * (2^32 - 1). */
+B2P_API int b2p_absent_dev(b2p_ctx* ctx, const uint32_t* valid, uint32_t n_rows, uint64_t T, double* out,
+                           uint32_t* out_valid);
 
 /* topk(k, v) / bottomk(k, v) per (group, step) over a dense grid whose rows are grouped by `index` (a row whose group id
  * is >= n_groups belongs to no group and keeps nothing).  A cell's rank key is (value in the f64 total order, tie[row]),
@@ -489,6 +499,10 @@ B2P_API int b2p_instant_fn(b2p_ctx* ctx, int32_t fn, double arg0, double arg1, c
                            uint64_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
 B2P_API int b2p_scalar_calculate(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const uint32_t* row_key,
                                  uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
+/* Host-pointer form of b2p_absent_dev (synchronous): valid [n_rows x Tw], out [T] and out_valid [Tw] are host
+ * pointers. */
+B2P_API int b2p_absent(b2p_ctx* ctx, const uint32_t* valid, uint32_t n_rows, uint64_t T, double* out,
+                       uint32_t* out_valid);
 
 /* ---- plan-level API over the Arrow C Data Interface ------------------------------------------------
  * GpuPromRangeExec: the whole sub-tree SeriesDivide -> SeriesNormalize -> RangeManipulate ->
@@ -650,6 +664,22 @@ B2P_API b2p_plan* b2p_plan_histogram_quantile_create(b2p_ctx* ctx, const char* l
  * (__tsid) child, and any sort over a count_values child.  Ownership as for b2p_plan_binary_create. */
 B2P_API b2p_plan* b2p_plan_sort_create(b2p_ctx* ctx, const char* function, b2p_plan* child, const char* const* labels,
                                        int32_t n_labels);
+/* absent(child), GpuPromAbsentExec: the reference's PromAbsentExec(start, end, interval, time index, value column, fake
+ * labels) over Aggregate(ts, first_value(value)) -> Sort(ts) of the child (create_absent_plan, planner.rs:3186-3245;
+ * absent.rs).  One row over the grid start + k * interval <= end (none when start > end) with the value 1.0 at every
+ * step at which no row of the child has a valid cell (a NaN cell counts as present; b2p_absent).  The labels are the
+ * (label_names[i], label_values[i]) pairs, the equality matchers of the argument's selector in matcher order: a name
+ * given twice keeps its last value, names are ordered byte-wise, an empty value is kept; the child's own labels play
+ * no part.  The export has columns {time_index, value_column, labels..}, Utf8 labels.  The child is any node: one without
+ * rows (or without columns) is absent at every step; an id-keyed or a count_values child is fine, because only its
+ * validity is read.  Nodes above see one row with these labels; element-wise stages on this node apply to it.  Plan
+ * errors at create (NULL is returned): a NULL ctx, child, name or label, interval <= 0, n_labels < 0, a label named like
+ * time_index or value_column.  Plan error at execute: a child with rows whose eval timestamps are not this node's
+ * grid.  Ownership as for b2p_plan_binary_create. */
+B2P_API b2p_plan* b2p_plan_absent_create(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval,
+                                         const char* time_index, const char* value_column,
+                                         const char* const* label_names, const char* const* label_values,
+                                         int32_t n_labels, b2p_plan* child);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

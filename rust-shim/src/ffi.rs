@@ -326,6 +326,11 @@ extern "C" {
         ctx: *mut b2p_ctx, desc: i32, vals: *const f64, valid: *const u32, n_rows: u32, t: u64, out_cells: *mut u64,
         out_n: *mut u64,
     ) -> c_int;
+    /// absent (K15): out_valid [Tw] = the steps at which no row of the device grid's validity [n_rows x Tw] has a bit
+    /// (bits past T cleared), out [T] = 1.0 there and 0.0 elsewhere.  Only validity words are read; no host round trip.
+    pub fn b2p_absent_dev(
+        ctx: *mut b2p_ctx, valid: *const u32, n_rows: u32, t: u64, out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- host-side helper (no device work): SeriesDivide + cadence scan of one sorted batch ---------------------------
     pub fn b2p_host_scan_series(
@@ -409,6 +414,10 @@ extern "C" {
         ctx: *mut b2p_ctx, desc: i32, vals: *const f64, valid: *const u32, n_rows: u32, t: u64, out_cells: *mut u64,
         out_n: *mut u64,
     ) -> c_int;
+    /// Host-pointer form of b2p_absent_dev (synchronous).
+    pub fn b2p_absent(
+        ctx: *mut b2p_ctx, valid: *const u32, n_rows: u32, t: u64, out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
 
     // ---- plan-level API over the Arrow C Data Interface -----------------------------------------------------------------
     pub fn b2p_plan_range_create(
@@ -464,6 +473,12 @@ extern "C" {
     /// sort_by_label forms only.  Ownership of `child` as for b2p_plan_binary_create.
     pub fn b2p_plan_sort_create(
         ctx: *mut b2p_ctx, function: *const c_char, child: *mut b2p_plan, labels: *const *const c_char, n_labels: i32,
+    ) -> *mut b2p_plan;
+    /// absent(child) over the grid (start, end, interval); `label_names` / `label_values` are the equality matchers of the
+    /// argument's selector in matcher order.  Ownership of `child` as for b2p_plan_binary_create.
+    pub fn b2p_plan_absent_create(
+        ctx: *mut b2p_ctx, start: i64, end: i64, interval: i64, time_index: *const c_char, value_column: *const c_char,
+        label_names: *const *const c_char, label_values: *const *const c_char, n_labels: i32, child: *mut b2p_plan,
     ) -> *mut b2p_plan;
     /// MOVES the batch: on success the release callbacks now belong to the plan.
     pub fn b2p_plan_push_batch(plan: *mut b2p_plan, batch: *mut FFI_ArrowArray, schema: *mut FFI_ArrowSchema) -> c_int;

@@ -98,6 +98,14 @@
 //!     <- GpuPromRangeExec                     => `match_sort`: the b2p_plan_sort_create arguments
 //! ```
 //!
+//! absent over a rewritten node (create_absent_plan, planner.rs:3186-3245):
+//!
+//! ```text
+//!   PromAbsentExec(start, end, step, ts, value, fake labels) <- SortExec(ts)
+//!     <- AggregateExec(group by ts, first_value(field)) [<- RepartitionExec <- AggregateExec(Partial)]
+//!     <- GpuPromRangeExec (on the same grid)   => `match_absent`: the b2p_plan_absent_create arguments
+//! ```
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
@@ -125,7 +133,7 @@ use crate::exec::{GpuPromRangeExec, GpuPromRangeParams, GpuPromStage};
 use crate::ffi::{B2pBinOp, B2pFn, B2pSetOp};
 // In-tree these are `crate::extension_plan::{..}`; named here the way the reference names them.
 use promql::extension_plan::{
-    HistogramFoldExec, RangeManipulateExec, ScalarCalculateExec, SeriesDivideExec, SeriesNormalizeExec,
+    AbsentExec, HistogramFoldExec, RangeManipulateExec, ScalarCalculateExec, SeriesDivideExec, SeriesNormalizeExec,
     UnionDistinctOnExec,
 };
 
@@ -318,6 +326,20 @@ pub struct GpuPromHistogramQuantileSpec {
 pub struct GpuPromSortSpec {
     pub function: String,
     pub labels: Vec<String>,
+    pub child: GpuPromRangeParams,
+}
+
+/// What `b2p_plan_absent_create` takes for a matched absent: the grid, the output's time index and value column names,
+/// the fake labels (the equality matchers of the argument's selector, as `Absent::try_new` kept them: one per name, by
+/// name) and the child node.
+#[derive(Debug, Clone)]
+pub struct GpuPromAbsentSpec {
+    pub start: i64,
+    pub end: i64,
+    pub interval: i64,
+    pub time_index: String,
+    pub value_column: String,
+    pub labels: Vec<(String, String)>,
     pub child: GpuPromRangeParams,
 }
 
@@ -691,6 +713,50 @@ impl GpuPromRewrite {
         }
         let function = if descending { "sort_by_label_desc" } else { "sort_by_label" };
         Some(GpuPromSortSpec { function: function.to_string(), labels, child: params.clone() })
+    }
+
+    /// `PromAbsentExec <- SortExec(ts) <- AggregateExec(ts, first_value(field)) [<- RepartitionExec <-
+    /// AggregateExec(Partial)] <- GpuPromRangeExec` (create_absent_plan, planner.rs:3186-3245) -> the arguments of
+    /// `b2p_plan_absent_create`.  The aggregate must group by the time index alone with one `first_value`, and the child
+    /// must be evaluated on the absent node's grid: the node reads the child's validity per step of that grid, where
+    /// the reference compares the aggregate's timestamps with its cursor.  Anything else stays on the CPU.
+    pub fn match_absent(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromAbsentSpec> {
+        let absent = plan.as_any().downcast_ref::<AbsentExec>()?;
+        let sort = absent.input().as_any().downcast_ref::<SortExec>()?;
+        let agg = sort.input().as_any().downcast_ref::<AggregateExec>()?;
+        let mut input = agg.input().clone();
+        if matches!(agg.mode(), AggregateMode::Final | AggregateMode::FinalPartitioned) {
+            let repart = input.as_any().downcast_ref::<RepartitionExec>()?;
+            let partial = repart.input().as_any().downcast_ref::<AggregateExec>()?;
+            if !matches!(partial.mode(), AggregateMode::Partial) {
+                return None;
+            }
+            input = partial.input().clone();
+        } else if !matches!(agg.mode(), AggregateMode::Single | AggregateMode::SinglePartitioned) {
+            return None;
+        }
+        let [a] = agg.aggr_expr() else { return None };
+        if a.fun().name() != "first_value" {
+            return None;
+        }
+        let child = input.as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let params = child.params();
+        let [(ts, _)] = agg.group_expr().expr() else { return None };
+        if ts.as_any().downcast_ref::<Column>()?.name() != params.time_index_column {
+            return None;
+        }
+        if (params.start, params.end, params.interval) != (absent.start(), absent.end(), absent.step()) {
+            return None;
+        }
+        Some(GpuPromAbsentSpec {
+            start: absent.start(),
+            end: absent.end(),
+            interval: absent.step(),
+            time_index: absent.time_index_column().to_string(),
+            value_column: absent.value_column().to_string(),
+            labels: absent.fake_labels().to_vec(),
+            child: params.clone(),
+        })
     }
 
     /// `ProjectionExec | FilterExec <- HashJoinExec(Inner, tags.. + ts)` over two `GpuPromRangeExec` -> the arguments of
