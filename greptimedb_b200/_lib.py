@@ -36,6 +36,7 @@ EXPORTED_SYMBOLS = [
     "b2p_histogram_fold", "b2p_plan_histogram_quantile_create",
     "b2p_sort_cells_dev", "b2p_sort_cells", "b2p_plan_sort_create",
     "b2p_absent_dev", "b2p_absent", "b2p_plan_absent_create",
+    "b2p_range_eval_fields_dev", "b2p_instant_select_fields_dev", "b2p_range_eval_fields", "b2p_instant_select_fields",
 ]
 
 
@@ -153,6 +154,10 @@ def load() -> C.CDLL:
         "b2p_absent": (C.c_int, [vp, vp, u32, u64, vp, vp]),
         "b2p_plan_absent_create": (vp, [vp, i64, i64, i64, C.c_char_p, C.c_char_p, C.POINTER(C.c_char_p),
                                         C.POINTER(C.c_char_p), i32, vp]),
+        "b2p_range_eval_fields_dev": (C.c_int, [vp, P, vp, vp, vp, i32, vp, u64, u32, vp, vp]),
+        "b2p_instant_select_fields_dev": (C.c_int, [vp, i64, i64, i64, i64, i64, vp, vp, vp, i32, vp, u64, u32, vp, vp]),
+        "b2p_range_eval_fields": (C.c_int, [vp, P, vp, vp, vp, i32, vp, vp, u64, u32, vp, vp]),
+        "b2p_instant_select_fields": (C.c_int, [vp, i64, i64, i64, i64, i64, vp, vp, vp, i32, vp, vp, u64, u32, vp, vp]),
         "b2p_plan_set_function": (C.c_int, [vp, C.c_char_p, C.POINTER(dbl), i32]),
         "b2p_plan_scalar_create": (vp, [vp, vp]),
     }

@@ -17,6 +17,7 @@
 #include "b2p_kernel_t.cuh"
 #include "b2p_kernel_lean.cuh"
 #include "b2p_kernels.cuh"
+#include "b2p_fields.cuh"
 
 using namespace b2p;
 
@@ -601,6 +602,176 @@ int b2p_instant_select_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t inter
   return B2P_OK;
 }
 
+// n_fields and the two pointer arrays of a multi-field call; they must hold before the host form sizes its staging
+static int check_fields(const void* vals, const void* outs, int32_t n_fields) {
+  if (n_fields < 1 || n_fields > B2P_MAX_FIELDS)
+    return fail(B2P_E_INVALID, "n_fields must be in [1, %d] (got %d)", B2P_MAX_FIELDS, (int)n_fields);
+  if (!vals || !outs) return fail(B2P_E_INVALID, "NULL argument");
+  return B2P_OK;
+}
+
+// NULL / alignment checks of the F columns and grids of a call that has rows and a non-empty grid
+static int check_field_columns(const double* const* vals, double* const* outs, int32_t n_fields, uint64_t n_rows) {
+  for (int32_t f = 0; f < n_fields; ++f) {
+    if ((!vals[f] && n_rows) || !outs[f]) return fail(B2P_E_INVALID, "NULL argument (field %d)", (int)f);
+    if (!aligned16(vals[f])) return fail(B2P_E_INVALID, "field %d column must be 16-byte aligned", (int)f);
+  }
+  return B2P_OK;
+}
+
+// Range functions that test is_null or go through arrow's null-skipping aggregates in the reference: sum / avg / min /
+// max_over_time (compute::sum / min / max; avg divides by the window's length, NULL slots included), stdvar /
+// stddev_over_time (`value.unwrap()` on each slot: a NULL panics), deriv and predict_linear (linear_regression_slices
+// skips is_null slots, functions.rs:126-144).  Every other function reads the value buffer as it is (`values()`: rate /
+// increase / delta, irate / idelta, resets, changes, last_over_time, quantile_over_time, holt_winters) or only the
+// window's length (count / present / absent_over_time), as SeriesNormalize's NaN filter reads `value(i)`
+// (normalize.rs:415-428): over NULL slots a multi-field call reproduces those from the buffer values alone.
+static bool reads_nulls(int fn) {
+  switch (fn) {
+    case B2P_FN_SUM_OVER_TIME: case B2P_FN_AVG_OVER_TIME: case B2P_FN_MIN_OVER_TIME: case B2P_FN_MAX_OVER_TIME:
+    case B2P_FN_STDVAR_OVER_TIME: case B2P_FN_STDDEV_OVER_TIME: case B2P_FN_DERIV: case B2P_FN_PREDICT_LINEAR:
+      return true;
+    default:
+      return false;
+  }
+}
+
+// The first field whose validity bitmap has a NULL slot in rows [0, n_rows), or -1 (field_valid or an entry NULL: none).
+// Synchronises once when a bitmap is given.
+static int first_null_field(b2p_ctx* c, const uint8_t* const* field_valid, int32_t n_fields, uint64_t n_rows, int* out) {
+  *out = -1;
+  if (!field_valid || n_rows == 0) return B2P_OK;
+  bool any = false;
+  for (int32_t f = 0; f < n_fields; ++f) any |= field_valid[f] != nullptr;
+  if (!any) return B2P_OK;
+  if (int rc = c->fd_null.ensure((size_t)kMaxFields * 4)) return rc;
+  uint32_t* flags = c->fd_null.as<uint32_t>();
+  CU(cudaMemsetAsync(flags, 0, (size_t)n_fields * 4, c->stream));
+  for (int32_t f = 0; f < n_fields; ++f) {
+    if (!field_valid[f]) continue;
+    null_slots_kernel<<<capped_grid(c, (n_rows + 7) / 8, 256, 8), 256, 0, c->stream>>>(field_valid[f], n_rows, flags + f);
+    c->launches++;
+    CU(cudaGetLastError());
+  }
+  uint32_t h[kMaxFields];
+  CU(cudaMemcpyAsync(h, flags, (size_t)n_fields * 4, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  for (int32_t f = 0; f < n_fields; ++f)
+    if (h[f]) { *out = f; break; }
+  return B2P_OK;
+}
+
+// An outstanding range call reads or writes the multi-field scratch, and b2p_sync may run it again there.
+static bool fields_scratch_pending(const b2p_ctx* c) {
+  auto in = [](const DevBuf& b, const void* p) {
+    const char* lo = b.as<char>();
+    return lo && static_cast<const char*>(p) >= lo && static_cast<const char*>(p) < lo + b.cap;
+  };
+  for (const b2p_ctx::Pending& pc : c->pending)
+    if (in(c->fd_val, pc.args.val) || in(c->fd_valid, pc.args.valid)) return true;
+  return false;
+}
+
+int b2p_range_eval_fields_dev(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* const* vals,
+                              const uint8_t* const* field_valid, int32_t n_fields, const uint64_t* offsets,
+                              uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int rc = check_fields(vals, outs, n_fields);
+  if (rc) return rc;
+  if (p && p->fn_id >= 0 && p->fn_id < B2P_FN__COUNT && reads_nulls(p->fn_id)) {
+    DeviceGuard g(c->device);
+    int f = -1;
+    if ((rc = first_null_field(c, field_valid, n_fields, n_rows, &f))) return rc;
+    if (f >= 0)
+      return fail(B2P_E_INVALID, "field %d has NULL slots: range function %d skips NULL slots in the reference, which a "
+                  "multi-field call does not reproduce", f, (int)p->fn_id);
+  }
+  if (n_fields == 1) return b2p_range_eval_dev(c, p, ts, vals[0], offsets, n_rows, n_series, outs[0], valid_words);
+  int64_t T = 0;
+  if ((rc = check_grid(p, n_series, &T))) return rc;
+  if (n_series == 0 || T == 0) return B2P_OK;
+  if (!offsets || !valid_words || (!ts && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
+  if ((rc = check_field_columns(vals, outs, n_fields, n_rows))) return rc;
+  DeviceGuard g(c->device);
+  const int F = n_fields;
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  const uint64_t words = (uint64_t)n_series * Tw;
+  const double* fv[kMaxFields];
+  for (int f = 0; f < F; ++f) fv[f] = vals[f];
+  if (fields_scratch_pending(c) && (rc = b2p_sync(c))) return rc;
+  if (p->filter_nan && n_rows) {
+    const uint64_t stride = (n_rows + 1) & ~1ull;  // 16-byte aligned columns
+    if ((rc = c->fd_val.ensure((size_t)F * stride * 8))) return rc;
+    double* base = c->fd_val.as<double>();
+    for (int f = 0; f < F; ++f) {
+      CU(cudaMemcpyAsync(base + f * stride, vals[f], n_rows * 8, cudaMemcpyDeviceToDevice, c->stream));
+      fv[f] = base + f * stride;
+    }
+    stage_begin(c, 0);
+    nan_union_kernel<<<capped_grid(c, n_rows, 256, 8), 256, 0, c->stream>>>(base, stride, F, n_rows);
+    c->launches++;
+    stage_end(c, 0);
+    CU(cudaGetLastError());
+  }
+  if ((rc = c->fd_valid.ensure((size_t)(F - 1) * words * 4))) return rc;
+  ValidAndArgs va{};
+  va.F = F; va.out = valid_words; va.n_words = words; va.Tw = Tw; va.T = (uint64_t)T;
+  va.in[0] = valid_words;
+  for (int f = 1; f < F; ++f) va.in[f] = c->fd_valid.as<uint32_t>() + (uint64_t)(f - 1) * words;
+  for (int f = 0; f < F; ++f)
+    if ((rc = range_call(c, p, ts, fv[f], offsets, n_rows, n_series, outs[f], const_cast<uint32_t*>(va.in[f]), nullptr)))
+      return rc;
+  if ((rc = b2p_sync(c))) return rc;  // slow-path fix-ups (and repeated calls) land before the conjunction reads
+  stage_begin(c, 3);
+  valid_and_kernel<<<capped_grid(c, words, 256, 16), 256, 0, c->stream>>>(va);
+  c->launches++;
+  stage_end(c, 3);
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+int b2p_instant_select_fields_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                                  int64_t offset, const int64_t* ts, const double* const* vals,
+                                  const uint8_t* const* field_valid, int32_t n_fields, const uint64_t* offsets,
+                                  uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int rc = check_fields(vals, outs, n_fields);
+  if (rc) return rc;
+  {  // the reference exports a NULL slot of the chosen row as a NULL in that field of an emitted row: one validity
+     // bitmap for all fields cannot carry it
+    DeviceGuard g(c->device);
+    int f = -1;
+    if ((rc = first_null_field(c, field_valid, n_fields, n_rows, &f))) return rc;
+    if (f >= 0)
+      return fail(B2P_E_INVALID, "field %d has NULL slots: the instant selector exports them as NULL in that field "
+                  "only, which a multi-field call does not reproduce", f);
+  }
+  if (n_fields == 1)
+    return b2p_instant_select_dev(c, start, end, interval, lookback, offset, ts, vals[0], offsets, n_rows, n_series,
+                                  outs[0], valid_words);
+  b2p_range_params p{};
+  p.start = start; p.end = end; p.interval = interval; p.range = lookback;
+  int64_t T = 0;
+  if ((rc = check_grid(&p, n_series, &T))) return rc;
+  if (n_series == 0 || T == 0) return B2P_OK;
+  if (!offsets || !valid_words || (!ts && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
+  if ((rc = check_field_columns(vals, outs, n_fields, n_rows))) return rc;
+  DeviceGuard g(c->device);
+  FieldsInstantArgs fa{};
+  InstantArgs& a = fa.g;
+  a.start = start; a.end = end; a.interval = interval; a.lookback = lookback; a.offset = offset;
+  a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
+  a.ts = ts; a.val = vals[0]; a.offsets = offsets; a.n_series = n_series; a.out = outs[0]; a.valid = valid_words;
+  fa.F = n_fields;
+  for (int f = 0; f < n_fields; ++f) { fa.vals[f] = vals[f]; fa.outs[f] = outs[f]; }
+  stage_begin(c, 1);
+  instant_fields_kernel<<<capped_grid(c, n_series, kWarpsPerCta, 8), kWarpsPerCta * 32, 0, c->stream>>>(fa);
+  c->launches++;
+  stage_end(c, 1);
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
 // sum by (..)(fn(..)) partials of groups [g_lo, g_hi) added into out_sum / out_cnt [n_groups x T].
 // Fused (no [n_series x T] intermediate) for rate / increase / delta whenever the first tier applies; otherwise the
 // range function is evaluated into context scratch and folded by the by-label kernel (two passes, synchronous).
@@ -1158,6 +1329,62 @@ int b2p_instant_select(b2p_ctx* c, int64_t start, int64_t end, int64_t interval,
   return s.end([&] {
     const int rc = b2p_instant_select_dev(c, start, end, interval, lookback, offset, in.ts, in.val, in.offsets, n_rows,
                                           n_series, d_out, d_valid);
+    return rc ? rc : b2p_sync(c);
+  });
+}
+
+int b2p_range_eval_fields(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* const* vals,
+                          const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid,
+                          const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int64_t T = 0;
+  if (int rc = check_grid(p, n_series, &T)) return rc;
+  if (int rc = check_fields(vals, outs, n_fields)) return rc;
+  if (n_series == 0 || T == 0) return B2P_OK;  // (no sample copies, no series offsets)
+  DeviceGuard g(c->device);
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  Staging s{c};
+  const SeriesIn in = stage_series(s, ts, nullptr, sid, 0u, offsets_host, n_rows, n_series);
+  const double* d_vals[kMaxFields];
+  double* d_outs[kMaxFields];
+  s.in_cols(vals, n_fields, n_rows * 8, d_vals);
+  const uint8_t* d_nulls[kMaxFields] = {};
+  if (field_valid) s.in_cols(field_valid, n_fields, (n_rows + 7) / 8, d_nulls);
+  s.out_cols(outs, n_fields, (size_t)n_series * (size_t)T * 8, d_outs);
+  uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
+  return s.end([&] {
+    const int rc = b2p_range_eval_fields_dev(c, p, in.ts, d_vals, field_valid ? d_nulls : nullptr, n_fields, in.offsets,
+                                             n_rows, n_series, d_outs, d_valid);
+    return rc ? rc : b2p_sync(c);
+  });
+}
+
+int b2p_instant_select_fields(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                              int64_t offset, const int64_t* ts, const double* const* vals,
+                              const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid,
+                              const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  b2p_range_params p{};
+  p.start = start; p.end = end; p.interval = interval; p.range = lookback;
+  int64_t T = 0;
+  if (int rc = check_grid(&p, n_series, &T)) return rc;
+  if (int rc = check_fields(vals, outs, n_fields)) return rc;
+  if (n_series == 0 || T == 0) return B2P_OK;  // (no sample copies, no series offsets)
+  DeviceGuard g(c->device);
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  Staging s{c};
+  const SeriesIn in = stage_series(s, ts, nullptr, sid, 0u, offsets_host, n_rows, n_series);
+  const double* d_vals[kMaxFields];
+  double* d_outs[kMaxFields];
+  s.in_cols(vals, n_fields, n_rows * 8, d_vals);
+  const uint8_t* d_nulls[kMaxFields] = {};
+  if (field_valid) s.in_cols(field_valid, n_fields, (n_rows + 7) / 8, d_nulls);
+  s.out_cols(outs, n_fields, (size_t)n_series * (size_t)T * 8, d_outs);
+  uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
+  return s.end([&] {
+    const int rc = b2p_instant_select_fields_dev(c, start, end, interval, lookback, offset, in.ts, d_vals,
+                                                 field_valid ? d_nulls : nullptr, n_fields,
+                                                 in.offsets, n_rows, n_series, d_outs, d_valid);
     return rc ? rc : b2p_sync(c);
   });
 }

@@ -222,6 +222,10 @@ struct b2p_ctx {
   DevBuf v_keys, v_alt, v_rank, v_seg, v_group, v_tmp;
   // subquery: the sample rows of one batch of child rows (ts, val, offsets) and CUB's temp (bound in subquery_run)
   DevBuf sq_ts, sq_val, sq_off, sq_tmp;
+  // multi-field range call: the value columns with K16's NaN union applied, and the validity bitmaps of fields 1.. before
+  // K18's conjunction (bound in b2p_range_eval_fields_dev)
+  DevBuf fd_val, fd_valid;
+  DevBuf fd_null;  // one NULL-slot flag per field (null_slots_kernel)
   // sort / sort_desc: row offsets, keys (double-buffered), the alternate cell buffer and CUB's temp (bound in sort_run)
   DevBuf so_off, so_keys, so_cells, so_tmp;
   // resident CTAs per SM of each persistent kernel instantiation and dynamic shared-memory size (persistent_grid)
@@ -301,12 +305,10 @@ int check_grid(const b2p_range_params* p, uint32_t n_series, int64_t* T_out);
 // An absent (NULL) host column is handed out as NULL and queues nothing, so the device form's argument check rejects
 // it.  A host call reads: stage the inputs, stage the outputs, end() with the device form.
 struct Staging {
-  static constexpr int kOutputs = 2;  // a host call returns two columns
   b2p_ctx* c;
   int next = 0, rc = B2P_OK;
   struct Back { void* host; const void* dev; size_t bytes; };
-  Back back[kOutputs];
-  int n_back = 0;
+  std::vector<Back> back;
 
   void cuda(cudaError_t e, const char* what) {  // a failed CUDA call becomes the sticky error
     if (e != cudaSuccess && !rc) rc = fail(B2P_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
@@ -328,8 +330,7 @@ struct Staging {
   template <class T>
   T* copy_back(T* host, T* dev, size_t bytes) {
     if (!host) return nullptr;
-    if (!rc && n_back == kOutputs) rc = fail(B2P_E_INVALID, "host call returns more than %d columns", kOutputs);
-    if (!rc) back[n_back++] = Back{host, dev, bytes};
+    if (!rc) back.push_back(Back{host, dev, bytes});
     return dev;
   }
   // a result buffer, copied to `host` by download(); NULL for an absent one
@@ -337,12 +338,31 @@ struct Staging {
   T* out(T* host, size_t bytes) {
     return host ? copy_back(host, static_cast<T*>(buf(bytes)), bytes) : nullptr;
   }
+  // n columns of `bytes` each in one buffer (each at a 16-byte aligned offset): device copies of the host columns, or
+  // result columns copied back to them; dev[i] is NULL for an absent host column
+  template <class T>
+  void in_cols(const T* const* hosts, int n, size_t bytes, const T** dev) {
+    const size_t stride = (bytes + 15) & ~(size_t)15;
+    char* d = static_cast<char*>(buf(stride * (size_t)n));
+    for (int i = 0; i < n; ++i) {
+      dev[i] = d && hosts[i] ? reinterpret_cast<const T*>(d + stride * (size_t)i) : nullptr;
+      if (dev[i] && bytes)
+        cuda(cudaMemcpyAsync(const_cast<T*>(dev[i]), hosts[i], bytes, cudaMemcpyHostToDevice, c->stream), "host-to-device copy");
+    }
+  }
+  template <class T>
+  void out_cols(T* const* hosts, int n, size_t bytes, T** dev) {
+    const size_t stride = (bytes + 15) & ~(size_t)15;
+    char* d = static_cast<char*>(buf(stride * (size_t)n));
+    for (int i = 0; i < n; ++i)
+      dev[i] = d && hosts[i] ? copy_back(hosts[i], reinterpret_cast<T*>(d + stride * (size_t)i), bytes) : nullptr;
+  }
   int download() {  // the results noted since the last download()
-    for (int i = 0; !rc && i < n_back; ++i)
+    for (size_t i = 0; !rc && i < back.size(); ++i)
       if (back[i].bytes)
         cuda(cudaMemcpyAsync(back[i].host, back[i].dev, back[i].bytes, cudaMemcpyDeviceToHost, c->stream),
              "device-to-host copy");
-    n_back = 0;
+    back.clear();
     return rc;
   }
   int finish() {  // download() and wait for it

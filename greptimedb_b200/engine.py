@@ -213,6 +213,63 @@ class Context:
                                                _ptr(sid), _ptr(offsets), ts.size, S, _ptr(out), _ptr(valid)))
         return out, valid
 
+    @staticmethod
+    def _ptr_array(cols):
+        """a host array of the columns' pointers (const double* const* / double* const*)"""
+        arr = (C.c_void_p * max(1, len(cols)))(*[_ptr(x) for x in cols])
+        return C.cast(arr, C.c_void_p), arr
+
+    def _series_count(self, sid, offsets):
+        if offsets is not None:
+            offsets = np.ascontiguousarray(offsets, np.uint64)
+            return None, offsets, offsets.size - 1
+        sid = np.ascontiguousarray(sid, np.uint32)
+        return sid, None, (int(sid.max()) + 1 if sid.size else 0)
+
+    @classmethod
+    def _field_bitmaps(cls, present):
+        """per-field bool masks (True = a value; None: no NULL slot) -> (void* to the Arrow validity bitmaps, keep-alive)"""
+        if present is None:
+            return None, None
+        bms = [None if m is None else np.packbits(np.asarray(m, bool), bitorder="little") for m in present]
+        ptr, arr = cls._ptr_array(bms)
+        return ptr, (bms, arr)
+
+    def range_eval_fields(self, p: RangeParams, ts, vals, sid=None, offsets=None, present=None):
+        """A range selector over F field columns of the same rows (vals: F value columns, their buffers as they are;
+        present: per-field bool masks of the non-NULL slots, or None) -> (outs [F,S,T] f64, valid_words [S,Tw] u32):
+        one validity bitmap, a cell valid only where every field's result is."""
+        ts = np.ascontiguousarray(ts, np.int64)
+        vals = [np.ascontiguousarray(v, np.float64) for v in vals]
+        nb, _keep3 = self._field_bitmaps(present)
+        sid, offsets, S = self._series_count(sid, offsets)
+        T = num_steps(p.start, p.end, p.interval)
+        outs = np.zeros((len(vals), S, T), np.float64)
+        valid = np.zeros((S, (T + 31) // 32), np.uint32)
+        vp, _keep = self._ptr_array(vals)
+        op, _keep2 = self._ptr_array(list(outs))
+        self._check(self._L.b2p_range_eval_fields(self._h, C.byref(p), _ptr(ts), vp, nb, len(vals), _ptr(sid),
+                                                  _ptr(offsets), ts.size, S, op, _ptr(valid)))
+        return outs, valid
+
+    def instant_select_fields(self, ts, vals, start, end, interval, lookback, offset=0, sid=None, offsets=None,
+                              present=None):
+        """The instant selector over F field columns -> (outs [F,S,T] f64, valid_words [S,Tw] u32): the row of each
+        step is chosen by field 0 (its stale-NaN test included) and every field is read from it."""
+        ts = np.ascontiguousarray(ts, np.int64)
+        vals = [np.ascontiguousarray(v, np.float64) for v in vals]
+        nb, _keep3 = self._field_bitmaps(present)
+        sid, offsets, S = self._series_count(sid, offsets)
+        T = num_steps(start, end, interval)
+        outs = np.zeros((len(vals), S, T), np.float64)
+        valid = np.zeros((S, (T + 31) // 32), np.uint32)
+        vp, _keep = self._ptr_array(vals)
+        op, _keep2 = self._ptr_array(list(outs))
+        self._check(self._L.b2p_instant_select_fields(self._h, start, end, interval, lookback, offset, _ptr(ts), vp, nb,
+                                                      len(vals), _ptr(sid), _ptr(offsets), ts.size, S, op,
+                                                      _ptr(valid)))
+        return outs, valid
+
     def group_aggregate(self, agg, vals, valid, gid, n_groups):
         vals = np.ascontiguousarray(vals, np.float64)
         valid = np.ascontiguousarray(valid, np.uint32)
@@ -424,6 +481,23 @@ class Context:
     def instant_select_dev(self, start, end, interval, lookback, offset, ts, val, offsets, n_rows, n_series, out, valid):
         self._check(self._L.b2p_instant_select_dev(self._h, start, end, interval, lookback, offset, _ptr(ts), _ptr(val),
                                                    _ptr(offsets), n_rows, n_series, _ptr(out), _ptr(valid)))
+
+    def range_eval_fields_dev(self, p, ts, vals, offsets, n_rows, n_series, outs, valid, field_valid=None):
+        """vals / outs: sequences of F device columns / grids (tensors or pointers); field_valid: None, or F device
+        Arrow validity bitmaps (None entries: no NULL slot)"""
+        vp, _keep = self._ptr_array(vals)
+        op, _keep2 = self._ptr_array(outs)
+        nb, _keep3 = self._ptr_array(field_valid) if field_valid is not None else (None, None)
+        self._check(self._L.b2p_range_eval_fields_dev(self._h, C.byref(p), _ptr(ts), vp, nb, len(vals), _ptr(offsets),
+                                                      n_rows, n_series, op, _ptr(valid)))
+
+    def instant_select_fields_dev(self, start, end, interval, lookback, offset, ts, vals, offsets, n_rows, n_series,
+                                  outs, valid, field_valid=None):
+        vp, _keep = self._ptr_array(vals)
+        op, _keep2 = self._ptr_array(outs)
+        nb, _keep3 = self._ptr_array(field_valid) if field_valid is not None else (None, None)
+        self._check(self._L.b2p_instant_select_fields_dev(self._h, start, end, interval, lookback, offset, _ptr(ts), vp,
+                                                          nb, len(vals), _ptr(offsets), n_rows, n_series, op, _ptr(valid)))
 
     def group_aggregate_dev(self, agg, vals, valid, gid, n_series, n_groups, T, out_val, out_cnt):
         aid = AGG_IDS[agg] if isinstance(agg, str) else int(agg)

@@ -22,6 +22,10 @@
  *                              offset | len<<32, src/promql/src/range_array.rs:247-254) — the narrow
  *                              boundary: Fn(&[ColumnarValue]) -> ColumnarValue, extrapolate_rate.rs:90-96
  *   b2p_instant_select[_dev]   InstantManipulateStream::manipulate         instant_manipulate.rs:473-585
+ *   b2p_range_eval_fields[_dev], b2p_instant_select_fields[_dev]
+ *                              the same two over a table with several field columns: RangeManipulate field_columns
+ *                              range_manipulate.rs:70-153, the UDF per field planner.rs:2180, the all-fields
+ *                              IS NOT NULL filter planner.rs:2774-2791
  *   b2p_group_aggregate[_dev]  DataFusion AggregateExec(Partial+Final) planned by
  *                              prom_aggr_expr_to_plan src/query/src/promql/planner.rs:334-452
  *                              (sum/avg/count/min/max/stddev/stdvar by labels + eval ts)
@@ -203,6 +207,48 @@ B2P_API int b2p_range_udf_dev(b2p_ctx* ctx, int32_t fn_id, const int64_t* ts, co
 B2P_API int b2p_instant_select_dev(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval, int64_t lookback,
                            int64_t offset, const int64_t* ts, const double* val, const uint64_t* offsets,
                            uint64_t n_rows, uint32_t n_series, double* out, uint32_t* valid_words);
+/* Multi-field tables (Influx line protocol / OTLP ingest: cpu(usage_user, usage_system, ..)): one timestamp column and
+ * n_fields Float64 value columns over the same rows, 1 <= n_fields <= B2P_MAX_FIELDS.  `vals` and `outs` are HOST
+ * arrays of n_fields DEVICE pointers: vals[f] is field f's column [n_rows], outs[f] its grid [n_series*T].  There is
+ * one validity bitmap for all fields.
+ *
+ * b2p_range_eval_fields_dev: the reference's RangeManipulate with field_columns (range_manipulate.rs:70-153), the prom_*
+ * UDF projected once per field (planner.rs:2180) and Filter(every field IS NOT NULL) (planner.rs:2774-2791).
+ *   - With p->filter_nan, a row in which ANY field is NaN is dropped for every field, as SeriesNormalize's filter over
+ *     all Float64 columns does (normalize.rs:415-428).  The union is taken on context copies of the value columns
+ *     (8 B per field and row of scratch); the caller's columns are never written.
+ *   - The windows come from the timestamps alone; each field runs the range tiers of b2p_range_eval_dev over the same
+ *     offsets, and a (series, step) cell is valid only where every field's result is.  A cell whose bit is 0 holds
+ *     0.0 or the value its own field computed there.
+ *   - The call synchronises once (the slow path's fix-ups must land before the conjunction), then enqueues the
+ *     conjunction; call b2p_sync() before reading the results, as for every *_dev call.
+ *   - n_fields == 1 is exactly b2p_range_eval_dev.
+ * b2p_instant_select_fields_dev: InstantManipulate over every field (instant_manipulate.rs:473-585).  The step's row is
+ * chosen once: the lookback search and the stale-NaN test read field 0 only (planner.rs:922), and every field is
+ * taken from that row, NaN or not.  n_fields == 1 is exactly b2p_instant_select_dev.
+ *
+ * NULL slots.  `field_valid` (may be NULL, as may any entry: no NULL slot) is a host array of n_fields DEVICE pointers
+ * to each field's Arrow validity bitmap (bit r of byte r/8, 1 = a value), (n_rows + 7) / 8 bytes.  vals[f] holds the
+ * field's value buffer as it is, NULL slots included.  The reference reads NULL slots in two ways:
+ *   - rate, increase, delta, irate, idelta, resets, changes, last_over_time, quantile_over_time and holt_winters read
+ *     the value buffer (`values()`), count / present / absent_over_time only the window's length, and the NaN filter
+ *     the buffer value (`value(i)`): the range call reproduces them from vals alone and ignores the bitmaps;
+ *   - sum / avg / min / max_over_time (arrow's null-skipping aggregates), stdvar / stddev_over_time (a NULL slot
+ *     panics) and deriv / predict_linear (`is_null` skipped, functions.rs:126-144): a range call of these functions
+ *     whose bitmaps hold a NULL slot in rows [0, n_rows) is refused with B2P_E_INVALID naming the field.
+ * The instant selector exports a NULL slot of the chosen row as a NULL in that field of an emitted row, which one
+ * validity bitmap cannot carry: an instant call whose bitmaps hold a NULL slot is refused the same way.  Checking the
+ * bitmaps synchronises once; with field_valid NULL nothing is read. */
+#define B2P_MAX_FIELDS 64
+B2P_API int b2p_range_eval_fields_dev(b2p_ctx* ctx, const b2p_range_params* p, const int64_t* ts,
+                                      const double* const* vals, const uint8_t* const* field_valid,
+                                      int32_t n_fields, const uint64_t* offsets,
+                                      uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words);
+B2P_API int b2p_instant_select_fields_dev(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                                          int64_t offset, const int64_t* ts, const double* const* vals,
+                                          const uint8_t* const* field_valid, int32_t n_fields,
+                                          const uint64_t* offsets, uint64_t n_rows,
+                                          uint32_t n_series, double* const* outs, uint32_t* valid_words);
 /* gid[s] in [0,n_groups) (or >= n_groups to drop the series).  members_* is scratch-free: the
  * library builds the group->series CSR itself.  out_val/out_cnt are [n_groups*T]; cnt==0 <=> the
  * group has no row at that step.  Partial results of several shards/GPUs combine by adding
@@ -434,6 +480,16 @@ B2P_API int b2p_instant_select(b2p_ctx* ctx, int64_t start, int64_t end, int64_t
                        int64_t offset, const int64_t* ts, const double* val, const uint32_t* sid,
                        const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* out,
                        uint32_t* valid_words);
+/* Host-pointer forms of b2p_range_eval_fields_dev / b2p_instant_select_fields_dev (synchronous): vals[f], field_valid[f]
+ * and outs[f] are host columns; sid may be NULL when offsets_host (n_series+1) is given instead.  One staged copy per call (no chunked
+ * pipeline): every column must fit on the device at once. */
+B2P_API int b2p_range_eval_fields(b2p_ctx* ctx, const b2p_range_params* p, const int64_t* ts, const double* const* vals,
+                                  const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid, const uint64_t* offsets_host, uint64_t n_rows,
+                                  uint32_t n_series, double* const* outs, uint32_t* valid_words);
+B2P_API int b2p_instant_select_fields(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                                      int64_t offset, const int64_t* ts, const double* const* vals,
+                                      const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid, const uint64_t* offsets_host, uint64_t n_rows,
+                                      uint32_t n_series, double* const* outs, uint32_t* valid_words);
 B2P_API int b2p_group_aggregate(b2p_ctx* ctx, int32_t agg, const double* vals, const uint32_t* valid_words,
                         const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val,
                         uint32_t* out_cnt);

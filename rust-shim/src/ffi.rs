@@ -222,6 +222,22 @@ extern "C" {
         ctx: *mut b2p_ctx, start: i64, end: i64, interval: i64, lookback: i64, offset: i64, ts: *const i64,
         val: *const f64, offsets: *const u64, n_rows: u64, n_series: u32, out: *mut f64, valid_words: *mut u32,
     ) -> c_int;
+    /// Selectors over a table with several Float64 field columns (1 ..= 64): `vals` / `outs` are host arrays of
+    /// n_fields device pointers, one validity bitmap for all fields.  The range form drops a row from every field when
+    /// any field is NaN (filter_nan) and keeps a cell only where every field's result is valid; the instant form picks
+    /// the row once, with the stale-NaN test on field 0.  `field_valid` (nullable) holds each field's Arrow validity
+    /// bitmap: calls the device cannot reproduce over NULL slots are refused (see the header).
+    pub fn b2p_range_eval_fields_dev(
+        ctx: *mut b2p_ctx, p: *const B2pRangeParams, ts: *const i64, vals: *const *const f64,
+        field_valid: *const *const u8, n_fields: i32,
+        offsets: *const u64, n_rows: u64, n_series: u32, outs: *const *mut f64, valid_words: *mut u32,
+    ) -> c_int;
+    pub fn b2p_instant_select_fields_dev(
+        ctx: *mut b2p_ctx, start: i64, end: i64, interval: i64, lookback: i64, offset: i64, ts: *const i64,
+        vals: *const *const f64, field_valid: *const *const u8, n_fields: i32, offsets: *const u64, n_rows: u64,
+        n_series: u32,
+        outs: *const *mut f64, valid_words: *mut u32,
+    ) -> c_int;
     pub fn b2p_group_aggregate_dev(
         ctx: *mut b2p_ctx, agg: i32, vals: *const f64, valid_words: *const u32, gid: *const u32, n_series: u32,
         n_groups: u32, t: u64, out_val: *mut f64, out_cnt: *mut u32,
@@ -351,6 +367,19 @@ extern "C" {
         ctx: *mut b2p_ctx, start: i64, end: i64, interval: i64, lookback: i64, offset: i64, ts: *const i64,
         val: *const f64, sid: *const u32, offsets_host: *const u64, n_rows: u64, n_series: u32, out: *mut f64,
         valid_words: *mut u32,
+    ) -> c_int;
+    /// Host-pointer forms of the two multi-field selectors (synchronous, one staged copy).
+    pub fn b2p_range_eval_fields(
+        ctx: *mut b2p_ctx, p: *const B2pRangeParams, ts: *const i64, vals: *const *const f64,
+        field_valid: *const *const u8, n_fields: i32,
+        sid: *const u32, offsets_host: *const u64, n_rows: u64, n_series: u32, outs: *const *mut f64,
+        valid_words: *mut u32,
+    ) -> c_int;
+    pub fn b2p_instant_select_fields(
+        ctx: *mut b2p_ctx, start: i64, end: i64, interval: i64, lookback: i64, offset: i64, ts: *const i64,
+        vals: *const *const f64, field_valid: *const *const u8, n_fields: i32, sid: *const u32,
+        offsets_host: *const u64, n_rows: u64,
+        n_series: u32, outs: *const *mut f64, valid_words: *mut u32,
     ) -> c_int;
     pub fn b2p_group_aggregate(
         ctx: *mut b2p_ctx, agg: i32, vals: *const f64, valid_words: *const u32, gid: *const u32, n_series: u32,
