@@ -29,42 +29,8 @@ constexpr int kSlowCtas = 132;        // slow-path grid (4 warps per CTA): one C
 constexpr int kSlowWarps = kSlowCtas * 4;
 constexpr size_t kArenaDefaultRows = 1u << 21;  // 32 MB: regions of 3 971 rows for the 528 slow-path warps
 
-void stage_begin_on(b2p_ctx* c, int stage, cudaStream_t s) { cudaEventRecord(c->ev[stage][0], s); }
-void stage_end_on(b2p_ctx* c, int stage, cudaStream_t s) {
-  cudaEventRecord(c->ev[stage][1], s);
-  c->ev_used[stage] = true;
-}
-
 // rate / increase / delta: the functions of the thread tier and of the fused by-label first tier
 constexpr bool rate_like(int fn) { return fn == B2P_FN_RATE || fn == B2P_FN_INCREASE || fn == B2P_FN_DELTA; }
-
-template <int FN, bool TS32>
-int launch_fast_t(b2p_ctx* c, const RangeArgs& a) {
-  constexpr size_t smem = (size_t)kWarpsPerCta * (2 * kRing * (8 + (TS32 ? 4 : 8)) + kRing / 8) + kRcpTable * 8;
-  auto kern = range_fast_kernel<FN, kRing, TS32>;
-  unsigned grid = 0;
-  if (int rc = persistent_grid(c, kern, smem, kWarpsPerCta, a.n_series, &grid)) return rc;
-  if (grid == 0) return B2P_OK;
-  kern<<<grid, kWarpsPerCta * 32, smem, c->stream>>>(a);
-  c->launches++;
-  CU(cudaGetLastError());
-  return B2P_OK;
-}
-
-// Long-window instantiation (32-bit time domain only): RING = kBigRing, one CTA per SM, over RangeArgs::b_list.
-template <int FN>
-int launch_big(b2p_ctx* c, const RangeArgs& a0) {
-  RangeArgs a = a0;
-  a.use_w_list = 2;
-  constexpr size_t smem = (size_t)kWarpsPerCta * (2 * kBigRing * (8 + 4) + kBigRing / 8) + kRcpTable * 8;
-  auto kern = range_fast_kernel<FN, kBigRing, true>;
-  unsigned grid = 0;  // the length of b_list is known on the device only
-  if (int rc = persistent_grid(c, kern, smem, kWarpsPerCta, kAllResident, &grid)) return rc;
-  kern<<<grid, kWarpsPerCta * 32, smem, c->stream>>>(a);
-  c->launches++;
-  CU(cudaGetLastError());
-  return B2P_OK;
-}
 
 // 32-bit relative timestamps when the whole query span (plus one lookback) fits 31 bits of ms.
 bool fits_ts32(const RangeArgs& a) {
@@ -72,12 +38,12 @@ bool fits_ts32(const RangeArgs& a) {
   return span >= 0 && span < 2147483000.0 && a.interval < 2147483000ll && a.range < 2147483000ll;
 }
 
-// Adaptive tiering verdict of a finished range call that started with K2L: more than half of the series handed on ->
-// the next 32 calls of this function use the next mode (plain -> bit words for rate / increase -> skip).
-void lean_verdict(b2p_ctx* c, int fn, uint64_t handed, uint64_t n_series) {
+// Adaptive tiering verdict of a finished range call that started with K2L in `mode`: more than half of the series
+// handed on -> the next 32 calls of this function use the next mode (plain -> bit words for rate / increase -> skip).
+void lean_verdict(b2p_ctx* c, int fn, int mode, uint64_t handed, uint64_t n_series) {
   if (!c->lean_adaptive || handed * 2 <= n_series) return;
   const bool counter = (fn == B2P_FN_RATE || fn == B2P_FN_INCREASE);
-  c->lean_mode[fn] = (c->last_lean_mode == 0 && counter) ? 1 : 2;
+  c->lean_mode[fn] = (mode == 0 && counter) ? 1 : 2;
   c->lean_backoff[fn] = 32;
 }
 
@@ -99,103 +65,99 @@ bool lean_ok(const b2p_ctx* c, int fn, const RangeArgs& a) {
   return (double)a.rel_max + 64.0 * (double)a.interval < 4294967295.0;
 }
 
-template <int FN>
-int launch_fast(b2p_ctx* c, const RangeArgs& a) {
-  return fits_ts32(a) ? launch_fast_t<FN, true>(c, a) : launch_fast_t<FN, false>(c, a);
+// The tiers a range call of `fn` over the geometry `a` starts with (changes no state).  Tier 1 (rate / increase /
+// delta, 32-bit time domain) is the thread tier (opt-in) or the lean warp-per-series kernel; what it declines goes to
+// tier 2 (warp per series) through w_list, long windows from there to the 1024-sample instantiation through b_list,
+// and what that declines to the exact slow kernel.  While a back-off lasts the first tier runs in the mode the last
+// verdict chose (mode 2: not at all).
+b2p_ctx::Tiers choose_tiers(const b2p_ctx* c, int fn, const RangeArgs& a) {
+  b2p_ctx::Tiers t;
+  t.thread_tier = c->thread_tier && fits_ts32(a) && rate_like(fn);
+  if (t.thread_tier || !lean_ok(c, fn, a)) return t;
+  if (c->lean_backoff[fn] > 0) t.lean_mode = c->lean_mode[fn];
+  t.first_tier = t.lean_mode != 2;
+  if (t.lean_mode == 0 && c->lean_force_flags) t.lean_mode = 1;
+  return t;
+}
+
+// One launch of a range kernel on the context's stream; a zero grid launches nothing.
+template <class Kern>
+int launch_kernel(b2p_ctx* c, Kern* kern, unsigned grid, unsigned threads, size_t smem, const RangeArgs& a) {
+  if (grid == 0) return B2P_OK;
+  kern<<<grid, threads, smem, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// The warp-per-series tier (K2): RING = kRing over the series (w_list after a first tier), or its long-window
+// instantiation RING = kBigRing (32-bit time domain only), one CTA per SM, over RangeArgs::b_list, whose length is
+// known on the device only.
+template <int FN, int RING, bool TS32>
+int launch_warp_tier(b2p_ctx* c, RangeArgs a) {
+  constexpr bool kBig = RING == kBigRing;
+  static_assert(!kBig || TS32, "the long-window instantiation is 32-bit only");
+  constexpr size_t smem = (size_t)kWarpsPerCta * (2 * RING * (8 + (TS32 ? 4 : 8)) + RING / 8) + kRcpTable * 8;
+  auto kern = range_fast_kernel<FN, RING, TS32>;
+  if (kBig) a.use_w_list = 2;
+  unsigned grid = 0;
+  if (int rc = persistent_grid(c, kern, smem, kWarpsPerCta, kBig ? kAllResident : a.n_series, &grid)) return rc;
+  return launch_kernel(c, kern, grid, kWarpsPerCta * 32, smem, a);
 }
 
 // Functions whose first tier has a uniform-cadence variant: the probe (or B2P_UNIFORM) writes Status::uniform, then
 // both variants are launched and the one the verdict does not name returns at once — no host round trip.
-static int cadence_verdict(b2p_ctx* c, const RangeArgs& a) {
-  if (c->uniform_mode < 0) {
-    cadence_probe_kernel<<<1, kProbeThreads, 0, c->stream>>>(a);
-    c->launches++;
-    CU(cudaGetLastError());
-  } else {
-    CU(cudaMemsetAsync(&a.status->uniform, c->uniform_mode ? 1 : 0, sizeof(uint32_t), c->stream));
-  }
+int cadence_verdict(b2p_ctx* c, const RangeArgs& a) {
+  if (c->uniform_mode < 0) return launch_kernel(c, cadence_probe_kernel, 1, kProbeThreads, 0, a);
+  CU(cudaMemsetAsync(&a.status->uniform, c->uniform_mode ? 1 : 0, sizeof(uint32_t), c->stream));
   return B2P_OK;
 }
 
-template <int FN, bool FLAGS, bool UNI>
-int launch_lean_variant(b2p_ctx* c, const RangeArgs& a) {
-  constexpr size_t smem = lean_smem_bytes(UNI);
-  auto kern = range_lean_kernel<FN, FLAGS, false, UNI>;
+// One variant of the first tier (range_lean_kernel).  Plain: a persistent grid over the series.  GROUPED (the fused
+// by-label SUM: rate / increase / delta walk the series group by group and add into gsum / gcnt): one CTA per SM that
+// takes its groups from a counter, so the grid can be any size; while tiles are being all-reduced a few SMs are left
+// to the collective's CTAs (they cannot be placed beside a resident 24-warp CTA).
+template <int FN, bool FLAGS, bool GROUPED, bool UNI>
+int launch_first_variant(b2p_ctx* c, const RangeArgs& a) {
+  constexpr size_t smem = GROUPED ? lean_grouped_smem_bytes(UNI) : lean_smem_bytes(UNI);
+  auto kern = range_lean_kernel<FN, FLAGS, GROUPED, UNI>;
   unsigned grid = 0;
-  if (int rc = persistent_grid(c, kern, smem, kLeanWarps, a.n_series, &grid)) return rc;
-  if (grid == 0) return B2P_OK;
-  kern<<<grid, kLeanWarps * 32, smem, c->stream>>>(a);
-  c->launches++;
-  CU(cudaGetLastError());
-  return B2P_OK;
+  if (int rc = persistent_grid(c, kern, smem, kLeanWarps, GROUPED ? kAllResident : a.n_series, &grid)) return rc;
+  if constexpr (GROUPED) {
+    const unsigned need = (a.g_hi - a.g_lo + kLeanWarps - 1) / kLeanWarps;
+    if (c->comm_reserve_now > 0 && grid > (unsigned)c->comm_reserve_now + 8u) grid -= (unsigned)c->comm_reserve_now;
+    if (need < grid) grid = need;
+  }
+  return launch_kernel(c, kern, grid, kLeanWarps * 32, smem, a);
 }
 
-template <int FN, bool FLAGS>
-int launch_lean(b2p_ctx* c, const RangeArgs& a) {
+// Both uniform-cadence variants of the first tier where FN has them (cadence_verdict names one on the device), else
+// the one variant.
+template <int FN, bool GROUPED, bool FLAGS>
+int launch_first_pair(b2p_ctx* c, const RangeArgs& a) {
   if constexpr (kLeanUniform<FN, FLAGS>) {
     int rc = cadence_verdict(c, a);
-    if (!rc && c->uniform_mode != 0) rc = launch_lean_variant<FN, FLAGS, true>(c, a);
-    if (!rc && c->uniform_mode != 1) rc = launch_lean_variant<FN, FLAGS, false>(c, a);
+    if (!rc && c->uniform_mode != 0) rc = launch_first_variant<FN, FLAGS, GROUPED, true>(c, a);
+    if (!rc && c->uniform_mode != 1) rc = launch_first_variant<FN, FLAGS, GROUPED, false>(c, a);
     return rc;
   } else {
-    return launch_lean_variant<FN, FLAGS, false>(c, a);
+    return launch_first_variant<FN, FLAGS, GROUPED, false>(c, a);
   }
 }
 
-// `with_flags`: the variant whose ring carries the reset / change bit words (always for resets() / changes(); for
-// rate / increase when the adaptive policy picked it; never for the other functions).
-template <int FN>
-int launch_lean_if_supported(b2p_ctx* c, const RangeArgs& a, bool with_flags) {
-  if constexpr (!LeanTraits<FN>::kSupported) {
-    return fail(B2P_E_INVALID, "fn_id %d has no lean tier", FN);
+// The first tier (K2L) of FN, plain or GROUPED.  `with_flags`: the variant whose ring carries the reset / change bit
+// words (always for resets() / changes(); for rate / increase when the adaptive policy picked it; never for the other
+// functions).
+template <int FN, bool GROUPED>
+int launch_first_tier(b2p_ctx* c, const RangeArgs& a, bool with_flags) {
+  if constexpr (GROUPED ? !rate_like(FN) : !LeanTraits<FN>::kSupported) {
+    return fail(B2P_E_INVALID, GROUPED ? "fn_id %d has no fused by-label tier" : "fn_id %d has no lean tier", FN);
   } else if constexpr (LeanTraits<FN>::kNeedsFlags) {
-    return launch_lean<FN, true>(c, a);
+    return launch_first_pair<FN, GROUPED, true>(c, a);
   } else if constexpr (LeanTraits<FN>::kHasFlagsVariant) {
-    return with_flags ? launch_lean<FN, true>(c, a) : launch_lean<FN, false>(c, a);
+    return with_flags ? launch_first_pair<FN, GROUPED, true>(c, a) : launch_first_pair<FN, GROUPED, false>(c, a);
   } else {
-    return launch_lean<FN, false>(c, a);
-  }
-}
-
-// First tier of the fused by-label SUM: rate / increase / delta walk the series group by group and add into
-// gsum / gcnt (range_lean_kernel<FN, FLAGS, GROUPED = true>).
-template <int FN, bool FLAGS, bool UNI>
-int launch_lean_grouped_variant(b2p_ctx* c, const RangeArgs& a) {
-  constexpr size_t smem = lean_grouped_smem_bytes(UNI);
-  auto kern = range_lean_kernel<FN, FLAGS, true, UNI>;
-  unsigned cap = 0;
-  if (int rc = persistent_grid(c, kern, smem, kLeanWarps, kAllResident, &cap)) return rc;
-  const unsigned n_g = a.g_hi - a.g_lo;
-  const unsigned need = (n_g + kLeanWarps - 1) / kLeanWarps;
-  // The grid is one CTA per SM and takes its groups from a counter, so it can be any size: while tiles are being
-  // all-reduced a few SMs are left to the collective's CTAs (they cannot be placed beside a resident 24-warp CTA).
-  if (c->comm_reserve_now > 0 && cap > (unsigned)c->comm_reserve_now + 8u) cap -= (unsigned)c->comm_reserve_now;
-  const unsigned grid = need < cap ? need : cap;
-  if (grid == 0) return B2P_OK;
-  kern<<<grid, kLeanWarps * 32, smem, c->stream>>>(a);
-  c->launches++;
-  CU(cudaGetLastError());
-  return B2P_OK;
-}
-template <int FN, bool FLAGS>
-int launch_lean_grouped(b2p_ctx* c, const RangeArgs& a) {
-  if constexpr (kLeanUniform<FN, FLAGS>) {
-    int rc = cadence_verdict(c, a);
-    if (!rc && c->uniform_mode != 0) rc = launch_lean_grouped_variant<FN, FLAGS, true>(c, a);
-    if (!rc && c->uniform_mode != 1) rc = launch_lean_grouped_variant<FN, FLAGS, false>(c, a);
-    return rc;
-  } else {
-    return launch_lean_grouped_variant<FN, FLAGS, false>(c, a);
-  }
-}
-template <int FN>
-int launch_lean_grouped_if_supported(b2p_ctx* c, const RangeArgs& a, bool with_flags) {
-  if constexpr (!rate_like(FN)) {
-    return fail(B2P_E_INVALID, "fn_id %d has no fused by-label tier", FN);
-  } else if constexpr (LeanTraits<FN>::kHasFlagsVariant) {
-    return with_flags ? launch_lean_grouped<FN, true>(c, a) : launch_lean_grouped<FN, false>(c, a);
-  } else {
-    return launch_lean_grouped<FN, false>(c, a);
+    return launch_first_pair<FN, GROUPED, false>(c, a);
   }
 }
 
@@ -203,27 +165,14 @@ template <int FN>
 int launch_thread_tier(b2p_ctx* c, const RangeArgs& a) {
   if constexpr (!rate_like(FN)) {
     return fail(B2P_E_INVALID, "fn_id %d has no thread tier", FN);
-  } else {
-    // at most the 1-warp CTAs whose rings fit in shared memory
+  } else {  // at most the 1-warp CTAs whose rings fit in shared memory
     const unsigned grid = capped_grid(c, a.n_series, 32, 220 * 1024 / (kTRing * 32 * 12 + 512));
-    if (grid == 0) return B2P_OK;
-    range_thread_kernel<FN><<<grid, 32, 0, c->stream>>>(a);
-    c->launches++;
-    CU(cudaGetLastError());
-    return B2P_OK;
+    return launch_kernel(c, range_thread_kernel<FN>, grid, 32, 0, a);
   }
 }
 
-template <int FN>
-int launch_slow(b2p_ctx* c, const RangeArgs& a) {
-  range_slow_kernel<FN><<<kSlowCtas, 128, 0, c->stream>>>(a);
-  c->launches++;
-  CU(cudaGetLastError());
-  return B2P_OK;
-}
-
 int dispatch_slow(b2p_ctx* c, int fn, const RangeArgs& a) {
-  return with_fn(fn, [&](auto k) { return launch_slow<decltype(k)::value>(c, a); });
+  return with_fn(fn, [&](auto k) { return launch_kernel(c, range_slow_kernel<decltype(k)::value>, kSlowCtas, 128, 0, a); });
 }
 
 // The window and time-domain fields of a range call over T steps (check_grid has accepted p); the first tier's gates
@@ -296,10 +245,10 @@ __global__ void comm_headstart_kernel(long long cycles) {
   while (clock64() - t0 < cycles) {}
 }
 
-// Launches every tier of one range call (first tier when `used_lean`/`thread_tier`, warp-per-series kernel, its
-// long-window instantiation, exact slow kernel) on the context's stream.
-static int launch_range_tiers(b2p_ctx* c, int fn, RangeArgs a, bool thread_tier, bool used_lean, int lean_mode,
-                              bool later_tile = false) {
+// Launches every tier of a range call (its first tier or thread tier, warp-per-series kernel, long-window
+// instantiation, exact slow kernel) on the context's stream.
+static int launch_range_tiers(b2p_ctx* c, const b2p_ctx::Pending& pc, bool later_tile = false) {
+  RangeArgs a = pc.args;
   int rc;
   if (!later_tile) {
     CU(cudaMemsetAsync(a.status, 0, sizeof(Status), c->stream));
@@ -308,93 +257,126 @@ static int launch_range_tiers(b2p_ctx* c, int fn, RangeArgs a, bool thread_tier,
     CU(cudaMemsetAsync(&a.status->w_count, 0, 3 * sizeof(uint32_t), c->stream));  // w_count, b_count, g_next
   }
   stage_begin(c, 1);
-  if (thread_tier || used_lean) {
-    rc = with_fn(fn, [&](auto k) {
+  if (pc.tiers.thread_tier || pc.tiers.first_tier) {
+    rc = with_fn(pc.fn, [&](auto k) {
       constexpr int FN = decltype(k)::value;
-      if (thread_tier) return launch_thread_tier<FN>(c, a);
-      return a.gsum ? launch_lean_grouped_if_supported<FN>(c, a, lean_mode == 1)
-                    : launch_lean_if_supported<FN>(c, a, lean_mode == 1);
+      if (pc.tiers.thread_tier) return launch_thread_tier<FN>(c, a);
+      const bool with_flags = pc.tiers.lean_mode == 1;
+      return a.gsum ? launch_first_tier<FN, true>(c, a, with_flags) : launch_first_tier<FN, false>(c, a, with_flags);
     });
     if (rc) return rc;
     a.use_w_list = 1;
   }
-  rc = with_fn(fn, [&](auto k) {
+  rc = with_fn(pc.fn, [&](auto k) {
     constexpr int FN = decltype(k)::value;
-    const int r = launch_fast<FN>(c, a);
-    return (r || !a.b_list) ? r : launch_big<FN>(c, a);
+    const int r = fits_ts32(a) ? launch_warp_tier<FN, kRing, true>(c, a) : launch_warp_tier<FN, kRing, false>(c, a);
+    return (r || !a.b_list) ? r : launch_warp_tier<FN, kBigRing, true>(c, a);
   });
   stage_end(c, 1);
   if (rc) return rc;
   stage_begin(c, 2);
-  rc = dispatch_slow(c, fn, a);
+  rc = dispatch_slow(c, pc.fn, a);
   stage_end(c, 2);
   return rc;
+}
+
+// The sticky verdict of the series-id scan (K0): read back (with whatever the stream has queued before it), cleared,
+// and returned as an error.
+static int take_k0(b2p_ctx* c) {
+  CU(cudaMemcpyAsync(c->h_k0, c->d_k0, sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  if (const uint32_t k0 = c->h_k0->k0_errors) {
+    CU(cudaMemsetAsync(c->d_k0, 0, sizeof(Status), c->stream));
+    return k0_fail(k0);
+  }
+  return B2P_OK;
+}
+
+// The arena rows a call whose slow path ran out of arena needs to be redone (0: it fit).
+static size_t redo_rows(const Status& st) { return st.arena_overflow ? (size_t)st.arena_needed + 1024 : 0; }
+
+// The outcome of one range call from the Status of each of its `n` records (one; or one per chunk of a host call):
+// the hand-off counters (summed over the records) and the adaptive verdict, taken over all of them with the tiers of
+// the last — unless `redo`: a redo is not a new call.  Returns the arena rows the largest record that ran out of
+// arena needs (0: every one fit).
+static size_t read_outcome(b2p_ctx* c, const b2p_ctx::Pending* recs, const Status* st, size_t n, bool redo) {
+  size_t need = 0;
+  long long slow = 0, handed = 0;
+  uint64_t series = 0;
+  for (size_t i = 0; i < n; ++i) {
+    slow += st[i].slow_count;
+    handed += st[i].w_count;
+    series += recs[i].n_series;
+    need = std::max(need, redo_rows(st[i]));
+  }
+  if (!redo) {
+    c->last_slow = slow;
+    c->last_w = handed;
+    const b2p_ctx::Pending& last = recs[n - 1];
+    if (last.tiers.first_tier) lean_verdict(c, last.fn, last.tiers.lean_mode, (uint64_t)handed, series);
+  }
+  return need;
+}
+
+// Runs again the calls in `redo`, whose slow path ran out of arena, after the arena has grown to `need` rows, until
+// every one fits.  They run one at a time, as they were admitted: they share the arena from offset 0.  A fused call
+// repeats its slow kernel only, over its intact work list (a series that did not fit the arena added nothing; no
+// other range call was admitted while it was outstanding); a merged call cannot be repeated.
+static int redo_calls(b2p_ctx* c, std::vector<b2p_ctx::Pending> redo, size_t need) {
+  for (int round = 0; round < 3 && !redo.empty(); ++round) {
+    int rc;
+    if ((rc = c->arena_ts.ensure(need * 8)) || (rc = c->arena_val.ensure(need * 8))) return rc;
+    c->arena_rows = need;
+    for (b2p_ctx::Pending& pc : redo) {
+      if (pc.kind == b2p_ctx::Pending::kMerged)
+        return fail(B2P_E_TOO_LARGE, "a series of %llu+ rows needs the exact slow path but does not fit its arena region; "
+                    "the merged partials are incomplete — set B2P_ARENA_ROWS >= %zu and repeat the query",
+                    (unsigned long long)(need / (size_t)kSlowWarps), need);
+      pc.args.arena_ts = c->arena_ts.as<int64_t>();
+      pc.args.arena_val = c->arena_val.as<double>();
+      pc.args.arena_cap = need;
+      if (pc.kind == b2p_ctx::Pending::kFused) {
+        Status& patch = c->h_ring[pc.slot];
+        patch.arena_overflow = 0; patch.arena_used = 0; patch.arena_needed = 0;
+        CU(cudaMemcpyAsync(c->d_ring + pc.slot, c->h_ring + pc.slot, sizeof(Status), cudaMemcpyHostToDevice, c->stream));
+        rc = dispatch_slow(c, pc.fn, pc.args);
+      } else {
+        rc = launch_range_tiers(c, pc);
+      }
+      if (rc) return rc;
+      CU(cudaStreamSynchronize(c->stream));
+    }
+    CU(cudaMemcpyAsync(c->h_ring, c->d_ring, kStatusSlots * sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    std::vector<b2p_ctx::Pending> again;
+    need = 0;
+    for (const b2p_ctx::Pending& pc : redo)
+      if (const size_t rows = read_outcome(c, &pc, &c->h_ring[pc.slot], 1, true)) {
+        again.push_back(pc);
+        need = std::max(need, rows);
+      }
+    redo.swap(again);
+  }
+  return redo.empty() ? B2P_OK : fail(B2P_E_NOMEM, "slow-path arena could not be sized");
 }
 
 int b2p_sync(b2p_ctx* c) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   DeviceGuard g(c->device);
-  for (int attempt = 0; attempt < 4; ++attempt) {
-    CU(cudaMemcpyAsync(c->h_ring, c->d_ring, kStatusSlots * sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaMemcpyAsync(c->h_k0, c->d_k0, sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    const uint32_t k0 = c->h_k0->k0_errors;
-    if (k0) {
-      CU(cudaMemsetAsync(c->d_k0, 0, sizeof(Status), c->stream));
-      c->pending.clear();
-      return k0_fail(k0);
+  CU(cudaMemcpyAsync(c->h_ring, c->d_ring, kStatusSlots * sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
+  std::vector<b2p_ctx::Pending> calls;
+  calls.swap(c->pending);
+  c->fused_pending = false;
+  if (int rc = take_k0(c)) return rc;
+  // the outstanding range calls, oldest first; those whose slow path ran out of arena are redone
+  std::vector<b2p_ctx::Pending> redo;
+  size_t need = 0;
+  for (const b2p_ctx::Pending& pc : calls)
+    if (const size_t rows = read_outcome(c, &pc, &c->h_ring[pc.slot], 1, false)) {
+      redo.push_back(pc);
+      need = std::max(need, rows);
     }
-    // verdicts of the outstanding range calls, oldest first; a call whose slow path ran out of arena is redone
-    // as a whole (all tiers, same modes) after the arena has grown to what the largest of them needs
-    size_t need = 0;
-    std::vector<b2p_ctx::Pending> redo;
-    for (auto& pc : c->pending) {
-      const Status st = c->h_ring[pc.slot];
-      c->last_slow = st.slow_count;
-      c->last_w = st.w_count;
-      if (pc.used_lean && !pc.verdict_taken) {
-        c->last_lean_mode = pc.lean_mode;
-        lean_verdict(c, pc.fn, st.w_count, pc.n_series);
-        pc.verdict_taken = true;
-      }
-      if (st.arena_overflow) {
-        if ((size_t)st.arena_needed + 1024 > need) need = (size_t)st.arena_needed + 1024;
-        redo.push_back(pc);
-      }
-    }
-    c->pending.clear();
-    c->fused_pending = false;
-    if (redo.empty()) return B2P_OK;
-    int rc;
-    if ((rc = c->arena_ts.ensure(need * 8))) return rc;
-    if ((rc = c->arena_val.ensure(need * 8))) return rc;
-    c->arena_rows = need;
-    for (auto& pc : redo) {
-      pc.args.arena_ts = c->arena_ts.as<int64_t>();
-      pc.args.arena_val = c->arena_val.as<double>();
-      pc.args.arena_cap = need;
-      if (pc.merged)
-        return fail(B2P_E_TOO_LARGE, "a series of %llu+ rows needs the exact slow path but does not fit its arena region; "
-                    "the merged partials are incomplete — set B2P_ARENA_ROWS >= %zu and repeat the query",
-                    (unsigned long long)(need / (size_t)kSlowWarps), need);
-      if (pc.fused) {
-        // partials were added in place: only the slow kernel runs again, over its intact work list (a series that
-        // did not fit the arena added nothing); no other range call was admitted while this one was outstanding
-        Status patch = c->h_ring[pc.slot];
-        patch.arena_overflow = 0; patch.arena_used = 0; patch.arena_needed = 0;
-        c->h_ring[pc.slot] = patch;
-        CU(cudaMemcpyAsync(c->d_ring + pc.slot, c->h_ring + pc.slot, sizeof(Status), cudaMemcpyHostToDevice, c->stream));
-        if ((rc = dispatch_slow(c, pc.fn, pc.args))) return rc;
-        c->pending.push_back(pc);
-        CU(cudaStreamSynchronize(c->stream));
-        continue;
-      }
-      if ((rc = launch_range_tiers(c, pc.fn, pc.args, pc.thread_tier, pc.used_lean, pc.lean_mode))) return rc;
-      c->pending.push_back(pc);
-      CU(cudaStreamSynchronize(c->stream));  // one redone call at a time: they share the arena from offset 0
-    }
-  }
-  return fail(B2P_E_NOMEM, "slow-path arena could not be sized");
+  return redo_calls(c, std::move(redo), need);
 }
 
 /* ---- device-pointer API ---------------------------------------------------------------------- */
@@ -433,17 +415,58 @@ struct GroupTarget {
   int allreduce_tiles;
 };
 
-// Can this range call add its results straight into by-label partials?  (first tier available for the function and
-// the query shape, and not switched off by the adaptive policy; groups balanced enough for group-exclusive warps)
+// Can this range call add its results straight into by-label partials?  (the first tier runs for the function and
+// the query shape, not switched off by the adaptive policy; groups balanced enough for group-exclusive warps)
 static bool fused_group_ok(b2p_ctx* c, const b2p_range_params* p, int64_t T, const b2p_group_index* idx) {
-  if (!rate_like(p->fn_id) || c->thread_tier) return false;
+  if (!rate_like(p->fn_id)) return false;
   if (T > 32 * (int64_t)kLeanFullWords) return false;  // per-warp word counters of the first tier
-  if (!lean_ok(c, p->fn_id, range_geometry(p, T))) return false;
-  if (c->lean_backoff[p->fn_id] > 0 && c->lean_mode[p->fn_id] == 2) return false;
+  if (!choose_tiers(c, p->fn_id, range_geometry(p, T)).first_tier) return false;
   // a group is walked by ONE warp: the largest group may not exceed a few times a warp's fair share
   const uint64_t warps = (uint64_t)c->num_sms * B2P_LEAN_MIN_BLOCKS * kLeanWarps;
   const uint64_t share = idx->n_series / warps + 1;
   return (uint64_t)idx->max_members <= 8 * share + 64;
+}
+
+// A fused call whose partials are all-reduced: its group range in `n_tiles` tiles, each tile's rows of gsum / gcnt
+// all-reduced over the context's communicator as soon as the tile is complete, on the (high-priority) communication
+// stream, while the next tile computes.
+static int launch_allreduce_tiles(b2p_ctx* c, const b2p_ctx::Pending& pc, uint32_t n_tiles) {
+  if (!c->comm && c->comm_ranks > 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
+  const RangeArgs& a = pc.args;
+  const uint64_t span = (uint64_t)a.g_hi - a.g_lo;
+  c->comm_reserve_now = (c->comm && n_tiles > 1) ? c->comm_reserve_sms : 0;
+  for (uint32_t t = 0; t < n_tiles; ++t) {
+    b2p_ctx::Pending tile = pc;
+    tile.args.g_lo = a.g_lo + (uint32_t)(span * t / n_tiles);
+    tile.args.g_hi = a.g_lo + (uint32_t)(span * (t + 1) / n_tiles);
+    if (tile.args.g_hi == tile.args.g_lo) continue;
+    if (int rc = launch_range_tiers(c, tile, t > 0)) return rc;
+    if (c->comm) {
+      const size_t off = (size_t)tile.args.g_lo * (size_t)a.T, cnt_n = (size_t)(tile.args.g_hi - tile.args.g_lo) * (size_t)a.T;
+      CU(cudaEventRecord(c->ev_comm_in, c->stream));
+      CU(cudaStreamWaitEvent(c->s_comm, c->ev_comm_in, 0));
+      // The next tile's kernels are released by a marker that sits directly IN FRONT of the all-reduce on the
+      // communication stream: when they become runnable the (few) NCCL CTAs are already next in line on the
+      // high-priority stream and get their SMs first; the persistent first-tier kernel fills what is left and its
+      // dynamic group counter keeps late CTAs from becoming a tail.
+      comm_marker_kernel<<<1, 32, 0, c->s_comm>>>();
+      CU(cudaEventRecord(c->ev_comm_go, c->s_comm));
+      CU(cudaStreamWaitEvent(c->stream, c->ev_comm_go, 0));
+      if (c->comm_headstart_cycles > 0) comm_headstart_kernel<<<1, 32, 0, c->stream>>>(c->comm_headstart_cycles);
+      stage_begin(c, 4, c->s_comm);
+      NCCL_TRY(g_nccl.GroupStart());
+      NCCL_TRY(g_nccl.AllReduce(a.gsum + off, a.gsum + off, cnt_n, Nccl::kFloat64, Nccl::kSum, c->comm, c->s_comm));
+      NCCL_TRY(g_nccl.AllReduce(a.gcnt + off, a.gcnt + off, cnt_n, Nccl::kUint32, Nccl::kSum, c->comm, c->s_comm));
+      NCCL_TRY(g_nccl.GroupEnd());
+      stage_end(c, 4, c->s_comm);
+    }
+  }
+  c->comm_reserve_now = 0;
+  if (c->comm) {  // everything after this call on the context's stream sees the merged partials
+    CU(cudaEventRecord(c->ev_comm_done, c->s_comm));
+    CU(cudaStreamWaitEvent(c->stream, c->ev_comm_done, 0));
+  }
+  return B2P_OK;
 }
 
 static int range_call(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
@@ -492,68 +515,16 @@ static int range_call(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, 
   a.use_w_list = 0;
   a.arena_ts = c->arena_ts.as<int64_t>(); a.arena_val = c->arena_val.as<double>(); a.arena_cap = c->arena_rows;
   a.win_scratch = c->win_scratch.as<unsigned long long>();
-  // tier 1 (rate / increase / delta, 32-bit time domain): thread per series (opt-in) or the lean warp-per-series
-  // kernel; what it declines goes to tier 2 (warp per series) through w_list, long windows from there to the
-  // 1024-sample instantiation through b_list, and what that declines to the exact slow kernel
-  const bool tier1 = c->thread_tier && fits_ts32(a) && rate_like(p->fn_id);
-  bool used_lean = false;
-  int mode = 0;
-  if (!tier1 && lean_ok(c, p->fn_id, a)) {
-    if (c->lean_backoff[p->fn_id] > 0) {
-      c->lean_backoff[p->fn_id]--;
-      mode = c->lean_mode[p->fn_id];
-    }
-    if (mode != 2) used_lean = true;
-    if (mode == 0 && c->lean_force_flags) mode = 1;
-  }
-  if (gt && !used_lean) return fail(B2P_E_INVALID, "fused by-label call without its first tier (internal)");
-  c->last_lean_mode = mode;
-  c->last_used_lean = used_lean;
-  c->last_range_series = n_series;
-  c->last_range_fn = p->fn_id;
-  if (gt && gt->allreduce_tiles > 0) {
-    if (!c->comm && c->comm_ranks > 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
-    const uint32_t n_t = (uint32_t)gt->allreduce_tiles;
-    const uint64_t span = (uint64_t)gt->g_hi - gt->g_lo;
-    c->comm_reserve_now = (c->comm && n_t > 1) ? c->comm_reserve_sms : 0;
-    for (uint32_t t = 0; t < n_t; ++t) {
-      a.g_lo = gt->g_lo + (uint32_t)(span * t / n_t);
-      a.g_hi = gt->g_lo + (uint32_t)(span * (t + 1) / n_t);
-      if (a.g_hi == a.g_lo) continue;
-      if ((rc = launch_range_tiers(c, p->fn_id, a, tier1, used_lean, mode, t > 0))) return rc;
-      if (c->comm) {
-        const size_t off = (size_t)a.g_lo * (size_t)T, cnt_n = (size_t)(a.g_hi - a.g_lo) * (size_t)T;
-        CU(cudaEventRecord(c->ev_comm_in, c->stream));
-        CU(cudaStreamWaitEvent(c->s_comm, c->ev_comm_in, 0));
-        // The next tile's kernels are released by a marker that sits directly IN FRONT of the all-reduce on the
-        // communication stream: when they become runnable the (few) NCCL CTAs are already next in line on the
-        // high-priority stream and get their SMs first; the persistent first-tier kernel fills what is left and its
-        // dynamic group counter keeps late CTAs from becoming a tail.
-        comm_marker_kernel<<<1, 32, 0, c->s_comm>>>();
-        CU(cudaEventRecord(c->ev_comm_go, c->s_comm));
-        CU(cudaStreamWaitEvent(c->stream, c->ev_comm_go, 0));
-        if (c->comm_headstart_cycles > 0) comm_headstart_kernel<<<1, 32, 0, c->stream>>>(c->comm_headstart_cycles);
-        stage_begin_on(c, 4, c->s_comm);
-        NCCL_TRY(g_nccl.GroupStart());
-        NCCL_TRY(g_nccl.AllReduce(a.gsum + off, a.gsum + off, cnt_n, Nccl::kFloat64, Nccl::kSum, c->comm, c->s_comm));
-        NCCL_TRY(g_nccl.AllReduce(a.gcnt + off, a.gcnt + off, cnt_n, Nccl::kUint32, Nccl::kSum, c->comm, c->s_comm));
-        NCCL_TRY(g_nccl.GroupEnd());
-        stage_end_on(c, 4, c->s_comm);
-      }
-    }
-    c->comm_reserve_now = 0;
-    if (c->comm) {  // everything after this call on the context's stream sees the merged partials
-      CU(cudaEventRecord(c->ev_comm_done, c->s_comm));
-      CU(cudaStreamWaitEvent(c->stream, c->ev_comm_done, 0));
-    }
-    a.g_lo = gt->g_lo; a.g_hi = gt->g_hi;
-  } else if ((rc = launch_range_tiers(c, p->fn_id, a, tier1, used_lean, mode))) {
-    return rc;
-  }
   b2p_ctx::Pending pc{};
-  pc.slot = slot; pc.fn = p->fn_id; pc.args = a; pc.lean_mode = mode; pc.thread_tier = tier1; pc.used_lean = used_lean;
-  pc.n_series = n_series; pc.verdict_taken = false; pc.fused = gt != nullptr;
-  pc.merged = gt && gt->allreduce_tiles > 0;
+  pc.slot = slot; pc.fn = p->fn_id; pc.args = a; pc.n_series = n_series;
+  pc.tiers = choose_tiers(c, p->fn_id, a);
+  // the choice read the back-off where the first tier applies: it runs, or mode 2 skips it
+  if ((pc.tiers.first_tier || pc.tiers.lean_mode == 2) && c->lean_backoff[p->fn_id] > 0) c->lean_backoff[p->fn_id]--;
+  if (gt && !pc.tiers.first_tier) return fail(B2P_E_INVALID, "fused by-label call without its first tier (internal)");
+  pc.kind = !gt ? b2p_ctx::Pending::kPlain : gt->allreduce_tiles > 0 ? b2p_ctx::Pending::kMerged : b2p_ctx::Pending::kFused;
+  rc = pc.kind == b2p_ctx::Pending::kMerged ? launch_allreduce_tiles(c, pc, (uint32_t)gt->allreduce_tiles)
+                                            : launch_range_tiers(c, pc);
+  if (rc) return rc;
   c->pending.push_back(pc);
   if (gt) c->fused_pending = true;
   return B2P_OK;
@@ -578,22 +549,33 @@ int b2p_range_udf_dev(b2p_ctx* c, int32_t fn_id, const int64_t* ts, const double
   return rc;
 }
 
+}  // extern "C"
+
+// The grid of an instant selector: check_grid over lookback windows, and the grid fields of its kernel arguments.
+static int instant_grid(int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
+                        uint32_t n_series, InstantArgs* a) {
+  b2p_range_params p{};
+  p.start = start; p.end = end; p.interval = interval; p.range = lookback;
+  int64_t T = 0;
+  if (int rc = check_grid(&p, n_series, &T)) return rc;
+  *a = InstantArgs{};
+  a->start = start; a->end = end; a->interval = interval; a->lookback = lookback; a->offset = offset;
+  a->T = T; a->Tw = (uint32_t)((T + 31) / 32); a->n_series = n_series;
+  return B2P_OK;
+}
+
+extern "C" {
+
 int b2p_instant_select_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
                            const int64_t* ts, const double* val, const uint64_t* offsets, uint64_t n_rows,
                            uint32_t n_series, double* out, uint32_t* valid_words) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  b2p_range_params p{};
-  p.start = start; p.end = end; p.interval = interval; p.range = lookback;
-  int64_t T = 0;
-  int rc = check_grid(&p, n_series, &T);
-  if (rc) return rc;
-  if (n_series == 0 || T == 0) return B2P_OK;
+  InstantArgs a;
+  if (int rc = instant_grid(start, end, interval, lookback, offset, n_series, &a)) return rc;
+  if (n_series == 0 || a.T == 0) return B2P_OK;
   if (!offsets || !out || !valid_words || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
   DeviceGuard g(c->device);
-  InstantArgs a{};
-  a.start = start; a.end = end; a.interval = interval; a.lookback = lookback; a.offset = offset;
-  a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
-  a.ts = ts; a.val = val; a.offsets = offsets; a.n_series = n_series; a.out = out; a.valid = valid_words;
+  a.ts = ts; a.val = val; a.offsets = offsets; a.out = out; a.valid = valid_words;
   stage_begin(c, 1);
   instant_kernel<<<capped_grid(c, n_series, kWarpsPerCta, 8), kWarpsPerCta * 32, 0, c->stream>>>(a);
   c->launches++;
@@ -661,14 +643,14 @@ static int first_null_field(b2p_ctx* c, const uint8_t* const* field_valid, int32
   return B2P_OK;
 }
 
-// An outstanding range call reads or writes the multi-field scratch, and b2p_sync may run it again there.
-static bool fields_scratch_pending(const b2p_ctx* c) {
-  auto in = [](const DevBuf& b, const void* p) {
-    const char* lo = b.as<char>();
-    return lo && static_cast<const char*>(p) >= lo && static_cast<const char*>(p) < lo + b.cap;
-  };
-  for (const b2p_ctx::Pending& pc : c->pending)
-    if (in(c->fd_val, pc.args.val) || in(c->fd_valid, pc.args.valid)) return true;
+// An outstanding range call reads or writes `b`, and b2p_sync may run it again there: `b` must not change before that.
+static bool pending_reads(const b2p_ctx* c, const DevBuf& b) {
+  const char* lo = b.as<char>();
+  auto in = [&](const void* p) { return lo && static_cast<const char*>(p) >= lo && static_cast<const char*>(p) < lo + b.cap; };
+  for (const b2p_ctx::Pending& pc : c->pending) {
+    const RangeArgs& a = pc.args;
+    if (in(a.ts) || in(a.val) || in(a.offsets) || in(a.out) || in(a.valid)) return true;
+  }
   return false;
 }
 
@@ -698,7 +680,7 @@ int b2p_range_eval_fields_dev(b2p_ctx* c, const b2p_range_params* p, const int64
   const uint64_t words = (uint64_t)n_series * Tw;
   const double* fv[kMaxFields];
   for (int f = 0; f < F; ++f) fv[f] = vals[f];
-  if (fields_scratch_pending(c) && (rc = b2p_sync(c))) return rc;
+  if ((pending_reads(c, c->fd_val) || pending_reads(c, c->fd_valid)) && (rc = b2p_sync(c))) return rc;
   if (p->filter_nan && n_rows) {
     const uint64_t stride = (n_rows + 1) & ~1ull;  // 16-byte aligned columns
     if ((rc = c->fd_val.ensure((size_t)F * stride * 8))) return rc;
@@ -749,19 +731,14 @@ int b2p_instant_select_fields_dev(b2p_ctx* c, int64_t start, int64_t end, int64_
   if (n_fields == 1)
     return b2p_instant_select_dev(c, start, end, interval, lookback, offset, ts, vals[0], offsets, n_rows, n_series,
                                   outs[0], valid_words);
-  b2p_range_params p{};
-  p.start = start; p.end = end; p.interval = interval; p.range = lookback;
-  int64_t T = 0;
-  if ((rc = check_grid(&p, n_series, &T))) return rc;
-  if (n_series == 0 || T == 0) return B2P_OK;
+  FieldsInstantArgs fa{};
+  InstantArgs& a = fa.g;
+  if ((rc = instant_grid(start, end, interval, lookback, offset, n_series, &a))) return rc;
+  if (n_series == 0 || a.T == 0) return B2P_OK;
   if (!offsets || !valid_words || (!ts && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
   if ((rc = check_field_columns(vals, outs, n_fields, n_rows))) return rc;
   DeviceGuard g(c->device);
-  FieldsInstantArgs fa{};
-  InstantArgs& a = fa.g;
-  a.start = start; a.end = end; a.interval = interval; a.lookback = lookback; a.offset = offset;
-  a.T = T; a.Tw = (uint32_t)((T + 31) / 32);
-  a.ts = ts; a.val = vals[0]; a.offsets = offsets; a.n_series = n_series; a.out = outs[0]; a.valid = valid_words;
+  a.ts = ts; a.val = vals[0]; a.offsets = offsets; a.out = outs[0]; a.valid = valid_words;
   fa.F = n_fields;
   for (int f = 0; f < n_fields; ++f) { fa.vals[f] = vals[f]; fa.outs[f] = outs[f]; }
   stage_begin(c, 1);
@@ -872,14 +849,6 @@ int scan_valid_cells(b2p_ctx* c, const uint32_t* valid, uint64_t T, uint32_t row
 }
 
 namespace {
-// A range call of this context that reads the subquery scratch and whose verdict b2p_sync has not taken yet: b2p_sync
-// may run it again from the scratch (slow-path arena overflow), so the scratch must not change before that.
-bool subquery_scratch_pending(const b2p_ctx* c) {
-  for (const b2p_ctx::Pending& pc : c->pending)
-    if (pc.args.ts == c->sq_ts.as<int64_t>()) return true;
-  return false;
-}
-
 // Rows are processed in batches of at most kSqBatchCells / T_inner rows (one row when a row alone is larger).  Per
 // batch: K13's count kernel, CUB's exclusive scan of the counts, K13's scatter, then the range call over the batch's
 // sample rows into its rows of out / out_valid.  The range call is given the batch's cell count as its row count: the
@@ -894,7 +863,8 @@ int subquery_run(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int
   const uint32_t Tw_in = (uint32_t)((T_inner + 31) / 32), Tw = (uint32_t)((T + 31) / 32);
   const uint32_t batch_rows = (uint32_t)std::min<uint64_t>(n_rows, std::max<uint64_t>(1, kSqBatchCells / T_inner));
   const uint64_t cells = (uint64_t)batch_rows * T_inner;
-  if (subquery_scratch_pending(c) && (rc = b2p_sync(c))) return rc;
+  // a range call of an earlier batch or call may still be run again from the scratch (it reads its timestamps there)
+  if (pending_reads(c, c->sq_ts) && (rc = b2p_sync(c))) return rc;
   if ((rc = c->sq_ts.ensure(cells * 8)) || (rc = c->sq_val.ensure(cells * 8)) ||
       (rc = c->sq_off.ensure(((size_t)batch_rows + 1) * 8)))
     return rc;
@@ -1032,16 +1002,15 @@ int b2p_host_scan_series(const int64_t* ts, const uint32_t* sid, const uint64_t*
   return rc;
 }
 
-// One chunk, no overlap: H2D -> K0/K2 -> D2H on the context stream.  sid values are global ids
-// (sid_base is subtracted on the device); offsets_host, when given, is already rebased to the chunk.
+// A call small enough for one shot, no overlap: H2D -> K0/K2 -> D2H on the context stream.
 static int range_eval_host_simple(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
-                                  const uint32_t* sid, uint32_t sid_base, const uint64_t* offsets_host, uint64_t n_rows,
-                                  uint32_t n_series, int64_t T, double* out, uint32_t* valid_words) {
+                                  const uint32_t* sid, const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series,
+                                  int64_t T, double* out, uint32_t* valid_words) {
   int rc;
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
   c->last_h2d_bytes = (long long)(n_rows * 16 + (offsets_host ? ((size_t)n_series + 1) * 8 : n_rows * 4));
   Staging s{c};
-  const SeriesIn in = stage_series(s, ts, val, sid, sid_base, offsets_host, n_rows, n_series);
+  const SeriesIn in = stage_series(s, ts, val, sid, 0u, offsets_host, n_rows, n_series);
   double* d_out = s.out(out, (size_t)n_series * (size_t)T * 8);
   uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
   if ((rc = s.rc) || (rc = b2p_range_eval_dev(c, p, in.ts, in.val, in.offsets, n_rows, n_series, d_out, d_valid)) ||
@@ -1059,6 +1028,44 @@ static uint64_t lower_bound_sid(const uint32_t* sid, uint64_t n, uint64_t key) {
   }
   return lo;
 }
+
+}  // extern "C"
+
+namespace {
+// One chunk of b2p_range_eval's pipeline: series [s0, s1), rows [r0, r1) of the host columns.
+struct Chunk {
+  uint32_t s0, s1;
+  uint64_t r0, r1;
+};
+
+// pinned host memory, freed with its owner
+struct FreeHost {
+  void operator()(void* p) const { cudaFreeHost(p); }
+};
+template <class T>
+using Pinned = std::unique_ptr<T[], FreeHost>;
+template <class T>
+int alloc_pinned(Pinned<T>& p, size_t n) {
+  T* raw = nullptr;
+  CU(cudaMallocHost(&raw, n * sizeof(T)));
+  p.reset(raw);
+  return B2P_OK;
+}
+
+// the host scan's worker threads, stopped and joined when their owner goes (before the pinned arrays they fill)
+struct ScanWorkers {
+  std::atomic<bool> stop{false};
+  std::vector<std::thread> threads;
+  void join() {
+    stop.store(true);
+    for (auto& t : threads)
+      if (t.joinable()) t.join();
+  }
+  ~ScanWorkers() { join(); }
+};
+}  // namespace
+
+extern "C" {
 
 int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val, const uint32_t* sid,
                    const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* out,
@@ -1079,7 +1086,7 @@ int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, con
   // ---- small inputs: one shot -------------------------------------------------------------------
   constexpr uint64_t kChunkRows = 4u << 20;  // ~84 MB of H2D per chunk
   if (n_rows <= kChunkRows + kChunkRows / 2 || n_series < 64)
-    return range_eval_host_simple(c, p, ts, val, sid, 0u, offsets_host, n_rows, n_series, T, out, valid_words);
+    return range_eval_host_simple(c, p, ts, val, sid, offsets_host, n_rows, n_series, T, out, valid_words);
 
   // ---- large inputs: series chunks, double-buffered; H2D(i+1) | K0+K2(i) | D2H(i-1) overlap -----------
   const uint64_t avg_rows = n_rows / n_series + 1;
@@ -1098,32 +1105,25 @@ int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, con
     c->pipe_ready = true;
   }
   if ((rc = c->p_status.ensure((size_t)n_chunks * sizeof(Status)))) return rc;  // device copies of each chunk's status
-  Status* h_stat = nullptr;
-  CU(cudaMallocHost(&h_stat, (size_t)n_chunks * sizeof(Status)));
-  uint64_t* h_offs[2] = {nullptr, nullptr};
-  if (offsets_host) {
-    for (int i = 0; i < 2; ++i) CU(cudaMallocHost(&h_offs[i], ((size_t)C + 1) * 8));
-  }
-  struct Cleanup {
-    Status* s; uint64_t* o0; uint64_t* o1;
-    ~Cleanup() { if (s) cudaFreeHost(s); if (o0) cudaFreeHost(o0); if (o1) cudaFreeHost(o1); }
-  } cleanup{h_stat, h_offs[0], h_offs[1]};
+  Pinned<Status> h_stat;
+  Pinned<uint64_t> h_offs[2];
+  if ((rc = alloc_pinned(h_stat, n_chunks))) return rc;
+  for (int i = 0; offsets_host && i < 2; ++i)
+    if ((rc = alloc_pinned(h_offs[i], (size_t)C + 1))) return rc;
 
-  // worst-case chunk row count (chunks are whole series)
+  // the chunk table (chunks are whole series) and the worst-case chunk row count
+  std::vector<Chunk> chunks(n_chunks);
   uint64_t max_rows = 0;
-  std::vector<uint64_t> chunk_row(n_chunks + 1, 0);
-  {
-    uint64_t prev = 0;
-    for (uint32_t i = 0; i < n_chunks; ++i) {
-      const uint64_t s1 = (uint64_t)(i + 1) * C < n_series ? (uint64_t)(i + 1) * C : n_series;
-      const uint64_t r1 = offsets_host ? offsets_host[s1] : lower_bound_sid(sid, n_rows, s1);
-      if (r1 < prev) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");
-      if (r1 - prev > max_rows) max_rows = r1 - prev;
-      prev = r1;
-      chunk_row[i + 1] = r1;
-    }
-    if (!offsets_host && prev != n_rows) return fail(B2P_E_UNSORTED, "series id >= n_series");
+  for (uint32_t i = 0; i < n_chunks; ++i) {
+    Chunk& k = chunks[i];
+    k.s0 = i * C;
+    k.s1 = (uint64_t)k.s0 + C < n_series ? k.s0 + C : n_series;
+    k.r0 = i ? chunks[i - 1].r1 : 0;
+    k.r1 = offsets_host ? offsets_host[k.s1] : lower_bound_sid(sid, n_rows, k.s1);
+    if (k.r1 < k.r0) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");
+    max_rows = std::max(max_rows, k.r1 - k.r0);
   }
+  if (!offsets_host && chunks.back().r1 != n_rows) return fail(B2P_E_UNSORTED, "series id >= n_series");
   // Host scan of every chunk, ahead of the copies (worker k takes chunks k, k + W, ..): 0 = not scanned yet, 1 = every
   // series of the chunk is equally spaced (its rebased offsets, first timestamps and cadences are in the pinned
   // descriptor arrays), 2 = take the ordinary route (ids out of order included: K0 reports those as before)
@@ -1131,49 +1131,38 @@ int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, con
   // handed over the call is already at 16 B/row, and the scan's per-call cost — pinned descriptor arrays, worker
   // threads — costs more than the 8 B/row it saves)
   const bool scan = c->host_ts_scan && !offsets_host;
-  uint64_t* h_doff = nullptr;
-  int64_t *h_t0 = nullptr, *h_cad = nullptr;
+  Pinned<uint64_t> h_doff;
+  Pinned<int64_t> h_t0, h_cad;
   std::unique_ptr<std::atomic<int>[]> scan_state;
-  std::atomic<bool> scan_stop{false};
-  std::vector<std::thread> scan_workers;
-  struct ScanJoin {
-    std::atomic<bool>& stop; std::vector<std::thread>& w; uint64_t*& a; int64_t*& b; int64_t*& d;
-    ~ScanJoin() {
-      stop.store(true);
-      for (auto& t : w) if (t.joinable()) t.join();
-      if (a) cudaFreeHost(a);
-      if (b) cudaFreeHost(b);
-      if (d) cudaFreeHost(d);
-    }
-  } scan_join{scan_stop, scan_workers, h_doff, h_t0, h_cad};
+  ScanWorkers workers;
   if (scan) {
-    CU(cudaMallocHost(&h_doff, ((size_t)n_series + n_chunks) * 8));
-    CU(cudaMallocHost(&h_t0, (size_t)n_series * 8));
-    CU(cudaMallocHost(&h_cad, (size_t)n_series * 8));
+    if ((rc = alloc_pinned(h_doff, (size_t)n_series + n_chunks)) || (rc = alloc_pinned(h_t0, n_series)) ||
+        (rc = alloc_pinned(h_cad, n_series)))
+      return rc;
     scan_state.reset(new std::atomic<int>[n_chunks]);
     for (uint32_t i = 0; i < n_chunks; ++i) scan_state[i].store(0);
     unsigned hw = std::thread::hardware_concurrency();
     unsigned W = hw >= 64 ? 16u : (hw >= 8 ? hw / 4 : 1u);
     if (W > n_chunks) W = n_chunks;
     std::atomic<int>* state = scan_state.get();
-    const uint64_t* rows = chunk_row.data();
+    const Chunk* table = chunks.data();
+    uint64_t* doff = h_doff.get();
+    int64_t *t0 = h_t0.get(), *cad = h_cad.get();
+    std::atomic<bool>& stop = workers.stop;
     try {
-    for (unsigned k = 0; k < W; ++k) {
-      scan_workers.emplace_back([=, &scan_stop]() {
-        for (uint32_t i = k; i < n_chunks && !scan_stop.load(std::memory_order_relaxed); i += W) {
-          const uint32_t s0 = i * C;
-          const uint32_t s1 = (uint64_t)s0 + C < n_series ? s0 + C : n_series;
-          const uint64_t r0 = rows[i], nr = rows[i + 1] - rows[i];
-          int32_t regular = 0;
-          const int rc_scan = host_scan_series(ts + r0, sid ? sid + r0 : nullptr, offsets_host ? offsets_host + s0 : nullptr, nr,
-                                               s1 - s0, s0, h_doff + s0 + i, h_t0 + s0, h_cad + s0, &regular);
-          state[i].store((rc_scan == B2P_OK && regular) ? 1 : 2, std::memory_order_release);
-        }
-      });
-    }
+      for (unsigned w = 0; w < W; ++w) {
+        workers.threads.emplace_back([=, &stop]() {
+          for (uint32_t i = w; i < n_chunks && !stop.load(std::memory_order_relaxed); i += W) {
+            const Chunk& k = table[i];
+            int32_t regular = 0;
+            const int rc_scan = host_scan_series(ts + k.r0, sid + k.r0, nullptr, k.r1 - k.r0, k.s1 - k.s0, k.s0,
+                                                 doff + k.s0 + i, t0 + k.s0, cad + k.s0, &regular);
+            state[i].store((rc_scan == B2P_OK && regular) ? 1 : 2, std::memory_order_release);
+          }
+        });
+      }
     } catch (...) {  // no threads to be had: every chunk the started workers do not reach takes the ordinary route
-      scan_stop.store(true);
-      for (auto& t : scan_workers) if (t.joinable()) t.join();
+      workers.join();
       for (uint32_t i = 0; i < n_chunks; ++i) {
         int zero = 0;
         state[i].compare_exchange_strong(zero, 2);
@@ -1192,36 +1181,35 @@ int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, con
   }
   CU(cudaStreamSynchronize(c->stream));
   c->last_h2d_bytes = 0;
-  uint64_t row_lo = 0;
+  std::vector<b2p_ctx::Pending> recs;  // each chunk's range call, read below with all the others
+  recs.reserve(n_chunks);
   for (uint32_t i = 0; i < n_chunks; ++i) {
     const int b = (int)(i & 1);
-    const uint32_t s0 = i * C;
-    const uint32_t s1 = (uint64_t)s0 + C < n_series ? s0 + C : n_series;
-    const uint32_t ns = s1 - s0;
-    const uint64_t row_hi = offsets_host ? offsets_host[s1] : lower_bound_sid(sid, n_rows, s1);
-    const uint64_t nr = row_hi - row_lo;
+    const Chunk& k = chunks[i];
+    const uint32_t ns = k.s1 - k.s0;
+    const uint64_t nr = k.r1 - k.r0;
     int described = 2;  // 1: the chunk's timestamp (and id) column is described by (offsets, t0, cadence)
     if (scan)
       while ((described = scan_state[i].load(std::memory_order_acquire)) == 0) std::this_thread::yield();
     // H2D of chunk i may start once chunk i-2's kernels no longer read this buffer pair
     if (i >= 2) CU(cudaStreamWaitEvent(c->s_h2d, c->ev_comp[b], 0));
-    CU(cudaMemcpyAsync(c->p_val[b].p, val + row_lo, nr * 8, cudaMemcpyHostToDevice, c->s_h2d));
+    CU(cudaMemcpyAsync(c->p_val[b].p, val + k.r0, nr * 8, cudaMemcpyHostToDevice, c->s_h2d));
     c->last_h2d_bytes += (long long)(nr * 8);
     if (described == 1) {
       c->last_h2d_bytes += (long long)(((size_t)ns + 1) * 8 + (size_t)ns * 16);
-      CU(cudaMemcpyAsync(c->p_off[b].p, h_doff + s0 + i, ((size_t)ns + 1) * 8, cudaMemcpyHostToDevice, c->s_h2d));
-      CU(cudaMemcpyAsync(c->p_t0[b].p, h_t0 + s0, (size_t)ns * 8, cudaMemcpyHostToDevice, c->s_h2d));
-      CU(cudaMemcpyAsync(c->p_cad[b].p, h_cad + s0, (size_t)ns * 8, cudaMemcpyHostToDevice, c->s_h2d));
+      CU(cudaMemcpyAsync(c->p_off[b].p, h_doff.get() + k.s0 + i, ((size_t)ns + 1) * 8, cudaMemcpyHostToDevice, c->s_h2d));
+      CU(cudaMemcpyAsync(c->p_t0[b].p, h_t0.get() + k.s0, (size_t)ns * 8, cudaMemcpyHostToDevice, c->s_h2d));
+      CU(cudaMemcpyAsync(c->p_cad[b].p, h_cad.get() + k.s0, (size_t)ns * 8, cudaMemcpyHostToDevice, c->s_h2d));
     } else {
-    c->last_h2d_bytes += (long long)(nr * 8 + (offsets_host ? ((size_t)ns + 1) * 8 : nr * 4));
-    CU(cudaMemcpyAsync(c->p_ts[b].p, ts + row_lo, nr * 8, cudaMemcpyHostToDevice, c->s_h2d));
-    if (offsets_host) {
-      if (i >= 2) CU(cudaEventSynchronize(c->ev_h2d[b]));  // the pinned rebase buffer is free again
-      for (uint32_t q = 0; q <= ns; ++q) h_offs[b][q] = offsets_host[s0 + q] - row_lo;
-      CU(cudaMemcpyAsync(c->p_off[b].p, h_offs[b], ((size_t)ns + 1) * 8, cudaMemcpyHostToDevice, c->s_h2d));
-    } else {
-      CU(cudaMemcpyAsync(c->p_sid[b].p, sid + row_lo, nr * 4, cudaMemcpyHostToDevice, c->s_h2d));
-    }
+      c->last_h2d_bytes += (long long)(nr * 8 + (offsets_host ? ((size_t)ns + 1) * 8 : nr * 4));
+      CU(cudaMemcpyAsync(c->p_ts[b].p, ts + k.r0, nr * 8, cudaMemcpyHostToDevice, c->s_h2d));
+      if (offsets_host) {
+        if (i >= 2) CU(cudaEventSynchronize(c->ev_h2d[b]));  // the pinned rebase buffer is free again
+        for (uint32_t q = 0; q <= ns; ++q) h_offs[b][q] = offsets_host[k.s0 + q] - k.r0;
+        CU(cudaMemcpyAsync(c->p_off[b].p, h_offs[b].get(), ((size_t)ns + 1) * 8, cudaMemcpyHostToDevice, c->s_h2d));
+      } else {
+        CU(cudaMemcpyAsync(c->p_sid[b].p, sid + k.r0, nr * 4, cudaMemcpyHostToDevice, c->s_h2d));
+      }
     }
     CU(cudaEventRecord(c->ev_h2d[b], c->s_h2d));
     // compute: after its inputs landed and after chunk i-2's results left the output buffers
@@ -1233,63 +1221,50 @@ int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, con
       c->launches++;
       CU(cudaGetLastError());
     } else if (!offsets_host &&
-        (rc = series_offsets_impl(c, c->p_sid[b].as<uint32_t>(), nr, ns, s0, c->p_off[b].as<uint64_t>())))
+               (rc = series_offsets_impl(c, c->p_sid[b].as<uint32_t>(), nr, ns, k.s0, c->p_off[b].as<uint64_t>()))) {
       return rc;
+    }
     if ((rc = b2p_range_eval_dev(c, p, c->p_ts[b].as<int64_t>(), c->p_val[b].as<double>(), c->p_off[b].as<uint64_t>(),
                                  nr, ns, c->p_out[b].as<double>(), c->p_valid[b].as<uint32_t>())))
       return rc;
-    {  // this chunk's verdict is read with all the others below: take the call out of the pending queue
-      const int slot = c->pending.back().slot;
-      c->pending.pop_back();
-      CU(cudaMemcpyAsync(c->p_status.as<Status>() + i, c->d_ring + slot, sizeof(Status), cudaMemcpyDeviceToDevice, c->stream));
-    }
+    // the chunk's call leaves the pending queue: its Status is copied aside, its buffer pair reused
+    recs.push_back(c->pending.back());
+    c->pending.pop_back();
+    CU(cudaMemcpyAsync(c->p_status.as<Status>() + i, c->d_ring + recs.back().slot, sizeof(Status),
+                       cudaMemcpyDeviceToDevice, c->stream));
     CU(cudaEventRecord(c->ev_comp[b], c->stream));
     // D2H
     CU(cudaStreamWaitEvent(c->s_d2h, c->ev_comp[b], 0));
-    CU(cudaMemcpyAsync(out + (size_t)s0 * (size_t)T, c->p_out[b].p, (size_t)ns * (size_t)T * 8, cudaMemcpyDeviceToHost,
+    CU(cudaMemcpyAsync(out + (size_t)k.s0 * (size_t)T, c->p_out[b].p, (size_t)ns * (size_t)T * 8, cudaMemcpyDeviceToHost,
                        c->s_d2h));
-    CU(cudaMemcpyAsync(valid_words + (size_t)s0 * Tw, c->p_valid[b].p, (size_t)ns * Tw * 4, cudaMemcpyDeviceToHost,
+    CU(cudaMemcpyAsync(valid_words + (size_t)k.s0 * Tw, c->p_valid[b].p, (size_t)ns * Tw * 4, cudaMemcpyDeviceToHost,
                        c->s_d2h));
     CU(cudaEventRecord(c->ev_d2h[b], c->s_d2h));
-    row_lo = row_hi;
   }
-  CU(cudaMemcpyAsync(h_stat, c->p_status.p, (size_t)n_chunks * sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(c->h_k0, c->d_k0, sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
+  CU(cudaMemcpyAsync(h_stat.get(), c->p_status.p, (size_t)n_chunks * sizeof(Status), cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->s_d2h));
-  if (const uint32_t k0 = c->h_k0->k0_errors) {
-    CU(cudaMemsetAsync(c->d_k0, 0, sizeof(Status), c->stream));
-    return k0_fail(k0);
+  if ((rc = take_k0(c))) return rc;
+  // one verdict over all chunks; a chunk whose slow path ran out of arena is redone alone, with its own tiers, from
+  // its host columns (its device buffers have been reused)
+  const size_t need = read_outcome(c, recs.data(), h_stat.get(), n_chunks, false);
+  for (uint32_t i = 0; need && i < n_chunks; ++i) {
+    if (!redo_rows(h_stat[i])) continue;
+    const Chunk& k = chunks[i];
+    const uint32_t ns = k.s1 - k.s0;
+    const uint64_t nr = k.r1 - k.r0;
+    std::vector<uint64_t> offs;
+    if (offsets_host)
+      for (uint32_t q = 0; q <= ns; ++q) offs.push_back(offsets_host[k.s0 + q] - k.r0);
+    c->last_h2d_bytes += (long long)(nr * 16 + (offsets_host ? ((size_t)ns + 1) * 8 : nr * 4));
+    Staging s{c};
+    const SeriesIn in = stage_series(s, ts + k.r0, val + k.r0, sid ? sid + k.r0 : nullptr, k.s0,
+                                     offsets_host ? offs.data() : nullptr, nr, ns);
+    b2p_ctx::Pending redo = recs[i];
+    redo.args.ts = in.ts; redo.args.val = in.val; redo.args.offsets = in.offsets;
+    redo.args.out = s.out(out + (size_t)k.s0 * (size_t)T, (size_t)ns * (size_t)T * 8);
+    redo.args.valid = s.out(valid_words + (size_t)k.s0 * Tw, (size_t)ns * Tw * 4);
+    if ((rc = s.end([&] { return redo_calls(c, {redo}, need); }))) return rc;
   }
-  // per-chunk verdicts; a chunk whose slow path ran out of arena is redone alone (b2p_sync grows the arena)
-  long long slow_total = 0, w_total = 0;
-  row_lo = 0;
-  for (uint32_t i = 0; i < n_chunks; ++i) {
-    const uint32_t s0 = i * C;
-    const uint32_t s1 = (uint64_t)s0 + C < n_series ? s0 + C : n_series;
-    const uint64_t row_hi = offsets_host ? offsets_host[s1] : lower_bound_sid(sid, n_rows, s1);
-    const Status st = h_stat[i];
-    slow_total += st.slow_count;
-    w_total += st.w_count;
-    if (st.arena_overflow) {
-      std::string tmp_offs;
-      const uint64_t* offs_chunk = nullptr;
-      if (offsets_host) {
-        tmp_offs.resize(((size_t)(s1 - s0) + 1) * 8);
-        uint64_t* o = reinterpret_cast<uint64_t*>(&tmp_offs[0]);
-        for (uint32_t q = 0; q <= s1 - s0; ++q) o[q] = offsets_host[s0 + q] - row_lo;
-        offs_chunk = o;
-      }
-      if ((rc = range_eval_host_simple(c, p, ts + row_lo, val + row_lo, sid ? sid + row_lo : nullptr, s0, offs_chunk,
-                                       row_hi - row_lo, s1 - s0, T, out + (size_t)s0 * (size_t)T,
-                                       valid_words + (size_t)s0 * Tw)))
-        return rc;
-    }
-    row_lo = row_hi;
-  }
-  c->last_slow = slow_total;
-  c->last_w = w_total;
-  if (c->last_used_lean) lean_verdict(c, p->fn_id, (uint64_t)w_total, n_series);
   return B2P_OK;
 }
 
@@ -1315,23 +1290,47 @@ int b2p_instant_select(b2p_ctx* c, int64_t start, int64_t end, int64_t interval,
                        const int64_t* ts, const double* val, const uint32_t* sid, const uint64_t* offsets_host,
                        uint64_t n_rows, uint32_t n_series, double* out, uint32_t* valid_words) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  b2p_range_params p{};
-  p.start = start; p.end = end; p.interval = interval; p.range = lookback;
-  int64_t T = 0;
-  if (int rc = check_grid(&p, n_series, &T)) return rc;
-  if (n_series == 0 || T == 0) return B2P_OK;  // (no sample copies, no series offsets)
+  InstantArgs grid;
+  if (int rc = instant_grid(start, end, interval, lookback, offset, n_series, &grid)) return rc;
+  if (n_series == 0 || grid.T == 0) return B2P_OK;  // (no sample copies, no series offsets)
   DeviceGuard g(c->device);
-  const uint32_t Tw = (uint32_t)((T + 31) / 32);
   Staging s{c};
   const SeriesIn in = stage_series(s, ts, val, sid, 0u, offsets_host, n_rows, n_series);
-  double* d_out = s.out(out, (size_t)n_series * (size_t)T * 8);
-  uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
+  double* d_out = s.out(out, (size_t)n_series * (size_t)grid.T * 8);
+  uint32_t* d_valid = s.out(valid_words, (size_t)n_series * grid.Tw * 4);
   return s.end([&] {
     const int rc = b2p_instant_select_dev(c, start, end, interval, lookback, offset, in.ts, in.val, in.offsets, n_rows,
                                           n_series, d_out, d_valid);
     return rc ? rc : b2p_sync(c);
   });
 }
+
+}  // extern "C"
+
+namespace {
+// The device copies of a multi-field host call over a [n_series x T] grid: the timestamps and series offsets, the value
+// columns, their NULL bitmaps (none when field_valid is NULL), the result grids and the validity bitmap.
+struct FieldsIn {
+  SeriesIn series;
+  const double* vals[kMaxFields];
+  const uint8_t* nulls[kMaxFields] = {};
+  double* outs[kMaxFields];
+  uint32_t* valid;
+};
+FieldsIn stage_fields(Staging& s, const int64_t* ts, const double* const* vals, const uint8_t* const* field_valid,
+                      int32_t n_fields, const uint32_t* sid, const uint64_t* offsets_host, uint64_t n_rows,
+                      uint32_t n_series, int64_t T, double* const* outs, uint32_t* valid_words) {
+  FieldsIn f;
+  f.series = stage_series(s, ts, nullptr, sid, 0u, offsets_host, n_rows, n_series);
+  s.in_cols(vals, n_fields, n_rows * 8, f.vals);
+  if (field_valid) s.in_cols(field_valid, n_fields, (n_rows + 7) / 8, f.nulls);
+  s.out_cols(outs, n_fields, (size_t)n_series * (size_t)T * 8, f.outs);
+  f.valid = s.out(valid_words, (size_t)n_series * (size_t)((T + 31) / 32) * 4);
+  return f;
+}
+}  // namespace
+
+extern "C" {
 
 int b2p_range_eval_fields(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* const* vals,
                           const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid,
@@ -1342,19 +1341,12 @@ int b2p_range_eval_fields(b2p_ctx* c, const b2p_range_params* p, const int64_t* 
   if (int rc = check_fields(vals, outs, n_fields)) return rc;
   if (n_series == 0 || T == 0) return B2P_OK;  // (no sample copies, no series offsets)
   DeviceGuard g(c->device);
-  const uint32_t Tw = (uint32_t)((T + 31) / 32);
   Staging s{c};
-  const SeriesIn in = stage_series(s, ts, nullptr, sid, 0u, offsets_host, n_rows, n_series);
-  const double* d_vals[kMaxFields];
-  double* d_outs[kMaxFields];
-  s.in_cols(vals, n_fields, n_rows * 8, d_vals);
-  const uint8_t* d_nulls[kMaxFields] = {};
-  if (field_valid) s.in_cols(field_valid, n_fields, (n_rows + 7) / 8, d_nulls);
-  s.out_cols(outs, n_fields, (size_t)n_series * (size_t)T * 8, d_outs);
-  uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
+  const FieldsIn f =
+      stage_fields(s, ts, vals, field_valid, n_fields, sid, offsets_host, n_rows, n_series, T, outs, valid_words);
   return s.end([&] {
-    const int rc = b2p_range_eval_fields_dev(c, p, in.ts, d_vals, field_valid ? d_nulls : nullptr, n_fields, in.offsets,
-                                             n_rows, n_series, d_outs, d_valid);
+    const int rc = b2p_range_eval_fields_dev(c, p, f.series.ts, f.vals, field_valid ? f.nulls : nullptr, n_fields,
+                                             f.series.offsets, n_rows, n_series, f.outs, f.valid);
     return rc ? rc : b2p_sync(c);
   });
 }
@@ -1364,27 +1356,18 @@ int b2p_instant_select_fields(b2p_ctx* c, int64_t start, int64_t end, int64_t in
                               const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid,
                               const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  b2p_range_params p{};
-  p.start = start; p.end = end; p.interval = interval; p.range = lookback;
-  int64_t T = 0;
-  if (int rc = check_grid(&p, n_series, &T)) return rc;
+  InstantArgs grid;
+  if (int rc = instant_grid(start, end, interval, lookback, offset, n_series, &grid)) return rc;
   if (int rc = check_fields(vals, outs, n_fields)) return rc;
-  if (n_series == 0 || T == 0) return B2P_OK;  // (no sample copies, no series offsets)
+  if (n_series == 0 || grid.T == 0) return B2P_OK;  // (no sample copies, no series offsets)
   DeviceGuard g(c->device);
-  const uint32_t Tw = (uint32_t)((T + 31) / 32);
   Staging s{c};
-  const SeriesIn in = stage_series(s, ts, nullptr, sid, 0u, offsets_host, n_rows, n_series);
-  const double* d_vals[kMaxFields];
-  double* d_outs[kMaxFields];
-  s.in_cols(vals, n_fields, n_rows * 8, d_vals);
-  const uint8_t* d_nulls[kMaxFields] = {};
-  if (field_valid) s.in_cols(field_valid, n_fields, (n_rows + 7) / 8, d_nulls);
-  s.out_cols(outs, n_fields, (size_t)n_series * (size_t)T * 8, d_outs);
-  uint32_t* d_valid = s.out(valid_words, (size_t)n_series * Tw * 4);
+  const FieldsIn f =
+      stage_fields(s, ts, vals, field_valid, n_fields, sid, offsets_host, n_rows, n_series, grid.T, outs, valid_words);
   return s.end([&] {
-    const int rc = b2p_instant_select_fields_dev(c, start, end, interval, lookback, offset, in.ts, d_vals,
-                                                 field_valid ? d_nulls : nullptr, n_fields,
-                                                 in.offsets, n_rows, n_series, d_outs, d_valid);
+    const int rc = b2p_instant_select_fields_dev(c, start, end, interval, lookback, offset, f.series.ts, f.vals,
+                                                 field_valid ? f.nulls : nullptr, n_fields, f.series.offsets, n_rows,
+                                                 n_series, f.outs, f.valid);
     return rc ? rc : b2p_sync(c);
   });
 }

@@ -140,10 +140,27 @@ struct b2p_ctx {
   b2p::Status* d_k0 = nullptr;
   b2p::Status* h_k0 = nullptr;    // pinned
   int next_slot = 0;
+  // The tiers a range call starts with: the thread tier (K2T), or the first tier (K2L) in `lean_mode` (0 plain, 1 with
+  // reset bit words; 2: the adaptive back-off skips it), and then the warp-per-series and slow tiers.
+  struct Tiers {
+    bool thread_tier = false;
+    bool first_tier = false;
+    int lean_mode = 0;
+  };
+  // The record of an admitted range call, until b2p_sync (or the host pipeline) has read its Status: enough to take its
+  // verdict and to run it again.
   struct Pending {
-    int slot; int fn; b2p::RangeArgs args; int lean_mode; bool thread_tier; bool used_lean; uint32_t n_series; bool verdict_taken;
-    bool fused;  // by-label partials were added in place: only the slow kernel may be repeated
-    bool merged; // ... and already all-reduced (or tiled): nothing can be repeated, an arena overflow is an error
+    enum Kind {
+      kPlain,
+      kFused,   // by-label partials were added in place: only the slow kernel may be repeated
+      kMerged,  // ... and already all-reduced (or tiled): nothing can be repeated, an arena overflow is an error
+    };
+    int slot;
+    int fn;
+    b2p::RangeArgs args;  // as admitted (use_w_list = 0)
+    Tiers tiers;
+    uint32_t n_series;
+    Kind kind;
   };
   std::vector<Pending> pending;
   DevBuf slow_list, w_list, b_list, arena_ts, arena_val, win_scratch;
@@ -173,10 +190,6 @@ struct b2p_ctx {
   // series on); 2 = skip K2L.  `lean_backoff` counts the calls a non-zero mode still lasts.
   int lean_mode[B2P_FN__COUNT] = {};
   int lean_backoff[B2P_FN__COUNT] = {};
-  int last_lean_mode = 0;
-  int last_range_fn = 0;
-  bool last_used_lean = false;  // the pending / last range call started with K2L
-  uint32_t last_range_series = 0;
   // first-tier variant for equally spaced samples (rate / increase / delta): -1 = cadence_probe_kernel decides per call
   // on the device, 0 / 1 = forced (B2P_UNIFORM)
   int uniform_mode = -1;
@@ -245,11 +258,12 @@ struct DeviceGuard {
   }
 };
 
-inline void stage_begin(b2p_ctx* c, int stage) {
-  cudaEventRecord(c->ev[stage][0], c->stream);
+// the CUDA events around a stage's kernels, on `s` (default: the context's stream)
+inline void stage_begin(b2p_ctx* c, int stage, cudaStream_t s = nullptr) {
+  cudaEventRecord(c->ev[stage][0], s ? s : c->stream);
 }
-inline void stage_end(b2p_ctx* c, int stage) {
-  cudaEventRecord(c->ev[stage][1], c->stream);
+inline void stage_end(b2p_ctx* c, int stage, cudaStream_t s = nullptr) {
+  cudaEventRecord(c->ev[stage][1], s ? s : c->stream);
   c->ev_used[stage] = true;
 }
 
