@@ -238,6 +238,11 @@ int upload_rcp_table() {
 extern "C" {
 
 __global__ void comm_marker_kernel() {}
+// a tiled call's counters before the next tile resets them: what b2p_last_*_series and the adaptive verdict read
+__global__ void tile_counts_kernel(Status* st) {
+  st->slow_tiles += st->slow_count;
+  st->w_tiles += st->w_count;
+}
 // holds the compute stream back for a few microseconds so that the all-reduce released at the same instant on the
 // communication stream has its CTAs placed before the persistent range kernel asks for every SM
 __global__ void comm_headstart_kernel(long long cycles) {
@@ -253,6 +258,9 @@ static int launch_range_tiers(b2p_ctx* c, const b2p_ctx::Pending& pc, bool later
   if (!later_tile) {
     CU(cudaMemsetAsync(a.status, 0, sizeof(Status), c->stream));
   } else {  // a further tile of the same fused call: new work lists, same verdict (overflow / arena fields stay)
+    tile_counts_kernel<<<1, 1, 0, c->stream>>>(a.status);
+    c->launches++;
+    CU(cudaGetLastError());
     CU(cudaMemsetAsync(&a.status->slow_count, 0, sizeof(uint32_t), c->stream));
     CU(cudaMemsetAsync(&a.status->w_count, 0, 3 * sizeof(uint32_t), c->stream));  // w_count, b_count, g_next
   }
@@ -296,16 +304,16 @@ static int take_k0(b2p_ctx* c) {
 static size_t redo_rows(const Status& st) { return st.arena_overflow ? (size_t)st.arena_needed + 1024 : 0; }
 
 // The outcome of one range call from the Status of each of its `n` records (one; or one per chunk of a host call):
-// the hand-off counters (summed over the records) and the adaptive verdict, taken over all of them with the tiers of
-// the last — unless `redo`: a redo is not a new call.  Returns the arena rows the largest record that ran out of
-// arena needs (0: every one fit).
+// the hand-off counters (summed over the records, and over the tiles of a tiled call) and the adaptive verdict, taken
+// over all of them with the tiers of the last — unless `redo`: a redo is not a new call.  Returns the arena rows the
+// largest record that ran out of arena needs (0: every one fit).
 static size_t read_outcome(b2p_ctx* c, const b2p_ctx::Pending* recs, const Status* st, size_t n, bool redo) {
   size_t need = 0;
   long long slow = 0, handed = 0;
   uint64_t series = 0;
   for (size_t i = 0; i < n; ++i) {
-    slow += st[i].slow_count;
-    handed += st[i].w_count;
+    slow += (long long)st[i].slow_tiles + st[i].slow_count;
+    handed += (long long)st[i].w_tiles + st[i].w_count;
     series += recs[i].n_series;
     need = std::max(need, redo_rows(st[i]));
   }
@@ -435,12 +443,14 @@ static int launch_allreduce_tiles(b2p_ctx* c, const b2p_ctx::Pending& pc, uint32
   const RangeArgs& a = pc.args;
   const uint64_t span = (uint64_t)a.g_hi - a.g_lo;
   c->comm_reserve_now = (c->comm && n_tiles > 1) ? c->comm_reserve_sms : 0;
+  bool launched = false;  // (with more tiles than groups the first tiles are empty: the first one run resets Status)
   for (uint32_t t = 0; t < n_tiles; ++t) {
     b2p_ctx::Pending tile = pc;
     tile.args.g_lo = a.g_lo + (uint32_t)(span * t / n_tiles);
     tile.args.g_hi = a.g_lo + (uint32_t)(span * (t + 1) / n_tiles);
     if (tile.args.g_hi == tile.args.g_lo) continue;
-    if (int rc = launch_range_tiers(c, tile, t > 0)) return rc;
+    if (int rc = launch_range_tiers(c, tile, launched)) return rc;
+    launched = true;
     if (c->comm) {
       const size_t off = (size_t)tile.args.g_lo * (size_t)a.T, cnt_n = (size_t)(tile.args.g_hi - tile.args.g_lo) * (size_t)a.T;
       CU(cudaEventRecord(c->ev_comm_in, c->stream));

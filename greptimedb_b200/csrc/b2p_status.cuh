@@ -16,6 +16,9 @@ struct Status {
   uint32_t uniform;         // cadence_probe_kernel's verdict: != 0 => the uniform-cadence variant of the first tier runs
   unsigned long long arena_used;    // (unused since the arena is split into per-warp regions)
   unsigned long long arena_needed;  // arena rows that make a region large enough for the longest deferred series
+  // a tiled call (all-reduced sum by) resets slow_count / w_count per tile: the counts of its earlier tiles
+  uint32_t slow_tiles;
+  uint32_t w_tiles;
 };
 
 // Status::k0_errors bits of the operators above the range functions

@@ -180,13 +180,14 @@ B2P_API int b2p_use_own_stream(b2p_ctx* ctx);
 /* Wait for the stream, finish slow-path fix-ups, surface deferred errors (B2P_E_UNSORTED, ...). */
 B2P_API int b2p_sync(b2p_ctx* ctx);
 B2P_API int64_t b2p_num_steps(int64_t start, int64_t end, int64_t interval);
-/* Series the last range/instant call routed to the exact slow path (diagnostic; after b2p_sync). */
+/* Series the last range/instant call routed to the exact slow path, summed over the chunks of a chunked b2p_range_eval
+ * and over the tiles of a tiled call (diagnostic; after b2p_sync). */
 B2P_API int64_t b2p_last_slow_series(b2p_ctx* ctx);
 /* bytes the last b2p_range_eval (host-pointer call) copied host -> device: fewer than 20 B/row when chunks of equally
  * spaced series went over as (offsets, first timestamp, cadence) descriptors instead of their timestamp / id columns */
 B2P_API int64_t b2p_last_h2d_bytes(b2p_ctx* ctx);
 /* Series the first tier (or the opt-in thread tier) handed to the warp-per-series kernel in the last range call,
- * summed over the chunks of a chunked b2p_range_eval (diagnostic; after b2p_sync). */
+ * summed over the chunks of a chunked b2p_range_eval and over the tiles of a tiled call (diagnostic; after b2p_sync). */
 B2P_API int64_t b2p_last_warp_tier_series(b2p_ctx* ctx);
 /* CUDA-event time (ms) of the kernels of the last *_dev / host call, by stage index:
  * 0 = series_offsets, 1 = range/instant fast kernel, 2 = slow-path kernel, 3 = aggregate /

@@ -5,9 +5,10 @@ What is compared: validity bitmaps bit for bit everywhere, and null slots hold 0
 big-ring, long-window, outstanding-call and fuzz tests compare every value with the oracle's *rescan* restatement
 (orc.range_query(..., rescan=True)) bit for bit (the library is compiled with -fmad=false and uses IEEE div/sqrt); a
 NaN only has to be a NaN there.  Where the comparison is with the reference's *sliding* restatement (the thread tier's
-arms, and the tests that predate the rescan grid: lean hand-off, uniform cadence, pipelined host path, fused sum by,
-bench shape) rate / increase / delta values are held to 1e-9 relative, because the two reference code paths differ in
-the last ulps (extrapolate_rate.rs:216-238), and the functions in BIT_EXACT bit for bit.  tests/test_gpu_range_tiers.py
+arms, and the tests that predate the rescan grid: lean hand-off, uniform cadence, pipelined host path, bench shape)
+rate / increase / delta values are held to 1e-9 relative, because the two reference code paths differ in the last ulps
+(extrapolate_rate.rs:216-238), and the functions in BIT_EXACT bit for bit.  The fused sum by tests hold group sums of
+the rescan grid to the error bound of recursive summation (tests/sum_by_check.py).  tests/test_gpu_range_tiers.py
 holds every tier to the rescan oracle on special values and at the kernels' window-length boundaries.
 """
 import math
@@ -16,6 +17,7 @@ import numpy as np
 import pytest
 
 from oracle import oracle as orc
+from tests import sum_by_check as sbc
 from tests.helpers import (check_expected, farr, fnum, load_sqlness, load_unit, pack_series, promql_series,
                            udf_case_inputs)
 
@@ -878,15 +880,6 @@ def _sum_by_case(S, N, G, resets, nan_every, seed, gid_mode="hash", jitter=1000)
     return T0, ts, val, sid, offsets, gid
 
 
-def _assert_finite_sums_close(got, exp, cnt, what):
-    """1e-9 relative wherever the group is present and both sums are finite; there must be such entries"""
-    both = (cnt > 0) & np.isfinite(got) & np.isfinite(exp)
-    assert both.any(), f"{what}: no finite group sum to compare"
-    with np.errstate(over="ignore"):
-        rel = np.abs(got[both] - exp[both]) / np.maximum(np.abs(exp[both]), 1e-300)
-    assert rel.max() <= 1e-9, f"{what}: max relative difference {rel.max()}"
-
-
 def _sum_by_values(val, values):
     """Special value classes for the fused sum by: "inf" sprinkles +-inf over the samples, "huge" scales the counters so
     that the largest sample is close to f64::MAX (rates near 1e305, group sums that overflow)."""
@@ -914,9 +907,9 @@ def test_fused_sum_by_matches_oracle_and_two_pass(ctx, ctx_lean_flags, fn, reset
     group by group, series it hands on (counter resets on the plain variant, NaN samples) are added by the later tiers
     from the step where the first tier stopped.  Checked against the two-pass composition on the same context (range
     eval into [S x T], then the by-label kernel's sum): counts bit for bit, and sums bit for bit where no series leaves
-    the first tier (series handed on are added after the first tier's, a different order: 1e-9 relative then); and
-    against the oracle's rescan rate + group aggregate: counts bit-exact, finite sums to 1e-9, and with +-inf samples
-    the same non-finite entries."""
+    the first tier (series handed on are added after the first tier's, a different order: both within the bound then); and
+    against the oracle's rescan rate + group aggregate: counts bit-exact, sums within the error bound of recursive
+    summation (tests/sum_by_check.py), and with +-inf samples the same non-finite entries."""
     import torch
     from greptimedb_b200 import make_params
     dev = torch.device("cuda:0")
@@ -929,6 +922,7 @@ def test_fused_sum_by_matches_oracle_and_two_pass(ctx, ctx_lean_flags, fn, reset
     op = orc.make_params(fn, T0, T0 + (N - 1) * 15_000, 15_000, 300_000)
     e_out, e_valid = orc.range_query(op, ts, val, sid, offsets, threads=8, rescan=True)
     e_sum, e_cnt = orc.group_aggregate("sum", e_out, e_valid, gid, G)
+    ref = sbc.reference(e_out, e_valid, gid, G)
     d_ts, d_val = torch.from_numpy(ts).to(dev), torch.from_numpy(val).to(dev)
     d_off = torch.from_numpy(offsets.astype(np.int64)).to(dev)
     d_gid = torch.from_numpy(gid.astype(np.int32)).to(dev)
@@ -947,7 +941,7 @@ def test_fused_sum_by_matches_oracle_and_two_pass(ctx, ctx_lean_flags, fn, reset
             got = gsum.cpu().numpy().reshape(G, T)
             cnt = gcnt.cpu().numpy().view(np.uint32).reshape(G, T)
             assert (cnt == e_cnt).all(), f"counts differ at {np.argwhere(cnt != e_cnt)[:4].tolist()}"
-            _assert_finite_sums_close(got, e_sum, cnt, "fused vs oracle")
+            sbc.check(ref, got, cnt, "bound", "fused vs oracle")
             if not (values == "huge" and fn == "delta"):
                 # (delta's signed rates near f64::MAX make partial sums overflow, and whether one does depends on the
                 # order of the addends; rate / increase rates are positive and their group sums stay finite)
@@ -965,7 +959,7 @@ def test_fused_sum_by_matches_oracle_and_two_pass(ctx, ctx_lean_flags, fn, reset
                 assert not diff.size, (f"fused sum by differs from range eval + sum at {diff[:4].tolist()}: "
                                        f"{got[tuple(diff[0])]} vs {t_sum[tuple(diff[0])]}")
             else:
-                _assert_finite_sums_close(got, t_sum, cnt, "fused vs two-pass")
+                sbc.check_pair((got, cnt), (t_sum, t_cnt), ref, "fused vs two-pass")
         finally:
             c.group_index_destroy(ix)
 
@@ -994,13 +988,10 @@ def test_fused_sum_by_falls_back_on_unbalanced_groups_and_other_functions(ctx):
             ctx.range_group_sum_indexed_dev(p, d_ts, d_val, d_off, S * N, S, ix, 0, G, gsum, gcnt)
             ctx.sync()
             op = orc.make_params(fn, T0, T0 + (N - 1) * 15_000, 15_000, 300_000)
-            e_out, e_valid = orc.range_query(op, ts, val, sid, offsets, threads=8)
-            e_sum, e_cnt = orc.group_aggregate("sum", e_out, e_valid, gid, G)
+            e_out, e_valid = orc.range_query(op, ts, val, sid, offsets, threads=8, rescan=True)
             got = gsum.cpu().numpy().reshape(G, T)
             cnt = gcnt.cpu().numpy().view(np.uint32).reshape(G, T)
-            assert (cnt == e_cnt).all()
-            rel = np.abs(got - e_sum) / np.maximum(np.abs(e_sum), 1e-300)
-            assert rel[e_cnt > 0].max() <= 1e-9
+            sbc.check(sbc.reference(e_out, e_valid, gid, G), got, cnt, "bound", f"{fn} two-pass fallback")
     finally:
         ctx.group_index_destroy(ix)
 
@@ -1031,13 +1022,10 @@ def test_fused_sum_by_long_windows_and_quirk_series_add_exactly_once(ctx):
             ctx.range_group_sum_indexed_dev(p, d_ts, d_val, d_off, S * N, S, ix, 0, G, gsum, gcnt)
             ctx.sync()
             op = orc.make_params("rate", T0, T0 + (N - 1) * 15_000, step, rng)
-            e_out, e_valid = orc.range_query(op, ts, val, sid, offsets, threads=8)
-            e_sum, e_cnt = orc.group_aggregate("sum", e_out, e_valid, gid, G)
+            e_out, e_valid = orc.range_query(op, ts, val, sid, offsets, threads=8, rescan=True)
             got = gsum.cpu().numpy().reshape(G, T)
             cnt = gcnt.cpu().numpy().view(np.uint32).reshape(G, T)
-            assert (cnt == e_cnt).all(), (rng, np.argwhere(cnt != e_cnt)[:4].tolist())
-            rel = np.abs(got - e_sum) / np.maximum(np.abs(e_sum), 1e-300)
-            assert rel[e_cnt > 0].max() <= 1e-9
+            sbc.check(sbc.reference(e_out, e_valid, gid, G), got, cnt, "bound", f"range {rng}")
     finally:
         ctx.group_index_destroy(ix)
 
