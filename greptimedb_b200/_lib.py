@@ -37,6 +37,7 @@ EXPORTED_SYMBOLS = [
     "b2p_sort_cells_dev", "b2p_sort_cells", "b2p_plan_sort_create",
     "b2p_absent_dev", "b2p_absent", "b2p_plan_absent_create",
     "b2p_range_eval_fields_dev", "b2p_instant_select_fields_dev", "b2p_range_eval_fields", "b2p_instant_select_fields",
+    "b2p_plan_range_create_fields", "b2p_sort_cells_fields_dev", "b2p_sort_cells_fields",
 ]
 
 
@@ -158,6 +159,10 @@ def load() -> C.CDLL:
         "b2p_instant_select_fields_dev": (C.c_int, [vp, i64, i64, i64, i64, i64, vp, vp, vp, i32, vp, u64, u32, vp, vp]),
         "b2p_range_eval_fields": (C.c_int, [vp, P, vp, vp, vp, i32, vp, vp, u64, u32, vp, vp]),
         "b2p_instant_select_fields": (C.c_int, [vp, i64, i64, i64, i64, i64, vp, vp, vp, i32, vp, vp, u64, u32, vp, vp]),
+        "b2p_plan_range_create_fields": (vp, [vp, C.c_char_p, P, C.c_char_p, C.POINTER(C.c_char_p), i32,
+                                              C.POINTER(C.c_char_p), i32, C.c_char_p, C.POINTER(C.c_char_p), i32]),
+        "b2p_sort_cells_fields_dev": (C.c_int, [vp, i32, vp, i32, vp, u32, u64, vp, vp]),
+        "b2p_sort_cells_fields": (C.c_int, [vp, i32, vp, i32, vp, u32, u64, vp, vp]),
         "b2p_plan_set_function": (C.c_int, [vp, C.c_char_p, C.POINTER(dbl), i32]),
         "b2p_plan_scalar_create": (vp, [vp, vp]),
     }

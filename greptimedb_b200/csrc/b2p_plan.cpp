@@ -289,33 +289,38 @@ Groups group_rows(const Labels& in, const std::vector<int>& cols, uint32_t rows)
 // Aggregators beyond enum b2p_agg that the aggregate node offers
 constexpr int kAggGroup = B2P_AGG_STDVAR + 1, kAggQuantile = B2P_AGG_STDVAR + 2;
 
-// The by-label aggregate of r's [rows x T] grid (the leaf's aggregate stage and AggregatePlan): r's rows grouped by
+// The by-label aggregate of r's [rows x T] grids (the leaf's aggregate stage and AggregatePlan): r's rows grouped by
 // their tuple over `cols` (of r.labels), folded on the device in row order, become one row per group in label order,
 // a group having a cell at step k iff one of its rows has.  op: enum b2p_agg, kAggGroup (1.0 wherever count is
-// non-zero) or kAggQuantile (param = φ).  Sets the rows, labels, grid and column layout; keeps T and the time index.
+// non-zero) or kAggQuantile (param = φ).  Each field is folded by its own call over the same group ids; the counts
+// depend on the shared validity alone, so field 0's decide the cells.  Sets the rows, labels, grids and column layout;
+// keeps T, the fields and the time index.
 void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& cols, NodeResult& r) {
   Groups groups = group_rows(r.labels, cols, r.rows);
-  const uint32_t G = (uint32_t)groups.rank.size(), Tw = r.Tw;
+  const uint32_t G = (uint32_t)groups.rank.size(), Tw = r.Tw, F = r.F;
   const size_t T = (size_t)r.T;
-  std::vector<double> gval((size_t)G * T);
-  std::vector<uint32_t> gcnt((size_t)G * T);
-  if (G > 0 && T > 0)
-    check(op == kAggQuantile ? b2p_group_quantile(ctx, param, r.val.data(), r.valid.data(), groups.id.data(), r.rows, G,
-                                                  (uint64_t)T, gval.data(), gcnt.data())
-                             : b2p_group_aggregate(ctx, op == kAggGroup ? B2P_AGG_COUNT : op, r.val.data(),
-                                                   r.valid.data(), groups.id.data(), r.rows, G, (uint64_t)T,
-                                                   gval.data(), gcnt.data()),
+  std::vector<double> gval((size_t)F * G * T);
+  std::vector<uint32_t> gcnt((size_t)G * T), fcnt(F > 1 ? (size_t)G * T : 0);
+  for (uint32_t f = 0; f < F && G > 0 && T > 0; ++f) {
+    double* gv = gval.data() + (size_t)f * G * T;
+    uint32_t* gc = f == 0 ? gcnt.data() : fcnt.data();
+    check(op == kAggQuantile ? b2p_group_quantile(ctx, param, r.field(f), r.valid.data(), groups.id.data(), r.rows, G,
+                                                  (uint64_t)T, gv, gc)
+                             : b2p_group_aggregate(ctx, op == kAggGroup ? B2P_AGG_COUNT : op, r.field(f),
+                                                   r.valid.data(), groups.id.data(), r.rows, G, (uint64_t)T, gv, gc),
           ErrorKind::Execution);
+  }
   r.labels = std::move(groups.labels);
   r.columns = Columns::TagsTimeValue;
   r.cell_order.clear();
-  r.val.assign((size_t)G * T, 0.0);
+  r.val.assign((size_t)F * G * T, 0.0);
   r.valid.assign((size_t)G * Tw, 0u);
   for (uint32_t g = 0; g < G; ++g) {
     const uint32_t row = groups.rank[g];
     for (size_t k = 0; k < T; ++k) {
       if (gcnt[g * T + k] == 0) continue;
-      r.val[row * T + k] = op == kAggGroup ? 1.0 : gval[g * T + k];
+      for (uint32_t f = 0; f < F; ++f)
+        r.val[((size_t)f * G + row) * T + k] = op == kAggGroup ? 1.0 : gval[((size_t)f * G + g) * T + k];
       r.valid[(size_t)row * Tw + (k >> 5)] |= 1u << (k & 31);
     }
   }
@@ -381,8 +386,22 @@ PromRangePlan::PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args) : PlanNode(ct
         throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: by-column " + b + " is not a tag column");
   }
   if (args_.interval <= 0) throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: interval must be positive");
-  if (args_.time_index.empty() || args_.field_column.empty())
-    throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: time index and field column are required");
+  const std::vector<std::string>& fields = args_.field_columns;
+  if (fields.empty() || fields.size() > B2P_MAX_FIELDS)
+    throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: between 1 and " + std::to_string(B2P_MAX_FIELDS) +
+                                         " field columns are required, got " + std::to_string(fields.size()));
+  if (args_.time_index.empty()) throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: time index and field column are required");
+  for (size_t f = 0; f < fields.size(); ++f) {
+    if (fields[f].empty()) throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: time index and field column are required");
+    if (std::find(fields.begin(), fields.begin() + (long)f, fields[f]) != fields.begin() + (long)f)
+      throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: field column " + fields[f] + " is given twice");
+  }
+  // with several fields the aggregate stage would name every field's column alike (sum(prom_rate)): AggregatePlan over
+  // this node is the multi-field route
+  if (fields.size() > 1 && agg_id_ >= 0)
+    throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: the aggregate stage takes one field column; use an aggregate node");
+  val_.resize(fields.size());
+  present_.resize(fields.size());
   series_.names = args_.tag_columns;
   series_.values.resize(args_.tag_columns.size());
 }
@@ -392,6 +411,8 @@ void PromRangePlan::set_histogram(const std::string& le_column, double quantile)
     throw PlanError(ErrorKind::Plan, "HistogramFold: le column " + le_column + " is not a tag column");
   if (!args_.aggregate.empty())
     throw PlanError(ErrorKind::Plan, "HistogramFold over an aggregate is not supported by this node");
+  if (args_.field_columns.size() > 1)
+    throw PlanError(ErrorKind::Plan, "HistogramFold over several field columns is not supported by this node");
   args_.histogram = true;
   args_.le_column = le_column;
   args_.quantile = quantile;
@@ -403,18 +424,20 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
   if (n == 0) return;  // an empty batch is skipped (never parks the stream, SURVEY appendix C-11)
   const int ti = b.find(args_.time_index);
   if (ti < 0) throw PlanError(ErrorKind::Plan, "No field named " + args_.time_index);  // field_not_found
-  const int fi = b.find(args_.field_column);
-  if (fi < 0) throw PlanError(ErrorKind::Plan, "No field named " + args_.field_column);
+  const size_t F = args_.field_columns.size();
+  std::vector<int> fi(F);
+  for (size_t f = 0; f < F; ++f) {
+    fi[f] = b.find(args_.field_columns[f]);
+    if (fi[f] < 0) throw PlanError(ErrorKind::Plan, "No field named " + args_.field_columns[f]);
+  }
   const char* tfmt = b.field(ti).format;
   if (!(starts_with(tfmt, "tsm:") || std::strcmp(tfmt, "l") == 0))
     throw PlanError(ErrorKind::Execution, "Time index Column downcast to TimestampMillisecondArray failed");
-  if (std::strcmp(b.field(fi).format, "g") != 0)
-    throw PlanError(ErrorKind::Execution, "field column " + args_.field_column + " is not Float64");
+  for (size_t f = 0; f < F; ++f)
+    if (std::strcmp(b.field(fi[f]).format, "g") != 0)
+      throw PlanError(ErrorKind::Execution, "field column " + args_.field_columns[f] + " is not Float64");
   const ArrowArray& ta = b.column(ti);
-  const ArrowArray& fa = b.column(fi);
   const int64_t* tsv = static_cast<const int64_t*>(ta.buffers[1]) + ta.offset + b.offset();
-  const double* fv = static_cast<const double*>(fa.buffers[1]) + fa.offset + b.offset();
-  const uint8_t* fvalid = fa.null_count != 0 ? static_cast<const uint8_t*>(fa.buffers[0]) : nullptr;
 
   // tag columns: Utf8 (int32 offsets) tuple, or a single UInt64 id
   struct TagCol {
@@ -459,10 +482,32 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
   // column is never built nor shipped.
   const size_t row_base = ts_.size();
   ts_.insert(ts_.end(), tsv, tsv + n);
-  val_.insert(val_.end(), fv, fv + n);
-  if (fvalid) {  // a NULL field value cannot be inside a window: treat it like the NaN the filter drops
-    for (int64_t row = 0; row < n; ++row)
-      if (!bit_set(fvalid, fa.offset + b.offset() + row)) val_[row_base + (size_t)row] = std::nan("");
+  for (size_t f = 0; f < F; ++f) {
+    const ArrowArray& fa = b.column(fi[f]);
+    const int64_t base = fa.offset + b.offset();
+    const double* fv = static_cast<const double*>(fa.buffers[1]) + base;
+    const uint8_t* fvalid = fa.null_count != 0 ? static_cast<const uint8_t*>(fa.buffers[0]) : nullptr;
+    std::vector<double>& v = val_[f];
+    v.insert(v.end(), fv, fv + n);
+    if (F == 1) {
+      if (fvalid) {  // a NULL field value cannot be inside a window: treat it like the NaN the filter drops
+        for (int64_t row = 0; row < n; ++row)
+          if (!bit_set(fvalid, base + row)) v[row_base + (size_t)row] = std::nan("");
+      }
+      continue;
+    }
+    // several fields: the device decides per function what a NULL slot means (b2p_range_eval_fields), so the slots go
+    // down as one bitmap per field, rows from bit 0; a field without a NULL so far has none
+    std::vector<uint8_t>& bits = present_[f];
+    if (!fvalid && bits.empty()) continue;
+    const size_t total = row_base + (size_t)n;
+    if (bits.empty()) bits.assign((row_base + 7) / 8, 0xFF);
+    bits.resize((total + 7) / 8, 0xFF);
+    for (int64_t row = 0; row < n; ++row) {
+      const size_t at = row_base + (size_t)row;
+      if (bit_set(fvalid, base + row)) bits[at >> 3] |= (uint8_t)(1u << (at & 7));
+      else bits[at >> 3] &= (uint8_t)~(1u << (at & 7));
+    }
   }
   auto start_series = [&](int64_t row) {
     offsets_.push_back((uint64_t)(row_base + (size_t)row));
@@ -531,23 +576,45 @@ void PromRangePlan::compute(NodeResult& r) {
   offsets_.resize((size_t)S);          // (a previous execute() appended the end marker)
   offsets_.push_back((uint64_t)ts_.size());
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  const uint32_t F = (uint32_t)args_.field_columns.size();
   const bool fold_on_device = args_.histogram && fn_id_ >= 0;  // the dense matrix then never reaches the host
-  std::vector<double> dense(fold_on_device ? 0 : (size_t)S * (size_t)T);
+  const size_t cells = (size_t)S * (size_t)T;
+  std::vector<double> dense(fold_on_device ? 0 : F * cells);
   std::vector<uint32_t> valid(fold_on_device ? 0 : (size_t)S * Tw);
-  if (S > 0 && T > 0 && !fold_on_device)
-    check(fn_id_ >= 0 ? b2p_range_eval(ctx_, &p, ts_.data(), val_.data(), nullptr, offsets_.data(), ts_.size(), S,
+  if (S > 0 && T > 0 && !fold_on_device && F == 1)
+    check(fn_id_ >= 0 ? b2p_range_eval(ctx_, &p, ts_.data(), val_[0].data(), nullptr, offsets_.data(), ts_.size(), S,
                                        dense.data(), valid.data(), nullptr)
                       : b2p_instant_select(ctx_, p.start, p.end, p.interval, args_.lookback_delta, p.offset, ts_.data(),
-                                           val_.data(), nullptr, offsets_.data(), ts_.size(), S, dense.data(),
+                                           val_[0].data(), nullptr, offsets_.data(), ts_.size(), S, dense.data(),
                                            valid.data()));  // InstantManipulate
+  if (S > 0 && T > 0 && F > 1) {
+    std::vector<const double*> vals(F);
+    std::vector<double*> outs(F);
+    std::vector<const uint8_t*> present(F);
+    bool any_null = false;
+    for (uint32_t f = 0; f < F; ++f) {
+      vals[f] = val_[f].data();
+      outs[f] = dense.data() + f * cells;
+      present_[f].resize(present_[f].empty() ? 0 : (ts_.size() + 7) / 8, 0xFF);
+      present[f] = present_[f].empty() ? nullptr : present_[f].data();
+      any_null = any_null || present[f];
+    }
+    const uint8_t* const* nulls = any_null ? present.data() : nullptr;
+    check(fn_id_ >= 0 ? b2p_range_eval_fields(ctx_, &p, ts_.data(), vals.data(), nulls, (int32_t)F, nullptr,
+                                              offsets_.data(), ts_.size(), S, outs.data(), valid.data())
+                      : b2p_instant_select_fields(ctx_, p.start, p.end, p.interval, args_.lookback_delta, p.offset,
+                                                  ts_.data(), vals.data(), nulls, (int32_t)F, nullptr, offsets_.data(),
+                                                  ts_.size(), S, outs.data(), valid.data()));
+  }
   r = NodeResult();
   r.T = T;
   r.Tw = Tw;
+  r.F = F;
   r.eval_ts.resize((size_t)T);  // also when there are no series: scalar() of such a node has a NaN row at every step
   for (int64_t k = 0; k < T; ++k) r.eval_ts[(size_t)k] = p.start + k * p.interval;
   r.time_index = args_.time_index;
-  r.value_name =
-      fn_id_ >= 0 ? args_.function + "(" + args_.time_index + "_range," + args_.field_column + ")" : args_.field_column;
+  for (const std::string& field : args_.field_columns)
+    r.value_names.push_back(fn_id_ >= 0 ? args_.function + "(" + args_.time_index + "_range," + field + ")" : field);
 
   if (args_.histogram) {
     // HistogramFold (histogram_fold.rs:754-820): group the series by their tags without `le`, order each group's
@@ -559,7 +626,7 @@ void PromRangePlan::compute(NodeResult& r) {
     r.valid.assign((size_t)H * Tw, 0u);
     if (H > 0 && T > 0) {
       if (fn_id_ < 0) throw PlanError(ErrorKind::Plan, "HistogramFold over an instant selector is not supported by this node");
-      check(b2p_range_histogram_fold(ctx_, &p, ts_.data(), val_.data(), nullptr, offsets_.data(), ts_.size(), S,
+      check(b2p_range_histogram_fold(ctx_, &p, ts_.data(), val_[0].data(), nullptr, offsets_.data(), ts_.size(), S,
                                      args_.quantile, ix.hist_off.data(), ix.bucket_series.data(), ix.bucket_le.data(),
                                      H, r.val.data(), r.valid.data()));
     }
@@ -575,7 +642,7 @@ void PromRangePlan::compute(NodeResult& r) {
       // prom_aggr_expr_to_plan: group keys = by-labels + eval ts; output sorted by (labels asc, ts asc).  Over an id key
       // the by-label is the id's decimal string, so those rows sort as strings ("10" before "9").
       aggregate_rows(ctx_, agg_id_, 0.0, series_.columns(args_.by_columns), r);
-      r.value_name = args_.aggregate + "(" + (fn_id_ >= 0 ? args_.function : args_.field_column) + ")";
+      r.value_names = {args_.aggregate + "(" + (fn_id_ >= 0 ? args_.function : args_.field_columns[0]) + ")"};
     }
   }
 }
@@ -625,38 +692,42 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     if (!L.id_keyed) c_tags[t]->offsets.push_back(0);
   };
   OwnedColumn* c_ts = nullptr;
-  OwnedColumn* c_val = nullptr;
-  OwnedColumn* c_label = nullptr;  // count_values' counted value
+  std::vector<OwnedColumn*> c_vals;  // [F]
+  OwnedColumn* c_label = nullptr;    // count_values' counted value
   const bool int_val = r.columns == Columns::CountTagsTimeLabel && r.value_is_count;
+  if (r.value_names.size() != r.F) throw PlanError(ErrorKind::Internal, "export: one value name per field expected");
+  auto add_vals = [&](const char* fmt) {
+    for (const std::string& name : r.value_names) c_vals.push_back(add_col(name, fmt));
+  };
   switch (r.columns) {
     case Columns::TimeValueTags:
       c_ts = add_col(r.time_index, "tsm:");
-      c_val = add_col(r.value_name, "g");
+      add_vals("g");
       for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
       break;
     case Columns::TagsTimeValue:
       for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
       c_ts = add_col(r.time_index, "tsm:");
-      c_val = add_col(r.value_name, "g");
+      add_vals("g");
       break;
     case Columns::ValueTagsTime:
-      c_val = add_col(r.value_name, "g");
+      add_vals("g");
       for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
       c_ts = add_col(r.time_index, "tsm:");
       break;
     case Columns::CountTagsTimeLabel:
-      c_val = add_col(r.value_name, int_val ? "l" : "g");
+      add_vals(int_val ? "l" : "g");
       for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
       c_ts = add_col(r.time_index, "tsm:");
       c_label = add_col(r.label_name, "g");
       break;
-    case Columns::TimeSorted: {
+    case Columns::TimeSorted: {  // (`or`, one field)
       c_ts = add_col(r.time_index, "tsm:");
       std::vector<std::string> names = L.names;
-      names.push_back(r.value_name);
+      names.push_back(r.value_names[0]);
       std::sort(names.begin(), names.end());
       for (const std::string& name : names) {
-        if (name == r.value_name && !c_val) c_val = add_col(name, "g");
+        if (name == r.value_names[0] && c_vals.empty()) c_vals.push_back(add_col(name, "g"));
         else add_tag((size_t)L.column(name));
       }
       break;
@@ -673,9 +744,11 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     const int64_t k = (int64_t)(cell % (uint64_t)r.T);
     if (!r.valid_at(row, k)) continue;
     c_ts->i64.push_back(r.eval_ts[(size_t)k]);
-    const double v = r.val[(size_t)row * (size_t)r.T + (size_t)k];
-    if (int_val) c_val->i64.push_back((int64_t)v);
-    else c_val->f64.push_back(v);
+    for (uint32_t f = 0; f < r.F; ++f) {
+      const double v = r.field(f)[(size_t)row * (size_t)r.T + (size_t)k];
+      if (int_val) c_vals[f]->i64.push_back((int64_t)v);
+      else c_vals[f]->f64.push_back(v);
+    }
     if (c_label) c_label->f64.push_back(r.label_val[(size_t)row * (size_t)r.T + (size_t)k]);
     for (size_t t = 0; t < c_tags.size(); ++t) {
       if (L.id_keyed) {
@@ -832,20 +905,27 @@ void PlanNode::run(NodeResult& r) {
       const bool has_rows = std::any_of(r.valid.begin(), r.valid.end(), [](uint32_t w) { return w != 0; });
       if (s.op >= B2P_IFN_CLAMP && lo > hi && has_rows)
         throw PlanError(ErrorKind::Execution, "min '" + rust_display(lo) + "' > max '" + rust_display(hi) + "'");
-      if (work)
-        check(b2p_instant_fn(ctx_, s.op, a0, a1, r.val.data(), r.valid.data(), r.rows, (uint64_t)r.T, r.val.data(),
+      // once per field (planner.rs:2416); a function keeps every bit, so the fields share the bitmap
+      for (uint32_t f = 0; f < r.F && work; ++f)
+        check(b2p_instant_fn(ctx_, s.op, a0, a1, r.field(f), r.valid.data(), r.rows, (uint64_t)r.T, r.field(f),
                              r.valid.data()));
-      std::string name = s.fn_name + "(" + r.value_name;
-      for (double a : s.args) name += "," + float_literal(a);
-      r.value_name = name + ")";
+      for (std::string& value : r.value_names) {
+        std::string name = s.fn_name + "(" + value;
+        for (double a : s.args) name += "," + float_literal(a);
+        value = name + ")";
+      }
       continue;
     }
-    if (work)
-      check(b2p_scalar_op(ctx_, s.op, s.return_bool ? 1 : 0, s.scalar_on_left ? 1 : 0, s.scalar, r.val.data(),
-                          r.valid.data(), r.rows, (uint64_t)r.T, r.val.data(), r.valid.data()));
-    if (!is_comparison(s.op) || s.return_bool) {  // a projection names its expression; a filter keeps the column
+    const bool filter = is_comparison(s.op) && !s.return_bool;
+    if (filter && r.F > 1)  // planner.rs:3976-3981
+      throw PlanError(ErrorKind::Plan, "Unsupported expr type: filter on multi-value input");
+    for (uint32_t f = 0; f < r.F && work; ++f)  // arithmetic and `bool` keep every bit (planner.rs:3930-3960)
+      check(b2p_scalar_op(ctx_, s.op, s.return_bool ? 1 : 0, s.scalar_on_left ? 1 : 0, s.scalar, r.field(f),
+                          r.valid.data(), r.rows, (uint64_t)r.T, r.field(f), r.valid.data()));
+    if (!filter) {  // a projection names its expression; a filter keeps the column
       const std::string lit = float_literal(s.scalar), sym = kOpSymbols[s.op];
-      r.value_name = s.scalar_on_left ? lit + " " + sym + " " + r.value_name : r.value_name + " " + sym + " " + lit;
+      for (std::string& value : r.value_names)
+        value = s.scalar_on_left ? lit + " " + sym + " " + value : value + " " + sym + " " + lit;
     }
   }
 }
@@ -907,18 +987,31 @@ void BinaryPlan::compute(NodeResult& r) {
   }
   const uint64_t n_pairs = lrow.size();
   if (n_pairs > UINT32_MAX) throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: more than 2^32 - 1 matched series pairs");
+  // the fields zip pairwise, field i with field i (align_binary_field_columns, planner.rs:3401-3414); a filter decides
+  // on its one pair and keeps every field of the lhs
+  const bool filter = is_comparison(op_) && !return_bool_;
+  const uint32_t pairs = std::min(L.F, R.F);
+  if (filter && pairs > 1) throw PlanError(ErrorKind::Plan, "Unsupported expr type: filter on multi-value input");
   r = NodeResult();
   r.T = L.T;
   r.Tw = L.Tw;
   r.rows = (uint32_t)n_pairs;
+  r.F = filter ? L.F : pairs;
   r.eval_ts = L.eval_ts;
-  r.val.assign((size_t)n_pairs * (size_t)r.T, 0.0);
+  r.val.assign((size_t)r.F * n_pairs * (size_t)r.T, 0.0);
   r.valid.assign((size_t)n_pairs * r.Tw, 0u);
-  if (n_pairs > 0 && r.T > 0)
-    check(b2p_binary_op(ctx_, op_, return_bool_ ? 1 : 0, L.val.data(), L.valid.data(), lrow.data(), L.rows, R.val.data(),
-                        R.valid.data(), rrow.data(), R.rows, n_pairs, (uint64_t)r.T, r.val.data(), r.valid.data()));
+  for (uint32_t f = 0; f < pairs && n_pairs > 0 && r.T > 0; ++f)  // arithmetic and `bool` keep the join's bits
+    check(b2p_binary_op(ctx_, op_, return_bool_ ? 1 : 0, L.field(f), L.valid.data(), lrow.data(), L.rows, R.field(f),
+                        R.valid.data(), rrow.data(), R.rows, n_pairs, (uint64_t)r.T, r.field(f), r.valid.data()));
+  // the lhs's other fields at the cells the comparison kept; a dropped cell holds 0.0, as the kernel writes it
+  for (uint32_t f = 1; filter && f < r.F; ++f)
+    for (uint64_t q = 0; q < n_pairs; ++q) {
+      const double* src = L.field(f) + (size_t)lrow[q] * (size_t)r.T;
+      double* dst = r.field(f) + (size_t)q * (size_t)r.T;
+      for (int64_t k = 0; k < r.T; ++k)
+        if (r.valid_at((uint32_t)q, k)) dst[k] = src[k];
+    }
   // output labels: a filter passes the lhs rows through; a projection emits the tag columns of `label_side`
-  const bool filter = is_comparison(op_) && !return_bool_;
   const bool from_lhs = filter || labels_from_lhs_;
   const NodeResult& side = from_lhs ? L : R;
   const std::vector<uint32_t>& srow = from_lhs ? lrow : rrow;
@@ -926,7 +1019,7 @@ void BinaryPlan::compute(NodeResult& r) {
   r.labels = side.labels.gather(srow);
   if (filter) {
     r.columns = L.columns;
-    r.value_name = L.value_name;
+    r.value_names = L.value_names;
     r.label_name = L.label_name;
     r.value_is_count = L.value_is_count;
     if (!L.label_val.empty()) {
@@ -936,7 +1029,8 @@ void BinaryPlan::compute(NodeResult& r) {
     }
   } else {
     r.columns = Columns::TagsTimeValue;
-    r.value_name = L.value_name + " " + kOpSymbols[op_] + " " + R.value_name;
+    for (uint32_t f = 0; f < r.F; ++f)
+      r.value_names.push_back(L.value_names[f] + " " + kOpSymbols[op_] + " " + R.value_names[f]);
   }
 }
 
@@ -993,6 +1087,19 @@ void SetOpPlan::compute(NodeResult& r) {
   lhs_->run(L);
   rhs_->run(R);
   const std::string what = std::string("set operator `") + kSetNames[op_] + "`: ";
+  // planner.rs:3656-3661 (`and` and `unless` both name it the AND operator), 3718-3730
+  if (op_ == B2P_SET_OR && L.F != R.F) {
+    auto list = [](const std::vector<std::string>& v) {
+      std::string out;
+      for (const std::string& x : v) out += (out.empty() ? "\"" : ", \"") + x + "\"";
+      return "[" + out + "]";
+    };
+    throw PlanError(ErrorKind::Plan, "Attempt to combine two tables with different column sets, left: " +
+                                         list(L.value_names) + ", right: " + list(R.value_names));
+  }
+  if (L.F > 1)
+    throw PlanError(ErrorKind::Plan, std::string("Multi fields calculation is not supported in ") +
+                                         (op_ == B2P_SET_OR ? "OR operator" : "AND operator"));
   if (L.T != R.T || (L.rows > 0 && R.rows > 0 && L.eval_ts != R.eval_ts))
     throw PlanError(ErrorKind::Plan, what + "both sides must be evaluated on the same steps");
   // the reference matches set operators on label values (planner.rs:3626-3630), which an id-keyed node does not carry
@@ -1067,7 +1174,7 @@ void SetOpPlan::compute(NodeResult& r) {
     check(b2p_setop(ctx_, op_, L.val.data(), L.valid.data(), lkey.data(), L.rows, R.val.data(), R.valid.data(),
                           rkey.data(), R.rows, (uint32_t)keys.ids.size(), (uint64_t)T, r.val.data(), r.valid.data()));
   r.time_index = L.time_index;
-  r.value_name = L.value_name;
+  r.value_names = L.value_names;
   r.columns = Columns::TimeSorted;
   r.labels.names = all;
   r.labels.values.resize(all.size());
@@ -1088,6 +1195,7 @@ ScalarPlan::ScalarPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child) : PlanNode
 void ScalarPlan::compute(NodeResult& r) {
   NodeResult C;
   child_->run(C);
+  if (C.F > 1) throw PlanError(ErrorKind::Plan, "Multi fields calculation is not supported in scalar");  // planner.rs:3155-3160
   // one dense key per label tuple over the child's tag columns (a tagless child is one series, an id-keyed one is keyed
   // by the id); a tuple with a NULL label gets B2P_NO_KEY (scalar_calculate.rs:543-569 compares NULL as None against
   // the "" it recorded)
@@ -1110,7 +1218,7 @@ void ScalarPlan::compute(NodeResult& r) {
   r.rows = 1;
   r.eval_ts = C.eval_ts;
   r.time_index = C.time_index;
-  r.value_name = "scalar(" + C.value_name + ")";
+  r.value_names = {"scalar(" + C.value_names[0] + ")"};
   r.val.assign((size_t)r.T, 0.0);
   r.valid.assign((size_t)r.Tw, 0u);
   if (r.T > 0)  // two rows of one series with a cell at the same step are bad data here, not a bad plan
@@ -1151,6 +1259,8 @@ TopkPlan::TopkPlan(b2p_ctx* ctx, bool bottom, double k, std::shared_ptr<PlanNode
 
 void TopkPlan::compute(NodeResult& r) {
   child_->run(r);
+  if (r.F > 1)  // planner.rs:2969-2974
+    throw PlanError(ErrorKind::Plan, "Unsupported expr type: topk or bottomk on multi-value input");
   const char* what = bottom_ ? "bottomk: " : "topk: ";
   // the window orders ties by the label values (planner.rs:2980-2996), which an id-keyed node does not carry
   if (r.labels.id_keyed) throw PlanError(ErrorKind::Plan, std::string(what) + "an id-keyed (__tsid) child has no label values to order by");
@@ -1225,11 +1335,13 @@ void AggregatePlan::compute(NodeResult& r) {
   // only the id, so it can group such a node as a whole and nothing else
   if (r.labels.id_keyed && modifier_ != Modifier::None)
     throw PlanError(ErrorKind::Plan, "GpuPromAggregateExec: an id-keyed (__tsid) child can only be aggregated without by / without");
-  const std::string child_value = r.value_name;
-  aggregate_rows(ctx_, op_, param_, group_columns(r.labels, modifier_, labels_), r);
-  r.value_name = op_ == kAggGroup      ? "max(" + float_literal(1.0) + ")"
-                 : op_ == kAggQuantile ? "quantile(" + float_literal(param_) + "," + child_value + ")"
-                                       : df_name_ + "(" + child_value + ")";
+  if (op_ == kAggGroup && r.F > 1)  // planner.rs:2815-2823
+    throw PlanError(ErrorKind::Plan, "Multi fields calculation is not supported in group()");
+  aggregate_rows(ctx_, op_, param_, group_columns(r.labels, modifier_, labels_), r);  // one aggregate per field
+  for (std::string& value : r.value_names)
+    value = op_ == kAggGroup      ? "max(" + float_literal(1.0) + ")"
+            : op_ == kAggQuantile ? "quantile(" + float_literal(param_) + "," + value + ")"
+                                  : df_name_ + "(" + value + ")";
 }
 
 // ---- CountValuesPlan -----------------------------------------------------------------------------------
@@ -1242,11 +1354,13 @@ CountValuesPlan::CountValuesPlan(b2p_ctx* ctx, std::string label, std::shared_pt
 
 void CountValuesPlan::compute(NodeResult& r) {
   child_->run(r);
+  if (r.F > 1)  // planner.rs:2874-2879
+    throw PlanError(ErrorKind::Plan, "Unsupported expr type: count_values on multi-value input");
   // keep_tsid is false for count_values (planner.rs:402): as for AggregatePlan, an id-keyed child groups as a whole only
   if (r.labels.id_keyed && modifier_ != Modifier::None)
     throw PlanError(ErrorKind::Plan, "GpuPromCountValuesExec: an id-keyed (__tsid) child can only be counted without by / without");
   const std::vector<int> cols = group_columns(r.labels, modifier_, labels_);
-  const std::string count_name = "count(" + r.value_name + ")";
+  const std::string count_name = "count(" + r.value_names[0] + ")";
   // the projection would have two columns of one name (planner.rs:425-430)
   bool clash = label_ == r.time_index || label_ == count_name;
   for (int c : cols) clash = clash || r.labels.names[(size_t)c] == label_;
@@ -1297,7 +1411,7 @@ void CountValuesPlan::compute(NodeResult& r) {
         if (r.valid_at(o, (int64_t)k)) r.cell_order.push_back((uint64_t)o * T + k);
   r.rows = n;
   r.columns = Columns::CountTagsTimeLabel;
-  r.value_name = count_name;
+  r.value_names = {count_name};
   r.label_name = label_;
   r.value_is_count = true;
 }
@@ -1329,22 +1443,32 @@ void SubqueryPlan::compute(NodeResult& r) {
   r.rows = C.rows;
   r.eval_ts.resize((size_t)r.T);
   for (int64_t k = 0; k < r.T; ++k) r.eval_ts[(size_t)k] = p_.start + k * p_.interval;
-  r.val.assign((size_t)r.rows * (size_t)r.T, 0.0);
+  r.F = C.F;
+  r.val.assign((size_t)r.F * r.rows * (size_t)r.T, 0.0);
   r.valid.assign((size_t)r.rows * r.Tw, 0u);
-  if (r.rows > 0 && r.T > 0)
-    check(b2p_subquery(ctx_, &p_, T_in > 0 ? C.eval_ts[0] : p_.start, step, C.val.data(), C.valid.data(), C.rows,
-                       (uint64_t)T_in, r.val.data(), r.valid.data()));
+  // the function once per field over the same windows (planner.rs:292-332), then the conjunction of the fields' IS NOT
+  // NULL: a cell is kept where every field's result is
+  std::vector<uint32_t> field_valid(r.F > 1 ? r.valid.size() : 0);
+  for (uint32_t f = 0; f < r.F && r.rows > 0 && r.T > 0; ++f) {
+    uint32_t* fv = f == 0 ? r.valid.data() : field_valid.data();
+    check(b2p_subquery(ctx_, &p_, T_in > 0 ? C.eval_ts[0] : p_.start, step, C.field(f), C.valid.data(), C.rows,
+                       (uint64_t)T_in, r.field(f), fv));
+    if (f > 0)
+      for (size_t w = 0; w < r.valid.size(); ++w) r.valid[w] &= fv[w];
+  }
   r.time_index = C.time_index;
   r.labels = std::move(C.labels);
-  std::string name = function_ + "(" + C.time_index + "_range," + C.value_name;
-  if (p_.fn_id == B2P_FN_RATE || p_.fn_id == B2P_FN_INCREASE || p_.fn_id == B2P_FN_DELTA) {
-    name += "," + C.time_index + ",Int64(" + std::to_string(p_.range) + ")";
-  } else if (p_.fn_id == B2P_FN_PREDICT_LINEAR || p_.fn_id == B2P_FN_QUANTILE_OVER_TIME) {
-    name += "," + float_literal(p_.param0);
-  } else if (p_.fn_id == B2P_FN_HOLT_WINTERS) {
-    name += "," + float_literal(p_.param0) + "," + float_literal(p_.param1);
+  for (const std::string& value : C.value_names) {
+    std::string name = function_ + "(" + C.time_index + "_range," + value;
+    if (p_.fn_id == B2P_FN_RATE || p_.fn_id == B2P_FN_INCREASE || p_.fn_id == B2P_FN_DELTA) {
+      name += "," + C.time_index + ",Int64(" + std::to_string(p_.range) + ")";
+    } else if (p_.fn_id == B2P_FN_PREDICT_LINEAR || p_.fn_id == B2P_FN_QUANTILE_OVER_TIME) {
+      name += "," + float_literal(p_.param0);
+    } else if (p_.fn_id == B2P_FN_HOLT_WINTERS) {
+      name += "," + float_literal(p_.param0) + "," + float_literal(p_.param1);
+    }
+    r.value_names.push_back(name + ")");
   }
-  r.value_name = name + ")";
 }
 
 // ---- HistogramQuantilePlan -----------------------------------------------------------------------------
@@ -1361,6 +1485,8 @@ void HistogramQuantilePlan::compute(NodeResult& r) {
     throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: an id-keyed (__tsid) child carries no " + le_column_ + " label");
   if (r.columns == Columns::CountTagsTimeLabel)
     throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: a count_values child is not supported by this node");
+  // the reference folds the first field only (planner.rs:3084-3092, a FIXME); this node does not copy that
+  if (r.F > 1) throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: a multi-field child is not supported by this node");
   r.cell_order.clear();
   const int le = r.labels.column(le_column_);
   if (le < 0) {  // create_histogram_plan: no le tag -> EmptyRelation, no rows and no columns
@@ -1413,7 +1539,11 @@ void SortPlan::compute(NodeResult& r) {
     if (r.rows == 0 || T == 0) return;
     r.cell_order.resize((size_t)r.rows * (size_t)T);
     uint64_t n = 0;
-    check(b2p_sort_cells(ctx_, desc_ ? 1 : 0, r.val.data(), r.valid.data(), r.rows, T, r.cell_order.data(), &n),
+    // by every field in turn (planner.rs:1066-1071): lexicographic over the fields
+    std::vector<const double*> vals(r.F);
+    for (uint32_t f = 0; f < r.F; ++f) vals[f] = r.field(f);
+    check(b2p_sort_cells_fields(ctx_, desc_ ? 1 : 0, vals.data(), (int32_t)r.F, r.valid.data(), r.rows, T,
+                                r.cell_order.data(), &n),
           ErrorKind::Execution);
     r.cell_order.resize((size_t)n);
     return;
@@ -1480,7 +1610,7 @@ void AbsentPlan::compute(NodeResult& r) {
     check(b2p_absent(ctx_, C.rows > 0 ? C.valid.data() : nullptr, C.rows, (uint64_t)r.T, r.val.data(), r.valid.data()),
           ErrorKind::Execution);
   r.time_index = time_index_;
-  r.value_name = value_column_;
+  r.value_names = {value_column_};
   for (const auto& [name, value] : labels_) {
     r.labels.names.push_back(name);
     r.labels.values.push_back({Label(value)});
@@ -1564,11 +1694,17 @@ extern "C" {
 
 const char* b2p_plan_last_error(void) { return g_err.c_str(); }
 
-b2p_plan* b2p_plan_range_create(b2p_ctx* ctx, const char* function, const b2p_range_params* p, const char* time_index,
-                                const char* field_column, const char* const* tag_columns, int32_t n_tags,
-                                const char* aggregate, const char* const* by_columns, int32_t n_by) {
+b2p_plan* b2p_plan_range_create_fields(b2p_ctx* ctx, const char* function, const b2p_range_params* p,
+                                       const char* time_index, const char* const* field_columns, int32_t n_fields,
+                                       const char* const* tag_columns, int32_t n_tags, const char* aggregate,
+                                       const char* const* by_columns, int32_t n_by) {
   return create([&] {
-    if (!function || !p || !time_index || !field_column) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    if (!function || !p || !time_index || !field_columns) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    if (n_fields < 1 || n_fields > B2P_MAX_FIELDS)
+      throw b2p::PlanError(b2p::ErrorKind::Plan, "n_fields must be in [1, " + std::to_string(B2P_MAX_FIELDS) + "], got " +
+                                                     std::to_string(n_fields));
+    for (int32_t f = 0; f < n_fields; ++f)
+      if (!field_columns[f]) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
     b2p::PromRangePlanArgs a;
     a.function = function;
     a.start = p->start;
@@ -1580,12 +1716,23 @@ b2p_plan* b2p_plan_range_create(b2p_ctx* ctx, const char* function, const b2p_ra
     a.param0 = p->param0;
     a.param1 = p->param1;
     a.time_index = time_index;
-    a.field_column = field_column;
+    a.field_columns = strings(field_columns, n_fields);
     a.tag_columns = strings(tag_columns, n_tags);
     if (aggregate && aggregate[0]) a.aggregate = aggregate;
     a.by_columns = strings(by_columns, n_by);
     return std::make_shared<b2p::PromRangePlan>(ctx, std::move(a));
   });
+}
+
+b2p_plan* b2p_plan_range_create(b2p_ctx* ctx, const char* function, const b2p_range_params* p, const char* time_index,
+                                const char* field_column, const char* const* tag_columns, int32_t n_tags,
+                                const char* aggregate, const char* const* by_columns, int32_t n_by) {
+  if (!field_column) {
+    g_err = "NULL argument";
+    return nullptr;
+  }
+  return b2p_plan_range_create_fields(ctx, function, p, time_index, &field_column, 1, tag_columns, n_tags, aggregate,
+                                      by_columns, n_by);
 }
 
 b2p_plan* b2p_plan_binary_create(b2p_ctx* ctx, int32_t op, int32_t return_bool, b2p_plan* lhs, b2p_plan* rhs,

@@ -57,7 +57,8 @@ struct PromRangePlanArgs {
   // RangeManipulate::new
   Millisecond start = 0, end = 0, interval = 0, range = 0;
   std::string time_index;
-  std::string field_column;
+  // RangeManipulate field_columns: 1 to B2P_MAX_FIELDS Float64 columns, every one selected (planner.rs:2180)
+  std::vector<std::string> field_columns;
   // SeriesNormalize::new
   Millisecond offset = 0;
   bool need_filter_out_nan = true;
@@ -110,16 +111,22 @@ enum class Columns {
   None,                // no column at all: histogram_quantile over a child without the le tag (an EmptyRelation)
 };
 
-// What a node computed, before it becomes Arrow: a dense [rows x T] grid with validity, the eval timestamps and one label
-// tuple per row.  Exported, row r emits one Arrow row per valid step k (rows in order, steps ascending).
+// What a node computed, before it becomes Arrow: F dense [rows x T] grids (one per field) under one validity, the eval
+// timestamps and one label tuple per row.  Exported, row r emits one Arrow row per valid step k (rows in order, steps
+// ascending) with F value columns.  One bitmap serves every field because no node that accepts F >= 2 clears a bit for
+// one field and not another: element-wise stages, arithmetic and `bool` keep bits, a join's bits are its presence, a
+// group has a cell wherever a member has, sort keeps bits, and the one per-value filter (a filtering comparison) is
+// refused for F >= 2 (DESIGN §8).
 struct NodeResult {
   int64_t T = 0;
   uint32_t Tw = 0;
   uint32_t rows = 0;
+  uint32_t F = 1;                // fields
   std::vector<int64_t> eval_ts;  // [T]
-  std::vector<double> val;       // [rows x T]; empty when rows == 0 or T == 0
+  std::vector<double> val;       // [F x rows x T], field f at f * rows * T; empty when rows == 0 or T == 0
   std::vector<uint32_t> valid;   // [rows x Tw]
-  std::string time_index, value_name;
+  std::string time_index;
+  std::vector<std::string> value_names;  // [F]
   Labels labels;
   Columns columns = Columns::TimeValueTags;
   // when not empty, the export emits these cells (row * T + step), in this order, instead of rows then steps; a cell
@@ -131,6 +138,9 @@ struct NodeResult {
   std::string label_name;
   bool value_is_count = false;
   bool valid_at(uint32_t r, int64_t k) const { return (valid[(size_t)r * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u; }
+  size_t grid() const { return (size_t)rows * (size_t)T; }
+  double* field(uint32_t f) { return val.data() + f * grid(); }
+  const double* field(uint32_t f) const { return val.data() + f * grid(); }
 };
 
 // One element-wise stage on top of a node's result: `node op scalar` / `scalar op node` (b2p_plan_set_scalar_op), or an
@@ -188,7 +198,9 @@ class PromRangePlan : public PlanNode {
   int fn_id_;
   int agg_id_;
   std::vector<int64_t> ts_;
-  std::vector<double> val_;
+  std::vector<std::vector<double>> val_;  // [field][row]
+  // F >= 2: each field's Arrow validity bitmap re-based to bit 0 of the first row (empty while the field has no NULL)
+  std::vector<std::vector<uint8_t>> present_;
   std::vector<uint64_t> offsets_;  // first row of every series (SeriesDivide's output), end marker added by execute()
   Labels series_;                  // [series] the labels of each series' first row
   int64_t num_series_ = 0;

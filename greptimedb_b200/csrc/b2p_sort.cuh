@@ -9,6 +9,10 @@
 // radix sort in row-major order and the sort is stable, so equal values keep the child's row, then step, order in
 // both directions.  CUB's floating-point key mode is not used: it ranks -0.0 and +0.0 equal and does not put negative
 // NaNs where total_cmp does.
+// Several fields (sort over a multi-field node: Sort(f0, f1, .. each ASC | DESC NULLS FIRST), planner.rs:2743-2749)
+// sort least significant key first: the scatter keys on the last field, and for each earlier field
+//   sort_rekey_kernel    one thread per pair: the pair's key reloaded from that field at its cell
+// precedes one more stable radix sort.  Stability makes the order lexicographic over the fields.
 #pragma once
 #include <cstdint>
 
@@ -48,6 +52,15 @@ __global__ void __launch_bounds__(256) sort_scatter_kernel(const SortArgs a) {
       base += __popc(word);
     }
   }
+}
+
+__global__ void __launch_bounds__(256) sort_rekey_kernel(const double* __restrict__ vals,
+                                                         const unsigned long long* __restrict__ cells,
+                                                         unsigned long long* __restrict__ keys, uint64_t n, int desc) {
+  const unsigned long long flip = desc ? ~0x8000000000000000ull : 0x8000000000000000ull;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+    keys[i] = (unsigned long long)total_key(__ldg(vals + cells[i])) ^ flip;
 }
 
 }  // namespace b2p

@@ -458,6 +458,24 @@ class Context:
                                            C.byref(n)))
         return out[:n.value].copy()
 
+    def sort_cells_fields(self, desc, vals, valid):
+        """sort / sort_desc over F fields: vals [F,R,T] (or F grids [R,T]) sharing valid [R,Tw] u32 -> u64 [n valid
+        cells], ordered lexicographically by the fields' values (field 0 first, the f64 total order), equal tuples in
+        row-major order."""
+        vals = [np.ascontiguousarray(v, np.float64) for v in vals]
+        valid = np.ascontiguousarray(valid, np.uint32)
+        R, T = vals[0].shape
+        if any(v.shape != (R, T) for v in vals):
+            raise ValueError(f"every field must be [{R}, {T}]")
+        if valid.shape != (R, (T + 31) // 32):
+            raise ValueError(f"valid must be [{R}, {(T + 31) // 32}] u32 words, got {valid.shape}")
+        out = np.zeros(max(R * T, 1), np.uint64)
+        n = C.c_uint64(0)
+        vp, _keep = self._ptr_array(vals)
+        self._check(self._L.b2p_sort_cells_fields(self._h, int(bool(desc)), vp, len(vals), _ptr(valid), R, T,
+                                                  _ptr(out), C.byref(n)))
+        return out[:n.value].copy()
+
     def absent(self, valid, T):
         """absent() over any grid's validity valid [R,Tw] u32 with T steps -> (out [T] f64, out_valid [Tw] u32): the steps
         at which no row has a valid cell (bits past T ignored), with the value 1.0; 0.0 and a clear bit elsewhere."""
@@ -627,6 +645,13 @@ class Context:
         first out_n written) and out_n (one device u64).  Synchronises the context's stream once (the cell count)."""
         self._check(self._L.b2p_sort_cells_dev(self._h, int(bool(desc)), _ptr(vals), _ptr(valid), n_rows, T,
                                                _ptr(out_cells), _ptr(out_n)))
+
+    def sort_cells_fields_dev(self, desc, vals, valid, n_rows, T, out_cells, out_n):
+        """Device form of sort_cells_fields(): vals a sequence of F device grids [n_rows,T] sharing valid [n_rows,Tw].
+        Synchronises the context's stream once (the cell count)."""
+        vp, _keep = self._ptr_array(vals)
+        self._check(self._L.b2p_sort_cells_fields_dev(self._h, int(bool(desc)), vp, len(vals), _ptr(valid), n_rows, T,
+                                                      _ptr(out_cells), _ptr(out_n)))
 
     def absent_dev(self, valid, n_rows, T, out, out_valid):
         """Device form of absent(): valid [n_rows,Tw] into out [T] / out_valid [Tw].  No host round trip."""

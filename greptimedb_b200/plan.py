@@ -13,7 +13,7 @@ sort / sort_desc / sort_by_label / sort_by_label_desc(node) and `AbsentPlan` is 
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Union
 
 from . import _lib
 from .engine import B2PError, Context, make_params, op_id, setop_id, topk_bottom
@@ -82,19 +82,23 @@ class _PlanNode:
 
 
 class PromRangeExec(_PlanNode):
+    """The range / instant leaf.  `field_column` is one field name, or a sequence of them for a table with several
+    Float64 field columns: every field is selected at once and execute() emits one value column per field."""
+
     def __init__(self, ctx: Context, function: str, start: int, end: int, interval: int, range: int, time_index: str,
-                 field_column: str, tag_columns: Sequence[str], offset: int = 0, need_filter_out_nan: bool = True,
-                 param0: float = 0.0, param1: float = 0.0, aggregate: Optional[str] = None,
-                 by_columns: Sequence[str] = (), lookback_delta: Optional[int] = None,
+                 field_column: Union[str, Sequence[str]], tag_columns: Sequence[str], offset: int = 0,
+                 need_filter_out_nan: bool = True, param0: float = 0.0, param1: float = 0.0,
+                 aggregate: Optional[str] = None, by_columns: Sequence[str] = (), lookback_delta: Optional[int] = None,
                  histogram_quantile: Optional[float] = None, le_column: str = "le"):
         self._L = _lib.load()
         self._ctx = ctx
         p = make_params(0, start, end, interval, range, offset=offset, filter_nan=need_filter_out_nan, param0=param0,
                         param1=param1)
-        tags, by = _cstr_array(tag_columns), _cstr_array(by_columns)
-        self._h = self._L.b2p_plan_range_create(ctx._h, function.encode(), C.byref(p), time_index.encode(),
-                                                field_column.encode(), tags, len(tag_columns),
-                                                (aggregate or "").encode(), by, len(by_columns))
+        fields = [field_column] if isinstance(field_column, str) else list(field_column)
+        tags, by, fa = _cstr_array(tag_columns), _cstr_array(by_columns), _cstr_array(fields)
+        self._h = self._L.b2p_plan_range_create_fields(ctx._h, function.encode(), C.byref(p), time_index.encode(), fa,
+                                                       len(fields), tags, len(tag_columns), (aggregate or "").encode(),
+                                                       by, len(by_columns))
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())
         if lookback_delta is not None:      # instant-vector selector (InstantManipulate) instead of a range function

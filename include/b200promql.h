@@ -57,6 +57,8 @@
  *                              + Filter, planner.rs:292-332
  *   b2p_sort_cells[_dev]       sort / sort_desc: Filter(value IS NOT NULL) -> Sort(value ASC | DESC, NULLS FIRST),
  *                              planner.rs:1060-1089, 2743-2772
+ *   b2p_sort_cells_fields[_dev] the same over several fields: Sort(f0, f1, .. ASC | DESC, NULLS FIRST),
+ *                              planner.rs:1066-1071, 2743-2749
  *
  * Data layout (HBM, struct-of-arrays, all row-sorted by (series id, timestamp) exactly like
  * the reference's required_input_ordering, series_divide.rs:410-440):
@@ -456,6 +458,16 @@ B2P_API int b2p_subquery_dev(b2p_ctx* ctx, const b2p_range_params* p, int64_t in
  * B2P_E_TOO_LARGE: n_rows >= 2^31 - 1. */
 B2P_API int b2p_sort_cells_dev(b2p_ctx* ctx, int32_t desc, const double* vals, const uint32_t* valid, uint32_t n_rows,
                                uint64_t T, uint64_t* out_cells, uint64_t* out_n);
+/* sort / sort_desc over a node with several fields (the reference sorts by every field in order, each ASC | DESC NULLS
+ * FIRST, planner.rs:1066-1071, 2743-2749): as b2p_sort_cells_dev, ordered lexicographically by the fields' values in
+ * the f64 total order, field 0 first, every field in the same direction.  `vals` is a HOST array of n_fields DEVICE
+ * grids [n_rows x T] sharing the bitmap `valid`; 1 <= n_fields <= B2P_MAX_FIELDS.  Equal tuples keep row-major order.
+ * It is a least-significant-key-first radix sort: the scatter keys on field n_fields - 1, then each earlier field reloads
+ * the pairs' keys (sort_rekey_kernel) before another stable sort, so the call makes n_fields radix sorts and
+ * n_fields - 1 rekey launches; the scratch stays 24 B per valid cell.  n_fields == 1 is exactly b2p_sort_cells_dev. */
+B2P_API int b2p_sort_cells_fields_dev(b2p_ctx* ctx, int32_t desc, const double* const* vals, int32_t n_fields,
+                                      const uint32_t* valid, uint32_t n_rows, uint64_t T, uint64_t* out_cells,
+                                      uint64_t* out_n);
 
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
@@ -551,6 +563,10 @@ B2P_API int b2p_subquery(b2p_ctx* ctx, const b2p_range_params* p, int64_t inner_
  * n_rows * T entries, the first *out_n written) and out_n are host pointers. */
 B2P_API int b2p_sort_cells(b2p_ctx* ctx, int32_t desc, const double* vals, const uint32_t* valid, uint32_t n_rows,
                            uint64_t T, uint64_t* out_cells, uint64_t* out_n);
+/* Host-pointer form of b2p_sort_cells_fields_dev (synchronous): vals[f] are host grids. */
+B2P_API int b2p_sort_cells_fields(b2p_ctx* ctx, int32_t desc, const double* const* vals, int32_t n_fields,
+                                  const uint32_t* valid, uint32_t n_rows, uint64_t T, uint64_t* out_cells,
+                                  uint64_t* out_n);
 
 /* Host-pointer forms of b2p_instant_fn_dev / b2p_scalar_calculate_dev (synchronous; device-found errors returned). */
 B2P_API int b2p_instant_fn(b2p_ctx* ctx, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
@@ -605,11 +621,30 @@ B2P_API b2p_plan* b2p_plan_range_create(b2p_ctx* ctx, const char* function, cons
                                         const char* time_index, const char* field_column,
                                         const char* const* tag_columns, int32_t n_tags, const char* aggregate,
                                         const char* const* by_columns, int32_t n_by);
+/* The same node over a table with several Float64 field columns (Influx line protocol / OTLP ingest), 1 <= n_fields <=
+ * B2P_MAX_FIELDS: every field is selected at once, as b2p_range_eval_fields / b2p_instant_select_fields evaluate them
+ * (a NaN in any field drops the row from every field with p->filter_nan; a cell is kept where every field's result
+ * is).  b2p_plan_range_create is this call with one field.  The export has columns {time index, one value per field in
+ * the given order, tags..}, each value named as the one-field node names its field.  The node's result carries
+ * n_fields values per cell under one validity, and the nodes above keep them (DESIGN §8): element-wise stages,
+ * arithmetic and `bool` apply per field; a binary node zips the fields pairwise (min of the two counts); an aggregate
+ * folds each field; sort orders by every field in turn; subquery applies its function per field; absent reads only
+ * validity.  Refused with the reference's Plan errors when a node sees two or more fields: a filtering comparison
+ * ("Unsupported expr type: filter on multi-value input"), topk / bottomk, count_values, group, scalar, and / or /
+ * unless, and histogram_quantile.  With two or more fields, NULL slots of a field are handed to the device as its Arrow
+ * validity bitmap (the calls the reference evaluates differently over a NULL slot are refused at execute, naming the
+ * field); with one field a NULL slot is read as NaN, as b2p_plan_range_create always has.  At create: a duplicate field,
+ * n_fields out of range, and `aggregate` with two or more fields are Plan errors; at push: a missing field ("No field
+ * named ..") is a Plan error and a non-Float64 one an Execution error. */
+B2P_API b2p_plan* b2p_plan_range_create_fields(b2p_ctx* ctx, const char* function, const b2p_range_params* p,
+                                               const char* time_index, const char* const* field_columns,
+                                               int32_t n_fields, const char* const* tag_columns, int32_t n_tags,
+                                               const char* aggregate, const char* const* by_columns, int32_t n_by);
 /* Turn the node into the instant-vector form: InstantManipulate(start, end, lookback_delta, interval, ...)
  * (instant_manipulate.rs:189-208) instead of RangeManipulate + prom_fn; `function` / range are then ignored. */
 B2P_API int b2p_plan_set_instant(b2p_plan* plan, int64_t lookback_delta);
 /* Add HistogramFold(le_column, field, time_index, quantile) (histogram_fold.rs:104-130) on top of the per-series
- * result: series that agree on every tag except `le` form one histogram. */
+ * result: series that agree on every tag except `le` form one histogram.  Refused for a node of two or more fields. */
 B2P_API int b2p_plan_set_histogram_quantile(b2p_plan* plan, const char* le_column, double quantile);
 /* `node op scalar` (or `scalar op node` with scalar_on_left) on top of any node, binary nodes included; calls chain in
  * order (rate(x[1m]) * 60 > 1 is two calls).  Arithmetic and `bool` keep every row (the value column is renamed like

@@ -2,7 +2,7 @@
 //!
 //! ```text
 //! [AggregateExec(Final) <- RepartitionExec <- AggregateExec(Partial) <-]
-//! FilterExec(prom_fn IS NOT NULL) <- ProjectionExec(prom_fn(ts_range, val, ts, range))
+//! FilterExec(prom_fn IS NOT NULL [AND ..]) <- ProjectionExec(prom_fn(ts_range, val, ts, range) [per field column])
 //!    <- PromRangeManipulateExec <- PromSeriesNormalizeExec <- PromSeriesDivideExec <- (scan)
 //! ```
 //!
@@ -45,7 +45,9 @@ pub struct GpuPromRangeParams {
     pub interval: Millisecond,
     pub range: Millisecond,
     pub time_index_column: String,
-    pub field_column: String,
+    /// RangeManipulate's field columns (1..=64 Float64 columns), every one selected; the node emits one value column per
+    /// field in this order (b2p_plan_range_create_fields).
+    pub field_columns: Vec<String>,
     // SeriesNormalize::new (normalize.rs:66-83)
     pub offset: Millisecond,
     pub need_filter_out_nan: bool,
@@ -214,7 +216,7 @@ impl DisplayAs for GpuPromRangeExec {
         match t {
             DisplayFormatType::Default | DisplayFormatType::Verbose | DisplayFormatType::TreeRender => write!(
                 f,
-                "GpuPromRangeExec: fn=[{}], req range=[{}..{}], interval=[{}], eval range=[{}], offset=[{}], time index=[{}], tags={:?}{}{}",
+                "GpuPromRangeExec: fn=[{}], req range=[{}..{}], interval=[{}], eval range=[{}], offset=[{}], time index=[{}], fields={:?}, tags={:?}{}{}",
                 if self.params.function.is_empty() { "instant" } else { &self.params.function },
                 self.params.start,
                 self.params.end,
@@ -222,6 +224,7 @@ impl DisplayAs for GpuPromRangeExec {
                 self.params.range,
                 self.params.offset,
                 self.params.time_index_column,
+                self.params.field_columns,
                 self.params.tag_columns,
                 self.params.aggregate.as_ref().map(|a| format!(", aggr=[{a} by {:?}]", self.params.by_columns)).unwrap_or_default(),
                 self.params.histogram.as_ref().map(|(le, q)| format!(", histogram_quantile=[{q}, le={le}]")).unwrap_or_default(),
@@ -250,7 +253,8 @@ impl PlanHandle {
             let c = |s: &str| CString::new(s).expect("column names contain no NUL");
             let function = c(&p.function);
             let time_index = c(&p.time_index_column);
-            let field = c(&p.field_column);
+            let fields: Vec<CString> = p.field_columns.iter().map(|s| c(s)).collect();
+            let field_ptrs: Vec<*const std::os::raw::c_char> = fields.iter().map(|s| s.as_ptr()).collect();
             let tags: Vec<CString> = p.tag_columns.iter().map(|s| c(s)).collect();
             let tag_ptrs: Vec<*const std::os::raw::c_char> = tags.iter().map(|s| s.as_ptr()).collect();
             let by: Vec<CString> = p.by_columns.iter().map(|s| c(s)).collect();
@@ -267,9 +271,9 @@ impl PlanHandle {
                 param0: p.param0,
                 param1: p.param1,
             };
-            let plan = ffi::b2p_plan_range_create(
-                ctx, function.as_ptr(), &params, time_index.as_ptr(), field.as_ptr(), tag_ptrs.as_ptr(), tag_ptrs.len() as i32,
-                aggregate.as_ptr(), by_ptrs.as_ptr(), by_ptrs.len() as i32,
+            let plan = ffi::b2p_plan_range_create_fields(
+                ctx, function.as_ptr(), &params, time_index.as_ptr(), field_ptrs.as_ptr(), field_ptrs.len() as i32,
+                tag_ptrs.as_ptr(), tag_ptrs.len() as i32, aggregate.as_ptr(), by_ptrs.as_ptr(), by_ptrs.len() as i32,
             );
             if plan.is_null() {
                 let e = ffi::plan_last_error();

@@ -342,6 +342,12 @@ extern "C" {
         ctx: *mut b2p_ctx, desc: i32, vals: *const f64, valid: *const u32, n_rows: u32, t: u64, out_cells: *mut u64,
         out_n: *mut u64,
     ) -> c_int;
+    /// sort / sort_desc over several fields: `vals` is a host array of n_fields device grids sharing `valid`; the cells
+    /// in lexicographic order over the fields (field 0 first), equal tuples in row-major order.
+    pub fn b2p_sort_cells_fields_dev(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const *const f64, n_fields: i32, valid: *const u32, n_rows: u32, t: u64,
+        out_cells: *mut u64, out_n: *mut u64,
+    ) -> c_int;
     /// absent (K15): out_valid [Tw] = the steps at which no row of the device grid's validity [n_rows x Tw] has a bit
     /// (bits past T cleared), out [T] = 1.0 there and 0.0 elsewhere.  Only validity words are read; no host round trip.
     pub fn b2p_absent_dev(
@@ -443,6 +449,11 @@ extern "C" {
         ctx: *mut b2p_ctx, desc: i32, vals: *const f64, valid: *const u32, n_rows: u32, t: u64, out_cells: *mut u64,
         out_n: *mut u64,
     ) -> c_int;
+    /// Host-pointer form of b2p_sort_cells_fields_dev (synchronous).
+    pub fn b2p_sort_cells_fields(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const *const f64, n_fields: i32, valid: *const u32, n_rows: u32, t: u64,
+        out_cells: *mut u64, out_n: *mut u64,
+    ) -> c_int;
     /// Host-pointer form of b2p_absent_dev (synchronous).
     pub fn b2p_absent(
         ctx: *mut b2p_ctx, valid: *const u32, n_rows: u32, t: u64, out: *mut f64, out_valid: *mut u32,
@@ -453,6 +464,12 @@ extern "C" {
         ctx: *mut b2p_ctx, function: *const c_char, p: *const B2pRangeParams, time_index: *const c_char,
         field_column: *const c_char, tag_columns: *const *const c_char, n_tags: i32, aggregate: *const c_char,
         by_columns: *const *const c_char, n_by: i32,
+    ) -> *mut b2p_plan;
+    /// The range / instant leaf over 1..=64 Float64 field columns, every one selected; one value column per field.
+    pub fn b2p_plan_range_create_fields(
+        ctx: *mut b2p_ctx, function: *const c_char, p: *const B2pRangeParams, time_index: *const c_char,
+        field_columns: *const *const c_char, n_fields: i32, tag_columns: *const *const c_char, n_tags: i32,
+        aggregate: *const c_char, by_columns: *const *const c_char, n_by: i32,
     ) -> *mut b2p_plan;
     pub fn b2p_plan_set_instant(plan: *mut b2p_plan, lookback_delta: i64) -> c_int;
     pub fn b2p_plan_set_histogram_quantile(plan: *mut b2p_plan, le_column: *const c_char, quantile: f64) -> c_int;

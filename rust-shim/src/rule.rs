@@ -7,8 +7,9 @@
 //! ```text
 //!   [SortPreservingMergeExec / SortExec(labels, ts)]                                  (planner.rs:443-449)
 //!   [AggregateExec(FinalPartitioned) <- RepartitionExec <- AggregateExec(Partial)]    prom_aggr_expr_to_plan
-//!   FilterExec: prom_fn(...)@i IS NOT NULL                                            planner.rs:1063
+//!   FilterExec: prom_fn(...)@i IS NOT NULL [AND ..]                                   planner.rs:1063, 2774-2791
 //!   ProjectionExec: expr=[ts, prom_fn(ts_range, val, ts, range_ms) as .., tags..]     planner.rs:1012-1101
+//!                   (one prom_fn call per field column of a multi-field table, planner.rs:2180)
 //!   PromRangeManipulateExec: req range=[..], interval=[..], eval range=[..]           range_manipulate.rs
 //!   PromSeriesNormalizeExec: offset=[..], time index=[..], filter NaN: [..]           normalize.rs
 //!   PromSeriesDivideExec: tags=[..]                                                   series_divide.rs
@@ -106,6 +107,11 @@
 //!     <- GpuPromRangeExec (on the same grid)   => `match_absent`: the b2p_plan_absent_create arguments
 //! ```
 //!
+//! Over a table with several field columns the rule takes the shapes the library evaluates per field (the leaf, the
+//! aggregate node with one aggregate per field, sort by every field, subqueries, absent, the binary zip) and leaves on
+//! the CPU those the library refuses there (the leaf's own aggregate, filtering comparisons over two or more fields,
+//! topk / bottomk, count_values, group, scalar, set operators with a multi-field side, histogram_quantile).
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
@@ -137,6 +143,73 @@ use promql::extension_plan::{
     UnionDistinctOnExec,
 };
 
+/// The projection indices a `FilterExec` keeps rows on: `c IS NOT NULL`, or the conjunction of such tests that closes a
+/// multi-field selector (`create_empty_values_filter_expr`, planner.rs:2774-2791), in ascending order; `None` for any
+/// other predicate.
+fn not_null_columns(pred: &Arc<dyn PhysicalExpr>) -> Option<Vec<usize>> {
+    let mut out = Vec::new();
+    let mut stack = vec![pred.clone()];
+    while let Some(e) = stack.pop() {
+        if let Some(b) = e.as_any().downcast_ref::<BinaryExpr>() {
+            if *b.op() != Operator::And {
+                return None;
+            }
+            stack.push(b.left().clone());
+            stack.push(b.right().clone());
+            continue;
+        }
+        let not_null = e.as_any().downcast_ref::<IsNotNullExpr>()?;
+        out.push(not_null.arg().as_any().downcast_ref::<Column>()?.index());
+    }
+    out.sort_unstable();
+    out.dedup();
+    Some(out)
+}
+
+/// The closing pair of a range selector or a subquery, `FilterExec(<its IS NOT NULL tests>) <- ProjectionExec(plain
+/// columns, one prom_fn call per field column)` (planner.rs:1012-1101, 2180, 2774-2791): the filtered columns are exactly
+/// the calls, every call is the same function with the same literal arguments, call i reads its value column as
+/// `prom_fn(ts_range, <field>, ..)`, and every other projected expression is a plain column.
+struct FieldUdfs {
+    function: String,
+    params: (f64, f64),
+    /// the value column each call reads, in projection order (the RangeManipulate's field columns)
+    fields: Vec<String>,
+    input: Arc<dyn ExecutionPlan>,
+}
+
+fn match_field_udfs(plan: &Arc<dyn ExecutionPlan>) -> Option<FieldUdfs> {
+    let filter = plan.as_any().downcast_ref::<FilterExec>()?;
+    let filtered = not_null_columns(filter.predicate())?;
+    let projection = filter.input().as_any().downcast_ref::<ProjectionExec>()?;
+    let mut function: Option<String> = None;
+    let mut params: Option<(f64, f64)> = None;
+    let (mut fields, mut calls) = (Vec::new(), Vec::new());
+    for (i, e) in projection.expr().iter().enumerate() {
+        if e.expr.as_any().downcast_ref::<Column>().is_some() {
+            continue;
+        }
+        let udf = e.expr.as_any().downcast_ref::<ScalarFunctionExpr>()?;
+        let name = udf.name();
+        B2pFn::from_udf_name(name)?;
+        // UDF arguments (planner.rs:2438-2474): (ts_range, value_range [, ts] [, range_length | scalar params ..])
+        let p = scalar_params(name, udf.args())?;
+        if function.get_or_insert_with(|| name.to_string()).as_str() != name {
+            return None;
+        }
+        let bits = |q: (f64, f64)| (q.0.to_bits(), q.1.to_bits());
+        if bits(*params.get_or_insert(p)) != bits(p) {
+            return None;
+        }
+        fields.push(udf.args().get(1)?.as_any().downcast_ref::<Column>()?.name().to_string());
+        calls.push(i);
+    }
+    if calls.is_empty() || calls != filtered {
+        return None;
+    }
+    Some(FieldUdfs { function: function?, params: params?, fields, input: projection.input().clone() })
+}
+
 #[derive(Debug)]
 pub struct GpuPromRewrite {
     device: i32,
@@ -147,42 +220,26 @@ impl GpuPromRewrite {
         Self { device }
     }
 
-    /// `FilterExec(prom_fn IS NOT NULL) <- ProjectionExec(prom_fn(..)) <- RangeManipulate <- Normalize <- Divide <- input`
+    /// `FilterExec(prom_fn IS NOT NULL [AND ..]) <- ProjectionExec(prom_fn(..) per field) <- RangeManipulate <- Normalize
+    /// <- Divide <- input`, one call per field column of the RangeManipulate, in its order (`match_field_udfs`); the time
+    /// index and the tags are plain columns, which the node emits unchanged.
     fn match_range_subtree(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<(GpuPromRangeParams, Arc<dyn ExecutionPlan>)> {
-        let filter = plan.as_any().downcast_ref::<FilterExec>()?;
-        // predicate: <column i> IS NOT NULL, where column i of the projection is the prom_* call
-        let not_null = filter.predicate().as_any().downcast_ref::<IsNotNullExpr>()?;
-        let filtered_col = not_null.arg().as_any().downcast_ref::<Column>()?.index();
-        let projection = filter.input().as_any().downcast_ref::<ProjectionExec>()?;
-        let (udf_expr, _alias) = {
-            let e = projection.expr().get(filtered_col)?;
-            (e.expr.clone(), e.alias.clone())
-        };
-        let udf = udf_expr.as_any().downcast_ref::<ScalarFunctionExpr>()?;
-        let function = udf.name().to_string();
-        B2pFn::from_udf_name(&function)?;
-        // every other projected expression must be a plain column (time index, tags): the node emits them unchanged
-        for (i, e) in projection.expr().iter().enumerate() {
-            if i != filtered_col && e.expr.as_any().downcast_ref::<Column>().is_none() {
-                return None;
-            }
-        }
-        let range_exec = projection.input().as_any().downcast_ref::<RangeManipulateExec>()?;
+        let udfs = match_field_udfs(plan)?;
+        let range_exec = udfs.input.as_any().downcast_ref::<RangeManipulateExec>()?;
         let normalize = range_exec.input().as_any().downcast_ref::<SeriesNormalizeExec>()?;
         let divide = normalize.input().as_any().downcast_ref::<SeriesDivideExec>()?;
-        if range_exec.field_columns().len() != 1 {
-            return None; // one value column per series on this path (the reference supports several; they stay on the CPU)
+        if !range_exec.field_columns().iter().eq(udfs.fields.iter()) {
+            return None;
         }
-        // UDF arguments (planner.rs:2438-2474): (ts_range, value_range [, ts] [, range_length | scalar params ..])
-        let (param0, param1) = scalar_params(&function, udf.args())?;
+        let (param0, param1) = udfs.params;
         let params = GpuPromRangeParams {
-            function,
+            function: udfs.function,
             start: range_exec.start(),
             end: range_exec.end(),
             interval: range_exec.interval(),
             range: range_exec.range(),
             time_index_column: range_exec.time_index_column().to_string(),
-            field_column: range_exec.field_columns()[0].clone(),
+            field_columns: range_exec.field_columns().to_vec(),
             offset: normalize.offset(),
             need_filter_out_nan: normalize.need_filter_out_nan(),
             tag_columns: divide.tag_columns().to_vec(),
@@ -211,6 +268,9 @@ impl GpuPromRewrite {
             return None;
         }
         let (mut params, input) = self.match_range_subtree(partial.input())?;
+        if params.field_columns.len() != 1 {
+            return None; // the library refuses the leaf's aggregate stage over several fields: `match_aggregate_node`
+        }
         let agg = match partial.aggr_expr()[0].fun().name() {
             "sum" => "sum",
             "avg" => "avg",
@@ -419,6 +479,9 @@ impl GpuPromRewrite {
         if filter != (op.is_comparison() && !return_bool) {
             return None;
         }
+        if filter && node.params().field_columns.len() != 1 {
+            return None; // refused over several fields (planner.rs:3976-3981)
+        }
         let (scalar, on_left) = match (float_literal(&l), float_literal(&r)) {
             (None, Some(v)) if l.as_any().downcast_ref::<Column>().is_some() => (v, false),
             (Some(v), None) if r.as_any().downcast_ref::<Column>().is_some() => (v, true),
@@ -463,6 +526,9 @@ impl GpuPromRewrite {
     pub fn match_scalar(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromScalarSpec> {
         let s = plan.as_any().downcast_ref::<ScalarCalculateExec>()?;
         let child = s.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        if child.params().field_columns.len() != 1 {
+            return None; // refused over several fields (planner.rs:3155-3160)
+        }
         Some(GpuPromScalarSpec { child: child.params().clone() })
     }
 
@@ -479,6 +545,9 @@ impl GpuPromRewrite {
             return None;
         }
         let child = window.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        if child.params().field_columns.len() != 1 {
+            return None; // refused over several fields (planner.rs:2969-2974)
+        }
         // rank <= Float64(k) (the UInt64 rank is cast to Float64, planner.rs:475)
         let pred = filter.predicate().as_any().downcast_ref::<BinaryExpr>()?;
         if *pred.op() != Operator::LtEq {
@@ -501,7 +570,9 @@ impl GpuPromRewrite {
     /// `AggregateExec(Final) <- RepartitionExec <- AggregateExec(Partial)` over a `GpuPromRangeExec` -> the arguments of
     /// `b2p_plan_aggregate_create`.  `quantile(Float64(φ), col)` needs a literal φ; `max(Float64(1))` is `group`
     /// (planner.rs:2836-2838).  A non-literal φ and group columns that are not tags of the child stay on the CPU;
-    /// count_values (which groups by the value column too) is `match_count_values`.
+    /// count_values (which groups by the value column too) is `match_count_values`.  Over a child with F field columns
+    /// the reference plans one aggregate of the same op per field (planner.rs:2824-2866): F aggregate expressions, the
+    /// i-th over the child's i-th value column; `group()` is refused there (planner.rs:2815-2823) and stays on the CPU.
     pub fn match_aggregate_node(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromAggregateSpec> {
         let fin = plan.as_any().downcast_ref::<AggregateExec>()?;
         if !matches!(fin.mode(), AggregateMode::FinalPartitioned | AggregateMode::Final) {
@@ -509,13 +580,32 @@ impl GpuPromRewrite {
         }
         let repart = fin.input().as_any().downcast_ref::<RepartitionExec>()?;
         let partial = repart.input().as_any().downcast_ref::<AggregateExec>()?;
-        let [a] = partial.aggr_expr() else { return None };
+        let [a, rest @ ..] = partial.aggr_expr() else { return None };
         if !matches!(partial.mode(), AggregateMode::Partial) {
             return None;
         }
         let child = partial.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        if 1 + rest.len() != child.params().field_columns.len() {
+            return None;
+        }
         let args = a.expressions();
         let first_literal = args.first().and_then(float_literal);
+        if !rest.is_empty() {
+            // the child's output is {time index, value per field, tags..}: aggregate i reads value column i
+            let schema = child.schema();
+            for (i, e) in partial.aggr_expr().iter().enumerate() {
+                let e_args = e.expressions();
+                if e.fun().name() != a.fun().name()
+                    || e_args.first().and_then(float_literal).map(f64::to_bits) != first_literal.map(f64::to_bits)
+                {
+                    return None;
+                }
+                let col = e_args.last()?.as_any().downcast_ref::<Column>()?;
+                if col.name() != schema.field(1 + i).name().as_str() {
+                    return None;
+                }
+            }
+        }
         let (op, param) = match a.fun().name() {
             "sum" => ("sum", 0.0),
             "avg" => ("avg", 0.0),
@@ -528,6 +618,9 @@ impl GpuPromRewrite {
             "quantile" => ("quantile", first_literal?),
             _ => return None,
         };
+        if op == "group" && !rest.is_empty() {
+            return None;
+        }
         // every group column other than the time index must be one of the child's tags: count_values (planned as
         // count with the value column among the group columns, planner.rs:420-424, 2833) goes to match_count_values,
         // and any other grouping the node cannot express stays on the CPU
@@ -565,6 +658,9 @@ impl GpuPromRewrite {
         }
         let child = partial.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
         let params = child.params();
+        if params.field_columns.len() != 1 {
+            return None; // refused over several fields (planner.rs:2874-2879)
+        }
         let mut by = Vec::new();
         let mut value = None;
         for (expr, _name) in partial.group_expr().expr() {
@@ -596,23 +692,12 @@ impl GpuPromRewrite {
     /// RangeManipulate windows every input batch as one series (range_manipulate.rs:603-630) and the node windows every
     /// child row, so only a child that hands one series per batch is taken: a range or instant node (SeriesDivide's
     /// batches), with or without element-wise stages, or its aggregate without `by` (one series).  An aggregate by labels
-    /// or a HistogramFold child stays on the CPU.
+    /// or a HistogramFold child stays on the CPU.  Over a multi-field child the function is projected once per field
+    /// and the filter is the conjunction of their IS NOT NULL (planner.rs:292-332), as for the leaf (`match_field_udfs`).
     pub fn match_subquery(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromSubquerySpec> {
-        let filter = plan.as_any().downcast_ref::<FilterExec>()?;
-        let not_null = filter.predicate().as_any().downcast_ref::<IsNotNullExpr>()?;
-        let filtered_col = not_null.arg().as_any().downcast_ref::<Column>()?.index();
-        let projection = filter.input().as_any().downcast_ref::<ProjectionExec>()?;
-        let udf_expr = projection.expr().get(filtered_col)?.expr.clone();
-        let udf = udf_expr.as_any().downcast_ref::<ScalarFunctionExpr>()?;
-        let function = udf.name().to_string();
-        B2pFn::from_udf_name(&function)?;
-        for (i, e) in projection.expr().iter().enumerate() {
-            if i != filtered_col && e.expr.as_any().downcast_ref::<Column>().is_none() {
-                return None;
-            }
-        }
-        let range_exec = projection.input().as_any().downcast_ref::<RangeManipulateExec>()?;
-        if range_exec.field_columns().len() != 1 || range_exec.range() <= 0 {
+        let udfs = match_field_udfs(plan)?;
+        let range_exec = udfs.input.as_any().downcast_ref::<RangeManipulateExec>()?;
+        if range_exec.range() <= 0 || !range_exec.field_columns().iter().eq(udfs.fields.iter()) {
             return None;
         }
         let child = range_exec.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
@@ -620,9 +705,12 @@ impl GpuPromRewrite {
         if params.histogram.is_some() || (params.aggregate.is_some() && !params.by_columns.is_empty()) {
             return None;
         }
-        let (param0, param1) = scalar_params(&function, udf.args())?;
+        if range_exec.field_columns().len() != params.field_columns.len() {
+            return None;
+        }
+        let (param0, param1) = udfs.params;
         Some(GpuPromSubquerySpec {
-            function,
+            function: udfs.function,
             start: range_exec.start(),
             end: range_exec.end(),
             interval: range_exec.interval(),
@@ -652,7 +740,11 @@ impl GpuPromRewrite {
         }
         let child = input.as_any().downcast_ref::<GpuPromRangeExec>()?;
         let le_column = fold.input().schema().field(fold.le_column_index()).name().to_string();
-        if child.params().histogram.is_some() || !child.params().tag_columns.iter().any(|t| *t == le_column) {
+        // several fields: the reference folds the first one only (a FIXME, planner.rs:3084-3092); the library refuses
+        if child.params().histogram.is_some()
+            || child.params().field_columns.len() != 1
+            || !child.params().tag_columns.iter().any(|t| *t == le_column)
+        {
             return None;
         }
         Some(GpuPromHistogramQuantileSpec { le_column, phi: fold.quantile(), child: child.params().clone() })
@@ -663,7 +755,9 @@ impl GpuPromRewrite {
     /// be the value column alone, NULLS FIRST (ascending: sort, descending: sort_desc), or one or more tag columns of the
     /// child, all in one direction, NULLS LAST (sort_by_label / sort_by_label_desc).  Any other key stays on the CPU: the
     /// time index, a column that is not a tag, mixed directions or null orderings.  The projection must pass the time
-    /// index, the value and the tags through as plain columns.
+    /// index, the value and the tags through as plain columns.  Over a multi-field child the filter is the conjunction
+    /// of the value columns' IS NOT NULL and sort / sort_desc key on every value column in order (planner.rs:1066-1071,
+    /// 2743-2749), which the library's multi-key sort reproduces.
     pub fn match_sort(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromSortSpec> {
         let plan = match plan.as_any().downcast_ref::<SortPreservingMergeExec>() {
             Some(m) => m.input(),
@@ -671,17 +765,19 @@ impl GpuPromRewrite {
         };
         let sort = plan.as_any().downcast_ref::<SortExec>()?;
         let filter = sort.input().as_any().downcast_ref::<FilterExec>()?;
-        let not_null = filter.predicate().as_any().downcast_ref::<IsNotNullExpr>()?;
-        let value_index = not_null.arg().as_any().downcast_ref::<Column>()?.index();
+        let value_indices = not_null_columns(filter.predicate())?;
         let projection = filter.input().as_any().downcast_ref::<ProjectionExec>()?;
         let child = projection.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
         let params = child.params();
+        if value_indices.len() != params.field_columns.len() {
+            return None;
+        }
         let mut names = Vec::new();
         for e in projection.expr() {
             e.expr.as_any().downcast_ref::<Column>()?;
             names.push(e.alias.clone());
         }
-        let value = names.get(value_index)?.clone();
+        let values = value_indices.iter().map(|&i| names.get(i).cloned()).collect::<Option<Vec<String>>>()?;
         let keys: Vec<(String, bool, bool)> = sort
             .expr()
             .iter()
@@ -694,7 +790,7 @@ impl GpuPromRewrite {
         if keys.iter().any(|(_, d, n)| *d != descending || *n != nulls_first) {
             return None;
         }
-        if keys.len() == 1 && keys[0].0 == value {
+        if keys.iter().map(|k| &k.0).eq(values.iter()) {
             if !nulls_first {
                 return None;
             }
@@ -760,14 +856,21 @@ impl GpuPromRewrite {
     }
 
     /// `ProjectionExec | FilterExec <- HashJoinExec(Inner, tags.. + ts)` over two `GpuPromRangeExec` -> the arguments of
-    /// `b2p_plan_binary_create`.  The join keys become `on(..)`; the projection's tag columns tell the label side.
+    /// `b2p_plan_binary_create`.  The join keys become `on(..)`; the projection's tag columns tell the label side.  Over
+    /// multi-field sides the projection holds one expression per zipped pair, min(F_l, F_r) of them, all of one operator
+    /// (planner.rs:712-777, 3401-3414); a filtering comparison over two or more pairs is refused there and stays here.
     pub fn match_binary_join(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromBinarySpec> {
-        let (expr, join_plan) = if let Some(f) = plan.as_any().downcast_ref::<FilterExec>() {
-            (f.predicate().clone(), f.input().clone())
+        let (exprs, join_plan) = if let Some(f) = plan.as_any().downcast_ref::<FilterExec>() {
+            (vec![f.predicate().clone()], f.input().clone())
         } else {
             let p = plan.as_any().downcast_ref::<ProjectionExec>()?;
-            let value = p.expr().iter().find(|e| e.expr.as_any().downcast_ref::<Column>().is_none())?;
-            (value.expr.clone(), p.input().clone())
+            let values: Vec<_> = p
+                .expr()
+                .iter()
+                .filter(|e| e.expr.as_any().downcast_ref::<Column>().is_none())
+                .map(|e| e.expr.clone())
+                .collect();
+            (values, p.input().clone())
         };
         let join = join_plan.as_any().downcast_ref::<HashJoinExec>()?;
         if *join.join_type() != JoinType::Inner || join.filter().is_some() {
@@ -775,7 +878,18 @@ impl GpuPromRewrite {
         }
         let lhs = join.left().as_any().downcast_ref::<GpuPromRangeExec>()?;
         let rhs = join.right().as_any().downcast_ref::<GpuPromRangeExec>()?;
-        let (op, _, _, return_bool) = binop_of(&expr)?;
+        let pairs = lhs.params().field_columns.len().min(rhs.params().field_columns.len());
+        let (op, _, _, return_bool) = binop_of(exprs.first()?)?;
+        for e in &exprs[1..] {
+            let (o, _, _, b) = binop_of(e)?;
+            if o != op || b != return_bool {
+                return None;
+            }
+        }
+        let filter = op.is_comparison() && !return_bool;
+        if (filter && pairs != 1) || (!filter && exprs.len() != pairs) {
+            return None;
+        }
         let mut on = Vec::new();
         let mut has_ts = false;
         for (l, r) in join.on() {
@@ -812,6 +926,9 @@ impl GpuPromRewrite {
         if let Some(u) = plan.as_any().downcast_ref::<UnionDistinctOnExec>() {
             let lhs = u.left().as_any().downcast_ref::<GpuPromRangeExec>()?;
             let rhs = u.right().as_any().downcast_ref::<GpuPromRangeExec>()?;
+            if lhs.params().field_columns.len() != 1 || rhs.params().field_columns.len() != 1 {
+                return None; // refused (planner.rs:3718-3730)
+            }
             let on = u.compare_keys().clone();
             return Some(GpuPromSetOpSpec { op: B2pSetOp::Or, lhs: lhs.params().clone(), rhs: rhs.params().clone(), on });
         }
@@ -831,6 +948,9 @@ impl GpuPromRewrite {
         }
         let lhs = distinct.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
         let rhs = join.right().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        if lhs.params().field_columns.len() != 1 {
+            return None; // refused (planner.rs:3656-3661)
+        }
         let mut on = Vec::new();
         let mut has_ts = false;
         for (l, r) in join.on() {
