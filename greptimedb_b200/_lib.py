@@ -38,6 +38,9 @@ EXPORTED_SYMBOLS = [
     "b2p_absent_dev", "b2p_absent", "b2p_plan_absent_create",
     "b2p_range_eval_fields_dev", "b2p_instant_select_fields_dev", "b2p_range_eval_fields", "b2p_instant_select_fields",
     "b2p_plan_range_create_fields", "b2p_sort_cells_fields_dev", "b2p_sort_cells_fields",
+    "b2p_instant_select_fields_i64_dev", "b2p_instant_select_fields_i64", "b2p_group_aggregate_i64_dev",
+    "b2p_group_aggregate_i64", "b2p_topk_i64_dev", "b2p_topk_i64", "b2p_count_values_i64_dev", "b2p_count_values_i64",
+    "b2p_sort_cells_i64_dev", "b2p_sort_cells_i64", "b2p_i64_to_f64_dev", "b2p_i64_to_f64",
 ]
 
 
@@ -163,6 +166,18 @@ def load() -> C.CDLL:
                                               C.POINTER(C.c_char_p), i32, C.c_char_p, C.POINTER(C.c_char_p), i32]),
         "b2p_sort_cells_fields_dev": (C.c_int, [vp, i32, vp, i32, vp, u32, u64, vp, vp]),
         "b2p_sort_cells_fields": (C.c_int, [vp, i32, vp, i32, vp, u32, u64, vp, vp]),
+        "b2p_instant_select_fields_i64_dev": (C.c_int, [vp, i64, i64, i64, i64, i64, vp, vp, vp, i32, vp, u64, u32, vp, vp]),
+        "b2p_instant_select_fields_i64": (C.c_int, [vp, i64, i64, i64, i64, i64, vp, vp, vp, i32, vp, vp, u64, u32, vp, vp]),
+        "b2p_group_aggregate_i64_dev": (C.c_int, [vp, i32, vp, vp, vp, u32, u32, u64, vp, vp]),
+        "b2p_group_aggregate_i64": (C.c_int, [vp, i32, vp, vp, vp, u32, u32, u64, vp, vp]),
+        "b2p_topk_i64_dev": (C.c_int, [vp, i32, dbl, vp, vp, vp, vp, u64, vp]),
+        "b2p_topk_i64": (C.c_int, [vp, i32, dbl, vp, vp, vp, u32, u32, vp, u64, vp]),
+        "b2p_count_values_i64_dev": (C.c_int, [vp, vp, vp, vp, u64, vp, vp]),
+        "b2p_count_values_i64": (C.c_int, [vp, vp, vp, vp, u32, u32, u64, vp, vp]),
+        "b2p_sort_cells_i64_dev": (C.c_int, [vp, i32, vp, vp, u32, u64, vp, vp]),
+        "b2p_sort_cells_i64": (C.c_int, [vp, i32, vp, vp, u32, u64, vp, vp]),
+        "b2p_i64_to_f64_dev": (C.c_int, [vp, vp, u64, vp]),
+        "b2p_i64_to_f64": (C.c_int, [vp, vp, u64, vp]),
         "b2p_plan_set_function": (C.c_int, [vp, C.c_char_p, C.POINTER(dbl), i32]),
         "b2p_plan_scalar_create": (vp, [vp, vp]),
     }

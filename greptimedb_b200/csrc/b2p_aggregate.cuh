@@ -35,9 +35,12 @@ struct GroupArgs {
 };
 
 // AGG is a compile-time constant so that the per-member fold is one or two instructions (sum / avg / count) instead
-// of a switch inside the inner loop.
-template <int AGG>
+// of a switch inside the inner loop.  I64: the cells hold Int64 (b2p_group_aggregate_i64): sum is the two's-complement
+// wrapping add (associative, so the bits do not depend on the order), min / max compare signed and write the i64 bits;
+// avg, stddev and stdvar read each value as (double)i64 and fold as for Float64.
+template <int AGG, bool I64 = false>
 __global__ void __launch_bounds__(256) group_aggregate_kernel(const GroupArgs a) {
+  constexpr bool kIntFold = I64 && (AGG == B2P_AGG_SUM || AGG == B2P_AGG_MIN || AGG == B2P_AGG_MAX);
   const int lane = threadIdx.x & 31;
   const uint64_t tiles = (a.T + 31) / 32;
   const uint64_t total = (uint64_t)a.n_groups * tiles;
@@ -58,9 +61,19 @@ __global__ void __launch_bounds__(256) group_aggregate_kernel(const GroupArgs a)
     const bool in = k < a.T;
     const uint32_t m0 = a.goff[g], m1 = a.goff[g + 1];
     double acc = 0.0, mean = 0.0, m2 = 0.0;
+    long long iacc = 0;
     uint32_t cnt = 0;
     auto fold = [&](double x) {
-      if constexpr (AGG == B2P_AGG_SUM || AGG == B2P_AGG_AVG) {
+      if constexpr (kIntFold) {
+        const long long xi = __double_as_longlong(x);
+        if constexpr (AGG == B2P_AGG_SUM) iacc = (long long)((unsigned long long)iacc + (unsigned long long)xi);
+        else if constexpr (AGG == B2P_AGG_MIN) iacc = (cnt == 0 || xi < iacc) ? xi : iacc;
+        else iacc = (cnt == 0 || xi > iacc) ? xi : iacc;
+      } else if constexpr (I64 && AGG != B2P_AGG_COUNT) {
+        x = (double)__double_as_longlong(x);
+      }
+      if constexpr (kIntFold || AGG == B2P_AGG_COUNT) {
+      } else if constexpr (AGG == B2P_AGG_SUM || AGG == B2P_AGG_AVG) {
         acc += x;
       } else if constexpr (AGG == B2P_AGG_COUNT) {
       } else if constexpr (AGG == B2P_AGG_MIN) {  // f64::total_cmp order (arrow-rs / DataFusion min, max): +NaN is greatest
@@ -107,6 +120,7 @@ __global__ void __launch_bounds__(256) group_aggregate_kernel(const GroupArgs a)
     }
     if (!in) continue;
     const size_t o = (size_t)g * a.T + k;
+    if constexpr (kIntFold) acc = __longlong_as_double(iacc);
     if (a.accumulate) {  // raw partials: SUM-type value and count
       a.out_val[o] += acc;
       a.out_cnt[o] += cnt;

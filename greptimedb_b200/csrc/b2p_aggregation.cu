@@ -32,9 +32,12 @@ uint32_t topk_ranks(double k) {
 //               34 MB at K = 10 on a 132-SM H100, whatever the input;
 //   state:      640 B per (group with a state, tile), i.e. 20 B per (group, step): multi-chunk groups, and on the
 //               general path every group of more than kk >= 33 members, so at most 0.61 B per input cell.
+// i64: the grid is Int64 (I64Key).
 int topk_run(b2p_ctx* c, int bottom, uint32_t kk, const double* vals, const uint32_t* valid, const b2p_group_index* ix,
-             const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
+             const uint32_t* tie, uint64_t T, uint32_t* out_valid, bool i64) {
   int rc;
+  auto* const chunk_kernel = i64 ? topk_chunk_kernel<I64Key> : topk_chunk_kernel<F64Key>;
+  auto* const select_kernel = i64 ? topk_select_kernel<I64Key> : topk_select_kernel<F64Key>;
   const uint32_t R = ix->n_series, G = ix->n_groups;
   const uint32_t Tw = (uint32_t)((T + 31) / 32), tiles = Tw;
   const size_t words = (size_t)R * Tw;
@@ -57,7 +60,7 @@ int topk_run(b2p_ctx* c, int bottom, uint32_t kk, const double* vals, const uint
   // slack absorbs the rounding of the chunk counts), and at least 256 members
   const size_t smem = kTopkWarps * topk_warp_bytes(K);
   unsigned cap = 0;
-  if ((rc = persistent_grid(c, topk_chunk_kernel, smem, kTopkWarps, kAllResident, &cap))) return rc;
+  if ((rc = persistent_grid(c, chunk_kernel, smem, kTopkWarps, kAllResident, &cap))) return rc;
   const uint64_t resident = (uint64_t)cap * kTopkWarps;
   const uint64_t U = resident - resident / 8;
   const uint64_t C = std::max<uint64_t>(256, ((uint64_t)in_groups * tiles + U - 1) / U);
@@ -106,12 +109,12 @@ int topk_run(b2p_ctx* c, int bottom, uint32_t kk, const double* vals, const uint
   a.out_valid = out_valid;
   const uint64_t chunk_units = (uint64_t)chunks.size() * tiles, merge_units = (uint64_t)merges.size() * tiles;
   unsigned g_chunk = 0, g_merge = 0, g_mark = 0;
-  if ((rc = persistent_grid(c, topk_chunk_kernel, smem, kTopkWarps, chunk_units, &g_chunk))) return rc;
+  if ((rc = persistent_grid(c, chunk_kernel, smem, kTopkWarps, chunk_units, &g_chunk))) return rc;
   if (merge_units && (rc = persistent_grid(c, topk_merge_kernel, smem, kTopkWarps, merge_units, &g_merge))) return rc;
   const uint32_t rounds = general ? (kk + kTopkMax - 1) / kTopkMax : 1;
   for (uint32_t r = 0; r < rounds; ++r) {
     a.round = (int)r;
-    topk_chunk_kernel<<<g_chunk, kTopkWarps * 32, smem, c->stream>>>(a);
+    chunk_kernel<<<g_chunk, kTopkWarps * 32, smem, c->stream>>>(a);
     c->launches++;
     CU(cudaGetLastError());
     if (merge_units) {
@@ -121,7 +124,7 @@ int topk_run(b2p_ctx* c, int bottom, uint32_t kk, const double* vals, const uint
     }
   }
   if (general) {
-    topk_select_kernel<<<capped_grid(c, chunk_units, 8, 16), 256, 0, c->stream>>>(a);
+    select_kernel<<<capped_grid(c, chunk_units, 8, 16), 256, 0, c->stream>>>(a);
   } else if (merge_units) {
     if ((rc = persistent_grid(c, topk_mark_kernel, 0, kTopkWarps, chunk_units, &g_mark))) return rc;
     topk_mark_kernel<<<g_mark, kTopkWarps * 32, 0, c->stream>>>(a);
@@ -234,8 +237,9 @@ struct CvBatch {
 // the key buffer once the sort has left it), so at most 20 B x kCvBatchCells = 2.7 GB unless one group alone has more
 // than kCvBatchCells / 32 = 4.2 M members (then 20 B x its members x 32); 8 B per (group, step) of a batch; 4 B per
 // in-range row; CUB's temp storage for the sort and the scan.
+// i64: the grid is Int64 (I64Key), and so are the distinct values out_val receives.
 int count_values_run(b2p_ctx* c, const double* vals, const uint32_t* valid, const b2p_group_index* ix, uint64_t T,
-                     double* out_val, uint32_t* out_cnt) {
+                     double* out_val, uint32_t* out_cnt, bool i64) {
   int rc;
   const uint32_t R = ix->n_series, G = ix->n_groups, Tw = (uint32_t)((T + 31) / 32);
   const uint32_t in_rows = G ? ix->goff_host[G] : 0u;
@@ -295,7 +299,7 @@ int count_values_run(b2p_ctx* c, const double* vals, const uint32_t* valid, cons
     const unsigned cell_grid = capped_grid(c, b.cells, 256, 8);
     count_values_segments_kernel<<<capped_grid(c, b.segments, 256, 8), 256, 0, c->stream>>>(a);
     const uint64_t tiles = (uint64_t)((a.m1 - a.m0 + 31) / 32) * ((b.W + 31) / 32);
-    count_values_scatter_kernel<<<capped_grid(c, tiles, 1, 8), 256, 0, c->stream>>>(a);
+    (i64 ? count_values_scatter_kernel<I64Key> : count_values_scatter_kernel<F64Key>)<<<capped_grid(c, tiles, 1, 8), 256, 0, c->stream>>>(a);
     c->launches += 2;
     CU(cudaGetLastError());
     cub::DoubleBuffer<unsigned long long> db(c->v_keys.as<unsigned long long>(), c->v_alt.as<unsigned long long>());
@@ -309,7 +313,7 @@ int count_values_run(b2p_ctx* c, const double* vals, const uint32_t* valid, cons
     CU(cudaGetLastError());
     bytes = c->v_tmp.cap;
     CU(cub::DeviceScan::InclusiveSum(c->v_tmp.p, bytes, a.rank, a.rank, (int)b.cells, c->stream));
-    count_values_rank_kernel<<<cell_grid, 256, 0, c->stream>>>(a);
+    (i64 ? count_values_rank_kernel<I64Key> : count_values_rank_kernel<F64Key>)<<<cell_grid, 256, 0, c->stream>>>(a);
     count_values_count_kernel<<<cell_grid, 256, 0, c->stream>>>(a);
     c->launches += 2;
     CU(cudaGetLastError());
@@ -330,6 +334,63 @@ int end_indexed(Staging& s, const uint32_t* gid, uint32_t n_rows, uint32_t n_gro
   b2p_group_index_destroy(s.c, ix);
   return rc;
 }
+
+// The device and host forms of topk / bottomk and count_values; i64: the grid is Int64
+int topk_dev(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uint32_t* valid, const b2p_group_index* ix,
+             const uint32_t* tie, uint64_t T, uint32_t* out_valid, bool i64) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_series == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !tie || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  const int rc = topk_run(c, bottom, topk_ranks(k), vals, valid, ix, tie, T, out_valid, i64);
+  stage_end(c, 3);
+  return rc;
+}
+
+int topk_host(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uint32_t* valid, const uint32_t* gid,
+              uint32_t n_rows, uint32_t n_groups, const uint32_t* tie, uint64_t T, uint32_t* out_valid, bool i64) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_rows == 0 || T == 0) return B2P_OK;  // (no group index to build)
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
+  uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
+  const uint32_t* d_tie = s.in(tie, (size_t)n_rows * 4);
+  uint32_t* d_out = s.copy_back(out_valid, d_valid, (size_t)n_rows * Tw * 4);  // topk runs in place
+  return end_indexed(s, gid, n_rows, n_groups, [&](const b2p_group_index* ix) {
+    return topk_dev(c, bottom, k, d_vals, d_valid, ix, d_tie, T, d_out, i64);
+  });
+}
+
+int count_values_dev(b2p_ctx* c, const double* vals, const uint32_t* valid, const b2p_group_index* ix, uint64_t T,
+                     double* out_val, uint32_t* out_cnt, bool i64) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_series == 0 || T == 0) return B2P_OK;
+  if (!vals || !valid || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  const int rc = count_values_run(c, vals, valid, ix, T, out_val, out_cnt, i64);
+  stage_end(c, 3);
+  return rc;
+}
+
+int count_values_host(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* gid, uint32_t n_rows,
+                      uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt, bool i64) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_rows == 0 || T == 0) return B2P_OK;  // (no group index to build)
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
+  double* d_out = s.out(out_val, (size_t)n_rows * T * 8);
+  uint32_t* d_cnt = s.out(out_cnt, (size_t)n_rows * T * 4);
+  return end_indexed(s, gid, n_rows, n_groups, [&](const b2p_group_index* ix) {
+    return count_values_dev(c, d_vals, d_valid, ix, T, d_out, d_cnt, i64);
+  });
+}
 }  // namespace
 
 extern "C" {
@@ -338,14 +399,12 @@ extern "C" {
 
 int b2p_topk_dev(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uint32_t* valid,
                  const b2p_group_index* ix, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
-  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
-  if (ix->n_series == 0 || T == 0) return B2P_OK;
-  if (!vals || !valid || !tie || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
-  DeviceGuard g(c->device);
-  stage_begin(c, 3);
-  const int rc = topk_run(c, bottom, topk_ranks(k), vals, valid, ix, tie, T, out_valid);
-  stage_end(c, 3);
-  return rc;
+  return topk_dev(c, bottom, k, vals, valid, ix, tie, T, out_valid, false);
+}
+
+int b2p_topk_i64_dev(b2p_ctx* c, int32_t bottom, double k, const int64_t* vals, const uint32_t* valid,
+                     const b2p_group_index* ix, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
+  return topk_dev(c, bottom, k, reinterpret_cast<const double*>(vals), valid, ix, tie, T, out_valid, true);
 }
 
 /* ---- quantile ------------------------------------------------------------------------------------------------ */
@@ -366,32 +425,26 @@ int b2p_group_quantile_dev(b2p_ctx* c, double phi, const double* vals, const uin
 
 int b2p_count_values_dev(b2p_ctx* c, const double* vals, const uint32_t* valid, const b2p_group_index* ix, uint64_t T,
                          double* out_val, uint32_t* out_cnt) {
-  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
-  if (ix->n_series == 0 || T == 0) return B2P_OK;
-  if (!vals || !valid || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
-  DeviceGuard g(c->device);
-  stage_begin(c, 3);
-  const int rc = count_values_run(c, vals, valid, ix, T, out_val, out_cnt);
-  stage_end(c, 3);
-  return rc;
+  return count_values_dev(c, vals, valid, ix, T, out_val, out_cnt, false);
+}
+
+int b2p_count_values_i64_dev(b2p_ctx* c, const int64_t* vals, const uint32_t* valid, const b2p_group_index* ix,
+                             uint64_t T, int64_t* out_val, uint32_t* out_cnt) {
+  return count_values_dev(c, reinterpret_cast<const double*>(vals), valid, ix, T, reinterpret_cast<double*>(out_val),
+                          out_cnt, true);
 }
 
 /* ---- host-pointer API ------------------------------------------------------------------------ */
 
 int b2p_topk(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uint32_t* valid, const uint32_t* gid,
              uint32_t n_rows, uint32_t n_groups, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
-  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  if (n_rows == 0 || T == 0) return B2P_OK;  // (no group index to build)
-  DeviceGuard g(c->device);
-  const size_t Tw = (size_t)((T + 31) / 32);
-  Staging s{c};
-  const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
-  uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
-  const uint32_t* d_tie = s.in(tie, (size_t)n_rows * 4);
-  uint32_t* d_out = s.copy_back(out_valid, d_valid, (size_t)n_rows * Tw * 4);  // topk runs in place
-  return end_indexed(s, gid, n_rows, n_groups, [&](const b2p_group_index* ix) {
-    return b2p_topk_dev(c, bottom, k, d_vals, d_valid, ix, d_tie, T, d_out);
-  });
+  return topk_host(c, bottom, k, vals, valid, gid, n_rows, n_groups, tie, T, out_valid, false);
+}
+
+int b2p_topk_i64(b2p_ctx* c, int32_t bottom, double k, const int64_t* vals, const uint32_t* valid, const uint32_t* gid,
+                 uint32_t n_rows, uint32_t n_groups, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
+  return topk_host(c, bottom, k, reinterpret_cast<const double*>(vals), valid, gid, n_rows, n_groups, tie, T, out_valid,
+                   true);
 }
 
 int b2p_group_quantile(b2p_ctx* c, double phi, const double* vals, const uint32_t* valid, const uint32_t* gid,
@@ -412,18 +465,13 @@ int b2p_group_quantile(b2p_ctx* c, double phi, const double* vals, const uint32_
 
 int b2p_count_values(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* gid, uint32_t n_rows,
                      uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
-  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
-  if (n_rows == 0 || T == 0) return B2P_OK;  // (no group index to build)
-  DeviceGuard g(c->device);
-  const size_t Tw = (size_t)((T + 31) / 32);
-  Staging s{c};
-  const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
-  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
-  double* d_out = s.out(out_val, (size_t)n_rows * T * 8);
-  uint32_t* d_cnt = s.out(out_cnt, (size_t)n_rows * T * 4);
-  return end_indexed(s, gid, n_rows, n_groups, [&](const b2p_group_index* ix) {
-    return b2p_count_values_dev(c, d_vals, d_valid, ix, T, d_out, d_cnt);
-  });
+  return count_values_host(c, vals, valid, gid, n_rows, n_groups, T, out_val, out_cnt, false);
+}
+
+int b2p_count_values_i64(b2p_ctx* c, const int64_t* vals, const uint32_t* valid, const uint32_t* gid, uint32_t n_rows,
+                         uint32_t n_groups, uint64_t T, int64_t* out_val, uint32_t* out_cnt) {
+  return count_values_host(c, reinterpret_cast<const double*>(vals), valid, gid, n_rows, n_groups, T,
+                           reinterpret_cast<double*>(out_val), out_cnt, true);
 }
 
 }  // extern "C"

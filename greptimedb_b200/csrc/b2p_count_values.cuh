@@ -14,7 +14,8 @@
 // value) (planner.rs:402-445).  DataFusion groups a Float64 by its bits (so -0.0 and +0.0, or two NaN payloads, are two
 // values) and arrow sorts it in the f64 total order; the 64-bit key u = total_key(v) ^ 2^63 is both: two cells share a
 // key iff they share their bits, and keys order as the total order does.  The result per (group, step) is its distinct
-// keys ascending with their multiplicities: row goff[g] + j of out_val / out_cnt holds the j-th, out_cnt 0 past the
+// keys ascending with their multiplicities (an Int64 grid, b2p_count_values_i64, keys on its bits ^ 2^63 instead, I64Key:
+// the two kernels that read or write values take the key as a template parameter): row goff[g] + j of out_val / out_cnt holds the j-th, out_cnt 0 past the
 // last.  A group has at most as many distinct values at a step as members, so the output is the input's size.
 //
 // A segment is the (group, step) column of a batch's key buffer: the group's cells at a step, one per member position
@@ -24,7 +25,7 @@
 #pragma once
 #include <cstdint>
 
-#include "b2p_quantile.cuh"  // quant_key / quant_value: the unsigned total-order key and its inverse
+#include "b2p_quantile.cuh"  // (and through it F64Key / I64Key: the unsigned order keys and their inverses)
 
 namespace b2p {
 
@@ -68,6 +69,7 @@ __global__ void __launch_bounds__(256) count_values_segments_kernel(const CvArgs
 // member row at a time (32 steps, one coalesced load per warp and member; the member ids and validity words are read
 // once per member), transposed through shared memory and written a step at a time (32 consecutive member positions of
 // one group are 32 consecutive keys of the segment).
+template <class Key = F64Key>
 __global__ void __launch_bounds__(256) count_values_scatter_kernel(const CvArgs a) {
   __shared__ unsigned long long sk[32][33];
   __shared__ uint32_t son[32];
@@ -90,7 +92,7 @@ __global__ void __launch_bounds__(256) count_values_scatter_kernel(const CvArgs 
         const uint32_t row = __ldg(a.members + m);
         const uint32_t w = __ldg(a.valid + (uint64_t)row * a.Tw + tile);
         on = live && ((w >> lane) & 1u);
-        if (on) key = quant_key(__ldg(a.vals + (uint64_t)row * a.T + k));
+        if (on) key = Key::key(__ldg(a.vals + (uint64_t)row * a.T + k));
       }
       sk[ml][lane] = key;
       const uint32_t bits = __ballot_sync(0xFFFFFFFFu, on);
@@ -143,13 +145,14 @@ __device__ __forceinline__ uint32_t cv_before(const CvArgs& a, uint32_t s) {
   return o ? a.rank[o - 1] : 0u;
 }
 
+template <class Key = F64Key>
 __global__ void __launch_bounds__(256) count_values_rank_kernel(const CvArgs a) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.cells; i += gridDim.x * blockDim.x) {
     uint32_t g, kk, j, s;
     if (!cv_head(a, i, g, kk, j, s)) continue;
     const uint32_t r = a.rank[i] - cv_before(a, s) - 1;  // the distinct key's rank in its segment
     const uint32_t row = __ldg(a.goff + g) + r;
-    a.out_val[(uint64_t)row * a.T + a.k0 + kk] = quant_value(a.sorted[i]);
+    a.out_val[(uint64_t)row * a.T + a.k0 + kk] = Key::value(a.sorted[i]);
     a.start[(uint64_t)(row - a.m0) * a.W + kk] = j;
   }
 }

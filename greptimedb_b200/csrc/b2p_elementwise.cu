@@ -279,6 +279,19 @@ int b2p_count_valid_words_dev(b2p_ctx* c, const uint32_t* cnt, uint64_t n_rows, 
   return B2P_OK;
 }
 
+/* ---- Int64 -> Float64 ------------------------------------------------------------------------------------------ */
+
+int b2p_i64_to_f64_dev(b2p_ctx* c, const int64_t* vals, uint64_t n, double* out) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n == 0) return B2P_OK;
+  if (!vals || !out) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  i64_to_f64_kernel<<<capped_grid(c, n, 256, 16), 256, 0, c->stream>>>(reinterpret_cast<const long long*>(vals), n, out);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
 /* ---- instant-vector functions and scalar() --------------------------------------------------------------------- */
 
 int b2p_instant_fn_dev(b2p_ctx* c, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,
@@ -440,6 +453,15 @@ int b2p_instant_fn(b2p_ctx* c, int32_t fn, double arg0, double arg1, const doubl
   double* d_out = s.copy_back(out, d_vals, vb);
   uint32_t* d_out_valid = out_valid == valid ? d_valid : s.copy_back(out_valid, d_valid, wb);
   return s.end([&] { return b2p_instant_fn_dev(c, fn, arg0, arg1, d_vals, d_valid, n_rows, T, d_out, d_out_valid); });
+}
+
+int b2p_i64_to_f64(b2p_ctx* c, const int64_t* vals, uint64_t n, double* out) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  DeviceGuard g(c->device);
+  Staging s{c};
+  int64_t* d = s.in(vals, (size_t)n * 8);
+  double* d_out = s.copy_back(out, reinterpret_cast<double*>(d), (size_t)n * 8);  // in place
+  return s.end([&] { return b2p_i64_to_f64_dev(c, d, n, d_out); });
 }
 
 int b2p_scalar_calculate(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* row_key,

@@ -59,7 +59,10 @@ struct FieldsInstantArgs {
   double* outs[kMaxFields];        // [n_series x T] per field
 };
 
-// K4 (instant_kernel) with F gathers: warp per series, lane per eval step.
+// K4 (instant_kernel) with F gathers: warp per series, lane per eval step.  STALE_TEST = false when field 0 is Int64
+// (b2p_instant_select_fields_i64): the reference looks for stale NaNs through a Float64 downcast only
+// (instant_manipulate.rs:490-527), so an Int64 field 0 is never tested, even where its bits are a NaN double.
+template <bool STALE_TEST = true>
 __global__ void __launch_bounds__(kWarpsPerCta * 32) instant_fields_kernel(const __grid_constant__ FieldsInstantArgs fa) {
   const InstantArgs& a = fa.g;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -100,7 +103,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) instant_fields_kernel(const
           if (t == te)
             while (j > 0 && ts[j - 1] + a.offset == te) --j;
           const bool fresh = (a.lookback > 0) ? (t + a.lookback > te) : (t == te);
-          if (fresh && !isnan(fa.vals[0][row0 + j])) {  // the staleness test reads field 0 alone
+          if (fresh && !(STALE_TEST && isnan(fa.vals[0][row0 + j]))) {  // the staleness test reads field 0 alone
             ok = true;
             row = row0 + j;
           }

@@ -33,10 +33,11 @@ int build_group_csr(b2p_ctx* c, const uint32_t* gid, uint32_t n_series, uint32_t
   return B2P_OK;
 }
 
-// accumulate = 1 (SUM / COUNT partials only): out_val / out_cnt are added to instead of overwritten
+// accumulate = 1 (SUM / COUNT partials only, Float64 only): out_val / out_cnt are added to instead of overwritten;
+// i64: the cells hold Int64
 int group_aggregate_csr(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* goff,
                         const uint32_t* members, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt,
-                        int accumulate, double* out_mean) {
+                        int accumulate, double* out_mean, bool i64) {
   GroupArgs a{};
   a.out_mean = out_mean;
   a.agg = agg; a.vals = vals; a.valid = valid_words; a.goff = goff;
@@ -44,7 +45,8 @@ int group_aggregate_csr(b2p_ctx* c, int32_t agg, const double* vals, const uint3
   a.out_val = out_val; a.out_cnt = out_cnt; a.accumulate = accumulate;
   const unsigned blocks = capped_grid(c, (uint64_t)n_groups * ((T + 31) / 32), 8, 32);
   return with_id<B2P_AGG_STDVAR + 1>(agg, "aggregator", [&](auto k) {
-    group_aggregate_kernel<decltype(k)::value><<<blocks, 256, 0, c->stream>>>(a);
+    if (i64) group_aggregate_kernel<decltype(k)::value, true><<<blocks, 256, 0, c->stream>>>(a);
+    else group_aggregate_kernel<decltype(k)::value><<<blocks, 256, 0, c->stream>>>(a);
     c->launches++;
     CU(cudaGetLastError());
     return B2P_OK;
@@ -54,7 +56,7 @@ int group_aggregate_csr(b2p_ctx* c, int32_t agg, const double* vals, const uint3
 namespace {
 int group_aggregate_impl(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* gid,
                          uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt,
-                         int accumulate, double* out_mean = nullptr) {
+                         int accumulate, double* out_mean = nullptr, bool i64 = false) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   if (agg < 0 || agg > B2P_AGG_STDVAR) return fail(B2P_E_INVALID, "unknown aggregator %d", agg);
   if (n_groups == 0 || T == 0) return B2P_OK;
@@ -67,7 +69,7 @@ int group_aggregate_impl(b2p_ctx* c, int32_t agg, const double* vals, const uint
   stage_begin(c, 3);
   if ((rc = build_group_csr(c, gid, n_series, n_groups, c->g_goff.as<uint32_t>(), c->g_vals_out.as<uint32_t>()))) return rc;
   rc = group_aggregate_csr(c, agg, vals, valid_words, c->g_goff.as<uint32_t>(), c->g_vals_out.as<uint32_t>(), n_groups, T,
-                           out_val, out_cnt, accumulate, out_mean);
+                           out_val, out_cnt, accumulate, out_mean, i64);
   stage_end(c, 3);
   return rc;
 }
@@ -79,6 +81,13 @@ int b2p_group_aggregate_dev(b2p_ctx* c, int32_t agg, const double* vals, const u
                             const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val,
                             uint32_t* out_cnt) {
   return group_aggregate_impl(c, agg, vals, valid_words, gid, n_series, n_groups, T, out_val, out_cnt, 0);
+}
+
+int b2p_group_aggregate_i64_dev(b2p_ctx* c, int32_t agg, const int64_t* vals, const uint32_t* valid_words,
+                                const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val,
+                                uint32_t* out_cnt) {
+  return group_aggregate_impl(c, agg, reinterpret_cast<const double*>(vals), valid_words, gid, n_series, n_groups, T,
+                              out_val, out_cnt, 0, nullptr, true);
 }
 
 int b2p_group_aggregate_partial_dev(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words,
@@ -308,8 +317,9 @@ int b2p_column_reduce_dev(b2p_ctx* c, const double* const* cols, uint32_t n_cols
 
 /* ---- host-pointer API ------------------------------------------------------------------------ */
 
-int b2p_group_aggregate(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* gid,
-                        uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
+namespace {
+int group_aggregate_host(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* gid,
+                         uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt, bool i64) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   DeviceGuard g(c->device);
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
@@ -320,8 +330,21 @@ int b2p_group_aggregate(b2p_ctx* c, int32_t agg, const double* vals, const uint3
   double* d_out = s.out(out_val, (size_t)n_groups * T * 8);
   uint32_t* d_cnt = s.out(out_cnt, (size_t)n_groups * T * 4);
   return s.end([&] {
-    return b2p_group_aggregate_dev(c, agg, d_vals, d_valid, d_gid, n_series, n_groups, T, d_out, d_cnt);
+    return group_aggregate_impl(c, agg, d_vals, d_valid, d_gid, n_series, n_groups, T, d_out, d_cnt, 0, nullptr, i64);
   });
+}
+}  // namespace
+
+int b2p_group_aggregate(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* gid,
+                        uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
+  return group_aggregate_host(c, agg, vals, valid_words, gid, n_series, n_groups, T, out_val, out_cnt, false);
+}
+
+int b2p_group_aggregate_i64(b2p_ctx* c, int32_t agg, const int64_t* vals, const uint32_t* valid_words,
+                            const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val,
+                            uint32_t* out_cnt) {
+  return group_aggregate_host(c, agg, reinterpret_cast<const double*>(vals), valid_words, gid, n_series, n_groups, T,
+                              out_val, out_cnt, true);
 }
 
 int b2p_histogram_quantile(b2p_ctx* c, double phi, const double* le, uint32_t n_buckets, const double* rates,

@@ -4,6 +4,8 @@
 //                                    clamp with one bound at ∓f64::MAX, chosen by the caller)
 //      scalar_reduce_kernel          scalar(): live rows, their min / max series key, live cells on B2P_NO_KEY rows
 //      scalar_write_kernel           scalar(): the one series' cells, or NaN at every step
+//      i64_to_f64_kernel             an Int64 grid read as Float64 ((double)i64, round to nearest): what DataFusion's
+//                                    coercion does before a Float64 projection, aggregate or filter of an Int64 column
 //
 // The reference projects the function over the value column and then filters `value IS NOT NULL`
 // (src/query/src/promql/planner.rs:1012-1101, 1063).  A function of a non-null f64 is never null, so validity never
@@ -222,6 +224,12 @@ __global__ void __launch_bounds__(256) scalar_write_kernel(const ScalarArgs a) {
     if (k < a.T) a.out[k] = ((word >> lane) & 1u) ? x : 0.0;
     if (lane == 0) a.out_valid[w] = word;
   }
+}
+
+// thread per cell; out may be vals
+__global__ void __launch_bounds__(256) i64_to_f64_kernel(const long long* vals, uint64_t n, double* out) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+    out[i] = __ll2double_rn(vals[i]);
 }
 
 }  // namespace b2p

@@ -42,6 +42,13 @@ bool starts_with(const char* s, const char* p) { return std::strncmp(s, p, std::
 
 bool bit_set(const uint8_t* bits, int64_t i) { return bits == nullptr || ((bits[i >> 3] >> (i & 7)) & 1); }
 
+// an Int64 cell's value: the int64_t whose bits the grid's 8-byte slot holds
+int64_t bits_i64(double v) {
+  int64_t b;
+  std::memcpy(&b, &v, sizeof b);
+  return b;
+}
+
 constexpr int64_t kArrowFlagNullable = 2;  // ARROW_FLAG_NULLABLE of the C Data Interface
 
 // Throws the PlanError of a failed b2p_* call, with the call's message: arguments the call rejects (B2P_E_INVALID,
@@ -50,6 +57,18 @@ void check(int rc, ErrorKind invalid = ErrorKind::Plan) {
   if (rc == B2P_OK) return;
   if (rc == B2P_E_INVALID || rc == B2P_E_TOO_LARGE) throw PlanError(invalid, b2p_last_error());
   throw PlanError(rc == B2P_E_UNSORTED ? ErrorKind::Internal : ErrorKind::Execution, b2p_last_error());
+}
+
+// Field f of r read as Float64 from here on: an Int64 field is coerced on the device ((double)i64, b2p_i64_to_f64), as
+// DataFusion coerces an Int64 column under a Float64 projection, aggregate or scalar()
+void field_to_f64(b2p_ctx* ctx, NodeResult& r, uint32_t f) {
+  if (!r.is_i64(f)) return;
+  if (r.grid() > 0) check(b2p_i64_to_f64(ctx, reinterpret_cast<const int64_t*>(r.field(f)), r.grid(), r.field(f)));
+  r.types[f] = ValueType::Float64;
+}
+void to_f64(b2p_ctx* ctx, NodeResult& r) {
+  for (uint32_t f = 0; f < r.F; ++f) field_to_f64(ctx, r, f);
+  r.types.clear();
 }
 
 // dense ids of keys, in first-insertion order
@@ -301,15 +320,29 @@ void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& 
   const size_t T = (size_t)r.T;
   std::vector<double> gval((size_t)F * G * T);
   std::vector<uint32_t> gcnt((size_t)G * T), fcnt(F > 1 ? (size_t)G * T : 0);
-  for (uint32_t f = 0; f < F && G > 0 && T > 0; ++f) {
+  // an Int64 field stays Int64 under sum, min and max (DataFusion's Int64 accumulators); the others give Float64
+  const bool int_result = op == B2P_AGG_SUM || op == B2P_AGG_MIN || op == B2P_AGG_MAX;
+  std::vector<ValueType> types;
+  for (uint32_t f = 0; f < F; ++f) {
+    const bool i64 = r.is_i64(f) && op != kAggQuantile && op != kAggGroup;
+    if (r.is_i64(f) && op == kAggQuantile) field_to_f64(ctx, r, f);
+    if (int_result && r.is_i64(f)) {
+      types.resize(F, ValueType::Float64);
+      types[f] = ValueType::Int64;
+    }
+    if (G == 0 || T == 0) continue;
     double* gv = gval.data() + (size_t)f * G * T;
     uint32_t* gc = f == 0 ? gcnt.data() : fcnt.data();
+    const int agg = op == kAggGroup ? B2P_AGG_COUNT : op;
     check(op == kAggQuantile ? b2p_group_quantile(ctx, param, r.field(f), r.valid.data(), groups.id.data(), r.rows, G,
                                                   (uint64_t)T, gv, gc)
-                             : b2p_group_aggregate(ctx, op == kAggGroup ? B2P_AGG_COUNT : op, r.field(f),
-                                                   r.valid.data(), groups.id.data(), r.rows, G, (uint64_t)T, gv, gc),
+          : i64 ? b2p_group_aggregate_i64(ctx, agg, reinterpret_cast<const int64_t*>(r.field(f)), r.valid.data(),
+                                          groups.id.data(), r.rows, G, (uint64_t)T, gv, gc)
+                : b2p_group_aggregate(ctx, agg, r.field(f), r.valid.data(), groups.id.data(), r.rows, G, (uint64_t)T,
+                                      gv, gc),
           ErrorKind::Execution);
   }
+  r.types = std::move(types);
   r.labels = std::move(groups.labels);
   r.columns = Columns::TagsTimeValue;
   r.cell_order.clear();
@@ -433,9 +466,19 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
   const char* tfmt = b.field(ti).format;
   if (!(starts_with(tfmt, "tsm:") || std::strcmp(tfmt, "l") == 0))
     throw PlanError(ErrorKind::Execution, "Time index Column downcast to TimestampMillisecondArray failed");
-  for (size_t f = 0; f < F; ++f)
-    if (std::strcmp(b.field(fi[f]).format, "g") != 0)
+  // Float64, or for the instant selector Int64 (BIGINT): its cells are copied as they are, and read as integers by the
+  // nodes above.  A range function over an Int64 column stays on the CPU.
+  std::vector<ValueType> types(F);
+  for (size_t f = 0; f < F; ++f) {
+    const char* fmt = b.field(fi[f]).format;
+    const bool int_ok = fn_id_ < 0 && !args_.histogram && agg_id_ < 0;
+    if (std::strcmp(fmt, "g") != 0 && !(int_ok && std::strcmp(fmt, "l") == 0))
       throw PlanError(ErrorKind::Execution, "field column " + args_.field_columns[f] + " is not Float64");
+    types[f] = fmt[0] == 'l' ? ValueType::Int64 : ValueType::Float64;
+  }
+  if (types_.empty()) types_ = types;
+  if (types != types_)
+    throw PlanError(ErrorKind::Execution, "GpuPromRangeExec: a field column changed its type between batches");
   const ArrowArray& ta = b.column(ti);
   const int64_t* tsv = static_cast<const int64_t*>(ta.buffers[1]) + ta.offset + b.offset();
 
@@ -489,15 +532,16 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
     const uint8_t* fvalid = fa.null_count != 0 ? static_cast<const uint8_t*>(fa.buffers[0]) : nullptr;
     std::vector<double>& v = val_[f];
     v.insert(v.end(), fv, fv + n);
-    if (F == 1) {
+    if (F == 1 && types_[0] == ValueType::Float64) {
       if (fvalid) {  // a NULL field value cannot be inside a window: treat it like the NaN the filter drops
         for (int64_t row = 0; row < n; ++row)
           if (!bit_set(fvalid, base + row)) v[row_base + (size_t)row] = std::nan("");
       }
       continue;
     }
-    // several fields: the device decides per function what a NULL slot means (b2p_range_eval_fields), so the slots go
-    // down as one bitmap per field, rows from bit 0; a field without a NULL so far has none
+    // several fields, or an Int64 field: the device decides per function what a NULL slot means
+    // (b2p_range_eval_fields), so the slots go down as one bitmap per field, rows from bit 0; a field without a NULL so
+    // far has none
     std::vector<uint8_t>& bits = present_[f];
     if (!fvalid && bits.empty()) continue;
     const size_t total = row_base + (size_t)n;
@@ -581,13 +625,14 @@ void PromRangePlan::compute(NodeResult& r) {
   const size_t cells = (size_t)S * (size_t)T;
   std::vector<double> dense(fold_on_device ? 0 : F * cells);
   std::vector<uint32_t> valid(fold_on_device ? 0 : (size_t)S * Tw);
-  if (S > 0 && T > 0 && !fold_on_device && F == 1)
+  const bool int0 = !types_.empty() && types_[0] == ValueType::Int64;  // (only the instant selector takes Int64)
+  if (S > 0 && T > 0 && !fold_on_device && F == 1 && !int0)
     check(fn_id_ >= 0 ? b2p_range_eval(ctx_, &p, ts_.data(), val_[0].data(), nullptr, offsets_.data(), ts_.size(), S,
                                        dense.data(), valid.data(), nullptr)
                       : b2p_instant_select(ctx_, p.start, p.end, p.interval, args_.lookback_delta, p.offset, ts_.data(),
                                            val_[0].data(), nullptr, offsets_.data(), ts_.size(), S, dense.data(),
                                            valid.data()));  // InstantManipulate
-  if (S > 0 && T > 0 && F > 1) {
+  if (S > 0 && T > 0 && (F > 1 || int0)) {
     std::vector<const double*> vals(F);
     std::vector<double*> outs(F);
     std::vector<const uint8_t*> present(F);
@@ -602,6 +647,9 @@ void PromRangePlan::compute(NodeResult& r) {
     const uint8_t* const* nulls = any_null ? present.data() : nullptr;
     check(fn_id_ >= 0 ? b2p_range_eval_fields(ctx_, &p, ts_.data(), vals.data(), nulls, (int32_t)F, nullptr,
                                               offsets_.data(), ts_.size(), S, outs.data(), valid.data())
+          : int0      ? b2p_instant_select_fields_i64(ctx_, p.start, p.end, p.interval, args_.lookback_delta, p.offset,
+                                                      ts_.data(), vals.data(), nulls, (int32_t)F, nullptr,
+                                                      offsets_.data(), ts_.size(), S, outs.data(), valid.data())
                       : b2p_instant_select_fields(ctx_, p.start, p.end, p.interval, args_.lookback_delta, p.offset,
                                                   ts_.data(), vals.data(), nulls, (int32_t)F, nullptr, offsets_.data(),
                                                   ts_.size(), S, outs.data(), valid.data()));
@@ -613,6 +661,7 @@ void PromRangePlan::compute(NodeResult& r) {
   r.eval_ts.resize((size_t)T);  // also when there are no series: scalar() of such a node has a NaN row at every step
   for (int64_t k = 0; k < T; ++k) r.eval_ts[(size_t)k] = p.start + k * p.interval;
   r.time_index = args_.time_index;
+  if (std::find(types_.begin(), types_.end(), ValueType::Int64) != types_.end()) r.types = types_;
   for (const std::string& field : args_.field_columns)
     r.value_names.push_back(fn_id_ >= 0 ? args_.function + "(" + args_.time_index + "_range," + field + ")" : field);
 
@@ -696,8 +745,8 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
   OwnedColumn* c_label = nullptr;    // count_values' counted value
   const bool int_val = r.columns == Columns::CountTagsTimeLabel && r.value_is_count;
   if (r.value_names.size() != r.F) throw PlanError(ErrorKind::Internal, "export: one value name per field expected");
-  auto add_vals = [&](const char* fmt) {
-    for (const std::string& name : r.value_names) c_vals.push_back(add_col(name, fmt));
+  auto add_vals = [&](const char* fmt) {  // "g" is each field's own type
+    for (uint32_t f = 0; f < r.F; ++f) c_vals.push_back(add_col(r.value_names[f], r.is_i64(f) ? "l" : fmt));
   };
   switch (r.columns) {
     case Columns::TimeValueTags:
@@ -719,7 +768,7 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       add_vals(int_val ? "l" : "g");
       for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
       c_ts = add_col(r.time_index, "tsm:");
-      c_label = add_col(r.label_name, "g");
+      c_label = add_col(r.label_name, r.label_is_i64 ? "l" : "g");
       break;
     case Columns::TimeSorted: {  // (`or`, one field)
       c_ts = add_col(r.time_index, "tsm:");
@@ -727,7 +776,7 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       names.push_back(r.value_names[0]);
       std::sort(names.begin(), names.end());
       for (const std::string& name : names) {
-        if (name == r.value_names[0] && c_vals.empty()) c_vals.push_back(add_col(name, "g"));
+        if (name == r.value_names[0] && c_vals.empty()) c_vals.push_back(add_col(name, r.is_i64(0) ? "l" : "g"));
         else add_tag((size_t)L.column(name));
       }
       break;
@@ -747,9 +796,14 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     for (uint32_t f = 0; f < r.F; ++f) {
       const double v = r.field(f)[(size_t)row * (size_t)r.T + (size_t)k];
       if (int_val) c_vals[f]->i64.push_back((int64_t)v);
+      else if (r.is_i64(f)) c_vals[f]->i64.push_back(bits_i64(v));
       else c_vals[f]->f64.push_back(v);
     }
-    if (c_label) c_label->f64.push_back(r.label_val[(size_t)row * (size_t)r.T + (size_t)k]);
+    if (c_label) {
+      const double v = r.label_val[(size_t)row * (size_t)r.T + (size_t)k];
+      if (r.label_is_i64) c_label->i64.push_back(bits_i64(v));
+      else c_label->f64.push_back(v);
+    }
     for (size_t t = 0; t < c_tags.size(); ++t) {
       if (L.id_keyed) {
         c_tags[t]->i64.push_back((int64_t)L.ids[row]);
@@ -896,6 +950,11 @@ void PlanNode::run(NodeResult& r) {
   if (!stages_.empty()) r.value_is_count = false;  // a stage's result is a Float64 projection
   for (const Stage& s : stages_) {
     const bool work = r.rows > 0 && r.T > 0;
+    // an Int64 value column under a stage: a filter would keep the Int64 column, which the reference tree does not
+    // pin; a projection reads it as Float64 (DataFusion's coercion against the Float64 literal or function)
+    if (r.any_i64() && !s.is_fn && is_comparison(s.op) && !s.return_bool)
+      throw PlanError(ErrorKind::Plan, "a filtering comparison over an Int64 value column is not supported by this node");
+    to_f64(ctx_, r);
     if (s.is_fn) {
       const double a0 = s.args.size() > 0 ? s.args[0] : 0.0, a1 = s.args.size() > 1 ? s.args[1] : 0.0;
       // clamp's bound check (clamp.rs:212-217); clamp_min / clamp_max meet the other bound at ±f64::MAX.  The reference
@@ -953,6 +1012,15 @@ void BinaryPlan::compute(NodeResult& r) {
   lhs_->run(L);
   rhs_->run(R);
   if (L.T != R.T) throw PlanError(ErrorKind::Plan, "both sides of a binary operator must be evaluated on the same steps");
+  // Int64 operands: against a Float64 side DataFusion coerces to Float64; between two Int64 sides it would run integer
+  // arithmetic, division and overflow, which the reference tree does not pin, and a filter would keep the Int64 column
+  for (uint32_t f = 0; f < std::min(L.F, R.F); ++f)
+    if (L.is_i64(f) && R.is_i64(f))
+      throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: a binary operator between two Int64 value columns is not supported by this node");
+  if (L.any_i64() && is_comparison(op_) && !return_bool_)
+    throw PlanError(ErrorKind::Plan, "a filtering comparison over an Int64 value column is not supported by this node");
+  to_f64(ctx_, L);
+  to_f64(ctx_, R);
   // join keys (planner.rs:696-729, 3436-3468): the rhs context's tag columns, narrowed by on / ignoring; none when a
   // side has no tags (every row pairs with every row); two id-keyed sides without a modifier join on the id
   std::vector<int> lcols, rcols;
@@ -1021,6 +1089,7 @@ void BinaryPlan::compute(NodeResult& r) {
     r.columns = L.columns;
     r.value_names = L.value_names;
     r.label_name = L.label_name;
+    r.label_is_i64 = L.label_is_i64;
     r.value_is_count = L.value_is_count;
     if (!L.label_val.empty()) {
       r.label_val.resize((size_t)n_pairs * (size_t)r.T);
@@ -1097,6 +1166,9 @@ void SetOpPlan::compute(NodeResult& r) {
     throw PlanError(ErrorKind::Plan, "Attempt to combine two tables with different column sets, left: " +
                                          list(L.value_names) + ", right: " + list(R.value_names));
   }
+  // `and` / `unless` keep the lhs column and its type; `or` over an Int64 side is not pinned by the reference tree
+  if (op_ == B2P_SET_OR && (L.any_i64() || R.any_i64()))
+    throw PlanError(ErrorKind::Plan, what + "an Int64 value column is not supported by this node");
   if (L.F > 1)
     throw PlanError(ErrorKind::Plan, std::string("Multi fields calculation is not supported in ") +
                                          (op_ == B2P_SET_OR ? "OR operator" : "AND operator"));
@@ -1196,6 +1268,7 @@ void ScalarPlan::compute(NodeResult& r) {
   NodeResult C;
   child_->run(C);
   if (C.F > 1) throw PlanError(ErrorKind::Plan, "Multi fields calculation is not supported in scalar");  // planner.rs:3155-3160
+  to_f64(ctx_, C);  // scalar() of an Int64 node is Float64
   // one dense key per label tuple over the child's tag columns (a tagless child is one series, an id-keyed one is keyed
   // by the id); a tuple with a NULL label gets B2P_NO_KEY (scalar_calculate.rs:543-569 compares NULL as None against
   // the "" it recorded)
@@ -1291,8 +1364,11 @@ void TopkPlan::compute(NodeResult& r) {
   std::vector<uint32_t> tie(r.rows);
   for (uint32_t p = 0; p < r.rows; ++p) tie[order[p]] = bottom_ ? p : r.rows - 1 - p;
   if (r.rows > 0 && r.T > 0)
-    check(b2p_topk(ctx_, bottom_ ? 1 : 0, k_, r.val.data(), r.valid.data(), gid.data(), r.rows,
-                   (uint32_t)groups.ids.size(), tie.data(), (uint64_t)r.T, r.valid.data()));
+    check(r.is_i64(0) ? b2p_topk_i64(ctx_, bottom_ ? 1 : 0, k_, reinterpret_cast<const int64_t*>(r.val.data()),
+                                     r.valid.data(), gid.data(), r.rows, (uint32_t)groups.ids.size(), tie.data(),
+                                     (uint64_t)r.T, r.valid.data())
+                      : b2p_topk(ctx_, bottom_ ? 1 : 0, k_, r.val.data(), r.valid.data(), gid.data(), r.rows,
+                                 (uint32_t)groups.ids.size(), tie.data(), (uint64_t)r.T, r.valid.data()));
   // export order (Sort(group labels, ts, rank)): group labels by Labels::less, then the step, then the rank
   r.cell_order.clear();
   for (uint32_t q = 0; q < r.rows; ++q)
@@ -1307,7 +1383,9 @@ void TopkPlan::compute(NodeResult& r) {
     }
     const uint64_t ka = a % T, kb = b % T;
     if (ka != kb) return ka < kb;
-    const int64_t va = total_key_host(r.val[a]), vb = total_key_host(r.val[b]);
+    const bool i64 = r.is_i64(0);  // (an Int64 value compares as the integer its bits are)
+    const int64_t va = i64 ? bits_i64(r.val[a]) : total_key_host(r.val[a]);
+    const int64_t vb = i64 ? bits_i64(r.val[b]) : total_key_host(r.val[b]);
     if (va != vb) return bottom_ ? va < vb : va > vb;
     return bottom_ ? tie[ra] < tie[rb] : tie[ra] > tie[rb];
   });
@@ -1371,9 +1449,14 @@ void CountValuesPlan::compute(NodeResult& r) {
   std::vector<double> cval((size_t)R * T);
   std::vector<uint32_t> ccnt((size_t)R * T);
   if (R > 0 && T > 0)
-    check(b2p_count_values(ctx_, r.val.data(), r.valid.data(), groups.id.data(), R, G, (uint64_t)T, cval.data(),
-                           ccnt.data()),
+    check(r.is_i64(0) ? b2p_count_values_i64(ctx_, reinterpret_cast<const int64_t*>(r.val.data()), r.valid.data(),
+                                             groups.id.data(), R, G, (uint64_t)T, reinterpret_cast<int64_t*>(cval.data()),
+                                             ccnt.data())
+                      : b2p_count_values(ctx_, r.val.data(), r.valid.data(), groups.id.data(), R, G, (uint64_t)T,
+                                         cval.data(), ccnt.data()),
           ErrorKind::Execution);
+  r.label_is_i64 = r.is_i64(0);  // the counted values keep the child's type (count_values.result:31-62)
+  r.types.clear();                // the count
   // b2p_count_values' rows: group g's members (rank rows) from goff[g]
   std::vector<uint32_t> goff((size_t)G + 1, 0u), place(G);
   for (uint32_t q = 0; q < R; ++q) ++goff[groups.id[q] + 1];
@@ -1432,6 +1515,7 @@ SubqueryPlan::SubqueryPlan(b2p_ctx* ctx, std::string function, const b2p_range_p
 void SubqueryPlan::compute(NodeResult& r) {
   NodeResult C;
   child_->run(C);
+  if (C.any_i64()) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: an Int64 value column is not supported by this node");
   const int64_t T_in = C.T;
   const int64_t step = T_in > 1 ? C.eval_ts[1] - C.eval_ts[0] : p_.interval;  // (one inner step: any positive step)
   bool regular = step > 0;
@@ -1487,6 +1571,7 @@ void HistogramQuantilePlan::compute(NodeResult& r) {
     throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: a count_values child is not supported by this node");
   // the reference folds the first field only (planner.rs:3084-3092, a FIXME); this node does not copy that
   if (r.F > 1) throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: a multi-field child is not supported by this node");
+  if (r.any_i64()) throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: an Int64 value column is not supported by this node");
   r.cell_order.clear();
   const int le = r.labels.column(le_column_);
   if (le < 0) {  // create_histogram_plan: no le tag -> EmptyRelation, no rows and no columns
@@ -1542,8 +1627,12 @@ void SortPlan::compute(NodeResult& r) {
     // by every field in turn (planner.rs:1066-1071): lexicographic over the fields
     std::vector<const double*> vals(r.F);
     for (uint32_t f = 0; f < r.F; ++f) vals[f] = r.field(f);
-    check(b2p_sort_cells_fields(ctx_, desc_ ? 1 : 0, vals.data(), (int32_t)r.F, r.valid.data(), r.rows, T,
-                                r.cell_order.data(), &n),
+    if (r.any_i64() && r.F > 1)
+      throw PlanError(ErrorKind::Plan, "GpuPromSortExec: a multi-field child with an Int64 value column is not supported by this node");
+    check(r.is_i64(0) ? b2p_sort_cells_i64(ctx_, desc_ ? 1 : 0, reinterpret_cast<const int64_t*>(vals[0]), r.valid.data(),
+                                           r.rows, T, r.cell_order.data(), &n)
+                      : b2p_sort_cells_fields(ctx_, desc_ ? 1 : 0, vals.data(), (int32_t)r.F, r.valid.data(), r.rows, T,
+                                              r.cell_order.data(), &n),
           ErrorKind::Execution);
     r.cell_order.resize((size_t)n);
     return;

@@ -13,6 +13,7 @@
 // Errors mirror DataFusionError kinds: Plan (bad arguments / missing column, like field_not_found,
 // range_manipulate.rs:127-133), Execution (wrong column type, range_manipulate.rs:700-705), Internal.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <memory>
@@ -111,6 +112,9 @@ enum class Columns {
   None,                // no column at all: histogram_quantile over a child without the le tag (an EmptyRelation)
 };
 
+// The Arrow type of a value column.  An Int64 cell holds the bits of its int64_t in the 8-byte slot of the grid.
+enum class ValueType { Float64, Int64 };
+
 // What a node computed, before it becomes Arrow: F dense [rows x T] grids (one per field) under one validity, the eval
 // timestamps and one label tuple per row.  Exported, row r emits one Arrow row per valid step k (rows in order, steps
 // ascending) with F value columns.  One bitmap serves every field because no node that accepts F >= 2 clears a bit for
@@ -127,6 +131,8 @@ struct NodeResult {
   std::vector<uint32_t> valid;   // [rows x Tw]
   std::string time_index;
   std::vector<std::string> value_names;  // [F]
+  // [F] each field's type, as the reference types the node's value column (DESIGN §1 a25); empty: every field Float64
+  std::vector<ValueType> types;
   Labels labels;
   Columns columns = Columns::TimeValueTags;
   // when not empty, the export emits these cells (row * T + step), in this order, instead of rows then steps; a cell
@@ -137,6 +143,9 @@ struct NodeResult {
   std::vector<double> label_val;
   std::string label_name;
   bool value_is_count = false;
+  bool label_is_i64 = false;  // count_values over an Int64 child: label_val holds int64_t bits, exported as Int64
+  bool is_i64(uint32_t f) const { return f < types.size() && types[f] == ValueType::Int64; }
+  bool any_i64() const { return std::find(types.begin(), types.end(), ValueType::Int64) != types.end(); }
   bool valid_at(uint32_t r, int64_t k) const { return (valid[(size_t)r * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u; }
   size_t grid() const { return (size_t)rows * (size_t)T; }
   double* field(uint32_t f) { return val.data() + f * grid(); }
@@ -198,7 +207,8 @@ class PromRangePlan : public PlanNode {
   int fn_id_;
   int agg_id_;
   std::vector<int64_t> ts_;
-  std::vector<std::vector<double>> val_;  // [field][row]
+  std::vector<std::vector<double>> val_;  // [field][row]; an Int64 field's rows hold int64_t bits
+  std::vector<ValueType> types_;          // [field], set by the first batch
   // F >= 2: each field's Arrow validity bitmap re-based to bit 0 of the first row (empty while the field has no NULL)
   std::vector<std::vector<uint8_t>> present_;
   std::vector<uint64_t> offsets_;  // first row of every series (SeriesDivide's output), end marker added by execute()

@@ -75,14 +75,8 @@ struct QuantArgs {
 constexpr size_t kQuantWarpBytes = (size_t)kQuantResident * 32 * 8;
 static_assert(kQuantWarpBytes >= 128 * 32 * 4, "the histogram must fit the warp's shared memory");
 
-__device__ __forceinline__ unsigned long long quant_key(double v) {
-  return (unsigned long long)total_key(v) ^ 0x8000000000000000ull;
-}
-__device__ __forceinline__ double quant_value(unsigned long long u) {
-  long long b = (long long)(u ^ 0x8000000000000000ull);
-  b ^= (long long)(((unsigned long long)(b >> 63)) >> 1);  // total_key is an involution
-  return __longlong_as_double(b);
-}
+__device__ __forceinline__ unsigned long long quant_key(double v) { return F64Key::key(v); }
+__device__ __forceinline__ double quant_value(unsigned long long u) { return F64Key::value(u); }
 // lo = floor(φ (n - 1)), n >= 1 and 0 <= φ <= 1
 __device__ __forceinline__ uint32_t quant_lo(double phi, uint32_t n) {
   const double f = floor(__dmul_rn(phi, (double)(n - 1)));

@@ -722,10 +722,14 @@ int b2p_range_eval_fields_dev(b2p_ctx* c, const b2p_range_params* p, const int64
   return B2P_OK;
 }
 
-int b2p_instant_select_fields_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
-                                  int64_t offset, const int64_t* ts, const double* const* vals,
-                                  const uint8_t* const* field_valid, int32_t n_fields, const uint64_t* offsets,
-                                  uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words) {
+}  // extern "C"
+
+namespace {
+// b2p_instant_select_fields_dev, and with i64 its Int64 form (field 0 is Int64: no staleness test, K17 for every F)
+int instant_select_fields(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
+                          const int64_t* ts, const double* const* vals, const uint8_t* const* field_valid,
+                          int32_t n_fields, const uint64_t* offsets, uint64_t n_rows, uint32_t n_series,
+                          double* const* outs, uint32_t* valid_words, bool i64) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   int rc = check_fields(vals, outs, n_fields);
   if (rc) return rc;
@@ -734,11 +738,14 @@ int b2p_instant_select_fields_dev(b2p_ctx* c, int64_t start, int64_t end, int64_
     DeviceGuard g(c->device);
     int f = -1;
     if ((rc = first_null_field(c, field_valid, n_fields, n_rows, &f))) return rc;
+    if (f >= 0 && i64 && n_fields == 1)
+      return fail(B2P_E_INVALID, "Int64 field has NULL slots: the instant selector exports a chosen NULL slot as a NULL "
+                  "value (no stale-NaN test reads it), which the dense grid does not carry");
     if (f >= 0)
       return fail(B2P_E_INVALID, "field %d has NULL slots: the instant selector exports them as NULL in that field "
                   "only, which a multi-field call does not reproduce", f);
   }
-  if (n_fields == 1)
+  if (n_fields == 1 && !i64)
     return b2p_instant_select_dev(c, start, end, interval, lookback, offset, ts, vals[0], offsets, n_rows, n_series,
                                   outs[0], valid_words);
   FieldsInstantArgs fa{};
@@ -752,11 +759,31 @@ int b2p_instant_select_fields_dev(b2p_ctx* c, int64_t start, int64_t end, int64_
   fa.F = n_fields;
   for (int f = 0; f < n_fields; ++f) { fa.vals[f] = vals[f]; fa.outs[f] = outs[f]; }
   stage_begin(c, 1);
-  instant_fields_kernel<<<capped_grid(c, n_series, kWarpsPerCta, 8), kWarpsPerCta * 32, 0, c->stream>>>(fa);
+  (i64 ? instant_fields_kernel<false> : instant_fields_kernel<true>)<<<capped_grid(c, n_series, kWarpsPerCta, 8),
+                                                                      kWarpsPerCta * 32, 0, c->stream>>>(fa);
   c->launches++;
   stage_end(c, 1);
   CU(cudaGetLastError());
   return B2P_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_instant_select_fields_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                                  int64_t offset, const int64_t* ts, const double* const* vals,
+                                  const uint8_t* const* field_valid, int32_t n_fields, const uint64_t* offsets,
+                                  uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words) {
+  return instant_select_fields(c, start, end, interval, lookback, offset, ts, vals, field_valid, n_fields, offsets,
+                               n_rows, n_series, outs, valid_words, false);
+}
+
+int b2p_instant_select_fields_i64_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                                      int64_t offset, const int64_t* ts, const double* const* vals,
+                                      const uint8_t* const* field_valid, int32_t n_fields, const uint64_t* offsets,
+                                      uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words) {
+  return instant_select_fields(c, start, end, interval, lookback, offset, ts, vals, field_valid, n_fields, offsets,
+                               n_rows, n_series, outs, valid_words, true);
 }
 
 // sum by (..)(fn(..)) partials of groups [g_lo, g_hi) added into out_sum / out_cnt [n_groups x T].
@@ -1361,10 +1388,14 @@ int b2p_range_eval_fields(b2p_ctx* c, const b2p_range_params* p, const int64_t* 
   });
 }
 
-int b2p_instant_select_fields(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
-                              int64_t offset, const int64_t* ts, const double* const* vals,
-                              const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid,
-                              const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words) {
+}  // extern "C"
+
+namespace {
+int instant_select_fields_host(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                               int64_t offset, const int64_t* ts, const double* const* vals,
+                               const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid,
+                               const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* const* outs,
+                               uint32_t* valid_words, bool i64) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   InstantArgs grid;
   if (int rc = instant_grid(start, end, interval, lookback, offset, n_series, &grid)) return rc;
@@ -1375,11 +1406,31 @@ int b2p_instant_select_fields(b2p_ctx* c, int64_t start, int64_t end, int64_t in
   const FieldsIn f =
       stage_fields(s, ts, vals, field_valid, n_fields, sid, offsets_host, n_rows, n_series, grid.T, outs, valid_words);
   return s.end([&] {
-    const int rc = b2p_instant_select_fields_dev(c, start, end, interval, lookback, offset, f.series.ts, f.vals,
-                                                 field_valid ? f.nulls : nullptr, n_fields, f.series.offsets, n_rows,
-                                                 n_series, f.outs, f.valid);
+    const int rc = instant_select_fields(c, start, end, interval, lookback, offset, f.series.ts, f.vals,
+                                         field_valid ? f.nulls : nullptr, n_fields, f.series.offsets, n_rows, n_series,
+                                         f.outs, f.valid, i64);
     return rc ? rc : b2p_sync(c);
   });
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_instant_select_fields(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                              int64_t offset, const int64_t* ts, const double* const* vals,
+                              const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid,
+                              const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* const* outs, uint32_t* valid_words) {
+  return instant_select_fields_host(c, start, end, interval, lookback, offset, ts, vals, field_valid, n_fields, sid,
+                                    offsets_host, n_rows, n_series, outs, valid_words, false);
+}
+
+int b2p_instant_select_fields_i64(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                                  int64_t offset, const int64_t* ts, const double* const* vals,
+                                  const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid,
+                                  const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series,
+                                  double* const* outs, uint32_t* valid_words) {
+  return instant_select_fields_host(c, start, end, interval, lookback, offset, ts, vals, field_valid, n_fields, sid,
+                                    offsets_host, n_rows, n_series, outs, valid_words, true);
 }
 
 int b2p_subquery(b2p_ctx* c, const b2p_range_params* p, int64_t inner_start, int64_t inner_interval, const double* vals,

@@ -421,4 +421,4 @@ int build_group_csr(b2p_ctx* c, const uint32_t* gid, uint32_t n_series, uint32_t
 // added to instead of overwritten
 int group_aggregate_csr(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* goff,
                         const uint32_t* members, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt,
-                        int accumulate, double* out_mean = nullptr);
+                        int accumulate, double* out_mean = nullptr, bool i64 = false);

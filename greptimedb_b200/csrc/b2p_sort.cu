@@ -16,9 +16,9 @@ namespace {
 // more stable radix sort.  The keys and the cell indices ping-pong between their two buffers (the cells between out_cells
 // and the context's so_cells); if the cells end in the latter they are copied back.  Scratch (context buffers so_*):
 // 8 B per row plus one (offsets), 24 B per valid cell (two key buffers, one cell buffer) and CUB's temp storage.
-// *n_host is the number of valid cells.
+// *n_host is the number of valid cells.  i64: the cells are Int64 (I64Key).
 int sort_run(b2p_ctx* c, int desc, const double* const* vals, int32_t n_fields, const uint32_t* valid, uint32_t rows,
-             uint64_t T, uint64_t* out_cells, uint64_t* out_n, uint64_t* n_host) {
+             uint64_t T, uint64_t* out_cells, uint64_t* out_n, uint64_t* n_host, bool i64) {
   int rc;
   if ((rc = c->so_off.ensure(((size_t)rows + 1) * 8))) return rc;
   unsigned long long* off = c->so_off.as<unsigned long long>();
@@ -36,7 +36,7 @@ int sort_run(b2p_ctx* c, int desc, const double* const* vals, int32_t n_fields, 
   a.offsets = off;
   a.keys = c->so_keys.as<unsigned long long>();
   a.cells = reinterpret_cast<unsigned long long*>(out_cells);
-  sort_scatter_kernel<<<cell_rows_grid(c, rows), 256, 0, c->stream>>>(a);
+  (i64 ? sort_scatter_kernel<I64Key> : sort_scatter_kernel<F64Key>)<<<cell_rows_grid(c, rows), 256, 0, c->stream>>>(a);
   c->launches++;
   CU(cudaGetLastError());
   cub::DoubleBuffer<unsigned long long> keys(a.keys, a.keys + n);
@@ -47,8 +47,8 @@ int sort_run(b2p_ctx* c, int desc, const double* const* vals, int32_t n_fields, 
   bytes = c->so_tmp.cap;
   CU(cub::DeviceRadixSort::SortPairs(c->so_tmp.p, bytes, keys, cells, n, 0, 64, c->stream));
   for (int32_t f = n_fields - 2; f >= 0; --f) {
-    sort_rekey_kernel<<<capped_grid(c, n, 256, 8), 256, 0, c->stream>>>(vals[f], cells.Current(), keys.Current(), n,
-                                                                         a.desc);
+    (i64 ? sort_rekey_kernel<I64Key> : sort_rekey_kernel<F64Key>)<<<capped_grid(c, n, 256, 8), 256, 0, c->stream>>>(
+        vals[f], cells.Current(), keys.Current(), n, a.desc);
     c->launches++;
     CU(cudaGetLastError());
     bytes = c->so_tmp.cap;
@@ -72,13 +72,10 @@ int check_sort_fields(const double* const* vals, int32_t n_fields) {
   if (!vals) return fail(B2P_E_INVALID, "NULL argument");
   return B2P_OK;
 }
-}  // namespace
 
-extern "C" {
-
-int b2p_sort_cells_fields_dev(b2p_ctx* c, int32_t desc, const double* const* vals, int32_t n_fields,
-                              const uint32_t* valid, uint32_t n_rows, uint64_t T, uint64_t* out_cells,
-                              uint64_t* out_n) {
+// the device and host forms of every sort entry point; i64: the grid is Int64 (one field)
+int sort_cells_dev(b2p_ctx* c, int32_t desc, const double* const* vals, int32_t n_fields, const uint32_t* valid,
+                   uint32_t n_rows, uint64_t T, uint64_t* out_cells, uint64_t* out_n, bool i64) {
   if (!c || !out_n) return fail(B2P_E_INVALID, "NULL argument");
   if (int rc = check_sort_fields(vals, n_fields)) return rc;
   if (int rc = check_sort_shape(n_rows, T)) return rc;
@@ -92,20 +89,13 @@ int b2p_sort_cells_fields_dev(b2p_ctx* c, int32_t desc, const double* const* val
     if (!vals[f]) return fail(B2P_E_INVALID, "NULL argument (field %d)", (int)f);
   uint64_t n = 0;
   stage_begin(c, 3);
-  const int rc = sort_run(c, desc, vals, n_fields, valid, n_rows, T, out_cells, out_n, &n);
+  const int rc = sort_run(c, desc, vals, n_fields, valid, n_rows, T, out_cells, out_n, &n, i64);
   stage_end(c, 3);
   return rc;
 }
 
-int b2p_sort_cells_dev(b2p_ctx* c, int32_t desc, const double* vals, const uint32_t* valid, uint32_t n_rows,
-                       uint64_t T, uint64_t* out_cells, uint64_t* out_n) {
-  return b2p_sort_cells_fields_dev(c, desc, &vals, 1, valid, n_rows, T, out_cells, out_n);
-}
-
-/* ---- host-pointer API ------------------------------------------------------------------------ */
-
-int b2p_sort_cells_fields(b2p_ctx* c, int32_t desc, const double* const* vals, int32_t n_fields, const uint32_t* valid,
-                          uint32_t n_rows, uint64_t T, uint64_t* out_cells, uint64_t* out_n) {
+int sort_cells_host(b2p_ctx* c, int32_t desc, const double* const* vals, int32_t n_fields, const uint32_t* valid,
+                    uint32_t n_rows, uint64_t T, uint64_t* out_cells, uint64_t* out_n, bool i64) {
   if (!c) return fail(B2P_E_INVALID, "NULL argument");
   if (int rc = check_sort_fields(vals, n_fields)) return rc;
   if (int rc = check_sort_shape(n_rows, T)) return rc;  // (before the cell column is sized)
@@ -117,16 +107,48 @@ int b2p_sort_cells_fields(b2p_ctx* c, int32_t desc, const double* const* vals, i
   const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
   uint64_t* d_cells = out_cells ? static_cast<uint64_t*>(s.buf(cells * 8)) : nullptr;
   uint64_t* d_n = s.out(out_n, 8);
-  if (int rc = s.end([&] { return b2p_sort_cells_fields_dev(c, desc, d_vals, n_fields, d_valid, n_rows, T, d_cells,
-                                                            d_n); }))
+  if (int rc = s.end([&] { return sort_cells_dev(c, desc, d_vals, n_fields, d_valid, n_rows, T, d_cells, d_n, i64); }))
     return rc;
   s.copy_back(out_cells, d_cells, *out_n * 8);  // only the valid cells' entries, now that their count is here
   return s.finish();
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_sort_cells_fields_dev(b2p_ctx* c, int32_t desc, const double* const* vals, int32_t n_fields,
+                              const uint32_t* valid, uint32_t n_rows, uint64_t T, uint64_t* out_cells,
+                              uint64_t* out_n) {
+  return sort_cells_dev(c, desc, vals, n_fields, valid, n_rows, T, out_cells, out_n, false);
+}
+
+int b2p_sort_cells_dev(b2p_ctx* c, int32_t desc, const double* vals, const uint32_t* valid, uint32_t n_rows,
+                       uint64_t T, uint64_t* out_cells, uint64_t* out_n) {
+  return b2p_sort_cells_fields_dev(c, desc, &vals, 1, valid, n_rows, T, out_cells, out_n);
+}
+
+int b2p_sort_cells_i64_dev(b2p_ctx* c, int32_t desc, const int64_t* vals, const uint32_t* valid, uint32_t n_rows,
+                           uint64_t T, uint64_t* out_cells, uint64_t* out_n) {
+  const double* v = reinterpret_cast<const double*>(vals);
+  return sort_cells_dev(c, desc, &v, 1, valid, n_rows, T, out_cells, out_n, true);
+}
+
+/* ---- host-pointer API ------------------------------------------------------------------------ */
+
+int b2p_sort_cells_fields(b2p_ctx* c, int32_t desc, const double* const* vals, int32_t n_fields, const uint32_t* valid,
+                          uint32_t n_rows, uint64_t T, uint64_t* out_cells, uint64_t* out_n) {
+  return sort_cells_host(c, desc, vals, n_fields, valid, n_rows, T, out_cells, out_n, false);
 }
 
 int b2p_sort_cells(b2p_ctx* c, int32_t desc, const double* vals, const uint32_t* valid, uint32_t n_rows, uint64_t T,
                    uint64_t* out_cells, uint64_t* out_n) {
   return b2p_sort_cells_fields(c, desc, &vals, 1, valid, n_rows, T, out_cells, out_n);
+}
+
+int b2p_sort_cells_i64(b2p_ctx* c, int32_t desc, const int64_t* vals, const uint32_t* valid, uint32_t n_rows, uint64_t T,
+                       uint64_t* out_cells, uint64_t* out_n) {
+  const double* v = reinterpret_cast<const double*>(vals);
+  return sort_cells_host(c, desc, &v, 1, valid, n_rows, T, out_cells, out_n, true);
 }
 
 }  // extern "C"

@@ -8,7 +8,8 @@
 // +0.0 < .. < +inf < +NaN, every bit pattern its own key), and its bitwise NOT for sort_desc.  The pairs enter the
 // radix sort in row-major order and the sort is stable, so equal values keep the child's row, then step, order in
 // both directions.  CUB's floating-point key mode is not used: it ranks -0.0 and +0.0 equal and does not put negative
-// NaNs where total_cmp does.
+// NaNs where total_cmp does.  An Int64 grid (b2p_sort_cells_i64) keys on its bits ^ 2^63 instead: the kernels take the
+// key as a template parameter (F64Key / I64Key, b2p_window.cuh).
 // Several fields (sort over a multi-field node: Sort(f0, f1, .. each ASC | DESC NULLS FIRST), planner.rs:2743-2749)
 // sort least significant key first: the scatter keys on the last field, and for each earlier field
 //   sort_rekey_kernel    one thread per pair: the pair's key reloaded from that field at its cell
@@ -32,10 +33,11 @@ struct SortArgs {
   unsigned long long* cells;            // [total]
 };
 
+template <class Key = F64Key>
 __global__ void __launch_bounds__(256) sort_scatter_kernel(const SortArgs a) {
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t below = (1u << lane) - 1u;
-  const unsigned long long flip = a.desc ? ~0x8000000000000000ull : 0x8000000000000000ull;
+  const unsigned long long flip = a.desc ? ~0ull : 0ull;
   const uint64_t warp0 = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
   for (uint64_t r = warp0; r < a.rows; r += n_warps) {
@@ -46,7 +48,7 @@ __global__ void __launch_bounds__(256) sort_scatter_kernel(const SortArgs a) {
       const uint64_t k = (uint64_t)w * 32 + lane;
       if ((word >> lane) & 1u) {
         const unsigned long long pos = base + __popc(word & below);
-        a.keys[pos] = (unsigned long long)total_key(__ldcs(row + k)) ^ flip;
+        a.keys[pos] = Key::key(__ldcs(row + k)) ^ flip;
         a.cells[pos] = r * a.T + k;
       }
       base += __popc(word);
@@ -54,13 +56,14 @@ __global__ void __launch_bounds__(256) sort_scatter_kernel(const SortArgs a) {
   }
 }
 
+template <class Key = F64Key>
 __global__ void __launch_bounds__(256) sort_rekey_kernel(const double* __restrict__ vals,
                                                          const unsigned long long* __restrict__ cells,
                                                          unsigned long long* __restrict__ keys, uint64_t n, int desc) {
-  const unsigned long long flip = desc ? ~0x8000000000000000ull : 0x8000000000000000ull;
+  const unsigned long long flip = desc ? ~0ull : 0ull;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    keys[i] = (unsigned long long)total_key(__ldg(vals + cells[i])) ^ flip;
+    keys[i] = Key::key(__ldg(vals + cells[i])) ^ flip;
 }
 
 }  // namespace b2p

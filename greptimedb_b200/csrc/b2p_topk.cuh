@@ -10,7 +10,8 @@
 // ranked by (value in the f64 total order, tie), descending for topk and ascending for bottomk, where tie [rows] is one
 // distinct ordinal per row that the caller derives from the label tuples (b2p_plan.cpp).  That is a strict total
 // order, so the kept set of a (group, step) is exactly its min(kk, valid cells) best cells.  Inside the kernels a
-// cell's key is (hi, lo) = (total key, tie), bit-inverted for bottomk, so that "better" is always "larger".
+// cell's key is (hi, lo) = (total key, tie), bit-inverted for bottomk, so that "better" is always "larger".  The two
+// kernels that read values take the key as a template parameter: F64Key, or I64Key for an Int64 grid (b2p_topk_i64).
 //
 // Only validity words are written: topk is a filter and every consumer reads a cell only where its bit is set.  The
 // last pass of a (chunk, tile) writes the tile's word of every member row of the chunk, so no word has two writers and
@@ -79,8 +80,9 @@ struct TopkArgs {
   uint32_t* out_valid;     // [rows x Tw]; may be valid
 };
 
+template <class Key>
 __device__ __forceinline__ void topk_key(double v, uint32_t tie, int bottom, unsigned long long& hi, uint32_t& lo) {
-  const unsigned long long k = (unsigned long long)total_key(v) ^ 0x8000000000000000ull;  // unsigned, order kept
+  const unsigned long long k = Key::key(v);  // unsigned, order kept
   hi = bottom ? ~k : k;
   lo = bottom ? ~tie : tie;
 }
@@ -193,6 +195,7 @@ __device__ void topk_write_words(const TopkArgs& a, uint32_t* sw, const uint32_t
 }
 
 // Streams the members of `ch` for one tile into the lane's heap (cells with want and below the bound, if any)
+template <class Key>
 __device__ __forceinline__ uint32_t topk_stream(const TopkArgs& a, const TopkChunk& ch, uint32_t tile, int lane,
                                                 bool want, const TopkState& st, TopkHeap& h) {
   constexpr uint32_t kAhead = 8;
@@ -226,7 +229,7 @@ __device__ __forceinline__ uint32_t topk_stream(const TopkArgs& a, const TopkChu
         if (!on[q]) continue;
         unsigned long long kh;
         uint32_t kl;
-        topk_key(v[q], tq, a.bottom, kh, kl);
+        topk_key<Key>(v[q], tq, a.bottom, kh, kl);
         if (bounded && !key_less(kh, kl, st.hi, st.lo)) continue;
         h.offer(n, a.K, th, tl, kh, kl, m0 + i0 + q);
       }
@@ -241,6 +244,7 @@ __host__ __device__ constexpr size_t topk_warp_bytes(uint32_t K) { return (size_
 // One warp per (chunk, tile).  Fast path: a single-chunk group writes its words here; a chunk of a larger group
 // leaves its list.  General path: chunks of groups of at most kk members are skipped (topk_select_kernel copies their
 // words), a single-chunk group takes its round's verdict here, a chunk of a larger group leaves its list.
+template <class Key = F64Key>
 __global__ void __launch_bounds__(kTopkWarps * 32) topk_chunk_kernel(const TopkArgs a) {
   extern __shared__ __align__(16) unsigned char topk_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -256,7 +260,7 @@ __global__ void __launch_bounds__(kTopkWarps * 32) topk_chunk_kernel(const TopkA
     const bool live = (uint64_t)tile * 32 + lane < a.T;
     const uint64_t si = ch.state != kTopkNone ? ((uint64_t)ch.state * a.tiles + tile) * 32 + lane : 0;
     const TopkState st = ch.state != kTopkNone ? topk_state_load(a, si) : TopkState{a.kk, 0u, 0ull, 0u};
-    const uint32_t n = topk_stream(a, ch, tile, lane, live && !st.done(), st, h);
+    const uint32_t n = topk_stream<Key>(a, ch, tile, lane, live && !st.done(), st, h);
     if (ch.cand != kTopkNone) {  // a chunk of a larger group: its list, for topk_merge_kernel
       const uint64_t cb = (uint64_t)ch.cand * a.tiles + tile;
       for (uint32_t s = 0; s < n; ++s) {
@@ -345,6 +349,7 @@ __global__ void __launch_bounds__(kTopkWarps * 32) topk_mark_kernel(const TopkAr
 
 // General path, one warp per (chunk, tile): a member's word has the valid cells at or above the (group, step)'s
 // threshold, or every valid cell (groups of at most kk members, and steps with fewer than kk cells)
+template <class Key = F64Key>
 __global__ void __launch_bounds__(256, 1) topk_select_kernel(const TopkArgs a) {
   constexpr uint32_t kAhead = 8;
   const int lane = threadIdx.x & 31;
@@ -392,7 +397,7 @@ __global__ void __launch_bounds__(256, 1) topk_select_kernel(const TopkArgs a) {
             if (keep && !all) {
               unsigned long long kh;
               uint32_t kl;
-              topk_key(v[q], tq, a.bottom, kh, kl);
+              topk_key<Key>(v[q], tq, a.bottom, kh, kl);
               keep = !key_less(kh, kl, th, tl);
             }
             const uint32_t word = __ballot_sync(0xFFFFFFFFu, keep);

@@ -430,6 +430,94 @@ class Context:
                                              _ptr(out), _ptr(cnt)))
         return out, cnt
 
+    def instant_select_fields_i64(self, ts, vals, start, end, interval, lookback, offset=0, sid=None, offsets=None,
+                                  present=None):
+        """The instant selector with an Int64 field 0 (int64 column; the other fields int64 or float64, moved bit for
+        bit) -> (outs [F,S,T] as int64 bits, valid_words [S,Tw] u32): no stale-NaN test."""
+        ts = np.ascontiguousarray(ts, np.int64)
+        vals = [np.ascontiguousarray(v) for v in vals]
+        if any(v.dtype.itemsize != 8 for v in vals):
+            raise ValueError("field columns must be 8-byte (int64 or float64)")
+        nb, _keep3 = self._field_bitmaps(present)
+        sid, offsets, S = self._series_count(sid, offsets)
+        T = num_steps(start, end, interval)
+        outs = np.zeros((len(vals), S, T), np.int64)
+        valid = np.zeros((S, (T + 31) // 32), np.uint32)
+        vp, _keep = self._ptr_array(vals)
+        op, _keep2 = self._ptr_array(list(outs))
+        self._check(self._L.b2p_instant_select_fields_i64(self._h, start, end, interval, lookback, offset, _ptr(ts), vp,
+                                                          nb, len(vals), _ptr(sid), _ptr(offsets), ts.size, S, op,
+                                                          _ptr(valid)))
+        return outs, valid
+
+    def sort_cells_i64_dev(self, desc, vals, valid, n_rows, T, out_cells, out_n):
+        """b2p_sort_cells_i64_dev over device tensors (int64 grid, int32 words; out_cells / out_n int64)."""
+        self._check(self._L.b2p_sort_cells_i64_dev(self._h, int(bool(desc)), _ptr(vals), _ptr(valid), n_rows, T,
+                                                   _ptr(out_cells), _ptr(out_n)))
+
+    def group_aggregate_i64_dev(self, agg, vals, valid, gid, n_series, n_groups, T, out_val, out_cnt):
+        """b2p_group_aggregate_i64_dev over device tensors."""
+        aid = AGG_IDS[agg] if isinstance(agg, str) else int(agg)
+        self._check(self._L.b2p_group_aggregate_i64_dev(self._h, aid, _ptr(vals), _ptr(valid), _ptr(gid), n_series,
+                                                        n_groups, T, _ptr(out_val), _ptr(out_cnt)))
+
+    # ---- Int64 (BIGINT) value grids: int64 cells in the same layout; the calls that read a value as a number ----------
+    def group_aggregate_i64(self, agg, vals, valid, gid, n_groups):
+        """group_aggregate over an int64 grid -> (out [G,T], cnt [G,T] u32): sum (wrapping), min and max as int64, the
+        other aggregators as float64 over (double)i64."""
+        vals = np.ascontiguousarray(vals, np.int64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        gid = np.ascontiguousarray(gid, np.uint32)
+        S, T = vals.shape
+        out = np.zeros((n_groups, T), np.float64)
+        cnt = np.zeros((n_groups, T), np.uint32)
+        aid = AGG_IDS[agg] if isinstance(agg, str) else int(agg)
+        self._check(self._L.b2p_group_aggregate_i64(self._h, aid, _ptr(vals), _ptr(valid), _ptr(gid), S, n_groups, T,
+                                                    _ptr(out), _ptr(cnt)))
+        return (out.view(np.int64) if aid in (AGG_IDS["sum"], AGG_IDS["min"], AGG_IDS["max"]) else out), cnt
+
+    def topk_i64(self, op, k, vals, valid, gid, n_groups, tie):
+        """topk over an int64 grid (signed order) -> the kept cells' validity words [S,Tw] u32."""
+        vals = np.ascontiguousarray(vals, np.int64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        gid = np.ascontiguousarray(gid, np.uint32)
+        tie = np.ascontiguousarray(tie, np.uint32)
+        S, T = vals.shape
+        ov = np.zeros((S, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_topk_i64(self._h, topk_bottom(op), float(k), _ptr(vals), _ptr(valid), _ptr(gid), S,
+                                         int(n_groups), _ptr(tie), T, _ptr(ov)))
+        return ov
+
+    def count_values_i64(self, vals, valid, gid, n_groups):
+        """count_values over an int64 grid -> (out [R,T] int64, cnt [R,T] u32), distinct values in signed order."""
+        vals = np.ascontiguousarray(vals, np.int64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        gid = np.ascontiguousarray(gid, np.uint32)
+        S, T = vals.shape
+        out = np.zeros((S, T), np.int64)
+        cnt = np.zeros((S, T), np.uint32)
+        self._check(self._L.b2p_count_values_i64(self._h, _ptr(vals), _ptr(valid), _ptr(gid), S, int(n_groups), T,
+                                                 _ptr(out), _ptr(cnt)))
+        return out, cnt
+
+    def sort_cells_i64(self, desc, vals, valid):
+        """sort / sort_desc over an int64 grid (signed order, ties in row-major order) -> u64 [n valid cells]."""
+        vals = np.ascontiguousarray(vals, np.int64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        R, T = vals.shape
+        out = np.zeros(max(R * T, 1), np.uint64)
+        n = C.c_uint64(0)
+        self._check(self._L.b2p_sort_cells_i64(self._h, int(bool(desc)), _ptr(vals), _ptr(valid), R, T, _ptr(out),
+                                               C.byref(n)))
+        return out[:n.value].copy()
+
+    def i64_to_f64(self, vals):
+        """(double)i64 of every cell, on the device."""
+        vals = np.ascontiguousarray(vals, np.int64)
+        out = np.zeros(vals.shape, np.float64)
+        self._check(self._L.b2p_i64_to_f64(self._h, _ptr(vals), vals.size, _ptr(out)))
+        return out
+
     def subquery(self, p: RangeParams, inner_start, inner_interval, vals, valid):
         """fn(<child>[range:step]): vals [R,T'] / valid [R,Tw'] u32 are the child's grid on the inner steps
         inner_start + k * inner_interval; every valid cell of a row is a sample of its series (NaN included).  p is the

@@ -59,6 +59,8 @@
  *                              planner.rs:1060-1089, 2743-2772
  *   b2p_sort_cells_fields[_dev] the same over several fields: Sort(f0, f1, .. ASC | DESC, NULLS FIRST),
  *                              planner.rs:1066-1071, 2743-2749
+ *   b2p_*_i64[_dev]            the instant selector, the by-label aggregate, topk / bottomk, count_values and sort over
+ *                              an Int64 (BIGINT) value column; b2p_i64_to_f64[_dev] the Float64 coercion of one
  *
  * Data layout (HBM, struct-of-arrays, all row-sorted by (series id, timestamp) exactly like
  * the reference's required_input_ordering, series_divide.rs:410-440):
@@ -469,6 +471,38 @@ B2P_API int b2p_sort_cells_fields_dev(b2p_ctx* ctx, int32_t desc, const double* 
                                       const uint32_t* valid, uint32_t n_rows, uint64_t T, uint64_t* out_cells,
                                       uint64_t* out_n);
 
+/* ---- Int64 (BIGINT) value columns ------------------------------------------------------------------------------
+ * An Int64 cell holds the bits of an int64_t in the same 8-byte slot a Float64 cell uses, so every layout above is
+ * unchanged and only the calls that read a value as a number have an Int64 form.  The reference reads such a column
+ * through the Arrow Int64 type: no stale-NaN test and no NaN filter (instant_manipulate.rs:490-527, normalize.rs:419),
+ * integer order and integer equality.  An i64 whose bits are a NaN double is an ordinary integer to every call here. */
+/* As b2p_instant_select_fields_dev with field 0 Int64: no staleness test, so every fresh row is selected (the other
+ * fields' cells, of either type, are copied bit for bit).  n_fields == 1 is the one-field Int64 selector. */
+B2P_API int b2p_instant_select_fields_i64_dev(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval,
+                                              int64_t lookback, int64_t offset, const int64_t* ts,
+                                              const double* const* vals, const uint8_t* const* field_valid,
+                                              int32_t n_fields, const uint64_t* offsets, uint64_t n_rows,
+                                              uint32_t n_series, double* const* outs, uint32_t* valid_words);
+/* As b2p_group_aggregate_dev over Int64 cells: sum is the two's-complement wrapping sum (DataFusion's Int64 Sum
+ * accumulator; wrapping add is associative, so the bits do not depend on the member order), min / max compare signed;
+ * these three write the int64_t bits into out_val.  avg, stddev and stdvar read each value as (double)i64 and write
+ * Float64 as b2p_group_aggregate_dev does; count writes the Float64 count. */
+B2P_API int b2p_group_aggregate_i64_dev(b2p_ctx* ctx, int32_t agg, const int64_t* vals, const uint32_t* valid_words,
+                                        const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T,
+                                        double* out_val, uint32_t* out_cnt);
+/* As b2p_topk_dev / b2p_count_values_dev / b2p_sort_cells_dev over Int64 cells: cells rank by signed value (key
+ * bits ^ 2^63); count_values' distinct values are the int64_t values, written to out_val as int64_t. */
+B2P_API int b2p_topk_i64_dev(b2p_ctx* ctx, int32_t bottom, double k, const int64_t* vals, const uint32_t* valid,
+                             const b2p_group_index* index, const uint32_t* tie, uint64_t T, uint32_t* out_valid);
+B2P_API int b2p_count_values_i64_dev(b2p_ctx* ctx, const int64_t* vals, const uint32_t* valid,
+                                     const b2p_group_index* index, uint64_t T, int64_t* out_val, uint32_t* out_cnt);
+B2P_API int b2p_sort_cells_i64_dev(b2p_ctx* ctx, int32_t desc, const int64_t* vals, const uint32_t* valid,
+                                   uint32_t n_rows, uint64_t T, uint64_t* out_cells, uint64_t* out_n);
+/* out[i] = (double)vals[i] (round to nearest even, as an Arrow Int64 -> Float64 cast) for i < n; out may be vals.  The
+ * coercion DataFusion applies where a Float64 operator (arithmetic with a Float64 side, a math function, scalar(),
+ * quantile) reads an Int64 column. */
+B2P_API int b2p_i64_to_f64_dev(b2p_ctx* ctx, const int64_t* vals, uint64_t n, double* out);
+
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
  * the id column `sid` (ids sid_base .. sid_base + n_series - 1, non-decreasing), or copied from `offsets_in`
@@ -567,6 +601,24 @@ B2P_API int b2p_sort_cells(b2p_ctx* ctx, int32_t desc, const double* vals, const
 B2P_API int b2p_sort_cells_fields(b2p_ctx* ctx, int32_t desc, const double* const* vals, int32_t n_fields,
                                   const uint32_t* valid, uint32_t n_rows, uint64_t T, uint64_t* out_cells,
                                   uint64_t* out_n);
+
+/* Host-pointer forms of the Int64 calls above (synchronous), staged as their Float64 twins stage. */
+B2P_API int b2p_instant_select_fields_i64(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                                          int64_t offset, const int64_t* ts, const double* const* vals,
+                                          const uint8_t* const* field_valid, int32_t n_fields, const uint32_t* sid,
+                                          const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series,
+                                          double* const* outs, uint32_t* valid_words);
+B2P_API int b2p_group_aggregate_i64(b2p_ctx* ctx, int32_t agg, const int64_t* vals, const uint32_t* valid_words,
+                                    const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T,
+                                    double* out_val, uint32_t* out_cnt);
+B2P_API int b2p_topk_i64(b2p_ctx* ctx, int32_t bottom, double k, const int64_t* vals, const uint32_t* valid,
+                         const uint32_t* gid, uint32_t n_rows, uint32_t n_groups, const uint32_t* tie, uint64_t T,
+                         uint32_t* out_valid);
+B2P_API int b2p_count_values_i64(b2p_ctx* ctx, const int64_t* vals, const uint32_t* valid, const uint32_t* gid,
+                                 uint32_t n_rows, uint32_t n_groups, uint64_t T, int64_t* out_val, uint32_t* out_cnt);
+B2P_API int b2p_sort_cells_i64(b2p_ctx* ctx, int32_t desc, const int64_t* vals, const uint32_t* valid, uint32_t n_rows,
+                               uint64_t T, uint64_t* out_cells, uint64_t* out_n);
+B2P_API int b2p_i64_to_f64(b2p_ctx* ctx, const int64_t* vals, uint64_t n, double* out);
 
 /* Host-pointer forms of b2p_instant_fn_dev / b2p_scalar_calculate_dev (synchronous; device-found errors returned). */
 B2P_API int b2p_instant_fn(b2p_ctx* ctx, int32_t fn, double arg0, double arg1, const double* vals, const uint32_t* valid,

@@ -348,6 +348,31 @@ extern "C" {
         ctx: *mut b2p_ctx, desc: i32, vals: *const *const f64, n_fields: i32, valid: *const u32, n_rows: u32, t: u64,
         out_cells: *mut u64, out_n: *mut u64,
     ) -> c_int;
+    /// Int64 (BIGINT) value columns: the cells hold i64 bits in the same 8-byte slots.  The instant selector with field 0
+    /// Int64 (no stale-NaN test); the by-label aggregate (sum wrapping, min / max signed, written as i64 bits; avg,
+    /// stddev, stdvar over (f64)i64); topk / count_values / sort ranking by signed value; the Float64 coercion.
+    pub fn b2p_instant_select_fields_i64_dev(
+        ctx: *mut b2p_ctx, start: i64, end: i64, interval: i64, lookback: i64, offset: i64, ts: *const i64,
+        vals: *const *const f64, field_valid: *const *const u8, n_fields: i32, offsets: *const u64, n_rows: u64,
+        n_series: u32, outs: *const *mut f64, valid_words: *mut u32,
+    ) -> c_int;
+    pub fn b2p_group_aggregate_i64_dev(
+        ctx: *mut b2p_ctx, agg: i32, vals: *const i64, valid_words: *const u32, gid: *const u32, n_series: u32,
+        n_groups: u32, t: u64, out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    pub fn b2p_topk_i64_dev(
+        ctx: *mut b2p_ctx, bottom: i32, k: f64, vals: *const i64, valid: *const u32, index: *const b2p_group_index,
+        tie: *const u32, t: u64, out_valid: *mut u32,
+    ) -> c_int;
+    pub fn b2p_count_values_i64_dev(
+        ctx: *mut b2p_ctx, vals: *const i64, valid: *const u32, index: *const b2p_group_index, t: u64,
+        out_val: *mut i64, out_cnt: *mut u32,
+    ) -> c_int;
+    pub fn b2p_sort_cells_i64_dev(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const i64, valid: *const u32, n_rows: u32, t: u64, out_cells: *mut u64,
+        out_n: *mut u64,
+    ) -> c_int;
+    pub fn b2p_i64_to_f64_dev(ctx: *mut b2p_ctx, vals: *const i64, n: u64, out: *mut f64) -> c_int;
     /// absent (K15): out_valid [Tw] = the steps at which no row of the device grid's validity [n_rows x Tw] has a bit
     /// (bits past T cleared), out [T] = 1.0 there and 0.0 elsewhere.  Only validity words are read; no host round trip.
     pub fn b2p_absent_dev(
@@ -454,6 +479,29 @@ extern "C" {
         ctx: *mut b2p_ctx, desc: i32, vals: *const *const f64, n_fields: i32, valid: *const u32, n_rows: u32, t: u64,
         out_cells: *mut u64, out_n: *mut u64,
     ) -> c_int;
+    /// Host-pointer forms of the Int64 calls (synchronous).
+    pub fn b2p_instant_select_fields_i64(
+        ctx: *mut b2p_ctx, start: i64, end: i64, interval: i64, lookback: i64, offset: i64, ts: *const i64,
+        vals: *const *const f64, field_valid: *const *const u8, n_fields: i32, sid: *const u32,
+        offsets_host: *const u64, n_rows: u64, n_series: u32, outs: *const *mut f64, valid_words: *mut u32,
+    ) -> c_int;
+    pub fn b2p_group_aggregate_i64(
+        ctx: *mut b2p_ctx, agg: i32, vals: *const i64, valid_words: *const u32, gid: *const u32, n_series: u32,
+        n_groups: u32, t: u64, out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    pub fn b2p_topk_i64(
+        ctx: *mut b2p_ctx, bottom: i32, k: f64, vals: *const i64, valid: *const u32, gid: *const u32, n_rows: u32,
+        n_groups: u32, tie: *const u32, t: u64, out_valid: *mut u32,
+    ) -> c_int;
+    pub fn b2p_count_values_i64(
+        ctx: *mut b2p_ctx, vals: *const i64, valid: *const u32, gid: *const u32, n_rows: u32, n_groups: u32, t: u64,
+        out_val: *mut i64, out_cnt: *mut u32,
+    ) -> c_int;
+    pub fn b2p_sort_cells_i64(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const i64, valid: *const u32, n_rows: u32, t: u64, out_cells: *mut u64,
+        out_n: *mut u64,
+    ) -> c_int;
+    pub fn b2p_i64_to_f64(ctx: *mut b2p_ctx, vals: *const i64, n: u64, out: *mut f64) -> c_int;
     /// Host-pointer form of b2p_absent_dev (synchronous).
     pub fn b2p_absent(
         ctx: *mut b2p_ctx, valid: *const u32, n_rows: u32, t: u64, out: *mut f64, out_valid: *mut u32,

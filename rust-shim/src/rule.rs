@@ -112,11 +112,16 @@
 //! the CPU those the library refuses there (the leaf's own aggregate, filtering comparisons over two or more fields,
 //! topk / bottomk, count_values, group, scalar, set operators with a multi-field side, histogram_quantile).
 //!
+//! Every sub-tree the rule rewrites starts at a range selector, whose field columns must be Float64: over an Int64
+//! (BIGINT) column the library evaluates only the instant selector and the nodes above it (DESIGN §1 a25), which this
+//! rule does not rewrite, so a query over an Int64 column stays on the CPU as a whole.
+//!
 //! Anything that does not match exactly is left alone — the CPU operators keep running for it.  The rule lives in the
 //! `promql` crate (src/promql/src/gpu/rule.rs) so that it can read the nodes' fields; the handful of `pub(crate)`
 //! getters it needs are listed in `rust-shim/README.md`.
 use std::sync::Arc;
 
+use datafusion::arrow::datatypes::DataType;
 use datafusion::common::tree_node::{Transformed, TreeNode};
 use datafusion::common::{Result as DataFusionResult, ScalarValue};
 use datafusion::config::ConfigOptions;
@@ -230,6 +235,16 @@ impl GpuPromRewrite {
         let divide = normalize.input().as_any().downcast_ref::<SeriesDivideExec>()?;
         if !range_exec.field_columns().iter().eq(udfs.fields.iter()) {
             return None;
+        }
+        // the library's range leaf takes Float64 field columns only: a range function over an Int64 (BIGINT) column is
+        // refused at push (DESIGN §1 a25), and so is everything built on such a leaf (subquery, histogram_quantile,
+        // arithmetic between two Int64 sides, `or`, a filter over an Int64 lhs, a multi-field sort with an Int64 field),
+        // so any other field type keeps the whole sub-tree on the CPU
+        let schema = divide.input().schema();
+        for field in range_exec.field_columns() {
+            if schema.field_with_name(field).ok()?.data_type() != &DataType::Float64 {
+                return None;
+            }
         }
         let (param0, param1) = udfs.params;
         let params = GpuPromRangeParams {
