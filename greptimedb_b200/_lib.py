@@ -41,6 +41,8 @@ EXPORTED_SYMBOLS = [
     "b2p_instant_select_fields_i64_dev", "b2p_instant_select_fields_i64", "b2p_group_aggregate_i64_dev",
     "b2p_group_aggregate_i64", "b2p_topk_i64_dev", "b2p_topk_i64", "b2p_count_values_i64_dev", "b2p_count_values_i64",
     "b2p_sort_cells_i64_dev", "b2p_sort_cells_i64", "b2p_i64_to_f64_dev", "b2p_i64_to_f64",
+    "b2p_step_fn_dev", "b2p_step_fn", "b2p_instant_timestamp_dev", "b2p_instant_timestamp",
+    "b2p_plan_empty_metric_create", "b2p_plan_set_timestamp",
 ]
 
 
@@ -180,6 +182,12 @@ def load() -> C.CDLL:
         "b2p_i64_to_f64": (C.c_int, [vp, vp, u64, vp]),
         "b2p_plan_set_function": (C.c_int, [vp, C.c_char_p, C.POINTER(dbl), i32]),
         "b2p_plan_scalar_create": (vp, [vp, vp]),
+        "b2p_step_fn_dev": (C.c_int, [vp, i32, vp, vp, u64, u64, vp]),
+        "b2p_step_fn": (C.c_int, [vp, i32, vp, vp, u64, u64, vp]),
+        "b2p_instant_timestamp_dev": (C.c_int, [vp, i64, i64, i64, i64, i64, vp, vp, u64, u32, vp, vp]),
+        "b2p_instant_timestamp": (C.c_int, [vp, i64, i64, i64, i64, i64, vp, vp, vp, u64, u32, vp, vp]),
+        "b2p_plan_empty_metric_create": (vp, [vp, i64, i64, i64, C.c_char_p, C.c_char_p, i32, dbl]),
+        "b2p_plan_set_timestamp": (C.c_int, [vp, i64]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)  # AttributeError here means the .so does not match the header

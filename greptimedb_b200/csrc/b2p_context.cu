@@ -35,6 +35,8 @@ int k0_fail(uint32_t k0) {
   if (k0 & kScalarKeyError) return fail(B2P_E_INVALID, "scalar(): a row's series key is >= n_rows");
   if (k0 & kScalarOverlapError)
     return fail(B2P_E_INVALID, "scalar(): two rows of one series have a cell at the same step");
+  if (k0 & kStepRangeError)
+    return fail(B2P_E_INVALID, "step function: an eval timestamp's year is outside [-262143, 262143]");
   if (k0 & 1u) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");
   return fail(B2P_E_UNSORTED, "series id >= n_series");
 }

@@ -8,6 +8,7 @@
 #include "b2p_binary.cuh"
 #include "b2p_instant.cuh"
 #include "b2p_setop.cuh"
+#include "b2p_time.cuh"
 
 using namespace b2p;
 
@@ -78,11 +79,35 @@ int instant_fn_bounds(int32_t fn, double arg0, double arg1, int* kfn, double* lo
   if (fn == B2P_IFN_CLAMP_MIN) *hi = DBL_MAX;
   if (fn == B2P_IFN_CLAMP_MAX) *lo = -DBL_MAX, *hi = arg0;
   if (fn == B2P_IFN_CLAMP_MIN || fn == B2P_IFN_CLAMP_MAX) *kfn = B2P_IFN_CLAMP;
-  if (fn < 0 || fn >= B2P_IFN__COUNT) return fail(B2P_E_INVALID, "unknown instant function %d", fn);
+  if (fn == B2P_IFN_NEG) *kfn = kFnNeg;
+  if (fn < 0 || (fn >= B2P_IFN__COUNT && fn != B2P_IFN_NEG)) return fail(B2P_E_INVALID, "unknown instant function %d", fn);
   if (*kfn == B2P_IFN_CLAMP && *lo > *hi) return fail(B2P_E_INVALID, "clamp: min %.17g > max %.17g", *lo, *hi);
   return B2P_OK;
 }
-static_assert((int)B2P_IFN_CLAMP == (int)kFnClamp && (int)B2P_IFN_CLAMP + 1 == (int)kFnKernelCount, "enum b2p_ifn and InstantFn disagree");
+static_assert((int)B2P_IFN_CLAMP == (int)kFnClamp && (int)kFnNeg + 1 == (int)kFnKernelCount,
+              "enum b2p_ifn and InstantFn disagree");
+static_assert((int)B2P_STEP_TIME == (int)kPartTime && (int)B2P_STEP_DAYS_IN_MONTH == (int)kPartDaysInMonth &&
+                  (int)B2P_STEP__COUNT == (int)kPartCount, "enum b2p_step_part and StepPart disagree");
+
+// K19: one CTA per (W steps, slab of rows); at most 16 CTAs per SM, the rows grid-strided beyond that
+int step_fn_run(b2p_ctx* c, int32_t part, const int64_t* eval_ts, const uint32_t* valid, uint64_t n_rows, uint64_t T,
+                double* out) {
+  StepFnArgs a{};
+  a.eval_ts = eval_ts; a.valid = valid; a.n_rows = n_rows; a.T = T; a.Tw = (uint32_t)((T + 31) / 32); a.out = out;
+  a.status = c->d_k0;
+  a.W = step_fn_width(T);
+  const uint64_t gx = (T + a.W - 1) / a.W, rows_per_pass = kStepThreads / a.W;
+  const uint64_t cap = std::max<uint64_t>(1, (uint64_t)c->num_sms * 16 / gx);
+  const uint64_t gy = std::min<uint64_t>(std::min<uint64_t>((n_rows + rows_per_pass - 1) / rows_per_pass, cap), 65535);
+  if (gx > INT32_MAX) return fail(B2P_E_TOO_LARGE, "step function: %llu steps", (unsigned long long)T);
+  const dim3 grid((unsigned)gx, (unsigned)gy);
+  return with_id<kPartCount>(part, "step part", [&](auto k) {
+    step_fn_kernel<decltype(k)::value><<<grid, kStepThreads, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    return B2P_OK;
+  });
+}
 
 // the scalar() reduction and write pass; the verdict stays on the device
 int scalar_calculate_run(b2p_ctx* c, const ScalarArgs& a0) {
@@ -349,6 +374,21 @@ int b2p_absent_dev(b2p_ctx* c, const uint32_t* valid, uint32_t n_rows, uint64_t 
   return rc;
 }
 
+/* ---- functions of the eval step ------------------------------------------------------------------------------ */
+
+int b2p_step_fn_dev(b2p_ctx* c, int32_t part, const int64_t* eval_ts, const uint32_t* valid, uint64_t n_rows,
+                    uint64_t T, double* out) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (part < 0 || part >= kPartCount) return fail(B2P_E_INVALID, "unknown step part %d", part);
+  if (n_rows == 0 || T == 0) return B2P_OK;
+  if (!eval_ts || !valid || !out) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  const int rc = step_fn_run(c, part, eval_ts, valid, n_rows, T, out);
+  stage_end(c, 3);
+  return rc;
+}
+
 /* ---- set operators ------------------------------------------------------------------------------------------- */
 
 int b2p_setop_dev(b2p_ctx* c, int32_t op, const double* lhs, const uint32_t* lhs_valid, const uint32_t* lhs_key,
@@ -453,6 +493,19 @@ int b2p_instant_fn(b2p_ctx* c, int32_t fn, double arg0, double arg1, const doubl
   double* d_out = s.copy_back(out, d_vals, vb);
   uint32_t* d_out_valid = out_valid == valid ? d_valid : s.copy_back(out_valid, d_valid, wb);
   return s.end([&] { return b2p_instant_fn_dev(c, fn, arg0, arg1, d_vals, d_valid, n_rows, T, d_out, d_out_valid); });
+}
+
+int b2p_step_fn(b2p_ctx* c, int32_t part, const int64_t* eval_ts, const uint32_t* valid, uint64_t n_rows, uint64_t T,
+                double* out) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  Staging s{c};
+  const int64_t* d_ts = s.in(eval_ts, (size_t)T * 8);
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
+  double* d_out = s.out(out, (size_t)n_rows * T * 8);
+  const int rc = s.end([&] { return b2p_step_fn_dev(c, part, d_ts, d_valid, n_rows, T, d_out); }, false);
+  return rc ? rc : take_row_error(c, kStepRangeError);  // (synchronises)
 }
 
 int b2p_i64_to_f64(b2p_ctx* c, const int64_t* vals, uint64_t n, double* out) {

@@ -1,7 +1,8 @@
 // b2p_instant.cuh — PromQL instant-vector math functions and scalar() over dense [rows x T] grids:
 //   K9 instant_fn_kernel<FN, VEC>   fn(v) per cell: abs ceil floor sqrt exp ln log2 log10, the trigonometric and
 //                                    hyperbolic functions, round, deg, rad, sgn, clamp (clamp_min / clamp_max are
-//                                    clamp with one bound at ∓f64::MAX, chosen by the caller)
+//                                    clamp with one bound at ∓f64::MAX, chosen by the caller), and unary minus
+//                                    (the sign bit flipped: -0.0 from 0.0 and a NaN's sign, as Rust's f64 Neg)
 //      scalar_reduce_kernel          scalar(): live rows, their min / max series key, live cells on B2P_NO_KEY rows
 //      scalar_write_kernel           scalar(): the one series' cells, or NaN at every step
 //      i64_to_f64_kernel             an Int64 grid read as Float64 ((double)i64, round to nearest): what DataFusion's
@@ -41,6 +42,7 @@ namespace b2p {
 enum InstantFn {
   kFnAbs = 0, kFnCeil, kFnFloor, kFnSqrt, kFnExp, kFnLn, kFnLog2, kFnLog10, kFnSin, kFnCos, kFnTan, kFnAsin, kFnAcos,
   kFnAtan, kFnSinh, kFnCosh, kFnTanh, kFnAsinh, kFnAcosh, kFnAtanh, kFnRound, kFnDeg, kFnRad, kFnSgn, kFnClamp,
+  kFnNeg,         // B2P_IFN_NEG
   kFnKernelCount  // clamp_min / clamp_max (ids kFnClamp + 1, + 2) run as kFnClamp
 };
 constexpr uint32_t kScalarNoKey = 0xFFFFFFFFu;
@@ -82,6 +84,7 @@ __device__ __forceinline__ double instant_fn(double v, double a0, double a1) {
   if (FN == kFnDeg) return __dmul_rn(v, 57.29577951308232);       // 180.0 / π in f64 (Rust's to_degrees constant)
   if (FN == kFnRad) return __dmul_rn(v, 0.017453292519943295);    // π / 180.0 in f64 (Rust's to_radians)
   if (FN == kFnSgn) return v == 0.0 ? 0.0 : v != v ? v : (v < 0.0 ? -1.0 : 1.0);
+  if (FN == kFnNeg) return __longlong_as_double(__double_as_longlong(v) ^ (long long)0x8000000000000000ull);
   return v < a0 ? a0 : v > a1 ? a1 : v;  // kFnClamp
 }
 

@@ -873,6 +873,9 @@ __global__ void __launch_bounds__(128) range_udf_kernel(const int64_t* __restric
 // K4: InstantManipulate (instant_manipulate.rs:473-585).  Warp per series, lane per eval step:
 // newest sample with t - lookback < ts <= t; a NaN newest sample is a stale marker -> no row.
 // (lookback == 0 selects ts == t only, matching the reference's cursor walk.)
+// TIMESTAMP: timestamp(<selector>), where the reference projects ts / 1000 into the value column before
+// InstantManipulate (planner.rs:905-909, 951-965): the chosen row's shifted timestamp (ts + offset) as
+// (double)t / 1000.0, no value read and no stale-NaN test (a selected stale-NaN sample is kept).
 // ---------------------------------------------------------------------------------------------
 struct InstantArgs {
   int64_t start, end, interval, lookback, offset;
@@ -886,6 +889,7 @@ struct InstantArgs {
   uint32_t* valid;
 };
 
+template <bool TIMESTAMP>
 __global__ void __launch_bounds__(kWarpsPerCta * 32) instant_kernel(const InstantArgs a) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t total_warps = gridDim.x * kWarpsPerCta;
@@ -895,7 +899,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) instant_kernel(const Instan
     double* out_s = a.out + (size_t)s * (size_t)a.T;
     uint32_t* vw_s = a.valid + (size_t)s * a.Tw;
     const int64_t* ts = a.ts + row0;
-    const double* val = a.val + row0;
+    const double* val = a.val + row0;  // (not read in TIMESTAMP mode)
     int64_t k_lo = a.T, k_hi = -1;
     if (n > 0) {
       const int64_t first_ts = ts[0] + a.offset, last_ts = ts[n - 1] + a.offset;
@@ -930,8 +934,13 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) instant_kernel(const Instan
             while (j > 0 && ts[j - 1] + a.offset == te) --j;
           const bool fresh = (a.lookback > 0) ? (t + a.lookback > te) : (t == te);
           if (fresh) {
-            const double v = val[j];
-            if (!isnan(v)) { ok = true; r = v; }
+            if constexpr (TIMESTAMP) {
+              ok = true;
+              r = (double)t / 1000.0;
+            } else {
+              const double v = val[j];
+              if (!isnan(v)) { ok = true; r = v; }
+            }
           }
         }
       }

@@ -59,6 +59,12 @@ void check(int rc, ErrorKind invalid = ErrorKind::Plan) {
   throw PlanError(rc == B2P_E_UNSORTED ? ErrorKind::Internal : ErrorKind::Execution, b2p_last_error());
 }
 
+// The nodes that read an Int32 (calendar) column as a number other than element-wise: DataFusion's integer result
+// types for them are not pinned by the reference tree, so the query stays on the CPU
+void refuse_i32(const NodeResult& r, const char* node) {
+  if (r.any_i32()) throw PlanError(ErrorKind::Plan, std::string(node) + ": an Int32 value column is not supported by this node");
+}
+
 // Field f of r read as Float64 from here on: an Int64 field is coerced on the device ((double)i64, b2p_i64_to_f64), as
 // DataFusion coerces an Int64 column under a Float64 projection, aggregate or scalar()
 void field_to_f64(b2p_ctx* ctx, NodeResult& r, uint32_t f) {
@@ -84,6 +90,7 @@ struct KeyIds {
 // ---- export helpers: an ArrowArray whose buffers live in a heap object ---------------------------------
 struct OwnedColumn {
   std::vector<int64_t> i64;
+  std::vector<int32_t> i32;
   std::vector<double> f64;
   std::vector<int32_t> offsets;
   std::string chars;
@@ -620,19 +627,23 @@ void PromRangePlan::compute(NodeResult& r) {
   offsets_.resize((size_t)S);          // (a previous execute() appended the end marker)
   offsets_.push_back((uint64_t)ts_.size());
   const uint32_t Tw = (uint32_t)((T + 31) / 32);
-  const uint32_t F = (uint32_t)args_.field_columns.size();
+  // timestamp(): one Float64 value whatever the fields, DEFAULT_FIELD_COLUMN (planner.rs:951-965); no value is read
+  const uint32_t F = timestamp_ ? 1u : (uint32_t)args_.field_columns.size();
   const bool fold_on_device = args_.histogram && fn_id_ >= 0;  // the dense matrix then never reaches the host
   const size_t cells = (size_t)S * (size_t)T;
   std::vector<double> dense(fold_on_device ? 0 : F * cells);
   std::vector<uint32_t> valid(fold_on_device ? 0 : (size_t)S * Tw);
-  const bool int0 = !types_.empty() && types_[0] == ValueType::Int64;  // (only the instant selector takes Int64)
-  if (S > 0 && T > 0 && !fold_on_device && F == 1 && !int0)
+  const bool int0 = !timestamp_ && !types_.empty() && types_[0] == ValueType::Int64;  // (only the instant selector)
+  if (S > 0 && T > 0 && timestamp_)
+    check(b2p_instant_timestamp(ctx_, p.start, p.end, p.interval, args_.lookback_delta, p.offset, ts_.data(), nullptr,
+                                offsets_.data(), ts_.size(), S, dense.data(), valid.data()));
+  else if (S > 0 && T > 0 && !fold_on_device && F == 1 && !int0)
     check(fn_id_ >= 0 ? b2p_range_eval(ctx_, &p, ts_.data(), val_[0].data(), nullptr, offsets_.data(), ts_.size(), S,
                                        dense.data(), valid.data(), nullptr)
                       : b2p_instant_select(ctx_, p.start, p.end, p.interval, args_.lookback_delta, p.offset, ts_.data(),
                                            val_[0].data(), nullptr, offsets_.data(), ts_.size(), S, dense.data(),
                                            valid.data()));  // InstantManipulate
-  if (S > 0 && T > 0 && (F > 1 || int0)) {
+  if (S > 0 && T > 0 && !timestamp_ && (F > 1 || int0)) {
     std::vector<const double*> vals(F);
     std::vector<double*> outs(F);
     std::vector<const uint8_t*> present(F);
@@ -661,9 +672,10 @@ void PromRangePlan::compute(NodeResult& r) {
   r.eval_ts.resize((size_t)T);  // also when there are no series: scalar() of such a node has a NaN row at every step
   for (int64_t k = 0; k < T; ++k) r.eval_ts[(size_t)k] = p.start + k * p.interval;
   r.time_index = args_.time_index;
-  if (std::find(types_.begin(), types_.end(), ValueType::Int64) != types_.end()) r.types = types_;
+  if (!timestamp_ && std::find(types_.begin(), types_.end(), ValueType::Int64) != types_.end()) r.types = types_;
   for (const std::string& field : args_.field_columns)
     r.value_names.push_back(fn_id_ >= 0 ? args_.function + "(" + args_.time_index + "_range," + field + ")" : field);
+  if (timestamp_) r.value_names = {"value"};
 
   if (args_.histogram) {
     // HistogramFold (histogram_fold.rs:754-820): group the series by their tags without `le`, order each group's
@@ -698,7 +710,8 @@ void PromRangePlan::compute(NodeResult& r) {
 
 namespace {
 
-const char* const kOpSymbols[] = {"+", "-", "*", "/", "%", "^", "atan2", "==", "!=", ">", "<", ">=", "<="};
+// as DataFusion displays the operators in a projection's name (Operator::Eq is "=")
+const char* const kOpSymbols[] = {"+", "-", "*", "/", "%", "^", "atan2", "=", "!=", ">", "<", ">=", "<="};
 
 bool is_comparison(int op) { return op >= B2P_OP_EQ && op <= B2P_OP_LE; }
 
@@ -746,7 +759,8 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
   const bool int_val = r.columns == Columns::CountTagsTimeLabel && r.value_is_count;
   if (r.value_names.size() != r.F) throw PlanError(ErrorKind::Internal, "export: one value name per field expected");
   auto add_vals = [&](const char* fmt) {  // "g" is each field's own type
-    for (uint32_t f = 0; f < r.F; ++f) c_vals.push_back(add_col(r.value_names[f], r.is_i64(f) ? "l" : fmt));
+    for (uint32_t f = 0; f < r.F; ++f)
+      c_vals.push_back(add_col(r.value_names[f], r.is_i64(f) ? "l" : r.is_i32(f) ? "i" : fmt));
   };
   switch (r.columns) {
     case Columns::TimeValueTags:
@@ -776,7 +790,8 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       names.push_back(r.value_names[0]);
       std::sort(names.begin(), names.end());
       for (const std::string& name : names) {
-        if (name == r.value_names[0] && c_vals.empty()) c_vals.push_back(add_col(name, r.is_i64(0) ? "l" : "g"));
+        if (name == r.value_names[0] && c_vals.empty())
+          c_vals.push_back(add_col(name, r.is_i64(0) ? "l" : r.is_i32(0) ? "i" : "g"));
         else add_tag((size_t)L.column(name));
       }
       break;
@@ -797,6 +812,7 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       const double v = r.field(f)[(size_t)row * (size_t)r.T + (size_t)k];
       if (int_val) c_vals[f]->i64.push_back((int64_t)v);
       else if (r.is_i64(f)) c_vals[f]->i64.push_back(bits_i64(v));
+      else if (r.is_i32(f)) c_vals[f]->i32.push_back((int32_t)v);
       else c_vals[f]->f64.push_back(v);
     }
     if (c_label) {
@@ -850,7 +866,9 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       a.n_buffers = 3;
     } else {
       c->buffers[0] = nullptr;
-      c->buffers[1] = (fmt == "g") ? static_cast<const void*>(c->f64.data()) : static_cast<const void*>(c->i64.data());
+      c->buffers[1] = fmt == "g"   ? static_cast<const void*>(c->f64.data())
+                      : fmt == "i" ? static_cast<const void*>(c->i32.data())
+                                   : static_cast<const void*>(c->i64.data());
       a.n_buffers = 2;
     }
     a.buffers = c->buffers;
@@ -905,6 +923,28 @@ const FnName kInstantFns[] = {
     {"clamp", B2P_IFN_CLAMP, 2, 2},   {"clamp_min", B2P_IFN_CLAMP_MIN, 1, 1}, {"clamp_max", B2P_IFN_CLAMP_MAX, 1, 1},
 };
 
+// the calendar functions: PromQL name, enum b2p_step_part and the date_part field DataFusion is asked for
+// (planner.rs:2222-2300); days_in_month is named after its whole expression (date_part_name)
+struct StepFnName {
+  const char* name;
+  int part;
+  const char* field;
+};
+const StepFnName kStepFns[] = {
+    {"minute", B2P_STEP_MINUTE, "minute"},     {"hour", B2P_STEP_HOUR, "hour"},
+    {"month", B2P_STEP_MONTH, "month"},        {"year", B2P_STEP_YEAR, "year"},
+    {"day_of_month", B2P_STEP_DAY_OF_MONTH, "day"}, {"day_of_week", B2P_STEP_DAY_OF_WEEK, "dow"},
+    {"day_of_year", B2P_STEP_DAY_OF_YEAR, "doy"}, {"days_in_month", B2P_STEP_DAYS_IN_MONTH, nullptr},
+};
+
+// the value column of a calendar stage as the reference's projection names it over the time index
+std::string date_part_name(const Stage& s, const std::string& ti) {
+  if (s.part == B2P_STEP_DAYS_IN_MONTH)
+    return "date_part(Utf8(\"day\"),date_trunc(Utf8(\"month\")," + ti +
+           ") + IntervalYearMonth(\"1\") - IntervalDayTime(\"IntervalDayTime { days: 1, milliseconds: 0 }\"))";
+  return "date_part(Utf8(\"" + s.fn_name + "\")," + ti + ")";
+}
+
 // an f64 as Rust's Display writes it: the shortest digits that round-trip, never an exponent ("12", "0.5", "inf")
 std::string rust_display(double x) {
   if (std::isnan(x)) return "NaN";
@@ -926,6 +966,17 @@ void PlanNode::add_scalar_op(int op, double scalar, bool scalar_on_left, bool re
 }
 
 void PlanNode::add_function(const std::string& name, const std::vector<double>& args) {
+  if (name == "negative" || std::any_of(std::begin(kStepFns), std::end(kStepFns), [&](const StepFnName& f) { return name == f.name; })) {
+    if (!args.empty()) throw PlanError(ErrorKind::Plan, name + " takes 0 argument(s) after the vector, got " + std::to_string(args.size()));
+    Stage s;
+    s.is_fn = true;
+    s.op = B2P_IFN_NEG;
+    s.fn_name = name;
+    for (const StepFnName& f : kStepFns)
+      if (name == f.name) s.part = f.part, s.fn_name = f.field ? f.field : "";
+    stages_.push_back(s);
+    return;
+  }
   for (const FnName& f : kInstantFns) {
     if (name != f.name) continue;
     const int n = (int)args.size();
@@ -950,11 +1001,28 @@ void PlanNode::run(NodeResult& r) {
   if (!stages_.empty()) r.value_is_count = false;  // a stage's result is a Float64 projection
   for (const Stage& s : stages_) {
     const bool work = r.rows > 0 && r.T > 0;
+    if (s.part >= 0) {
+      // a calendar function: one date_part projection over the time index whatever the node's fields, typed Int32
+      // (DataFusion's date_part width; not in the reference tree), labels and validity kept (K19)
+      r.F = 1;
+      r.val.resize(r.grid());
+      if (work)
+        check(b2p_step_fn(ctx_, s.part, r.eval_ts.data(), r.valid.data(), r.rows, (uint64_t)r.T, r.field(0)));
+      r.types = {ValueType::Int32};
+      r.value_names = {date_part_name(s, r.time_index)};
+      continue;
+    }
+    if (s.is_fn && s.op == B2P_IFN_NEG && (r.any_i64() || r.any_i32()))  // integer negation and its overflow
+      throw PlanError(ErrorKind::Plan, "unary minus over an integer value column is not supported by this node");
     // an Int64 value column under a stage: a filter would keep the Int64 column, which the reference tree does not
     // pin; a projection reads it as Float64 (DataFusion's coercion against the Float64 literal or function)
     if (r.any_i64() && !s.is_fn && is_comparison(s.op) && !s.return_bool)
       throw PlanError(ErrorKind::Plan, "a filtering comparison over an Int64 value column is not supported by this node");
+    // an Int32 (calendar) column: a filter keeps it, every projection reads it as Float64 (its cells already are)
+    const std::vector<ValueType> kept = r.any_i32() && !s.is_fn && is_comparison(s.op) && !s.return_bool
+                                            ? r.types : std::vector<ValueType>{};
     to_f64(ctx_, r);
+    r.types = kept;
     if (s.is_fn) {
       const double a0 = s.args.size() > 0 ? s.args[0] : 0.0, a1 = s.args.size() > 1 ? s.args[1] : 0.0;
       // clamp's bound check (clamp.rs:212-217); clamp_min / clamp_max meet the other bound at ±f64::MAX.  The reference
@@ -969,6 +1037,10 @@ void PlanNode::run(NodeResult& r) {
         check(b2p_instant_fn(ctx_, s.op, a0, a1, r.field(f), r.valid.data(), r.rows, (uint64_t)r.T, r.field(f),
                              r.valid.data()));
       for (std::string& value : r.value_names) {
+        if (s.op == B2P_IFN_NEG) {
+          value = "(- " + value + ")";
+          continue;
+        }
         std::string name = s.fn_name + "(" + value;
         for (double a : s.args) name += "," + float_literal(a);
         value = name + ")";
@@ -1012,12 +1084,30 @@ void BinaryPlan::compute(NodeResult& r) {
   lhs_->run(L);
   rhs_->run(R);
   if (L.T != R.T) throw PlanError(ErrorKind::Plan, "both sides of a binary operator must be evaluated on the same steps");
+  // `scalar cmp vector`: the reference filters the vector and keeps its rows, labels, values and time index
+  // (planner.rs:765-771, project_binary_join_side on the right).  time() is scalar-typed, so it is evaluated as
+  // `vector cmp' scalar` with the mirrored comparison; an EmptyMetric literal may be vector(s), whose matching this
+  // layer does not model there, so that shape is refused.
+  int op = op_;
+  if (is_comparison(op_) && !return_bool_ && !R.scalar_like && !R.literal_row) {
+    if (L.literal_row)
+      throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: a filtering comparison with a literal EmptyMetric lhs against a vector is not supported by this node");
+    if (L.scalar_like) {
+      std::swap(L, R);
+      op = op_ == B2P_OP_GT ? B2P_OP_LT : op_ == B2P_OP_LT ? B2P_OP_GT : op_ == B2P_OP_GE ? B2P_OP_LE
+           : op_ == B2P_OP_LE ? B2P_OP_GE : op_;  // (== and != are symmetric)
+    }
+  }
   // Int64 operands: against a Float64 side DataFusion coerces to Float64; between two Int64 sides it would run integer
   // arithmetic, division and overflow, which the reference tree does not pin, and a filter would keep the Int64 column
   for (uint32_t f = 0; f < std::min(L.F, R.F); ++f)
     if (L.is_i64(f) && R.is_i64(f))
       throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: a binary operator between two Int64 value columns is not supported by this node");
-  if (L.any_i64() && is_comparison(op_) && !return_bool_)
+  // an Int32 (calendar) side meets a Float64 side only: DataFusion's integer result types are not pinned here
+  if ((L.any_i32() && (R.any_i32() || R.any_i64())) || (R.any_i32() && L.any_i64()))
+    throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: a binary operator between two integer value columns is not supported by this node");
+  const std::vector<ValueType> lhs_i32 = L.any_i32() ? L.types : std::vector<ValueType>{};
+  if (L.any_i64() && is_comparison(op) && !return_bool_)
     throw PlanError(ErrorKind::Plan, "a filtering comparison over an Int64 value column is not supported by this node");
   to_f64(ctx_, L);
   to_f64(ctx_, R);
@@ -1057,7 +1147,7 @@ void BinaryPlan::compute(NodeResult& r) {
   if (n_pairs > UINT32_MAX) throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: more than 2^32 - 1 matched series pairs");
   // the fields zip pairwise, field i with field i (align_binary_field_columns, planner.rs:3401-3414); a filter decides
   // on its one pair and keeps every field of the lhs
-  const bool filter = is_comparison(op_) && !return_bool_;
+  const bool filter = is_comparison(op) && !return_bool_;
   const uint32_t pairs = std::min(L.F, R.F);
   if (filter && pairs > 1) throw PlanError(ErrorKind::Plan, "Unsupported expr type: filter on multi-value input");
   r = NodeResult();
@@ -1069,7 +1159,7 @@ void BinaryPlan::compute(NodeResult& r) {
   r.val.assign((size_t)r.F * n_pairs * (size_t)r.T, 0.0);
   r.valid.assign((size_t)n_pairs * r.Tw, 0u);
   for (uint32_t f = 0; f < pairs && n_pairs > 0 && r.T > 0; ++f)  // arithmetic and `bool` keep the join's bits
-    check(b2p_binary_op(ctx_, op_, return_bool_ ? 1 : 0, L.field(f), L.valid.data(), lrow.data(), L.rows, R.field(f),
+    check(b2p_binary_op(ctx_, op, return_bool_ ? 1 : 0, L.field(f), L.valid.data(), lrow.data(), L.rows, R.field(f),
                         R.valid.data(), rrow.data(), R.rows, n_pairs, (uint64_t)r.T, r.field(f), r.valid.data()));
   // the lhs's other fields at the cells the comparison kept; a dropped cell holds 0.0, as the kernel writes it
   for (uint32_t f = 1; filter && f < r.F; ++f)
@@ -1087,6 +1177,7 @@ void BinaryPlan::compute(NodeResult& r) {
   r.labels = side.labels.gather(srow);
   if (filter) {
     r.columns = L.columns;
+    r.types = lhs_i32;  // a filter keeps the lhs column and its type
     r.value_names = L.value_names;
     r.label_name = L.label_name;
     r.label_is_i64 = L.label_is_i64;
@@ -1099,7 +1190,7 @@ void BinaryPlan::compute(NodeResult& r) {
   } else {
     r.columns = Columns::TagsTimeValue;
     for (uint32_t f = 0; f < r.F; ++f)
-      r.value_names.push_back(L.value_names[f] + " " + kOpSymbols[op_] + " " + R.value_names[f]);
+      r.value_names.push_back(L.value_names[f] + " " + kOpSymbols[op] + " " + R.value_names[f]);
   }
 }
 
@@ -1169,6 +1260,8 @@ void SetOpPlan::compute(NodeResult& r) {
   // `and` / `unless` keep the lhs column and its type; `or` over an Int64 side is not pinned by the reference tree
   if (op_ == B2P_SET_OR && (L.any_i64() || R.any_i64()))
     throw PlanError(ErrorKind::Plan, what + "an Int64 value column is not supported by this node");
+  if (op_ == B2P_SET_OR && L.any_i32() != R.any_i32())  // `or` of Int32 with Int32 stays Int32
+    throw PlanError(ErrorKind::Plan, what + "an Int32 value column against another type is not supported by this node");
   if (L.F > 1)
     throw PlanError(ErrorKind::Plan, std::string("Multi fields calculation is not supported in ") +
                                          (op_ == B2P_SET_OR ? "OR operator" : "AND operator"));
@@ -1247,6 +1340,7 @@ void SetOpPlan::compute(NodeResult& r) {
                           rkey.data(), R.rows, (uint32_t)keys.ids.size(), (uint64_t)T, r.val.data(), r.valid.data()));
   r.time_index = L.time_index;
   r.value_names = L.value_names;
+  r.types = L.types;
   r.columns = Columns::TimeSorted;
   r.labels.names = all;
   r.labels.values.resize(all.size());
@@ -1267,6 +1361,7 @@ ScalarPlan::ScalarPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child) : PlanNode
 void ScalarPlan::compute(NodeResult& r) {
   NodeResult C;
   child_->run(C);
+  refuse_i32(C, "GpuPromScalarExec");
   if (C.F > 1) throw PlanError(ErrorKind::Plan, "Multi fields calculation is not supported in scalar");  // planner.rs:3155-3160
   to_f64(ctx_, C);  // scalar() of an Int64 node is Float64
   // one dense key per label tuple over the child's tag columns (a tagless child is one series, an id-keyed one is keyed
@@ -1409,6 +1504,7 @@ AggregatePlan::AggregatePlan(b2p_ctx* ctx, const std::string& op, double param, 
 
 void AggregatePlan::compute(NodeResult& r) {
   child_->run(r);
+  refuse_i32(r, "GpuPromAggregateExec");
   // the reference would re-attach the tag columns of an id-keyed input (ensure_tag_columns_available); this layer has
   // only the id, so it can group such a node as a whole and nothing else
   if (r.labels.id_keyed && modifier_ != Modifier::None)
@@ -1432,6 +1528,7 @@ CountValuesPlan::CountValuesPlan(b2p_ctx* ctx, std::string label, std::shared_pt
 
 void CountValuesPlan::compute(NodeResult& r) {
   child_->run(r);
+  refuse_i32(r, "GpuPromCountValuesExec");
   if (r.F > 1)  // planner.rs:2874-2879
     throw PlanError(ErrorKind::Plan, "Unsupported expr type: count_values on multi-value input");
   // keep_tsid is false for count_values (planner.rs:402): as for AggregatePlan, an id-keyed child groups as a whole only
@@ -1515,6 +1612,7 @@ SubqueryPlan::SubqueryPlan(b2p_ctx* ctx, std::string function, const b2p_range_p
 void SubqueryPlan::compute(NodeResult& r) {
   NodeResult C;
   child_->run(C);
+  refuse_i32(C, "GpuPromSubqueryExec");
   if (C.any_i64()) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: an Int64 value column is not supported by this node");
   const int64_t T_in = C.T;
   const int64_t step = T_in > 1 ? C.eval_ts[1] - C.eval_ts[0] : p_.interval;  // (one inner step: any positive step)
@@ -1565,6 +1663,7 @@ HistogramQuantilePlan::HistogramQuantilePlan(b2p_ctx* ctx, std::string le_column
 
 void HistogramQuantilePlan::compute(NodeResult& r) {
   child_->run(r);
+  refuse_i32(r, "GpuPromHistogramFoldExec");
   if (r.labels.id_keyed)
     throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: an id-keyed (__tsid) child carries no " + le_column_ + " label");
   if (r.columns == Columns::CountTagsTimeLabel)
@@ -1703,6 +1802,38 @@ void AbsentPlan::compute(NodeResult& r) {
   for (const auto& [name, value] : labels_) {
     r.labels.names.push_back(name);
     r.labels.values.push_back({Label(value)});
+  }
+}
+
+// ---- EmptyMetricPlan ---------------------------------------------------------------------------------
+EmptyMetricPlan::EmptyMetricPlan(b2p_ctx* ctx, Millisecond start, Millisecond end, Millisecond interval,
+                                 std::string time_index, std::string value_column, int kind, double literal)
+    : PlanNode(ctx), start_(start), end_(end), interval_(interval), time_index_(std::move(time_index)),
+      value_column_(std::move(value_column)), kind_(kind), literal_(literal) {
+  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuEmptyMetricExec: NULL context");
+  if (interval_ <= 0) throw PlanError(ErrorKind::Plan, "GpuEmptyMetricExec: interval must be positive");
+  if (kind_ < B2P_EMPTY_NONE || kind_ > B2P_EMPTY_LITERAL)
+    throw PlanError(ErrorKind::Plan, "GpuEmptyMetricExec: unknown kind " + std::to_string(kind_));
+}
+
+void EmptyMetricPlan::compute(NodeResult& r) {
+  r = NodeResult();
+  r.T = b2p_num_steps(start_, end_, interval_);
+  r.Tw = (uint32_t)((r.T + 31) / 32);
+  r.rows = r.T > 0 ? 1 : 0;
+  r.F = kind_ == B2P_EMPTY_NONE ? 0 : 1;
+  r.eval_ts.resize((size_t)r.T);
+  for (int64_t k = 0; k < r.T; ++k) r.eval_ts[(size_t)k] = start_ + k * interval_;
+  r.time_index = time_index_;
+  r.valid.assign((size_t)r.rows * r.Tw, ~0u);
+  r.val.assign((size_t)r.F * r.grid(), kind_ == B2P_EMPTY_LITERAL ? literal_ : 0.0);
+  if (kind_ == B2P_EMPTY_TIME) {  // time(): ts / 1000 (build_special_time_expr, empty_metric.rs:393-402), K19
+    if (r.rows > 0) check(b2p_step_fn(ctx_, B2P_STEP_TIME, r.eval_ts.data(), r.valid.data(), 1, (uint64_t)r.T, r.field(0)));
+    r.value_names = {time_index_ + " / " + float_literal(1000.0)};
+    r.scalar_like = true;
+  } else if (kind_ == B2P_EMPTY_LITERAL) {
+    r.value_names = {value_column_};
+    r.literal_row = true;
   }
 }
 
@@ -1919,6 +2050,20 @@ b2p_plan* b2p_plan_absent_create(b2p_ctx* ctx, int64_t start, int64_t end, int64
     }
     return std::make_shared<b2p::AbsentPlan>(ctx, start, end, interval, time_index, value_column, labels, child->node);
   });
+}
+
+b2p_plan* b2p_plan_empty_metric_create(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval,
+                                       const char* time_index, const char* value_column, int32_t kind, double literal) {
+  return create([&] {
+    if (!time_index || !value_column) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    return std::make_shared<b2p::EmptyMetricPlan>(ctx, start, end, interval, time_index, value_column, kind, literal);
+  });
+}
+
+int b2p_plan_set_timestamp(b2p_plan* plan, int64_t lookback_delta) {
+  if (!plan) return B2P_E_INVALID;
+  if (!plan->range()) return not_a_range_node();
+  return plan->range()->set_timestamp(lookback_delta);
 }
 
 int b2p_plan_set_instant(b2p_plan* plan, int64_t lookback_delta) {

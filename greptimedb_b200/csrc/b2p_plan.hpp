@@ -112,8 +112,9 @@ enum class Columns {
   None,                // no column at all: histogram_quantile over a child without the le tag (an EmptyRelation)
 };
 
-// The Arrow type of a value column.  An Int64 cell holds the bits of its int64_t in the 8-byte slot of the grid.
-enum class ValueType { Float64, Int64 };
+// The Arrow type of a value column.  An Int64 cell holds the bits of its int64_t in the 8-byte slot of the grid; an Int32
+// cell (a calendar function's date_part) holds its exact value as a double, so Int32 changes only the export.
+enum class ValueType { Float64, Int64, Int32 };
 
 // What a node computed, before it becomes Arrow: F dense [rows x T] grids (one per field) under one validity, the eval
 // timestamps and one label tuple per row.  Exported, row r emits one Arrow row per valid step k (rows in order, steps
@@ -144,8 +145,12 @@ struct NodeResult {
   std::string label_name;
   bool value_is_count = false;
   bool label_is_i64 = false;  // count_values over an Int64 child: label_val holds int64_t bits, exported as Int64
+  // an EmptyMetric row: time() (scalar-typed in PromQL) or a literal (a scalar, or vector(s)); read by the binary node
+  bool scalar_like = false, literal_row = false;
   bool is_i64(uint32_t f) const { return f < types.size() && types[f] == ValueType::Int64; }
   bool any_i64() const { return std::find(types.begin(), types.end(), ValueType::Int64) != types.end(); }
+  bool is_i32(uint32_t f) const { return f < types.size() && types[f] == ValueType::Int32; }
+  bool any_i32() const { return std::find(types.begin(), types.end(), ValueType::Int32) != types.end(); }
   bool valid_at(uint32_t r, int64_t k) const { return (valid[(size_t)r * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u; }
   size_t grid() const { return (size_t)rows * (size_t)T; }
   double* field(uint32_t f) { return val.data() + f * grid(); }
@@ -157,6 +162,7 @@ struct NodeResult {
 struct Stage {
   bool is_fn = false;
   int op = 0;                 // enum b2p_binop; enum b2p_ifn when is_fn
+  int part = -1;              // enum b2p_step_part of a calendar stage (is_fn; `op` unused)
   double scalar = 0.0;
   bool scalar_on_left = false, return_bool = false;
   std::string fn_name;        // the function as the reference's projection names it ("abs", "prom_round", ...)
@@ -197,6 +203,12 @@ class PromRangePlan : public PlanNode {
     return 0;
   }
   void set_histogram(const std::string& le_column, double quantile);
+  // timestamp(<selector>): the instant form whose value is the chosen sample's timestamp in seconds (K4's timestamp
+  // mode); the result is one Float64 column named `value` whatever the table's fields
+  int set_timestamp(Millisecond lookback_delta) {
+    timestamp_ = true;
+    return set_instant(lookback_delta);
+  }
 
  protected:
   // runs the sub-plan on the device
@@ -206,6 +218,7 @@ class PromRangePlan : public PlanNode {
   PromRangePlanArgs args_;
   int fn_id_;
   int agg_id_;
+  bool timestamp_ = false;
   std::vector<int64_t> ts_;
   std::vector<std::vector<double>> val_;  // [field][row]; an Int64 field's rows hold int64_t bits
   std::vector<ValueType> types_;          // [field], set by the first batch
@@ -427,6 +440,26 @@ class AbsentPlan : public PlanNode {
   std::string time_index_, value_column_;
   std::vector<std::pair<std::string, std::string>> labels_;  // by name, one per name
   std::shared_ptr<PlanNode> child_;
+};
+
+// EmptyMetric(start, end, interval, time_index, field_column, field_expr) (empty_metric.rs): one tagless row over
+// start + k * interval <= end (none when start > end) with every cell valid, and a value column by `kind`: none
+// (B2P_EMPTY_NONE, only the time index), time() (B2P_EMPTY_TIME, `<time index> / Float64(1000)`, K19) or a number
+// (B2P_EMPTY_LITERAL: vector(s), pi(), a literal).  `hour()` and the other calendar functions without an argument are a
+// calendar stage on this node.  Plan errors at create: interval <= 0, a NULL name, an unknown kind.
+class EmptyMetricPlan : public PlanNode {
+ public:
+  EmptyMetricPlan(b2p_ctx* ctx, Millisecond start, Millisecond end, Millisecond interval, std::string time_index,
+                  std::string value_column, int kind, double literal);
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  Millisecond start_, end_, interval_;
+  std::string time_index_, value_column_;
+  int kind_;
+  double literal_;
 };
 
 int function_id_from_name(const std::string& prom_name);  // -1 when unknown

@@ -576,22 +576,43 @@ static int instant_grid(int64_t start, int64_t end, int64_t interval, int64_t lo
 
 extern "C" {
 
+}  // extern "C"
+
+// K4 over the grid `a`; `val` is not read (and may be NULL) in timestamp mode
+static int instant_select_run(b2p_ctx* c, InstantArgs& a, const int64_t* ts, const double* val, const uint64_t* offsets,
+                              uint64_t n_rows, double* out, uint32_t* valid_words, bool timestamp) {
+  if (a.n_series == 0 || a.T == 0) return B2P_OK;
+  if (!offsets || !out || !valid_words || ((!ts || (!val && !timestamp)) && n_rows))
+    return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  a.ts = ts; a.val = val; a.offsets = offsets; a.out = out; a.valid = valid_words;
+  stage_begin(c, 1);
+  (timestamp ? instant_kernel<true> : instant_kernel<false>)<<<capped_grid(c, a.n_series, kWarpsPerCta, 8),
+                                                               kWarpsPerCta * 32, 0, c->stream>>>(a);
+  c->launches++;
+  stage_end(c, 1);
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+extern "C" {
+
 int b2p_instant_select_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
                            const int64_t* ts, const double* val, const uint64_t* offsets, uint64_t n_rows,
                            uint32_t n_series, double* out, uint32_t* valid_words) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   InstantArgs a;
   if (int rc = instant_grid(start, end, interval, lookback, offset, n_series, &a)) return rc;
-  if (n_series == 0 || a.T == 0) return B2P_OK;
-  if (!offsets || !out || !valid_words || ((!ts || !val) && n_rows)) return fail(B2P_E_INVALID, "NULL argument");
-  DeviceGuard g(c->device);
-  a.ts = ts; a.val = val; a.offsets = offsets; a.out = out; a.valid = valid_words;
-  stage_begin(c, 1);
-  instant_kernel<<<capped_grid(c, n_series, kWarpsPerCta, 8), kWarpsPerCta * 32, 0, c->stream>>>(a);
-  c->launches++;
-  stage_end(c, 1);
-  CU(cudaGetLastError());
-  return B2P_OK;
+  return instant_select_run(c, a, ts, val, offsets, n_rows, out, valid_words, false);
+}
+
+int b2p_instant_timestamp_dev(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                              int64_t offset, const int64_t* ts, const uint64_t* offsets, uint64_t n_rows,
+                              uint32_t n_series, double* out, uint32_t* valid_words) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  InstantArgs a;
+  if (int rc = instant_grid(start, end, interval, lookback, offset, n_series, &a)) return rc;
+  return instant_select_run(c, a, ts, nullptr, offsets, n_rows, out, valid_words, true);
 }
 
 // n_fields and the two pointer arrays of a multi-field call; they must hold before the host form sizes its staging
@@ -1323,9 +1344,13 @@ int b2p_range_udf(b2p_ctx* c, int32_t fn_id, const int64_t* ts, const double* va
   });
 }
 
-int b2p_instant_select(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
-                       const int64_t* ts, const double* val, const uint32_t* sid, const uint64_t* offsets_host,
-                       uint64_t n_rows, uint32_t n_series, double* out, uint32_t* valid_words) {
+}  // extern "C"
+
+// the host forms of b2p_instant_select_dev and b2p_instant_timestamp_dev (val NULL: no value column is staged)
+static int instant_select_host(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                               int64_t offset, const int64_t* ts, const double* val, const uint32_t* sid,
+                               const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* out,
+                               uint32_t* valid_words, bool timestamp) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   InstantArgs grid;
   if (int rc = instant_grid(start, end, interval, lookback, offset, n_series, &grid)) return rc;
@@ -1336,10 +1361,28 @@ int b2p_instant_select(b2p_ctx* c, int64_t start, int64_t end, int64_t interval,
   double* d_out = s.out(out, (size_t)n_series * (size_t)grid.T * 8);
   uint32_t* d_valid = s.out(valid_words, (size_t)n_series * grid.Tw * 4);
   return s.end([&] {
-    const int rc = b2p_instant_select_dev(c, start, end, interval, lookback, offset, in.ts, in.val, in.offsets, n_rows,
-                                          n_series, d_out, d_valid);
+    const int rc = timestamp ? b2p_instant_timestamp_dev(c, start, end, interval, lookback, offset, in.ts, in.offsets,
+                                                         n_rows, n_series, d_out, d_valid)
+                             : b2p_instant_select_dev(c, start, end, interval, lookback, offset, in.ts, in.val,
+                                                      in.offsets, n_rows, n_series, d_out, d_valid);
     return rc ? rc : b2p_sync(c);
   });
+}
+
+extern "C" {
+
+int b2p_instant_select(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
+                       const int64_t* ts, const double* val, const uint32_t* sid, const uint64_t* offsets_host,
+                       uint64_t n_rows, uint32_t n_series, double* out, uint32_t* valid_words) {
+  return instant_select_host(c, start, end, interval, lookback, offset, ts, val, sid, offsets_host, n_rows, n_series,
+                             out, valid_words, false);
+}
+
+int b2p_instant_timestamp(b2p_ctx* c, int64_t start, int64_t end, int64_t interval, int64_t lookback, int64_t offset,
+                          const int64_t* ts, const uint32_t* sid, const uint64_t* offsets_host, uint64_t n_rows,
+                          uint32_t n_series, double* out, uint32_t* valid_words) {
+  return instant_select_host(c, start, end, interval, lookback, offset, ts, nullptr, sid, offsets_host, n_rows,
+                             n_series, out, valid_words, true);
 }
 
 }  // extern "C"

@@ -26,6 +26,7 @@ constexpr uint32_t kBinRowError = 4u;          // binary operator: a pair's row 
 constexpr uint32_t kSetKeyError = 8u;          // set operator: a row's key is >= n_keys and not B2P_NO_KEY
 constexpr uint32_t kScalarKeyError = 16u;      // scalar(): a row key >= n_rows and not B2P_NO_KEY
 constexpr uint32_t kScalarOverlapError = 32u;  // scalar(): two rows of one key have a cell at one step
+constexpr uint32_t kStepRangeError = 64u;      // step function (K19): an eval timestamp outside the calendar's years
 
 struct RangeArgs {
   // query

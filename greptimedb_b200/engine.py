@@ -38,7 +38,15 @@ NO_KEY = 0xFFFFFFFF
 IFN_IDS = {"abs": 0, "ceil": 1, "floor": 2, "sqrt": 3, "exp": 4, "ln": 5, "log2": 6, "log10": 7, "sin": 8, "cos": 9,
            "tan": 10, "asin": 11, "acos": 12, "atan": 13, "sinh": 14, "cosh": 15, "tanh": 16, "asinh": 17,
            "acosh": 18, "atanh": 19, "round": 20, "deg": 21, "rad": 22, "sgn": 23, "clamp": 24, "clamp_min": 25,
-           "clamp_max": 26}
+           "clamp_max": 26, "neg": 28}
+
+# enum b2p_step_part: time() and the calendar functions under their PromQL names
+STEP_PARTS = {"time": 0, "minute": 1, "hour": 2, "day_of_month": 3, "day_of_week": 4, "day_of_year": 5, "month": 6,
+              "year": 7, "days_in_month": 8}
+
+
+def step_part(part) -> int:
+    return STEP_PARTS[part] if isinstance(part, str) else int(part)
 
 
 def ifn_id(fn) -> int:
@@ -377,6 +385,28 @@ class Context:
                                            _ptr(out), _ptr(ov)))
         return out, ov
 
+    def step_fn(self, part, eval_ts, valid):
+        """K19: f(eval_ts[k]) at every valid cell of a [S,T] grid (part: "time", "hour", ... or enum b2p_step_part)
+        -> out [S,T] f64 (0.0 where invalid); validity is unchanged."""
+        eval_ts = np.ascontiguousarray(eval_ts, np.int64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        S, T = valid.shape[0], eval_ts.size
+        out = np.zeros((S, T), np.float64)
+        self._check(self._L.b2p_step_fn(self._h, step_part(part), _ptr(eval_ts), _ptr(valid), S, T, _ptr(out)))
+        return out
+
+    def instant_timestamp(self, ts, start, end, interval, lookback, offset=0, sid=None, offsets=None):
+        """timestamp(<selector>): the instant selector's rows with the chosen sample's (ts + offset) / 1000 as the
+        value and no stale-NaN test -> (out [S,T] f64, valid_words [S,Tw] u32)."""
+        ts = np.ascontiguousarray(ts, np.int64)
+        sid, offsets, S = self._series_count(sid, offsets)
+        T = num_steps(start, end, interval)
+        out = np.zeros((S, T), np.float64)
+        valid = np.zeros((S, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_instant_timestamp(self._h, start, end, interval, lookback, offset, _ptr(ts), _ptr(sid),
+                                                  _ptr(offsets), ts.size, S, _ptr(out), _ptr(valid)))
+        return out, valid
+
     def scalar_calculate(self, vals, valid, row_key):
         """scalar() over a grid whose rows carry dense series keys (NO_KEY: a label tuple with a NULL)
         -> (out [T] f64, valid_words [Tw] u32)."""
@@ -702,6 +732,14 @@ class Context:
     def instant_fn_dev(self, fn, vals, valid, n_rows, T, out, out_valid, arg0=0.0, arg1=0.0):
         self._check(self._L.b2p_instant_fn_dev(self._h, ifn_id(fn), float(arg0), float(arg1), _ptr(vals), _ptr(valid),
                                                n_rows, T, _ptr(out), _ptr(out_valid)))
+
+    def step_fn_dev(self, part, eval_ts, valid, n_rows, T, out):
+        """Device form of step_fn(): eval_ts [T] (int64), valid [n_rows,Tw] into out [n_rows,T]."""
+        self._check(self._L.b2p_step_fn_dev(self._h, step_part(part), _ptr(eval_ts), _ptr(valid), n_rows, T, _ptr(out)))
+
+    def instant_timestamp_dev(self, start, end, interval, lookback, offset, ts, offsets, n_rows, n_series, out, valid):
+        self._check(self._L.b2p_instant_timestamp_dev(self._h, start, end, interval, lookback, offset, _ptr(ts),
+                                                      _ptr(offsets), n_rows, n_series, _ptr(out), _ptr(valid)))
 
     def scalar_calculate_dev(self, vals, valid, row_key, n_rows, T, out, out_valid):
         self._check(self._L.b2p_scalar_calculate_dev(self._h, _ptr(vals), _ptr(valid), _ptr(row_key), n_rows, T,

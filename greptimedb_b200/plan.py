@@ -8,7 +8,8 @@ top of any node, `function` an instant-vector function (abs, clamp_min, prom_rou
 `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels), `SetOpPlan` applies `and` / `or` / `unless`
 to two nodes, `ScalarPlan` is scalar(node), `TopkPlan` is topk / bottomk(k, node) [by | without (labels)],
 `SubqueryPlan` is fn(node[range:step]), `HistogramQuantilePlan` is histogram_quantile(phi, node), `SortPlan` is
-sort / sort_desc / sort_by_label / sort_by_label_desc(node) and `AbsentPlan` is absent(node).
+sort / sort_desc / sort_by_label / sort_by_label_desc(node), `AbsentPlan` is absent(node) and `EmptyMetricPlan` is
+time(), vector(s) or a number as a one-row node; `PromRangeExec.timestamp()` is timestamp(<selector>).
 """
 from __future__ import annotations
 
@@ -107,6 +108,14 @@ class PromRangeExec(_PlanNode):
             rc = self._L.b2p_plan_set_histogram_quantile(self._h, le_column.encode(), float(histogram_quantile))
             if rc != 0:
                 raise B2PError(rc, self._L.b2p_plan_last_error().decode())
+
+    def timestamp(self, lookback_delta: int = 300_000) -> "PromRangeExec":
+        """timestamp(<selector>): the instant form whose value is each chosen sample's timestamp in seconds (no value
+        column read, no stale-NaN test); execute() emits one Float64 column `value`.  Returns self."""
+        rc = self._L.b2p_plan_set_timestamp(self._h, int(lookback_delta))
+        if rc != 0:
+            raise B2PError(rc, self._L.b2p_plan_last_error().decode())
+        return self
 
     def push(self, batch) -> None:
         """Feed one pyarrow.RecordBatch (moved into the plan through the C Data Interface)."""
@@ -309,5 +318,23 @@ class AbsentPlan(_PlanNode):
         names, values = _cstr_array([n for n, _ in labels]), _cstr_array([v for _, v in labels])
         self._h = self._L.b2p_plan_absent_create(ctx._h, int(start), int(end), int(interval), time_index.encode(),
                                                  value_column.encode(), names, values, len(labels), child._h)
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class EmptyMetricPlan(_PlanNode):
+    """EmptyMetric: one tagless row over start, start + interval, .. <= end (none when start > end), every cell valid.
+    kind "none" exports only the time index; "time" is time() (value t / 1000, named `<time_index> / Float64(1000)`);
+    "literal" is vector(s), pi() or a number (`literal` at every step, named value_column).  The calendar functions
+    without an argument are .function("hour") etc. on this node."""
+
+    KINDS = {"none": 0, "time": 1, "literal": 2}
+
+    def __init__(self, ctx: Context, start: int, end: int, interval: int, kind: str = "time", literal: float = 0.0,
+                 time_index: str = "time", value_column: str = "value"):
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._h = self._L.b2p_plan_empty_metric_create(ctx._h, int(start), int(end), int(interval), time_index.encode(),
+                                                       value_column.encode(), self.KINDS[kind], float(literal))
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())

@@ -149,7 +149,15 @@ enum b2p_ifn { B2P_IFN_ABS = 0, B2P_IFN_CEIL = 1, B2P_IFN_FLOOR = 2, B2P_IFN_SQR
                B2P_IFN_ACOS = 12, B2P_IFN_ATAN = 13, B2P_IFN_SINH = 14, B2P_IFN_COSH = 15, B2P_IFN_TANH = 16,
                B2P_IFN_ASINH = 17, B2P_IFN_ACOSH = 18, B2P_IFN_ATANH = 19, B2P_IFN_ROUND = 20, B2P_IFN_DEG = 21,
                B2P_IFN_RAD = 22, B2P_IFN_SGN = 23, B2P_IFN_CLAMP = 24, B2P_IFN_CLAMP_MIN = 25, B2P_IFN_CLAMP_MAX = 26,
-               B2P_IFN__COUNT = 27 };
+               B2P_IFN__COUNT = 27 /* the math functions above; 27 itself is no function */,
+               B2P_IFN_NEG = 28 /* unary minus: the sign bit flipped (-0.0, a NaN's sign), as Rust's f64 Neg */ };
+
+/* Functions of the eval step alone (b2p_step_fn): time() in seconds, and the calendar parts of the UTC millisecond
+ * timestamp as DataFusion's date_part gives them (planner.rs:2222-2300, 3994-4009): DAY_OF_WEEK counts from Sunday = 0,
+ * DAY_OF_YEAR from 1, DAYS_IN_MONTH is the last day of the step's month. */
+enum b2p_step_part { B2P_STEP_TIME = 0, B2P_STEP_MINUTE = 1, B2P_STEP_HOUR = 2, B2P_STEP_DAY_OF_MONTH = 3,
+                     B2P_STEP_DAY_OF_WEEK = 4, B2P_STEP_DAY_OF_YEAR = 5, B2P_STEP_MONTH = 6, B2P_STEP_YEAR = 7,
+                     B2P_STEP_DAYS_IN_MONTH = 8, B2P_STEP__COUNT = 9 };
 
 /* PromQL set operators; they work per (match key, step) cell and copy cells, never compute values. */
 enum b2p_setop { B2P_SET_AND = 0, B2P_SET_OR = 1, B2P_SET_UNLESS = 2 };
@@ -213,6 +221,13 @@ B2P_API int b2p_range_udf_dev(b2p_ctx* ctx, int32_t fn_id, const int64_t* ts, co
 B2P_API int b2p_instant_select_dev(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval, int64_t lookback,
                            int64_t offset, const int64_t* ts, const double* val, const uint64_t* offsets,
                            uint64_t n_rows, uint32_t n_series, double* out, uint32_t* valid_words);
+/* timestamp(<selector>): the instant selector of b2p_instant_select_dev with the value column replaced by the sample's
+ * timestamp, as the reference projects ts / 1000 before InstantManipulate (planner.rs:905-909, 951-965): the chosen
+ * row's ts + offset as (double)t / 1000.0.  No value column is read, so there is no stale-NaN test: a selected
+ * stale-NaN sample is kept, whatever the table's value type. */
+B2P_API int b2p_instant_timestamp_dev(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                                      int64_t offset, const int64_t* ts, const uint64_t* offsets, uint64_t n_rows,
+                                      uint32_t n_series, double* out, uint32_t* valid_words);
 /* Multi-field tables (Influx line protocol / OTLP ingest: cpu(usage_user, usage_system, ..)): one timestamp column and
  * n_fields Float64 value columns over the same rows, 1 <= n_fields <= B2P_MAX_FIELDS.  `vals` and `outs` are HOST
  * arrays of n_fields DEVICE pointers: vals[f] is field f's column [n_rows], outs[f] its grid [n_series*T].  There is
@@ -383,6 +398,14 @@ B2P_API int b2p_setop_dev(b2p_ctx* ctx, int32_t op /* enum b2p_setop */, const d
  * a clamp bound pair with lo > hi (clamp_min(v, +inf) and clamp_max(v, -inf) included). */
 B2P_API int b2p_instant_fn_dev(b2p_ctx* ctx, int32_t fn /* enum b2p_ifn */, double arg0, double arg1, const double* vals,
                                const uint32_t* valid, uint64_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
+/* K19: a function of the eval step (enum b2p_step_part) at every valid cell of a dense grid: out[r*T + k] =
+ * f(eval_ts[k]) where bit k of row r is set, 0.0 elsewhere; valid is read, never written.  TIME is (double)ts / 1000.0
+ * (one IEEE division, as build_special_time_expr, empty_metric.rs:393-402); the calendar parts are integers in Float64
+ * cells, proleptic Gregorian in UTC, negative epochs included.  A step whose year is outside [-262143, 262143] (chrono's
+ * date range) is written 0.0 and found on the device: B2P_E_INVALID from b2p_sync.  eval_ts [T] is a device array.
+ * B2P_E_INVALID: an unknown part, a NULL argument. */
+B2P_API int b2p_step_fn_dev(b2p_ctx* ctx, int32_t part /* enum b2p_step_part */, const int64_t* eval_ts,
+                            const uint32_t* valid, uint64_t n_rows, uint64_t T, double* out);
 /* scalar(v), the reference's ScalarCalculate (scalar_calculate.rs:532-637), over the whole grid: row_key[r] is a dense
  * series id (< n_rows) or B2P_NO_KEY for a row whose labels include a NULL.  When every row with a cell carries one key
  * (a B2P_NO_KEY row: only while it has exactly one cell), out [T] / out_valid [Tw] are that series' cells, bit copies;
@@ -528,6 +551,10 @@ B2P_API int b2p_instant_select(b2p_ctx* ctx, int64_t start, int64_t end, int64_t
                        int64_t offset, const int64_t* ts, const double* val, const uint32_t* sid,
                        const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series, double* out,
                        uint32_t* valid_words);
+/* Host-pointer form of b2p_instant_timestamp_dev (synchronous), staged as b2p_instant_select stages. */
+B2P_API int b2p_instant_timestamp(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval, int64_t lookback,
+                                  int64_t offset, const int64_t* ts, const uint32_t* sid, const uint64_t* offsets_host,
+                                  uint64_t n_rows, uint32_t n_series, double* out, uint32_t* valid_words);
 /* Host-pointer forms of b2p_range_eval_fields_dev / b2p_instant_select_fields_dev (synchronous): vals[f], field_valid[f]
  * and outs[f] are host columns; sid may be NULL when offsets_host (n_series+1) is given instead.  One staged copy per call (no chunked
  * pipeline): every column must fit on the device at once. */
@@ -625,6 +652,9 @@ B2P_API int b2p_instant_fn(b2p_ctx* ctx, int32_t fn, double arg0, double arg1, c
                            uint64_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
 B2P_API int b2p_scalar_calculate(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const uint32_t* row_key,
                                  uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid);
+/* Host-pointer form of b2p_step_fn_dev (synchronous; a step out of range is returned directly). */
+B2P_API int b2p_step_fn(b2p_ctx* ctx, int32_t part, const int64_t* eval_ts, const uint32_t* valid, uint64_t n_rows,
+                        uint64_t T, double* out);
 /* Host-pointer form of b2p_absent_dev (synchronous): valid [n_rows x Tw], out [T] and out_valid [Tw] are host
  * pointers. */
 B2P_API int b2p_absent(b2p_ctx* ctx, const uint32_t* valid, uint32_t n_rows, uint64_t T, double* out,
@@ -728,11 +758,18 @@ B2P_API b2p_plan* b2p_plan_setop_create(b2p_ctx* ctx, int32_t op /* enum b2p_set
                                         const char* matching /* NULL | "on" | "ignoring" */,
                                         const char* const* labels, int32_t n_labels);
 /* Instant-vector function on top of any node, named as the reference's projection shows it: abs ceil floor sqrt exp ln
- * log2 log10 sin cos tan asin acos atan sinh cosh tanh asinh acosh atanh, degrees, radians, signum (no argument),
+ * log2 log10 sin cos tan asin acos atan sinh cosh tanh asinh acosh atanh, degrees, radians, signum, negative (unary
+ * minus, named (- <value>); refused at execute over an Int64 or Int32 column) (no argument),
  * prom_round (0 or 1: to_nearest, default 0), clamp (lo, hi), clamp_min (lo), clamp_max (hi).  Functions and
  * b2p_plan_set_scalar_op calls form one chain, applied in call order; the value column is renamed like the projection
  * (abs(val), clamp(val,Float64(0),Float64(12))).  B2P_E_INVALID: unknown name or wrong argument count.  A clamp with
- * lo > hi fails at execute, when the node has rows, with the reference's Execution error "min '12' > max '0'". */
+ * lo > hi fails at execute, when the node has rows, with the reference's Execution error "min '12' > max '0'".
+ * The calendar functions minute hour month year day_of_month day_of_week day_of_year days_in_month (no argument) are
+ * K19 over the node's eval timestamps: one value column whatever the node's field count, named
+ * date_part(Utf8("<part>"),<time index>) (days_in_month after its whole expression) and typed Int32; labels and
+ * validity are kept.  Int32 is accepted by the stages above (read as Float64), by a binary operator against a Float64
+ * side (Float64) or as the lhs of a filtering comparison (kept), by and / unless (the lhs kept), by `or` with an Int32
+ * side, and by sort*, topk / bottomk and absent; every other node refuses it with a Plan error at execute. */
 B2P_API int b2p_plan_set_function(b2p_plan* plan, const char* name, const double* args, int32_t n_args);
 /* scalar(child), GpuPromScalarExec: a tagless node with one row over the child's steps, columns {time index,
  * scalar(<value name>)}; usable under scalar operators and functions and as a child of the binary and set nodes (a
@@ -825,6 +862,23 @@ B2P_API b2p_plan* b2p_plan_absent_create(b2p_ctx* ctx, int64_t start, int64_t en
                                          const char* time_index, const char* value_column,
                                          const char* const* label_names, const char* const* label_values,
                                          int32_t n_labels, b2p_plan* child);
+/* EmptyMetric(start, end, interval, time_index, value_column, field_expr) (empty_metric.rs), GpuEmptyMetricExec: one
+ * tagless row over start + k * interval <= end (no row when start > end) with every cell valid.  kind B2P_EMPTY_NONE
+ * exports only the time index (no_field_expr); B2P_EMPTY_TIME is time(), the value (double)t / 1000.0 (K19) named
+ * `<time_index> / Float64(1000)`; B2P_EMPTY_LITERAL is vector(s), pi() or a number literal, `literal` at every step,
+ * named value_column.  The binary node pairs it with every row of the other side, as it pairs scalar(); the calendar
+ * functions without an argument (hour(), ..) are b2p_plan_set_function on this node.  Plan errors at create (NULL is
+ * returned): interval <= 0, a NULL name, an unknown kind. */
+enum b2p_empty_metric_kind { B2P_EMPTY_NONE = 0, B2P_EMPTY_TIME = 1, B2P_EMPTY_LITERAL = 2 };
+B2P_API b2p_plan* b2p_plan_empty_metric_create(b2p_ctx* ctx, int64_t start, int64_t end, int64_t interval,
+                                               const char* time_index, const char* value_column,
+                                               int32_t kind /* enum b2p_empty_metric_kind */, double literal);
+/* timestamp(<selector>): turn a range node into the instant form (as b2p_plan_set_instant) whose value is the chosen
+ * sample's timestamp in seconds, b2p_instant_timestamp: no value column is read and there is no stale-NaN test, for
+ * Float64, Int64 and multi-field tables alike; the result is one Float64 column named `value`.  timestamp() of any
+ * other expression keeps its child's values in the reference (its flag reaches only a vector selector, through
+ * parentheses, planner.rs:244-290, 2358-2366): that needs no node. */
+B2P_API int b2p_plan_set_timestamp(b2p_plan* plan, int64_t lookback_delta);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

@@ -58,6 +58,9 @@ pub struct GpuPromRangeParams {
     pub param1: f64,
     /// InstantManipulate::new lookback (instant_manipulate.rs:189-208) when `function` is empty.
     pub lookback_delta: Millisecond,
+    /// timestamp(<selector>): the instant form whose value is the chosen sample's timestamp in seconds
+    /// (b2p_plan_set_timestamp, planner.rs:905-909, 951-965); `function` is empty.
+    pub timestamp: bool,
     /// prom_aggr_expr_to_plan (planner.rs:334-452): "sum" | "avg" | "count" | "min" | "max" | "stddev" | "stdvar".
     pub aggregate: Option<String>,
     pub by_columns: Vec<String>,
@@ -281,7 +284,14 @@ impl PlanHandle {
                 return Err(DataFusionError::Plan(e));
             }
             let h = Self { ctx, plan };
-            if p.function.is_empty() && ffi::b2p_plan_set_instant(plan, p.lookback_delta) != ffi::B2P_OK {
+            let instant = if p.timestamp {
+                ffi::b2p_plan_set_timestamp(plan, p.lookback_delta)
+            } else if p.function.is_empty() {
+                ffi::b2p_plan_set_instant(plan, p.lookback_delta)
+            } else {
+                ffi::B2P_OK
+            };
+            if instant != ffi::B2P_OK {
                 return Err(DataFusionError::Plan(ffi::plan_last_error()));
             }
             if let Some((le, q)) = &p.histogram {

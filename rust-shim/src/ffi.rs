@@ -148,6 +148,36 @@ pub enum B2pIfn {
     Clamp = 24,
     ClampMin = 25,
     ClampMax = 26,
+    // 27 is B2P_IFN__COUNT, no function
+    /// unary minus: the sign bit flipped
+    Neg = 28,
+}
+
+/// `enum b2p_step_part`: what `b2p_step_fn` computes from an eval timestamp (time() in seconds, the calendar parts).
+#[repr(i32)]
+#[derive(Debug, Clone, Copy, PartialEq, Eq)]
+pub enum B2pStepPart {
+    Time = 0,
+    Minute = 1,
+    Hour = 2,
+    DayOfMonth = 3,
+    DayOfWeek = 4,
+    DayOfYear = 5,
+    Month = 6,
+    Year = 7,
+    DaysInMonth = 8,
+}
+
+/// `enum b2p_empty_metric_kind`: the value column of `b2p_plan_empty_metric_create`.
+#[repr(i32)]
+#[derive(Debug, Clone, Copy, PartialEq, Eq)]
+pub enum B2pEmptyMetricKind {
+    /// only the time index (EmptyMetric without a field expression)
+    None = 0,
+    /// time(): the eval timestamp in seconds
+    Time = 1,
+    /// vector(s), pi() or a number literal
+    Literal = 2,
 }
 
 /// `B2P_NO_KEY`: the key of a row that no row of the other side matches (scalar(): a row with a NULL label).
@@ -507,6 +537,26 @@ extern "C" {
         ctx: *mut b2p_ctx, valid: *const u32, n_rows: u32, t: u64, out: *mut f64, out_valid: *mut u32,
     ) -> c_int;
 
+    // ---- functions of the eval step and timestamp() ---------------------------------------------------------------------
+    /// K19: `part` (enum b2p_step_part: time, minute, hour, day_of_month, day_of_week, day_of_year, month, year,
+    /// days_in_month) of eval_ts[k] at every valid cell of a [n_rows x t] grid; validity is read, never written.
+    pub fn b2p_step_fn_dev(
+        ctx: *mut b2p_ctx, part: i32, eval_ts: *const i64, valid: *const u32, n_rows: u64, t: u64, out: *mut f64,
+    ) -> c_int;
+    pub fn b2p_step_fn(
+        ctx: *mut b2p_ctx, part: i32, eval_ts: *const i64, valid: *const u32, n_rows: u64, t: u64, out: *mut f64,
+    ) -> c_int;
+    /// timestamp(<selector>): the instant selector with the chosen sample's (ts + offset) / 1000 as the value; no value
+    /// column, no stale-NaN test.
+    pub fn b2p_instant_timestamp_dev(
+        ctx: *mut b2p_ctx, start: i64, end: i64, interval: i64, lookback: i64, offset: i64, ts: *const i64,
+        offsets: *const u64, n_rows: u64, n_series: u32, out: *mut f64, valid_words: *mut u32,
+    ) -> c_int;
+    pub fn b2p_instant_timestamp(
+        ctx: *mut b2p_ctx, start: i64, end: i64, interval: i64, lookback: i64, offset: i64, ts: *const i64,
+        sid: *const u32, offsets_host: *const u64, n_rows: u64, n_series: u32, out: *mut f64, valid_words: *mut u32,
+    ) -> c_int;
+
     // ---- plan-level API over the Arrow C Data Interface -----------------------------------------------------------------
     pub fn b2p_plan_range_create(
         ctx: *mut b2p_ctx, function: *const c_char, p: *const B2pRangeParams, time_index: *const c_char,
@@ -536,6 +586,14 @@ extern "C" {
     pub fn b2p_plan_set_function(plan: *mut b2p_plan, name: *const c_char, args: *const f64, n_args: i32) -> c_int;
     /// Ownership as for b2p_plan_binary_create.
     pub fn b2p_plan_scalar_create(ctx: *mut b2p_ctx, child: *mut b2p_plan) -> *mut b2p_plan;
+    /// EmptyMetric: one tagless row over start..=end by interval; `kind` 0 = only the time index, 1 = time(),
+    /// 2 = `literal` (vector(s), pi(), a number).
+    pub fn b2p_plan_empty_metric_create(
+        ctx: *mut b2p_ctx, start: i64, end: i64, interval: i64, time_index: *const c_char, value_column: *const c_char,
+        kind: i32, literal: f64,
+    ) -> *mut b2p_plan;
+    /// timestamp(<selector>) on a range node: the instant form whose value is the sample's timestamp in seconds.
+    pub fn b2p_plan_set_timestamp(plan: *mut b2p_plan, lookback_delta: i64) -> c_int;
     /// `modifier`: NULL, "by" or "without"; ownership of `child` as for b2p_plan_binary_create.
     pub fn b2p_plan_topk_create(
         ctx: *mut b2p_ctx, bottom: i32, k: f64, child: *mut b2p_plan, modifier: *const c_char,

@@ -107,6 +107,19 @@
 //!     <- GpuPromRangeExec (on the same grid)   => `match_absent`: the b2p_plan_absent_create arguments
 //! ```
 //!
+//! The time family (planner.rs:905-965, 2222-2300, 3994-4009; empty_metric.rs):
+//!
+//! ```text
+//!   EmptyMetricExec(start, end, interval, expr: none | CAST(CAST(ts AS Int64) AS Float64) / 1000 | Float64(c))
+//!     [<- under ProjectionExec(date_part(..))]  => `match_empty_metric`: the b2p_plan_empty_metric_create arguments
+//!   InstantManipulateExec <- ProjectionExec(ts, CAST(CAST(ts AS Int64) AS Float64) / 1000 AS value, tags..)
+//!     <- SeriesNormalize <- SeriesDivide       => a timestamp leaf (b2p_plan_set_timestamp)
+//!   ProjectionExec(date_part(Utf8(part), ts) | days_in_month's date_part(..) | (- col))
+//!     <- GpuPromRangeExec                     => the same node with the calendar / `negative` stage appended
+//!   ProjectionExec(the child's columns, unchanged) <- GpuPromRangeExec      (timestamp(<any other expression>))
+//!                                             => the child itself
+//! ```
+//!
 //! Over a table with several field columns the rule takes the shapes the library evaluates per field (the leaf, the
 //! aggregate node with one aggregate per field, sort by every field, subqueries, absent, the binary zip) and leaves on
 //! the CPU those the library refuses there (the leaf's own aggregate, filtering comparisons over two or more fields,
@@ -127,7 +140,7 @@ use datafusion::common::{Result as DataFusionResult, ScalarValue};
 use datafusion::config::ConfigOptions;
 use datafusion::common::JoinType;
 use datafusion::logical_expr::Operator;
-use datafusion::physical_expr::expressions::{BinaryExpr, CastExpr, Column, IsNotNullExpr, Literal};
+use datafusion::physical_expr::expressions::{BinaryExpr, CastExpr, Column, IsNotNullExpr, Literal, NegativeExpr};
 use datafusion::physical_expr::{PhysicalExpr, ScalarFunctionExpr};
 use datafusion::physical_optimizer::PhysicalOptimizerRule;
 use datafusion::physical_plan::aggregates::{AggregateExec, AggregateMode};
@@ -141,11 +154,11 @@ use datafusion::physical_plan::windows::BoundedWindowAggExec;
 use datafusion::physical_plan::ExecutionPlan;
 
 use crate::exec::{GpuPromRangeExec, GpuPromRangeParams, GpuPromStage};
-use crate::ffi::{B2pBinOp, B2pFn, B2pSetOp};
+use crate::ffi::{B2pBinOp, B2pEmptyMetricKind, B2pFn, B2pSetOp};
 // In-tree these are `crate::extension_plan::{..}`; named here the way the reference names them.
 use promql::extension_plan::{
-    AbsentExec, HistogramFoldExec, RangeManipulateExec, ScalarCalculateExec, SeriesDivideExec, SeriesNormalizeExec,
-    UnionDistinctOnExec,
+    AbsentExec, EmptyMetricExec, HistogramFoldExec, InstantManipulateExec, RangeManipulateExec, ScalarCalculateExec,
+    SeriesDivideExec, SeriesNormalizeExec, UnionDistinctOnExec,
 };
 
 /// The projection indices a `FilterExec` keeps rows on: `c IS NOT NULL`, or the conjunction of such tests that closes a
@@ -261,6 +274,7 @@ impl GpuPromRewrite {
             param0,
             param1,
             lookback_delta: 0,
+            timestamp: false,
             aggregate: None,
             by_columns: vec![],
             histogram: None,
@@ -470,6 +484,101 @@ fn float_literal(e: &Arc<dyn PhysicalExpr>) -> Option<f64> {
     }
 }
 
+fn scalar_literal(e: &Arc<dyn PhysicalExpr>) -> Option<&ScalarValue> {
+    Some(e.as_any().downcast_ref::<Literal>()?.value())
+}
+
+fn column_named(e: &Arc<dyn PhysicalExpr>, name: &str) -> bool {
+    e.as_any().downcast_ref::<Column>().is_some_and(|c| c.name() == name)
+}
+
+/// `CAST(CAST(<ts> AS Int64) AS Float64) / Float64(1000)`: build_special_time_expr (empty_metric.rs:393-402), the
+/// value of time() and of timestamp()
+fn is_special_time_expr(e: &Arc<dyn PhysicalExpr>, ts: &str) -> bool {
+    let Some(b) = e.as_any().downcast_ref::<BinaryExpr>() else { return false };
+    if *b.op() != Operator::Divide || float_literal(b.right()) != Some(1000.0) {
+        return false;
+    }
+    let Some(outer) = b.left().as_any().downcast_ref::<CastExpr>() else { return false };
+    let Some(inner) = outer.expr().as_any().downcast_ref::<CastExpr>() else { return false };
+    outer.cast_type() == &DataType::Float64 && inner.cast_type() == &DataType::Int64 && column_named(inner.expr(), ts)
+}
+
+/// The calendar function (the library's stage name) of a `date_part(Utf8(field), ts)` projection, or of days_in_month's
+/// `date_part(Utf8("day"), date_trunc(Utf8("month"), ts) + IntervalYearMonth(1) - IntervalDayTime(1 day))`
+/// (planner.rs:2222-2300); `None` for any other expression, which stays on the CPU.
+fn calendar_fn(e: &Arc<dyn PhysicalExpr>, ts: &str) -> Option<&'static str> {
+    let f = e.as_any().downcast_ref::<ScalarFunctionExpr>()?;
+    if f.name() != "date_part" {
+        return None;
+    }
+    let [field, arg] = f.args() else { return None };
+    let ScalarValue::Utf8(Some(field)) = scalar_literal(field)? else { return None };
+    if column_named(arg, ts) {
+        return match field.as_str() {
+            "minute" => Some("minute"),
+            "hour" => Some("hour"),
+            "month" => Some("month"),
+            "year" => Some("year"),
+            "day" => Some("day_of_month"),
+            "dow" => Some("day_of_week"),
+            "doy" => Some("day_of_year"),
+            _ => None,
+        };
+    }
+    if field != "day" {
+        return None;
+    }
+    // `date_trunc(..) + (1 month - 1 day)`: the interval either as the planner wrote it or folded into one literal
+    let plus = arg.as_any().downcast_ref::<BinaryExpr>()?;
+    if *plus.op() != Operator::Plus {
+        return None;
+    }
+    let one_month_less_a_day = match scalar_literal(plus.right()) {
+        Some(ScalarValue::IntervalMonthDayNano(Some(v))) => v.months == 1 && v.days == -1 && v.nanoseconds == 0,
+        Some(_) => false,
+        None => {
+            let minus = plus.right().as_any().downcast_ref::<BinaryExpr>()?;
+            *minus.op() == Operator::Minus
+                && matches!(scalar_literal(minus.left()), Some(ScalarValue::IntervalYearMonth(Some(1))))
+                && matches!(scalar_literal(minus.right()),
+                            Some(ScalarValue::IntervalDayTime(Some(d))) if d.days == 1 && d.milliseconds == 0)
+        }
+    };
+    let trunc = plus.left().as_any().downcast_ref::<ScalarFunctionExpr>()?;
+    let [unit, col] = trunc.args() else { return None };
+    let month = matches!(scalar_literal(unit), Some(ScalarValue::Utf8(Some(u))) if u == "month");
+    (one_month_less_a_day && trunc.name() == "date_trunc" && month && column_named(col, ts)).then_some("days_in_month")
+}
+
+/// The one projected expression of a `ProjectionExec` that is not a plain column (`None` when there are none or two).
+fn single_expression(p: &ProjectionExec) -> Option<Arc<dyn PhysicalExpr>> {
+    let mut value = None;
+    for e in p.expr() {
+        if e.expr.as_any().downcast_ref::<Column>().is_none() {
+            if value.is_some() {
+                return None;
+            }
+            value = Some(e.expr.clone());
+        }
+    }
+    value
+}
+
+/// What `b2p_plan_empty_metric_create` takes for a matched `EmptyMetricExec`, and the calendar stage of `hour()` etc.
+/// without an argument (a `date_part` projection over it).
+#[derive(Debug, Clone)]
+pub struct GpuPromEmptyMetricSpec {
+    pub start: i64,
+    pub end: i64,
+    pub interval: i64,
+    pub time_index: String,
+    pub value_column: String,
+    pub kind: B2pEmptyMetricKind,
+    pub literal: f64,
+    pub stages: Vec<GpuPromStage>,
+}
+
 impl GpuPromRewrite {
     /// `ProjectionExec(col op lit)` / `FilterExec(col cmp lit)` over a `GpuPromRangeExec` -> the node's parameters with
     /// the scalar operator appended; every other projected expression must be a plain column.
@@ -522,6 +631,16 @@ impl GpuPromRewrite {
         }
         let value = value?;
         let node = p.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        // a calendar function of the node's eval time, or unary minus (planner.rs:552): stages without arguments
+        let stage = calendar_fn(&value, &node.params().time_index_column).or_else(|| {
+            let neg = value.as_any().downcast_ref::<NegativeExpr>()?;
+            neg.arg().as_any().downcast_ref::<Column>().map(|_| "negative")
+        });
+        if let Some(name) = stage {
+            let mut params = node.params().clone();
+            params.stages.push(GpuPromStage::Function(name.to_string(), vec![]));
+            return Some((params, node.input().clone()));
+        }
         let f = value.as_any().downcast_ref::<ScalarFunctionExpr>()?;
         let name = f.name();
         let &(_, n_args) = INSTANT_FNS.iter().find(|(n, _)| *n == name)?;
@@ -534,6 +653,98 @@ impl GpuPromRewrite {
         let mut params = node.params().clone();
         params.stages.push(GpuPromStage::Function(name.to_string(), args));
         Some((params, node.input().clone()))
+    }
+
+    /// `InstantManipulateExec <- ProjectionExec(ts, CAST(CAST(ts AS Int64) AS Float64) / 1000 AS value, tags..) <-
+    /// SeriesNormalize <- SeriesDivide <- input`: timestamp(<selector>) (planner.rs:905-909, 951-965) -> a timestamp
+    /// leaf.  The leaf reads no value; it is given the scan's first Float64 or Int64 column, which every batch carries.
+    fn match_timestamp_leaf(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<(GpuPromRangeParams, Arc<dyn ExecutionPlan>)> {
+        let instant = plan.as_any().downcast_ref::<InstantManipulateExec>()?;
+        let p = instant.input().as_any().downcast_ref::<ProjectionExec>()?;
+        let normalize = p.input().as_any().downcast_ref::<SeriesNormalizeExec>()?;
+        let divide = normalize.input().as_any().downcast_ref::<SeriesDivideExec>()?;
+        let ts = instant.time_index_column();
+        if !is_special_time_expr(&single_expression(p)?, ts) {
+            return None;
+        }
+        let tags = divide.tag_columns();
+        let schema = divide.input().schema();
+        let field = schema.fields().iter().find(|f| {
+            f.name() != ts
+                && !tags.contains(f.name())
+                && matches!(f.data_type(), DataType::Float64 | DataType::Int64)
+        })?;
+        let params = GpuPromRangeParams {
+            function: String::new(),
+            start: instant.start(),
+            end: instant.end(),
+            interval: instant.interval(),
+            range: 0,
+            time_index_column: ts.to_string(),
+            field_columns: vec![field.name().clone()],
+            offset: normalize.offset(),
+            need_filter_out_nan: normalize.need_filter_out_nan(),
+            tag_columns: tags.to_vec(),
+            param0: 0.0,
+            param1: 0.0,
+            lookback_delta: instant.lookback_delta(),
+            timestamp: true,
+            aggregate: None,
+            by_columns: vec![],
+            histogram: None,
+            stages: vec![],
+        };
+        Some((params, divide.input().clone()))
+    }
+
+    /// `ProjectionExec` of the child's columns in the child's order over a `GpuPromRangeExec`: what the reference plans
+    /// for timestamp(<any other expression>), whose `timestamp_fn` flag reaches only a vector selector
+    /// (planner.rs:244-290, 2358-2366) -> the child itself.
+    fn match_passthrough(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<(GpuPromRangeParams, Arc<dyn ExecutionPlan>)> {
+        let p = plan.as_any().downcast_ref::<ProjectionExec>()?;
+        let node = p.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let child = node.schema();
+        if p.expr().len() != child.fields().len() {
+            return None;
+        }
+        for (i, e) in p.expr().iter().enumerate() {
+            let c = e.expr.as_any().downcast_ref::<Column>()?;
+            if c.index() != i || e.alias != *child.field(i).name() {
+                return None;
+            }
+        }
+        Some((node.params().clone(), node.input().clone()))
+    }
+
+    /// `[ProjectionExec(date_part(..)) <-] EmptyMetricExec` (empty_metric.rs; time(), vector(s), pi(), a literal, and
+    /// the calendar functions without an argument) -> the arguments of `b2p_plan_empty_metric_create` and its stage.
+    pub fn match_empty_metric(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromEmptyMetricSpec> {
+        let (input, stage) = match plan.as_any().downcast_ref::<ProjectionExec>() {
+            Some(p) => {
+                let ts = p.input().schema().field(0).name().clone();
+                (p.input().clone(), Some(calendar_fn(&single_expression(p)?, &ts)?))
+            }
+            None => (plan.clone(), None),
+        };
+        let em = input.as_any().downcast_ref::<EmptyMetricExec>()?;
+        let schema = em.schema();
+        let time_index = schema.field(0).name().clone();
+        let (kind, literal) = match em.expr() {
+            None => (B2pEmptyMetricKind::None, 0.0),
+            Some(e) if is_special_time_expr(e, &time_index) => (B2pEmptyMetricKind::Time, 0.0),
+            Some(e) => (B2pEmptyMetricKind::Literal, float_literal(e)?),
+        };
+        let value_column = if schema.fields().len() > 1 { schema.field(1).name().clone() } else { String::new() };
+        Some(GpuPromEmptyMetricSpec {
+            start: em.start(),
+            end: em.end(),
+            interval: em.interval(),
+            time_index,
+            value_column,
+            kind,
+            literal,
+            stages: stage.map(|n| GpuPromStage::Function(n.to_string(), vec![])).into_iter().collect(),
+        })
     }
 
     /// `ScalarCalculateExec <- GpuPromRangeExec` -> the child of `b2p_plan_scalar_create` (no Rust execution node for the
@@ -1011,8 +1222,10 @@ impl PhysicalOptimizerRule for GpuPromRewrite {
             let matched = self
                 .match_aggregate(&node)
                 .or_else(|| self.match_range_subtree(&node))
+                .or_else(|| self.match_timestamp_leaf(&node))
                 .or_else(|| self.match_scalar_op(&node))
-                .or_else(|| self.match_function(&node));
+                .or_else(|| self.match_function(&node))
+                .or_else(|| self.match_passthrough(&node));
             match matched {
                 Some((params, input)) => {
                     // the replaced node's schema is kept verbatim, so parents (Sort, CoalesceBatches, MergeScan ..) see no change
