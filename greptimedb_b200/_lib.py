@@ -43,6 +43,7 @@ EXPORTED_SYMBOLS = [
     "b2p_sort_cells_i64_dev", "b2p_sort_cells_i64", "b2p_i64_to_f64_dev", "b2p_i64_to_f64",
     "b2p_step_fn_dev", "b2p_step_fn", "b2p_instant_timestamp_dev", "b2p_instant_timestamp",
     "b2p_plan_empty_metric_create", "b2p_plan_set_timestamp",
+    "b2p_plan_label_replace_create", "b2p_plan_label_join_create", "b2p_label_regex_check", "b2p_label_regex_replace",
 ]
 
 
@@ -188,6 +189,10 @@ def load() -> C.CDLL:
         "b2p_instant_timestamp": (C.c_int, [vp, i64, i64, i64, i64, i64, vp, vp, vp, u64, u32, vp, vp]),
         "b2p_plan_empty_metric_create": (vp, [vp, i64, i64, i64, C.c_char_p, C.c_char_p, i32, dbl]),
         "b2p_plan_set_timestamp": (C.c_int, [vp, i64]),
+        "b2p_plan_label_replace_create": (vp, [vp, vp, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p]),
+        "b2p_plan_label_join_create": (vp, [vp, vp, C.c_char_p, C.c_char_p, C.POINTER(C.c_char_p), i32]),
+        "b2p_label_regex_check": (C.c_int, [C.c_char_p]),
+        "b2p_label_regex_replace": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, u64, C.POINTER(u64)]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)  # AttributeError here means the .so does not match the header

@@ -1,6 +1,7 @@
 // b2p_plan.cpp — host side of GpuPromRangeExec (see b2p_plan.hpp) and its C entry points.
 // Pure host C++: everything numeric goes through the C ABI (b2p_range_eval / b2p_group_aggregate).
 #include "b2p_plan.hpp"
+#include "b2p_regex.hpp"
 
 #include <algorithm>
 #include <cctype>
@@ -796,6 +797,12 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       }
       break;
     }
+    case Columns::TimeValueLastTag:
+      c_ts = add_col(r.time_index, "tsm:");
+      add_vals("g");
+      if (!L.names.empty()) add_tag(L.names.size() - 1);
+      for (size_t t = 0; t + 1 < L.names.size(); ++t) add_tag(t);
+      break;
     case Columns::None:  // (no rows either)
       break;
   }
@@ -1837,6 +1844,102 @@ void EmptyMetricPlan::compute(NodeResult& r) {
   }
 }
 
+
+// ---- LabelPlan -----------------------------------------------------------------------------------------
+LabelPlan::LabelPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child, std::string dst, std::string replacement,
+                     std::string src, const std::string& regex)
+    : PlanNode(ctx), child_(std::move(child)), join_(false), dst_(std::move(dst)), replacement_(std::move(replacement)),
+      src_(std::move(src)) {
+  // build_regexp_replace_label_expr's order: the destination name, then the raw regex (planner.rs:2531-2562); both
+  // come before the child, so they can be checked without one
+  if (!valid_label_name(dst_)) throw PlanError(ErrorKind::Plan, "Invalid destination label name in label_replace(): " + dst_);
+  regex_ = std::make_unique<LabelRegex>(regex);
+  if (regex_->verdict() == RegexVerdict::Invalid)
+    throw PlanError(ErrorKind::Plan, "Invalid regular expression in label_replace(): " + regex);
+  if (regex_->verdict() == RegexVerdict::Unsupported)
+    throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: the regular expression " + regex + " is not supported by this node: " +
+                                         regex_->message());
+  empty_regex_ = regex.empty();
+  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: NULL child");
+}
+
+LabelPlan::LabelPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child, std::string dst, std::string separator,
+                     std::vector<std::string> srcs)
+    : PlanNode(ctx), child_(std::move(child)), join_(true), dst_(std::move(dst)), replacement_(std::move(separator)),
+      srcs_(std::move(srcs)) {
+  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: NULL child");
+  if (srcs_.empty()) throw PlanError(ErrorKind::Plan, "Invalid function argument for label_join");  // planner.rs:2687-2692
+}
+
+LabelPlan::~LabelPlan() = default;
+
+void LabelPlan::compute(NodeResult& r) {
+  child_->run(r);  // the child's result is this node's: grid, validity and the rest stay where they are
+  if (r.columns == Columns::None) return;  // no columns and no rows: nothing to label
+  if (r.labels.id_keyed)
+    throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: an id-keyed (__tsid) child has no label values to rewrite");
+  if (r.columns == Columns::CountTagsTimeLabel)
+    throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: a count_values child is not supported by this node");
+  Labels& L = r.labels;
+  auto is_column = [&](const std::string& name) {
+    return name == r.time_index || std::find(r.value_names.begin(), r.value_names.end(), name) != r.value_names.end();
+  };
+  const std::string fn = join_ ? "label_join" : "label_replace";
+  const int src = join_ ? -1 : L.column(src_);
+  if (!join_) {
+    const bool noop = src >= 0 ? empty_regex_ : replacement_.empty();
+    if (noop) {  // the projection {time index, values.., tags..} (planner.rs:2346-2351)
+      r.columns = Columns::TimeValueTags;
+      return;
+    }
+    if (L.column(dst_) >= 0) throw PlanError(ErrorKind::Plan, "vector cannot contain metrics with the same labelset");
+  }
+  if (is_column(dst_))
+    throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: " + fn + "() into " + dst_ + ", the name of the time index or a value column, is not supported by this node");
+  std::vector<Label> out(r.rows);
+  if (!join_ && src < 0) {  // the literal replacement on every row
+    std::fill(out.begin(), out.end(), Label(replacement_));
+  } else if (!join_) {  // regexp_replace over the source column, once per distinct value; NULL stays NULL
+    std::unordered_map<std::string, std::string> done;
+    const std::vector<Label>& in = L.values[(size_t)src];
+    for (uint32_t q = 0; q < r.rows; ++q) {
+      if (!in[q]) continue;
+      auto it = done.find(*in[q]);
+      if (it == done.end()) it = done.emplace(*in[q], regex_->replace(*in[q], replacement_)).first;
+      out[q] = it->second;
+    }
+  } else {  // concat_ws(separator, src..): "" and absent sources are NULL literals, and NULLs are skipped
+    std::vector<int> cols;
+    for (const std::string& s : srcs_) {
+      if (!s.empty() && is_column(s))
+        throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: label_join() over " + s + ", the time index or a value column, is not supported by this node");
+      if (!s.empty() && L.column(s) >= 0) cols.push_back(L.column(s));
+    }
+    // (no cache: joining the parts costs less than hashing them)
+    for (uint32_t q = 0; q < r.rows; ++q) {
+      std::string v;
+      bool first = true;
+      for (int c : cols) {
+        const Label& part = L.values[(size_t)c][q];
+        if (!part) continue;
+        if (!first) v += replacement_;
+        v += *part;
+        first = false;
+      }
+      out[q] = std::move(v);
+    }
+    const int old = L.column(dst_);  // dropped from the tags, then added as the new one (planner.rs:2318-2321)
+    if (old >= 0) {
+      L.names.erase(L.names.begin() + old);
+      L.values.erase(L.values.begin() + old);
+    }
+  }
+  L.names.push_back(dst_);
+  L.values.push_back(std::move(out));
+  r.columns = Columns::TimeValueLastTag;
+  r.scalar_like = r.literal_row = false;
+}
+
 }  // namespace b2p
 
 // ---- C entry points -----------------------------------------------------------------------------------
@@ -2058,6 +2161,56 @@ b2p_plan* b2p_plan_empty_metric_create(b2p_ctx* ctx, int64_t start, int64_t end,
     if (!time_index || !value_column) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
     return std::make_shared<b2p::EmptyMetricPlan>(ctx, start, end, interval, time_index, value_column, kind, literal);
   });
+}
+
+b2p_plan* b2p_plan_label_replace_create(b2p_ctx* ctx, b2p_plan* child, const char* dst, const char* replacement,
+                                        const char* src, const char* regex) {
+  return create([&] {
+    if (!dst || !replacement || !src || !regex) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    return std::make_shared<b2p::LabelPlan>(ctx, child ? child->node : nullptr, dst, replacement, src, regex);
+  });
+}
+
+b2p_plan* b2p_plan_label_join_create(b2p_ctx* ctx, b2p_plan* child, const char* dst, const char* separator,
+                                     const char* const* srcs, int32_t n_srcs) {
+  return create([&] {
+    if (!child || !dst || !separator || n_srcs < 0 || (n_srcs > 0 && !srcs))
+      throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    for (int32_t i = 0; i < n_srcs; ++i)
+      if (!srcs[i]) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    return std::make_shared<b2p::LabelPlan>(ctx, child->node, dst, separator, strings(srcs, n_srcs));
+  });
+}
+
+int b2p_label_regex_check(const char* regex) {
+  if (!regex) {
+    g_err = "NULL argument";
+    return B2P_E_INVALID;
+  }
+  const b2p::LabelRegex re(regex);
+  g_err = re.message();
+  return (int)re.verdict();
+}
+
+int b2p_label_regex_replace(const char* regex, const char* replacement, const char* input, char* out, uint64_t cap,
+                            uint64_t* out_len) {
+  if (!regex || !replacement || !input || (cap > 0 && !out)) {
+    g_err = "NULL argument";
+    return B2P_E_INVALID;
+  }
+  const b2p::LabelRegex re(regex);
+  if (re.verdict() != b2p::RegexVerdict::Ok) {
+    g_err = re.message();
+    return B2P_E_INVALID;
+  }
+  const std::string v = re.replace(input, replacement);
+  if (out_len) *out_len = v.size();
+  if (v.size() + 1 > cap) {
+    g_err = "the result needs " + std::to_string(v.size() + 1) + " bytes";
+    return B2P_E_TOO_LARGE;
+  }
+  std::memcpy(out, v.c_str(), v.size() + 1);
+  return B2P_OK;
 }
 
 int b2p_plan_set_timestamp(b2p_plan* plan, int64_t lookback_delta) {

@@ -110,6 +110,8 @@ enum class Columns {
   ValueTagsTime,  // {value, tags.., time index}: topk / bottomk
   CountTagsTimeLabel,  // {count Int64 (Float64 under an element-wise stage), tags.., time index, label}: count_values
   None,                // no column at all: histogram_quantile over a child without the le tag (an EmptyRelation)
+  TimeValueLastTag,    // {time index, value, the last tag, the other tags..}: label_replace / label_join, whose new tag
+                       // is the last one for the nodes above and comes first among the tags in its own projection
 };
 
 // The Arrow type of a value column.  An Int64 cell holds the bits of its int64_t in the 8-byte slot of the grid; an Int32
@@ -460,6 +462,40 @@ class EmptyMetricPlan : public PlanNode {
   std::string time_index_, value_column_;
   int kind_;
   double literal_;
+};
+
+// label_replace(child, dst, replacement, src, regex) / label_join(child, dst, separator, srcs..), GpuPromLabelExec: the
+// reference's Projection(time index, values.., <label expr> AS dst, tags..) over any node (planner.rs:1012-1101,
+// 2306-2356, 2504-2700).  The child's grid, validity, eval timestamps, types, cell order and counted values are moved,
+// not copied; only the label tuples change, each distinct source value of label_replace evaluated once (label_join
+// concatenates per row, which costs less than a lookup).  Nodes above see dst appended to the tags (label_join first drops a tag named dst); the export is
+// {time index, values.., dst, other tags..} (Columns::TimeValueLastTag) whatever the child's layout, because the
+// reference's projection always lists its columns so.  A no-op label_replace exports {time index, values.., tags..} and
+// keeps the child's flags; a node that adds a label clears scalar_like / literal_row, so the binary node joins a labelled
+// vector(1) on labels.  Rows are never merged.  Plan errors: at create, an invalid dst name, a regex Rust rejects, a
+// regex outside b2p_regex.hpp's supported list, label_join without sources; at execute, the reference's same-labelset
+// error, an id-keyed (__tsid) child, a count_values child (the reference drops its counted-value column here, which
+// this layer does not model), dst or a label_join source named like the time index or a value column.
+class LabelPlan : public PlanNode {
+ public:
+  // label_replace
+  LabelPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child, std::string dst, std::string replacement, std::string src,
+            const std::string& regex);
+  // label_join
+  LabelPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child, std::string dst, std::string separator,
+            std::vector<std::string> srcs);
+  ~LabelPlan() override;
+
+ protected:
+  void compute(NodeResult& r) override;
+
+ private:
+  std::shared_ptr<PlanNode> child_;
+  bool join_;
+  std::string dst_, replacement_, src_;  // replacement_ is label_join's separator
+  std::vector<std::string> srcs_;
+  std::unique_ptr<class LabelRegex> regex_;
+  bool empty_regex_ = false;
 };
 
 int function_id_from_name(const std::string& prom_name);  // -1 when unknown

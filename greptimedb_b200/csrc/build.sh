@@ -13,7 +13,7 @@ FLAGS=(-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -fmad=fals
 OBJ="$(mktemp -d)"
 trap 'rm -rf "${OBJ}"' EXIT
 pids=()
-for src in "${HERE}"/b2p_*.cu "${HERE}/b2p_plan.cpp"; do
+for src in "${HERE}"/b2p_*.cu "${HERE}/b2p_plan.cpp" "${HERE}/b2p_regex.cpp"; do
   "${NVCC}" "${FLAGS[@]}" -c -o "${OBJ}/$(basename "${src}").o" "${src}" &
   pids+=($!)
 done

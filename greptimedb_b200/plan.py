@@ -8,8 +8,10 @@ top of any node, `function` an instant-vector function (abs, clamp_min, prom_rou
 `BinaryPlan` combines two nodes (`lhs op rhs`, vector matching on labels), `SetOpPlan` applies `and` / `or` / `unless`
 to two nodes, `ScalarPlan` is scalar(node), `TopkPlan` is topk / bottomk(k, node) [by | without (labels)],
 `SubqueryPlan` is fn(node[range:step]), `HistogramQuantilePlan` is histogram_quantile(phi, node), `SortPlan` is
-sort / sort_desc / sort_by_label / sort_by_label_desc(node), `AbsentPlan` is absent(node) and `EmptyMetricPlan` is
-time(), vector(s) or a number as a one-row node; `PromRangeExec.timestamp()` is timestamp(<selector>).
+sort / sort_desc / sort_by_label / sort_by_label_desc(node), `AbsentPlan` is absent(node), `EmptyMetricPlan` is
+time(), vector(s) or a number as a one-row node, `LabelReplacePlan` / `LabelJoinPlan` are label_replace / label_join over
+any node; `PromRangeExec.timestamp()` is timestamp(<selector>).  `label_regex_check` / `label_regex_replace` run the
+label_replace regex engine on one string, no device needed.
 """
 from __future__ import annotations
 
@@ -338,3 +340,58 @@ class EmptyMetricPlan(_PlanNode):
                                                        value_column.encode(), self.KINDS[kind], float(literal))
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class LabelReplacePlan(_PlanNode):
+    """label_replace(child, dst, replacement, src, regex): dst = the expanded replacement where the whole src value
+    matches `regex` (Rust `regex` syntax, the supported subset), the src value where it does not, NULL where it is NULL;
+    the literal replacement on every row when src is not a tag; a no-op when src is a tag and regex is "", or src is not
+    a tag and replacement is "".  The child's values and rows are kept; nodes above see dst as the last tag, execute()
+    emits {time index, values.., dst, tags..}.  The child stays usable and is kept alive by this node."""
+
+    def __init__(self, ctx: Context, child: _PlanNode, dst: str, replacement: str, src: str, regex: str):
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (child,)
+        self._h = self._L.b2p_plan_label_replace_create(ctx._h, child._h, dst.encode(), replacement.encode(),
+                                                        src.encode(), regex.encode())
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+class LabelJoinPlan(_PlanNode):
+    """label_join(child, dst, separator, *srcs): dst = the source labels' values joined by `separator`, skipping a
+    source that is "", absent or NULL on the row (concat_ws); a tag named dst is replaced.  Layout as for
+    LabelReplacePlan.  The child stays usable and is kept alive by this node."""
+
+    def __init__(self, ctx: Context, child: _PlanNode, dst: str, separator: str, *srcs: str):
+        self._L = _lib.load()
+        self._ctx = ctx
+        self._children = (child,)
+        arr = _cstr_array(list(srcs))
+        self._h = self._L.b2p_plan_label_join_create(ctx._h, child._h, dst.encode(), separator.encode(), arr, len(srcs))
+        if not self._h:
+            raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+
+REGEX_OK, REGEX_INVALID, REGEX_UNSUPPORTED = 0, 1, 2
+
+
+def label_regex_check(regex: str) -> int:
+    """REGEX_OK, REGEX_INVALID (Rust's regex crate rejects it) or REGEX_UNSUPPORTED (valid in Rust, refused here)."""
+    return int(_lib.load().b2p_label_regex_check(regex.encode()))
+
+
+def label_regex_replace(regex: str, replacement: str, value: str) -> str:
+    """regexp_replace(value, "^(?s:" + regex + ")$", replacement) as label_replace evaluates one label value."""
+    L = _lib.load()
+    need = C.c_uint64(0)
+    cap = 256
+    while True:
+        buf = C.create_string_buffer(cap)
+        rc = L.b2p_label_regex_replace(regex.encode(), replacement.encode(), value.encode(), buf, cap, C.byref(need))
+        if rc == 0:
+            return buf.raw[:need.value].decode()
+        if rc != -5:  # B2P_E_TOO_LARGE: retry with room for the result
+            raise B2PError(rc, L.b2p_plan_last_error().decode())
+        cap = need.value + 1

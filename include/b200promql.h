@@ -879,6 +879,45 @@ B2P_API b2p_plan* b2p_plan_empty_metric_create(b2p_ctx* ctx, int64_t start, int6
  * other expression keeps its child's values in the reference (its flag reaches only a vector selector, through
  * parentheses, planner.rs:244-290, 2358-2366): that needs no node. */
 B2P_API int b2p_plan_set_timestamp(b2p_plan* plan, int64_t lookback_delta);
+/* label_replace(child, dst, replacement, src, regex), GpuPromLabelExec: the reference's Projection(time index, values..,
+ * regexp_replace(src, "^(?s:" + regex + ")$", replacement) AS dst, tags..) over the child (planner.rs:2330-2352,
+ * 2518-2616).  No per-cell work: the child's grid, validity and row order are moved into the result and only the label
+ * tuples change, each distinct source value evaluated once (b2p_regex.hpp states the engine).  In the reference's order:
+ *   - dst failing ^[a-zA-Z_][a-zA-Z0-9_]*$ or starting with "__": "Invalid destination label name in label_replace(): <dst>";
+ *   - regex rejected by Rust's regex crate: "Invalid regular expression in label_replace(): <regex>";
+ *   - src a tag of the child and regex "": the child unchanged (a no-op);
+ *   - src not a tag ("" included): a no-op when replacement is "", else dst = replacement on every row;
+ *   - dst already a tag of the child (on either branch that adds it, dst == src included): "vector cannot contain metrics
+ *     with the same labelset";
+ *   - else dst = the expanded replacement where the whole src value matches, the src value itself where it does not,
+ *     NULL where it is NULL.
+ * Rows are never merged: two series that end up with one label tuple stay two rows.  Nodes above see dst appended to the
+ * child's tags; the export is {time index, values.., dst, the child's tags..} ({time index, values.., tags..} for a
+ * no-op).  A tagless literal or time() child that gains a label is joined on labels by the binary node from then on.
+ * Plan errors, at create: the two texts above, a regex that is valid in Rust but outside the supported list
+ * (b2p_label_regex_check), then a NULL child (so the first two need no node); at execute: an id-keyed (__tsid) child, a count_values child, dst named like the time index
+ * or a value column.  Ownership as for b2p_plan_binary_create.  NULL on error (b2p_plan_last_error). */
+B2P_API b2p_plan* b2p_plan_label_replace_create(b2p_ctx* ctx, b2p_plan* child, const char* dst, const char* replacement,
+                                                const char* src, const char* regex);
+/* label_join(child, dst, separator, srcs..), GpuPromLabelExec: the reference's Projection(time index, values..,
+ * concat_ws(separator, src..) AS dst, tags..) (planner.rs:2306-2327, 2619-2700).  A source "" or one the child does not
+ * have is NULL, and concat_ws skips NULLs (all NULL gives ""; a NULL tag value is skipped too).  dst is not validated;
+ * when it is a tag of the child, that tag is dropped and dst takes its place at the end of the tags.  Layout, moves and
+ * rows as for b2p_plan_label_replace_create.  Plan errors, at create: n_srcs == 0 ("Invalid function argument for
+ * label_join"); at execute: an id-keyed (__tsid) or count_values child, a source or dst named like the time index or a
+ * value column (the reference would read cell values as labels).  Ownership as for b2p_plan_binary_create. */
+B2P_API b2p_plan* b2p_plan_label_join_create(b2p_ctx* ctx, b2p_plan* child, const char* dst, const char* separator,
+                                             const char* const* srcs, int32_t n_srcs);
+/* Host only, no context: what the plan layer makes of a label_replace regex.  0: supported; 1: invalid (Rust's regex
+ * crate rejects it); 2: valid in Rust but outside the list in b2p_regex.hpp (the query stays on the CPU).
+ * b2p_plan_last_error says why for 1 and 2.  B2P_E_INVALID for a NULL regex. */
+B2P_API int b2p_label_regex_check(const char* regex);
+/* Host only, no context: regexp_replace(input, "^(?s:" + regex + ")$", replacement) as label_replace evaluates one
+ * value.  Writes the result and a terminating NUL to out when it fits in cap bytes; *out_len (when not NULL) gets the
+ * result's length either way.  B2P_OK, B2P_E_TOO_LARGE when it does not fit, B2P_E_INVALID for a NULL argument or a
+ * regex whose verdict is not 0 (b2p_plan_last_error says why). */
+B2P_API int b2p_label_regex_replace(const char* regex, const char* replacement, const char* input, char* out,
+                                    uint64_t cap, uint64_t* out_len);
 B2P_API int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSchema* schema);
 B2P_API int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema);
 B2P_API int64_t b2p_plan_num_series(b2p_plan* plan);

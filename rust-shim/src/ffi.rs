@@ -594,6 +594,25 @@ extern "C" {
     ) -> *mut b2p_plan;
     /// timestamp(<selector>) on a range node: the instant form whose value is the sample's timestamp in seconds.
     pub fn b2p_plan_set_timestamp(plan: *mut b2p_plan, lookback_delta: i64) -> c_int;
+    /// label_replace(child, dst, replacement, src, regex); ownership of `child` as for b2p_plan_binary_create.
+    pub fn b2p_plan_label_replace_create(
+        ctx: *mut b2p_ctx, child: *mut b2p_plan, dst: *const c_char, replacement: *const c_char, src: *const c_char,
+        regex: *const c_char,
+    ) -> *mut b2p_plan;
+    /// label_join(child, dst, separator, srcs..); ownership of `child` as for b2p_plan_binary_create.
+    pub fn b2p_plan_label_join_create(
+        ctx: *mut b2p_ctx, child: *mut b2p_plan, dst: *const c_char, separator: *const c_char,
+        srcs: *const *const c_char, n_srcs: i32,
+    ) -> *mut b2p_plan;
+    /// Host only: 0 = a label_replace regex the library evaluates, 1 = Rust's regex crate rejects it, 2 = valid in Rust
+    /// but outside the library's supported list (the query stays on the CPU).
+    pub fn b2p_label_regex_check(regex: *const c_char) -> c_int;
+    /// Host only: regexp_replace(input, "^(?s:" + regex + ")$", replacement) into `out` (NUL-terminated, `cap` bytes);
+    /// `out_len` gets the result's length.
+    pub fn b2p_label_regex_replace(
+        regex: *const c_char, replacement: *const c_char, input: *const c_char, out: *mut c_char, cap: u64,
+        out_len: *mut u64,
+    ) -> c_int;
     /// `modifier`: NULL, "by" or "without"; ownership of `child` as for b2p_plan_binary_create.
     pub fn b2p_plan_topk_create(
         ctx: *mut b2p_ctx, bottom: i32, k: f64, child: *mut b2p_plan, modifier: *const c_char,

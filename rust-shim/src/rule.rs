@@ -120,6 +120,13 @@
 //!                                             => the child itself
 //! ```
 //!
+//! label_replace / label_join (planner.rs:2306-2356, 2504-2700):
+//!
+//! ```text
+//!   ProjectionExec(ts, values.., regexp_replace(tag, "^(?s:re)$", r) | Utf8(r) | concat_ws(sep, tag | NULL, ..) AS dst,
+//!     tags..) <- GpuPromRangeExec              => `match_label`: the b2p_plan_label_{replace,join}_create arguments
+//! ```
+//!
 //! Over a table with several field columns the rule takes the shapes the library evaluates per field (the leaf, the
 //! aggregate node with one aggregate per field, sort by every field, subqueries, absent, the binary zip) and leaves on
 //! the CPU those the library refuses there (the leaf's own aggregate, filtering comparisons over two or more fields,
@@ -430,6 +437,40 @@ pub struct GpuPromAbsentSpec {
     pub value_column: String,
     pub labels: Vec<(String, String)>,
     pub child: GpuPromRangeParams,
+}
+
+/// What `b2p_plan_label_replace_create` / `b2p_plan_label_join_create` take for a matched label projection: label_replace
+/// (dst, replacement, src, the raw regex) when `join` is false, label_join (dst, separator in `replacement`, srcs with
+/// "" for a NULL source) when it is true, and the child node.
+#[derive(Debug, Clone)]
+pub struct GpuPromLabelSpec {
+    pub join: bool,
+    pub dst: String,
+    pub replacement: String,
+    pub src: String,
+    pub regex: String,
+    pub srcs: Vec<String>,
+    pub child: GpuPromRangeParams,
+}
+
+/// Whether the library evaluates a label_replace regex (`b2p_label_regex_check` == 0): a pattern it reports invalid or
+/// unsupported keeps the query on the CPU, which gives the reference's error or result itself.
+fn label_regex_supported(regex: &str) -> bool {
+    let Ok(c) = std::ffi::CString::new(regex) else { return false };
+    // SAFETY: a host-only call on a NUL-terminated string that outlives it
+    unsafe { crate::ffi::b2p_label_regex_check(c.as_ptr()) == 0 }
+}
+
+/// `^(?s:<raw>)$` -> raw: the pattern build_regexp_replace_label_expr wrapped (planner.rs:2579)
+fn unwrap_label_regex(wrapped: &str) -> Option<&str> {
+    wrapped.strip_prefix("^(?s:")?.strip_suffix(")$")
+}
+
+fn utf8_literal(e: &Arc<dyn PhysicalExpr>) -> Option<String> {
+    match scalar_literal(e)? {
+        ScalarValue::Utf8(Some(v)) => Some(v.clone()),
+        _ => None,
+    }
 }
 
 /// The instant-vector functions the library evaluates, by ScalarFunctionExpr::name(), with the number of literal
@@ -1035,6 +1076,77 @@ impl GpuPromRewrite {
         }
         let function = if descending { "sort_by_label_desc" } else { "sort_by_label" };
         Some(GpuPromSortSpec { function: function.to_string(), labels, child: params.clone() })
+    }
+
+    /// `ProjectionExec(plain columns, one generated `<expr> AS dst`) <- GpuPromRangeExec`, the projection
+    /// label_replace / label_join plan (planner.rs:1012-1101, 2306-2356, 2518-2700), with `<expr>` one of
+    /// `regexp_replace(<tag column>, Utf8("^(?s:<raw>)$"), Utf8(r))`, `Utf8(r)` (a source that is not a tag) or
+    /// `concat_ws(Utf8(sep), <tag column> | NULL, ..)` -> the arguments of `b2p_plan_label_replace_create` /
+    /// `b2p_plan_label_join_create`.  A regex the library does not support, a source column that is not a tag of the
+    /// child (the time index or a value column), an id-keyed child and every other shape stay on the CPU.  No-op
+    /// label_replace plans have no generated expression: `match_passthrough` takes them.
+    pub fn match_label(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromLabelSpec> {
+        let p = plan.as_any().downcast_ref::<ProjectionExec>()?;
+        let child = p.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
+        let params = child.params();
+        if params.tag_columns == [String::from("__tsid")] {
+            return None;
+        }
+        let mut generated = None;
+        for e in p.expr() {
+            if e.expr.as_any().downcast_ref::<Column>().is_none() {
+                if generated.is_some() {
+                    return None;
+                }
+                generated = Some((e.expr.clone(), e.alias.clone()));
+            }
+        }
+        let (expr, dst) = generated?;
+        let tag = |e: &Arc<dyn PhysicalExpr>| {
+            let c = e.as_any().downcast_ref::<Column>()?;
+            params.tag_columns.iter().any(|t| t == c.name()).then(|| c.name().to_string())
+        };
+        let spec = |join, replacement: String, src: String, regex: String, srcs: Vec<String>| GpuPromLabelSpec {
+            join,
+            dst: dst.clone(),
+            replacement,
+            src,
+            regex,
+            srcs,
+            child: params.clone(),
+        };
+        if let Some(r) = utf8_literal(&expr) {
+            return (!r.is_empty()).then(|| spec(false, r, String::new(), String::new(), vec![]));
+        }
+        let f = expr.as_any().downcast_ref::<ScalarFunctionExpr>()?;
+        match f.name() {
+            "regexp_replace" => {
+                let [src, pattern, replacement] = f.args() else { return None };
+                let src = tag(src)?;
+                let pattern = utf8_literal(pattern)?;
+                let raw = unwrap_label_regex(&pattern)?;
+                if !label_regex_supported(raw) {
+                    return None;
+                }
+                Some(spec(false, utf8_literal(replacement)?, src, raw.to_string(), vec![]))
+            }
+            "concat_ws" => {
+                let (sep, args) = f.args().split_first()?;
+                let srcs = args
+                    .iter()
+                    .map(|a| match scalar_literal(a) {
+                        Some(ScalarValue::Null) | Some(ScalarValue::Utf8(None)) => Some(String::new()),
+                        Some(_) => None,
+                        None => tag(a),
+                    })
+                    .collect::<Option<Vec<String>>>()?;
+                if srcs.is_empty() {
+                    return None;
+                }
+                Some(spec(true, utf8_literal(sep)?, String::new(), String::new(), srcs))
+            }
+            _ => None,
+        }
     }
 
     /// `PromAbsentExec <- SortExec(ts) <- AggregateExec(ts, first_value(field)) [<- RepartitionExec <-
