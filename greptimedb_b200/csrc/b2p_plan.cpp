@@ -60,22 +60,42 @@ void check(int rc, ErrorKind invalid = ErrorKind::Plan) {
   throw PlanError(rc == B2P_E_UNSORTED ? ErrorKind::Internal : ErrorKind::Execution, b2p_last_error());
 }
 
-// The nodes that read an Int32 (calendar) column as a number other than element-wise: DataFusion's integer result
-// types for them are not pinned by the reference tree, so the query stays on the CPU
-void refuse_i32(const NodeResult& r, const char* node) {
-  if (r.any_i32()) throw PlanError(ErrorKind::Plan, std::string(node) + ": an Int32 value column is not supported by this node");
-}
-
-// Field f of r read as Float64 from here on: an Int64 field is coerced on the device ((double)i64, b2p_i64_to_f64), as
-// DataFusion coerces an Int64 column under a Float64 projection, aggregate or scalar()
+// Field f of r read as Float64 from here on.  Only an Int64 field's cells change: they are coerced on the device
+// ((double)i64, b2p_i64_to_f64), as DataFusion coerces an Int64 column under a Float64 projection, aggregate or
+// scalar(); Int32 and Count cells already hold their value as a double, and converting them would misread them.
 void field_to_f64(b2p_ctx* ctx, NodeResult& r, uint32_t f) {
-  if (!r.is_i64(f)) return;
-  if (r.grid() > 0) check(b2p_i64_to_f64(ctx, reinterpret_cast<const int64_t*>(r.field(f)), r.grid(), r.field(f)));
+  if (r.types[f] == ValueType::Int64 && r.grid() > 0)
+    check(b2p_i64_to_f64(ctx, reinterpret_cast<const int64_t*>(r.field(f)), r.grid(), r.field(f)));
   r.types[f] = ValueType::Float64;
 }
 void to_f64(b2p_ctx* ctx, NodeResult& r) {
   for (uint32_t f = 0; f < r.F; ++f) field_to_f64(ctx, r, f);
-  r.types.clear();
+}
+
+// r's steps: the grid start + k * interval <= end
+void set_grid(NodeResult& r, Millisecond start, Millisecond end, Millisecond interval) {
+  r.T = b2p_num_steps(start, end, interval);
+  r.Tw = (uint32_t)((r.T + 31) / 32);
+  r.eval_ts.resize((size_t)r.T);
+  for (int64_t k = 0; k < r.T; ++k) r.eval_ts[(size_t)k] = start + k * interval;
+}
+
+// The shapes of child result a node may refuse (DESIGN §1 a24-a27).  Int32: DataFusion's integer result types are not
+// pinned by the reference tree for a node that reads the number other than element-wise.  Counted: a count_values
+// result, whose counted value the reference carries as a column this layer does not model above it.
+enum class Shape { MultiField, Int32, Int64, IdKeyed, Counted };
+
+// A node's contract with its one child, checked before the node's work: the first listed shape the child has is a Plan
+// error with its text (an empty text accepts the shape after all)
+void check_child(const NodeResult& c, std::initializer_list<std::pair<Shape, std::string>> refused) {
+  for (const auto& [shape, text] : refused) {
+    const bool hit = shape == Shape::MultiField ? c.F > 1
+                     : shape == Shape::Int32    ? c.has(ValueType::Int32)
+                     : shape == Shape::Int64    ? c.has(ValueType::Int64)
+                     : shape == Shape::IdKeyed  ? c.labels.id_keyed
+                                                : c.columns == Columns::CountTagsTimeLabel;
+    if (hit && !text.empty()) throw PlanError(ErrorKind::Plan, text);
+  }
 }
 
 // dense ids of keys, in first-insertion order
@@ -320,8 +340,8 @@ constexpr int kAggGroup = B2P_AGG_STDVAR + 1, kAggQuantile = B2P_AGG_STDVAR + 2;
 // their tuple over `cols` (of r.labels), folded on the device in row order, become one row per group in label order,
 // a group having a cell at step k iff one of its rows has.  op: enum b2p_agg, kAggGroup (1.0 wherever count is
 // non-zero) or kAggQuantile (param = φ).  Each field is folded by its own call over the same group ids; the counts
-// depend on the shared validity alone, so field 0's decide the cells.  Sets the rows, labels, grids and column layout;
-// keeps T, the fields and the time index.
+// depend on the shared validity alone, so field 0's decide the cells.  Sets the rows, labels, grids, types and column
+// layout, drops a counted column; keeps T, the fields and the time index.
 void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& cols, NodeResult& r) {
   Groups groups = group_rows(r.labels, cols, r.rows);
   const uint32_t G = (uint32_t)groups.rank.size(), Tw = r.Tw, F = r.F;
@@ -330,14 +350,11 @@ void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& 
   std::vector<uint32_t> gcnt((size_t)G * T), fcnt(F > 1 ? (size_t)G * T : 0);
   // an Int64 field stays Int64 under sum, min and max (DataFusion's Int64 accumulators); the others give Float64
   const bool int_result = op == B2P_AGG_SUM || op == B2P_AGG_MIN || op == B2P_AGG_MAX;
-  std::vector<ValueType> types;
+  std::vector<ValueType> types(F, ValueType::Float64);
   for (uint32_t f = 0; f < F; ++f) {
-    const bool i64 = r.is_i64(f) && op != kAggQuantile && op != kAggGroup;
-    if (r.is_i64(f) && op == kAggQuantile) field_to_f64(ctx, r, f);
-    if (int_result && r.is_i64(f)) {
-      types.resize(F, ValueType::Float64);
-      types[f] = ValueType::Int64;
-    }
+    const bool i64 = r.types[f] == ValueType::Int64 && op != kAggQuantile && op != kAggGroup;
+    if (op == kAggQuantile) field_to_f64(ctx, r, f);
+    if (int_result && r.types[f] == ValueType::Int64) types[f] = ValueType::Int64;
     if (G == 0 || T == 0) continue;
     double* gv = gval.data() + (size_t)f * G * T;
     uint32_t* gc = f == 0 ? gcnt.data() : fcnt.data();
@@ -354,6 +371,7 @@ void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& 
   r.labels = std::move(groups.labels);
   r.columns = Columns::TagsTimeValue;
   r.cell_order.clear();
+  r.counted.reset();
   r.val.assign((size_t)F * G * T, 0.0);
   r.valid.assign((size_t)G * Tw, 0u);
   for (uint32_t g = 0; g < G; ++g) {
@@ -414,7 +432,7 @@ HistogramIndex histogram_index(const Labels& in, int le, uint32_t rows) {
 
 // ---- PromRangePlan -------------------------------------------------------------------------------------
 PromRangePlan::PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args) : PlanNode(ctx), args_(std::move(args)) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromRangeExec: NULL context");
+  require("GpuPromRangeExec", {});
   fn_id_ = args_.function.empty() ? -1 : function_id_from_name(args_.function);
   if (fn_id_ < 0 && !args_.function.empty())
     throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: unknown range function " + args_.function);
@@ -623,11 +641,13 @@ void PromRangePlan::compute(NodeResult& r) {
   p.offset = args_.offset;
   p.param0 = args_.param0;
   p.param1 = args_.param1;
-  const int64_t T = b2p_num_steps(p.start, p.end, p.interval);
+  r = NodeResult();
+  set_grid(r, p.start, p.end, p.interval);  // also when there are no series: scalar() of such a node has a NaN row at every step
+  const int64_t T = r.T;
+  const uint32_t Tw = r.Tw;
   const uint32_t S = (uint32_t)num_series_;
   offsets_.resize((size_t)S);          // (a previous execute() appended the end marker)
   offsets_.push_back((uint64_t)ts_.size());
-  const uint32_t Tw = (uint32_t)((T + 31) / 32);
   // timestamp(): one Float64 value whatever the fields, DEFAULT_FIELD_COLUMN (planner.rs:951-965); no value is read
   const uint32_t F = timestamp_ ? 1u : (uint32_t)args_.field_columns.size();
   const bool fold_on_device = args_.histogram && fn_id_ >= 0;  // the dense matrix then never reaches the host
@@ -666,14 +686,9 @@ void PromRangePlan::compute(NodeResult& r) {
                                                   ts_.data(), vals.data(), nulls, (int32_t)F, nullptr, offsets_.data(),
                                                   ts_.size(), S, outs.data(), valid.data()));
   }
-  r = NodeResult();
-  r.T = T;
-  r.Tw = Tw;
   r.F = F;
-  r.eval_ts.resize((size_t)T);  // also when there are no series: scalar() of such a node has a NaN row at every step
-  for (int64_t k = 0; k < T; ++k) r.eval_ts[(size_t)k] = p.start + k * p.interval;
+  r.types = timestamp_ || types_.empty() ? std::vector<ValueType>(F, ValueType::Float64) : types_;
   r.time_index = args_.time_index;
-  if (!timestamp_ && std::find(types_.begin(), types_.end(), ValueType::Int64) != types_.end()) r.types = types_;
   for (const std::string& field : args_.field_columns)
     r.value_names.push_back(fn_id_ >= 0 ? args_.function + "(" + args_.time_index + "_range," + field + ")" : field);
   if (timestamp_) r.value_names = {"value"};
@@ -757,33 +772,44 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
   OwnedColumn* c_ts = nullptr;
   std::vector<OwnedColumn*> c_vals;  // [F]
   OwnedColumn* c_label = nullptr;    // count_values' counted value
-  const bool int_val = r.columns == Columns::CountTagsTimeLabel && r.value_is_count;
   if (r.value_names.size() != r.F) throw PlanError(ErrorKind::Internal, "export: one value name per field expected");
-  auto add_vals = [&](const char* fmt) {  // "g" is each field's own type
-    for (uint32_t f = 0; f < r.F; ++f)
-      c_vals.push_back(add_col(r.value_names[f], r.is_i64(f) ? "l" : r.is_i32(f) ? "i" : fmt));
+  if (r.types.size() != r.F) throw PlanError(ErrorKind::Internal, "export: one type per field expected");
+  if (r.columns == Columns::CountTagsTimeLabel && !r.counted)
+    throw PlanError(ErrorKind::Internal, "export: the count_values layout without its counted column");
+  // the Arrow format of a column of type t, and how a cell of it is stored
+  auto format = [](ValueType t) { return t == ValueType::Float64 ? "g" : t == ValueType::Int32 ? "i" : "l"; };
+  auto put = [](OwnedColumn* c, ValueType t, double v) {
+    switch (t) {
+      case ValueType::Float64: c->f64.push_back(v); break;
+      case ValueType::Int64: c->i64.push_back(bits_i64(v)); break;
+      case ValueType::Int32: c->i32.push_back((int32_t)v); break;
+      case ValueType::Count: c->i64.push_back((int64_t)v); break;
+    }
+  };
+  auto add_vals = [&] {
+    for (uint32_t f = 0; f < r.F; ++f) c_vals.push_back(add_col(r.value_names[f], format(r.types[f])));
   };
   switch (r.columns) {
     case Columns::TimeValueTags:
       c_ts = add_col(r.time_index, "tsm:");
-      add_vals("g");
+      add_vals();
       for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
       break;
     case Columns::TagsTimeValue:
       for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
       c_ts = add_col(r.time_index, "tsm:");
-      add_vals("g");
+      add_vals();
       break;
     case Columns::ValueTagsTime:
-      add_vals("g");
+      add_vals();
       for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
       c_ts = add_col(r.time_index, "tsm:");
       break;
     case Columns::CountTagsTimeLabel:
-      add_vals(int_val ? "l" : "g");
+      add_vals();
       for (size_t t = 0; t < L.names.size(); ++t) add_tag(t);
       c_ts = add_col(r.time_index, "tsm:");
-      c_label = add_col(r.label_name, r.label_is_i64 ? "l" : "g");
+      c_label = add_col(r.counted->name, format(r.counted->type));
       break;
     case Columns::TimeSorted: {  // (`or`, one field)
       c_ts = add_col(r.time_index, "tsm:");
@@ -792,14 +818,14 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
       std::sort(names.begin(), names.end());
       for (const std::string& name : names) {
         if (name == r.value_names[0] && c_vals.empty())
-          c_vals.push_back(add_col(name, r.is_i64(0) ? "l" : r.is_i32(0) ? "i" : "g"));
+          c_vals.push_back(add_col(name, format(r.types[0])));
         else add_tag((size_t)L.column(name));
       }
       break;
     }
     case Columns::TimeValueLastTag:
       c_ts = add_col(r.time_index, "tsm:");
-      add_vals("g");
+      add_vals();
       if (!L.names.empty()) add_tag(L.names.size() - 1);
       for (size_t t = 0; t + 1 < L.names.size(); ++t) add_tag(t);
       break;
@@ -815,18 +841,9 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     const int64_t k = (int64_t)(cell % (uint64_t)r.T);
     if (!r.valid_at(row, k)) continue;
     c_ts->i64.push_back(r.eval_ts[(size_t)k]);
-    for (uint32_t f = 0; f < r.F; ++f) {
-      const double v = r.field(f)[(size_t)row * (size_t)r.T + (size_t)k];
-      if (int_val) c_vals[f]->i64.push_back((int64_t)v);
-      else if (r.is_i64(f)) c_vals[f]->i64.push_back(bits_i64(v));
-      else if (r.is_i32(f)) c_vals[f]->i32.push_back((int32_t)v);
-      else c_vals[f]->f64.push_back(v);
-    }
-    if (c_label) {
-      const double v = r.label_val[(size_t)row * (size_t)r.T + (size_t)k];
-      if (r.label_is_i64) c_label->i64.push_back(bits_i64(v));
-      else c_label->f64.push_back(v);
-    }
+    const size_t at = (size_t)row * (size_t)r.T + (size_t)k;
+    for (uint32_t f = 0; f < r.F; ++f) put(c_vals[f], r.types[f], r.field(f)[at]);
+    if (c_label) put(c_label, r.counted->type, r.counted->values[at]);
     for (size_t t = 0; t < c_tags.size(); ++t) {
       if (L.id_keyed) {
         c_tags[t]->i64.push_back((int64_t)L.ids[row]);
@@ -1003,9 +1020,14 @@ void PlanNode::add_function(const std::string& name, const std::vector<double>& 
   throw PlanError(ErrorKind::Plan, "unsupported instant-vector function " + name);
 }
 
+void PlanNode::require(const char* node, std::initializer_list<const PlanNode*> children, bool device) const {
+  if (device && !ctx_) throw PlanError(ErrorKind::Internal, std::string(node) + ": NULL context");
+  for (const PlanNode* c : children)
+    if (!c) throw PlanError(ErrorKind::Plan, std::string(node) + ": NULL child");
+}
+
 void PlanNode::run(NodeResult& r) {
   compute(r);
-  if (!stages_.empty()) r.value_is_count = false;  // a stage's result is a Float64 projection
   for (const Stage& s : stages_) {
     const bool work = r.rows > 0 && r.T > 0;
     if (s.part >= 0) {
@@ -1019,17 +1041,16 @@ void PlanNode::run(NodeResult& r) {
       r.value_names = {date_part_name(s, r.time_index)};
       continue;
     }
-    if (s.is_fn && s.op == B2P_IFN_NEG && (r.any_i64() || r.any_i32()))  // integer negation and its overflow
+    const bool filter = !s.is_fn && is_comparison(s.op) && !s.return_bool;
+    if (s.is_fn && s.op == B2P_IFN_NEG && (r.has(ValueType::Int64) || r.has(ValueType::Int32)))  // integer negation and its overflow
       throw PlanError(ErrorKind::Plan, "unary minus over an integer value column is not supported by this node");
     // an Int64 value column under a stage: a filter would keep the Int64 column, which the reference tree does not
     // pin; a projection reads it as Float64 (DataFusion's coercion against the Float64 literal or function)
-    if (r.any_i64() && !s.is_fn && is_comparison(s.op) && !s.return_bool)
+    if (filter && r.has(ValueType::Int64))
       throw PlanError(ErrorKind::Plan, "a filtering comparison over an Int64 value column is not supported by this node");
-    // an Int32 (calendar) column: a filter keeps it, every projection reads it as Float64 (its cells already are)
-    const std::vector<ValueType> kept = r.any_i32() && !s.is_fn && is_comparison(s.op) && !s.return_bool
-                                            ? r.types : std::vector<ValueType>{};
-    to_f64(ctx_, r);
-    r.types = kept;
+    // a filter keeps an Int32 (calendar) column; every other stage's result, and a filter's over a count, is Float64
+    for (uint32_t f = 0; f < r.F; ++f)
+      if (!(filter && r.types[f] == ValueType::Int32)) field_to_f64(ctx_, r, f);
     if (s.is_fn) {
       const double a0 = s.args.size() > 0 ? s.args[0] : 0.0, a1 = s.args.size() > 1 ? s.args[1] : 0.0;
       // clamp's bound check (clamp.rs:212-217); clamp_min / clamp_max meet the other bound at ±f64::MAX.  The reference
@@ -1054,7 +1075,6 @@ void PlanNode::run(NodeResult& r) {
       }
       continue;
     }
-    const bool filter = is_comparison(s.op) && !s.return_bool;
     if (filter && r.F > 1)  // planner.rs:3976-3981
       throw PlanError(ErrorKind::Plan, "Unsupported expr type: filter on multi-value input");
     for (uint32_t f = 0; f < r.F && work; ++f)  // arithmetic and `bool` keep every bit (planner.rs:3930-3960)
@@ -1081,8 +1101,7 @@ BinaryPlan::BinaryPlan(b2p_ctx* ctx, int op, bool return_bool, std::shared_ptr<P
                        bool labels_from_lhs)
     : PlanNode(ctx), op_(op), return_bool_(return_bool), lhs_(std::move(lhs)), rhs_(std::move(rhs)),
       matching_(matching), labels_(std::move(labels)), labels_from_lhs_(labels_from_lhs) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromBinaryExec: NULL context");
-  if (!lhs_ || !rhs_) throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: NULL child");
+  require("GpuPromBinaryExec", {lhs_.get(), rhs_.get()});
   check_op(op_, return_bool_);
 }
 
@@ -1108,14 +1127,15 @@ void BinaryPlan::compute(NodeResult& r) {
   // Int64 operands: against a Float64 side DataFusion coerces to Float64; between two Int64 sides it would run integer
   // arithmetic, division and overflow, which the reference tree does not pin, and a filter would keep the Int64 column
   for (uint32_t f = 0; f < std::min(L.F, R.F); ++f)
-    if (L.is_i64(f) && R.is_i64(f))
+    if (L.is(f, ValueType::Int64) && R.is(f, ValueType::Int64))
       throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: a binary operator between two Int64 value columns is not supported by this node");
   // an Int32 (calendar) side meets a Float64 side only: DataFusion's integer result types are not pinned here
-  if ((L.any_i32() && (R.any_i32() || R.any_i64())) || (R.any_i32() && L.any_i64()))
+  if (L.has(ValueType::Int32) ? R.has(ValueType::Int32) || R.has(ValueType::Int64) : R.has(ValueType::Int32) && L.has(ValueType::Int64))
     throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: a binary operator between two integer value columns is not supported by this node");
-  const std::vector<ValueType> lhs_i32 = L.any_i32() ? L.types : std::vector<ValueType>{};
-  if (L.any_i64() && is_comparison(op) && !return_bool_)
+  const bool filter = is_comparison(op) && !return_bool_;
+  if (filter && L.has(ValueType::Int64))
     throw PlanError(ErrorKind::Plan, "a filtering comparison over an Int64 value column is not supported by this node");
+  const std::vector<ValueType> lhs_types = L.types;  // a filter keeps the lhs column and its type
   to_f64(ctx_, L);
   to_f64(ctx_, R);
   // join keys (planner.rs:696-729, 3436-3468): the rhs context's tag columns, narrowed by on / ignoring; none when a
@@ -1154,7 +1174,6 @@ void BinaryPlan::compute(NodeResult& r) {
   if (n_pairs > UINT32_MAX) throw PlanError(ErrorKind::Plan, "GpuPromBinaryExec: more than 2^32 - 1 matched series pairs");
   // the fields zip pairwise, field i with field i (align_binary_field_columns, planner.rs:3401-3414); a filter decides
   // on its one pair and keeps every field of the lhs
-  const bool filter = is_comparison(op) && !return_bool_;
   const uint32_t pairs = std::min(L.F, R.F);
   if (filter && pairs > 1) throw PlanError(ErrorKind::Plan, "Unsupported expr type: filter on multi-value input");
   r = NodeResult();
@@ -1162,6 +1181,7 @@ void BinaryPlan::compute(NodeResult& r) {
   r.Tw = L.Tw;
   r.rows = (uint32_t)n_pairs;
   r.F = filter ? L.F : pairs;
+  r.types = filter ? lhs_types : std::vector<ValueType>(pairs, ValueType::Float64);
   r.eval_ts = L.eval_ts;
   r.val.assign((size_t)r.F * n_pairs * (size_t)r.T, 0.0);
   r.valid.assign((size_t)n_pairs * r.Tw, 0u);
@@ -1184,15 +1204,12 @@ void BinaryPlan::compute(NodeResult& r) {
   r.labels = side.labels.gather(srow);
   if (filter) {
     r.columns = L.columns;
-    r.types = lhs_i32;  // a filter keeps the lhs column and its type
     r.value_names = L.value_names;
-    r.label_name = L.label_name;
-    r.label_is_i64 = L.label_is_i64;
-    r.value_is_count = L.value_is_count;
-    if (!L.label_val.empty()) {
-      r.label_val.resize((size_t)n_pairs * (size_t)r.T);
+    if (L.counted) {  // the kept rows' counted values
+      r.counted = CountedColumn{L.counted->name, L.counted->type, std::vector<double>((size_t)n_pairs * (size_t)r.T)};
       for (uint64_t p = 0; p < n_pairs; ++p)
-        std::copy_n(L.label_val.begin() + (size_t)lrow[p] * (size_t)r.T, (size_t)r.T, r.label_val.begin() + (size_t)p * (size_t)r.T);
+        std::copy_n(L.counted->values.begin() + (size_t)lrow[p] * (size_t)r.T, (size_t)r.T,
+                    r.counted->values.begin() + (size_t)p * (size_t)r.T);
     }
   } else {
     r.columns = Columns::TagsTimeValue;
@@ -1208,7 +1225,7 @@ const char* const kSetNames[] = {"and", "or", "unless"};
 
 // left.distinct() of `and` / `unless` (planner.rs:3549-3703): a cell whose labels, step and value bits (DataFusion's
 // group equality on f64) equal those of a cell of an earlier row is dropped.  Only rows that share a label tuple can
-// hold such cells, so only they are compared.  count_values' counted value is a column of the row too.
+// hold such cells, so only they are compared.  A counted value is a column of the row too.
 void drop_duplicate_cells(NodeResult& n) {
   if (n.rows < 2 || n.T == 0) return;
   std::vector<int> all(n.labels.names.size());
@@ -1229,7 +1246,7 @@ void drop_duplicate_cells(NodeResult& n) {
           const double y = n.val[(size_t)g[j] * (size_t)n.T + (size_t)k];
           const size_t a = (size_t)g[i] * (size_t)n.T + (size_t)k, b = (size_t)g[j] * (size_t)n.T + (size_t)k;
           if (n.valid_at(g[j], k) && std::memcmp(&x, &y, sizeof x) == 0 &&
-              (n.label_val.empty() || std::memcmp(&n.label_val[a], &n.label_val[b], sizeof(double)) == 0)) {
+              (!n.counted || std::memcmp(&n.counted->values[a], &n.counted->values[b], sizeof(double)) == 0)) {
             n.valid[(size_t)g[i] * n.Tw + (size_t)(k >> 5)] &= ~(1u << (k & 31));
             n.val[(size_t)g[i] * (size_t)n.T + (size_t)k] = 0.0;
             break;
@@ -1244,8 +1261,7 @@ void drop_duplicate_cells(NodeResult& n) {
 SetOpPlan::SetOpPlan(b2p_ctx* ctx, int op, std::shared_ptr<PlanNode> lhs, std::shared_ptr<PlanNode> rhs,
                      Matching matching, std::vector<std::string> labels)
     : PlanNode(ctx), op_(op), lhs_(std::move(lhs)), rhs_(std::move(rhs)), matching_(matching), labels_(std::move(labels)) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromSetOpExec: NULL context");
-  if (!lhs_ || !rhs_) throw PlanError(ErrorKind::Plan, "GpuPromSetOpExec: NULL child");
+  require("GpuPromSetOpExec", {lhs_.get(), rhs_.get()});
   if (op_ < B2P_SET_AND || op_ > B2P_SET_UNLESS) throw PlanError(ErrorKind::Plan, "unknown set operator " + std::to_string(op_));
 }
 
@@ -1265,9 +1281,9 @@ void SetOpPlan::compute(NodeResult& r) {
                                          list(L.value_names) + ", right: " + list(R.value_names));
   }
   // `and` / `unless` keep the lhs column and its type; `or` over an Int64 side is not pinned by the reference tree
-  if (op_ == B2P_SET_OR && (L.any_i64() || R.any_i64()))
+  if (op_ == B2P_SET_OR && (L.has(ValueType::Int64) || R.has(ValueType::Int64)))
     throw PlanError(ErrorKind::Plan, what + "an Int64 value column is not supported by this node");
-  if (op_ == B2P_SET_OR && L.any_i32() != R.any_i32())  // `or` of Int32 with Int32 stays Int32
+  if (op_ == B2P_SET_OR && L.has(ValueType::Int32) != R.has(ValueType::Int32))  // `or` of Int32 with Int32 stays Int32
     throw PlanError(ErrorKind::Plan, what + "an Int32 value column against another type is not supported by this node");
   if (L.F > 1)
     throw PlanError(ErrorKind::Plan, std::string("Multi fields calculation is not supported in ") +
@@ -1347,7 +1363,7 @@ void SetOpPlan::compute(NodeResult& r) {
                           rkey.data(), R.rows, (uint32_t)keys.ids.size(), (uint64_t)T, r.val.data(), r.valid.data()));
   r.time_index = L.time_index;
   r.value_names = L.value_names;
-  r.types = L.types;
+  r.types = {L.has(ValueType::Int32) ? ValueType::Int32 : ValueType::Float64};  // (a count is Float64 here)
   r.columns = Columns::TimeSorted;
   r.labels.names = all;
   r.labels.values.resize(all.size());
@@ -1361,15 +1377,14 @@ void SetOpPlan::compute(NodeResult& r) {
 
 // ---- ScalarPlan ----------------------------------------------------------------------------------------
 ScalarPlan::ScalarPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child) : PlanNode(ctx), child_(std::move(child)) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromScalarExec: NULL context");
-  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromScalarExec: NULL child");
+  require("GpuPromScalarExec", {child_.get()});
 }
 
 void ScalarPlan::compute(NodeResult& r) {
   NodeResult C;
   child_->run(C);
-  refuse_i32(C, "GpuPromScalarExec");
-  if (C.F > 1) throw PlanError(ErrorKind::Plan, "Multi fields calculation is not supported in scalar");  // planner.rs:3155-3160
+  check_child(C, {{Shape::Int32, "GpuPromScalarExec: an Int32 value column is not supported by this node"},
+                  {Shape::MultiField, "Multi fields calculation is not supported in scalar"}});  // planner.rs:3155-3160
   to_f64(ctx_, C);  // scalar() of an Int64 node is Float64
   // one dense key per label tuple over the child's tag columns (a tagless child is one series, an id-keyed one is keyed
   // by the id); a tuple with a NULL label gets B2P_NO_KEY (scalar_calculate.rs:543-569 compares NULL as None against
@@ -1428,17 +1443,16 @@ std::vector<int> group_columns(const Labels& L, Modifier modifier, const std::ve
 TopkPlan::TopkPlan(b2p_ctx* ctx, bool bottom, double k, std::shared_ptr<PlanNode> child, Modifier modifier,
                    std::vector<std::string> labels)
     : PlanNode(ctx), bottom_(bottom), k_(k), child_(std::move(child)), modifier_(modifier), labels_(std::move(labels)) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromTopkExec: NULL context");
-  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromTopkExec: NULL child");
+  require("GpuPromTopkExec", {child_.get()});
 }
 
 void TopkPlan::compute(NodeResult& r) {
   child_->run(r);
-  if (r.F > 1)  // planner.rs:2969-2974
-    throw PlanError(ErrorKind::Plan, "Unsupported expr type: topk or bottomk on multi-value input");
-  const char* what = bottom_ ? "bottomk: " : "topk: ";
-  // the window orders ties by the label values (planner.rs:2980-2996), which an id-keyed node does not carry
-  if (r.labels.id_keyed) throw PlanError(ErrorKind::Plan, std::string(what) + "an id-keyed (__tsid) child has no label values to order by");
+  // planner.rs:2969-2974; the window orders ties by the label values (planner.rs:2980-2996), which an id-keyed node
+  // does not carry
+  check_child(r, {{Shape::MultiField, "Unsupported expr type: topk or bottomk on multi-value input"},
+                  {Shape::IdKeyed, std::string(bottom_ ? "bottomk: " : "topk: ") +
+                                       "an id-keyed (__tsid) child has no label values to order by"}});
   const Labels& L = r.labels;
   const std::vector<int> gcols = group_columns(L, modifier_, labels_);
   KeyIds groups;
@@ -1466,7 +1480,7 @@ void TopkPlan::compute(NodeResult& r) {
   std::vector<uint32_t> tie(r.rows);
   for (uint32_t p = 0; p < r.rows; ++p) tie[order[p]] = bottom_ ? p : r.rows - 1 - p;
   if (r.rows > 0 && r.T > 0)
-    check(r.is_i64(0) ? b2p_topk_i64(ctx_, bottom_ ? 1 : 0, k_, reinterpret_cast<const int64_t*>(r.val.data()),
+    check(r.is(0, ValueType::Int64) ? b2p_topk_i64(ctx_, bottom_ ? 1 : 0, k_, reinterpret_cast<const int64_t*>(r.val.data()),
                                      r.valid.data(), gid.data(), r.rows, (uint32_t)groups.ids.size(), tie.data(),
                                      (uint64_t)r.T, r.valid.data())
                       : b2p_topk(ctx_, bottom_ ? 1 : 0, k_, r.val.data(), r.valid.data(), gid.data(), r.rows,
@@ -1485,21 +1499,22 @@ void TopkPlan::compute(NodeResult& r) {
     }
     const uint64_t ka = a % T, kb = b % T;
     if (ka != kb) return ka < kb;
-    const bool i64 = r.is_i64(0);  // (an Int64 value compares as the integer its bits are)
+    const bool i64 = r.is(0, ValueType::Int64);  // (an Int64 value compares as the integer its bits are)
     const int64_t va = i64 ? bits_i64(r.val[a]) : total_key_host(r.val[a]);
     const int64_t vb = i64 ? bits_i64(r.val[b]) : total_key_host(r.val[b]);
     if (va != vb) return bottom_ ? va < vb : va > vb;
     return bottom_ ? tie[ra] < tie[rb] : tie[ra] > tie[rb];
   });
+  // topk's layout: the rows, and a counted column, stay the child's; a count is exported as Float64
   r.columns = Columns::ValueTagsTime;
+  if (r.is(0, ValueType::Count)) r.types[0] = ValueType::Float64;
 }
 
 // ---- AggregatePlan -------------------------------------------------------------------------------------
 AggregatePlan::AggregatePlan(b2p_ctx* ctx, const std::string& op, double param, std::shared_ptr<PlanNode> child,
                              Modifier modifier, std::vector<std::string> labels)
     : PlanNode(ctx), param_(param), child_(std::move(child)), modifier_(modifier), labels_(std::move(labels)) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromAggregateExec: NULL context");
-  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromAggregateExec: NULL child");
+  require("GpuPromAggregateExec", {child_.get()});
   // create_aggregate_exprs, planner.rs:2808-2897: the DataFusion function each aggregator becomes
   if (op == "count_values") throw PlanError(ErrorKind::Plan, "GpuPromAggregateExec: count_values is not supported by this node");
   if (op == "topk" || op == "bottomk")
@@ -1511,13 +1526,11 @@ AggregatePlan::AggregatePlan(b2p_ctx* ctx, const std::string& op, double param, 
 
 void AggregatePlan::compute(NodeResult& r) {
   child_->run(r);
-  refuse_i32(r, "GpuPromAggregateExec");
   // the reference would re-attach the tag columns of an id-keyed input (ensure_tag_columns_available); this layer has
-  // only the id, so it can group such a node as a whole and nothing else
-  if (r.labels.id_keyed && modifier_ != Modifier::None)
-    throw PlanError(ErrorKind::Plan, "GpuPromAggregateExec: an id-keyed (__tsid) child can only be aggregated without by / without");
-  if (op_ == kAggGroup && r.F > 1)  // planner.rs:2815-2823
-    throw PlanError(ErrorKind::Plan, "Multi fields calculation is not supported in group()");
+  // only the id, so it can group such a node as a whole and nothing else.  group(): planner.rs:2815-2823
+  check_child(r, {{Shape::Int32, "GpuPromAggregateExec: an Int32 value column is not supported by this node"},
+                  {Shape::IdKeyed, modifier_ == Modifier::None ? "" : "GpuPromAggregateExec: an id-keyed (__tsid) child can only be aggregated without by / without"},
+                  {Shape::MultiField, op_ == kAggGroup ? "Multi fields calculation is not supported in group()" : ""}});
   aggregate_rows(ctx_, op_, param_, group_columns(r.labels, modifier_, labels_), r);  // one aggregate per field
   for (std::string& value : r.value_names)
     value = op_ == kAggGroup      ? "max(" + float_literal(1.0) + ")"
@@ -1529,18 +1542,16 @@ void AggregatePlan::compute(NodeResult& r) {
 CountValuesPlan::CountValuesPlan(b2p_ctx* ctx, std::string label, std::shared_ptr<PlanNode> child, Modifier modifier,
                                  std::vector<std::string> labels)
     : PlanNode(ctx), label_(std::move(label)), child_(std::move(child)), modifier_(modifier), labels_(std::move(labels)) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromCountValuesExec: NULL context");
-  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromCountValuesExec: NULL child");
+  require("GpuPromCountValuesExec", {child_.get()});
 }
 
 void CountValuesPlan::compute(NodeResult& r) {
   child_->run(r);
-  refuse_i32(r, "GpuPromCountValuesExec");
-  if (r.F > 1)  // planner.rs:2874-2879
-    throw PlanError(ErrorKind::Plan, "Unsupported expr type: count_values on multi-value input");
-  // keep_tsid is false for count_values (planner.rs:402): as for AggregatePlan, an id-keyed child groups as a whole only
-  if (r.labels.id_keyed && modifier_ != Modifier::None)
-    throw PlanError(ErrorKind::Plan, "GpuPromCountValuesExec: an id-keyed (__tsid) child can only be counted without by / without");
+  // planner.rs:2874-2879; keep_tsid is false for count_values (planner.rs:402): as for AggregatePlan, an id-keyed
+  // child groups as a whole only
+  check_child(r, {{Shape::Int32, "GpuPromCountValuesExec: an Int32 value column is not supported by this node"},
+                  {Shape::MultiField, "Unsupported expr type: count_values on multi-value input"},
+                  {Shape::IdKeyed, modifier_ == Modifier::None ? "" : "GpuPromCountValuesExec: an id-keyed (__tsid) child can only be counted without by / without"}});
   const std::vector<int> cols = group_columns(r.labels, modifier_, labels_);
   const std::string count_name = "count(" + r.value_names[0] + ")";
   // the projection would have two columns of one name (planner.rs:425-430)
@@ -1553,14 +1564,15 @@ void CountValuesPlan::compute(NodeResult& r) {
   std::vector<double> cval((size_t)R * T);
   std::vector<uint32_t> ccnt((size_t)R * T);
   if (R > 0 && T > 0)
-    check(r.is_i64(0) ? b2p_count_values_i64(ctx_, reinterpret_cast<const int64_t*>(r.val.data()), r.valid.data(),
+    check(r.is(0, ValueType::Int64) ? b2p_count_values_i64(ctx_, reinterpret_cast<const int64_t*>(r.val.data()), r.valid.data(),
                                              groups.id.data(), R, G, (uint64_t)T, reinterpret_cast<int64_t*>(cval.data()),
                                              ccnt.data())
                       : b2p_count_values(ctx_, r.val.data(), r.valid.data(), groups.id.data(), R, G, (uint64_t)T,
                                          cval.data(), ccnt.data()),
           ErrorKind::Execution);
-  r.label_is_i64 = r.is_i64(0);  // the counted values keep the child's type (count_values.result:31-62)
-  r.types.clear();                // the count
+  // the counted values keep the child's type (count_values.result:31-62)
+  r.counted = CountedColumn{label_, r.is(0, ValueType::Int64) ? ValueType::Int64 : ValueType::Float64, {}};
+  r.types = {ValueType::Count};
   // b2p_count_values' rows: group g's members (rank rows) from goff[g]
   std::vector<uint32_t> goff((size_t)G + 1, 0u), place(G);
   for (uint32_t q = 0; q < R; ++q) ++goff[groups.id[q] + 1];
@@ -1581,14 +1593,14 @@ void CountValuesPlan::compute(NodeResult& r) {
   r.labels = groups.labels.gather(lab);
   r.val.assign((size_t)n * T, 0.0);
   r.valid.assign((size_t)n * Tw, 0u);
-  r.label_val.assign((size_t)n * T, 0.0);
+  r.counted->values.assign((size_t)n * T, 0.0);
   r.cell_order.clear();
   for (uint32_t o = 0; o < n; ++o)
     for (size_t k = 0; k < T; ++k) {
       const size_t c = (size_t)src[o] * T + k;
       if (ccnt[c] == 0) continue;
       r.val[(size_t)o * T + k] = (double)ccnt[c];
-      r.label_val[(size_t)o * T + k] = cval[c];
+      r.counted->values[(size_t)o * T + k] = cval[c];
       r.valid[(size_t)o * Tw + (k >> 5)] |= 1u << (k & 31);
     }
   // export order Sort(group labels, ts, value): a group's rows by step, then rank (rank order is value order)
@@ -1599,15 +1611,12 @@ void CountValuesPlan::compute(NodeResult& r) {
   r.rows = n;
   r.columns = Columns::CountTagsTimeLabel;
   r.value_names = {count_name};
-  r.label_name = label_;
-  r.value_is_count = true;
 }
 
 // ---- SubqueryPlan --------------------------------------------------------------------------------------
 SubqueryPlan::SubqueryPlan(b2p_ctx* ctx, std::string function, const b2p_range_params& p, std::shared_ptr<PlanNode> child)
     : PlanNode(ctx), function_(std::move(function)), p_(p), child_(std::move(child)) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromSubqueryExec: NULL context");
-  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: NULL child");
+  require("GpuPromSubqueryExec", {child_.get()});
   p_.fn_id = function_id_from_name(function_);
   if (p_.fn_id < 0) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: unknown range function " + function_);
   if (p_.interval <= 0) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: interval must be positive");
@@ -1619,20 +1628,18 @@ SubqueryPlan::SubqueryPlan(b2p_ctx* ctx, std::string function, const b2p_range_p
 void SubqueryPlan::compute(NodeResult& r) {
   NodeResult C;
   child_->run(C);
-  refuse_i32(C, "GpuPromSubqueryExec");
-  if (C.any_i64()) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: an Int64 value column is not supported by this node");
+  check_child(C, {{Shape::Int32, "GpuPromSubqueryExec: an Int32 value column is not supported by this node"},
+                  {Shape::Int64, "GpuPromSubqueryExec: an Int64 value column is not supported by this node"}});
   const int64_t T_in = C.T;
   const int64_t step = T_in > 1 ? C.eval_ts[1] - C.eval_ts[0] : p_.interval;  // (one inner step: any positive step)
   bool regular = step > 0;
   for (int64_t k = 1; regular && k < T_in; ++k) regular = C.eval_ts[(size_t)k] == C.eval_ts[0] + k * step;
   if (!regular) throw PlanError(ErrorKind::Plan, "GpuPromSubqueryExec: the child's eval timestamps are not a regular grid");
   r = NodeResult();
-  r.T = b2p_num_steps(p_.start, p_.end, p_.interval);
-  r.Tw = (uint32_t)((r.T + 31) / 32);
+  set_grid(r, p_.start, p_.end, p_.interval);
   r.rows = C.rows;
-  r.eval_ts.resize((size_t)r.T);
-  for (int64_t k = 0; k < r.T; ++k) r.eval_ts[(size_t)k] = p_.start + k * p_.interval;
   r.F = C.F;
+  r.types.assign(r.F, ValueType::Float64);
   r.val.assign((size_t)r.F * r.rows * (size_t)r.T, 0.0);
   r.valid.assign((size_t)r.rows * r.Tw, 0u);
   // the function once per field over the same windows (planner.rs:292-332), then the conjunction of the fields' IS NOT
@@ -1664,21 +1671,19 @@ void SubqueryPlan::compute(NodeResult& r) {
 HistogramQuantilePlan::HistogramQuantilePlan(b2p_ctx* ctx, std::string le_column, double phi,
                                              std::shared_ptr<PlanNode> child)
     : PlanNode(ctx), le_column_(std::move(le_column)), phi_(phi), child_(std::move(child)) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromHistogramFoldExec: NULL context");
-  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: NULL child");
+  require("GpuPromHistogramFoldExec", {child_.get()});
 }
 
 void HistogramQuantilePlan::compute(NodeResult& r) {
   child_->run(r);
-  refuse_i32(r, "GpuPromHistogramFoldExec");
-  if (r.labels.id_keyed)
-    throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: an id-keyed (__tsid) child carries no " + le_column_ + " label");
-  if (r.columns == Columns::CountTagsTimeLabel)
-    throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: a count_values child is not supported by this node");
   // the reference folds the first field only (planner.rs:3084-3092, a FIXME); this node does not copy that
-  if (r.F > 1) throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: a multi-field child is not supported by this node");
-  if (r.any_i64()) throw PlanError(ErrorKind::Plan, "GpuPromHistogramFoldExec: an Int64 value column is not supported by this node");
+  check_child(r, {{Shape::Int32, "GpuPromHistogramFoldExec: an Int32 value column is not supported by this node"},
+                  {Shape::IdKeyed, "GpuPromHistogramFoldExec: an id-keyed (__tsid) child carries no " + le_column_ + " label"},
+                  {Shape::Counted, "GpuPromHistogramFoldExec: a count_values child is not supported by this node"},
+                  {Shape::MultiField, "GpuPromHistogramFoldExec: a multi-field child is not supported by this node"},
+                  {Shape::Int64, "GpuPromHistogramFoldExec: an Int64 value column is not supported by this node"}});
   r.cell_order.clear();
+  r.counted.reset();  // (the folded rows are new rows)
   const int le = r.labels.column(le_column_);
   if (le < 0) {  // create_histogram_plan: no le tag -> EmptyRelation, no rows and no columns
     r.rows = 0;
@@ -1706,8 +1711,7 @@ void HistogramQuantilePlan::compute(NodeResult& r) {
 SortPlan::SortPlan(b2p_ctx* ctx, const std::string& function, std::shared_ptr<PlanNode> child,
                    std::vector<std::string> labels)
     : PlanNode(ctx), child_(std::move(child)), labels_(std::move(labels)) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromSortExec: NULL context");
-  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromSortExec: NULL child");
+  require("GpuPromSortExec", {child_.get()});
   if (function != "sort" && function != "sort_desc" && function != "sort_by_label" && function != "sort_by_label_desc")
     throw PlanError(ErrorKind::Plan, "GpuPromSortExec: unknown function " + function);
   by_label_ = function.compare(0, 13, "sort_by_label") == 0;
@@ -1719,9 +1723,11 @@ SortPlan::SortPlan(b2p_ctx* ctx, const std::string& function, std::shared_ptr<Pl
 
 void SortPlan::compute(NodeResult& r) {
   child_->run(r);
-  // the reference carries count_values' counted value as a tag, which this layer does not model
-  if (r.columns == Columns::CountTagsTimeLabel)
-    throw PlanError(ErrorKind::Plan, "GpuPromSortExec: a count_values child is not supported by this node");
+  // a multi-field child with an Int64 field is refused where sort has cells to order
+  const bool int_keys = !by_label_ && r.rows > 0 && r.T > 0 && r.has(ValueType::Int64);
+  check_child(r, {{Shape::Counted, "GpuPromSortExec: a count_values child is not supported by this node"},
+                  {Shape::MultiField, int_keys ? "GpuPromSortExec: a multi-field child with an Int64 value column is not supported by this node" : ""},
+                  {Shape::IdKeyed, by_label_ ? "GpuPromSortExec: an id-keyed (__tsid) child has no label values to sort by" : ""}});
   r.cell_order.clear();
   if (r.columns == Columns::None) return;  // no columns, no rows: the same empty batch
   r.columns = Columns::TimeValueTags;
@@ -1733,9 +1739,7 @@ void SortPlan::compute(NodeResult& r) {
     // by every field in turn (planner.rs:1066-1071): lexicographic over the fields
     std::vector<const double*> vals(r.F);
     for (uint32_t f = 0; f < r.F; ++f) vals[f] = r.field(f);
-    if (r.any_i64() && r.F > 1)
-      throw PlanError(ErrorKind::Plan, "GpuPromSortExec: a multi-field child with an Int64 value column is not supported by this node");
-    check(r.is_i64(0) ? b2p_sort_cells_i64(ctx_, desc_ ? 1 : 0, reinterpret_cast<const int64_t*>(vals[0]), r.valid.data(),
+    check(r.is(0, ValueType::Int64) ? b2p_sort_cells_i64(ctx_, desc_ ? 1 : 0, reinterpret_cast<const int64_t*>(vals[0]), r.valid.data(),
                                            r.rows, T, r.cell_order.data(), &n)
                       : b2p_sort_cells_fields(ctx_, desc_ ? 1 : 0, vals.data(), (int32_t)r.F, r.valid.data(), r.rows, T,
                                               r.cell_order.data(), &n),
@@ -1743,7 +1747,6 @@ void SortPlan::compute(NodeResult& r) {
     r.cell_order.resize((size_t)n);
     return;
   }
-  if (r.labels.id_keyed) throw PlanError(ErrorKind::Plan, "GpuPromSortExec: an id-keyed (__tsid) child has no label values to sort by");
   std::vector<const std::vector<Label>*> cols;
   for (const std::string& l : labels_) {
     const int c = r.labels.column(l);
@@ -1774,8 +1777,7 @@ AbsentPlan::AbsentPlan(b2p_ctx* ctx, Millisecond start, Millisecond end, Millise
                        std::shared_ptr<PlanNode> child)
     : PlanNode(ctx), start_(start), end_(end), interval_(interval), time_index_(std::move(time_index)),
       value_column_(std::move(value_column)), child_(std::move(child)) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuPromAbsentExec: NULL context");
-  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromAbsentExec: NULL child");
+  require("GpuPromAbsentExec", {child_.get()});
   if (interval_ <= 0) throw PlanError(ErrorKind::Plan, "GpuPromAbsentExec: interval must be positive");
   // Absent::try_new: the fake labels collected into a HashMap (the last value of a name wins), sorted by name
   std::map<std::string, std::string> by_name;
@@ -1791,11 +1793,8 @@ void AbsentPlan::compute(NodeResult& r) {
   NodeResult C;
   child_->run(C);
   r = NodeResult();
-  r.T = b2p_num_steps(start_, end_, interval_);
-  r.Tw = (uint32_t)((r.T + 31) / 32);
+  set_grid(r, start_, end_, interval_);
   r.rows = 1;
-  r.eval_ts.resize((size_t)r.T);
-  for (int64_t k = 0; k < r.T; ++k) r.eval_ts[(size_t)k] = start_ + k * interval_;
   // the reference's cursor walks this grid and skips a step only when a child timestamp equals it
   if (C.rows > 0 && C.eval_ts != r.eval_ts)
     throw PlanError(ErrorKind::Plan, "GpuPromAbsentExec: the child's eval timestamps are not the grid (start, end, interval)");
@@ -1817,7 +1816,7 @@ EmptyMetricPlan::EmptyMetricPlan(b2p_ctx* ctx, Millisecond start, Millisecond en
                                  std::string time_index, std::string value_column, int kind, double literal)
     : PlanNode(ctx), start_(start), end_(end), interval_(interval), time_index_(std::move(time_index)),
       value_column_(std::move(value_column)), kind_(kind), literal_(literal) {
-  if (!ctx_) throw PlanError(ErrorKind::Internal, "GpuEmptyMetricExec: NULL context");
+  require("GpuEmptyMetricExec", {});
   if (interval_ <= 0) throw PlanError(ErrorKind::Plan, "GpuEmptyMetricExec: interval must be positive");
   if (kind_ < B2P_EMPTY_NONE || kind_ > B2P_EMPTY_LITERAL)
     throw PlanError(ErrorKind::Plan, "GpuEmptyMetricExec: unknown kind " + std::to_string(kind_));
@@ -1825,12 +1824,10 @@ EmptyMetricPlan::EmptyMetricPlan(b2p_ctx* ctx, Millisecond start, Millisecond en
 
 void EmptyMetricPlan::compute(NodeResult& r) {
   r = NodeResult();
-  r.T = b2p_num_steps(start_, end_, interval_);
-  r.Tw = (uint32_t)((r.T + 31) / 32);
+  set_grid(r, start_, end_, interval_);
   r.rows = r.T > 0 ? 1 : 0;
   r.F = kind_ == B2P_EMPTY_NONE ? 0 : 1;
-  r.eval_ts.resize((size_t)r.T);
-  for (int64_t k = 0; k < r.T; ++k) r.eval_ts[(size_t)k] = start_ + k * interval_;
+  r.types.assign(r.F, ValueType::Float64);
   r.time_index = time_index_;
   r.valid.assign((size_t)r.rows * r.Tw, ~0u);
   r.val.assign((size_t)r.F * r.grid(), kind_ == B2P_EMPTY_LITERAL ? literal_ : 0.0);
@@ -1860,14 +1857,14 @@ LabelPlan::LabelPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child, std::string 
     throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: the regular expression " + regex + " is not supported by this node: " +
                                          regex_->message());
   empty_regex_ = regex.empty();
-  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: NULL child");
+  require("GpuPromLabelExec", {child_.get()}, false);
 }
 
 LabelPlan::LabelPlan(b2p_ctx* ctx, std::shared_ptr<PlanNode> child, std::string dst, std::string separator,
                      std::vector<std::string> srcs)
     : PlanNode(ctx), child_(std::move(child)), join_(true), dst_(std::move(dst)), replacement_(std::move(separator)),
       srcs_(std::move(srcs)) {
-  if (!child_) throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: NULL child");
+  require("GpuPromLabelExec", {child_.get()}, false);
   if (srcs_.empty()) throw PlanError(ErrorKind::Plan, "Invalid function argument for label_join");  // planner.rs:2687-2692
 }
 
@@ -1875,11 +1872,9 @@ LabelPlan::~LabelPlan() = default;
 
 void LabelPlan::compute(NodeResult& r) {
   child_->run(r);  // the child's result is this node's: grid, validity and the rest stay where they are
+  check_child(r, {{Shape::IdKeyed, "GpuPromLabelExec: an id-keyed (__tsid) child has no label values to rewrite"},
+                  {Shape::Counted, "GpuPromLabelExec: a count_values child is not supported by this node"}});
   if (r.columns == Columns::None) return;  // no columns and no rows: nothing to label
-  if (r.labels.id_keyed)
-    throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: an id-keyed (__tsid) child has no label values to rewrite");
-  if (r.columns == Columns::CountTagsTimeLabel)
-    throw PlanError(ErrorKind::Plan, "GpuPromLabelExec: a count_values child is not supported by this node");
   Labels& L = r.labels;
   auto is_column = [&](const std::string& name) {
     return name == r.time_index || std::find(r.value_names.begin(), r.value_names.end(), name) != r.value_names.end();

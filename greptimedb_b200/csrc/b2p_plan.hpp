@@ -16,6 +16,7 @@
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <initializer_list>
 #include <memory>
 #include <optional>
 #include <stdexcept>
@@ -108,15 +109,24 @@ enum class Columns {
   TagsTimeValue,  // {tags.., time index, value}: the by-label aggregate, and arithmetic between two vectors
   TimeSorted,     // {time index, then the tags and the value column in name order}: `or`
   ValueTagsTime,  // {value, tags.., time index}: topk / bottomk
-  CountTagsTimeLabel,  // {count Int64 (Float64 under an element-wise stage), tags.., time index, label}: count_values
+  CountTagsTimeLabel,  // {count, tags.., time index, counted value}: count_values
   None,                // no column at all: histogram_quantile over a child without the le tag (an EmptyRelation)
   TimeValueLastTag,    // {time index, value, the last tag, the other tags..}: label_replace / label_join, whose new tag
                        // is the last one for the nodes above and comes first among the tags in its own projection
 };
 
-// The Arrow type of a value column.  An Int64 cell holds the bits of its int64_t in the 8-byte slot of the grid; an Int32
-// cell (a calendar function's date_part) holds its exact value as a double, so Int32 changes only the export.
-enum class ValueType { Float64, Int64, Int32 };
+// The type of a value column.  An Int64 cell holds the bits of its int64_t in the 8-byte slot of the grid.  An Int32 cell
+// (a calendar function's date_part) and a Count cell (count_values' count, exported as Int64) hold their exact value as a
+// double, so those two change only the export: every node reads them as Float64.
+enum class ValueType { Float64, Int64, Int32, Count };
+
+// count_values' counted value, a column of each of its rows: its name, its type (Float64, or Int64 cells holding int64_t
+// bits) and the cells [rows x T].  Nodes that keep the rows keep it; nodes that build new rows drop it.
+struct CountedColumn {
+  std::string name;
+  ValueType type;
+  std::vector<double> values;
+};
 
 // What a node computed, before it becomes Arrow: F dense [rows x T] grids (one per field) under one validity, the eval
 // timestamps and one label tuple per row.  Exported, row r emits one Arrow row per valid step k (rows in order, steps
@@ -128,31 +138,25 @@ struct NodeResult {
   int64_t T = 0;
   uint32_t Tw = 0;
   uint32_t rows = 0;
-  uint32_t F = 1;                // fields
+  uint32_t F = 1;                // fields; whatever sets F sets types
   std::vector<int64_t> eval_ts;  // [T]
   std::vector<double> val;       // [F x rows x T], field f at f * rows * T; empty when rows == 0 or T == 0
   std::vector<uint32_t> valid;   // [rows x Tw]
   std::string time_index;
   std::vector<std::string> value_names;  // [F]
-  // [F] each field's type, as the reference types the node's value column (DESIGN §1 a25); empty: every field Float64
-  std::vector<ValueType> types;
+  std::vector<ValueType> types{ValueType::Float64};  // [F] as the reference types each value column (DESIGN §1 a25)
   Labels labels;
   Columns columns = Columns::TimeValueTags;
   // when not empty, the export emits these cells (row * T + step), in this order, instead of rows then steps; a cell
   // whose bit a later stage cleared is skipped
   std::vector<uint64_t> cell_order;
-  // count_values (Columns::CountTagsTimeLabel): each cell's counted value [rows x T], exported as the column label_name;
-  // value_is_count exports the value column as Int64 (an element-wise stage on top clears it)
-  std::vector<double> label_val;
-  std::string label_name;
-  bool value_is_count = false;
-  bool label_is_i64 = false;  // count_values over an Int64 child: label_val holds int64_t bits, exported as Int64
-  // an EmptyMetric row: time() (scalar-typed in PromQL) or a literal (a scalar, or vector(s)); read by the binary node
+  std::optional<CountedColumn> counted;  // the rows of a count_values result, and of the nodes that keep them
+  // an EmptyMetric row: time() (scalar-typed in PromQL) or a literal (a scalar, or vector(s)); read by the binary node.
+  // The aggregate node, topk and count_values pass their child's on, so sum(vector(1)) > x is refused as vector(1) > x
+  // is: this layer does not model the matching of either
   bool scalar_like = false, literal_row = false;
-  bool is_i64(uint32_t f) const { return f < types.size() && types[f] == ValueType::Int64; }
-  bool any_i64() const { return std::find(types.begin(), types.end(), ValueType::Int64) != types.end(); }
-  bool is_i32(uint32_t f) const { return f < types.size() && types[f] == ValueType::Int32; }
-  bool any_i32() const { return std::find(types.begin(), types.end(), ValueType::Int32) != types.end(); }
+  bool is(uint32_t f, ValueType t) const { return f < types.size() && types[f] == t; }
+  bool has(ValueType t) const { return std::find(types.begin(), types.end(), t) != types.end(); }
   bool valid_at(uint32_t r, int64_t k) const { return (valid[(size_t)r * Tw + (size_t)(k >> 5)] >> (k & 31)) & 1u; }
   size_t grid() const { return (size_t)rows * (size_t)T; }
   double* field(uint32_t f) { return val.data() + f * grid(); }
@@ -185,6 +189,9 @@ class PlanNode {
 
  protected:
   virtual void compute(NodeResult& r) = 0;
+  // the argument checks every node makes: a NULL context (unless the node does no device work) is an Internal error,
+  // then a NULL child a Plan error, "<node>: NULL context" / "<node>: NULL child"
+  void require(const char* node, std::initializer_list<const PlanNode*> children, bool device = true) const;
   b2p_ctx* ctx_;
 
  private:
@@ -342,7 +349,7 @@ class AggregatePlan : public PlanNode {
 // value), planner.rs:402-445.  Group labels as for AggregatePlan (group_rows / group_columns); the per-step distinct
 // values and counts are b2p_count_values.  Rows: per group in Labels::less order, one for each rank of a distinct value
 // that occurs at some step, labelled with the group labels and holding the count (named count(<child value name>)), so
-// the nodes above count, sum or compare them; the counted values ride along in label_val for the export.
+// the nodes above count, sum or compare them; the counted values ride along in `counted` for the export.
 class CountValuesPlan : public PlanNode {
  public:
   CountValuesPlan(b2p_ctx* ctx, std::string label, std::shared_ptr<PlanNode> child, Modifier modifier,

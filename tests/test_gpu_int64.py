@@ -279,38 +279,6 @@ def test_absent_and_and_keep_working(ctx):
     assert both.schema.field("val").type == pa.int64() and set(both.column("host").to_pylist()) == {"host1"}
 
 
-# ---- refusals -------------------------------------------------------------------------------------------------------
-def test_refusals(ctx):
-    from greptimedb_b200 import B2PError
-    from greptimedb_b200.plan import (BinaryPlan, HistogramQuantilePlan, SetOpPlan, SortPlan, SubqueryPlan)
-    rows = GOLDEN["tables"]["sort"]["rows"]
-    with pytest.raises(B2PError, match="field column val is not Float64"):
-        leaf(ctx, rows, function="prom_rate")
-    cases = [
-        (lambda: BinaryPlan(ctx, "+", leaf(ctx, rows), leaf(ctx, rows)),
-         "a binary operator between two Int64 value columns is not supported"),
-        (lambda: BinaryPlan(ctx, ">", leaf(ctx, rows), leaf(ctx, rows, val_type=pa.float64())),
-         "a filtering comparison over an Int64 value column is not supported"),
-        (lambda: leaf(ctx, rows).scalar_op(">", 1.0), "a filtering comparison over an Int64 value column is not supported"),
-        (lambda: SetOpPlan(ctx, "or", leaf(ctx, rows), leaf(ctx, rows)), "an Int64 value column is not supported"),
-        (lambda: SubqueryPlan(ctx, "prom_max_over_time", leaf(ctx, rows), 0, 15_000, 5_000, 10_000),
-         "GpuPromSubqueryExec: an Int64 value column is not supported"),
-        (lambda: HistogramQuantilePlan(ctx, 0.5, leaf(ctx, rows), le="idc"),
-         "GpuPromHistogramFoldExec: an Int64 value column is not supported"),
-    ]
-    for make, msg in cases:
-        with pytest.raises(B2PError, match=msg):
-            make().execute()
-    # a mixed two-field node under sort
-    from greptimedb_b200.plan import PromRangeExec
-    b = pa.record_batch([pa.array([0], pa.timestamp("ms")), pa.array(["a"]), pa.array([1.0]), pa.array([1], pa.int64())],
-                        names=["ts", "host", "f", "i"])
-    ex = PromRangeExec(ctx, "", 0, 5000, 5000, 0, "ts", ["f", "i"], ["host"], lookback_delta=io.LOOKBACK)
-    ex.push(b)
-    with pytest.raises(B2PError, match="a multi-field child with an Int64 value column"):
-        SortPlan(ctx, "sort", ex).execute()
-
-
 # ---- the Int64 instant selector, the device forms, topk's general path, NULL slots ----------------------------------
 @pytest.mark.parametrize("F", [1, 2])
 def test_instant_select_fields_i64(ctx, F):

@@ -512,30 +512,6 @@ def test_absent_over_a_multi_field_child(ctx):
 
 
 # ---- refusals -------------------------------------------------------------------------------------------------------------
-def test_refusals_at_execute(ctx):
-    from greptimedb_b200 import B2PError
-    from greptimedb_b200 import plan as P
-    tab = Table(6, 80, 2, seed=80)
-    one = Table(6, 80, 1, seed=80)
-    cases = [
-        (lambda: P.TopkPlan(ctx, "topk", 1, leaf(ctx, tab)), mp.REFUSALS["topk"]),
-        (lambda: P.TopkPlan(ctx, "bottomk", 1, leaf(ctx, tab)), mp.REFUSALS["topk"]),
-        (lambda: P.CountValuesPlan(ctx, "v", leaf(ctx, tab)), mp.REFUSALS["count_values"]),
-        (lambda: P.AggregatePlan(ctx, "group", leaf(ctx, tab)), mp.REFUSALS["group"]),
-        (lambda: P.ScalarPlan(ctx, leaf(ctx, tab)), mp.REFUSALS["scalar"]),
-        (lambda: P.SetOpPlan(ctx, "and", leaf(ctx, tab), leaf(ctx, one)), mp.REFUSALS["and"]),
-        (lambda: P.SetOpPlan(ctx, "unless", leaf(ctx, tab), leaf(ctx, tab)), mp.REFUSALS["unless"]),
-        (lambda: P.SetOpPlan(ctx, "or", leaf(ctx, tab), leaf(ctx, tab)), mp.REFUSALS["or"]),
-        (lambda: P.SetOpPlan(ctx, "or", leaf(ctx, one), leaf(ctx, tab)), "Attempt to combine two tables with different "
-                                                                           "column sets"),
-        (lambda: P.HistogramQuantilePlan(ctx, 0.5, leaf(ctx, tab)), "multi-field child"),
-    ]
-    for make, msg in cases:
-        with pytest.raises(B2PError, match=msg.replace("(", r"\(").replace(")", r"\)")):
-            make().execute()
-    P.SetOpPlan(ctx, "and", leaf(ctx, one), leaf(ctx, tab)).execute()  # only the lhs's fields matter to `and`
-
-
 def test_refusals_at_create_and_push(ctx):
     from greptimedb_b200 import B2PError, make_params
     from greptimedb_b200.plan import PromRangeExec, _cstr_array

@@ -367,58 +367,6 @@ def test_calendar_stage_and_unary_minus_over_every_node(ctx, kind):
         assert (bits(minus.column(m).to_numpy()) == (bits(x) ^ np.int64(-2**63))).all()
 
 
-def test_int32_refusals_and_accepted_paths(ctx):
-    from greptimedb_b200 import B2PError
-    from greptimedb_b200.plan import (AbsentPlan, AggregatePlan, BinaryPlan, CountValuesPlan, EmptyMetricPlan,
-                                      HistogramQuantilePlan, ScalarPlan, SetOpPlan, SortPlan, SubqueryPlan, TopkPlan)
-
-    def cal():
-        return EmptyMetricPlan(ctx, 0, 120_000, 60_000, "none").function("hour")
-
-    def f64():
-        return EmptyMetricPlan(ctx, 0, 120_000, 60_000, "time")
-
-    refused = {
-        "GpuPromAggregateExec: an Int32": lambda: AggregatePlan(ctx, "sum", cal()),
-        "GpuPromCountValuesExec: an Int32": lambda: CountValuesPlan(ctx, "v", cal()),
-        "GpuPromScalarExec: an Int32": lambda: ScalarPlan(ctx, cal()),
-        "GpuPromSubqueryExec: an Int32": lambda: SubqueryPlan(
-            ctx, "prom_max_over_time", EmptyMetricPlan(ctx, -60_000, 120_000, 60_000, "none").function("hour"),
-            0, 120_000, 60_000, 120_000),
-        "GpuPromHistogramFoldExec: an Int32": lambda: HistogramQuantilePlan(ctx, 0.5, cal()),
-        "an Int32 value column against another type": lambda: SetOpPlan(ctx, "or", cal(), f64()),
-        "between two integer value columns": lambda: BinaryPlan(ctx, "+", cal(), cal()),
-        "unary minus over an integer value column": lambda: cal().function("negative"),
-    }
-    for what, make in refused.items():
-        with pytest.raises(B2PError) as ei:
-            make().execute()
-        assert ei.value.code == -1 and what in str(ei.value), (what, str(ei.value))
-    hours = [0, 0, 0]
-    typ = lambda out, name: out.schema.field(name).type
-    val = 'date_part(Utf8("hour"),time)'
-    # stages coerce to Float64; a filter keeps Int32
-    assert typ(cal().scalar_op("+", 1.0).execute(), val + " + Float64(1)") == pa.float64()
-    assert typ(cal().function("abs").execute(), "abs(" + val + ")") == pa.float64()
-    assert typ(cal().scalar_op(">=", 0.0).execute(), val) == pa.int32()
-    # against a Float64 side: arithmetic and `bool` give Float64, a vector-vector filter keeps the Int32 lhs
-    assert typ(BinaryPlan(ctx, "*", cal(), f64()).execute(), val + " * time / Float64(1000)") == pa.float64()
-    assert typ(BinaryPlan(ctx, "<=", cal(), f64(), return_bool=True).execute(), val + " <= time / Float64(1000)") == pa.float64()
-    out = BinaryPlan(ctx, "<=", cal(), f64()).execute()
-    assert typ(out, val) == pa.int32() and out.column(val).to_pylist() == hours
-    # and / unless keep the lhs; `or` of two Int32 sides stays Int32
-    assert typ(SetOpPlan(ctx, "and", cal(), f64()).execute(), val) == pa.int32()
-    assert typ(SetOpPlan(ctx, "unless", cal(), f64()).execute(), val) == pa.int32()
-    assert typ(SetOpPlan(ctx, "or", cal(), cal()).execute(), val) == pa.int32()
-    # sort, topk / bottomk and absent
-    out = SortPlan(ctx, "sort_desc", cal()).execute()
-    assert typ(out, val) == pa.int32() and out.column(val).to_pylist() == hours
-    for op in ("topk", "bottomk"):
-        out = TopkPlan(ctx, op, 1, cal()).execute()
-        assert typ(out, val) == pa.int32() and out.column(val).to_pylist() == hours, op
-    assert AbsentPlan(ctx, cal(), 0, 120_000, 60_000, "time", "value").execute().num_rows == 0
-
-
 def test_empty_metric_unit_vectors_and_create_errors(ctx):
     from greptimedb_b200 import B2PError
     from greptimedb_b200.plan import EmptyMetricPlan
