@@ -44,6 +44,7 @@ EXPORTED_SYMBOLS = [
     "b2p_step_fn_dev", "b2p_step_fn", "b2p_instant_timestamp_dev", "b2p_instant_timestamp",
     "b2p_plan_empty_metric_create", "b2p_plan_set_timestamp",
     "b2p_plan_label_replace_create", "b2p_plan_label_join_create", "b2p_label_regex_check", "b2p_label_regex_replace",
+    "b2p_plan_set_label_columns",
 ]
 
 
@@ -126,6 +127,7 @@ def load() -> C.CDLL:
                                        C.POINTER(C.c_char_p), i32]),
         "b2p_plan_set_instant": (C.c_int, [vp, i64]),
         "b2p_plan_set_histogram_quantile": (C.c_int, [vp, C.c_char_p, dbl]),
+        "b2p_plan_set_label_columns": (C.c_int, [vp, C.POINTER(C.c_char_p), i32]),
         "b2p_plan_push_batch": (C.c_int, [vp, vp, vp]),
         "b2p_plan_execute": (C.c_int, [vp, vp, vp]),
         "b2p_plan_num_series": (i64, [vp]),

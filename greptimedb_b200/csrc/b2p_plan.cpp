@@ -272,7 +272,8 @@ Labels Labels::gather(const std::vector<uint32_t>& rows) const {
   Labels out;
   out.names = names;
   out.id_keyed = id_keyed;
-  if (id_keyed)
+  out.tsid = tsid;
+  if (id_keyed || tsid)
     for (uint32_t r : rows) out.ids.push_back(ids[r]);
   out.values.resize(values.size());
   for (size_t t = 0; t < values.size(); ++t) {
@@ -295,8 +296,9 @@ namespace {
 
 // The rows of `in` grouped by their tuple over `cols`, for output in label order (the by-label aggregate, HistogramFold)
 struct Groups {
-  std::vector<uint32_t> id;    // [row] its group, numbered in order of first appearance
-  std::vector<uint32_t> rank;  // [group] its place in label order
+  std::vector<uint32_t> id;     // [row] its group, numbered in order of first appearance
+  std::vector<uint32_t> first;  // [group] its first row
+  std::vector<uint32_t> rank;   // [group] its place in label order
   Labels labels;               // [place] the group's tuple over `cols` (ids as decimal strings)
 };
 
@@ -304,7 +306,7 @@ Groups group_rows(const Labels& in, const std::vector<int>& cols, uint32_t rows)
   Groups g;
   g.id.resize(rows);
   KeyIds ids;
-  std::vector<uint32_t> first;  // [group] its first row
+  std::vector<uint32_t>& first = g.first;
   std::string key;
   for (uint32_t r = 0; r < rows; ++r) {
     in.key(r, cols, key);
@@ -333,6 +335,15 @@ Groups group_rows(const Labels& in, const std::vector<int>& cols, uint32_t rows)
   return g;
 }
 
+// keep_tsid (planner.rs:347-416): an aggregate other than count_values keeps first_value(__tsid) as __tsid when its
+// child carries __tsid and it groups on the child's full label set (a metric-engine leaf's declared label columns)
+bool keeps_tsid(const Labels& in, std::vector<int> cols) {
+  if (!in.tsid) return false;
+  std::sort(cols.begin(), cols.end());
+  cols.erase(std::unique(cols.begin(), cols.end()), cols.end());
+  return cols.size() == in.names.size() && (cols.empty() || cols.front() >= 0);
+}
+
 // Aggregators beyond enum b2p_agg that the aggregate node offers
 constexpr int kAggGroup = B2P_AGG_STDVAR + 1, kAggQuantile = B2P_AGG_STDVAR + 2;
 
@@ -341,9 +352,15 @@ constexpr int kAggGroup = B2P_AGG_STDVAR + 1, kAggQuantile = B2P_AGG_STDVAR + 2;
 // a group having a cell at step k iff one of its rows has.  op: enum b2p_agg, kAggGroup (1.0 wherever count is
 // non-zero) or kAggQuantile (param = φ).  Each field is folded by its own call over the same group ids; the counts
 // depend on the shared validity alone, so field 0's decide the cells.  Sets the rows, labels, grids, types and column
-// layout, drops a counted column; keeps T, the fields and the time index.
+// layout, drops a counted column; keeps T, the fields and the time index.  A group keeps its first member's __tsid
+// where keeps_tsid says so.
 void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& cols, NodeResult& r) {
   Groups groups = group_rows(r.labels, cols, r.rows);
+  if (keeps_tsid(r.labels, cols)) {
+    groups.labels.tsid = true;
+    groups.labels.ids.resize(groups.first.size());
+    for (size_t g = 0; g < groups.first.size(); ++g) groups.labels.ids[groups.rank[g]] = r.labels.ids[groups.first[g]];
+  }
   const uint32_t G = (uint32_t)groups.rank.size(), Tw = r.Tw, F = r.F;
   const size_t T = (size_t)r.T;
   std::vector<double> gval((size_t)F * G * T);
@@ -430,6 +447,12 @@ HistogramIndex histogram_index(const Labels& in, int le, uint32_t rows) {
 
 }  // namespace
 
+namespace {
+bool contains(const std::vector<std::string>& v, const std::string& x) { return std::find(v.begin(), v.end(), x) != v.end(); }
+// the metric engine's series id column (DATA_SCHEMA_TSID_COLUMN_NAME)
+const char* const kTsid = "__tsid";
+}  // namespace
+
 // ---- PromRangePlan -------------------------------------------------------------------------------------
 PromRangePlan::PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args) : PlanNode(ctx), args_(std::move(args)) {
   require("GpuPromRangeExec", {});
@@ -440,10 +463,10 @@ PromRangePlan::PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args) : PlanNode(ct
   if (!args_.aggregate.empty()) {
     agg_id_ = aggregate_id_from_name(args_.aggregate);
     if (agg_id_ < 0) throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: unsupported aggregator " + args_.aggregate);
-    for (const auto& b : args_.by_columns)
-      if (std::find(args_.tag_columns.begin(), args_.tag_columns.end(), b) == args_.tag_columns.end())
-        throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: by-column " + b + " is not a tag column");
   }
+  // a leaf keyed on __tsid alone may be a metric-engine leaf whose by-columns name its label columns, which come
+  // later: it checks them at set_label_columns() and push()
+  if (args_.tag_columns != std::vector<std::string>{kTsid}) check_key_columns();
   if (args_.interval <= 0) throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: interval must be positive");
   const std::vector<std::string>& fields = args_.field_columns;
   if (fields.empty() || fields.size() > B2P_MAX_FIELDS)
@@ -465,8 +488,39 @@ PromRangePlan::PromRangePlan(b2p_ctx* ctx, PromRangePlanArgs args) : PlanNode(ct
   series_.values.resize(args_.tag_columns.size());
 }
 
+// the label columns of a metric-engine leaf, the tag columns of any other
+void PromRangePlan::check_key_columns() const {
+  const std::vector<std::string>& keys = args_.label_columns.empty() ? args_.tag_columns : args_.label_columns;
+  for (const auto& b : args_.by_columns)
+    if (agg_id_ >= 0 && !contains(keys, b))
+      throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: by-column " + b + " is not a tag column");
+  if (args_.histogram && !contains(keys, args_.le_column))
+    throw PlanError(ErrorKind::Plan, "HistogramFold: le column " + args_.le_column + " is not a tag column");
+}
+
+void PromRangePlan::set_label_columns(std::vector<std::string> names) {
+  if (args_.tag_columns != std::vector<std::string>{kTsid})
+    throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: label columns need the one tag column to be the UInt64 id __tsid");
+  if (have_last_) throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: label columns must be set before the first batch");
+  if (names.empty()) throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: at least one label column is required");
+  for (size_t i = 0; i < names.size(); ++i) {
+    const std::string& n = names[i];
+    if (n.empty() || n == args_.time_index || n == args_.tag_columns[0] || contains(args_.field_columns, n))
+      throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: label column \"" + n +
+                                           "\" is named like the time index, a field column or the id column");
+    if (std::find(names.begin(), names.begin() + (long)i, n) != names.begin() + (long)i)
+      throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: label column " + n + " is given twice");
+  }
+  args_.label_columns = std::move(names);
+  series_ = Labels();
+  series_.names = args_.label_columns;
+  series_.values.resize(series_.names.size());
+  series_.tsid = true;
+  check_key_columns();
+}
+
 void PromRangePlan::set_histogram(const std::string& le_column, double quantile) {
-  if (std::find(args_.tag_columns.begin(), args_.tag_columns.end(), le_column) == args_.tag_columns.end())
+  if (!contains(args_.label_columns.empty() ? args_.tag_columns : args_.label_columns, le_column))
     throw PlanError(ErrorKind::Plan, "HistogramFold: le column " + le_column + " is not a tag column");
   if (!args_.aggregate.empty())
     throw PlanError(ErrorKind::Plan, "HistogramFold over an aggregate is not supported by this node");
@@ -481,6 +535,7 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
   const RecordBatch& b = *batch;
   const int64_t n = b.num_rows();
   if (n == 0) return;  // an empty batch is skipped (never parks the stream, SURVEY appendix C-11)
+  check_key_columns();
   const int ti = b.find(args_.time_index);
   if (ti < 0) throw PlanError(ErrorKind::Plan, "No field named " + args_.time_index);  // field_not_found
   const size_t F = args_.field_columns.size();
@@ -516,33 +571,52 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
     int64_t base;
     const uint64_t* ids;
   };
+  const bool metric_engine = !args_.label_columns.empty();
+  auto column = [&](int ci) {  // a Utf8 column (offsets, data) or the UInt64 id column
+    const ArrowArray& ca = b.column(ci);
+    TagCol tc{};
+    tc.base = ca.offset + b.offset();
+    tc.valid = ca.null_count != 0 ? static_cast<const uint8_t*>(ca.buffers[0]) : nullptr;
+    if (std::strcmp(b.field(ci).format, "u") == 0) {
+      tc.off = static_cast<const int32_t*>(ca.buffers[1]);
+      tc.data = static_cast<const char*>(ca.buffers[2]);
+    } else {
+      tc.ids = static_cast<const uint64_t*>(ca.buffers[1]);
+    }
+    return tc;
+  };
   std::vector<TagCol> tcols;
   for (size_t t = 0; t < args_.tag_columns.size(); ++t) {
     const int ci = b.find(args_.tag_columns[t]);
     if (ci < 0) throw PlanError(ErrorKind::Plan, "No field named " + args_.tag_columns[t]);
-    const ArrowArray& ca = b.column(ci);
     const char* fmt = b.field(ci).format;
-    TagCol tc{};
-    tc.base = ca.offset + b.offset();
-    tc.valid = ca.null_count != 0 ? static_cast<const uint8_t*>(ca.buffers[0]) : nullptr;
-    if (std::strcmp(fmt, "u") == 0) {
-      tc.off = static_cast<const int32_t*>(ca.buffers[1]);
-      tc.data = static_cast<const char*>(ca.buffers[2]);
-    } else if (std::strcmp(fmt, "L") == 0 && args_.tag_columns.size() == 1) {
-      tc.ids = static_cast<const uint64_t*>(ca.buffers[1]);
-      series_.id_keyed = true;
-      series_.values.clear();
-    } else {
+    if (std::strcmp(fmt, "L") == 0 && args_.tag_columns.size() == 1) {
+      if (!metric_engine) {
+        series_.id_keyed = true;
+        series_.values.clear();
+      }
+    } else if (metric_engine) {
+      throw PlanError(ErrorKind::Plan, "GpuPromRangeExec: label columns need the tag column " + args_.tag_columns[t] +
+                                           " to be a UInt64 id");
+    } else if (std::strcmp(fmt, "u") != 0) {
       throw PlanError(ErrorKind::Execution, "tag column " + args_.tag_columns[t] + " must be Utf8 (or one UInt64 id)");
     }
-    tcols.push_back(tc);
+    tcols.push_back(column(ci));
   }
-  auto tag_at = [&](size_t t, int64_t row) -> Label {
-    const TagCol& tc = tcols[t];
+  // a metric-engine leaf's label columns: read at the first row of each series only
+  std::vector<TagCol> lcols;
+  for (const std::string& l : args_.label_columns) {
+    const int ci = b.find(l);
+    if (ci < 0) throw PlanError(ErrorKind::Plan, "No field named " + l);
+    if (std::strcmp(b.field(ci).format, "u") != 0) throw PlanError(ErrorKind::Execution, "label column " + l + " must be Utf8");
+    lcols.push_back(column(ci));
+  }
+  auto utf8_at = [&](const TagCol& tc, int64_t row) -> Label {
     const int64_t r = tc.base + row;
     if (!bit_set(tc.valid, r)) return std::nullopt;
     return std::string(tc.data + tc.off[r], (size_t)(tc.off[r + 1] - tc.off[r]));
   };
+  auto tag_at = [&](size_t t, int64_t row) -> Label { return utf8_at(tcols[t], row); };
 
   // Columns are taken over in bulk (the Arrow values buffers are already the device layout): one memcpy per column
   // and batch, no per-row growth.  SeriesDivide only has to find the rows where a new series starts
@@ -583,18 +657,17 @@ void PromRangePlan::push(std::unique_ptr<RecordBatch> batch) {
     offsets_.push_back((uint64_t)(row_base + (size_t)row));
     ++num_series_;
   };
-  if (series_.id_keyed) {
+  if (series_.id_keyed || series_.tsid) {
     const uint64_t* ids = tcols[0].ids + tcols[0].base;
+    auto open_id_series = [&](int64_t row) {
+      series_.ids.push_back(ids[row]);
+      for (size_t l = 0; l < lcols.size(); ++l) series_.values[l].push_back(utf8_at(lcols[l], row));
+      start_series(row);
+    };
     int64_t row = 0;
-    if (!have_last_ || ids[0] != last_id_) {
-      series_.ids.push_back(ids[0]);
-      start_series(0);
-    }
+    if (!have_last_ || ids[0] != last_id_) open_id_series(0);
     for (row = 1; row < n; ++row)
-      if (ids[row] != ids[row - 1]) {  // (a tight compare loop the compiler vectorises)
-        series_.ids.push_back(ids[row]);
-        start_series(row);
-      }
+      if (ids[row] != ids[row - 1]) open_id_series(row);  // (a tight compare loop the compiler vectorises)
     last_id_ = ids[n - 1];
   } else if (!tcols.empty()) {
     // adjacent-row compare on the raw Utf8 buffers; label strings are only materialised for the first row of a series
@@ -645,6 +718,7 @@ void PromRangePlan::compute(NodeResult& r) {
   set_grid(r, p.start, p.end, p.interval);  // also when there are no series: scalar() of such a node has a NaN row at every step
   const int64_t T = r.T;
   const uint32_t Tw = r.Tw;
+  check_key_columns();
   const uint32_t S = (uint32_t)num_series_;
   offsets_.resize((size_t)S);          // (a previous execute() appended the end marker)
   offsets_.push_back((uint64_t)ts_.size());
@@ -712,6 +786,9 @@ void PromRangePlan::compute(NodeResult& r) {
   } else {
     // rows of Filter(prom_fn IS NOT NULL): {time_index (eval ts), prom_fn(...), tags...}, series-major order
     r.labels = series_;
+    // a range function's and timestamp()'s projection lists time, value and tags: __tsid stays only on the instant
+    // selector, which passes every column through (planner.rs:1055-1058, 2714)
+    if (fn_id_ >= 0 || timestamp_) r.labels.drop_tsid();
     r.val = std::move(dense);
     r.valid = std::move(valid);
     r.rows = S;
@@ -832,6 +909,8 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     case Columns::None:  // (no rows either)
       break;
   }
+  // a kept __tsid, after every other column (the reference's own position varies by node; its root projection drops it)
+  OwnedColumn* c_tsid = L.tsid && r.columns != Columns::None ? add_col("__tsid", "L") : nullptr;
   int64_t n_out = 0;
   const bool ordered = !r.cell_order.empty();
   const uint64_t n_cells = ordered ? r.cell_order.size() : (uint64_t)r.rows * (uint64_t)r.T;
@@ -844,6 +923,7 @@ void export_result(const NodeResult& r, ArrowArray* out, ArrowSchema* out_schema
     const size_t at = (size_t)row * (size_t)r.T + (size_t)k;
     for (uint32_t f = 0; f < r.F; ++f) put(c_vals[f], r.types[f], r.field(f)[at]);
     if (c_label) put(c_label, r.counted->type, r.counted->values[at]);
+    if (c_tsid) c_tsid->i64.push_back((int64_t)L.ids[row]);
     for (size_t t = 0; t < c_tags.size(); ++t) {
       if (L.id_keyed) {
         c_tags[t]->i64.push_back((int64_t)L.ids[row]);
@@ -1039,6 +1119,7 @@ void PlanNode::run(NodeResult& r) {
         check(b2p_step_fn(ctx_, s.part, r.eval_ts.data(), r.valid.data(), r.rows, (uint64_t)r.T, r.field(0)));
       r.types = {ValueType::Int32};
       r.value_names = {date_part_name(s, r.time_index)};
+      r.labels.drop_tsid();  // a projection of time, value and tags (planner.rs:1055-1058)
       continue;
     }
     const bool filter = !s.is_fn && is_comparison(s.op) && !s.return_bool;
@@ -1052,6 +1133,9 @@ void PlanNode::run(NodeResult& r) {
     for (uint32_t f = 0; f < r.F; ++f)
       if (!(filter && r.types[f] == ValueType::Int32)) field_to_f64(ctx_, r, f);
     if (s.is_fn) {
+      // as a calendar stage; unary minus, arithmetic, `bool` and filters keep it: projection_for_each_field_column
+      // (planner.rs:543-553, 3926-3955)
+      if (s.op != B2P_IFN_NEG) r.labels.drop_tsid();
       const double a0 = s.args.size() > 0 ? s.args[0] : 0.0, a1 = s.args.size() > 1 ? s.args[1] : 0.0;
       // clamp's bound check (clamp.rs:212-217); clamp_min / clamp_max meet the other bound at ±f64::MAX.  The reference
       // checks inside the function's invoke, once per input batch, so a node without rows gives no error
@@ -1139,9 +1223,15 @@ void BinaryPlan::compute(NodeResult& r) {
   to_f64(ctx_, L);
   to_f64(ctx_, R);
   // join keys (planner.rs:696-729, 3436-3468): the rhs context's tag columns, narrowed by on / ignoring; none when a
-  // side has no tags (every row pairs with every row); two id-keyed sides without a modifier join on the id
+  // side has no tags (every row pairs with every row); two id-keyed sides, or two sides that carry __tsid, without a
+  // modifier join on the id (binary_join_key_columns: without on / ignoring the match is one-to-one)
   std::vector<int> lcols, rcols;
-  const bool by_id = L.labels.id_keyed && R.labels.id_keyed && matching_ == Matching::None;
+  const bool by_tsid = L.labels.tsid && R.labels.tsid && matching_ == Matching::None;
+  const bool by_id = by_tsid || (L.labels.id_keyed && R.labels.id_keyed && matching_ == Matching::None);
+  auto row_key = [&](const Labels& labels, uint32_t q, const std::vector<int>& cols, std::string& key) {
+    if (by_tsid) key.assign(reinterpret_cast<const char*>(&labels.ids[q]), sizeof(uint64_t));
+    else labels.key(q, cols, key);
+  };
   if (by_id) {
     lcols.push_back(0);
     rcols.push_back(0);
@@ -1157,12 +1247,12 @@ void BinaryPlan::compute(NodeResult& r) {
   std::string key;
   rhs_by_key.reserve(R.rows);
   for (uint32_t q = 0; q < R.rows; ++q) {
-    R.labels.key(q, rcols, key);
+    row_key(R.labels, q, rcols, key);
     rhs_by_key[key].push_back(q);
   }
   std::vector<uint32_t> lrow, rrow;
   for (uint32_t q = 0; q < L.rows; ++q) {
-    L.labels.key(q, lcols, key);
+    row_key(L.labels, q, lcols, key);
     const auto it = rhs_by_key.find(key);
     if (it == rhs_by_key.end()) continue;
     for (uint32_t m : it->second) {
@@ -1196,7 +1286,8 @@ void BinaryPlan::compute(NodeResult& r) {
       for (int64_t k = 0; k < r.T; ++k)
         if (r.valid_at((uint32_t)q, k)) dst[k] = src[k];
     }
-  // output labels: a filter passes the lhs rows through; a projection emits the tag columns of `label_side`
+  // output labels: a filter passes the lhs rows through; a projection emits the tag columns of `label_side`; either
+  // keeps that side's __tsid (project_binary_join_side, projection_for_each_field_column, planner.rs:779-838, 3926-3955)
   const bool from_lhs = filter || labels_from_lhs_;
   const NodeResult& side = from_lhs ? L : R;
   const std::vector<uint32_t>& srow = from_lhs ? lrow : rrow;
@@ -1372,6 +1463,12 @@ void SetOpPlan::compute(NodeResult& r) {
     r.labels.values[t].reserve((size_t)n);
     for (uint32_t q = 0; q < L.rows; ++q) r.labels.values[t].push_back(L.labels.value(lall[t], q));
     for (uint32_t q = 0; q < R.rows; ++q) r.labels.values[t].push_back(R.labels.value(rall[t], q));
+  }
+  // __tsid only when both sides carry it (planner.rs:3776-3800, 3903); `and` / `unless` keep the lhs's (3632)
+  if (L.labels.tsid && R.labels.tsid) {
+    r.labels.tsid = true;
+    r.labels.ids = L.labels.ids;
+    r.labels.ids.insert(r.labels.ids.end(), R.labels.ids.begin(), R.labels.ids.end());
   }
 }
 
@@ -1654,6 +1751,7 @@ void SubqueryPlan::compute(NodeResult& r) {
   }
   r.time_index = C.time_index;
   r.labels = std::move(C.labels);
+  r.labels.drop_tsid();  // a range function's projection (planner.rs:292-332)
   for (const std::string& value : C.value_names) {
     std::string name = function_ + "(" + C.time_index + "_range," + value;
     if (p_.fn_id == B2P_FN_RATE || p_.fn_id == B2P_FN_INCREASE || p_.fn_id == B2P_FN_DELTA) {
@@ -1729,6 +1827,7 @@ void SortPlan::compute(NodeResult& r) {
                   {Shape::MultiField, int_keys ? "GpuPromSortExec: a multi-field child with an Int64 value column is not supported by this node" : ""},
                   {Shape::IdKeyed, by_label_ ? "GpuPromSortExec: an id-keyed (__tsid) child has no label values to sort by" : ""}});
   r.cell_order.clear();
+  r.labels.drop_tsid();  // the function projection of time, value and tags (planner.rs:1055-1089)
   if (r.columns == Columns::None) return;  // no columns, no rows: the same empty batch
   r.columns = Columns::TimeValueTags;
   const uint64_t T = (uint64_t)r.T;
@@ -1874,6 +1973,7 @@ void LabelPlan::compute(NodeResult& r) {
   child_->run(r);  // the child's result is this node's: grid, validity and the rest stay where they are
   check_child(r, {{Shape::IdKeyed, "GpuPromLabelExec: an id-keyed (__tsid) child has no label values to rewrite"},
                   {Shape::Counted, "GpuPromLabelExec: a count_values child is not supported by this node"}});
+  r.labels.drop_tsid();  // its projection lists time, values and tags (create_tag_column_exprs, planner.rs:2714)
   if (r.columns == Columns::None) return;  // no columns and no rows: nothing to label
   Labels& L = r.labels;
   auto is_column = [&](const std::string& name) {
@@ -2218,6 +2318,17 @@ int b2p_plan_set_instant(b2p_plan* plan, int64_t lookback_delta) {
   if (!plan) return B2P_E_INVALID;
   if (!plan->range()) return not_a_range_node();
   return plan->range()->set_instant(lookback_delta);
+}
+
+int b2p_plan_set_label_columns(b2p_plan* plan, const char* const* names, int32_t n) {
+  if (!plan) return B2P_E_INVALID;
+  if (!plan->range()) return not_a_range_node();
+  return guarded([&] {
+    if (n < 0 || (n > 0 && !names)) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    for (int32_t i = 0; i < n; ++i)
+      if (!names[i]) throw b2p::PlanError(b2p::ErrorKind::Plan, "NULL argument");
+    plan->range()->set_label_columns(strings(names, n));
+  });
 }
 
 int b2p_plan_set_histogram_quantile(b2p_plan* plan, const char* le_column, double quantile) {

@@ -66,11 +66,15 @@ struct PromRangePlanArgs {
   bool need_filter_out_nan = true;
   // SeriesDivide::new — Utf8 tag columns, or one UInt64 column (__tsid, TagIdentifier::Id)
   std::vector<std::string> tag_columns;
+  // a metric-engine leaf (planner.rs:1725-1800): the Utf8 label columns that travel beside the one UInt64 id tag
+  // column.  Series still divide on the id; each series takes its labels from its first row (RangeManipulate's
+  // take([0; T])).  The metric engine gives one tsid one label set; this node does not check it.
+  std::vector<std::string> label_columns;
   // UDF scalar arguments (quantile phi / predict_linear t / smoothing sf, tf)
   double param0 = 0.0, param1 = 0.0;
   // optional prom_aggr_expr_to_plan stage: "", "sum", "avg", "count", "min", "max", "stddev", "stdvar"
   std::string aggregate;
-  std::vector<std::string> by_columns;  // must be a subset of tag_columns
+  std::vector<std::string> by_columns;  // must be a subset of tag_columns (label_columns on a metric-engine leaf)
   // function == "" selects the instant-vector form instead: InstantManipulate::new(start, end, lookback_delta,
   // interval, time_index, field_column) (instant_manipulate.rs:189-208); `range` is ignored
   Millisecond lookback_delta = 300000;
@@ -86,11 +90,14 @@ struct PromRangePlanArgs {
 using Label = std::optional<std::string>;
 
 // The label tuples of a node's rows: the tag names and, per row, either one UInt64 id (the single tag column is an id
-// such as __tsid) or one Label per tag.
+// such as __tsid) or one Label per tag.  Rows of a metric-engine table may also carry their __tsid beside the label
+// values (`tsid`): every match, group, order and rewrite reads the values; only the binary node's one-to-one join
+// reads the ids, and the export adds them as a UInt64 column `__tsid` after every other column.
 struct Labels {
   std::vector<std::string> names;
   bool id_keyed = false;
-  std::vector<uint64_t> ids;               // [row] when id_keyed
+  bool tsid = false;                       // the rows carry __tsid in `ids` beside `values` (never with id_keyed)
+  std::vector<uint64_t> ids;               // [row] when id_keyed or tsid
   std::vector<std::vector<Label>> values;  // [tag][row] when not id_keyed (empty when it is)
 
   int column(const std::string& name) const;  // -1 when absent
@@ -101,6 +108,12 @@ struct Labels {
   void key(uint32_t r, const std::vector<int>& cols, std::string& key) const;
   Labels gather(const std::vector<uint32_t>& rows) const;  // the given rows, in that order
   static bool less(const Label& a, const Label& b);         // the order of label values in sorted output
+  // drops the __tsid beside the values: the node's projection lists the time index, values and tags only
+  void drop_tsid() {
+    if (!tsid) return;
+    tsid = false;
+    ids.clear();
+  }
 };
 
 // The column order of an exported batch
@@ -212,6 +225,8 @@ class PromRangePlan : public PlanNode {
     return 0;
   }
   void set_histogram(const std::string& le_column, double quantile);
+  // the metric-engine form: `names` are Utf8 label columns beside the one UInt64 id tag column (before push())
+  void set_label_columns(std::vector<std::string> names);
   // timestamp(<selector>): the instant form whose value is the chosen sample's timestamp in seconds (K4's timestamp
   // mode); the result is one Float64 column named `value` whatever the table's fields
   int set_timestamp(Millisecond lookback_delta) {
@@ -240,6 +255,7 @@ class PromRangePlan : public PlanNode {
   std::vector<Label> last_key_;
   uint64_t last_id_ = 0;
   bool have_last_ = false;
+  void check_key_columns() const;  // by-columns and the le column name a tag or label column
 };
 
 // Label matching modifier of a binary or set operator

@@ -86,13 +86,18 @@ class _PlanNode:
 
 class PromRangeExec(_PlanNode):
     """The range / instant leaf.  `field_column` is one field name, or a sequence of them for a table with several
-    Float64 field columns: every field is selected at once and execute() emits one value column per field."""
+    Float64 field columns: every field is selected at once and execute() emits one value column per field.
+    `label_columns` makes it a metric-engine leaf: `tag_columns` is the one UInt64 `__tsid` column the series divide
+    on, and the label columns (Utf8) travel beside it, read at each series' first row; `by_columns` and `le_column` then
+    name label columns.  Nodes above read the labels; a UInt64 `__tsid` column is exported last where the reference
+    keeps it."""
 
     def __init__(self, ctx: Context, function: str, start: int, end: int, interval: int, range: int, time_index: str,
                  field_column: Union[str, Sequence[str]], tag_columns: Sequence[str], offset: int = 0,
                  need_filter_out_nan: bool = True, param0: float = 0.0, param1: float = 0.0,
                  aggregate: Optional[str] = None, by_columns: Sequence[str] = (), lookback_delta: Optional[int] = None,
-                 histogram_quantile: Optional[float] = None, le_column: str = "le"):
+                 histogram_quantile: Optional[float] = None, le_column: str = "le",
+                 label_columns: Optional[Sequence[str]] = None):
         self._L = _lib.load()
         self._ctx = ctx
         p = make_params(0, start, end, interval, range, offset=offset, filter_nan=need_filter_out_nan, param0=param0,
@@ -104,6 +109,10 @@ class PromRangeExec(_PlanNode):
                                                        by, len(by_columns))
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+        if label_columns is not None:       # the metric-engine form: __tsid plus label columns
+            rc = self._L.b2p_plan_set_label_columns(self._h, _cstr_array(list(label_columns)), len(label_columns))
+            if rc != 0:
+                raise B2PError(rc, self._L.b2p_plan_last_error().decode())
         if lookback_delta is not None:      # instant-vector selector (InstantManipulate) instead of a range function
             self._L.b2p_plan_set_instant(self._h, int(lookback_delta))
         if histogram_quantile is not None:  # HistogramFold on top

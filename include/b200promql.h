@@ -669,7 +669,10 @@ B2P_API int b2p_absent(b2p_ctx* ctx, const uint32_t* valid, uint32_t n_rows, uin
  * RangeManipulate::new range_manipulate.rs:86-110, UDF names planner.rs:2183-2221).
  * Input batches must be sorted by (tag columns, time index) — SeriesDivideExec's own requirement.
  * `function` is the UDF name ("prom_rate", ...); p->fn_id is ignored.  tag columns: Utf8, or a single
- * UInt64 id column.  aggregate: NULL/"" or "sum|avg|count|min|max|stddev|stdvar" with by_columns ⊆ tags.
+ * UInt64 id column (with label columns beside it: b2p_plan_set_label_columns).  aggregate: NULL/"" or
+ * "sum|avg|count|min|max|stddev|stdvar" with by_columns ⊆ tags, checked at create (⊆ label columns on a
+ * metric-engine leaf: a leaf keyed on `__tsid` alone checks a by-column that is not `__tsid` at
+ * b2p_plan_set_label_columns and at push instead).
  * b2p_plan_push_batch MOVES the batch (its release callbacks are taken over). b2p_plan_execute
  * fills caller-provided ArrowArray/ArrowSchema structs; the caller releases them. */
 #ifndef ARROW_C_DATA_INTERFACE
@@ -725,6 +728,22 @@ B2P_API b2p_plan* b2p_plan_range_create_fields(b2p_ctx* ctx, const char* functio
 /* Turn the node into the instant-vector form: InstantManipulate(start, end, lookback_delta, interval, ...)
  * (instant_manipulate.rs:189-208) instead of RangeManipulate + prom_fn; `function` / range are then ignored. */
 B2P_API int b2p_plan_set_instant(b2p_plan* plan, int64_t lookback_delta);
+/* The metric-engine form of a leaf (planner.rs:1300-1350, 1725-1800): Prometheus remote write tables divide their
+ * series on the one UInt64 tag column `__tsid` (a hash of the label set), and `names` are the n >= 1 Utf8 label
+ * columns that travel beside it.  Batches are sorted by (__tsid, time index); series divide on the id alone, and each
+ * series takes its label values (NULL allowed) from its first row.  The metric engine gives one id one label set;
+ * this node does not check it.  The nodes above group, match, order and rewrite on the label values, as over a leaf
+ * keyed on those columns; the by-columns of the aggregate stage and the le column of HistogramFold name label columns.
+ * __tsid rides along as a UInt64 column `__tsid`, exported after every other column, where the reference keeps it:
+ * the instant selector, unary minus, scalar arithmetic, `bool` and filtering stages, both binary forms (the label side's; two sides
+ * that carry it with no on / ignoring join on it one-to-one), `and` / `unless` (the lhs's), `or` (when both sides have
+ * it), topk / bottomk, and an aggregate other than count_values that groups on every label column (the group's first
+ * member's id, keep_tsid planner.rs:347-416).  Every other node drops it.  Call before the first push and before
+ * b2p_plan_set_histogram_quantile: at the call, a leaf whose tag columns are not exactly `__tsid`, no label column,
+ * one named like the time index, a field or the tag column, and one given twice are Plan errors; at push, a `__tsid`
+ * column that is not UInt64 and a missing label column are Plan errors and a non-Utf8 label column an Execution
+ * error. */
+B2P_API int b2p_plan_set_label_columns(b2p_plan* plan, const char* const* names, int32_t n);
 /* Add HistogramFold(le_column, field, time_index, quantile) (histogram_fold.rs:104-130) on top of the per-series
  * result: series that agree on every tag except `le` form one histogram.  Refused for a node of two or more fields. */
 B2P_API int b2p_plan_set_histogram_quantile(b2p_plan* plan, const char* le_column, double quantile);

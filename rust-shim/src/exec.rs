@@ -53,6 +53,9 @@ pub struct GpuPromRangeParams {
     pub need_filter_out_nan: bool,
     // SeriesDivide::new (series_divide.rs:83-110): Utf8 tag columns, or the single `__tsid: UInt64` column
     pub tag_columns: Vec<String>,
+    /// A metric-engine scan (planner.rs:1725-1800): the Utf8 label columns that travel beside the `__tsid` tag column
+    /// (b2p_plan_set_label_columns); empty otherwise.
+    pub label_columns: Vec<String>,
     // UDF scalars: quantile phi / predict_linear t / smoothing factors
     pub param0: f64,
     pub param1: f64,
@@ -68,6 +71,19 @@ pub struct GpuPromRangeParams {
     pub histogram: Option<(String, f64)>,
     /// Element-wise stages on top, in order: `node op scalar` projections / filters and instant-vector functions.
     pub stages: Vec<GpuPromStage>,
+}
+
+impl GpuPromRangeParams {
+    /// The label columns the nodes above group, match, order and rewrite on: a metric-engine leaf's label columns,
+    /// otherwise its tag columns.
+    pub fn labels(&self) -> &[String] {
+        if self.label_columns.is_empty() { &self.tag_columns } else { &self.label_columns }
+    }
+
+    /// The label-less `__tsid` form: the one tag column is the id and no label travels beside it.
+    pub fn id_only(&self) -> bool {
+        self.label_columns.is_empty() && self.tag_columns == [String::from("__tsid")]
+    }
 }
 
 /// One element-wise stage of a `GpuPromRangeExec` (b2p_plan_set_scalar_op / b2p_plan_set_function).
@@ -284,6 +300,13 @@ impl PlanHandle {
                 return Err(DataFusionError::Plan(e));
             }
             let h = Self { ctx, plan };
+            if !p.label_columns.is_empty() {
+                let labels: Vec<CString> = p.label_columns.iter().map(|s| c(s)).collect();
+                let label_ptrs: Vec<*const std::os::raw::c_char> = labels.iter().map(|s| s.as_ptr()).collect();
+                if ffi::b2p_plan_set_label_columns(plan, label_ptrs.as_ptr(), label_ptrs.len() as i32) != ffi::B2P_OK {
+                    return Err(DataFusionError::Plan(ffi::plan_last_error()));
+                }
+            }
             let instant = if p.timestamp {
                 ffi::b2p_plan_set_timestamp(plan, p.lookback_delta)
             } else if p.function.is_empty() {

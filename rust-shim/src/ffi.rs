@@ -571,6 +571,8 @@ extern "C" {
     ) -> *mut b2p_plan;
     pub fn b2p_plan_set_instant(plan: *mut b2p_plan, lookback_delta: i64) -> c_int;
     pub fn b2p_plan_set_histogram_quantile(plan: *mut b2p_plan, le_column: *const c_char, quantile: f64) -> c_int;
+    /// The metric-engine leaf: Utf8 label columns beside the one UInt64 `__tsid` tag column (before the first push).
+    pub fn b2p_plan_set_label_columns(plan: *mut b2p_plan, names: *const *const c_char, n: i32) -> c_int;
     pub fn b2p_plan_set_scalar_op(plan: *mut b2p_plan, op: i32, scalar: f64, scalar_on_left: i32, return_bool: i32) -> c_int;
     /// The node shares ownership of both children; their handles stay valid and must still be destroyed.
     pub fn b2p_plan_binary_create(

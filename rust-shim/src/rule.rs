@@ -141,7 +141,7 @@
 //! getters it needs are listed in `rust-shim/README.md`.
 use std::sync::Arc;
 
-use datafusion::arrow::datatypes::DataType;
+use datafusion::arrow::datatypes::{DataType, SchemaRef};
 use datafusion::common::tree_node::{Transformed, TreeNode};
 use datafusion::common::{Result as DataFusionResult, ScalarValue};
 use datafusion::config::ConfigOptions;
@@ -201,6 +201,26 @@ struct FieldUdfs {
     /// the value column each call reads, in projection order (the RangeManipulate's field columns)
     fields: Vec<String>,
     input: Arc<dyn ExecutionPlan>,
+}
+
+/// The label columns of a metric-engine scan (planner.rs:1725-1800, 1834): when SeriesDivide runs on `__tsid` alone,
+/// the Utf8 columns of its input other than the time index, the fields and `__tsid`, which travel beside the id and
+/// which the nodes above read.  Empty for any other divide.
+fn metric_engine_labels(tags: &[String], schema: &SchemaRef, time_index: &str, fields: &[String]) -> Vec<String> {
+    if tags != [String::from("__tsid")] {
+        return vec![];
+    }
+    schema
+        .fields()
+        .iter()
+        .filter(|f| {
+            f.name() != time_index
+                && f.name() != "__tsid"
+                && !fields.contains(f.name())
+                && matches!(f.data_type(), DataType::Utf8)
+        })
+        .map(|f| f.name().clone())
+        .collect()
 }
 
 fn match_field_udfs(plan: &Arc<dyn ExecutionPlan>) -> Option<FieldUdfs> {
@@ -278,6 +298,8 @@ impl GpuPromRewrite {
             offset: normalize.offset(),
             need_filter_out_nan: normalize.need_filter_out_nan(),
             tag_columns: divide.tag_columns().to_vec(),
+            label_columns: metric_engine_labels(divide.tag_columns(), &divide.input().schema(),
+                                                range_exec.time_index_column(), range_exec.field_columns()),
             param0,
             param1,
             lookback_delta: 0,
@@ -323,7 +345,7 @@ impl GpuPromRewrite {
         for (expr, _name) in partial.group_expr().expr() {
             let col = expr.as_any().downcast_ref::<Column>()?;
             if col.name() != params.time_index_column {
-                if !params.tag_columns.iter().any(|t| t == col.name()) {
+                if !params.labels().iter().any(|t| t == col.name()) {
                     return None;
                 }
                 by.push(col.name().to_string());
@@ -726,6 +748,7 @@ impl GpuPromRewrite {
             offset: normalize.offset(),
             need_filter_out_nan: normalize.need_filter_out_nan(),
             tag_columns: tags.to_vec(),
+            label_columns: metric_engine_labels(tags, &schema, ts, &[field.name().clone()]),
             param0: 0.0,
             param1: 0.0,
             lookback_delta: instant.lookback_delta(),
@@ -896,12 +919,14 @@ impl GpuPromRewrite {
         for (expr, _name) in partial.group_expr().expr() {
             let c = expr.as_any().downcast_ref::<Column>()?;
             if c.name() != params.time_index_column {
-                if !params.tag_columns.iter().any(|t| t == c.name()) {
+                if !params.labels().iter().any(|t| t == c.name()) {
                     return None;
                 }
                 by.push(c.name().to_string());
             }
         }
+        // keep_tsid (planner.rs:347-416) needs no check here: the child is a range-function or timestamp leaf, whose
+        // projection drops __tsid in the reference and in the library alike, so neither keeps it above
         Some(GpuPromAggregateSpec { op, param, by, child: params.clone() })
     }
 
@@ -935,7 +960,7 @@ impl GpuPromRewrite {
             if c.name() == params.time_index_column {
                 continue;
             }
-            if params.tag_columns.iter().any(|t| t == c.name()) {
+            if params.labels().iter().any(|t| t == c.name()) {
                 by.push(c.name().to_string());
             } else if value.replace(c.name().to_string()).is_some() {
                 return None;
@@ -994,8 +1019,9 @@ impl GpuPromRewrite {
     /// element-wise stages) whose Utf8 tag columns include the le column; the library's node accepts any node, but
     /// this matcher only builds the ones the rule rewrites into a `GpuPromRangeExec`.  Left on the CPU: a leaf that
     /// already carries its own HistogramFold, and a `__tsid`-keyed input.  The reference strips `__tsid` with a
-    /// `ProjectionExec` before the fold (strip_tsid_column, planner.rs:3064), so such an input does not match here.
-    /// The library could not fold it anyway: an id-keyed node carries no le label.
+    /// `ProjectionExec` before the fold (strip_tsid_column, planner.rs:3064), so such an input does not match here
+    /// even when its leaf carries the labels (a metric-engine leaf): that shape stays on the CPU until this matcher
+    /// looks through the strip projection.  A label-less id-keyed node carries no le label at all.
     pub fn match_histogram_quantile(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromHistogramQuantileSpec> {
         let fold = plan.as_any().downcast_ref::<HistogramFoldExec>()?;
         let mut input = fold.input().clone();
@@ -1010,7 +1036,7 @@ impl GpuPromRewrite {
         // several fields: the reference folds the first one only (a FIXME, planner.rs:3084-3092); the library refuses
         if child.params().histogram.is_some()
             || child.params().field_columns.len() != 1
-            || !child.params().tag_columns.iter().any(|t| *t == le_column)
+            || !child.params().labels().iter().any(|t| *t == le_column)
         {
             return None;
         }
@@ -1064,12 +1090,12 @@ impl GpuPromRewrite {
             let function = if descending { "sort_desc" } else { "sort" };
             return Some(GpuPromSortSpec { function: function.to_string(), labels: vec![], child: params.clone() });
         }
-        if nulls_first || params.tag_columns == [String::from("__tsid")] {
+        if nulls_first || params.id_only() {
             return None;
         }
         let mut labels = Vec::new();
         for (name, _, _) in &keys {
-            if !params.tag_columns.iter().any(|t| t == name) || !names.iter().any(|n| n == name) {
+            if !params.labels().iter().any(|t| t == name) || !names.iter().any(|n| n == name) {
                 return None;
             }
             labels.push(name.clone());
@@ -1083,13 +1109,13 @@ impl GpuPromRewrite {
     /// `regexp_replace(<tag column>, Utf8("^(?s:<raw>)$"), Utf8(r))`, `Utf8(r)` (a source that is not a tag) or
     /// `concat_ws(Utf8(sep), <tag column> | NULL, ..)` -> the arguments of `b2p_plan_label_replace_create` /
     /// `b2p_plan_label_join_create`.  A regex the library does not support, a source column that is not a tag of the
-    /// child (the time index or a value column), an id-keyed child and every other shape stay on the CPU.  No-op
+    /// child (the time index or a value column), a label-less id-keyed child and every other shape stay on the CPU.  No-op
     /// label_replace plans have no generated expression: `match_passthrough` takes them.
     pub fn match_label(&self, plan: &Arc<dyn ExecutionPlan>) -> Option<GpuPromLabelSpec> {
         let p = plan.as_any().downcast_ref::<ProjectionExec>()?;
         let child = p.input().as_any().downcast_ref::<GpuPromRangeExec>()?;
         let params = child.params();
-        if params.tag_columns == [String::from("__tsid")] {
+        if params.id_only() {
             return None;
         }
         let mut generated = None;
@@ -1104,7 +1130,7 @@ impl GpuPromRewrite {
         let (expr, dst) = generated?;
         let tag = |e: &Arc<dyn PhysicalExpr>| {
             let c = e.as_any().downcast_ref::<Column>()?;
-            params.tag_columns.iter().any(|t| t == c.name()).then(|| c.name().to_string())
+            params.labels().iter().any(|t| t == c.name()).then(|| c.name().to_string())
         };
         let spec = |join, replacement: String, src: String, regex: String, srcs: Vec<String>| GpuPromLabelSpec {
             join,
