@@ -45,6 +45,8 @@ EXPORTED_SYMBOLS = [
     "b2p_plan_empty_metric_create", "b2p_plan_set_timestamp",
     "b2p_plan_label_replace_create", "b2p_plan_label_join_create", "b2p_label_regex_check", "b2p_label_regex_replace",
     "b2p_plan_set_label_columns",
+    "b2p_topk_allgather_dev", "b2p_last_exchange_bytes", "b2p_topk_shard_plan", "b2p_topk_shard_candidates_dev",
+    "b2p_topk_shard_merge_dev", "b2p_topk_shard_mark_dev",
 ]
 
 
@@ -195,6 +197,13 @@ def load() -> C.CDLL:
         "b2p_plan_label_join_create": (vp, [vp, vp, C.c_char_p, C.c_char_p, C.POINTER(C.c_char_p), i32]),
         "b2p_label_regex_check": (C.c_int, [C.c_char_p]),
         "b2p_label_regex_replace": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, u64, C.POINTER(u64)]),
+        "b2p_topk_allgather_dev": (C.c_int, [vp, i32, dbl, vp, vp, vp, vp, u64, vp]),
+        "b2p_last_exchange_bytes": (i64, [vp]),
+        "b2p_topk_shard_plan": (C.c_int, [vp, dbl, vp, u32, u64, i32, C.POINTER(u32), C.POINTER(u32), C.POINTER(u32),
+                                          C.POINTER(u64), C.POINTER(u64)]),
+        "b2p_topk_shard_candidates_dev": (C.c_int, [vp, i32, dbl, vp, vp, vp, vp, u64, vp, i32, u32, u32, vp, vp]),
+        "b2p_topk_shard_merge_dev": (C.c_int, [vp, dbl, vp, u32, u64, i32, u32, u32, vp, vp]),
+        "b2p_topk_shard_mark_dev": (C.c_int, [vp, i32, dbl, vp, vp, vp, vp, u64, vp, i32, u32, vp, vp]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)  # AttributeError here means the .so does not match the header

@@ -76,7 +76,7 @@ int topk_run(b2p_ctx* c, int bottom, uint32_t kk, const double* vals, const uint
       chunks.push_back(TopkChunk{b, e, kTopkNone, general ? n_state++ : kTopkNone});
     } else {
       const uint32_t nc = (uint32_t)((s + C - 1) / C);
-      merges.push_back(TopkMerge{n_cand, n_cand + nc, n_state, 0});
+      merges.push_back(TopkMerge{n_cand, n_cand + nc, n_state, 1});
       for (uint32_t i = 0; i < nc; ++i)
         chunks.push_back(TopkChunk{b + (uint32_t)((uint64_t)s * i / nc), b + (uint32_t)((uint64_t)s * (i + 1) / nc),
                                    n_cand++, n_state});
@@ -133,6 +133,266 @@ int topk_run(b2p_ctx* c, int bottom, uint32_t kk, const double* vals, const uint
   }
   c->launches++;
   CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// ---- sharded topk / bottomk: the rows of every rank, one exchange of candidates ---------------------------------------
+// The exchange is derived from kk, T, the rank count and the global group sizes only, so every rank derives the same
+// batches and block sizes.  Exchanged groups (G_x) are the groups of more than kk members globally, in id order.  The
+// (exchanged group, tile) units are cut into batches whose blocks and state fit topk_exchange_cap: all the tiles of as
+// many groups as fit, or groups x1 tile when one tile of every group does not fit.  Batch b covers tiles
+// [t0, t0 + nt) of groups [x0, x0 + nx).
+struct TopkShard {
+  uint32_t kk = 0, K = 0, rounds = 0;
+  int mode = 0;                   // 0: nothing kept; 1: every valid cell kept; 2: exchange
+  std::vector<uint32_t> xg;       // exchanged group ids, ascending
+  uint32_t tiles = 0, tb = 1, xb = 1, n_tb = 1, n_xb = 1, n_batches = 1;
+  uint32_t n_ranks = 1;
+  struct Batch { uint32_t x0, nx, t0, nt; };
+  Batch batch(uint32_t b) const {
+    const uint32_t x0 = (b % n_xb) * xb, t0 = (b / n_xb) * tb;
+    return Batch{x0, std::min<uint32_t>(xb, (uint32_t)xg.size() - x0), t0, std::min(tb, tiles - t0)};
+  }
+  uint64_t slot_bytes() const { return (uint64_t)K * 12 + 4; }  // per (group, step): K keys (8 B + 4 B tie) and a count
+  uint64_t block_bytes(const Batch& bt) const { return (uint64_t)bt.nx * bt.nt * 32 * slot_bytes(); }
+  uint64_t state_bytes(const Batch& bt) const { return (uint64_t)bt.nx * bt.nt * 32 * 20; }
+};
+
+int shard_plan(const b2p_ctx* c, double k, const uint32_t* sizes, uint32_t n_groups, uint64_t T, int32_t n_ranks,
+               TopkShard& sh) {
+  if (n_ranks < 1) return fail(B2P_E_INVALID, "n_ranks %d < 1", n_ranks);
+  if (n_groups && !sizes) return fail(B2P_E_INVALID, "NULL argument");
+  sh.n_ranks = (uint32_t)n_ranks;
+  sh.kk = topk_ranks(k);
+  sh.tiles = (uint32_t)((T + 31) / 32);
+  uint32_t largest = 0;
+  for (uint32_t g = 0; g < n_groups; ++g) largest = std::max(largest, sizes[g]);
+  sh.mode = sh.kk == 0 ? 0 : (sh.kk >= largest ? 1 : 2);
+  if (sh.mode != 2 || T == 0) return B2P_OK;  // one batch without rounds: the words alone
+  for (uint32_t g = 0; g < n_groups; ++g)
+    if (sizes[g] > sh.kk) sh.xg.push_back(g);
+  sh.K = std::min(sh.kk, kTopkMax);
+  sh.rounds = sh.kk > kTopkMax ? (sh.kk + kTopkMax - 1) / kTopkMax : 1;
+  const uint64_t X = sh.xg.size();
+  const uint64_t unit = (uint64_t)(sh.n_ranks + 1) * 32 * sh.slot_bytes() + 32 * 20;  // send, gathered, state
+  const uint64_t fit = std::max<uint64_t>(1, c->topk_exchange_cap / unit);
+  if (X * sh.tiles <= fit) {
+    sh.xb = (uint32_t)X; sh.tb = sh.tiles;
+  } else if (X <= fit) {
+    sh.xb = (uint32_t)X; sh.tb = (uint32_t)(fit / X);
+  } else {
+    sh.xb = (uint32_t)fit; sh.tb = 1;
+  }
+  sh.n_xb = (uint32_t)((X + sh.xb - 1) / sh.xb);
+  sh.n_tb = (sh.tiles + sh.tb - 1) / sh.tb;
+  sh.n_batches = sh.n_xb * sh.n_tb;
+  return B2P_OK;
+}
+
+// This rank's chunks of the batch's exchanged groups (each chunk leaves a candidate list; state = the group's place in
+// the batch) and one merge per exchanged group, with no chunk where the rank holds no member; the tables go to t_table
+// and a is set up over them (candidate lists in t_cand).  The same inputs give the same tables, so the mark of a batch
+// finds the lists its candidates step left.
+int shard_local(b2p_ctx* c, const TopkShard& sh, const TopkShard::Batch& bt, const b2p_group_index* ix, TopkArgs& a) {
+  int rc;
+  const size_t smem = kTopkWarps * topk_warp_bytes(sh.K);
+  unsigned cap = 0;
+  if ((rc = persistent_grid(c, topk_chunk_kernel<F64Key>, smem, kTopkWarps, kAllResident, &cap))) return rc;
+  const uint64_t resident = (uint64_t)cap * kTopkWarps, U = resident - resident / 8;
+  uint64_t members = 0;
+  for (uint32_t i = 0; i < bt.nx; ++i) {
+    const uint32_t g = sh.xg[bt.x0 + i];
+    if (g < ix->n_groups) members += ix->goff_host[g + 1] - ix->goff_host[g];
+  }
+  const uint64_t C = std::max<uint64_t>(256, (members * bt.nt + U - 1) / U);
+  std::vector<TopkChunk> chunks;
+  std::vector<TopkMerge> merges;
+  uint32_t n_cand = 0;
+  for (uint32_t i = 0; i < bt.nx; ++i) {
+    const uint32_t g = sh.xg[bt.x0 + i];
+    const uint32_t b = g < ix->n_groups ? ix->goff_host[g] : 0, e = g < ix->n_groups ? ix->goff_host[g + 1] : 0;
+    const uint32_t s = e - b, nc = (uint32_t)((s + C - 1) / C);
+    merges.push_back(TopkMerge{n_cand, n_cand + nc, i, 1});
+    for (uint32_t j = 0; j < nc; ++j)
+      chunks.push_back(TopkChunk{b + (uint32_t)((uint64_t)s * j / nc), b + (uint32_t)((uint64_t)s * (j + 1) / nc),
+                                 n_cand++, i});
+  }
+  const size_t tb_chunks = chunks.size() * sizeof(TopkChunk), tb_merges = merges.size() * sizeof(TopkMerge);
+  if ((rc = c->t_table.ensure(tb_chunks + tb_merges + 16))) return rc;
+  if (tb_chunks) CU(cudaMemcpyAsync(c->t_table.p, chunks.data(), tb_chunks, cudaMemcpyHostToDevice, c->stream));
+  CU(cudaMemcpyAsync(c->t_table.as<char>() + tb_chunks, merges.data(), tb_merges, cudaMemcpyHostToDevice, c->stream));
+  const size_t cand_units = (size_t)n_cand * bt.nt, cand_slots = cand_units * sh.K * 32;
+  if ((rc = c->t_cand.ensure(cand_slots * 16 + cand_units * 32 * 4 + 64))) return rc;
+  a.members = ix->members;
+  a.chunks = c->t_table.as<TopkChunk>(); a.n_chunks = (uint32_t)chunks.size();
+  a.merges = reinterpret_cast<const TopkMerge*>(c->t_table.as<char>() + tb_chunks); a.n_merges = (uint32_t)merges.size();
+  a.c_hi = c->t_cand.as<unsigned long long>();
+  a.c_lo = reinterpret_cast<uint32_t*>(a.c_hi + cand_slots);
+  a.c_pos = a.c_lo + cand_slots;
+  a.c_n = a.c_pos + cand_slots;
+  return B2P_OK;
+}
+
+// The arguments every shard step shares; state: the batch's selection state, [unit][lane] sections hi, lo, rem, flags
+TopkArgs shard_args(const TopkShard& sh, const TopkShard::Batch& bt, uint64_t T, void* state) {
+  TopkArgs a{};
+  a.T = T; a.Tw = sh.tiles; a.tiles = bt.nt; a.tile0 = bt.t0;
+  a.K = sh.K; a.kk = sh.kk; a.general = sh.rounds > 1 ? 1 : 0;
+  const size_t cells = (size_t)bt.nx * bt.nt * 32;
+  a.s_hi = static_cast<unsigned long long*>(state);
+  a.s_lo = reinterpret_cast<uint32_t*>(a.s_hi + cells);
+  a.s_rem = a.s_lo + cells;
+  a.s_flags = a.s_rem + cells;
+  return a;
+}
+
+template <class Kern>
+int topk_launch(b2p_ctx* c, Kern* kern, size_t smem, uint64_t units, const TopkArgs& a) {
+  unsigned grid = 0;
+  if (int rc = persistent_grid(c, kern, smem, kTopkWarps, units, &grid)) return rc;
+  if (grid == 0) return B2P_OK;
+  kern<<<grid, kTopkWarps * 32, smem, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// A block of bt's units: [hi: units x K x 32 u64][lo: units x K x 32 u32][n: units x 32 u32]; the gathered blocks of R
+// ranks: each section of every rank in rank order, [hi of rank 0 .. R-1][lo ..][n ..], as three all-gathers lay them
+struct ShardBlock {
+  unsigned long long* hi;
+  uint32_t* lo;
+  uint32_t* n;
+};
+ShardBlock shard_block(const TopkShard& sh, const TopkShard::Batch& bt, void* p, uint32_t ranks) {
+  const size_t slots = (size_t)bt.nx * bt.nt * sh.K * 32 * ranks;
+  ShardBlock k;
+  k.hi = static_cast<unsigned long long*>(p);
+  k.lo = reinterpret_cast<uint32_t*>(k.hi + slots);
+  k.n = k.lo + slots;
+  return k;
+}
+
+// Per-rank step: this rank's best K keys below the bound of every (exchanged group, step) of the batch -> block
+int shard_candidates(b2p_ctx* c, const TopkShard& sh, uint32_t b, uint32_t round, int bottom, const double* vals,
+                     const uint32_t* valid, const b2p_group_index* ix, const uint32_t* tie, uint64_t T, void* state,
+                     void* block) {
+  const TopkShard::Batch bt = sh.batch(b);
+  TopkArgs a = shard_args(sh, bt, T, state);
+  int rc;
+  if ((rc = shard_local(c, sh, bt, ix, a))) return rc;
+  a.vals = vals; a.valid = valid; a.tie = tie; a.bottom = bottom ? 1 : 0; a.round = (int)round;
+  const size_t smem = kTopkWarps * topk_warp_bytes(sh.K);
+  if ((rc = topk_launch(c, topk_chunk_kernel<F64Key>, smem, (uint64_t)a.n_chunks * bt.nt, a))) return rc;
+  const ShardBlock x = shard_block(sh, bt, block, 1);
+  a.x_hi = x.hi; a.x_lo = x.lo; a.x_n = x.n;
+  if ((rc = topk_launch(c, topk_merge_kernel, smem, (uint64_t)bt.nx * bt.nt, a))) return rc;
+  c->last_exchange_bytes += (long long)sh.block_bytes(bt);
+  return B2P_OK;
+}
+
+// Merge step: the verdict of the round over the gathered blocks of every rank -> state
+int shard_merge(b2p_ctx* c, const TopkShard& sh, uint32_t b, uint32_t round, const void* blocks, void* state, uint64_t T) {
+  const TopkShard::Batch bt = sh.batch(b);
+  TopkArgs a = shard_args(sh, bt, T, state);
+  std::vector<TopkMerge> merges(bt.nx);
+  for (uint32_t i = 0; i < bt.nx; ++i) merges[i] = TopkMerge{i, i + sh.n_ranks * bt.nx, i, bt.nx};
+  int rc;
+  if ((rc = c->x_table.ensure(merges.size() * sizeof(TopkMerge)))) return rc;
+  CU(cudaMemcpyAsync(c->x_table.p, merges.data(), merges.size() * sizeof(TopkMerge), cudaMemcpyHostToDevice, c->stream));
+  const ShardBlock x = shard_block(sh, bt, const_cast<void*>(blocks), sh.n_ranks);
+  a.merges = c->x_table.as<TopkMerge>(); a.n_merges = bt.nx;
+  a.c_hi = x.hi; a.c_lo = x.lo; a.c_n = x.n;
+  a.round = (int)round;
+  return topk_launch(c, topk_merge_kernel, kTopkWarps * topk_warp_bytes(sh.K), (uint64_t)bt.nx * bt.nt, a);
+}
+
+// Mark step: this rank's words of the batch from the state after the last round.  Batch 0 first writes the words of
+// every row the exchange does not decide: 0 when nothing is kept and for rows of no group, the valid cells otherwise
+// (the exchanged groups' rows are overwritten by their batches).
+int shard_mark(b2p_ctx* c, const TopkShard& sh, uint32_t b, int bottom, const double* vals, const uint32_t* valid,
+               const b2p_group_index* ix, const uint32_t* tie, uint64_t T, const void* state, uint32_t* out_valid) {
+  const uint32_t R = ix->n_series;
+  const size_t words = (size_t)R * sh.tiles;
+  if (b == 0 && words) {
+    if (sh.mode == 0) {
+      CU(cudaMemsetAsync(out_valid, 0, words * 4, c->stream));
+    } else {
+      topk_copy_kernel<<<capped_grid(c, words, 256, 16), 256, 0, c->stream>>>(valid, ix->gid, ix->n_groups, R, T,
+                                                                              sh.tiles, 0, out_valid);
+      c->launches++;
+      CU(cudaGetLastError());
+    }
+  }
+  if (sh.mode != 2) return B2P_OK;
+  const TopkShard::Batch bt = sh.batch(b);
+  TopkArgs a = shard_args(sh, bt, T, const_cast<void*>(state));
+  int rc;
+  if ((rc = shard_local(c, sh, bt, ix, a))) return rc;
+  if (a.n_chunks == 0) return B2P_OK;
+  a.vals = vals; a.valid = valid; a.tie = tie; a.bottom = bottom ? 1 : 0; a.out_valid = out_valid;
+  const uint64_t units = (uint64_t)a.n_chunks * bt.nt;
+  if (sh.rounds > 1) {
+    topk_select_kernel<F64Key><<<capped_grid(c, units, 8, 16), 256, 0, c->stream>>>(a);
+    c->launches++;
+    CU(cudaGetLastError());
+    return B2P_OK;
+  }
+  return topk_launch(c, topk_mark_kernel, 0, units, a);
+}
+
+// The composed call: the global group sizes (one all-reduce and one read-back), then per batch the rounds of
+// candidates, all-gather and merge, and the mark.  Without a communicator (one rank) the block is its own gather.
+int topk_allgather_run(b2p_ctx* c, int bottom, double k, const double* vals, const uint32_t* valid,
+                       const b2p_group_index* ix, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
+  int rc;
+  const uint32_t G = ix->n_groups;
+  std::vector<uint32_t> sizes(G);
+  for (uint32_t g = 0; g < G; ++g) sizes[g] = ix->goff_host[g + 1] - ix->goff_host[g];
+  if (c->comm && G) {
+    if ((rc = c->x_size.ensure((size_t)G * 4))) return rc;
+    CU(cudaMemcpyAsync(c->x_size.p, sizes.data(), (size_t)G * 4, cudaMemcpyHostToDevice, c->stream));
+    NCCL_TRY(g_nccl.AllReduce(c->x_size.p, c->x_size.p, G, Nccl::kUint32, Nccl::kSum, c->comm, c->stream));
+    CU(cudaMemcpyAsync(sizes.data(), c->x_size.p, (size_t)G * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+  }
+  TopkShard sh;
+  if ((rc = shard_plan(c, k, sizes.data(), G, T, c->comm_ranks, sh))) return rc;
+  c->last_exchange_bytes = 0;
+  if (sh.mode == 2) {
+    const TopkShard::Batch b0 = sh.batch(0);  // the largest block
+    if ((rc = c->x_send.ensure(sh.block_bytes(b0))) || (rc = c->x_state.ensure(sh.state_bytes(b0)))) return rc;
+    if (c->comm && (rc = c->x_recv.ensure(sh.block_bytes(b0) * sh.n_ranks))) return rc;
+  }
+  for (uint32_t b = 0; b < sh.n_batches; ++b) {
+    for (uint32_t r = 0; r < sh.rounds; ++r) {
+      if ((rc = shard_candidates(c, sh, b, r, bottom, vals, valid, ix, tie, T, c->x_state.p, c->x_send.p))) return rc;
+      const void* gathered = c->x_send.p;
+      if (c->comm) {
+        const TopkShard::Batch bt = sh.batch(b);
+        const size_t n_slots = (size_t)bt.nx * bt.nt * sh.K * 32, n_units = (size_t)bt.nx * bt.nt * 32;
+        const ShardBlock s = shard_block(sh, bt, c->x_send.p, 1), g = shard_block(sh, bt, c->x_recv.p, sh.n_ranks);
+        NCCL_TRY(g_nccl.GroupStart());
+        NCCL_TRY(g_nccl.AllGather(s.hi, g.hi, n_slots, Nccl::kUint64, c->comm, c->stream));
+        NCCL_TRY(g_nccl.AllGather(s.lo, g.lo, n_slots, Nccl::kUint32, c->comm, c->stream));
+        NCCL_TRY(g_nccl.AllGather(s.n, g.n, n_units, Nccl::kUint32, c->comm, c->stream));
+        NCCL_TRY(g_nccl.GroupEnd());
+        gathered = c->x_recv.p;
+      }
+      if ((rc = shard_merge(c, sh, b, r, gathered, c->x_state.p, T))) return rc;
+    }
+    if ((rc = shard_mark(c, sh, b, bottom, vals, valid, ix, tie, T, c->x_state.p, out_valid))) return rc;
+  }
+  return B2P_OK;
+}
+
+// Argument checks of the per-rank steps: the exchange of (k, sizes, T, n_ranks), and batch / round inside it
+int shard_check(b2p_ctx* c, double k, const uint32_t* sizes, uint32_t n_groups, uint64_t T, int32_t n_ranks,
+                uint32_t batch, uint32_t round, bool rounds, TopkShard& sh) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (int rc = shard_plan(c, k, sizes, n_groups, T, n_ranks, sh)) return rc;
+  if (batch >= sh.n_batches) return fail(B2P_E_INVALID, "batch %u of %u", batch, sh.n_batches);
+  if (rounds && round >= sh.rounds) return fail(B2P_E_INVALID, "round %u of %u", round, sh.rounds);
   return B2P_OK;
 }
 
@@ -405,6 +665,68 @@ int b2p_topk_dev(b2p_ctx* c, int32_t bottom, double k, const double* vals, const
 int b2p_topk_i64_dev(b2p_ctx* c, int32_t bottom, double k, const int64_t* vals, const uint32_t* valid,
                      const b2p_group_index* ix, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
   return topk_dev(c, bottom, k, reinterpret_cast<const double*>(vals), valid, ix, tie, T, out_valid, true);
+}
+
+/* ---- topk / bottomk over sharded rows ------------------------------------------------------------------------- */
+
+int b2p_topk_shard_plan(b2p_ctx* c, double k, const uint32_t* group_sizes, uint32_t n_groups, uint64_t T,
+                        int32_t n_ranks, uint32_t* n_batches, uint32_t* n_rounds, uint32_t* slots,
+                        uint64_t* block_bytes, uint64_t* state_bytes) {
+  TopkShard sh;
+  if (int rc = shard_check(c, k, group_sizes, n_groups, T, n_ranks, 0, 0, false, sh)) return rc;
+  if (!n_batches || !n_rounds || !slots || !block_bytes || !state_bytes) return fail(B2P_E_INVALID, "NULL argument");
+  *n_batches = sh.n_batches; *n_rounds = sh.rounds; *slots = sh.K;
+  *block_bytes = sh.mode == 2 ? sh.block_bytes(sh.batch(0)) : 0;
+  *state_bytes = sh.mode == 2 ? sh.state_bytes(sh.batch(0)) : 0;
+  return B2P_OK;
+}
+
+int b2p_topk_shard_candidates_dev(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uint32_t* valid,
+                                  const b2p_group_index* ix, const uint32_t* tie, uint64_t T,
+                                  const uint32_t* group_sizes, int32_t n_ranks, uint32_t batch, uint32_t round,
+                                  void* state, void* block) {
+  if (!ix) return fail(B2P_E_INVALID, "NULL argument");
+  TopkShard sh;
+  if (int rc = shard_check(c, k, group_sizes, ix->n_groups, T, n_ranks, batch, round, true, sh)) return rc;
+  if ((ix->n_series && (!vals || !valid || !tie)) || !state || !block) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  c->last_exchange_bytes = 0;
+  return shard_candidates(c, sh, batch, round, bottom, vals, valid, ix, tie, T, state, block);
+}
+
+int b2p_topk_shard_merge_dev(b2p_ctx* c, double k, const uint32_t* group_sizes, uint32_t n_groups, uint64_t T,
+                             int32_t n_ranks, uint32_t batch, uint32_t round, const void* blocks, void* state) {
+  TopkShard sh;
+  if (int rc = shard_check(c, k, group_sizes, n_groups, T, n_ranks, batch, round, true, sh)) return rc;
+  if (!blocks || !state) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  return shard_merge(c, sh, batch, round, blocks, state, T);
+}
+
+int b2p_topk_shard_mark_dev(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uint32_t* valid,
+                            const b2p_group_index* ix, const uint32_t* tie, uint64_t T, const uint32_t* group_sizes,
+                            int32_t n_ranks, uint32_t batch, const void* state, uint32_t* out_valid) {
+  if (!ix) return fail(B2P_E_INVALID, "NULL argument");
+  TopkShard sh;
+  if (int rc = shard_check(c, k, group_sizes, ix->n_groups, T, n_ranks, batch, 0, false, sh)) return rc;
+  if (ix->n_series && (!vals || !valid || !tie || !out_valid)) return fail(B2P_E_INVALID, "NULL argument");
+  if (sh.mode == 2 && !state) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  return shard_mark(c, sh, batch, bottom, vals, valid, ix, tie, T, state, out_valid);
+}
+
+int b2p_topk_allgather_dev(b2p_ctx* c, int32_t bottom, double k, const double* vals, const uint32_t* valid,
+                           const b2p_group_index* ix, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_series && (!vals || !valid || !tie || !out_valid)) return fail(B2P_E_INVALID, "NULL argument");
+  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
+  c->last_exchange_bytes = 0;
+  if (T == 0) return B2P_OK;  // (every rank has the same T)
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  const int rc = topk_allgather_run(c, bottom, k, vals, valid, ix, tie, T, out_valid);
+  stage_end(c, 3);
+  return rc;
 }
 
 /* ---- quantile ------------------------------------------------------------------------------------------------ */

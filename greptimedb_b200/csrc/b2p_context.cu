@@ -100,6 +100,7 @@ b2p_ctx* b2p_create(int device) {
   if (const char* e = getenv("B2P_COMM_RESERVE_SMS")) c->comm_reserve_sms = atoi(e);
   if (const char* e = getenv("B2P_COMM_HEADSTART_US")) c->comm_headstart_cycles = (long long)(atof(e) * 1980.0);
   if (const char* e = getenv("B2P_ARENA_ROWS")) c->arena_rows_wanted = (size_t)strtoull(e, nullptr, 10);
+  if (const char* e = getenv("B2P_TOPK_EXCHANGE_BYTES")) c->topk_exchange_cap = (size_t)strtoull(e, nullptr, 10);
   return c;
 }
 
@@ -144,6 +145,7 @@ int b2p_use_own_stream(b2p_ctx* c) {
 
 int64_t b2p_last_slow_series(b2p_ctx* c) { return c ? c->last_slow : -1; }
 int64_t b2p_last_h2d_bytes(b2p_ctx* c) { return c ? c->last_h2d_bytes : -1; }
+int64_t b2p_last_exchange_bytes(b2p_ctx* c) { return c ? c->last_exchange_bytes : -1; }
 int64_t b2p_last_warp_tier_series(b2p_ctx* c) { return c ? c->last_w : -1; }
 int64_t b2p_launch_count(b2p_ctx* c) { return c ? c->launches : -1; }
 

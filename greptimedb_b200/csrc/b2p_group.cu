@@ -114,6 +114,9 @@ int b2p_group_index_create_dev(b2p_ctx* c, const uint32_t* gid, uint32_t n_serie
   if (!rc && n_series) {
     cudaMemcpyAsync(ix->gid, gid, (size_t)n_series * 4, cudaMemcpyDeviceToDevice, c->stream);
     rc = build_group_csr(c, ix->gid, n_series, n_groups, ix->goff, ix->members);
+  } else if (!rc) {  // no rows: every group is empty (a rank of a sharded topk may hold none)
+    const cudaError_t e = cudaMemsetAsync(ix->goff, 0, ((size_t)n_groups + 1) * 4, c->stream);
+    if (e != cudaSuccess) rc = fail(B2P_E_CUDA, "group index offsets: %s", cudaGetErrorString(e));
   }
   if (!rc) {
     // largest group (host-side scan of the offsets: the index is built once per label assignment)

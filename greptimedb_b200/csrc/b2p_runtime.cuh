@@ -37,7 +37,7 @@ int k0_fail(uint32_t k0);
 
 // NCCL, bound at run time: libnccl.so.2 is not a link dependency (single-GPU users never need it), and inside a
 // process that already loaded an NCCL (e.g. the one bundled with torch) dlopen hands back that same library.
-// Only the handful of entry points the by-label all-reduce needs; enum values are NCCL's ABI (nccl.h).
+// Only the handful of entry points the by-label all-reduce and the sharded topk need; enum values are NCCL's ABI (nccl.h).
 struct Nccl {
   typedef struct ncclComm* comm_t;
   struct unique_id { char internal[128]; };
@@ -47,6 +47,7 @@ struct Nccl {
   int (*CommInitRank)(comm_t*, int, unique_id, int) = nullptr;
   int (*CommDestroy)(comm_t) = nullptr;
   int (*AllReduce)(const void*, void*, size_t, int, int, comm_t, cudaStream_t) = nullptr;
+  int (*AllGather)(const void*, void*, size_t, int, comm_t, cudaStream_t) = nullptr;
   int (*GroupStart)() = nullptr;
   int (*GroupEnd)() = nullptr;
   const char* (*GetErrorString)(int) = nullptr;
@@ -66,6 +67,7 @@ struct Nccl {
     CommInitRank = reinterpret_cast<decltype(CommInitRank)>(sym("ncclCommInitRank"));
     CommDestroy = reinterpret_cast<decltype(CommDestroy)>(sym("ncclCommDestroy"));
     AllReduce = reinterpret_cast<decltype(AllReduce)>(sym("ncclAllReduce"));
+    AllGather = reinterpret_cast<decltype(AllGather)>(sym("ncclAllGather"));
     GroupStart = reinterpret_cast<decltype(GroupStart)>(sym("ncclGroupStart"));
     GroupEnd = reinterpret_cast<decltype(GroupEnd)>(sym("ncclGroupEnd"));
     GetErrorString = reinterpret_cast<decltype(GetErrorString)>(sym("ncclGetErrorString"));
@@ -228,6 +230,11 @@ struct b2p_ctx {
   DevBuf ab_acc;
   // topk / bottomk: chunk and merge tables, candidate lists, selection state (b2p_topk.cuh; bound in topk_run)
   DevBuf t_table, t_cand, t_state;
+  // sharded topk (b2p_aggregation.cu, shard_*): the merge table over the ranks' blocks, the group sizes all-reduced by
+  // b2p_topk_allgather_dev, its candidate block, the gathered blocks and the selection state of one batch
+  DevBuf x_table, x_size, x_send, x_recv, x_state;
+  size_t topk_exchange_cap = size_t(128) << 20;  // bytes of blocks and state per batch (B2P_TOPK_EXCHANGE_BYTES)
+  long long last_exchange_bytes = 0;             // candidate bytes of this rank's blocks in the last sharded topk
   // quantile: chunk table, state and histograms of the groups of several chunks (b2p_quantile.cuh; bound in quantile_run)
   DevBuf q_table, q_state, q_hist;
   // count_values: key and sorted-key buffers, ranks and starts, segment tables, member groups, CUB's temp (bound in

@@ -30,6 +30,12 @@
 // ceil(kk / kTopkMax) rounds the kk-th best key is known, and topk_select_kernel reads the values once more and keeps
 // every cell at or above it.  Groups of at most kk members keep every valid cell and take no part in the rounds.
 // Cost: ceil(kk / 32) + 1 reads of the group's cells; measured in DESIGN.md section 4.
+//
+// Sharded (b2p_topk_shard_*, b2p_topk_allgather_dev): a rank is one more kind of chunk.  The chunk kernel leaves each
+// local chunk's list, topk_merge_kernel in export mode (x_hi set) writes the rank's best K of a group below the bound
+// into a candidate block instead of taking a verdict, the blocks of every rank are gathered, and topk_merge_kernel
+// with a stride (the groups of one block apart) takes the verdict over the ranks' blocks.  tile0 shifts every kernel
+// to tiles [tile0, tile0 + tiles), so scratch and blocks cover one batch of tiles at a time.
 #pragma once
 #include <cstdint>
 
@@ -48,8 +54,8 @@ constexpr uint32_t kTopkAll = 2u;          // state flag: every valid cell of th
 // (groups of several chunks) or kTopkNone; state: the group's selection state (several chunks, or the general path)
 // or kTopkNone.
 struct TopkChunk { uint32_t begin, end, cand, state; };
-// A group of several chunks: candidate blocks [cand_begin, cand_end), all of its chunks
-struct TopkMerge { uint32_t cand_begin, cand_end, state, pad; };
+// A group of several chunks: candidate blocks cand_begin, cand_begin + stride, .. below cand_end
+struct TopkMerge { uint32_t cand_begin, cand_end, state, stride; };
 
 struct TopkArgs {
   const double* vals;      // [rows x T]
@@ -62,6 +68,7 @@ struct TopkArgs {
   uint32_t n_merges;
   uint64_t T;
   uint32_t Tw, tiles;
+  uint32_t tile0;          // the tiles run are [tile0, tile0 + tiles); scratch is indexed by tile - tile0
   uint32_t K;              // heap slots per lane: kk on the fast path, kTopkMax on the general path
   uint32_t kk;
   int bottom;
@@ -78,6 +85,11 @@ struct TopkArgs {
   uint32_t* s_rem;
   uint32_t* s_flags;
   uint32_t* out_valid;     // [rows x Tw]; may be valid
+  // export mode of topk_merge_kernel (sharded): a merge's best K below the bound, [merge][tile][slot][lane], and their
+  // count [merge][tile][lane], written instead of the verdict
+  unsigned long long* x_hi;
+  uint32_t* x_lo;
+  uint32_t* x_n;
 };
 
 template <class Key>
@@ -175,8 +187,8 @@ __device__ void topk_verdict(const TopkArgs& a, uint64_t si, TopkState st, TopkH
   a.s_rem[si] = st.rem; a.s_flags[si] = st.flags; a.s_hi[si] = st.hi; a.s_lo[si] = st.lo;
 }
 
-// The words of members [begin, end) for one tile from a list of n kept-or-not entries (pos at [s * 32], lane-offset):
-// keep(s) decides; a word has the bit of every lane whose list holds the member and keeps it
+// The words of members [begin, end) for one tile of the grid from a list of n kept-or-not entries (pos at [s * 32],
+// lane-offset): keep(s) decides; a word has the bit of every lane whose list holds the member and keeps it
 template <class Keep>
 __device__ void topk_write_words(const TopkArgs& a, uint32_t* sw, const uint32_t* pos, uint32_t n, uint32_t begin,
                                  uint32_t end, uint32_t tile, int lane, Keep keep) {
@@ -199,7 +211,8 @@ template <class Key>
 __device__ __forceinline__ uint32_t topk_stream(const TopkArgs& a, const TopkChunk& ch, uint32_t tile, int lane,
                                                 bool want, const TopkState& st, TopkHeap& h) {
   constexpr uint32_t kAhead = 8;
-  const uint64_t step = (uint64_t)tile * 32 + lane;
+  const uint32_t gt = a.tile0 + tile;
+  const uint64_t step = (uint64_t)gt * 32 + lane;
   const bool bounded = (st.flags & kTopkBound) != 0;
   uint32_t n = 0;
   unsigned long long th = 0;
@@ -209,7 +222,7 @@ __device__ __forceinline__ uint32_t topk_stream(const TopkArgs& a, const TopkChu
     const uint32_t j = m0 + lane;
     const bool in = j < ch.end;
     const uint32_t row = in ? __ldg(a.members + j) : 0u;
-    const uint32_t w = in ? __ldg(a.valid + (uint64_t)row * a.Tw + tile) : 0u;
+    const uint32_t w = in ? __ldg(a.valid + (uint64_t)row * a.Tw + gt) : 0u;
     const uint32_t t = in ? __ldg(a.tie + row) : 0u;
     const uint32_t nb = min(32u, ch.end - m0);
     for (uint32_t i0 = 0; i0 < nb; i0 += kAhead) {
@@ -257,7 +270,7 @@ __global__ void __launch_bounds__(kTopkWarps * 32) topk_chunk_kernel(const TopkA
     const uint32_t c = (uint32_t)(u / a.tiles), tile = (uint32_t)(u - (uint64_t)c * a.tiles);
     const TopkChunk ch = a.chunks[c];
     if (a.general && ch.state == kTopkNone) continue;
-    const bool live = (uint64_t)tile * 32 + lane < a.T;
+    const bool live = (uint64_t)(a.tile0 + tile) * 32 + lane < a.T;
     const uint64_t si = ch.state != kTopkNone ? ((uint64_t)ch.state * a.tiles + tile) * 32 + lane : 0;
     const TopkState st = ch.state != kTopkNone ? topk_state_load(a, si) : TopkState{a.kk, 0u, 0ull, 0u};
     const uint32_t n = topk_stream<Key>(a, ch, tile, lane, live && !st.done(), st, h);
@@ -271,13 +284,14 @@ __global__ void __launch_bounds__(kTopkWarps * 32) topk_chunk_kernel(const TopkA
     } else if (a.general) {
       if (live) topk_verdict(a, si, st, h, n);
     } else {  // the whole group: every listed cell is kept
-      topk_write_words(a, sw, h.pos, n, ch.begin, ch.end, tile, lane, [](uint32_t) { return true; });
+      topk_write_words(a, sw, h.pos, n, ch.begin, ch.end, a.tile0 + tile, lane, [](uint32_t) { return true; });
     }
     __syncwarp();  // the heap is reused by the next unit
   }
 }
 
-// One warp per (multi-chunk group, tile): the best K of the chunks' lists, then the round's verdict
+// One warp per (multi-chunk group, tile): the best K of the chunks' lists, then the round's verdict, or in export mode
+// the best K themselves
 __global__ void __launch_bounds__(kTopkWarps * 32) topk_merge_kernel(const TopkArgs a) {
   extern __shared__ __align__(16) unsigned char topk_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -286,7 +300,10 @@ __global__ void __launch_bounds__(kTopkWarps * 32) topk_merge_kernel(const TopkA
   const uint64_t n_warps = (uint64_t)gridDim.x * kTopkWarps;
   for (uint64_t u = (uint64_t)blockIdx.x * kTopkWarps + warp; u < units; u += n_warps) {
     const uint32_t m = (uint32_t)(u / a.tiles), tile = (uint32_t)(u - (uint64_t)m * a.tiles);
-    if ((uint64_t)tile * 32 + lane >= a.T) continue;  // (no shuffles below)
+    if ((uint64_t)(a.tile0 + tile) * 32 + lane >= a.T) {  // (no shuffles below)
+      if (a.x_n) a.x_n[((uint64_t)m * a.tiles + tile) * 32 + lane] = 0u;
+      continue;
+    }
     const TopkMerge g = a.merges[m];
     const uint64_t si = ((uint64_t)g.state * a.tiles + tile) * 32 + lane;
     const TopkState st = topk_state_load(a, si);
@@ -297,28 +314,36 @@ __global__ void __launch_bounds__(kTopkWarps * 32) topk_merge_kernel(const TopkA
       // kAhead candidates (and the next list's count) are loaded before any is offered: one memory latency per batch
       constexpr uint32_t kAhead = 16;
       uint32_t cn = g.cand_begin < g.cand_end ? a.c_n[((uint64_t)g.cand_begin * a.tiles + tile) * 32 + lane] : 0u;
-      for (uint32_t c = g.cand_begin; c < g.cand_end; ++c) {
+      for (uint32_t c = g.cand_begin; c < g.cand_end; c += g.stride) {
         const uint64_t cb = (uint64_t)c * a.tiles + tile;
-        const uint32_t cn_next = c + 1 < g.cand_end ? a.c_n[(cb + a.tiles) * 32 + lane] : 0u;
+        const uint32_t cn_next = c + g.stride < g.cand_end ? a.c_n[(cb + (uint64_t)g.stride * a.tiles) * 32 + lane] : 0u;
         for (uint32_t s0 = 0; s0 < cn; s0 += kAhead) {
           unsigned long long ch[kAhead];
-          uint32_t cl[kAhead], cp[kAhead];
+          uint32_t cl[kAhead];
 #pragma unroll
           for (uint32_t q = 0; q < kAhead; ++q) {
             const uint64_t i = (cb * a.K + s0 + q) * 32 + lane;
             const bool in = s0 + q < cn;
             ch[q] = in ? a.c_hi[i] : 0ull;
             cl[q] = in ? a.c_lo[i] : 0u;
-            cp[q] = in ? a.c_pos[i] : 0u;
           }
 #pragma unroll
-          for (uint32_t q = 0; q < kAhead; ++q)
-            if (s0 + q < cn) h.offer(n, a.K, th, tl, ch[q], cl[q], cp[q]);
+          for (uint32_t q = 0; q < kAhead; ++q)  // (a verdict reads keys only: the member position is not carried)
+            if (s0 + q < cn) h.offer(n, a.K, th, tl, ch[q], cl[q], 0u);
         }
         cn = cn_next;
       }
     }
-    topk_verdict(a, si, st, h, n);
+    if (a.x_hi) {
+      const uint64_t xb = (uint64_t)m * a.tiles + tile;
+      for (uint32_t s = 0; s < n; ++s) {
+        a.x_hi[(xb * a.K + s) * 32 + lane] = h.hi[s * 32];
+        a.x_lo[(xb * a.K + s) * 32 + lane] = h.lo[s * 32];
+      }
+      a.x_n[xb * 32 + lane] = n;
+    } else {
+      topk_verdict(a, si, st, h, n);
+    }
   }
 }
 
@@ -333,7 +358,7 @@ __global__ void __launch_bounds__(kTopkWarps * 32) topk_mark_kernel(const TopkAr
     const uint32_t c = (uint32_t)(u / a.tiles), tile = (uint32_t)(u - (uint64_t)c * a.tiles);
     const TopkChunk ch = a.chunks[c];
     if (ch.cand == kTopkNone) continue;
-    const bool live = (uint64_t)tile * 32 + lane < a.T;
+    const bool live = (uint64_t)(a.tile0 + tile) * 32 + lane < a.T;
     const uint64_t si = ((uint64_t)ch.state * a.tiles + tile) * 32 + lane;
     const uint64_t cb = (uint64_t)ch.cand * a.tiles + tile;
     const uint32_t n = live ? a.c_n[cb * 32 + lane] : 0u;
@@ -341,7 +366,7 @@ __global__ void __launch_bounds__(kTopkWarps * 32) topk_mark_kernel(const TopkAr
     const unsigned long long th = live ? a.s_hi[si] : 0ull;
     const uint32_t tl = live ? a.s_lo[si] : 0u;
     const uint64_t base = cb * a.K * 32 + lane;
-    topk_write_words(a, sw_all[warp], a.c_pos + base, n, ch.begin, ch.end, tile, lane, [&](uint32_t s) {
+    topk_write_words(a, sw_all[warp], a.c_pos + base, n, ch.begin, ch.end, a.tile0 + tile, lane, [&](uint32_t s) {
       return all || !key_less(a.c_hi[base + (uint64_t)s * 32], a.c_lo[base + (uint64_t)s * 32], th, tl);
     });
   }
@@ -358,7 +383,8 @@ __global__ void __launch_bounds__(256, 1) topk_select_kernel(const TopkArgs a) {
   for (uint64_t u = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; u < units; u += n_warps) {
     const uint32_t c = (uint32_t)(u / a.tiles), tile = (uint32_t)(u - (uint64_t)c * a.tiles);
     const TopkChunk ch = a.chunks[c];
-    const uint64_t step = (uint64_t)tile * 32 + lane;
+    const uint32_t gt = a.tile0 + tile;
+    const uint64_t step = (uint64_t)gt * 32 + lane;
     const bool live = step < a.T;
     bool all = true;
     unsigned long long th = 0;
@@ -368,12 +394,12 @@ __global__ void __launch_bounds__(256, 1) topk_select_kernel(const TopkArgs a) {
       all = (a.s_flags[si] & kTopkAll) != 0;
       th = a.s_hi[si]; tl = a.s_lo[si];
     }
-    const uint32_t live_bits = a.T - (uint64_t)tile * 32 >= 32 ? 0xFFFFFFFFu : (1u << (a.T - (uint64_t)tile * 32)) - 1u;
+    const uint32_t live_bits = a.T - (uint64_t)gt * 32 >= 32 ? 0xFFFFFFFFu : (1u << (a.T - (uint64_t)gt * 32)) - 1u;
     for (uint32_t m0 = ch.begin; m0 < ch.end; m0 += 32) {
       const uint32_t j = m0 + lane;
       const bool in = j < ch.end;
       const uint32_t row = in ? __ldg(a.members + j) : 0u;
-      const uint32_t w = in ? a.valid[(uint64_t)row * a.Tw + tile] & live_bits : 0u;
+      const uint32_t w = in ? a.valid[(uint64_t)row * a.Tw + gt] & live_bits : 0u;
       const uint32_t t = in ? __ldg(a.tie + row) : 0u;
       const uint32_t nb = min(32u, ch.end - m0);
       uint32_t mine = w;  // groups that keep every cell
@@ -406,7 +432,7 @@ __global__ void __launch_bounds__(256, 1) topk_select_kernel(const TopkArgs a) {
         }
       }
       __syncwarp();
-      if (in) a.out_valid[(uint64_t)row * a.Tw + tile] = mine;
+      if (in) a.out_valid[(uint64_t)row * a.Tw + gt] = mine;
     }
   }
 }

@@ -111,6 +111,104 @@ def merge_partials(agg: str, val_t, cnt_t, mean_t=None, group=None):
     return val_t, cnt_t
 
 
+def topk_key_host(bottom: bool, vals: np.ndarray, tie: np.ndarray):
+    """The rank key of every cell of K10, (hi, lo) = (f64 total-order key as u64, tie), both bit-inverted for bottomk so
+    that better is always larger."""
+    b = np.ascontiguousarray(vals, np.float64).view(np.uint64)
+    hi = np.where(b >> np.uint64(63) != 0, ~b, b | np.uint64(1 << 63))
+    lo = np.broadcast_to(np.asarray(tie, np.uint32)[:, None], hi.shape)
+    return (~hi, ~lo) if bottom else (hi, lo.copy())
+
+
+def merge_topk_candidates(bottom: bool, kk: int, vals: np.ndarray, ok: np.ndarray, gid: np.ndarray, n_groups: int,
+                          tie: np.ndarray, group=None, slots_max: int = 32):
+    """Host mirror of b2p_topk_allgather_dev (same exchange, torch.distributed instead of the library's NCCL
+    communicator; used by the gloo tests): this rank's rows [R, T] (ok: valid cells, gid >= n_groups: no group, tie
+    distinct across every rank) -> (kept [R, T] bool, exchanged group count, rounds, slots).
+      - the per-group member counts are all-reduced; kk = 0 keeps nothing, kk >= the largest group every valid cell, a
+        group of at most kk members every valid cell;
+      - every other group is exchanged: per round and step each rank sends its best min(kk, slots_max) keys below the
+        bound and their count, all-gathered; the merge's verdict is "all" (fewer than that many left, within what is
+        still to take), the threshold (the rem-th best), or the next bound (the smallest of the slots taken);
+      - each rank keeps its own valid cells at or above the threshold, or every one below the bounds taken ("all")."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    R, T = vals.shape
+    gid = np.asarray(gid, np.int64)
+    ing = gid < n_groups
+    local = np.bincount(gid[ing], minlength=n_groups).astype(np.int64)
+    sizes_t = torch.from_numpy(local.copy())
+    dist.all_reduce(sizes_t, op=dist.ReduceOp.SUM, group=group)
+    sizes = sizes_t.numpy()
+    kept = np.zeros((R, T), bool)
+    if kk == 0 or n_groups == 0:
+        return kept, 0, 0, 0
+    if kk >= sizes.max():
+        kept[ing] = ok[ing]
+        return kept, 0, 0, 0
+    small = ing & (sizes[np.where(ing, gid, 0)] <= kk)
+    kept[small] = ok[small]
+    xg = np.flatnonzero(sizes > kk)
+    K = min(kk, slots_max)
+    rounds = -(-kk // slots_max) if kk > slots_max else 1
+    hi, lo = topk_key_host(bottom, vals, tie)
+    X = xg.size
+    rem = np.full((X, T), kk, np.int64)
+    done = np.zeros((X, T), bool)                   # "all": every cell below the bound is kept
+    th_hi = np.zeros((X, T), np.uint64)             # bound (rounds) / threshold (rem == 0)
+    th_lo = np.zeros((X, T), np.uint32)
+    bounded = np.zeros((X, T), bool)
+    members = [np.flatnonzero(gid == g) for g in xg]
+
+    def below(h, l, i):  # cells strictly below the bound of group i
+        return ~bounded[i] | (h < th_hi[i]) | ((h == th_hi[i]) & (l < th_lo[i]))
+
+    for _ in range(rounds):
+        s_hi = np.zeros((X, T, K), np.uint64)
+        s_lo = np.zeros((X, T, K), np.uint32)
+        s_n = np.zeros((X, T), np.int64)
+        for i, rows in enumerate(members):
+            if rows.size == 0:
+                continue
+            h, l = hi[rows], lo[rows]
+            live = ok[rows] & below(h, l, i) & ~done[i] & (rem[i] > 0)
+            order = np.lexsort((l, h, live), axis=0)[::-1]   # live first, then the best
+            n = np.minimum(live.sum(axis=0), K)
+            take = min(K, rows.size)
+            s_hi[i, :, :take] = np.take_along_axis(h, order[:take], axis=0).T
+            s_lo[i, :, :take] = np.take_along_axis(l, order[:take], axis=0).T
+            s_n[i] = n
+        parts = []
+        for t in (torch.from_numpy(s_hi.view(np.int64)), torch.from_numpy(s_lo.astype(np.int64)), torch.from_numpy(s_n)):
+            out = [torch.empty_like(t) for _ in range(world)]
+            dist.all_gather(out, t, group=group)
+            parts.append([o.numpy() for o in out])
+        g_hi = np.concatenate([p.view(np.uint64) for p in parts[0]], axis=2)      # [X, T, world * K]
+        g_lo = np.concatenate([p.astype(np.uint32) for p in parts[1]], axis=2)
+        g_on = np.concatenate([np.arange(K)[None, None, :] < p[:, :, None] for p in parts[2]], axis=2)
+        order = np.lexsort((g_lo, g_hi, g_on), axis=2)[:, :, ::-1]
+        n = np.minimum(g_on.sum(axis=2), K)
+        active = ~done & (rem > 0)
+        fits = active & (n < K) & (n <= rem)
+        cut = active & ~fits & (rem <= n)
+        more = active & ~fits & ~cut
+        done |= fits
+        j = np.clip(np.where(cut, rem, K) - 1, 0, None)[:, :, None]
+        pick_hi = np.take_along_axis(np.take_along_axis(g_hi, order, axis=2), j, axis=2)[:, :, 0]
+        pick_lo = np.take_along_axis(np.take_along_axis(g_lo, order, axis=2), j, axis=2)[:, :, 0]
+        upd = cut | more
+        th_hi[upd], th_lo[upd] = pick_hi[upd], pick_lo[upd]
+        bounded |= more
+        rem[cut] = 0
+        rem[more] -= K
+    for i, rows in enumerate(members):
+        h, l = hi[rows], lo[rows]
+        at_or_above = (h > th_hi[i]) | ((h == th_hi[i]) & (l >= th_lo[i]))
+        kept[rows] = ok[rows] & np.where(done[i], True, at_or_above)
+    return kept, X, rounds, K
+
+
 def partial_state_host(agg: str, vals: np.ndarray, valid: np.ndarray, gid: np.ndarray, n_groups: int):
     """Host mirror of b2p_group_aggregate_partial_dev for stddev / stdvar: (M2, cnt, mean) per (group, step), Welford in
     series order like the by-label kernel."""

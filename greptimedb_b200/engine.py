@@ -750,6 +750,42 @@ class Context:
         self._check(self._L.b2p_topk_dev(self._h, topk_bottom(op), float(k), _ptr(vals), _ptr(valid), index, _ptr(tie),
                                          T, _ptr(out_valid)))
 
+    def topk_allgather_dev(self, op, k, vals, valid, index, tie, T, out_valid):
+        """topk / bottomk over rows sharded across the ranks of the context's communicator (or one rank without one):
+        this rank's kept cells into out_valid; tie must be distinct across every rank."""
+        self._check(self._L.b2p_topk_allgather_dev(self._h, topk_bottom(op), float(k), _ptr(vals), _ptr(valid), index,
+                                                   _ptr(tie), T, _ptr(out_valid)))
+
+    def last_exchange_bytes(self) -> int:
+        return int(self._L.b2p_last_exchange_bytes(self._h))
+
+    def topk_shard_plan(self, k, group_sizes, T, n_ranks) -> dict:
+        """The exchange of a sharded topk from the global member count of every group (host u32 [n_groups])."""
+        sizes = np.ascontiguousarray(group_sizes, np.uint32)
+        out = [C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint64(), C.c_uint64()]
+        self._check(self._L.b2p_topk_shard_plan(self._h, float(k), _ptr(sizes), sizes.size, T, n_ranks,
+                                                *[C.byref(o) for o in out]))
+        names = ("n_batches", "n_rounds", "slots", "block_bytes", "state_bytes")
+        return {n: int(o.value) for n, o in zip(names, out)}
+
+    def topk_shard_candidates_dev(self, op, k, vals, valid, index, tie, T, group_sizes, n_ranks, batch, rnd, state,
+                                  block):
+        sizes = np.ascontiguousarray(group_sizes, np.uint32)
+        self._check(self._L.b2p_topk_shard_candidates_dev(self._h, topk_bottom(op), float(k), _ptr(vals), _ptr(valid),
+                                                          index, _ptr(tie), T, _ptr(sizes), n_ranks, batch, rnd,
+                                                          _ptr(state), _ptr(block)))
+
+    def topk_shard_merge_dev(self, k, group_sizes, T, n_ranks, batch, rnd, blocks, state):
+        sizes = np.ascontiguousarray(group_sizes, np.uint32)
+        self._check(self._L.b2p_topk_shard_merge_dev(self._h, float(k), _ptr(sizes), sizes.size, T, n_ranks, batch, rnd,
+                                                     _ptr(blocks), _ptr(state)))
+
+    def topk_shard_mark_dev(self, op, k, vals, valid, index, tie, T, group_sizes, n_ranks, batch, state, out_valid):
+        sizes = np.ascontiguousarray(group_sizes, np.uint32)
+        self._check(self._L.b2p_topk_shard_mark_dev(self._h, topk_bottom(op), float(k), _ptr(vals), _ptr(valid), index,
+                                                    _ptr(tie), T, _ptr(sizes), n_ranks, batch, _ptr(state),
+                                                    _ptr(out_valid)))
+
     def group_quantile_dev(self, phi, vals, valid, index, T, out_val, out_cnt):
         """quantile(phi) over the rows of a group index (group_index_create_dev) into out_val / out_cnt [G,T]."""
         self._check(self._L.b2p_group_quantile_dev(self._h, float(phi), _ptr(vals), _ptr(valid), index, T,

@@ -435,6 +435,60 @@ B2P_API int b2p_absent_dev(b2p_ctx* ctx, const uint32_t* valid, uint32_t n_rows,
 B2P_API int b2p_topk_dev(b2p_ctx* ctx, int32_t bottom, double k, const double* vals, const uint32_t* valid,
                          const b2p_group_index* index, const uint32_t* tie, uint64_t T, uint32_t* out_valid);
 
+/* topk / bottomk over rows sharded across ranks (Float64 only).  Every rank passes its own rows as for b2p_topk_dev: its
+ * index over the same n_groups global group ids, and tie values distinct across ALL ranks (the row's global ordinal in
+ * the op's direction, derived from the label tuples by the caller); each series lies whole on one rank.  On return (stream
+ * order) out_valid holds this rank's kept cells, and the union over the ranks is bit for bit what b2p_topk_dev writes
+ * over the concatenation of every rank's rows with the same gid and tie.
+ *
+ * kk is the rank count of b2p_topk_dev's k.  From the global member count of each group: kk = 0 keeps nothing, kk >= the
+ * largest group keeps every valid cell, and otherwise a group of at most kk members keeps every valid cell and the
+ * others (G_x groups, "exchanged") are exchanged.  Per (exchanged group, step) and round, each rank sends its best
+ * slots = min(kk, 32) keys (f64 total-order key and tie, 12 B) below the previous round's bound plus a 4-byte count; a
+ * merge over the ranks' blocks finds the kk-th best key, and each rank keeps its own cells at or above it: the global
+ * top kk of a group are among the union of each rank's own top kk.  kk <= 32 takes one round and marks the kept cells
+ * from the rank's own candidates; kk > 32 takes ceil(kk / 32) rounds and then reads the values once more.
+ * The (exchanged group, 32-step tile) units are cut into batches whose blocks and state fit the context's cap
+ * (128 MB; B2P_TOPK_EXCHANGE_BYTES at b2p_create, which must be the same on every rank).
+ *
+ * b2p_topk_allgather_dev: the whole call over the context's communicator: one all-reduce of the n_groups x 4 B member
+ * counts and one read-back of them (synchronises once), then per batch and round three ncclAllGather calls in one group.
+ * Without a communicator and n_ranks == 1 (no b2p_comm_init) it gives b2p_topk_dev's words.  b2p_last_exchange_bytes()
+ * then gives the bytes of this rank's candidate blocks:
+ *     rounds x G_x x 32 ceil(T / 32) x (12 slots + 4),
+ * 0 when no group has more than kk members globally (the all-reduce of the counts is not included).
+ *
+ * The steps it is built from, so that one GPU can run R ranks (one context each) through the same kernels.  group_sizes
+ * is a HOST array of the n_groups global member counts; every step derives the same exchange from (k, group_sizes, T,
+ * n_ranks).  b2p_topk_shard_plan gives n_batches, n_rounds (0 without exchanged groups), slots, and the largest block
+ * and state of a batch in bytes (0 without exchanged groups).  Then, for every batch b and round r < n_rounds:
+ *   b2p_topk_shard_candidates_dev on every rank writes its block (block_bytes of b2p_topk_shard_plan suffice; the
+ *     batch's own size is nx x nt x 32 x (12 slots + 4) for its nx groups and nt tiles): three sections, keys hi
+ *     [u x slots x 32] u64, ties [u x slots x 32] u32, counts [u x 32] u32 for u = nx x nt units; reads state after
+ *     round 0;
+ *   the blocks are gathered section by section: [hi of rank 0 .. R-1][ties of rank 0 .. R-1][counts of rank 0 .. R-1];
+ *   b2p_topk_shard_merge_dev over the gathered blocks writes the batch's state (state_bytes, device);
+ * and b2p_topk_shard_mark_dev(b) on every rank writes its words of batch b from that state; batch 0 also writes every
+ * word the exchange does not decide.  A rank's mark must follow its own last candidates step of the batch on the same
+ * context (its candidate lists stay in context scratch), before the next batch's. */
+B2P_API int b2p_topk_allgather_dev(b2p_ctx* ctx, int32_t bottom, double k, const double* vals, const uint32_t* valid,
+                                   const b2p_group_index* index, const uint32_t* tie, uint64_t T, uint32_t* out_valid);
+B2P_API int64_t b2p_last_exchange_bytes(b2p_ctx* ctx);
+B2P_API int b2p_topk_shard_plan(b2p_ctx* ctx, double k, const uint32_t* group_sizes, uint32_t n_groups, uint64_t T,
+                                int32_t n_ranks, uint32_t* n_batches, uint32_t* n_rounds, uint32_t* slots,
+                                uint64_t* block_bytes, uint64_t* state_bytes);
+B2P_API int b2p_topk_shard_candidates_dev(b2p_ctx* ctx, int32_t bottom, double k, const double* vals,
+                                          const uint32_t* valid, const b2p_group_index* index, const uint32_t* tie,
+                                          uint64_t T, const uint32_t* group_sizes, int32_t n_ranks, uint32_t batch,
+                                          uint32_t round, void* state, void* block);
+B2P_API int b2p_topk_shard_merge_dev(b2p_ctx* ctx, double k, const uint32_t* group_sizes, uint32_t n_groups,
+                                     uint64_t T, int32_t n_ranks, uint32_t batch, uint32_t round, const void* blocks,
+                                     void* state);
+B2P_API int b2p_topk_shard_mark_dev(b2p_ctx* ctx, int32_t bottom, double k, const double* vals, const uint32_t* valid,
+                                    const b2p_group_index* index, const uint32_t* tie, uint64_t T,
+                                    const uint32_t* group_sizes, int32_t n_ranks, uint32_t batch, const void* state,
+                                    uint32_t* out_valid);
+
 /* quantile(phi, v) by label (K11, QuantileAccumulator::evaluate, src/promql/src/functions/quantile_aggr.rs:110-116 over
  * quantile_with_scratch, quantile.rs:201-225): per (group, step) the n valid cells of the index's member rows; phi NaN
  * gives NaN, phi < 0 -inf, phi > 1 +inf; otherwise, sorted by f64::total_cmp, rank = phi (n - 1), lo = floor(rank),

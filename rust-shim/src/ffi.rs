@@ -348,6 +348,33 @@ extern "C" {
         ctx: *mut b2p_ctx, bottom: i32, k: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index,
         tie: *const u32, t: u64, out_valid: *mut u32,
     ) -> c_int;
+    /// topk / bottomk over rows sharded across the communicator's ranks: this rank's kept cells; `tie` distinct across
+    /// every rank.  Without a communicator (one rank) the words of `b2p_topk_dev`.
+    pub fn b2p_topk_allgather_dev(
+        ctx: *mut b2p_ctx, bottom: i32, k: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index,
+        tie: *const u32, t: u64, out_valid: *mut u32,
+    ) -> c_int;
+    /// Bytes of this rank's candidate blocks in the last sharded topk.
+    pub fn b2p_last_exchange_bytes(ctx: *mut b2p_ctx) -> i64;
+    /// The steps of the sharded topk; `group_sizes` is a host array of the global member counts [n_groups].
+    pub fn b2p_topk_shard_plan(
+        ctx: *mut b2p_ctx, k: f64, group_sizes: *const u32, n_groups: u32, t: u64, n_ranks: i32, n_batches: *mut u32,
+        n_rounds: *mut u32, slots: *mut u32, block_bytes: *mut u64, state_bytes: *mut u64,
+    ) -> c_int;
+    pub fn b2p_topk_shard_candidates_dev(
+        ctx: *mut b2p_ctx, bottom: i32, k: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index,
+        tie: *const u32, t: u64, group_sizes: *const u32, n_ranks: i32, batch: u32, round: u32, state: *mut c_void,
+        block: *mut c_void,
+    ) -> c_int;
+    pub fn b2p_topk_shard_merge_dev(
+        ctx: *mut b2p_ctx, k: f64, group_sizes: *const u32, n_groups: u32, t: u64, n_ranks: i32, batch: u32,
+        round: u32, blocks: *const c_void, state: *mut c_void,
+    ) -> c_int;
+    pub fn b2p_topk_shard_mark_dev(
+        ctx: *mut b2p_ctx, bottom: i32, k: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index,
+        tie: *const u32, t: u64, group_sizes: *const u32, n_ranks: i32, batch: u32, state: *const c_void,
+        out_valid: *mut u32,
+    ) -> c_int;
     /// quantile(phi) per (group, step) into out_val / out_cnt [n_groups x T]; cnt 0 = no row.
     pub fn b2p_group_quantile_dev(
         ctx: *mut b2p_ctx, phi: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index, t: u64,
