@@ -159,11 +159,18 @@ def binary_rows(lhs, rhs, op, return_bool=False, on=None, ignoring=None, label_s
     return (list(ltags) if from_lhs else list(rtags)), out
 
 
+def scalar_value(op, scalar, v, scalar_on_left=False, return_bool=False):
+    """One cell `v op scalar` (or `scalar op v`) -> value, or None when a filtering comparison drops it; a filter keeps
+    the vector's value on either side."""
+    out, ov = scalar_op(op, scalar, np.array([[v]], np.float64), np.array([[1]], np.uint32), scalar_on_left, return_bool)
+    return float(out[0, 0]) if ov[0, 0] & 1 else None
+
+
 def scalar_rows(rows, op, scalar, scalar_on_left=False, return_bool=False):
     """Row-literal `rows op scalar` (or `scalar op rows`): a projection, or a filter keeping the vector's value."""
     out = []
     for r in rows:
-        v = binary_value(op, scalar, r[-1], return_bool) if scalar_on_left else binary_value(op, r[-1], scalar, return_bool)
+        v = scalar_value(op, scalar, r[-1], scalar_on_left, return_bool)
         if v is not None:
             out.append(tuple(r[:-1]) + (v,))
     return out
