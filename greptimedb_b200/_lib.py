@@ -47,6 +47,8 @@ EXPORTED_SYMBOLS = [
     "b2p_plan_set_label_columns",
     "b2p_topk_allgather_dev", "b2p_last_exchange_bytes", "b2p_topk_shard_plan", "b2p_topk_shard_candidates_dev",
     "b2p_topk_shard_merge_dev", "b2p_topk_shard_mark_dev",
+    "b2p_quantile_allreduce_dev", "b2p_quantile_shard_plan", "b2p_quantile_shard_pass_dev",
+    "b2p_quantile_shard_advance_dev",
 ]
 
 
@@ -204,6 +206,10 @@ def load() -> C.CDLL:
         "b2p_topk_shard_candidates_dev": (C.c_int, [vp, i32, dbl, vp, vp, vp, vp, u64, vp, i32, u32, u32, vp, vp]),
         "b2p_topk_shard_merge_dev": (C.c_int, [vp, dbl, vp, u32, u64, i32, u32, u32, vp, vp]),
         "b2p_topk_shard_mark_dev": (C.c_int, [vp, i32, dbl, vp, vp, vp, vp, u64, vp, i32, u32, vp, vp]),
+        "b2p_quantile_allreduce_dev": (C.c_int, [vp, dbl, vp, vp, vp, u64, vp, vp]),
+        "b2p_quantile_shard_plan": (C.c_int, [vp, u32, u64, C.POINTER(u32), C.POINTER(u64), C.POINTER(u64)]),
+        "b2p_quantile_shard_pass_dev": (C.c_int, [vp, dbl, vp, vp, vp, u64, u32, u32, vp]),
+        "b2p_quantile_shard_advance_dev": (C.c_int, [vp, dbl, u32, u64, u32, u32, vp, u32, vp, vp, C.POINTER(u64)]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)  # AttributeError here means the .so does not match the header

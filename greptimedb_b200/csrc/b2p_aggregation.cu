@@ -136,6 +136,18 @@ int topk_run(b2p_ctx* c, int bottom, uint32_t kk, const double* vals, const uint
   return B2P_OK;
 }
 
+// Cuts X items x `tiles` tiles into batches of at most `fit` (item, tile) units: every tile of every item when they fit,
+// else every item x as many tiles as fit, else `fit` items x 1 tile -> xb items and tb tiles per batch
+void cut_batches(uint64_t X, uint32_t tiles, uint64_t fit, uint32_t& xb, uint32_t& tb) {
+  if (X * tiles <= fit) {
+    xb = (uint32_t)X; tb = tiles;
+  } else if (X <= fit) {
+    xb = (uint32_t)X; tb = (uint32_t)(fit / X);
+  } else {
+    xb = (uint32_t)fit; tb = 1;
+  }
+}
+
 // ---- sharded topk / bottomk: the rows of every rank, one exchange of candidates ---------------------------------------
 // The exchange is derived from kk, T, the rank count and the global group sizes only, so every rank derives the same
 // batches and block sizes.  Exchanged groups (G_x) are the groups of more than kk members globally, in id order.  The
@@ -175,14 +187,7 @@ int shard_plan(const b2p_ctx* c, double k, const uint32_t* sizes, uint32_t n_gro
   sh.rounds = sh.kk > kTopkMax ? (sh.kk + kTopkMax - 1) / kTopkMax : 1;
   const uint64_t X = sh.xg.size();
   const uint64_t unit = (uint64_t)(sh.n_ranks + 1) * 32 * sh.slot_bytes() + 32 * 20;  // send, gathered, state
-  const uint64_t fit = std::max<uint64_t>(1, c->topk_exchange_cap / unit);
-  if (X * sh.tiles <= fit) {
-    sh.xb = (uint32_t)X; sh.tb = sh.tiles;
-  } else if (X <= fit) {
-    sh.xb = (uint32_t)X; sh.tb = (uint32_t)(fit / X);
-  } else {
-    sh.xb = (uint32_t)fit; sh.tb = 1;
-  }
+  cut_batches(X, sh.tiles, std::max<uint64_t>(1, c->topk_exchange_cap / unit), sh.xb, sh.tb);
   sh.n_xb = (uint32_t)((X + sh.xb - 1) / sh.xb);
   sh.n_tb = (sh.tiles + sh.tb - 1) / sh.tb;
   sh.n_batches = sh.n_xb * sh.n_tb;
@@ -397,8 +402,7 @@ int shard_check(b2p_ctx* c, double k, const uint32_t* sizes, uint32_t n_groups, 
 }
 
 template <class Kern>
-int quantile_launch(b2p_ctx* c, Kern* kern, uint64_t units, const QuantArgs& a) {
-  const size_t smem = kQuantWarps * kQuantWarpBytes;
+int quantile_launch(b2p_ctx* c, Kern* kern, size_t smem, uint64_t units, const QuantArgs& a) {
   unsigned grid = 0;
   if (int rc = persistent_grid(c, kern, smem, kQuantWarps, units, &grid)) return rc;
   if (grid == 0) return B2P_OK;
@@ -427,11 +431,11 @@ int quantile_run(b2p_ctx* c, double phi, const double* vals, const uint32_t* val
   a.T = T; a.Tw = Tw; a.tiles = Tw; a.phi = phi;
   a.count_only = !(phi >= 0.0 && phi <= 1.0) ? 1 : 0;
   a.out_val = out_val; a.out_cnt = out_cnt;
-  if ((rc = quantile_launch(c, quantile_resident_kernel, (uint64_t)G * Tw, a))) return rc;
+  const size_t smem = kQuantWarps * kQuantWarpBytes;
+  if ((rc = quantile_launch(c, quantile_resident_kernel, smem, (uint64_t)G * Tw, a))) return rc;
   if (a.count_only || ix->max_members <= kQuantResident) return B2P_OK;
   unsigned cap = 0;
-  if ((rc = persistent_grid(c, quantile_pass_kernel, kQuantWarps * kQuantWarpBytes, kQuantWarps, kAllResident, &cap)))
-    return rc;
+  if ((rc = persistent_grid(c, quantile_pass_kernel<8>, smem, kQuantWarps, kAllResident, &cap))) return rc;
   const uint64_t resident = (uint64_t)cap * kQuantWarps, U = resident - resident / 8;
   uint64_t large = 0;
   for (uint32_t g = 0; g < G; ++g) {
@@ -474,11 +478,153 @@ int quantile_run(b2p_ctx* c, double phi, const double* vals, const uint32_t* val
   const uint64_t units = (uint64_t)chunks.size() * Tw;
   for (uint32_t p = 0; p < (a.n_slots ? kQuantPasses : 1u); ++p) {
     a.pass = (int)p;
-    if ((rc = quantile_launch(c, quantile_pass_kernel, units, a))) return rc;
+    if ((rc = quantile_launch(c, quantile_pass_kernel<8>, smem, units, a))) return rc;
     if (!a.n_slots) break;
-    quantile_advance_kernel<<<capped_grid(c, (uint64_t)a.n_slots * T, 256, 8), 256, 0, c->stream>>>(a);
+    quantile_advance_kernel<8><<<capped_grid(c, (uint64_t)a.n_slots * T, 256, 8), 256, 0, c->stream>>>(a);
     c->launches++;
     CU(cudaGetLastError());
+  }
+  return B2P_OK;
+}
+
+// ---- sharded quantile: the rows of every rank, one all-reduce of digit counts per pass ----------------------------------
+// The 4-bit select of b2p_quantile.cuh over the union of the ranks' rows.  Every rank derives the same batches from
+// (n_groups, T, topk_exchange_cap): the (group, tile) units are cut into batches whose block (kUnitBlock per unit) and
+// state (kUnitState per unit) fit the cap.  Batch b covers tiles [t0, t0 + nt) of groups [g0, g0 + ng).  Its block is
+// [counts: units x 16 x 32 u32][r_lo: units x 32 u64][r_hi: units x 32 u64]; its state [units x 32] QuantState.
+struct QuantShard {
+  static constexpr uint64_t kCountBytes = (1u << kQuantShardBits) * 32 * 4;
+  static constexpr uint64_t kUnitBlock = kCountBytes + 2 * 32 * 8;  // 2 560 B
+  static constexpr uint64_t kUnitState = 32 * sizeof(QuantState);   // 1 792 B
+  uint32_t n_groups = 0, tiles = 0, gb = 1, tb = 1, n_gb = 0, n_batches = 0;
+  struct Batch {
+    uint32_t g0, ng, t0, nt;
+    uint64_t units() const { return (uint64_t)ng * nt; }
+  };
+  Batch batch(uint32_t b) const {
+    const uint32_t g0 = (b % n_gb) * gb, t0 = (b / n_gb) * tb;
+    return Batch{g0, std::min(gb, n_groups - g0), t0, std::min(tb, tiles - t0)};
+  }
+};
+static_assert(QuantShard::kUnitBlock == 2560, "b200promql.h states 2 560 B per (group, tile) unit and pass");
+
+QuantShard quantile_shard_plan(const b2p_ctx* c, uint32_t n_groups, uint64_t T) {
+  QuantShard sh;
+  sh.n_groups = n_groups;
+  sh.tiles = (uint32_t)((T + 31) / 32);
+  if (n_groups == 0 || T == 0) return sh;  // no batch
+  const uint64_t fit = std::max<uint64_t>(1, c->topk_exchange_cap / (QuantShard::kUnitBlock + QuantShard::kUnitState));
+  cut_batches(n_groups, sh.tiles, fit, sh.gb, sh.tb);
+  sh.n_gb = (n_groups + sh.gb - 1) / sh.gb;
+  sh.n_batches = sh.n_gb * ((sh.tiles + sh.tb - 1) / sh.tb);
+  return sh;
+}
+
+// The arguments both steps share: the batch, the state and the sections of a block
+QuantArgs quantile_shard_args(const QuantShard& sh, const QuantShard::Batch& bt, double phi, uint64_t T, void* state,
+                              void* block) {
+  QuantArgs a{};
+  a.T = T; a.Tw = sh.tiles; a.tiles = bt.nt; a.tile0 = bt.t0; a.group0 = bt.g0; a.n_slots = bt.ng;
+  a.phi = phi;
+  a.count_only = !(phi >= 0.0 && phi <= 1.0) ? 1 : 0;
+  a.state = static_cast<QuantState*>(state);
+  a.hist = static_cast<uint32_t*>(block);
+  a.r_lo = reinterpret_cast<unsigned long long*>(static_cast<char*>(block) + bt.units() * QuantShard::kCountBytes);
+  a.r_hi = a.r_lo + bt.units() * 32;
+  return a;
+}
+
+// Per-rank step: zeroes the block (counts and r_lo 0, r_hi ~0; pass 0 also clears the batch's state), then this rank's
+// chunks of the batch's groups add one pass's counts or extremes into it.  Chunks are cut as quantile_run cuts them.
+int quantile_shard_pass(b2p_ctx* c, const QuantShard& sh, uint32_t b, uint32_t pass, double phi, const double* vals,
+                        const uint32_t* valid, const b2p_group_index* ix, uint64_t T, void* block) {
+  int rc;
+  const QuantShard::Batch bt = sh.batch(b);
+  const uint64_t units = bt.units();
+  if (pass == 0) {
+    if ((rc = c->qx_state.ensure(units * QuantShard::kUnitState))) return rc;
+    CU(cudaMemsetAsync(c->qx_state.p, 0, units * QuantShard::kUnitState, c->stream));
+  }
+  char* blk = static_cast<char*>(block);
+  CU(cudaMemsetAsync(blk, 0, units * (QuantShard::kCountBytes + 32 * 8), c->stream));
+  CU(cudaMemsetAsync(blk + units * (QuantShard::kCountBytes + 32 * 8), 0xFF, units * 32 * 8, c->stream));
+  c->last_exchange_bytes += (long long)(units * QuantShard::kUnitBlock);
+  const size_t smem = kQuantWarps * quant_pass_warp_bytes<kQuantShardBits>();
+  unsigned cap = 0;
+  if ((rc = persistent_grid(c, quantile_pass_kernel<kQuantShardBits>, smem, kQuantWarps, kAllResident, &cap))) return rc;
+  const uint64_t resident = (uint64_t)cap * kQuantWarps, U = resident - resident / 8;
+  uint64_t members = 0;
+  for (uint32_t g = bt.g0; g < bt.g0 + bt.ng; ++g) members += ix->goff_host[g + 1] - ix->goff_host[g];
+  const uint64_t C = std::min<uint64_t>(kQuantChunkMax, std::max<uint64_t>(256, (members * bt.nt + U - 1) / U));
+  std::vector<QuantChunk> chunks;
+  for (uint32_t i = 0; i < bt.ng; ++i) {
+    const uint32_t g = bt.g0 + i, gb = ix->goff_host[g], s = ix->goff_host[g + 1] - gb;
+    const uint32_t nc = (uint32_t)((s + C - 1) / C);
+    for (uint32_t j = 0; j < nc; ++j)
+      chunks.push_back(QuantChunk{gb + (uint32_t)((uint64_t)s * j / nc), gb + (uint32_t)((uint64_t)s * (j + 1) / nc), g, i});
+  }
+  if (chunks.empty()) return B2P_OK;  // no member of the batch's groups on this rank: its block stays zero
+  const size_t tb_chunks = chunks.size() * sizeof(QuantChunk);
+  if ((rc = c->qx_table.ensure(tb_chunks))) return rc;
+  CU(cudaMemcpyAsync(c->qx_table.p, chunks.data(), tb_chunks, cudaMemcpyHostToDevice, c->stream));
+  QuantArgs a = quantile_shard_args(sh, bt, phi, T, c->qx_state.p, block);
+  a.vals = vals; a.valid = valid; a.members = ix->members;
+  a.chunks = c->qx_table.as<QuantChunk>(); a.n_chunks = (uint32_t)chunks.size();
+  return quantile_launch(c, quantile_pass_kernel<kQuantShardBits>, smem, (uint64_t)a.n_chunks * bt.nt, a);
+}
+
+// Merge step: the n_blocks blocks of the batch (the batch's block size apart) advance this context's state; finished
+// cells are written to out_val / out_cnt, and *live receives the count of the others (read back: synchronises)
+int quantile_shard_advance(b2p_ctx* c, const QuantShard& sh, uint32_t b, double phi, uint64_t T, const void* blocks,
+                           uint32_t n_blocks, double* out_val, uint32_t* out_cnt, uint64_t* live) {
+  int rc;
+  const QuantShard::Batch bt = sh.batch(b);
+  const uint64_t units = bt.units();
+  if (c->qx_state.cap < units * QuantShard::kUnitState)
+    return fail(B2P_E_INVALID, "no selection state for batch %u: its pass 0 runs first on this context", b);
+  if ((rc = c->qx_live.ensure(8))) return rc;
+  QuantArgs a = quantile_shard_args(sh, bt, phi, T, c->qx_state.p, const_cast<void*>(blocks));
+  a.block_stride = units * QuantShard::kUnitBlock;
+  a.n_blocks = n_blocks;
+  a.live = c->qx_live.as<unsigned long long>();
+  a.out_val = out_val; a.out_cnt = out_cnt;
+  CU(cudaMemsetAsync(a.live, 0, 8, c->stream));
+  quantile_advance_kernel<kQuantShardBits><<<capped_grid(c, units * 32, 256, 8), 256, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  unsigned long long left = 0;
+  CU(cudaMemcpyAsync(&left, a.live, 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  *live = left;
+  return B2P_OK;
+}
+
+// The composed call: per batch and pass, this rank's block, one group of three in-place all-reduces (counts SUM, r_lo
+// MAX, r_hi MIN), and the advance over the one merged block, until no cell is left.  Without a communicator (one rank)
+// the block is its own merge.
+int quantile_allreduce_run(b2p_ctx* c, double phi, const double* vals, const uint32_t* valid, const b2p_group_index* ix,
+                           uint64_t T, double* out_val, uint32_t* out_cnt) {
+  int rc;
+  const QuantShard sh = quantile_shard_plan(c, ix->n_groups, T);
+  if (sh.n_batches && (rc = c->x_send.ensure(sh.batch(0).units() * QuantShard::kUnitBlock))) return rc;
+  for (uint32_t b = 0; b < sh.n_batches; ++b) {
+    const uint64_t units = sh.batch(b).units();
+    for (uint32_t p = 0; p < kQuantShardPasses; ++p) {
+      if ((rc = quantile_shard_pass(c, sh, b, p, phi, vals, valid, ix, T, c->x_send.p))) return rc;
+      if (c->comm) {
+        char* blk = c->x_send.as<char>();
+        void* r_lo = blk + units * QuantShard::kCountBytes;
+        void* r_hi = blk + units * (QuantShard::kCountBytes + 32 * 8);
+        NCCL_TRY(g_nccl.GroupStart());
+        NCCL_TRY(g_nccl.AllReduce(blk, blk, units * (1u << kQuantShardBits) * 32, Nccl::kUint32, Nccl::kSum, c->comm, c->stream));
+        NCCL_TRY(g_nccl.AllReduce(r_lo, r_lo, units * 32, Nccl::kUint64, Nccl::kMax, c->comm, c->stream));
+        NCCL_TRY(g_nccl.AllReduce(r_hi, r_hi, units * 32, Nccl::kUint64, Nccl::kMin, c->comm, c->stream));
+        NCCL_TRY(g_nccl.GroupEnd());
+      }
+      uint64_t live = 0;
+      if ((rc = quantile_shard_advance(c, sh, b, phi, T, c->x_send.p, 1, out_val, out_cnt, &live))) return rc;
+      if (live == 0) break;  // from the merged state alone, so every rank stops after the same pass
+    }
   }
   return B2P_OK;
 }
@@ -739,6 +885,57 @@ int b2p_group_quantile_dev(b2p_ctx* c, double phi, const double* vals, const uin
   DeviceGuard g(c->device);
   stage_begin(c, 3);
   const int rc = quantile_run(c, phi, vals, valid, ix, T, out_val, out_cnt);
+  stage_end(c, 3);
+  return rc;
+}
+
+/* ---- quantile over sharded rows ------------------------------------------------------------------------------ */
+
+int b2p_quantile_shard_plan(b2p_ctx* c, uint32_t n_groups, uint64_t T, uint32_t* n_batches, uint64_t* block_bytes,
+                            uint64_t* state_bytes) {
+  if (!c || !n_batches || !block_bytes || !state_bytes) return fail(B2P_E_INVALID, "NULL argument");
+  const QuantShard sh = quantile_shard_plan(c, n_groups, T);
+  *n_batches = sh.n_batches;
+  *block_bytes = sh.n_batches ? sh.batch(0).units() * QuantShard::kUnitBlock : 0;
+  *state_bytes = sh.n_batches ? sh.batch(0).units() * QuantShard::kUnitState : 0;
+  return B2P_OK;
+}
+
+int b2p_quantile_shard_pass_dev(b2p_ctx* c, double phi, const double* vals, const uint32_t* valid,
+                                const b2p_group_index* ix, uint64_t T, uint32_t batch, uint32_t pass, void* block) {
+  if (!c || !ix || !block) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_series && (!vals || !valid)) return fail(B2P_E_INVALID, "NULL argument");
+  const QuantShard sh = quantile_shard_plan(c, ix->n_groups, T);
+  if (batch >= sh.n_batches) return fail(B2P_E_INVALID, "batch %u of %u", batch, sh.n_batches);
+  if (pass >= kQuantShardPasses) return fail(B2P_E_INVALID, "pass %u of at most %u", pass, kQuantShardPasses);
+  DeviceGuard g(c->device);
+  c->last_exchange_bytes = 0;
+  return quantile_shard_pass(c, sh, batch, pass, phi, vals, valid, ix, T, block);
+}
+
+int b2p_quantile_shard_advance_dev(b2p_ctx* c, double phi, uint32_t n_groups, uint64_t T, uint32_t batch, uint32_t pass,
+                                   const void* blocks, uint32_t n_blocks, double* out_val, uint32_t* out_cnt,
+                                   uint64_t* live) {
+  if (!c || !blocks || !out_val || !out_cnt || !live) return fail(B2P_E_INVALID, "NULL argument");
+  if (n_blocks == 0) return fail(B2P_E_INVALID, "n_blocks is 0");
+  const QuantShard sh = quantile_shard_plan(c, n_groups, T);
+  if (batch >= sh.n_batches) return fail(B2P_E_INVALID, "batch %u of %u", batch, sh.n_batches);
+  if (pass >= kQuantShardPasses) return fail(B2P_E_INVALID, "pass %u of at most %u", pass, kQuantShardPasses);
+  DeviceGuard g(c->device);
+  return quantile_shard_advance(c, sh, batch, phi, T, blocks, n_blocks, out_val, out_cnt, live);
+}
+
+int b2p_quantile_allreduce_dev(b2p_ctx* c, double phi, const double* vals, const uint32_t* valid,
+                               const b2p_group_index* ix, uint64_t T, double* out_val, uint32_t* out_cnt) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if ((ix->n_series && (!vals || !valid)) || (ix->n_groups && T && (!out_val || !out_cnt)))
+    return fail(B2P_E_INVALID, "NULL argument");
+  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
+  c->last_exchange_bytes = 0;
+  if (ix->n_groups == 0 || T == 0) return B2P_OK;  // (every rank has the same n_groups and T)
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  const int rc = quantile_allreduce_run(c, phi, vals, valid, ix, T, out_val, out_cnt);
   stage_end(c, 3);
   return rc;
 }

@@ -233,10 +233,14 @@ struct b2p_ctx {
   // sharded topk (b2p_aggregation.cu, shard_*): the merge table over the ranks' blocks, the group sizes all-reduced by
   // b2p_topk_allgather_dev, its candidate block, the gathered blocks and the selection state of one batch
   DevBuf x_table, x_size, x_send, x_recv, x_state;
-  size_t topk_exchange_cap = size_t(128) << 20;  // bytes of blocks and state per batch (B2P_TOPK_EXCHANGE_BYTES)
-  long long last_exchange_bytes = 0;             // candidate bytes of this rank's blocks in the last sharded topk
+  // bytes of blocks and state per batch of the sharded topk and of the sharded quantile (B2P_TOPK_EXCHANGE_BYTES)
+  size_t topk_exchange_cap = size_t(128) << 20;
+  long long last_exchange_bytes = 0;  // bytes of this rank's blocks in the last sharded topk or quantile
   // quantile: chunk table, state and histograms of the groups of several chunks (b2p_quantile.cuh; bound in quantile_run)
   DevBuf q_table, q_state, q_hist;
+  // sharded quantile (b2p_aggregation.cu, quantile_shard_*): this rank's chunk table of a batch, the batch's selection
+  // state (kept from pass to pass) and the count of cells left after an advance; the composed call's block is x_send
+  DevBuf qx_table, qx_state, qx_live;
   // count_values: key and sorted-key buffers, ranks and starts, segment tables, member groups, CUB's temp (bound in
   // count_values_run)
   DevBuf v_keys, v_alt, v_rank, v_seg, v_group, v_tmp;

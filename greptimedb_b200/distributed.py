@@ -231,3 +231,122 @@ def partial_state_host(agg: str, vals: np.ndarray, valid: np.ndarray, gid: np.nd
         mean[g, k] = nm
         cnt[g, k] += 1
     return m2, cnt, mean
+
+
+QUANT_SHARD_PASSES = 17                       # sixteen 4-bit digits, then one extreme pass
+QUANT_UNIT_BYTES = 16 * 32 * 4 + 2 * 32 * 8   # block bytes per (group, 32-step tile) and pass
+
+
+def merge_quantile_digits(phi, vals: np.ndarray, ok: np.ndarray, gid: np.ndarray, n_groups: int, group=None):
+    """Host mirror of b2p_quantile_allreduce_dev (same select, torch.distributed instead of the library's NCCL
+    communicator; used by the gloo tests): this rank's rows [R, T] (ok: valid cells, gid >= n_groups: no group) ->
+    (out [G, T] f64, cnt [G, T] u32, passes run, block bytes sent), the same on every rank.
+      - per (group, step) the state is a prefix of `level` fixed 4-bit digits of the key u = total_key ^ 2^63 and lo's
+        rank k among the keys under it; each pass every rank counts the next digit of its keys under the prefix (16
+        bins), or takes its largest key under p_lo and smallest under p_hi (the extreme pass);
+      - the counts are all-reduced by SUM as int64, the extremes by MAX / MIN as int64 after XOR with 2^63 (which keeps
+        the unsigned order), and every rank advances the same state from the merged block;
+      - the passes stop when no cell is left, at most 17; phi outside [0, 1] or NaN stops after the count."""
+    import math
+    import torch
+    import torch.distributed as dist
+    sign, full = np.uint64(1 << 63), np.uint64(0xFFFFFFFFFFFFFFFF)
+    vals = np.ascontiguousarray(vals, np.float64)
+    R, T = vals.shape
+    G = int(n_groups)
+    out = np.zeros((G, T), np.float64)
+    cnt = np.zeros((G, T), np.uint32)
+    if G == 0 or T == 0:
+        return out, cnt, 0, 0
+    bits = vals.view(np.uint64)
+    keys = np.where(bits >> np.uint64(63) != 0, ~bits, bits | sign)
+    gid = np.asarray(gid, np.int64)
+    rr, rt = np.nonzero(np.asarray(ok, bool) & (gid < G)[:, None])
+    rg, rk = gid[rr], keys[rr, rt]
+    count_only = not (0.0 <= phi <= 1.0)
+    mode = np.zeros((G, T), np.int64)             # 0 select, 1 extreme, 2 done
+    level = np.zeros((G, T), np.int64)
+    k = np.zeros((G, T), np.int64)
+    eq = np.zeros((G, T), bool)
+    p_lo = np.zeros((G, T), np.uint64)
+    p_hi = np.zeros((G, T), np.uint64)
+
+    def under(p, lv):
+        sh = np.minimum(64 - 4 * lv, 63).astype(np.uint64)
+        return (lv == 0) | ((rk >> sh) == (p >> sh))
+
+    def value(u):  # keys -> f64
+        return np.ascontiguousarray(np.where(u >> np.uint64(63) != 0, u ^ sign, ~u), np.uint64).view(np.float64)
+
+    passes = 0
+    for _ in range(QUANT_SHARD_PASSES):
+        passes += 1
+        cm, lv = mode[rg, rt], level[rg, rt]
+        sel = (cm == 0) & under(p_lo[rg, rt], lv)
+        dig = ((rk >> np.maximum(60 - 4 * lv, 0).astype(np.uint64)) & np.uint64(15)).astype(np.int64)
+        hist = np.zeros((G, T, 16), np.int64)
+        np.add.at(hist, (rg[sel], rt[sel], dig[sel]), 1)
+        lo_m = (cm == 1) & under(p_lo[rg, rt], lv)
+        hi_m = (cm == 1) & ~eq[rg, rt] & under(p_hi[rg, rt], lv)
+        r_lo = np.zeros((G, T), np.uint64)
+        r_hi = np.full((G, T), full, np.uint64)
+        np.maximum.at(r_lo, (rg[lo_m], rt[lo_m]), rk[lo_m])
+        np.minimum.at(r_hi, (rg[hi_m], rt[hi_m]), rk[hi_m])
+        h_t = torch.from_numpy(hist)
+        lo_t = torch.from_numpy((r_lo ^ sign).view(np.int64))
+        hi_t = torch.from_numpy((r_hi ^ sign).view(np.int64))
+        dist.all_reduce(h_t, op=dist.ReduceOp.SUM, group=group)
+        dist.all_reduce(lo_t, op=dist.ReduceOp.MAX, group=group)
+        dist.all_reduce(hi_t, op=dist.ReduceOp.MIN, group=group)
+        hist = h_t.numpy()
+        r_lo = lo_t.numpy().view(np.uint64) ^ sign
+        r_hi = hi_t.numpy().view(np.uint64) ^ sign
+        for g, t in zip(*np.nonzero(mode != 2)):
+            if mode[g, t] == 1:                   # the extremes are s[lo] and s[hi]
+                p_lo[g, t] = r_lo[g, t]
+                p_hi[g, t] = r_lo[g, t] if eq[g, t] else r_hi[g, t]
+                mode[g, t] = 2
+                continue
+            bins = [int(c) for c in hist[g, t]]
+            if level[g, t] == 0:
+                n = sum(bins)
+                cnt[g, t] = n
+                if n == 0 or count_only:
+                    mode[g, t] = 2
+                    continue
+                k[g, t] = min(math.floor(phi * float(n - 1)), n - 1)
+                if k[g, t] == n - 1:              # hi = lo: the largest key
+                    mode[g, t], eq[g, t] = 1, True
+                    continue
+            kk, cum, blo, bhi, klo = int(k[g, t]), 0, 16, 15, 0
+            for b, c in enumerate(bins):
+                if blo == 16 and cum + c > kk:
+                    blo, klo = b, kk - cum
+                if cum + c > kk + 1:
+                    bhi = b
+                    break
+                cum += c
+            shift = np.uint64(60 - 4 * int(level[g, t]))
+            p_hi[g, t] = p_lo[g, t] | (np.uint64(bhi) << shift)
+            p_lo[g, t] |= np.uint64(blo) << shift
+            k[g, t] = klo
+            level[g, t] += 1
+            if blo == bhi:
+                if level[g, t] == 16:
+                    p_hi[g, t] = p_lo[g, t]
+                    mode[g, t] = 2
+            else:
+                mode[g, t] = 2 if level[g, t] == 16 else 1
+        if (mode != 2).sum() == 0:
+            break
+    has = cnt > 0
+    if count_only:
+        out[has] = np.nan if math.isnan(phi) else (-np.inf if phi < 0 else np.inf)
+    else:  # s[lo] (1 - w) + s[hi] w, each operation rounded (no FMA), one group's row at a time
+        for g in range(G):
+            rank = np.float64(phi) * (np.maximum(cnt[g], 1) - 1).astype(np.float64)
+            w = rank - np.floor(rank)
+            with np.errstate(invalid="ignore", over="ignore"):
+                res = value(p_lo[g]) * (np.float64(1.0) - w) + value(p_hi[g]) * w
+            out[g] = np.where(has[g], res, 0.0)
+    return out, cnt, passes, passes * G * ((T + 31) // 32) * QUANT_UNIT_BYTES

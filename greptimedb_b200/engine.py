@@ -791,6 +791,30 @@ class Context:
         self._check(self._L.b2p_group_quantile_dev(self._h, float(phi), _ptr(vals), _ptr(valid), index, T,
                                                    _ptr(out_val), _ptr(out_cnt)))
 
+    def quantile_allreduce_dev(self, phi, vals, valid, index, T, out_val, out_cnt):
+        """quantile(phi) by label over rows sharded across the ranks of the context's communicator (or one rank without
+        one): every rank's out_val / out_cnt [G,T] receive the result over the union of the ranks' rows."""
+        self._check(self._L.b2p_quantile_allreduce_dev(self._h, float(phi), _ptr(vals), _ptr(valid), index, T,
+                                                       _ptr(out_val), _ptr(out_cnt)))
+
+    def quantile_shard_plan(self, n_groups, T) -> dict:
+        """The batches of a sharded quantile: n_batches and the largest block and state of a batch in bytes."""
+        out = [C.c_uint32(), C.c_uint64(), C.c_uint64()]
+        self._check(self._L.b2p_quantile_shard_plan(self._h, n_groups, T, *[C.byref(o) for o in out]))
+        return {n: int(o.value) for n, o in zip(("n_batches", "block_bytes", "state_bytes"), out)}
+
+    def quantile_shard_pass_dev(self, phi, vals, valid, index, T, batch, pss, block):
+        """This rank's block of one pass of a batch (pass 0 also clears the context's state of the batch)."""
+        self._check(self._L.b2p_quantile_shard_pass_dev(self._h, float(phi), _ptr(vals), _ptr(valid), index, T, batch,
+                                                        pss, _ptr(block)))
+
+    def quantile_shard_advance_dev(self, phi, n_groups, T, batch, pss, blocks, n_blocks, out_val, out_cnt) -> int:
+        """Merges n_blocks blocks, advances the context's state and writes the finished cells -> cells left."""
+        live = C.c_uint64()
+        self._check(self._L.b2p_quantile_shard_advance_dev(self._h, float(phi), n_groups, T, batch, pss, _ptr(blocks),
+                                                           n_blocks, _ptr(out_val), _ptr(out_cnt), C.byref(live)))
+        return int(live.value)
+
     def count_values_dev(self, vals, valid, index, T, out_val, out_cnt):
         """count_values over the rows of a group index (group_index_create_dev) into out_val / out_cnt [rows,T], rows in
         the index's member order."""

@@ -499,6 +499,51 @@ B2P_API int b2p_topk_shard_mark_dev(b2p_ctx* ctx, int32_t bottom, double k, cons
 B2P_API int b2p_group_quantile_dev(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid,
                                    const b2p_group_index* index, uint64_t T, double* out_val, uint32_t* out_cnt);
 
+/* quantile(phi, v) by label over rows sharded across ranks (Float64 only).  Every rank passes its own rows as for
+ * b2p_group_quantile_dev, with an index over the same n_groups global group ids; each series lies whole on one rank.  On
+ * return (stream order) EVERY rank's out_val / out_cnt [n_groups x T] holds the full result, bit for bit what
+ * b2p_group_quantile_dev writes over the concatenation of every rank's rows.
+ *
+ * The select is K11's radix select on the 64-bit total-order key with 4-bit digits (16 bins).  Per pass each rank
+ * histograms the next digit of its keys under the current prefix into a block, the blocks are added (integer counts,
+ * so in any order), and every rank advances the same state from the merged counts: the rows never move.  The extreme
+ * pass merges the largest key under p_lo (MAX) and the smallest under p_hi (MIN).  A (group, step) is done after at most
+ * 17 passes (16 digits and the extreme pass); phi outside [0, 1] or NaN after one (the count).  Per (group, 32-step tile)
+ * unit and pass the block is 2 560 B: counts [16 x 32] u32, then r_lo [32] u64, then r_hi [32] u64, each section
+ * unit-major over the batch.  The units are cut into batches whose block and state (1 792 B per unit) fit the context's
+ * exchange cap (128 MB; B2P_TOPK_EXCHANGE_BYTES at b2p_create, which also bounds the sharded topk's exchange and must be
+ * the same on every rank).
+ *
+ * b2p_quantile_allreduce_dev: the whole call over the context's communicator: per batch and pass, the rank's block, one
+ * ncclGroupStart/End of three in-place ncclAllReduce calls (counts u32 SUM, r_lo u64 MAX, r_hi u64 MIN) and the
+ * advance, which reads back the count of unfinished cells (so each pass synchronises once).  A batch stops after the
+ * pass that leaves none; that count comes from the merged state alone, so every rank makes the same collective calls.
+ * Without a communicator and n_ranks == 1 (no b2p_comm_init) it gives b2p_group_quantile_dev's output.
+ * b2p_last_exchange_bytes() then gives the bytes of this rank's blocks: sum over batches of passes run x units x 2 560.
+ *
+ * The steps it is built from, so that one GPU can run R ranks (one context each) through the same kernels.
+ * b2p_quantile_shard_plan gives n_batches (0 when n_groups or T is 0) and the largest block and state of a batch in
+ * bytes.  Then for every batch b and pass p = 0, 1, .. < 17:
+ *   b2p_quantile_shard_pass_dev on every rank zeroes its block (the batch's block is units x 2 560 B, at most
+ *     block_bytes) and adds this rank's counts or extremes of the pass into it; pass 0 first clears the batch's
+ *     selection state, which the context keeps;
+ *   b2p_quantile_shard_advance_dev on every rank merges the n_blocks blocks laid one after another (each the batch's
+ *     block size; one all-reduced block, or every rank's block in any order), advances its context's state, writes the
+ *     cells it finishes into out_val / out_cnt and returns in *live (host) the count of cells still unfinished; it
+ *     synchronises the stream.  The batch is done after the pass whose live is 0.
+ * A rank's pass must follow its own previous advance on the same context.  B2P_E_INVALID: a NULL argument, a batch or
+ * pass out of range, n_blocks 0, an advance before its batch's pass 0 on the context, no communicator with n_ranks > 1. */
+B2P_API int b2p_quantile_allreduce_dev(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid,
+                                       const b2p_group_index* index, uint64_t T, double* out_val, uint32_t* out_cnt);
+B2P_API int b2p_quantile_shard_plan(b2p_ctx* ctx, uint32_t n_groups, uint64_t T, uint32_t* n_batches,
+                                    uint64_t* block_bytes, uint64_t* state_bytes);
+B2P_API int b2p_quantile_shard_pass_dev(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid,
+                                        const b2p_group_index* index, uint64_t T, uint32_t batch, uint32_t pass,
+                                        void* block);
+B2P_API int b2p_quantile_shard_advance_dev(b2p_ctx* ctx, double phi, uint32_t n_groups, uint64_t T, uint32_t batch,
+                                           uint32_t pass, const void* blocks, uint32_t n_blocks, double* out_val,
+                                           uint32_t* out_cnt, uint64_t* live);
+
 /* count_values(label, v) by label (K12; the reference's Aggregate(groupBy = [group labels.., ts, value], count(value)),
  * planner.rs:402-445): per (group, step) the distinct values of the valid cells of the index's member rows, a value
  * being its bits (-0.0 and +0.0 are two values, and so are NaNs with different bits), in the f64 total order.  Output

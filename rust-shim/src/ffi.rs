@@ -380,6 +380,25 @@ extern "C" {
         ctx: *mut b2p_ctx, phi: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index, t: u64,
         out_val: *mut f64, out_cnt: *mut u32,
     ) -> c_int;
+    /// quantile(phi) by label over rows sharded across the communicator's ranks: every rank receives the full
+    /// [n_groups x T] result.  Without a communicator (one rank) the output of `b2p_group_quantile_dev`.
+    pub fn b2p_quantile_allreduce_dev(
+        ctx: *mut b2p_ctx, phi: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index, t: u64,
+        out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    /// The steps of the sharded quantile: batches, then per batch and pass a rank's block and the advance over the
+    /// merged blocks (`live`: cells left, read back).
+    pub fn b2p_quantile_shard_plan(
+        ctx: *mut b2p_ctx, n_groups: u32, t: u64, n_batches: *mut u32, block_bytes: *mut u64, state_bytes: *mut u64,
+    ) -> c_int;
+    pub fn b2p_quantile_shard_pass_dev(
+        ctx: *mut b2p_ctx, phi: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index, t: u64,
+        batch: u32, pass: u32, block: *mut c_void,
+    ) -> c_int;
+    pub fn b2p_quantile_shard_advance_dev(
+        ctx: *mut b2p_ctx, phi: f64, n_groups: u32, t: u64, batch: u32, pass: u32, blocks: *const c_void,
+        n_blocks: u32, out_val: *mut f64, out_cnt: *mut u32, live: *mut u64,
+    ) -> c_int;
     /// count_values per (group, step) into out_val / out_cnt [n_series x T], rows in the index's member order: a group's
     /// j-th row holds its j-th smallest distinct value (by bits, f64 total order) and its multiplicity; cnt 0 = none.
     pub fn b2p_count_values_dev(
