@@ -14,7 +14,7 @@
 //     additionally drops the cell when the comparison is false, and a kept cell holds the vector operand's value (the lhs
 //     of a vector-vector pair).  An invalid cell holds 0.0.
 //   * `-fmad=false` and IEEE div: + - * / % and every comparison are bit-identical to the CPU; pow / atan2 are CUDA's
-//     (DESIGN.md section 2 states the bound against glibc).
+//     (DESIGN.md section 2 states the bound against glibc), except pow's cases where glibc is exact (pow_exact_cases).
 //
 // Work unit: one warp per (pair, 32-step tile) — one AND of the two validity words and one ballot per output word.  With
 // T even every row starts 16-byte aligned, and the VEC variant has each lane load two steps with one 128-bit access (a
@@ -68,6 +68,42 @@ __device__ __forceinline__ bool is_snan(double x) {
   return (u & 0x7FF8000000000000ull) == 0x7FF0000000000000ull && (u & 0x000FFFFFFFFFFFFFull) != 0;
 }
 
+// pow where glibc's is exact and CUDA's can be an ulp off (pow(19, 2) = 361.00000000000006, pow(2, -1012), 10^17):
+// x^1, x^2 and x^-1 are one IEEE operation, x^0.5 of a positive x is sqrt, 2^k is built from its bits (k < -1074
+// rounds to 0, k > 1023 to inf, as glibc's does), and an integer x to an integer y in [3, 64] is multiplied out when
+// every product is exact (fma(p, q, -pq) == 0; integers cannot underflow).  Every other pair is CUDA's pow.
+__device__ __forceinline__ double pow_exact_cases(double x, double y) {
+  if (y == 1.0) return x;
+  if (y == 2.0) return __dmul_rn(x, x);
+  if (y == -1.0) return __ddiv_rn(1.0, x);
+  if (y == 0.5 && x > 0.0) return __dsqrt_rn(x);
+  const bool y_int = y == rint(y) && fabs(y) <= 2048.0;
+  if (x == 2.0 && y_int) {
+    const int k = (int)y;
+    if (k > 1023) return __longlong_as_double(0x7FF0000000000000ll);
+    if (k >= -1022) return __longlong_as_double((long long)(k + 1023) << 52);
+    return k >= -1074 ? __longlong_as_double(1ll << (k + 1074)) : 0.0;
+  }
+  if (y_int && y >= 3.0 && y <= 64.0 && x == rint(x) && x != 0.0 && fabs(x) < 9007199254740992.0) {
+    double r = 1.0, p = x;
+    bool exact = true;
+    for (int n = (int)y;;) {
+      if (n & 1) {
+        const double q = __dmul_rn(r, p);
+        exact = exact && __fma_rn(r, p, -q) == 0.0 && fabs(q) <= 1.7976931348623157e308;
+        r = q;
+      }
+      n >>= 1;
+      if (!n || !exact) break;
+      const double q = __dmul_rn(p, p);
+      exact = exact && __fma_rn(p, p, -q) == 0.0 && fabs(q) <= 1.7976931348623157e308;
+      p = q;
+    }
+    if (exact) return r;
+  }
+  return pow(x, y);
+}
+
 template <int OP>
 __device__ __forceinline__ double bin_arith(double a, double b) {
   if (OP == kOpAdd) return __dadd_rn(a, b);
@@ -79,7 +115,7 @@ __device__ __forceinline__ double bin_arith(double a, double b) {
     // glibc's pow (what f64::powf calls) returns NaN when an operand is a signaling NaN, pow(sNaN, 0) and pow(1, sNaN)
     // included, where CUDA's follows C99 Annex F and returns 1
     if (is_snan(a) || is_snan(b)) return __dadd_rn(a, b);
-    return pow(a, b);
+    return pow_exact_cases(a, b);
   }
   return atan2(a, b);
 }

@@ -18,7 +18,7 @@
 //     `v < lo ? lo : v > hi ? hi : v` with IEEE comparisons (clamp.rs:75-224), so a NaN value passes through with its
 //     bits and a NaN bound never binds.
 //   * the transcendental functions are CUDA's; DESIGN.md section 2 states their measured ulp bound against glibc (which
-//     Rust's std calls).
+//     Rust's std calls).  log2 of a power of two is its exponent, exact as glibc's.
 //
 // scalar(v) is ScalarCalculate (src/promql/src/extension_plan/scalar_calculate.rs:532-637): over the whole query, not
 // per step.  When every live row (a row with at least one cell) carries one series key, the output is that series'
@@ -58,6 +58,16 @@ struct InstantFnArgs {
   uint32_t* out_valid;      // may be valid (then it is not written)
 };
 
+// log2 of a power of two (subnormals included) is its exponent, exactly, as glibc gives it; CUDA's log2 can be an ulp
+// off there (log2(8) = 2.9999999999999996, log2(2^-1012) = -1011.9999999999999).  Every other operand is CUDA's.
+__device__ __forceinline__ double log2_pow2_exact(double v) {
+  const long long b = __double_as_longlong(v);
+  const long long e = b >> 52, m = b & 0x000FFFFFFFFFFFFFll;  // (negative and NaN bit patterns fail both tests)
+  if (e > 0 && e < 0x7FF && m == 0) return (double)(e - 1023);
+  if (e == 0 && m != 0 && (m & (m - 1)) == 0) return (double)(-1074 + 63 - __clzll(m));
+  return log2(v);
+}
+
 template <int FN>
 __device__ __forceinline__ double instant_fn(double v, double a0, double a1) {
   if (FN == kFnAbs) return fabs(v);
@@ -66,7 +76,7 @@ __device__ __forceinline__ double instant_fn(double v, double a0, double a1) {
   if (FN == kFnSqrt) return __dsqrt_rn(v);
   if (FN == kFnExp) return exp(v);
   if (FN == kFnLn) return log(v);
-  if (FN == kFnLog2) return log2(v);
+  if (FN == kFnLog2) return log2_pow2_exact(v);
   if (FN == kFnLog10) return log10(v);
   if (FN == kFnSin) return sin(v);
   if (FN == kFnCos) return cos(v);

@@ -11,14 +11,13 @@ from oracle import oracle as orc
 from tests import binary_oracle as bor
 from tests.binary_helpers import (LOOKBACK, count_rows, dense_rows, expected_rows, load_binary, oracle_node,
                                   sum_rate_table, table_arrays)
+from tests.ulp_bounds import POW_ATAN2_ULPS   # pow / atan2 are CUDA's, not glibc's: DESIGN.md section 2
 
 pytestmark = pytest.mark.gpu
 G = load_binary()
 CASES = {c["name"]: c for c in G["cases"]}
 ARITH = ["+", "-", "*", "/", "%", "^", "atan2"]
 CMP = ["==", "!=", ">", "<", ">=", "<="]
-# pow / atan2 are CUDA's, not glibc's: the largest distance DESIGN.md section 2 states, in units in the last place
-POW_ATAN2_ULPS = 2
 
 
 @pytest.fixture(scope="module")

@@ -12,15 +12,12 @@ import pytest
 from tests import instant_fn_oracle as ifo
 from tests.binary_helpers import dense_rows, oracle_node
 from tests.instant_fn_helpers import G, ORACLE_FN, check_rows, select
+from tests.ulp_bounds import ULP_BOUND, ulp_distance   # every test of these functions holds the same bound
 
 pytestmark = pytest.mark.gpu
 EXACT = ["abs", "ceil", "floor", "sqrt", "round", "deg", "rad", "sgn", "clamp", "clamp_min", "clamp_max"]
 ALL = EXACT + list(ifo.TRANSCENDENTAL)
 ARGS = {"round": (0.1, 0.0), "clamp": (-2.0, 3.5), "clamp_min": (0.0, 0.0), "clamp_max": (1.0, 0.0)}
-# max ulp distance from glibc per function: the distance measured on an H100 over the 2^20 seeded operands of
-# test_ulp_bound_over_a_million_operands (DESIGN.md section 2); every test of these functions holds the same bound
-ULP_BOUND = {"exp": 1, "ln": 1, "log2": 1, "log10": 2, "sin": 1, "cos": 1, "tan": 2, "asin": 2, "acos": 1, "atan": 1,
-             "sinh": 2, "cosh": 2, "tanh": 3, "asinh": 2, "acosh": 2, "atanh": 2}
 
 
 @pytest.fixture(scope="module")
@@ -63,18 +60,6 @@ def operands(rng, fn, n):
     if fn == "acosh":
         return 1.0 + np.abs(logu)
     return logu   # atan, asinh
-
-
-def ulp_distance(a, b):
-    """|a - b| in units in the last place (0 when both are NaN or equal; huge when one is NaN)."""
-    def ordered(x):   # the bit pattern as a monotone int64 (subtracted in integers: float64 cannot hold 2^63)
-        i = np.ascontiguousarray(x, np.float64).view(np.int64)
-        return np.where(i < 0, np.int64(-0x8000000000000000) - i, i)
-    with np.errstate(over="ignore"):
-        d = np.abs(ordered(a) - ordered(b)).astype(np.float64)
-    both_nan = np.isnan(a) & np.isnan(b)
-    one_nan = np.isnan(a) ^ np.isnan(b)
-    return np.where(both_nan, 0.0, np.where(one_nan, np.inf, d))
 
 
 def grid(rng, rows, T, fn):
