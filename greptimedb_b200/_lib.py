@@ -49,6 +49,9 @@ EXPORTED_SYMBOLS = [
     "b2p_topk_shard_merge_dev", "b2p_topk_shard_mark_dev",
     "b2p_quantile_allreduce_dev", "b2p_quantile_shard_plan", "b2p_quantile_shard_pass_dev",
     "b2p_quantile_shard_advance_dev",
+    "b2p_count_values_shard_heights_dev", "b2p_count_values_allgather_dev", "b2p_count_values_allgather_i64_dev",
+    "b2p_count_values_shard_plan", "b2p_count_values_shard_pack_dev", "b2p_count_values_shard_pack_i64_dev",
+    "b2p_count_values_shard_merge_dev", "b2p_count_values_shard_merge_i64_dev",
 ]
 
 
@@ -210,6 +213,14 @@ def load() -> C.CDLL:
         "b2p_quantile_shard_plan": (C.c_int, [vp, u32, u64, C.POINTER(u32), C.POINTER(u64), C.POINTER(u64)]),
         "b2p_quantile_shard_pass_dev": (C.c_int, [vp, dbl, vp, vp, vp, u64, u32, u32, vp]),
         "b2p_quantile_shard_advance_dev": (C.c_int, [vp, dbl, u32, u64, u32, u32, vp, u32, vp, vp, C.POINTER(u64)]),
+        "b2p_count_values_shard_heights_dev": (C.c_int, [vp, vp, vp, u64, vp]),
+        "b2p_count_values_allgather_dev": (C.c_int, [vp, vp, vp, vp, u64, vp, vp, vp]),
+        "b2p_count_values_allgather_i64_dev": (C.c_int, [vp, vp, vp, vp, u64, vp, vp, vp]),
+        "b2p_count_values_shard_plan": (C.c_int, [vp, vp, i32, u32, u64, C.POINTER(u32), C.POINTER(u64)]),
+        "b2p_count_values_shard_pack_dev": (C.c_int, [vp, vp, vp, vp, u64, vp, i32, i32, u32, vp]),
+        "b2p_count_values_shard_pack_i64_dev": (C.c_int, [vp, vp, vp, vp, u64, vp, i32, i32, u32, vp]),
+        "b2p_count_values_shard_merge_dev": (C.c_int, [vp, vp, i32, u32, u64, u32, vp, vp, vp]),
+        "b2p_count_values_shard_merge_i64_dev": (C.c_int, [vp, vp, i32, u32, u64, u32, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)  # AttributeError here means the .so does not match the header

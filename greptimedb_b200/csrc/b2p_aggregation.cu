@@ -727,6 +727,256 @@ int count_values_run(b2p_ctx* c, const double* vals, const uint32_t* valid, cons
   return B2P_OK;
 }
 
+// ---- sharded count_values: every rank's distinct values and counts, one all-gather per batch ----------------------
+// The exchange is derived from (heights, n_ranks, n_groups, T, topk_exchange_cap) only, so every rank derives the same
+// batches.  Group g has U_g = sum over ranks of h_r(g) output rows from uoff[g].  Windows of W steps (every step when
+// the costliest group fits the cap over all of them, else a multiple of 32, at least 32), each cut into runs of whole
+// groups whose send block, gathered blocks and merge scratch fit the cap; a group too large for the cap alone is a
+// batch of its own.  Batches without an output row are left out.  Per step of a batch: (R + 1) x P' x 12 B of blocks
+// (P' = max over ranks of its summed heights), 28 B of merge scratch per merged entry (arranged and sorted key and
+// count, the run rank; the start and sum tables reuse the sort's alternate buffers) and 4 B per segment.
+struct CvShard {
+  static constexpr uint64_t kEntry = 12;        // key u64 and count u32
+  static constexpr uint64_t kMergeEntry = 28;
+  static constexpr uint64_t kMergeSegment = 4;
+  uint32_t n_ranks = 1, n_groups = 0;
+  uint64_t T = 0;
+  const uint32_t* h = nullptr;   // [n_ranks x n_groups], host
+  std::vector<uint32_t> uoff;    // [n_groups + 1]
+  struct Batch {
+    uint32_t g0, g1, k0, W;
+    uint64_t P;                  // entries of each rank's block: W x max over ranks of the batch's summed heights
+    uint64_t rows;               // output rows of the batch: sum of U_g
+  };
+  std::vector<Batch> batches;
+  uint32_t height(uint32_t r, uint32_t g) const { return h[(uint64_t)r * n_groups + g]; }
+  uint64_t max_block() const {
+    uint64_t p = 0;
+    for (const Batch& b : batches) p = std::max(p, b.P);
+    return p * kEntry;
+  }
+};
+
+int cv_shard_plan(const b2p_ctx* c, const uint32_t* heights, int32_t n_ranks, uint32_t n_groups, uint64_t T,
+                  CvShard& sh) {
+  if (n_ranks < 1) return fail(B2P_E_INVALID, "n_ranks %d < 1", n_ranks);
+  if (n_groups && !heights) return fail(B2P_E_INVALID, "NULL argument");
+  const uint32_t R = (uint32_t)n_ranks, G = n_groups;
+  sh.n_ranks = R; sh.n_groups = G; sh.T = T; sh.h = heights;
+  sh.uoff.assign(G + 1, 0u);
+  uint64_t worst = 0;
+  for (uint32_t g = 0; g < G; ++g) {
+    uint64_t u = 0, hm = 0;
+    for (uint32_t r = 0; r < R; ++r) {
+      u += sh.height(r, g);
+      hm = std::max<uint64_t>(hm, sh.height(r, g));
+    }
+    if (sh.uoff[g] + u > UINT32_MAX) return fail(B2P_E_TOO_LARGE, "count_values: more than 2^32 - 1 output rows");
+    if (u * std::min<uint64_t>(32, T) > (uint64_t)INT32_MAX)
+      return fail(B2P_E_TOO_LARGE, "count_values: a group of %llu merged rows is too large", (unsigned long long)u);
+    sh.uoff[g + 1] = sh.uoff[g] + (uint32_t)u;
+    if (u) worst = std::max(worst, (R + 1) * CvShard::kEntry * hm + CvShard::kMergeEntry * u + CvShard::kMergeSegment);
+  }
+  if (T == 0 || G == 0 || sh.uoff[G] == 0) return B2P_OK;  // no batch
+  const uint64_t cap = c->topk_exchange_cap;
+  const uint64_t W = std::min<uint64_t>((T + 31) / 32 * 32, std::max<uint64_t>(32, cap / worst / 32 * 32));
+  std::vector<uint64_t> run(R);
+  for (uint64_t k0 = 0; k0 < T; k0 += W) {
+    const uint64_t Wb = std::min<uint64_t>(W, T - k0);
+    for (uint32_t g = 0; g < G;) {
+      const uint32_t g0 = g;
+      std::fill(run.begin(), run.end(), 0);
+      uint64_t pmax = 0, rows = 0;
+      for (; g < G; ++g) {
+        uint64_t pm = pmax;
+        for (uint32_t r = 0; r < R; ++r) pm = std::max(pm, run[r] + sh.height(r, g));
+        const uint64_t u = sh.uoff[g + 1] - sh.uoff[g];
+        const uint64_t bytes = ((R + 1) * CvShard::kEntry * pm + CvShard::kMergeEntry * (rows + u) +
+                                CvShard::kMergeSegment * (g + 1 - g0)) * Wb;
+        if (g > g0 && bytes > cap) break;
+        for (uint32_t r = 0; r < R; ++r) run[r] += sh.height(r, g);
+        pmax = pm;
+        rows += u;
+      }
+      if (rows == 0) continue;  // groups without a value on any rank: no output row
+      if (std::max<uint64_t>(rows, g - g0) * Wb > (uint64_t)INT32_MAX)
+        return fail(B2P_E_TOO_LARGE, "count_values: a batch of %llu merged rows is too large", (unsigned long long)rows);
+      sh.batches.push_back(CvShard::Batch{g0, g, (uint32_t)k0, (uint32_t)Wb, pmax * Wb, rows});
+    }
+  }
+  return B2P_OK;
+}
+
+// This rank's row of heights against its own index: h_r(g) <= its member count of g
+int cv_shard_check_rank(const CvShard& sh, const b2p_group_index* ix, uint32_t rank) {
+  if (ix->n_groups != sh.n_groups) return fail(B2P_E_INVALID, "index of %u groups, heights of %u", ix->n_groups, sh.n_groups);
+  if (rank >= sh.n_ranks) return fail(B2P_E_INVALID, "rank %u of %u", rank, sh.n_ranks);
+  for (uint32_t g = 0; g < sh.n_groups; ++g)
+    if (sh.height(rank, g) > ix->goff_host[g + 1] - ix->goff_host[g])
+      return fail(B2P_E_INVALID, "heights: %u rows of group %u on rank %u, which has %u", sh.height(rank, g), g, rank,
+                  ix->goff_host[g + 1] - ix->goff_host[g]);
+  return B2P_OK;
+}
+
+// h_r(g) of this rank into `heights` (host): [n_groups], or with a communicator every rank's row [n_ranks x n_groups]
+// (one in-place all-gather).  Reads the table back, so it synchronises the stream.
+int cv_shard_heights(b2p_ctx* c, const uint32_t* cnt, const b2p_group_index* ix, uint64_t T, uint32_t* heights) {
+  int rc;
+  const uint32_t G = ix->n_groups, R = c->comm ? (uint32_t)c->comm_ranks : 1u;
+  if (G == 0) return B2P_OK;
+  if ((rc = c->x_size.ensure((size_t)R * G * 4))) return rc;
+  uint32_t* mine = c->x_size.as<uint32_t>() + (c->comm ? (size_t)c->comm_rank * G : 0);
+  CU(cudaMemsetAsync(mine, 0, (size_t)G * 4, c->stream));
+  const uint32_t in_rows = ix->goff_host[G];
+  if (in_rows && T) {
+    count_values_heights_kernel<<<capped_grid(c, in_rows, 8, 16), 256, 0, c->stream>>>(cnt, ix->gid, ix->members,
+                                                                                        ix->goff, in_rows, T, mine);
+    c->launches++;
+    CU(cudaGetLastError());
+  }
+  if (c->comm)
+    NCCL_TRY(g_nccl.AllGather(mine, c->x_size.p, G, Nccl::kUint32, c->comm, c->stream));
+  CU(cudaMemcpyAsync(heights, c->x_size.p, (size_t)R * G * 4, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return B2P_OK;
+}
+
+// Per-rank step: this rank's block of batch b, [keys: P u64][counts: P u32] (P the batch's padded entry count; the
+// entries past the rank's own are not written and never read).  i64: the grid is Int64 (I64Key).
+int cv_shard_pack(b2p_ctx* c, const CvShard& sh, uint32_t b, uint32_t rank, const double* vals, const uint32_t* cnt,
+                  const b2p_group_index* ix, void* block, bool i64) {
+  int rc;
+  const CvShard::Batch& bt = sh.batches[b];
+  const uint32_t ng = bt.g1 - bt.g0;
+  std::vector<uint32_t> hoff(ng + 1, 0u);
+  for (uint32_t q = 0; q < ng; ++q) hoff[q + 1] = hoff[q] + sh.height(rank, bt.g0 + q);
+  c->last_exchange_bytes += (long long)(bt.P * CvShard::kEntry);
+  if (hoff[ng] == 0) return B2P_OK;  // no entry of this rank in the batch
+  if ((rc = c->x_table.ensure((ng + 1) * 4))) return rc;
+  CU(cudaMemcpyAsync(c->x_table.p, hoff.data(), (ng + 1) * 4, cudaMemcpyHostToDevice, c->stream));
+  CvShardArgs a{};
+  a.T = sh.T; a.k0 = bt.k0; a.W = bt.W; a.g0 = bt.g0; a.ng = ng;
+  a.off = c->x_table.as<uint32_t>();
+  a.vals = vals; a.cnt = cnt; a.goff = ix->goff;
+  a.bkeys = static_cast<unsigned long long*>(block);
+  a.bcnt = reinterpret_cast<uint32_t*>(a.bkeys + bt.P);
+  (i64 ? count_values_pack_kernel<I64Key> : count_values_pack_kernel<F64Key>)
+      <<<capped_grid(c, (uint64_t)hoff[ng] * bt.W, 256, 8), 256, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// Merge step: the n_ranks gathered blocks of batch b, [keys of rank 0 .. R-1][counts of rank 0 .. R-1] (each rank's
+// section P entries), into the batch's rows of out_val / out_cnt.  Per batch: the tables, the segment offsets, the
+// arrange, CUB's segmented sort of (key, count) pairs, the head flags, CUB's scans of the flags and of the counts, the
+// run starts and the output; no host round trip.
+int cv_shard_merge(b2p_ctx* c, const CvShard& sh, uint32_t b, const void* blocks, double* out_val, uint32_t* out_cnt,
+                   bool i64) {
+  int rc;
+  const CvShard::Batch& bt = sh.batches[b];
+  const uint32_t ng = bt.g1 - bt.g0, R = sh.n_ranks;
+  // tables: uoff relative to the batch [ng + 1], the prefix over ranks of each group's heights [ng x (R + 1)], and
+  // each rank's entry offset of each group within its block [ng x R]
+  std::vector<uint32_t> tab((size_t)(ng + 1) + (size_t)ng * (R + 1) + (size_t)ng * R, 0u);
+  uint32_t* uo = tab.data();
+  uint32_t* pre = uo + ng + 1;
+  uint32_t* hoffs = pre + (size_t)ng * (R + 1);
+  std::vector<uint32_t> run(R, 0u);
+  for (uint32_t q = 0; q < ng; ++q) {
+    const uint32_t g = bt.g0 + q;
+    uo[q + 1] = sh.uoff[g + 1] - sh.uoff[bt.g0];
+    for (uint32_t r = 0; r < R; ++r) {
+      pre[(size_t)q * (R + 1) + r + 1] = pre[(size_t)q * (R + 1) + r] + sh.height(r, g);
+      hoffs[(size_t)q * R + r] = run[r];
+      run[r] += sh.height(r, g);
+    }
+  }
+  const uint32_t cells = (uint32_t)(bt.rows * bt.W), n_seg = ng * bt.W;
+  size_t sort_bytes = 0, scan_bytes = 0;
+  {
+    cub::DoubleBuffer<unsigned long long> dk(nullptr, nullptr);
+    cub::DoubleBuffer<uint32_t> dv(nullptr, nullptr);
+    CU(cub::DeviceSegmentedSort::SortPairs(nullptr, sort_bytes, dk, dv, (int)cells, (int)n_seg, (const uint32_t*)nullptr,
+                                           (const uint32_t*)nullptr, c->stream));
+    CU(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)cells, c->stream));
+  }
+  if ((rc = c->x_table.ensure(tab.size() * 4)) || (rc = c->v_keys.ensure((size_t)cells * 8)) ||
+      (rc = c->v_alt.ensure((size_t)cells * 8)) || (rc = c->vx_cnt.ensure((size_t)cells * 4)) ||
+      (rc = c->vx_alt.ensure((size_t)cells * 4)) || (rc = c->v_rank.ensure((size_t)cells * 4)) ||
+      (rc = c->v_seg.ensure(((size_t)n_seg + 1) * 4)) || (rc = c->v_tmp.ensure(std::max<size_t>({16, sort_bytes, scan_bytes}))))
+    return rc;
+  CU(cudaMemcpyAsync(c->x_table.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, c->stream));
+  CvShardArgs a{};
+  a.T = sh.T; a.k0 = bt.k0; a.W = bt.W; a.g0 = bt.g0; a.ng = ng;
+  a.off = c->x_table.as<uint32_t>();
+  a.hpre = a.off + ng + 1;
+  a.hoffs = a.hpre + (size_t)ng * (R + 1);
+  a.n_ranks = R; a.P = bt.P;
+  a.gkeys = static_cast<const unsigned long long*>(blocks);
+  a.gcnt = reinterpret_cast<const uint32_t*>(a.gkeys + (uint64_t)R * bt.P);
+  a.cells = cells;
+  a.seg_off = c->v_seg.as<uint32_t>();
+  a.keys = c->v_keys.as<unsigned long long>();
+  a.kcnt = c->vx_cnt.as<uint32_t>();
+  a.rank = c->v_rank.as<uint32_t>();
+  a.out_val = out_val; a.out_cnt = out_cnt; a.out_row0 = sh.uoff[bt.g0];
+  const unsigned cell_grid = capped_grid(c, cells, 256, 8);
+  count_values_merge_segments_kernel<<<capped_grid(c, n_seg, 256, 8), 256, 0, c->stream>>>(a);
+  count_values_merge_arrange_kernel<<<cell_grid, 256, 0, c->stream>>>(a);
+  c->launches += 2;
+  CU(cudaGetLastError());
+  cub::DoubleBuffer<unsigned long long> dk(c->v_keys.as<unsigned long long>(), c->v_alt.as<unsigned long long>());
+  cub::DoubleBuffer<uint32_t> dv(c->vx_cnt.as<uint32_t>(), c->vx_alt.as<uint32_t>());
+  size_t bytes = c->v_tmp.cap;
+  CU(cub::DeviceSegmentedSort::SortPairs(c->v_tmp.p, bytes, dk, dv, (int)cells, (int)n_seg, a.seg_off, a.seg_off + 1,
+                                         c->stream));
+  a.sorted = dk.Current();
+  a.scnt = dv.Current();
+  a.csum = dv.Alternate();
+  a.start = reinterpret_cast<uint32_t*>(dk.Alternate());
+  count_values_merge_head_kernel<<<cell_grid, 256, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  bytes = c->v_tmp.cap;
+  CU(cub::DeviceScan::InclusiveSum(c->v_tmp.p, bytes, a.rank, a.rank, (int)cells, c->stream));
+  bytes = c->v_tmp.cap;
+  CU(cub::DeviceScan::InclusiveSum(c->v_tmp.p, bytes, a.scnt, a.csum, (int)cells, c->stream));
+  count_values_merge_rank_kernel<<<cell_grid, 256, 0, c->stream>>>(a);
+  (i64 ? count_values_merge_count_kernel<I64Key> : count_values_merge_count_kernel<F64Key>)
+      <<<cell_grid, 256, 0, c->stream>>>(a);
+  c->launches += 2;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// The composed call: per batch this rank's block, two all-gathers (keys, counts) in one group and the merge.  Without
+// a communicator (one rank) the block is its own gather.
+int cv_allgather_run(b2p_ctx* c, const CvShard& sh, const double* vals, const uint32_t* cnt, const b2p_group_index* ix,
+                     double* out_val, uint32_t* out_cnt, bool i64) {
+  int rc;
+  if (sh.batches.empty()) return B2P_OK;
+  const uint64_t block = sh.max_block();
+  if ((rc = c->x_send.ensure(block))) return rc;
+  if (c->comm && (rc = c->x_recv.ensure(block * sh.n_ranks))) return rc;
+  for (uint32_t b = 0; b < (uint32_t)sh.batches.size(); ++b) {
+    if ((rc = cv_shard_pack(c, sh, b, (uint32_t)c->comm_rank, vals, cnt, ix, c->x_send.p, i64))) return rc;
+    const void* gathered = c->x_send.p;
+    if (c->comm) {
+      const uint64_t P = sh.batches[b].P;
+      const unsigned long long* sk = c->x_send.as<unsigned long long>();
+      unsigned long long* gk = c->x_recv.as<unsigned long long>();
+      NCCL_TRY(g_nccl.GroupStart());
+      NCCL_TRY(g_nccl.AllGather(sk, gk, P, Nccl::kUint64, c->comm, c->stream));
+      NCCL_TRY(g_nccl.AllGather(sk + P, gk + P * sh.n_ranks, P, Nccl::kUint32, c->comm, c->stream));
+      NCCL_TRY(g_nccl.GroupEnd());
+      gathered = c->x_recv.p;
+    }
+    if ((rc = cv_shard_merge(c, sh, b, gathered, out_val, out_cnt, i64))) return rc;
+  }
+  return B2P_OK;
+}
+
 // The end of a host call over a group index: stages gid, builds a temporary index of it, runs `dev(ix)`, finishes `s`
 // and destroys the index once the copies have completed.
 template <class Dev>
@@ -780,6 +1030,48 @@ int count_values_dev(b2p_ctx* c, const double* vals, const uint32_t* valid, cons
   const int rc = count_values_run(c, vals, valid, ix, T, out_val, out_cnt, i64);
   stage_end(c, 3);
   return rc;
+}
+
+// The device forms of the sharded count_values; i64: the grid is Int64
+int cv_allgather_dev(b2p_ctx* c, const double* vals, const uint32_t* cnt, const b2p_group_index* ix, uint64_t T,
+                     const uint32_t* heights, double* out_val, uint32_t* out_cnt, bool i64) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_series && T && (!vals || !cnt)) return fail(B2P_E_INVALID, "NULL argument");
+  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
+  c->last_exchange_bytes = 0;
+  CvShard sh;
+  if (int rc = cv_shard_plan(c, heights, c->comm_ranks, ix->n_groups, T, sh)) return rc;
+  if (int rc = cv_shard_check_rank(sh, ix, (uint32_t)c->comm_rank)) return rc;
+  if (!sh.batches.empty() && (!out_val || !out_cnt)) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  stage_begin(c, 3);
+  const int rc = cv_allgather_run(c, sh, vals, cnt, ix, out_val, out_cnt, i64);
+  stage_end(c, 3);
+  return rc;
+}
+
+int cv_shard_pack_dev(b2p_ctx* c, const double* vals, const uint32_t* cnt, const b2p_group_index* ix, uint64_t T,
+                      const uint32_t* heights, int32_t n_ranks, int32_t rank, uint32_t batch, void* block, bool i64) {
+  if (!c || !ix || !block) return fail(B2P_E_INVALID, "NULL argument");
+  if (ix->n_series && (!vals || !cnt)) return fail(B2P_E_INVALID, "NULL argument");
+  if (rank < 0) return fail(B2P_E_INVALID, "rank %d < 0", rank);
+  CvShard sh;
+  if (int rc = cv_shard_plan(c, heights, n_ranks, ix->n_groups, T, sh)) return rc;
+  if (int rc = cv_shard_check_rank(sh, ix, (uint32_t)rank)) return rc;
+  if (batch >= sh.batches.size()) return fail(B2P_E_INVALID, "batch %u of %zu", batch, sh.batches.size());
+  DeviceGuard g(c->device);
+  c->last_exchange_bytes = 0;
+  return cv_shard_pack(c, sh, batch, (uint32_t)rank, vals, cnt, ix, block, i64);
+}
+
+int cv_shard_merge_dev(b2p_ctx* c, const uint32_t* heights, int32_t n_ranks, uint32_t n_groups, uint64_t T,
+                       uint32_t batch, const void* blocks, double* out_val, uint32_t* out_cnt, bool i64) {
+  if (!c || !blocks || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  CvShard sh;
+  if (int rc = cv_shard_plan(c, heights, n_ranks, n_groups, T, sh)) return rc;
+  if (batch >= sh.batches.size()) return fail(B2P_E_INVALID, "batch %u of %zu", batch, sh.batches.size());
+  DeviceGuard g(c->device);
+  return cv_shard_merge(c, sh, batch, blocks, out_val, out_cnt, i64);
 }
 
 int count_values_host(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* gid, uint32_t n_rows,
@@ -951,6 +1243,65 @@ int b2p_count_values_i64_dev(b2p_ctx* c, const int64_t* vals, const uint32_t* va
                              uint64_t T, int64_t* out_val, uint32_t* out_cnt) {
   return count_values_dev(c, reinterpret_cast<const double*>(vals), valid, ix, T, reinterpret_cast<double*>(out_val),
                           out_cnt, true);
+}
+
+/* ---- count_values over sharded rows -------------------------------------------------------------------------- */
+
+int b2p_count_values_shard_heights_dev(b2p_ctx* c, const uint32_t* local_cnt, const b2p_group_index* ix, uint64_t T,
+                                       uint32_t* heights) {
+  if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
+  if ((ix->n_series && T && !local_cnt) || (ix->n_groups && !heights)) return fail(B2P_E_INVALID, "NULL argument");
+  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
+  DeviceGuard g(c->device);
+  return cv_shard_heights(c, local_cnt, ix, T, heights);
+}
+
+int b2p_count_values_allgather_dev(b2p_ctx* c, const double* local_val, const uint32_t* local_cnt,
+                                   const b2p_group_index* ix, uint64_t T, const uint32_t* heights, double* out_val,
+                                   uint32_t* out_cnt) {
+  return cv_allgather_dev(c, local_val, local_cnt, ix, T, heights, out_val, out_cnt, false);
+}
+
+int b2p_count_values_allgather_i64_dev(b2p_ctx* c, const int64_t* local_val, const uint32_t* local_cnt,
+                                       const b2p_group_index* ix, uint64_t T, const uint32_t* heights, int64_t* out_val,
+                                       uint32_t* out_cnt) {
+  return cv_allgather_dev(c, reinterpret_cast<const double*>(local_val), local_cnt, ix, T, heights,
+                          reinterpret_cast<double*>(out_val), out_cnt, true);
+}
+
+int b2p_count_values_shard_plan(b2p_ctx* c, const uint32_t* heights, int32_t n_ranks, uint32_t n_groups, uint64_t T,
+                                uint32_t* n_batches, uint64_t* block_bytes) {
+  if (!c || !n_batches || !block_bytes) return fail(B2P_E_INVALID, "NULL argument");
+  CvShard sh;
+  if (int rc = cv_shard_plan(c, heights, n_ranks, n_groups, T, sh)) return rc;
+  *n_batches = (uint32_t)sh.batches.size();
+  *block_bytes = sh.max_block();
+  return B2P_OK;
+}
+
+int b2p_count_values_shard_pack_dev(b2p_ctx* c, const double* local_val, const uint32_t* local_cnt,
+                                    const b2p_group_index* ix, uint64_t T, const uint32_t* heights, int32_t n_ranks,
+                                    int32_t rank, uint32_t batch, void* block) {
+  return cv_shard_pack_dev(c, local_val, local_cnt, ix, T, heights, n_ranks, rank, batch, block, false);
+}
+
+int b2p_count_values_shard_pack_i64_dev(b2p_ctx* c, const int64_t* local_val, const uint32_t* local_cnt,
+                                        const b2p_group_index* ix, uint64_t T, const uint32_t* heights, int32_t n_ranks,
+                                        int32_t rank, uint32_t batch, void* block) {
+  return cv_shard_pack_dev(c, reinterpret_cast<const double*>(local_val), local_cnt, ix, T, heights, n_ranks, rank,
+                           batch, block, true);
+}
+
+int b2p_count_values_shard_merge_dev(b2p_ctx* c, const uint32_t* heights, int32_t n_ranks, uint32_t n_groups,
+                                     uint64_t T, uint32_t batch, const void* blocks, double* out_val, uint32_t* out_cnt) {
+  return cv_shard_merge_dev(c, heights, n_ranks, n_groups, T, batch, blocks, out_val, out_cnt, false);
+}
+
+int b2p_count_values_shard_merge_i64_dev(b2p_ctx* c, const uint32_t* heights, int32_t n_ranks, uint32_t n_groups,
+                                         uint64_t T, uint32_t batch, const void* blocks, int64_t* out_val,
+                                         uint32_t* out_cnt) {
+  return cv_shard_merge_dev(c, heights, n_ranks, n_groups, T, batch, blocks, reinterpret_cast<double*>(out_val),
+                            out_cnt, true);
 }
 
 /* ---- host-pointer API ------------------------------------------------------------------------ */

@@ -183,4 +183,184 @@ __global__ void __launch_bounds__(256) count_values_member_group_kernel(const ui
     mgroup[m] = __ldg(gid + __ldg(members + m));
 }
 
+// ---- sharded count_values: every rank's distinct values and counts, merged ---------------------------------------
+// A rank's K12 output fills each group's rows as a prefix at every step, so its first h_r(g) rows (h_r(g) = the most
+// distinct values the group has at one step) hold every (key, count) it has.  Per batch of whole groups [g0, g0 + ng)
+// over steps [k0, k0 + W), a rank's block is those rows' cells as (key u64, count u32) entries, segment-major: segment
+// (q, kk) of group g0 + q and step k0 + kk starts at W * hoff(q) + kk * h(q), hoff the prefix of the rank's heights
+// over the batch.  The merge lays every rank's entries of segment (q, kk) side by side (U(q) = sum over ranks of h) at
+// W * uoff(q) + kk * U(q), sorts each segment by key with its counts, and writes each run of equal keys with the sum of
+// its counts.  A cell past a rank's distinct values is packed as key ~0 with count 0: it sorts into the last run of
+// its segment, and a run whose counts add up to 0 is no value.  The count decides, not the position: ~0 is also the key
+// of the largest positive NaN (and of INT64_MAX), whose entries may land anywhere in that run.
+struct CvShardArgs {
+  uint64_t T;
+  uint32_t k0, W, g0, ng;
+  const uint32_t* off;        // [ng + 1] per-step entry offsets of the batch's groups: hoff (pack) or uoff (merge)
+  // pack: this rank's K12 output [rows x T] (rows in member order) and its index's goff
+  const double* vals;
+  const uint32_t* cnt;
+  const uint32_t* goff;
+  unsigned long long* bkeys;  // [P] the block: keys, then counts
+  uint32_t* bcnt;
+  // merge: the gathered blocks, [keys of rank 0 .. R-1][counts of rank 0 .. R-1], each rank's block P entries
+  uint32_t n_ranks;
+  uint64_t P;
+  const unsigned long long* gkeys;
+  const uint32_t* gcnt;
+  const uint32_t* hpre;       // [ng x (R + 1)] the prefix over ranks of h_r(g0 + q): rank r's entries of a segment
+  const uint32_t* hoffs;      // [ng x R] hoff of rank r at group q
+  uint32_t cells;             // W * uoff[ng]
+  uint32_t* seg_off;          // [ng * W + 1]
+  unsigned long long* keys;   // [cells] arranged, the sort's input
+  uint32_t* kcnt;
+  const unsigned long long* sorted;  // [cells] after the sort, and their counts
+  const uint32_t* scnt;
+  uint32_t* rank;             // [cells] head flags, then (scanned in place) the inclusive count of runs
+  uint32_t* csum;             // [cells] inclusive u32 sum of the sorted counts (wrapping: only differences within a
+                              // run are read, and a run's sum is at most its group's member count)
+  uint32_t* start;            // [cells] (uoff(q) + j) * W + kk: where run j of segment (q, kk) starts in the batch
+  double* out_val;            // [out rows x T], the batch's rows from out_row0
+  uint32_t* out_cnt;
+  uint32_t out_row0;
+};
+
+// the group q of the batch whose rows [off[q], off[q + 1]) hold row position p < off[ng]
+__device__ __forceinline__ uint32_t cv_shard_group(const uint32_t* off, uint32_t ng, uint32_t p) {
+  uint32_t lo = 0, hi = ng;  // off[lo] <= p < off[hi]
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) / 2;
+    if (__ldg(off + mid) <= p) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// h_r(g) of this rank: 1 + the largest place in its group of a row with a count at some step.  One warp per row of the
+// K12 output (member position m < in_rows); heights zeroed by the caller.
+__global__ void __launch_bounds__(256) count_values_heights_kernel(const uint32_t* cnt, const uint32_t* gid,
+                                                                    const uint32_t* members, const uint32_t* goff,
+                                                                    uint32_t in_rows, uint64_t T, uint32_t* heights) {
+  const int lane = threadIdx.x & 31;
+  const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x / 32);
+  for (uint64_t m = (uint64_t)blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32; m < in_rows; m += warps) {
+    const uint32_t* row = cnt + m * T;
+    bool any = false;
+    for (uint64_t k = lane; k < T && !any; k += 32) any = __ldg(row + k) != 0u;
+    if (__any_sync(0xFFFFFFFFu, any) && lane == 0) {
+      const uint32_t g = __ldg(gid + __ldg(members + m));
+      atomicMax(heights + g, (uint32_t)m - __ldg(goff + g) + 1u);
+    }
+  }
+}
+
+// Pack: one thread per (row p of the rank's block, step kk), kk fastest (the K12 output is read a row at a time)
+template <class Key = F64Key>
+__global__ void __launch_bounds__(256) count_values_pack_kernel(const CvShardArgs a) {
+  const uint64_t n = (uint64_t)__ldg(a.off + a.ng) * a.W;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t p = (uint32_t)(i / a.W), kk = (uint32_t)(i - (uint64_t)p * a.W);
+    const uint32_t q = cv_shard_group(a.off, a.ng, p);
+    const uint32_t o = __ldg(a.off + q), h = __ldg(a.off + q + 1) - o, j = p - o;
+    const uint64_t cell = (uint64_t)(__ldg(a.goff + a.g0 + q) + j) * a.T + a.k0 + kk;
+    const uint32_t c = __ldg(a.cnt + cell);
+    const uint64_t e = (uint64_t)o * a.W + (uint64_t)kk * h + j;
+    a.bkeys[e] = c ? Key::key(__ldg(a.vals + cell)) : ~0ull;
+    a.bcnt[e] = c;
+  }
+}
+
+// Merge, 1: segment offsets (one thread per segment)
+__global__ void __launch_bounds__(256) count_values_merge_segments_kernel(const CvShardArgs a) {
+  const uint32_t n_seg = a.ng * a.W;
+  for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += gridDim.x * blockDim.x) {
+    const uint32_t q = s / a.W, kk = s - q * a.W;
+    const uint32_t o = __ldg(a.off + q), u = __ldg(a.off + q + 1) - o;
+    a.seg_off[s] = o * a.W + kk * u;
+    if (s == n_seg - 1) a.seg_off[n_seg] = a.cells;
+  }
+}
+
+// Merged entry i of the batch: its group q, step kk and place j in segment (q, kk) of U entries
+__device__ __forceinline__ void cv_merge_place(const CvShardArgs& a, uint32_t i, uint32_t& q, uint32_t& kk, uint32_t& j,
+                                               uint32_t& u) {
+  q = cv_shard_group(a.off, a.ng, i / a.W);
+  const uint32_t o = __ldg(a.off + q);
+  u = __ldg(a.off + q + 1) - o;
+  const uint32_t rel = i - o * a.W;
+  kk = rel / u;
+  j = rel - kk * u;
+}
+
+// Merge, 2: every rank's entries of a segment side by side, rank by rank (one thread per merged entry)
+__global__ void __launch_bounds__(256) count_values_merge_arrange_kernel(const CvShardArgs a) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.cells; i += gridDim.x * blockDim.x) {
+    uint32_t q, kk, j, u;
+    cv_merge_place(a, i, q, kk, j, u);
+    const uint32_t* pre = a.hpre + (uint64_t)q * (a.n_ranks + 1);
+    uint32_t r = 0;
+    while (__ldg(pre + r + 1) <= j) ++r;  // the rank whose entries hold place j
+    const uint32_t jr = j - __ldg(pre + r), h = __ldg(pre + r + 1) - __ldg(pre + r);
+    const uint64_t src = (uint64_t)r * a.P + (uint64_t)__ldg(a.hoffs + (uint64_t)q * a.n_ranks + r) * a.W +
+                         (uint64_t)kk * h + jr;
+    a.keys[i] = __ldg(a.gkeys + src);
+    a.kcnt[i] = __ldg(a.gcnt + src);
+  }
+}
+
+// Merge, 3 (after the segmented sort): 1 where a run of equal keys starts in its segment
+__global__ void __launch_bounds__(256) count_values_merge_head_kernel(const CvShardArgs a) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.cells; i += gridDim.x * blockDim.x) {
+    uint32_t q, kk, j, u;
+    cv_merge_place(a, i, q, kk, j, u);
+    a.rank[i] = (j == 0 || a.sorted[i] != a.sorted[i - 1]) ? 1u : 0u;
+  }
+}
+
+// runs of the batch before segment s (the scan is over the whole batch)
+__device__ __forceinline__ uint32_t cv_merge_before(const CvShardArgs& a, uint32_t s) {
+  const uint32_t o = a.seg_off[s];
+  return o ? a.rank[o - 1] : 0u;
+}
+
+// Merge, 4 (after the scans): where each run starts
+__global__ void __launch_bounds__(256) count_values_merge_rank_kernel(const CvShardArgs a) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.cells; i += gridDim.x * blockDim.x) {
+    uint32_t q, kk, j, u;
+    cv_merge_place(a, i, q, kk, j, u);
+    if (!(j == 0 || a.sorted[i] != a.sorted[i - 1])) continue;
+    const uint32_t r = a.rank[i] - cv_merge_before(a, q * a.W + kk) - 1;  // the run's place in its segment
+    a.start[(uint64_t)(__ldg(a.off + q) + r) * a.W + kk] = i;
+  }
+}
+
+// the sum of the sorted counts over entries [b, e) of the batch, e > b
+__device__ __forceinline__ uint32_t cv_merge_sum(const CvShardArgs& a, uint32_t b, uint32_t e) {
+  return a.csum[e - 1] - (b ? a.csum[b - 1] : 0u);
+}
+
+// Merge, 5: one thread per output cell (merged row p of the batch, step kk), row-major like the start table: the j-th
+// run's key and count sum, or 0 / 0 past the runs (and in place of a last run whose counts add up to 0)
+template <class Key = F64Key>
+__global__ void __launch_bounds__(256) count_values_merge_count_kernel(const CvShardArgs a) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.cells; i += gridDim.x * blockDim.x) {
+    const uint32_t p = i / a.W, kk = i - p * a.W;
+    const uint32_t q = cv_shard_group(a.off, a.ng, p);
+    const uint32_t o = __ldg(a.off + q), j = p - o, s = q * a.W + kk;
+    const uint32_t e = a.seg_off[s + 1];  // the segment is not empty: its group has row p
+    const uint32_t runs = a.rank[e - 1] - cv_merge_before(a, s);
+    const uint32_t last = a.start[(uint64_t)(o + runs - 1) * a.W + kk];
+    const uint32_t d = cv_merge_sum(a, last, e) ? runs : runs - 1;  // distinct values at this step
+    const uint64_t out = (uint64_t)(a.out_row0 + p) * a.T + a.k0 + kk;
+    if (j < d) {
+      const uint32_t st = a.start[i];
+      const uint32_t next = j + 1 < runs ? a.start[i + a.W] : e;
+      a.out_val[out] = Key::value(a.sorted[st]);
+      a.out_cnt[out] = cv_merge_sum(a, st, next);
+    } else {
+      a.out_val[out] = 0.0;
+      a.out_cnt[out] = 0u;
+    }
+  }
+}
+
 }  // namespace b2p

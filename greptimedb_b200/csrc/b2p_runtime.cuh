@@ -233,9 +233,9 @@ struct b2p_ctx {
   // sharded topk (b2p_aggregation.cu, shard_*): the merge table over the ranks' blocks, the group sizes all-reduced by
   // b2p_topk_allgather_dev, its candidate block, the gathered blocks and the selection state of one batch
   DevBuf x_table, x_size, x_send, x_recv, x_state;
-  // bytes of blocks and state per batch of the sharded topk and of the sharded quantile (B2P_TOPK_EXCHANGE_BYTES)
+  // bytes of blocks and state per batch of the sharded topk, quantile and count_values (B2P_TOPK_EXCHANGE_BYTES)
   size_t topk_exchange_cap = size_t(128) << 20;
-  long long last_exchange_bytes = 0;  // bytes of this rank's blocks in the last sharded topk or quantile
+  long long last_exchange_bytes = 0;  // bytes of this rank's blocks in the last sharded topk, quantile or count_values
   // quantile: chunk table, state and histograms of the groups of several chunks (b2p_quantile.cuh; bound in quantile_run)
   DevBuf q_table, q_state, q_hist;
   // sharded quantile (b2p_aggregation.cu, quantile_shard_*): this rank's chunk table of a batch, the batch's selection
@@ -244,6 +244,10 @@ struct b2p_ctx {
   // count_values: key and sorted-key buffers, ranks and starts, segment tables, member groups, CUB's temp (bound in
   // count_values_run)
   DevBuf v_keys, v_alt, v_rank, v_seg, v_group, v_tmp;
+  // sharded count_values (b2p_aggregation.cu, cv_shard_*): the merge's counts and their sort buffer; its keys, runs,
+  // segment table and CUB's temp are K12's v_keys / v_alt / v_rank / v_seg / v_tmp, its tables x_table, its block
+  // x_send, the gathered blocks x_recv and the heights x_size
+  DevBuf vx_cnt, vx_alt;
   // subquery: the sample rows of one batch of child rows (ts, val, offsets) and CUB's temp (bound in subquery_run)
   DevBuf sq_ts, sq_val, sq_off, sq_tmp;
   // multi-field range call: the value columns with K16's NaN union applied, and the validity bitmaps of fields 1.. before

@@ -350,3 +350,79 @@ def merge_quantile_digits(phi, vals: np.ndarray, ok: np.ndarray, gid: np.ndarray
                 res = value(p_lo[g]) * (np.float64(1.0) - w) + value(p_hi[g]) * w
             out[g] = np.where(has[g], res, 0.0)
     return out, cnt, passes, passes * G * ((T + 31) // 32) * QUANT_UNIT_BYTES
+
+
+CV_ENTRY_BYTES = 12                           # one (key u64, count u32) entry of a count_values block
+
+
+def merge_count_values(vals: np.ndarray, cnt: np.ndarray, gid: np.ndarray, n_groups: int, group=None):
+    """Host mirror of b2p_count_values_allgather_dev (same exchange, torch.distributed instead of the library's NCCL
+    communicator; used by the gloo tests): this rank's count_values output (vals / cnt [R, T], rows in member order:
+    rows stably sorted by gid, rows of gid >= n_groups last) -> (out [U, T] f64, cnt [U, T] u32, out_goff [G + 1],
+    block bytes sent), the same on every rank.
+      - h_r(g) = the number of leading rows of group g with a count at some step; the heights are all-gathered and
+        group g gets U_g = sum over ranks of h_r(g) rows from out_goff[g];
+      - each rank sends the first h_r(g) rows of each group as (key u64, count u32) entries, a cell without a count as
+        the largest key with count 0, padded to the largest rank's rows; the blocks are all-gathered;
+      - per (group, step) the entries of every rank are sorted by key, each run of equal keys is one value with the sum
+        of its counts, and a run whose counts add up to 0 is no value."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    vals = np.ascontiguousarray(vals, np.float64)
+    cnt = np.asarray(cnt, np.uint32)
+    R, T = vals.shape
+    G = int(n_groups)
+    gid = np.asarray(gid, np.int64)
+    goff = np.searchsorted(np.sort(gid), np.arange(G + 1))
+    has = (cnt != 0).any(axis=1) if T else np.zeros(R, bool)
+    h = np.zeros(G, np.int64)
+    for g in range(G):
+        rows = np.flatnonzero(has[goff[g]:goff[g + 1]])
+        h[g] = rows[-1] + 1 if rows.size else 0
+    parts = [torch.empty(G, dtype=torch.int64) for _ in range(world)]
+    dist.all_gather(parts, torch.from_numpy(h.copy()), group=group)
+    heights = np.stack([p.numpy() for p in parts]) if G else np.zeros((world, 0), np.int64)
+    U = heights.sum(axis=0)
+    out_goff = np.concatenate([[0], np.cumsum(U)]).astype(np.int64)
+    P = int(heights.sum(axis=1).max()) if G else 0
+    bits = vals.view(np.uint64)
+    keys = np.where(bits >> np.uint64(63) != 0, ~bits, bits | np.uint64(1 << 63))
+    mine = np.concatenate([np.arange(goff[g], goff[g] + h[g]) for g in range(G)] + [np.zeros(0, np.int64)])
+    s_key = np.full((P, T), np.uint64(0xFFFFFFFFFFFFFFFF), np.uint64)
+    s_cnt = np.zeros((P, T), np.int64)
+    s_key[:mine.size] = np.where(cnt[mine] != 0, keys[mine], np.uint64(0xFFFFFFFFFFFFFFFF))
+    s_cnt[:mine.size] = cnt[mine]
+    got = []
+    for t in (torch.from_numpy(s_key.view(np.int64)), torch.from_numpy(s_cnt)):
+        out = [torch.empty_like(t) for _ in range(world)]
+        dist.all_gather(out, t, group=group)
+        got.append([o.numpy() for o in out])
+    e_g, e_k, e_key, e_cnt = [], [], [], []
+    for r in range(world):
+        row_g = np.repeat(np.arange(G), heights[r])
+        e_g.append(np.repeat(row_g, T))
+        e_k.append(np.tile(np.arange(T), row_g.size))
+        e_key.append(got[0][r][:row_g.size].view(np.uint64).reshape(-1))
+        e_cnt.append(got[1][r][:row_g.size].reshape(-1))
+    e_g, e_k, e_key, e_cnt = (np.concatenate(x) for x in (e_g, e_k, e_key, e_cnt))
+    U_all = int(out_goff[-1])
+    out_v = np.zeros((U_all, T), np.float64)
+    out_c = np.zeros((U_all, T), np.uint32)
+    if e_g.size:
+        order = np.lexsort((e_key, e_k, e_g))
+        g_s, k_s, key_s, c_s = e_g[order], e_k[order], e_key[order], e_cnt[order]
+        head = np.ones(g_s.size, bool)
+        head[1:] = (g_s[1:] != g_s[:-1]) | (k_s[1:] != k_s[:-1]) | (key_s[1:] != key_s[:-1])
+        starts = np.flatnonzero(head)
+        sums = np.add.reduceat(c_s, starts)
+        keep = starts[sums > 0]
+        sums = sums[sums > 0]
+        g_r, k_r = g_s[keep], k_s[keep]
+        seg = g_r * T + k_r
+        first = np.searchsorted(seg, seg)              # each (group, step)'s first value
+        j = np.arange(seg.size) - first
+        u = key_s[keep]
+        out_v[out_goff[g_r] + j, k_r] = np.where(u >> np.uint64(63) != 0, u ^ np.uint64(1 << 63), ~u).view(np.float64)
+        out_c[out_goff[g_r] + j, k_r] = sums
+    return out_v, out_c, out_goff, P * T * CV_ENTRY_BYTES

@@ -821,6 +821,56 @@ class Context:
         self._check(self._L.b2p_count_values_dev(self._h, _ptr(vals), _ptr(valid), index, T, _ptr(out_val),
                                                  _ptr(out_cnt)))
 
+    def count_values_i64_dev(self, vals, valid, index, T, out_val, out_cnt):
+        """count_values over an int64 grid and the rows of a group index into out_val (int64) / out_cnt [rows,T]."""
+        self._check(self._L.b2p_count_values_i64_dev(self._h, _ptr(vals), _ptr(valid), index, T, _ptr(out_val),
+                                                     _ptr(out_cnt)))
+
+    def count_values_shard_heights_dev(self, local_cnt, index, T, n_groups, n_ranks=1) -> np.ndarray:
+        """h_r(g) of this rank's count_values output (rows in member order): with a communicator of n_ranks ranks every
+        rank's row, the same table everywhere; without one (n_ranks 1) this rank's.  -> host u32 [n_ranks, n_groups].
+        Synchronises the context's stream."""
+        heights = np.zeros((n_ranks, n_groups), np.uint32)
+        self._check(self._L.b2p_count_values_shard_heights_dev(self._h, _ptr(local_cnt), index, T, _ptr(heights)))
+        return heights
+
+    @staticmethod
+    def count_values_shard_rows(heights) -> np.ndarray:
+        """out_goff [n_groups + 1] of a sharded count_values: group g's rows from out_goff[g], sum over ranks of h_r(g)"""
+        u = np.asarray(heights, np.int64).sum(axis=0)
+        return np.concatenate([[0], np.cumsum(u)]).astype(np.int64)
+
+    def count_values_allgather_dev(self, local_val, local_cnt, index, T, heights, out_val, out_cnt, i64=False):
+        """count_values by label over rows sharded across the ranks of the context's communicator (or one rank without
+        one): this rank's count_values output and the heights table -> every rank's out_val / out_cnt
+        [out_goff[G], T] (count_values_shard_rows) receive the merged rows."""
+        h = np.ascontiguousarray(heights, np.uint32)
+        f = self._L.b2p_count_values_allgather_i64_dev if i64 else self._L.b2p_count_values_allgather_dev
+        self._check(f(self._h, _ptr(local_val), _ptr(local_cnt), index, T, _ptr(h), _ptr(out_val), _ptr(out_cnt)))
+
+    def count_values_shard_plan(self, heights, T) -> dict:
+        """The batches of a sharded count_values from the heights table [n_ranks, n_groups]: n_batches and the largest
+        rank block in bytes."""
+        h = np.ascontiguousarray(heights, np.uint32)
+        out = [C.c_uint32(), C.c_uint64()]
+        self._check(self._L.b2p_count_values_shard_plan(self._h, _ptr(h), h.shape[0], h.shape[1], T,
+                                                        *[C.byref(o) for o in out]))
+        return {n: int(o.value) for n, o in zip(("n_batches", "block_bytes"), out)}
+
+    def count_values_shard_pack_dev(self, local_val, local_cnt, index, T, heights, rank, batch, block, i64=False):
+        """This rank's block of one batch: [keys P u64][counts P u32]; last_exchange_bytes() gives P x 12."""
+        h = np.ascontiguousarray(heights, np.uint32)
+        f = self._L.b2p_count_values_shard_pack_i64_dev if i64 else self._L.b2p_count_values_shard_pack_dev
+        self._check(f(self._h, _ptr(local_val), _ptr(local_cnt), index, T, _ptr(h), h.shape[0], rank, batch,
+                      _ptr(block)))
+
+    def count_values_shard_merge_dev(self, heights, T, batch, blocks, out_val, out_cnt, i64=False):
+        """Merges the gathered blocks of one batch ([keys of rank 0 .. R-1][counts of rank 0 .. R-1], rank r's block
+        from row r of heights) into the batch's rows of out_val / out_cnt."""
+        h = np.ascontiguousarray(heights, np.uint32)
+        f = self._L.b2p_count_values_shard_merge_i64_dev if i64 else self._L.b2p_count_values_shard_merge_dev
+        self._check(f(self._h, _ptr(h), h.shape[0], h.shape[1], T, batch, _ptr(blocks), _ptr(out_val), _ptr(out_cnt)))
+
     def subquery_dev(self, p, inner_start, inner_interval, vals, valid, n_rows, T_inner, out, out_valid):
         """Device form of subquery(): vals [n_rows,T_inner] / valid [n_rows,Tw'] into out [n_rows,T] / out_valid."""
         self._check(self._L.b2p_subquery_dev(self._h, C.byref(p), int(inner_start), int(inner_interval), _ptr(vals),

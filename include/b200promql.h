@@ -555,6 +555,70 @@ B2P_API int b2p_quantile_shard_advance_dev(b2p_ctx* ctx, double phi, uint32_t n_
 B2P_API int b2p_count_values_dev(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const b2p_group_index* index,
                                  uint64_t T, double* out_val, uint32_t* out_cnt);
 
+/* count_values(label, v) by label over rows sharded across ranks.  Every rank first runs b2p_count_values_dev (or
+ * b2p_count_values_i64_dev) over its own rows, with an index over the same n_groups global group ids; each series lies
+ * whole on one rank.  That output, local_val / local_cnt [n_rows x T] in the index's member order, is the input here:
+ * per (group, step) it is already the rank's distinct values ascending with their multiplicities, and the global
+ * answer is the union of the ranks' lists with the counts of equal values added (integer sums: the same bits on every
+ * rank whatever the order of the blocks).  No row moves.
+ *
+ * b2p_count_values_shard_heights_dev: h_r(g), the number of leading rows of group g that have a count at some step
+ * (the most distinct values g has at one step on this rank), into the HOST array heights.  With a communicator one
+ * ncclAllGather of the n_groups x 4 B vector fills heights [n_ranks x n_groups] (row r: rank r), the same table on every
+ * rank; without one (n_ranks == 1) it writes [n_groups].  Reads the table back, so it synchronises the stream.  Group g
+ * then has U_g = sum over ranks of h_r(g) output rows (at most its global member count) from out_goff[g] =
+ * sum over g' < g of U_g'; the caller sizes out_val / out_cnt [out_goff[n_groups] x T] from the table.
+ *
+ * b2p_count_values_allgather_dev / _i64_dev: the whole call over the context's communicator.  On return (stream order)
+ * every rank's row out_goff[g] + j is bit for bit row goff[g] + j of b2p_count_values_dev (_i64_dev) over the
+ * concatenation of every rank's rows with the same gid, j < U_g; count 0 and value 0 past the step's distinct values.
+ * Per batch of whole groups over a window of steps each rank packs the first h_r(g) rows of each of its groups as
+ * (key u64, count u32) entries, (group, step)-segment-major, padded to the batch's largest rank block (known to every
+ * rank from heights), two ncclAllGather calls in one group (keys, counts) gather the blocks, and the merge sorts each
+ * (group, step) segment's sum over ranks of h_r(g) entries by key (CUB's segmented sort of pairs) and writes each run
+ * of equal keys with the sum of its counts.  A cell past a rank's distinct values is packed as the largest key with
+ * count 0; a run whose counts add up to 0 is no value, so the largest positive NaN (or INT64_MAX), whose key is the
+ * same, is counted wherever it sorts.  Batches fit the context's exchange cap with their merge scratch (128 MB;
+ * B2P_TOPK_EXCHANGE_BYTES at b2p_create, which also bounds the sharded topk's and quantile's exchanges and must be the
+ * same on every rank); a group too large for the cap alone is a batch of its own over 32 steps.
+ * b2p_last_exchange_bytes() then gives the bytes of this rank's blocks: sum over batches of W_b x (the largest over
+ * ranks of the batch's summed h_r(g)) x 12.  Without a communicator and n_ranks == 1 (no b2p_comm_init) the output is
+ * the first U_g rows of each group of b2p_count_values_dev.
+ *
+ * The steps it is built from, so that one GPU can run R ranks (one context each) through the same kernels; heights is
+ * the HOST table [n_ranks x n_groups], and every step derives the same batches from (heights, n_ranks, n_groups, T, the
+ * cap); no state is kept in the context between calls.  b2p_count_values_shard_plan gives n_batches (0 when no group
+ * has a value) and the largest rank block in bytes.  Then for every batch b:
+ *   b2p_count_values_shard_pack_dev (_i64_dev) on every rank writes its block, [keys: P u64][counts: P u32] for the
+ *     batch's P entries per rank (P x 12 B, at most block_bytes); entries past the rank's own are not written;
+ *   the blocks are gathered section by section: [keys of rank 0 .. R-1][counts of rank 0 .. R-1];
+ *   b2p_count_values_shard_merge_dev (_i64_dev) over the gathered blocks writes the batch's rows of out_val / out_cnt.
+ * B2P_E_INVALID: a NULL argument, a batch out of range, n_ranks > 1 without a communicator in the composed call, a row
+ * of heights for this rank (the composed call's, or pack's `rank`) above its own member count of a group;
+ * B2P_E_TOO_LARGE: a group or batch too large for CUB's int sizes. */
+B2P_API int b2p_count_values_shard_heights_dev(b2p_ctx* ctx, const uint32_t* local_cnt, const b2p_group_index* index,
+                                               uint64_t T, uint32_t* heights);
+B2P_API int b2p_count_values_allgather_dev(b2p_ctx* ctx, const double* local_val, const uint32_t* local_cnt,
+                                           const b2p_group_index* index, uint64_t T, const uint32_t* heights,
+                                           double* out_val, uint32_t* out_cnt);
+B2P_API int b2p_count_values_allgather_i64_dev(b2p_ctx* ctx, const int64_t* local_val, const uint32_t* local_cnt,
+                                               const b2p_group_index* index, uint64_t T, const uint32_t* heights,
+                                               int64_t* out_val, uint32_t* out_cnt);
+B2P_API int b2p_count_values_shard_plan(b2p_ctx* ctx, const uint32_t* heights, int32_t n_ranks, uint32_t n_groups,
+                                        uint64_t T, uint32_t* n_batches, uint64_t* block_bytes);
+B2P_API int b2p_count_values_shard_pack_dev(b2p_ctx* ctx, const double* local_val, const uint32_t* local_cnt,
+                                            const b2p_group_index* index, uint64_t T, const uint32_t* heights,
+                                            int32_t n_ranks, int32_t rank, uint32_t batch, void* block);
+B2P_API int b2p_count_values_shard_pack_i64_dev(b2p_ctx* ctx, const int64_t* local_val, const uint32_t* local_cnt,
+                                                const b2p_group_index* index, uint64_t T, const uint32_t* heights,
+                                                int32_t n_ranks, int32_t rank, uint32_t batch, void* block);
+B2P_API int b2p_count_values_shard_merge_dev(b2p_ctx* ctx, const uint32_t* heights, int32_t n_ranks,
+                                             uint32_t n_groups, uint64_t T, uint32_t batch, const void* blocks,
+                                             double* out_val, uint32_t* out_cnt);
+B2P_API int b2p_count_values_shard_merge_i64_dev(b2p_ctx* ctx, const uint32_t* heights, int32_t n_ranks,
+                                                 uint32_t n_groups, uint64_t T, uint32_t batch, const void* blocks,
+                                                 int64_t* out_val, uint32_t* out_cnt);
+
 /* Subquery fn(<expr>[range:step]) (K13; RangeManipulate(start, end, interval, range) directly over the inner plan,
  * prom_subquery_expr_to_plan, planner.rs:292-332): vals / valid [n_rows x T_inner] are a child's grid on the inner steps
  * inner_start + k * inner_interval (the reference plans them from start - range + inner_interval to end).  Every valid

@@ -405,6 +405,42 @@ extern "C" {
         ctx: *mut b2p_ctx, vals: *const f64, valid: *const u32, index: *const b2p_group_index, t: u64,
         out_val: *mut f64, out_cnt: *mut u32,
     ) -> c_int;
+    /// count_values by label over rows sharded across the communicator's ranks, from each rank's
+    /// `b2p_count_values_dev` output.  `heights` (host) is every rank's row of h_r(g) [n_ranks x n_groups] (one row
+    /// without a communicator); group g gets the sum over ranks of its heights as output rows.
+    pub fn b2p_count_values_shard_heights_dev(
+        ctx: *mut b2p_ctx, local_cnt: *const u32, index: *const b2p_group_index, t: u64, heights: *mut u32,
+    ) -> c_int;
+    pub fn b2p_count_values_allgather_dev(
+        ctx: *mut b2p_ctx, local_val: *const f64, local_cnt: *const u32, index: *const b2p_group_index, t: u64,
+        heights: *const u32, out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    pub fn b2p_count_values_allgather_i64_dev(
+        ctx: *mut b2p_ctx, local_val: *const i64, local_cnt: *const u32, index: *const b2p_group_index, t: u64,
+        heights: *const u32, out_val: *mut i64, out_cnt: *mut u32,
+    ) -> c_int;
+    /// The steps of the sharded count_values: batches, then per batch every rank's block and the merge over the
+    /// gathered blocks ([keys of rank 0 .. R-1][counts of rank 0 .. R-1]).
+    pub fn b2p_count_values_shard_plan(
+        ctx: *mut b2p_ctx, heights: *const u32, n_ranks: i32, n_groups: u32, t: u64, n_batches: *mut u32,
+        block_bytes: *mut u64,
+    ) -> c_int;
+    pub fn b2p_count_values_shard_pack_dev(
+        ctx: *mut b2p_ctx, local_val: *const f64, local_cnt: *const u32, index: *const b2p_group_index, t: u64,
+        heights: *const u32, n_ranks: i32, rank: i32, batch: u32, block: *mut c_void,
+    ) -> c_int;
+    pub fn b2p_count_values_shard_pack_i64_dev(
+        ctx: *mut b2p_ctx, local_val: *const i64, local_cnt: *const u32, index: *const b2p_group_index, t: u64,
+        heights: *const u32, n_ranks: i32, rank: i32, batch: u32, block: *mut c_void,
+    ) -> c_int;
+    pub fn b2p_count_values_shard_merge_dev(
+        ctx: *mut b2p_ctx, heights: *const u32, n_ranks: i32, n_groups: u32, t: u64, batch: u32, blocks: *const c_void,
+        out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    pub fn b2p_count_values_shard_merge_i64_dev(
+        ctx: *mut b2p_ctx, heights: *const u32, n_ranks: i32, n_groups: u32, t: u64, batch: u32, blocks: *const c_void,
+        out_val: *mut i64, out_cnt: *mut u32,
+    ) -> c_int;
     /// fn(<child>[range:step]) over a child's grid [n_rows x T_inner] on the inner steps inner_start + k * inner_interval:
     /// every valid cell of a row is one sample of its series (NaN included); p is the outer grid, range and function
     /// (offset and filter_nan 0).  out [n_rows x T] / out_valid [n_rows x Tw] as b2p_range_eval_dev.
