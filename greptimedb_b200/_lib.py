@@ -52,6 +52,9 @@ EXPORTED_SYMBOLS = [
     "b2p_count_values_shard_heights_dev", "b2p_count_values_allgather_dev", "b2p_count_values_allgather_i64_dev",
     "b2p_count_values_shard_plan", "b2p_count_values_shard_pack_dev", "b2p_count_values_shard_pack_i64_dev",
     "b2p_count_values_shard_merge_dev", "b2p_count_values_shard_merge_i64_dev",
+    "b2p_sort_shard_counts_dev", "b2p_sort_cells_allgather_dev", "b2p_sort_cells_allgather_fields_dev",
+    "b2p_sort_cells_allgather_i64_dev", "b2p_sort_shard_pack_dev", "b2p_sort_shard_pack_i64_dev",
+    "b2p_sort_shard_merge_dev", "b2p_sort_shard_merge_i64_dev",
 ]
 
 
@@ -221,6 +224,14 @@ def load() -> C.CDLL:
         "b2p_count_values_shard_pack_i64_dev": (C.c_int, [vp, vp, vp, vp, u64, vp, i32, i32, u32, vp]),
         "b2p_count_values_shard_merge_dev": (C.c_int, [vp, vp, i32, u32, u64, u32, vp, vp, vp]),
         "b2p_count_values_shard_merge_i64_dev": (C.c_int, [vp, vp, i32, u32, u64, u32, vp, vp, vp]),
+        "b2p_sort_shard_counts_dev": (C.c_int, [vp, vp, u32, u64, vp]),
+        "b2p_sort_cells_allgather_dev": (C.c_int, [vp, i32, vp, vp, vp, u32, u64, vp, vp, vp]),
+        "b2p_sort_cells_allgather_fields_dev": (C.c_int, [vp, i32, vp, i32, vp, vp, u32, u64, vp, vp, vp]),
+        "b2p_sort_cells_allgather_i64_dev": (C.c_int, [vp, i32, vp, vp, vp, u32, u64, vp, vp, vp]),
+        "b2p_sort_shard_pack_dev": (C.c_int, [vp, i32, vp, i32, vp, vp, u32, u64, u64, vp]),
+        "b2p_sort_shard_pack_i64_dev": (C.c_int, [vp, i32, vp, vp, vp, u32, u64, u64, vp]),
+        "b2p_sort_shard_merge_dev": (C.c_int, [vp, i32, i32, vp, i32, vp, vp, vp]),
+        "b2p_sort_shard_merge_i64_dev": (C.c_int, [vp, i32, vp, i32, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)  # AttributeError here means the .so does not match the header

@@ -6,7 +6,7 @@
 //   b2p_group.cu        group index, by-label aggregates, all-reduce of partials, HistogramFold, column reduce
 //   b2p_elementwise.cu  binary operators, instant-vector functions, scalar(), absent(), set operators
 //   b2p_aggregation.cu  topk / bottomk, quantile, count_values
-//   b2p_sort.cu         sort / sort_desc
+//   b2p_sort.cu         sort / sort_desc, and over rows sharded across ranks
 // There is NO CPU fallback anywhere: every entry point either launches the CUDA kernels or returns an error.
 #pragma once
 #include <cuda_runtime.h>
@@ -37,7 +37,8 @@ int k0_fail(uint32_t k0);
 
 // NCCL, bound at run time: libnccl.so.2 is not a link dependency (single-GPU users never need it), and inside a
 // process that already loaded an NCCL (e.g. the one bundled with torch) dlopen hands back that same library.
-// Only the handful of entry points the by-label all-reduce and the sharded topk need; enum values are NCCL's ABI (nccl.h).
+// Only the handful of entry points the by-label all-reduce and the sharded topk, quantile, count_values and sort need
+// (the sharded sort broadcasts each rank's block of its own size); enum values are NCCL's ABI (nccl.h).
 struct Nccl {
   typedef struct ncclComm* comm_t;
   struct unique_id { char internal[128]; };
@@ -48,6 +49,7 @@ struct Nccl {
   int (*CommDestroy)(comm_t) = nullptr;
   int (*AllReduce)(const void*, void*, size_t, int, int, comm_t, cudaStream_t) = nullptr;
   int (*AllGather)(const void*, void*, size_t, int, comm_t, cudaStream_t) = nullptr;
+  int (*Broadcast)(const void*, void*, size_t, int, int, comm_t, cudaStream_t) = nullptr;
   int (*GroupStart)() = nullptr;
   int (*GroupEnd)() = nullptr;
   const char* (*GetErrorString)(int) = nullptr;
@@ -68,6 +70,7 @@ struct Nccl {
     CommDestroy = reinterpret_cast<decltype(CommDestroy)>(sym("ncclCommDestroy"));
     AllReduce = reinterpret_cast<decltype(AllReduce)>(sym("ncclAllReduce"));
     AllGather = reinterpret_cast<decltype(AllGather)>(sym("ncclAllGather"));
+    Broadcast = reinterpret_cast<decltype(Broadcast)>(sym("ncclBroadcast"));
     GroupStart = reinterpret_cast<decltype(GroupStart)>(sym("ncclGroupStart"));
     GroupEnd = reinterpret_cast<decltype(GroupEnd)>(sym("ncclGroupEnd"));
     GetErrorString = reinterpret_cast<decltype(GetErrorString)>(sym("ncclGetErrorString"));
@@ -233,9 +236,10 @@ struct b2p_ctx {
   // sharded topk (b2p_aggregation.cu, shard_*): the merge table over the ranks' blocks, the group sizes all-reduced by
   // b2p_topk_allgather_dev, its candidate block, the gathered blocks and the selection state of one batch
   DevBuf x_table, x_size, x_send, x_recv, x_state;
-  // bytes of blocks and state per batch of the sharded topk, quantile and count_values (B2P_TOPK_EXCHANGE_BYTES)
+  // bytes of blocks and state per batch of the sharded topk, quantile and count_values (B2P_TOPK_EXCHANGE_BYTES; the
+  // sharded sort's exchange is its answer, N x 8 (F + 1) B on every rank, and is not cut into batches)
   size_t topk_exchange_cap = size_t(128) << 20;
-  long long last_exchange_bytes = 0;  // bytes of this rank's blocks in the last sharded topk, quantile or count_values
+  long long last_exchange_bytes = 0;  // bytes of this rank's blocks in the last sharded topk, quantile, count_values or sort
   // quantile: chunk table, state and histograms of the groups of several chunks (b2p_quantile.cuh; bound in quantile_run)
   DevBuf q_table, q_state, q_hist;
   // sharded quantile (b2p_aggregation.cu, quantile_shard_*): this rank's chunk table of a batch, the batch's selection
@@ -256,6 +260,9 @@ struct b2p_ctx {
   DevBuf fd_null;  // one NULL-slot flag per field (null_slots_kernel)
   // sort / sort_desc: row offsets, keys (double-buffered), the alternate cell buffer and CUB's temp (bound in sort_run)
   DevBuf so_off, so_keys, so_cells, so_tmp;
+  // sharded sort (b2p_sort.cu, shard_*): the row-id flag and K14's device count of a pack, and the merge's two run
+  // buffers (ping-pong between rounds); its pair table is x_table, the gathered blocks x_recv and the counts x_size
+  DevBuf sx_flag, sx_run[2];
   // resident CTAs per SM of each persistent kernel instantiation and dynamic shared-memory size (persistent_grid)
   std::map<std::pair<const void*, size_t>, int> blocks_per_sm;
 };

@@ -426,3 +426,56 @@ def merge_count_values(vals: np.ndarray, cnt: np.ndarray, gid: np.ndarray, n_gro
         out_v[out_goff[g_r] + j, k_r] = np.where(u >> np.uint64(63) != 0, u ^ np.uint64(1 << 63), ~u).view(np.float64)
         out_c[out_goff[g_r] + j, k_r] = sums
     return out_v, out_c, out_goff, P * T * CV_ENTRY_BYTES
+
+
+def merge_sorted_runs(desc: bool, vals, ok: np.ndarray, row_id: np.ndarray, group=None):
+    """Host mirror of b2p_sort_cells_allgather_dev (same blocks, torch.distributed instead of the library's NCCL
+    communicator; used by the gloo tests): this rank's grid vals [R, T] (float64, or int64 for the Int64 form; a
+    sequence of F float64 grids for several fields), ok [R, T] bool and row_id [R] (strictly increasing, distinct
+    across ranks) -> (global cells u64 [N], values [N] (a list of F arrays for several fields), bytes sent), the same on
+    every rank.
+      - each rank's valid cells become (key of field 0 .. F-1, global cell row_id[r] * T + k) entries, the key
+        total_key ^ 2^63 (Int64: bits ^ 2^63), inverted for desc, sorted: its run;
+      - the counts are all-gathered, every run is padded to the largest and all-gathered;
+      - the runs are merged by (keys, cell) ascending, and the values decoded from the keys."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    many = isinstance(vals, (list, tuple))
+    grids = [np.asarray(v) for v in vals] if many else [np.asarray(vals)]
+    i64 = grids[0].dtype == np.int64
+    ok = np.asarray(ok, bool)
+    R, T = ok.shape
+    F = len(grids)
+    row_id = np.asarray(row_id, np.uint64)
+    if R > 1 and not (row_id[1:] > row_id[:-1]).all():
+        raise ValueError("row_id must be strictly increasing along the rank's rows")
+    sign = np.uint64(1 << 63)
+    flip = np.uint64(0xFFFFFFFFFFFFFFFF) if desc else np.uint64(0)
+    cells = np.flatnonzero(ok.reshape(-1)).astype(np.uint64)
+    keys = []
+    for g in grids:
+        b = np.ascontiguousarray(g).reshape(-1).view(np.uint64)[cells]
+        k = b ^ sign if i64 else np.where(b >> np.uint64(63) != 0, ~b, b | sign)
+        keys.append(k ^ flip)
+    glob = row_id[cells // np.uint64(T)] * np.uint64(T) + cells % np.uint64(T) if T else cells
+    n = torch.tensor([cells.size], dtype=torch.int64)
+    ns = [torch.zeros(1, dtype=torch.int64) for _ in range(world)]
+    dist.all_gather(ns, n, group=group)
+    ns = [int(x.item()) for x in ns]
+    P = max(ns)
+    block = np.zeros((F + 1, P), np.uint64)
+    if cells.size:
+        order = np.lexsort([glob] + keys[::-1])
+        block[:F, :cells.size] = np.stack(keys)[:, order]
+        block[F, :cells.size] = glob[order]
+    got = [torch.empty((F + 1, P), dtype=torch.int64) for _ in range(world)]
+    dist.all_gather(got, torch.from_numpy(block.view(np.int64)), group=group)
+    runs = np.concatenate([g.numpy().view(np.uint64)[:, :m] for g, m in zip(got, ns)], axis=1)
+    merged = runs[:, np.lexsort([runs[F]] + [runs[f] for f in range(F - 1, -1, -1)])]
+    out = []
+    for f in range(F):
+        u = merged[f] ^ flip
+        bits = u ^ sign if i64 else np.where(u >> np.uint64(63) != 0, u ^ sign, ~u)
+        out.append(bits.view(np.int64 if i64 else np.float64))
+    return merged[F].copy(), (out if many else out[0]), int(cells.size) * 8 * (F + 1)

@@ -889,6 +889,57 @@ class Context:
         self._check(self._L.b2p_sort_cells_fields_dev(self._h, int(bool(desc)), vp, len(vals), _ptr(valid), n_rows, T,
                                                       _ptr(out_cells), _ptr(out_n)))
 
+    def sort_shard_counts_dev(self, valid, n_rows, T, n_ranks=1) -> np.ndarray:
+        """The valid cells of this rank's grid: with a communicator of n_ranks ranks every rank's count, the same table
+        everywhere; without one (n_ranks 1) this rank's.  -> host u64 [n_ranks].  Synchronises the context's stream."""
+        counts = np.zeros(n_ranks, np.uint64)
+        self._check(self._L.b2p_sort_shard_counts_dev(self._h, _ptr(valid), n_rows, T, _ptr(counts)))
+        return counts
+
+    def sort_cells_allgather_dev(self, desc, vals, valid, row_id, n_rows, T, counts, out_cells, out_vals, i64=False):
+        """sort / sort_desc over rows sharded across the ranks of the context's communicator (or one rank without one):
+        vals one device grid [n_rows,T] (int64 with i64) or a sequence of F Float64 grids, row_id [n_rows] u32 the rows'
+        global ordinals, counts the sort_shard_counts_dev table -> every rank's out_cells [N] (u64 global cells
+        row_id * T + k) and out_vals [N] (one tensor, or a sequence of F) in the global order."""
+        c = np.ascontiguousarray(counts, np.uint64)
+        d = int(bool(desc))
+        if isinstance(vals, (list, tuple)):
+            vp, _keep = self._ptr_array(vals)
+            op, _keep_out = self._ptr_array(out_vals)
+            self._check(self._L.b2p_sort_cells_allgather_fields_dev(self._h, d, vp, len(vals), _ptr(valid), _ptr(row_id),
+                                                                    n_rows, T, _ptr(c), _ptr(out_cells), op))
+            return
+        f = self._L.b2p_sort_cells_allgather_i64_dev if i64 else self._L.b2p_sort_cells_allgather_dev
+        self._check(f(self._h, d, _ptr(vals), _ptr(valid), _ptr(row_id), n_rows, T, _ptr(c), _ptr(out_cells),
+                      _ptr(out_vals)))
+
+    def sort_shard_pack_dev(self, desc, vals, valid, row_id, n_rows, T, count, block, i64=False):
+        """This rank's block, [F x count keys u64][count global cells u64], count its entry of the counts table;
+        vals one grid or a sequence of F Float64 grids.  Synchronises the context's stream once (K14's count)."""
+        d = int(bool(desc))
+        if i64:
+            self._check(self._L.b2p_sort_shard_pack_i64_dev(self._h, d, _ptr(vals), _ptr(valid), _ptr(row_id), n_rows,
+                                                            T, int(count), _ptr(block)))
+            return
+        cols = list(vals) if isinstance(vals, (list, tuple)) else [vals]
+        vp, _keep = self._ptr_array(cols)
+        self._check(self._L.b2p_sort_shard_pack_dev(self._h, d, vp, len(cols), _ptr(valid), _ptr(row_id), n_rows, T,
+                                                    int(count), _ptr(block)))
+
+    def sort_shard_merge_dev(self, desc, counts, blocks, out_cells, out_vals, i64=False):
+        """Merges the blocks laid back to back in rank order (block r: counts[r] entries) into out_cells [N] and
+        out_vals [N] (one tensor, or a sequence of F for F fields)."""
+        c = np.ascontiguousarray(counts, np.uint64)
+        d = int(bool(desc))
+        if i64:
+            self._check(self._L.b2p_sort_shard_merge_i64_dev(self._h, d, _ptr(c), c.size, _ptr(blocks),
+                                                             _ptr(out_cells), _ptr(out_vals)))
+            return
+        outs = list(out_vals) if isinstance(out_vals, (list, tuple)) else [out_vals]
+        op, _keep = self._ptr_array(outs)
+        self._check(self._L.b2p_sort_shard_merge_dev(self._h, d, len(outs), _ptr(c), c.size, _ptr(blocks),
+                                                     _ptr(out_cells), op))
+
     def absent_dev(self, valid, n_rows, T, out, out_valid):
         """Device form of absent(): valid [n_rows,Tw] into out [T] / out_valid [Tw].  No host round trip."""
         self._check(self._L.b2p_absent_dev(self._h, _ptr(valid), n_rows, T, _ptr(out), _ptr(out_valid)))

@@ -657,6 +657,66 @@ B2P_API int b2p_sort_cells_fields_dev(b2p_ctx* ctx, int32_t desc, const double* 
                                       const uint32_t* valid, uint32_t n_rows, uint64_t T, uint64_t* out_cells,
                                       uint64_t* out_n);
 
+/* sort / sort_desc over rows sharded across ranks (the reference's MergeSort over a MergeScan of per-datanode sorts,
+ * dist_plan/merge_sort.rs, planner.rs:55-98): every rank sorts its own cells with K14, the sorted runs are exchanged,
+ * and a merge writes the global order on every rank.  Every rank passes its own vals / valid [n_rows x T] and
+ * row_id [n_rows] (device u32), the row's global ordinal in the child's row order: strictly increasing along a rank's
+ * rows (distributed.shard_rows keeps the global order; the call checks it) and distinct across ranks (not checked).
+ * Local cell (r, k) is global cell row_id[r] * T + k, so T <= 2^32.
+ *
+ * b2p_sort_shard_counts_dev: this rank's number of valid cells (K13's count).  With a communicator one ncclAllGather of
+ * 8 B per rank fills the HOST table counts [n_ranks] (entry r: rank r), the same on every rank; without one it fills
+ * counts[0].  Reads the table back, so it synchronises the stream.  N = the sum of counts sizes the outputs.
+ *
+ * b2p_sort_cells_allgather_dev (_fields_dev, _i64_dev): the whole call over the context's communicator.  On return
+ * (stream order) every rank's out_cells [N] holds the global cells and out_vals [N] their values, bit for bit what
+ * b2p_sort_cells_dev (_fields_dev, _i64_dev) writes over the global grid whose row i is the row with row_id i: the f64
+ * total order (Int64: signed order), ascending or descending, equal values in (row, step) order.  The values are
+ * decoded from the exchanged keys (a bijection), so NaN payloads and signed zeros come back bit for bit.  _fields_dev:
+ * vals and out_vals are HOST arrays of n_fields device pointers, the keys compared lexicographically as
+ * b2p_sort_cells_fields_dev does.  Each rank packs its run as one block, [field 0 keys: n u64] .. [field F-1 keys: n
+ * u64][global cells: n u64] (keys flipped for desc), into its place in the gathered buffer, and one ncclBroadcast per
+ * rank with cells, rooted there and of that rank's size, in one group, lays every block back to back on every rank;
+ * when N == 0 no rank makes a collective call.  b2p_last_exchange_bytes() then gives the bytes this rank sent,
+ * n_local x 8 x (n_fields + 1).  The exchange is the answer itself, so it is not cut into batches under
+ * B2P_TOPK_EXCHANGE_BYTES.  Scratch per rank: the gathered blocks (N x 8 (F + 1) B), K14's over the local cells (24 B
+ * per local valid cell, 8 B per row), and the merge's run buffers (N x 8 (F + 1) B, twice from five ranks with cells
+ * on).  The merge is ceil(log2 R) rounds of pairwise merge-path merges (one copy round for one rank), each reading and
+ * writing N x 8 (F + 1) B.  Without a communicator and n_ranks == 1 (no b2p_comm_init) it is b2p_sort_cells_dev's
+ * order with the values beside it.
+ *
+ * The steps it is built from, so that one GPU can run R ranks (one context each) through the same kernels; the context
+ * keeps no state between them.  counts is the HOST table of every rank's count:
+ *   b2p_sort_shard_pack_dev (_i64_dev) writes this rank's block, count = its own entry of the table (8 (F + 1) count B);
+ *   the blocks are laid back to back in rank order, block r of counts[r] entries;
+ *   b2p_sort_shard_merge_dev (_i64_dev) over them writes out_cells / out_vals on every rank.
+ * B2P_E_INVALID: a NULL argument, n_ranks > 1 without a communicator in the composed call, a rank's count that is not
+ * its entry of counts, a row_id that is not strictly increasing; B2P_E_TOO_LARGE: T > 2^32 or n_rows >= 2^31 - 1;
+ * B2P_E_NOMEM: the scratch could not be allocated. */
+B2P_API int b2p_sort_shard_counts_dev(b2p_ctx* ctx, const uint32_t* valid, uint32_t n_rows, uint64_t T,
+                                      uint64_t* counts);
+B2P_API int b2p_sort_cells_allgather_dev(b2p_ctx* ctx, int32_t desc, const double* vals, const uint32_t* valid,
+                                         const uint32_t* row_id, uint32_t n_rows, uint64_t T, const uint64_t* counts,
+                                         uint64_t* out_cells, double* out_vals);
+B2P_API int b2p_sort_cells_allgather_fields_dev(b2p_ctx* ctx, int32_t desc, const double* const* vals,
+                                                int32_t n_fields, const uint32_t* valid, const uint32_t* row_id,
+                                                uint32_t n_rows, uint64_t T, const uint64_t* counts,
+                                                uint64_t* out_cells, double* const* out_vals);
+B2P_API int b2p_sort_cells_allgather_i64_dev(b2p_ctx* ctx, int32_t desc, const int64_t* vals, const uint32_t* valid,
+                                             const uint32_t* row_id, uint32_t n_rows, uint64_t T,
+                                             const uint64_t* counts, uint64_t* out_cells, int64_t* out_vals);
+B2P_API int b2p_sort_shard_pack_dev(b2p_ctx* ctx, int32_t desc, const double* const* vals, int32_t n_fields,
+                                    const uint32_t* valid, const uint32_t* row_id, uint32_t n_rows, uint64_t T,
+                                    uint64_t count, void* block);
+B2P_API int b2p_sort_shard_pack_i64_dev(b2p_ctx* ctx, int32_t desc, const int64_t* vals, const uint32_t* valid,
+                                        const uint32_t* row_id, uint32_t n_rows, uint64_t T, uint64_t count,
+                                        void* block);
+B2P_API int b2p_sort_shard_merge_dev(b2p_ctx* ctx, int32_t desc, int32_t n_fields, const uint64_t* counts,
+                                     int32_t n_ranks, const void* blocks, uint64_t* out_cells,
+                                     double* const* out_vals);
+B2P_API int b2p_sort_shard_merge_i64_dev(b2p_ctx* ctx, int32_t desc, const uint64_t* counts, int32_t n_ranks,
+                                         const void* blocks, uint64_t* out_cells, int64_t* out_vals);
+
 /* ---- Int64 (BIGINT) value columns ------------------------------------------------------------------------------
  * An Int64 cell holds the bits of an int64_t in the same 8-byte slot a Float64 cell uses, so every layout above is
  * unchanged and only the calls that read a value as a number have an Int64 form.  The reference reads such a column

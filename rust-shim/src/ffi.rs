@@ -460,6 +460,42 @@ extern "C" {
         ctx: *mut b2p_ctx, desc: i32, vals: *const *const f64, n_fields: i32, valid: *const u32, n_rows: u32, t: u64,
         out_cells: *mut u64, out_n: *mut u64,
     ) -> c_int;
+    /// sort / sort_desc over rows sharded across the communicator's ranks: every rank's count of valid cells (host
+    /// `counts` [n_ranks], one entry without a communicator), then every rank's sorted run, exchanged and merged into
+    /// the global cells row_id[r] * t + k and their values on every rank.  `row_id` (device) is strictly increasing.
+    pub fn b2p_sort_shard_counts_dev(
+        ctx: *mut b2p_ctx, valid: *const u32, n_rows: u32, t: u64, counts: *mut u64,
+    ) -> c_int;
+    pub fn b2p_sort_cells_allgather_dev(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const f64, valid: *const u32, row_id: *const u32, n_rows: u32, t: u64,
+        counts: *const u64, out_cells: *mut u64, out_vals: *mut f64,
+    ) -> c_int;
+    pub fn b2p_sort_cells_allgather_fields_dev(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const *const f64, n_fields: i32, valid: *const u32, row_id: *const u32,
+        n_rows: u32, t: u64, counts: *const u64, out_cells: *mut u64, out_vals: *const *mut f64,
+    ) -> c_int;
+    pub fn b2p_sort_cells_allgather_i64_dev(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const i64, valid: *const u32, row_id: *const u32, n_rows: u32, t: u64,
+        counts: *const u64, out_cells: *mut u64, out_vals: *mut i64,
+    ) -> c_int;
+    /// The steps of the sharded sort: every rank's block ([keys of field 0 .. F-1][global cells], `count` entries),
+    /// and the merge over the blocks laid back to back in rank order.
+    pub fn b2p_sort_shard_pack_dev(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const *const f64, n_fields: i32, valid: *const u32, row_id: *const u32,
+        n_rows: u32, t: u64, count: u64, block: *mut c_void,
+    ) -> c_int;
+    pub fn b2p_sort_shard_pack_i64_dev(
+        ctx: *mut b2p_ctx, desc: i32, vals: *const i64, valid: *const u32, row_id: *const u32, n_rows: u32, t: u64,
+        count: u64, block: *mut c_void,
+    ) -> c_int;
+    pub fn b2p_sort_shard_merge_dev(
+        ctx: *mut b2p_ctx, desc: i32, n_fields: i32, counts: *const u64, n_ranks: i32, blocks: *const c_void,
+        out_cells: *mut u64, out_vals: *const *mut f64,
+    ) -> c_int;
+    pub fn b2p_sort_shard_merge_i64_dev(
+        ctx: *mut b2p_ctx, desc: i32, counts: *const u64, n_ranks: i32, blocks: *const c_void, out_cells: *mut u64,
+        out_vals: *mut i64,
+    ) -> c_int;
     /// Int64 (BIGINT) value columns: the cells hold i64 bits in the same 8-byte slots.  The instant selector with field 0
     /// Int64 (no stale-NaN test); the by-label aggregate (sum wrapping, min / max signed, written as i64 bits; avg,
     /// stddev, stdvar over (f64)i64); topk / count_values / sort ranking by signed value; the Float64 coercion.
