@@ -266,20 +266,27 @@ def print_rows(expr, tables):
 
 
 def instant_select(ts, vals, offsets, start, end, interval, lookback):
-    """InstantManipulate over F field columns with an Int64 field 0: at each step t the last row of the series with
-    ts <= t is chosen when ts + lookback > t; no stale-NaN test.  Rows strictly increasing in ts.  -> (outs [F,S,T]
-    int64 bits, ok [S,T])"""
+    """InstantManipulate over F field columns with an Int64 field 0: at each step t the row in front of t is chosen,
+    the last row with ts <= t or, where rows share ts == t, the first of them (instant_manipulate.rs:523-541), when
+    it is fresh: ts + lookback > t, or ts == t at lookback 0; no stale-NaN test.  Rows sorted by ts.
+    -> (outs [F,S,T] int64 bits, ok [S,T])"""
     T = (end - start) // interval + 1
     S = len(offsets) - 1
+    steps = start + np.arange(T, dtype=np.int64) * interval
+    cols = [np.ascontiguousarray(v).view(np.int64) for v in vals]
     outs = np.zeros((len(vals), S, T), np.int64)
     ok = np.zeros((S, T), bool)
     for s in range(S):
         r0, r1 = int(offsets[s]), int(offsets[s + 1])
-        for k in range(T):
-            t = start + k * interval
-            j = int(np.searchsorted(ts[r0:r1], t, side="right")) - 1
-            if j >= 0 and ts[r0 + j] + lookback > t:
-                ok[s, k] = True
-                for f, v in enumerate(vals):
-                    outs[f, s, k] = np.ascontiguousarray(v).view(np.int64)[r0 + j]
+        t_s = np.asarray(ts[r0:r1], np.int64)
+        if t_s.size == 0:
+            continue
+        j = np.searchsorted(t_s, steps, side="right") - 1
+        has = j >= 0
+        at = t_s[np.maximum(j, 0)]
+        on_step = has & (at == steps)
+        j = np.where(on_step, np.searchsorted(t_s, steps, side="left"), j)
+        ok[s] = on_step if lookback <= 0 else has & (at + lookback > steps)
+        for f, col in enumerate(cols):
+            outs[f, s] = np.where(ok[s], col[r0 + np.maximum(j, 0)], 0)
     return outs, ok
