@@ -70,7 +70,9 @@ __device__ __forceinline__ double log2_pow2_exact(double v) {
 
 template <int FN>
 __device__ __forceinline__ double instant_fn(double v, double a0, double a1) {
-  if (FN == kFnAbs) return fabs(v);
+  // the sign bit cleared, a NaN's too, as Rust's f64::abs does; PTX abs.f64 leaves a NaN's sign unspecified (it kept
+  // -NaN), and the sign of a NaN decides where it falls in the total order that comparisons and sort use
+  if (FN == kFnAbs) return __longlong_as_double(__double_as_longlong(v) & 0x7FFFFFFFFFFFFFFFll);
   if (FN == kFnCeil) return ceil(v);
   if (FN == kFnFloor) return floor(v);
   if (FN == kFnSqrt) return __dsqrt_rn(v);
