@@ -124,6 +124,16 @@ __global__ void __launch_bounds__(256) series_offsets_kernel(const uint32_t* __r
     for (uint32_t s = threadIdx.x; s <= n_series; s += blockDim.x) offsets[s] = 0;
 }
 
+// Launched after K0, in its stream: once a column has been flagged (bit 0 or 1; the higher bits belong to other
+// operators), K0 has left offsets unwritten (past the last in-range id) or in the order of racing writes (after a
+// decrease).  Every series is made empty, so the kernels queued before b2p_sync reads the verdict read no row.
+__global__ void __launch_bounds__(256) series_offsets_clear_kernel(uint64_t* __restrict__ offsets, uint32_t n_series,
+                                                                   const Status* __restrict__ status) {
+  if ((status->k0_errors & 3u) == 0) return;
+  for (uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; s <= n_series; s += (uint64_t)gridDim.x * blockDim.x)
+    offsets[s] = 0;
+}
+
 // ---------------------------------------------------------------------------------------------
 // K2 fast path.
 //

@@ -405,7 +405,9 @@ static int series_offsets_impl(b2p_ctx* c, const uint32_t* sid, uint64_t n_rows,
   if (blocks == 0) blocks = 1;
   stage_begin(c, 0);
   series_offsets_kernel<<<blocks, 256, 0, c->stream>>>(sid, n_rows, n_series, sid_base, offsets, c->d_k0);
-  c->launches++;
+  series_offsets_clear_kernel<<<capped_grid(c, (uint64_t)n_series + 1, 256, 1), 256, 0, c->stream>>>(offsets, n_series,
+                                                                                                    c->d_k0);
+  c->launches += 2;
   stage_end(c, 0);
   CU(cudaGetLastError());
   return B2P_OK;
@@ -990,9 +992,24 @@ int b2p_synth_fill_dev(b2p_ctx* c, uint64_t series_begin, uint64_t n_series, uin
 /* ---- host-pointer API ------------------------------------------------------------------------ */
 }  // extern "C"
 
+// A host offsets column as every tier reads it, offsets[s] .. offsets[s + 1] without a clamp: non-decreasing, its last
+// entry <= n_rows (rows before its first entry or past its last belong to no series).  The rule b2p_host_scan_series
+// applies; B2P_E_INVALID, checked before anything is copied.
+static int check_host_offsets(const uint64_t* offsets, uint64_t n_rows, uint32_t n_series) {
+  for (uint32_t s = 0; s < n_series; ++s)
+    if (offsets[s + 1] < offsets[s])
+      return fail(B2P_E_INVALID, "offsets decrease at series %u (%llu -> %llu)", s, (unsigned long long)offsets[s],
+                  (unsigned long long)offsets[s + 1]);
+  if (offsets[n_series] > n_rows)
+    return fail(B2P_E_INVALID, "offsets[n_series] = %llu exceeds n_rows = %llu", (unsigned long long)offsets[n_series],
+                (unsigned long long)n_rows);
+  return B2P_OK;
+}
+
 SeriesIn stage_series(Staging& s, const int64_t* ts, const double* val, const uint32_t* sid, uint32_t sid_base,
                       const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series) {
   if (!sid && !offsets_host && !s.rc) s.rc = fail(B2P_E_INVALID, "need sid or offsets_host");
+  if (offsets_host && !s.rc) s.rc = check_host_offsets(offsets_host, n_rows, n_series);
   SeriesIn in{s.in(ts, n_rows * 8), s.in(val, n_rows * 8), nullptr};
   if (offsets_host) {
     in.offsets = s.in(offsets_host, ((size_t)n_series + 1) * 8);
@@ -1147,6 +1164,7 @@ int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, con
     return range_eval_host_simple(c, p, ts, val, sid, offsets_host, n_rows, n_series, T, out, valid_words);
 
   // ---- large inputs: series chunks, double-buffered; H2D(i+1) | K0+K2(i) | D2H(i-1) overlap -----------
+  if (offsets_host && (rc = check_host_offsets(offsets_host, n_rows, n_series))) return rc;
   const uint64_t avg_rows = n_rows / n_series + 1;
   uint32_t C = (uint32_t)(kChunkRows / avg_rows);
   if (C < 64) C = 64;
@@ -1178,7 +1196,7 @@ int b2p_range_eval(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, con
     k.s1 = (uint64_t)k.s0 + C < n_series ? k.s0 + C : n_series;
     k.r0 = i ? chunks[i - 1].r1 : 0;
     k.r1 = offsets_host ? offsets_host[k.s1] : lower_bound_sid(sid, n_rows, k.s1);
-    if (k.r1 < k.r0) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");
+    if (k.r1 < k.r0) return fail(B2P_E_UNSORTED, "series-id column is not non-decreasing");  // (offsets: checked above)
     max_rows = std::max(max_rows, k.r1 - k.r0);
   }
   if (!offsets_host && chunks.back().r1 != n_rows) return fail(B2P_E_UNSORTED, "series id >= n_series");

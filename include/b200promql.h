@@ -209,6 +209,10 @@ B2P_API double b2p_last_kernel_ms(b2p_ctx* ctx, int stage);
 B2P_API int64_t b2p_launch_count(b2p_ctx* ctx);
 
 /* ---- device-pointer API (asynchronous) --------------------------------------------------- */
+/* SeriesDivide: offsets[s] = the first row whose id is >= s, offsets[n_series] = n_rows.  sid must be 16-byte aligned
+ * (B2P_E_INVALID before any launch).  Ids that decrease somewhere, or an id >= n_series, are B2P_E_UNSORTED from the
+ * next b2p_sync; the offsets such a column leaves are all 0 (every series empty), so a call queued on them before the
+ * verdict, such as b2p_range_eval_dev, reads no row. */
 B2P_API int b2p_series_offsets_dev(b2p_ctx* ctx, const uint32_t* sid, uint64_t n_rows, uint32_t n_series,
                            uint64_t* offsets /* [n_series+1] */);
 B2P_API int b2p_range_eval_dev(b2p_ctx* ctx, const b2p_range_params* p, const int64_t* ts, const double* val,
@@ -763,7 +767,11 @@ B2P_API int b2p_host_scan_series(const int64_t* ts, const uint32_t* sid, const u
 
 /* ---- host-pointer API (synchronous; H2D + kernels + D2H inside) ----------------------------- */
 /* sid may be NULL when offsets_host (n_series+1) is given instead. out_ts (may be NULL) receives
- * the T eval timestamps. Pinned host buffers are copied directly; pageable ones are staged. */
+ * the T eval timestamps. Pinned host buffers are copied directly; pageable ones are staged.
+ * Every host entry below that takes offsets_host refuses, with B2P_E_INVALID and before anything is copied, offsets that
+ * decrease or whose last entry exceeds n_rows (the rule of b2p_host_scan_series); rows before offsets_host[0] or past
+ * offsets_host[n_series] belong to no series.  An id column that is not non-decreasing or holds an id >= n_series is
+ * B2P_E_UNSORTED. */
 B2P_API int b2p_range_eval(b2p_ctx* ctx, const b2p_range_params* p, const int64_t* ts, const double* val,
                    const uint32_t* sid, const uint64_t* offsets_host, uint64_t n_rows, uint32_t n_series,
                    double* out, uint32_t* valid_words, int64_t* out_ts);
