@@ -165,11 +165,19 @@ __global__ void __launch_bounds__(256) group_finalize_kernel(int32_t agg, double
 // phase 0: every value becomes its key in place; groups this rank has no row for become the neutral key of min / max
 // (INT64_MAX / INT64_MIN).  phase 1 (after the all-reduce, cnt = global count): keys map back to values (total_key is an
 // involution, NaN payloads survive), groups absent everywhere read 0.0 again, like a freshly built partial.
-__global__ void __launch_bounds__(256) minmax_neutral_kernel(bool is_min, double* val, const uint32_t* cnt, uint64_t n, int phase) {
+// i64: the cells are Int64 partials (b2p_group_aggregate_partial_i64_dev), already their own signed key.
+__global__ void __launch_bounds__(256) minmax_neutral_kernel(bool is_min, double* val, const uint32_t* cnt, uint64_t n, int phase,
+                                                             bool i64 = false) {
   long long* key = reinterpret_cast<long long*>(val);
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    if (phase == 0) key[i] = cnt[i] ? total_key(val[i]) : (is_min ? 0x7fffffffffffffffll : (-0x7fffffffffffffffll - 1));
-    else val[i] = cnt[i] ? __longlong_as_double(total_key(__longlong_as_double(key[i]))) : 0.0;
+    if (phase == 0) {
+      const long long k = i64 ? key[i] : total_key(val[i]);
+      key[i] = cnt[i] ? k : (is_min ? 0x7fffffffffffffffll : (-0x7fffffffffffffffll - 1));
+    } else if (!cnt[i]) {
+      key[i] = 0;
+    } else if (!i64) {
+      val[i] = __longlong_as_double(total_key(__longlong_as_double(key[i])));
+    }
   }
 }
 // (cnt, mean, M2) states of population variance.  phase 0: wsum = cnt * mean, cnt_r = cnt (kept: cnt becomes global);

@@ -1333,6 +1333,86 @@ int b2p_group_quantile(b2p_ctx* c, double phi, const double* vals, const uint32_
   });
 }
 
+int b2p_quantile_allreduce(b2p_ctx* c, double phi, const double* vals, const uint32_t* valid, const uint32_t* gid,
+                           uint32_t n_rows, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_groups == 0 || T == 0) return B2P_OK;  // (every rank has the same n_groups and T)
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
+  double* d_out = s.out(out_val, (size_t)n_groups * T * 8);
+  uint32_t* d_cnt = s.out(out_cnt, (size_t)n_groups * T * 4);
+  return end_indexed(s, gid, n_rows, n_groups, [&](const b2p_group_index* ix) {
+    return b2p_quantile_allreduce_dev(c, phi, d_vals, d_valid, ix, T, d_out, d_cnt);
+  });
+}
+
+}  // extern "C"
+
+namespace {
+// The sharded count_values from host columns: K12 over this rank's rows with an index over the global group ids, the
+// heights table (all-gathered), out_goff from it, then the exchange and merge into [out_goff[n_groups] x T] rows, which
+// must fit cap_rows.  Every rank makes the same collective calls (a rank without rows included).
+int count_values_allgather_host(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* gid,
+                                uint32_t n_rows, uint32_t n_groups, uint64_t T, uint64_t cap_rows, uint32_t* out_goff,
+                                double* out_val, uint32_t* out_cnt, bool i64) {
+  if (!c || !out_goff) return fail(B2P_E_INVALID, "NULL argument");
+  std::fill(out_goff, out_goff + (size_t)n_groups + 1, 0u);
+  if (n_groups == 0 || T == 0) return B2P_OK;  // (every rank has the same n_groups and T)
+  if (n_rows && (!vals || !valid || !gid)) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const size_t Tw = (size_t)((T + 31) / 32);
+  Staging s{c};
+  const double* d_vals = s.in(vals, (size_t)n_rows * T * 8);
+  const uint32_t* d_valid = s.in(valid, (size_t)n_rows * Tw * 4);
+  double* l_val = static_cast<double*>(s.buf((size_t)n_rows * T * 8));
+  uint32_t* l_cnt = static_cast<uint32_t*>(s.buf((size_t)n_rows * T * 4));
+  double* o_val = static_cast<double*>(s.buf(cap_rows * T * 8));
+  uint32_t* o_cnt = static_cast<uint32_t*>(s.buf(cap_rows * T * 4));
+  return end_indexed(s, gid, n_rows, n_groups, [&](const b2p_group_index* ix) {
+    int rc = count_values_dev(c, d_vals, d_valid, ix, T, l_val, l_cnt, i64);
+    const uint32_t R = c->comm ? (uint32_t)c->comm_ranks : 1u;
+    std::vector<uint32_t> heights((size_t)R * n_groups);
+    if (!rc) rc = b2p_count_values_shard_heights_dev(c, l_cnt, ix, T, heights.data());
+    if (rc) return rc;
+    for (uint32_t q = 0; q < n_groups; ++q) {
+      uint64_t u = 0;
+      for (uint32_t r = 0; r < R; ++r) u += heights[(size_t)r * n_groups + q];
+      if (out_goff[q] + u > cap_rows) return fail(B2P_E_TOO_LARGE, "count_values: more merged rows than %llu",
+                                                  (unsigned long long)cap_rows);
+      out_goff[q + 1] = out_goff[q] + (uint32_t)u;
+    }
+    const size_t U = out_goff[n_groups];
+    CU(cudaMemsetAsync(o_val, 0, U * T * 8, c->stream));
+    CU(cudaMemsetAsync(o_cnt, 0, U * T * 4, c->stream));
+    if ((rc = cv_allgather_dev(c, l_val, l_cnt, ix, T, heights.data(), o_val, o_cnt, i64))) return rc;
+    if (U && !out_val) return fail(B2P_E_INVALID, "NULL argument");
+    CU(cudaMemcpyAsync(out_val, o_val, U * T * 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(out_cnt, o_cnt, U * T * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    return B2P_OK;
+  });
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_count_values_allgather(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* gid,
+                               uint32_t n_rows, uint32_t n_groups, uint64_t T, uint64_t cap_rows, uint32_t* out_goff,
+                               double* out_val, uint32_t* out_cnt) {
+  return count_values_allgather_host(c, vals, valid, gid, n_rows, n_groups, T, cap_rows, out_goff, out_val, out_cnt,
+                                     false);
+}
+
+int b2p_count_values_allgather_i64(b2p_ctx* c, const int64_t* vals, const uint32_t* valid, const uint32_t* gid,
+                                   uint32_t n_rows, uint32_t n_groups, uint64_t T, uint64_t cap_rows,
+                                   uint32_t* out_goff, int64_t* out_val, uint32_t* out_cnt) {
+  return count_values_allgather_host(c, reinterpret_cast<const double*>(vals), valid, gid, n_rows, n_groups, T,
+                                     cap_rows, out_goff, reinterpret_cast<double*>(out_val), out_cnt, true);
+}
+
 int b2p_count_values(b2p_ctx* c, const double* vals, const uint32_t* valid, const uint32_t* gid, uint32_t n_rows,
                      uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {
   return count_values_host(c, vals, valid, gid, n_rows, n_groups, T, out_val, out_cnt, false);

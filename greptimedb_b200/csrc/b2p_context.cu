@@ -146,6 +146,7 @@ int b2p_use_own_stream(b2p_ctx* c) {
 int64_t b2p_last_slow_series(b2p_ctx* c) { return c ? c->last_slow : -1; }
 int64_t b2p_last_h2d_bytes(b2p_ctx* c) { return c ? c->last_h2d_bytes : -1; }
 int64_t b2p_last_exchange_bytes(b2p_ctx* c) { return c ? c->last_exchange_bytes : -1; }
+int64_t b2p_last_group_keys_bytes(b2p_ctx* c) { return c ? c->last_group_keys_bytes : -1; }
 int64_t b2p_last_warp_tier_series(b2p_ctx* c) { return c ? c->last_w : -1; }
 int64_t b2p_launch_count(b2p_ctx* c) { return c ? c->launches : -1; }
 
@@ -193,6 +194,11 @@ int b2p_comm_init(b2p_ctx* c, const void* id_bytes, size_t bytes, int n_ranks, i
   CU(cudaEventCreateWithFlags(&c->ev_comm_done, cudaEventDisableTiming));
   CU(cudaEventCreateWithFlags(&c->ev_comm_go, cudaEventDisableTiming));
   return B2P_OK;
+}
+
+int32_t b2p_comm_ranks(b2p_ctx* c, int32_t* rank) {
+  if (rank) *rank = c && c->comm ? c->comm_rank : 0;
+  return c && c->comm ? c->comm_ranks : 0;
 }
 
 int b2p_comm_destroy(b2p_ctx* c) {

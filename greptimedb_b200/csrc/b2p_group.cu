@@ -100,6 +100,15 @@ int b2p_group_aggregate_partial_dev(b2p_ctx* c, int32_t agg, const double* vals,
                               var ? out_mean : nullptr);
 }
 
+int b2p_group_aggregate_partial_i64_dev(b2p_ctx* c, int32_t agg, const int64_t* vals, const uint32_t* valid_words,
+                                        const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T,
+                                        double* out_val, uint32_t* out_cnt) {
+  if (agg != B2P_AGG_SUM && agg != B2P_AGG_MIN && agg != B2P_AGG_MAX)
+    return fail(B2P_E_INVALID, "Int64 partials exist for sum, min and max only (aggregator %d)", agg);
+  return group_aggregate_impl(c, agg, reinterpret_cast<const double*>(vals), valid_words, gid, n_series, n_groups, T,
+                              out_val, out_cnt, 0, nullptr, true);
+}
+
 int b2p_group_index_create_dev(b2p_ctx* c, const uint32_t* gid, uint32_t n_series, uint32_t n_groups,
                                b2p_group_index** out_index) {
   if (!c || !out_index || (!gid && n_series)) return fail(B2P_E_INVALID, "NULL argument");
@@ -213,6 +222,95 @@ int b2p_allreduce_partials_dev(b2p_ctx* c, int32_t agg, double* val, uint32_t* c
     stage_end(c, 4);
   }
   CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// The Int64 partials of SUM / MIN / MAX (b2p_group_aggregate_partial_i64_dev), merged in place on the context's stream.
+//   SUM        val is added as uint64: modular addition is the wrapping sum in any rank order (a signed NCCL sum is not
+//              promised to wrap)
+//   MIN / MAX  val is reduced as int64 after groups absent on a rank (cnt == 0) took INT64_MAX / INT64_MIN; groups absent
+//              everywhere read 0 again
+// cnt is added in both.
+int b2p_allreduce_partials_i64_dev(b2p_ctx* c, int32_t agg, double* val, uint32_t* cnt, uint64_t n) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (agg != B2P_AGG_SUM && agg != B2P_AGG_MIN && agg != B2P_AGG_MAX)
+    return fail(B2P_E_INVALID, "Int64 partials exist for sum, min and max only (aggregator %d)", agg);
+  if (n == 0) return B2P_OK;
+  if (!val || !cnt) return fail(B2P_E_INVALID, "NULL argument");
+  if (!c->comm) {
+    if (c->comm_ranks == 1) return B2P_OK;
+    return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
+  }
+  DeviceGuard g(c->device);
+  const unsigned blocks = capped_grid(c, n, 256, 16);
+  const bool minmax = agg != B2P_AGG_SUM;
+  if (minmax) {
+    minmax_neutral_kernel<<<blocks, 256, 0, c->stream>>>(agg == B2P_AGG_MIN, val, cnt, n, 0, true);
+    c->launches++;
+  }
+  NCCL_TRY(g_nccl.GroupStart());
+  NCCL_TRY(g_nccl.AllReduce(val, val, n, minmax ? Nccl::kInt64 : Nccl::kUint64,
+                            agg == B2P_AGG_MIN ? Nccl::kMin : agg == B2P_AGG_MAX ? Nccl::kMax : Nccl::kSum, c->comm,
+                            c->stream));
+  NCCL_TRY(g_nccl.AllReduce(cnt, cnt, n, Nccl::kUint32, Nccl::kSum, c->comm, c->stream));
+  NCCL_TRY(g_nccl.GroupEnd());
+  if (minmax) {
+    minmax_neutral_kernel<<<blocks, 256, 0, c->stream>>>(agg == B2P_AGG_MIN, val, cnt, n, 1, true);
+    c->launches++;
+  }
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+
+// This rank's byte count into sizes[0], or with a communicator every rank's into sizes[n_ranks] (one all-gather of 8 B
+// per rank); reads the table back, so it synchronises the stream.
+int b2p_group_keys_sizes(b2p_ctx* c, uint64_t bytes, uint64_t* sizes) {
+  if (!c || !sizes) return fail(B2P_E_INVALID, "NULL argument");
+  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
+  DeviceGuard g(c->device);
+  int rc;
+  const uint32_t R = c->comm ? (uint32_t)c->comm_ranks : 1u;
+  if ((rc = c->x_size.ensure((size_t)R * 8))) return rc;
+  unsigned long long* mine = c->x_size.as<unsigned long long>() + (c->comm ? c->comm_rank : 0);
+  const unsigned long long b = bytes;
+  CU(cudaMemcpyAsync(mine, &b, 8, cudaMemcpyHostToDevice, c->stream));
+  if (c->comm) NCCL_TRY(g_nccl.AllGather(mine, c->x_size.p, 1, Nccl::kUint64, c->comm, c->stream));
+  CU(cudaMemcpyAsync(sizes, c->x_size.p, (size_t)R * 8, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return B2P_OK;
+}
+
+// Every rank's block, laid back to back in rank order into the host buffer `out` (sum of sizes bytes): this rank's block
+// goes to its place in one device buffer, then one ncclBroadcast per rank with bytes, in one group, each from that
+// rank's place (no block is padded), and the buffer comes back.  Synchronises the stream.
+int b2p_group_keys_allgather(b2p_ctx* c, const void* block, const uint64_t* sizes, void* out) {
+  if (!c || !sizes) return fail(B2P_E_INVALID, "NULL argument");
+  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
+  const uint32_t R = c->comm ? (uint32_t)c->comm_ranks : 1u, me = c->comm ? (uint32_t)c->comm_rank : 0u;
+  uint64_t N = 0, mine = 0;
+  for (uint32_t r = 0; r < R; ++r) {
+    if (r == me) mine = N;
+    N += sizes[r];
+  }
+  if ((sizes[me] && !block) || (N && !out)) return fail(B2P_E_INVALID, "NULL argument");
+  c->last_group_keys_bytes = (long long)sizes[me];
+  if (N == 0) return B2P_OK;
+  DeviceGuard g(c->device);
+  int rc;
+  if ((rc = c->x_recv.ensure(N))) return rc;
+  unsigned char* all = static_cast<unsigned char*>(c->x_recv.p);
+  if (sizes[me]) CU(cudaMemcpyAsync(all + mine, block, sizes[me], cudaMemcpyHostToDevice, c->stream));
+  if (c->comm) {
+    NCCL_TRY(g_nccl.GroupStart());
+    uint64_t off = 0;
+    for (uint32_t r = 0; r < R; ++r) {
+      if (sizes[r]) NCCL_TRY(g_nccl.Broadcast(all + off, all + off, sizes[r], Nccl::kUint8, (int)r, c->comm, c->stream));
+      off += sizes[r];
+    }
+    NCCL_TRY(g_nccl.GroupEnd());
+  }
+  CU(cudaMemcpyAsync(out, all, N, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
   return B2P_OK;
 }
 
@@ -336,7 +434,53 @@ int group_aggregate_host(b2p_ctx* c, int32_t agg, const double* vals, const uint
     return group_aggregate_impl(c, agg, d_vals, d_valid, d_gid, n_series, n_groups, T, d_out, d_cnt, 0, nullptr, i64);
   });
 }
+
+// The sharded by-label aggregate from host columns: this rank's partials over the global group ids, the all-reduce of
+// every rank's, then the finalise (Float64; an Int64 sum / min / max needs none).  A rank without rows still takes part.
+int group_allreduce_host(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* gid,
+                         uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt, bool i64) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n_groups == 0 || T == 0) return B2P_OK;  // (every rank has the same n_groups and T)
+  if ((n_series && (!vals || !valid_words || !gid)) || !out_val || !out_cnt) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  const uint32_t Tw = (uint32_t)((T + 31) / 32);
+  const uint64_t n = (uint64_t)n_groups * T;
+  const bool var = agg == B2P_AGG_STDDEV || agg == B2P_AGG_STDVAR;
+  Staging s{c};
+  auto in = [&](const auto* host, size_t bytes) {  // (a rank without rows stages an empty buffer, never NULL)
+    return n_series ? s.in(host, bytes) : static_cast<decltype(host)>(s.buf(0));
+  };
+  const double* d_vals = in(vals, (size_t)n_series * T * 8);
+  const uint32_t* d_valid = in(valid_words, (size_t)n_series * Tw * 4);
+  const uint32_t* d_gid = in(gid, (size_t)n_series * 4);
+  double* d_out = s.out(out_val, n * 8);
+  uint32_t* d_cnt = s.out(out_cnt, n * 4);
+  double* d_mean = var ? static_cast<double*>(s.buf(n * 8)) : nullptr;
+  return s.end([&] {
+    int rc = i64 ? b2p_group_aggregate_partial_i64_dev(c, agg, reinterpret_cast<const int64_t*>(d_vals), d_valid, d_gid,
+                                                       n_series, n_groups, T, d_out, d_cnt)
+                 : b2p_group_aggregate_partial_dev(c, agg, d_vals, d_valid, d_gid, n_series, n_groups, T, d_out, d_cnt,
+                                                   d_mean);
+    if (!rc) rc = i64 ? b2p_allreduce_partials_i64_dev(c, agg, d_out, d_cnt, n)
+                      : b2p_allreduce_partials_dev(c, agg, d_out, d_cnt, d_mean, n);
+    if (!rc && !i64) rc = b2p_group_finalize_dev(c, agg, d_out, d_cnt, n);
+    return rc;
+  });
+}
 }  // namespace
+
+int b2p_group_aggregate_allreduce(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words,
+                                  const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val,
+                                  uint32_t* out_cnt) {
+  return group_allreduce_host(c, agg, vals, valid_words, gid, n_series, n_groups, T, out_val, out_cnt, false);
+}
+
+int b2p_group_aggregate_allreduce_i64(b2p_ctx* c, int32_t agg, const int64_t* vals, const uint32_t* valid_words,
+                                      const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T,
+                                      double* out_val, uint32_t* out_cnt) {
+  return group_allreduce_host(c, agg, reinterpret_cast<const double*>(vals), valid_words, gid, n_series, n_groups, T,
+                              out_val, out_cnt, true);
+}
 
 int b2p_group_aggregate(b2p_ctx* c, int32_t agg, const double* vals, const uint32_t* valid_words, const uint32_t* gid,
                         uint32_t n_series, uint32_t n_groups, uint64_t T, double* out_val, uint32_t* out_cnt) {

@@ -344,6 +344,182 @@ bool keeps_tsid(const Labels& in, std::vector<int> cols) {
   return cols.size() == in.names.size() && (cols.empty() || cols.front() >= 0);
 }
 
+// ---- the group-label agreement of a sharded node (b2p_group_keys_merge's block layout, include/b200promql.h) ----
+constexpr uint32_t kNullTag = 0xFFFFFFFFu, kFlagTsid = 1u;
+
+// a block: the rank's row count and field types, then its groups in Labels order, each its tuple over the group
+// columns and, with kFlagTsid, its __tsid
+struct KeyBlock {
+  uint32_t n_labels = 0, flags = 0;
+  uint64_t n_rows = 0;
+  std::vector<uint8_t> types;              // [field] enum ValueType
+  std::vector<std::vector<Label>> tuples;  // [group][label]
+  std::vector<uint64_t> ids;               // [group] with kFlagTsid
+};
+
+// What every rank of a sharded node agrees: the global group table in Labels order (with ids where kept), this rank's
+// groups -> global ids, the rows of all ranks and the field types of the ranks that have rows
+struct Agreement {
+  Labels labels;
+  uint32_t n_groups = 0;
+  std::vector<uint32_t> l2g;  // [this rank's place] -> global id
+  uint64_t n_rows = 0;
+  std::vector<ValueType> types;
+};
+
+bool tuple_less(const std::vector<Label>& a, const std::vector<Label>& b) {
+  for (size_t t = 0; t < a.size(); ++t) {
+    if (Labels::less(a[t], b[t])) return true;
+    if (Labels::less(b[t], a[t])) return false;
+  }
+  return false;
+}
+
+template <class T>
+void put(std::string& out, T v) {
+  out.append(reinterpret_cast<const char*>(&v), sizeof v);  // (little-endian hosts only, as the project's targets are)
+}
+
+// `groups` [place] (Labels order), with their ids when `tsid`; the block of a rank with n_rows rows of these types
+std::string serialize_keys(const Labels& groups, uint32_t G, bool tsid, uint64_t n_rows,
+                           const std::vector<ValueType>& types) {
+  std::string out;
+  put<uint32_t>(out, G);
+  put<uint32_t>(out, (uint32_t)groups.values.size());
+  put<uint32_t>(out, tsid ? kFlagTsid : 0u);
+  put<uint32_t>(out, (uint32_t)types.size());
+  put<uint64_t>(out, n_rows);
+  for (ValueType t : types) put<uint8_t>(out, (uint8_t)t);
+  for (uint32_t g = 0; g < G; ++g) {
+    if (tsid) put<uint64_t>(out, groups.ids[g]);
+    for (const std::vector<Label>& col : groups.values) {
+      const Label& v = col[g];
+      put<uint32_t>(out, v ? (uint32_t)v->size() : kNullTag);
+      if (v) out += *v;
+    }
+  }
+  return out;
+}
+
+KeyBlock parse_keys(const uint8_t* p, uint64_t size, int rank) {
+  auto bad = [&](const char* what) {
+    return PlanError(ErrorKind::Plan, "b2p_group_keys_merge: block " + std::to_string(rank) + " " + what);
+  };
+  uint64_t at = 0;
+  auto get = [&](auto& v) {
+    if (size - at < sizeof v) throw bad("is truncated");
+    std::memcpy(&v, p + at, sizeof v);
+    at += sizeof v;
+  };
+  KeyBlock b;
+  uint32_t G = 0, F = 0;
+  get(G);
+  get(b.n_labels);
+  get(b.flags);
+  get(F);
+  get(b.n_rows);
+  if (b.flags & ~kFlagTsid) throw bad("has unknown flags");
+  if ((G == 0) != (b.n_rows == 0)) throw bad("has rows without groups or groups without rows");
+  if (F > size - at) throw bad("is truncated");
+  b.types.resize(F);
+  for (uint8_t& t : b.types) {
+    get(t);
+    if (t > (uint8_t)ValueType::Count) throw bad("has an unknown field type");
+  }
+  for (uint32_t g = 0; g < G; ++g) {
+    if (b.flags & kFlagTsid) get(b.ids.emplace_back());
+    std::vector<Label> t(b.n_labels);
+    for (Label& v : t) {
+      uint32_t n = 0;
+      get(n);
+      if (n == kNullTag) continue;
+      if (size - at < n) throw bad("is truncated");
+      v = std::string(reinterpret_cast<const char*>(p + at), n);
+      at += n;
+    }
+    if (!b.tuples.empty() && !tuple_less(b.tuples.back(), t)) throw bad("is not strictly in label order");
+    b.tuples.push_back(std::move(t));
+  }
+  if (at != size) throw bad("is longer than its groups");
+  return b;
+}
+
+// The R-way merge: the global table in Labels order without duplicates (a duplicate keeps the lowest rank's id), and
+// l2g [block rank's groups] -> global id.  The heads are scanned in rank order and replaced on a strictly smaller tuple
+// only, so the table is a function of the blocks alone, whichever rank merges.  The field types are those of the ranks
+// with rows, which must agree (a rank without rows has read no batch, so its types are only a default).
+Agreement merge_keys(const std::vector<KeyBlock>& blocks, int rank) {
+  const KeyBlock& b0 = blocks.at(0);
+  Agreement a;
+  a.labels.tsid = (b0.flags & kFlagTsid) != 0;
+  a.labels.values.resize(b0.n_labels);
+  const KeyBlock* typed = nullptr;
+  for (size_t r = 0; r < blocks.size(); ++r) {
+    const KeyBlock& b = blocks[r];
+    if (b.n_labels != b0.n_labels || b.flags != b0.flags || b.types.size() != b0.types.size())
+      throw PlanError(ErrorKind::Plan, "b2p_group_keys_merge: block " + std::to_string(r) +
+                                           " is unlike block 0 in its labels, flags or fields");
+    a.n_rows += b.n_rows;
+    if (!b.n_rows) continue;
+    if (typed && typed->types != b.types)
+      throw PlanError(ErrorKind::Plan, "a sharded node's ranks read different value types (block " + std::to_string(r) +
+                                           " against the first rank with rows)");
+    if (!typed) typed = &b;
+  }
+  for (uint8_t t : (typed ? typed : &b0)->types) a.types.push_back((ValueType)t);
+  a.l2g.assign(blocks.at((size_t)rank).tuples.size(), 0u);
+  std::vector<size_t> head(blocks.size(), 0);
+  for (;; ++a.n_groups) {
+    int m = -1;
+    for (size_t r = 0; r < blocks.size(); ++r)
+      if (head[r] < blocks[r].tuples.size() && (m < 0 || tuple_less(blocks[r].tuples[head[r]], blocks[m].tuples[head[m]])))
+        m = (int)r;
+    if (m < 0) break;
+    const std::vector<Label>& t = blocks[m].tuples[head[m]];
+    for (size_t c = 0; c < t.size(); ++c) a.labels.values[c].push_back(t[c]);
+    if (a.labels.tsid) a.labels.ids.push_back(blocks[m].ids[head[m]]);
+    for (size_t r = 0; r < blocks.size(); ++r) {  // every head equal to t (none is smaller)
+      if (head[r] >= blocks[r].tuples.size() || (r != (size_t)m && tuple_less(t, blocks[r].tuples[head[r]]))) continue;
+      if ((int)r == rank) a.l2g[head[r]] = a.n_groups;
+      ++head[r];
+    }
+  }
+  return a;
+}
+
+// The agreement of a sharded node over r's rows grouped as `groups` (their ids when `groups.labels.tsid`): this rank's
+// block exchanged over the context's communicator and merged.  r takes the agreed field types, so a rank that read no
+// batch folds with the types of the ranks that did, and every rank makes the same collective calls.
+Agreement agree_groups(b2p_ctx* ctx, const Groups& groups, NodeResult& r) {
+  int32_t rank = 0;
+  const int32_t R = b2p_comm_ranks(ctx, &rank);
+  const std::string mine = serialize_keys(groups.labels, (uint32_t)groups.first.size(), groups.labels.tsid, r.rows,
+                                          r.types);
+  std::vector<uint64_t> sizes((size_t)R);
+  check(b2p_group_keys_sizes(ctx, mine.size(), sizes.data()), ErrorKind::Execution);
+  std::vector<uint8_t> all((size_t)std::accumulate(sizes.begin(), sizes.end(), uint64_t(0)));
+  check(b2p_group_keys_allgather(ctx, mine.data(), sizes.data(), all.data()), ErrorKind::Execution);
+  std::vector<KeyBlock> blocks;
+  uint64_t off = 0;
+  for (int32_t q = 0; q < R; ++q) {
+    blocks.push_back(parse_keys(all.data() + off, sizes[(size_t)q], q));
+    off += sizes[(size_t)q];
+  }
+  Agreement a = merge_keys(blocks, rank);
+  a.labels.names = groups.labels.names;
+  r.types = a.types;
+  return a;
+}
+
+// Groups over the global table of a sharded node: the ids become global ids, the places the identity (the global ids
+// are already in label order)
+void take_global(Groups& groups, Agreement& a) {
+  for (uint32_t& id : groups.id) id = a.l2g[groups.rank[id]];
+  groups.rank.resize(a.n_groups);
+  std::iota(groups.rank.begin(), groups.rank.end(), 0u);
+  groups.labels = std::move(a.labels);
+}
+
 // Aggregators beyond enum b2p_agg that the aggregate node offers
 constexpr int kAggGroup = B2P_AGG_STDVAR + 1, kAggQuantile = B2P_AGG_STDVAR + 2;
 
@@ -353,13 +529,18 @@ constexpr int kAggGroup = B2P_AGG_STDVAR + 1, kAggQuantile = B2P_AGG_STDVAR + 2;
 // non-zero) or kAggQuantile (param = φ).  Each field is folded by its own call over the same group ids; the counts
 // depend on the shared validity alone, so field 0's decide the cells.  Sets the rows, labels, grids, types and column
 // layout, drops a counted column; keeps T, the fields and the time index.  A group keeps its first member's __tsid
-// where keeps_tsid says so.
-void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& cols, NodeResult& r) {
+// where keeps_tsid says so.  `sharded` (a sharded node over a communicator): the groups are the global table every rank
+// agrees (agree_groups), and each fold merges every rank's partials, so every rank ends with the same result.
+void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& cols, NodeResult& r, bool sharded = false) {
   Groups groups = group_rows(r.labels, cols, r.rows);
   if (keeps_tsid(r.labels, cols)) {
     groups.labels.tsid = true;
     groups.labels.ids.resize(groups.first.size());
     for (size_t g = 0; g < groups.first.size(); ++g) groups.labels.ids[groups.rank[g]] = r.labels.ids[groups.first[g]];
+  }
+  if (sharded) {
+    Agreement a = agree_groups(ctx, groups, r);
+    take_global(groups, a);
   }
   const uint32_t G = (uint32_t)groups.rank.size(), Tw = r.Tw, F = r.F;
   const size_t T = (size_t)r.T;
@@ -370,19 +551,30 @@ void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& 
   std::vector<ValueType> types(F, ValueType::Float64);
   for (uint32_t f = 0; f < F; ++f) {
     const bool i64 = r.types[f] == ValueType::Int64 && op != kAggQuantile && op != kAggGroup;
-    if (op == kAggQuantile) field_to_f64(ctx, r, f);
+    // the sharded Int64 avg / stddev / stdvar / count read the Float64 coercion, which is what K3 reads in one pass
+    if (op == kAggQuantile || (sharded && i64 && !int_result)) field_to_f64(ctx, r, f);
     if (int_result && r.types[f] == ValueType::Int64) types[f] = ValueType::Int64;
-    if (G == 0 || T == 0) continue;
+    if (G == 0 || T == 0) continue;  // (G and T are the same on every rank)
     double* gv = gval.data() + (size_t)f * G * T;
     uint32_t* gc = f == 0 ? gcnt.data() : fcnt.data();
     const int agg = op == kAggGroup ? B2P_AGG_COUNT : op;
-    check(op == kAggQuantile ? b2p_group_quantile(ctx, param, r.field(f), r.valid.data(), groups.id.data(), r.rows, G,
-                                                  (uint64_t)T, gv, gc)
-          : i64 ? b2p_group_aggregate_i64(ctx, agg, reinterpret_cast<const int64_t*>(r.field(f)), r.valid.data(),
-                                          groups.id.data(), r.rows, G, (uint64_t)T, gv, gc)
-                : b2p_group_aggregate(ctx, agg, r.field(f), r.valid.data(), groups.id.data(), r.rows, G, (uint64_t)T,
-                                      gv, gc),
-          ErrorKind::Execution);
+    if (sharded)
+      check(op == kAggQuantile ? b2p_quantile_allreduce(ctx, param, r.field(f), r.valid.data(), groups.id.data(), r.rows,
+                                                        G, (uint64_t)T, gv, gc)
+            : i64 && int_result ? b2p_group_aggregate_allreduce_i64(ctx, agg, reinterpret_cast<const int64_t*>(r.field(f)),
+                                                                    r.valid.data(), groups.id.data(), r.rows, G,
+                                                                    (uint64_t)T, gv, gc)
+                                : b2p_group_aggregate_allreduce(ctx, agg, r.field(f), r.valid.data(), groups.id.data(),
+                                                                r.rows, G, (uint64_t)T, gv, gc),
+            ErrorKind::Execution);
+    else
+      check(op == kAggQuantile ? b2p_group_quantile(ctx, param, r.field(f), r.valid.data(), groups.id.data(), r.rows, G,
+                                                    (uint64_t)T, gv, gc)
+            : i64 ? b2p_group_aggregate_i64(ctx, agg, reinterpret_cast<const int64_t*>(r.field(f)), r.valid.data(),
+                                            groups.id.data(), r.rows, G, (uint64_t)T, gv, gc)
+                  : b2p_group_aggregate(ctx, agg, r.field(f), r.valid.data(), groups.id.data(), r.rows, G, (uint64_t)T,
+                                        gv, gc),
+            ErrorKind::Execution);
   }
   r.types = std::move(types);
   r.labels = std::move(groups.labels);
@@ -795,7 +987,7 @@ void PromRangePlan::compute(NodeResult& r) {
     if (agg_id_ >= 0) {
       // prom_aggr_expr_to_plan: group keys = by-labels + eval ts; output sorted by (labels asc, ts asc).  Over an id key
       // the by-label is the id's decimal string, so those rows sort as strings ("10" before "9").
-      aggregate_rows(ctx_, agg_id_, 0.0, series_.columns(args_.by_columns), r);
+      aggregate_rows(ctx_, agg_id_, 0.0, series_.columns(args_.by_columns), r, sharded_ && sharded_run("GpuPromRangeExec"));
       r.value_names = {args_.aggregate + "(" + (fn_id_ >= 0 ? args_.function : args_.field_columns[0]) + ")"};
     }
   }
@@ -1104,6 +1296,23 @@ void PlanNode::require(const char* node, std::initializer_list<const PlanNode*> 
   if (device && !ctx_) throw PlanError(ErrorKind::Internal, std::string(node) + ": NULL context");
   for (const PlanNode* c : children)
     if (!c) throw PlanError(ErrorKind::Plan, std::string(node) + ": NULL child");
+}
+
+bool PlanNode::sharded_run(const char* node) const {
+  if (b2p_comm_ranks(ctx_, nullptr) == 0) return false;
+  std::vector<const PlanNode*> todo = children();
+  while (!todo.empty()) {
+    const PlanNode* n = todo.back();
+    todo.pop_back();
+    if (n->sharded_)
+      throw PlanError(ErrorKind::Plan, std::string(node) + ": a sharded node below a sharded node: its result is "
+                                                           "already on every rank, and merging it again would count every copy");
+    if (const char* what = n->cross_row())
+      throw PlanError(ErrorKind::Plan, std::string(node) + ": a sharded node over " + what + ", which computes over rows "
+                                                           "other ranks hold: its result on one rank is not the query's");
+    for (const PlanNode* c : n->children()) todo.push_back(c);
+  }
+  return true;
 }
 
 void PlanNode::run(NodeResult& r) {
@@ -1622,13 +1831,14 @@ AggregatePlan::AggregatePlan(b2p_ctx* ctx, const std::string& op, double param, 
 }
 
 void AggregatePlan::compute(NodeResult& r) {
+  const bool sharded = sharded_ && sharded_run("GpuPromAggregateExec");
   child_->run(r);
   // the reference would re-attach the tag columns of an id-keyed input (ensure_tag_columns_available); this layer has
   // only the id, so it can group such a node as a whole and nothing else.  group(): planner.rs:2815-2823
   check_child(r, {{Shape::Int32, "GpuPromAggregateExec: an Int32 value column is not supported by this node"},
                   {Shape::IdKeyed, modifier_ == Modifier::None ? "" : "GpuPromAggregateExec: an id-keyed (__tsid) child can only be aggregated without by / without"},
                   {Shape::MultiField, op_ == kAggGroup ? "Multi fields calculation is not supported in group()" : ""}});
-  aggregate_rows(ctx_, op_, param_, group_columns(r.labels, modifier_, labels_), r);  // one aggregate per field
+  aggregate_rows(ctx_, op_, param_, group_columns(r.labels, modifier_, labels_), r, sharded);  // one aggregate per field
   for (std::string& value : r.value_names)
     value = op_ == kAggGroup      ? "max(" + float_literal(1.0) + ")"
             : op_ == kAggQuantile ? "quantile(" + float_literal(param_) + "," + value + ")"
@@ -1643,6 +1853,7 @@ CountValuesPlan::CountValuesPlan(b2p_ctx* ctx, std::string label, std::shared_pt
 }
 
 void CountValuesPlan::compute(NodeResult& r) {
+  const bool sharded = sharded_ && sharded_run("GpuPromCountValuesExec");
   child_->run(r);
   // planner.rs:2874-2879; keep_tsid is false for count_values (planner.rs:402): as for AggregatePlan, an id-keyed
   // child groups as a whole only
@@ -1656,24 +1867,40 @@ void CountValuesPlan::compute(NodeResult& r) {
   for (int c : cols) clash = clash || r.labels.names[(size_t)c] == label_;
   if (clash) throw PlanError(ErrorKind::Plan, "GpuPromCountValuesExec: the label \"" + label_ + "\" names another column of the result");
   Groups groups = group_rows(r.labels, cols, r.rows);
+  uint64_t cap = 0;  // sharded: the rows of every rank, which bound the merged rows
+  if (sharded) {
+    Agreement a = agree_groups(ctx_, groups, r);
+    cap = a.n_rows;
+    take_global(groups, a);
+  }
   const uint32_t G = (uint32_t)groups.rank.size(), R = r.rows, Tw = r.Tw;
   const size_t T = (size_t)r.T;
-  std::vector<double> cval((size_t)R * T);
-  std::vector<uint32_t> ccnt((size_t)R * T);
-  if (R > 0 && T > 0)
-    check(r.is(0, ValueType::Int64) ? b2p_count_values_i64(ctx_, reinterpret_cast<const int64_t*>(r.val.data()), r.valid.data(),
-                                             groups.id.data(), R, G, (uint64_t)T, reinterpret_cast<int64_t*>(cval.data()),
-                                             ccnt.data())
-                      : b2p_count_values(ctx_, r.val.data(), r.valid.data(), groups.id.data(), R, G, (uint64_t)T,
-                                         cval.data(), ccnt.data()),
-          ErrorKind::Execution);
-  // the counted values keep the child's type (count_values.result:31-62)
-  r.counted = CountedColumn{label_, r.is(0, ValueType::Int64) ? ValueType::Int64 : ValueType::Float64, {}};
-  r.types = {ValueType::Count};
-  // b2p_count_values' rows: group g's members (rank rows) from goff[g]
+  const bool i64 = r.is(0, ValueType::Int64);
+  // b2p_count_values' rows: group g's members (rank rows) from goff[g]; sharded, the merged rows of group g from goff[g]
   std::vector<uint32_t> goff((size_t)G + 1, 0u), place(G);
-  for (uint32_t q = 0; q < R; ++q) ++goff[groups.id[q] + 1];
-  std::partial_sum(goff.begin(), goff.end(), goff.begin());
+  std::vector<double> cval((sharded ? cap : R) * T);
+  std::vector<uint32_t> ccnt(cval.size());
+  if (sharded) {
+    check(i64 ? b2p_count_values_allgather_i64(ctx_, reinterpret_cast<const int64_t*>(r.val.data()), r.valid.data(),
+                                               groups.id.data(), R, G, (uint64_t)T, cap, goff.data(),
+                                               reinterpret_cast<int64_t*>(cval.data()), ccnt.data())
+              : b2p_count_values_allgather(ctx_, r.val.data(), r.valid.data(), groups.id.data(), R, G, (uint64_t)T,
+                                           cap, goff.data(), cval.data(), ccnt.data()),
+          ErrorKind::Execution);
+  } else {
+    if (R > 0 && T > 0)
+      check(i64 ? b2p_count_values_i64(ctx_, reinterpret_cast<const int64_t*>(r.val.data()), r.valid.data(),
+                                       groups.id.data(), R, G, (uint64_t)T, reinterpret_cast<int64_t*>(cval.data()),
+                                       ccnt.data())
+                : b2p_count_values(ctx_, r.val.data(), r.valid.data(), groups.id.data(), R, G, (uint64_t)T, cval.data(),
+                                   ccnt.data()),
+            ErrorKind::Execution);
+    for (uint32_t q = 0; q < R; ++q) ++goff[groups.id[q] + 1];
+    std::partial_sum(goff.begin(), goff.end(), goff.begin());
+  }
+  // the counted values keep the child's type (count_values.result:31-62)
+  r.counted = CountedColumn{label_, i64 ? ValueType::Int64 : ValueType::Float64, {}};
+  r.types = {ValueType::Count};
   for (uint32_t g = 0; g < G; ++g) place[groups.rank[g]] = g;
   // output rows: the groups in label order, each with its rank rows that hold a value at some step
   std::vector<uint32_t> src, lab, first(1, 0u);
@@ -2356,6 +2583,39 @@ int b2p_plan_push_batch(b2p_plan* plan, struct ArrowArray* batch, struct ArrowSc
 int b2p_plan_execute(b2p_plan* plan, struct ArrowArray* out, struct ArrowSchema* out_schema) {
   if (!plan) return B2P_E_INVALID;
   return guarded([&] { plan->node->execute(out, out_schema); });
+}
+
+int b2p_plan_set_sharded(b2p_plan* plan) {
+  if (!plan) return B2P_E_INVALID;
+  return guarded([&] {
+    if (!plan->node->set_sharded())
+      throw b2p::PlanError(b2p::ErrorKind::Plan, "b2p_plan_set_sharded: only an aggregate node, a count_values node "
+                                                 "or a range / instant leaf with an aggregate stage has a sharded form");
+  });
+}
+
+int b2p_group_keys_merge(const void* const* blocks, const uint64_t* sizes, int32_t n_ranks, int32_t rank,
+                         void* out_table, uint64_t* out_table_bytes, uint32_t* n_groups, uint32_t* local_to_global) {
+  return guarded([&] {
+    if (!blocks || !sizes || n_ranks < 1 || rank < 0 || rank >= n_ranks || !out_table || !out_table_bytes || !n_groups)
+      throw b2p::PlanError(b2p::ErrorKind::Plan, "b2p_group_keys_merge: bad arguments");
+    std::vector<b2p::KeyBlock> parsed;
+    uint64_t total = 0;
+    for (int32_t r = 0; r < n_ranks; ++r) {
+      if (!blocks[r] && sizes[r]) throw b2p::PlanError(b2p::ErrorKind::Plan, "b2p_group_keys_merge: NULL block");
+      parsed.push_back(b2p::parse_keys(static_cast<const uint8_t*>(blocks[r]), sizes[r], r));
+      total += sizes[r];
+    }
+    b2p::Agreement a = b2p::merge_keys(parsed, rank);
+    const std::vector<uint32_t>& l2g = a.l2g;
+    *n_groups = a.n_groups;
+    if (!l2g.empty() && !local_to_global) throw b2p::PlanError(b2p::ErrorKind::Plan, "b2p_group_keys_merge: NULL local_to_global");
+    const std::string bytes = b2p::serialize_keys(a.labels, a.n_groups, a.labels.tsid, a.n_rows, a.types);
+    if (bytes.size() > total) throw b2p::PlanError(b2p::ErrorKind::Plan, "b2p_group_keys_merge: the table exceeds the blocks");
+    std::memcpy(out_table, bytes.data(), bytes.size());
+    *out_table_bytes = bytes.size();
+    std::copy(l2g.begin(), l2g.end(), local_to_global);
+  });
 }
 
 int64_t b2p_plan_num_series(b2p_plan* plan) { return plan && plan->range() ? plan->range()->num_series() : -1; }

@@ -199,9 +199,19 @@ class PlanNode {
   void execute(ArrowArray* out, ArrowSchema* out_schema);
   void add_scalar_op(int op, double scalar, bool scalar_on_left, bool return_bool);
   void add_function(const std::string& name, const std::vector<double>& args);
+  // b2p_plan_set_sharded: false on a node without a sharded form
+  virtual bool set_sharded() { return false; }
 
  protected:
   virtual void compute(NodeResult& r) = 0;
+  // A sharded node's check before its work: false without a communicator (the node then runs unsharded); with one, a
+  // Plan error for a node below that is sharded or not row-local, else true
+  bool sharded_run(const char* node) const;
+  // the children a sharded node's check walks (the row-local nodes' and the sharded nodes')
+  virtual std::vector<const PlanNode*> children() const { return {}; }
+  // what the node computes over rows other ranks hold, nullptr when it is row-local
+  virtual const char* cross_row() const { return nullptr; }
+  bool sharded_ = false;
   // the argument checks every node makes: a NULL context (unless the node does no device work) is an Internal error,
   // then a NULL child a Plan error, "<node>: NULL context" / "<node>: NULL child"
   void require(const char* node, std::initializer_list<const PlanNode*> children, bool device = true) const;
@@ -256,6 +266,10 @@ class PromRangePlan : public PlanNode {
   uint64_t last_id_ = 0;
   bool have_last_ = false;
   void check_key_columns() const;  // by-columns and the le column name a tag or label column
+  bool set_sharded() override { return agg_id_ >= 0 && (sharded_ = true); }
+  const char* cross_row() const override {
+    return agg_id_ >= 0 ? "an aggregate stage" : args_.histogram ? "histogram_quantile" : nullptr;
+  }
 };
 
 // Label matching modifier of a binary or set operator
@@ -282,6 +296,7 @@ class BinaryPlan : public PlanNode {
   Matching matching_;
   std::vector<std::string> labels_;
   bool labels_from_lhs_;
+  const char* cross_row() const override { return "a binary operator"; }
 };
 
 // Set operator `and` / `or` / `unless` over two nodes (b2p_plan_setop_create): the reference's left.distinct()
@@ -300,6 +315,7 @@ class SetOpPlan : public PlanNode {
   std::shared_ptr<PlanNode> lhs_, rhs_;
   Matching matching_;
   std::vector<std::string> labels_;
+  const char* cross_row() const override { return "a set operator"; }
 };
 
 // scalar(child), the reference's ScalarCalculateExec (planner.rs:3141-3183, scalar_calculate.rs:532-637): a tagless node
@@ -314,6 +330,7 @@ class ScalarPlan : public PlanNode {
 
  private:
   std::shared_ptr<PlanNode> child_;
+  const char* cross_row() const override { return "scalar()"; }
 };
 
 // topk(k, child) / bottomk(k, child) [by | without (labels)], the reference's Window(row_number()) -> Filter(rank <= k)
@@ -336,6 +353,7 @@ class TopkPlan : public PlanNode {
   std::shared_ptr<PlanNode> child_;
   Modifier modifier_;
   std::vector<std::string> labels_;
+  const char* cross_row() const override { return "topk / bottomk"; }
 };
 
 // <op>(child) [by | without (labels)] over any node, GpuPromAggregateExec: the reference's Aggregate(group labels + ts,
@@ -358,6 +376,9 @@ class AggregatePlan : public PlanNode {
   std::shared_ptr<PlanNode> child_;
   Modifier modifier_;
   std::vector<std::string> labels_;
+  bool set_sharded() override { return sharded_ = true; }
+  std::vector<const PlanNode*> children() const override { return {child_.get()}; }
+  const char* cross_row() const override { return "an aggregate"; }
 };
 
 // count_values(label, child) [by | without (labels)], GpuPromCountValuesExec: the reference's Aggregate(groupBy = [group
@@ -379,6 +400,9 @@ class CountValuesPlan : public PlanNode {
   std::shared_ptr<PlanNode> child_;
   Modifier modifier_;
   std::vector<std::string> labels_;
+  bool set_sharded() override { return sharded_ = true; }
+  std::vector<const PlanNode*> children() const override { return {child_.get()}; }
+  const char* cross_row() const override { return "count_values"; }
 };
 
 // fn(child[range:step]), GpuPromSubqueryExec: the reference's RangeManipulate(start, end, interval, range) directly over
@@ -401,6 +425,7 @@ class SubqueryPlan : public PlanNode {
   std::string function_;
   b2p_range_params p_;
   std::shared_ptr<PlanNode> child_;
+  std::vector<const PlanNode*> children() const override { return {child_.get()}; }
 };
 
 // histogram_quantile(φ, child), GpuPromHistogramFoldExec: the reference's HistogramFold(le, field, time index, φ) over
@@ -422,6 +447,7 @@ class HistogramQuantilePlan : public PlanNode {
   std::string le_column_;
   double phi_;
   std::shared_ptr<PlanNode> child_;
+  const char* cross_row() const override { return "histogram_quantile"; }
 };
 
 // sort / sort_desc / sort_by_label / sort_by_label_desc (child [, labels]), GpuPromSortExec: the reference's
@@ -442,6 +468,7 @@ class SortPlan : public PlanNode {
   bool desc_ = false, by_label_ = false;
   std::shared_ptr<PlanNode> child_;
   std::vector<std::string> labels_;
+  const char* cross_row() const override { return "sort"; }
 };
 
 // absent(child), GpuPromAbsentExec: the reference's PromAbsentExec(start, end, interval, time index, value column, fake
@@ -465,6 +492,7 @@ class AbsentPlan : public PlanNode {
   std::string time_index_, value_column_;
   std::vector<std::pair<std::string, std::string>> labels_;  // by name, one per name
   std::shared_ptr<PlanNode> child_;
+  const char* cross_row() const override { return "absent()"; }
 };
 
 // EmptyMetric(start, end, interval, time_index, field_column, field_expr) (empty_metric.rs): one tagless row over
@@ -485,6 +513,7 @@ class EmptyMetricPlan : public PlanNode {
   std::string time_index_, value_column_;
   int kind_;
   double literal_;
+  const char* cross_row() const override { return "an EmptyMetric row (time(), vector(), a literal), which every rank holds whole"; }
 };
 
 // label_replace(child, dst, replacement, src, regex) / label_join(child, dst, separator, srcs..), GpuPromLabelExec: the
@@ -519,6 +548,7 @@ class LabelPlan : public PlanNode {
   std::vector<std::string> srcs_;
   std::unique_ptr<class LabelRegex> regex_;
   bool empty_regex_ = false;
+  std::vector<const PlanNode*> children() const override { return {child_.get()}; }
 };
 
 int function_id_from_name(const std::string& prom_name);  // -1 when unknown

@@ -43,7 +43,7 @@ struct Nccl {
   typedef struct ncclComm* comm_t;
   struct unique_id { char internal[128]; };
   enum { kSum = 0, kMax = 2, kMin = 3 };
-  enum { kUint32 = 3, kInt64 = 4, kUint64 = 5, kFloat64 = 8 };
+  enum { kUint8 = 1, kUint32 = 3, kInt64 = 4, kUint64 = 5, kFloat64 = 8 };
   int (*GetUniqueId)(unique_id*) = nullptr;
   int (*CommInitRank)(comm_t*, int, unique_id, int) = nullptr;
   int (*CommDestroy)(comm_t) = nullptr;
@@ -240,6 +240,7 @@ struct b2p_ctx {
   // sharded sort's exchange is its answer, N x 8 (F + 1) B on every rank, and is not cut into batches)
   size_t topk_exchange_cap = size_t(128) << 20;
   long long last_exchange_bytes = 0;  // bytes of this rank's blocks in the last sharded topk, quantile, count_values or sort
+  long long last_group_keys_bytes = 0;  // bytes of this rank's block in the last group-label agreement
   // quantile: chunk table, state and histograms of the groups of several chunks (b2p_quantile.cuh; bound in quantile_run)
   DevBuf q_table, q_state, q_hist;
   // sharded quantile (b2p_aggregation.cu, quantile_shard_*): this rank's chunk table of a batch, the batch's selection

@@ -479,3 +479,122 @@ def merge_sorted_runs(desc: bool, vals, ok: np.ndarray, row_id: np.ndarray, grou
         bits = u ^ sign if i64 else np.where(u >> np.uint64(63) != 0, u ^ sign, ~u)
         out.append(bits.view(np.int64 if i64 else np.float64))
     return merged[F].copy(), (out if many else out[0]), int(cells.size) * 8 * (F + 1)
+
+
+# ---- group-label agreement of a sharded plan node (b2p_plan_set_sharded; block layout of b2p_group_keys_merge) ----
+GK_NULL = 0xFFFFFFFF   # the length tag of a NULL label
+GK_FLAG_TSID = 1       # every group carries its u64 __tsid
+
+
+def label_order_key(v):
+    """The plan layer's order of one label value (Labels::less): "" first, then NULL, then the other strings by their
+    UTF-8 bytes."""
+    if v is None:
+        return (1, b"")
+    return (0, b"") if v == "" else (2, v.encode())
+
+
+def tuple_order_key(t):
+    return tuple(label_order_key(v) for v in t)
+
+
+def group_tuples(tuples):
+    """group_rows' table over rows labelled `tuples` (each a tuple of str / None): the distinct tuples in label order."""
+    return sorted(set(tuple(t) for t in tuples), key=tuple_order_key)
+
+
+def serialize_group_keys(tuples, n_labels: int, ids=None, n_rows=None, types=()) -> bytes:
+    """One rank's block: its groups (distinct, in label order) with their __tsid when `ids` is given, its row count
+    (default: one per group; 0 exactly when there is no group) and its field types (0 Float64, 1 Int64, 2 Int32,
+    3 a count)."""
+    import struct
+    n_rows = len(tuples) if n_rows is None else n_rows
+    out = [struct.pack("<IIIIQ", len(tuples), n_labels, GK_FLAG_TSID if ids is not None else 0, len(types), n_rows),
+           bytes(bytearray(types))]
+    for g, t in enumerate(tuples):
+        if ids is not None:
+            out.append(struct.pack("<Q", int(ids[g])))
+        for v in t:
+            if v is None:
+                out.append(struct.pack("<I", GK_NULL))
+            else:
+                b = v.encode()
+                out.append(struct.pack("<I", len(b)) + b)
+    return b"".join(out)
+
+
+def parse_group_keys(buf: bytes):
+    """-> (tuples, ids or None, n_labels, n_rows, types) of one block"""
+    import struct
+    G, L, flags, F, n_rows = struct.unpack_from("<IIIIQ", buf, 0)
+    types = tuple(buf[24:24 + F])
+    at, tuples, ids = 24 + F, [], [] if flags & GK_FLAG_TSID else None
+    for _ in range(G):
+        if ids is not None:
+            ids.append(struct.unpack_from("<Q", buf, at)[0])
+            at += 8
+        t = []
+        for _ in range(L):
+            n = struct.unpack_from("<I", buf, at)[0]
+            at += 4
+            if n == GK_NULL:
+                t.append(None)
+            else:
+                t.append(bytes(buf[at:at + n]).decode())
+                at += n
+        tuples.append(tuple(t))
+    assert at == len(buf), "block longer than its groups"
+    return tuples, ids, L, n_rows, types
+
+
+def merge_group_keys(blocks, rank: int):
+    """Host mirror of b2p_group_keys_merge: the R-way merge of the blocks (rank order) into the global table without
+    duplicates (a duplicate keeps the lowest rank's id) -> (table tuples, table ids or None, local_to_global of block
+    `rank`, rows of all blocks, the field types of the blocks with rows)."""
+    parsed = [parse_group_keys(b) for b in blocks]
+    typed = [p[4] for p in parsed if p[3]]
+    assert all(t == typed[0] for t in typed), "the ranks with rows read different value types"
+    types = typed[0] if typed else parsed[0][4]
+    heads = [0] * len(parsed)
+    table, ids, l2g = [], [] if parsed[0][1] is not None else None, [0] * len(parsed[rank][0])
+    while True:
+        m = None
+        for r, p in enumerate(parsed):
+            t = p[0]
+            if heads[r] < len(t) and (m is None or tuple_order_key(t[heads[r]]) < tuple_order_key(parsed[m][0][heads[m]])):
+                m = r
+        if m is None:
+            return table, ids, l2g, sum(p[3] for p in parsed), types
+        t = parsed[m][0][heads[m]]
+        if ids is not None:
+            ids.append(parsed[m][1][heads[m]])
+        for r, p in enumerate(parsed):
+            ts = p[0]
+            if heads[r] < len(ts) and ts[heads[r]] == t:
+                if r == rank:
+                    l2g[heads[r]] = len(table)
+                heads[r] += 1
+        table.append(t)
+
+
+def agree_group_keys(tuples, n_labels: int, ids=None, group=None):
+    """Host mirror of a sharded node's group-label agreement (the same exchange as b2p_group_keys_sizes /
+    b2p_group_keys_allgather, torch.distributed instead of the library's NCCL communicator; used by the gloo tests):
+    this rank's groups (distinct, label order, with their __tsid when `ids` is given) -> (global table, its ids or
+    None, local_to_global, this rank's block bytes), the same table on every rank.  One all-gather of the 8-byte block
+    sizes, then one broadcast per rank with bytes."""
+    import torch
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    me = dist.get_rank(group)
+    mine = serialize_group_keys(tuples, n_labels, ids)  # (no field types: the mirror agrees the labels)
+    sizes = [torch.zeros(1, dtype=torch.int64) for _ in range(world)]
+    dist.all_gather(sizes, torch.tensor([len(mine)], dtype=torch.int64), group=group)
+    blocks = []
+    for r, n in enumerate(int(s.item()) for s in sizes):
+        buf = torch.frombuffer(bytearray(mine), dtype=torch.uint8) if r == me else torch.zeros(n, dtype=torch.uint8)
+        if n:
+            dist.broadcast(buf, src=r, group=group)
+        blocks.append(buf.numpy().tobytes())
+    table, table_ids, l2g, _, _ = merge_group_keys(blocks, me)
+    return table, table_ids, l2g, len(mine)

@@ -63,6 +63,12 @@ class _PlanNode:
             raise B2PError(rc, self._L.b2p_plan_last_error().decode())
         return self
 
+    def _set_sharded(self):
+        rc = self._L.b2p_plan_set_sharded(self._h)
+        if rc != 0:
+            raise B2PError(rc, self._L.b2p_plan_last_error().decode())
+        return self
+
     def execute(self):
         """-> pyarrow.RecordBatch with the rows the reference's plan would emit."""
         import pyarrow as pa
@@ -138,6 +144,12 @@ class PromRangeExec(_PlanNode):
 
     def num_series(self) -> int:
         return int(self._L.b2p_plan_num_series(self._h))
+
+    def sharded(self) -> "PromRangeExec":
+        """Mark the leaf's aggregate stage sharded (b2p_plan_set_sharded): every rank pushes its own shard of series and
+        execute() gives every rank the aggregate over the union, through the context's communicator (without one, the
+        unsharded node).  A leaf without an aggregate stage raises.  Returns self."""
+        return self._set_sharded()
 
 
 class BinaryPlan(_PlanNode):
@@ -240,6 +252,12 @@ class AggregatePlan(_PlanNode):
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())
 
+    def sharded(self) -> "AggregatePlan":
+        """Mark the node sharded (b2p_plan_set_sharded): every rank runs the plan over its own shard of series and
+        execute() gives every rank the aggregate over the union, through the context's communicator (without one, the
+        unsharded node).  The child subtree must be row-local.  Returns self."""
+        return self._set_sharded()
+
 
 class CountValuesPlan(_PlanNode):
     """count_values(label, child) per (group labels, step), with `by` or `without` labels (neither: one group per step):
@@ -261,6 +279,12 @@ class CountValuesPlan(_PlanNode):
         self._h = self._L.b2p_plan_count_values_create(ctx._h, label.encode(), child._h, modifier, arr, len(labels))
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+    def sharded(self) -> "CountValuesPlan":
+        """Mark the node sharded (b2p_plan_set_sharded): every rank runs the plan over its own shard of series and
+        execute() gives every rank count_values over the union, through the context's communicator (without one, the
+        unsharded node).  The child subtree must be row-local.  Returns self."""
+        return self._set_sharded()
 
 
 class SubqueryPlan(_PlanNode):

@@ -334,6 +334,42 @@ B2P_API int b2p_comm_destroy(b2p_ctx* ctx);
 B2P_API int b2p_allreduce_partials_dev(b2p_ctx* ctx, int32_t agg, double* val, uint32_t* cnt, double* mean, uint64_t n);
 /* Wide avg_over_time (config 5): per-column (sum, count) of every rank added in place. */
 B2P_API int b2p_allreduce_columns_dev(b2p_ctx* ctx, double* sum, uint64_t* cnt, uint32_t n_cols);
+/* Int64 partials of SUM / MIN / MAX (any other aggregator is B2P_E_INVALID): exactly b2p_group_aggregate_i64_dev's output
+ * (K3's Int64 fold: wrapping sum, signed min / max; int64_t bits in out_val, 0 where cnt is 0), which is already the
+ * state another rank's partial merges with. */
+B2P_API int b2p_group_aggregate_partial_i64_dev(b2p_ctx* ctx, int32_t agg, const int64_t* vals, const uint32_t* valid_words,
+                                                const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T,
+                                                double* out_val, uint32_t* out_cnt);
+/* In-place merge of every rank's Int64 partials [n] (asynchronous): SUM adds the bits as uint64 (ncclSum; modular
+ * addition is the wrapping sum whatever the rank order), MIN / MAX reduce them as int64 (ncclMin / ncclMax) after a
+ * group absent on a rank took INT64_MAX / INT64_MIN, and a group absent everywhere reads 0; cnt is added.  Without a
+ * communicator and n_ranks == 1 it returns at once. */
+B2P_API int b2p_allreduce_partials_i64_dev(b2p_ctx* ctx, int32_t agg, double* val, uint32_t* cnt, uint64_t n);
+/* The number of ranks of the context's communicator (0 without one) and, in *rank (may be NULL), this rank (0 without
+ * one).  No device work. */
+B2P_API int32_t b2p_comm_ranks(b2p_ctx* ctx, int32_t* rank);
+/* Host-pointer forms of the sharded by-label aggregate, what a sharded plan node runs: this rank's rows (vals / valid /
+ * gid as for b2p_group_aggregate, gid over the n_groups GLOBAL group ids, any rank may have no row) become its partials
+ * (b2p_group_aggregate_partial_dev / _i64_dev), every rank's are merged (b2p_allreduce_partials_dev / _i64_dev) and
+ * finalised (b2p_group_finalize_dev); out_val / out_cnt [n_groups x T] come back as b2p_group_aggregate writes them over
+ * the union of the ranks' rows.  Float64: every aggregator; Int64: sum, min and max.  Collective: every rank calls with
+ * the same agg, n_groups and T.  Synchronous. */
+B2P_API int b2p_group_aggregate_allreduce(b2p_ctx* ctx, int32_t agg, const double* vals, const uint32_t* valid_words,
+                                          const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T,
+                                          double* out_val, uint32_t* out_cnt);
+B2P_API int b2p_group_aggregate_allreduce_i64(b2p_ctx* ctx, int32_t agg, const int64_t* vals, const uint32_t* valid_words,
+                                              const uint32_t* gid, uint32_t n_series, uint32_t n_groups, uint64_t T,
+                                              double* out_val, uint32_t* out_cnt);
+/* The group-label agreement's exchange of exact bytes (the plan layer's sharded nodes; the blocks are
+ * b2p_group_keys_merge's).  b2p_group_keys_sizes: this rank's block size `bytes`; one ncclAllGather of the 8-byte sizes
+ * fills the HOST array sizes [n_ranks] (row r: rank r), the same on every rank; without a communicator sizes[0] = bytes.
+ * b2p_group_keys_allgather: every rank's block, back to back in rank order, into the HOST buffer out (sum of sizes
+ * bytes): this rank's block goes to its place in one device buffer, then one ncclBroadcast per rank with bytes, in one
+ * NCCL group (no block is padded).  b2p_last_group_keys_bytes() then gives this rank's block bytes (the all-gather of
+ * the sizes adds 8 B per rank).  Both synchronise the stream. */
+B2P_API int b2p_group_keys_sizes(b2p_ctx* ctx, uint64_t bytes, uint64_t* sizes);
+B2P_API int b2p_group_keys_allgather(b2p_ctx* ctx, const void* block, const uint64_t* sizes, void* out);
+B2P_API int64_t b2p_last_group_keys_bytes(b2p_ctx* ctx);
 /* sum by (..)(fn(..)) over ALL ranks: this rank's fused partials, computed in n_tiles group ranges; each range's rows
  * of out_sum / out_cnt are all-reduced on a high-priority communication stream as soon as they are complete, while
  * the next range computes (kernel time of the last tile's all-reduce: b2p_last_kernel_ms(ctx, 4)).  On return
@@ -539,6 +575,23 @@ B2P_API int b2p_group_quantile_dev(b2p_ctx* ctx, double phi, const double* vals,
  * pass out of range, n_blocks 0, an advance before its batch's pass 0 on the context, no communicator with n_ranks > 1. */
 B2P_API int b2p_quantile_allreduce_dev(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid,
                                        const b2p_group_index* index, uint64_t T, double* out_val, uint32_t* out_cnt);
+/* Host-pointer form of b2p_quantile_allreduce_dev (vals / valid / gid as for b2p_group_quantile, gid over the n_groups
+ * global group ids): what a sharded quantile plan node runs.  Synchronous. */
+B2P_API int b2p_quantile_allreduce(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid,
+                                   const uint32_t* gid, uint32_t n_rows, uint32_t n_groups, uint64_t T, double* out_val,
+                                   uint32_t* out_cnt);
+/* Host-pointer form of the sharded count_values (vals / valid / gid as for b2p_count_values, gid over the n_groups global
+ * group ids): what a sharded count_values plan node runs.  b2p_count_values_dev (_i64_dev) over this rank's rows, the
+ * heights table of b2p_count_values_shard_heights_dev, then b2p_count_values_allgather_dev (_i64_dev).  out_goff
+ * [n_groups + 1] (host) receives the merged rows' offsets, the same on every rank; out_val / out_cnt receive
+ * [out_goff[n_groups] x T] rows, which must fit cap_rows (B2P_E_TOO_LARGE otherwise; every rank decides alike when every
+ * rank passes the same cap, e.g. the rows of all ranks).  Collective; synchronous. */
+B2P_API int b2p_count_values_allgather(b2p_ctx* ctx, const double* vals, const uint32_t* valid, const uint32_t* gid,
+                                       uint32_t n_rows, uint32_t n_groups, uint64_t T, uint64_t cap_rows,
+                                       uint32_t* out_goff, double* out_val, uint32_t* out_cnt);
+B2P_API int b2p_count_values_allgather_i64(b2p_ctx* ctx, const int64_t* vals, const uint32_t* valid, const uint32_t* gid,
+                                           uint32_t n_rows, uint32_t n_groups, uint64_t T, uint64_t cap_rows,
+                                           uint32_t* out_goff, int64_t* out_val, uint32_t* out_cnt);
 B2P_API int b2p_quantile_shard_plan(b2p_ctx* ctx, uint32_t n_groups, uint64_t T, uint32_t* n_batches,
                                     uint64_t* block_bytes, uint64_t* state_bytes);
 B2P_API int b2p_quantile_shard_pass_dev(b2p_ctx* ctx, double phi, const double* vals, const uint32_t* valid,
@@ -754,6 +807,21 @@ B2P_API int b2p_sort_cells_i64_dev(b2p_ctx* ctx, int32_t desc, const int64_t* va
 B2P_API int b2p_i64_to_f64_dev(b2p_ctx* ctx, const int64_t* vals, uint64_t n, double* out);
 
 /* ---- host-side helper (no device work) -------------------------------------------------------- */
+/* The merge of the group-label agreement (b2p_plan_set_sharded), host only, so that one process can play R ranks.  A
+ * block is one rank's groups in Labels order (the plan layer's sorted group order: per label "" first, then NULL, then
+ * the other strings in byte order), all little-endian: u32 n_groups, u32 n_labels, u32 flags (bit 0: every group carries
+ * a u64 __tsid), u32 n_fields, u64 n_rows (the rank's rows: 0 exactly when n_groups is 0), one u8 per field (its value
+ * type: 0 Float64, 1 Int64, 2 Int32, 3 a count), then per group [u64 __tsid] and per label a u32 tag (0xFFFFFFFF:
+ * NULL, else the byte length) followed by the bytes.  The merge is an R-way merge of the blocks in rank order into the global table (the same block layout,
+ * written to out_table, whose capacity must be the sum of sizes; *out_table_bytes its length; its n_rows the sum, its
+ * field types those of the blocks with rows), dropping duplicate tuples (a duplicate keeps the lowest rank's __tsid), so every rank derives the identical table from the identical
+ * blocks whatever its own rank; *n_groups is the global count and local_to_global [rank's n_groups] maps block `rank`'s
+ * groups to their global ids (the table's order).  B2P_E_INVALID: a NULL argument, a block that is truncated, longer
+ * than its groups, not strictly in Labels order, unlike block 0 in n_labels, flags or n_fields, or with rows whose field
+ * types differ from another block's with rows. */
+B2P_API int b2p_group_keys_merge(const void* const* blocks, const uint64_t* sizes, int32_t n_ranks, int32_t rank,
+                                 void* out_table, uint64_t* out_table_bytes, uint32_t* n_groups,
+                                 uint32_t* local_to_global);
 /* SeriesDivide (series_divide.rs:540-670) plus a cadence scan of one sorted batch on the HOST: series boundaries from
  * the id column `sid` (ids sid_base .. sid_base + n_series - 1, non-decreasing), or copied from `offsets_in`
  * (n_series + 1) when sid is NULL, into offsets_out (n_series + 1); and per series t0 = its first timestamp and
@@ -1059,6 +1127,22 @@ B2P_API b2p_plan* b2p_plan_aggregate_create(b2p_ctx* ctx, const char* op, double
 B2P_API b2p_plan* b2p_plan_count_values_create(b2p_ctx* ctx, const char* label, b2p_plan* child,
                                                const char* modifier /* NULL | "by" | "without" */,
                                                const char* const* labels, int32_t n_labels);
+/* Marks an aggregate node (every op), a count_values node, or a range / instant leaf with an aggregate stage, as
+ * SHARDED (before execute): every rank runs the same plan over its own shard of series (each series whole on one rank),
+ * and after execute every rank holds the result over the union of the shards, its export identical bit for bit on every
+ * rank; nodes above run on that replicated result unchanged.  The node uses the context's communicator (b2p_comm_init);
+ * without one it is exactly the unsharded node.  With one, at execute: the ranks agree one group table (each rank's
+ * group label tuples, NULL distinct from "", plus the group's __tsid where the aggregate keeps it, its row count and its
+ * field types, serialised as b2p_group_keys_merge reads them, exchanged by b2p_group_keys_sizes /
+ * b2p_group_keys_allgather and merged on every rank; a rank without rows takes the field types of the ranks with rows,
+ * and ranks with rows whose types differ are a Plan error on every rank), then fold over the global group ids:
+ * b2p_group_aggregate_allreduce (_i64 for an Int64 sum / min / max; group is count's cells with the value 1.0; an Int64
+ * avg / stddev / stdvar / group reads the Float64 coercion), b2p_quantile_allreduce or b2p_count_values_allgather
+ * (_i64; at most the rows of all ranks).  Plan errors at execute: a child subtree with a node that is not row-local
+ * (binary and set operators, topk, sort, absent, scalar(), count_values, aggregates, histogram_quantile, and an
+ * EmptyMetric row, which every rank holds whole; leaves over the rank's series, element-wise stages, label_replace /
+ * label_join and subqueries are row-local) or another sharded node below.  Any other node: a Plan error at the call. */
+B2P_API int b2p_plan_set_sharded(b2p_plan* plan);
 /* function(child[range:step]), GpuPromSubqueryExec (planner.rs:292-332): RangeManipulate(p->start, p->end, p->interval,
  * p->range) directly over the child, then the range function `function` ("prom_max_over_time", ...; p->fn_id is
  * ignored; param0 / param1 as for b2p_plan_range_create) and Filter(IS NOT NULL).  The child is any node; the caller

@@ -301,6 +301,27 @@ extern "C" {
     pub fn b2p_comm_destroy(ctx: *mut b2p_ctx) -> c_int;
     pub fn b2p_allreduce_partials_dev(ctx: *mut b2p_ctx, agg: i32, val: *mut f64, cnt: *mut u32, mean: *mut f64, n: u64) -> c_int;
     pub fn b2p_allreduce_columns_dev(ctx: *mut b2p_ctx, sum: *mut f64, cnt: *mut u64, n_cols: u32) -> c_int;
+    /// Int64 partials of sum / min / max (K3's Int64 fold) and their cross-rank merge.
+    pub fn b2p_group_aggregate_partial_i64_dev(
+        ctx: *mut b2p_ctx, agg: i32, vals: *const i64, valid_words: *const u32, gid: *const u32, n_series: u32,
+        n_groups: u32, t: u64, out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    pub fn b2p_allreduce_partials_i64_dev(ctx: *mut b2p_ctx, agg: i32, val: *mut f64, cnt: *mut u32, n: u64) -> c_int;
+    /// Ranks of the context's communicator (0 without one); this rank in `rank`.
+    pub fn b2p_comm_ranks(ctx: *mut b2p_ctx, rank: *mut i32) -> i32;
+    /// Host-pointer sharded by-label aggregate: partials, all-reduce, finalise (collective).
+    pub fn b2p_group_aggregate_allreduce(
+        ctx: *mut b2p_ctx, agg: i32, vals: *const f64, valid_words: *const u32, gid: *const u32, n_series: u32,
+        n_groups: u32, t: u64, out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    pub fn b2p_group_aggregate_allreduce_i64(
+        ctx: *mut b2p_ctx, agg: i32, vals: *const i64, valid_words: *const u32, gid: *const u32, n_series: u32,
+        n_groups: u32, t: u64, out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    /// The group-label agreement's exchange: every rank's block size, then every rank's block (host buffers).
+    pub fn b2p_group_keys_sizes(ctx: *mut b2p_ctx, bytes: u64, sizes: *mut u64) -> c_int;
+    pub fn b2p_group_keys_allgather(ctx: *mut b2p_ctx, block: *const c_void, sizes: *const u64, out: *mut c_void) -> c_int;
+    pub fn b2p_last_group_keys_bytes(ctx: *mut b2p_ctx) -> i64;
     pub fn b2p_range_group_sum_allreduce_dev(
         ctx: *mut b2p_ctx, p: *const B2pRangeParams, ts: *const i64, val: *const f64, offsets: *const u64, n_rows: u64,
         n_series: u32, index: *const b2p_group_index, n_tiles: i32, out_sum: *mut f64, out_cnt: *mut u32,
@@ -379,6 +400,20 @@ extern "C" {
     pub fn b2p_group_quantile_dev(
         ctx: *mut b2p_ctx, phi: f64, vals: *const f64, valid: *const u32, index: *const b2p_group_index, t: u64,
         out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    /// Host-pointer form of `b2p_quantile_allreduce_dev` (gid over the global group ids).
+    pub fn b2p_quantile_allreduce(
+        ctx: *mut b2p_ctx, phi: f64, vals: *const f64, valid: *const u32, gid: *const u32, n_rows: u32, n_groups: u32,
+        t: u64, out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    /// Host-pointer sharded count_values: merged rows from `out_goff`, at most `cap_rows` of them (collective).
+    pub fn b2p_count_values_allgather(
+        ctx: *mut b2p_ctx, vals: *const f64, valid: *const u32, gid: *const u32, n_rows: u32, n_groups: u32, t: u64,
+        cap_rows: u64, out_goff: *mut u32, out_val: *mut f64, out_cnt: *mut u32,
+    ) -> c_int;
+    pub fn b2p_count_values_allgather_i64(
+        ctx: *mut b2p_ctx, vals: *const i64, valid: *const u32, gid: *const u32, n_rows: u32, n_groups: u32, t: u64,
+        cap_rows: u64, out_goff: *mut u32, out_val: *mut i64, out_cnt: *mut u32,
     ) -> c_int;
     /// quantile(phi) by label over rows sharded across the communicator's ranks: every rank receives the full
     /// [n_groups x T] result.  Without a communicator (one rank) the output of `b2p_group_quantile_dev`.
@@ -528,6 +563,11 @@ extern "C" {
     ) -> c_int;
 
     // ---- host-side helper (no device work): SeriesDivide + cadence scan of one sorted batch ---------------------------
+    /// The merge of the group-label agreement over R blocks (host only).
+    pub fn b2p_group_keys_merge(
+        blocks: *const *const c_void, sizes: *const u64, n_ranks: i32, rank: i32, out_table: *mut c_void,
+        out_table_bytes: *mut u64, n_groups: *mut u32, local_to_global: *mut u32,
+    ) -> c_int;
     pub fn b2p_host_scan_series(
         ts: *const i64, sid: *const u32, offsets_in: *const u64, n_rows: u64, n_series: u32, sid_base: u32,
         offsets_out: *mut u64, t0: *mut i64, cadence: *mut i64, all_regular: *mut i32,
@@ -691,6 +731,8 @@ extern "C" {
     pub fn b2p_plan_set_histogram_quantile(plan: *mut b2p_plan, le_column: *const c_char, quantile: f64) -> c_int;
     /// The metric-engine leaf: Utf8 label columns beside the one UInt64 `__tsid` tag column (before the first push).
     pub fn b2p_plan_set_label_columns(plan: *mut b2p_plan, names: *const *const c_char, n: i32) -> c_int;
+    /// Marks an aggregate node, or a leaf with an aggregate stage, sharded over the context's communicator.
+    pub fn b2p_plan_set_sharded(plan: *mut b2p_plan) -> c_int;
     pub fn b2p_plan_set_scalar_op(plan: *mut b2p_plan, op: i32, scalar: f64, scalar_on_left: i32, return_bool: i32) -> c_int;
     /// The node shares ownership of both children; their handles stay valid and must still be destroyed.
     pub fn b2p_plan_binary_create(
