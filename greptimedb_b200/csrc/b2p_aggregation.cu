@@ -377,11 +377,12 @@ int topk_allgather_run(b2p_ctx* c, int bottom, double k, const double* vals, con
         const TopkShard::Batch bt = sh.batch(b);
         const size_t n_slots = (size_t)bt.nx * bt.nt * sh.K * 32, n_units = (size_t)bt.nx * bt.nt * 32;
         const ShardBlock s = shard_block(sh, bt, c->x_send.p, 1), g = shard_block(sh, bt, c->x_recv.p, sh.n_ranks);
-        NCCL_TRY(g_nccl.GroupStart());
-        NCCL_TRY(g_nccl.AllGather(s.hi, g.hi, n_slots, Nccl::kUint64, c->comm, c->stream));
-        NCCL_TRY(g_nccl.AllGather(s.lo, g.lo, n_slots, Nccl::kUint32, c->comm, c->stream));
-        NCCL_TRY(g_nccl.AllGather(s.n, g.n, n_units, Nccl::kUint32, c->comm, c->stream));
-        NCCL_TRY(g_nccl.GroupEnd());
+        if ((rc = nccl_group([&] {
+               NCCL_TRY(g_nccl.AllGather(s.hi, g.hi, n_slots, Nccl::kUint64, c->comm, c->stream));
+               NCCL_TRY(g_nccl.AllGather(s.lo, g.lo, n_slots, Nccl::kUint32, c->comm, c->stream));
+               NCCL_TRY(g_nccl.AllGather(s.n, g.n, n_units, Nccl::kUint32, c->comm, c->stream));
+               return B2P_OK;
+             }))) return rc;
         gathered = c->x_recv.p;
       }
       if ((rc = shard_merge(c, sh, b, r, gathered, c->x_state.p, T))) return rc;
@@ -615,11 +616,12 @@ int quantile_allreduce_run(b2p_ctx* c, double phi, const double* vals, const uin
         char* blk = c->x_send.as<char>();
         void* r_lo = blk + units * QuantShard::kCountBytes;
         void* r_hi = blk + units * (QuantShard::kCountBytes + 32 * 8);
-        NCCL_TRY(g_nccl.GroupStart());
-        NCCL_TRY(g_nccl.AllReduce(blk, blk, units * (1u << kQuantShardBits) * 32, Nccl::kUint32, Nccl::kSum, c->comm, c->stream));
-        NCCL_TRY(g_nccl.AllReduce(r_lo, r_lo, units * 32, Nccl::kUint64, Nccl::kMax, c->comm, c->stream));
-        NCCL_TRY(g_nccl.AllReduce(r_hi, r_hi, units * 32, Nccl::kUint64, Nccl::kMin, c->comm, c->stream));
-        NCCL_TRY(g_nccl.GroupEnd());
+        if ((rc = nccl_group([&] {
+               NCCL_TRY(g_nccl.AllReduce(blk, blk, units * (1u << kQuantShardBits) * 32, Nccl::kUint32, Nccl::kSum, c->comm, c->stream));
+               NCCL_TRY(g_nccl.AllReduce(r_lo, r_lo, units * 32, Nccl::kUint64, Nccl::kMax, c->comm, c->stream));
+               NCCL_TRY(g_nccl.AllReduce(r_hi, r_hi, units * 32, Nccl::kUint64, Nccl::kMin, c->comm, c->stream));
+               return B2P_OK;
+             }))) return rc;
       }
       uint64_t live = 0;
       if ((rc = quantile_shard_advance(c, sh, b, phi, T, c->x_send.p, 1, out_val, out_cnt, &live))) return rc;
@@ -821,24 +823,19 @@ int cv_shard_check_rank(const CvShard& sh, const b2p_group_index* ix, uint32_t r
 // h_r(g) of this rank into `heights` (host): [n_groups], or with a communicator every rank's row [n_ranks x n_groups]
 // (one in-place all-gather).  Reads the table back, so it synchronises the stream.
 int cv_shard_heights(b2p_ctx* c, const uint32_t* cnt, const b2p_group_index* ix, uint64_t T, uint32_t* heights) {
-  int rc;
-  const uint32_t G = ix->n_groups, R = c->comm ? (uint32_t)c->comm_ranks : 1u;
+  const uint32_t G = ix->n_groups;
   if (G == 0) return B2P_OK;
-  if ((rc = c->x_size.ensure((size_t)R * G * 4))) return rc;
-  uint32_t* mine = c->x_size.as<uint32_t>() + (c->comm ? (size_t)c->comm_rank * G : 0);
-  CU(cudaMemsetAsync(mine, 0, (size_t)G * 4, c->stream));
-  const uint32_t in_rows = ix->goff_host[G];
-  if (in_rows && T) {
-    count_values_heights_kernel<<<capped_grid(c, in_rows, 8, 16), 256, 0, c->stream>>>(cnt, ix->gid, ix->members,
-                                                                                        ix->goff, in_rows, T, mine);
-    c->launches++;
-    CU(cudaGetLastError());
-  }
-  if (c->comm)
-    NCCL_TRY(g_nccl.AllGather(mine, c->x_size.p, G, Nccl::kUint32, c->comm, c->stream));
-  CU(cudaMemcpyAsync(heights, c->x_size.p, (size_t)R * G * 4, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return B2P_OK;
+  return rank_table(c, G, Nccl::kUint32, heights, [&](void* mine) {
+    CU(cudaMemsetAsync(mine, 0, (size_t)G * 4, c->stream));
+    const uint32_t in_rows = ix->goff_host[G];
+    if (in_rows && T) {
+      count_values_heights_kernel<<<capped_grid(c, in_rows, 8, 16), 256, 0, c->stream>>>(
+          cnt, ix->gid, ix->members, ix->goff, in_rows, T, static_cast<uint32_t*>(mine));
+      c->launches++;
+      CU(cudaGetLastError());
+    }
+    return B2P_OK;
+  });
 }
 
 // Per-rank step: this rank's block of batch b, [keys: P u64][counts: P u32] (P the batch's padded entry count; the
@@ -966,10 +963,11 @@ int cv_allgather_run(b2p_ctx* c, const CvShard& sh, const double* vals, const ui
       const uint64_t P = sh.batches[b].P;
       const unsigned long long* sk = c->x_send.as<unsigned long long>();
       unsigned long long* gk = c->x_recv.as<unsigned long long>();
-      NCCL_TRY(g_nccl.GroupStart());
-      NCCL_TRY(g_nccl.AllGather(sk, gk, P, Nccl::kUint64, c->comm, c->stream));
-      NCCL_TRY(g_nccl.AllGather(sk + P, gk + P * sh.n_ranks, P, Nccl::kUint32, c->comm, c->stream));
-      NCCL_TRY(g_nccl.GroupEnd());
+      if ((rc = nccl_group([&] {
+             NCCL_TRY(g_nccl.AllGather(sk, gk, P, Nccl::kUint64, c->comm, c->stream));
+             NCCL_TRY(g_nccl.AllGather(sk + P, gk + P * sh.n_ranks, P, Nccl::kUint32, c->comm, c->stream));
+             return B2P_OK;
+           }))) return rc;
       gathered = c->x_recv.p;
     }
     if ((rc = cv_shard_merge(c, sh, b, gathered, out_val, out_cnt, i64))) return rc;
@@ -1037,7 +1035,6 @@ int cv_allgather_dev(b2p_ctx* c, const double* vals, const uint32_t* cnt, const 
                      const uint32_t* heights, double* out_val, uint32_t* out_cnt, bool i64) {
   if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
   if (ix->n_series && T && (!vals || !cnt)) return fail(B2P_E_INVALID, "NULL argument");
-  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
   c->last_exchange_bytes = 0;
   CvShard sh;
   if (int rc = cv_shard_plan(c, heights, c->comm_ranks, ix->n_groups, T, sh)) return rc;
@@ -1157,7 +1154,6 @@ int b2p_topk_allgather_dev(b2p_ctx* c, int32_t bottom, double k, const double* v
                            const b2p_group_index* ix, const uint32_t* tie, uint64_t T, uint32_t* out_valid) {
   if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
   if (ix->n_series && (!vals || !valid || !tie || !out_valid)) return fail(B2P_E_INVALID, "NULL argument");
-  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
   c->last_exchange_bytes = 0;
   if (T == 0) return B2P_OK;  // (every rank has the same T)
   DeviceGuard g(c->device);
@@ -1222,7 +1218,6 @@ int b2p_quantile_allreduce_dev(b2p_ctx* c, double phi, const double* vals, const
   if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
   if ((ix->n_series && (!vals || !valid)) || (ix->n_groups && T && (!out_val || !out_cnt)))
     return fail(B2P_E_INVALID, "NULL argument");
-  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
   c->last_exchange_bytes = 0;
   if (ix->n_groups == 0 || T == 0) return B2P_OK;  // (every rank has the same n_groups and T)
   DeviceGuard g(c->device);
@@ -1251,7 +1246,6 @@ int b2p_count_values_shard_heights_dev(b2p_ctx* c, const uint32_t* local_cnt, co
                                        uint32_t* heights) {
   if (!c || !ix) return fail(B2P_E_INVALID, "NULL argument");
   if ((ix->n_series && T && !local_cnt) || (ix->n_groups && !heights)) return fail(B2P_E_INVALID, "NULL argument");
-  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
   DeviceGuard g(c->device);
   return cv_shard_heights(c, local_cnt, ix, T, heights);
 }
@@ -1373,7 +1367,7 @@ int count_values_allgather_host(b2p_ctx* c, const double* vals, const uint32_t* 
   uint32_t* o_cnt = static_cast<uint32_t*>(s.buf(cap_rows * T * 4));
   return end_indexed(s, gid, n_rows, n_groups, [&](const b2p_group_index* ix) {
     int rc = count_values_dev(c, d_vals, d_valid, ix, T, l_val, l_cnt, i64);
-    const uint32_t R = c->comm ? (uint32_t)c->comm_ranks : 1u;
+    const uint32_t R = (uint32_t)c->comm_ranks;
     std::vector<uint32_t> heights((size_t)R * n_groups);
     if (!rc) rc = b2p_count_values_shard_heights_dev(c, l_cnt, ix, T, heights.data());
     if (rc) return rc;

@@ -161,7 +161,7 @@ double b2p_last_kernel_ms(b2p_ctx* c, int stage) {
   return (double)ms;
 }
 
-/* ---- multi-GPU: all-reduce of by-label partials over NCCL ----------------------------------------- */
+/* ---- multi-GPU: the NCCL communicator and the exchanges of the sharded operators ----------------- */
 
 int b2p_comm_unique_id(void* out_id, size_t bytes) {
   if (!out_id || bytes < sizeof(Nccl::unique_id)) return fail(B2P_E_INVALID, "need a %zu-byte buffer", sizeof(Nccl::unique_id));
@@ -197,7 +197,7 @@ int b2p_comm_init(b2p_ctx* c, const void* id_bytes, size_t bytes, int n_ranks, i
 }
 
 int32_t b2p_comm_ranks(b2p_ctx* c, int32_t* rank) {
-  if (rank) *rank = c && c->comm ? c->comm_rank : 0;
+  if (rank) *rank = c ? c->comm_rank : 0;
   return c && c->comm ? c->comm_ranks : 0;
 }
 
@@ -210,7 +210,29 @@ int b2p_comm_destroy(b2p_ctx* c) {
   NCCL_TRY(g_nccl.CommDestroy(c->comm));
   c->comm = nullptr;
   c->comm_ranks = 1;
+  c->comm_rank = 0;
   return B2P_OK;
 }
 
 }  // extern "C"
+
+int allreduce_with_counts(b2p_ctx* c, void* val, int type, int op, uint32_t* cnt, uint64_t n, cudaStream_t s) {
+  return nccl_group([&] {
+    NCCL_TRY(g_nccl.AllReduce(val, val, n, type, op, c->comm, s));
+    NCCL_TRY(g_nccl.AllReduce(cnt, cnt, n, Nccl::kUint32, Nccl::kSum, c->comm, s));
+    return B2P_OK;
+  });
+}
+
+int gather_blocks(b2p_ctx* c, void* buf, const uint64_t* sizes, size_t entry_bytes, int type) {
+  if (!c->comm) return B2P_OK;
+  return nccl_group([&] {
+    char* at = static_cast<char*>(buf);
+    for (int r = 0; r < c->comm_ranks; ++r) {
+      const size_t bytes = sizes[r] * entry_bytes;
+      if (bytes) NCCL_TRY(g_nccl.Broadcast(at, at, bytes / Nccl::bytes(type), type, r, c->comm, c->stream));
+      at += bytes;
+    }
+    return B2P_OK;
+  });
+}

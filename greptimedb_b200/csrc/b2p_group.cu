@@ -186,18 +186,13 @@ int b2p_allreduce_partials_dev(b2p_ctx* c, int32_t agg, double* val, uint32_t* c
   if (!val || !cnt) return fail(B2P_E_INVALID, "NULL argument");
   const bool var = agg == B2P_AGG_STDDEV || agg == B2P_AGG_STDVAR;
   if (var && !mean) return fail(B2P_E_INVALID, "stddev / stdvar partials need the per-group means");
-  if (!c->comm) {
-    if (c->comm_ranks == 1) return B2P_OK;  // single rank: nothing to merge
-    return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
-  }
+  if (!c->comm) return B2P_OK;  // single rank: nothing to merge
   DeviceGuard g(c->device);
   const unsigned blocks = capped_grid(c, n, 256, 16);
   if (agg == B2P_AGG_MIN || agg == B2P_AGG_MAX) {
     minmax_neutral_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(agg == B2P_AGG_MIN, val, cnt, n, 0);
-    NCCL_TRY(g_nccl.GroupStart());
-    NCCL_TRY(g_nccl.AllReduce(val, val, n, Nccl::kInt64, agg == B2P_AGG_MIN ? Nccl::kMin : Nccl::kMax, c->comm, c->stream));
-    NCCL_TRY(g_nccl.AllReduce(cnt, cnt, n, Nccl::kUint32, Nccl::kSum, c->comm, c->stream));
-    NCCL_TRY(g_nccl.GroupEnd());
+    const int op = agg == B2P_AGG_MIN ? Nccl::kMin : Nccl::kMax;
+    if (int rc = allreduce_with_counts(c, val, Nccl::kInt64, op, cnt, n, c->stream)) return rc;
     minmax_neutral_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(agg == B2P_AGG_MIN, val, cnt, n, 1);
     c->launches += 2;
   } else if (var) {
@@ -206,19 +201,13 @@ int b2p_allreduce_partials_dev(b2p_ctx* c, int32_t agg, double* val, uint32_t* c
     double* wsum = c->m_tmp0.as<double>();    // cnt_r * mean_r -> global sum
     uint32_t* cnt_r = c->m_tmp1.as<uint32_t>();  // this rank's counts (cnt itself becomes the global count)
     variance_merge_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(0, val, cnt, mean, wsum, cnt_r, n);
-    NCCL_TRY(g_nccl.GroupStart());
-    NCCL_TRY(g_nccl.AllReduce(wsum, wsum, n, Nccl::kFloat64, Nccl::kSum, c->comm, c->stream));
-    NCCL_TRY(g_nccl.AllReduce(cnt, cnt, n, Nccl::kUint32, Nccl::kSum, c->comm, c->stream));
-    NCCL_TRY(g_nccl.GroupEnd());
+    if ((rc = allreduce_with_counts(c, wsum, Nccl::kFloat64, Nccl::kSum, cnt, n, c->stream))) return rc;
     variance_merge_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(1, val, cnt, mean, wsum, cnt_r, n);
     NCCL_TRY(g_nccl.AllReduce(val, val, n, Nccl::kFloat64, Nccl::kSum, c->comm, c->stream));
     c->launches += 2;
   } else {
     stage_begin(c, 4);
-    NCCL_TRY(g_nccl.GroupStart());
-    NCCL_TRY(g_nccl.AllReduce(val, val, n, Nccl::kFloat64, Nccl::kSum, c->comm, c->stream));
-    NCCL_TRY(g_nccl.AllReduce(cnt, cnt, n, Nccl::kUint32, Nccl::kSum, c->comm, c->stream));
-    NCCL_TRY(g_nccl.GroupEnd());
+    if (int rc = allreduce_with_counts(c, val, Nccl::kFloat64, Nccl::kSum, cnt, n, c->stream)) return rc;
     stage_end(c, 4);
   }
   CU(cudaGetLastError());
@@ -237,10 +226,7 @@ int b2p_allreduce_partials_i64_dev(b2p_ctx* c, int32_t agg, double* val, uint32_
     return fail(B2P_E_INVALID, "Int64 partials exist for sum, min and max only (aggregator %d)", agg);
   if (n == 0) return B2P_OK;
   if (!val || !cnt) return fail(B2P_E_INVALID, "NULL argument");
-  if (!c->comm) {
-    if (c->comm_ranks == 1) return B2P_OK;
-    return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
-  }
+  if (!c->comm) return B2P_OK;
   DeviceGuard g(c->device);
   const unsigned blocks = capped_grid(c, n, 256, 16);
   const bool minmax = agg != B2P_AGG_SUM;
@@ -248,12 +234,8 @@ int b2p_allreduce_partials_i64_dev(b2p_ctx* c, int32_t agg, double* val, uint32_
     minmax_neutral_kernel<<<blocks, 256, 0, c->stream>>>(agg == B2P_AGG_MIN, val, cnt, n, 0, true);
     c->launches++;
   }
-  NCCL_TRY(g_nccl.GroupStart());
-  NCCL_TRY(g_nccl.AllReduce(val, val, n, minmax ? Nccl::kInt64 : Nccl::kUint64,
-                            agg == B2P_AGG_MIN ? Nccl::kMin : agg == B2P_AGG_MAX ? Nccl::kMax : Nccl::kSum, c->comm,
-                            c->stream));
-  NCCL_TRY(g_nccl.AllReduce(cnt, cnt, n, Nccl::kUint32, Nccl::kSum, c->comm, c->stream));
-  NCCL_TRY(g_nccl.GroupEnd());
+  const int op = agg == B2P_AGG_MIN ? Nccl::kMin : agg == B2P_AGG_MAX ? Nccl::kMax : Nccl::kSum;
+  if (int rc = allreduce_with_counts(c, val, minmax ? Nccl::kInt64 : Nccl::kUint64, op, cnt, n, c->stream)) return rc;
   if (minmax) {
     minmax_neutral_kernel<<<blocks, 256, 0, c->stream>>>(agg == B2P_AGG_MIN, val, cnt, n, 1, true);
     c->launches++;
@@ -266,18 +248,12 @@ int b2p_allreduce_partials_i64_dev(b2p_ctx* c, int32_t agg, double* val, uint32_
 // per rank); reads the table back, so it synchronises the stream.
 int b2p_group_keys_sizes(b2p_ctx* c, uint64_t bytes, uint64_t* sizes) {
   if (!c || !sizes) return fail(B2P_E_INVALID, "NULL argument");
-  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
   DeviceGuard g(c->device);
-  int rc;
-  const uint32_t R = c->comm ? (uint32_t)c->comm_ranks : 1u;
-  if ((rc = c->x_size.ensure((size_t)R * 8))) return rc;
-  unsigned long long* mine = c->x_size.as<unsigned long long>() + (c->comm ? c->comm_rank : 0);
   const unsigned long long b = bytes;
-  CU(cudaMemcpyAsync(mine, &b, 8, cudaMemcpyHostToDevice, c->stream));
-  if (c->comm) NCCL_TRY(g_nccl.AllGather(mine, c->x_size.p, 1, Nccl::kUint64, c->comm, c->stream));
-  CU(cudaMemcpyAsync(sizes, c->x_size.p, (size_t)R * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return B2P_OK;
+  return rank_table(c, 1, Nccl::kUint64, sizes, [&](void* mine) {
+    CU(cudaMemcpyAsync(mine, &b, 8, cudaMemcpyHostToDevice, c->stream));
+    return B2P_OK;
+  });
 }
 
 // Every rank's block, laid back to back in rank order into the host buffer `out` (sum of sizes bytes): this rank's block
@@ -285,8 +261,7 @@ int b2p_group_keys_sizes(b2p_ctx* c, uint64_t bytes, uint64_t* sizes) {
 // rank's place (no block is padded), and the buffer comes back.  Synchronises the stream.
 int b2p_group_keys_allgather(b2p_ctx* c, const void* block, const uint64_t* sizes, void* out) {
   if (!c || !sizes) return fail(B2P_E_INVALID, "NULL argument");
-  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
-  const uint32_t R = c->comm ? (uint32_t)c->comm_ranks : 1u, me = c->comm ? (uint32_t)c->comm_rank : 0u;
+  const uint32_t R = (uint32_t)c->comm_ranks, me = (uint32_t)c->comm_rank;
   uint64_t N = 0, mine = 0;
   for (uint32_t r = 0; r < R; ++r) {
     if (r == me) mine = N;
@@ -300,15 +275,7 @@ int b2p_group_keys_allgather(b2p_ctx* c, const void* block, const uint64_t* size
   if ((rc = c->x_recv.ensure(N))) return rc;
   unsigned char* all = static_cast<unsigned char*>(c->x_recv.p);
   if (sizes[me]) CU(cudaMemcpyAsync(all + mine, block, sizes[me], cudaMemcpyHostToDevice, c->stream));
-  if (c->comm) {
-    NCCL_TRY(g_nccl.GroupStart());
-    uint64_t off = 0;
-    for (uint32_t r = 0; r < R; ++r) {
-      if (sizes[r]) NCCL_TRY(g_nccl.Broadcast(all + off, all + off, sizes[r], Nccl::kUint8, (int)r, c->comm, c->stream));
-      off += sizes[r];
-    }
-    NCCL_TRY(g_nccl.GroupEnd());
-  }
+  if ((rc = gather_blocks(c, all, sizes, 1, Nccl::kUint8))) return rc;
   CU(cudaMemcpyAsync(out, all, N, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   return B2P_OK;
@@ -319,16 +286,14 @@ int b2p_allreduce_columns_dev(b2p_ctx* c, double* sum, uint64_t* cnt, uint32_t n
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
   if (n_cols == 0) return B2P_OK;
   if (!sum || !cnt) return fail(B2P_E_INVALID, "NULL argument");
-  if (!c->comm) {
-    if (c->comm_ranks == 1) return B2P_OK;
-    return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
-  }
+  if (!c->comm) return B2P_OK;
   DeviceGuard g(c->device);
   stage_begin(c, 4);
-  NCCL_TRY(g_nccl.GroupStart());
-  NCCL_TRY(g_nccl.AllReduce(sum, sum, n_cols, Nccl::kFloat64, Nccl::kSum, c->comm, c->stream));
-  NCCL_TRY(g_nccl.AllReduce(cnt, cnt, n_cols, Nccl::kUint64, Nccl::kSum, c->comm, c->stream));
-  NCCL_TRY(g_nccl.GroupEnd());
+  if (int rc = nccl_group([&] {
+        NCCL_TRY(g_nccl.AllReduce(sum, sum, n_cols, Nccl::kFloat64, Nccl::kSum, c->comm, c->stream));
+        NCCL_TRY(g_nccl.AllReduce(cnt, cnt, n_cols, Nccl::kUint64, Nccl::kSum, c->comm, c->stream));
+        return B2P_OK;
+      })) return rc;
   stage_end(c, 4);
   return B2P_OK;
 }

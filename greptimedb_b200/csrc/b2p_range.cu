@@ -441,7 +441,6 @@ static bool fused_group_ok(b2p_ctx* c, const b2p_range_params* p, int64_t T, con
 // all-reduced over the context's communicator as soon as the tile is complete, on the (high-priority) communication
 // stream, while the next tile computes.
 static int launch_allreduce_tiles(b2p_ctx* c, const b2p_ctx::Pending& pc, uint32_t n_tiles) {
-  if (!c->comm && c->comm_ranks > 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
   const RangeArgs& a = pc.args;
   const uint64_t span = (uint64_t)a.g_hi - a.g_lo;
   c->comm_reserve_now = (c->comm && n_tiles > 1) ? c->comm_reserve_sms : 0;
@@ -466,10 +465,8 @@ static int launch_allreduce_tiles(b2p_ctx* c, const b2p_ctx::Pending& pc, uint32
       CU(cudaStreamWaitEvent(c->stream, c->ev_comm_go, 0));
       if (c->comm_headstart_cycles > 0) comm_headstart_kernel<<<1, 32, 0, c->stream>>>(c->comm_headstart_cycles);
       stage_begin(c, 4, c->s_comm);
-      NCCL_TRY(g_nccl.GroupStart());
-      NCCL_TRY(g_nccl.AllReduce(a.gsum + off, a.gsum + off, cnt_n, Nccl::kFloat64, Nccl::kSum, c->comm, c->s_comm));
-      NCCL_TRY(g_nccl.AllReduce(a.gcnt + off, a.gcnt + off, cnt_n, Nccl::kUint32, Nccl::kSum, c->comm, c->s_comm));
-      NCCL_TRY(g_nccl.GroupEnd());
+      if (int rc = allreduce_with_counts(c, a.gsum + off, Nccl::kFloat64, Nccl::kSum, a.gcnt + off, cnt_n, c->s_comm))
+        return rc;
       stage_end(c, 4, c->s_comm);
     }
   }

@@ -37,13 +37,15 @@ int k0_fail(uint32_t k0);
 
 // NCCL, bound at run time: libnccl.so.2 is not a link dependency (single-GPU users never need it), and inside a
 // process that already loaded an NCCL (e.g. the one bundled with torch) dlopen hands back that same library.
-// Only the handful of entry points the by-label all-reduce and the sharded topk, quantile, count_values and sort need
-// (the sharded sort broadcasts each rank's block of its own size); enum values are NCCL's ABI (nccl.h).
+// Only the entry points the by-label all-reduce and the sharded operators need, called through nccl_group (every
+// group), allreduce_with_counts (partials and their counts), rank_table (a per-rank table) and gather_blocks
+// (variable-size blocks); enum values are NCCL's ABI (nccl.h).
 struct Nccl {
   typedef struct ncclComm* comm_t;
   struct unique_id { char internal[128]; };
   enum { kSum = 0, kMax = 2, kMin = 3 };
   enum { kUint8 = 1, kUint32 = 3, kInt64 = 4, kUint64 = 5, kFloat64 = 8 };
+  static size_t bytes(int type) { return type == kUint8 ? 1 : type == kUint32 ? 4 : 8; }  // of one element
   int (*GetUniqueId)(unique_id*) = nullptr;
   int (*CommInitRank)(comm_t*, int, unique_id, int) = nullptr;
   int (*CommDestroy)(comm_t) = nullptr;
@@ -85,6 +87,17 @@ extern Nccl g_nccl;
     int r__ = (x);                                                                                           \
     if (r__ != 0) return fail(B2P_E_CUDA, "%s: %s", #x, g_nccl.GetErrorString ? g_nccl.GetErrorString(r__) : "NCCL error"); \
   } while (0)
+
+// ncclGroupStart, body() (which enqueues collectives and returns a status), then ncclGroupEnd on every path: NCCL's
+// group depth is per thread, so a group left open by a failed enqueue would defer every later collective of the
+// thread.  Returns the first error.
+template <class Body>
+int nccl_group(Body&& body) {
+  NCCL_TRY(g_nccl.GroupStart());
+  const int rc = body(), end = g_nccl.GroupEnd();
+  if (!rc && end) return fail(B2P_E_CUDA, "ncclGroupEnd: %s", g_nccl.GetErrorString(end));
+  return rc;
+}
 
 // A device allocation that grows on demand and is freed with its owner (the context).
 struct DevBuf {
@@ -169,7 +182,8 @@ struct b2p_ctx {
   };
   std::vector<Pending> pending;
   DevBuf slow_list, w_list, b_list, arena_ts, arena_val, win_scratch;
-  // multi-GPU (one process per GPU): communicator of the by-label all-reduce, its stream and join event
+  // multi-GPU (one process per GPU): communicator of the by-label all-reduce, its stream and join event.  Invariant:
+  // comm == nullptr => comm_ranks == 1 && comm_rank == 0, so without a communicator a context is rank 0 of one.
   Nccl::comm_t comm = nullptr;
   int comm_ranks = 1, comm_rank = 0;
   long long comm_headstart_cycles = 60000;  // ~30 us at 1.98 GHz, the H100's top SM clock (B2P_COMM_HEADSTART_US overrides)
@@ -280,6 +294,27 @@ struct DeviceGuard {
     if (prev >= 0 && cur != prev) cudaSetDevice(prev);
   }
 };
+
+// The per-rank table [n_ranks x count] of NCCL `type` in x_size: fill(mine) enqueues this rank's slot, the slots are
+// all-gathered in place (with a communicator) and the table is copied to `host`.  Synchronises the stream.
+template <class Fill>
+int rank_table(b2p_ctx* c, size_t count, int type, void* host, Fill&& fill) {
+  const size_t bytes = count * Nccl::bytes(type), table = (size_t)c->comm_ranks * bytes;
+  if (int rc = c->x_size.ensure(table)) return rc;
+  char* mine = c->x_size.as<char>() + (size_t)c->comm_rank * bytes;
+  if (int rc = fill(mine)) return rc;
+  if (c->comm) NCCL_TRY(g_nccl.AllGather(mine, c->x_size.p, count, type, c->comm, c->stream));
+  CU(cudaMemcpyAsync(host, c->x_size.p, table, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return B2P_OK;
+}
+
+// b2p_context.cu: one group of two in-place all-reduces on `s`: n partials of NCCL `type` by `op`, and their n u32
+// counts added
+int allreduce_with_counts(b2p_ctx* c, void* val, int type, int op, uint32_t* cnt, uint64_t n, cudaStream_t s);
+// b2p_context.cu: the blocks of `buf`, back to back in rank order (block r: sizes[r] entries of `entry_bytes`), this
+// rank's in place: with a communicator, one ncclBroadcast of NCCL `type` per rank with entries, in one group.
+int gather_blocks(b2p_ctx* c, void* buf, const uint64_t* sizes, size_t entry_bytes, int type);
 
 // the CUDA events around a stage's kernels, on `s` (default: the context's stream)
 inline void stage_begin(b2p_ctx* c, int stage, cudaStream_t s = nullptr) {

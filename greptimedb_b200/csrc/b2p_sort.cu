@@ -151,22 +151,17 @@ int check_shard_grid(const double* const* vals, int32_t n_fields, const uint32_t
 // This rank's valid cells (K13's count) into counts[0], or with a communicator every rank's into counts[n_ranks] (one
 // in-place all-gather of 8 B per rank).  Reads the table back, so it synchronises the stream.
 int shard_counts(b2p_ctx* c, const uint32_t* valid, uint32_t n_rows, uint64_t T, uint64_t* counts) {
-  int rc;
-  const uint32_t R = c->comm ? (uint32_t)c->comm_ranks : 1u;
-  if ((rc = c->x_size.ensure((size_t)R * 8))) return rc;
-  unsigned long long* mine = c->x_size.as<unsigned long long>() + (c->comm ? c->comm_rank : 0);
-  if (n_rows && T) {
-    if ((rc = c->so_off.ensure(((size_t)n_rows + 1) * 8))) return rc;
-    unsigned long long* off = c->so_off.as<unsigned long long>();
-    if ((rc = scan_valid_cells(c, valid, T, n_rows, off, c->so_tmp))) return rc;
-    CU(cudaMemcpyAsync(mine, off + n_rows, 8, cudaMemcpyDeviceToDevice, c->stream));
-  } else {
-    CU(cudaMemsetAsync(mine, 0, 8, c->stream));
-  }
-  if (c->comm) NCCL_TRY(g_nccl.AllGather(mine, c->x_size.p, 1, Nccl::kUint64, c->comm, c->stream));
-  CU(cudaMemcpyAsync(counts, c->x_size.p, (size_t)R * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  return B2P_OK;
+  return rank_table(c, 1, Nccl::kUint64, counts, [&](void* mine) {
+    if (n_rows && T) {
+      if (int rc = c->so_off.ensure(((size_t)n_rows + 1) * 8)) return rc;
+      unsigned long long* off = c->so_off.as<unsigned long long>();
+      if (int rc = scan_valid_cells(c, valid, T, n_rows, off, c->so_tmp)) return rc;
+      CU(cudaMemcpyAsync(mine, off + n_rows, 8, cudaMemcpyDeviceToDevice, c->stream));
+    } else {
+      CU(cudaMemsetAsync(mine, 0, 8, c->stream));
+    }
+    return B2P_OK;
+  });
 }
 
 // Per-rank step: K14 over the rank's rows with its cells written into the block's last section, then the pack in
@@ -284,7 +279,6 @@ int sort_allgather(b2p_ctx* c, int desc, const double* const* vals, int32_t F, c
                    unsigned long long* out_cells, double* const* out_vals, bool i64) {
   if (!c || !counts || !out_vals) return fail(B2P_E_INVALID, "NULL argument");
   if (int rc = check_shard_grid(vals, F, valid, row_id, n_rows, T)) return rc;
-  if (!c->comm && c->comm_ranks != 1) return fail(B2P_E_INVALID, "no communicator: call b2p_comm_init first");
   const uint32_t R = (uint32_t)c->comm_ranks, me = (uint32_t)c->comm_rank;
   uint64_t N = 0, mine = 0;
   for (uint32_t r = 0; r < R; ++r) {
@@ -302,16 +296,7 @@ int sort_allgather(b2p_ctx* c, int desc, const double* const* vals, int32_t F, c
   unsigned long long* all = c->x_recv.as<unsigned long long>();
   stage_begin(c, 3);
   if ((rc = shard_pack(c, desc, vals, F, valid, row_id, n_rows, T, counts[me], all + mine * E, i64))) return rc;
-  if (c->comm && N) {
-    NCCL_TRY(g_nccl.GroupStart());
-    uint64_t off = 0;
-    for (uint32_t r = 0; r < R; ++r) {
-      if (counts[r])
-        NCCL_TRY(g_nccl.Broadcast(all + off, all + off, counts[r] * E, Nccl::kUint64, (int)r, c->comm, c->stream));
-      off += counts[r] * E;
-    }
-    NCCL_TRY(g_nccl.GroupEnd());
-  }
+  if (N && (rc = gather_blocks(c, all, counts, E * 8, Nccl::kUint64))) return rc;
   rc = shard_merge(c, desc, F, counts, R, all, out_cells, out_vals, i64);
   stage_end(c, 3);
   c->last_exchange_bytes = (long long)(counts[me] * E * 8);

@@ -67,6 +67,30 @@ def finalize_host(agg: str, sum_a: np.ndarray, cnt_a: np.ndarray) -> np.ndarray:
     return out
 
 
+_SIGN = np.uint64(1 << 63)
+
+
+def _key(x):
+    """u64 total-order key of float64 values: unsigned order of the keys is f64::total_cmp order"""
+    b = np.ascontiguousarray(x, np.float64).view(np.uint64)
+    return np.where(b >> np.uint64(63) != 0, ~b, b | _SIGN)
+
+
+def _value(u):
+    """float64 values of u64 total-order keys (the inverse of _key)"""
+    return np.ascontiguousarray(np.where(u >> np.uint64(63) != 0, u ^ _SIGN, ~u), np.uint64).view(np.float64)
+
+
+def _all_gather(arr, group):
+    """every rank's numpy array `arr` (the same shape and dtype on every rank), in rank order"""
+    import torch
+    import torch.distributed as dist
+    t = torch.from_numpy(np.ascontiguousarray(arr))
+    out = [torch.empty_like(t) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(out, t, group=group)
+    return [o.numpy() for o in out]
+
+
 def total_key(x):
     """f64::total_cmp key of a float64 tensor as int64: the bit pattern with the 63 low bits flipped where the sign bit
     is set.  Applied to the int64 keys (or their bit patterns) it gives the bit patterns back: an involution."""
@@ -114,8 +138,7 @@ def merge_partials(agg: str, val_t, cnt_t, mean_t=None, group=None):
 def topk_key_host(bottom: bool, vals: np.ndarray, tie: np.ndarray):
     """The rank key of every cell of K10, (hi, lo) = (f64 total-order key as u64, tie), both bit-inverted for bottomk so
     that better is always larger."""
-    b = np.ascontiguousarray(vals, np.float64).view(np.uint64)
-    hi = np.where(b >> np.uint64(63) != 0, ~b, b | np.uint64(1 << 63))
+    hi = _key(vals)
     lo = np.broadcast_to(np.asarray(tie, np.uint32)[:, None], hi.shape)
     return (~hi, ~lo) if bottom else (hi, lo.copy())
 
@@ -133,7 +156,6 @@ def merge_topk_candidates(bottom: bool, kk: int, vals: np.ndarray, ok: np.ndarra
       - each rank keeps its own valid cells at or above the threshold, or every one below the bounds taken ("all")."""
     import torch
     import torch.distributed as dist
-    world = dist.get_world_size(group)
     R, T = vals.shape
     gid = np.asarray(gid, np.int64)
     ing = gid < n_groups
@@ -179,11 +201,7 @@ def merge_topk_candidates(bottom: bool, kk: int, vals: np.ndarray, ok: np.ndarra
             s_hi[i, :, :take] = np.take_along_axis(h, order[:take], axis=0).T
             s_lo[i, :, :take] = np.take_along_axis(l, order[:take], axis=0).T
             s_n[i] = n
-        parts = []
-        for t in (torch.from_numpy(s_hi.view(np.int64)), torch.from_numpy(s_lo.astype(np.int64)), torch.from_numpy(s_n)):
-            out = [torch.empty_like(t) for _ in range(world)]
-            dist.all_gather(out, t, group=group)
-            parts.append([o.numpy() for o in out])
+        parts = [_all_gather(a, group) for a in (s_hi.view(np.int64), s_lo.astype(np.int64), s_n)]
         g_hi = np.concatenate([p.view(np.uint64) for p in parts[0]], axis=2)      # [X, T, world * K]
         g_lo = np.concatenate([p.astype(np.uint32) for p in parts[1]], axis=2)
         g_on = np.concatenate([np.arange(K)[None, None, :] < p[:, :, None] for p in parts[2]], axis=2)
@@ -258,8 +276,7 @@ def merge_quantile_digits(phi, vals: np.ndarray, ok: np.ndarray, gid: np.ndarray
     cnt = np.zeros((G, T), np.uint32)
     if G == 0 or T == 0:
         return out, cnt, 0, 0
-    bits = vals.view(np.uint64)
-    keys = np.where(bits >> np.uint64(63) != 0, ~bits, bits | sign)
+    keys = _key(vals)
     gid = np.asarray(gid, np.int64)
     rr, rt = np.nonzero(np.asarray(ok, bool) & (gid < G)[:, None])
     rg, rk = gid[rr], keys[rr, rt]
@@ -274,9 +291,6 @@ def merge_quantile_digits(phi, vals: np.ndarray, ok: np.ndarray, gid: np.ndarray
     def under(p, lv):
         sh = np.minimum(64 - 4 * lv, 63).astype(np.uint64)
         return (lv == 0) | ((rk >> sh) == (p >> sh))
-
-    def value(u):  # keys -> f64
-        return np.ascontiguousarray(np.where(u >> np.uint64(63) != 0, u ^ sign, ~u), np.uint64).view(np.float64)
 
     passes = 0
     for _ in range(QUANT_SHARD_PASSES):
@@ -347,7 +361,7 @@ def merge_quantile_digits(phi, vals: np.ndarray, ok: np.ndarray, gid: np.ndarray
             rank = np.float64(phi) * (np.maximum(cnt[g], 1) - 1).astype(np.float64)
             w = rank - np.floor(rank)
             with np.errstate(invalid="ignore", over="ignore"):
-                res = value(p_lo[g]) * (np.float64(1.0) - w) + value(p_hi[g]) * w
+                res = _value(p_lo[g]) * (np.float64(1.0) - w) + _value(p_hi[g]) * w
             out[g] = np.where(has[g], res, 0.0)
     return out, cnt, passes, passes * G * ((T + 31) // 32) * QUANT_UNIT_BYTES
 
@@ -366,7 +380,6 @@ def merge_count_values(vals: np.ndarray, cnt: np.ndarray, gid: np.ndarray, n_gro
         the largest key with count 0, padded to the largest rank's rows; the blocks are all-gathered;
       - per (group, step) the entries of every rank are sorted by key, each run of equal keys is one value with the sum
         of its counts, and a run whose counts add up to 0 is no value."""
-    import torch
     import torch.distributed as dist
     world = dist.get_world_size(group)
     vals = np.ascontiguousarray(vals, np.float64)
@@ -380,24 +393,18 @@ def merge_count_values(vals: np.ndarray, cnt: np.ndarray, gid: np.ndarray, n_gro
     for g in range(G):
         rows = np.flatnonzero(has[goff[g]:goff[g + 1]])
         h[g] = rows[-1] + 1 if rows.size else 0
-    parts = [torch.empty(G, dtype=torch.int64) for _ in range(world)]
-    dist.all_gather(parts, torch.from_numpy(h.copy()), group=group)
-    heights = np.stack([p.numpy() for p in parts]) if G else np.zeros((world, 0), np.int64)
+    parts = _all_gather(h, group)
+    heights = np.stack(parts) if G else np.zeros((world, 0), np.int64)
     U = heights.sum(axis=0)
     out_goff = np.concatenate([[0], np.cumsum(U)]).astype(np.int64)
     P = int(heights.sum(axis=1).max()) if G else 0
-    bits = vals.view(np.uint64)
-    keys = np.where(bits >> np.uint64(63) != 0, ~bits, bits | np.uint64(1 << 63))
+    keys = _key(vals)
     mine = np.concatenate([np.arange(goff[g], goff[g] + h[g]) for g in range(G)] + [np.zeros(0, np.int64)])
     s_key = np.full((P, T), np.uint64(0xFFFFFFFFFFFFFFFF), np.uint64)
     s_cnt = np.zeros((P, T), np.int64)
     s_key[:mine.size] = np.where(cnt[mine] != 0, keys[mine], np.uint64(0xFFFFFFFFFFFFFFFF))
     s_cnt[:mine.size] = cnt[mine]
-    got = []
-    for t in (torch.from_numpy(s_key.view(np.int64)), torch.from_numpy(s_cnt)):
-        out = [torch.empty_like(t) for _ in range(world)]
-        dist.all_gather(out, t, group=group)
-        got.append([o.numpy() for o in out])
+    got = [_all_gather(a, group) for a in (s_key.view(np.int64), s_cnt)]
     e_g, e_k, e_key, e_cnt = [], [], [], []
     for r in range(world):
         row_g = np.repeat(np.arange(G), heights[r])
@@ -423,7 +430,7 @@ def merge_count_values(vals: np.ndarray, cnt: np.ndarray, gid: np.ndarray, n_gro
         first = np.searchsorted(seg, seg)              # each (group, step)'s first value
         j = np.arange(seg.size) - first
         u = key_s[keep]
-        out_v[out_goff[g_r] + j, k_r] = np.where(u >> np.uint64(63) != 0, u ^ np.uint64(1 << 63), ~u).view(np.float64)
+        out_v[out_goff[g_r] + j, k_r] = _value(u)
         out_c[out_goff[g_r] + j, k_r] = sums
     return out_v, out_c, out_goff, P * T * CV_ENTRY_BYTES
 
@@ -438,9 +445,6 @@ def merge_sorted_runs(desc: bool, vals, ok: np.ndarray, row_id: np.ndarray, grou
         total_key ^ 2^63 (Int64: bits ^ 2^63), inverted for desc, sorted: its run;
       - the counts are all-gathered, every run is padded to the largest and all-gathered;
       - the runs are merged by (keys, cell) ascending, and the values decoded from the keys."""
-    import torch
-    import torch.distributed as dist
-    world = dist.get_world_size(group)
     many = isinstance(vals, (list, tuple))
     grids = [np.asarray(v) for v in vals] if many else [np.asarray(vals)]
     i64 = grids[0].dtype == np.int64
@@ -455,29 +459,24 @@ def merge_sorted_runs(desc: bool, vals, ok: np.ndarray, row_id: np.ndarray, grou
     cells = np.flatnonzero(ok.reshape(-1)).astype(np.uint64)
     keys = []
     for g in grids:
-        b = np.ascontiguousarray(g).reshape(-1).view(np.uint64)[cells]
-        k = b ^ sign if i64 else np.where(b >> np.uint64(63) != 0, ~b, b | sign)
+        b = np.ascontiguousarray(g).reshape(-1)[cells]
+        k = b.view(np.uint64) ^ sign if i64 else _key(b)
         keys.append(k ^ flip)
     glob = row_id[cells // np.uint64(T)] * np.uint64(T) + cells % np.uint64(T) if T else cells
-    n = torch.tensor([cells.size], dtype=torch.int64)
-    ns = [torch.zeros(1, dtype=torch.int64) for _ in range(world)]
-    dist.all_gather(ns, n, group=group)
-    ns = [int(x.item()) for x in ns]
+    ns = [int(x[0]) for x in _all_gather(np.array([cells.size], np.int64), group)]
     P = max(ns)
     block = np.zeros((F + 1, P), np.uint64)
     if cells.size:
         order = np.lexsort([glob] + keys[::-1])
         block[:F, :cells.size] = np.stack(keys)[:, order]
         block[F, :cells.size] = glob[order]
-    got = [torch.empty((F + 1, P), dtype=torch.int64) for _ in range(world)]
-    dist.all_gather(got, torch.from_numpy(block.view(np.int64)), group=group)
-    runs = np.concatenate([g.numpy().view(np.uint64)[:, :m] for g, m in zip(got, ns)], axis=1)
+    got = _all_gather(block.view(np.int64), group)
+    runs = np.concatenate([g.view(np.uint64)[:, :m] for g, m in zip(got, ns)], axis=1)
     merged = runs[:, np.lexsort([runs[F]] + [runs[f] for f in range(F - 1, -1, -1)])]
     out = []
     for f in range(F):
         u = merged[f] ^ flip
-        bits = u ^ sign if i64 else np.where(u >> np.uint64(63) != 0, u ^ sign, ~u)
-        out.append(bits.view(np.int64 if i64 else np.float64))
+        out.append((u ^ sign).view(np.int64) if i64 else _value(u))
     return merged[F].copy(), (out if many else out[0]), int(cells.size) * 8 * (F + 1)
 
 
@@ -585,13 +584,10 @@ def agree_group_keys(tuples, n_labels: int, ids=None, group=None):
     sizes, then one broadcast per rank with bytes."""
     import torch
     import torch.distributed as dist
-    world = dist.get_world_size(group)
     me = dist.get_rank(group)
     mine = serialize_group_keys(tuples, n_labels, ids)  # (no field types: the mirror agrees the labels)
-    sizes = [torch.zeros(1, dtype=torch.int64) for _ in range(world)]
-    dist.all_gather(sizes, torch.tensor([len(mine)], dtype=torch.int64), group=group)
     blocks = []
-    for r, n in enumerate(int(s.item()) for s in sizes):
+    for r, n in enumerate(int(s[0]) for s in _all_gather(np.array([len(mine)], np.int64), group)):
         buf = torch.frombuffer(bytearray(mine), dtype=torch.uint8) if r == me else torch.zeros(n, dtype=torch.uint8)
         if n:
             dist.broadcast(buf, src=r, group=group)

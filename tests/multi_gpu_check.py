@@ -10,25 +10,17 @@ import sys
 
 import numpy as np
 import torch
-import torch.distributed as dist
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from tests.ranks import rank_session  # noqa: E402
 
 
-def main():
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    dist.init_process_group("nccl", device_id=dev)
-    from greptimedb_b200 import Context, make_params
+def main(s):
+    rank, world, dev, ctx = s.rank, s.world, s.dev, s.ctx
+    from greptimedb_b200 import make_params
     from greptimedb_b200 import distributed as D
     from oracle import oracle as orc
-    ctx = Context(local)
-    ctx.use_own_stream()
-    box = [ctx.comm_unique_id() if rank == 0 else None]
-    dist.broadcast_object_list(box, src=0)
-    ctx.comm_init(box[0], world, rank)
 
     S, N, G, T0 = 2400, 500, 61, 1_700_000_000_000
     ts, val, sid = orc.synth_fill(0, S, N, T0, 15_000, 1000, 1, 0x5EED)
@@ -111,15 +103,9 @@ def main():
         ctx.sync()
         got, cnt = pv.cpu().numpy().reshape(TG, TT), pc.cpu().numpy().view(np.uint32).reshape(TG, TT)
         ok = ok and bool((cnt == e_c).all()) and bool((got.view(np.uint64) == e_val.view(np.uint64)).all())
-    ctx.comm_destroy()
-    ctx.close()
-    verdict = torch.tensor([1.0 if (ok and worst <= 1e-9) else 0.0], device=dev)
-    dist.all_reduce(verdict, op=dist.ReduceOp.MIN)
-    if rank == 0:
-        print(f"MULTI_GPU_CHECK world={world} ok={bool(verdict.item() == 1.0)} worst_rel={worst:.3e}", flush=True)
-    dist.destroy_process_group()
-    sys.exit(0 if verdict.item() == 1.0 else 1)
+    s.note = f"worst_rel={worst:.3e}"
+    return [] if ok and worst <= 1e-9 else [f"rank {rank}: counts or values differ, worst_rel={worst:.3e}"]
 
 
 if __name__ == "__main__":
-    main()
+    rank_session("MULTI_GPU_CHECK", main)

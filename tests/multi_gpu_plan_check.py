@@ -1,5 +1,5 @@
 """Multi-rank check of sharded plan nodes over the library's communicator (run under torchrun, one rank per GPU; started
-by tests/test_multi_gpu_plan.py when at least two GPUs are visible): every rank regenerates the same table from a seed,
+by tests/test_multi_gpu.py when at least two GPUs are visible): every rank regenerates the same table from a seed,
 pushes the series distributed.shard_of_series gives it into a sharded aggregate node (and, over Float64, a leaf with a
 sharded aggregate stage) and a sharded count_values node, and its export must equal the unsharded node over the whole table on
 its own GPU: bit for bit for count, group, min, max, quantile, count_values and Int64 sum; the Float64 sum and avg bit
@@ -14,11 +14,11 @@ import sys
 
 import numpy as np
 import pyarrow as pa
-import torch
 import torch.distributed as dist
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from tests.ranks import rank_session  # noqa: E402
 
 EXACT = {"count", "group", "min", "max", "quantile"}
 
@@ -102,18 +102,12 @@ def mirror(plain, world, op, by, i64, owner_of):
     return out
 
 
-def main():
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    dist.init_process_group("nccl", device_id=dev)
+def main(s):
+    rank, world, ctx = s.rank, s.world, s.ctx
     from greptimedb_b200 import Context
     from greptimedb_b200 import distributed as D
     from greptimedb_b200.plan import AggregatePlan, CountValuesPlan
-    plain, ctx = Context(local), Context(local)
-    box = [ctx.comm_unique_id() if rank == 0 else None]
-    dist.broadcast_object_list(box, src=0)
-    ctx.comm_init(box[0], world, rank)
+    plain = Context(ctx.device)
     owner_of = lambda s: int(D.shard_of_series(np.array([s], np.uint32), world)[0])  # noqa: E731
     mine = lambda s: owner_of(s) == rank  # noqa: E731
     bad, digests = [], []
@@ -168,17 +162,9 @@ def main():
     dist.all_gather_object(every, digests)
     if any(d != every[0] for d in every):
         bad.append("exports differ across ranks")
-    for b in bad:
-        print(b, flush=True)
-    verdict = torch.tensor([0.0 if bad else 1.0], device=dev)
-    dist.all_reduce(verdict, op=dist.ReduceOp.MIN)
-    if rank == 0:
-        print(f"MULTI_GPU_PLAN_CHECK world={world} ok={bool(verdict.item() == 1.0)}", flush=True)
-    ctx.comm_destroy()
-    ctx.close()
     plain.close()
-    dist.destroy_process_group()
+    return bad
 
 
 if __name__ == "__main__":
-    main()
+    rank_session("MULTI_GPU_PLAN_CHECK", main)

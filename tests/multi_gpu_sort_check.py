@@ -1,5 +1,5 @@
 """Multi-rank check of the sharded sort over the library's communicator (run under torchrun, one rank per GPU; started
-by tests/test_multi_gpu_sort.py when at least two GPUs are visible): every rank regenerates the same grid from a seed
+by tests/test_multi_gpu.py when at least two GPUs are visible): every rank regenerates the same grid from a seed
 (the total-order specials, T = 1 and T = 37, and two fields), keeps the rows distributed.shard_rows gives it with their
 global row ids, counts its cells, and runs b2p_sort_cells_allgather_dev in both directions; every rank's cells and
 values == b2p_sort_cells_dev (_fields_dev) over all rows on its own GPU, bit for bit.  torch.distributed only carries
@@ -9,26 +9,17 @@ import sys
 
 import numpy as np
 import torch
-import torch.distributed as dist
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from tests.ranks import rank_session  # noqa: E402
 
 
-def main():
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    dist.init_process_group("nccl", device_id=dev)
-    from greptimedb_b200 import Context
+def main(s):
+    rank, world, dev, ctx = s.rank, s.world, s.dev, s.ctx
     from greptimedb_b200 import distributed as D
     from tests import select_keys as sk
     from tests.test_sort_oracle import TOTAL_ORDER
-    ctx = Context(local)
-    ctx.use_own_stream()
-    box = [ctx.comm_unique_id() if rank == 0 else None]
-    dist.broadcast_object_list(box, src=0)
-    ctx.comm_init(box[0], world, rank)
     bad = []
     for R, T, F in ((200_000, 1, 1), (3000, 37, 1), (3000, 37, 2)):
         rng = np.random.default_rng(R + T + F)
@@ -69,17 +60,8 @@ def main():
                     bad.append(f"values differ: R={R} T={T} F={F} desc={desc} field {f} rank={rank}")
             if sent != int(counts[rank]) * 8 * (F + 1):
                 bad.append(f"exchange bytes {sent} on rank {rank}")
-    ctx.comm_destroy()
-    ctx.close()
-    verdict = torch.tensor([0.0 if bad else 1.0], device=dev)
-    dist.all_reduce(verdict, op=dist.ReduceOp.MIN)
-    for b in bad:
-        print(b, flush=True)
-    if rank == 0:
-        print(f"MULTI_GPU_SORT_CHECK world={world} ok={bool(verdict.item() == 1.0)}", flush=True)
-    dist.destroy_process_group()
-    sys.exit(0 if verdict.item() == 1.0 else 1)
+    return bad
 
 
 if __name__ == "__main__":
-    main()
+    rank_session("MULTI_GPU_SORT_CHECK", main)

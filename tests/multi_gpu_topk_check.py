@@ -1,5 +1,5 @@
 """Multi-rank check of the sharded topk / bottomk over the library's communicator (run under torchrun, one rank per
-GPU; started by tests/test_multi_gpu_topk.py when at least two GPUs are visible): rate() over series hash-sharded with
+GPU; started by tests/test_multi_gpu.py when at least two GPUs are visible): rate() over series hash-sharded with
 distributed.shard_rows, then b2p_topk_allgather_dev for k = 5 and k = 40 (rounds), with one group and by 7 groups; the
 union of the ranks' kept cells == select_keys.topk over the oracle's full grid, bit for bit.  torch.distributed only
 carries the 128-byte communicator id and the verdict."""
@@ -8,26 +8,18 @@ import sys
 
 import numpy as np
 import torch
-import torch.distributed as dist
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from tests.ranks import rank_session  # noqa: E402
 
 
-def main():
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    torch.cuda.set_device(local)
-    dev = torch.device("cuda", local)
-    dist.init_process_group("nccl", device_id=dev)
-    from greptimedb_b200 import Context, make_params
+def main(s):
+    rank, world, dev, ctx = s.rank, s.world, s.dev, s.ctx
+    from greptimedb_b200 import make_params
     from greptimedb_b200 import distributed as D
     from oracle import oracle as orc
     from tests import select_keys as sk
-    ctx = Context(local)
-    ctx.use_own_stream()
-    box = [ctx.comm_unique_id() if rank == 0 else None]
-    dist.broadcast_object_list(box, src=0)
-    ctx.comm_init(box[0], world, rank)
 
     S, N, T0 = 1200, 300, 1_700_000_000_000
     ts, val, sid = orc.synth_fill(0, S, N, T0, 15_000, 1000, 1, 0x70B)
@@ -68,17 +60,8 @@ def main():
                 if not (got == exp).all():
                     bad.append(f"{op}({k}) by {G} groups: {int((got != exp).sum())} words differ on rank {rank}")
         ctx.group_index_destroy(ix)
-    ctx.comm_destroy()
-    ctx.close()
-    verdict = torch.tensor([0.0 if bad else 1.0], device=dev)
-    dist.all_reduce(verdict, op=dist.ReduceOp.MIN)
-    for b in bad:
-        print(b, flush=True)
-    if rank == 0:
-        print(f"MULTI_GPU_TOPK_CHECK world={world} ok={bool(verdict.item() == 1.0)}", flush=True)
-    dist.destroy_process_group()
-    sys.exit(0 if verdict.item() == 1.0 else 1)
+    return bad
 
 
 if __name__ == "__main__":
-    main()
+    rank_session("MULTI_GPU_TOPK_CHECK", main)

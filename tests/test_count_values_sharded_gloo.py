@@ -4,15 +4,10 @@ output (select_keys.count_values over its rows), the host mirror of b2p_count_va
 rows equal the first U_g rows of each group of select_keys.count_values over all rows, bit for bit; the rows past U_g
 have count 0.  Classes: hashed, uneven and empty shards; the same values on both ranks and disjoint values; ±0.0 and NaN
 payloads split across ranks; the largest positive NaN on one rank only; a group present on one rank only."""
-import os
-import socket
-import sys
-
 import numpy as np
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests.ranks import spawn_gloo
+
 MAX_NAN = 0x7FFFFFFFFFFFFFFF
 
 
@@ -78,11 +73,7 @@ def local_heights(vals, ok, gid, n_groups, mine):
     return h
 
 
-def _worker(rank, world, port, q):
-    sys.path.insert(0, ROOT)
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _worker(rank, world):
     from greptimedb_b200 import distributed as D
     from tests import select_keys as sk
     res = []
@@ -90,28 +81,14 @@ def _worker(rank, world, port, q):
         mine = np.flatnonzero(owner == rank)
         lv, lc = sk.count_values(vals[mine], ok[mine], gid[mine], n_groups)
         res.append(D.merge_count_values(lv, lc, np.sort(gid[mine]), n_groups))
-    q.put((rank, res))
-    dist.barrier()
-    dist.destroy_process_group()
+    return res
 
 
 def test_sharded_count_values_equals_the_unsharded_count():
     from greptimedb_b200 import distributed as D
     from tests import select_keys as sk
     world = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=600) for _ in range(world))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got = spawn_gloo(_worker, world, timeout=600)
     for i, (name, vals, ok, gid, n_groups, owner) in enumerate(cases()):
         exp, exp_cnt = sk.count_values(vals, ok, gid, n_groups)
         (o0, c0, u0, b0), (o1, c1, u1, b1) = got[0][i], got[1][i]

@@ -1,32 +1,13 @@
 """World-size-2 gloo test (CPU) of the N>1 host logic: hash-sharding of series, per-rank partial
 (sum, cnt), one all-reduce, finalize == unsharded result.  The per-shard compute is the oracle here
 (the CUDA kernels need a GPU; tests/test_gpu_parity.py covers them)."""
-import os
-import socket
-import sys
-
 import numpy as np
-import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests.ranks import spawn_gloo
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _worker(rank, world, port, q):
-    sys.path.insert(0, ROOT)
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _worker(rank, world):
     from greptimedb_b200 import distributed as D
     from oracle import oracle as orc
     S, N, G, T0 = 96, 200, 7, 1_700_000_000_000
@@ -71,32 +52,11 @@ def _worker(rank, world, port, q):
         e_avg, e_cnt = orc.group_aggregate("avg", full_out, full_valid, gid, G)
         ok_cnt = bool((ct.numpy() == e_cnt).all()) and ok_all
         rel = np.abs(res - e_avg) / np.maximum(np.abs(e_avg), 1e-300)
-        q.put((ok_cnt, float(rel[e_cnt > 0].max()), int(owned.size)))
-    else:
-        q.put((ok_all, 0.0, int(owned.size)))
-    dist.barrier()
-    dist.destroy_process_group()
+        return ok_cnt, float(rel[e_cnt > 0].max()), int(owned.size)
+    return ok_all, 0.0, int(owned.size)
 
 
-def _run(target, world=2):
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=target, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    results = [q.get(timeout=240) for _ in range(world)]
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    return results
-
-
-def _worker_total_order(rank, world, port, q):
-    sys.path.insert(0, ROOT)
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _worker_total_order(rank, world):
     from greptimedb_b200 import distributed as D
     from oracle import oracle as orc
     from tests.helpers import total_order_case
@@ -115,22 +75,20 @@ def _worker_total_order(rank, world, port, q):
         for g, k in diff[:4]:
             bad.append(f"{agg} group {g} step {k}: merged {got[g, k]!r} ({got[g, k:k + 1].view(np.uint64)[0]:#x}), "
                        f"single pass {e_val[g, k]!r} ({e_val[g, k:k + 1].view(np.uint64)[0]:#x})")
-    q.put((not bad, "; ".join(bad), 0))
-    dist.barrier()
-    dist.destroy_process_group()
+    return not bad, "; ".join(bad), 0
 
 
 def test_min_max_merge_follows_the_total_order_across_ranks():
     """NaN (both signs, with and without payload), -0.0 and +0.0 members of one group on different ranks, in every
     placement order: the merged min / max equals the single-pass total-order aggregate bit for bit, and a group absent on
     one rank or on both merges like the single pass too (the neutral element, then 0.0)."""
-    for ok, msg, _ in _run(_worker_total_order):
+    for ok, msg, _ in spawn_gloo(_worker_total_order):
         assert ok, msg
 
 
 def test_sharded_partials_allreduce_equals_unsharded():
     world = 2
-    results = _run(_worker, world)
+    results = spawn_gloo(_worker, world)
     assert all(r[0] for r in results)
     assert max(r[1] for r in results) <= 1e-9          # summation order differs across shards: 1e-9 rel, like the reference
     assert sum(r[2] for r in results) == 96              # every series owned exactly once

@@ -18,6 +18,7 @@ import pytest
 
 from oracle import oracle as orc
 from tests.helpers import total_order_case
+from tests.ranks import one_rank_comm
 
 pytestmark = pytest.mark.gpu
 
@@ -346,23 +347,16 @@ def test_two_shards_on_one_gpu_merge_to_the_single_pass(ctx):
 
 
 def test_single_rank_communicator_round_trips_the_partials():
-    """comm_init(id, 1, 0) then allreduce_partials_dev: min / max partials (NaN payloads, -0.0, absent groups) come back
+    """Over a one-rank communicator, allreduce_partials_dev: min / max partials (NaN payloads, -0.0, absent groups) come back
     bit for bit, absent groups as 0.0 whatever they held; variance states within 1e-12 relative or 1e-12 of the data
     scale (the one-rank mean cnt * mean / cnt may be an ulp off).  On one GPU this is the only run of the merge kernels
     and their total-order key conversion."""
     import torch
-    from greptimedb_b200 import B2PError, Context
+    from greptimedb_b200 import Context
     c = Context(0)
     try:
         c.use_torch_stream()
-        try:
-            uid = c.comm_unique_id()
-        except B2PError as e:
-            if "libnccl" in str(e):
-                pytest.skip(f"NCCL cannot be loaded: {e}")
-            raise
-        c.comm_init(uid, 1, 0)
-        try:
+        with one_rank_comm(c):
             tv, tvalid, tgid, TG = total_order_case()
             for vals, valid, gid, G in ((tv, tvalid, tgid, TG), _mixed_case(7)):
                 T = vals.shape[1]
@@ -387,8 +381,6 @@ def test_single_rank_communicator_round_trips_the_partials():
                         err = np.abs(g_[ok] - e_[ok])
                         assert not ((err > 1e-12 * np.abs(e_[ok])) & (err > 1e-12 * scale ** 2)).any(), agg
                     assert (got[pc == 0] == 0.0).all(), agg
-        finally:
-            c.comm_destroy()
     finally:
         c.close()
 

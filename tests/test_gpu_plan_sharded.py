@@ -9,6 +9,7 @@ import pyarrow as pa
 import pytest
 
 from tests.binary_oracle import _words
+from tests.ranks import one_rank_comm
 
 pytestmark = pytest.mark.gpu
 
@@ -19,17 +20,10 @@ I64_MIN, I64_MAX = -(1 << 63), (1 << 63) - 1
 @pytest.fixture(scope="module")
 def ctxs():
     """(plain context, context with a one-rank communicator)"""
-    from greptimedb_b200 import B2PError, Context
+    from greptimedb_b200 import Context
     plain, comm = Context(0), Context(0)
-    try:
-        uid = comm.comm_unique_id()
-    except B2PError as e:
-        if "libnccl" in str(e):
-            pytest.skip(f"NCCL cannot be loaded: {e}")
-        raise
-    comm.comm_init(uid, 1, 0)
-    yield plain, comm
-    comm.comm_destroy()
+    with one_rank_comm(comm):
+        yield plain, comm
     comm.close()
     plain.close()
 

@@ -10,6 +10,7 @@ import pytest
 
 from tests import nibble_keys as nk
 from tests import select_keys as sk
+from tests.ranks import one_rank_comm
 
 pytestmark = pytest.mark.gpu
 
@@ -245,23 +246,13 @@ def test_composed_call_without_communicator_is_the_single_rank_quantile():
 
 
 def test_single_rank_communicator_round_trips_the_counts():
-    """comm_init(id, 1, 0), then the composed call over NCCL's all-reduces: the output of b2p_group_quantile_dev"""
-    from greptimedb_b200 import B2PError
+    """Over a one-rank communicator, the composed call over NCCL's all-reduces: the output of b2p_group_quantile_dev"""
     T = 70
     vals, ok, gid, n_groups = mixed_grid(4, T, big=3000)
     full = Rank(np.arange(gid.size), vals, sk.words(ok), gid, n_groups)
     try:
-        try:
-            uid = full.ctx.comm_unique_id()
-        except B2PError as e:
-            if "libnccl" in str(e):
-                pytest.skip(f"NCCL cannot be loaded: {e}")
-            raise
-        full.ctx.comm_init(uid, 1, 0)
-        try:
+        with one_rank_comm(full.ctx):
             composed_check(full, vals, ok, gid, n_groups, T)
-        finally:
-            full.ctx.comm_destroy()
     finally:
         full.close()
 

@@ -3,10 +3,13 @@ are simulated on one GPU, one context each: every rank counts its valid cells, t
 every rank packs its block, the blocks are laid back to back in rank order, and every rank merges them; one more merge
 takes the table and the blocks rotated.  Every merge's out_cells must equal b2p_sort_cells_dev over the global grid
 bit for bit, and out_vals the grid's value bits at those cells."""
+import contextlib
+
 import numpy as np
 import pytest
 
 from tests import select_keys as sk
+from tests.ranks import one_rank_comm
 
 pytestmark = pytest.mark.gpu
 
@@ -214,29 +217,19 @@ def test_int64(n_ranks):
 def composed(desc, grids, ok, T, i64=False, comm=False):
     """the composed call over every row on one context (without a communicator, or over a one-rank one)"""
     import torch
-    from greptimedb_b200 import B2PError
     valid = words_with_junk(ok)
     r = Rank(np.arange(ok.shape[0]), grids, valid, T, i64)
     try:
-        if comm:
-            try:
-                uid = r.ctx.comm_unique_id()
-            except B2PError as e:
-                if "libnccl" in str(e):
-                    pytest.skip(f"NCCL cannot be loaded: {e}")
-                raise
-            r.ctx.comm_init(uid, 1, 0)
-        counts = r.ctx.sort_shard_counts_dev(r.valid, r.rows.size, T)
-        N = int(counts.sum())
-        cells = torch.full((max(N, 1),), -1, dtype=torch.int64, device="cuda")
-        dt = torch.int64 if i64 else torch.float64
-        outs = [torch.full((max(N, 1),), -7, dtype=dt, device="cuda") for _ in grids]
-        r.ctx.sort_cells_allgather_dev(desc, r.grid(), r.valid, r.row_id, r.rows.size, T, counts, cells,
-                                       outs if len(grids) > 1 else outs[0], i64=i64)
-        torch.cuda.synchronize()
-        sent = r.ctx.last_exchange_bytes()
-        if comm:
-            r.ctx.comm_destroy()
+        with one_rank_comm(r.ctx) if comm else contextlib.nullcontext():
+            counts = r.ctx.sort_shard_counts_dev(r.valid, r.rows.size, T)
+            N = int(counts.sum())
+            cells = torch.full((max(N, 1),), -1, dtype=torch.int64, device="cuda")
+            dt = torch.int64 if i64 else torch.float64
+            outs = [torch.full((max(N, 1),), -7, dtype=dt, device="cuda") for _ in grids]
+            r.ctx.sort_cells_allgather_dev(desc, r.grid(), r.valid, r.row_id, r.rows.size, T, counts, cells,
+                                           outs if len(grids) > 1 else outs[0], i64=i64)
+            torch.cuda.synchronize()
+            sent = r.ctx.last_exchange_bytes()
     finally:
         r.close()
     exp = single_sort(desc, grids, valid, T, i64)

@@ -18,6 +18,7 @@ reproduces bit for bit:
 Every test asserts the route it means from range_group_sum_fused(), last_warp_tier_series() and last_slow_series(); a
 tiled call's counters cover all of its tiles.
 """
+import contextlib
 import functools
 import os
 
@@ -26,6 +27,7 @@ import pytest
 
 from oracle import oracle as orc
 from tests import sum_by_check as sbc
+from tests.ranks import one_rank_comm
 from tests.range_values import F64_MAX, SUBNORMAL
 
 pytestmark = pytest.mark.gpu
@@ -51,19 +53,6 @@ def _context(**env):
                 os.environ[k] = v
 
 
-def _with_comm(c):
-    """a one-rank communicator on c, or None when NCCL cannot be loaded"""
-    from greptimedb_b200 import B2PError
-    try:
-        uid = c.comm_unique_id()
-    except B2PError as e:
-        if "libnccl" in str(e):
-            return None
-        raise
-    c.comm_init(uid, 1, 0)
-    return c
-
-
 @pytest.fixture(scope="module")
 def ctxs():
     """One context per first-tier route, the adaptive policy off so that each runs the variant it names.  "comm" and
@@ -72,19 +61,18 @@ def ctxs():
     off = {"B2P_LEAN_ADAPTIVE": "0"}
     c = {"default": _context(**off), "uniform": _context(B2P_UNIFORM="1", **off),
          "general": _context(B2P_UNIFORM="0", **off), "flags": _context(B2P_LEAN_FORCE_FLAGS="1", **off)}
-    comms = []
-    for name, env in (("comm", {}), ("comm16", {"B2P_COMM_RESERVE_SMS": "16", "B2P_COMM_HEADSTART_US": "0"})):
-        x = _context(**off, **env)
-        if _with_comm(x) is None:
-            x.close()
-            continue
-        c[name] = x
-        comms.append(x)
-    for x in c.values():
-        x.use_own_stream()
-    yield c
-    for x in comms:
-        x.comm_destroy()
+    with contextlib.ExitStack() as comms:
+        for name, env in (("comm", {}), ("comm16", {"B2P_COMM_RESERVE_SMS": "16", "B2P_COMM_HEADSTART_US": "0"})):
+            x = _context(**off, **env)
+            try:
+                comms.enter_context(one_rank_comm(x))
+            except pytest.skip.Exception:  # NCCL cannot be loaded: the routes without a communicator still run
+                x.close()
+                continue
+            c[name] = x
+        for x in c.values():
+            x.use_own_stream()
+        yield c
     for x in c.values():
         x.close()
 

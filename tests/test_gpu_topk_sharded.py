@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from tests import select_keys as sk
+from tests.ranks import one_rank_comm
 
 pytestmark = pytest.mark.gpu
 
@@ -235,23 +236,13 @@ def test_composed_call_without_communicator_is_the_single_rank_topk():
 
 
 def test_single_rank_communicator_round_trips_the_candidates():
-    """comm_init(id, 1, 0), then the composed call over NCCL's all-reduce and all-gather: the words of b2p_topk_dev"""
-    from greptimedb_b200 import B2PError
+    """Over a one-rank communicator, the composed call over NCCL's all-reduce and all-gather: the words of b2p_topk_dev"""
     T = 70
     vals, ok, gid, n_groups, tie = grid(4, T)
     full = Rank(np.arange(gid.size), vals, sk.words(ok), gid, n_groups, tie)
     try:
-        try:
-            uid = full.ctx.comm_unique_id()
-        except B2PError as e:
-            if "libnccl" in str(e):
-                pytest.skip(f"NCCL cannot be loaded: {e}")
-            raise
-        full.ctx.comm_init(uid, 1, 0)
-        try:
+        with one_rank_comm(full.ctx):
             composed_check(full, vals, ok, gid, n_groups, tie, T)
-        finally:
-            full.ctx.comm_destroy()
     finally:
         full.close()
 

@@ -3,16 +3,12 @@ group_rows' table over its own rows, and the host mirror (distributed.agree_grou
 one broadcast per rank) gives both ranks the same table, equal to group_rows over the union, with each rank's groups
 mapped to their place in it.  Classes: hashed, uneven and empty shards; a group on one rank only; NULL against "";
 id-keyed children (ids as decimal strings); multi-byte UTF-8; `by` and `without`; __tsid carried."""
-import os
-import socket
-import sys
 import zlib
 
 import numpy as np
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests.ranks import spawn_gloo
+
 NAMES = ["host", "idc", "zone"]
 
 
@@ -36,11 +32,7 @@ def cases():
     return out
 
 
-def _worker(rank, world, port, q):
-    sys.path.insert(0, ROOT)
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _worker(rank, world):
     from greptimedb_b200 import distributed as D
     res = []
     for name, series, owner, cols in cases():
@@ -48,27 +40,13 @@ def _worker(rank, world, port, q):
         res.append((mine,) + D.agree_group_keys(mine, len(cols)))
         ids = [zlib.crc32(repr(t).encode()) for t in mine]  # one id per full tuple, whichever rank holds it
         res.append((mine,) + D.agree_group_keys(mine, len(cols), ids))
-    q.put((rank, res))
-    dist.barrier()
-    dist.destroy_process_group()
+    return res
 
 
 def test_agreement_equals_group_rows_over_the_union():
     from greptimedb_b200 import distributed as D
     world = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=600) for _ in range(world))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got = spawn_gloo(_worker, world, timeout=600)
     for i, (name, series, owner, cols) in enumerate(cases()):
         union = D.group_tuples([tuple(t[c] for c in cols) for t in series])
         for j in (2 * i, 2 * i + 1):

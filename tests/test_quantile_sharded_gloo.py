@@ -4,15 +4,11 @@ ranks' results equal select_keys.quantile over all rows, bit for bit.  The grids
 and the nibble-depth classes (s[lo] and s[hi] on different ranks), rows of no group and rows without a valid cell; the
 shards are hashed, uneven, and one is empty."""
 import math
-import os
-import socket
-import sys
 
 import numpy as np
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests.ranks import spawn_gloo
+
 PHIS = (math.nan, -0.5, 1.5, 0.0, 1.0, 0.5, 0.99)
 
 
@@ -37,38 +33,20 @@ def cases():
     return out
 
 
-def _worker(rank, world, port, q):
-    sys.path.insert(0, ROOT)
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _worker(rank, world):
     from greptimedb_b200 import distributed as D
     res = []
     for name, phi, vals, ok, gid, n_groups, owner in cases():
         mine = np.flatnonzero(owner == rank)
         res.append(D.merge_quantile_digits(phi, vals[mine], ok[mine], gid[mine], n_groups))
-    q.put((rank, res))
-    dist.barrier()
-    dist.destroy_process_group()
+    return res
 
 
 def test_sharded_quantile_equals_the_unsharded_select():
     from greptimedb_b200 import distributed as D
     from tests import select_keys as sk
     world = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=600) for _ in range(world))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got = spawn_gloo(_worker, world, timeout=600)
     all_cases = cases()
     assert len(all_cases) == 4 * len(PHIS)
     for i, (name, phi, vals, ok, gid, n_groups, owner) in enumerate(all_cases):

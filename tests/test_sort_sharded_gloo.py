@@ -5,15 +5,10 @@ whole grid bit for bit (select_keys.sort and sort_oracle.value_order for one Flo
 for several, signed order for Int64).  Classes: both directions; the total-order specials split across ranks; equal
 values on both ranks, whose order the row ids decide; hashed, uneven and empty shards; two and three fields with ties
 in field 0 across ranks; Int64 with INT64_MIN and INT64_MAX."""
-import os
-import socket
-import sys
-
 import numpy as np
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests.ranks import spawn_gloo
+
 I64_MIN, I64_MAX = np.iinfo(np.int64).min, np.iinfo(np.int64).max
 
 
@@ -71,11 +66,7 @@ def expected(desc, vals, ok):
     return order, [g.reshape(-1)[order.astype(np.int64)] for g in grids]
 
 
-def _worker(rank, world, port, q):
-    sys.path.insert(0, ROOT)
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _worker(rank, world):
     from greptimedb_b200 import distributed as D
     res = []
     for name, vals, ok, owner in cases():
@@ -83,26 +74,12 @@ def _worker(rank, world, port, q):
         local = [v[mine] for v in vals] if isinstance(vals, list) else vals[mine]
         for desc in (False, True):
             res.append(D.merge_sorted_runs(desc, local, ok[mine], mine.astype(np.uint32)))
-    q.put((rank, res))
-    dist.barrier()
-    dist.destroy_process_group()
+    return res
 
 
 def test_sharded_sort_equals_the_sort_of_the_union():
     world = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=600) for _ in range(world))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got = spawn_gloo(_worker, world, timeout=600)
     i = 0
     for name, vals, ok, owner in cases():
         F = len(vals) if isinstance(vals, list) else 1

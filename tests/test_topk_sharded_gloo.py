@@ -2,15 +2,10 @@
 of b2p_topk_allgather_dev (distributed.merge_topk_candidates) exchanges candidates, and the union of the ranks' kept
 cells equals select_keys.topk over all rows.  The grids hold adversarial total-order keys (NaN payloads of both signs,
 ±0, ±inf, sentinel and equal-key columns) with value ties across ranks; the shards are hashed, uneven, and empty."""
-import os
-import socket
-import sys
-
 import numpy as np
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests.ranks import spawn_gloo
+
 KKS = (0, 1, 2, 5, 32, 33, 70)
 
 
@@ -38,11 +33,7 @@ def cases():
     return out
 
 
-def _worker(rank, world, port, q):
-    sys.path.insert(0, ROOT)
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _worker(rank, world):
     from greptimedb_b200 import distributed as D
     res = {}
     for name, vals, ok, gid, n_groups, tie, owner, slots in cases():
@@ -53,27 +44,13 @@ def _worker(rank, world, port, q):
                 kept, X, rounds, K = D.merge_topk_candidates(bottom, kk, vals[mine], ok[mine], gid[mine], n_groups,
                                                              tie[mine], slots_max=slots)
                 res[(name, bottom, kk)] = (mine, kept, X, rounds, K)
-    q.put((rank, res))
-    dist.barrier()
-    dist.destroy_process_group()
+    return res
 
 
 def test_sharded_topk_union_equals_the_unsharded_selection():
     from tests import select_keys as sk
     world = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=300) for _ in range(world))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got = spawn_gloo(_worker, world, timeout=300)
     checked = 0
     for name, vals, ok, gid, n_groups, tie, owner, slots in cases():
         sizes = np.bincount(gid[gid < n_groups], minlength=n_groups)
