@@ -445,6 +445,41 @@ __global__ void __launch_bounds__(256) histogram_uniform_index_kernel(const doub
   if (blockIdx.x == 0 && threadIdx.x == 0) hist_off[n_hist] = (uint32_t)n;
 }
 
+// Row move of the sharded HistogramFold: out row dst[i] = in row src[i], T f64 values and Tw validity words per row (the
+// shuffle's pack and the placement of the gathered results).  One warp per row, lane-strided: each row is a run of
+// coalesced reads and writes.  kVec: T is even and both grids are 16-byte aligned, so every row starts on 16 bytes and
+// moves as double2.  HBM-bound: 2 x (8 T + 4 Tw) B per row.
+struct RowMoveArgs {
+  const double* in;
+  const uint32_t* in_valid;
+  const uint32_t* src;
+  const uint32_t* dst;
+  uint32_t n;
+  uint64_t T;
+  uint32_t Tw;
+  double* out;
+  uint32_t* out_valid;
+};
+
+template <bool kVec>
+__global__ void __launch_bounds__(256) row_move_kernel(const RowMoveArgs a) {
+  const uint32_t lane = threadIdx.x & 31;
+  for (uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < a.n;
+       i += ((uint64_t)gridDim.x * blockDim.x) >> 5) {
+    const uint64_t s = a.src[i], d = a.dst[i];
+    if (kVec) {
+      const double2* in = reinterpret_cast<const double2*>(a.in + s * a.T);
+      double2* out = reinterpret_cast<double2*>(a.out + d * a.T);
+      for (uint64_t k = lane; k < a.T / 2; k += 32) __stcs(out + k, __ldcs(in + k));
+    } else {
+      const double* in = a.in + s * a.T;
+      double* out = a.out + d * a.T;
+      for (uint64_t k = lane; k < a.T; k += 32) __stcs(out + k, __ldcs(in + k));
+    }
+    for (uint32_t k = lane; k < a.Tw; k += 32) a.out_valid[d * a.Tw + k] = a.in_valid[s * a.Tw + k];
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // K6.  Deterministic two-stage per-column reduction; NaN rows are skipped like SeriesNormalize's
 // filter.  Stage 1: grid (blocks_per_col, n_cols), each block reduces a contiguous slab with 128-bit

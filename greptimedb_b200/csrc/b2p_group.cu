@@ -1,6 +1,9 @@
 // b2p_group.cu — by-label entry points of the C ABI: the group index, by-label aggregates and their partials, the
 // all-reduce of partials over NCCL, HistogramFold / histogram_quantile and the column reduce.
+#include <algorithm>
+#include <cmath>
 #include <new>
+#include <numeric>
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -357,6 +360,76 @@ int b2p_histogram_quantile_dev(b2p_ctx* c, double phi, const double* le, uint32_
                                 rates, valid_words, T, out, out_valid_words);
 }
 
+}  // extern "C"
+
+namespace {
+// out row dst[i] = in row src[i] for i < n, values and validity words (row_move_kernel); device pointers
+int row_move(b2p_ctx* c, const double* in, const uint32_t* in_valid, const uint32_t* src, const uint32_t* dst, uint32_t n,
+             uint64_t T, double* out, uint32_t* out_valid) {
+  if (n == 0 || T == 0) return B2P_OK;
+  const RowMoveArgs a{in, in_valid, src, dst, n, T, (uint32_t)((T + 31) / 32), out, out_valid};
+  const unsigned blocks = capped_grid(c, (uint64_t)n * 32, 256, 8);
+  if (T % 2 == 0 && aligned16(in) && aligned16(out)) row_move_kernel<true><<<blocks, 256, 0, c->stream>>>(a);
+  else row_move_kernel<false><<<blocks, 256, 0, c->stream>>>(a);
+  c->launches++;
+  CU(cudaGetLastError());
+  return B2P_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_row_move_dev(b2p_ctx* c, const double* in, const uint32_t* in_valid, const uint32_t* src, const uint32_t* dst,
+                     uint32_t n, uint64_t T, double* out, uint32_t* out_valid) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  if (n == 0 || T == 0) return B2P_OK;
+  if (!in || !in_valid || !src || !dst || !out || !out_valid) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  return row_move(c, in, in_valid, src, dst, n, T, out, out_valid);
+}
+
+// A histogram's owner: the rank with the most of its buckets, the lowest on a tie (a function of the table alone).
+int b2p_histogram_shard_owners(const uint32_t* counts, int32_t n_ranks, uint32_t n_hist, uint32_t* owner) {
+  if (n_ranks < 1) return fail(B2P_E_INVALID, "n_ranks %d < 1", n_ranks);
+  if (n_hist && (!counts || !owner)) return fail(B2P_E_INVALID, "NULL argument");
+  for (uint32_t h = 0; h < n_hist; ++h) {
+    uint32_t best = 0;
+    for (uint32_t r = 1; r < (uint32_t)n_ranks; ++r)
+      if (counts[(size_t)r * n_hist + h] > counts[(size_t)best * n_hist + h]) best = r;
+    owner[h] = best;
+  }
+  return B2P_OK;
+}
+
+// The HistogramFold index over n buckets: histogram, then bound ascending with NaN last (-0.0 ties +0.0), then (rank,
+// row).  The keys are distinct wherever (rank, row) is, so the order is total and any sort gives it.  The plan layer's
+// unsharded index is this call with rank 0 and row = the row itself.
+int b2p_histogram_shard_index(const uint32_t* hist, const double* le, const uint32_t* rank, const uint32_t* row,
+                              uint32_t n, uint32_t n_hist, uint32_t* hist_off, uint32_t* bucket_series, double* bucket_le) {
+  if (!hist_off || (n && (!hist || !le || !rank || !row || !bucket_series || !bucket_le)))
+    return fail(B2P_E_INVALID, "NULL argument");
+  std::fill(hist_off, hist_off + (size_t)n_hist + 1, 0u);
+  for (uint32_t i = 0; i < n; ++i) {
+    if (hist[i] >= n_hist) return fail(B2P_E_INVALID, "hist[%u] = %u is not a histogram (n_hist = %u)", i, hist[i], n_hist);
+    hist_off[hist[i] + 1]++;
+  }
+  for (uint32_t h = 0; h < n_hist; ++h) hist_off[h + 1] += hist_off[h];
+  {  // the buckets by histogram (a counting sort), then each histogram's by (bound, rank, row)
+    std::vector<uint32_t> at(hist_off, hist_off + n_hist);
+    for (uint32_t i = 0; i < n; ++i) bucket_series[at[hist[i]]++] = i;
+  }
+  const auto less = [&](uint32_t x, uint32_t y) {
+    const bool nx = std::isnan(le[x]), ny = std::isnan(le[y]);
+    if (nx != ny) return ny;
+    if (!nx && le[x] != le[y]) return le[x] < le[y];
+    if (rank[x] != rank[y]) return rank[x] < rank[y];
+    return row[x] < row[y];
+  };
+  for (uint32_t h = 0; h < n_hist; ++h) std::sort(bucket_series + hist_off[h], bucket_series + hist_off[h + 1], less);
+  for (uint32_t j = 0; j < n; ++j) bucket_le[j] = le[bucket_series[j]];
+  return B2P_OK;
+}
+
 int b2p_column_reduce_dev(b2p_ctx* c, const double* const* cols, uint32_t n_cols, uint64_t n_rows, double* out_sum,
                           uint64_t* out_cnt) {
   if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
@@ -540,6 +613,332 @@ int b2p_range_histogram_fold(b2p_ctx* c, const b2p_range_params* p, const int64_
     return r ? r : b2p_histogram_fold_dev(c, phi, d_hist_off, d_bucket_series, d_bucket_le, n_hist, d_rates,
                                           d_rates_valid, (uint64_t)T, d_out, d_out_valid);
   });
+}
+
+}  // extern "C"
+
+namespace {
+// What travels with each shuffled bucket row of the sharded HistogramFold
+struct BucketHeader {
+  double le;
+  uint32_t hist, rank, row, pad;
+};
+static_assert(sizeof(BucketHeader) == 24, "the bucket header is 24 bytes on every rank");
+
+size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
+
+// The sharded HistogramFold's plan, from the counts table alone (so every rank derives the same one): owners, each
+// histogram's place among its owner's, the batches of contiguous histograms, this rank's largest batch send and
+// receive, and its rows by (histogram, row).
+struct HistShard {
+  uint32_t H = 0, R = 1, me = 0, Tw = 0, n_rows = 0;
+  uint64_t T = 0;
+  const double* row_le = nullptr;
+  std::vector<uint32_t> counts;          // [R x H]
+  std::vector<uint32_t> owner, pos;      // [H]
+  std::vector<uint64_t> own_n;           // [R] histograms each rank owns
+  std::vector<uint32_t> cut;             // batch b: histograms cut[b] .. cut[b + 1]
+  uint64_t send_max = 0, recv_max = 0, mine_off = 0;
+  std::vector<uint32_t> loff, lrows;     // this rank's rows of histogram h: lrows[loff[h] .. loff[h + 1]]
+  uint64_t cnt(uint32_t r, uint32_t h) const { return counts[(size_t)r * H + h]; }
+  uint64_t grid_rows() const { return (uint64_t)n_rows + recv_max; }  // the fold's grid: own rows, then a batch's received
+};
+
+// Step 1 to 3 of b2p_histogram_fold_allgather (collective: one all-gather).  The table carries one more column per rank,
+// set where that rank's row_hist names no histogram, so such a rank fails on every rank alike, after the collective.
+int hist_shard_plan(b2p_ctx* c, const uint32_t* row_hist, const double* row_le, uint32_t n_rows, uint32_t n_hist,
+                    uint64_t T, HistShard& sh) {
+  const uint32_t H = n_hist, R = (uint32_t)c->comm_ranks, me = (uint32_t)c->comm_rank;
+  sh.H = H; sh.R = R; sh.me = me; sh.T = T; sh.Tw = (uint32_t)((T + 31) / 32); sh.n_rows = n_rows;
+  sh.row_le = row_le;
+  std::vector<uint32_t> mine((size_t)H + 1, 0u);
+  for (uint32_t i = 0; i < n_rows; ++i) {
+    if (row_hist[i] >= H) mine[H] = 1;
+    else ++mine[row_hist[i]];
+  }
+  std::vector<uint32_t> table((size_t)R * (H + 1));
+  if (int rc = rank_table(c, (size_t)H + 1, Nccl::kUint32, table.data(), [&](void* slot) {
+        CU(cudaMemcpyAsync(slot, mine.data(), ((size_t)H + 1) * 4, cudaMemcpyHostToDevice, c->stream));
+        return B2P_OK;
+      }))
+    return rc;
+  sh.counts.resize((size_t)R * H);
+  uint64_t total = 0;
+  for (uint32_t r = 0; r < R; ++r) {
+    if (table[(size_t)r * (H + 1) + H])
+      return fail(B2P_E_INVALID, "histogram_quantile: rank %u passed a row_hist entry >= n_hist (%u)", r, H);
+    for (uint32_t h = 0; h < H; ++h) total += sh.counts[(size_t)r * H + h] = table[(size_t)r * (H + 1) + h];
+  }
+  if (total > UINT32_MAX) return fail(B2P_E_TOO_LARGE, "histogram_quantile: more than 2^32 - 1 bucket rows over the ranks");
+  // 2. owners, and each histogram's place among its owner's
+  sh.owner.resize(H);
+  sh.pos.resize(H);
+  sh.own_n.assign(R, 0);
+  b2p_histogram_shard_owners(sh.counts.data(), (int32_t)R, H, sh.owner.data());
+  for (uint32_t h = 0; h < H; ++h) sh.pos[h] = (uint32_t)sh.own_n[sh.owner[h]]++;
+  for (uint32_t r = 0; r < me; ++r) sh.mine_off += sh.own_n[r];
+  // 3. batches: a histogram joins the batch while every rank's sent and received rows of the batch fit the cap
+  const uint64_t row_bytes = T * 8 + (uint64_t)sh.Tw * 4 + sizeof(BucketHeader);
+  sh.cut.assign(1, 0u);
+  std::vector<uint64_t> load(R, 0);
+  uint64_t send_b = 0, recv_b = 0;  // this rank's rows of the current batch
+  for (uint32_t h = 0; h < H; ++h) {
+    const uint32_t o = sh.owner[h];
+    uint64_t moved = 0;
+    for (uint32_t r = 0; r < R; ++r) moved += r == o ? 0 : sh.cnt(r, h);
+    bool over = false;
+    for (uint32_t r = 0; r < R && h > sh.cut.back(); ++r)
+      over = over || (load[r] + (r == o ? moved : sh.cnt(r, h))) * row_bytes > c->topk_exchange_cap;
+    if (over) {
+      sh.cut.push_back(h);
+      std::fill(load.begin(), load.end(), 0);
+      send_b = recv_b = 0;
+    }
+    for (uint32_t r = 0; r < R; ++r) load[r] += r == o ? moved : sh.cnt(r, h);
+    if (o == me) recv_b += moved;
+    else send_b += sh.cnt(me, h);
+    sh.send_max = std::max(sh.send_max, send_b);
+    sh.recv_max = std::max(sh.recv_max, recv_b);
+  }
+  sh.cut.push_back(H);
+  // this rank's rows by (histogram, row)
+  sh.loff.assign((size_t)H + 1, 0u);
+  sh.lrows.resize(n_rows);
+  for (uint32_t i = 0; i < n_rows; ++i) ++sh.loff[row_hist[i] + 1];
+  std::partial_sum(sh.loff.begin(), sh.loff.end(), sh.loff.begin());
+  std::vector<uint32_t> at(sh.loff.begin(), sh.loff.end() - 1);
+  for (uint32_t i = 0; i < n_rows; ++i) sh.lrows[at[row_hist[i]]++] = i;
+  return B2P_OK;
+}
+
+// Steps 4 to 7 over this rank's rows in g_val / g_valid (sh.grid_rows() rows of room): the shuffle, the owners' folds
+// into a_val / a_valid [H] (every owner's results, rank by rank), their gather and placement into out / out_valid.
+// Where no histogram is split across ranks no row is packed or sent and no point-to-point group is opened: each rank
+// folds its own histograms over its own rows, and only the results travel.
+int hist_shard_run(b2p_ctx* c, const HistShard& sh, double phi, double* g_val, uint32_t* g_valid, double* a_val,
+                   uint32_t* a_valid, double* d_out, uint32_t* d_out_valid) {
+  int rc;
+  const uint32_t H = sh.H, R = sh.R, me = sh.me, Tw = sh.Tw, n_rows = sh.n_rows;
+  const uint64_t T = sh.T, G = sh.grid_rows(), send_max = sh.send_max, recv_max = sh.recv_max, mine_off = sh.mine_off;
+  const uint64_t row_bytes = T * 8 + (uint64_t)Tw * 4 + sizeof(BucketHeader);
+  const std::vector<uint32_t>&owner = sh.owner, &pos = sh.pos, &cut = sh.cut, &loff = sh.loff, &lrows = sh.lrows;
+  const std::vector<uint64_t>& own_n = sh.own_n;
+  const double* row_le = sh.row_le;
+  auto cnt = [&](uint32_t r, uint32_t h) { return sh.cnt(r, h); };
+  const size_t sv = align16(send_max * T * 8), sw = align16(send_max * Tw * 4);
+  const size_t tab = std::max<size_t>(align16(((size_t)H + 1) * 4) + align16(G * 4) + G * 8, 2 * align16((size_t)std::max<uint64_t>(send_max, H) * 4));
+  if ((rc = c->x_send.ensure(sv + sw + send_max * sizeof(BucketHeader))) || (rc = c->x_recv.ensure(recv_max * sizeof(BucketHeader))) ||
+      (rc = c->x_table.ensure(tab)))
+    return rc;
+  char* xs = c->x_send.as<char>();
+  double* s_val = reinterpret_cast<double*>(xs);
+  uint32_t* s_valid = reinterpret_cast<uint32_t*>(xs + sv);
+  char* s_hdr = xs + sv + sw;
+  char* r_hdr = c->x_recv.as<char>();
+  uint32_t* t_u32 = c->x_table.as<uint32_t>();
+  // the two u32 columns of a move (src, dst), uploaded and moved
+  auto move = [&](const std::vector<uint32_t>& src, const std::vector<uint32_t>& dst, const double* in,
+                  const uint32_t* in_valid, double* o_val, uint32_t* o_valid) {
+    const size_t n = src.size(), half = align16(n * 4) / 4;
+    if (n == 0) return B2P_OK;
+    CU(cudaMemcpyAsync(t_u32, src.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(t_u32 + half, dst.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
+    return row_move(c, in, in_valid, t_u32, t_u32 + half, (uint32_t)n, T, o_val, o_valid);
+  };
+  uint64_t sent = 0;
+  for (size_t b = 0; b + 1 < cut.size(); ++b) {
+    const uint32_t h0 = cut[b], h1 = cut[b + 1];
+    // 4. this rank's rows of histograms it does not own, grouped by owner, in (histogram, row) order
+    std::vector<uint64_t> send_n(R, 0), recv_n(R, 0);
+    std::vector<uint32_t> src, dst;
+    std::vector<BucketHeader> hdr;
+    for (uint32_t q = 0; q < R; ++q)
+      for (uint32_t h = h0; h < h1; ++h) {
+        if (owner[h] != q) continue;
+        if (q == me) {
+          for (uint32_t r = 0; r < R; ++r) recv_n[r] += r == me ? 0 : cnt(r, h);
+          continue;
+        }
+        send_n[q] += cnt(me, h);
+        for (uint32_t j = loff[h]; j < loff[h + 1]; ++j) {
+          src.push_back(lrows[j]);
+          hdr.push_back(BucketHeader{row_le[lrows[j]], h, me, lrows[j], 0u});
+        }
+      }
+    dst.resize(src.size());
+    std::iota(dst.begin(), dst.end(), 0u);
+    if (!hdr.empty()) CU(cudaMemcpyAsync(s_hdr, hdr.data(), hdr.size() * sizeof(BucketHeader), cudaMemcpyHostToDevice, c->stream));
+    if ((rc = move(src, dst, g_val, g_valid, s_val, s_valid))) return rc;
+    sent += src.size();
+    uint64_t n_recv = 0;
+    for (uint32_t r = 0; r < R; ++r) n_recv += recv_n[r];
+    // 5. the shuffle: one group of point-to-point calls, rows into the grid after this rank's own
+    if (c->comm && (n_recv || !src.empty()) && (rc = nccl_group([&] {
+          uint64_t so = 0, ro = 0;
+          for (uint32_t q = 0; q < R; ++q) {
+            if (send_n[q]) {
+              NCCL_TRY(g_nccl.Send(s_val + so * T, send_n[q] * T, Nccl::kFloat64, (int)q, c->comm, c->stream));
+              NCCL_TRY(g_nccl.Send(s_valid + so * Tw, send_n[q] * Tw, Nccl::kUint32, (int)q, c->comm, c->stream));
+              NCCL_TRY(g_nccl.Send(s_hdr + so * sizeof(BucketHeader), send_n[q] * sizeof(BucketHeader), Nccl::kUint8,
+                                   (int)q, c->comm, c->stream));
+            }
+            if (recv_n[q]) {
+              const uint64_t at = n_rows + ro;
+              NCCL_TRY(g_nccl.Recv(g_val + at * T, recv_n[q] * T, Nccl::kFloat64, (int)q, c->comm, c->stream));
+              NCCL_TRY(g_nccl.Recv(g_valid + at * Tw, recv_n[q] * Tw, Nccl::kUint32, (int)q, c->comm, c->stream));
+              NCCL_TRY(g_nccl.Recv(r_hdr + ro * sizeof(BucketHeader), recv_n[q] * sizeof(BucketHeader), Nccl::kUint8,
+                                   (int)q, c->comm, c->stream));
+            }
+            so += send_n[q];
+            ro += recv_n[q];
+          }
+          return B2P_OK;
+        })))
+      return rc;
+    // 6. the owner's index over [its rows | the received rows] and K5 into its results
+    uint32_t p0 = UINT32_MAX, nh = 0;
+    for (uint32_t h = h0; h < h1; ++h)
+      if (owner[h] == me) {
+        if (p0 == UINT32_MAX) p0 = pos[h];
+        ++nh;
+      }
+    if (nh == 0) continue;
+    std::vector<BucketHeader> rh(n_recv);
+    if (n_recv) {
+      CU(cudaMemcpyAsync(rh.data(), r_hdr, n_recv * sizeof(BucketHeader), cudaMemcpyDeviceToHost, c->stream));
+      CU(cudaStreamSynchronize(c->stream));
+    }
+    std::vector<uint32_t> ih, irank, irow, buf_row;
+    std::vector<double> ile;
+    auto entry = [&](uint32_t h, double le, uint32_t r, uint32_t row, uint32_t at) {
+      ih.push_back(pos[h] - p0);
+      ile.push_back(le);
+      irank.push_back(r);
+      irow.push_back(row);
+      buf_row.push_back(at);
+    };
+    for (uint32_t h = h0; h < h1; ++h)
+      if (owner[h] == me)
+        for (uint32_t j = loff[h]; j < loff[h + 1]; ++j) entry(h, row_le[lrows[j]], me, lrows[j], lrows[j]);
+    for (uint64_t i = 0; i < n_recv; ++i) {
+      const BucketHeader& x = rh[i];
+      if (x.hist < h0 || x.hist >= h1 || owner[x.hist] != me)
+        return fail(B2P_E_INVALID, "histogram_quantile: received a bucket of histogram %u, not one of this rank's", x.hist);
+      entry(x.hist, x.le, x.rank, x.row, (uint32_t)(n_rows + i));
+    }
+    const uint32_t ne = (uint32_t)ih.size();
+    std::vector<uint32_t> hoff(nh + 1), bs(ne);
+    std::vector<double> ble(ne);
+    if ((rc = b2p_histogram_shard_index(ih.data(), ile.data(), irank.data(), irow.data(), ne, nh, hoff.data(), bs.data(),
+                                        ble.data())))
+      return rc;
+    for (uint32_t& x : bs) x = buf_row[x];
+    uint32_t* d_hoff = t_u32;
+    uint32_t* d_bs = t_u32 + align16((size_t)(nh + 1) * 4) / 4;
+    double* d_ble = reinterpret_cast<double*>(reinterpret_cast<char*>(d_bs) + align16((size_t)ne * 4));
+    CU(cudaMemcpyAsync(d_hoff, hoff.data(), (size_t)(nh + 1) * 4, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(d_bs, bs.data(), (size_t)ne * 4, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(d_ble, ble.data(), (size_t)ne * 8, cudaMemcpyHostToDevice, c->stream));
+    if ((rc = b2p_histogram_fold_dev(c, phi, d_hoff, d_bs, d_ble, nh, g_val, g_valid, T, a_val + (mine_off + p0) * T,
+                                     a_valid + (mine_off + p0) * Tw)))
+      return rc;
+  }
+  // 7. every owner's results to every rank, then placed in global order
+  if ((rc = gather_blocks(c, a_val, own_n.data(), T * 8, Nccl::kFloat64)) ||
+      (rc = gather_blocks(c, a_valid, own_n.data(), (size_t)Tw * 4, Nccl::kUint32)))
+    return rc;
+  c->last_exchange_bytes = (long long)(sent * row_bytes + own_n[me] * (T * 8 + (uint64_t)Tw * 4));
+  std::vector<uint32_t> src(H), dst;
+  std::iota(src.begin(), src.end(), 0u);
+  for (uint32_t r = 0; r < R; ++r)
+    for (uint32_t h = 0; h < H; ++h)
+      if (owner[h] == r) dst.push_back(h);
+  return move(src, dst, a_val, a_valid, d_out, d_out_valid);
+}
+
+int hist_shard_check(b2p_ctx* c, uint32_t n_rows, uint64_t T, const uint32_t* row_hist, const double* row_le,
+                     uint32_t n_hist, double* out, uint32_t* out_valid_words) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  c->last_exchange_bytes = 0;
+  if (n_hist == 0 || T == 0) return B2P_OK;
+  if ((n_rows && (!row_hist || !row_le)) || !out || !out_valid_words) return fail(B2P_E_INVALID, "NULL argument");
+  return B2P_OK;
+}
+
+// b2p_histogram_fold_allgather: this rank's host grid staged into the fold's grid, then the plan and the run
+int histogram_fold_allgather_host(b2p_ctx* c, double phi, const double* rates, const uint32_t* valid_words,
+                                  uint32_t n_rows, uint64_t T, const uint32_t* row_hist, const double* row_le,
+                                  uint32_t n_hist, double* out, uint32_t* out_valid_words) {
+  if (int rc = hist_shard_check(c, n_rows, T, row_hist, row_le, n_hist, out, out_valid_words)) return rc;
+  if (n_hist == 0 || T == 0) return B2P_OK;  // (every rank has the same n_hist and T)
+  if (n_rows && (!rates || !valid_words)) return fail(B2P_E_INVALID, "NULL argument");
+  DeviceGuard g(c->device);
+  HistShard sh;
+  if (int rc = hist_shard_plan(c, row_hist, row_le, n_rows, n_hist, T, sh)) return rc;
+  const uint64_t G = sh.grid_rows(), Tw = sh.Tw;
+  Staging s{c};
+  double* g_val = static_cast<double*>(s.buf(G * T * 8));
+  uint32_t* g_valid = static_cast<uint32_t*>(s.buf(G * Tw * 4));
+  if (n_rows && g_val && g_valid) {
+    s.cuda(cudaMemcpyAsync(g_val, rates, (size_t)n_rows * T * 8, cudaMemcpyHostToDevice, c->stream), "host-to-device copy");
+    s.cuda(cudaMemcpyAsync(g_valid, valid_words, (size_t)n_rows * Tw * 4, cudaMemcpyHostToDevice, c->stream),
+           "host-to-device copy");
+  }
+  double* a_val = static_cast<double*>(s.buf((size_t)n_hist * T * 8));
+  uint32_t* a_valid = static_cast<uint32_t*>(s.buf((size_t)n_hist * Tw * 4));
+  double* d_out = s.out(out, (size_t)n_hist * T * 8);
+  uint32_t* d_out_valid = s.out(out_valid_words, (size_t)n_hist * Tw * 4);
+  return s.end([&] { return hist_shard_run(c, sh, phi, g_val, g_valid, a_val, a_valid, d_out, d_out_valid); });
+}
+
+// b2p_range_histogram_fold_allgather: the range function writes this rank's series straight into the fold's grid, so
+// the dense matrix never leaves the device, whether or not any histogram is split
+int range_histogram_fold_allgather_host(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
+                                        const uint32_t* sid, const uint64_t* offsets_host, uint64_t n_samples,
+                                        uint32_t n_series, double phi, const uint32_t* row_hist, const double* row_le,
+                                        uint32_t n_hist, double* out, uint32_t* out_valid_words) {
+  if (!c) return fail(B2P_E_INVALID, "ctx is NULL");
+  int64_t T = 0;
+  if (int rc = check_grid(p, n_series, &T)) return rc;
+  if (int rc = hist_shard_check(c, n_series, (uint64_t)T, row_hist, row_le, n_hist, out, out_valid_words)) return rc;
+  if (n_hist == 0 || T == 0) return B2P_OK;  // (every rank has the same n_hist and T)
+  DeviceGuard g(c->device);
+  int rc;
+  if (!c->pending.empty() && (rc = b2p_sync(c))) return rc;
+  HistShard sh;
+  if ((rc = hist_shard_plan(c, row_hist, row_le, n_series, n_hist, (uint64_t)T, sh))) return rc;
+  const uint64_t G = sh.grid_rows(), Tw = sh.Tw;
+  Staging s{c};
+  const SeriesIn in = n_series ? stage_series(s, ts, val, sid, 0u, offsets_host, n_samples, n_series) : SeriesIn{};
+  double* g_val = static_cast<double*>(s.buf(G * (uint64_t)T * 8));
+  uint32_t* g_valid = static_cast<uint32_t*>(s.buf(G * Tw * 4));
+  double* a_val = static_cast<double*>(s.buf((size_t)n_hist * (size_t)T * 8));
+  uint32_t* a_valid = static_cast<uint32_t*>(s.buf((size_t)n_hist * Tw * 4));
+  double* d_out = s.out(out, (size_t)n_hist * (size_t)T * 8);
+  uint32_t* d_out_valid = s.out(out_valid_words, (size_t)n_hist * Tw * 4);
+  return s.end([&] {
+    int r = n_series ? b2p_range_eval_dev(c, p, in.ts, in.val, in.offsets, n_samples, n_series, g_val, g_valid) : B2P_OK;
+    if (!r && n_series) r = b2p_sync(c);  // slow-path fix-ups land before the fold reads
+    return r ? r : hist_shard_run(c, sh, phi, g_val, g_valid, a_val, a_valid, d_out, d_out_valid);
+  });
+}
+}  // namespace
+
+extern "C" {
+
+int b2p_histogram_fold_allgather(b2p_ctx* c, double phi, const double* rates, const uint32_t* valid_words,
+                                 uint32_t n_rows, uint64_t T, const uint32_t* row_hist, const double* row_le,
+                                 uint32_t n_hist, double* out, uint32_t* out_valid_words) {
+  return histogram_fold_allgather_host(c, phi, rates, valid_words, n_rows, T, row_hist, row_le, n_hist, out,
+                                       out_valid_words);
+}
+
+int b2p_range_histogram_fold_allgather(b2p_ctx* c, const b2p_range_params* p, const int64_t* ts, const double* val,
+                                       const uint32_t* sid, const uint64_t* offsets_host, uint64_t n_samples,
+                                       uint32_t n_series, double phi, const uint32_t* row_hist, const double* row_le,
+                                       uint32_t n_hist, double* out, uint32_t* out_valid_words) {
+  return range_histogram_fold_allgather_host(c, p, ts, val, sid, offsets_host, n_samples, n_series, phi, row_hist,
+                                             row_le, n_hist, out, out_valid_words);
 }
 
 }  // extern "C"

@@ -597,44 +597,69 @@ void aggregate_rows(b2p_ctx* ctx, int op, double param, const std::vector<int>& 
 
 // The HistogramFold index over `rows` rows labelled `in` (histogram_fold.rs:754-820): rows that agree on every tag but
 // column `le` form one histogram, histograms in label order; each histogram's buckets in ascending le order (parsed as
-// le.parse::<f64>().unwrap_or(NaN), :791-796, NULL as NaN), NaN bounds last, ties in row order.  The CSR
-// hist_off / bucket_series / bucket_le is what b2p_histogram_fold[_dev] and b2p_range_histogram_fold take.
+// le.parse::<f64>().unwrap_or(NaN), :791-796, NULL as NaN), NaN bounds last, ties in row order: the order of
+// b2p_histogram_shard_index, which the sharded fold uses too.  The CSR hist_off / bucket_series / bucket_le is what
+// b2p_histogram_fold[_dev] and b2p_range_histogram_fold take.
 struct HistogramIndex {
   Groups hist;  // the histograms; hist.labels are their tags without le
   std::vector<uint32_t> hist_off, bucket_series;
   std::vector<double> bucket_le;
 };
 
-HistogramIndex histogram_index(const Labels& in, int le, uint32_t rows) {
-  HistogramIndex ix;
-  std::vector<int> cols;  // the tags without le
+// the histograms of `rows` rows labelled `in`: the rows grouped by their tags without column `le`
+Groups histogram_groups(const Labels& in, int le, uint32_t rows) {
+  std::vector<int> cols;
   for (int t = 0; t < (int)in.names.size(); ++t)
     if (t != le) cols.push_back(t);
-  ix.hist = group_rows(in, cols, rows);
-  const uint32_t H = (uint32_t)ix.hist.rank.size();
+  return group_rows(in, cols, rows);
+}
+
+// each row's parsed bound
+std::vector<double> bucket_bounds(const Labels& in, int le, uint32_t rows) {
   std::vector<double> sle(rows);
   for (uint32_t s = 0; s < rows; ++s) {
     const Label& v = in.values[(size_t)le][s];
     sle[s] = v ? parse_f64_like_rust(*v) : std::nan("");
   }
-  // a strict weak ordering: histogram, then le ascending with NaN last; stable_sort keeps ties in row order
-  auto place = [&](uint32_t s) { return ix.hist.rank[ix.hist.id[s]]; };
+  return sle;
+}
+
+HistogramIndex histogram_index(const Labels& in, int le, uint32_t rows) {
+  HistogramIndex ix;
+  ix.hist = histogram_groups(in, le, rows);
+  const uint32_t H = (uint32_t)ix.hist.rank.size();
+  const std::vector<double> sle = bucket_bounds(in, le, rows);
+  std::vector<uint32_t> place(rows), rank(rows, 0u), row(rows);
+  std::iota(row.begin(), row.end(), 0u);
+  for (uint32_t s = 0; s < rows; ++s) place[s] = ix.hist.rank[ix.hist.id[s]];
+  ix.hist_off.resize((size_t)H + 1);
   ix.bucket_series.resize(rows);
-  std::iota(ix.bucket_series.begin(), ix.bucket_series.end(), 0u);
-  std::stable_sort(ix.bucket_series.begin(), ix.bucket_series.end(), [&](uint32_t x, uint32_t y) {
-    if (place(x) != place(y)) return place(x) < place(y);
-    const bool nx = std::isnan(sle[x]), ny = std::isnan(sle[y]);
-    if (nx != ny) return ny;
-    return !nx && sle[x] < sle[y];
-  });
-  ix.hist_off.assign((size_t)H + 1, 0u);
   ix.bucket_le.resize(rows);
-  for (uint32_t i = 0; i < rows; ++i) {
-    ix.bucket_le[i] = sle[ix.bucket_series[i]];
-    ix.hist_off[place(ix.bucket_series[i]) + 1]++;
-  }
-  for (uint32_t h = 0; h < H; ++h) ix.hist_off[h + 1] += ix.hist_off[h];
+  check(b2p_histogram_shard_index(place.data(), sle.data(), rank.data(), row.data(), rows, H, ix.hist_off.data(),
+                                  ix.bucket_series.data(), ix.bucket_le.data()));
   return ix;
+}
+
+// histogram_quantile over r's rows sharded across ranks: the histograms are agreed (agree_groups, which also gives r
+// the field types of the ranks with rows), refuse(r, n_hist) raises what the node refuses on those agreed types on every
+// rank alike, then fold(row_hist, row_le, n_hist, out, out_valid) folds each histogram on one rank and replicates the
+// result (a b2p_*histogram_fold_allgather call; not made when there is no histogram or step, the same on every rank).
+// r becomes the [n_hist x T] rows in label order, the same on every rank.
+template <class Refuse, class Fold>
+void fold_sharded(b2p_ctx* ctx, int le, NodeResult& r, Refuse&& refuse, Fold&& fold) {
+  Groups hist = histogram_groups(r.labels, le, r.rows);
+  Agreement a = agree_groups(ctx, hist, r);
+  refuse(r, a.n_groups);
+  take_global(hist, a);
+  const uint32_t H = (uint32_t)hist.rank.size();
+  const std::vector<double> sle = bucket_bounds(r.labels, le, r.rows);
+  std::vector<double> out((size_t)H * (size_t)r.T, 0.0);
+  std::vector<uint32_t> out_valid((size_t)H * r.Tw, 0u);
+  if (H > 0 && r.T > 0) check(fold(hist.id.data(), sle.data(), H, out.data(), out_valid.data()), ErrorKind::Execution);
+  r.val = std::move(out);
+  r.valid = std::move(out_valid);
+  r.labels = std::move(hist.labels);
+  r.rows = H;
 }
 
 }  // namespace
@@ -916,6 +941,7 @@ void PromRangePlan::compute(NodeResult& r) {
   offsets_.push_back((uint64_t)ts_.size());
   // timestamp(): one Float64 value whatever the fields, DEFAULT_FIELD_COLUMN (planner.rs:951-965); no value is read
   const uint32_t F = timestamp_ ? 1u : (uint32_t)args_.field_columns.size();
+  const bool sharded = sharded_ && sharded_run("GpuPromRangeExec");
   const bool fold_on_device = args_.histogram && fn_id_ >= 0;  // the dense matrix then never reaches the host
   const size_t cells = (size_t)S * (size_t)T;
   std::vector<double> dense(fold_on_device ? 0 : F * cells);
@@ -963,6 +989,22 @@ void PromRangePlan::compute(NodeResult& r) {
     // HistogramFold (histogram_fold.rs:754-820): group the series by their tags without `le`, order each group's
     // buckets by le ascending (parsed as f64, "+Inf" last), one output row per (group, eval ts)
     if (series_.id_keyed) throw PlanError(ErrorKind::Plan, "HistogramFold needs the le tag column, not a tsid key");
+    if (sharded) {
+      // b2p_range_histogram_fold_allgather: the range function writes into the sharded fold's grid on the device
+      r.labels = series_;
+      r.rows = S;
+      const auto refuse = [&](const NodeResult&, uint32_t H) {
+        if (H > 0 && T > 0 && fn_id_ < 0)
+          throw PlanError(ErrorKind::Plan, "HistogramFold over an instant selector is not supported by this node");
+      };
+      fold_sharded(ctx_, series_.column(args_.le_column), r, refuse,
+                   [&](const uint32_t* row_hist, const double* row_le, uint32_t H, double* out, uint32_t* out_valid) {
+                     return b2p_range_histogram_fold_allgather(ctx_, &p, ts_.data(), val_[0].data(), nullptr,
+                                                               offsets_.data(), ts_.size(), S, args_.quantile,
+                                                               row_hist, row_le, H, out, out_valid);
+                   });
+      return;
+    }
     HistogramIndex ix = histogram_index(series_, series_.column(args_.le_column), S);
     const uint32_t H = (uint32_t)ix.hist.rank.size();
     r.val.assign((size_t)H * (size_t)T, 0.0);
@@ -987,7 +1029,7 @@ void PromRangePlan::compute(NodeResult& r) {
     if (agg_id_ >= 0) {
       // prom_aggr_expr_to_plan: group keys = by-labels + eval ts; output sorted by (labels asc, ts asc).  Over an id key
       // the by-label is the id's decimal string, so those rows sort as strings ("10" before "9").
-      aggregate_rows(ctx_, agg_id_, 0.0, series_.columns(args_.by_columns), r, sharded_ && sharded_run("GpuPromRangeExec"));
+      aggregate_rows(ctx_, agg_id_, 0.0, series_.columns(args_.by_columns), r, sharded);
       r.value_names = {args_.aggregate + "(" + (fn_id_ >= 0 ? args_.function : args_.field_columns[0]) + ")"};
     }
   }
@@ -2000,13 +2042,17 @@ HistogramQuantilePlan::HistogramQuantilePlan(b2p_ctx* ctx, std::string le_column
 }
 
 void HistogramQuantilePlan::compute(NodeResult& r) {
+  const bool sharded = sharded_ && sharded_run("GpuPromHistogramFoldExec");
   child_->run(r);
   // the reference folds the first field only (planner.rs:3084-3092, a FIXME); this node does not copy that
-  check_child(r, {{Shape::Int32, "GpuPromHistogramFoldExec: an Int32 value column is not supported by this node"},
+  const std::string int32 = "GpuPromHistogramFoldExec: an Int32 value column is not supported by this node";
+  const std::string int64 = "GpuPromHistogramFoldExec: an Int64 value column is not supported by this node";
+  // sharded, the value types a rank read from its batches are known only after the agreement (fold_sharded)
+  check_child(r, {{Shape::Int32, sharded ? "" : int32},
                   {Shape::IdKeyed, "GpuPromHistogramFoldExec: an id-keyed (__tsid) child carries no " + le_column_ + " label"},
                   {Shape::Counted, "GpuPromHistogramFoldExec: a count_values child is not supported by this node"},
                   {Shape::MultiField, "GpuPromHistogramFoldExec: a multi-field child is not supported by this node"},
-                  {Shape::Int64, "GpuPromHistogramFoldExec: an Int64 value column is not supported by this node"}});
+                  {Shape::Int64, sharded ? "" : int64}});
   r.cell_order.clear();
   r.counted.reset();  // (the folded rows are new rows)
   const int le = r.labels.column(le_column_);
@@ -2016,6 +2062,15 @@ void HistogramQuantilePlan::compute(NodeResult& r) {
     r.valid.clear();
     r.labels = Labels();
     r.columns = Columns::None;
+    return;
+  }
+  if (sharded) {
+    fold_sharded(
+        ctx_, le, r, [&](const NodeResult& c, uint32_t) { check_child(c, {{Shape::Int32, int32}, {Shape::Int64, int64}}); },
+        [&](const uint32_t* row_hist, const double* row_le, uint32_t H, double* out, uint32_t* out_valid) {
+          return b2p_histogram_fold_allgather(ctx_, phi_, r.val.data(), r.valid.data(), r.rows, (uint64_t)r.T, row_hist,
+                                              row_le, H, out, out_valid);
+        });
     return;
   }
   HistogramIndex ix = histogram_index(r.labels, le, r.rows);
@@ -2589,8 +2644,9 @@ int b2p_plan_set_sharded(b2p_plan* plan) {
   if (!plan) return B2P_E_INVALID;
   return guarded([&] {
     if (!plan->node->set_sharded())
-      throw b2p::PlanError(b2p::ErrorKind::Plan, "b2p_plan_set_sharded: only an aggregate node, a count_values node "
-                                                 "or a range / instant leaf with an aggregate stage has a sharded form");
+      throw b2p::PlanError(b2p::ErrorKind::Plan, "b2p_plan_set_sharded: only an aggregate node, a count_values node, "
+                                                 "a histogram_quantile node or a range / instant leaf with an aggregate "
+                                                 "or HistogramFold stage has a sharded form");
   });
 }
 

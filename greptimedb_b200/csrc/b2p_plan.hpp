@@ -266,7 +266,7 @@ class PromRangePlan : public PlanNode {
   uint64_t last_id_ = 0;
   bool have_last_ = false;
   void check_key_columns() const;  // by-columns and the le column name a tag or label column
-  bool set_sharded() override { return agg_id_ >= 0 && (sharded_ = true); }
+  bool set_sharded() override { return (agg_id_ >= 0 || args_.histogram) && (sharded_ = true); }
   const char* cross_row() const override {
     return agg_id_ >= 0 ? "an aggregate stage" : args_.histogram ? "histogram_quantile" : nullptr;
   }
@@ -435,10 +435,14 @@ class SubqueryPlan : public PlanNode {
 // the child's value name, and the export the child's column layout (a topk child's cell_order is dropped).  A child
 // without the le tag gives no rows and an export without columns (the reference's EmptyRelation).  Plan errors at
 // execute: an id-keyed child (this layer's __tsid form has no le label) and a count_values child (its counted value
-// would be a Float64 tag of the fold in the reference, which is not modelled here).
+// would be a Float64 tag of the fold in the reference, which is not modelled here).  Sharded (b2p_plan_set_sharded, over
+// a communicator): the histograms are agreed across ranks and b2p_histogram_fold_allgather folds each on one rank; the
+// result is the unsharded node's over every rank's child rows in rank order, the same bytes on every rank.  The Int32 /
+// Int64 refusals are then decided on the agreed value types, on every rank alike.
 class HistogramQuantilePlan : public PlanNode {
  public:
   HistogramQuantilePlan(b2p_ctx* ctx, std::string le_column, double phi, std::shared_ptr<PlanNode> child);
+  bool set_sharded() override { return sharded_ = true; }
 
  protected:
   void compute(NodeResult& r) override;
@@ -447,6 +451,7 @@ class HistogramQuantilePlan : public PlanNode {
   std::string le_column_;
   double phi_;
   std::shared_ptr<PlanNode> child_;
+  std::vector<const PlanNode*> children() const override { return {child_.get()}; }
   const char* cross_row() const override { return "histogram_quantile"; }
 };
 

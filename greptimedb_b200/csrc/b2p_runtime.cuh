@@ -39,7 +39,8 @@ int k0_fail(uint32_t k0);
 // process that already loaded an NCCL (e.g. the one bundled with torch) dlopen hands back that same library.
 // Only the entry points the by-label all-reduce and the sharded operators need, called through nccl_group (every
 // group), allreduce_with_counts (partials and their counts), rank_table (a per-rank table) and gather_blocks
-// (variable-size blocks); enum values are NCCL's ABI (nccl.h).
+// (variable-size blocks); Send / Recv are the sharded HistogramFold's point-to-point shuffle.  Enum values are NCCL's
+// ABI (nccl.h).
 struct Nccl {
   typedef struct ncclComm* comm_t;
   struct unique_id { char internal[128]; };
@@ -52,6 +53,8 @@ struct Nccl {
   int (*AllReduce)(const void*, void*, size_t, int, int, comm_t, cudaStream_t) = nullptr;
   int (*AllGather)(const void*, void*, size_t, int, comm_t, cudaStream_t) = nullptr;
   int (*Broadcast)(const void*, void*, size_t, int, int, comm_t, cudaStream_t) = nullptr;
+  int (*Send)(const void*, size_t, int, int, comm_t, cudaStream_t) = nullptr;
+  int (*Recv)(void*, size_t, int, int, comm_t, cudaStream_t) = nullptr;
   int (*GroupStart)() = nullptr;
   int (*GroupEnd)() = nullptr;
   const char* (*GetErrorString)(int) = nullptr;
@@ -73,6 +76,8 @@ struct Nccl {
     AllReduce = reinterpret_cast<decltype(AllReduce)>(sym("ncclAllReduce"));
     AllGather = reinterpret_cast<decltype(AllGather)>(sym("ncclAllGather"));
     Broadcast = reinterpret_cast<decltype(Broadcast)>(sym("ncclBroadcast"));
+    Send = reinterpret_cast<decltype(Send)>(sym("ncclSend"));
+    Recv = reinterpret_cast<decltype(Recv)>(sym("ncclRecv"));
     GroupStart = reinterpret_cast<decltype(GroupStart)>(sym("ncclGroupStart"));
     GroupEnd = reinterpret_cast<decltype(GroupEnd)>(sym("ncclGroupEnd"));
     GetErrorString = reinterpret_cast<decltype(GetErrorString)>(sym("ncclGetErrorString"));

@@ -594,3 +594,112 @@ def agree_group_keys(tuples, n_labels: int, ids=None, group=None):
         blocks.append(buf.numpy().tobytes())
     table, table_ids, l2g, _, _ = merge_group_keys(blocks, me)
     return table, table_ids, l2g, len(mine)
+
+
+HIST_HEADER_BYTES = 24  # (bound f64, histogram u32, rank u32, row u32, pad u32) with each shuffled bucket row
+
+
+def histogram_owners(counts):
+    """The owner of each histogram from the counts table [n_ranks, n_hist]: the rank with the most of its buckets, the
+    lowest on a tie (b2p_histogram_shard_owners)"""
+    counts = np.asarray(counts)
+    return np.argmax(counts, axis=0).astype(np.int64) if counts.size else np.zeros(counts.shape[1], np.int64)
+
+
+def _fold_cells(phi, bounds, counters):
+    """K5 over one (histogram, step): the present buckets' bounds (ascending, NaN last) and counters -> its value
+    (None: no bucket present)"""
+    import math
+    n = len(bounds)
+    if n == 0:
+        return None
+    if n < 2 or not (math.isinf(bounds[-1]) and bounds[-1] > 0):
+        return math.nan
+    cnt, prev = [], 0.0
+    for i, v in enumerate(counters):  # non-finite -> previous, decreasing -> previous (histogram_fold.rs:1074-1092)
+        c = v if math.isfinite(v) else prev
+        if i > 0 and c < prev:
+            c = prev
+        prev = c
+        cnt.append(c)
+    if phi < 0:
+        return -math.inf
+    if phi > 1:
+        return math.inf
+    if math.isnan(phi) or not all(a <= b for a, b in zip(bounds, bounds[1:])):
+        return math.nan
+    expected = cnt[-1] * phi
+    fit = next((i for i, c in enumerate(cnt) if not c < expected), n)  # n: no counter reaches it (negative counters)
+    if fit >= n - 1:
+        return bounds[n - 2]
+    uc, ub = cnt[fit], bounds[fit]
+    lb, lc = (0.0 if math.isnan(bounds[0]) else min(bounds[0], 0.0)), 0.0  # f64::min ignores NaN
+    if fit > 0:
+        lb, lc = bounds[fit - 1], cnt[fit - 1]
+    if abs(uc - lc) < 1e-10:
+        return math.nan
+    return lb + (ub - lb) / (uc - lc) * (expected - lc)
+
+
+def histogram_fold_sharded(phi, rates, ok, row_hist, row_le, n_hist: int, group=None):
+    """Host mirror of b2p_histogram_fold_allgather (the same owners and shuffle, torch.distributed instead of the
+    library's NCCL communicator; used by the gloo tests): this rank's bucket rows rates / ok [R, T] (ok: the cell has a
+    value), each row's global histogram id row_hist [R] and parsed bound row_le [R] -> (out [n_hist, T] f64,
+    ok [n_hist, T] bool, bytes this rank sent), the same on every rank.
+      - each rank's bucket count per histogram is all-gathered; a histogram's owner is the rank with the most of them,
+        the lowest on a tie;
+      - each rank sends its rows of histograms it does not own, with their headers (bound, histogram, rank, row), to
+        the owner (here: an all-gather of every rank's sent rows, padded to the largest, from which each owner takes its
+        own);
+      - the owner folds each of its histograms over its buckets ordered by (bound ascending, NaN last, rank, row);
+      - every owner's results are all-gathered and placed in histogram order."""
+    import torch.distributed as dist
+    world, me = dist.get_world_size(group), dist.get_rank(group)
+    rates = np.ascontiguousarray(rates, np.float64)
+    ok = np.asarray(ok, bool)
+    R, T = rates.shape
+    H = int(n_hist)
+    Tw = (T + 31) // 32
+    row_hist = np.asarray(row_hist, np.int64)
+    row_le = np.asarray(row_le, np.float64)
+    counts = np.stack(_all_gather(np.bincount(row_hist, minlength=H).astype(np.int64), group))
+    owner = histogram_owners(counts)
+    mine = np.flatnonzero(owner[row_hist] == me) if R else np.zeros(0, np.int64)
+    sent = np.flatnonzero(owner[row_hist] != me) if R else np.zeros(0, np.int64)
+    sent = sent[np.lexsort((sent, row_hist[sent]))] if sent.size else sent
+    P = int(max(_all_gather(np.array([sent.size], np.int64), group))[0])
+    s_val, s_ok, s_hdr = np.zeros((P, T)), np.zeros((P, T), bool), np.full((P, 3), -1, np.int64)
+    s_le = np.zeros(P)
+    s_val[:sent.size], s_ok[:sent.size], s_le[:sent.size] = rates[sent], ok[sent], row_le[sent]
+    s_hdr[:sent.size] = np.stack([row_hist[sent], np.full(sent.size, me), sent], axis=1)
+    got = [_all_gather(a, group) for a in (s_val, s_ok, s_le, s_hdr)]
+    # the owner's buckets: (histogram, bound, rank, row, values, cells)
+    buckets = [(int(row_hist[i]), float(row_le[i]), me, int(i), rates[i], ok[i]) for i in mine]
+    for r in range(world):
+        for j in range(P):
+            h, src, row = (int(x) for x in got[3][r][j])
+            if h >= 0 and owner[h] == me:
+                buckets.append((h, float(got[2][r][j]), src, row, got[0][r][j], got[1][r][j]))
+    buckets.sort(key=lambda b: (b[0], np.isnan(b[1]), 0.0 if np.isnan(b[1]) else b[1], b[2], b[3]))
+    own = np.flatnonzero(owner == me)
+    o_val, o_ok = np.zeros((own.size, T)), np.zeros((own.size, T), bool)
+    place = {int(h): i for i, h in enumerate(own)}
+    by_hist = {}
+    for b in buckets:
+        by_hist.setdefault(b[0], []).append(b)
+    for h, bs in by_hist.items():
+        for k in range(T):
+            present = [b for b in bs if b[5][k]]
+            v = _fold_cells(phi, [b[1] for b in present], [float(b[4][k]) for b in present])
+            if v is not None:
+                o_val[place[h], k], o_ok[place[h], k] = v, True
+    n_own = np.bincount(owner, minlength=world)
+    Q = int(n_own.max()) if H else 0
+    p_val, p_ok = np.zeros((Q, T)), np.zeros((Q, T), bool)
+    p_val[:own.size], p_ok[:own.size] = o_val, o_ok
+    all_val, all_ok = _all_gather(p_val, group), _all_gather(p_ok, group)
+    out, out_ok = np.zeros((H, T)), np.zeros((H, T), bool)
+    for r in range(world):
+        hs = np.flatnonzero(owner == r)
+        out[hs], out_ok[hs] = all_val[r][:hs.size], all_ok[r][:hs.size]
+    return out, out_ok, sent.size * (8 * T + 4 * Tw + HIST_HEADER_BYTES) + own.size * (8 * T + 4 * Tw)

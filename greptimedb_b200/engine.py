@@ -327,6 +327,85 @@ class Context:
                                                _ptr(bucket_le), H, _ptr(rates), _ptr(valid), R, T, _ptr(out), _ptr(ov)))
         return out, ov
 
+    def histogram_fold_allgather(self, phi, rates, valid, row_hist, row_le, n_hist):
+        """histogram_quantile over bucket rows sharded across the ranks of the context's communicator (collective; every
+        rank passes the same phi, n_hist and T): this rank's grid rates [R,T] / valid [R,Tw] u32, each row's global
+        histogram id row_hist [R] and parsed bound row_le [R] -> (out [n_hist,T] f64, valid_words [n_hist,Tw] u32), the
+        same on every rank.  Without a communicator: histogram_fold over this rank's rows."""
+        rates = np.ascontiguousarray(rates, np.float64)
+        valid = np.ascontiguousarray(valid, np.uint32)
+        row_hist = np.ascontiguousarray(row_hist, np.uint32)
+        row_le = np.ascontiguousarray(row_le, np.float64)
+        R, T = rates.shape
+        if valid.shape != (R, (T + 31) // 32) or row_hist.shape != (R,) or row_le.shape != (R,):
+            raise ValueError(f"valid must be [{R}, {(T + 31) // 32}] u32 words, row_hist and row_le [{R}]")
+        out = np.zeros((n_hist, T), np.float64)
+        ov = np.zeros((n_hist, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_histogram_fold_allgather(self._h, float(phi), _ptr(rates), _ptr(valid), R, T,
+                                                         _ptr(row_hist), _ptr(row_le), n_hist, _ptr(out), _ptr(ov)))
+        return out, ov
+
+    def range_histogram_fold_allgather(self, p: RangeParams, phi, ts, val, offsets, row_hist, row_le, n_hist):
+        """histogram_quantile(phi, fn(bucket series)) over series sharded across the ranks of the context's
+        communicator (collective): this rank's samples ts / val with series offsets [S+1], each series' global histogram
+        id row_hist [S] and parsed bound row_le [S] -> (out [n_hist,T] f64, valid_words [n_hist,Tw] u32), the same on
+        every rank.  The range function's grid stays on the device."""
+        ts = np.ascontiguousarray(ts, np.int64)
+        val = np.ascontiguousarray(val, np.float64)
+        offsets = np.ascontiguousarray(offsets, np.uint64)
+        row_hist = np.ascontiguousarray(row_hist, np.uint32)
+        row_le = np.ascontiguousarray(row_le, np.float64)
+        S = offsets.size - 1
+        if row_hist.shape != (S,) or row_le.shape != (S,):
+            raise ValueError(f"row_hist and row_le must hold one entry per series ({S})")
+        T = num_steps(p.start, p.end, p.interval)
+        out = np.zeros((n_hist, T), np.float64)
+        ov = np.zeros((n_hist, (T + 31) // 32), np.uint32)
+        self._check(self._L.b2p_range_histogram_fold_allgather(self._h, C.byref(p), _ptr(ts), _ptr(val), None,
+                                                               _ptr(offsets), ts.size, S, float(phi), _ptr(row_hist),
+                                                               _ptr(row_le), n_hist, _ptr(out), _ptr(ov)))
+        return out, ov
+
+    @staticmethod
+    def histogram_shard_owners(counts) -> np.ndarray:
+        """The owner of each histogram from the counts table [n_ranks, n_hist]: the rank holding most of its buckets,
+        the lowest on a tie -> u32 [n_hist]."""
+        counts = np.ascontiguousarray(counts, np.uint32)
+        R, H = counts.shape
+        owner = np.zeros(H, np.uint32)
+        L = _lib.load()
+        rc = L.b2p_histogram_shard_owners(_ptr(counts), R, H, _ptr(owner))
+        if rc != 0:
+            raise B2PError(rc, L.b2p_last_error().decode())
+        return owner
+
+    @staticmethod
+    def histogram_shard_index(hist, le, rank, row, n_hist):
+        """The HistogramFold index over buckets given by (histogram, bound, source rank, source row): histogram, bound
+        ascending with NaN last, then (rank, row) -> (hist_off [n_hist+1], bucket_series [n] (positions in the input),
+        bucket_le [n])."""
+        hist = np.ascontiguousarray(hist, np.uint32)
+        le = np.ascontiguousarray(le, np.float64)
+        rank = np.ascontiguousarray(rank, np.uint32)
+        row = np.ascontiguousarray(row, np.uint32)
+        n = hist.size
+        if not (le.size == rank.size == row.size == n):
+            raise ValueError("hist, le, rank and row must have one entry per bucket")
+        hist_off = np.zeros(n_hist + 1, np.uint32)
+        bucket_series = np.zeros(n, np.uint32)
+        bucket_le = np.zeros(n, np.float64)
+        L = _lib.load()
+        rc = L.b2p_histogram_shard_index(_ptr(hist), _ptr(le), _ptr(rank), _ptr(row), n, n_hist, _ptr(hist_off),
+                                         _ptr(bucket_series), _ptr(bucket_le))
+        if rc != 0:
+            raise B2PError(rc, L.b2p_last_error().decode())
+        return hist_off, bucket_series, bucket_le
+
+    def row_move_dev(self, inp, in_valid, src, dst, n, T, out, out_valid):
+        """out row dst[i] = inp row src[i] for i < n (T f64 values and Tw u32 words per row); device pointers."""
+        self._check(self._L.b2p_row_move_dev(self._h, _ptr(inp), _ptr(in_valid), _ptr(src), _ptr(dst), n, T, _ptr(out),
+                                             _ptr(out_valid)))
+
     def binary_op(self, op, lhs, lhs_valid, lhs_row, rhs, rhs_valid, rhs_row, return_bool=False):
         """lhs[lhs_row[p]] op rhs[rhs_row[p]] for every pair p -> (out [P,T] f64, valid_words [P,Tw] u32)."""
         lhs = np.ascontiguousarray(lhs, np.float64)

@@ -146,9 +146,10 @@ class PromRangeExec(_PlanNode):
         return int(self._L.b2p_plan_num_series(self._h))
 
     def sharded(self) -> "PromRangeExec":
-        """Mark the leaf's aggregate stage sharded (b2p_plan_set_sharded): every rank pushes its own shard of series and
-        execute() gives every rank the aggregate over the union, through the context's communicator (without one, the
-        unsharded node).  A leaf without an aggregate stage raises.  Returns self."""
+        """Mark the leaf's aggregate or HistogramFold stage sharded (b2p_plan_set_sharded): every rank pushes its own
+        shard of series and execute() gives every rank the aggregate or histogram_quantile over the union, through the
+        context's communicator (without one, the unsharded node).  A leaf without such a stage raises.  Returns
+        self."""
         return self._set_sharded()
 
 
@@ -318,6 +319,13 @@ class HistogramQuantilePlan(_PlanNode):
         self._h = self._L.b2p_plan_histogram_quantile_create(ctx._h, le.encode(), float(phi), child._h)
         if not self._h:
             raise B2PError(-1, self._L.b2p_plan_last_error().decode())
+
+    def sharded(self) -> "HistogramQuantilePlan":
+        """Mark the node sharded (b2p_plan_set_sharded): every rank runs the plan over its own shard of series, which
+        may split a histogram's buckets across ranks, and execute() gives every rank the node over every rank's child
+        rows in rank order, through the context's communicator (without one, the unsharded node).  The child subtree
+        must be row-local.  Returns self."""
+        return self._set_sharded()
 
 
 class SortPlan(_PlanNode):

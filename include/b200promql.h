@@ -883,6 +883,59 @@ B2P_API int b2p_range_histogram_fold(b2p_ctx* ctx, const b2p_range_params* p, co
 B2P_API int b2p_histogram_fold(b2p_ctx* ctx, double phi, const uint32_t* hist_off, const uint32_t* bucket_series,
                                const double* bucket_le, uint32_t n_hist, const double* rates, const uint32_t* valid_words,
                                uint32_t n_rows, uint64_t T, double* out, uint32_t* out_valid_words);
+/* histogram_quantile over bucket rows sharded across ranks (collective and synchronous; every rank calls it with the
+ * same n_hist, T and phi).  rates / valid_words are this rank's [n_rows x T] grid and bitmap, row_hist [n_rows] each
+ * row's global histogram id (< n_hist) and row_le [n_rows] its parsed bound (NaN: NULL or unparsable).  out
+ * [n_hist x T] / out_valid_words [n_hist x Tw] receive the same bytes on every rank: b2p_histogram_fold over every
+ * rank's rows concatenated in rank order, each histogram's buckets in the order of b2p_histogram_shard_index (bound
+ * ascending, NaN last, ties in (rank, row) order).
+ *   1. one all-gather of each rank's bucket count per histogram, [n_ranks x n_hist] u32;
+ *   2. owners (b2p_histogram_shard_owners): the rank holding most of a histogram's buckets, the lowest on a tie;
+ *   3. batches of contiguous histograms in which every rank's sent and received rows, (8 T + 4 Tw + 24) B each, fit the
+ *      context's exchange cap (B2P_TOPK_EXCHANGE_BYTES, equal on every rank; a histogram too large alone is a batch of
+ *      its own).  Per batch each rank packs its rows of histograms it does not own (b2p_row_move_dev), grouped by
+ *      owner in (histogram, row) order, each with a 24-byte header (bound, histogram, rank, row), and sends them with
+ *      ncclSend / ncclRecv in one group; the owner folds its histograms (K5) over [its rows | the received rows]
+ *      with the index b2p_histogram_shard_index builds from the headers;
+ *   4. every owner's result rows go to every rank (one ncclBroadcast per owner) and are placed in histogram order.
+ * The counts table decides everything after it, so every rank derives the same batches, sends and receives: no size
+ * is exchanged.  Where every histogram is whole on one rank no bucket row moves.  b2p_last_exchange_bytes() gives the
+ * bytes this rank sent: its packed rows with their headers and its result block.  Without a communicator the output
+ * is b2p_histogram_fold's over its own rows.  B2P_E_INVALID: a NULL argument; a row_hist entry >= n_hist on any rank
+ * (the counts table carries each rank's verdict, so every rank returns it).  B2P_E_TOO_LARGE: more than 2^32 - 1
+ * bucket rows over all ranks, also on every rank.  A failure local to one rank — a NULL argument or a bad grid before
+ * the first collective, a device allocation or copy failing during the call — returns on that rank only, while the
+ * other ranks wait in their next collective; as with the other sharded calls, the caller must then tear down the
+ * communicator on every rank.
+ *
+ * b2p_range_histogram_fold_allgather is the same call over this rank's bucket SERIES: the range function (p, samples
+ * as b2p_range_histogram_fold takes them) writes the [n_series x T] rates straight into the fold's grid on the device,
+ * row_hist / row_le give each series' histogram and bound.  Whether or not a histogram is split, the dense matrix never
+ * leaves the device; where none is split no bucket row is sent and each rank runs K5 over its own series, as
+ * b2p_range_histogram_fold would, and only the results are gathered.
+ *
+ * The steps it is built from, so one GPU can play R ranks through the same code:
+ *   b2p_histogram_shard_owners (host only): owner [n_hist] from the counts table [n_ranks x n_hist];
+ *   b2p_histogram_shard_index (host only): the fold index over n buckets, each given by its histogram (< n_hist),
+ *     bound, source rank and source row: histogram, then bound ascending with NaN last (-0.0 ties +0.0), then
+ *     (rank, row).  hist_off [n_hist + 1], bucket_series [n] (the buckets' positions in the input) and bucket_le [n]
+ *     are what b2p_histogram_fold[_dev] take.  B2P_E_INVALID: a NULL argument, a hist entry >= n_hist;
+ *   b2p_row_move_dev: out row dst[i] = in row src[i] for i < n, T f64 values and Tw u32 words per row, device pointers
+ *     (16-byte copies where T is even and both grids are 16-byte aligned). */
+B2P_API int b2p_histogram_fold_allgather(b2p_ctx* ctx, double phi, const double* rates, const uint32_t* valid_words,
+                                         uint32_t n_rows, uint64_t T, const uint32_t* row_hist, const double* row_le,
+                                         uint32_t n_hist, double* out, uint32_t* out_valid_words);
+B2P_API int b2p_range_histogram_fold_allgather(b2p_ctx* ctx, const b2p_range_params* p, const int64_t* ts,
+                                               const double* val, const uint32_t* sid, const uint64_t* offsets_host,
+                                               uint64_t n_samples, uint32_t n_series, double phi,
+                                               const uint32_t* row_hist, const double* row_le, uint32_t n_hist,
+                                               double* out, uint32_t* out_valid_words);
+B2P_API int b2p_histogram_shard_owners(const uint32_t* counts, int32_t n_ranks, uint32_t n_hist, uint32_t* owner);
+B2P_API int b2p_histogram_shard_index(const uint32_t* hist, const double* le, const uint32_t* rank, const uint32_t* row,
+                                      uint32_t n, uint32_t n_hist, uint32_t* hist_off, uint32_t* bucket_series,
+                                      double* bucket_le);
+B2P_API int b2p_row_move_dev(b2p_ctx* ctx, const double* in, const uint32_t* in_valid, const uint32_t* src,
+                             const uint32_t* dst, uint32_t n, uint64_t T, double* out, uint32_t* out_valid);
 /* Host-pointer forms of b2p_binary_op_dev / b2p_scalar_op_dev (synchronous; row-index errors are returned directly). */
 B2P_API int b2p_binary_op(b2p_ctx* ctx, int32_t op, int32_t return_bool, const double* lhs, const uint32_t* lhs_valid,
                           const uint32_t* lhs_row, uint32_t n_lhs_rows, const double* rhs, const uint32_t* rhs_valid,

@@ -336,6 +336,24 @@ extern "C" {
         ctx: *mut b2p_ctx, phi: f64, hist_off: *const u32, bucket_series: *const u32, bucket_le: *const f64,
         n_hist: u32, rates: *const f64, valid_words: *const u32, t: u64, out: *mut f64, out_valid_words: *mut u32,
     ) -> c_int;
+    pub fn b2p_histogram_fold_allgather(
+        ctx: *mut b2p_ctx, phi: f64, rates: *const f64, valid_words: *const u32, n_rows: u32, t: u64,
+        row_hist: *const u32, row_le: *const f64, n_hist: u32, out: *mut f64, out_valid_words: *mut u32,
+    ) -> c_int;
+    pub fn b2p_range_histogram_fold_allgather(
+        ctx: *mut b2p_ctx, p: *const B2pRangeParams, ts: *const i64, val: *const f64, sid: *const u32,
+        offsets_host: *const u64, n_samples: u64, n_series: u32, phi: f64, row_hist: *const u32, row_le: *const f64,
+        n_hist: u32, out: *mut f64, out_valid_words: *mut u32,
+    ) -> c_int;
+    pub fn b2p_histogram_shard_owners(counts: *const u32, n_ranks: i32, n_hist: u32, owner: *mut u32) -> c_int;
+    pub fn b2p_histogram_shard_index(
+        hist: *const u32, le: *const f64, rank: *const u32, row: *const u32, n: u32, n_hist: u32, hist_off: *mut u32,
+        bucket_series: *mut u32, bucket_le: *mut f64,
+    ) -> c_int;
+    pub fn b2p_row_move_dev(
+        ctx: *mut b2p_ctx, input: *const f64, in_valid: *const u32, src: *const u32, dst: *const u32, n: u32, t: u64,
+        out: *mut f64, out_valid: *mut u32,
+    ) -> c_int;
     pub fn b2p_column_reduce_dev(
         ctx: *mut b2p_ctx, cols: *const *const f64, n_cols: u32, n_rows: u64, out_sum: *mut f64, out_cnt: *mut u64,
     ) -> c_int;
